@@ -14,14 +14,26 @@
 // Because activations are stored time-major ([item][row][channel]) a Conv1d tap is just a TMA box whose
 // row coordinate is shifted by j*dil: no im2col is ever materialised.
 //
+// Two kernels.  gemm_tc_kernel runs the element-wise epilogues (bias, LeakyReLU + BatchNorm, Conv2d):
 // CTA = 160 threads, persistent over (m_tile, n_tile):
 //   warp 4      TMA producer: per k-block four boxes (A_hi, A_lo: 128 rows x 64 ch; W_hi, W_lo: BN x 64)
 //               into a 128B-swizzled, NSTAGE-deep shared-memory ring, completion on full[] mbarriers
 //   warps 0-3   one warpgroup: 24 wgmma per k-block (two m64 halves x four k-steps x three products) into
 //               registers, the slot is released one k-block later; then the accumulator goes through shared
 //               memory (row m of the tile -> thread m) and the same threads run the epilogue: bias, LeakyReLU,
-//               BatchNorm affine, then float32 rows, the next layer's hi/lo 16-bit planes or the fused poolings.
+//               BatchNorm affine, then float32 rows or the next layer's hi/lo 16-bit planes.
 //               The producer fills the ring for the next tile meanwhile.
+// gemm_tc_pool_kernel runs the two pooling epilogues (TC_POOL, TC_MAXPOOL3), whose cross-row reductions take about as
+// long as the tile's MMAs; CTA = 384 threads, persistent over tiles taken in m-major order from a per-stream atomic
+// counter (a CTA that becomes resident late runs fewer tiles):
+//   warpgroup 0     (setmaxnreg 40) one thread fetches the CTA's next tile, hands its index to the consumer whose turn it
+//                   is, and loads per k-block four boxes (128 or BN rows x 32 ch) into a 64B-swizzled ring
+//   warpgroups 1-2  (setmaxnreg 232) ping-pong consumers: each runs whole 128 x BN tiles, alternately; an ordering barrier
+//                   hands the tensor cores to the other consumer once a tile's MMAs are issued, so one consumer's
+//                   pooling epilogue overlaps the other's mainloop.  The accumulator goes to shared memory 64 columns
+//                   at a time, already through bias / LeakyReLU / BatchNorm (TC_POOL) or the weight scale (TC_MAXPOOL3).
+// Both issue the same wgmma sequence (k order, lo.hi, hi.lo, hi.hi per k-step) and the same epilogue arithmetic for an
+// output element whichever CTA or warpgroup runs its tile.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <math.h>
@@ -29,6 +41,9 @@
 #include <string.h>
 
 #include <algorithm>
+#include <map>
+#include <mutex>
+#include <utility>
 
 #include "dg_common.cuh"
 #include "tc_ptx.cuh"
@@ -36,6 +51,8 @@
 namespace dg {
 
 constexpr int TC_BM = 128, TC_BK = 64, TC_THREADS = 160;
+constexpr int TC_POOL_BK = 32, TC_POOL_THREADS = 384;   // gemm_tc_pool_kernel
+constexpr int TC_SMEM_MAX = 227 * 1024;                 // dynamic shared memory per CTA on sm_90
 
 struct TcArgs {
   long long M;          // output rows
@@ -67,12 +84,13 @@ struct TcArgs {
   // bias + MaxPool1d(3) over rows ([M / 3, ldc]), pool_part the per-tile InstanceNorm partial sums of the pre-bias pooled values:
   // [m_tiles][2 (item of the tile)][2 (sum, sum of squares)][N] over the pooled frames < pool3_T of an item
   int tile_rows, pool3_T;
+  unsigned* tile_ctr;      // gemm_tc_pool_kernel, [2]: tiles handed out past the first wave, CTAs finished (both back to 0)
 };
 
 enum TcEpi { TC_BIAS_F32 = 0, TC_LEAKY_BN_SPLIT = 1, TC_LEAKY_BN_F32 = 2, TC_CONV2D = 3, TC_POOL = 4, TC_MAXPOOL3 = 5 };
 
 // ------------------------------------------------------------------------------------ the kernel
-// Layout: [NSTAGE stages of (A hi, A lo, W hi, W lo)] [parameters] [barriers] [accumulator tile] [pooling staging]
+// Layout: [NSTAGE stages of (A hi, A lo, W hi, W lo)] [parameters] [barriers] [accumulator tile]
 template <int BN>
 struct TcSmem {
   static constexpr int A_BYTES = TC_BM * TC_BK * 2;     // 16 KB per plane
@@ -83,12 +101,7 @@ struct TcSmem {
   // the finished accumulator, one float32 row per tile row (+4 floats: 128-bit row reads without bank conflicts)
   static constexpr int ACC_LD = BN + 4;
   static constexpr int ACC_BYTES = TC_BM * ACC_LD * 4;
-  // TC_POOL: activation chunk [128][33] + row weights [128][4] + cross-row-group staging [4][2][8][32], all float
-  static constexpr int POOL_BYTES = (128 * 33 + 128 * 4 + 4 * 2 * 8 * 32) * 4;
-  // TC_MAXPOOL3: accumulator chunk [128][33] + cross-row-group staging [4][2][2][32], all float
-  static constexpr int POOL3_BYTES = (128 * 33 + 4 * 2 * 2 * 32) * 4;
   static constexpr int TOTAL = NSTAGE * STAGE_BYTES + PARAM_BYTES + 256 + ACC_BYTES + 1024;   // + barriers + alignment slack
-  static constexpr int extra(int epi) { return epi == 4 ? POOL_BYTES : (epi == 5 ? POOL3_BYTES : 0); }
 };
 
 // 32 consecutive accumulator columns of this thread's row
@@ -107,9 +120,9 @@ __device__ __forceinline__ void acc_ld32(const float* p, uint32_t (&r)[32]) {
 // Executed by the 128 threads of the warpgroup; thread et = 32 quad + lane owns row et of the tile.  `mt` = index of the
 // 128-row tile (rows mt * 128 ..), `acc_row` = this thread's row of the finished accumulator in shared memory.
 template <int BN, int EPI>
-__device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params, float* pool_stage, const float* acc_row,
+__device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params, const float* acc_row,
                                                  long long mt, int n0, int quad, int lane, int et, bool stage_params) {
-    const long long m = mt * (EPI == TC_MAXPOOL3 ? a.tile_rows : TC_BM) + quad * 32 + lane;
+    const long long m = mt * TC_BM + quad * 32 + lane;
     // stage the per-column parameters of this tile (named barrier 1: the 128 epilogue threads only); with a single
     // column tile they are the same for every tile of this CTA: staged once
     if (stage_params) {
@@ -118,7 +131,7 @@ __device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params,
         const int n = n0 + i;
         const bool ok = n < a.N;
         params[i] = (ok && a.bias) ? a.bias[n] : 0.f;
-        constexpr bool has_bn = EPI != TC_BIAS_F32 && EPI != TC_MAXPOOL3;
+        constexpr bool has_bn = EPI != TC_BIAS_F32;
         params[BN + i] = (ok && has_bn) ? a.bn_scale[n] * (EPI == TC_CONV2D ? a.acc_scale : 1.f) : 1.f;   // (2^-k: exact)
         params[2 * BN + i] = (ok && has_bn) ? a.bn_shift[n] : 0.f;
       }
@@ -147,140 +160,12 @@ __device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params,
         }
       }
     }
-    // TC_POOL: the rows' pooling weights go to shared memory; `brow` = first row of the tile that belongs to the NEXT item
-    // (a 128-row tile covers at most two items)
-    int brow = TC_BM;
-    if (EPI == TC_POOL) {
-      float4 pw = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (m < a.M) pw = *reinterpret_cast<const float4*>(a.pool_w + m * 4);
-      reinterpret_cast<float4*>(pool_stage + 128 * 33)[quad * 32 + lane] = pw;     // row of the tile
-      const long long first = (long long)mt * TC_BM;
-      const long long nxt = (first / a.pool_item_rows + 1) * a.pool_item_rows;
-      brow = nxt - first < TC_BM ? (int)(nxt - first) : TC_BM;
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-    }
 #pragma unroll 1
     for (int c = 0; c < BN; c += 32) {
       uint32_t r[32];
       acc_ld32(acc_row + c, r);
-      if (EPI != TC_POOL && EPI != TC_MAXPOOL3 && n0 + c >= a.N) continue;
+      if (n0 + c >= a.N) continue;
       float v[32];
-      if (EPI == TC_POOL) {
-        // bias -> LeakyReLU -> BatchNorm affine, then the deviation from the per-channel pivot (the BatchNorm shift) goes to
-        // shared memory; thread (row group rg, column col) then sums its 32 rows for the K speakers -- independent
-        // accumulators, no cross-lane traffic -- split at `brow` between the tile's two items
-        float* dsm = pool_stage;                    // [128][33]
-        const float4* wsm = reinterpret_cast<const float4*>(pool_stage + 128 * 33);
-        float* stg = pool_stage + 128 * 33 + 128 * 4;   // [rg 4][item 2][8][32]
-#pragma unroll
-        for (int q4 = 0; q4 < 8; q4++) {       // parameters as 128-bit loads
-          const float4 b4 = *reinterpret_cast<const float4*>(params + c + 4 * q4);
-          const float4 s4 = *reinterpret_cast<const float4*>(params + BN + c + 4 * q4);
-          const float4 h4 = *reinterpret_cast<const float4*>(params + 2 * BN + c + 4 * q4);
-          const float bb[4] = {b4.x, b4.y, b4.z, b4.w}, ss[4] = {s4.x, s4.y, s4.z, s4.w}, hh[4] = {h4.x, h4.y, h4.z, h4.w};
-#pragma unroll
-          for (int e = 0; e < 4; e++) {
-            const float x = leaky(fmaf(__uint_as_float(r[4 * q4 + e]), a.acc_scale, bb[e]));
-            dsm[(quad * 32 + lane) * 33 + 4 * q4 + e] = fmaf(x, ss[e], hh[e]) - hh[e];
-          }
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        {
-          const int rg = et >> 5, col = et & 31, r_lo = rg * 32, r_hi = r_lo + 32;
-#pragma unroll
-          for (int sg = 0; sg < 2; sg++) {
-            const int lo = sg == 0 ? r_lo : max(r_lo, brow), hi = sg == 0 ? min(r_hi, brow) : r_hi;
-            float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
-            if (a.pool_K <= 3) {               // the usual three local speakers: the fourth weight is not touched
-#pragma unroll 8
-              for (int rr = lo; rr < hi; rr++) {
-                const float dv = dsm[rr * 33 + col];
-                const float4 w4 = wsm[rr];
-                const float a0 = w4.x * dv, a1 = w4.y * dv, a2 = w4.z * dv;
-                s1[0] += a0; s1[1] += a1; s1[2] += a2;
-                s2[0] = fmaf(a0, dv, s2[0]); s2[1] = fmaf(a1, dv, s2[1]); s2[2] = fmaf(a2, dv, s2[2]);
-              }
-            } else {
-#pragma unroll 8
-              for (int rr = lo; rr < hi; rr++) {
-                const float dv = dsm[rr * 33 + col];
-                const float4 w4 = wsm[rr];
-                const float a0 = w4.x * dv, a1 = w4.y * dv, a2 = w4.z * dv, a3 = w4.w * dv;
-                s1[0] += a0; s1[1] += a1; s1[2] += a2; s1[3] += a3;
-                s2[0] = fmaf(a0, dv, s2[0]); s2[1] = fmaf(a1, dv, s2[1]); s2[2] = fmaf(a2, dv, s2[2]); s2[3] = fmaf(a3, dv, s2[3]);
-              }
-            }
-#pragma unroll
-            for (int k = 0; k < 4; k++) {
-              stg[((rg * 2 + sg) * 8 + 2 * k) * 32 + col] = s1[k];
-              stg[((rg * 2 + sg) * 8 + 2 * k + 1) * 32 + col] = s2[k];
-            }
-          }
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        // 2 items x K speakers x 2 sums x 32 columns: the four row groups' totals are added in a fixed order
-        {
-          const int col = et & 31, twoK = 2 * a.pool_K;
-          for (int q = et >> 5; q < 2 * twoK; q += 4) {
-            const int sg = q >= twoK ? 1 : 0, j = q - sg * twoK;
-            const float tot = ((stg[((0 * 2 + sg) * 8 + j) * 32 + col] + stg[((1 * 2 + sg) * 8 + j) * 32 + col]) +
-                               stg[((2 * 2 + sg) * 8 + j) * 32 + col]) + stg[((3 * 2 + sg) * 8 + j) * 32 + col];
-            const int n = n0 + c + col;
-            if (n < a.N && mt < a.m_tiles) a.pool_part[(((size_t)mt * 2 + sg) * 8 + j) * a.N + n] = tot;
-          }
-        }
-        continue;
-      }
-      if (EPI == TC_MAXPOOL3) {
-        // bias + MaxPool1d(3) over the rows of the tile (42 windows of three rows: through shared memory), and the
-        // InstanceNorm partial sums of the pooled values, split at `brow3` between the tile's two items
-        float* dsm = pool_stage;                    // [128][33]
-        float* stg = pool_stage + a.tile_rows * 33; // [rg 4][item 2][2][32]
-        if (quad * 32 + lane < a.tile_rows) {        // (the staging buffer holds tile_rows rows)
-#pragma unroll
-          for (int i = 0; i < 32; i++) dsm[(quad * 32 + lane) * 33 + i] = __uint_as_float(r[i]) * a.acc_scale;
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        {
-          const int col = et & 31, rg = et >> 5, n = n0 + c + col;
-          const long long first = mt * (long long)a.tile_rows;                  // first un-pooled row of the tile
-          const long long item0 = first / a.pool_item_rows;
-          const long long nxt = (item0 + 1) * a.pool_item_rows;
-          const int brow3 = nxt - first < a.tile_rows ? (int)(nxt - first) / 3 : a.tile_rows / 3;   // first window of the next item
-          const long long p_first = first / 3;                                  // first pooled row of the tile
-          const int f0 = (int)(p_first - item0 * (a.pool_item_rows / 3));       // its frame index inside item0
-          const long long Mp = a.M / 3;
-          const float bias = params[c + col];
-          float s1[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};
-          for (int pr = rg; pr < a.tile_rows / 3; pr += 4) {
-            const float v = fmaxf(fmaxf(dsm[(3 * pr) * 33 + col], dsm[(3 * pr + 1) * 33 + col]), dsm[(3 * pr + 2) * 33 + col]);
-            const int sg = pr >= brow3 ? 1 : 0;
-            const int frame = sg ? pr - brow3 : f0 + pr;
-            const long long P = p_first + pr;
-            if (P < Mp) {
-              if (n < a.N) a.out_f32[P * a.ldc + n] = v + bias;
-              if (frame < a.pool3_T) {
-                s1[sg] += v;
-                s2[sg] = fmaf(v, v, s2[sg]);
-              }
-            }
-          }
-#pragma unroll
-          for (int sg = 0; sg < 2; sg++) {
-            stg[((rg * 2 + sg) * 2 + 0) * 32 + col] = s1[sg];
-            stg[((rg * 2 + sg) * 2 + 1) * 32 + col] = s2[sg];
-          }
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        {   // 2 items x 2 sums x 32 columns = 128 values, one per thread: the four row groups in a fixed order
-          const int col = et & 31, q = et >> 5, sg = q >> 1, j = q & 1, n = n0 + c + col;
-          const float tot = ((stg[((0 * 2 + sg) * 2 + j) * 32 + col] + stg[((1 * 2 + sg) * 2 + j) * 32 + col]) +
-                             stg[((2 * 2 + sg) * 2 + j) * 32 + col]) + stg[((3 * 2 + sg) * 2 + j) * 32 + col];
-          if (n < a.N) a.pool_part[(((size_t)mt * 2 + sg) * 2 + j) * a.N + n] = tot;
-        }
-        asm volatile("bar.sync 1, 128;" ::: "memory");     // the chunk buffer is rewritten by the next 32 columns
-        continue;
-      }
       if (EPI == TC_CONV2D) {
         // BatchNorm2d(eval) affine -> (+ residual) -> ReLU
 #pragma unroll
@@ -403,7 +288,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
   uint64_t* full = bars;                 // [NSTAGE] TMA -> MMA
   uint64_t* empty = bars + NSTAGE;       // [NSTAGE] MMA -> TMA
   float* acc_s = reinterpret_cast<float*>(smem + NSTAGE * S::STAGE_BYTES + S::PARAM_BYTES + 256);   // [128][ACC_LD]
-  float* pool_stage = acc_s + TC_BM * S::ACC_LD;                                     // TC_POOL / TC_MAXPOOL3 only
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // warp-uniform
   const int num_tiles = a.m_tiles * a.n_tiles;
@@ -424,7 +308,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       int stage = 0, phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
-        const int m0 = mt * (EPI == TC_MAXPOOL3 ? a.tile_rows : TC_BM), n0 = nt * BN;
+        const int m0 = mt * TC_BM, n0 = nt * BN;
         for (int j = 0; j < a.KW; j++) {
           for (int cb = 0; cb < a.cin_blocks; cb++) {
             mbar_wait(&empty[stage], phase ^ 1);
@@ -499,14 +383,363 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       }
     }
     asm volatile("bar.sync 1, 128;" ::: "memory");
-    tc_epilogue_tile<BN, EPI>(a, params, pool_stage, acc_s + et * S::ACC_LD, mt, nt * BN, quad, lane, et,
+    tc_epilogue_tile<BN, EPI>(a, params, acc_s + et * S::ACC_LD, mt, nt * BN, quad, lane, et,
                               a.n_tiles > 1 || tile == (int)blockIdx.x);
   }
 }
 
+// ------------------------------------------------------------------------------------ the pooling kernel
+// Layout: [NSTAGE stages of (A hi, A lo, W hi, W lo)] [barriers] [consumer 0: parameters | chunk | pooling staging]
+// [consumer 1: the same]
+template <int BN>
+struct TcPoolSmem {
+  static constexpr int A_BYTES = TC_BM * TC_POOL_BK * 2;     // 8 KB per plane
+  static constexpr int W_BYTES = BN * TC_POOL_BK * 2;
+  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;
+  // 128 / 144 KB of operands in flight at BN = 128 (TC_POOL) / 64 (TC_MAXPOOL3)
+  static constexpr int NSTAGE = BN == 128 ? 4 : 6;
+  static constexpr int BAR_BYTES = 256;
+  static constexpr int PARAM_FLOATS = 3 * BN;
+  // CHUNK_W accumulator columns of every tile row, as [CHUNK_W / 32][128][33] (conflict-free column reads)
+  static constexpr int CHUNK_W = 64;
+  static constexpr int CHUNK_FLOATS = CHUNK_W / 32 * TC_BM * 33;
+  // TC_POOL: row weights [128][4] + cross-row-group staging [4][2][8][32]; TC_MAXPOOL3: staging [4][2][2][32]
+  __host__ __device__ static constexpr int extra_floats(int epi) { return epi == 4 ? 128 * 4 + 4 * 2 * 8 * 32 : (epi == 5 ? 4 * 2 * 2 * 32 : 0); }
+  __host__ __device__ static constexpr int consumer_floats(int epi) { return PARAM_FLOATS + CHUNK_FLOATS + extra_floats(epi); }
+  __host__ __device__ static constexpr int total(int epi) { return NSTAGE * STAGE_BYTES + BAR_BYTES + 2 * consumer_floats(epi) * 4 + 1024; }   // + alignment slack
+};
+static_assert(TcPoolSmem<128>::total(4) <= TC_SMEM_MAX && TcPoolSmem<64>::total(5) <= TC_SMEM_MAX, "gemm_tc: shared memory");
+
+// ------------------------------------------------------------------------------------ the epilogue of one 128-row tile
+// Executed by the 128 threads of a consumer warpgroup; thread et = 32 quad + lane owns row et of the tile.  `mt` = index
+// of the 128-row tile (rows mt * 128 ..), `acc` = the finished accumulator in registers, `bar` = the warpgroup's named
+// barrier.
+template <int BN, int EPI>
+__device__ __forceinline__ void tc_pool_epilogue_tile(const TcArgs& a, float* params, float* chunk, float* pool_stage,
+                                                 const float (&acc)[2][BN / 2], int bar, long long mt, int n0, int quad,
+                                                 int lane, int et, bool stage_params) {
+    const long long m = mt * (EPI == TC_MAXPOOL3 ? a.tile_rows : TC_BM) + quad * 32 + lane;
+    // stage the per-column parameters of this tile; with a single column tile they are the same for every tile of this
+    // warpgroup: staged once
+    if (stage_params) {
+      named_sync(bar, 128);
+      for (int i = et; i < BN; i += 128) {
+        const int n = n0 + i;
+        const bool ok = n < a.N;
+        params[i] = (ok && a.bias) ? a.bias[n] : 0.f;
+        constexpr bool has_bn = EPI != TC_BIAS_F32 && EPI != TC_MAXPOOL3;
+        params[BN + i] = (ok && has_bn) ? a.bn_scale[n] : 1.f;
+        params[2 * BN + i] = (ok && has_bn) ? a.bn_shift[n] : 0.f;
+      }
+      named_sync(bar, 128);
+    }
+    // TC_POOL: the rows' pooling weights go to shared memory; `brow` = first row of the tile that belongs to the NEXT item
+    // (a 128-row tile covers at most two items)
+    int brow = TC_BM;
+    if (EPI == TC_POOL) {
+      float4 pw = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (m < a.M) pw = *reinterpret_cast<const float4*>(a.pool_w + m * 4);
+      reinterpret_cast<float4*>(pool_stage)[quad * 32 + lane] = pw;     // row of the tile
+      const long long first = (long long)mt * TC_BM;
+      const long long nxt = (first / a.pool_item_rows + 1) * a.pool_item_rows;
+      brow = nxt - first < TC_BM ? (int)(nxt - first) : TC_BM;
+      named_sync(bar, 128);
+    }
+    // accumulator fragment of this thread (tc_ptx.cuh): acc[h][4 j + e] is row 64 h + 16 quad + lane / 4 + 8 (e / 2),
+    // column 8 j + 2 (lane % 4) + e % 2.  The tile goes through shared memory CW columns at a time (the registers of a
+    // staged chunk are free for the reductions), which run 32 columns at a time.
+    constexpr int CW = TcPoolSmem<BN>::CHUNK_W;
+    const int fr0 = 16 * quad + (lane >> 2), fc0 = 2 * (lane & 3);
+#pragma unroll
+    for (int c0 = 0; c0 < BN; c0 += CW) {
+      {
+        // every thread is past its reads of the previous chunk (the closing barrier of its last 32 columns)
+#pragma unroll
+        for (int c = c0; c < c0 + CW; c += 32) {
+          float* dsm = chunk + (c - c0) / 32 * (128 * 33);   // [128][33]
+#pragma unroll
+          for (int jj = 0; jj < 4; jj++) {
+#pragma unroll
+            for (int e1 = 0; e1 < 2; e1++) {
+              const int col = 8 * jj + fc0 + e1;
+              float bb = 0.f, ss = 0.f, hh = 0.f;
+              if (EPI == TC_POOL) bb = params[c + col], ss = params[BN + c + col], hh = params[2 * BN + c + col];
+#pragma unroll
+              for (int h = 0; h < 2; h++) {
+#pragma unroll
+                for (int e2 = 0; e2 < 2; e2++) {   // (MAXPOOL3: rows past tile_rows are not read)
+                  const float y = acc[h][4 * (c / 8 + jj) + 2 * e2 + e1];
+                  float* d = dsm + (64 * h + fr0 + 8 * e2) * 33 + col;
+                  if (EPI == TC_POOL) {
+                    // bias -> LeakyReLU -> BatchNorm affine, then the deviation from the per-channel pivot (the BatchNorm shift)
+                    const float x = leaky(fmaf(y, a.acc_scale, bb));
+                    *d = fmaf(x, ss, hh) - hh;
+                  } else {
+                    *d = y * a.acc_scale;
+                  }
+                }
+              }
+            }
+          }
+        }
+      }
+      named_sync(bar, 128);
+#pragma unroll
+      for (int c = c0; c < c0 + CW; c += 32) {
+        if (EPI == TC_POOL) {
+          // thread (row group rg, column col) sums its 32 rows of d for the K speakers -- independent accumulators, no
+          // cross-lane traffic -- split at `brow` between the tile's two items
+          const float* dsm = chunk + (c - c0) / 32 * (128 * 33);
+          const float4* wsm = reinterpret_cast<const float4*>(pool_stage);
+          float* stg = pool_stage + 128 * 4;          // [rg 4][item 2][8][32]
+          if (c != c0) named_sync(bar, 128);   // the previous 32 columns' totals are read from stg
+          {
+            const int rg = et >> 5, col = et & 31, r_lo = rg * 32, r_hi = r_lo + 32;
+#pragma unroll
+            for (int sg = 0; sg < 2; sg++) {
+              const int lo = sg == 0 ? r_lo : max(r_lo, brow), hi = sg == 0 ? min(r_hi, brow) : r_hi;
+              float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
+              if (a.pool_K <= 3) {               // the usual three local speakers: the fourth weight is not touched
+#pragma unroll 8
+                for (int rr = lo; rr < hi; rr++) {
+                  const float dv = dsm[rr * 33 + col];
+                  const float4 w4 = wsm[rr];
+                  const float a0 = w4.x * dv, a1 = w4.y * dv, a2 = w4.z * dv;
+                  s1[0] += a0; s1[1] += a1; s1[2] += a2;
+                  s2[0] = fmaf(a0, dv, s2[0]); s2[1] = fmaf(a1, dv, s2[1]); s2[2] = fmaf(a2, dv, s2[2]);
+                }
+              } else {
+#pragma unroll 8
+                for (int rr = lo; rr < hi; rr++) {
+                  const float dv = dsm[rr * 33 + col];
+                  const float4 w4 = wsm[rr];
+                  const float a0 = w4.x * dv, a1 = w4.y * dv, a2 = w4.z * dv, a3 = w4.w * dv;
+                  s1[0] += a0; s1[1] += a1; s1[2] += a2; s1[3] += a3;
+                  s2[0] = fmaf(a0, dv, s2[0]); s2[1] = fmaf(a1, dv, s2[1]); s2[2] = fmaf(a2, dv, s2[2]); s2[3] = fmaf(a3, dv, s2[3]);
+                }
+              }
+#pragma unroll
+              for (int k = 0; k < 4; k++) {
+                stg[((rg * 2 + sg) * 8 + 2 * k) * 32 + col] = s1[k];
+                stg[((rg * 2 + sg) * 8 + 2 * k + 1) * 32 + col] = s2[k];
+              }
+            }
+          }
+          named_sync(bar, 128);
+          // 2 items x K speakers x 2 sums x 32 columns: the four row groups' totals are added in a fixed order
+          {
+            const int col = et & 31, twoK = 2 * a.pool_K;
+            for (int q = et >> 5; q < 2 * twoK; q += 4) {
+              const int sg = q >= twoK ? 1 : 0, j = q - sg * twoK;
+              const float tot = ((stg[((0 * 2 + sg) * 8 + j) * 32 + col] + stg[((1 * 2 + sg) * 8 + j) * 32 + col]) +
+                                 stg[((2 * 2 + sg) * 8 + j) * 32 + col]) + stg[((3 * 2 + sg) * 8 + j) * 32 + col];
+              const int n = n0 + c + col;
+              if (n < a.N && mt < a.m_tiles) a.pool_part[(((size_t)mt * 2 + sg) * 8 + j) * a.N + n] = tot;
+            }
+          }
+          if (c + 32 == c0 + CW) named_sync(bar, 128);     // the chunk buffer is rewritten by the next chunk
+          continue;
+        }
+        if (EPI == TC_MAXPOOL3) {
+          // bias + MaxPool1d(3) over the rows of the tile (42 windows of three rows: through shared memory), and the
+          // InstanceNorm partial sums of the pooled values, split at `brow3` between the tile's two items
+          const float* dsm = chunk + (c - c0) / 32 * (128 * 33);   // [128][33]
+          float* stg = pool_stage;                    // [rg 4][item 2][2][32]
+          {
+            const int col = et & 31, rg = et >> 5, n = n0 + c + col;
+            const long long first = mt * (long long)a.tile_rows;                  // first un-pooled row of the tile
+            const long long item0 = first / a.pool_item_rows;
+            const long long nxt = (item0 + 1) * a.pool_item_rows;
+            const int brow3 = nxt - first < a.tile_rows ? (int)(nxt - first) / 3 : a.tile_rows / 3;   // first window of the next item
+            const long long p_first = first / 3;                                  // first pooled row of the tile
+            const int f0 = (int)(p_first - item0 * (a.pool_item_rows / 3));       // its frame index inside item0
+            const long long Mp = a.M / 3;
+            const float bias = params[c + col];
+            float s1[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};
+            for (int pr = rg; pr < a.tile_rows / 3; pr += 4) {
+              const float v = fmaxf(fmaxf(dsm[(3 * pr) * 33 + col], dsm[(3 * pr + 1) * 33 + col]), dsm[(3 * pr + 2) * 33 + col]);
+              const int sg = pr >= brow3 ? 1 : 0;
+              const int frame = sg ? pr - brow3 : f0 + pr;
+              const long long P = p_first + pr;
+              if (P < Mp) {
+                if (n < a.N) a.out_f32[P * a.ldc + n] = v + bias;
+                if (frame < a.pool3_T) {
+                  s1[sg] += v;
+                  s2[sg] = fmaf(v, v, s2[sg]);
+                }
+              }
+            }
+#pragma unroll
+            for (int sg = 0; sg < 2; sg++) {
+              stg[((rg * 2 + sg) * 2 + 0) * 32 + col] = s1[sg];
+              stg[((rg * 2 + sg) * 2 + 1) * 32 + col] = s2[sg];
+            }
+          }
+          named_sync(bar, 128);
+          {   // 2 items x 2 sums x 32 columns = 128 values, one per thread: the four row groups in a fixed order
+            const int col = et & 31, q = et >> 5, sg = q >> 1, j = q & 1, n = n0 + c + col;
+            const float tot = ((stg[((0 * 2 + sg) * 2 + j) * 32 + col] + stg[((1 * 2 + sg) * 2 + j) * 32 + col]) +
+                               stg[((2 * 2 + sg) * 2 + j) * 32 + col]) + stg[((3 * 2 + sg) * 2 + j) * 32 + col];
+            if (n < a.N) a.pool_part[(((size_t)mt * 2 + sg) * 2 + j) * a.N + n] = tot;
+          }
+          named_sync(bar, 128);     // stg (and after the last 32 columns the chunk buffer) is rewritten next
+          continue;
+        }
+      }
+    }
+}
+
+// Named barriers besides 0: 1 + c = the 128 threads of consumer c (epilogue staging); 3 + c = consumer c may issue its
+// mainloop (256 threads: consumer c waits, the other consumer arrives once its own MMAs are issued).
+template <int BN, int EPI, bool F16>
+__global__ void __launch_bounds__(TC_POOL_THREADS, 1)
+gemm_tc_pool_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
+               const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo, TcArgs a) {
+  using S = TcPoolSmem<BN>;
+  constexpr int NSTAGE = S::NSTAGE;
+  extern __shared__ unsigned char smem_raw[];
+  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NSTAGE * S::STAGE_BYTES);
+  uint64_t* full = bars;                      // [NSTAGE] TMA -> MMA
+  uint64_t* empty = bars + NSTAGE;            // [NSTAGE] MMA -> TMA
+  uint64_t* tile_full = bars + 2 * NSTAGE;    // [2] producer -> consumer c: tile_idx[c] holds its next tile
+  uint64_t* tile_empty = tile_full + 2;       // [2] consumer c -> producer: tile_idx[c] has been read
+  volatile int* tile_idx = reinterpret_cast<volatile int*>(tile_empty + 2);   // [2]
+  float* cons = reinterpret_cast<float*>(smem + NSTAGE * S::STAGE_BYTES + S::BAR_BYTES);
+
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // warp-uniform
+  const int wg = warp >> 2;
+  const int num_tiles = a.m_tiles * a.n_tiles;
+  const int kblocks = a.KW * a.cin_blocks;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < NSTAGE; s++) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 1);
+    }
+    for (int c = 0; c < 2; c++) {
+      mbar_init(&tile_full[c], 1);
+      mbar_init(&tile_empty[c], 128);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    // ===================================================================== tile scheduler + TMA producer
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      int stage = 0, phase = 0;
+      // i = position in this CTA's sequence of tiles, run by consumer i % 2.  The first tile is blockIdx.x, the later ones
+      // come from the counter.  Two end marks follow the last tile: -1 (its consumer passes the turn on), then -2.
+      for (int i = 0, tile = blockIdx.x;; i++) {
+        const int c = i & 1;
+        mbar_wait(&tile_empty[c], ((i >> 1) & 1) ^ 1);
+        if (tile >= num_tiles) {
+          tile_idx[c] = -1;
+          mbar_arrive(&tile_full[c]);
+          mbar_wait(&tile_empty[c ^ 1], (((i + 1) >> 1) & 1) ^ 1);
+          tile_idx[c ^ 1] = -2;
+          mbar_arrive(&tile_full[c ^ 1]);
+          break;
+        }
+        tile_idx[c] = tile;
+        mbar_arrive(&tile_full[c]);
+        const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
+        const int m0 = mt * (EPI == TC_MAXPOOL3 ? a.tile_rows : TC_BM), n0 = nt * BN;
+        for (int j = 0; j < a.KW; j++) {
+          for (int cb = 0; cb < a.cin_blocks; cb++) {
+            mbar_wait(&empty[stage], phase ^ 1);
+            unsigned char* st = smem + stage * S::STAGE_BYTES;
+            mbar_expect_tx(&full[stage], S::STAGE_BYTES);
+            const int kcol = (j * a.cin_blocks + cb) * TC_POOL_BK;
+            tma_load_2d(st, &tmA_hi, cb * TC_POOL_BK, m0 + a.tap_off[j], &full[stage]);
+            tma_load_2d(st + S::A_BYTES, &tmA_lo, cb * TC_POOL_BK, m0 + a.tap_off[j], &full[stage]);
+            tma_load_2d(st + 2 * S::A_BYTES, &tmW_hi, kcol, n0, &full[stage]);
+            tma_load_2d(st + 2 * S::A_BYTES + S::W_BYTES, &tmW_lo, kcol, n0, &full[stage]);
+            if (++stage == NSTAGE) {
+              stage = 0;
+              phase ^= 1;
+            }
+          }
+        }
+        tile = (int)gridDim.x + (int)atomicAdd(&a.tile_ctr[0], 1u);
+      }
+      // every CTA has taken its last tile once all have counted themselves here: the last one returns the counter to 0
+      // for the next launch on this stream
+      __threadfence();
+      if (atomicAdd(&a.tile_ctr[1], 1u) == gridDim.x - 1) {
+        atomicExch(&a.tile_ctr[0], 0u);
+        atomicExch(&a.tile_ctr[1], 0u);
+      }
+    }
+    return;
+  }
+  // ===================================================================== MMA + epilogue (consumers c = 0, 1)
+  setmaxnreg_inc<232>();
+  const int c = wg - 1, quad = warp & 3, et = threadIdx.x - 128 * wg;
+  float* params = cons + c * S::consumer_floats(EPI);   // bias | bn_scale | bn_shift
+  float* chunk = params + S::PARAM_FLOATS;
+  float* pool_stage = chunk + S::CHUNK_FLOATS;          // TC_POOL / TC_MAXPOOL3 only
+  const int bar = 1 + c, turn = 3 + c, turn_other = 3 + (c ^ 1);
+  if (c == 1) named_arrive(3, 256);                     // consumer 0 issues the first mainloop
+  for (int n = 0;; n++) {
+    mbar_wait(&tile_full[c], n & 1);
+    const int tile = tile_idx[c];
+    mbar_arrive(&tile_empty[c]);
+    named_sync(turn, 256);
+    if (tile < 0) {
+      if (tile == -1) named_arrive(turn_other, 256);
+      break;
+    }
+    const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
+    const int pos = (2 * n + c) * kblocks;              // ring position of the tile's first k-block
+    int stage = pos % NSTAGE, phase = (pos / NSTAGE) & 1;
+    float acc[2][BN / 2];
+    int prev = -1;                       // slot of the previous k-block: released once its MMAs are complete
+    for (int kb = 0; kb < kblocks; kb++) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * S::STAGE_BYTES);
+      const uint64_t a_hi = wg_desc_sw64(sa), a_lo = wg_desc_sw64(sa + S::A_BYTES);
+      const uint64_t w_hi = wg_desc_sw64(sa + 2 * S::A_BYTES), w_lo = wg_desc_sw64(sa + 2 * S::A_BYTES + S::W_BYTES);
+      constexpr uint64_t HALF = (uint64_t)((64 * TC_POOL_BK * 2) >> 4);   // rows 64..127 of the A tile
+      wg_fence_acc(acc[0]);
+      wg_fence_acc(acc[1]);
+      wg_fence();
+#pragma unroll
+      for (int ks = 0; ks < TC_POOL_BK / 16; ks++) {
+        const uint64_t adv = (uint64_t)((ks * 32) >> 4);   // +32 bytes per 16-element k-step
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+          wgmma_ss<BN, F16>(acc[h], a_lo + adv + h * HALF, w_hi + adv, (kb | ks) != 0);
+          wgmma_ss<BN, F16>(acc[h], a_hi + adv + h * HALF, w_lo + adv, 1);
+          wgmma_ss<BN, F16>(acc[h], a_hi + adv + h * HALF, w_hi + adv, 1);
+        }
+      }
+      wg_commit();
+      wg_wait<1>();
+      wg_fence_acc(acc[0]);
+      wg_fence_acc(acc[1]);
+      if (prev >= 0 && et == 0) mbar_arrive(&empty[prev]);
+      prev = stage;
+      if (++stage == NSTAGE) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    named_arrive(turn_other, 256);       // the other consumer's MMAs queue behind these while they drain
+    wg_wait<0>();
+    wg_fence_acc(acc[0]);
+    wg_fence_acc(acc[1]);
+    if (et == 0) mbar_arrive(&empty[prev]);
+    tc_pool_epilogue_tile<BN, EPI>(a, params, chunk, pool_stage, acc, bar, mt, nt * BN, quad, lane, et, a.n_tiles > 1 || n == 0);
+  }
+}
+
 // ------------------------------------------------------------------------------------ host side
-// bf16 matrix [rows, cols] row-major (cols contiguous, row pitch `ld` elements); box = 64 cols x box_rows
-static int make_map(CUtensorMap* m, const void* base, long long rows, int cols, int ld, int box_rows) {
+// bf16 matrix [rows, cols] row-major (cols contiguous, row pitch `ld` elements); box = box_cols x box_rows, swizzled by the
+// box row's width (64 or 128 bytes)
+static int make_map(CUtensorMap* m, const void* base, long long rows, int cols, int ld, int box_cols, int box_rows) {
   EncodeTiledFn fn = encode_fn();
   if (!fn) {
     set_error("cuTensorMapEncodeTiled is not available from the driver");
@@ -514,10 +747,11 @@ static int make_map(CUtensorMap* m, const void* base, long long rows, int cols, 
   }
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {(cuuint32_t)TC_BK, (cuuint32_t)box_rows};
+  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  box_cols * 2 == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled failed with code " + std::to_string((int)r));
@@ -526,21 +760,54 @@ static int make_map(CUtensorMap* m, const void* base, long long rows, int cols, 
   return 0;
 }
 
-template <int BN, int EPI>
-static int launch_tc(const TcGemm& g, cudaStream_t st) {
-  using S = TcSmem<BN>;
-  CUtensorMap ta_hi, ta_lo, tw_hi, tw_lo;
+// Tile counters of the dynamic schedule, one pair per (device, stream): launches on one stream run one after another and
+// each leaves its counter at 0, launches on different streams may overlap and never share one.
+constexpr int TC_CTR_SLOTS = 1024;
+__device__ unsigned g_tc_tile_ctr[TC_CTR_SLOTS][2];
+
+static unsigned* tile_counter(cudaStream_t st) {
+  static std::mutex mu;
+  static std::map<std::pair<int, cudaStream_t>, int> slot_of;
+  static int used[64] = {};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) {
+    set_error("gemm_tc: no current CUDA device");
+    return nullptr;
+  }
+  int slot;
+  {
+    std::lock_guard<std::mutex> lock(mu);
+    auto it = slot_of.find({dev, st});
+    if (it != slot_of.end()) {
+      slot = it->second;
+    } else {
+      if (used[dev] == TC_CTR_SLOTS) {
+        set_error("gemm_tc: more than " + std::to_string(TC_CTR_SLOTS) + " streams have launched GEMMs on one device");
+        return nullptr;
+      }
+      slot = slot_of[{dev, st}] = used[dev]++;
+    }
+  }
+  void* base = nullptr;
+  if (cudaGetSymbolAddress(&base, g_tc_tile_ctr) != cudaSuccess) {
+    set_error("gemm_tc: cannot address the tile counters");
+    return nullptr;
+  }
+  return static_cast<unsigned*>(base) + 2 * slot;
+}
+
+// operand maps and kernel arguments of one launch; tiles of `bn` columns and `bk`-wide k-blocks
+static int tc_setup(const TcGemm& g, int bn, int bk, int epi, CUtensorMap* maps, TcArgs& a) {
   const int Ktot = g.KW * g.Cin;
-  const int n_tiles = (g.N + BN - 1) / BN;
-  if (make_map(&ta_hi, g.A_hi, g.Mtot, g.Cin, g.lda, TC_BM) || make_map(&ta_lo, g.A_lo, g.Mtot, g.Cin, g.lda, TC_BM) ||
-      make_map(&tw_hi, g.W_hi, g.Npad, Ktot, Ktot, BN) || make_map(&tw_lo, g.W_lo, g.Npad, Ktot, Ktot, BN))
+  if (make_map(&maps[0], g.A_hi, g.Mtot, g.Cin, g.lda, bk, TC_BM) || make_map(&maps[1], g.A_lo, g.Mtot, g.Cin, g.lda, bk, TC_BM) ||
+      make_map(&maps[2], g.W_hi, g.Npad, Ktot, Ktot, bk, bn) || make_map(&maps[3], g.W_lo, g.Npad, Ktot, Ktot, bk, bn))
     return -2;
-  TcArgs a{};
-  a.M = g.M; a.N = g.N; a.n_tiles = n_tiles;
-  a.tile_rows = EPI == TC_MAXPOOL3 ? g.pool3_tile_rows : TC_BM;
+  a = TcArgs{};
+  a.M = g.M; a.N = g.N; a.n_tiles = (g.N + bn - 1) / bn;
+  a.tile_rows = epi == TC_MAXPOOL3 ? g.pool3_tile_rows : TC_BM;
   a.pool3_T = g.pool3_T;
   a.m_tiles = (int)((g.M + a.tile_rows - 1) / a.tile_rows);
-  a.KW = g.KW; a.dil = g.dil; a.cin_blocks = g.Cin / TC_BK;
+  a.KW = g.KW; a.dil = g.dil; a.cin_blocks = g.Cin / bk;
   a.bias = g.bias; a.bn_scale = g.bn_scale; a.bn_shift = g.bn_shift;
   a.out_f32 = g.out_f32; a.out_hi = reinterpret_cast<__nv_bfloat16*>(g.out_hi);
   a.out_lo = reinterpret_cast<__nv_bfloat16*>(g.out_lo); a.ldc = g.ldc;
@@ -552,18 +819,46 @@ static int launch_tc(const TcGemm& g, cudaStream_t st) {
   a.res_lo = reinterpret_cast<const __nv_bfloat16*>(g.res_lo);
   a.pool_w = g.pool_w; a.pool_part = g.pool_part; a.pool_item_rows = g.pool_item_rows; a.pool_K = g.pool_K;
   {
-    const bool planes = EPI == TC_LEAKY_BN_SPLIT;
+    const bool planes = epi == TC_LEAKY_BN_SPLIT;
     const uintptr_t base = planes ? ((uintptr_t)g.out_hi | (uintptr_t)g.out_lo) : (uintptr_t)g.out_f32;
     a.vec8 = base % 32 == 0 && (g.ldc * (planes ? 2 : 4)) % 32 == 0;
   }
+  return 0;
+}
+
+static int tc_grid(const TcGemm& g, const TcArgs& a) {
+  const int sms = g.sm_limit > 0 ? std::min(g.sm_limit, usable_sms()) : usable_sms();
+  const int tiles = a.m_tiles * a.n_tiles;
+  return tiles < sms ? tiles : sms;
+}
+
+template <int BN, int EPI>
+static int launch_tc(const TcGemm& g, cudaStream_t st) {
+  using S = TcSmem<BN>;
+  CUtensorMap m[4];
+  TcArgs a;
+  if (tc_setup(g, BN, TC_BK, EPI, m, a)) return -2;
   auto kern = a.f16 ? gemm_tc_kernel<BN, EPI, true> : gemm_tc_kernel<BN, EPI, false>;
   static bool attr_done[2][64] = {};
   if (first_use_on_device(attr_done[a.f16]))
-    DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL + S::extra(EPI)));
-  const int sms = g.sm_limit > 0 ? std::min(g.sm_limit, usable_sms()) : usable_sms();
-  const int tiles = a.m_tiles * a.n_tiles;
-  const int grid = tiles < sms ? tiles : sms;
-  kern<<<grid, TC_THREADS, S::TOTAL + S::extra(EPI), st>>>(ta_hi, ta_lo, tw_hi, tw_lo, a);
+    DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
+  kern<<<tc_grid(g, a), TC_THREADS, S::TOTAL, st>>>(m[0], m[1], m[2], m[3], a);
+  DG_LAUNCHED();
+  return 0;
+}
+
+template <int BN, int EPI>
+static int launch_tc_pool(const TcGemm& g, cudaStream_t st) {
+  using S = TcPoolSmem<BN>;
+  CUtensorMap m[4];
+  TcArgs a;
+  if (tc_setup(g, BN, TC_POOL_BK, EPI, m, a)) return -2;
+  if (!(a.tile_ctr = tile_counter(st))) return -2;
+  auto kern = a.f16 ? gemm_tc_pool_kernel<BN, EPI, true> : gemm_tc_pool_kernel<BN, EPI, false>;
+  static bool attr_done[2][64] = {};
+  if (first_use_on_device(attr_done[a.f16]))
+    DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::total(EPI)));
+  kern<<<tc_grid(g, a), TC_POOL_THREADS, S::total(EPI), st>>>(m[0], m[1], m[2], m[3], a);
   DG_LAUNCHED();
   return 0;
 }
@@ -590,7 +885,7 @@ int launch_gemm_tc(const TcGemm& g, cudaStream_t st) {
       set_error("gemm_tc (pool): needs 128-wide tiles, 1..4 speakers and items of at least 128 rows");
       return -1;
     }
-    return launch_tc<128, TC_POOL>(g, st);
+    return launch_tc_pool<128, TC_POOL>(g, st);
   }
   if (g.epi == TC_MAXPOOL3) {
     if (g.Npad != 64 || !g.out_f32 || !g.pool_part || g.pool3_T < 1 || g.pool3_tile_rows < 3 || g.pool3_tile_rows > 126 ||
@@ -598,7 +893,7 @@ int launch_gemm_tc(const TcGemm& g, cudaStream_t st) {
       set_error("gemm_tc (maxpool3): needs 64 output channels and tiles of 3..126 rows (a multiple of 3) that divide the item");
       return -1;
     }
-    return launch_tc<64, TC_MAXPOOL3>(g, st);
+    return launch_tc_pool<64, TC_MAXPOOL3>(g, st);
   }
   if (g.Npad == 64 && g.epi == TC_BIAS_F32) return launch_tc<64, TC_BIAS_F32>(g, st);
   switch (g.epi) {

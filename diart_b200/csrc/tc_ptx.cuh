@@ -65,6 +65,15 @@ __device__ __forceinline__ void split_h16(float x, int f16, uint16_t& hi, uint16
 }
 __device__ __forceinline__ uint32_t pack_u16x2(uint16_t a, uint16_t b) { return (uint32_t)a | ((uint32_t)b << 16); }
 
+// named barriers: `n` threads (a multiple of 32) of the CTA; bar.arrive signals without waiting
+__device__ __forceinline__ void named_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// per-thread register budget of the executing warpgroup (all 128 threads execute it)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // 32 bytes per lane as two 128-bit global stores.  `p` must be 16-byte aligned.
 __device__ __forceinline__ void st_global_v8(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t e, uint32_t f,
                                              uint32_t g, uint32_t h) {
@@ -88,6 +97,15 @@ __device__ __forceinline__ uint64_t wg_desc(uint32_t smem_addr) {
   d |= (uint64_t)1 << 16;                        // leading byte offset (unused for swizzled K-major)
   d |= (uint64_t)(1024 >> 4) << 32;              // stride byte offset
   d |= (uint64_t)1 << 62;                        // SWIZZLE_128B
+  return d;
+}
+// K-major, 64B-swizzled operand tile: rows of 64 B (32 16-bit k-values), 8-row groups 512 B apart
+__device__ __forceinline__ uint64_t wg_desc_sw64(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);   // start address
+  d |= (uint64_t)1 << 16;                        // leading byte offset (unused for swizzled K-major)
+  d |= (uint64_t)(512 >> 4) << 32;               // stride byte offset
+  d |= (uint64_t)2 << 62;                        // SWIZZLE_64B
   return d;
 }
 // K-major operand without swizzle: core matrices of 8 rows x 16 B (128 contiguous bytes); `lbo` = byte stride between
