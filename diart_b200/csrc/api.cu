@@ -128,27 +128,17 @@ struct Tensors {
   }
 };
 
-// DG_SIMT=1 forces the float32 SIMT GEMMs everywhere (A/B switch for the parity tests and bench)
-static bool use_tensor_cores() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("DG_SIMT");
-    v = (e && e[0] == '1') ? 0 : 1;
-  }
-  return v == 1;
-}
-
 static int upload_u16(DevBuf& b, const std::vector<uint16_t>& h) {
   if (b.ensure(h.size() * 2)) return -2;
   DG_CUDA(cudaMemcpy(b.p, h.data(), h.size() * 2, cudaMemcpyHostToDevice));
   return 0;
 }
 
-// float32 [N][K] host weights -> zero-padded 16-bit hi/lo device planes [Npad][K]
+// float32 [N][K] host weights -> zero-padded fp16 hi/lo device planes [Npad][K]
 static int upload_split(DevBuf& hi, DevBuf& lo, const std::vector<float>& w_nk, int N, int Npad, int K) {
   std::vector<uint16_t> h((size_t)Npad * K), l((size_t)Npad * K);
-  hi.wscale = lo.wscale = weight_plane_scale(w_nk.data(), (size_t)N * K, split_f16());
-  split_weights_host(w_nk.data(), N, Npad, K, h.data(), l.data(), split_f16(), hi.wscale);
+  hi.wscale = lo.wscale = weight_plane_scale(w_nk.data(), (size_t)N * K);
+  split_weights_host(w_nk.data(), N, Npad, K, h.data(), l.data(), hi.wscale);
   return (upload_u16(hi, h) || upload_u16(lo, l)) ? DG_ECUDA : 0;
 }
 
@@ -161,9 +151,9 @@ static int upload(DevBuf& b, const std::vector<float>& h) {
 // ------------------------------------------------------------------------------ SincNet front end
 struct SincWeights {
   float wn_gamma = 1.f, wn_beta = 0.f;
-  DevBuf filt, g0, b0, w1, bias1, g1, b1, w2, bias2, g2, b2;
-  DevBuf w1_hi, w1_lo, w2_hi, w2_lo;   // tensor-core path: 16-bit hi/lo planes [64][448] (taps folded into K: 5 x 80 + pad) and [64][5*64]
-  DevBuf filt_planes;                  // sinc filter bank as 16-bit planes [3][80][256] (hi, lo; lo2 for the bf16 mode)
+  DevBuf g0, b0, bias1, g1, b1, bias2, g2, b2;
+  DevBuf w1_hi, w1_lo, w2_hi, w2_lo;   // conv weights as fp16 hi/lo planes [64][448] (taps folded into K: 5 x 80 + pad) and [64][5*64]
+  DevBuf filt_planes;                  // sinc filter bank as fp16 planes [2][80][256] (hi, lo)
   DevBuf cf;                           // folded wav-norm affine: beta * sum_k h[f][k]
   DevBuf hsum;                         // sum_k h[f][k] (stream form of the sinc layer)
 };
@@ -206,10 +196,9 @@ static int prep_sincnet(const Tensors& t, const std::string& pre, SincWeights& w
   if (!lo || !bd) return DG_EWEIGHT;
   std::vector<float> h;
   sinc_filters(lo, bd, h);
-  if (upload(w.filt, h)) return DG_ECUDA;
   {
-    std::vector<uint16_t> fp(3 * 80 * 256);
-    sinc_tc_pack_filters(h.data(), fp.data(), split_f16());
+    std::vector<uint16_t> fp(2 * 80 * 256);
+    sinc_tc_pack_filters(h.data(), fp.data());
     if (upload_u16(w.filt_planes, fp)) return DG_ECUDA;
     std::vector<float> cf(80);
     sinc_tc_affine_consts(h.data(), w.wn_beta, cf.data());
@@ -230,19 +219,6 @@ static int prep_sincnet(const Tensors& t, const std::string& pre, SincWeights& w
       (rc = pad_vec(pre + "norm1d.1.weight", 60, 64, w.g1)) || (rc = pad_vec(pre + "norm1d.1.bias", 60, 64, w.b1)) ||
       (rc = pad_vec(pre + "norm1d.2.weight", 60, 64, w.g2)) || (rc = pad_vec(pre + "norm1d.2.bias", 60, 64, w.b2)) ||
       (rc = pad_vec(pre + "conv1d.1.bias", 60, 64, w.bias1)) || (rc = pad_vec(pre + "conv1d.2.bias", 60, 64, w.bias2)))
-    return rc;
-  // Conv1d weights [out][in][k] -> shifted-window GEMM layout [(tap*Cin_pad + c)][out_pad]
-  auto conv_w = [&](const std::string& name, int out, int in, int k, int in_pad, int out_pad, DevBuf& dst) -> int {
-    const float* s = t.get(name, (int64_t)out * in * k);
-    if (!s) return DG_EWEIGHT;
-    std::vector<float> v((size_t)k * in_pad * out_pad, 0.f);
-    for (int o = 0; o < out; o++)
-      for (int c = 0; c < in; c++)
-        for (int j = 0; j < k; j++) v[((size_t)j * in_pad + c) * out_pad + o] = s[((size_t)o * in + c) * k + j];
-    return upload(dst, v) ? DG_ECUDA : 0;
-  };
-  if ((rc = conv_w(pre + "conv1d.1.weight", 60, 80, 5, 80, 64, w.w1)) ||
-      (rc = conv_w(pre + "conv1d.2.weight", 60, 60, 5, 64, 64, w.w2)))
     return rc;
   auto conv_w_tc = [&](const std::string& name, int out, int in, int k, int in_pad, DevBuf& hi, DevBuf& lo) -> int {
     const float* s = t.get(name, (int64_t)out * in * k);
@@ -272,8 +248,8 @@ static int prep_sincnet(const Tensors& t, const std::string& pre, SincWeights& w
 // ones, so the fused pipeline computes them once per step
 struct SincPrep {
   DevBuf wmean, wrstd, wh, wl;
-  // stream form (needs a hop hint; DG_STREAM_SINC=0 disables it): planes of the raw stream and the device flag "this batch is a run of
-  // overlapping windows"; `hop` > 0 means the stream-form launches were enqueued for this batch
+  // stream form (needs a hop hint): planes of the raw stream and the device flag "this batch is a run of overlapping
+  // windows"; `hop` > 0 means the stream-form launches were enqueued for this batch
   DevBuf swh, swl, flag, spart;
   int hop = 0;
   int ensure(int B, const Geom& g) {
@@ -286,28 +262,22 @@ struct SincPrep {
   }
 };
 struct SincWork {
-  DevBuf wmean, wrstd, p0, sc0, sh0, p1, sc1, sh1, p2, sc2, sh2;
-  DevBuf a0h, a0l, c1, a1h, a1l, c2;   // tensor-core path: 16-bit planes of the conv inputs, un-pooled conv outputs
+  DevBuf p0, sc0, sh0, p1, sc1, sh1, p2, sc2, sh2;
+  DevBuf a0h, a0l, c1, a1h, a1l, c2;   // fp16 planes of the conv inputs; un-pooled conv outputs of the un-fused path
   DevBuf craw, part;                   // stream form: raw convolution of the stream [P][80], statistics partials
   DevBuf part3;                        // per-tile InstanceNorm partial sums of the pooling GEMM epilogues (conv1, conv2)
   SincPrep own_prep;                   // statistics + waveform planes when no shared ones are supplied
   const float* out = nullptr;          // conv2 output that the next layer normalises on load ...
   int out_pool = 0;                    // ... 1: still un-pooled (rows = 3x), MaxPool1d(3) is applied on load
-  int ensure_tc(int B, const Geom& g) {
-    const size_t tail = 64;
-    if (a0h.ensure(((size_t)B * g.S0 + tail) * 128 * 2) || a0l.ensure(((size_t)B * g.S0 + tail) * 128 * 2) ||
-        c1.ensure(((size_t)B * g.S0 + tail) * 64 * 4) || a1h.ensure(((size_t)B * g.S1 + tail) * 64 * 2) ||
-        a1l.ensure(((size_t)B * g.S1 + tail) * 64 * 2) || c2.ensure(((size_t)B * g.S1 + tail) * 64 * 4))
-      return DG_ECUDA;
-    return 0;
-  }
   int ensure(int B, const Geom& g) {
     const size_t tail = 64;  // spare rows so shifted windows of the last tile stay in bounds
-    if (wmean.ensure(B * 4) || wrstd.ensure(B * 4) || p0.ensure(((size_t)B * g.S0 + tail) * 80 * 4) ||
-        sc0.ensure((size_t)B * 80 * 4) || sh0.ensure((size_t)B * 80 * 4) ||
+    if (p0.ensure(((size_t)B * g.S0 + tail) * 80 * 4) || sc0.ensure((size_t)B * 80 * 4) || sh0.ensure((size_t)B * 80 * 4) ||
         p1.ensure(((size_t)B * g.S1 + tail) * 64 * 4) || sc1.ensure((size_t)B * 64 * 4) ||
         sh1.ensure((size_t)B * 64 * 4) || p2.ensure(((size_t)B * g.S2 + tail) * 64 * 4) ||
-        sc2.ensure((size_t)B * 64 * 4) || sh2.ensure((size_t)B * 64 * 4))
+        sc2.ensure((size_t)B * 64 * 4) || sh2.ensure((size_t)B * 64 * 4) ||
+        a0h.ensure(((size_t)B * g.S0 + tail) * 128 * 2) || a0l.ensure(((size_t)B * g.S0 + tail) * 128 * 2) ||
+        c1.ensure(((size_t)B * g.S0 + tail) * 64 * 4) || a1h.ensure(((size_t)B * g.S1 + tail) * 64 * 2) ||
+        a1l.ensure(((size_t)B * g.S1 + tail) * 64 * 2) || c2.ensure(((size_t)B * g.S1 + tail) * 64 * 4))
       return DG_ECUDA;
     return 0;
   }
@@ -317,12 +287,10 @@ static int run_sinc_prep(SincPrep& p, const float* wav, int B, const Geom& g, cu
                          bool overlap_known = false) {
   int rc;
   if ((rc = p.ensure(B, g))) return rc;
-  // stream form of the sinc layer: on by default (DG_STREAM_SINC=0 disables it), only with a hop hint from the caller;
-  // the device flag written by overlap_check decides per batch, so a wrong hint costs a few empty launches, never a
-  // wrong result
-  static const bool stream_on = !(getenv("DG_STREAM_SINC") && getenv("DG_STREAM_SINC")[0] == '0');
+  // stream form of the sinc layer: only with a hop hint from the caller; the device flag written by overlap_check
+  // decides per batch, so a wrong hint costs a few empty launches, never a wrong result
   p.hop = 0;
-  if (stream_on && hop > 0 && B >= 4 && hop % 40 == 0 && g.S % 4 == 0 && hop < g.S && ((uintptr_t)wav & 15) == 0) {
+  if (hop > 0 && B >= 4 && hop % 40 == 0 && g.S % 4 == 0 && hop < g.S && ((uintptr_t)wav & 15) == 0) {
     if ((rc = p.ensure_stream(B, g, hop))) return rc;
     if (overlap_known) {   // the batch was formed on the device from ONE stream (dg_stream): nothing to verify
       DG_CUDA(cudaMemsetAsync(p.flag.p, 1, sizeof(int), st));
@@ -351,120 +319,82 @@ static int run_sincnet(const SincWeights& w, SincWork& k, const float* wav, int 
                        const SincPrep* shared = nullptr) {
   int rc;
   if ((rc = k.ensure(B, g))) return rc;
-  if (use_tensor_cores()) {
-    if ((rc = k.ensure_tc(B, g))) return rc;
-    const int* stream_flag = nullptr;      // device flag "the stream form produced the conv1 operand planes of this batch"
-    static const bool sinc_simt = getenv("DG_SINC_SIMT") && getenv("DG_SINC_SIMT")[0] == '1';
-    if (sinc_simt) {
-      if ((rc = launch_wave_stats(wav, B, g.S, k.wmean.as<float>(), k.wrstd.as<float>(), st))) return rc;
-      rc = launch_sinc0(wav, k.wmean.as<float>(), k.wrstd.as<float>(), w.wn_gamma, w.wn_beta, w.filt.as<float>(), B,
-                        g, k.p0.as<float>(), st);
-    } else {
-      const SincPrep* prep = shared;
-      if (!prep) {
-        if ((rc = run_sinc_prep(k.own_prep, wav, B, g, st))) return rc;
-        prep = &k.own_prep;
-      }
-      if (prep->hop) {   // stream form: one convolution of the unique samples + a per-window affine / |.| / pool pass
-        const SincStreamGeom sg = sinc_stream_geom(B, g, prep->hop);
-        if (k.craw.ensure(((size_t)sg.P + 16) * 80 * 4) || k.part.ensure(sinc_pool_part_floats(B, g, prep->hop) * 4)) return DG_ECUDA;
-        // raw convolution of the stream, then statistics and normalised operand planes straight from it (p0 is never written)
-        if ((rc = launch_sinc0_tc_stream(w.filt_planes.p, B, g, prep->hop, prep->swh.p, prep->swl.p, k.craw.as<float>(),
-                                         prep->flag.as<int>(), st)) ||
-            (rc = launch_sinc_pool_fused(k.craw.as<float>(), prep->wmean.as<float>(), prep->wrstd.as<float>(), w.cf.as<float>(),
-                                         w.hsum.as<float>(), w.wn_gamma, B, g, prep->hop, w.g0.as<float>(), w.b0.as<float>(),
-                                         k.part.as<float>(), k.sc0.as<float>(), k.sh0.as<float>(), k.a0h.p, k.a0l.p,
-                                         prep->flag.as<int>(), st)))
-          return rc;
-        stream_flag = prep->flag.as<int>();
-      }
-      rc = launch_sinc0_tc(w.wn_gamma, w.cf.as<float>(), w.filt_planes.p, B, g, prep->wh.p, prep->wl.p,
-                           k.p0.as<float>(), st, prep->hop ? prep->flag.as<int>() : nullptr);
-    }
-    if (rc) return rc;
-    if ((rc = launch_instnorm_stats(k.p0.as<float>(), B, g.S0, g.T0, 80, 80, w.g0.as<float>(), w.b0.as<float>(),
-                                    k.sc0.as<float>(), k.sh0.as<float>(), st, 0, stream_flag)))
+  const int* stream_flag = nullptr;      // device flag "the stream form produced the conv1 operand planes of this batch"
+  const SincPrep* prep = shared;
+  if (!prep) {
+    if ((rc = run_sinc_prep(k.own_prep, wav, B, g, st))) return rc;
+    prep = &k.own_prep;
+  }
+  if (prep->hop) {   // stream form: one convolution of the unique samples + a per-window affine / |.| / pool pass
+    const SincStreamGeom sg = sinc_stream_geom(B, g, prep->hop);
+    if (k.craw.ensure(((size_t)sg.P + 16) * 80 * 4) || k.part.ensure(sinc_pool_part_floats(B, g, prep->hop) * 4)) return DG_ECUDA;
+    // raw convolution of the stream, then statistics and normalised operand planes straight from it (p0 is never written)
+    if ((rc = launch_sinc0_tc_stream(w.filt_planes.p, B, g, prep->hop, prep->swh.p, prep->swl.p, k.craw.as<float>(),
+                                     prep->flag.as<int>(), st)) ||
+        (rc = launch_sinc_pool_fused(k.craw.as<float>(), prep->wmean.as<float>(), prep->wrstd.as<float>(), w.cf.as<float>(),
+                                     w.hsum.as<float>(), w.wn_gamma, B, g, prep->hop, w.g0.as<float>(), w.b0.as<float>(),
+                                     k.part.as<float>(), k.sc0.as<float>(), k.sh0.as<float>(), k.a0h.p, k.a0l.p,
+                                     prep->flag.as<int>(), st)))
       return rc;
-    // Conv1d(80,60,5): normalised input as 16-bit hi/lo planes (80-channel rows), un-pooled float32 output
-    const long long M0 = (long long)B * g.S0, M1 = (long long)B * g.S1;
-    if ((rc = launch_split_ex(k.p0.as<float>(), M0, 80, 80, 80, 0, g.S0, k.sc0.as<float>(), k.sh0.as<float>(),
-                              k.a0h.p, k.a0l.p, st, stream_flag)))
-      return rc;
-    // conv1 / conv2 with MaxPool1d(3) and the InstanceNorm partial sums in the GEMM epilogue (TC_MAXPOOL3): the un-pooled maps are
-    // never written, the statistics pass reads 2 x 2 x 64 floats per tile.  Needs a tile of 96..126 rows that divides the item at both stages;
-    // DG_NO_POOL3_FUSE=1 = the round-1 path (un-pooled float32 map -> instnorm_stats -> split with pooling on load)
-    static const bool pool3_on = !(getenv("DG_NO_POOL3_FUSE") && getenv("DG_NO_POOL3_FUSE")[0] == '1');
-    const int tr0 = gemm_tc_pool3_tile_rows(g.S0), tr1 = gemm_tc_pool3_tile_rows(g.S1);
-    if (pool3_on && tr0 && tr1) {
-      if (k.part3.ensure((size_t)(M0 / tr0) * 2 * 2 * 64 * 4)) return DG_ECUDA;
-      TcGemm t{};
-      t.A_hi = k.a0h.p; t.A_lo = k.a0l.p; t.lda = 80; t.Cin = 448; t.KW = 1; t.dil = 1; t.Mtot = M0; t.M = M0;
-      t.W_hi = w.w1_hi.p; t.w_scale = w.w1_hi.wscale; t.W_lo = w.w1_lo.p; t.Npad = 64; t.N = 64; t.bias = w.bias1.as<float>();
-      t.out_f32 = k.p1.as<float>(); t.ldc = 64; t.epi = 5; t.tag = "sinc_conv1";
-      t.pool_part = k.part3.as<float>(); t.pool_item_rows = g.S0; t.pool3_T = g.T1; t.pool3_tile_rows = tr0;
-      if ((rc = launch_gemm_tc(t, st)) ||
-          (rc = launch_instnorm_finalize(k.part3.as<float>(), B, g.S0, tr0, g.T1, 64, 64, w.bias1.as<float>(), w.g1.as<float>(),
-                                         w.b1.as<float>(), k.sc1.as<float>(), k.sh1.as<float>(), 64, st)) ||
-          (rc = launch_split_ex(k.p1.as<float>(), M1, 64, 64, 64, 0, g.S1, k.sc1.as<float>(), k.sh1.as<float>(), k.a1h.p, k.a1l.p, st)))
-        return rc;
-      t.A_hi = k.a1h.p; t.A_lo = k.a1l.p; t.lda = 64; t.Cin = 64; t.KW = 5; t.Mtot = M1; t.M = M1;
-      t.W_hi = w.w2_hi.p; t.w_scale = w.w2_hi.wscale; t.W_lo = w.w2_lo.p; t.bias = w.bias2.as<float>();
-      t.out_f32 = k.p2.as<float>(); t.tag = "sinc_conv2";
-      t.pool_item_rows = g.S1; t.pool3_T = g.T2; t.pool3_tile_rows = tr1;
-      if ((rc = launch_gemm_tc(t, st))) return rc;
-      k.out = k.p2.as<float>();
-      k.out_pool = 0;
-      return launch_instnorm_finalize(k.part3.as<float>(), B, g.S1, tr1, g.T2, 64, 64, w.bias2.as<float>(), w.g2.as<float>(),
-                                      w.b2.as<float>(), k.sc2.as<float>(), k.sh2.as<float>(), 64, st);
-    }
+    stream_flag = prep->flag.as<int>();
+  }
+  if ((rc = launch_sinc0_tc(w.wn_gamma, w.cf.as<float>(), w.filt_planes.p, B, g, prep->wh.p, prep->wl.p, k.p0.as<float>(), st,
+                            stream_flag)))
+    return rc;
+  if ((rc = launch_instnorm_stats(k.p0.as<float>(), B, g.S0, g.T0, 80, 80, w.g0.as<float>(), w.b0.as<float>(),
+                                  k.sc0.as<float>(), k.sh0.as<float>(), st, 0, stream_flag)))
+    return rc;
+  // Conv1d(80,60,5): normalised input as fp16 hi/lo planes (80-channel rows)
+  const long long M0 = (long long)B * g.S0, M1 = (long long)B * g.S1;
+  if ((rc = launch_split_ex(k.p0.as<float>(), M0, 80, 80, 80, 0, g.S0, k.sc0.as<float>(), k.sh0.as<float>(),
+                            k.a0h.p, k.a0l.p, st, stream_flag)))
+    return rc;
+  // conv1 / conv2 with MaxPool1d(3) and the InstanceNorm partial sums in the GEMM epilogue (TC_MAXPOOL3): the un-pooled maps are
+  // never written, the statistics pass reads 2 x 2 x 64 floats per tile.  Needs a tile of 96..126 rows that divides the item at both
+  // stages; otherwise the un-pooled float32 map -> instnorm_stats -> split with pooling on load
+  const int tr0 = gemm_tc_pool3_tile_rows(g.S0), tr1 = gemm_tc_pool3_tile_rows(g.S1);
+  if (tr0 && tr1) {
+    if (k.part3.ensure((size_t)(M0 / tr0) * 2 * 2 * 64 * 4)) return DG_ECUDA;
     TcGemm t{};
     t.A_hi = k.a0h.p; t.A_lo = k.a0l.p; t.lda = 80; t.Cin = 448; t.KW = 1; t.dil = 1; t.Mtot = M0; t.M = M0;
     t.W_hi = w.w1_hi.p; t.w_scale = w.w1_hi.wscale; t.W_lo = w.w1_lo.p; t.Npad = 64; t.N = 64; t.bias = w.bias1.as<float>();
-    t.out_f32 = k.c1.as<float>(); t.ldc = 64; t.epi = 0; t.tag = "sinc_conv1";
-    if ((rc = launch_gemm_tc(t, st))) return rc;
-    if ((rc = launch_instnorm_stats(k.c1.as<float>(), B, g.S0, g.T1, 64, 64, w.g1.as<float>(), w.b1.as<float>(),
-                                    k.sc1.as<float>(), k.sh1.as<float>(), st, 1)))
-      return rc;
-    // Conv1d(60,60,5) on MaxPool(conv1) -> norm -> leaky, again un-pooled output
-    if ((rc = launch_split_ex(k.c1.as<float>(), M1, 64, 64, 64, 1, g.S1, k.sc1.as<float>(), k.sh1.as<float>(),
-                              k.a1h.p, k.a1l.p, st)))
+    t.out_f32 = k.p1.as<float>(); t.ldc = 64; t.epi = 5; t.tag = "sinc_conv1";
+    t.pool_part = k.part3.as<float>(); t.pool_item_rows = g.S0; t.pool3_T = g.T1; t.pool3_tile_rows = tr0;
+    if ((rc = launch_gemm_tc(t, st)) ||
+        (rc = launch_instnorm_finalize(k.part3.as<float>(), B, g.S0, tr0, g.T1, 64, 64, w.bias1.as<float>(), w.g1.as<float>(),
+                                       w.b1.as<float>(), k.sc1.as<float>(), k.sh1.as<float>(), 64, st)) ||
+        (rc = launch_split_ex(k.p1.as<float>(), M1, 64, 64, 64, 0, g.S1, k.sc1.as<float>(), k.sh1.as<float>(), k.a1h.p, k.a1l.p, st)))
       return rc;
     t.A_hi = k.a1h.p; t.A_lo = k.a1l.p; t.lda = 64; t.Cin = 64; t.KW = 5; t.Mtot = M1; t.M = M1;
     t.W_hi = w.w2_hi.p; t.w_scale = w.w2_hi.wscale; t.W_lo = w.w2_lo.p; t.bias = w.bias2.as<float>();
-    t.out_f32 = k.c2.as<float>(); t.tag = "sinc_conv2";
+    t.out_f32 = k.p2.as<float>(); t.tag = "sinc_conv2";
+    t.pool_item_rows = g.S1; t.pool3_T = g.T2; t.pool3_tile_rows = tr1;
     if ((rc = launch_gemm_tc(t, st))) return rc;
-    k.out = k.c2.as<float>();
-    k.out_pool = 1;
-    return launch_instnorm_stats(k.c2.as<float>(), B, g.S1, g.T2, 64, 64, w.g2.as<float>(), w.b2.as<float>(),
-                                 k.sc2.as<float>(), k.sh2.as<float>(), st, 1);
+    k.out = k.p2.as<float>();
+    k.out_pool = 0;
+    return launch_instnorm_finalize(k.part3.as<float>(), B, g.S1, tr1, g.T2, 64, 64, w.bias2.as<float>(), w.g2.as<float>(),
+                                    w.b2.as<float>(), k.sc2.as<float>(), k.sh2.as<float>(), 64, st);
   }
-  k.out = k.p2.as<float>();
-  k.out_pool = 0;
-  if ((rc = launch_wave_stats(wav, B, g.S, k.wmean.as<float>(), k.wrstd.as<float>(), st))) return rc;
-  if ((rc = launch_sinc0(wav, k.wmean.as<float>(), k.wrstd.as<float>(), w.wn_gamma, w.wn_beta, w.filt.as<float>(), B,
-                         g, k.p0.as<float>(), st)))
+  TcGemm t{};
+  t.A_hi = k.a0h.p; t.A_lo = k.a0l.p; t.lda = 80; t.Cin = 448; t.KW = 1; t.dil = 1; t.Mtot = M0; t.M = M0;
+  t.W_hi = w.w1_hi.p; t.w_scale = w.w1_hi.wscale; t.W_lo = w.w1_lo.p; t.Npad = 64; t.N = 64; t.bias = w.bias1.as<float>();
+  t.out_f32 = k.c1.as<float>(); t.ldc = 64; t.epi = 0; t.tag = "sinc_conv1";
+  if ((rc = launch_gemm_tc(t, st))) return rc;
+  if ((rc = launch_instnorm_stats(k.c1.as<float>(), B, g.S0, g.T1, 64, 64, w.g1.as<float>(), w.b1.as<float>(),
+                                  k.sc1.as<float>(), k.sh1.as<float>(), st, 1)))
     return rc;
-  if ((rc = launch_instnorm_stats(k.p0.as<float>(), B, g.S0, g.T0, 80, 80, w.g0.as<float>(), w.b0.as<float>(),
-                                  k.sc0.as<float>(), k.sh0.as<float>(), st)))
+  // Conv1d(60,60,5) on MaxPool(conv1) -> norm -> leaky, again un-pooled output
+  if ((rc = launch_split_ex(k.c1.as<float>(), M1, 64, 64, 64, 1, g.S1, k.sc1.as<float>(), k.sh1.as<float>(),
+                            k.a1h.p, k.a1l.p, st)))
     return rc;
-  GemmArgs a{};
-  a.A = k.p0.as<float>(); a.lda = 80; a.Cin = 80; a.KW = 5; a.dil = 1;
-  a.Mtot = (long long)B * g.S0; a.M = (long long)B * g.S0;
-  a.W = w.w1.as<float>(); a.ldw = 64; a.N = 64; a.bias = w.bias1.as<float>();
-  a.in_sc = k.sc0.as<float>(); a.in_sh = k.sh0.as<float>(); a.item_rows = g.S0;
-  a.C = k.p1.as<float>(); a.ldc = 64; a.epi = EPI_BIAS_POOL3; a.tag = "sinc_conv1";
-  if ((rc = launch_gemm(a, st))) return rc;
-  if ((rc = launch_instnorm_stats(k.p1.as<float>(), B, g.S1, g.T1, 64, 64, w.g1.as<float>(), w.b1.as<float>(),
-                                  k.sc1.as<float>(), k.sh1.as<float>(), st)))
-    return rc;
-  a.A = k.p1.as<float>(); a.lda = 64; a.Cin = 64;
-  a.Mtot = (long long)B * g.S1; a.M = (long long)B * g.S1;
-  a.W = w.w2.as<float>(); a.bias = w.bias2.as<float>();
-  a.in_sc = k.sc1.as<float>(); a.in_sh = k.sh1.as<float>(); a.item_rows = g.S1;
-  a.C = k.p2.as<float>(); a.tag = "sinc_conv2";
-  if ((rc = launch_gemm(a, st))) return rc;
-  return launch_instnorm_stats(k.p2.as<float>(), B, g.S2, g.T2, 64, 64, w.g2.as<float>(), w.b2.as<float>(),
-                               k.sc2.as<float>(), k.sh2.as<float>(), st);
+  t.A_hi = k.a1h.p; t.A_lo = k.a1l.p; t.lda = 64; t.Cin = 64; t.KW = 5; t.Mtot = M1; t.M = M1;
+  t.W_hi = w.w2_hi.p; t.w_scale = w.w2_hi.wscale; t.W_lo = w.w2_lo.p; t.bias = w.bias2.as<float>();
+  t.out_f32 = k.c2.as<float>(); t.tag = "sinc_conv2";
+  if ((rc = launch_gemm_tc(t, st))) return rc;
+  k.out = k.c2.as<float>();
+  k.out_pool = 1;
+  return launch_instnorm_stats(k.c2.as<float>(), B, g.S1, g.T2, 64, 64, w.g2.as<float>(), w.b2.as<float>(),
+                               k.sc2.as<float>(), k.sh2.as<float>(), st, 1);
 }
 
 }  // namespace dg
@@ -477,18 +407,18 @@ struct dg_seg {
   int ps_speakers = 0;             // > 0: powerset model with this many local speakers (dg_seg_set_powerset)
   DevBuf ps_masks;                 // speaker bit set of every powerset class
   SincWeights sw;
-  DevBuf wih[4], bih[4], whh[4];   // input projections [in_pad][1024], bias [1024], packed W_hh
-  DevBuf wih_hi[4], wih_lo[4];     // the same as 16-bit hi/lo planes [1024][in_pad] for the tensor-core path
-  DevBuf whh_hi[4], whh_lo[4];     // W_hh as 16-bit hi/lo planes [2][512][128] for the tensor-core recurrence
-  DevBuf l1w, l1b, l2w, l2b, cw, cb;
-  DevBuf l1_hi, l1_lo, l2_hi, l2_lo, ones128, zeros128;   // head Linears as 16-bit hi/lo planes [128][in] (tensor-core path)
+  DevBuf bih[4];                   // input projection bias b_ih + b_hh [1024]
+  DevBuf wih_hi[4], wih_lo[4];     // input projections as fp16 hi/lo planes [1024][in_pad]
+  DevBuf whh_hi[4], whh_lo[4];     // W_hh as fp16 hi/lo planes [2][512][128] for the tensor-core recurrence
+  DevBuf l1b, l2b, cw, cb;
+  DevBuf l1_hi, l1_lo, l2_hi, l2_lo, ones128, zeros128;   // head Linears as fp16 hi/lo planes [128][in]
   // activations: two independent sets ("lanes") so that the fused pipeline can run the segmentation chains of
   // two consecutive steps concurrently (the recurrence occupies only 32 SMs)
   struct Scratch {
     SincWork work;
-    DevBuf gx, hA, hB, y1, y2;
-    DevBuf xh, xl;                 // bf16 hi/lo planes of the current in-projection input
-    DevBuf y1h, y1l;               // bf16 planes of the first head Linear's output
+    DevBuf gx, y2;
+    DevBuf xh, xl;                 // fp16 hi/lo planes of the current in-projection input
+    DevBuf y1h, y1l;               // fp16 planes of the first head Linear's output
   } scr[2];
   int lane = 0;
   const SincPrep* shared_prep = nullptr;   // set by the fused pipeline: statistics + planes computed once per step
@@ -500,7 +430,8 @@ static int seg_prepare(dg_seg* h, const Tensors& t) {
   if ((rc = prep_sincnet(t, "sincnet.", h->sw))) return rc;
   for (int L = 0; L < 4; L++) {
     const int in = L == 0 ? 60 : 256, in_pad = L == 0 ? 64 : 256;
-    std::vector<float> w((size_t)in_pad * 1024, 0.f), b(1024, 0.f), packed(lstm_whh_packed_floats());
+    // gate rows n = direction * 512 + r of both directions, input channels padded to in_pad
+    std::vector<float> w_nk((size_t)1024 * in_pad, 0.f), b(1024, 0.f);
     const float* hh[2];
     for (int d = 0; d < 2; d++) {
       const std::string sfx = "_l" + std::to_string(L) + (d ? "_reverse" : "");
@@ -510,38 +441,25 @@ static int seg_prepare(dg_seg* h, const Tensors& t) {
       hh[d] = t.get("lstm.weight_hh" + sfx, 512 * 128);
       if (!wi || !bi || !bh || !hh[d]) return DG_EWEIGHT;
       for (int r = 0; r < 512; r++) {
-        for (int c = 0; c < in; c++) w[(size_t)c * 1024 + d * 512 + r] = wi[(size_t)r * in + c];
+        for (int c = 0; c < in; c++) w_nk[(size_t)(d * 512 + r) * in_pad + c] = wi[(size_t)r * in + c];
         b[d * 512 + r] = bi[r] + bh[r];
       }
     }
-    lstm_pack_whh(hh[0], hh[1], packed.data());
-    if (upload(h->wih[L], w) || upload(h->bih[L], b) || upload(h->whh[L], packed)) return DG_ECUDA;
-    std::vector<float> w_nk((size_t)1024 * in_pad, 0.f);
-    for (int n = 0; n < 1024; n++)
-      for (int c = 0; c < in; c++) w_nk[(size_t)n * in_pad + c] = w[(size_t)c * 1024 + n];
-    if (upload_split(h->wih_hi[L], h->wih_lo[L], w_nk, 1024, 1024, in_pad)) return DG_ECUDA;
+    if (upload(h->bih[L], b) || upload_split(h->wih_hi[L], h->wih_lo[L], w_nk, 1024, 1024, in_pad)) return DG_ECUDA;
     {
       std::vector<uint16_t> rh(lstm_tc_plane_elems()), rl(lstm_tc_plane_elems());
-      h->whh_hi[L].wscale = lstm_tc_pack_whh(hh[0], hh[1], rh.data(), rl.data(), split_f16());
+      h->whh_hi[L].wscale = lstm_tc_pack_whh(hh[0], hh[1], rh.data(), rl.data());
       if (upload_u16(h->whh_hi[L], rh) || upload_u16(h->whh_lo[L], rl)) return DG_ECUDA;
     }
   }
-  auto linear_t = [&](const std::string& name, int out, int in, DevBuf& dw, DevBuf& db) -> int {
-    const float* w = t.get(name + ".weight", (int64_t)out * in);
-    const float* b = t.get(name + ".bias", out);
-    if (!w || !b) return DG_EWEIGHT;
-    std::vector<float> wt((size_t)in * out), bv(b, b + out);
-    for (int o = 0; o < out; o++)
-      for (int c = 0; c < in; c++) wt[(size_t)c * out + o] = w[(size_t)o * in + c];
-    return (upload(dw, wt) || upload(db, bv)) ? DG_ECUDA : 0;
-  };
-  if ((rc = linear_t("linear.0", 128, 256, h->l1w, h->l1b)) || (rc = linear_t("linear.1", 128, 128, h->l2w, h->l2b)))
-    return rc;
   {
     const float* w0 = t.get("linear.0.weight", 128 * 256);
+    const float* b0 = t.get("linear.0.bias", 128);
     const float* w1 = t.get("linear.1.weight", 128 * 128);
-    if (!w0 || !w1) return DG_EWEIGHT;
-    if (upload_split(h->l1_hi, h->l1_lo, std::vector<float>(w0, w0 + 128 * 256), 128, 128, 256) ||
+    const float* b1 = t.get("linear.1.bias", 128);
+    if (!w0 || !b0 || !w1 || !b1) return DG_EWEIGHT;
+    if (upload(h->l1b, std::vector<float>(b0, b0 + 128)) || upload(h->l2b, std::vector<float>(b1, b1 + 128)) ||
+        upload_split(h->l1_hi, h->l1_lo, std::vector<float>(w0, w0 + 128 * 256), 128, 128, 256) ||
         upload_split(h->l2_hi, h->l2_lo, std::vector<float>(w1, w1 + 128 * 128), 128, 128, 128) ||
         upload(h->ones128, std::vector<float>(128, 1.f)) || upload(h->zeros128, std::vector<float>(128, 0.f)))
       return DG_ECUDA;
@@ -698,80 +616,37 @@ static int seg_forward_impl(dg_seg* h, const float* wav, int B, int S, float* se
   int rc;
   if ((rc = run_sincnet(h->sw, w.work, wav, B, g, st, h->shared_prep))) return rc;
   const size_t rows = (size_t)B * g.S2 + 64;
-  if (w.gx.ensure(rows * 1024 * 4) || w.hA.ensure(rows * 256 * 4) || w.hB.ensure(rows * 256 * 4) ||
-      w.y1.ensure(rows * 128 * 4) || w.y2.ensure(rows * 128 * 4))
+  if (w.gx.ensure(rows * 1024 * 4) || w.y2.ensure(rows * 128 * 4) || w.xh.ensure(rows * 256 * 2) ||
+      w.xl.ensure(rows * 256 * 2) || w.y1h.ensure(rows * 128 * 2) || w.y1l.ensure(rows * 128 * 2))
     return DG_ECUDA;
   const long long M = (long long)B * g.S2;
-  float* hin = nullptr;
-  float* hbuf[2] = {w.hA.as<float>(), w.hB.as<float>()};
-  const bool tc = use_tensor_cores();
-  if (tc && (w.xh.ensure(rows * 256 * 2) || w.xl.ensure(rows * 256 * 2))) return DG_ECUDA;
+  if ((rc = launch_split_ex(w.work.out, M, 64, 64, 64, w.work.out_pool, g.S2, w.work.sc2.as<float>(), w.work.sh2.as<float>(),
+                            w.xh.p, w.xl.p, st)))
+    return rc;
   for (int L = 0; L < 4; L++) {
-    if (tc) {
-      const int cin = L == 0 ? 64 : 256;
-      static const bool lstm_simt = getenv("DG_LSTM_SIMT") && getenv("DG_LSTM_SIMT")[0] == '1';
-      if (L == 0)
-        rc = launch_split_ex(w.work.out, M, 64, 64, 64, w.work.out_pool, g.S2, w.work.sc2.as<float>(),
-                             w.work.sh2.as<float>(), w.xh.p, w.xl.p, st);
-      else if (lstm_simt)
-        rc = launch_split(hin, M, 256, g.S2, nullptr, nullptr, w.xh.p, w.xl.p, st);
-      if (rc) return rc;
-      TcGemm t{};
-      t.A_hi = w.xh.p; t.A_lo = w.xl.p; t.lda = cin; t.Cin = cin; t.KW = 1; t.dil = 1; t.Mtot = M; t.M = M;
-      t.W_hi = h->wih_hi[L].p; t.w_scale = h->wih_hi[L].wscale; t.W_lo = h->wih_lo[L].p; t.Npad = 1024; t.N = 1024; t.bias = h->bih[L].as<float>();
-      t.out_f32 = w.gx.as<float>(); t.ldc = 1024; t.epi = 0; t.tag = "lstm_inproj";
-      if ((rc = launch_gemm_tc(t, st))) return rc;
-      float* hout = hbuf[L & 1];
-      // the tensor-core recurrence writes h_t straight into the operand planes of the next GEMM (the in-projection that
-      // read them has completed in stream order); the SIMT recurrence (DG_LSTM_SIMT=1) goes through float32 + split
-      if (lstm_simt)
-        rc = launch_lstm_layer(w.gx.as<float>(), h->whh[L].as<float>(), B, g.T2, g.S2, hout, st);
-      else
-        rc = launch_lstm_layer_tc(w.gx.as<float>(), h->whh_hi[L].p, h->whh_lo[L].p, h->whh_hi[L].wscale, B, g.T2, g.S2, nullptr, w.xh.p, w.xl.p, st);
-      if (rc) return rc;
-      hin = hout;
-      continue;
-    }
-    GemmArgs a{};
-    if (L == 0) {
-      a.A = w.work.p2.as<float>(); a.lda = 64; a.Cin = 64;
-      a.in_sc = w.work.sc2.as<float>(); a.in_sh = w.work.sh2.as<float>(); a.item_rows = g.S2;
-    } else {
-      a.A = hin; a.lda = 256; a.Cin = 256;
-    }
-    a.KW = 1; a.dil = 1; a.Mtot = M; a.M = M;
-    a.W = h->wih[L].as<float>(); a.ldw = 1024; a.N = 1024; a.bias = h->bih[L].as<float>();
-    a.C = w.gx.as<float>(); a.ldc = 1024; a.epi = EPI_BIAS; a.tag = "lstm_inproj";
-    if ((rc = launch_gemm(a, st))) return rc;
-    float* hout = hbuf[L & 1];
-    if ((rc = launch_lstm_layer(w.gx.as<float>(), h->whh[L].as<float>(), B, g.T2, g.S2, hout, st))) return rc;
-    hin = hout;
-  }
-  if (tc) {
-    // Linear(256,128) -> leaky -> Linear(128,128) -> leaky on the tensor-core GEMM (identity "BatchNorm")
-    if (w.y1h.ensure(rows * 128 * 2) || w.y1l.ensure(rows * 128 * 2)) return DG_ECUDA;
-    static const bool lstm_simt2 = getenv("DG_LSTM_SIMT") && getenv("DG_LSTM_SIMT")[0] == '1';
-    if (lstm_simt2 && (rc = launch_split(hin, M, 256, g.S2, nullptr, nullptr, w.xh.p, w.xl.p, st))) return rc;
+    const int cin = L == 0 ? 64 : 256;
     TcGemm t{};
-    t.A_hi = w.xh.p; t.A_lo = w.xl.p; t.lda = 256; t.Cin = 256; t.KW = 1; t.dil = 1; t.Mtot = M; t.M = M;
-    t.W_hi = h->l1_hi.p; t.w_scale = h->l1_hi.wscale; t.W_lo = h->l1_lo.p; t.Npad = 128; t.N = 128; t.bias = h->l1b.as<float>();
-    t.bn_scale = h->ones128.as<float>(); t.bn_shift = h->zeros128.as<float>();
-    t.out_hi = w.y1h.p; t.out_lo = w.y1l.p; t.ldc = 128; t.epi = 1; t.tag = "seg_linear";
+    t.A_hi = w.xh.p; t.A_lo = w.xl.p; t.lda = cin; t.Cin = cin; t.KW = 1; t.dil = 1; t.Mtot = M; t.M = M;
+    t.W_hi = h->wih_hi[L].p; t.w_scale = h->wih_hi[L].wscale; t.W_lo = h->wih_lo[L].p; t.Npad = 1024; t.N = 1024; t.bias = h->bih[L].as<float>();
+    t.out_f32 = w.gx.as<float>(); t.ldc = 1024; t.epi = 0; t.tag = "lstm_inproj";
     if ((rc = launch_gemm_tc(t, st))) return rc;
-    t.A_hi = w.y1h.p; t.A_lo = w.y1l.p; t.lda = 128; t.Cin = 128;
-    t.W_hi = h->l2_hi.p; t.w_scale = h->l2_hi.wscale; t.W_lo = h->l2_lo.p; t.bias = h->l2b.as<float>();
-    t.out_hi = nullptr; t.out_lo = nullptr; t.out_f32 = w.y2.as<float>(); t.epi = 2;
-    if ((rc = launch_gemm_tc(t, st))) return rc;
-    return seg_head_final(h, w.y2.as<float>(), B, g, seg, st);
+    // the recurrence writes h_t straight into the operand planes of the next GEMM (the in-projection that read them has
+    // completed in stream order)
+    if ((rc = launch_lstm_layer_tc(w.gx.as<float>(), h->whh_hi[L].p, h->whh_lo[L].p, h->whh_hi[L].wscale, B, g.T2, g.S2, nullptr,
+                                   w.xh.p, w.xl.p, st)))
+      return rc;
   }
-  GemmArgs a{};
-  a.A = hin; a.lda = 256; a.Cin = 256; a.KW = 1; a.dil = 1; a.Mtot = M; a.M = M;
-  a.W = h->l1w.as<float>(); a.ldw = 128; a.N = 128; a.bias = h->l1b.as<float>();
-  a.C = w.y1.as<float>(); a.ldc = 128; a.epi = EPI_BIAS_LEAKY; a.tag = "seg_linear";
-  if ((rc = launch_gemm(a, st))) return rc;
-  a.A = w.y1.as<float>(); a.lda = 128; a.Cin = 128;
-  a.W = h->l2w.as<float>(); a.bias = h->l2b.as<float>(); a.C = w.y2.as<float>();
-  if ((rc = launch_gemm(a, st))) return rc;
+  // Linear(256,128) -> leaky -> Linear(128,128) -> leaky on the tensor-core GEMM (identity "BatchNorm")
+  TcGemm t{};
+  t.A_hi = w.xh.p; t.A_lo = w.xl.p; t.lda = 256; t.Cin = 256; t.KW = 1; t.dil = 1; t.Mtot = M; t.M = M;
+  t.W_hi = h->l1_hi.p; t.w_scale = h->l1_hi.wscale; t.W_lo = h->l1_lo.p; t.Npad = 128; t.N = 128; t.bias = h->l1b.as<float>();
+  t.bn_scale = h->ones128.as<float>(); t.bn_shift = h->zeros128.as<float>();
+  t.out_hi = w.y1h.p; t.out_lo = w.y1l.p; t.ldc = 128; t.epi = 1; t.tag = "seg_linear";
+  if ((rc = launch_gemm_tc(t, st))) return rc;
+  t.A_hi = w.y1h.p; t.A_lo = w.y1l.p; t.lda = 128; t.Cin = 128;
+  t.W_hi = h->l2_hi.p; t.w_scale = h->l2_hi.wscale; t.W_lo = h->l2_lo.p; t.bias = h->l2b.as<float>();
+  t.out_hi = nullptr; t.out_lo = nullptr; t.out_f32 = w.y2.as<float>(); t.epi = 2;
+  if ((rc = launch_gemm_tc(t, st))) return rc;
   return seg_head_final(h, w.y2.as<float>(), B, g, seg, st);
 }
 
@@ -784,14 +659,14 @@ extern "C" int dg_seg_destroy(dg_seg* h) {
 struct dg_emb {
   int device = 0, pool_mode = 31, D = 512;
   SincWeights sw;
-  DevBuf tw[5], tb[5], bns[5], bnh[5];
-  DevBuf tw_hi[5], tw_lo[5];             // bf16 hi/lo planes [Npad][K] for the tensor-core path
+  DevBuf tb[5], bns[5], bnh[5];
+  DevBuf tw_hi[5], tw_lo[5];             // TDNN weights as fp16 hi/lo planes [Npad][K]
   DevBuf ew_hi, ew_lo, ph, pl;           // Linear(3000, D): weights [Dpad][3008], pooled statistics planes
-  DevBuf xh, xl, aH, aL, bH, bL;         // bf16 hi/lo activation planes
-  DevBuf ew, eb;
+  DevBuf xh, xl, aH, aL, bH, bL;         // fp16 hi/lo activation planes
+  DevBuf eb;
   SincWork work;
   UseGuard guard;
-  DevBuf tA, tB, t5, pooled, eraw;
+  DevBuf t5, pooled, eraw;
   DevBuf idx0, idx1, lam1;
   int tab_F = -1, tab_T = -1;
   DevBuf flags, uniq, grp, gathered;   // compatibility path
@@ -850,15 +725,13 @@ static int emb_prepare(dg_emb* h, const Tensors& t) {
     const float* rm = t.get(bn + ".running_mean", out);
     const float* rv = t.get(bn + ".running_var", out);
     if (!w || !b || !gm || !bt || !rm || !rv) return DG_EWEIGHT;
-    std::vector<float> wt((size_t)k * in_pad * out, 0.f), bv(b, b + out), sc(out), sf(out);
+    std::vector<float> bv(b, b + out), sc(out), sf(out);
     for (int o = 0; o < out; o++) {
-      for (int c = 0; c < in; c++)
-        for (int j = 0; j < k; j++) wt[((size_t)j * in_pad + c) * out + o] = w[((size_t)o * in + c) * k + j];
       // BatchNorm1d(eval): (x - mean) / sqrt(var + 1e-5) * gamma + beta  ==  x * sc + sf
       sc[o] = gm[o] / sqrtf(rv[o] + 1e-5f);
       sf[o] = bt[o] - rm[o] * sc[o];
     }
-    if (upload(h->tw[L], wt) || upload(h->tb[L], bv) || upload(h->bns[L], sc) || upload(h->bnh[L], sf)) return DG_ECUDA;
+    if (upload(h->tb[L], bv) || upload(h->bns[L], sc) || upload(h->bnh[L], sf)) return DG_ECUDA;
     {
       const int K = k * in_pad, npad = (out + 255) / 256 * 256;
       std::vector<float> w_nk((size_t)out * K, 0.f);
@@ -879,10 +752,7 @@ static int emb_prepare(dg_emb* h, const Tensors& t) {
   const float* ew = t.get("embedding.weight", dn * 3000);
   const float* eb = t.get("embedding.bias", dn);
   if (!ew || !eb) return DG_EWEIGHT;
-  std::vector<float> wt((size_t)3000 * dn);
-  for (int o = 0; o < dn; o++)
-    for (int c = 0; c < 3000; c++) wt[(size_t)c * dn + o] = ew[(size_t)o * 3000 + c];
-  if (upload(h->ew, wt) || upload(h->eb, std::vector<float>(eb, eb + dn))) return DG_ECUDA;
+  if (upload(h->eb, std::vector<float>(eb, eb + dn))) return DG_ECUDA;
   {
     std::vector<float> w_nk((size_t)dn * 3008, 0.f);
     for (int o = 0; o < dn; o++) memcpy(&w_nk[(size_t)o * 3008], ew + (size_t)o * 3000, 3000 * sizeof(float));
@@ -1170,7 +1040,7 @@ extern "C" int dg_emb_debug_trunk(dg_emb* h, const float* wav_dev, int U, int S,
     std::vector<uint16_t> hi(rows * C), lo(rows * C);
     DG_CUDA(cudaMemcpy(hi.data(), r.act[s][r.dbg_buf][0].p, rows * C * 2, cudaMemcpyDeviceToHost));
     DG_CUDA(cudaMemcpy(lo.data(), r.act[s][r.dbg_buf][1].p, rows * C * 2, cudaMemcpyDeviceToHost));
-    for (size_t i = 0; i < rows * C; i++) full[i] = host_h16_to_f32(hi[i], split_f16()) + host_h16_to_f32(lo[i], split_f16());
+    for (size_t i = 0; i < rows * C; i++) full[i] = host_h16_to_f32(hi[i]) + host_h16_to_f32(lo[i]);
   }
   for (int u = 0; u < U; u++)
     for (int w = 0; w < W; w++)
@@ -1249,80 +1119,49 @@ static int build_tables(dg_emb* h, int F, int T, cudaStream_t st) {
   return 0;
 }
 
-// waveform [U,S] -> t5 [U*S2, 1500]; returns the number of valid frames
-// DG_NO_POOL_FUSE=1: A/B switch, TDNN5 writes its map and stats_pool reads it back (the round-1 path)
-static bool pool_fusion_on() {
-  static const bool off = getenv("DG_NO_POOL_FUSE") && getenv("DG_NO_POOL_FUSE")[0] == '1';
-  return !off && use_tensor_cores();
-}
-
+// waveform [U,S] -> t5 [U*S2, 1500]; returns the number of valid frames.
 // `defer_last`: stop before TDNN5 (its operand planes are left in h->t4h / t4l) -- the caller runs it fused with the pooling
 static int emb_trunk(dg_emb* h, const float* wav, int U, const Geom& g, cudaStream_t st, int* T_out, bool defer_last = false) {
   int rc;
   if (h->variant == 1) return resnet_trunk(h, wav, U, g.S, st, T_out);
   if ((rc = run_sincnet(h->sw, h->work, wav, U, g, st, h->shared_prep))) return rc;
   const size_t rows = (size_t)U * g.S2 + 64;
-  if (h->tA.ensure(rows * 512 * 4) || h->tB.ensure(rows * 512 * 4) || h->t5.ensure(rows * 1500 * 4)) return DG_ECUDA;
+  if (h->t5.ensure(rows * 1500 * 4)) return DG_ECUDA;
   h->pool_x = h->t5.as<float>();
   h->pool_item_pitch = (long long)g.S2 * 1500;
   h->pool_row_pitch = 1500;
   h->pool_C = 1500;
   const long long M = (long long)U * g.S2;
-  if (use_tensor_cores()) {
-    if (h->xh.ensure(rows * 64 * 2) || h->xl.ensure(rows * 64 * 2) || h->aH.ensure(rows * 512 * 2) ||
-        h->aL.ensure(rows * 512 * 2) || h->bH.ensure(rows * 512 * 2) || h->bL.ensure(rows * 512 * 2))
-      return DG_ECUDA;
-    if ((rc = launch_split_ex(h->work.out, M, 64, 64, 64, h->work.out_pool, g.S2, h->work.sc2.as<float>(),
-                              h->work.sh2.as<float>(), h->xh.p, h->xl.p, st)))
-      return rc;
-    const void *ih = h->xh.p, *il = h->xl.p;
-    int cin = 64, T = g.T2;
-    void* oh[2] = {h->aH.p, h->bH.p};
-    void* ol[2] = {h->aL.p, h->bL.p};
-    static const char* kTags[5] = {"tdnn1", "tdnn2", "tdnn3", "tdnn4", "tdnn5"};
-    for (int L = 0; L < 5; L++) {
-      if (L == 4 && defer_last) {
-        h->t4h = ih;
-        h->t4l = il;
-        T -= (TD_K[L] - 1) * TD_DIL[L];
-        break;
-      }
-      TcGemm t{};
-      t.A_hi = ih; t.A_lo = il; t.lda = cin; t.Cin = cin; t.KW = TD_K[L]; t.dil = TD_DIL[L]; t.Mtot = M; t.M = M;
-      t.W_hi = h->tw_hi[L].p; t.w_scale = h->tw_hi[L].wscale; t.W_lo = h->tw_lo[L].p; t.Npad = (TD_OUT[L] + 255) / 256 * 256; t.N = TD_OUT[L];
-      t.bias = h->tb[L].as<float>(); t.bn_scale = h->bns[L].as<float>(); t.bn_shift = h->bnh[L].as<float>();
-      t.tag = kTags[L];
-      if (L == 4) {
-        t.out_f32 = h->t5.as<float>(); t.ldc = 1500; t.epi = 2;
-      } else {
-        t.out_hi = oh[L & 1]; t.out_lo = ol[L & 1]; t.ldc = 512; t.epi = 1;
-      }
-      if ((rc = launch_gemm_tc(t, st))) return rc;
-      ih = oh[L & 1]; il = ol[L & 1];
-      cin = TD_OUT[L];
-      T -= (TD_K[L] - 1) * TD_DIL[L];
-    }
-    *T_out = T;
-    return 0;
-  }
-  const float* in = h->work.p2.as<float>();
+  if (h->xh.ensure(rows * 64 * 2) || h->xl.ensure(rows * 64 * 2) || h->aH.ensure(rows * 512 * 2) ||
+      h->aL.ensure(rows * 512 * 2) || h->bH.ensure(rows * 512 * 2) || h->bL.ensure(rows * 512 * 2))
+    return DG_ECUDA;
+  if ((rc = launch_split_ex(h->work.out, M, 64, 64, 64, h->work.out_pool, g.S2, h->work.sc2.as<float>(),
+                            h->work.sh2.as<float>(), h->xh.p, h->xl.p, st)))
+    return rc;
+  const void *ih = h->xh.p, *il = h->xl.p;
   int cin = 64, T = g.T2;
-  float* bufs[2] = {h->tA.as<float>(), h->tB.as<float>()};
+  void* oh[2] = {h->aH.p, h->bH.p};
+  void* ol[2] = {h->aL.p, h->bL.p};
+  static const char* kTags[5] = {"tdnn1", "tdnn2", "tdnn3", "tdnn4", "tdnn5"};
   for (int L = 0; L < 5; L++) {
-    GemmArgs a{};
-    a.A = in; a.lda = cin; a.Cin = cin; a.KW = TD_K[L]; a.dil = TD_DIL[L];
-    a.Mtot = M; a.M = M;
-    a.W = h->tw[L].as<float>(); a.ldw = TD_OUT[L]; a.N = TD_OUT[L]; a.bias = h->tb[L].as<float>();
-    a.bn_scale = h->bns[L].as<float>(); a.bn_shift = h->bnh[L].as<float>();
-    if (L == 0) {
-      a.in_sc = h->work.sc2.as<float>(); a.in_sh = h->work.sh2.as<float>(); a.item_rows = g.S2;
+    if (L == 4 && defer_last) {
+      h->t4h = ih;
+      h->t4l = il;
+      T -= (TD_K[L] - 1) * TD_DIL[L];
+      break;
     }
-    float* out = L == 4 ? h->t5.as<float>() : bufs[L & 1];
-    a.C = out; a.ldc = TD_OUT[L]; a.epi = EPI_BIAS_LEAKY_BN;
-    static const char* kTags[5] = {"tdnn1", "tdnn2", "tdnn3", "tdnn4", "tdnn5"};
-    a.tag = kTags[L];
-    if ((rc = launch_gemm(a, st))) return rc;
-    in = out;
+    TcGemm t{};
+    t.A_hi = ih; t.A_lo = il; t.lda = cin; t.Cin = cin; t.KW = TD_K[L]; t.dil = TD_DIL[L]; t.Mtot = M; t.M = M;
+    t.W_hi = h->tw_hi[L].p; t.w_scale = h->tw_hi[L].wscale; t.W_lo = h->tw_lo[L].p; t.Npad = (TD_OUT[L] + 255) / 256 * 256; t.N = TD_OUT[L];
+    t.bias = h->tb[L].as<float>(); t.bn_scale = h->bns[L].as<float>(); t.bn_shift = h->bnh[L].as<float>();
+    t.tag = kTags[L];
+    if (L == 4) {
+      t.out_f32 = h->t5.as<float>(); t.ldc = 1500; t.epi = 2;
+    } else {
+      t.out_hi = oh[L & 1]; t.out_lo = ol[L & 1]; t.ldc = 512; t.epi = 1;
+    }
+    if ((rc = launch_gemm_tc(t, st))) return rc;
+    ih = oh[L & 1]; il = ol[L & 1];
     cin = TD_OUT[L];
     T -= (TD_K[L] - 1) * TD_DIL[L];
   }
@@ -1356,37 +1195,22 @@ static int emb_tdnn5_pool(dg_emb* h, int U, const Geom& g, const float* weights,
 }
 
 static int emb_project(dg_emb* h, int rows, int normalize, float norm, float* out, cudaStream_t st) {
-  if (use_tensor_cores() || h->variant == 1) {
-    int rc;
-    const int nfeat = 2 * h->pool_C, kpad = (nfeat + 63) / 64 * 64;     // 3000 -> 3008, 5120 -> 5120
-    if (h->ph.ensure(((size_t)rows + 128) * kpad * 2) || h->pl.ensure(((size_t)rows + 128) * kpad * 2)) return DG_ECUDA;
-    if ((rc = launch_split_ex(h->pooled.as<float>(), rows, nfeat, nfeat, kpad, 0, 1, nullptr, nullptr, h->ph.p, h->pl.p, st)))
-      return rc;
-    float* dst = out;
-    if (normalize) {
-      if (h->eraw.ensure((size_t)rows * h->D * 4)) return DG_ECUDA;
-      dst = h->eraw.as<float>();
-    }
-    TcGemm t{};
-    t.A_hi = h->ph.p; t.A_lo = h->pl.p; t.lda = kpad; t.Cin = kpad; t.KW = 1; t.dil = 1; t.Mtot = rows; t.M = rows;
-    t.W_hi = h->ew_hi.p; t.w_scale = h->ew_hi.wscale; t.W_lo = h->ew_lo.p; t.Npad = (h->D + 255) / 256 * 256; t.N = h->D;
-    t.bias = h->eb.as<float>(); t.out_f32 = dst; t.ldc = h->D; t.epi = 0; t.tag = "emb_linear";
-    if ((rc = launch_gemm_tc(t, st))) return rc;
-    return normalize ? launch_l2norm(dst, rows, h->D, norm, out, st) : 0;
-  }
-  GemmArgs a{};
-  a.A = h->pooled.as<float>(); a.lda = 3000; a.Cin = 3000; a.KW = 1; a.dil = 1; a.Mtot = rows; a.M = rows;
-  a.W = h->ew.as<float>(); a.ldw = h->D; a.N = h->D; a.bias = h->eb.as<float>();
-  a.ldc = h->D; a.epi = EPI_BIAS; a.tag = "emb_linear";
-  if (!normalize) {
-    a.C = out;
-    return launch_gemm(a, st);
-  }
-  if (h->eraw.ensure((size_t)rows * h->D * 4)) return DG_ECUDA;
-  a.C = h->eraw.as<float>();
   int rc;
-  if ((rc = launch_gemm(a, st))) return rc;
-  return launch_l2norm(h->eraw.as<float>(), rows, h->D, norm, out, st);
+  const int nfeat = 2 * h->pool_C, kpad = (nfeat + 63) / 64 * 64;     // 3000 -> 3008, 5120 -> 5120
+  if (h->ph.ensure(((size_t)rows + 128) * kpad * 2) || h->pl.ensure(((size_t)rows + 128) * kpad * 2)) return DG_ECUDA;
+  if ((rc = launch_split_ex(h->pooled.as<float>(), rows, nfeat, nfeat, kpad, 0, 1, nullptr, nullptr, h->ph.p, h->pl.p, st)))
+    return rc;
+  float* dst = out;
+  if (normalize) {
+    if (h->eraw.ensure((size_t)rows * h->D * 4)) return DG_ECUDA;
+    dst = h->eraw.as<float>();
+  }
+  TcGemm t{};
+  t.A_hi = h->ph.p; t.A_lo = h->pl.p; t.lda = kpad; t.Cin = kpad; t.KW = 1; t.dil = 1; t.Mtot = rows; t.M = rows;
+  t.W_hi = h->ew_hi.p; t.w_scale = h->ew_hi.wscale; t.W_lo = h->ew_lo.p; t.Npad = (h->D + 255) / 256 * 256; t.N = h->D;
+  t.bias = h->eb.as<float>(); t.out_f32 = dst; t.ldc = h->D; t.epi = 0; t.tag = "emb_linear";
+  if ((rc = launch_gemm_tc(t, st))) return rc;
+  return normalize ? launch_l2norm(dst, rows, h->D, norm, out, st) : 0;
 }
 
 extern "C" int dg_emb_forward(dg_emb* h, const float* wav, const float* weights, int B, int S, int F, int K,
@@ -1405,7 +1229,7 @@ extern "C" int dg_emb_forward(dg_emb* h, const float* wav, const float* weights,
     ~Done() { if (on) use_end(h->guard, me, st); }
   } done{h, me, st, !g_in_pipeline};
   if (!g_in_pipeline && (rc = use_begin(h->guard, me, st))) return rc;
-  const bool fuse = weights && h->variant == 0 && K <= 4 && g.S2 >= 128 && pool_fusion_on();
+  const bool fuse = weights && h->variant == 0 && K <= 4 && g.S2 >= 128;
   if ((rc = emb_trunk(h, wav, B, g, st, &T, fuse))) return rc;
   if (weights && (rc = build_tables(h, F, T, st))) return rc;
   if (fuse) {
@@ -1637,19 +1461,19 @@ extern "C" int dg_cluster_merge(dg_cluster* h, const double* records_dev, int wo
 }
 
 // ================================================================================== self test
-extern "C" int dg_selftest_split_host(const float* x, long long n, int f16, unsigned short* hi, unsigned short* lo) {
+extern "C" int dg_selftest_split_f16_host(const float* x, long long n, unsigned short* hi, unsigned short* lo) {
   if (!x || !hi || !lo || n < 0) {
-    set_error("dg_selftest_split_host: null argument");
+    set_error("dg_selftest_split_f16_host: null argument");
     return DG_EINVAL;
   }
   for (long long i = 0; i < n; i++) {
-    hi[i] = host_f32_to_h16(x[i], f16);
-    lo[i] = host_f32_to_h16(x[i] - host_h16_to_f32(hi[i], f16), f16);
+    hi[i] = host_f32_to_h16(x[i]);
+    lo[i] = host_f32_to_h16(x[i] - host_h16_to_f32(hi[i]));
   }
   return DG_OK;
 }
 
-// Runs the same shifted-window GEMM through the float32 SIMT kernel and through the wgmma split-precision
+// Runs the same shifted-window GEMM through the float32 reference kernel (gemm.cu) and through the wgmma split-precision
 // kernel on seeded random data and reports the largest absolute difference and the output scale.
 extern "C" int dg_selftest_gemm_tc(int M, int Cin, int KW, int dil, int N, int epi, float* max_abs_diff,
                                    float* out_rms) {
@@ -1693,7 +1517,7 @@ extern "C" int dg_selftest_gemm_tc(int M, int Cin, int KW, int dil, int N, int e
   g.bn_shift = dH.as<float>(); g.C = dC0.as<float>(); g.ldc = N; g.epi = epi == 0 ? EPI_BIAS : EPI_BIAS_LEAKY_BN;
   g.tag = "selftest_simt";
   if ((rc = launch_gemm(g, nullptr))) return rc;
-  if ((rc = launch_split(dA.as<float>(), Mtot, Cin, 1, nullptr, nullptr, dAh.p, dAl.p, nullptr))) return rc;
+  if ((rc = launch_split_ex(dA.as<float>(), Mtot, Cin, Cin, Cin, 0, 1, nullptr, nullptr, dAh.p, dAl.p, nullptr))) return rc;
   TcGemm t{};
   t.A_hi = dAh.p; t.A_lo = dAl.p; t.lda = Cin; t.Cin = Cin; t.KW = KW; t.dil = dil; t.Mtot = Mtot; t.M = M;
   t.W_hi = dWh.p; t.w_scale = dWh.wscale; t.W_lo = dWl.p; t.Npad = npad; t.N = N; t.bias = dB.as<float>(); t.bn_scale = dS.as<float>();
@@ -1709,7 +1533,7 @@ extern "C" int dg_selftest_gemm_tc(int M, int Cin, int KW, int dil, int N, int e
     ol.resize((size_t)M * N);
     DG_CUDA(cudaMemcpy(oh.data(), dOh.p, oh.size() * 2, cudaMemcpyDeviceToHost));
     DG_CUDA(cudaMemcpy(ol.data(), dOl.p, ol.size() * 2, cudaMemcpyDeviceToHost));
-    for (size_t i = 0; i < c1.size(); i++) c1[i] = host_h16_to_f32(oh[i], split_f16()) + host_h16_to_f32(ol[i], split_f16());
+    for (size_t i = 0; i < c1.size(); i++) c1[i] = host_h16_to_f32(oh[i]) + host_h16_to_f32(ol[i]);
   } else {
     DG_CUDA(cudaMemcpy(c1.data(), dC1.p, c1.size() * 4, cudaMemcpyDeviceToHost));
   }
@@ -1917,19 +1741,15 @@ static int pipeline_nets(dg_pipeline* h, const float* wav, int B, int S, int F, 
     InPipeline() { g_in_pipeline = true; }
     ~InPipeline() { g_in_pipeline = false; }
   } in_pipeline;
-  // waveform statistics + standardised 16-bit planes once, for both networks' SincNets
-  static const bool sinc_simt = getenv("DG_SINC_SIMT") && getenv("DG_SINC_SIMT")[0] == '1';
-  const SincPrep* shared = nullptr;
-  if (!sinc_simt) {
-    if ((rc = run_sinc_prep(h->prep[lane], wav, B, g, s_seg, stream_hop ? stream_hop : h->hop, stream_hop != 0))) return rc;
-    DG_CUDA(cudaEventRecord(h->e_prep[lane], s_seg));
-    DG_DIAG(prep, s_seg);
-    DG_CUDA(cudaStreamWaitEvent(h->s_emb, h->e_prep[lane], 0));
-    shared = &h->prep[lane];
-  }
+  // waveform statistics + standardised fp16 planes once, for both networks' SincNets
+  if ((rc = run_sinc_prep(h->prep[lane], wav, B, g, s_seg, stream_hop ? stream_hop : h->hop, stream_hop != 0))) return rc;
+  DG_CUDA(cudaEventRecord(h->e_prep[lane], s_seg));
+  DG_DIAG(prep, s_seg);
+  DG_CUDA(cudaStreamWaitEvent(h->s_emb, h->e_prep[lane], 0));
+  const SincPrep* shared = &h->prep[lane];
   // embedding trunk first in host order (low-priority stream, grid capped to the SMs the LSTM leaves free)
   int T = 0;
-  const bool fuse_pool = h->emb->variant == 0 && K <= 4 && g.S2 >= 128 && pool_fusion_on();
+  const bool fuse_pool = h->emb->variant == 0 && K <= 4 && g.S2 >= 128;
   {
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->seg->device);
@@ -2002,8 +1822,9 @@ extern "C" int dg_pipeline_step(dg_pipeline* h, const float* wav, int B, int S, 
   int rc, F = 0, K = 0;
   if ((rc = dg_seg_dims(h->seg, S, &F, &K))) return rc;
   if (h->osp.ensure((size_t)B * F * K * 4)) return DG_ECUDA;
+  // DG_NO_OVERLAP=1 (diagnostic): the networks and the clustering back to back on `stream`, for kernel-alone timings
   static const bool serial = getenv("DG_NO_OVERLAP") && getenv("DG_NO_OVERLAP")[0] == '1';
-  if (serial || !use_tensor_cores()) {
+  if (serial) {
     if ((rc = dg_seg_forward(h->seg, wav, B, S, seg, stream))) return rc;
     if ((rc = dg_osp(seg, B, F, K, h->gamma, h->beta, h->normalize_weights, h->osp.as<float>(), stream))) return rc;
     if ((rc = dg_emb_forward(h->emb, wav, h->osp.as<float>(), B, S, F, K, 1, 1.f, emb, stream))) return rc;
@@ -2456,22 +2277,23 @@ extern "C" int dg_post_step(dg_post* h, const float* seg_dev, const int32_t* map
   return post_finish(h, B, header_host, turns_host, turn_cap_host, n_turns, st);
 }
 
+// worker threads of the host gather, created at the first dg_pipeline_call_host: all cores but two, at most 24
+static GatherPool& gather_pool(dg_pipeline* h) {
+  if (!h->gather) h->gather.reset(new GatherPool(std::max(1, std::min((int)std::thread::hardware_concurrency() - 2, 24))));
+  return *h->gather;
+}
+
 // ---- the whole body of SpeakerDiarization.__call__ (reference diarization.py:172-232) in one call: B separate host windows
 //      (as rearrange_audio_stream emits them) are gathered into pinned staging by worker threads while earlier rows are
 //      already on their way to the device, then fused step + post-path, one D2H of the turn list.
 static int upload_rows(dg_pipeline* h, const float* const* rows, int B, int S, float* pin, float* dst_dev, cudaStream_t st) {
   const int R = 4;                                    // rows per work item (1.3 MB at S = 80000)
   const int items = (B + R - 1) / R;
-  if (!h->gather) {
-    int n = (int)std::thread::hardware_concurrency();
-    static const int env_threads = getenv("DG_GATHER_THREADS") ? atoi(getenv("DG_GATHER_THREADS")) : 0;
-    n = env_threads > 0 ? env_threads : std::max(1, std::min(n - 2, 24));
-    h->gather.reset(new GatherPool(n));
-  }
+  GatherPool& pool = gather_pool(h);
   std::vector<std::atomic<int>> done(items);
   for (auto& d : done) d.store(0, std::memory_order_relaxed);
   std::atomic<int> next{0};
-  h->gather->start([&]() {
+  pool.start([&]() {
     for (;;) {
       const int it = next.fetch_add(1, std::memory_order_relaxed);
       if (it >= items) return;
@@ -2495,7 +2317,7 @@ static int upload_rows(dg_pipeline* h, const float* const* rows, int B, int S, f
       err = cudaMemcpyAsync(dst_dev + (size_t)r0 * S, pin + (size_t)r0 * S, (size_t)(r1 - r0) * S * 4, cudaMemcpyHostToDevice, st);
     sent = upto;
   }
-  h->gather->wait();          // (`next` and `done` live on this frame)
+  pool.wait();          // (`next` and `done` live on this frame)
   DG_CUDA(err);
   return 0;
 }
@@ -2507,14 +2329,9 @@ static int upload_rows(dg_pipeline* h, const float* const* rows, int B, int S, f
 // stream (pin_stream[0 .. S + (r0 + nb - 1) hop) is then valid), 0 if some window does not (the caller falls back to the
 // full gather for this and the following sub-batches).
 static int pack_stream_rows(dg_pipeline* h, const float* const* rows, int r0, int nb, int S, int hop, float* pin_stream) {
-  if (!h->gather) {
-    int n = (int)std::thread::hardware_concurrency();
-    static const int env_threads = getenv("DG_GATHER_THREADS") ? atoi(getenv("DG_GATHER_THREADS")) : 0;
-    n = env_threads > 0 ? env_threads : std::max(1, std::min(n - 2, 24));
-    h->gather.reset(new GatherPool(n));
-  }
+  GatherPool& pool = gather_pool(h);
   std::atomic<int> next{r0}, bad{0};
-  h->gather->start([&]() {
+  pool.start([&]() {
     for (;;) {
       const int r = next.fetch_add(1, std::memory_order_relaxed);
       if (r >= r0 + nb || bad.load(std::memory_order_relaxed)) return;
@@ -2527,7 +2344,7 @@ static int pack_stream_rows(dg_pipeline* h, const float* const* rows, int r0, in
       }
     }
   });
-  h->gather->wait();
+  pool.wait();
   return bad.load() ? 0 : 1;
 }
 
@@ -2570,48 +2387,24 @@ extern "C" int dg_pipeline_call_host(dg_pipeline* h, dg_post* post, const float*
   }
   // The batch runs as up to three sub-batches through the pipelined machinery (dg_pipeline_submit_host): the upload of
   // sub-batch j+1 and its front end overlap the recurrence of sub-batch j; clustering stays in chunk order on its one stream,
-  // so the result is exactly that of one step over the whole batch.  DG_CALL_SPLIT = 1..3 (default 2 from 128 windows on).
-  // sub-batch sizes: DG_CALL_PLAN="n1,n2[,n3]" (windows; must add up to B) or DG_CALL_SPLIT = 1..3 equal parts; default
-  // from 192 windows on: three parts -- a short first one so that the device starts early and a short last one, because
-  // its dependent chain (1172 recurrence steps + its share of the clustering) is what the caller waits for at the end
+  // so the result is exactly that of one step over the whole batch.  From 64 windows on: two halves; from 192 windows on:
+  // three parts -- a short first one so that the device starts early and a short last one, because its dependent chain
+  // (1172 recurrence steps + its share of the clustering) is what the caller waits for at the end
   int plan[DG_MAX_INFLIGHT] = {B, 0, 0}, ns = 1;
-  {
-    static const int split_env = getenv("DG_CALL_SPLIT") ? atoi(getenv("DG_CALL_SPLIT")) : 0;
-    static const std::string plan_env = getenv("DG_CALL_PLAN") ? getenv("DG_CALL_PLAN") : "";
-    int vals[DG_MAX_INFLIGHT] = {0, 0, 0}, nv = 0, sum = 0;
-    if (!plan_env.empty()) {
-      std::stringstream ss(plan_env);
-      std::string tok;
-      while (nv < DG_MAX_INFLIGHT && std::getline(ss, tok, ',')) {
-        vals[nv] = atoi(tok.c_str());
-        sum += vals[nv];
-        if (vals[nv++] < 1) sum = -1 << 20;
-      }
-    }
-    if (nv > 0 && sum == B) {
-      ns = nv;
-      for (int j = 0; j < nv; j++) plan[j] = vals[j];
-    } else if (split_env > 0) {
-      ns = std::max(1, std::min({split_env, DG_MAX_INFLIGHT, B / 8 > 0 ? B / 8 : 1}));
-      const int Bs = (B + ns - 1) / ns;
-      for (int j = 0, left = B; j < ns; j++, left -= Bs) plan[j] = std::min(Bs, left);
-      while (ns > 1 && plan[ns - 1] <= 0) ns--;
-    } else if (B >= 192) {
-      ns = 3;
-      plan[0] = (B * 5 / 16 + 7) / 8 * 8;
-      plan[2] = (B * 4 / 16 + 7) / 8 * 8;
-      plan[1] = B - plan[0] - plan[2];
-    } else if (B >= 64) {
-      ns = 2;
-      plan[0] = (B / 2 + 7) / 8 * 8;
-      plan[1] = B - plan[0];
-    }
+  if (B >= 192) {
+    ns = 3;
+    plan[0] = (B * 5 / 16 + 7) / 8 * 8;
+    plan[2] = (B * 4 / 16 + 7) / 8 * 8;
+    plan[1] = B - plan[0] - plan[2];
+  } else if (B >= 64) {
+    ns = 2;
+    plan[0] = (B / 2 + 7) / 8 * 8;
+    plan[1] = B - plan[0];
   }
   // consecutive windows of one stream (hop known from dg_pipeline_set_hop): verified on the host, uploaded once (see
-  // pack_stream_rows); DG_CALL_NO_DEDUP=1 = always the full gather
-  static const bool no_dedup = getenv("DG_CALL_NO_DEDUP") && getenv("DG_CALL_NO_DEDUP")[0] == '1';
+  // pack_stream_rows)
   const int hop = h->hop;
-  bool as_stream = !no_dedup && hop > 0 && hop < S && hop % 4 == 0 && S % 4 == 0 && B >= 2;
+  bool as_stream = hop > 0 && hop < S && hop % 4 == 0 && S % 4 == 0 && B >= 2;
   const size_t stream_len = (size_t)S + (size_t)(B - 1) * (hop > 0 ? hop : 0);
   if (as_stream && h->call_stream.ensure((stream_len + 64) * 4)) return DG_ECUDA;
   float* pin = reinterpret_cast<float*>(h->pin_wav);

@@ -104,31 +104,26 @@ bool stream_stats_ok(int S, int hop);
 size_t stream_stats_doubles(int B, int S, int hop);
 int launch_stream_stats(const float* wav, int B, int S, int hop, double* part, float* mean, float* rstd, const int* flag,
                         cudaStream_t st);
-int launch_sinc0(const float* wav, const float* mean, const float* rstd, float wn_gamma, float wn_beta,
-                 const float* filt /*[251][80]*/, int B, const Geom& g, float* p0 /*[B,S0,80]*/, cudaStream_t st);
 int launch_instnorm_stats(const float* x, int B, int stride_rows, int T, int C, int ldc, const float* gamma,
                           const float* beta, float* sc, float* sh, cudaStream_t st, int pool = 0, const int* skip_flag = nullptr);
 int launch_instnorm_finalize(const float* part, int B, int item_rows, int tile_rows, int T, int C, int N, const float* bias,
                              const float* gamma, const float* beta, float* sc, float* sh, int ld, cudaStream_t st);
-// gemm.cu
-enum Epi { EPI_BIAS = 0, EPI_BIAS_LEAKY = 1, EPI_BIAS_LEAKY_BN = 2, EPI_BIAS_POOL3 = 3 };
+// gemm.cu -- float32 reference GEMM of the wgmma self-test (dg_selftest_gemm_tc)
+enum Epi { EPI_BIAS = 0, EPI_BIAS_LEAKY_BN = 2 };
 struct GemmArgs {
   const float* A;      // [Mrows_in, lda]
   int lda;             // channel stride of A (>= Cin)
   int Cin;             // channels consumed per tap (multiple of 4)
   int KW, dil;         // taps, dilation (rows)
   long long Mtot;      // rows of A that exist (reads past it return 0)
-  long long M;         // output rows to produce (before pooling)
+  long long M;         // output rows to produce
   const float* W;      // [KW*Cin, ldw]
   int ldw;             // column stride of W (>= N, multiple of 4)
   int N;               // valid output channels
   const float* bias;   // [N] or null
   const float* bn_scale;  // [N] (EPI_BIAS_LEAKY_BN)
   const float* bn_shift;
-  const float* in_sc;  // per-(item, channel) instance-norm scale/shift applied (+leaky) on load, or null
-  const float* in_sh;
-  int item_rows;       // rows per item (for in_sc indexing)
-  float* C;            // [M or M/3, ldc]
+  float* C;            // [M, ldc]
   int ldc;
   int epi;
   const char* tag;   // kernel label for profiling (layer name)
@@ -136,11 +131,11 @@ struct GemmArgs {
 int launch_gemm(const GemmArgs& a, cudaStream_t st);
 // gemm_tc.cu -- wgmma / TMA path (hi/lo split precision, three products)
 struct TcGemm {
-  const void* A_hi;    // bf16 [Mtot, lda]
+  const void* A_hi;    // fp16 [Mtot, lda]
   const void* A_lo;
   int lda, Cin, KW, dil;
   long long Mtot, M;
-  const void* W_hi;    // bf16 [Npad, KW*Cin]  (n-major: row n holds its K weights, tap-major)
+  const void* W_hi;    // fp16 [Npad, KW*Cin]  (n-major: row n holds its K weights, tap-major)
   const void* W_lo;
   float w_scale;       // power-of-two factor the W planes were multiplied by (0 = 1): undone on the accumulator
   int Npad, N;
@@ -148,7 +143,7 @@ struct TcGemm {
   const float* bn_scale;
   const float* bn_shift;
   float* out_f32;      // [M, ldc] (float32 epilogues)
-  void* out_hi;        // bf16 [M, ldc] (split epilogue)
+  void* out_hi;        // fp16 [M, ldc] (split epilogue)
   void* out_lo;
   int ldc;
   int epi;             // 0 bias -> f32, 1 bias+leaky+bn -> hi/lo planes, 2 bias+leaky+bn -> f32, 3 conv2d (see below)
@@ -179,20 +174,16 @@ inline int gemm_tc_pool3_tile_rows(int item_rows) {
   return 0;
 }
 int launch_gemm_tc(const TcGemm& g, cudaStream_t st);
-int launch_split(const float* x, long long rows, int C, int item_rows, const float* sc, const float* sh, void* hi,
-                 void* lo, cudaStream_t st);
 int launch_split_ex(const float* x, long long rows_out, int C, int ld_in, int ld_out, int pool, int item_rows,
                     const float* sc, const float* sh, void* hi, void* lo, cudaStream_t st, const int* skip_flag = nullptr);
-// element type of the 16-bit operand planes: 1 = fp16 (default), 0 = bf16 (DG_SPLIT_BF16=1); fixed at first use
-int split_f16();
-void split_weights_host(const float* w, int N, int Npad, int K, uint16_t* hi, uint16_t* lo, int f16, float scale = 1.f);
-float weight_plane_scale(const float* w, size_t n, int f16);   // power of two that keeps the lo plane of small weights normal
-uint16_t host_f32_to_h16(float f, int f16);
-float host_h16_to_f32(uint16_t h, int f16);
+void split_weights_host(const float* w, int N, int Npad, int K, uint16_t* hi, uint16_t* lo, float scale = 1.f);
+float weight_plane_scale(const float* w, size_t n);   // power of two that keeps the lo plane of small weights normal
+uint16_t host_f32_to_h16(float f);
+float host_h16_to_f32(uint16_t h);
 // sinc_tc.cu -- SincNet stage 0 on wgmma (overlapping-row TMA view of the waveform)
 int sinc_tc_rows_per_item(const Geom& g);
 size_t sinc_tc_plane_elems(int B, const Geom& g);
-void sinc_tc_pack_filters(const float* filt, uint16_t* planes /*[3][80][256]*/, int f16);
+void sinc_tc_pack_filters(const float* filt, uint16_t* planes /*[2][80][256]*/);
 void sinc_tc_affine_consts(const float* filt, float beta, float* cf);
 int launch_sinc_prep(const float* wav, const float* mean, const float* rstd, int B, const Geom& g, void* planes_hi,
                      void* planes_lo, cudaStream_t st, const int* skip_flag = nullptr);
@@ -211,21 +202,14 @@ int launch_stream_prep(const float* wav, int B, const Geom& g, int hop, void* pl
                        cudaStream_t st);
 int launch_sinc0_tc_stream(const void* w_planes, int B, const Geom& g, int hop, const void* planes_hi, const void* planes_lo,
                            float* craw, const int* flag, cudaStream_t st);
-int launch_sinc_pool(const float* craw, const float* mean, const float* rstd, const float* cf, const float* hsum, float gamma,
-                     int B, const Geom& g, int hop, float* p0, const int* flag, cudaStream_t st);
 size_t sinc_pool_part_floats(int B, const Geom& g, int hop);
 int launch_sinc_pool_fused(const float* craw, const float* mean, const float* rstd, const float* cf, const float* hsum, float gamma,
                            int B, const Geom& g, int hop, const float* g0, const float* b0, float* part, float* sc, float* sh,
                            void* planes_hi, void* planes_lo, const int* flag, cudaStream_t st);
-// lstm.cu
-int launch_lstm_layer(const float* gx /*[B*stride,1024]*/, const float* whh_packed, int B, int T, int stride,
-                      float* hout /*[B*stride,256]*/, cudaStream_t st);
-size_t lstm_whh_packed_floats();
-void lstm_pack_whh(const float* whh_fwd /*[512][128]*/, const float* whh_bwd, float* packed);
 // lstm_tc.cu -- recurrence on wgmma (W_hh hi plane in registers, lo plane in shared memory)
 size_t lstm_tc_plane_elems();
 int lstm_tc_ctas(int B);   // CTAs (= SMs) one recurrence launch occupies at batch B
-float lstm_tc_pack_whh(const float* whh_fwd, const float* whh_bwd, uint16_t* hi, uint16_t* lo, int f16);   // -> plane scale
+float lstm_tc_pack_whh(const float* whh_fwd, const float* whh_bwd, uint16_t* hi, uint16_t* lo);   // -> plane scale
 // hout (float32) and / or out_hi, out_lo (16-bit planes of the next GEMM's operand) receive h_t
 int launch_lstm_layer_tc(const float* gx, const void* whh_hi, const void* whh_lo, float w_scale, int B, int T, int stride,
                          float* hout, void* out_hi, void* out_lo, cudaStream_t st);

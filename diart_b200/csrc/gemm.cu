@@ -1,33 +1,28 @@
-// Shifted-window GEMM (fp32 SIMT): every dense layer of the path is
-//     C[m, n] = epi( sum_{j<KW} sum_{c<Cin} pro(A[m + j*dil, c]) * W[j*Cin + c, n] + bias[n] )
-// over the flattened time-major activation matrix (dg_common.cuh, Geom): Conv1d(80,60,5),
-// Conv1d(60,60,5) of SincNet, the LSTM input projections, the Linear layers of PyanNet's head, the
-// five TDNN layers of XVectorSincNet (dilated Conv1d -> LeakyReLU -> BatchNorm1d(eval)) and the
-// final Linear(3000,512).  `pro` is the previous InstanceNorm1d+LeakyReLU applied on load, `epi` one
-// of bias / bias+leaky / bias+leaky+BN / bias+MaxPool1d(3).
-// Restates pyannote.audio (SURVEY.md Appendix A.2-A.4); reached from the reference through
-// src/diart/models.py:131-133.
+// Shifted-window GEMM in float32 on the CUDA cores: the reference that dg_selftest_gemm_tc (tests/test_gpu_gemm_tc.py)
+// compares the wgmma split-precision GEMM of gemm_tc.cu against.  No network layer runs on it.
+//     C[m, n] = epi( sum_{j<KW} sum_{c<Cin} A[m + j*dil, c] * W[j*Cin + c, n] + bias[n] )
+// over a time-major activation matrix (dg_common.cuh, Geom); `epi` is bias, or bias -> LeakyReLU -> BatchNorm1d(eval)
+// affine, the two element-wise epilogues of the TDNN layers and the Linear layers.
 #include "dg_common.cuh"
 
 namespace dg {
 
-constexpr int BN_T = 64, BK_T = 16, G_THREADS = 128;
+constexpr int BM_T = 128, BN_T = 64, BK_T = 16, G_THREADS = 128;
 
-// TM rows per thread: 8 -> 128-row tiles, 6 -> 96-row tiles (pooling needs multiples of 3)
-template <int TM, int EPI, bool PRO>
+template <int EPI>
 __global__ void __launch_bounds__(G_THREADS) gemm_kernel(GemmArgs a) {
-  constexpr int BM = 16 * TM;
-  __shared__ __align__(16) float As[2][BK_T][BM + 4];
+  constexpr int TM = 8;   // rows per thread
+  __shared__ __align__(16) float As[2][BK_T][BM_T + 4];
   __shared__ __align__(16) float Ws[2][BK_T][BN_T];
   const int tid = threadIdx.x;
-  const long long m0 = (long long)blockIdx.x * BM;
+  const long long m0 = (long long)blockIdx.x * BM_T;
   const int n0 = blockIdx.y * BN_T;
   const int Ktot = a.KW * a.Cin;
   const int nkb = (Ktot + BK_T - 1) / BK_T;
   const int ty = tid >> 3, tx = tid & 7;   // 16 x 8 threads; thread tile TM x 8
 
   // ---- A loader: BM rows x 4 float4 per k-block -> BM*4/128 float4 per thread
-  constexpr int A_PER = BM * 4 / G_THREADS;
+  constexpr int A_PER = BM_T * 4 / G_THREADS;
   // ---- W loader: 16 rows x 16 float4 -> 2 per thread
   float4 a_reg[A_PER], w_reg[2];
 
@@ -42,18 +37,7 @@ __global__ void __launch_bounds__(G_THREADS) gemm_kernel(GemmArgs a) {
       if (k < Ktot) {
         const int j = k / a.Cin, c = k - j * a.Cin;
         const long long row = m0 + r + (long long)j * a.dil;
-        if (row < a.Mtot) {
-          v = *reinterpret_cast<const float4*>(a.A + row * a.lda + c);
-          if (PRO) {
-            const long long item = row / a.item_rows;
-            const float4 s = *reinterpret_cast<const float4*>(a.in_sc + item * a.Cin + c);
-            const float4 h = *reinterpret_cast<const float4*>(a.in_sh + item * a.Cin + c);
-            v.x = leaky(fmaf(v.x, s.x, h.x));
-            v.y = leaky(fmaf(v.y, s.y, h.y));
-            v.z = leaky(fmaf(v.z, s.z, h.z));
-            v.w = leaky(fmaf(v.w, s.w, h.w));
-          }
-        }
+        if (row < a.Mtot) v = *reinterpret_cast<const float4*>(a.A + row * a.lda + c);
       }
       a_reg[i] = v;
     }
@@ -100,19 +84,10 @@ __global__ void __launch_bounds__(G_THREADS) gemm_kernel(GemmArgs a) {
 #pragma unroll
     for (int kk = 0; kk < BK_T; kk++) {
       float av[TM], wv[8];
-      if (TM == 8) {
-        const float4 x0 = *reinterpret_cast<const float4*>(&As[buf][kk][ty * 8]);
-        const float4 x1 = *reinterpret_cast<const float4*>(&As[buf][kk][ty * 8 + 4]);
-        av[0] = x0.x; av[1] = x0.y; av[2] = x0.z; av[3] = x0.w;
-        av[4] = x1.x; av[5] = x1.y; av[6] = x1.z; av[7] = x1.w;
-      } else {
-#pragma unroll
-        for (int i = 0; i < TM; i += 2) {
-          const float2 x = *reinterpret_cast<const float2*>(&As[buf][kk][ty * TM + i]);
-          av[i] = x.x;
-          av[i + 1] = x.y;
-        }
-      }
+      const float4 x0 = *reinterpret_cast<const float4*>(&As[buf][kk][ty * 8]);
+      const float4 x1 = *reinterpret_cast<const float4*>(&As[buf][kk][ty * 8 + 4]);
+      av[0] = x0.x; av[1] = x0.y; av[2] = x0.z; av[3] = x0.w;
+      av[4] = x1.x; av[5] = x1.y; av[6] = x1.z; av[7] = x1.w;
       const float4 w0 = *reinterpret_cast<const float4*>(&Ws[buf][kk][tx * 4]);
       const float4 w1 = *reinterpret_cast<const float4*>(&Ws[buf][kk][32 + tx * 4]);
       wv[0] = w0.x; wv[1] = w0.y; wv[2] = w0.z; wv[3] = w0.w;
@@ -132,7 +107,7 @@ __global__ void __launch_bounds__(G_THREADS) gemm_kernel(GemmArgs a) {
 #pragma unroll
   for (int half = 0; half < 2; half++) {
     const int n = n0 + half * 32 + tx * 4;
-    if (n >= a.N) continue;   // N is a multiple of 4 everywhere on the path
+    if (n >= a.N) continue;   // N is a multiple of 4 (checked by the launcher)
     float4 bias = make_float4(0.f, 0.f, 0.f, 0.f);
     if (a.bias) bias = *reinterpret_cast<const float4*>(a.bias + n);
     float4 bsc = make_float4(1.f, 1.f, 1.f, 1.f), bsh = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -140,34 +115,18 @@ __global__ void __launch_bounds__(G_THREADS) gemm_kernel(GemmArgs a) {
       bsc = *reinterpret_cast<const float4*>(a.bn_scale + n);
       bsh = *reinterpret_cast<const float4*>(a.bn_shift + n);
     }
-    if (EPI == EPI_BIAS_POOL3) {
 #pragma unroll
-      for (int g = 0; g < TM / 3; g++) {
-        const long long m = m0 + ty * TM + g * 3;
-        if (m >= a.M) continue;
-        float4 v;
-        v.x = fmaxf(fmaxf(acc[g * 3][half * 4 + 0], acc[g * 3 + 1][half * 4 + 0]), acc[g * 3 + 2][half * 4 + 0]) + bias.x;
-        v.y = fmaxf(fmaxf(acc[g * 3][half * 4 + 1], acc[g * 3 + 1][half * 4 + 1]), acc[g * 3 + 2][half * 4 + 1]) + bias.y;
-        v.z = fmaxf(fmaxf(acc[g * 3][half * 4 + 2], acc[g * 3 + 1][half * 4 + 2]), acc[g * 3 + 2][half * 4 + 2]) + bias.z;
-        v.w = fmaxf(fmaxf(acc[g * 3][half * 4 + 3], acc[g * 3 + 1][half * 4 + 3]), acc[g * 3 + 2][half * 4 + 3]) + bias.w;
-        *reinterpret_cast<float4*>(a.C + (m / 3) * a.ldc + n) = v;
+    for (int i = 0; i < TM; i++) {
+      const long long m = m0 + ty * TM + i;
+      if (m >= a.M) continue;
+      float4 v = make_float4(acc[i][half * 4 + 0] + bias.x, acc[i][half * 4 + 1] + bias.y,
+                             acc[i][half * 4 + 2] + bias.z, acc[i][half * 4 + 3] + bias.w);
+      if (EPI == EPI_BIAS_LEAKY_BN) {
+        v.x = leaky(v.x); v.y = leaky(v.y); v.z = leaky(v.z); v.w = leaky(v.w);
+        v.x = fmaf(v.x, bsc.x, bsh.x); v.y = fmaf(v.y, bsc.y, bsh.y);
+        v.z = fmaf(v.z, bsc.z, bsh.z); v.w = fmaf(v.w, bsc.w, bsh.w);
       }
-    } else {
-#pragma unroll
-      for (int i = 0; i < TM; i++) {
-        const long long m = m0 + ty * TM + i;
-        if (m >= a.M) continue;
-        float4 v = make_float4(acc[i][half * 4 + 0] + bias.x, acc[i][half * 4 + 1] + bias.y,
-                               acc[i][half * 4 + 2] + bias.z, acc[i][half * 4 + 3] + bias.w);
-        if (EPI == EPI_BIAS_LEAKY || EPI == EPI_BIAS_LEAKY_BN) {
-          v.x = leaky(v.x); v.y = leaky(v.y); v.z = leaky(v.z); v.w = leaky(v.w);
-        }
-        if (EPI == EPI_BIAS_LEAKY_BN) {
-          v.x = fmaf(v.x, bsc.x, bsh.x); v.y = fmaf(v.y, bsc.y, bsh.y);
-          v.z = fmaf(v.z, bsc.z, bsh.z); v.w = fmaf(v.w, bsc.w, bsh.w);
-        }
-        *reinterpret_cast<float4*>(a.C + m * a.ldc + n) = v;
-      }
+      *reinterpret_cast<float4*>(a.C + m * a.ldc + n) = v;
     }
   }
 }
@@ -178,24 +137,9 @@ int launch_gemm(const GemmArgs& a, cudaStream_t st) {
     set_error("gemm: channel counts must be multiples of 4");
     return -1;
   }
-  const bool pro = a.in_sc != nullptr;
-  dim3 block(G_THREADS);
-  if (a.epi == EPI_BIAS_POOL3) {
-    dim3 grid((unsigned)((a.M + 95) / 96), (a.N + BN_T - 1) / BN_T);
-    if (pro) gemm_kernel<6, EPI_BIAS_POOL3, true><<<grid, block, 0, st>>>(a);
-    else gemm_kernel<6, EPI_BIAS_POOL3, false><<<grid, block, 0, st>>>(a);
-  } else {
-    dim3 grid((unsigned)((a.M + 127) / 128), (a.N + BN_T - 1) / BN_T);
-    if (a.epi == EPI_BIAS) {
-      if (pro) gemm_kernel<8, EPI_BIAS, true><<<grid, block, 0, st>>>(a);
-      else gemm_kernel<8, EPI_BIAS, false><<<grid, block, 0, st>>>(a);
-    } else if (a.epi == EPI_BIAS_LEAKY) {
-      gemm_kernel<8, EPI_BIAS_LEAKY, false><<<grid, block, 0, st>>>(a);
-    } else {
-      if (pro) gemm_kernel<8, EPI_BIAS_LEAKY_BN, true><<<grid, block, 0, st>>>(a);
-      else gemm_kernel<8, EPI_BIAS_LEAKY_BN, false><<<grid, block, 0, st>>>(a);
-    }
-  }
+  const dim3 grid((unsigned)((a.M + BM_T - 1) / BM_T), (a.N + BN_T - 1) / BN_T);
+  if (a.epi == EPI_BIAS) gemm_kernel<EPI_BIAS><<<grid, G_THREADS, 0, st>>>(a);
+  else gemm_kernel<EPI_BIAS_LEAKY_BN><<<grid, G_THREADS, 0, st>>>(a);
   DG_LAUNCHED();
   return 0;
 }

@@ -6,10 +6,9 @@
 // LeakyReLU -> BatchNorm1d(eval)) and the LSTM input projections of PyanNet (SURVEY.md Appendix
 // A.3/A.4; reached from the reference through src/diart/models.py:131-133) -- must stay at float32-level
 // accuracy because their outputs feed hard thresholds (tau_active, rho_update, delta_new).  Each float32
-// operand x is therefore carried as two 16-bit planes, hi = rn16(x) and lo = rn16(x - hi) -- fp16 by default
-// (22 significand bits for the pair), bf16 with DG_SPLIT_BF16=1 (16 bits) -- and every k-step issues three
-// wgmma (hi*hi + lo*hi + hi*lo) into the same float32 register accumulator.  Measured against the float32
-// SIMT GEMM: < 1e-5 relative (tests/test_gpu_gemm_tc.py).
+// operand x is therefore carried as two fp16 planes, hi = rn16(x) and lo = rn16(x - hi) (22 significand bits
+// for the pair), and every k-step issues three wgmma (hi*hi + lo*hi + hi*lo) into the same float32 register
+// accumulator.  Measured against the float32 reference GEMM of gemm.cu: < 1e-5 relative (tests/test_gpu_gemm_tc.py).
 //
 // Because activations are stored time-major ([item][row][channel]) a Conv1d tap is just a TMA box whose
 // row coordinate is shifted by j*dil: no im2col is ever materialised.
@@ -66,7 +65,6 @@ struct TcArgs {
   __nv_bfloat16* out_hi;   // EPI_*_SPLIT: [M, ldc] each
   __nv_bfloat16* out_lo;
   int ldc;
-  int f16;              // operand planes are fp16 (1) or bf16 (0)
   float acc_scale;      // 1 / (power-of-two scale of the weight planes): applied to the accumulator in the epilogue
   int vec8;             // output rows are 32-byte aligned: 32 bytes per lane and store pair
   int tap_off[9];       // row offset of every tap (Conv1d: j * dil; Conv2d on a zero-padded map: (dw-1) * Hp + (dh-1))
@@ -179,8 +177,8 @@ __device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params,
             const uint32_t hw[4] = {hq.x, hq.y, hq.z, hq.w}, lw[4] = {lq.x, lq.y, lq.z, lq.w};
 #pragma unroll
             for (int e = 0; e < 4; e++) {
-              v[8 * q + 2 * e] += h16_to_f32((uint16_t)(hw[e] & 0xFFFFu), a.f16) + h16_to_f32((uint16_t)(lw[e] & 0xFFFFu), a.f16);
-              v[8 * q + 2 * e + 1] += h16_to_f32((uint16_t)(hw[e] >> 16), a.f16) + h16_to_f32((uint16_t)(lw[e] >> 16), a.f16);
+              v[8 * q + 2 * e] += h16_to_f32((uint16_t)(hw[e] & 0xFFFFu)) + h16_to_f32((uint16_t)(lw[e] & 0xFFFFu));
+              v[8 * q + 2 * e + 1] += h16_to_f32((uint16_t)(hw[e] >> 16)) + h16_to_f32((uint16_t)(lw[e] >> 16));
             }
           }
         }
@@ -200,8 +198,8 @@ __device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params,
 #pragma unroll
             for (int i = 0; i < 16; i++) {
               uint16_t h0, l0, h1, l1;
-              split_h16(v[2 * i], a.f16, h0, l0);
-              split_h16(v[2 * i + 1], a.f16, h1, l1);
+              split_h16(v[2 * i], h0, l0);
+              split_h16(v[2 * i + 1], h1, l1);
               hi[i] = pack_u16x2(h0, h1);
               lo[i] = pack_u16x2(l0, l1);
             }
@@ -231,8 +229,8 @@ __device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params,
 #pragma unroll
           for (int i = 0; i < 16; i++) {
             uint16_t h0, l0, h1, l1;
-            split_h16(v[2 * i], a.f16, h0, l0);
-            split_h16(v[2 * i + 1], a.f16, h1, l1);
+            split_h16(v[2 * i], h0, l0);
+            split_h16(v[2 * i + 1], h1, l1);
             hi[i] = pack_u16x2(h0, h1);
             lo[i] = pack_u16x2(l0, l1);
           }
@@ -275,7 +273,7 @@ __device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params,
     }
 }
 
-template <int BN, int EPI, bool F16>
+template <int BN, int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo, TcArgs a) {
@@ -350,9 +348,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         const uint64_t adv = (uint64_t)((ks * 32) >> 4);   // +32 bytes per 16-element k-step
 #pragma unroll
         for (int h = 0; h < 2; h++) {
-          wgmma_ss<BN, F16>(acc[h], a_lo + adv + h * HALF, w_hi + adv, (kb | ks) != 0);
-          wgmma_ss<BN, F16>(acc[h], a_hi + adv + h * HALF, w_lo + adv, 1);
-          wgmma_ss<BN, F16>(acc[h], a_hi + adv + h * HALF, w_hi + adv, 1);
+          wgmma_ss<BN>(acc[h], a_lo + adv + h * HALF, w_hi + adv, (kb | ks) != 0);
+          wgmma_ss<BN>(acc[h], a_hi + adv + h * HALF, w_lo + adv, 1);
+          wgmma_ss<BN>(acc[h], a_hi + adv + h * HALF, w_hi + adv, 1);
         }
       }
       wg_commit();
@@ -591,7 +589,7 @@ __device__ __forceinline__ void tc_pool_epilogue_tile(const TcArgs& a, float* pa
 
 // Named barriers besides 0: 1 + c = the 128 threads of consumer c (epilogue staging); 3 + c = consumer c may issue its
 // mainloop (256 threads: consumer c waits, the other consumer arrives once its own MMAs are issued).
-template <int BN, int EPI, bool F16>
+template <int BN, int EPI>
 __global__ void __launch_bounds__(TC_POOL_THREADS, 1)
 gemm_tc_pool_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo, TcArgs a) {
@@ -711,9 +709,9 @@ gemm_tc_pool_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
         const uint64_t adv = (uint64_t)((ks * 32) >> 4);   // +32 bytes per 16-element k-step
 #pragma unroll
         for (int h = 0; h < 2; h++) {
-          wgmma_ss<BN, F16>(acc[h], a_lo + adv + h * HALF, w_hi + adv, (kb | ks) != 0);
-          wgmma_ss<BN, F16>(acc[h], a_hi + adv + h * HALF, w_lo + adv, 1);
-          wgmma_ss<BN, F16>(acc[h], a_hi + adv + h * HALF, w_hi + adv, 1);
+          wgmma_ss<BN>(acc[h], a_lo + adv + h * HALF, w_hi + adv, (kb | ks) != 0);
+          wgmma_ss<BN>(acc[h], a_hi + adv + h * HALF, w_lo + adv, 1);
+          wgmma_ss<BN>(acc[h], a_hi + adv + h * HALF, w_hi + adv, 1);
         }
       }
       wg_commit();
@@ -737,7 +735,7 @@ gemm_tc_pool_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
 }
 
 // ------------------------------------------------------------------------------------ host side
-// bf16 matrix [rows, cols] row-major (cols contiguous, row pitch `ld` elements); box = box_cols x box_rows, swizzled by the
+// 16-bit matrix [rows, cols] row-major (cols contiguous, row pitch `ld` elements); box = box_cols x box_rows, swizzled by the
 // box row's width (64 or 128 bytes)
 static int make_map(CUtensorMap* m, const void* base, long long rows, int cols, int ld, int box_cols, int box_rows) {
   EncodeTiledFn fn = encode_fn();
@@ -811,7 +809,6 @@ static int tc_setup(const TcGemm& g, int bn, int bk, int epi, CUtensorMap* maps,
   a.bias = g.bias; a.bn_scale = g.bn_scale; a.bn_shift = g.bn_shift;
   a.out_f32 = g.out_f32; a.out_hi = reinterpret_cast<__nv_bfloat16*>(g.out_hi);
   a.out_lo = reinterpret_cast<__nv_bfloat16*>(g.out_lo); a.ldc = g.ldc;
-  a.f16 = split_f16();
   a.acc_scale = g.w_scale > 0.f ? 1.f / g.w_scale : 1.f;
   for (int j = 0; j < 9; j++) a.tap_off[j] = j < g.KW ? (g.tap_off ? g.tap_off[j] : j * g.dil) : 0;
   a.Wp = g.Wp; a.Hp = g.Hp; a.Wop = g.Wop; a.Hop = g.Hop; a.stride2 = g.stride2; a.relu = g.relu;
@@ -838,9 +835,9 @@ static int launch_tc(const TcGemm& g, cudaStream_t st) {
   CUtensorMap m[4];
   TcArgs a;
   if (tc_setup(g, BN, TC_BK, EPI, m, a)) return -2;
-  auto kern = a.f16 ? gemm_tc_kernel<BN, EPI, true> : gemm_tc_kernel<BN, EPI, false>;
-  static bool attr_done[2][64] = {};
-  if (first_use_on_device(attr_done[a.f16]))
+  auto kern = gemm_tc_kernel<BN, EPI>;
+  static bool attr_done[64] = {};
+  if (first_use_on_device(attr_done))
     DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
   kern<<<tc_grid(g, a), TC_THREADS, S::TOTAL, st>>>(m[0], m[1], m[2], m[3], a);
   DG_LAUNCHED();
@@ -854,9 +851,9 @@ static int launch_tc_pool(const TcGemm& g, cudaStream_t st) {
   TcArgs a;
   if (tc_setup(g, BN, TC_POOL_BK, EPI, m, a)) return -2;
   if (!(a.tile_ctr = tile_counter(st))) return -2;
-  auto kern = a.f16 ? gemm_tc_pool_kernel<BN, EPI, true> : gemm_tc_pool_kernel<BN, EPI, false>;
-  static bool attr_done[2][64] = {};
-  if (first_use_on_device(attr_done[a.f16]))
+  auto kern = gemm_tc_pool_kernel<BN, EPI>;
+  static bool attr_done[64] = {};
+  if (first_use_on_device(attr_done))
     DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::total(EPI)));
   kern<<<tc_grid(g, a), TC_POOL_THREADS, S::total(EPI), st>>>(m[0], m[1], m[2], m[3], a);
   DG_LAUNCHED();
@@ -868,7 +865,7 @@ int launch_gemm_tc(const TcGemm& g, cudaStream_t st) {
   if (g.Cin % TC_BK || g.lda % 8 || g.ldc % (g.epi == TC_LEAKY_BN_SPLIT ? 8 : 4) || (g.Npad % 128 && g.Npad != 64 && g.Npad != 32) ||
       g.KW < 1 || g.KW > 9) {
     set_error("gemm_tc: Cin must be a multiple of 64, A pitch a multiple of 8, output pitch a multiple of 4 "
-              "(8 for bf16 planes), padded N 32, 64 or a multiple of 128, at most 9 taps");
+              "(8 for 16-bit planes), padded N 32, 64 or a multiple of 128, at most 9 taps");
     return -1;
   }
   if (g.epi == TC_CONV2D) {
@@ -913,7 +910,7 @@ int launch_gemm_tc(const TcGemm& g, cudaStream_t st) {
 __global__ void __launch_bounds__(256) split_kernel(const float* __restrict__ x, long long rows_out, int C, int ld_in,
                                                     int ld_out, int pool, int item_rows, const float* __restrict__ sc,
                                                     const float* __restrict__ sh, __nv_bfloat16* __restrict__ hi,
-                                                    __nv_bfloat16* __restrict__ lo, int f16, const int* __restrict__ skip_flag) {
+                                                    __nv_bfloat16* __restrict__ lo, const int* __restrict__ skip_flag) {
   if (skip_flag && *skip_flag != 0) return;
   const int q_per_row = ld_out >> 2;
   const long long n4 = rows_out * q_per_row;
@@ -940,10 +937,10 @@ __global__ void __launch_bounds__(256) split_kernel(const float* __restrict__ x,
       }
     }
     uint16_t h0, h1, h2, h3, l0, l1, l2, l3;
-    split_h16(v.x, f16, h0, l0);
-    split_h16(v.y, f16, h1, l1);
-    split_h16(v.z, f16, h2, l2);
-    split_h16(v.w, f16, h3, l3);
+    split_h16(v.x, h0, l0);
+    split_h16(v.y, h1, l1);
+    split_h16(v.z, h2, l2);
+    split_h16(v.w, h3, l3);
     reinterpret_cast<uint2*>(hi)[i] = make_uint2(pack_u16x2(h0, h1), pack_u16x2(h2, h3));
     reinterpret_cast<uint2*>(lo)[i] = make_uint2(pack_u16x2(l0, l1), pack_u16x2(l2, l3));
   }
@@ -961,26 +958,15 @@ int launch_split_ex(const float* x, long long rows_out, int C, int ld_in, int ld
   const int cap = usable_sms() * 16;
   const int grid = (int)(want < cap ? want : cap);
   split_kernel<<<grid, 256, 0, st>>>(x, rows_out, C, ld_in, ld_out, pool, item_rows, sc, sh,
-                                     reinterpret_cast<__nv_bfloat16*>(hi), reinterpret_cast<__nv_bfloat16*>(lo), split_f16(), skip_flag);
+                                     reinterpret_cast<__nv_bfloat16*>(hi), reinterpret_cast<__nv_bfloat16*>(lo), skip_flag);
   DG_LAUNCHED();
   return 0;
 }
 
-int launch_split(const float* x, long long rows, int C, int item_rows, const float* sc, const float* sh, void* hi,
-                 void* lo, cudaStream_t st) {
-  return launch_split_ex(x, rows, C, C, C, 0, item_rows, sc, sh, hi, lo, st);
-}
-
-int split_f16() {
-  static const int f16 = !(getenv("DG_SPLIT_BF16") && getenv("DG_SPLIT_BF16")[0] == '1');
-  return f16;
-}
-
-// host-side conversions, round to nearest even (fp16: subnormals kept, finite overflow saturates like cvt.satfinite)
-uint16_t host_f32_to_h16(float f, int f16) {
+// host-side fp16 conversions, round to nearest even (subnormals kept, finite overflow saturates like cvt.satfinite)
+uint16_t host_f32_to_h16(float f) {
   uint32_t u;
   memcpy(&u, &f, 4);
-  if (!f16) return (uint16_t)((u + 0x7FFFu + ((u >> 16) & 1u)) >> 16);
   const uint32_t sign = (u >> 16) & 0x8000u;
   const uint32_t au = u & 0x7FFFFFFFu;
   if (au > 0x7F800000u) return (uint16_t)(sign | 0x7FFFu);                  // NaN
@@ -996,43 +982,35 @@ uint16_t host_f32_to_h16(float f, int f16) {
   const uint32_t bits = e >= -14 ? (uint32_t)((e + 14) << 10) + q : q;
   return (uint16_t)(sign | bits);
 }
-float host_h16_to_f32(uint16_t h, int f16) {
-  uint32_t u;
-  if (!f16) {
-    u = (uint32_t)h << 16;
-  } else {
-    const uint32_t sign = ((uint32_t)h & 0x8000u) << 16, e = (h >> 10) & 31u, m = h & 0x3FFu;
-    if (e == 0) {
-      const float v = (float)m * 5.9604644775390625e-08f;                  // m * 2^-24
-      float r = sign ? -v : v;
-      return r;
-    }
-    u = e == 31 ? (sign | 0x7F800000u | (m << 13)) : (sign | ((e + 112u) << 23) | (m << 13));
+float host_h16_to_f32(uint16_t h) {
+  const uint32_t sign = ((uint32_t)h & 0x8000u) << 16, e = (h >> 10) & 31u, m = h & 0x3FFu;
+  if (e == 0) {
+    const float v = (float)m * 5.9604644775390625e-08f;                  // m * 2^-24
+    return sign ? -v : v;
   }
+  const uint32_t u = e == 31 ? (sign | 0x7F800000u | (m << 13)) : (sign | ((e + 112u) << 23) | (m << 13));
   float f;
   memcpy(&f, &u, 4);
   return f;
 }
 
-// host: float32 [N][K] -> zero-padded 16-bit hi/lo planes [Npad][K]
-void split_weights_host(const float* w, int N, int Npad, int K, uint16_t* hi, uint16_t* lo, int f16, float scale) {
+// host: float32 [N][K] -> zero-padded fp16 hi/lo planes [Npad][K]
+void split_weights_host(const float* w, int N, int Npad, int K, uint16_t* hi, uint16_t* lo, float scale) {
   for (size_t i = 0; i < (size_t)Npad * K; i++) hi[i] = lo[i] = 0;
   for (int n = 0; n < N; n++)
     for (int k = 0; k < K; k++) {
       const float f = w[(size_t)n * K + k] * scale;          // power of two: exact
-      const uint16_t h = host_f32_to_h16(f, f16);
+      const uint16_t h = host_f32_to_h16(f);
       hi[(size_t)n * K + k] = h;
-      lo[(size_t)n * K + k] = host_f32_to_h16(f - host_h16_to_f32(h, f16), f16);
+      lo[(size_t)n * K + k] = host_f32_to_h16(f - host_h16_to_f32(h));
     }
 }
 
 // Power-of-two scale of a weight tensor's fp16 planes: the largest magnitude lands in [2^12, 2^13), so that the lo plane
 // (|lo| <= 2^-11 |w|) of every weight down to 2^-15 of the largest one stays a NORMAL fp16 number (un-scaled, lo goes
 // subnormal below |w| = 0.125 and the pair keeps only an absolute 2^-25).  The accumulator is multiplied by 1 / scale in
-// the epilogue (an exact operation).  bf16 planes have float32's exponent range: scale 1.  DG_NO_WSCALE=1 disables it (A/B).
-float weight_plane_scale(const float* w, size_t n, int f16) {
-  static const bool off = getenv("DG_NO_WSCALE") && getenv("DG_NO_WSCALE")[0] == '1';
-  if (!f16 || off) return 1.f;
+// the epilogue (an exact operation).
+float weight_plane_scale(const float* w, size_t n) {
   float mx = 0.f;
   for (size_t i = 0; i < n; i++) {
     const float v = fabsf(w[i]);

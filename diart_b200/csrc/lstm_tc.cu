@@ -1,4 +1,4 @@
-// Bidirectional LSTM recurrence of PyanNet on the tensor cores (wgmma), split precision (hi + lo 16-bit planes).
+// Bidirectional LSTM recurrence of PyanNet on the tensor cores (wgmma), split precision (hi + lo fp16 planes).
 // (nn.LSTM(60,128,num_layers=4,bidirectional), SURVEY.md Appendix A.3; reached from the reference through
 // src/diart/models.py:131-133.)  The input projections are hoisted into gemm_tc.cu; this kernel runs the 293
 // dependent steps of one layer.
@@ -50,12 +50,10 @@ __device__ __forceinline__ float rcp_approx(float x) {
 // owns rows 16 w .. 16 w + 15: row 16 w + u % 8 holds gate 2 t, row 16 w + 8 + u % 8 gate 2 t + 1
 __host__ __device__ constexpr int lt_row(int g, int u) { return (u >> 5) * 128 + (g >> 1) * 64 + ((u & 31) >> 3) * 16 + (g & 1) * 8 + (u & 7); }
 
-template <bool F16>
 __global__ void __launch_bounds__(LT_THREADS, 1)
 lstm_tc_kernel(const __grid_constant__ CUtensorMap tm_wlo, const float* __restrict__ gx /*[item][frame][1024]*/,
                const uint16_t* __restrict__ w_hi /*[2][512][128], packed rows*/, int B, int T, int stride, int groups_per_dir,
                float* __restrict__ hout, uint16_t* __restrict__ out_hi, uint16_t* __restrict__ out_lo, float acc_scale) {
-  constexpr int f16 = F16 ? 1 : 0;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   unsigned char* wsm = smem;                         // [k-block][512 x 128 B]   (W_lo)
@@ -130,9 +128,9 @@ lstm_tc_kernel(const __grid_constant__ CUtensorMap tm_wlo, const float* __restri
 #pragma unroll
       for (int t = 0; t < 2; t++) {
         const uint64_t al = wg_desc(wlo + (ks >> 2) * 65536 + t * 64 * 128) + (uint64_t)(((ks & 3) * 32) >> 4);
-        wgmma_rs<8, F16>(acc[t], wa[t][ks], bl, ks != 0);      // W_hi . h_lo
-        wgmma_ss<8, F16>(acc[t], al, bh, 1);                   // W_lo . h_hi
-        wgmma_rs<8, F16>(acc[t], wa[t][ks], bh, 1);            // W_hi . h_hi
+        wgmma_rs<8>(acc[t], wa[t][ks], bl, ks != 0);      // W_hi . h_lo
+        wgmma_ss<8>(acc[t], al, bh, 1);                   // W_lo . h_hi
+        wgmma_rs<8>(acc[t], wa[t][ks], bh, 1);            // W_hi . h_hi
       }
     }
     wg_commit();
@@ -161,7 +159,7 @@ lstm_tc_kernel(const __grid_constant__ CUtensorMap tm_wlo, const float* __restri
       // h = tanh(c') / (1 + e^-o)
       const float eo = ex2_approx(fminf(fmaf(acc[1][2 + e], acc_scale, xg[3][e]) * -L2E, 40.f));
       h[e] = valid[e] ? (ec - 1.f) * rcp_approx((1.f + eo) * (ec + 1.f)) : 0.f;
-      split_h16(h[e], f16, hh[e], hl[e]);
+      split_h16(h[e], hh[e], hl[e]);
     }
     const uint32_t dst = h_addr + (buf ^ 1) * (LT_H_BYTES / 2);
 #pragma unroll
@@ -188,18 +186,18 @@ lstm_tc_kernel(const __grid_constant__ CUtensorMap tm_wlo, const float* __restri
 
 size_t lstm_tc_plane_elems() { return (size_t)2 * 512 * 128; }
 
-// torch weight_hh_l{L}[_reverse] ([512][128], gate order i,f,g,o) -> 16-bit hi / lo planes [2][512][128], rows in the kernel's
+// torch weight_hh_l{L}[_reverse] ([512][128], gate order i,f,g,o) -> fp16 hi / lo planes [2][512][128], rows in the kernel's
 // order (lt_row); returns the power-of-two factor both planes were multiplied by (weight_plane_scale; one factor for both
 // directions)
-float lstm_tc_pack_whh(const float* whh_fwd, const float* whh_bwd, uint16_t* hi, uint16_t* lo, int f16) {
-  const float s0 = weight_plane_scale(whh_fwd, 512 * 128, f16), s1 = weight_plane_scale(whh_bwd, 512 * 128, f16);
+float lstm_tc_pack_whh(const float* whh_fwd, const float* whh_bwd, uint16_t* hi, uint16_t* lo) {
+  const float s0 = weight_plane_scale(whh_fwd, 512 * 128), s1 = weight_plane_scale(whh_bwd, 512 * 128);
   const float scale = s0 < s1 ? s0 : s1;
   std::vector<float> perm((size_t)512 * 128);
   for (int d = 0; d < 2; d++) {
     const float* w = d == 0 ? whh_fwd : whh_bwd;
     for (int g = 0; g < 4; g++)
       for (int u = 0; u < 128; u++) memcpy(&perm[(size_t)lt_row(g, u) * 128], w + ((size_t)g * 128 + u) * 128, 128 * sizeof(float));
-    split_weights_host(perm.data(), 512, 512, 128, hi + (size_t)d * 512 * 128, lo + (size_t)d * 512 * 128, f16, scale);
+    split_weights_host(perm.data(), 512, 512, 128, hi + (size_t)d * 512 * 128, lo + (size_t)d * 512 * 128, scale);
   }
   return scale;
 }
@@ -228,10 +226,9 @@ int launch_lstm_layer_tc(const float* gx, const void* whh_hi, const void* whh_lo
     set_error("cuTensorMapEncodeTiled failed for W_hh");
     return -2;
   }
-  const int f16 = split_f16();
-  auto kern = f16 ? lstm_tc_kernel<true> : lstm_tc_kernel<false>;
-  static bool attr_done[2][64] = {};
-  if (first_use_on_device(attr_done[f16])) DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM));
+  auto kern = lstm_tc_kernel;
+  static bool attr_done[64] = {};
+  if (first_use_on_device(attr_done)) DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, LT_SMEM));
   const int gpd = (B + LT_NB - 1) / LT_NB;
   const float inv = w_scale > 0.f ? 1.f / w_scale : 1.f;
   kern<<<2 * gpd, LT_THREADS, LT_SMEM, st>>>(tm, gx, reinterpret_cast<const uint16_t*>(whh_hi), B, T, stride, gpd, hout,

@@ -22,16 +22,16 @@
 
 namespace dg {
 
-// waveform [B, S] float32 -> hi / lo 16-bit planes of x * 2^15 (what pyannote feeds kaldi.fbank), [B * S (+ tail zeros)]
+// waveform [B, S] float32 -> hi / lo fp16 planes of x * 2^15 (what pyannote feeds kaldi.fbank), [B * S (+ tail zeros)]
 __global__ void __launch_bounds__(256) fb_planes_kernel(const float* __restrict__ wav, long long n, uint16_t* __restrict__ hi,
-                                                        uint16_t* __restrict__ lo, int f16) {
+                                                        uint16_t* __restrict__ lo) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < (n >> 2); i += (long long)gridDim.x * blockDim.x) {
     const float4 v = reinterpret_cast<const float4*>(wav)[i];
     uint16_t h0, h1, h2, h3, l0, l1, l2, l3;
-    split_h16(v.x * 32768.f, f16, h0, l0);
-    split_h16(v.y * 32768.f, f16, h1, l1);
-    split_h16(v.z * 32768.f, f16, h2, l2);
-    split_h16(v.w * 32768.f, f16, h3, l3);
+    split_h16(v.x * 32768.f, h0, l0);
+    split_h16(v.y * 32768.f, h1, l1);
+    split_h16(v.z * 32768.f, h2, l2);
+    split_h16(v.w * 32768.f, h3, l3);
     reinterpret_cast<uint2*>(hi)[i] = make_uint2(pack_u16x2(h0, h1), pack_u16x2(h2, h3));
     reinterpret_cast<uint2*>(lo)[i] = make_uint2(pack_u16x2(l0, l1), pack_u16x2(l2, l3));
   }
@@ -46,7 +46,7 @@ int launch_fb_planes(const float* wav, long long n, void* hi, void* lo, cudaStre
   const long long want = ((n >> 2) + 255) / 256;
   const long long cap = usable_sms() * 16LL;
   fb_planes_kernel<<<(int)(want < cap ? want : cap), 256, 0, st>>>(wav, n, reinterpret_cast<uint16_t*>(hi),
-                                                                             reinterpret_cast<uint16_t*>(lo), split_f16());
+                                                                             reinterpret_cast<uint16_t*>(lo));
   DG_LAUNCHED();
   return 0;
 }
@@ -107,7 +107,7 @@ int launch_fb_mean(const float* logmel, int B, int T, float* mean, cudaStream_t 
 __global__ void __launch_bounds__(256) rn_stem_kernel(const float* __restrict__ logmel, const float* __restrict__ mean, int T,
                                                       const float* __restrict__ w, const float* __restrict__ sc,
                                                       const float* __restrict__ sh, uint16_t* __restrict__ hi,
-                                                      uint16_t* __restrict__ lo, int f16) {
+                                                      uint16_t* __restrict__ lo) {
   __shared__ float ws[32 * 9], ss[32], bs[32];
   for (int i = threadIdx.x; i < 288; i += blockDim.x) ws[i] = w[i];
   if (threadIdx.x < 32) {
@@ -145,8 +145,8 @@ __global__ void __launch_bounds__(256) rn_stem_kernel(const float* __restrict__ 
       v[e] = fmaxf(fmaf(acc, ss[c], bs[c]), 0.f);
     }
     uint16_t h0, l0, h1, l1;
-    split_h16(v[0], f16, h0, l0);
-    split_h16(v[1], f16, h1, l1);
+    split_h16(v[0], h0, l0);
+    split_h16(v[1], h1, l1);
     oh[c2] = pack_u16x2(h0, h1);
     ol[c2] = pack_u16x2(l0, l1);
   }
@@ -163,8 +163,7 @@ int launch_rn_stem(const float* logmel, const float* mean, int B, int T, const f
                    void* hi, void* lo, cudaStream_t st) {
   ProfScope _ps("resnet_stem", st);
   dim3 grid((T * 80 + 255) / 256, B);
-  rn_stem_kernel<<<grid, 256, 0, st>>>(logmel, mean, T, w, sc, sh, reinterpret_cast<uint16_t*>(hi), reinterpret_cast<uint16_t*>(lo),
-                                       split_f16());
+  rn_stem_kernel<<<grid, 256, 0, st>>>(logmel, mean, T, w, sc, sh, reinterpret_cast<uint16_t*>(hi), reinterpret_cast<uint16_t*>(lo));
   DG_LAUNCHED();
   return 0;
 }

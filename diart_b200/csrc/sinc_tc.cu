@@ -16,8 +16,8 @@
 //   * items are laid out back to back with 667 rows each, so 128-row tiles run across item boundaries
 //     (rows 665/666 of an item are padding that the epilogue drops).
 //
-// hi/lo split precision as in gemm_tc.cu.  CTA = 288 threads: warp 8 TMA producer (A tiles, 3-stage ring; the 120 KB
-// filter bank hi/lo/lo2 is loaded once and stays resident), warps 0-7 two warpgroups, one per 64-row half of the tile, each
+// hi/lo split precision as in gemm_tc.cu.  CTA = 288 threads: warp 8 TMA producer (A tiles, 3-stage ring; the 80 KB
+// filter bank hi/lo is loaded once and stays resident), warps 0-7 two warpgroups, one per 64-row half of the tile, each
 // with the three class accumulators (3 x m64n80 wgmma, float32 in registers) and the epilogue straight from the registers.
 #include <stdlib.h>
 #include <string.h>
@@ -27,20 +27,19 @@
 
 namespace dg {
 
-constexpr int ST_ROWS = 128, ST_N = 80, ST_KB = 4, ST_NSTAGE = 3, ST_WP = 3;   // 3 filter planes: hi, lo, lo2
+constexpr int ST_ROWS = 128, ST_N = 80, ST_KB = 4, ST_NSTAGE = 3, ST_WP = 2;   // 2 filter planes: hi, lo
 constexpr int ST_A_BYTES = ST_ROWS * 64 * 2;           // 16 KB per plane per k-block
 constexpr int ST_STAGE = 2 * ST_A_BYTES;               // hi + lo
 constexpr int ST_W_BYTES = ST_N * 64 * 2;              // 10 KB per plane per k-block
-constexpr int ST_W_TOTAL = ST_KB * ST_WP * ST_W_BYTES; // 120 KB
+constexpr int ST_W_TOTAL = ST_KB * ST_WP * ST_W_BYTES; // 80 KB
 constexpr int ST_SMEM = ST_W_TOTAL + ST_NSTAGE * ST_STAGE + 256 + 1024;
 constexpr int ST_THREADS = 288;
 
 struct SincTcMaps {
   CUtensorMap a_hi[4], a_lo[4];   // shifted copies of the normalised waveform, hi / lo planes
-  CUtensorMap w[3];               // filter bank [80][256]: 16-bit hi, lo and (bf16 mode) second-order lo2 planes
+  CUtensorMap w[ST_WP];           // filter bank [80][256]: fp16 hi and lo planes
 };
 
-template <bool F16>
 __global__ void __launch_bounds__(ST_THREADS, 1)
 sinc0_tc_kernel(const __grid_constant__ SincTcMaps maps, int row_tiles, int rows_total, int rows_per_item, int T0,
                 int S0, float* __restrict__ p0, float gamma, const float* __restrict__ cf,
@@ -107,7 +106,7 @@ sinc0_tc_kernel(const __grid_constant__ SincTcMaps maps, int row_tiles, int rows
     int prev = -1;
     for (int kb = 0; kb < ST_KB; kb++) {
       const uint32_t wa = smem_u32(wsm + kb * ST_WP * ST_W_BYTES);
-      const uint64_t w_hi = wg_desc(wa), w_lo = wg_desc(wa + ST_W_BYTES), w_l2 = wg_desc(wa + 2 * ST_W_BYTES);
+      const uint64_t w_hi = wg_desc(wa), w_lo = wg_desc(wa + ST_W_BYTES);
 #pragma unroll
       for (int s3 = 0; s3 < 3; s3++) {
         mbar_wait(&full[stage], phase);
@@ -118,16 +117,10 @@ sinc0_tc_kernel(const __grid_constant__ SincTcMaps maps, int row_tiles, int rows
 #pragma unroll
         for (int ks = 0; ks < 4; ks++) {
           const uint64_t adv = (uint64_t)((ks * 32) >> 4);
-          // five of the nine hi/lo/lo2 products: everything down to 2^-24 of the leading term.  This
-          // layer's error is amplified by every later layer, so the filters carry 24 significand bits.
-          // (fp16 planes: hi + lo already carry 22 bits of both operands, three products suffice)
-          if (!F16) {
-            wgmma_ss<ST_N, F16>(acc[s3], a_lo + adv, w_lo + adv, (kb | ks) != 0);
-            wgmma_ss<ST_N, F16>(acc[s3], a_hi + adv, w_l2 + adv, 1);
-          }
-          wgmma_ss<ST_N, F16>(acc[s3], a_lo + adv, w_hi + adv, F16 ? (uint32_t)((kb | ks) != 0) : 1u);
-          wgmma_ss<ST_N, F16>(acc[s3], a_hi + adv, w_lo + adv, 1);
-          wgmma_ss<ST_N, F16>(acc[s3], a_hi + adv, w_hi + adv, 1);
+          // hi + lo carry 22 significand bits of both operands: three products
+          wgmma_ss<ST_N>(acc[s3], a_lo + adv, w_hi + adv, (kb | ks) != 0);
+          wgmma_ss<ST_N>(acc[s3], a_hi + adv, w_lo + adv, 1);
+          wgmma_ss<ST_N>(acc[s3], a_hi + adv, w_hi + adv, 1);
         }
         wg_commit();
         wg_wait<1>();
@@ -184,10 +177,10 @@ sinc0_tc_kernel(const __grid_constant__ SincTcMaps maps, int row_tiles, int rows
   }
 }
 
-// normalised waveform -> four shifted copies, 16-bit hi / lo planes:  plane[c][b*Lp + i] = split(xn[b][i + 2c])
+// normalised waveform -> four shifted copies, fp16 hi / lo planes:  plane[c][b*Lp + i] = split(xn[b][i + 2c])
 __global__ void __launch_bounds__(256) sinc_prep_kernel(const float* __restrict__ wav, const float* __restrict__ mean,
                                                         const float* __restrict__ rstd, int S, int Lp, size_t plane_elems,
-                                                        uint16_t* __restrict__ hi, uint16_t* __restrict__ lo, int f16,
+                                                        uint16_t* __restrict__ hi, uint16_t* __restrict__ lo,
                                                         const int* __restrict__ skip_flag) {
   if (skip_flag && *skip_flag != 0) return;     // the stream form does the work
   const int b = blockIdx.y;
@@ -196,7 +189,7 @@ __global__ void __launch_bounds__(256) sinc_prep_kernel(const float* __restrict_
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < Lp + 8; i += gridDim.x * blockDim.x) {
     const float v = i < S ? (x[i] - mu) * sc : 0.f;            // standardised waveform; the affine is applied in sinc0's epilogue
     uint16_t h, l;
-    split_h16(v, f16, h, l);
+    split_h16(v, h, l);
 #pragma unroll
     for (int c = 0; c < 4; c++) {
       const int j = i - 2 * c;                                 // copy c holds xn[j + 2c] at position j
@@ -235,18 +228,14 @@ int sinc_tc_rows_per_item(const Geom& g) {
 }
 size_t sinc_tc_plane_elems(int B, const Geom& g) { return (size_t)B * sinc_tc_rows_per_item(g) * 120 + 1024; }
 
-// filt [251][80] float32 (k-major) -> three 16-bit planes [3][80][256] (n-major, K padded with zeros):
-// hi = rn16(w), lo = rn16(w - hi), lo2 = rn16(w - hi - lo)
-void sinc_tc_pack_filters(const float* filt, uint16_t* planes, int f16) {
-  static float w[80 * 256], r[80 * 256];
-  static uint16_t dummy[80 * 256];
+// filt [251][80] float32 (k-major) -> two fp16 planes [2][80][256] (n-major, K padded with zeros):
+// hi = rn16(w), lo = rn16(w - hi)
+void sinc_tc_pack_filters(const float* filt, uint16_t* planes) {
+  static float w[80 * 256];
   memset(w, 0, sizeof(w));
   for (int k = 0; k < 251; k++)
     for (int f = 0; f < 80; f++) w[f * 256 + k] = filt[k * 80 + f];
-  split_weights_host(w, 80, 80, 256, planes, planes + 80 * 256, f16);
-  for (int i = 0; i < 80 * 256; i++)
-    r[i] = (w[i] - host_h16_to_f32(planes[i], f16)) - host_h16_to_f32(planes[80 * 256 + i], f16);
-  split_weights_host(r, 80, 80, 256, planes + 2 * 80 * 256, dummy, f16);      // third plane: used by the bf16 mode only
+  split_weights_host(w, 80, 80, 256, planes, planes + 80 * 256);
 }
 
 // per-filter constant of the folded InstanceNorm1d(1) affine: cf[f] = beta * sum_k h[f][k]
@@ -258,7 +247,7 @@ void sinc_tc_affine_consts(const float* filt /*[251][80]*/, float beta, float* c
   }
 }
 
-// standardised waveform -> four shifted 16-bit hi/lo copies (shared by every SincNet that reads this batch)
+// standardised waveform -> four shifted fp16 hi/lo copies (shared by every SincNet that reads this batch)
 int launch_sinc_prep(const float* wav, const float* mean, const float* rstd, int B, const Geom& g, void* planes_hi,
                      void* planes_lo, cudaStream_t st, const int* skip_flag) {
   const int rpi = sinc_tc_rows_per_item(g), Lp = rpi * 120;
@@ -269,7 +258,7 @@ int launch_sinc_prep(const float* wav, const float* mean, const float* rstd, int
   const int want_x = (2048 + B - 1) / B, max_x = (Lp + 8 + 255) / 256;
   dim3 grid(want_x < max_x ? want_x : max_x, B);
   sinc_prep_kernel<<<grid, 256, 0, st>>>(wav, mean, rstd, g.S, Lp, plane, reinterpret_cast<uint16_t*>(planes_hi),
-                                         reinterpret_cast<uint16_t*>(planes_lo), split_f16(), skip_flag);
+                                         reinterpret_cast<uint16_t*>(planes_lo), skip_flag);
   DG_LAUNCHED();
   return 0;
 }
@@ -287,10 +276,9 @@ static int sinc0_launch_common(const void* w_planes, uint64_t rows, int rpi, siz
   for (int pl = 0; pl < ST_WP; pl++)
     if (make_map2(&maps.w[pl], reinterpret_cast<const uint16_t*>(w_planes) + (size_t)pl * 80 * 256, 256, 80, 512, ST_N))
       return -2;
-  const int f16 = split_f16();
-  auto kern = f16 ? sinc0_tc_kernel<true> : sinc0_tc_kernel<false>;
-  static bool attr_done[2][64] = {};
-  if (first_use_on_device(attr_done[f16])) DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, ST_SMEM));
+  auto kern = sinc0_tc_kernel;
+  static bool attr_done[64] = {};
+  if (first_use_on_device(attr_done)) DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, ST_SMEM));
   const int sms = usable_sms();
   const int row_tiles = (int)((rows + ST_ROWS - 1) / ST_ROWS);
   const int tiles = row_tiles * 4;
@@ -349,10 +337,10 @@ SincStreamGeom sinc_stream_geom(int B, const Geom& g, int hop) {
   return sg;
 }
 
-// raw stream -> four shifted 16-bit hi / lo copies:  plane[c][i] = split(stream[i + 2c])
+// raw stream -> four shifted fp16 hi / lo copies:  plane[c][i] = split(stream[i + 2c])
 __global__ void __launch_bounds__(256) stream_prep_kernel(const float* __restrict__ wav, int S, int hop, int Ls, int Lp,
                                                           size_t plane_elems, uint16_t* __restrict__ hi,
-                                                          uint16_t* __restrict__ lo, int f16, const int* __restrict__ flag) {
+                                                          uint16_t* __restrict__ lo, const int* __restrict__ flag) {
   if (*flag == 0) return;
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < Lp + 8; i += gridDim.x * blockDim.x) {
     float v = 0.f;
@@ -361,7 +349,7 @@ __global__ void __launch_bounds__(256) stream_prep_kernel(const float* __restric
       v = wav[(size_t)b * S + (i - b * hop)];
     }
     uint16_t h, l;
-    split_h16(v, f16, h, l);
+    split_h16(v, h, l);
 #pragma unroll
     for (int c = 0; c < 4; c++) {
       const int j = i - 2 * c;
@@ -379,7 +367,7 @@ int launch_stream_prep(const float* wav, int B, const Geom& g, int hop, void* pl
   ProfScope _ps("sinc0_prep", st);
   const int Lp = sg.rows * 120;
   stream_prep_kernel<<<(Lp + 8 + 255) / 256, 256, 0, st>>>(wav, g.S, hop, sg.Ls, Lp, sg.plane, reinterpret_cast<uint16_t*>(planes_hi),
-                                                          reinterpret_cast<uint16_t*>(planes_lo), split_f16(), flag);
+                                                          reinterpret_cast<uint16_t*>(planes_lo), flag);
   DG_LAUNCHED();
   return 0;
 }
@@ -391,39 +379,6 @@ int launch_sinc0_tc_stream(const void* w_planes, int B, const Geom& g, int hop, 
   ProfScope _ps("sinc0", st);
   return sinc0_launch_common(w_planes, (uint64_t)sg.rows, sg.rows, sg.plane, planes_hi, planes_lo, 0, 0, nullptr, 1.f, nullptr,
                              craw, sg.P, flag, 1, st);
-}
-
-// p0[b][p][f] = max_{j<3} | A_b * craw[b*hop/10 + 3p + j][f] + cf[f] - A_b * mu_b * hsum[f] |,  A_b = gamma * rstd_b
-__global__ void __launch_bounds__(256) sinc_pool_kernel(const float* __restrict__ craw, const float* __restrict__ mean,
-                                                        const float* __restrict__ rstd, const float* __restrict__ cf,
-                                                        const float* __restrict__ hsum, float gamma, int hop10, int T0, int S0,
-                                                        float* __restrict__ p0, const int* __restrict__ flag) {
-  if (*flag == 0) return;
-  const int b = blockIdx.y;
-  const float A = gamma * rstd[b], Am = A * mean[b];
-  const float4* src = reinterpret_cast<const float4*>(craw + (size_t)b * hop10 * ST_N);
-  float4* dst = reinterpret_cast<float4*>(p0 + (size_t)b * S0 * ST_N);
-  for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < T0 * 20; idx += gridDim.x * blockDim.x) {
-    const int p = idx / 20, f4 = idx - p * 20;
-    const float4 c4 = reinterpret_cast<const float4*>(cf)[f4], h4 = reinterpret_cast<const float4*>(hsum)[f4];
-    const float bx = fmaf(-Am, h4.x, c4.x), by = fmaf(-Am, h4.y, c4.y), bz = fmaf(-Am, h4.z, c4.z), bw = fmaf(-Am, h4.w, c4.w);
-    const float4 u0 = src[(size_t)(3 * p) * 20 + f4], u1 = src[(size_t)(3 * p + 1) * 20 + f4], u2 = src[(size_t)(3 * p + 2) * 20 + f4];
-    float4 v;
-    v.x = fmaxf(fmaxf(fabsf(fmaf(A, u0.x, bx)), fabsf(fmaf(A, u1.x, bx))), fabsf(fmaf(A, u2.x, bx)));
-    v.y = fmaxf(fmaxf(fabsf(fmaf(A, u0.y, by)), fabsf(fmaf(A, u1.y, by))), fabsf(fmaf(A, u2.y, by)));
-    v.z = fmaxf(fmaxf(fabsf(fmaf(A, u0.z, bz)), fabsf(fmaf(A, u1.z, bz))), fabsf(fmaf(A, u2.z, bz)));
-    v.w = fmaxf(fmaxf(fabsf(fmaf(A, u0.w, bw)), fabsf(fmaf(A, u1.w, bw))), fabsf(fmaf(A, u2.w, bw)));
-    dst[(size_t)p * 20 + f4] = v;
-  }
-}
-
-int launch_sinc_pool(const float* craw, const float* mean, const float* rstd, const float* cf, const float* hsum, float gamma,
-                     int B, const Geom& g, int hop, float* p0, const int* flag, cudaStream_t st) {
-  ProfScope _ps("sinc0_pool", st);
-  dim3 grid((g.T0 * 20 + 255) / 256 < 64 ? (g.T0 * 20 + 255) / 256 : 64, B);
-  sinc_pool_kernel<<<grid, 256, 0, st>>>(craw, mean, rstd, cf, hsum, gamma, hop / 10, g.T0, g.S0, p0, flag);
-  DG_LAUNCHED();
-  return 0;
 }
 
 // ---- stream form, fused tail: the pooled map p0 is never written.  The raw convolution of the stream (68 MB at B = 256) stays
@@ -561,13 +516,13 @@ __global__ void __launch_bounds__(96) sinc_pool_finalize_kernel(int hop10, int T
   sh[(size_t)b * ST_N + f] = b0[f] - (float)mu * gsc;
 }
 
-// p0 recomputed -> leaky(p0 * sc + sh) -> 16-bit hi / lo planes [B * S0][80]
+// p0 recomputed -> leaky(p0 * sc + sh) -> fp16 hi / lo planes [B * S0][80]
 __global__ void __launch_bounds__(SP_THREADS) sinc_pool_split_kernel(const float* __restrict__ craw, long long P,
                                                                      const float* __restrict__ mean, const float* __restrict__ rstd,
                                                                      const float* __restrict__ cf, const float* __restrict__ hsum,
                                                                      float gamma, int B, int hop10, int T0, int S0,
                                                                      const float* __restrict__ sc, const float* __restrict__ sh,
-                                                                     uint16_t* __restrict__ hi, uint16_t* __restrict__ lo, int f16,
+                                                                     uint16_t* __restrict__ hi, uint16_t* __restrict__ lo,
                                                                      const int* __restrict__ flag) {
   if (*flag == 0) return;
   __shared__ float4 rows[(SP_R + 2) * 20];
@@ -589,10 +544,10 @@ __global__ void __launch_bounds__(SP_THREADS) sinc_pool_split_kernel(const float
       const int r = (int)((long long)b * hop10 + 3LL * p - r0);
       const float4 v = sp_value_sm(rows, r, f4, A, bias);
       uint16_t h0, h1, h2, h3, l0, l1, l2, l3;
-      split_h16(leaky(fmaf(v.x, s4.x, h4.x)), f16, h0, l0);
-      split_h16(leaky(fmaf(v.y, s4.y, h4.y)), f16, h1, l1);
-      split_h16(leaky(fmaf(v.z, s4.z, h4.z)), f16, h2, l2);
-      split_h16(leaky(fmaf(v.w, s4.w, h4.w)), f16, h3, l3);
+      split_h16(leaky(fmaf(v.x, s4.x, h4.x)), h0, l0);
+      split_h16(leaky(fmaf(v.y, s4.y, h4.y)), h1, l1);
+      split_h16(leaky(fmaf(v.z, s4.z, h4.z)), h2, l2);
+      split_h16(leaky(fmaf(v.w, s4.w, h4.w)), h3, l3);
       oh[(size_t)p * 20 + f4] = make_uint2(pack_u16x2(h0, h1), pack_u16x2(h2, h3));
       ol[(size_t)p * 20 + f4] = make_uint2(pack_u16x2(l0, l1), pack_u16x2(l2, l3));
     }
@@ -622,7 +577,7 @@ int launch_sinc_pool_fused(const float* craw, const float* mean, const float* rs
   ProfScope _ps("sinc0_pool_split", st);
   sinc_pool_split_kernel<<<blocks, SP_THREADS, 0, st>>>(craw, sg.P, mean, rstd, cf, hsum, gamma, B, hop10, g.T0, g.S0, sc, sh,
                                                         reinterpret_cast<uint16_t*>(planes_hi), reinterpret_cast<uint16_t*>(planes_lo),
-                                                        split_f16(), flag);
+                                                        flag);
   DG_LAUNCHED();
   return 0;
 }

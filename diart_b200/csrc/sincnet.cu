@@ -1,6 +1,6 @@
-// SincNet front end, stage 0 (shared by the segmentation and the embedding net, separate weights):
-//   InstanceNorm1d(1, affine) on the waveform -> ParamSincFB 80 x k251 stride 10 -> |.| -> MaxPool1d(3)
-// plus the per-(item, channel) InstanceNorm statistics that the next layer applies on load.
+// SincNet front end (shared by the segmentation and the embedding net, separate weights): the waveform statistics of
+// InstanceNorm1d(1, affine) and the per-(item, channel) InstanceNorm statistics that the next layer applies on load.
+// The convolutions themselves run on the tensor cores (sinc_tc.cu, gemm_tc.cu).
 // Restates pyannote.audio's SincNet.forward (SURVEY.md Appendix A.2); reached from the reference
 // through src/diart/models.py:131-133.
 #include "dg_common.cuh"
@@ -103,90 +103,6 @@ int launch_stream_stats(const float* wav, int B, int S, int hop, double* part, f
   stream_sums_kernel<<<blocks, 256, 0, st>>>(wav, B, S, hop, sub, part, flag);
   DG_LAUNCHED();
   stream_stats_kernel<<<(B + 127) / 128, 128, 0, st>>>(part, B, S, hop, sub, mean, rstd, flag);
-  DG_LAUNCHED();
-  return 0;
-}
-
-// ---------------------------------------------------------------------------------------------
-// sinc0: one CTA tile = 64 pooled outputs (192 conv positions) x 80 filters of one item.
-// Persistent CTAs keep the 80 KB filter bank in shared memory and walk the (item, tile) list.
-// Thread tile: 1 pooled output (3 conv positions) x 8 filters; lanes run over pooled positions,
-// warps over (position half, filter group).  fp32 FMA throughout.
-// ---------------------------------------------------------------------------------------------
-constexpr int SINC_K = 251, SINC_F = 80, SINC_TP = 64, SINC_THREADS = 640;
-constexpr int SINC_XSEG = 30 * (SINC_TP - 1) + 20 + SINC_K;  // 2161 samples feed one tile
-
-__global__ void __launch_bounds__(SINC_THREADS, 1)
-sinc0_kernel(const float* __restrict__ wav, const float* __restrict__ mean, const float* __restrict__ rstd,
-             float wn_gamma, float wn_beta, const float* __restrict__ filt, int B, int S, int T0, int S0,
-             int tiles_per_item, float* __restrict__ p0) {
-  extern __shared__ float smem[];
-  float* hs = smem;                       // [251][80]
-  float* xs = smem + SINC_K * SINC_F;     // [SINC_XSEG padded]
-  for (int i = threadIdx.x; i < SINC_K * SINC_F / 4; i += blockDim.x)
-    reinterpret_cast<float4*>(hs)[i] = reinterpret_cast<const float4*>(filt)[i];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int phalf = warp & 1, fg = warp >> 1;          // 2 position halves x 10 filter groups
-  const int pl = phalf * 32 + lane;                    // pooled position within the tile
-  const int total = B * tiles_per_item;
-  for (int tile = blockIdx.x; tile < total; tile += gridDim.x) {
-    const int b = tile / tiles_per_item, p_base = (tile - b * tiles_per_item) * SINC_TP;
-    const float mu = mean[b], sc = rstd[b] * wn_gamma;
-    const float* x = wav + (size_t)b * S;
-    const int x0 = 30 * p_base;
-    __syncthreads();
-    for (int i = threadIdx.x; i < SINC_XSEG; i += blockDim.x) {
-      int gi = x0 + i;
-      // InstanceNorm1d(1, affine): (x - mean) * rstd * gamma + beta
-      xs[i] = gi < S ? (x[gi] - mu) * sc + wn_beta : 0.f;
-    }
-    __syncthreads();
-    const int p = p_base + pl;
-    float acc[3][8];
-#pragma unroll
-    for (int j = 0; j < 3; j++)
-#pragma unroll
-      for (int f = 0; f < 8; f++) acc[j][f] = 0.f;
-    const float* xp = xs + 30 * pl;
-    const float* hp = hs + fg * 8;
-#pragma unroll 2
-    for (int k = 0; k < SINC_K; k++) {
-      const float4 h0 = *reinterpret_cast<const float4*>(hp + k * SINC_F);
-      const float4 h1 = *reinterpret_cast<const float4*>(hp + k * SINC_F + 4);
-      const float hv[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
-#pragma unroll
-      for (int j = 0; j < 3; j++) {
-        const float xv = xp[10 * j + k];
-#pragma unroll
-        for (int f = 0; f < 8; f++) acc[j][f] = fmaf(xv, hv[f], acc[j][f]);
-      }
-    }
-    if (p < T0) {
-      float v[8];
-#pragma unroll
-      for (int f = 0; f < 8; f++) v[f] = fmaxf(fmaxf(fabsf(acc[0][f]), fabsf(acc[1][f])), fabsf(acc[2][f]));
-      float* o = p0 + ((size_t)b * S0 + p) * SINC_F + fg * 8;
-      *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1], v[2], v[3]);
-      *reinterpret_cast<float4*>(o + 4) = make_float4(v[4], v[5], v[6], v[7]);
-    }
-  }
-}
-
-int launch_sinc0(const float* wav, const float* mean, const float* rstd, float wn_gamma, float wn_beta,
-                 const float* filt, int B, const Geom& g, float* p0, cudaStream_t st) {
-  ProfScope _ps("sinc0", st);
-  static bool attr_done[64] = {};
-  const size_t smem = (size_t)(SINC_K * SINC_F + ((SINC_XSEG + 3) & ~3)) * sizeof(float);
-  if (first_use_on_device(attr_done))
-    DG_CUDA(cudaFuncSetAttribute(sinc0_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int tiles_per_item = (g.T0 + SINC_TP - 1) / SINC_TP;
-  const int total = B * tiles_per_item;
-  const int grid = total < 2 * sms ? total : 2 * sms;
-  sinc0_kernel<<<grid, SINC_THREADS, smem, st>>>(wav, mean, rstd, wn_gamma, wn_beta, filt, B, g.S, g.T0, g.S0,
-                                                  tiles_per_item, p0);
   DG_LAUNCHED();
   return 0;
 }

@@ -45,23 +45,21 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
       : "memory");
 }
 
-// ---- 16-bit operand planes.  A float32 value travels as hi + lo; the element type is fp16 (default: |x| < 65504 and
-// 22 significand bits for the pair) or bf16 (16 bits for the pair, float32 range).  `f16` is warp-uniform.
-__device__ __forceinline__ uint16_t f32_to_h16(float x, int f16) {
+// ---- 16-bit operand planes.  A float32 value travels as hi + lo, both fp16: |x| < 65504 and 22 significand bits for
+// the pair.
+__device__ __forceinline__ uint16_t f32_to_h16(float x) {
   uint16_t r;
-  if (f16) asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(r) : "f"(x));
-  else asm("cvt.rn.bf16.f32 %0, %1;" : "=h"(r) : "f"(x));
+  asm("cvt.rn.satfinite.f16.f32 %0, %1;" : "=h"(r) : "f"(x));
   return r;
 }
-__device__ __forceinline__ float h16_to_f32(uint16_t h, int f16) {
+__device__ __forceinline__ float h16_to_f32(uint16_t h) {
   float f;
-  if (f16) asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(h));
-  else f = __uint_as_float((uint32_t)h << 16);
+  asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(h));
   return f;
 }
-__device__ __forceinline__ void split_h16(float x, int f16, uint16_t& hi, uint16_t& lo) {
-  hi = f32_to_h16(x, f16);
-  lo = f32_to_h16(x - h16_to_f32(hi, f16), f16);
+__device__ __forceinline__ void split_h16(float x, uint16_t& hi, uint16_t& lo) {
+  hi = f32_to_h16(x);
+  lo = f32_to_h16(x - h16_to_f32(hi));
 }
 __device__ __forceinline__ uint32_t pack_u16x2(uint16_t a, uint16_t b) { return (uint32_t)a | ((uint32_t)b << 16); }
 
@@ -129,93 +127,51 @@ __device__ __forceinline__ void wg_fence_acc(float (&d)[R]) {
 }
 
 // D (+)= A . B^T, A and B from shared memory (descriptors), both K-major; `acc` = 0 overwrites D
-template <int N, bool F16>
+template <int N>
 __device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc);
 // the same with A from registers (mma.m16n8k16 A-fragment layout per warp, rows 16 w .. 16 w + 15 of the 64)
-template <int N, bool F16>
+template <int N>
 __device__ __forceinline__ void wgmma_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t b, uint32_t acc);
 
 template <>
-__device__ __forceinline__ void wgmma_ss<8, true>(float (&d)[4], uint64_t a, uint64_t b, uint32_t acc) {
+__device__ __forceinline__ void wgmma_ss<8>(float (&d)[4], uint64_t a, uint64_t b, uint32_t acc) {
   asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %6, 0;\n"
                "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 {%0, %1, %2, %3}, %4, %5, p, 1, 1, 0, 0;\n}"
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
                : "l"(a), "l"(b), "r"(acc));
 }
 template <>
-__device__ __forceinline__ void wgmma_ss<8, false>(float (&d)[4], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %6, 0;\n"
-               "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 {%0, %1, %2, %3}, %4, %5, p, 1, 1, 0, 0;\n}"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "l"(a), "l"(b), "r"(acc));
-}
-template <>
-__device__ __forceinline__ void wgmma_ss<32, true>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+__device__ __forceinline__ void wgmma_ss<32>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
   asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
                "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}"
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
                : "l"(a), "l"(b), "r"(acc));
 }
 template <>
-__device__ __forceinline__ void wgmma_ss<32, false>(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
-               "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-               : "l"(a), "l"(b), "r"(acc));
-}
-template <>
-__device__ __forceinline__ void wgmma_ss<64, true>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+__device__ __forceinline__ void wgmma_ss<64>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
   asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
                "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}"
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
                : "l"(a), "l"(b), "r"(acc));
 }
 template <>
-__device__ __forceinline__ void wgmma_ss<64, false>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
-               "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-               : "l"(a), "l"(b), "r"(acc));
-}
-template <>
-__device__ __forceinline__ void wgmma_ss<80, true>(float (&d)[40], uint64_t a, uint64_t b, uint32_t acc) {
+__device__ __forceinline__ void wgmma_ss<80>(float (&d)[40], uint64_t a, uint64_t b, uint32_t acc) {
   asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %42, 0;\n"
                "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, 0, 0;\n}"
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
                : "l"(a), "l"(b), "r"(acc));
 }
 template <>
-__device__ __forceinline__ void wgmma_ss<80, false>(float (&d)[40], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %42, 0;\n"
-               "wgmma.mma_async.sync.aligned.m64n80k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, 0, 0;\n}"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
-               : "l"(a), "l"(b), "r"(acc));
-}
-template <>
-__device__ __forceinline__ void wgmma_ss<128, true>(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+__device__ __forceinline__ void wgmma_ss<128>(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
   asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
                "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}"
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
                : "l"(a), "l"(b), "r"(acc));
 }
 template <>
-__device__ __forceinline__ void wgmma_ss<128, false>(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
-               "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-               : "l"(a), "l"(b), "r"(acc));
-}
-template <>
-__device__ __forceinline__ void wgmma_rs<8, true>(float (&d)[4], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
+__device__ __forceinline__ void wgmma_rs<8>(float (&d)[4], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
   asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %9, 0;\n"
                "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 {%0, %1, %2, %3}, {%4, %5, %6, %7}, %8, p, 1, 1, 0;\n}"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
-}
-template <>
-__device__ __forceinline__ void wgmma_rs<8, false>(float (&d)[4], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
-  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %9, 0;\n"
-               "wgmma.mma_async.sync.aligned.m64n8k16.f32.bf16.bf16 {%0, %1, %2, %3}, {%4, %5, %6, %7}, %8, p, 1, 1, 0;\n}"
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc));
 }

@@ -130,7 +130,7 @@ int dg_pipeline_step(dg_pipeline* h, const float* wav_dev /*[B,S]*/, int B, int 
                      int32_t* map_dev /*[B,K]*/, float* permuted_dev /*[B,F,M] or NULL*/, void* stream);
 /* Hint: consecutive windows of a batch are `hop_samples` apart in ONE stream (reference config.step x sample_rate;
  * windows as `rearrange_audio_stream` emits them, src/diart/operators.py:44-100).  The pipeline then verifies the overlap on the device for every batch (bit comparison) and, when it holds, runs the
- * sinc layer once over the unique samples instead of once per window (DG_STREAM_SINC=0 disables this).  0 = no hint
+ * sinc layer once over the unique samples instead of once per window.  0 = no hint
  * (default).  Results never depend on the hint being right. */
 int dg_pipeline_set_hop(dg_pipeline* h, int hop_samples);
 /* Same with HOST buffers: H2D of the waveforms and D2H of the results inside the call
@@ -218,13 +218,12 @@ int64_t dg_launch_count(void);
  * every kernel launch is bracketed by two events; dg_profile_report() synchronises the device and
  * writes {"kernel": {"count": n, "ms": total}, ...} into buf. */
 int dg_profile_enable(int enable);
-/* test hook: the same random shifted-window GEMM through the float32 SIMT kernel and the wgmma (bf16x3)
- * kernel; epi 0 = bias -> f32, 1 = bias+leaky+bn -> bf16 hi/lo planes, 2 = bias+leaky+bn -> f32. */
+/* test hook: the same random shifted-window GEMM through the float32 reference kernel and the wgmma (fp16 hi/lo,
+ * three products) kernel; epi 0 = bias -> f32, 1 = bias+leaky+bn -> fp16 hi/lo planes, 2 = bias+leaky+bn -> f32. */
 int dg_selftest_gemm_tc(int M, int Cin, int KW, int dil, int N, int epi, float* max_abs_diff, float* out_rms);
-/* test hook (host only, no GPU): the weight-side split of float32 values into the two 16-bit operand planes
- * (hi = rn16(x), lo = rn16(x - hi)); f16 = 1 -> IEEE fp16 (saturating), 0 -> bf16.  What the device does to
- * activations with cvt.rn(.satfinite).f16/bf16.f32. */
-int dg_selftest_split_host(const float* x, long long n, int f16, unsigned short* hi, unsigned short* lo);
+/* test hook (host only, no GPU): the weight-side split of float32 values into the two IEEE fp16 operand planes
+ * (hi = rn16(x), lo = rn16(x - hi), saturating).  What the device does to activations with cvt.rn.satfinite.f16.f32. */
+int dg_selftest_split_f16_host(const float* x, long long n, unsigned short* hi, unsigned short* lo);
 int dg_profile_report(char* buf, int cap);
 
 /* ---- shared-identity mode (extension beyond the reference; SURVEY.md 8(e), BASELINE config 5): G ranks diarize

@@ -36,9 +36,9 @@ def test_argument_errors_without_gpu():
     assert lib.dg_cluster_create(64, 512, 0.6, 0.3, 1.0, 0, ctypes.byref(out)) == -1   # > 32 global speakers
 
 
-def test_host_operand_split_matches_ieee():
-    """The host-side hi/lo split of weights (fp16 default, bf16 alternative) is IEEE round-to-nearest-even:
-    checked against numpy float16 / a bit-level bf16 model, including subnormals, ties and saturation."""
+def test_host_fp16_split_matches_ieee():
+    """The host-side hi/lo split of weights into fp16 planes is IEEE round-to-nearest-even: checked against numpy
+    float16, including subnormals, ties and saturation."""
     import numpy as np
 
     lib = _lib.lib()
@@ -49,27 +49,16 @@ def test_host_operand_split_matches_ieee():
                   3.0e-8, 8.9e-8, 1.0009766, 1.0004883, 1.0014648, np.inf, -np.inf], np.float32)])
     hi = np.empty(x.size, np.uint16)
     lo = np.empty(x.size, np.uint16)
-    for f16 in (1, 0):
-        assert lib.dg_selftest_split_host(x.ctypes.data, x.size, f16, hi.ctypes.data, lo.ctypes.data) == 0
-        if f16:
-            with np.errstate(over="ignore"):
-                ref_hi = np.clip(x, -65504, 65504).astype(np.float16)
-                ref_hi = np.where(np.abs(x) >= 65520, np.sign(x) * np.float16(65504), x.astype(np.float16)).astype(np.float16)
-                res = x - ref_hi.astype(np.float32)
-                ref_lo = np.where(np.abs(res) >= 65520, np.sign(res) * np.float16(65504), res.astype(np.float16)).astype(np.float16)
-            assert np.array_equal(hi, ref_hi.view(np.uint16))
-            fin = np.isfinite(x)
-            assert np.array_equal(lo[fin], ref_lo.view(np.uint16)[fin])
-            back = hi.view(np.float16).astype(np.float64) + lo.view(np.float16).astype(np.float64)
-            ok = fin & (np.abs(x) < 6e4)
-            # 22 significand bits for the pair, with the absolute floor of the fp16 subnormal step (2^-25 after rounding)
-            assert np.all(np.abs(back[ok] - x[ok]) <= np.maximum(np.abs(x[ok]) * 2.0 ** -21, 2.0 ** -25 * 1.0001))
-        else:
-            def bf16(v):
-                u = v.view(np.uint32).astype(np.uint64)
-                return (((u + 0x7FFF + ((u >> 16) & 1)) >> 16) & 0xFFFF).astype(np.uint16)
-            fin = np.isfinite(x)
-            ref_hi = bf16(x)
-            assert np.array_equal(hi[fin], ref_hi[fin])
-            res = (x - (ref_hi.astype(np.uint32) << 16).view(np.float32)).astype(np.float32)
-            assert np.array_equal(lo[fin], bf16(res)[fin])
+    assert lib.dg_selftest_split_f16_host(x.ctypes.data, x.size, hi.ctypes.data, lo.ctypes.data) == 0
+    with np.errstate(over="ignore"):
+        ref_hi = np.clip(x, -65504, 65504).astype(np.float16)
+        ref_hi = np.where(np.abs(x) >= 65520, np.sign(x) * np.float16(65504), x.astype(np.float16)).astype(np.float16)
+        res = x - ref_hi.astype(np.float32)
+        ref_lo = np.where(np.abs(res) >= 65520, np.sign(res) * np.float16(65504), res.astype(np.float16)).astype(np.float16)
+    assert np.array_equal(hi, ref_hi.view(np.uint16))
+    fin = np.isfinite(x)
+    assert np.array_equal(lo[fin], ref_lo.view(np.uint16)[fin])
+    back = hi.view(np.float16).astype(np.float64) + lo.view(np.float16).astype(np.float64)
+    ok = fin & (np.abs(x) < 6e4)
+    # 22 significand bits for the pair, with the absolute floor of the fp16 subnormal step (2^-25 after rounding)
+    assert np.all(np.abs(back[ok] - x[ok]) <= np.maximum(np.abs(x[ok]) * 2.0 ** -21, 2.0 ** -25 * 1.0001))
