@@ -59,7 +59,6 @@ int launch_stats_pool_ex(const float* x, int stride, int T, int C, const float* 
 struct DevBuf {
   void* p = nullptr;
   size_t bytes = 0;
-  float wscale = 1.f;   // weight hi planes: the power-of-two factor both planes were multiplied by (upload_split)
   int ensure(size_t n) {
     if (n <= bytes) return 0;
     if (p) cudaFree(p);
@@ -81,27 +80,79 @@ struct DevBuf {
   }
 };
 
+// An owned CUDA handle, freed by `Free`; movable, not copyable.  A handle struct that holds its streams, events and pinned
+// memory this way frees everything it created, also when its creation fails halfway.
+template <class H, cudaError_t (*Free)(H)>
+struct Owned {
+  H h = nullptr;
+  Owned() = default;
+  Owned(Owned&& o) noexcept : h(o.h) { o.h = nullptr; }
+  Owned& operator=(Owned&& o) noexcept {
+    std::swap(h, o.h);
+    return *this;
+  }
+  ~Owned() {
+    if (h) Free(h);
+  }
+  operator H() const { return h; }
+};
+struct Stream : Owned<cudaStream_t, cudaStreamDestroy> {
+  int create(int priority = 0) {   // 0: the default priority
+    DG_CUDA(cudaStreamCreateWithPriority(&h, cudaStreamNonBlocking, priority));
+    return 0;
+  }
+};
+struct Event : Owned<cudaEvent_t, cudaEventDestroy> {
+  int create() {
+    DG_CUDA(cudaEventCreateWithFlags(&h, cudaEventDisableTiming));
+    return 0;
+  }
+};
+struct PinnedBuf : Owned<void*, cudaFreeHost> {
+  size_t bytes = 0;
+  int ensure(size_t n) {   // like DevBuf::ensure, without clearing
+    if (n <= bytes) return 0;
+    if (h) cudaFreeHost(h);
+    h = nullptr;
+    bytes = 0;
+    DG_CUDA(cudaHostAlloc(&h, n, cudaHostAllocDefault));
+    bytes = n;
+    return 0;
+  }
+  template <class T>
+  T* as() const { return reinterpret_cast<T*>(h); }
+};
+
 // A model handle owns ONE set of activation buffers per scratch lane.  A new user of a lane -- another pipeline built on the same
 // handle, or a block-level call on another stream -- first waits, stream-ordered, for the previous user's last kernel; without it
 // two users in flight would silently overwrite each other's activations.  (Host threads: a handle is single-threaded.)
 struct UseGuard {
-  cudaEvent_t e = nullptr;
-  const void* owner = nullptr;
-  ~UseGuard() {
-    if (e) cudaEventDestroy(e);
+  Event e;                       // recorded at the end of the last use
+  const void* owner = nullptr;   // who made it
+};
+// One use of a lane by `owner` on `st`: the constructor makes `st` wait for a previous user's end (`rc` = its result); end(), or
+// the destructor on any other exit, records this use's end, so that the next user also waits for what an error left enqueued.
+struct LaneUse {
+  UseGuard& u;
+  const void* owner;
+  cudaStream_t st;
+  int rc;
+  bool open = true;
+  LaneUse(UseGuard& u_, const void* owner_, cudaStream_t st_) : u(u_), owner(owner_), st(st_), rc(begin()) {}
+  ~LaneUse() { end(); }
+  int end() {
+    if (!open) return 0;
+    open = false;
+    if (!u.e && u.e.create()) return DG_ECUDA;
+    DG_CUDA(cudaEventRecord(u.e, st));
+    u.owner = owner;
+    return 0;
+  }
+  int begin() {
+    if (u.e && u.owner != owner) DG_CUDA(cudaStreamWaitEvent(st, u.e, 0));
+    return 0;
   }
 };
-static thread_local bool g_in_pipeline = false;      // the fused pipeline brackets its own uses (per lane)
-static int use_begin(UseGuard& u, const void* owner, cudaStream_t st) {
-  if (u.e && u.owner != owner) DG_CUDA(cudaStreamWaitEvent(st, u.e, 0));
-  return 0;
-}
-static int use_end(UseGuard& u, const void* owner, cudaStream_t st) {
-  if (!u.e) DG_CUDA(cudaEventCreateWithFlags(&u.e, cudaEventDisableTiming));
-  DG_CUDA(cudaEventRecord(u.e, st));
-  u.owner = owner;
-  return 0;
-}
 
 struct Tensors {
   std::map<std::string, std::pair<const float*, int64_t>> m;
@@ -134,12 +185,36 @@ static int upload_u16(DevBuf& b, const std::vector<uint16_t>& h) {
   return 0;
 }
 
-// float32 [N][K] host weights -> zero-padded fp16 hi/lo device planes [Npad][K]
-static int upload_split(DevBuf& hi, DevBuf& lo, const std::vector<float>& w_nk, int N, int Npad, int K) {
+// The B operand of a tensor-core GEMM: fp16 hi/lo planes [Npad][K] of float32 weights that were multiplied by `scale` (a power
+// of two) before the split.  Npad, the row count the GEMM's tiles read, is decided here once, at upload.
+struct WeightPlanes {
+  DevBuf hi, lo;
+  float scale = 1.f;
+  int Npad = 0, K = 0;
+};
+
+// float32 [N][K] host weights -> zero-padded planes [Npad][K]
+static int upload_split(WeightPlanes& w, const std::vector<float>& w_nk, int N, int Npad, int K) {
   std::vector<uint16_t> h((size_t)Npad * K), l((size_t)Npad * K);
-  hi.wscale = lo.wscale = weight_plane_scale(w_nk.data(), (size_t)N * K);
-  split_weights_host(w_nk.data(), N, Npad, K, h.data(), l.data(), hi.wscale);
-  return (upload_u16(hi, h) || upload_u16(lo, l)) ? DG_ECUDA : 0;
+  w.scale = weight_plane_scale(w_nk.data(), (size_t)N * K);
+  w.Npad = Npad;
+  w.K = K;
+  split_weights_host(w_nk.data(), N, Npad, K, h.data(), l.data(), w.scale);
+  return (upload_u16(w.hi, h) || upload_u16(w.lo, l)) ? DG_ECUDA : 0;
+}
+
+// points `t` at its weight planes; the launch's taps and channels (KW, Cin) must span exactly the planes' K
+static int set_weights(TcGemm& t, const WeightPlanes& w) {
+  if (t.KW * t.Cin != w.K) {
+    set_error(std::string(t.tag ? t.tag : "gemm_tc") + ": the launch reads K = " + std::to_string(t.KW * t.Cin) +
+              " but the weight planes have K = " + std::to_string(w.K));
+    return DG_EINVAL;
+  }
+  t.W_hi = w.hi.p;
+  t.W_lo = w.lo.p;
+  t.w_scale = w.scale;
+  t.Npad = w.Npad;
+  return 0;
 }
 
 static int upload(DevBuf& b, const std::vector<float>& h) {
@@ -152,7 +227,7 @@ static int upload(DevBuf& b, const std::vector<float>& h) {
 struct SincWeights {
   float wn_gamma = 1.f, wn_beta = 0.f;
   DevBuf g0, b0, bias1, g1, b1, bias2, g2, b2;
-  DevBuf w1_hi, w1_lo, w2_hi, w2_lo;   // conv weights as fp16 hi/lo planes [64][448] (taps folded into K: 5 x 80 + pad) and [64][5*64]
+  WeightPlanes w1, w2;                 // conv weights [64][448] (taps folded into K: 5 x 80 + pad) and [64][5*64]
   DevBuf filt_planes;                  // sinc filter bank as fp16 planes [2][80][256] (hi, lo)
   DevBuf cf;                           // folded wav-norm affine: beta * sum_k h[f][k]
   DevBuf hsum;                         // sum_k h[f][k] (stream form of the sinc layer)
@@ -220,14 +295,14 @@ static int prep_sincnet(const Tensors& t, const std::string& pre, SincWeights& w
       (rc = pad_vec(pre + "norm1d.2.weight", 60, 64, w.g2)) || (rc = pad_vec(pre + "norm1d.2.bias", 60, 64, w.b2)) ||
       (rc = pad_vec(pre + "conv1d.1.bias", 60, 64, w.bias1)) || (rc = pad_vec(pre + "conv1d.2.bias", 60, 64, w.bias2)))
     return rc;
-  auto conv_w_tc = [&](const std::string& name, int out, int in, int k, int in_pad, DevBuf& hi, DevBuf& lo) -> int {
+  auto conv_w_tc = [&](const std::string& name, int out, int in, int k, int in_pad, WeightPlanes& dst) -> int {
     const float* s = t.get(name, (int64_t)out * in * k);
     if (!s) return DG_EWEIGHT;
     std::vector<float> w_nk((size_t)out * k * in_pad, 0.f);
     for (int o = 0; o < out; o++)
       for (int c = 0; c < in; c++)
         for (int j = 0; j < k; j++) w_nk[(size_t)o * k * in_pad + j * in_pad + c] = s[((size_t)o * in + c) * k + j];
-    return upload_split(hi, lo, w_nk, out, 64, k * in_pad);
+    return upload_split(dst, w_nk, out, 64, k * in_pad);
   };
   {
     // Conv1d(80, 60, 5) with its taps folded into K: the input planes are 80-channel rows (pitch 160 B), so the im2col row of
@@ -238,9 +313,9 @@ static int prep_sincnet(const Tensors& t, const std::string& pre, SincWeights& w
     for (int o = 0; o < 60; o++)
       for (int c = 0; c < 80; c++)
         for (int j = 0; j < 5; j++) w_nk[(size_t)o * 448 + j * 80 + c] = s1[((size_t)o * 80 + c) * 5 + j];
-    if (upload_split(w.w1_hi, w.w1_lo, w_nk, 60, 64, 448)) return DG_ECUDA;
+    if (upload_split(w.w1, w_nk, 60, 64, 448)) return DG_ECUDA;
   }
-  if ((rc = conv_w_tc(pre + "conv1d.2.weight", 60, 60, 5, 64, w.w2_hi, w.w2_lo))) return rc;
+  if ((rc = conv_w_tc(pre + "conv1d.2.weight", 60, 60, 5, 64, w.w2))) return rc;
   return 0;
 }
 
@@ -357,19 +432,17 @@ static int run_sincnet(const SincWeights& w, SincWork& k, const float* wav, int 
     if (k.part3.ensure((size_t)(M0 / tr0) * 2 * 2 * 64 * 4)) return DG_ECUDA;
     TcGemm t{};
     t.A_hi = k.a0h.p; t.A_lo = k.a0l.p; t.lda = 80; t.Cin = 448; t.KW = 1; t.dil = 1; t.Mtot = M0; t.M = M0;
-    t.W_hi = w.w1_hi.p; t.w_scale = w.w1_hi.wscale; t.W_lo = w.w1_lo.p; t.Npad = 64; t.N = 64; t.bias = w.bias1.as<float>();
-    t.out_f32 = k.p1.as<float>(); t.ldc = 64; t.epi = 5; t.tag = "sinc_conv1";
+    t.N = 64; t.bias = w.bias1.as<float>(); t.out_f32 = k.p1.as<float>(); t.ldc = 64; t.epi = 5; t.tag = "sinc_conv1";
     t.pool_part = k.part3.as<float>(); t.pool_item_rows = g.S0; t.pool3_T = g.T1; t.pool3_tile_rows = tr0;
-    if ((rc = launch_gemm_tc(t, st)) ||
+    if ((rc = set_weights(t, w.w1)) || (rc = launch_gemm_tc(t, st)) ||
         (rc = launch_instnorm_finalize(k.part3.as<float>(), B, g.S0, tr0, g.T1, 64, 64, w.bias1.as<float>(), w.g1.as<float>(),
                                        w.b1.as<float>(), k.sc1.as<float>(), k.sh1.as<float>(), 64, st)) ||
         (rc = launch_split_ex(k.p1.as<float>(), M1, 64, 64, 64, 0, g.S1, k.sc1.as<float>(), k.sh1.as<float>(), k.a1h.p, k.a1l.p, st)))
       return rc;
     t.A_hi = k.a1h.p; t.A_lo = k.a1l.p; t.lda = 64; t.Cin = 64; t.KW = 5; t.Mtot = M1; t.M = M1;
-    t.W_hi = w.w2_hi.p; t.w_scale = w.w2_hi.wscale; t.W_lo = w.w2_lo.p; t.bias = w.bias2.as<float>();
-    t.out_f32 = k.p2.as<float>(); t.tag = "sinc_conv2";
+    t.bias = w.bias2.as<float>(); t.out_f32 = k.p2.as<float>(); t.tag = "sinc_conv2";
     t.pool_item_rows = g.S1; t.pool3_T = g.T2; t.pool3_tile_rows = tr1;
-    if ((rc = launch_gemm_tc(t, st))) return rc;
+    if ((rc = set_weights(t, w.w2)) || (rc = launch_gemm_tc(t, st))) return rc;
     k.out = k.p2.as<float>();
     k.out_pool = 0;
     return launch_instnorm_finalize(k.part3.as<float>(), B, g.S1, tr1, g.T2, 64, 64, w.bias2.as<float>(), w.g2.as<float>(),
@@ -377,9 +450,8 @@ static int run_sincnet(const SincWeights& w, SincWork& k, const float* wav, int 
   }
   TcGemm t{};
   t.A_hi = k.a0h.p; t.A_lo = k.a0l.p; t.lda = 80; t.Cin = 448; t.KW = 1; t.dil = 1; t.Mtot = M0; t.M = M0;
-  t.W_hi = w.w1_hi.p; t.w_scale = w.w1_hi.wscale; t.W_lo = w.w1_lo.p; t.Npad = 64; t.N = 64; t.bias = w.bias1.as<float>();
-  t.out_f32 = k.c1.as<float>(); t.ldc = 64; t.epi = 0; t.tag = "sinc_conv1";
-  if ((rc = launch_gemm_tc(t, st))) return rc;
+  t.N = 64; t.bias = w.bias1.as<float>(); t.out_f32 = k.c1.as<float>(); t.ldc = 64; t.epi = 0; t.tag = "sinc_conv1";
+  if ((rc = set_weights(t, w.w1)) || (rc = launch_gemm_tc(t, st))) return rc;
   if ((rc = launch_instnorm_stats(k.c1.as<float>(), B, g.S0, g.T1, 64, 64, w.g1.as<float>(), w.b1.as<float>(),
                                   k.sc1.as<float>(), k.sh1.as<float>(), st, 1)))
     return rc;
@@ -388,9 +460,8 @@ static int run_sincnet(const SincWeights& w, SincWork& k, const float* wav, int 
                             k.a1h.p, k.a1l.p, st)))
     return rc;
   t.A_hi = k.a1h.p; t.A_lo = k.a1l.p; t.lda = 64; t.Cin = 64; t.KW = 5; t.Mtot = M1; t.M = M1;
-  t.W_hi = w.w2_hi.p; t.w_scale = w.w2_hi.wscale; t.W_lo = w.w2_lo.p; t.bias = w.bias2.as<float>();
-  t.out_f32 = k.c2.as<float>(); t.tag = "sinc_conv2";
-  if ((rc = launch_gemm_tc(t, st))) return rc;
+  t.bias = w.bias2.as<float>(); t.out_f32 = k.c2.as<float>(); t.tag = "sinc_conv2";
+  if ((rc = set_weights(t, w.w2)) || (rc = launch_gemm_tc(t, st))) return rc;
   k.out = k.c2.as<float>();
   k.out_pool = 1;
   return launch_instnorm_stats(k.c2.as<float>(), B, g.S1, g.T2, 64, 64, w.g2.as<float>(), w.b2.as<float>(),
@@ -408,10 +479,11 @@ struct dg_seg {
   DevBuf ps_masks;                 // speaker bit set of every powerset class
   SincWeights sw;
   DevBuf bih[4];                   // input projection bias b_ih + b_hh [1024]
-  DevBuf wih_hi[4], wih_lo[4];     // input projections as fp16 hi/lo planes [1024][in_pad]
-  DevBuf whh_hi[4], whh_lo[4];     // W_hh as fp16 hi/lo planes [2][512][128] for the tensor-core recurrence
+  WeightPlanes wih[4];             // input projections [1024][in_pad]
+  WeightPlanes whh[4];             // W_hh [2][512][128] as lstm_tc_pack_whh lays it out (hi, lo, scale; no GEMM shape)
   DevBuf l1b, l2b, cw, cb;
-  DevBuf l1_hi, l1_lo, l2_hi, l2_lo, ones128, zeros128;   // head Linears as fp16 hi/lo planes [128][in]
+  WeightPlanes l1, l2;             // head Linears [128][in]
+  DevBuf ones128, zeros128;
   // activations: two independent sets ("lanes") so that the fused pipeline can run the segmentation chains of
   // two consecutive steps concurrently (the recurrence occupies only 32 SMs)
   struct Scratch {
@@ -420,9 +492,7 @@ struct dg_seg {
     DevBuf xh, xl;                 // fp16 hi/lo planes of the current in-projection input
     DevBuf y1h, y1l;               // fp16 planes of the first head Linear's output
   } scr[2];
-  int lane = 0;
-  const SincPrep* shared_prep = nullptr;   // set by the fused pipeline: statistics + planes computed once per step
-  UseGuard guard[2];                       // per scratch lane
+  UseGuard guard[2];               // per scratch lane
 };
 
 static int seg_prepare(dg_seg* h, const Tensors& t) {
@@ -445,11 +515,11 @@ static int seg_prepare(dg_seg* h, const Tensors& t) {
         b[d * 512 + r] = bi[r] + bh[r];
       }
     }
-    if (upload(h->bih[L], b) || upload_split(h->wih_hi[L], h->wih_lo[L], w_nk, 1024, 1024, in_pad)) return DG_ECUDA;
+    if (upload(h->bih[L], b) || upload_split(h->wih[L], w_nk, 1024, 1024, in_pad)) return DG_ECUDA;
     {
       std::vector<uint16_t> rh(lstm_tc_plane_elems()), rl(lstm_tc_plane_elems());
-      h->whh_hi[L].wscale = lstm_tc_pack_whh(hh[0], hh[1], rh.data(), rl.data());
-      if (upload_u16(h->whh_hi[L], rh) || upload_u16(h->whh_lo[L], rl)) return DG_ECUDA;
+      h->whh[L].scale = lstm_tc_pack_whh(hh[0], hh[1], rh.data(), rl.data());
+      if (upload_u16(h->whh[L].hi, rh) || upload_u16(h->whh[L].lo, rl)) return DG_ECUDA;
     }
   }
   {
@@ -459,8 +529,8 @@ static int seg_prepare(dg_seg* h, const Tensors& t) {
     const float* b1 = t.get("linear.1.bias", 128);
     if (!w0 || !b0 || !w1 || !b1) return DG_EWEIGHT;
     if (upload(h->l1b, std::vector<float>(b0, b0 + 128)) || upload(h->l2b, std::vector<float>(b1, b1 + 128)) ||
-        upload_split(h->l1_hi, h->l1_lo, std::vector<float>(w0, w0 + 128 * 256), 128, 128, 256) ||
-        upload_split(h->l2_hi, h->l2_lo, std::vector<float>(w1, w1 + 128 * 128), 128, 128, 128) ||
+        upload_split(h->l1, std::vector<float>(w0, w0 + 128 * 256), 128, 128, 256) ||
+        upload_split(h->l2, std::vector<float>(w1, w1 + 128 * 128), 128, 128, 128) ||
         upload(h->ones128, std::vector<float>(128, 1.f)) || upload(h->zeros128, std::vector<float>(128, 0.f)))
       return DG_ECUDA;
   }
@@ -593,28 +663,14 @@ static int seg_head_final(dg_seg* h, const float* y2, int B, const Geom& g, floa
   return launch_seg_final(y2, h->cw.as<float>(), h->cb.as<float>(), B, g.T2, g.S2, h->K, seg, st);
 }
 
-static int seg_forward_impl(dg_seg* h, const float* wav, int B, int S, float* seg, void* stream);
-extern "C" int dg_seg_forward(dg_seg* h, const float* wav, int B, int S, float* seg, void* stream) {
-  if (!h || !wav || !seg || B < 1 || S < 3000) {
-    set_error("dg_seg_forward: bad arguments (need B >= 1, S >= 3000)");
-    return DG_EINVAL;
-  }
-  if (g_in_pipeline) return seg_forward_impl(h, wav, B, S, seg, stream);
+// the forward on scratch lane `lane`, without the use bracket; `prep`: waveform statistics + planes the caller computed (or null)
+static int seg_forward_lane(dg_seg* h, int lane, const SincPrep* prep, const float* wav, int B, int S, float* seg,
+                            cudaStream_t st) {
   DG_CUDA(cudaSetDevice(h->device));
-  UseGuard& u = h->guard[h->lane & 1];
-  int rc = use_begin(u, stream ? stream : (void*)h, (cudaStream_t)stream);
-  if (!rc) rc = seg_forward_impl(h, wav, B, S, seg, stream);
-  if (!rc) rc = use_end(u, stream ? stream : (void*)h, (cudaStream_t)stream);
-  return rc;
-}
-
-static int seg_forward_impl(dg_seg* h, const float* wav, int B, int S, float* seg, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  DG_CUDA(cudaSetDevice(h->device));
-  dg_seg::Scratch& w = h->scr[h->lane & 1];
+  dg_seg::Scratch& w = h->scr[lane];
   const Geom g = make_geom(S);
   int rc;
-  if ((rc = run_sincnet(h->sw, w.work, wav, B, g, st, h->shared_prep))) return rc;
+  if ((rc = run_sincnet(h->sw, w.work, wav, B, g, st, prep))) return rc;
   const size_t rows = (size_t)B * g.S2 + 64;
   if (w.gx.ensure(rows * 1024 * 4) || w.y2.ensure(rows * 128 * 4) || w.xh.ensure(rows * 256 * 2) ||
       w.xl.ensure(rows * 256 * 2) || w.y1h.ensure(rows * 128 * 2) || w.y1l.ensure(rows * 128 * 2))
@@ -627,27 +683,37 @@ static int seg_forward_impl(dg_seg* h, const float* wav, int B, int S, float* se
     const int cin = L == 0 ? 64 : 256;
     TcGemm t{};
     t.A_hi = w.xh.p; t.A_lo = w.xl.p; t.lda = cin; t.Cin = cin; t.KW = 1; t.dil = 1; t.Mtot = M; t.M = M;
-    t.W_hi = h->wih_hi[L].p; t.w_scale = h->wih_hi[L].wscale; t.W_lo = h->wih_lo[L].p; t.Npad = 1024; t.N = 1024; t.bias = h->bih[L].as<float>();
-    t.out_f32 = w.gx.as<float>(); t.ldc = 1024; t.epi = 0; t.tag = "lstm_inproj";
-    if ((rc = launch_gemm_tc(t, st))) return rc;
+    t.N = 1024; t.bias = h->bih[L].as<float>(); t.out_f32 = w.gx.as<float>(); t.ldc = 1024; t.epi = 0; t.tag = "lstm_inproj";
+    if ((rc = set_weights(t, h->wih[L])) || (rc = launch_gemm_tc(t, st))) return rc;
     // the recurrence writes h_t straight into the operand planes of the next GEMM (the in-projection that read them has
     // completed in stream order)
-    if ((rc = launch_lstm_layer_tc(w.gx.as<float>(), h->whh_hi[L].p, h->whh_lo[L].p, h->whh_hi[L].wscale, B, g.T2, g.S2, nullptr,
+    if ((rc = launch_lstm_layer_tc(w.gx.as<float>(), h->whh[L].hi.p, h->whh[L].lo.p, h->whh[L].scale, B, g.T2, g.S2, nullptr,
                                    w.xh.p, w.xl.p, st)))
       return rc;
   }
   // Linear(256,128) -> leaky -> Linear(128,128) -> leaky on the tensor-core GEMM (identity "BatchNorm")
   TcGemm t{};
   t.A_hi = w.xh.p; t.A_lo = w.xl.p; t.lda = 256; t.Cin = 256; t.KW = 1; t.dil = 1; t.Mtot = M; t.M = M;
-  t.W_hi = h->l1_hi.p; t.w_scale = h->l1_hi.wscale; t.W_lo = h->l1_lo.p; t.Npad = 128; t.N = 128; t.bias = h->l1b.as<float>();
-  t.bn_scale = h->ones128.as<float>(); t.bn_shift = h->zeros128.as<float>();
+  t.N = 128; t.bias = h->l1b.as<float>(); t.bn_scale = h->ones128.as<float>(); t.bn_shift = h->zeros128.as<float>();
   t.out_hi = w.y1h.p; t.out_lo = w.y1l.p; t.ldc = 128; t.epi = 1; t.tag = "seg_linear";
-  if ((rc = launch_gemm_tc(t, st))) return rc;
-  t.A_hi = w.y1h.p; t.A_lo = w.y1l.p; t.lda = 128; t.Cin = 128;
-  t.W_hi = h->l2_hi.p; t.w_scale = h->l2_hi.wscale; t.W_lo = h->l2_lo.p; t.bias = h->l2b.as<float>();
+  if ((rc = set_weights(t, h->l1)) || (rc = launch_gemm_tc(t, st))) return rc;
+  t.A_hi = w.y1h.p; t.A_lo = w.y1l.p; t.lda = 128; t.Cin = 128; t.bias = h->l2b.as<float>();
   t.out_hi = nullptr; t.out_lo = nullptr; t.out_f32 = w.y2.as<float>(); t.epi = 2;
-  if ((rc = launch_gemm_tc(t, st))) return rc;
+  if ((rc = set_weights(t, h->l2)) || (rc = launch_gemm_tc(t, st))) return rc;
   return seg_head_final(h, w.y2.as<float>(), B, g, seg, st);
+}
+
+extern "C" int dg_seg_forward(dg_seg* h, const float* wav, int B, int S, float* seg, void* stream) {
+  if (!h || !wav || !seg || B < 1 || S < 3000) {
+    set_error("dg_seg_forward: bad arguments (need B >= 1, S >= 3000)");
+    return DG_EINVAL;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  DG_CUDA(cudaSetDevice(h->device));
+  LaneUse use(h->guard[0], stream ? stream : (void*)h, st);
+  int rc;
+  if ((rc = use.rc) || (rc = seg_forward_lane(h, 0, nullptr, wav, B, S, seg, st))) return rc;
+  return use.end();
 }
 
 extern "C" int dg_seg_destroy(dg_seg* h) {
@@ -660,8 +726,9 @@ struct dg_emb {
   int device = 0, pool_mode = 31, D = 512;
   SincWeights sw;
   DevBuf tb[5], bns[5], bnh[5];
-  DevBuf tw_hi[5], tw_lo[5];             // TDNN weights as fp16 hi/lo planes [Npad][K]
-  DevBuf ew_hi, ew_lo, ph, pl;           // Linear(3000, D): weights [Dpad][3008], pooled statistics planes
+  WeightPlanes tw[5];                    // TDNN weights [Npad][K]
+  WeightPlanes ew;                       // Linear(3000, D) weights [Dpad][3008] (WeSpeaker: Linear(5120, D))
+  DevBuf ph, pl;                         // pooled statistics planes
   DevBuf xh, xl, aH, aL, bH, bL;         // fp16 hi/lo activation planes
   DevBuf eb;
   SincWork work;
@@ -670,7 +737,6 @@ struct dg_emb {
   DevBuf idx0, idx1, lam1;
   int tab_F = -1, tab_T = -1;
   DevBuf flags, uniq, grp, gathered;   // compatibility path
-  const SincPrep* shared_prep = nullptr;
   // what the pooling reads after a trunk pass: x(item, t, c) = pool_x[item * pool_item_pitch + t * pool_row_pitch + c], c < pool_C
   const float* pool_x = nullptr;
   long long pool_item_pitch = 0;
@@ -685,14 +751,16 @@ struct dg_emb {
 struct ResConv {                       // Conv2d (3x3 pad 1 or 1x1, no bias) + folded BatchNorm2d(eval)
   int cin = 0, cout = 0, ksize = 3, stride = 1;
   int KW = 9, cin_gemm = 0, lda = 0;   // GEMM view: taps, channels consumed per tap, row pitch of the input planes
-  DevBuf w_hi, w_lo, sc, sh;
+  WeightPlanes w;
+  DevBuf sc, sh;
 };
 struct ResBlock {
   ResConv c1, c2, sc;
   bool has_sc = false;
 };
 struct ResNet {
-  DevBuf fb_hi, fb_lo, banks, k_lo, k_hi, stem_w, stem_sc, stem_sh;
+  WeightPlanes fb;               // kaldi fbank frame operator [640][448]
+  DevBuf banks, k_lo, k_hi, stem_w, stem_sc, stem_sh;
   std::vector<ResBlock> blocks;
   int stage_of[16];
   // work buffers: planes of the waveform, spectrum, log-mel map, three plane pairs per stage, float32 final map
@@ -738,7 +806,7 @@ static int emb_prepare(dg_emb* h, const Tensors& t) {
       for (int o = 0; o < out; o++)
         for (int c = 0; c < in; c++)
           for (int j = 0; j < k; j++) w_nk[(size_t)o * K + j * in_pad + c] = w[((size_t)o * in + c) * k + j];
-      if (upload_split(h->tw_hi[L], h->tw_lo[L], w_nk, out, npad, K)) return DG_ECUDA;
+      if (upload_split(h->tw[L], w_nk, out, npad, K)) return DG_ECUDA;
     }
     in = out;
     in_pad = out;
@@ -756,7 +824,7 @@ static int emb_prepare(dg_emb* h, const Tensors& t) {
   {
     std::vector<float> w_nk((size_t)dn * 3008, 0.f);
     for (int o = 0; o < dn; o++) memcpy(&w_nk[(size_t)o * 3008], ew + (size_t)o * 3000, 3000 * sizeof(float));
-    if (upload_split(h->ew_hi, h->ew_lo, w_nk, (int)dn, ((int)dn + 255) / 256 * 256, 3008)) return DG_ECUDA;
+    if (upload_split(h->ew, w_nk, (int)dn, ((int)dn + 255) / 256 * 256, 3008)) return DG_ECUDA;
   }
   return 0;
 }
@@ -800,7 +868,7 @@ static int resnet_conv_prepare(const Tensors& t, const std::string& conv, const 
     sc[o] = gm[o] / sqrtf(rv[o] + 1e-5f);
     sh[o] = bt[o] - rm[o] * sc[o];
   }
-  if (upload_split(c.w_hi, c.w_lo, w_nk, cout, npad, K) || upload(c.sc, sc) || upload(c.sh, sh)) return DG_ECUDA;
+  if (upload_split(c.w, w_nk, cout, npad, K) || upload(c.sc, sc) || upload(c.sh, sh)) return DG_ECUDA;
   return 0;
 }
 
@@ -814,7 +882,7 @@ static int resnet_prepare(dg_emb* h, const Tensors& t) {
     fbank_frame_operator(op);                                   // [514][400]
     std::vector<float> w_nk((size_t)514 * 448, 0.f);
     for (int n = 0; n < 514; n++) memcpy(&w_nk[(size_t)n * 448], &op[(size_t)n * 400], 400 * sizeof(float));
-    if (upload_split(r.fb_hi, r.fb_lo, w_nk, 514, 640, 448)) return DG_ECUDA;
+    if (upload_split(r.fb, w_nk, 514, 640, 448)) return DG_ECUDA;
     std::vector<float> banks;
     std::vector<int> lo, hi;
     fbank_mel_banks(banks, lo, hi);
@@ -867,7 +935,7 @@ static int resnet_prepare(dg_emb* h, const Tensors& t) {
     for (int half = 0; half < 2; half++)
       for (int hh = 0; hh < 10; hh++)
         for (int c = 0; c < 256; c++) w_nk[(size_t)o * 5120 + half * 2560 + hh * 256 + c] = ew[(size_t)o * 5120 + half * 2560 + c * 10 + hh];
-  if (upload_split(h->ew_hi, h->ew_lo, w_nk, (int)dn, ((int)dn + 255) / 256 * 256, 5120) ||
+  if (upload_split(h->ew, w_nk, (int)dn, ((int)dn + 255) / 256 * 256, 5120) ||
       upload(h->eb, std::vector<float>(eb, eb + dn)))
     return DG_ECUDA;
   h->pool_C = 2560;
@@ -906,12 +974,12 @@ static int resnet_conv(const ResConv& c, const void* in_hi, const void* in_lo, i
   TcGemm t{};
   const long long rows = (long long)U * Wp * Hp;
   t.A_hi = in_hi; t.A_lo = in_lo; t.lda = c.lda; t.Cin = c.cin_gemm; t.KW = c.KW; t.dil = 1; t.Mtot = rows; t.M = rows;
-  t.W_hi = c.w_hi.p; t.w_scale = c.w_hi.wscale; t.W_lo = c.w_lo.p; t.Npad = c.cout <= 64 ? c.cout : (c.cout + 127) / 128 * 128; t.N = c.cout;
-  t.bn_scale = c.sc.as<float>(); t.bn_shift = c.sh.as<float>();
+  t.N = c.cout; t.bn_scale = c.sc.as<float>(); t.bn_shift = c.sh.as<float>();
   t.out_hi = out_hi; t.out_lo = out_lo; t.out_f32 = out_f32; t.ldc = c.cout; t.epi = 3; t.tag = tag;
   t.tap_off = taps; t.Wp = Wp; t.Hp = Hp; t.Wop = Wop; t.Hop = Hop; t.stride2 = c.stride == 2; t.relu = relu;
   t.res_hi = res_hi; t.res_lo = res_lo;
-  return launch_gemm_tc(t, st);
+  const int rc = set_weights(t, c.w);
+  return rc ? rc : launch_gemm_tc(t, st);
 }
 
 // waveform [U,S] -> float32 final map [U][W3 + 2][H3 + 2][256] (h->pool_x descriptor), frames W3
@@ -946,9 +1014,8 @@ static int resnet_trunk(dg_emb* h, const float* wav, int U, int S, cudaStream_t 
     TcGemm t{};
     t.A_hi = r.wav_hi.p; t.A_lo = r.wav_lo.p; t.lda = 160; t.Cin = 448; t.KW = 1; t.dil = 1;
     t.Mtot = (long long)U * rpi; t.M = (long long)U * rpi;
-    t.W_hi = r.fb_hi.p; t.w_scale = r.fb_hi.wscale; t.W_lo = r.fb_lo.p; t.Npad = 640; t.N = 640; t.out_f32 = r.spec.as<float>(); t.ldc = 640; t.epi = 0;
-    t.tag = "fbank_dft";
-    if ((rc = launch_gemm_tc(t, st))) return rc;
+    t.N = 640; t.out_f32 = r.spec.as<float>(); t.ldc = 640; t.epi = 0; t.tag = "fbank_dft";
+    if ((rc = set_weights(t, r.fb)) || (rc = launch_gemm_tc(t, st))) return rc;
   }
   if ((rc = launch_fb_mel(r.spec.as<float>(), 640, rpi, g.T0, U, r.banks.as<float>(), r.k_lo.as<int>(), r.k_hi.as<int>(),
                           r.logmel.as<float>(), st)) ||
@@ -1120,11 +1187,13 @@ static int build_tables(dg_emb* h, int F, int T, cudaStream_t st) {
 }
 
 // waveform [U,S] -> t5 [U*S2, 1500]; returns the number of valid frames.
-// `defer_last`: stop before TDNN5 (its operand planes are left in h->t4h / t4l) -- the caller runs it fused with the pooling
-static int emb_trunk(dg_emb* h, const float* wav, int U, const Geom& g, cudaStream_t st, int* T_out, bool defer_last = false) {
+// `defer_last`: stop before TDNN5 (its operand planes are left in h->t4h / t4l) -- the caller runs it fused with the pooling.
+// `prep`: waveform statistics + planes the caller computed (or null)
+static int emb_trunk(dg_emb* h, const float* wav, int U, const Geom& g, cudaStream_t st, int* T_out, bool defer_last,
+                     const SincPrep* prep) {
   int rc;
   if (h->variant == 1) return resnet_trunk(h, wav, U, g.S, st, T_out);
-  if ((rc = run_sincnet(h->sw, h->work, wav, U, g, st, h->shared_prep))) return rc;
+  if ((rc = run_sincnet(h->sw, h->work, wav, U, g, st, prep))) return rc;
   const size_t rows = (size_t)U * g.S2 + 64;
   if (h->t5.ensure(rows * 1500 * 4)) return DG_ECUDA;
   h->pool_x = h->t5.as<float>();
@@ -1152,15 +1221,14 @@ static int emb_trunk(dg_emb* h, const float* wav, int U, const Geom& g, cudaStre
     }
     TcGemm t{};
     t.A_hi = ih; t.A_lo = il; t.lda = cin; t.Cin = cin; t.KW = TD_K[L]; t.dil = TD_DIL[L]; t.Mtot = M; t.M = M;
-    t.W_hi = h->tw_hi[L].p; t.w_scale = h->tw_hi[L].wscale; t.W_lo = h->tw_lo[L].p; t.Npad = (TD_OUT[L] + 255) / 256 * 256; t.N = TD_OUT[L];
-    t.bias = h->tb[L].as<float>(); t.bn_scale = h->bns[L].as<float>(); t.bn_shift = h->bnh[L].as<float>();
+    t.N = TD_OUT[L]; t.bias = h->tb[L].as<float>(); t.bn_scale = h->bns[L].as<float>(); t.bn_shift = h->bnh[L].as<float>();
     t.tag = kTags[L];
     if (L == 4) {
       t.out_f32 = h->t5.as<float>(); t.ldc = 1500; t.epi = 2;
     } else {
       t.out_hi = oh[L & 1]; t.out_lo = ol[L & 1]; t.ldc = 512; t.epi = 1;
     }
-    if ((rc = launch_gemm_tc(t, st))) return rc;
+    if ((rc = set_weights(t, h->tw[L])) || (rc = launch_gemm_tc(t, st))) return rc;
     ih = oh[L & 1]; il = ol[L & 1];
     cin = TD_OUT[L];
     T -= (TD_K[L] - 1) * TD_DIL[L];
@@ -1171,11 +1239,11 @@ static int emb_trunk(dg_emb* h, const float* wav, int U, const Geom& g, cudaStre
 
 // TDNN5 (Conv1d(512, 1500, 1) -> LeakyReLU -> BatchNorm) fused with the K weighted statistics poolings: the [rows, 1500] map
 // (455 MB at B = 256) is never written; the epilogue leaves per-tile partial sums, pool_finalize turns them into mean / std.
-static int emb_tdnn5_pool(dg_emb* h, int U, const Geom& g, const float* weights, int F, int K, int T, cudaStream_t st) {
+static int emb_tdnn5_pool(dg_emb* h, int U, const Geom& g, const float* weights, int F, int K, int T, float eps,
+                          cudaStream_t st) {
   int rc;
   const long long M = (long long)U * g.S2;
   const int m_tiles = (int)((M + 127) / 128);
-  const float eps = h->pool_mode == 31 ? 1e-8f : 0.f;
   if (h->pool_rw.ensure(((size_t)M + 128) * 16) || h->pool_vs.ensure((size_t)U * K * 8) ||
       h->pool_part.ensure((size_t)m_tiles * 2 * 8 * 1500 * 4) || h->pooled.ensure((size_t)U * K * 3000 * 4))
     return DG_ECUDA;
@@ -1184,11 +1252,10 @@ static int emb_tdnn5_pool(dg_emb* h, int U, const Geom& g, const float* weights,
     return rc;
   TcGemm t{};
   t.A_hi = h->t4h; t.A_lo = h->t4l; t.lda = 512; t.Cin = 512; t.KW = 1; t.dil = 1; t.Mtot = M; t.M = M;
-  t.W_hi = h->tw_hi[4].p; t.w_scale = h->tw_hi[4].wscale; t.W_lo = h->tw_lo[4].p; t.Npad = 1536; t.N = 1500;
-  t.bias = h->tb[4].as<float>(); t.bn_scale = h->bns[4].as<float>(); t.bn_shift = h->bnh[4].as<float>();
+  t.N = 1500; t.bias = h->tb[4].as<float>(); t.bn_scale = h->bns[4].as<float>(); t.bn_shift = h->bnh[4].as<float>();
   t.ldc = 1500; t.epi = 4; t.tag = "tdnn5";
   t.pool_w = h->pool_rw.as<float>(); t.pool_part = h->pool_part.as<float>(); t.pool_item_rows = g.S2; t.pool_K = K;
-  if ((rc = launch_gemm_tc(t, st))) return rc;
+  if ((rc = set_weights(t, h->tw[4])) || (rc = launch_gemm_tc(t, st))) return rc;
   h->pool_C = 1500;
   return launch_pool_finalize(h->pool_part.as<float>(), h->pool_vs.as<float>(), h->bnh[4].as<float>(), U, K, 1500, g.S2, T, eps,
                               h->pooled.as<float>(), st);
@@ -1207,10 +1274,42 @@ static int emb_project(dg_emb* h, int rows, int normalize, float norm, float* ou
   }
   TcGemm t{};
   t.A_hi = h->ph.p; t.A_lo = h->pl.p; t.lda = kpad; t.Cin = kpad; t.KW = 1; t.dil = 1; t.Mtot = rows; t.M = rows;
-  t.W_hi = h->ew_hi.p; t.w_scale = h->ew_hi.wscale; t.W_lo = h->ew_lo.p; t.Npad = (h->D + 255) / 256 * 256; t.N = h->D;
-  t.bias = h->eb.as<float>(); t.out_f32 = dst; t.ldc = h->D; t.epi = 0; t.tag = "emb_linear";
-  if ((rc = launch_gemm_tc(t, st))) return rc;
+  t.N = h->D; t.bias = h->eb.as<float>(); t.out_f32 = dst; t.ldc = h->D; t.epi = 0; t.tag = "emb_linear";
+  if ((rc = set_weights(t, h->ew)) || (rc = launch_gemm_tc(t, st))) return rc;
   return normalize ? launch_l2norm(dst, rows, h->D, norm, out, st) : 0;
+}
+
+// epsilon of the weighted statistics pooling: 1e-8 for pyannote's StatsPool with weights, none without them
+static float pool_eps(const dg_emb* h, const float* weights) { return weights && h->pool_mode == 31 ? 1e-8f : 0.f; }
+
+// the pooling can run fused with TDNN5 (emb_tdnn5_pool) for pooling weights of this many speakers at this chunk size
+static bool pool_fusable(const dg_emb* h, int K, const Geom& g) { return h->variant == 0 && K <= 4 && g.S2 >= 128; }
+
+// Sets g_sm_limit for its lifetime (0: no cap).
+struct SmLimit {
+  const int prev;
+  explicit SmLimit(int limit) : prev(g_sm_limit) { g_sm_limit = limit; }
+  ~SmLimit() { g_sm_limit = prev; }
+};
+
+// Everything after the embedding trunk: interpolation tables, the K weighted statistics poolings of each item -- fused with
+// TDNN5 when `fuse` (the trunk was run with defer_last) -- and the projection, into out [B*K, D].  `sm_cap` caps the grids of
+// the fused part (the un-fused pooling and its projection are not capped).
+static int emb_tail(dg_emb* h, int B, const Geom& g, const float* weights, int F, int K, int T, bool fuse, int normalize,
+                    float norm, float* out, cudaStream_t st, int sm_cap = 0) {
+  int rc;
+  if (weights && (rc = build_tables(h, F, T, st))) return rc;
+  const float eps = pool_eps(h, weights);
+  if (fuse) {
+    SmLimit cap(sm_cap);
+    if ((rc = emb_tdnn5_pool(h, B, g, weights, F, K, T, eps, st))) return rc;
+    return emb_project(h, B * K, normalize, norm, out, st);
+  }
+  if (h->pooled.ensure((size_t)B * K * 2 * h->pool_C * 4)) return DG_ECUDA;
+  if ((rc = launch_stats_pool(h->pool_x, B, g.S2, T, h->pool_C, weights, F, K, h->idx0.as<int>(), h->idx1.as<int>(),
+                              h->lam1.as<float>(), eps, h->pooled.as<float>(), st, h->pool_item_pitch, h->pool_row_pitch)))
+    return rc;
+  return emb_project(h, B * K, normalize, norm, out, st);
 }
 
 extern "C" int dg_emb_forward(dg_emb* h, const float* wav, const float* weights, int B, int S, int F, int K,
@@ -1223,26 +1322,11 @@ extern "C" int dg_emb_forward(dg_emb* h, const float* wav, const float* weights,
   DG_CUDA(cudaSetDevice(h->device));
   const Geom g = make_geom(S);
   int rc, T = 0;
-  const void* me = stream ? stream : (void*)h;
-  struct Done {              // every exit of this call marks the end of the use
-    dg_emb* h; const void* me; cudaStream_t st; bool on;
-    ~Done() { if (on) use_end(h->guard, me, st); }
-  } done{h, me, st, !g_in_pipeline};
-  if (!g_in_pipeline && (rc = use_begin(h->guard, me, st))) return rc;
-  const bool fuse = weights && h->variant == 0 && K <= 4 && g.S2 >= 128;
-  if ((rc = emb_trunk(h, wav, B, g, st, &T, fuse))) return rc;
-  if (weights && (rc = build_tables(h, F, T, st))) return rc;
-  if (fuse) {
-    if ((rc = emb_tdnn5_pool(h, B, g, weights, F, K, T, st))) return rc;
-    return emb_project(h, B * K, normalize, norm, out, st);
-  }
-  if (h->pooled.ensure((size_t)B * K * 2 * h->pool_C * 4)) return DG_ECUDA;
-  const float eps = h->pool_mode == 31 ? 1e-8f : 0.f;
-  if ((rc = launch_stats_pool(h->pool_x, B, g.S2, T, h->pool_C, weights, F, K, h->idx0.as<int>(),
-                              h->idx1.as<int>(), h->lam1.as<float>(), weights ? eps : 0.f,
-                              h->pooled.as<float>(), st, h->pool_item_pitch, h->pool_row_pitch)))
-    return rc;
-  return emb_project(h, B * K, normalize, norm, out, st);
+  LaneUse use(h->guard, stream ? stream : (void*)h, st);
+  if ((rc = use.rc)) return rc;
+  const bool fuse = weights && pool_fusable(h, K, g);
+  if ((rc = emb_trunk(h, wav, B, g, st, &T, fuse, nullptr))) return rc;
+  return emb_tail(h, B, g, weights, F, K, T, fuse, normalize, norm, out, st);
 }
 
 extern "C" int dg_emb_forward_rows(dg_emb* h, const float* wav, const float* weights, int N, int S, int F, float* out,
@@ -1255,12 +1339,8 @@ extern "C" int dg_emb_forward_rows(dg_emb* h, const float* wav, const float* wei
   DG_CUDA(cudaSetDevice(h->device));
   const Geom g = make_geom(S);
   int rc, T = 0;
-  const void* me = stream ? stream : (void*)h;
-  struct Done {
-    dg_emb* h; const void* me; cudaStream_t st; bool on;
-    ~Done() { if (on) use_end(h->guard, me, st); }
-  } done{h, me, st, !g_in_pipeline};
-  if (!g_in_pipeline && (rc = use_begin(h->guard, me, st))) return rc;
+  LaneUse use(h->guard, stream ? stream : (void*)h, st);
+  if ((rc = use.rc)) return rc;
   // consecutive identical rows (the reference repeats each waveform once per local speaker,
   // src/diart/blocks/embedding.py:57-59) share one trunk pass
   if (h->flags.ensure((size_t)N * 4)) return DG_ECUDA;
@@ -1294,13 +1374,12 @@ extern "C" int dg_emb_forward_rows(dg_emb* h, const float* wav, const float* wei
   memcpy(packed.data() + G, gq0.data(), G * 4);
   memcpy(packed.data() + 2 * G, gnq.data(), G * 4);
   DG_CUDA(cudaMemcpyAsync(h->grp.p, packed.data(), (size_t)3 * G * 4, cudaMemcpyHostToDevice, st));
-  if ((rc = emb_trunk(h, trunk_in, U, g, st, &T))) return rc;
+  if ((rc = emb_trunk(h, trunk_in, U, g, st, &T, false, nullptr))) return rc;
   if (weights && (rc = build_tables(h, F, T, st))) return rc;
   if (h->pooled.ensure((size_t)N * 2 * h->pool_C * 4)) return DG_ECUDA;
-  const float eps = (weights && h->pool_mode == 31) ? 1e-8f : 0.f;
   const int* gp = h->grp.as<int>();
   if ((rc = launch_stats_pool_ex(h->pool_x, g.S2, T, h->pool_C, weights, F, 1, 1, G, gp, gp + G, gp + 2 * G,
-                                 h->idx0.as<int>(), h->idx1.as<int>(), h->lam1.as<float>(), eps,
+                                 h->idx0.as<int>(), h->idx1.as<int>(), h->lam1.as<float>(), pool_eps(h, weights),
                                  h->pooled.as<float>(), st, h->pool_item_pitch, h->pool_row_pitch)))
     return rc;
   rc = emb_project(h, N, 0, 1.f, out, st);
@@ -1503,9 +1582,10 @@ extern "C" int dg_selftest_gemm_tc(int M, int Cin, int KW, int dil, int N, int e
     bsc[n] = 1.f + rnd();
     bsh[n] = rnd();
   }
-  DevBuf dA, dWkn, dWh, dWl, dB, dS, dH, dAh, dAl, dC0, dC1, dOh, dOl;
+  DevBuf dA, dWkn, dB, dS, dH, dAh, dAl, dC0, dC1, dOh, dOl;
+  WeightPlanes dW;
   if (upload(dA, A) || upload(dWkn, Wkn) || upload(dB, bias) || upload(dS, bsc) || upload(dH, bsh) ||
-      upload_split(dWh, dWl, Wnk, N, npad, K))
+      upload_split(dW, Wnk, N, npad, K))
     return DG_ECUDA;
   if (dAh.ensure((size_t)Mtot * Cin * 2) || dAl.ensure((size_t)Mtot * Cin * 2) || dC0.ensure((size_t)M * N * 4) ||
       dC1.ensure((size_t)M * N * 4) || dOh.ensure((size_t)M * N * 2) || dOl.ensure((size_t)M * N * 2))
@@ -1520,10 +1600,10 @@ extern "C" int dg_selftest_gemm_tc(int M, int Cin, int KW, int dil, int N, int e
   if ((rc = launch_split_ex(dA.as<float>(), Mtot, Cin, Cin, Cin, 0, 1, nullptr, nullptr, dAh.p, dAl.p, nullptr))) return rc;
   TcGemm t{};
   t.A_hi = dAh.p; t.A_lo = dAl.p; t.lda = Cin; t.Cin = Cin; t.KW = KW; t.dil = dil; t.Mtot = Mtot; t.M = M;
-  t.W_hi = dWh.p; t.w_scale = dWh.wscale; t.W_lo = dWl.p; t.Npad = npad; t.N = N; t.bias = dB.as<float>(); t.bn_scale = dS.as<float>();
+  t.N = N; t.bias = dB.as<float>(); t.bn_scale = dS.as<float>();
   t.bn_shift = dH.as<float>(); t.out_f32 = dC1.as<float>(); t.out_hi = dOh.p; t.out_lo = dOl.p; t.ldc = N;
   t.epi = epi; t.tag = "selftest_tc";
-  if ((rc = launch_gemm_tc(t, nullptr))) return rc;
+  if ((rc = set_weights(t, dW)) || (rc = launch_gemm_tc(t, nullptr))) return rc;
   DG_CUDA(cudaDeviceSynchronize());
   std::vector<float> c0((size_t)M * N), c1((size_t)M * N);
   DG_CUDA(cudaMemcpy(c0.data(), dC0.p, c0.size() * 4, cudaMemcpyDeviceToHost));
@@ -1630,34 +1710,31 @@ struct dg_pipeline {
   float gamma, beta;
   int normalize_weights;
   int hop = 0;          // samples between consecutive windows of a batch (hint, dg_pipeline_set_hop); 0 = unknown
+  // Members are destroyed in reverse order: the streams and events (declared last) first, then the pinned staging, then
+  // the device buffers and worker threads.
   DevBuf osp, wav, segd, embd, mapd, permd;
-  cudaStream_t st = nullptr;
-  // two-stream overlap inside a step: the segmentation chain (critical path, high priority) and the
-  // embedding trunk (independent of it until the pooling weights exist) run concurrently
-  cudaStream_t s_seg = nullptr, s_seg2 = nullptr, s_emb = nullptr, s_clu = nullptr, s_h2d = nullptr, s_d2h = nullptr;
   DevBuf osp2;
-  cudaEvent_t e_osp2 = nullptr;
   SincPrep prep[2];
-  cudaEvent_t e_prep[2] = {nullptr, nullptr};
-  cudaEvent_t e_start = nullptr, e_osp = nullptr, e_emb = nullptr, e_done = nullptr;
   // pipelining (dg_pipeline_submit* / collect*): up to DG_MAX_INFLIGHT steps outstanding.  Step n uses result / input
   // slot n % 3 and scratch lane n & 1: two steps compute concurrently (lanes), the third slot lets the host upload the
   // waveforms of step n+2 while steps n and n+1 are on the device
   DevBuf slot_wav[3], slot_seg[3], slot_emb[3], slot_map[3];
-  cudaEvent_t e_h2d[3] = {nullptr, nullptr, nullptr}, e_slot_done[3] = {nullptr, nullptr, nullptr};
-  cudaEvent_t e_lane_done[2] = {nullptr, nullptr};
   int slot_B[3] = {0, 0, 0}, slot_S[3] = {0, 0, 0}, outstanding = 0;
   long long next_step = 0;
-  // shared-identity mode inside the pipelined flow: export / merge run on the clustering stream, in order with the clustering
-  // of the submitted steps, so the networks of the next steps keep running meanwhile
-  cudaEvent_t e_ident = nullptr, e_ident_in = nullptr;
   long long ident_merged_upto = 0;      // steps below this index have had their maps relabelled by a merge
-  bool overlap_known = false;     // the current dg_pipeline_step batch was formed from a dg_stream (windows overlap by construction)
-  void* pin_wav = nullptr;        // pinned staging of dg_pipeline_call_host (B separate host windows -> one upload)
-  size_t pin_wav_bytes = 0;
   std::unique_ptr<GatherPool> gather;   // worker threads of the host gather (created at the first dg_pipeline_call_host)
   DevBuf call_stream;                   // device image of the stream a dg_pipeline_call_host batch was cut from
   long long call_h2d_bytes = 0;         // bytes the last dg_pipeline_call_host uploaded
+  PinnedBuf pin_wav;                    // pinned staging of dg_pipeline_call_host (B separate host windows -> one upload)
+  Stream st;
+  // two-stream overlap inside a step: the segmentation chain (critical path, high priority) and the
+  // embedding trunk (independent of it until the pooling weights exist) run concurrently
+  Stream s_seg, s_seg2, s_emb, s_clu, s_h2d, s_d2h;
+  Event e_osp2, e_prep[2], e_start, e_osp, e_emb, e_done;
+  Event e_h2d[3], e_slot_done[3], e_lane_done[2];
+  // shared-identity mode inside the pipelined flow: export / merge run on the clustering stream, in order with the clustering
+  // of the submitted steps, so the networks of the next steps keep running meanwhile (created at the first export)
+  Event e_ident, e_ident_in;
 };
 
 extern "C" int dg_pipeline_create(dg_seg* seg, dg_emb* emb, dg_cluster* clu, float gamma, float beta,
@@ -1678,34 +1755,20 @@ extern "C" int dg_pipeline_create(dg_seg* seg, dg_emb* emb, dg_cluster* clu, flo
   h->seg = seg; h->emb = emb; h->clu = clu;
   h->gamma = gamma; h->beta = beta; h->normalize_weights = normalize_weights;
   DG_CUDA(cudaSetDevice(seg->device));
-  DG_CUDA(cudaStreamCreateWithFlags(&h->st, cudaStreamNonBlocking));
   int lo = 0, hi = 0;
   DG_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-  DG_CUDA(cudaStreamCreateWithPriority(&h->s_seg, cudaStreamNonBlocking, hi));
-  DG_CUDA(cudaStreamCreateWithPriority(&h->s_emb, cudaStreamNonBlocking, lo));
-  DG_CUDA(cudaEventCreateWithFlags(&h->e_start, cudaEventDisableTiming));
-  DG_CUDA(cudaEventCreateWithFlags(&h->e_osp, cudaEventDisableTiming));
-  DG_CUDA(cudaEventCreateWithFlags(&h->e_emb, cudaEventDisableTiming));
-  DG_CUDA(cudaEventCreateWithFlags(&h->e_done, cudaEventDisableTiming));
-  DG_CUDA(cudaStreamCreateWithPriority(&h->s_clu, cudaStreamNonBlocking, hi));
-  DG_CUDA(cudaStreamCreateWithPriority(&h->s_seg2, cudaStreamNonBlocking, hi));
-  DG_CUDA(cudaEventCreateWithFlags(&h->e_osp2, cudaEventDisableTiming));
-  DG_CUDA(cudaEventCreateWithFlags(&h->e_prep[0], cudaEventDisableTiming));
-  DG_CUDA(cudaEventCreateWithFlags(&h->e_prep[1], cudaEventDisableTiming));
-  DG_CUDA(cudaStreamCreateWithFlags(&h->s_h2d, cudaStreamNonBlocking));
-  DG_CUDA(cudaStreamCreateWithFlags(&h->s_d2h, cudaStreamNonBlocking));
-  for (int i = 0; i < 3; i++) {
-    DG_CUDA(cudaEventCreateWithFlags(&h->e_h2d[i], cudaEventDisableTiming));
-    DG_CUDA(cudaEventCreateWithFlags(&h->e_slot_done[i], cudaEventDisableTiming));
-  }
-  for (int i = 0; i < 2; i++) DG_CUDA(cudaEventCreateWithFlags(&h->e_lane_done[i], cudaEventDisableTiming));
+  if (h->st.create() || h->s_seg.create(hi) || h->s_emb.create(lo) || h->s_clu.create(hi) || h->s_seg2.create(hi) ||
+      h->s_h2d.create() || h->s_d2h.create())
+    return DG_ECUDA;
+  for (Event* e : {&h->e_start, &h->e_osp, &h->e_emb, &h->e_done, &h->e_osp2, &h->e_prep[0], &h->e_prep[1], &h->e_h2d[0],
+                   &h->e_h2d[1], &h->e_h2d[2], &h->e_slot_done[0], &h->e_slot_done[1], &h->e_slot_done[2],
+                   &h->e_lane_done[0], &h->e_lane_done[1]})
+    if (e->create()) return DG_ECUDA;
   DG_CUDA(cudaEventRecord(h->e_emb, h->s_emb));   // so that the first step's wait on it is well defined
   *out = h.release();
   return DG_OK;
 }
 
-// segmentation chain on s_seg and embedding chain on s_emb, both starting after `start`; on return
-// e_emb (recorded on s_emb) marks seg, osp and emb complete
 // DG_CALL_TIMING=1: device time stamps of the sub-batches of dg_pipeline_call_host (diagnostic)
 struct CallDiag {
   cudaEvent_t t0 = nullptr, up[3], prep[3], trunk[3], seg[3], emb[3], clu[3];
@@ -1723,6 +1786,17 @@ static thread_local CallDiag* g_diag = nullptr;
     if (g_diag) cudaEventRecord(g_diag->field[g_diag->j], stream);    \
   } while (0)
 
+// grid cap of the embedding stream's persistent kernels while the segmentation stream runs a recurrence over B windows: the
+// SMs the recurrence leaves free, or no cap if that would be half of the device or less
+static int emb_sm_cap(int device, int B) {
+  int sms = 132;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+  const int lstm_ctas = lstm_tc_ctas(B);
+  return sms - lstm_ctas > sms / 2 ? sms - lstm_ctas : 0;
+}
+
+// segmentation chain on s_seg and embedding chain on s_emb, both starting after `start`; on return
+// e_emb (recorded on s_emb) marks seg, osp and emb complete
 static int pipeline_nets(dg_pipeline* h, const float* wav, int B, int S, int F, int K, float* seg, float* emb,
                          cudaEvent_t start, int lane = 0, int stream_hop = 0) {
   int rc;
@@ -1736,68 +1810,35 @@ static int pipeline_nets(dg_pipeline* h, const float* wav, int B, int S, int F, 
   DG_CUDA(cudaStreamWaitEvent(s_seg, start, 0));
   DG_CUDA(cudaStreamWaitEvent(h->s_emb, start, 0));
   // another pipeline (or a block-level call) that used these model handles' scratch last: stream-ordered hand-over
-  if ((rc = use_begin(h->seg->guard[lane], h, s_seg)) || (rc = use_begin(h->emb->guard, h, h->s_emb))) return rc;
-  struct InPipeline {
-    InPipeline() { g_in_pipeline = true; }
-    ~InPipeline() { g_in_pipeline = false; }
-  } in_pipeline;
+  LaneUse seg_use(h->seg->guard[lane], h, s_seg), emb_use(h->emb->guard, h, h->s_emb);
+  if ((rc = seg_use.rc) || (rc = emb_use.rc)) return rc;
   // waveform statistics + standardised fp16 planes once, for both networks' SincNets
-  if ((rc = run_sinc_prep(h->prep[lane], wav, B, g, s_seg, stream_hop ? stream_hop : h->hop, stream_hop != 0))) return rc;
+  SincPrep& prep = h->prep[lane];
+  if ((rc = run_sinc_prep(prep, wav, B, g, s_seg, stream_hop ? stream_hop : h->hop, stream_hop != 0))) return rc;
   DG_CUDA(cudaEventRecord(h->e_prep[lane], s_seg));
   DG_DIAG(prep, s_seg);
   DG_CUDA(cudaStreamWaitEvent(h->s_emb, h->e_prep[lane], 0));
-  const SincPrep* shared = &h->prep[lane];
   // embedding trunk first in host order (low-priority stream, grid capped to the SMs the LSTM leaves free)
   int T = 0;
-  const bool fuse_pool = h->emb->variant == 0 && K <= 4 && g.S2 >= 128;
+  const bool fuse = pool_fusable(h->emb, K, g);
+  const int sm_cap = emb_sm_cap(h->seg->device, B);
   {
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->seg->device);
-    const int lstm_ctas = lstm_tc_ctas(B);
-    g_sm_limit = sms - lstm_ctas > sms / 2 ? sms - lstm_ctas : 0;
-    h->emb->shared_prep = shared;
-    rc = emb_trunk(h->emb, wav, B, g, h->s_emb, &T, fuse_pool);
-    h->emb->shared_prep = nullptr;
-    g_sm_limit = 0;
-    if (rc) return rc;
-    DG_DIAG(trunk, h->s_emb);
+    SmLimit cap(sm_cap);
+    if ((rc = emb_trunk(h->emb, wav, B, g, h->s_emb, &T, fuse, &prep))) return rc;
   }
-  h->seg->lane = lane;
-  h->seg->shared_prep = shared;
-  rc = dg_seg_forward(h->seg, wav, B, S, seg, s_seg);
-  h->seg->lane = 0;
-  h->seg->shared_prep = nullptr;
-  if (rc) return rc;
+  DG_DIAG(trunk, h->s_emb);
+  if ((rc = seg_forward_lane(h->seg, lane, &prep, wav, B, S, seg, s_seg))) return rc;
   if ((rc = dg_osp(seg, B, F, K, h->gamma, h->beta, h->normalize_weights, osp.as<float>(), s_seg))) return rc;
   DG_CUDA(cudaEventRecord(e_osp, s_seg));
-  if ((rc = use_end(h->seg->guard[lane], h, s_seg))) return rc;
+  if ((rc = seg_use.end())) return rc;
   DG_DIAG(seg, s_seg);
   DG_CUDA(cudaStreamWaitEvent(h->s_emb, e_osp, 0));
-  if ((rc = build_tables(h->emb, F, T, h->s_emb))) return rc;
-  if (fuse_pool) {
-    // TDNN5 needs the pooling weights: it runs here, after the segmentation of this step, fused with the pooling
-    // (persistent grid capped like the trunk's: the other lane's recurrence may hold 2 x ceil(B/16) SMs at this point)
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->seg->device);
-    const int lstm_ctas = lstm_tc_ctas(B);
-    g_sm_limit = sms - lstm_ctas > sms / 2 ? sms - lstm_ctas : 0;
-    rc = emb_tdnn5_pool(h->emb, B, g, osp.as<float>(), F, K, T, h->s_emb);
-    if (!rc) rc = emb_project(h->emb, B * K, 1, 1.f, emb, h->s_emb);
-    g_sm_limit = 0;
-    if (rc) return rc;
-    DG_CUDA(cudaEventRecord(h->e_emb, h->s_emb));
-    DG_DIAG(emb, h->s_emb);
-    return use_end(h->emb->guard, h, h->s_emb);
-  }
-  if (h->emb->pooled.ensure((size_t)B * K * 2 * h->emb->pool_C * 4)) return DG_ECUDA;
-  if ((rc = launch_stats_pool(h->emb->pool_x, B, g.S2, T, h->emb->pool_C, osp.as<float>(), F, K,
-                              h->emb->idx0.as<int>(), h->emb->idx1.as<int>(), h->emb->lam1.as<float>(),
-                              h->emb->pool_mode == 31 ? 1e-8f : 0.f, h->emb->pooled.as<float>(), h->s_emb,
-                              h->emb->pool_item_pitch, h->emb->pool_row_pitch)))
-    return rc;
-  if ((rc = emb_project(h->emb, B * K, 1, 1.f, emb, h->s_emb))) return rc;
+  // a fused TDNN5 needs the pooling weights: it runs here, after the segmentation of this step, with its grid capped like the
+  // trunk's (the other lane's recurrence may hold 2 x ceil(B/16) SMs at this point)
+  if ((rc = emb_tail(h->emb, B, g, osp.as<float>(), F, K, T, fuse, 1, 1.f, emb, h->s_emb, sm_cap))) return rc;
   DG_CUDA(cudaEventRecord(h->e_emb, h->s_emb));
-  return use_end(h->emb->guard, h, h->s_emb);
+  DG_DIAG(emb, h->s_emb);
+  return emb_use.end();
 }
 
 extern "C" int dg_pipeline_set_hop(dg_pipeline* h, int hop_samples) {
@@ -1809,16 +1850,10 @@ extern "C" int dg_pipeline_set_hop(dg_pipeline* h, int hop_samples) {
   return DG_OK;
 }
 
-extern "C" int dg_pipeline_step(dg_pipeline* h, const float* wav, int B, int S, float* seg, float* emb, int32_t* map,
-                                float* permuted, void* stream) {
-  if (!h || !wav || !seg || !emb || !map || B < 1) {
-    set_error("dg_pipeline_step: bad arguments");
-    return DG_EINVAL;
-  }
-  if (h->outstanding) {
-    set_error("dg_pipeline_step: submitted steps are outstanding; collect them first");
-    return DG_EINVAL;
-  }
+// dg_pipeline_step after its argument checks.  stream_hop > 0: the batch was formed on the device from one dg_stream, whose
+// windows are that many samples apart (the sinc layer takes its stream form without the overlap check)
+static int pipeline_step(dg_pipeline* h, const float* wav, int B, int S, float* seg, float* emb, int32_t* map,
+                         float* permuted, void* stream, int stream_hop) {
   int rc, F = 0, K = 0;
   if ((rc = dg_seg_dims(h->seg, S, &F, &K))) return rc;
   if (h->osp.ensure((size_t)B * F * K * 4)) return DG_ECUDA;
@@ -1833,12 +1868,25 @@ extern "C" int dg_pipeline_step(dg_pipeline* h, const float* wav, int B, int S, 
   cudaStream_t st = (cudaStream_t)stream;
   DG_CUDA(cudaSetDevice(h->seg->device));
   DG_CUDA(cudaEventRecord(h->e_start, st));
-  if ((rc = pipeline_nets(h, wav, B, S, F, K, seg, emb, h->e_start, 0, h->overlap_known ? h->hop : 0))) return rc;
+  if ((rc = pipeline_nets(h, wav, B, S, F, K, seg, emb, h->e_start, 0, stream_hop))) return rc;
   DG_CUDA(cudaStreamWaitEvent(h->s_clu, h->e_emb, 0));
   if ((rc = dg_cluster_step(h->clu, seg, emb, B, F, K, map, permuted, h->s_clu))) return rc;
   DG_CUDA(cudaEventRecord(h->e_done, h->s_clu));
   DG_CUDA(cudaStreamWaitEvent(st, h->e_done, 0));
   return DG_OK;
+}
+
+extern "C" int dg_pipeline_step(dg_pipeline* h, const float* wav, int B, int S, float* seg, float* emb, int32_t* map,
+                                float* permuted, void* stream) {
+  if (!h || !wav || !seg || !emb || !map || B < 1) {
+    set_error("dg_pipeline_step: bad arguments");
+    return DG_EINVAL;
+  }
+  if (h->outstanding) {
+    set_error("dg_pipeline_step: submitted steps are outstanding; collect them first");
+    return DG_EINVAL;
+  }
+  return pipeline_step(h, wav, B, S, seg, emb, map, permuted, stream, 0);
 }
 
 // ---- pipelined variants (up to three steps outstanding, two computing): the sequential clustering of step i and the host copies overlap the
@@ -2012,21 +2060,13 @@ struct dg_stream {
   int device = 0, S = 0, hop = 0, C = 0;
   long long wpos = 0, rpos = 0;          // absolute sample counters: pushed / start of the next window
   DevBuf ring;
-  float* pin = nullptr;                  // pinned mirror of the ring (staging for the uploads)
-  cudaStream_t st = nullptr;             // uploads
-  cudaEvent_t e_up = nullptr, e_read = nullptr;
+  PinnedBuf pin;                         // pinned mirror of the ring (staging for the uploads)
+  Stream st;                             // uploads
+  Event e_up, e_read;
   // uploads still reading the pinned mirror: (first absolute sample, event); a region of the mirror is rewritten only
   // after the upload that last used it has completed
-  std::deque<std::pair<long long, cudaEvent_t>> inflight;
-  std::vector<cudaEvent_t> spare;
-  ~dg_stream() {
-    for (auto& e : inflight) cudaEventDestroy(e.second);
-    for (auto& e : spare) cudaEventDestroy(e);
-    if (pin) cudaFreeHost(pin);
-    if (st) cudaStreamDestroy(st);
-    if (e_up) cudaEventDestroy(e_up);
-    if (e_read) cudaEventDestroy(e_read);
-  }
+  std::deque<std::pair<long long, Event>> inflight;
+  std::vector<Event> spare;
 };
 
 extern "C" int dg_stream_create(int chunk_samples, int step_samples, int max_windows, int device, dg_stream** out) {
@@ -2040,11 +2080,9 @@ extern "C" int dg_stream_create(int chunk_samples, int step_samples, int max_win
   h->device = device; h->S = chunk_samples; h->hop = step_samples;
   // room for the windows being read, a full batch being uploaded meanwhile, and the overlap tail
   h->C = ((chunk_samples + 2 * max_windows * step_samples + 1023) / 1024) * 1024;
-  if (h->ring.ensure((size_t)h->C * 4)) return DG_ECUDA;
-  DG_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&h->pin), (size_t)h->C * 4, cudaHostAllocDefault));
-  DG_CUDA(cudaStreamCreateWithFlags(&h->st, cudaStreamNonBlocking));
-  DG_CUDA(cudaEventCreateWithFlags(&h->e_up, cudaEventDisableTiming));
-  DG_CUDA(cudaEventCreateWithFlags(&h->e_read, cudaEventDisableTiming));
+  if (h->ring.ensure((size_t)h->C * 4) || h->pin.ensure((size_t)h->C * 4) || h->st.create() || h->e_up.create() ||
+      h->e_read.create())
+    return DG_ECUDA;
   DG_CUDA(cudaEventRecord(h->e_read, h->st));
   *out = h.release();
   return DG_OK;
@@ -2060,7 +2098,7 @@ extern "C" int dg_stream_reset(dg_stream* h) {
   DG_CUDA(cudaSetDevice(h->device));
   DG_CUDA(cudaStreamSynchronize(h->st));
   h->wpos = h->rpos = 0;
-  for (auto& e : h->inflight) h->spare.push_back(e.second);
+  for (auto& e : h->inflight) h->spare.push_back(std::move(e.second));
   h->inflight.clear();
   return DG_OK;
 }
@@ -2089,26 +2127,27 @@ extern "C" int dg_stream_push_host(dg_stream* h, const float* samples, int n) {
   // the mirror region [wpos, wpos + n) was last used by the uploads of samples one lap earlier: wait for those
   while (!h->inflight.empty() && h->inflight.front().first < h->wpos + n - h->C) {
     DG_CUDA(cudaEventSynchronize(h->inflight.front().second));
-    h->spare.push_back(h->inflight.front().second);
+    h->spare.push_back(std::move(h->inflight.front().second));
     h->inflight.pop_front();
   }
+  float* pin = h->pin.as<float>();
   int done = 0;
   while (done < n) {
     const int at = (int)((h->wpos + done) % h->C);
     const int len = std::min(n - done, h->C - at);
-    memcpy(h->pin + at, samples + done, (size_t)len * 4);
-    DG_CUDA(cudaMemcpyAsync(h->ring.as<float>() + at, h->pin + at, (size_t)len * 4, cudaMemcpyHostToDevice, h->st));
+    memcpy(pin + at, samples + done, (size_t)len * 4);
+    DG_CUDA(cudaMemcpyAsync(h->ring.as<float>() + at, pin + at, (size_t)len * 4, cudaMemcpyHostToDevice, h->st));
     done += len;
   }
-  cudaEvent_t ev;
+  Event ev;
   if (!h->spare.empty()) {
-    ev = h->spare.back();
+    ev = std::move(h->spare.back());
     h->spare.pop_back();
-  } else {
-    DG_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  } else if (ev.create()) {
+    return DG_ECUDA;
   }
   DG_CUDA(cudaEventRecord(ev, h->st));
-  h->inflight.emplace_back(h->wpos, ev);
+  h->inflight.emplace_back(h->wpos, std::move(ev));
   h->wpos += n;
   DG_CUDA(cudaEventRecord(h->e_up, h->st));
   return DG_OK;
@@ -2150,11 +2189,7 @@ struct dg_post {
   DevBuf hamming, hist_seg[2], hist_map[2], plan, header, turns, total;
   int cur = 0, n_hist = 0, cap_B = 0;
   int turn_cap = 0;
-  void* pin = nullptr;            // pinned staging: plan in, header + total + turn prefix out
-  size_t pin_bytes = 0;
-  ~dg_post() {
-    if (pin) cudaFreeHost(pin);
-  }
+  PinnedBuf pin;                  // pinned staging: plan in, header + total + turn prefix out
 };
 
 static const int DG_POST_PREFIX = 16384;   // turns copied back together with the header (one D2H in the common case)
@@ -2197,13 +2232,7 @@ static int post_ensure(dg_post* h, int B) {
   if (h->plan.ensure((size_t)B * stride * 4) || h->header.ensure((size_t)B * 16 + 16) ||
       h->turns.ensure((size_t)h->turn_cap * 4))
     return DG_ECUDA;
-  const size_t need = (size_t)B * stride * 4 + (size_t)B * 16 + 16 + (size_t)DG_POST_PREFIX * 4;
-  if (need > h->pin_bytes) {
-    if (h->pin) cudaFreeHost(h->pin);
-    h->pin = nullptr;
-    DG_CUDA(cudaHostAlloc(&h->pin, need, cudaHostAllocDefault));
-    h->pin_bytes = need;
-  }
+  if (h->pin.ensure((size_t)B * stride * 4 + (size_t)B * 16 + 16 + (size_t)DG_POST_PREFIX * 4)) return DG_ECUDA;
   h->cap_B = B;
   return 0;
 }
@@ -2214,7 +2243,7 @@ static int post_enqueue(dg_post* h, const float* seg_dev, const int32_t* map_dev
   int rc;
   if ((rc = post_ensure(h, B))) return rc;
   const int stride = 4 + h->nw;
-  unsigned char* pin = reinterpret_cast<unsigned char*>(h->pin);
+  unsigned char* pin = h->pin.as<unsigned char>();
   const size_t plan_bytes = (size_t)B * stride * 4;
   memcpy(pin, plan_host, plan_bytes);
   DG_CUDA(cudaMemcpyAsync(h->plan.p, pin, plan_bytes, cudaMemcpyHostToDevice, st));
@@ -2244,7 +2273,7 @@ static int post_enqueue(dg_post* h, const float* seg_dev, const int32_t* map_dev
 static int post_finish(dg_post* h, int B, int32_t* header_host, uint32_t* turns_host, int turn_cap_host, int* n_turns,
                        cudaStream_t st) {
   const int stride = 4 + h->nw;
-  unsigned char* out = reinterpret_cast<unsigned char*>(h->pin) + (size_t)B * stride * 4;
+  unsigned char* out = h->pin.as<unsigned char>() + (size_t)B * stride * 4;
   unsigned int total = 0;
   memcpy(&total, out + (size_t)B * 16, 4);
   if (n_turns) *n_turns = (int)total;
@@ -2378,13 +2407,7 @@ extern "C" int dg_pipeline_call_host(dg_pipeline* h, dg_post* post, const float*
     g_diag = &diag;
   }
   if (h->segd.ensure((size_t)B * F * K * 4) || h->mapd.ensure((size_t)B * K * 4)) return DG_ECUDA;
-  const size_t bytes = (size_t)B * S * 4;
-  if (bytes > h->pin_wav_bytes) {
-    if (h->pin_wav) cudaFreeHost(h->pin_wav);
-    h->pin_wav = nullptr;
-    DG_CUDA(cudaHostAlloc(&h->pin_wav, bytes, cudaHostAllocDefault));
-    h->pin_wav_bytes = bytes;
-  }
+  if (h->pin_wav.ensure((size_t)B * S * 4)) return DG_ECUDA;
   // The batch runs as up to three sub-batches through the pipelined machinery (dg_pipeline_submit_host): the upload of
   // sub-batch j+1 and its front end overlap the recurrence of sub-batch j; clustering stays in chunk order on its one stream,
   // so the result is exactly that of one step over the whole batch.  From 64 windows on: two halves; from 192 windows on:
@@ -2407,7 +2430,7 @@ extern "C" int dg_pipeline_call_host(dg_pipeline* h, dg_post* post, const float*
   bool as_stream = hop > 0 && hop < S && hop % 4 == 0 && S % 4 == 0 && B >= 2;
   const size_t stream_len = (size_t)S + (size_t)(B - 1) * (hop > 0 ? hop : 0);
   if (as_stream && h->call_stream.ensure((stream_len + 64) * 4)) return DG_ECUDA;
-  float* pin = reinterpret_cast<float*>(h->pin_wav);
+  float* pin = h->pin_wav.as<float>();
   h->call_h2d_bytes = 0;
   int slots[DG_MAX_INFLIGHT], nbs[DG_MAX_INFLIGHT];
   for (int j = 0, r0 = 0; j < ns; r0 += plan[j], j++) {
@@ -2498,10 +2521,7 @@ extern "C" int dg_pipeline_identity_export(dg_pipeline* h, double* record_dev, v
     return DG_EINVAL;
   }
   DG_CUDA(cudaSetDevice(h->seg->device));
-  if (!h->e_ident) {
-    DG_CUDA(cudaEventCreateWithFlags(&h->e_ident, cudaEventDisableTiming));
-    DG_CUDA(cudaEventCreateWithFlags(&h->e_ident_in, cudaEventDisableTiming));
-  }
+  if (!h->e_ident && (h->e_ident.create() || h->e_ident_in.create())) return DG_ECUDA;
   int rc;
   if ((rc = dg_cluster_export_delta(h->clu, record_dev, h->s_clu))) return rc;
   DG_CUDA(cudaEventRecord(h->e_ident, h->s_clu));
@@ -2592,13 +2612,9 @@ extern "C" int dg_pipeline_call_stream(dg_pipeline* h, dg_post* post, dg_stream*
       h->mapd.ensure((size_t)B * K * 4))
     return DG_ECUDA;
   if ((rc = stream_expand(s, B, h->wav.as<float>(), h->st))) return rc;
-  const int hop_saved = h->hop;
-  h->hop = s->hop;
-  h->overlap_known = true;
-  rc = dg_pipeline_step(h, h->wav.as<float>(), B, S, h->segd.as<float>(), h->embd.as<float>(), h->mapd.as<int32_t>(), nullptr, h->st);
-  h->overlap_known = false;
-  h->hop = hop_saved;
-  if (rc) return rc;
+  if ((rc = pipeline_step(h, h->wav.as<float>(), B, S, h->segd.as<float>(), h->embd.as<float>(), h->mapd.as<int32_t>(),
+                          nullptr, h->st, s->hop)))
+    return rc;
   if ((rc = post_enqueue(post, h->segd.as<float>(), h->mapd.as<int32_t>(), B, plan_host, h->st))) return rc;
   if (seg_host) DG_CUDA(cudaMemcpyAsync(seg_host, h->segd.p, (size_t)B * F * K * 4, cudaMemcpyDeviceToHost, h->st));
   if (map_host) DG_CUDA(cudaMemcpyAsync(map_host, h->mapd.p, (size_t)B * K * 4, cudaMemcpyDeviceToHost, h->st));
@@ -2607,23 +2623,6 @@ extern "C" int dg_pipeline_call_stream(dg_pipeline* h, dg_post* post, dg_stream*
 }
 
 extern "C" int dg_pipeline_destroy(dg_pipeline* h) {
-  if (h) {
-    if (h->s_seg) cudaStreamDestroy(h->s_seg);
-    if (h->s_emb) cudaStreamDestroy(h->s_emb);
-    if (h->s_clu) cudaStreamDestroy(h->s_clu);
-    if (h->s_seg2) cudaStreamDestroy(h->s_seg2);
-    if (h->e_osp2) cudaEventDestroy(h->e_osp2);
-    if (h->e_prep[0]) cudaEventDestroy(h->e_prep[0]);
-    if (h->e_prep[1]) cudaEventDestroy(h->e_prep[1]);
-    if (h->s_h2d) cudaStreamDestroy(h->s_h2d);
-    if (h->s_d2h) cudaStreamDestroy(h->s_d2h);
-    for (cudaEvent_t e : {h->e_start, h->e_osp, h->e_emb, h->e_done, h->e_h2d[0], h->e_h2d[1], h->e_h2d[2],
-                          h->e_slot_done[0], h->e_slot_done[1], h->e_slot_done[2], h->e_lane_done[0], h->e_lane_done[1],
-                          h->e_ident, h->e_ident_in})
-      if (e) cudaEventDestroy(e);
-  }
-  if (h && h->st) cudaStreamDestroy(h->st);
-  if (h && h->pin_wav) cudaFreeHost(h->pin_wav);
   delete h;
   return DG_OK;
 }

@@ -149,7 +149,6 @@ struct TcGemm {
   int epi;             // 0 bias -> f32, 1 bias+leaky+bn -> hi/lo planes, 2 bias+leaky+bn -> f32, 3 conv2d (see below)
   const char* tag;
   const int* tap_off;  // host array [KW]: row offset of every tap; null = j * dil (Conv1d)
-  int sm_limit;        // > 0: cap of the persistent grid (a lower-priority stream leaves SMs to the other one)
   // epi 3 (Conv2d on zero-padded channels-last maps, rows = (item, w, h) of a [Wp][Hp] map): BatchNorm2d affine (bn_scale,
   // bn_shift) -> + residual planes -> ReLU -> hi/lo planes (and / or float32) at the same position of the [Wop][Hop] map;
   // stride2: the convolution is evaluated at every centre and only the odd (w, h) are kept

@@ -823,8 +823,8 @@ static int tc_setup(const TcGemm& g, int bn, int bk, int epi, CUtensorMap* maps,
   return 0;
 }
 
-static int tc_grid(const TcGemm& g, const TcArgs& a) {
-  const int sms = g.sm_limit > 0 ? std::min(g.sm_limit, usable_sms()) : usable_sms();
+static int tc_grid(const TcArgs& a) {
+  const int sms = usable_sms();
   const int tiles = a.m_tiles * a.n_tiles;
   return tiles < sms ? tiles : sms;
 }
@@ -839,7 +839,7 @@ static int launch_tc(const TcGemm& g, cudaStream_t st) {
   static bool attr_done[64] = {};
   if (first_use_on_device(attr_done))
     DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-  kern<<<tc_grid(g, a), TC_THREADS, S::TOTAL, st>>>(m[0], m[1], m[2], m[3], a);
+  kern<<<tc_grid(a), TC_THREADS, S::TOTAL, st>>>(m[0], m[1], m[2], m[3], a);
   DG_LAUNCHED();
   return 0;
 }
@@ -855,7 +855,7 @@ static int launch_tc_pool(const TcGemm& g, cudaStream_t st) {
   static bool attr_done[64] = {};
   if (first_use_on_device(attr_done))
     DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::total(EPI)));
-  kern<<<tc_grid(g, a), TC_POOL_THREADS, S::total(EPI), st>>>(m[0], m[1], m[2], m[3], a);
+  kern<<<tc_grid(a), TC_POOL_THREADS, S::total(EPI), st>>>(m[0], m[1], m[2], m[3], a);
   DG_LAUNCHED();
   return 0;
 }
