@@ -82,6 +82,12 @@ SIGNATURES = {
     "dg_pipeline_call_stream": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.POINTER(C.c_int), _P, _P]),
     "dg_pipeline_call_host": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, _P, C.c_int, C.POINTER(C.c_int), _P, _P]),
     "dg_pipeline_last_call_h2d_bytes": (C.c_int64, [_P]),
+    "dg_resample_create": (C.c_int, [C.c_int, C.c_int, _P, C.c_int, C.c_int, C.POINTER(_P)]),
+    "dg_resample_out_len": (C.c_int64, [_P, C.c_int64]),
+    "dg_resample_forward": (C.c_int, [_P, _P, C.c_int, C.c_int64, _P, _P]),
+    "dg_resample_destroy": (C.c_int, [_P]),
+    "dg_stream_create_resampled": (C.c_int, [C.c_int, C.c_int, _P, C.c_int, C.c_int, C.POINTER(_P)]),
+    "dg_stream_crop_host": (C.c_int, [_P, C.c_int, _P, _P]),
 }
 
 

@@ -22,7 +22,7 @@ from . import base
 from .aggregation import DelayedAggregation
 from .clustering import OnlineSpeakerClustering
 from .embedding import OverlapAwareSpeakerEmbedding
-from .post import DevicePostPath, aggregate_audio
+from .post import DevicePostPath, aggregate_audio, resampled_stream_audio
 from .segmentation import SpeakerSegmentation
 from .utils import Binarize
 
@@ -242,10 +242,19 @@ class SpeakerDiarization(base.Pipeline):
         """``__call__`` for the next ``batch_size`` windows (default: all available) of a
         :class:`diart_b200.operators.DeviceAudioStream`: the windows never exist on the host, only each new sample was
         uploaded once.  Returns the same ``[(Annotation, SlidingWindowFeature), ...]`` as ``__call__`` on the windows
-        ``rearrange_audio_stream`` would have emitted."""
+        ``rearrange_audio_stream`` would have emitted.
+
+        A stream at another source rate is resampled on the device (reference: ``blocks.Resample`` after
+        ``rearrange_audio_stream(source_rate)``); the result is then ``__call__`` on the resampled windows with the
+        reference's time base, and the audio outputs are crops of the resampled windows, of which only the cropped ranges
+        return to the host."""
         B = stream.available if batch_size is None else int(batch_size)
         assert B >= 1, "Pipeline expected at least 1 input"
         expected = int(np.rint(self.config.duration * self.config.sample_rate))
+        if getattr(stream, "resampled", False):
+            assert stream.sample_rate == self.config.sample_rate, \
+                f"the stream resamples to {stream.sample_rate} Hz, the pipeline runs at {self.config.sample_rate} Hz"
+            return self._call_resampled_stream(stream, B, expected)
         assert stream.chunk_samples == expected, f"Expected {expected} samples per chunk, but got {stream.chunk_samples}"
         if self._native_models() is None:
             raise _lib.DiartB200Error("call_stream needs the native segmentation and embedding models")
@@ -265,6 +274,30 @@ class SpeakerDiarization(base.Pipeline):
                                                           C.byref(n_turns), None, None))
         annotations = post.annotations(header, turns, n_turns.value, out_start, out_res, self.timestamp_shift)
         audio, self.chunk_buffer = aggregate_audio(self.chunk_buffer, waves, post.nw, self.config.step, self.config.latency)
+        stream.advance(B, keep_windows=post.nw)
+        return list(zip(annotations, audio))
+
+    def _call_resampled_stream(self, stream, B: int, expected: int):
+        """call_stream on a stream whose windows are resampled on the device (see call_stream)"""
+        n = stream.window_samples
+        assert n == expected, f"Expected {expected} samples per chunk, but got {n}"
+        if self._native_models() is None:
+            raise _lib.DiartB200Error("call_stream needs the native segmentation and embedding models")
+        h, F, K, D = self._ensure_fused(expected)
+        post = self._ensure_post(F, K)
+        first = stream.windows_emitted
+        starts = np.array([stream.window_start_time(first + i) for i in range(B)], dtype=np.float64)
+        res = stream.window_resolution
+        s0, e0 = starts[0], starts[0] + n * res                           # extent of the first window
+        plan, out_start, out_res = post.plan(starts, (e0 - s0 if e0 > s0 else 0.0) / F)
+        header, turns = post.buffers(B)
+        n_turns = C.c_int()
+        with torch.cuda.device(self.segmentation.device):
+            _lib.check(_lib.lib().dg_pipeline_call_stream(h, post.handle, stream.handle, B, plan.ctypes.data,
+                                                          header.ctypes.data, turns.ctypes.data, len(turns),
+                                                          C.byref(n_turns), None, None))
+        annotations = post.annotations(header, turns, n_turns.value, out_start, out_res, self.timestamp_shift)
+        audio = resampled_stream_audio(stream, first, B, post.nw, self.config.step, self.config.latency)
         stream.advance(B, keep_windows=post.nw)
         return list(zip(annotations, audio))
 

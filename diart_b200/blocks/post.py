@@ -197,6 +197,63 @@ def aggregate_audio(chunk_buffer: List[SlidingWindowFeature], new: Sequence[Slid
     return outs, (buf[len(buf) - keep:] if keep else [])
 
 
+def resampled_stream_audio(stream, first: int, B: int, nw: int, step: float, latency: float) -> List[SlidingWindowFeature]:
+    """``aggregate_audio`` for chunks ``first .. first + B - 1`` of a resampled ``DeviceAudioStream`` whose windows were just
+    formed on the device and never copied back.  Chunk c crops its oldest buffered window, window max(c + 1 - nw, 0) of the
+    stream, with the arithmetic of ``aggregate_audio``; the windows of this batch are all some chunk's oldest until
+    ``nw - 1`` chunks later, so their crops for later chunks are fetched now and kept on the stream.  Only the cropped
+    ranges (about one step of audio per chunk) come back from the device."""
+    n, res = stream.window_samples, stream.window_resolution
+    stash = stream.audio_stash
+    todo = {}                                          # chunk -> (oldest window, lo, cnt, lo1, cnt1 or None, start, end, fixed)
+    for c in range(first, first + B + nw - 1):
+        o = max(c + 1 - nw, 0) if nw > 1 else c
+        if c in stash or not (first <= o < first + B):
+            if c < first + B and c not in stash:
+                raise ValueError(f"chunk {c} needs window {o}, which is no longer on the device")
+            continue
+        s0 = stream.window_start_time(o)                # d0 = p0 = res: the window's SlidingWindow
+        w_start = stream.window_start_time(c)
+        w_end = w_start + n * res
+        start = w_end - latency
+        end = start + step
+        fixed = end - start if end > start else 0.0
+        lo = int(np.rint((start - s0 - 0.5 * res) / res))
+        cnt = int(np.rint(fixed / res))
+        nbuf = min(c + 1, nw)
+        lo1 = cnt1 = None
+        if nbuf == 1 and w_start == 0:
+            lo1 = int(np.rint((0.0 - s0 - 0.5 * res) / res))
+            cnt1 = int(np.rint(end / res))
+        todo[c] = (o, lo, cnt, lo1, cnt1, start, end, fixed)
+    ranges = []
+    for c, (o, lo, cnt, lo1, cnt1, *_) in todo.items():
+        spans = [(lo, cnt)] + ([(lo1, cnt1)] if lo1 is not None else [])
+        a = min(min(max(l, 0), n - 1) for l, _ in spans)
+        b = max(min(max(l + k - 1, 0), n - 1) for l, k in spans) + 1
+        ranges.append((o, a, b - a))
+    flat = stream.crops(ranges) if ranges else np.zeros(0, np.float32)
+    off = 0
+    for (c, (o, lo, cnt, lo1, cnt1, start, end, fixed)), (_, a, k) in zip(todo.items(), ranges):
+        piece = flat[off:off + k, None]
+        off += k
+
+        def crop(l, m):
+            if l >= 0 and l + m <= n:
+                return piece[l - a:l - a + m]
+            return piece[np.clip(np.arange(l, l + m), 0, n - 1) - a]
+        if lo1 is not None:
+            out = crop(lo1, cnt1).copy()
+            out[-cnt:] = crop(lo, cnt)
+            r = end / out.shape[0]
+            stash[c] = SlidingWindowFeature(out, SlidingWindow(start=0, duration=r, step=r))
+        else:
+            out = crop(lo, cnt)
+            r = fixed / out.shape[0]
+            stash[c] = SlidingWindowFeature(out, SlidingWindow(start=start, duration=r, step=r))
+    return [stash.pop(c) for c in range(first, first + B)]
+
+
 def _crop(data: np.ndarray, lo: int, cnt: int, n: int) -> np.ndarray:
     if lo >= 0 and lo + cnt <= n:
         return data[lo:lo + cnt]

@@ -262,6 +262,33 @@ int launch_expand_windows(const float* ring, long long r0, int C, int hop, int S
 int launch_post_history(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map, int n_hist,
                         int B, int F, int K, int keep, float* new_seg, int32_t* new_map, cudaStream_t st);
 size_t cluster_prep_doubles(int B, int K);
+// resample.cu -- polyphase sinc resampling (torchaudio's defaults): reduced ratio o / n, half-width w, T = 2w + o taps per phase
+struct RsGeom {
+  int o, n, w, T;
+};
+// one item = one window of source samples, x = 0 outside [start, start + len) (absolute sample indices, taken mod C for a
+// ring); outputs [j_lo, j_lo + j_cnt) of it are written to out + out_off
+struct RsItem {
+  long long start, len, j_lo, j_cnt, out_off;
+};
+struct RsJob {
+  const float* x;
+  long long C;            // ring capacity, 0: x is a dense array
+  const RsItem* items;    // device array, one per item, or null: item b = base shifted by b * start_step / b * out_step
+  RsItem base;
+  long long start_step, out_step;
+  const float* W;         // [n][T]
+  RsGeom g;
+  float* out;
+};
+long long resample_out_len(const RsGeom& g, long long L);   // ceil(n L / o)
+bool resample_geom_ok(const RsGeom& g);                     // the source span of one block fits in shared memory
+// per-window form (and crops): `items` items, none with more than max_out outputs
+int launch_resample(const RsJob& j, int items, long long max_out, cudaStream_t st);
+// stream form (hop % o == 0): windows b = 0 .. B-1 of a ring start at rpos + b hop; ys: scratch of
+// ((B-1) hop / o + ceil(out_len / n)) n floats; out [B][out_len]
+int launch_resample_stream(const float* ring, long long C, long long rpos, long long hop, long long L, int B, const float* W,
+                           const RsGeom& g, float* ys, float* out, cudaStream_t st);
 
 void fbank_frame_operator(std::vector<float>& op /*[514][400]*/);
 void fbank_mel_banks(std::vector<float>& banks /*[80][257]*/, std::vector<int>& k_lo, std::vector<int>& k_hi);

@@ -212,6 +212,34 @@ int dg_pipeline_call_stream(dg_pipeline* h, dg_post* post, dg_stream* stream, in
                             int32_t* header_host, uint32_t* turns_host, int turn_cap_host, int* n_turns,
                             float* seg_host /*nullable*/, int32_t* map_host /*nullable*/);
 
+/* ---- resampling: torchaudio's T.Resample(orig, new) with its defaults (sinc_interp_hann, lowpass_filter_width 6,
+ *      rolloff 0.99), what the reference's blocks.Resample applies to every window of a source at another rate (reference
+ *      src/diart/blocks/utils.py:62-89, inference.py:101-123).  With g = gcd(orig, new), o = orig / g, n = new / g:
+ *        y[r n + p] = sum_k x[r o + k - width] taps[p][k],  x = 0 outside the window,  output length ceil(n L / o).
+ *      taps_host float32 [n][2 width + o] = torchaudio.functional.functional._get_sinc_resample_kernel (bit-identical;
+ *      diart_b200.operators.sinc_resample_kernel builds it); width must be torchaudio's for the two rates. ---- */
+typedef struct dg_resample dg_resample;
+int dg_resample_create(int orig_rate, int new_rate, const float* taps_host, int width, int device, dg_resample** out);
+/* output samples of an L-sample window, -1 on bad arguments */
+int64_t dg_resample_out_len(const dg_resample* h, int64_t num_samples);
+/* per-window form: in_dev [B, L] -> out_dev [B, dg_resample_out_len(h, L)], stream-ordered */
+int dg_resample_forward(dg_resample* h, const float* in_dev, int B, int64_t L, float* out_dev, void* stream);
+int dg_resample_destroy(dg_resample* h);
+/* dg_stream_create for a source at the resampler's original rate (no multiple-of-4 rule): chunk, step, push_host and
+ * available count source-rate samples (rearrange_audio_stream at the source rate); dg_stream_windows returns the windows
+ * resampled, [B, dg_resample_out_len(rs, chunk)].  When step % o == 0 every output of the batch's unique source samples is
+ * computed once and only the frames whose taps cross a window edge are recomputed per window; otherwise each window is
+ * resampled from the ring.  Both give the same bits as dg_resample_forward on the stacked source windows.  The stream
+ * borrows `rs`.  dg_pipeline_submit_stream / call_stream take such a stream like any other, with the per-window form of the
+ * sinc layer (resampled windows are not exact hops of one stream at their edges). */
+int dg_stream_create_resampled(int chunk_samples, int step_samples, dg_resample* rs, int max_windows, int device,
+                               dg_stream** out);
+/* resampled stream only: outputs [first, first + count) of window `window` (0 = first window since create / reset) for n
+ * ranges_host int64 [n][3] = {window, first, count}, packed into out_host; bit-identical to those of dg_stream_windows.  The
+ * window's source samples must still be in the ring (it was formed by the last dg_stream_windows / pipeline call, and nothing
+ * was pushed since).  Synchronous. */
+int dg_stream_crop_host(dg_stream* h, int n, const int64_t* ranges_host, float* out_host);
+
 /* number of kernels launched by this library since load (bench.py's gpu_launches) */
 int64_t dg_launch_count(void);
 /* per-kernel CUDA-event timing on the launching stream (bench.py's roofline leg).  While enabled,
