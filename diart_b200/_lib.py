@@ -88,6 +88,9 @@ SIGNATURES = {
     "dg_resample_destroy": (C.c_int, [_P]),
     "dg_stream_create_resampled": (C.c_int, [C.c_int, C.c_int, _P, C.c_int, C.c_int, C.POINTER(_P)]),
     "dg_stream_crop_host": (C.c_int, [_P, C.c_int, _P, _P]),
+    "dg_sweep_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, C.POINTER(_P)]),
+    "dg_sweep_run": (C.c_int, [_P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, C.c_int, C.POINTER(C.c_int), _P]),
+    "dg_sweep_destroy": (C.c_int, [_P]),
 }
 
 

@@ -59,42 +59,12 @@ class DevicePostPath:
     def plan(self, starts: np.ndarray, res: float):
         """starts (B,) float64 chunk start times, res = seconds per score frame of this batch ->
         (plan int32 (B, 4 + nw), out_start (B,), out_res (B,)); advances the buffer history by B chunks."""
-        nw, F = self.nw, self.F
-        B = len(starts)
-        H = len(self._hist_start)
+        plan, out_start, out_res = post_plan(starts, res, self._hist_start, self._hist_res, self.nw, self.F, self.step,
+                                             self.latency)
+        B, H = len(starts), len(self._hist_start)
         s_all = np.concatenate([self._hist_start, starts])
         r_all = np.concatenate([self._hist_res, np.full(B, res)])
-        c = np.arange(B)
-        nb = np.minimum(H + c + 1, nw)
-        end = starts + F * res                                  # buffers[-1].extent.end (duration == step)
-        f_start = end - self.latency                            # aggregation.py:216-217
-        f_end = f_start + self.step
-        fixed = np.where(f_end > f_start, f_end - f_start, 0.0)  # Segment.duration
-        # buffer j of chunk c (oldest first) is entry H + c - (nb - 1) + j of the concatenated history
-        j = np.arange(nw)[None, :]
-        idx = (H + c - (nb - 1))[:, None] + j
-        valid = j < nb[:, None]
-        idx = np.where(valid, idx, 0)
-        s_j, r_j = s_all[idx], r_all[idx]
-        lo = np.ceil((f_start[:, None] - r_j - s_j) / r_j)      # SlidingWindow.crop, mode="loose"
-        cnt = np.floor((fixed[:, None] + r_j) / r_j)            # SlidingWindow.samples(fixed, mode="loose")
-        nf = cnt[:, 0]
-        if np.any(valid & (cnt != nf[:, None])):
-            raise ValueError("all input arrays must have the same shape")   # what np.stack raises in the reference
-        plan = np.zeros((B, 4 + nw), dtype=np.int32)
-        plan[:, 0] = nb
-        plan[:, 1] = nf
-        plan[:, 4:] = np.where(valid, lo, 0)
-        out_start, out_res = f_start.copy(), fixed / nf
-        # first buffer of a stream: everything before the region is emitted too (aggregation.py:188-212)
-        first = (nb == 1) & (starts == 0)
-        if first.any():
-            first_nf = np.floor((f_end + res) / res)            # crop of Segment(0, region.end), fixed = its duration
-            plan[:, 2] = np.where(first, first_nf, 0)
-            plan[:, 3] = np.where(first, np.ceil((0.0 - res - starts) / res), 0)
-            out_start = np.where(first, 0.0, out_start)
-            out_res = np.where(first, f_end / np.maximum(first_nf, 1), out_res)
-        keep = min(nw - 1, H + B)
+        keep = min(self.nw - 1, H + B)
         self._hist_start = s_all[len(s_all) - keep:] if keep else np.zeros(0)
         self._hist_res = r_all[len(r_all) - keep:] if keep else np.zeros(0)
         return plan, out_start, out_res
@@ -110,19 +80,7 @@ class DevicePostPath:
                     out_res: np.ndarray, shift: float = 0.0, uri: Optional[str] = None) -> List[Annotation]:
         """packed turns -> one Annotation per chunk, segments at frame middles (blocks/utils.py:45-58)"""
         B = len(header)
-        t = turns[:n_turns]
-        # each chunk's turns are one contiguous block; sorted by offset the blocks tile [0, n_turns)
-        order = np.argsort(header[:, 0], kind="stable")
-        order = order[header[order, 1] > 0]
-        chunk_of = np.repeat(order, header[order, 1])
-        g = (t >> 20).astype(np.int64)
-        on = ((t >> 10) & 1023).astype(np.float64)
-        off = (t & 1023).astype(np.float64)
-        s0, r0 = out_start[chunk_of], out_res[chunk_of]
-        a = s0 + on * r0
-        b = s0 + off * r0
-        t_on = 0.5 * (a + (a + r0)) + shift                     # SlidingWindow[i].middle
-        t_off = 0.5 * (b + (b + r0)) + shift
+        _, g, t_on, t_off = turn_times(header, turns, n_turns, out_start, out_res, shift)
         t_on, t_off, g = t_on.tolist(), t_off.tolist(), g.tolist()
         labels = self.labels
         modality = "speech" if shift == 0 else None             # the reference's shifted copy drops the modality
@@ -148,6 +106,70 @@ class DevicePostPath:
                                                header.ctypes.data, turns.ctypes.data, len(turns), C.byref(n),
                                                _lib.stream_ptr(self.device)))
         return self.annotations(header, turns, n.value, out_start, out_res, shift)
+
+
+def post_plan(starts: np.ndarray, res: float, hist_start: np.ndarray, hist_res: np.ndarray, nw: int, F: int, step: float,
+              latency: float):
+    """The integer plan of dg_post_step for a batch of chunks starting at ``starts`` (B,) float64, ``res`` seconds per
+    score frame, after the chunks of the history (``hist_start``, ``hist_res``: the last nw - 1 chunks seen, oldest first)
+    -> (plan int32 (B, 4 + nw), out_start (B,), out_res (B,))."""
+    B = len(starts)
+    H = len(hist_start)
+    s_all = np.concatenate([hist_start, starts])
+    r_all = np.concatenate([hist_res, np.full(B, res)])
+    c = np.arange(B)
+    nb = np.minimum(H + c + 1, nw)
+    end = starts + F * res                                  # buffers[-1].extent.end (duration == step)
+    f_start = end - latency                                 # aggregation.py:216-217
+    f_end = f_start + step
+    fixed = np.where(f_end > f_start, f_end - f_start, 0.0)  # Segment.duration
+    # buffer j of chunk c (oldest first) is entry H + c - (nb - 1) + j of the concatenated history
+    j = np.arange(nw)[None, :]
+    idx = (H + c - (nb - 1))[:, None] + j
+    valid = j < nb[:, None]
+    idx = np.where(valid, idx, 0)
+    s_j, r_j = s_all[idx], r_all[idx]
+    lo = np.ceil((f_start[:, None] - r_j - s_j) / r_j)      # SlidingWindow.crop, mode="loose"
+    cnt = np.floor((fixed[:, None] + r_j) / r_j)            # SlidingWindow.samples(fixed, mode="loose")
+    nf = cnt[:, 0]
+    if np.any(valid & (cnt != nf[:, None])):
+        raise ValueError("all input arrays must have the same shape")   # what np.stack raises in the reference
+    plan = np.zeros((B, 4 + nw), dtype=np.int32)
+    plan[:, 0] = nb
+    plan[:, 1] = nf
+    plan[:, 4:] = np.where(valid, lo, 0)
+    out_start, out_res = f_start.copy(), fixed / nf
+    # first buffer of a stream: everything before the region is emitted too (aggregation.py:188-212)
+    first = (nb == 1) & (starts == 0)
+    if first.any():
+        first_nf = np.floor((f_end + res) / res)            # crop of Segment(0, region.end), fixed = its duration
+        plan[:, 2] = np.where(first, first_nf, 0)
+        plan[:, 3] = np.where(first, np.ceil((0.0 - res - starts) / res), 0)
+        out_start = np.where(first, 0.0, out_start)
+        out_res = np.where(first, f_end / np.maximum(first_nf, 1), out_res)
+    return plan, out_start, out_res
+
+
+def turn_times(header: np.ndarray, turns: np.ndarray, n_turns: int, out_start: np.ndarray, out_res: np.ndarray,
+               shift: float = 0.0):
+    """packed turns -> (row of ``header`` each turn belongs to, speaker, on time, off time), segments at frame middles
+    (blocks/utils.py:45-58).  ``header`` (R, 4) rows may be several states' headers over the same chunks (row r is chunk
+    r % len(out_start))."""
+    t = turns[:n_turns]
+    # each row's turns are one contiguous block; sorted by offset the blocks tile [0, n_turns)
+    order = np.argsort(header[:, 0], kind="stable")
+    order = order[header[order, 1] > 0]
+    row_of = np.repeat(order, header[order, 1])
+    chunk_of = row_of % len(out_start)
+    g = (t >> 20).astype(np.int64)
+    on = ((t >> 10) & 1023).astype(np.float64)
+    off = (t & 1023).astype(np.float64)
+    s0, r0 = out_start[chunk_of], out_res[chunk_of]
+    a = s0 + on * r0
+    b = s0 + off * r0
+    t_on = 0.5 * (a + (a + r0)) + shift                     # SlidingWindow[i].middle
+    t_off = 0.5 * (b + (b + r0)) + shift
+    return row_of, g, t_on, t_off
 
 
 def aggregate_audio(chunk_buffer: List[SlidingWindowFeature], new: Sequence[SlidingWindowFeature], nw: int, step: float,

@@ -1,6 +1,7 @@
 // C ABI of libdiartb200.so (include/diart_b200.h): handles, weight preparation, workspaces and the
 // launch sequences of the two networks, the clustering step and the fused pipeline step.
 #include <math.h>
+#include <cmath>
 #include <stdlib.h>
 #include <string.h>
 
@@ -2477,6 +2478,133 @@ extern "C" int dg_post_step(dg_post* h, const float* seg_dev, const int32_t* map
   if ((rc = post_enqueue(h, seg_dev, map_dev, B, plan_host, st))) return rc;
   DG_CUDA(cudaStreamSynchronize(st));
   return post_finish(h, B, header_host, turns_host, turn_cap_host, n_turns, st);
+}
+
+// ============================================================================= hyper-parameter sweep
+// T independent clustering + post-path states over ONE set of network outputs (seg, emb of a whole file): the reference tunes
+// tau_active, rho_update and delta_new by re-running its whole pipeline per trial (Optimizer.objective -> Benchmark), although
+// none of the three reaches the networks.  Clustering: one CTA per state (cluster.cu); post-path: one CTA per (chunk, state)
+// over all chunks at once, without history (post.cu).
+struct dg_sweep {
+  int device = 0, M = 0, D = 0, F = 0, K = 0, nw = 1;
+  DevBuf hamming, in, centers, active, init, prep, prep_d, maps, header, turns, total;
+  PinnedBuf pin;                  // params, taus and plan in; error flags, header, total and a turn prefix out
+};
+
+extern "C" int dg_sweep_create(int max_speakers, int dim, int frames, int local_speakers, int num_windows,
+                               const double* hamming_host, int device, dg_sweep** out) {
+  if (!out || !hamming_host || max_speakers < 1 || max_speakers > 32 || dim < 1 || local_speakers < 1 || local_speakers > 8 ||
+      local_speakers > max_speakers || frames < 1 || frames > 1023 || num_windows < 1 || num_windows > 256) {
+    set_error("dg_sweep_create: need 1 <= max_speakers <= 32, dim >= 1, 1 <= local_speakers <= min(8, max_speakers), "
+              "1 <= frames <= 1023, 1 <= num_windows <= 256");
+    return DG_EINVAL;
+  }
+  DG_CUDA(cudaSetDevice(device));
+  std::unique_ptr<dg_sweep> h(new dg_sweep());
+  h->device = device; h->M = max_speakers; h->D = dim; h->F = frames; h->K = local_speakers; h->nw = num_windows;
+  if (h->hamming.ensure((size_t)frames * 8) || h->total.ensure(16)) return DG_ECUDA;
+  DG_CUDA(cudaMemcpy(h->hamming.p, hamming_host, (size_t)frames * 8, cudaMemcpyHostToDevice));
+  *out = h.release();
+  return DG_OK;
+}
+
+extern "C" int dg_sweep_destroy(dg_sweep* h) {
+  delete h;
+  return DG_OK;
+}
+
+extern "C" int dg_sweep_run(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, const double* params_host, int T,
+                            const int32_t* plan_host, int32_t* maps_dev, double* centers_dev, int32_t* header_host,
+                            uint32_t* turns_host, int turn_cap_host, int* n_turns, void* stream) {
+  if (!h || !seg_dev || !emb_dev || !params_host || !plan_host || !header_host || !turns_host || N < 1 || T < 1 ||
+      T > 65535) {
+    set_error("dg_sweep_run: bad arguments (need N >= 1, 1 <= T <= 65535, non-null buffers)");
+    return DG_EINVAL;
+  }
+  for (int i = 0; i < 3 * T; i++)
+    if (!std::isfinite(params_host[i])) {
+      set_error("dg_sweep_run: trial " + std::to_string(i / 3) + " has a parameter that is not finite");
+      return DG_EINVAL;
+    }
+  DG_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int stride = 4 + h->nw, M = h->M, D = h->D, K = h->K, F = h->F;
+  // host -> device: params [T][3], taus [T], plan [N][stride], one copy
+  const size_t params_b = (size_t)T * 24, taus_b = (size_t)T * 8, plan_b = (size_t)N * stride * 4;
+  const size_t in_b = params_b + taus_b + plan_b;
+  // device -> host: error flags [T][2], header [T][N][4], total, a prefix of the turns
+  const size_t init_b = (size_t)T * 8, header_b = (size_t)T * N * 16;
+  const size_t out_b = init_b + header_b + 16 + (size_t)DG_POST_PREFIX * 4;
+  // the device turn buffer starts at a guess and grows to the true count (the kernel counts every turn, writes those that fit)
+  const size_t turn_guess = std::max<size_t>((size_t)T * N * 8, (size_t)DG_POST_PREFIX);
+  if (h->in.ensure(in_b) || h->centers.ensure((size_t)T * M * D * 8) || h->active.ensure((size_t)T * 32 * 4) ||
+      h->init.ensure(init_b) || h->prep.ensure(cluster_prep_floats(N, K) * 4 + 16) ||
+      h->prep_d.ensure(cluster_prep_doubles(N, K) * 8 + 16) || (!maps_dev && h->maps.ensure((size_t)T * N * K * 4)) ||
+      h->header.ensure(header_b) || h->turns.ensure(turn_guess * 4) || h->pin.ensure(std::max(in_b, out_b)))
+    return DG_ECUDA;
+  unsigned char* pin = h->pin.as<unsigned char>();
+  double* p_taus = reinterpret_cast<double*>(pin + params_b);
+  memcpy(pin, params_host, params_b);
+  for (int t = 0; t < T; t++) p_taus[t] = params_host[3 * t];
+  memcpy(pin + params_b + taus_b, plan_host, plan_b);
+  unsigned char* din = h->in.as<unsigned char>();
+  DG_CUDA(cudaMemcpyAsync(din, pin, in_b, cudaMemcpyHostToDevice, st));
+  const double* d_params = reinterpret_cast<const double*>(din);
+  const double* d_taus = reinterpret_cast<const double*>(din + params_b);
+  const int32_t* d_plan = reinterpret_cast<const int32_t*>(din + params_b + taus_b);
+  int32_t* maps = maps_dev ? maps_dev : h->maps.as<int32_t>();
+  // every state starts empty (reference: a new OnlineSpeakerClustering per trial)
+  DG_CUDA(cudaMemsetAsync(h->centers.p, 0, (size_t)T * M * D * 8, st));
+  DG_CUDA(cudaMemsetAsync(h->active.p, 0, (size_t)T * 32 * 4, st));
+  DG_CUDA(cudaMemsetAsync(h->init.p, 0, init_b, st));
+  ClusterParams p{};
+  p.M = M;
+  p.D = D;
+  p.metric = 0;
+  int rc;
+  if ((rc = launch_cluster_sweep(p, d_params, T, seg_dev, emb_dev, N, F, K, h->centers.as<double>(), h->active.as<int>(),
+                                 h->init.as<int>(), h->prep.as<float>(), h->prep_d.as<double>(), maps, st)))
+    return rc;
+  if (centers_dev)
+    DG_CUDA(cudaMemcpyAsync(centers_dev, h->centers.p, (size_t)T * M * D * 8, cudaMemcpyDeviceToDevice, st));
+  unsigned int total = 0;
+  for (int attempt = 0; attempt < 2; attempt++) {
+    const int cap = (int)std::min<size_t>(h->turns.bytes / 4, (size_t)INT32_MAX);
+    DG_CUDA(cudaMemsetAsync(h->total.p, 0, 4, st));
+    if ((rc = launch_post(seg_dev, maps, nullptr, nullptr, 0, N, F, K, M, h->nw, d_plan, stride, h->hamming.as<double>(), 0.0,
+                          h->header.as<int32_t>(), h->turns.as<uint32_t>(), cap, h->total.as<unsigned int>(), st, d_taus, T)))
+      return rc;
+    DG_CUDA(cudaMemcpyAsync(pin, h->init.p, init_b, cudaMemcpyDeviceToHost, st));
+    DG_CUDA(cudaMemcpyAsync(pin + init_b, h->header.p, header_b, cudaMemcpyDeviceToHost, st));
+    DG_CUDA(cudaMemcpyAsync(pin + init_b + header_b, h->total.p, 4, cudaMemcpyDeviceToHost, st));
+    DG_CUDA(cudaMemcpyAsync(pin + init_b + header_b + 16, h->turns.p, (size_t)std::min(DG_POST_PREFIX, cap) * 4,
+                            cudaMemcpyDeviceToHost, st));
+    DG_CUDA(cudaStreamSynchronize(st));
+    memcpy(&total, pin + init_b + header_b, 4);
+    if (total <= (unsigned int)cap) break;
+    // more turns than the device buffer holds: grow it to the count and binarise again (the maps are unchanged)
+    if (h->turns.ensure((size_t)total * 4)) return DG_ECUDA;
+  }
+  const int32_t* flags = reinterpret_cast<const int32_t*>(pin);
+  for (int t = 0; t < T; t++)
+    if (flags[2 * t + 1]) {
+      set_error("Cannot update unknown centers");   // reference clustering.py:98 (AssertionError)
+      return DG_EINVAL;
+    }
+  if (n_turns) *n_turns = (int)total;
+  memcpy(header_host, pin + init_b, header_b);
+  if ((long long)total > (long long)turn_cap_host) {
+    set_error("dg_sweep_run: turn buffer too small (" + std::to_string(total) + " turns)");
+    return DG_EINVAL;
+  }
+  const unsigned int pre = std::min<unsigned int>(total, (unsigned int)DG_POST_PREFIX);
+  memcpy(turns_host, pin + init_b + header_b + 16, (size_t)pre * 4);
+  if (total > pre) {     // a second copy for what did not travel with the header
+    DG_CUDA(cudaMemcpyAsync(turns_host + pre, h->turns.as<uint32_t>() + pre, (size_t)(total - pre) * 4,
+                            cudaMemcpyDeviceToHost, st));
+    DG_CUDA(cudaStreamSynchronize(st));
+  }
+  return DG_OK;
 }
 
 // worker threads of the host gather, created at the first dg_pipeline_call_host: all cores but two, at most 24

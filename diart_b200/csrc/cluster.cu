@@ -12,7 +12,7 @@
 // Two kernels per batch:
 //   cluster_prep  (parallel over chunks)  per-speaker max / mean of the segmentation, NaN flags and
 //                                         float64 norms of the embeddings.
-//   cluster_seq   (one CTA per stream)    walks the B chunks in order: float64 cosine distances to
+//   cluster_seq   (one CTA per state)     walks the B chunks in order: float64 cosine distances to
 //                                         the active centroids (8 warps), the assignment logic
 //                                         (warp 0), then centroid update + SpeakerMap.apply scatter
 //                                         (all threads).
@@ -188,13 +188,22 @@ __device__ __forceinline__ void cp_async4(void* smem, const void* gmem) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(s), "l"(gmem));
 }
 
-constexpr int SEQ_THREADS = 512;
+constexpr int SEQ_THREADS = 512;        // one stream's state: the pipeline
+constexpr int SWEEP_THREADS = 256;      // many independent states (hyper-parameter sweep): 2 CTAs per SM by registers
 
-__global__ void __launch_bounds__(SEQ_THREADS)
-cluster_seq_kernel(ClusterParams p, const float* __restrict__ seg, const float* __restrict__ emb, int B, int F, int K,
-                   double* __restrict__ centers, int* __restrict__ g_active, int* __restrict__ g_init,
-                   const float* __restrict__ prep, const double* __restrict__ prep_d, int32_t* __restrict__ map_out,
-                   float* __restrict__ permuted, unsigned* __restrict__ dbg) {
+// One CTA per clustering state.  CTA t owns centroid table t ([M][D] at centers + t M D), active flags t ([32]), the
+// `initialized` pair t and the map rows t ([B][K]); `trials` (nullable) holds {tau, rho, delta} per state as float64, NULL
+// = the thresholds of `p` (single state, grid of one).  Every state reads the same chunks and the same prep results.  The
+// arithmetic does not depend on THREADS: each centroid's distances are one warp's, the updates are element-wise.  STATES =
+// false compiles the single-state form of the pipeline (no per-state indexing).
+template <int THREADS, bool STATES>
+__global__ void __launch_bounds__(THREADS)
+cluster_seq_kernel(ClusterParams p, const double* __restrict__ trials, const float* __restrict__ seg,
+                   const float* __restrict__ emb, int B, int F, int K, double* __restrict__ centers,
+                   int* __restrict__ g_active, int* __restrict__ g_init, const float* __restrict__ prep,
+                   const double* __restrict__ prep_d, int32_t* __restrict__ map_out, float* __restrict__ permuted,
+                   unsigned* __restrict__ dbg) {
+  constexpr int SEQ_THREADS = THREADS;
   __shared__ SeqShared sh;
   __shared__ float prs[2][CK * 3];      // per-chunk max / mean / nan flag, double buffered
   __shared__ double ens[2][CK];         // per-chunk embedding norms
@@ -202,6 +211,19 @@ cluster_seq_kernel(ClusterParams p, const float* __restrict__ seg, const float* 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int M = p.M, D = p.D;
   constexpr int NW = SEQ_THREADS / 32;
+  float tau_f = p.tau_f, rho_f = p.rho_f;
+  double delta = p.delta;
+  if constexpr (STATES) {
+    const int trial = blockIdx.x;
+    centers += (size_t)trial * M * D;
+    g_active += (size_t)trial * CM;
+    g_init += (size_t)trial * 2;
+    map_out += (size_t)trial * B * K;
+    // numpy compares the float32 scores with a Python float in float32 (as dg_cluster_create)
+    tau_f = (float)trials[trial * 3 + 0];
+    rho_f = (float)trials[trial * 3 + 1];
+    delta = trials[trial * 3 + 2];
+  }
   double* cs = reinterpret_cast<double*>(dyn);                 // centroids [M][D], resident for the whole batch
   double* ed = cs + (size_t)M * D;                             // the current chunk's embeddings as float64 [K][D] (converted once
                                                                // per chunk by all threads instead of once per centroid warp)
@@ -304,8 +326,8 @@ cluster_seq_kernel(ClusterParams p, const float* __restrict__ seg, const float* 
       unsigned active_spk = 0, long_spk = 0;
       for (int k = 0; k < K; k++) {
         // np.max(seg) >= tau, np.mean(seg) >= rho: float32 array vs Python float -> float32 compare
-        if (pr[k * 3 + 0] >= p.tau_f && pr[k * 3 + 2] == 0.f) active_spk |= 1u << k;   // clustering.py:137-145
-        if (pr[k * 3 + 1] >= p.rho_f) long_spk |= 1u << k;
+        if (pr[k * 3 + 0] >= tau_f && pr[k * 3 + 2] == 0.f) active_spk |= 1u << k;   // clustering.py:137-145
+        if (pr[k * 3 + 1] >= rho_f) long_spk |= 1u << k;
       }
       int n_upd = 0, n_new = 0;
       if (!init) {                                                                      // clustering.py:149-158
@@ -342,7 +364,7 @@ cluster_seq_kernel(ClusterParams p, const float* __restrict__ seg, const float* 
           if (!((mapped >> k) & 1u)) continue;
           const int c = __shfl_sync(FULL, c4r, k);
           const double cost = __shfl_sync(FULL, sel(dmap, k), c);
-          if (cost >= p.delta) {
+          if (cost >= delta) {
             put(valid, k, INVALID);
             dirty = true;
           }
@@ -466,32 +488,48 @@ cluster_seq_kernel(ClusterParams p, const float* __restrict__ seg, const float* 
   }
 }
 
+// bytes of dynamic shared memory one state needs: centroids, the current chunk's embeddings as float64, the double-buffered
+// float32 landing zone
+static size_t cluster_seq_dyn(int M, int D, int K) {
+  return (size_t)M * D * sizeof(double) + (size_t)K * D * sizeof(double) + (size_t)2 * K * D * sizeof(float);
+}
+
+static int check_cluster_shape(const char* who, const ClusterParams& p, int K) {
+  if (K > CK || p.M > CM || K > p.M) {
+    set_error(std::string(who) + ": need local speakers <= 8, max_speakers <= 32 and local <= max");
+    return -1;
+  }
+  if (cluster_seq_dyn(p.M, p.D, K) > 200 * 1024) {
+    set_error(std::string(who) + ": max_speakers * dim too large for the resident centroid table (limit 200 KB)");
+    return -1;
+  }
+  return 0;
+}
+
+template <int THREADS, bool STATES>
+static int cluster_seq_allow_dyn() {   // per device: the opt-in above 48 KB is a property of (function, device)
+  static bool attr_done[64] = {};
+  if (first_use_on_device(attr_done))
+    DG_CUDA(cudaFuncSetAttribute(cluster_seq_kernel<THREADS, STATES>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  return 0;
+}
+
 int launch_cluster_step(const ClusterParams& p, const float* seg, const float* emb, int B, int F, int K,
                         double* centers, int* active, int* initialized, float* prep, double* prep_d, int32_t* map,
                         float* permuted, cudaStream_t st) {
   ProfScope _ps("cluster_step", st);
-  if (K > CK || p.M > CM || K > p.M) {
-    set_error("cluster_step: need local speakers <= 8, max_speakers <= 32 and local <= max");
-    return -1;
-  }
+  if (check_cluster_shape("cluster_step", p, K)) return -1;
   if (B <= 0) return 0;
   cluster_prep_kernel<<<B, 128, 0, st>>>(seg, emb, F, K, p.D, prep, prep_d);
   DG_LAUNCHED();
-  const size_t dyn = (size_t)p.M * p.D * sizeof(double) + (size_t)K * p.D * sizeof(double) + (size_t)2 * K * p.D * sizeof(float);
-  if (dyn > 200 * 1024) {
-    set_error("cluster_step: max_speakers * dim too large for the resident centroid table (limit 200 KB)");
-    return -1;
-  }
-  {   // per device: the opt-in above 48 KB is a property of (function, device)
-    static bool attr_done[64] = {};
-    if (first_use_on_device(attr_done))
-      DG_CUDA(cudaFuncSetAttribute(cluster_seq_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  }
+  const size_t dyn = cluster_seq_dyn(p.M, p.D, K);
+  if (int rc = cluster_seq_allow_dyn<SEQ_THREADS, false>()) return rc;
   static const bool timing = getenv("DG_CLUSTER_TIMING") && getenv("DG_CLUSTER_TIMING")[0] == '1';
   if (timing) {   // diagnostic: SM-clock stamps per chunk (distances | assignment logic | update + hand-over), synchronises
     unsigned* dbg = nullptr;
     DG_CUDA(cudaMalloc(&dbg, (size_t)B * 4 * sizeof(unsigned)));
-    cluster_seq_kernel<<<1, SEQ_THREADS, dyn, st>>>(p, seg, emb, B, F, K, centers, active, initialized, prep, prep_d, map, permuted, dbg);
+    cluster_seq_kernel<SEQ_THREADS, false><<<1, SEQ_THREADS, dyn, st>>>(p, nullptr, seg, emb, B, F, K, centers, active, initialized,
+                                                                prep, prep_d, map, permuted, dbg);
     DG_CUDA(cudaStreamSynchronize(st));
     std::vector<unsigned> hb((size_t)B * 4);
     DG_CUDA(cudaMemcpy(hb.data(), dbg, hb.size() * 4, cudaMemcpyDeviceToHost));
@@ -509,8 +547,25 @@ int launch_cluster_step(const ClusterParams& p, const float* seg, const float* e
     DG_LAUNCHED();
     return 0;
   }
-  cluster_seq_kernel<<<1, SEQ_THREADS, dyn, st>>>(p, seg, emb, B, F, K, centers, active, initialized, prep, prep_d, map,
-                                          permuted, nullptr);
+  cluster_seq_kernel<SEQ_THREADS, false><<<1, SEQ_THREADS, dyn, st>>>(p, nullptr, seg, emb, B, F, K, centers, active, initialized,
+                                                              prep, prep_d, map, permuted, nullptr);
+  DG_LAUNCHED();
+  return 0;
+}
+
+// T independent states over the same B chunks, each from its own {tau, rho, delta} (trials_dev [T][3] float64): one prep pass,
+// then one CTA per state.  States beyond the resident CTAs run in later waves of the same launch.
+int launch_cluster_sweep(const ClusterParams& p, const double* trials_dev, int T, const float* seg, const float* emb, int B,
+                         int F, int K, double* centers, int* active, int* initialized, float* prep, double* prep_d,
+                         int32_t* maps, cudaStream_t st) {
+  ProfScope _ps("cluster_sweep", st);
+  if (check_cluster_shape("cluster_sweep", p, K)) return -1;
+  if (B <= 0 || T <= 0) return 0;
+  cluster_prep_kernel<<<B, 128, 0, st>>>(seg, emb, F, K, p.D, prep, prep_d);
+  DG_LAUNCHED();
+  if (int rc = cluster_seq_allow_dyn<SWEEP_THREADS, true>()) return rc;
+  cluster_seq_kernel<SWEEP_THREADS, true><<<T, SWEEP_THREADS, cluster_seq_dyn(p.M, p.D, K), st>>>(
+      p, trials_dev, seg, emb, B, F, K, centers, active, initialized, prep, prep_d, maps, nullptr, nullptr);
   DG_LAUNCHED();
   return 0;
 }

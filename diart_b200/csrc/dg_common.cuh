@@ -253,11 +253,17 @@ int launch_cluster_merge(const double* records, int world, int rank, const Clust
                          int* active, double* base, int* base_active, int* initialized, int32_t* relabel,
                          cudaStream_t st);
 int launch_relabel_maps(int32_t* maps, int n, const int32_t* relabel, cudaStream_t st);
+// T independent states, thresholds trials_dev [T][3] = {tau, rho, delta} float64; centers [T][M][D], active [T][32],
+// initialized [T][2], maps [T][B][K]
+int launch_cluster_sweep(const ClusterParams& p, const double* trials_dev, int T, const float* seg, const float* emb, int B,
+                         int F, int K, double* centers, int* active, int* initialized, float* prep, double* prep_d,
+                         int32_t* maps, cudaStream_t st);
 size_t cluster_prep_floats(int B, int K);
 // post.cu -- aggregation + binarisation + run-length turns (reference diarization.py:205-232)
 int launch_post(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map, int n_hist, int B,
                 int F, int K, int M, int nw, const int32_t* plan, int plan_stride, const double* hamming, double tau,
-                int32_t* header, uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st);
+                int32_t* header, uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st,
+                const double* taus = nullptr /*[T]: per-state thresholds, map [T][B][K], header [T][B][4]*/, int T = 1);
 int launch_expand_windows(const float* ring, long long r0, int C, int hop, int S, int B, float* wav, cudaStream_t st);
 int launch_post_history(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map, int n_hist,
                         int B, int F, int K, int keep, float* new_seg, int32_t* new_map, cudaStream_t st);

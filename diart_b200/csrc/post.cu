@@ -14,6 +14,11 @@
 //
 // One CTA per chunk.  Output: per chunk {offset, count, frames} and a packed turn list (speaker << 20 | on << 10 | off),
 // each chunk's turns contiguous, ordered by speaker then time (the order Binarize emits them).
+//
+// A second grid dimension runs independent states over the same scores and plan (hyper-parameter sweep): CTA (c, t) reads
+// maps row block t ([B][K] at map + t B K), thresholds at taus[t] (NULL: `tau`, one state) and writes header row block t.  The
+// turns of all states share one counter; each state's headers locate its turns.  STATES = false compiles the single-state
+// form of the pipeline.
 #include "dg_common.cuh"
 
 namespace dg {
@@ -22,14 +27,20 @@ constexpr int POST_THREADS = 256;
 
 // plan row (int32): [0] nb buffers aggregated, [1] nf frames of the region crop, [2] first_nf (> 0: first buffer of a
 // stream, output = crop of [0, region.end) with its last nf frames replaced), [3] first_lo, [4 ..] lo of each buffer
+template <bool STATES>
 __global__ void __launch_bounds__(POST_THREADS)
 post_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map, const float* __restrict__ hist_seg,
             const int32_t* __restrict__ hist_map, int n_hist, int B, int F, int K, int M, int nw,
             const int32_t* __restrict__ plan, int plan_stride, const double* __restrict__ hamming, double tau,
-            int32_t* __restrict__ header /*[B][4]*/, uint32_t* __restrict__ turns, int turn_cap,
-            unsigned int* __restrict__ total) {
+            const double* __restrict__ taus, int32_t* __restrict__ header /*[gridDim.y][B][4]*/, uint32_t* __restrict__ turns,
+            int turn_cap, unsigned int* __restrict__ total) {
   extern __shared__ unsigned char sm_raw[];
   const int c = blockIdx.x;
+  if constexpr (STATES) {
+    map += (size_t)blockIdx.y * B * K;
+    header += (size_t)blockIdx.y * B * 4;
+    tau = taus[blockIdx.y];
+  }
   const int32_t* pl = plan + (size_t)c * plan_stride;
   const int nb = pl[0], nf = pl[1], first_nf = pl[2], first_lo = pl[3];
   const int nfo = first_nf > 0 ? first_nf : nf;
@@ -140,8 +151,13 @@ __global__ void post_history_kernel(const float* __restrict__ seg, const int32_t
 
 int launch_post(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map, int n_hist, int B,
                 int F, int K, int M, int nw, const int32_t* plan, int plan_stride, const double* hamming, double tau,
-                int32_t* header, uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st) {
+                int32_t* header, uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st, const double* taus,
+                int T) {
   ProfScope _ps("post_aggregate", st);
+  if (T < 1 || T > 65535 || (T > 1 && !taus)) {
+    set_error("post: 1 <= states <= 65535, per-state thresholds for more than one");
+    return -1;
+  }
   if (M > 64 || F > 1023 || K > 127) {
     set_error("post: at most 64 global speakers, 1023 frames");
     return -1;
@@ -156,12 +172,17 @@ int launch_post(const float* seg, const int32_t* map, const float* hist_seg, con
     cudaGetDevice(&dev);
     static bool done[64] = {};
     if (dev < 64 && !done[dev]) {
-      DG_CUDA(cudaFuncSetAttribute(post_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+      DG_CUDA(cudaFuncSetAttribute(post_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+      DG_CUDA(cudaFuncSetAttribute(post_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
       done[dev] = true;
     }
   }
-  post_kernel<<<B, POST_THREADS, smem, st>>>(seg, map, hist_seg, hist_map, n_hist, B, F, K, M, nw, plan, plan_stride, hamming,
-                                            tau, header, turns, turn_cap, total);
+  if (taus)
+    post_kernel<true><<<dim3(B, T), POST_THREADS, smem, st>>>(seg, map, hist_seg, hist_map, n_hist, B, F, K, M, nw, plan,
+                                                              plan_stride, hamming, tau, taus, header, turns, turn_cap, total);
+  else
+    post_kernel<false><<<B, POST_THREADS, smem, st>>>(seg, map, hist_seg, hist_map, n_hist, B, F, K, M, nw, plan, plan_stride,
+                                                      hamming, tau, nullptr, header, turns, turn_cap, total);
   DG_LAUNCHED();
   return 0;
 }

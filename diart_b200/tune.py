@@ -1,0 +1,292 @@
+"""Hyper-parameter sweep of ``SpeakerDiarization`` on the device: one network pass per file, many trials per clustering launch.
+
+The reference tunes ``tau_active``, ``rho_update`` and ``delta_new`` (``SpeakerDiarization.hyper_parameters()``) with
+``diart.tune``: ``Optimizer.objective`` (reference ``src/diart/optim.py:98-122``) runs a full ``Benchmark`` per trial, i.e. the
+segmentation and embedding networks once per trial and file.  None of the three parameters reaches the networks -- they
+are read by the clustering (``blocks/clustering.py:137-142,168``) and by ``Binarize(tau_active)`` only.  So here a file
+goes through the networks ONCE (the fused pipeline, batches of 256) and ``dg_sweep_run`` clusters and post-processes the
+resulting scores and embeddings for T trials at once (one CTA per trial state, ``csrc/cluster.cu``; one CTA per chunk
+and trial, ``csrc/post.cu``).
+
+For each trial :meth:`HyperParameterSweep.run` returns what ``Benchmark.run_single`` (``inference.py:308-357``) returns
+for a pipeline with that trial's parameters: the whole-file prediction that ``PredictionAccumulator(uri)`` (patch
+collar 0.05 s) collects over the per-chunk outputs, assembled from the packed turn list without building per-chunk
+annotations.  Scoring (DER) is left to the caller, as ``Benchmark.evaluate`` does.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import time
+from dataclasses import dataclass
+from typing import Dict, List, Mapping, Optional, Sequence
+
+import numpy as np
+import torch
+
+from . import _lib
+from .blocks.diarization import SpeakerDiarization, SpeakerDiarizationConfig
+from .blocks.post import post_plan, turn_times
+from .core import Annotation, Segment
+from .operators import DeviceAudioStream
+
+NETWORK_BATCH = 256           # windows per network step (the benchmarked batch)
+TRIALS_PER_LAUNCH = 1024      # trials per dg_sweep_run; more run as further launches over the same network outputs
+PATCH_COLLAR = 0.05           # PredictionAccumulator's default (sinks.py)
+
+
+def trial_params(trials: Sequence[Mapping[str, float]], config: SpeakerDiarizationConfig) -> np.ndarray:
+    """trials (dicts keyed by the reference's HyperParameter names) -> float64 (T, 3) {tau_active, rho_update, delta_new};
+    a missing key takes the config's value.  Other keys (gamma, beta, latency, step, max_speakers, ...) change the network
+    pass or the plan and cannot vary within one sweep: ValueError."""
+    names = [hp.name for hp in SpeakerDiarization.hyper_parameters()]
+    trials = list(trials)
+    if not trials:
+        raise ValueError("at least one trial is needed")
+    out = np.empty((len(trials), len(names)), dtype=np.float64)
+    for i, trial in enumerate(trials):
+        unknown = sorted(set(trial) - set(names))
+        if unknown:
+            raise ValueError(f"trial {i}: {unknown} cannot be swept (only {names}; the others change the network pass or "
+                             f"the plan and stay fixed per sweep)")
+        out[i] = [float(trial.get(n, getattr(config, n))) for n in names]
+    return out
+
+
+@dataclass
+class FileWindows:
+    """What ``FileAudioSource`` + ``rearrange_audio_stream`` make of one file."""
+    samples: np.ndarray       # the padded file, zero-filled to whole blocks of `step` samples
+    offset: int               # first sample of window 0
+    num_windows: int
+    starts: np.ndarray        # float64 (num_windows,) start time of each window (before the timestamp shift)
+    padding: tuple            # (left, right) seconds, config.get_file_padding
+    chunk_samples: int
+    step_samples: int
+
+    def window(self, i: int) -> np.ndarray:
+        a = self.offset + i * self.step_samples
+        return self.samples[a:a + self.chunk_samples]
+
+
+def file_windows(waveform: np.ndarray, config: SpeakerDiarizationConfig) -> FileWindows:
+    """The windows ``Benchmark.run_single`` feeds a pipeline for a 1-D waveform at ``config.sample_rate``: padding from
+    ``config.get_file_padding`` (reference ``inference.py:332``), blocks of ``step`` seconds with the last incomplete one
+    zero-padded (``sources.py:88-127``), then ``rearrange_audio_stream``'s windows (``operators.py:44-100``)."""
+    x = np.asarray(waveform, dtype=np.float32)
+    if x.ndim != 1:
+        raise ValueError(f"expected a 1-D waveform, got shape {x.shape}")
+    sr = config.sample_rate
+    left, right = config.get_file_padding(file_duration=len(x) / sr)
+    n_left = int(np.rint(left * sr)) if left > 0 else 0
+    n_right = int(np.rint(right * sr)) if right > 0 else 0
+    block = int(np.rint(config.step * sr))                    # FileAudioSource(block_duration=step)
+    chunk, step = int(round(sr * config.duration)), int(round(sr * config.step))
+    n = n_left + len(x) + n_right
+    n_blocks = -(-n // block)
+    samples = np.zeros(n_blocks * block, dtype=np.float32)
+    samples[n_left:n_left + len(x)] = x
+    # rearrange_audio_stream: each block of `step` samples extends the chunk; once it holds more than `chunk` samples it is
+    # truncated to the last `chunk` and its start time advances by `step`; a chunk of exactly `chunk` samples is emitted
+    first = -(-chunk // step)                                 # blocks until the first emission
+    num_windows = max(0, n_blocks - first + 1)
+    t, starts = 0.0, np.empty(num_windows)
+    if first * step > chunk:
+        t += config.step
+    for i in range(num_windows):
+        if i:
+            t += config.step
+        starts[i] = t
+    return FileWindows(samples, first * step - chunk, num_windows, starts, (left, right), chunk, step)
+
+
+def assemble_predictions(header: np.ndarray, turns: np.ndarray, n_turns: int, out_start: np.ndarray, out_res: np.ndarray,
+                         labels: Sequence[str], shift: float = 0.0, uri: Optional[str] = None,
+                         collar: float = PATCH_COLLAR) -> List[Annotation]:
+    """header int32 (T, N, 4) + packed turns of T trials over the same N chunks -> per trial the whole-file prediction of
+    ``PredictionAccumulator(uri, collar)`` over that trial's per-chunk annotations (``DevicePostPath.annotations``).
+
+    Vectorised ``Annotation.support(collar)`` (``core.py``): per trial and label (labels in string order), segments sorted
+    by (start, end); a segment joins the current one when it starts before its end or less than ``collar`` after it."""
+    T, N = header.shape[:2]
+    row, g, s, e = turn_times(header.reshape(T * N, 4), turns, n_turns, out_start, out_res, shift)
+    live = (e - s) > 1e-6                                     # Annotation drops empty segments (Segment.__bool__)
+    row, g, s, e = row[live], g[live], s[live], e[live]
+    trial = row // N
+    M = len(labels)
+    rank = np.empty(M, dtype=np.int64)
+    rank[sorted(range(M), key=lambda i: str(labels[i]))] = np.arange(M)
+    order = np.lexsort((e, s, rank[g], trial))
+    trial, g, s, e = trial[order], g[order], s[order], e[order]
+    gid = trial * M + rank[g]
+    # running maximum of the ends within each (trial, label) group: ranks of the end values, offset per group, so that one
+    # integer maximum-scan restarts at every group
+    u, inv = np.unique(e, return_inverse=True)
+    span = np.int64(len(u))
+    cm = u[np.maximum.accumulate(gid * span + inv) - gid * span]
+    first = np.ones(len(s), dtype=bool)
+    first[1:] = gid[1:] != gid[:-1]
+    prev = np.empty_like(cm)
+    prev[0:1] = 0.0
+    prev[1:] = cm[:-1]
+    joins = ~first & ((s - prev < collar) | (s <= prev))
+    heads = np.flatnonzero(~joins)
+    tails = np.append(heads[1:], len(s))[:len(heads)] - 1
+    m_start, m_end, m_trial, m_g = s[heads].tolist(), cm[tails].tolist(), trial[heads].tolist(), g[heads].tolist()
+    modality = "speech" if shift == 0 else None               # what the first per-chunk annotation carries
+    out = [Annotation(uri=uri, modality=modality) for _ in range(T)]
+    track = [0] * T
+    for a, b, t, k in zip(m_start, m_end, m_trial, m_g):
+        out[t][Segment(a, b), track[t]] = labels[k]
+        track[t] += 1
+    return out
+
+
+@dataclass
+class SweepOutputs:
+    header: np.ndarray        # int32 (T, N, 4)
+    turns: np.ndarray         # uint32, n_turns valid
+    n_turns: int
+    out_start: np.ndarray     # (N,) per-chunk output start / resolution
+    out_res: np.ndarray
+    maps: Optional[torch.Tensor] = None      # int32 (T, N, K) on the device
+    centers: Optional[torch.Tensor] = None   # float64 (T, M, D) on the device
+    device_seconds: float = 0.0
+
+
+class HyperParameterSweep:
+    """Runs ``SpeakerDiarization(config)`` over a file for many (tau_active, rho_update, delta_new) trials at the cost of one
+    network pass.  Needs the native segmentation and embedding models.
+
+        sweep = HyperParameterSweep(config)
+        predictions = sweep.run(waveform, uri="file1", trials=[{"tau_active": 0.5}, {"delta_new": 0.8, "rho_update": 0.2}])
+    """
+
+    def __init__(self, config: SpeakerDiarizationConfig):
+        self.config = config
+        self.pipeline = SpeakerDiarization(config)
+        if self.pipeline._native_models() is None:
+            raise _lib.DiartB200Error("HyperParameterSweep needs the native segmentation and embedding models")
+        self.device = self.pipeline.segmentation.device
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self._h: Optional[C.c_void_p] = None
+        self._dims = None
+        self._turns = np.empty(0, dtype=np.uint32)
+        self.timing: Dict[str, float] = {}        # seconds of the last run: network, sweep (device events), assembly
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None) is not None:
+                _lib.lib().dg_sweep_destroy(self._h)
+        except Exception:  # noqa: BLE001
+            pass
+
+    # ------------------------------------------------------------------ network pass
+    def network_pass(self, fw: FileWindows):
+        """scores (N, F, K) and embeddings (N, K, D) of every window, on the device: the fused pipeline in batches of 256
+        (its own clustering runs too; its maps are not used)"""
+        cfg, pipe = self.config, self.pipeline
+        pipe.reset()
+        stream = DeviceAudioStream(cfg.duration, cfg.step, cfg.sample_rate, max_windows=NETWORK_BATCH, device=self.device)
+        pushed, segs, embs, inflight = fw.offset, [], [], []
+        with torch.cuda.device(self.device):
+            for i0 in range(0, fw.num_windows, NETWORK_BATCH):
+                B = min(NETWORK_BATCH, fw.num_windows - i0)
+                need = fw.offset + (i0 + B - 1) * fw.step_samples + fw.chunk_samples
+                stream.push(fw.samples[pushed:need])
+                pushed = need
+                inflight.append(stream.windows(B))           # must stay alive until collected
+                pipe.submit(inflight[-1])
+                if len(inflight) == 2:
+                    seg, emb, _ = pipe.collect()
+                    segs.append(seg)
+                    embs.append(emb)
+                    inflight.pop(0)
+            while inflight:
+                seg, emb, _ = pipe.collect()
+                segs.append(seg)
+                embs.append(emb)
+                inflight.pop(0)
+            seg, emb = torch.cat(segs), torch.cat(embs)
+        return seg, emb
+
+    # ------------------------------------------------------------------ clustering + post-path for T trials
+    def _handle(self, F: int, K: int, D: int):
+        nw = int(round(self.config.latency / self.config.step))
+        dims = (F, K, D, nw)
+        if self._h is None or self._dims != dims:
+            if self._h is not None:
+                _lib.lib().dg_sweep_destroy(self._h)
+                self._h = None
+            ham = np.ascontiguousarray(np.hamming(F), dtype=np.float64)
+            h = C.c_void_p()
+            _lib.check(_lib.lib().dg_sweep_create(int(self.config.max_speakers), D, F, K, nw, ham.ctypes.data,
+                                                  self.device.index, C.byref(h)))
+            self._h, self._dims = h, dims
+        return self._h, nw
+
+    def sweep(self, seg: torch.Tensor, emb: torch.Tensor, starts: np.ndarray, params: np.ndarray,
+              keep_state: bool = False) -> SweepOutputs:
+        """dg_sweep_run over device scores / embeddings of N chunks starting at ``starts`` for params (T, 3)"""
+        N, F, K = seg.shape
+        D = emb.shape[2]
+        M = int(self.config.max_speakers)
+        h, nw = self._handle(F, K, D)
+        res = self._seg_resolution(float(starts[0]), F)
+        plan, out_start, out_res = post_plan(np.asarray(starts, dtype=np.float64), res, np.zeros(0), np.zeros(0), nw, F,
+                                             self.config.step, self.config.latency)
+        plan = np.ascontiguousarray(plan)
+        params = np.ascontiguousarray(params, dtype=np.float64)
+        T = len(params)
+        header = np.empty((T, N, 4), dtype=np.int32)
+        maps = torch.empty((T, N, K), dtype=torch.int32, device=self.device) if keep_state else None
+        centers = torch.empty((T, M, D), dtype=torch.float64, device=self.device) if keep_state else None
+        if len(self._turns) < T * N * 8:
+            self._turns = np.empty(T * N * 8, dtype=np.uint32)
+        n = C.c_int()
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream(self.device)
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            for attempt in range(2):
+                e0.record(st)
+                rc = _lib.lib().dg_sweep_run(h, seg.data_ptr(), emb.data_ptr(), N, params.ctypes.data, T, plan.ctypes.data,
+                                             _lib.ptr(maps), _lib.ptr(centers), header.ctypes.data, self._turns.ctypes.data,
+                                             len(self._turns), C.byref(n), st.cuda_stream)
+                e1.record(st)
+                if rc == -1 and n.value > len(self._turns):   # more turns than the host buffer: grow it, run again
+                    self._turns = np.empty(n.value, dtype=np.uint32)
+                    continue
+                _lib.check(rc)
+                break
+            e1.synchronize()
+        return SweepOutputs(header, self._turns[:n.value].copy(), n.value, out_start, out_res, maps, centers,
+                            e0.elapsed_time(e1) / 1e3)
+
+    def _seg_resolution(self, start: float, F: int) -> float:
+        # SpeakerDiarization.__call__: waveforms[0].extent.duration / F, the extent of a window of 1 / sample_rate frames
+        sr = self.config.sample_rate
+        end = start + int(np.rint(self.config.duration * sr)) * (1 / sr)
+        return (end - start if end > start else 0.0) / F
+
+    # ------------------------------------------------------------------ the public entry
+    def run(self, waveform: np.ndarray, uri: Optional[str] = None,
+            trials: Sequence[Mapping[str, float]] = ({},)) -> List[Annotation]:
+        """1-D float32 waveform at ``config.sample_rate`` -> one whole-file prediction per trial (the prediction
+        ``Benchmark.run_single`` returns for a pipeline with that trial's tau_active / rho_update / delta_new)"""
+        params = trial_params(trials, self.config)
+        t0 = time.perf_counter()
+        fw = file_windows(waveform, self.config)
+        seg, emb = self.network_pass(fw)
+        torch.cuda.synchronize(self.device)
+        t1 = time.perf_counter()
+        labels = [f"speaker{g}" for g in range(int(self.config.max_speakers))]
+        shift = -fw.padding[0]
+        out, dev, host = [], 0.0, 0.0
+        for i in range(0, len(params), TRIALS_PER_LAUNCH):
+            r = self.sweep(seg, emb, fw.starts, params[i:i + TRIALS_PER_LAUNCH])
+            dev += r.device_seconds
+            t2 = time.perf_counter()
+            out += assemble_predictions(r.header, r.turns, r.n_turns, r.out_start, r.out_res, labels, shift, uri)
+            host += time.perf_counter() - t2
+        self.timing = {"network": t1 - t0, "sweep": dev, "assembly": host}
+        return out

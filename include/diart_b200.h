@@ -47,6 +47,7 @@ typedef struct dg_cluster dg_cluster;
 typedef struct dg_pipeline dg_pipeline;
 typedef struct dg_post dg_post;
 typedef struct dg_stream dg_stream;
+typedef struct dg_sweep dg_sweep;
 
 const char* dg_last_error(void);
 int dg_version(void);
@@ -190,6 +191,31 @@ int dg_pipeline_call_host(dg_pipeline* h, dg_post* post, const float* const* row
                           const int32_t* plan_host, int32_t* header_host, uint32_t* turns_host, int turn_cap_host,
                           int* n_turns, float* seg_host /*nullable*/, int32_t* map_host /*nullable*/);
 int64_t dg_pipeline_last_call_h2d_bytes(const dg_pipeline* h);
+
+/* ---- hyper-parameter sweep: the reference tunes tau_active, rho_update and delta_new by running its whole pipeline once per
+ *      trial over every file (Optimizer.objective -> Benchmark, reference src/diart/optim.py:98-122, inference.py:392-432).
+ *      None of the three reaches the networks, so here one file's network outputs (seg_dev [N,F,K], emb_dev [N,K,D], e.g.
+ *      from dg_pipeline_submit / collect) are clustered and post-processed for T trials at once: T independent
+ *      OnlineSpeakerClustering states (cosine, max_speakers), each followed by the dg_post_* post-path with its own tau, all
+ *      N chunks in one pass without history.  Per trial the result is the one a fresh pipeline with that trial's thresholds
+ *      produces over the same N chunks.
+ *      dg_sweep_create takes the limits of dg_cluster_create and dg_post_create (max_speakers <= 32, local_speakers <= 8 and
+ *      <= max_speakers, frames <= 1023, 1 <= num_windows <= 256) and hamming_host = np.hamming(frames) in float64.
+ *      dg_sweep_run:
+ *        params_host float64 [T][3] = {tau_active, rho_update, delta_new} per trial (finite), 1 <= T <= 65535, N >= 1;
+ *        plan_host   int32 [N][4 + num_windows]: the dg_post_step plan of the N chunks as ONE batch of a fresh stream;
+ *        maps_dev    int32 [T][N][K] or NULL: each trial's speaker maps (dg_cluster_step's map_dev);
+ *        centers_dev float64 [T][M][D] or NULL: each trial's final centroids (zero rows for inactive speakers);
+ *        header_host int32 [T][N][4] and turns_host uint32 [turn_cap_host]: as dg_post_step, the turns of all trials in one
+ *        list, located by each trial's headers.  When the turns exceed turn_cap_host the call fails with DG_EINVAL and
+ *        *n_turns holds the count needed.
+ *      Synchronous (synchronises `stream`). ---- */
+int dg_sweep_create(int max_speakers, int dim, int frames, int local_speakers, int num_windows, const double* hamming_host,
+                    int device, dg_sweep** out);
+int dg_sweep_run(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, const double* params_host, int T,
+                 const int32_t* plan_host, int32_t* maps_dev, double* centers_dev, int32_t* header_host, uint32_t* turns_host,
+                 int turn_cap_host, int* n_turns, void* stream);
+int dg_sweep_destroy(dg_sweep* h);
 
 /* ---- device-side audio stream: rearrange_audio_stream (reference src/diart/operators.py:44-100) with the ring buffer in
  *      HBM.  The host pushes every sample ONCE (step_samples new samples per chunk instead of chunk_samples: 8.2 MB
