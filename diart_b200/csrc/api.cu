@@ -2488,6 +2488,7 @@ extern "C" int dg_post_step(dg_post* h, const float* seg_dev, const int32_t* map
 struct dg_sweep {
   int device = 0, M = 0, D = 0, F = 0, K = 0, nw = 1;
   DevBuf hamming, in, centers, active, init, prep, prep_d, maps, header, turns, total;
+  DevBuf score_in, hoff, hseg, comp;   // dg_sweep_score: chunk times and reference, hypothesis segments, components
   PinnedBuf pin;                  // params, taus and plan in; error flags, header, total and a turn prefix out
 };
 
@@ -2513,28 +2514,36 @@ extern "C" int dg_sweep_destroy(dg_sweep* h) {
   return DG_OK;
 }
 
-extern "C" int dg_sweep_run(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, const double* params_host, int T,
-                            const int32_t* plan_host, int32_t* maps_dev, double* centers_dev, int32_t* header_host,
-                            uint32_t* turns_host, int turn_cap_host, int* n_turns, void* stream) {
-  if (!h || !seg_dev || !emb_dev || !params_host || !plan_host || !header_host || !turns_host || N < 1 || T < 1 ||
-      T > 65535) {
-    set_error("dg_sweep_run: bad arguments (need N >= 1, 1 <= T <= 65535, non-null buffers)");
+// the argument checks dg_sweep_run and dg_sweep_score share (before any launch)
+static int sweep_check(const char* who, dg_sweep* h, const float* seg_dev, const float* emb_dev, int N,
+                       const double* params_host, int T, const int32_t* plan_host) {
+  if (!h || !seg_dev || !emb_dev || !params_host || !plan_host || N < 1 || T < 1 || T > 65535) {
+    set_error(std::string(who) + ": bad arguments (need N >= 1, 1 <= T <= 65535, non-null buffers)");
     return DG_EINVAL;
   }
   for (int i = 0; i < 3 * T; i++)
     if (!std::isfinite(params_host[i])) {
-      set_error("dg_sweep_run: trial " + std::to_string(i / 3) + " has a parameter that is not finite");
+      set_error(std::string(who) + ": trial " + std::to_string(i / 3) + " has a parameter that is not finite");
       return DG_EINVAL;
     }
-  DG_CUDA(cudaSetDevice(h->device));
-  cudaStream_t st = (cudaStream_t)stream;
+  return DG_OK;
+}
+
+// pinned output layout of sweep_cluster_post: error flags [T][2], header [T][N][4], total (16 bytes), a prefix of the turns
+static size_t sweep_out_bytes(int T, int N) { return (size_t)T * 8 + (size_t)T * N * 16 + 16 + (size_t)DG_POST_PREFIX * 4; }
+
+// Clustering + post-path of T trials over the N chunks: header [T][N][4] and turns stay on the device (h->header, h->turns),
+// the turn count comes back in *total.  with_header: the header and a prefix of the turns travel to the pinned buffer in the
+// same copy as the count (sweep_out_bytes layout).  Synchronises `st`.
+static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, const double* params_host,
+                              int T, const int32_t* plan_host, int32_t* maps_dev, double* centers_dev, bool with_header,
+                              cudaStream_t st, unsigned int* total_out) {
   const int stride = 4 + h->nw, M = h->M, D = h->D, K = h->K, F = h->F;
   // host -> device: params [T][3], taus [T], plan [N][stride], one copy
   const size_t params_b = (size_t)T * 24, taus_b = (size_t)T * 8, plan_b = (size_t)N * stride * 4;
   const size_t in_b = params_b + taus_b + plan_b;
-  // device -> host: error flags [T][2], header [T][N][4], total, a prefix of the turns
   const size_t init_b = (size_t)T * 8, header_b = (size_t)T * N * 16;
-  const size_t out_b = init_b + header_b + 16 + (size_t)DG_POST_PREFIX * 4;
+  const size_t out_b = sweep_out_bytes(T, N);
   // the device turn buffer starts at a guess and grows to the true count (the kernel counts every turn, writes those that fit)
   const size_t turn_guess = std::max<size_t>((size_t)T * N * 8, (size_t)DG_POST_PREFIX);
   if (h->in.ensure(in_b) || h->centers.ensure((size_t)T * M * D * 8) || h->active.ensure((size_t)T * 32 * 4) ||
@@ -2575,10 +2584,11 @@ extern "C" int dg_sweep_run(dg_sweep* h, const float* seg_dev, const float* emb_
                           h->header.as<int32_t>(), h->turns.as<uint32_t>(), cap, h->total.as<unsigned int>(), st, d_taus, T)))
       return rc;
     DG_CUDA(cudaMemcpyAsync(pin, h->init.p, init_b, cudaMemcpyDeviceToHost, st));
-    DG_CUDA(cudaMemcpyAsync(pin + init_b, h->header.p, header_b, cudaMemcpyDeviceToHost, st));
+    if (with_header) DG_CUDA(cudaMemcpyAsync(pin + init_b, h->header.p, header_b, cudaMemcpyDeviceToHost, st));
     DG_CUDA(cudaMemcpyAsync(pin + init_b + header_b, h->total.p, 4, cudaMemcpyDeviceToHost, st));
-    DG_CUDA(cudaMemcpyAsync(pin + init_b + header_b + 16, h->turns.p, (size_t)std::min(DG_POST_PREFIX, cap) * 4,
-                            cudaMemcpyDeviceToHost, st));
+    if (with_header)
+      DG_CUDA(cudaMemcpyAsync(pin + init_b + header_b + 16, h->turns.p, (size_t)std::min(DG_POST_PREFIX, cap) * 4,
+                              cudaMemcpyDeviceToHost, st));
     DG_CUDA(cudaStreamSynchronize(st));
     memcpy(&total, pin + init_b + header_b, 4);
     if (total <= (unsigned int)cap) break;
@@ -2591,6 +2601,26 @@ extern "C" int dg_sweep_run(dg_sweep* h, const float* seg_dev, const float* emb_
       set_error("Cannot update unknown centers");   // reference clustering.py:98 (AssertionError)
       return DG_EINVAL;
     }
+  *total_out = total;
+  return DG_OK;
+}
+
+extern "C" int dg_sweep_run(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, const double* params_host, int T,
+                            const int32_t* plan_host, int32_t* maps_dev, double* centers_dev, int32_t* header_host,
+                            uint32_t* turns_host, int turn_cap_host, int* n_turns, void* stream) {
+  if (!header_host || !turns_host) {
+    set_error("dg_sweep_run: bad arguments (need N >= 1, 1 <= T <= 65535, non-null buffers)");
+    return DG_EINVAL;
+  }
+  int rc;
+  if ((rc = sweep_check("dg_sweep_run", h, seg_dev, emb_dev, N, params_host, T, plan_host))) return rc;
+  DG_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned int total = 0;
+  if ((rc = sweep_cluster_post(h, seg_dev, emb_dev, N, params_host, T, plan_host, maps_dev, centers_dev, true, st, &total)))
+    return rc;
+  const unsigned char* pin = h->pin.as<unsigned char>();
+  const size_t init_b = (size_t)T * 8, header_b = (size_t)T * N * 16;
   if (n_turns) *n_turns = (int)total;
   memcpy(header_host, pin + init_b, header_b);
   if ((long long)total > (long long)turn_cap_host) {
@@ -2603,6 +2633,107 @@ extern "C" int dg_sweep_run(dg_sweep* h, const float* seg_dev, const float* emb_
     DG_CUDA(cudaMemcpyAsync(turns_host + pre, h->turns.as<uint32_t>() + pre, (size_t)(total - pre) * 4,
                             cudaMemcpyDeviceToHost, st));
     DG_CUDA(cudaStreamSynchronize(st));
+  }
+  return DG_OK;
+}
+
+// the reference rows: finite, start < end, labels in [0, R), each label's rows in time order without overlap
+static int sweep_check_reference(const double* ref_host, const int32_t* ref_label_host, int S, int R) {
+  if (R < 0 || R > 32 || S < 0 || (S > 0 && (!ref_host || !ref_label_host))) {
+    set_error("dg_sweep_score: need 0 <= reference labels <= 32, rows >= 0, non-null reference arrays");
+    return DG_EINVAL;
+  }
+  double last[32];
+  for (int r = 0; r < 32; r++) last[r] = -INFINITY;
+  for (int i = 0; i < S; i++) {
+    const double a = ref_host[2 * i], b = ref_host[2 * i + 1];
+    const int r = ref_label_host[i];
+    if (r < 0 || r >= R) {
+      set_error("dg_sweep_score: reference row " + std::to_string(i) + " has a label outside [0, R)");
+      return DG_EINVAL;
+    }
+    if (!std::isfinite(a) || !std::isfinite(b) || !(a < b)) {
+      set_error("dg_sweep_score: reference row " + std::to_string(i) + " is not finite, empty or reversed");
+      return DG_EINVAL;
+    }
+    if (a < last[r]) {
+      set_error("dg_sweep_score: reference row " + std::to_string(i) + " is out of order or overlaps an earlier row of its label");
+      return DG_EINVAL;
+    }
+    last[r] = b;
+  }
+  return DG_OK;
+}
+
+extern "C" int dg_sweep_score(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, const double* params_host,
+                              int T, const int32_t* plan_host, const double* out_start_host, const double* out_res_host,
+                              double shift, double collar, const double* ref_host, const int32_t* ref_label_host, int S,
+                              int R, double* components_host, int32_t* hyp_offsets_dev, double* hyp_segments_dev,
+                              int hyp_cap, void* stream) {
+  int rc;
+  if ((rc = sweep_check("dg_sweep_score", h, seg_dev, emb_dev, N, params_host, T, plan_host))) return rc;
+  if (!out_start_host || !out_res_host || !components_host || hyp_cap < 0 || !std::isfinite(shift) ||
+      !std::isfinite(collar) || collar < 0) {
+    set_error("dg_sweep_score: bad arguments (need chunk times, a components buffer, finite shift, finite collar >= 0, "
+              "hyp_cap >= 0)");
+    return DG_EINVAL;
+  }
+  for (int c = 0; c < N; c++)
+    if (!std::isfinite(out_start_host[c]) || !std::isfinite(out_res_host[c])) {
+      set_error("dg_sweep_score: chunk " + std::to_string(c) + " has an output time that is not finite");
+      return DG_EINVAL;
+    }
+  if ((rc = sweep_check_reference(ref_host, ref_label_host, S, R))) return rc;
+  DG_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned int total = 0;
+  if ((rc = sweep_cluster_post(h, seg_dev, emb_dev, N, params_host, T, plan_host, nullptr, nullptr, false, st, &total)))
+    return rc;
+  const int M = h->M, TM = T * M;
+  // host -> device, one copy: out_start [N], out_res [N], reference segments [S][2] grouped by label, label offsets [R + 1]
+  const size_t times_b = (size_t)N * 16, rseg_b = (size_t)S * 16, roff_b = (size_t)(R + 1) * 4;
+  const size_t in_b = times_b + rseg_b + roff_b, comp_b = (size_t)T * 40;
+  if (h->score_in.ensure(in_b) || h->hoff.ensure((size_t)(TM + 1) * 4) || h->hseg.ensure((size_t)std::max(total, 1u) * 16) ||
+      h->comp.ensure(comp_b) || h->pin.ensure(std::max(in_b, comp_b + 16)))
+    return DG_ECUDA;
+  unsigned char* pin = h->pin.as<unsigned char>();
+  memcpy(pin, out_start_host, (size_t)N * 8);
+  memcpy(pin + (size_t)N * 8, out_res_host, (size_t)N * 8);
+  double* rseg = reinterpret_cast<double*>(pin + times_b);
+  int32_t* roff = reinterpret_cast<int32_t*>(pin + times_b + rseg_b);
+  for (int r = 0; r <= R; r++) roff[r] = 0;
+  for (int i = 0; i < S; i++) roff[ref_label_host[i] + 1]++;
+  for (int r = 0; r < R; r++) roff[r + 1] += roff[r];
+  int fill[32];
+  for (int r = 0; r < R; r++) fill[r] = roff[r];
+  for (int i = 0; i < S; i++) {     // stable: each label keeps its rows' order
+    const int o = fill[ref_label_host[i]]++;
+    rseg[2 * o] = ref_host[2 * i];
+    rseg[2 * o + 1] = ref_host[2 * i + 1];
+  }
+  unsigned char* din = h->score_in.as<unsigned char>();
+  DG_CUDA(cudaMemcpyAsync(din, pin, in_b, cudaMemcpyHostToDevice, st));
+  const double* d_start = reinterpret_cast<const double*>(din);
+  const double* d_res = d_start + N;
+  const double* d_rseg = reinterpret_cast<const double*>(din + times_b);
+  const int* d_roff = reinterpret_cast<const int*>(din + times_b + rseg_b);
+  int* hoff = h->hoff.as<int>();
+  if ((rc = launch_der_hyp_count(h->header.as<int32_t>(), h->turns.as<uint32_t>(), T, N, M, d_start, d_res, shift, collar,
+                                 hoff, st)) ||
+      (rc = launch_der_hyp_write(h->header.as<int32_t>(), h->turns.as<uint32_t>(), T, N, M, d_start, d_res, shift, collar,
+                                 hoff, h->hseg.as<double>(), hyp_segments_dev, hyp_cap, st)) ||
+      (rc = launch_der_score(hoff, h->hseg.as<double>(), T, M, d_roff, d_rseg, R, h->comp.as<double>(), st)))
+    return rc;
+  if (hyp_offsets_dev) DG_CUDA(cudaMemcpyAsync(hyp_offsets_dev, hoff, (size_t)(TM + 1) * 4, cudaMemcpyDeviceToDevice, st));
+  DG_CUDA(cudaMemcpyAsync(pin, h->comp.p, comp_b, cudaMemcpyDeviceToHost, st));
+  DG_CUDA(cudaMemcpyAsync(pin + comp_b, hoff + TM, 4, cudaMemcpyDeviceToHost, st));
+  DG_CUDA(cudaStreamSynchronize(st));
+  memcpy(components_host, pin, comp_b);
+  int n_seg = 0;
+  memcpy(&n_seg, pin + comp_b, 4);
+  if (hyp_segments_dev && n_seg > hyp_cap) {
+    set_error("dg_sweep_score: hypothesis segment buffer too small (" + std::to_string(n_seg) + " segments)");
+    return DG_EINVAL;
   }
   return DG_OK;
 }

@@ -268,6 +268,16 @@ int launch_expand_windows(const float* ring, long long r0, int C, int hop, int S
 int launch_post_history(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map, int n_hist,
                         int B, int F, int K, int keep, float* new_seg, int32_t* new_map, cudaStream_t st);
 size_t cluster_prep_doubles(int B, int K);
+// der.cu -- DER components of sweep trials.  Hypothesis segments: count per (trial, label) and scan into offsets [T*M+1],
+// then write [offsets[T*M]][2] start / end (and, when segs_copy is given, the first copy_cap of them there too)
+int launch_der_hyp_count(const int32_t* header, const uint32_t* turns, int T, int N, int M, const double* out_start,
+                         const double* out_res, double shift, double collar, int* offsets, cudaStream_t st);
+int launch_der_hyp_write(const int32_t* header, const uint32_t* turns, int T, int N, int M, const double* out_start,
+                         const double* out_res, double shift, double collar, int* offsets, double* segs, double* segs_copy,
+                         int copy_cap, cudaStream_t st);
+// reference: R labels, offsets roff [R+1] into rseg [S][2]; comp [T][5] = {false alarm, missed, confusion, correct, total}
+int launch_der_score(const int* hoff, const double* hseg, int T, int M, const int* roff, const double* rseg, int R,
+                     double* comp, cudaStream_t st);
 // resample.cu -- polyphase sinc resampling (torchaudio's defaults): reduced ratio o / n, half-width w, T = 2w + o taps per phase
 struct RsGeom {
   int o, n, w, T;

@@ -11,14 +11,20 @@ and trial, ``csrc/post.cu``).
 For each trial :meth:`HyperParameterSweep.run` returns what ``Benchmark.run_single`` (``inference.py:308-357``) returns
 for a pipeline with that trial's parameters: the whole-file prediction that ``PredictionAccumulator(uri)`` (patch
 collar 0.05 s) collects over the per-chunk outputs, assembled from the packed turn list without building per-chunk
-annotations.  Scoring (DER) is left to the caller, as ``Benchmark.evaluate`` does.
+annotations.
+
+:meth:`HyperParameterSweep.score` goes one step further and returns what ``Benchmark.evaluate`` (``inference.py:359-390``)
+computes from those predictions: the diarization error rate components of every trial against a reference
+(``DiarizationErrorRate(collar=0, skip_overlap=False)``; definition in DESIGN.md "DER scoring"), evaluated on the device by
+``dg_sweep_score`` (``csrc/der.cu``) without building any ``Annotation``.  :meth:`HyperParameterSweep.score_files` sums them over
+files: its ``total.der`` is the value ``Optimizer.objective`` minimises.
 """
 from __future__ import annotations
 
 import ctypes as C
 import time
 from dataclasses import dataclass
-from typing import Dict, List, Mapping, Optional, Sequence
+from typing import Dict, Iterable, List, Mapping, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -32,6 +38,7 @@ from .operators import DeviceAudioStream
 NETWORK_BATCH = 256           # windows per network step (the benchmarked batch)
 TRIALS_PER_LAUNCH = 1024      # trials per dg_sweep_run; more run as further launches over the same network outputs
 PATCH_COLLAR = 0.05           # PredictionAccumulator's default (sinks.py)
+MAX_REFERENCE_LABELS = 32     # one lane per reference label in the scoring kernel
 
 
 def trial_params(trials: Sequence[Mapping[str, float]], config: SpeakerDiarizationConfig) -> np.ndarray:
@@ -139,6 +146,68 @@ def assemble_predictions(header: np.ndarray, turns: np.ndarray, n_turns: int, ou
         out[t][Segment(a, b), track[t]] = labels[k]
         track[t] += 1
     return out
+
+
+def reference_arrays(annotation: Annotation) -> Tuple[np.ndarray, np.ndarray, List]:
+    """A reference annotation -> (rows float64 (S, 2) start / end, labels int32 (S,), label names) for ``dg_sweep_score``:
+    labels numbered in string order, empty segments dropped (``Segment.__bool__``), each label reduced to the union of its
+    segments (rows of one label sorted, touching or overlapping segments merged).
+
+    pyannote.metrics scores a reference as given; where one label overlaps itself it may count that label twice in the
+    overlap.  The union counts it once: the two agree for every reference in which no label overlaps itself.
+    More than 32 labels: ValueError."""
+    by_label: Dict = {}
+    for segment, _, label in annotation.itertracks(yield_label=True):
+        if segment:
+            by_label.setdefault(label, []).append((segment.start, segment.end))
+    names = sorted(by_label, key=str)
+    if len(names) > MAX_REFERENCE_LABELS:
+        raise ValueError(f"the reference has {len(names)} labels; at most {MAX_REFERENCE_LABELS} can be scored")
+    rows, labels = [], []
+    for r, name in enumerate(names):
+        segs = sorted(by_label[name])
+        cur_s, cur_e = segs[0]
+        for a, b in segs[1:]:
+            if a <= cur_e:
+                cur_e = max(cur_e, b)
+            else:
+                rows.append((cur_s, cur_e))
+                labels.append(r)
+                cur_s, cur_e = a, b
+        rows.append((cur_s, cur_e))
+        labels.append(r)
+    return (np.array(rows, dtype=np.float64).reshape(-1, 2), np.array(labels, dtype=np.int32), names)
+
+
+@dataclass
+class DERComponents:
+    """Diarization error rate components in seconds, one entry per trial (float64 (T,) each)."""
+    false_alarm: np.ndarray
+    missed_detection: np.ndarray
+    confusion: np.ndarray
+    correct: np.ndarray
+    total: np.ndarray
+
+    @classmethod
+    def from_array(cls, comp: np.ndarray) -> "DERComponents":
+        """float64 (T, 5) in dg_sweep_score's order {false alarm, missed detection, confusion, correct, total}"""
+        comp = np.asarray(comp, dtype=np.float64).reshape(-1, 5)
+        return cls(*(comp[:, i].copy() for i in range(5)))
+
+    def as_array(self) -> np.ndarray:
+        return np.stack([self.false_alarm, self.missed_detection, self.confusion, self.correct, self.total], axis=1)
+
+    @property
+    def der(self) -> np.ndarray:
+        """(false alarm + missed detection + confusion) / total per trial, as a fraction; with total = 0: 0 when the
+        numerator is 0, else 1"""
+        num = self.false_alarm + self.missed_detection + self.confusion
+        safe = np.where(self.total > 0, self.total, 1.0)
+        return np.where(self.total > 0, num / safe, np.where(num > 0, 1.0, 0.0))
+
+    def __add__(self, other: "DERComponents") -> "DERComponents":
+        """the components of several files summed per trial (the "TOTAL" row of pyannote's report)"""
+        return DERComponents.from_array(self.as_array() + other.as_array())
 
 
 @dataclass
@@ -262,6 +331,45 @@ class HyperParameterSweep:
         return SweepOutputs(header, self._turns[:n.value].copy(), n.value, out_start, out_res, maps, centers,
                             e0.elapsed_time(e1) / 1e3)
 
+    def sweep_score(self, seg: torch.Tensor, emb: torch.Tensor, fw: FileWindows, params: np.ndarray, ref_rows: np.ndarray,
+                    ref_labels: np.ndarray, num_ref_labels: int, segments: bool = False):
+        """dg_sweep_score over device scores / embeddings of ``fw``'s chunks for params (T, 3) against a reference in
+        ``reference_arrays`` form -> (components (T, 5), device seconds, hypothesis offsets, hypothesis segments).  The last
+        two are device tensors when ``segments`` (int32 (T * max_speakers + 1,) and float64 (n, 2), see the C header), else
+        None."""
+        N, F, K = seg.shape
+        h, nw = self._handle(F, K, emb.shape[2])
+        res = self._seg_resolution(float(fw.starts[0]), F)
+        plan, out_start, out_res = post_plan(np.asarray(fw.starts, dtype=np.float64), res, np.zeros(0), np.zeros(0), nw, F,
+                                             self.config.step, self.config.latency)
+        plan = np.ascontiguousarray(plan)
+        out_start = np.ascontiguousarray(out_start, dtype=np.float64)
+        out_res = np.ascontiguousarray(out_res, dtype=np.float64)
+        params = np.ascontiguousarray(params, dtype=np.float64)
+        rows = np.ascontiguousarray(ref_rows, dtype=np.float64)
+        labels = np.ascontiguousarray(ref_labels, dtype=np.int32)
+        T, M = len(params), int(self.config.max_speakers)
+        comp = np.empty((T, 5), dtype=np.float64)
+        offsets = hseg = None
+        if segments:
+            offsets = torch.empty(T * M + 1, dtype=torch.int32, device=self.device)
+            hseg = torch.empty((T * N * 8, 2), dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream(self.device)
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(st)
+            rc = _lib.lib().dg_sweep_score(h, seg.data_ptr(), emb.data_ptr(), N, params.ctypes.data, T, plan.ctypes.data,
+                                           out_start.ctypes.data, out_res.ctypes.data, -fw.padding[0], PATCH_COLLAR,
+                                           rows.ctypes.data, labels.ctypes.data, len(rows), int(num_ref_labels),
+                                           comp.ctypes.data, _lib.ptr(offsets), _lib.ptr(hseg),
+                                           0 if hseg is None else hseg.shape[0], st.cuda_stream)
+            e1.record(st)
+            _lib.check(rc)
+            e1.synchronize()
+        if segments:
+            hseg = hseg[:int(offsets[-1])]
+        return comp, e0.elapsed_time(e1) / 1e3, offsets, hseg
+
     def _seg_resolution(self, start: float, F: int) -> float:
         # SpeakerDiarization.__call__: waveforms[0].extent.duration / F, the extent of a window of 1 / sample_rate frames
         sr = self.config.sample_rate
@@ -290,3 +398,35 @@ class HyperParameterSweep:
             host += time.perf_counter() - t2
         self.timing = {"network": t1 - t0, "sweep": dev, "assembly": host}
         return out
+
+    def score(self, waveform: np.ndarray, reference: Annotation,
+              trials: Sequence[Mapping[str, float]] = ({},)) -> DERComponents:
+        """1-D float32 waveform at ``config.sample_rate`` and its reference annotation -> the diarization error rate
+        components of every trial's whole-file prediction (the one :meth:`run` returns) against the reference.  One network
+        pass, one ``dg_sweep_score`` per 1024 trials; no annotation is built.  At most 32 reference labels."""
+        params = trial_params(trials, self.config)
+        rows, labels, names = reference_arrays(reference)
+        t0 = time.perf_counter()
+        fw = file_windows(waveform, self.config)
+        seg, emb = self.network_pass(fw)
+        torch.cuda.synchronize(self.device)
+        t1 = time.perf_counter()
+        comps, dev = [], 0.0
+        for i in range(0, len(params), TRIALS_PER_LAUNCH):
+            comp, secs, _, _ = self.sweep_score(seg, emb, fw, params[i:i + TRIALS_PER_LAUNCH], rows, labels, len(names))
+            comps.append(comp)
+            dev += secs
+        self.timing = {"network": t1 - t0, "score": dev}
+        return DERComponents.from_array(np.concatenate(comps))
+
+    def score_files(self, files: Iterable[Tuple[np.ndarray, Annotation]],
+                    trials: Sequence[Mapping[str, float]] = ({},)) -> Tuple[List[DERComponents], DERComponents]:
+        """``files``: (waveform, reference) pairs -> (components per file, their sum).  ``total.der`` per trial is the
+        value the reference's ``Optimizer.objective`` minimises over a dataset (a fraction, not a percentage)."""
+        per_file = [self.score(waveform, reference, trials) for waveform, reference in files]
+        if not per_file:
+            raise ValueError("at least one file is needed")
+        total = per_file[0]
+        for c in per_file[1:]:
+            total = total + c
+        return per_file, total

@@ -216,6 +216,24 @@ int dg_sweep_run(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N,
                  const int32_t* plan_host, int32_t* maps_dev, double* centers_dev, int32_t* header_host, uint32_t* turns_host,
                  int turn_cap_host, int* n_turns, void* stream);
 int dg_sweep_destroy(dg_sweep* h);
+/* ---- dg_sweep_score: the same clustering and post-path as dg_sweep_run, then each trial's diarization error rate components
+ *      against one reference (DiarizationErrorRate(collar=0, skip_overlap=False), the metric of the reference's
+ *      Benchmark.evaluate; definition in DESIGN.md "DER scoring").  The turns never leave the device.
+ *        seg_dev ... plan_host   as dg_sweep_run;
+ *        out_start_host, out_res_host float64 [N]: each chunk's output start and frame resolution (blocks/post.py post_plan),
+ *        shift: added to every turn time (the file's timestamp shift), collar >= 0: the merge collar of the whole-file
+ *        prediction (PredictionAccumulator's, 0.05 s);
+ *        ref_host float64 [S][2] {start, end} with start < end, ref_label_host int32 [S] in [0, R), R <= 32 labels; the rows of
+ *        one label in time order and not overlapping (touching is allowed);
+ *        components_host float64 [T][5] = {false alarm, missed detection, confusion, correct, total} seconds;
+ *        hyp_offsets_dev int32 [T * max_speakers + 1] or NULL: offsets of each (trial, label)'s merged hypothesis segments,
+ *        hyp_segments_dev float64 [hyp_cap][2] or NULL: the segments {start, end}, (trial, label) major, in time order.  When
+ *        they exceed hyp_cap the call fails with DG_EINVAL after writing the components and the offsets.
+ *      Every argument is checked before any launch.  Synchronous (synchronises `stream`). ---- */
+int dg_sweep_score(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, const double* params_host, int T,
+                   const int32_t* plan_host, const double* out_start_host, const double* out_res_host, double shift,
+                   double collar, const double* ref_host, const int32_t* ref_label_host, int S, int R,
+                   double* components_host, int32_t* hyp_offsets_dev, double* hyp_segments_dev, int hyp_cap, void* stream);
 
 /* ---- device-side audio stream: rearrange_audio_stream (reference src/diart/operators.py:44-100) with the ring buffer in
  *      HBM.  The host pushes every sample ONCE (step_samples new samples per chunk instead of chunk_samples: 8.2 MB
