@@ -1705,6 +1705,16 @@ class GatherPool {
   bool stop_ = false;
 };
 
+// a step's outputs: scores [B, F, K], embeddings [B, K, D], speaker maps [B, K], permuted scores [B, F, M]
+struct StepShape {
+  int B = 0, F = 0, K = 0;
+  size_t seg_bytes() const { return (size_t)B * F * K * 4; }
+  size_t emb_bytes(int D) const { return (size_t)B * K * D * 4; }
+  size_t map_bytes() const { return (size_t)B * K * 4; }
+  size_t permuted_bytes(int M) const { return (size_t)B * F * M * 4; }
+};
+struct StepOut { float *seg, *emb; int32_t* map; float* permuted; };   // where a step's outputs are or go; null: not wanted
+
 struct dg_pipeline {
   dg_seg* seg;
   dg_emb* emb;
@@ -1714,14 +1724,14 @@ struct dg_pipeline {
   int hop = 0;          // samples between consecutive windows of a batch (hint, dg_pipeline_set_hop); 0 = unknown
   // Members are destroyed in reverse order: the streams and events (declared last) first, then the pinned staging, then
   // the device buffers and worker threads.
-  DevBuf osp, wav, segd, embd, mapd, permd;
-  DevBuf osp2;
+  DevBuf wav, segd, embd, mapd, permd, osp[2];
   SincPrep prep[2];
-  // pipelining (dg_pipeline_submit* / collect*): up to DG_MAX_INFLIGHT steps outstanding.  Step n uses result / input
-  // slot n % 3 and scratch lane n & 1: two steps compute concurrently (lanes), the third slot lets the host upload the
-  // waveforms of step n+2 while steps n and n+1 are on the device
+  // Every step runs through pipeline_enqueue.  Submitted step n (up to DG_MAX_INFLIGHT outstanding) uses result / input slot
+  // n % 3 and scratch lane n & 1: two steps compute concurrently while the host uploads step n+2.  Synchronous steps use lane
+  // 0 and the caller's buffers or wav / segd / ..., never a slot (collected pointers stay valid), and do not count in next_step.
   DevBuf slot_wav[3], slot_seg[3], slot_emb[3], slot_map[3];
-  int slot_B[3] = {0, 0, 0}, slot_S[3] = {0, 0, 0}, outstanding = 0;
+  StepShape slot_shape[3];
+  int outstanding = 0;
   long long next_step = 0;
   long long ident_merged_upto = 0;      // steps below this index have had their maps relabelled by a merge
   std::unique_ptr<GatherPool> gather;   // worker threads of the host gather (created at the first dg_pipeline_call_host)
@@ -1731,12 +1741,13 @@ struct dg_pipeline {
   Stream st;
   // two-stream overlap inside a step: the segmentation chain (critical path, high priority) and the
   // embedding trunk (independent of it until the pooling weights exist) run concurrently
-  Stream s_seg, s_seg2, s_emb, s_clu, s_h2d, s_d2h;
-  Event e_osp2, e_prep[2], e_start, e_osp, e_emb, e_done;
+  Stream s_seg[2], s_emb, s_clu, s_h2d, s_d2h;
+  Event e_osp[2], e_prep[2], e_start, e_emb, e_done;
   Event e_h2d[3], e_slot_done[3], e_lane_done[2];
   // shared-identity mode inside the pipelined flow: export / merge run on the clustering stream, in order with the clustering
   // of the submitted steps, so the networks of the next steps keep running meanwhile (created at the first export)
   Event e_ident, e_ident_in;
+  StepOut slot_out(int s) const { return {slot_seg[s].as<float>(), slot_emb[s].as<float>(), slot_map[s].as<int32_t>()}; }
 };
 
 extern "C" int dg_pipeline_create(dg_seg* seg, dg_emb* emb, dg_cluster* clu, float gamma, float beta,
@@ -1759,10 +1770,10 @@ extern "C" int dg_pipeline_create(dg_seg* seg, dg_emb* emb, dg_cluster* clu, flo
   DG_CUDA(cudaSetDevice(seg->device));
   int lo = 0, hi = 0;
   DG_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-  if (h->st.create() || h->s_seg.create(hi) || h->s_emb.create(lo) || h->s_clu.create(hi) || h->s_seg2.create(hi) ||
+  if (h->st.create() || h->s_seg[0].create(hi) || h->s_emb.create(lo) || h->s_clu.create(hi) || h->s_seg[1].create(hi) ||
       h->s_h2d.create() || h->s_d2h.create())
     return DG_ECUDA;
-  for (Event* e : {&h->e_start, &h->e_osp, &h->e_emb, &h->e_done, &h->e_osp2, &h->e_prep[0], &h->e_prep[1], &h->e_h2d[0],
+  for (Event* e : {&h->e_start, &h->e_osp[0], &h->e_emb, &h->e_done, &h->e_osp[1], &h->e_prep[0], &h->e_prep[1], &h->e_h2d[0],
                    &h->e_h2d[1], &h->e_h2d[2], &h->e_slot_done[0], &h->e_slot_done[1], &h->e_slot_done[2],
                    &h->e_lane_done[0], &h->e_lane_done[1]})
     if (e->create()) return DG_ECUDA;
@@ -1799,16 +1810,16 @@ static int emb_sm_cap(int device, int B) {
 
 // segmentation chain on s_seg and embedding chain on s_emb, both starting after `start`; on return
 // e_emb (recorded on s_emb) marks seg, osp and emb complete
-static int pipeline_nets(dg_pipeline* h, const float* wav, int B, int S, int F, int K, float* seg, float* emb,
-                         cudaEvent_t start, int lane = 0, int stream_hop = 0) {
+static int pipeline_nets(dg_pipeline* h, const float* wav, int S, const StepShape& sh, float* seg, float* emb,
+                         cudaEvent_t start, int lane, int stream_hop) {
   int rc;
+  const int B = sh.B, F = sh.F, K = sh.K;
   const Geom g = make_geom(S);
   // lane 0 / 1: segmentation stream, scratch set, OSP buffer and event of this step (consecutive pipelined steps
   // alternate, so step i+1's segmentation chain can start while step i's is still in its recurrence)
-  cudaStream_t s_seg = lane ? h->s_seg2 : h->s_seg;
-  DevBuf& osp = lane ? h->osp2 : h->osp;
-  cudaEvent_t e_osp = lane ? h->e_osp2 : h->e_osp;
-  if (osp.ensure((size_t)B * F * K * 4)) return DG_ECUDA;
+  cudaStream_t s_seg = h->s_seg[lane];
+  DevBuf& osp = h->osp[lane];
+  if (osp.ensure(sh.seg_bytes())) return DG_ECUDA;
   DG_CUDA(cudaStreamWaitEvent(s_seg, start, 0));
   DG_CUDA(cudaStreamWaitEvent(h->s_emb, start, 0));
   // another pipeline (or a block-level call) that used these model handles' scratch last: stream-ordered hand-over
@@ -1831,10 +1842,10 @@ static int pipeline_nets(dg_pipeline* h, const float* wav, int B, int S, int F, 
   DG_DIAG(trunk, h->s_emb);
   if ((rc = seg_forward_lane(h->seg, lane, &prep, wav, B, S, seg, s_seg))) return rc;
   if ((rc = dg_osp(seg, B, F, K, h->gamma, h->beta, h->normalize_weights, osp.as<float>(), s_seg))) return rc;
-  DG_CUDA(cudaEventRecord(e_osp, s_seg));
+  DG_CUDA(cudaEventRecord(h->e_osp[lane], s_seg));
   if ((rc = seg_use.end())) return rc;
   DG_DIAG(seg, s_seg);
-  DG_CUDA(cudaStreamWaitEvent(h->s_emb, e_osp, 0));
+  DG_CUDA(cudaStreamWaitEvent(h->s_emb, h->e_osp[lane], 0));
   // a fused TDNN5 needs the pooling weights: it runs here, after the segmentation of this step, with its grid capped like the
   // trunk's (the other lane's recurrence may hold 2 x ceil(B/16) SMs at this point)
   if ((rc = emb_tail(h->emb, B, g, osp.as<float>(), F, K, T, fuse, 1, 1.f, emb, h->s_emb, sm_cap))) return rc;
@@ -1852,29 +1863,57 @@ extern "C" int dg_pipeline_set_hop(dg_pipeline* h, int hop_samples) {
   return DG_OK;
 }
 
-// dg_pipeline_step after its argument checks.  stream_hop > 0: the batch was formed on the device from one dg_stream, whose
-// windows are that many samples apart (the sinc layer takes its stream form without the overlap check)
-static int pipeline_step(dg_pipeline* h, const float* wav, int B, int S, float* seg, float* emb, int32_t* map,
-                         float* permuted, void* stream, int stream_hop) {
-  int rc, F = 0, K = 0;
-  if ((rc = dg_seg_dims(h->seg, S, &F, &K))) return rc;
-  if (h->osp.ensure((size_t)B * F * K * 4)) return DG_ECUDA;
-  // DG_NO_OVERLAP=1 (diagnostic): the networks and the clustering back to back on `stream`, for kernel-alone timings
+// Enqueues one step: networks on scratch lane `lane` after `start`, clustering on s_clu, outputs to `out`.  stream_hop > 0:
+// the batch was cut on the device from one stream, windows that many samples apart (sinc layer in stream form, no overlap
+// check).  slot >= 0: a submitted step in that result slot, marked clustered by e_slot_done[slot]; else by e_done.
+static int pipeline_enqueue(dg_pipeline* h, const float* wav, int S, const StepShape& sh, int lane, cudaEvent_t start,
+                            int stream_hop, const StepOut& out, int slot) {
+  int rc;
+  // the slot's previous occupant (three submits ago) must be fully clustered, and the lane's previous user past its
+  // embeddings, before their buffers are rewritten
+  for (cudaStream_t s : {(cudaStream_t)h->s_seg[lane], (cudaStream_t)h->s_emb}) {
+    if (slot >= 0) DG_CUDA(cudaStreamWaitEvent(s, h->e_slot_done[slot], 0));
+    DG_CUDA(cudaStreamWaitEvent(s, h->e_lane_done[lane], 0));
+  }
+  if ((rc = pipeline_nets(h, wav, S, sh, out.seg, out.emb, start, lane, stream_hop))) return rc;
+  // the lane's scratch (waveform planes, segmentation activations, OSP weights) is free as soon as this step's embeddings
+  // exist -- the clustering reads only the step's outputs -- so the step after next may start before this one is clustered
+  DG_CUDA(cudaEventRecord(h->e_lane_done[lane], h->s_emb));
+  DG_CUDA(cudaStreamWaitEvent(h->s_clu, h->e_emb, 0));
+  if ((rc = dg_cluster_step(h->clu, out.seg, out.emb, sh.B, sh.F, sh.K, out.map, out.permuted, h->s_clu))) return rc;
+  DG_CUDA(cudaEventRecord(slot >= 0 ? h->e_slot_done[slot] : h->e_done, h->s_clu));
+  DG_DIAG(clu, h->s_clu);
+  return DG_OK;
+}
+
+// a synchronous step: lane 0, no slot; `st` waits for its clustering
+static int pipeline_step(dg_pipeline* h, const float* wav, int S, const StepShape& sh, const StepOut& out, cudaStream_t st,
+                         int stream_hop) {
+  int rc;
+  // DG_NO_OVERLAP=1 (diagnostic): the networks and the clustering back to back on `st`, for kernel-alone timings
   static const bool serial = getenv("DG_NO_OVERLAP") && getenv("DG_NO_OVERLAP")[0] == '1';
   if (serial) {
-    if ((rc = dg_seg_forward(h->seg, wav, B, S, seg, stream))) return rc;
-    if ((rc = dg_osp(seg, B, F, K, h->gamma, h->beta, h->normalize_weights, h->osp.as<float>(), stream))) return rc;
-    if ((rc = dg_emb_forward(h->emb, wav, h->osp.as<float>(), B, S, F, K, 1, 1.f, emb, stream))) return rc;
-    return dg_cluster_step(h->clu, seg, emb, B, F, K, map, permuted, stream);
+    if (h->osp[0].ensure(sh.seg_bytes())) return DG_ECUDA;
+    if ((rc = dg_seg_forward(h->seg, wav, sh.B, S, out.seg, st))) return rc;
+    if ((rc = dg_osp(out.seg, sh.B, sh.F, sh.K, h->gamma, h->beta, h->normalize_weights, h->osp[0].as<float>(), st))) return rc;
+    if ((rc = dg_emb_forward(h->emb, wav, h->osp[0].as<float>(), sh.B, S, sh.F, sh.K, 1, 1.f, out.emb, st))) return rc;
+    return dg_cluster_step(h->clu, out.seg, out.emb, sh.B, sh.F, sh.K, out.map, out.permuted, st);
   }
-  cudaStream_t st = (cudaStream_t)stream;
   DG_CUDA(cudaSetDevice(h->seg->device));
   DG_CUDA(cudaEventRecord(h->e_start, st));
-  if ((rc = pipeline_nets(h, wav, B, S, F, K, seg, emb, h->e_start, 0, stream_hop))) return rc;
-  DG_CUDA(cudaStreamWaitEvent(h->s_clu, h->e_emb, 0));
-  if ((rc = dg_cluster_step(h->clu, seg, emb, B, F, K, map, permuted, h->s_clu))) return rc;
-  DG_CUDA(cudaEventRecord(h->e_done, h->s_clu));
+  if ((rc = pipeline_enqueue(h, wav, S, sh, 0, h->e_start, stream_hop, out, -1))) return rc;
   DG_CUDA(cudaStreamWaitEvent(st, h->e_done, 0));
+  return DG_OK;
+}
+
+// `st` waits for `done` (if any), then copies the outputs of a step of shape `sh` from `src` to the non-null members of `dst`
+static int copy_out(const dg_pipeline* h, cudaStream_t st, cudaEvent_t done, const StepShape& sh, const StepOut& src,
+                    const StepOut& dst, cudaMemcpyKind kind) {
+  if (done) DG_CUDA(cudaStreamWaitEvent(st, done, 0));
+  if (dst.seg) DG_CUDA(cudaMemcpyAsync(dst.seg, src.seg, sh.seg_bytes(), kind, st));
+  if (dst.emb) DG_CUDA(cudaMemcpyAsync(dst.emb, src.emb, sh.emb_bytes(h->emb->D), kind, st));
+  if (dst.map) DG_CUDA(cudaMemcpyAsync(dst.map, src.map, sh.map_bytes(), kind, st));
+  if (dst.permuted) DG_CUDA(cudaMemcpyAsync(dst.permuted, src.permuted, sh.permuted_bytes(h->clu->p.M), kind, st));
   return DG_OK;
 }
 
@@ -1888,47 +1927,24 @@ extern "C" int dg_pipeline_step(dg_pipeline* h, const float* wav, int B, int S, 
     set_error("dg_pipeline_step: submitted steps are outstanding; collect them first");
     return DG_EINVAL;
   }
-  return pipeline_step(h, wav, B, S, seg, emb, map, permuted, stream, 0);
+  int rc, F = 0, K = 0;
+  if ((rc = dg_seg_dims(h->seg, S, &F, &K))) return rc;
+  return pipeline_step(h, wav, S, {B, F, K}, {seg, emb, map, permuted}, (cudaStream_t)stream, 0);
 }
 
 // ---- pipelined variants (up to three steps outstanding, two computing): the sequential clustering of step i and the host copies overlap the
 //      networks of step i+1.  Per stream the chunk order is preserved: clustering runs on one stream.
-static int pipeline_slot_prepare(dg_pipeline* h, int slot, int B, int S, int F, int K, bool host_in) {
-  const int D = h->emb->D;
-  if (h->osp.ensure((size_t)B * F * K * 4) || h->slot_seg[slot].ensure((size_t)B * F * K * 4) ||
-      h->slot_emb[slot].ensure((size_t)B * K * D * 4) || h->slot_map[slot].ensure((size_t)B * K * 4) ||
-      (host_in && h->slot_wav[slot].ensure((size_t)B * S * 4)))
-    return DG_ECUDA;
-  return DG_OK;
-}
-
 static const int DG_MAX_INFLIGHT = 3;
 
-static int pipeline_submit_common(dg_pipeline* h, const float* wav_dev, int B, int S, int F, int K, int slot,
-                                  cudaEvent_t start, int stream_hop = 0) {
+// enqueues submitted step next_step (result slot next_step % 3, lane next_step & 1) and books it outstanding
+static int pipeline_submit(dg_pipeline* h, const float* wav, int S, const StepShape& sh, cudaEvent_t start, int stream_hop) {
   int rc;
-  const int lane = (int)(h->next_step & 1);
-  cudaStream_t s_lane = lane ? h->s_seg2 : h->s_seg;
-  // the slot's previous occupant (three submits ago) and the lane's previous user (two submits ago) must be fully
-  // clustered before their buffers are rewritten
-  DG_CUDA(cudaStreamWaitEvent(s_lane, h->e_slot_done[slot], 0));
-  DG_CUDA(cudaStreamWaitEvent(h->s_emb, h->e_slot_done[slot], 0));
-  DG_CUDA(cudaStreamWaitEvent(s_lane, h->e_lane_done[lane], 0));
-  DG_CUDA(cudaStreamWaitEvent(h->s_emb, h->e_lane_done[lane], 0));
-  if ((rc = pipeline_nets(h, wav_dev, B, S, F, K, h->slot_seg[slot].as<float>(), h->slot_emb[slot].as<float>(), start,
-                          lane, stream_hop)))
-    return rc;
-  // the lane's scratch (waveform planes, segmentation activations, OSP weights) is free as soon as this step's embeddings
-  // exist -- the clustering reads only the slot buffers -- so the step after next may start before this one is clustered
-  DG_CUDA(cudaEventRecord(h->e_lane_done[lane], h->s_emb));
-  DG_CUDA(cudaStreamWaitEvent(h->s_clu, h->e_emb, 0));
-  if ((rc = dg_cluster_step(h->clu, h->slot_seg[slot].as<float>(), h->slot_emb[slot].as<float>(), B, F, K,
-                            h->slot_map[slot].as<int32_t>(), nullptr, h->s_clu)))
-    return rc;
-  DG_CUDA(cudaEventRecord(h->e_slot_done[slot], h->s_clu));
-  DG_DIAG(clu, h->s_clu);
-  h->slot_B[slot] = B;
-  h->slot_S[slot] = S;
+  const int slot = (int)(h->next_step % 3);
+  if (h->slot_seg[slot].ensure(sh.seg_bytes()) || h->slot_emb[slot].ensure(sh.emb_bytes(h->emb->D)) ||
+      h->slot_map[slot].ensure(sh.map_bytes()))
+    return DG_ECUDA;
+  if ((rc = pipeline_enqueue(h, wav, S, sh, (int)(h->next_step & 1), start, stream_hop, h->slot_out(slot), slot))) return rc;
+  h->slot_shape[slot] = sh;
   h->next_step++;
   h->outstanding++;
   return DG_OK;
@@ -1946,10 +1962,8 @@ extern "C" int dg_pipeline_submit(dg_pipeline* h, const float* wav_dev, int B, i
   int rc, F = 0, K = 0;
   if ((rc = dg_seg_dims(h->seg, S, &F, &K))) return rc;
   DG_CUDA(cudaSetDevice(h->seg->device));
-  const int slot = (int)(h->next_step % 3);
-  if ((rc = pipeline_slot_prepare(h, slot, B, S, F, K, false))) return rc;
   DG_CUDA(cudaEventRecord(h->e_start, (cudaStream_t)stream));
-  return pipeline_submit_common(h, wav_dev, B, S, F, K, slot, h->e_start);
+  return pipeline_submit(h, wav_dev, S, {B, F, K}, h->e_start, 0);
 }
 
 extern "C" int dg_pipeline_collect(dg_pipeline* h, const float** seg_dev, const float** emb_dev,
@@ -1974,14 +1988,9 @@ extern "C" int dg_pipeline_collect_copy(dg_pipeline* h, float* seg_dev, float* e
     return DG_EINVAL;
   }
   const int slot = (int)((h->next_step - h->outstanding) % 3);
-  int F = 0, K = 0;
-  const int B = h->slot_B[slot], D = h->emb->D;
-  dg_seg_dims(h->seg, h->slot_S[slot], &F, &K);
-  cudaStream_t st = (cudaStream_t)stream;
-  DG_CUDA(cudaStreamWaitEvent(st, h->e_slot_done[slot], 0));
-  if (seg_dev) DG_CUDA(cudaMemcpyAsync(seg_dev, h->slot_seg[slot].p, (size_t)B * F * K * 4, cudaMemcpyDeviceToDevice, st));
-  if (emb_dev) DG_CUDA(cudaMemcpyAsync(emb_dev, h->slot_emb[slot].p, (size_t)B * K * D * 4, cudaMemcpyDeviceToDevice, st));
-  if (map_dev) DG_CUDA(cudaMemcpyAsync(map_dev, h->slot_map[slot].p, (size_t)B * K * 4, cudaMemcpyDeviceToDevice, st));
+  const int rc = copy_out(h, (cudaStream_t)stream, h->e_slot_done[slot], h->slot_shape[slot], h->slot_out(slot),
+                          {seg_dev, emb_dev, map_dev, nullptr}, cudaMemcpyDeviceToDevice);
+  if (rc) return rc;
   h->outstanding--;
   return DG_OK;
 }
@@ -1999,11 +2008,11 @@ extern "C" int dg_pipeline_submit_host(dg_pipeline* h, const float* wav_host, in
   if ((rc = dg_seg_dims(h->seg, S, &F, &K))) return rc;
   DG_CUDA(cudaSetDevice(h->seg->device));
   const int slot = (int)(h->next_step % 3);
-  if ((rc = pipeline_slot_prepare(h, slot, B, S, F, K, true))) return rc;
+  if (h->slot_wav[slot].ensure((size_t)B * S * 4)) return DG_ECUDA;
   DG_CUDA(cudaStreamWaitEvent(h->s_h2d, h->e_slot_done[slot], 0));
   DG_CUDA(cudaMemcpyAsync(h->slot_wav[slot].p, wav_host, (size_t)B * S * 4, cudaMemcpyHostToDevice, h->s_h2d));
   DG_CUDA(cudaEventRecord(h->e_h2d[slot], h->s_h2d));
-  return pipeline_submit_common(h, h->slot_wav[slot].as<float>(), B, S, F, K, slot, h->e_h2d[slot]);
+  return pipeline_submit(h, h->slot_wav[slot].as<float>(), S, {B, F, K}, h->e_h2d[slot], 0);
 }
 
 extern "C" int dg_pipeline_collect_host(dg_pipeline* h, float* seg_host, float* emb_host, int32_t* map_host) {
@@ -2012,16 +2021,9 @@ extern "C" int dg_pipeline_collect_host(dg_pipeline* h, float* seg_host, float* 
     return DG_EINVAL;
   }
   const int slot = (int)((h->next_step - h->outstanding) % 3);
-  int F = 0, K = 0;
-  const int B = h->slot_B[slot], D = h->emb->D;
-  dg_seg_dims(h->seg, h->slot_S[slot], &F, &K);
-  DG_CUDA(cudaStreamWaitEvent(h->s_d2h, h->e_slot_done[slot], 0));
-  if (seg_host)
-    DG_CUDA(cudaMemcpyAsync(seg_host, h->slot_seg[slot].p, (size_t)B * F * K * 4, cudaMemcpyDeviceToHost, h->s_d2h));
-  if (emb_host)
-    DG_CUDA(cudaMemcpyAsync(emb_host, h->slot_emb[slot].p, (size_t)B * K * D * 4, cudaMemcpyDeviceToHost, h->s_d2h));
-  if (map_host)
-    DG_CUDA(cudaMemcpyAsync(map_host, h->slot_map[slot].p, (size_t)B * K * 4, cudaMemcpyDeviceToHost, h->s_d2h));
+  const int rc = copy_out(h, h->s_d2h, h->e_slot_done[slot], h->slot_shape[slot], h->slot_out(slot),
+                          {seg_host, emb_host, map_host, nullptr}, cudaMemcpyDeviceToHost);
+  if (rc) return rc;
   DG_CUDA(cudaStreamSynchronize(h->s_d2h));
   h->outstanding--;
   return DG_OK;
@@ -2033,23 +2035,19 @@ extern "C" int dg_pipeline_step_host(dg_pipeline* h, const float* wav_host, int 
     set_error("dg_pipeline_step_host: bad arguments");
     return DG_EINVAL;
   }
-  int rc, F = 0, K = 0;
-  if ((rc = dg_seg_dims(h->seg, S, &F, &K))) return rc;
-  const int D = h->emb->D, M = h->clu->p.M;
+  int rc;
+  StepShape sh = {B};
+  if ((rc = dg_seg_dims(h->seg, S, &sh.F, &sh.K))) return rc;
   DG_CUDA(cudaSetDevice(h->seg->device));
-  if (h->wav.ensure((size_t)B * S * 4) || h->segd.ensure((size_t)B * F * K * 4) ||
-      h->embd.ensure((size_t)B * K * D * 4) || h->mapd.ensure((size_t)B * K * 4) ||
-      (permuted_host && h->permd.ensure((size_t)B * F * M * 4)))
+  if (h->wav.ensure((size_t)B * S * 4) || h->segd.ensure(sh.seg_bytes()) || h->embd.ensure(sh.emb_bytes(h->emb->D)) ||
+      h->mapd.ensure(sh.map_bytes()) || (permuted_host && h->permd.ensure(sh.permuted_bytes(h->clu->p.M))))
     return DG_ECUDA;
   DG_CUDA(cudaMemcpyAsync(h->wav.p, wav_host, (size_t)B * S * 4, cudaMemcpyHostToDevice, h->st));
-  if ((rc = dg_pipeline_step(h, h->wav.as<float>(), B, S, h->segd.as<float>(), h->embd.as<float>(),
-                             h->mapd.as<int32_t>(), permuted_host ? h->permd.as<float>() : nullptr, h->st)))
+  const StepOut dev = {h->segd.as<float>(), h->embd.as<float>(), h->mapd.as<int32_t>(),
+                       permuted_host ? h->permd.as<float>() : nullptr};
+  if ((rc = dg_pipeline_step(h, h->wav.as<float>(), B, S, dev.seg, dev.emb, dev.map, dev.permuted, h->st))) return rc;
+  if ((rc = copy_out(h, h->st, nullptr, sh, dev, {seg_host, emb_host, map_host, permuted_host}, cudaMemcpyDeviceToHost)))
     return rc;
-  if (seg_host) DG_CUDA(cudaMemcpyAsync(seg_host, h->segd.p, (size_t)B * F * K * 4, cudaMemcpyDeviceToHost, h->st));
-  if (emb_host) DG_CUDA(cudaMemcpyAsync(emb_host, h->embd.p, (size_t)B * K * D * 4, cudaMemcpyDeviceToHost, h->st));
-  if (map_host) DG_CUDA(cudaMemcpyAsync(map_host, h->mapd.p, (size_t)B * K * 4, cudaMemcpyDeviceToHost, h->st));
-  if (permuted_host)
-    DG_CUDA(cudaMemcpyAsync(permuted_host, h->permd.p, (size_t)B * F * M * 4, cudaMemcpyDeviceToHost, h->st));
   DG_CUDA(cudaStreamSynchronize(h->st));
   return DG_OK;
 }
@@ -2809,6 +2807,24 @@ static int pack_stream_rows(dg_pipeline* h, const float* const* rows, int r0, in
   return bad.load() ? 0 : 1;
 }
 
+static bool post_fits(const dg_pipeline* h, const dg_post* post, const StepShape& sh) {
+  return sh.F == post->F && sh.K == post->K && h->clu->p.M == post->M && post->device == h->seg->device;
+}
+
+// end of dg_pipeline_call_host / _call_stream, with the batch's scores and maps in segd / mapd (ordered on h->st): post-path,
+// optional downloads, one synchronise (time stamp in *synced, if given), turn list
+static int call_finish(dg_pipeline* h, dg_post* post, const StepShape& sh, const int32_t* plan_host, int32_t* header_host,
+                       uint32_t* turns_host, int turn_cap_host, int* n_turns, float* seg_host, int32_t* map_host,
+                       std::chrono::steady_clock::time_point* synced) {
+  int rc;
+  const StepOut dev = {h->segd.as<float>(), nullptr, h->mapd.as<int32_t>(), nullptr};
+  if ((rc = post_enqueue(post, dev.seg, dev.map, sh.B, plan_host, h->st))) return rc;
+  if ((rc = copy_out(h, h->st, nullptr, sh, dev, {seg_host, nullptr, map_host, nullptr}, cudaMemcpyDeviceToHost))) return rc;
+  DG_CUDA(cudaStreamSynchronize(h->st));
+  if (synced) *synced = std::chrono::steady_clock::now();
+  return post_finish(post, sh.B, header_host, turns_host, turn_cap_host, n_turns, h->st);
+}
+
 extern "C" int dg_pipeline_call_host(dg_pipeline* h, dg_post* post, const float* const* rows_host, int B, int S,
                                      const int32_t* plan_host, int32_t* header_host, uint32_t* turns_host, int turn_cap_host,
                                      int* n_turns, float* seg_host, int32_t* map_host) {
@@ -2816,14 +2832,13 @@ extern "C" int dg_pipeline_call_host(dg_pipeline* h, dg_post* post, const float*
     set_error("dg_pipeline_call_host: bad arguments");
     return DG_EINVAL;
   }
-  int rc, F = 0, K = 0;
-  if ((rc = dg_seg_dims(h->seg, S, &F, &K))) return rc;
-  if (F != post->F || K != post->K || h->clu->p.M != post->M || post->device != h->seg->device) {
+  int rc;
+  StepShape sh = {B};
+  if ((rc = dg_seg_dims(h->seg, S, &sh.F, &sh.K))) return rc;
+  if (!post_fits(h, post, sh)) {
     set_error("dg_pipeline_call_host: post handle was created for other dimensions");
     return DG_EINVAL;
   }
-  const int D = h->emb->D;
-  (void)D;
   if (h->outstanding) {
     set_error("dg_pipeline_call_host: submitted steps are outstanding; collect them first");
     return DG_EINVAL;
@@ -2838,7 +2853,7 @@ extern "C" int dg_pipeline_call_host(dg_pipeline* h, dg_post* post, const float*
     cudaEventRecord(diag.t0, h->s_h2d);
     g_diag = &diag;
   }
-  if (h->segd.ensure((size_t)B * F * K * 4) || h->mapd.ensure((size_t)B * K * 4)) return DG_ECUDA;
+  if (h->segd.ensure(sh.seg_bytes()) || h->mapd.ensure(sh.map_bytes())) return DG_ECUDA;
   if (h->pin_wav.ensure((size_t)B * S * 4)) return DG_ECUDA;
   // The batch runs as up to three sub-batches through the pipelined machinery (dg_pipeline_submit_host): the upload of
   // sub-batch j+1 and its front end overlap the recurrence of sub-batch j; clustering stays in chunk order on its one stream,
@@ -2864,11 +2879,10 @@ extern "C" int dg_pipeline_call_host(dg_pipeline* h, dg_post* post, const float*
   if (as_stream && h->call_stream.ensure((stream_len + 64) * 4)) return DG_ECUDA;
   float* pin = h->pin_wav.as<float>();
   h->call_h2d_bytes = 0;
-  int slots[DG_MAX_INFLIGHT], nbs[DG_MAX_INFLIGHT];
   for (int j = 0, r0 = 0; j < ns; r0 += plan[j], j++) {
     const int nb = plan[j];
     const int slot = (int)(h->next_step % 3);
-    if ((rc = pipeline_slot_prepare(h, slot, nb, S, F, K, true))) return rc;
+    if (h->slot_wav[slot].ensure((size_t)nb * S * 4)) return DG_ECUDA;
     DG_CUDA(cudaStreamWaitEvent(h->s_h2d, h->e_slot_done[slot], 0));
     if (as_stream && !pack_stream_rows(h, rows_host, r0, nb, S, hop, pin)) as_stream = false;
     int stream_hop = 0;
@@ -2891,25 +2905,15 @@ extern "C" int dg_pipeline_call_host(dg_pipeline* h, dg_post* post, const float*
     DG_CUDA(cudaEventRecord(h->e_h2d[slot], h->s_h2d));
     if (g_diag) g_diag->j = j;
     DG_DIAG(up, h->s_h2d);
-    if ((rc = pipeline_submit_common(h, h->slot_wav[slot].as<float>(), nb, S, F, K, slot, h->e_h2d[slot], stream_hop))) return rc;
-    slots[j] = slot;
-    nbs[j] = nb;
+    if ((rc = pipeline_submit(h, h->slot_wav[slot].as<float>(), S, {nb, sh.F, sh.K}, h->e_h2d[slot], stream_hop))) return rc;
   }
-  for (int j = 0, r0 = 0; j < ns; r0 += nbs[j], j++) {     // gather the sub-batches' scores / maps, in order
-    DG_CUDA(cudaStreamWaitEvent(h->st, h->e_slot_done[slots[j]], 0));
-    DG_CUDA(cudaMemcpyAsync(h->segd.as<float>() + (size_t)r0 * F * K, h->slot_seg[slots[j]].p, (size_t)nbs[j] * F * K * 4,
-                            cudaMemcpyDeviceToDevice, h->st));
-    DG_CUDA(cudaMemcpyAsync(h->mapd.as<int32_t>() + (size_t)r0 * K, h->slot_map[slots[j]].p, (size_t)nbs[j] * K * 4,
-                            cudaMemcpyDeviceToDevice, h->st));
-    h->outstanding--;
-  }
+  for (int j = 0, r0 = 0; j < ns; r0 += plan[j], j++)     // collect the sub-batches' scores / maps, in order
+    if ((rc = dg_pipeline_collect_copy(h, h->segd.as<float>() + (size_t)r0 * sh.F * sh.K, nullptr,
+                                       h->mapd.as<int32_t>() + (size_t)r0 * sh.K, h->st)))
+      return rc;
   const auto tc1 = std::chrono::steady_clock::now();
-  if ((rc = post_enqueue(post, h->segd.as<float>(), h->mapd.as<int32_t>(), B, plan_host, h->st))) return rc;
-  if (seg_host) DG_CUDA(cudaMemcpyAsync(seg_host, h->segd.p, (size_t)B * F * K * 4, cudaMemcpyDeviceToHost, h->st));
-  if (map_host) DG_CUDA(cudaMemcpyAsync(map_host, h->mapd.p, (size_t)B * K * 4, cudaMemcpyDeviceToHost, h->st));
-  DG_CUDA(cudaStreamSynchronize(h->st));
-  const auto tc2 = std::chrono::steady_clock::now();
-  rc = post_finish(post, B, header_host, turns_host, turn_cap_host, n_turns, h->st);
+  auto tc2 = tc1;
+  rc = call_finish(h, post, sh, plan_host, header_host, turns_host, turn_cap_host, n_turns, seg_host, map_host, &tc2);
   g_diag = nullptr;
   if (call_timing) {
     static int shown = 0;
@@ -2919,7 +2923,7 @@ extern "C" int dg_pipeline_call_host(dg_pipeline* h, dg_post* post, const float*
         cudaEvent_t ev[6] = {diag.up[j], diag.prep[j], diag.trunk[j], diag.seg[j], diag.emb[j], diag.clu[j]};
         for (int q = 0; q < 6; q++) cudaEventElapsedTime(&t[q], diag.t0, ev[q]);
         fprintf(stderr, "  sub-batch %d (%d windows), ms after entry: uploaded %.2f | front end %.2f | embedding trunk %.2f | segmentation + "
-                        "OSP %.2f | embeddings %.2f | clustered %.2f\n", j, nbs[j], t[0], t[1], t[2], t[3], t[4], t[5]);
+                        "OSP %.2f | embeddings %.2f | clustered %.2f\n", j, plan[j], t[0], t[1], t[2], t[3], t[4], t[5]);
       }
     }
     static double acc[3] = {0, 0, 0};
@@ -2975,10 +2979,8 @@ extern "C" int dg_pipeline_identity_merge(dg_pipeline* h, const double* records_
   bool merged = false;
   for (long long step = first; step < h->next_step; step++) {
     const int slot = (int)(step % 3);
-    int F = 0, K = 0;
-    dg_seg_dims(h->seg, h->slot_S[slot], &F, &K);
     int32_t* maps = h->slot_map[slot].as<int32_t>();
-    const int n = h->slot_B[slot] * K;
+    const int n = h->slot_shape[slot].B * h->slot_shape[slot].K;
     if (!merged) {
       if ((rc = dg_cluster_merge(h->clu, records_dev, world, rank, maps, n, h->s_clu))) return rc;
       merged = true;
@@ -3012,12 +3014,12 @@ extern "C" int dg_pipeline_submit_stream(dg_pipeline* h, dg_stream* s, int B) {
   if ((rc = dg_seg_dims(h->seg, S, &F, &K))) return rc;
   DG_CUDA(cudaSetDevice(h->seg->device));
   const int slot = (int)(h->next_step % 3);
-  if ((rc = pipeline_slot_prepare(h, slot, B, S, F, K, true))) return rc;
+  if (h->slot_wav[slot].ensure((size_t)B * S * 4)) return DG_ECUDA;
   DG_CUDA(cudaStreamWaitEvent(h->s_h2d, h->e_slot_done[slot], 0));
   if ((rc = stream_expand(s, B, h->slot_wav[slot].as<float>(), h->s_h2d))) return rc;
   DG_CUDA(cudaEventRecord(h->e_h2d[slot], h->s_h2d));
   // resampled windows differ from exact hops of one stream at their edges: no stream-form claim for them
-  return pipeline_submit_common(h, h->slot_wav[slot].as<float>(), B, S, F, K, slot, h->e_h2d[slot], s->rs ? 0 : s->hop);
+  return pipeline_submit(h, h->slot_wav[slot].as<float>(), S, {B, F, K}, h->e_h2d[slot], s->rs ? 0 : s->hop);
 }
 
 // SpeakerDiarization.__call__ for the next B windows of a device-side stream: fused step + post-path, synchronous
@@ -3032,27 +3034,22 @@ extern "C" int dg_pipeline_call_stream(dg_pipeline* h, dg_post* post, dg_stream*
     set_error("dg_pipeline_call_stream: submitted steps are outstanding; collect them first");
     return DG_EINVAL;
   }
-  int rc, F = 0, K = 0;
+  int rc;
   const int S = stream_window_len(s);
-  if ((rc = dg_seg_dims(h->seg, S, &F, &K))) return rc;
-  if (F != post->F || K != post->K || h->clu->p.M != post->M || post->device != h->seg->device || s->device != h->seg->device) {
+  StepShape sh = {B};
+  if ((rc = dg_seg_dims(h->seg, S, &sh.F, &sh.K))) return rc;
+  if (!post_fits(h, post, sh) || s->device != h->seg->device) {
     set_error("dg_pipeline_call_stream: handles were created for other dimensions / devices");
     return DG_EINVAL;
   }
-  const int D = h->emb->D;
   DG_CUDA(cudaSetDevice(h->seg->device));
-  if (h->wav.ensure((size_t)B * S * 4) || h->segd.ensure((size_t)B * F * K * 4) || h->embd.ensure((size_t)B * K * D * 4) ||
-      h->mapd.ensure((size_t)B * K * 4))
+  if (h->wav.ensure((size_t)B * S * 4) || h->segd.ensure(sh.seg_bytes()) || h->embd.ensure(sh.emb_bytes(h->emb->D)) ||
+      h->mapd.ensure(sh.map_bytes()))
     return DG_ECUDA;
   if ((rc = stream_expand(s, B, h->wav.as<float>(), h->st))) return rc;
-  if ((rc = pipeline_step(h, h->wav.as<float>(), B, S, h->segd.as<float>(), h->embd.as<float>(), h->mapd.as<int32_t>(),
-                          nullptr, h->st, s->rs ? 0 : s->hop)))
-    return rc;
-  if ((rc = post_enqueue(post, h->segd.as<float>(), h->mapd.as<int32_t>(), B, plan_host, h->st))) return rc;
-  if (seg_host) DG_CUDA(cudaMemcpyAsync(seg_host, h->segd.p, (size_t)B * F * K * 4, cudaMemcpyDeviceToHost, h->st));
-  if (map_host) DG_CUDA(cudaMemcpyAsync(map_host, h->mapd.p, (size_t)B * K * 4, cudaMemcpyDeviceToHost, h->st));
-  DG_CUDA(cudaStreamSynchronize(h->st));
-  return post_finish(post, B, header_host, turns_host, turn_cap_host, n_turns, h->st);
+  const StepOut dev = {h->segd.as<float>(), h->embd.as<float>(), h->mapd.as<int32_t>(), nullptr};
+  if ((rc = pipeline_step(h, h->wav.as<float>(), S, sh, dev, h->st, s->rs ? 0 : s->hop))) return rc;
+  return call_finish(h, post, sh, plan_host, header_host, turns_host, turn_cap_host, n_turns, seg_host, map_host, nullptr);
 }
 
 extern "C" int dg_pipeline_destroy(dg_pipeline* h) {
