@@ -173,13 +173,32 @@ extern "C" int dg_sweep_destroy(dg_sweep* h) {
   return DG_OK;
 }
 
-// the argument checks dg_sweep_run and dg_sweep_score share (before any launch)
-static int sweep_check(const char* who, dg_sweep* h, const float* seg_dev, const float* emb_dev, int N,
-                       const double* params_host, int T, const int32_t* plan_host) {
-  if (!h || !seg_dev || !emb_dev || !params_host || !plan_host || N < 1 || T < 1 || T > 65535) {
-    set_error(std::string(who) + ": bad arguments (need N >= 1, 1 <= T <= 65535, non-null buffers)");
+// at most this many (file, trial) states per call: der_hyp runs one warp per (state, label) with up to 32 labels and
+// numbers its threads in int32
+static const long long DG_SWEEP_MAX_STATES = 1LL << 21;
+
+// the argument checks dg_sweep_run(_files) and dg_sweep_score(_files) share (before any launch); chunk_off [nf + 1] splits
+// the N chunks into the files' ranges
+static int sweep_check(const char* who, dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int nf,
+                       const int32_t* chunk_off, const double* params_host, int T, const int32_t* plan_host) {
+  if (!h || !seg_dev || !emb_dev || !params_host || !plan_host || N < 1 || T < 1 || T > 65535 || nf < 1 || !chunk_off) {
+    set_error(std::string(who) + ": bad arguments (need N >= 1, 1 <= T <= 65535, num_files >= 1, non-null buffers)");
     return DG_EINVAL;
   }
+  if ((long long)nf * T > DG_SWEEP_MAX_STATES) {
+    set_error(std::string(who) + ": " + std::to_string((long long)nf * T) + " (file, trial) states; at most " +
+              std::to_string(DG_SWEEP_MAX_STATES) + " per call");
+    return DG_EINVAL;
+  }
+  if (chunk_off[0] != 0 || chunk_off[nf] != N) {
+    set_error(std::string(who) + ": chunk offsets must start at 0 and end at N");
+    return DG_EINVAL;
+  }
+  for (int f = 0; f < nf; f++)
+    if (chunk_off[f + 1] <= chunk_off[f]) {
+      set_error(std::string(who) + ": file " + std::to_string(f) + " has no chunks (offsets must increase)");
+      return DG_EINVAL;
+    }
   for (int i = 0; i < 3 * T; i++)
     if (!std::isfinite(params_host[i])) {
       set_error(std::string(who) + ": trial " + std::to_string(i / 3) + " has a parameter that is not finite");
@@ -188,24 +207,53 @@ static int sweep_check(const char* who, dg_sweep* h, const float* seg_dev, const
   return DG_OK;
 }
 
-// pinned output layout of sweep_cluster_post: error flags [T][2], then header [T][N][4], turn count, turn prefix
-static TurnOut sweep_out(int T, int N) { return {(size_t)T * 8, (size_t)T * N * 16}; }
+// The launch order of the nf * T (file, trial) states, states [nf * T][2] = {file, trial}: longest file first (equal lengths
+// in file order), then trial.  A state's time is its file's chunk count; when the states outnumber the resident CTAs, the
+// long ones start in the first wave and the last wave holds short ones.
+static void sweep_state_order(int nf, const int32_t* chunk_off, int T, int32_t* states) {
+  std::vector<int> order(nf);
+  for (int f = 0; f < nf; f++) order[f] = f;
+  std::stable_sort(order.begin(), order.end(),
+                   [&](int a, int b) { return chunk_off[a + 1] - chunk_off[a] > chunk_off[b + 1] - chunk_off[b]; });
+  size_t i = 0;
+  for (int f : order)
+    for (int t = 0; t < T; t++, i++) {
+      states[2 * i] = f;
+      states[2 * i + 1] = t;
+    }
+}
 
-// Clustering + post-path of T trials over the N chunks: header [T][N][4] and turns stay on the device (h->header, h->turns),
-// the turn count comes back in *total.  with_header: the header and a prefix of the turns travel to the pinned buffer in the
-// same copy as the count (sweep_out layout).  Synchronises `st`.
-static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, const double* params_host,
-                              int T, const int32_t* plan_host, int32_t* maps_dev, double* centers_dev, bool with_header,
-                              cudaStream_t st, unsigned int* total_out) {
-  const int stride = 4 + h->nw, M = h->M, D = h->D, K = h->K, F = h->F;
-  // host -> device: params [T][3], taus [T], plan [N][stride], one copy
-  const size_t params_b = (size_t)T * 24, taus_b = (size_t)T * 8, plan_b = (size_t)N * stride * 4;
-  const size_t in_b = params_b + taus_b + plan_b;
-  const TurnOut lay = sweep_out(T, N);
+extern "C" int dg_sweep_state_order(int num_files, const int32_t* chunk_offsets_host, int T, int32_t* states_host) {
+  if (num_files < 1 || T < 1 || !chunk_offsets_host || !states_host) {
+    set_error("dg_sweep_state_order: bad arguments (need num_files >= 1, T >= 1, non-null buffers)");
+    return DG_EINVAL;
+  }
+  sweep_state_order(num_files, chunk_offsets_host, T, states_host);
+  return DG_OK;
+}
+
+// pinned output layout of sweep_cluster_post over S states: error flags [S][2], then header [T][N][4], turn count, turn prefix
+static TurnOut sweep_out(int S, int T, int N) { return {(size_t)S * 8, (size_t)T * N * 16}; }
+
+// Clustering + post-path of T trials over the nf files whose chunks [chunk_off[f], chunk_off[f + 1]) make up the N chunks:
+// header [T][N][4] and turns stay on the device (h->header, h->turns), the turn count comes back in *total.  with_header: the
+// header and a prefix of the turns travel to the pinned buffer in the same copy as the count (sweep_out layout).  The plan
+// is the files' plans, each that of a fresh stream, concatenated: a chunk's aggregated buffers are the nw - 1 chunks before
+// it at most, never those of the previous file (post.cu: chunk c reads chunks c - (nb - 1) .. c, nb <= its index in its file
+// + 1), so the post-path runs over all N chunks at once.  Synchronises `st`.
+static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int nf, const int32_t* chunk_off,
+                              const double* params_host, int T, const int32_t* plan_host, int32_t* maps_dev,
+                              double* centers_dev, bool with_header, cudaStream_t st, unsigned int* total_out) {
+  const int stride = 4 + h->nw, M = h->M, D = h->D, K = h->K, F = h->F, S = nf * T;
+  // host -> device, one copy: params [T][3], taus [T], states [S][2] (launch order), plan [N][stride], chunk offsets [nf + 1]
+  const size_t params_b = (size_t)T * 24, taus_b = (size_t)T * 8, states_b = (size_t)S * 8, plan_b = (size_t)N * stride * 4;
+  const size_t off_b = (size_t)(nf + 1) * 4;
+  const size_t in_b = params_b + taus_b + states_b + plan_b + off_b;
+  const TurnOut lay = sweep_out(S, T, N);
   const size_t init_b = lay.at, header_b = lay.header_bytes;
   // the device turn buffer starts at a guess and grows to the true count (the kernel counts every turn, writes those that fit)
   const size_t turn_guess = std::max<size_t>((size_t)T * N * 8, (size_t)DG_POST_PREFIX);
-  if (h->in.ensure(in_b) || h->centers.ensure((size_t)T * M * D * 8) || h->active.ensure((size_t)T * 32 * 4) ||
+  if (h->in.ensure(in_b) || h->centers.ensure((size_t)S * M * D * 8) || h->active.ensure((size_t)S * 32 * 4) ||
       h->init.ensure(init_b) || h->prep.ensure(cluster_prep_floats(N, K) * 4 + 16) ||
       h->prep_d.ensure(cluster_prep_doubles(N, K) * 8 + 16) || (!maps_dev && h->maps.ensure((size_t)T * N * K * 4)) ||
       h->header.ensure(header_b) || h->turns.ensure(turn_guess * 4) || h->pin.ensure(std::max(in_b, lay.end())))
@@ -214,27 +262,32 @@ static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* em
   double* p_taus = reinterpret_cast<double*>(pin + params_b);
   memcpy(pin, params_host, params_b);
   for (int t = 0; t < T; t++) p_taus[t] = params_host[3 * t];
-  memcpy(pin + params_b + taus_b, plan_host, plan_b);
+  sweep_state_order(nf, chunk_off, T, reinterpret_cast<int32_t*>(pin + params_b + taus_b));
+  memcpy(pin + params_b + taus_b + states_b, plan_host, plan_b);
+  memcpy(pin + params_b + taus_b + states_b + plan_b, chunk_off, off_b);
   unsigned char* din = h->in.as<unsigned char>();
   DG_CUDA(cudaMemcpyAsync(din, pin, in_b, cudaMemcpyHostToDevice, st));
   const double* d_params = reinterpret_cast<const double*>(din);
   const double* d_taus = reinterpret_cast<const double*>(din + params_b);
-  const int32_t* d_plan = reinterpret_cast<const int32_t*>(din + params_b + taus_b);
+  const int2* d_states = reinterpret_cast<const int2*>(din + params_b + taus_b);
+  const int32_t* d_plan = reinterpret_cast<const int32_t*>(din + params_b + taus_b + states_b);
+  const int* d_off = reinterpret_cast<const int*>(din + params_b + taus_b + states_b + plan_b);
   int32_t* maps = maps_dev ? maps_dev : h->maps.as<int32_t>();
-  // every state starts empty (reference: a new OnlineSpeakerClustering per trial)
-  DG_CUDA(cudaMemsetAsync(h->centers.p, 0, (size_t)T * M * D * 8, st));
-  DG_CUDA(cudaMemsetAsync(h->active.p, 0, (size_t)T * 32 * 4, st));
+  // every state starts empty (reference: a new OnlineSpeakerClustering per trial and file)
+  DG_CUDA(cudaMemsetAsync(h->centers.p, 0, (size_t)S * M * D * 8, st));
+  DG_CUDA(cudaMemsetAsync(h->active.p, 0, (size_t)S * 32 * 4, st));
   DG_CUDA(cudaMemsetAsync(h->init.p, 0, init_b, st));
   ClusterParams p{};
   p.M = M;
   p.D = D;
   p.metric = 0;
   int rc;
-  if ((rc = launch_cluster_sweep(p, d_params, T, seg_dev, emb_dev, N, F, K, h->centers.as<double>(), h->active.as<int>(),
-                                 h->init.as<int>(), h->prep.as<float>(), h->prep_d.as<double>(), maps, st)))
+  if ((rc = launch_cluster_sweep(p, d_params, T, d_states, S, d_off, seg_dev, emb_dev, N, F, K, h->centers.as<double>(),
+                                 h->active.as<int>(), h->init.as<int>(), h->prep.as<float>(), h->prep_d.as<double>(), maps,
+                                 st)))
     return rc;
   if (centers_dev)
-    DG_CUDA(cudaMemcpyAsync(centers_dev, h->centers.p, (size_t)T * M * D * 8, cudaMemcpyDeviceToDevice, st));
+    DG_CUDA(cudaMemcpyAsync(centers_dev, h->centers.p, (size_t)S * M * D * 8, cudaMemcpyDeviceToDevice, st));
   unsigned int total = 0;
   for (int attempt = 0; attempt < 2; attempt++) {
     const int cap = (int)std::min<size_t>(h->turns.bytes / 4, (size_t)INT32_MAX);
@@ -255,8 +308,8 @@ static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* em
     if (h->turns.ensure((size_t)total * 4)) return DG_ECUDA;
   }
   const int32_t* flags = reinterpret_cast<const int32_t*>(pin);
-  for (int t = 0; t < T; t++)
-    if (flags[2 * t + 1]) {
+  for (int s = 0; s < S; s++)
+    if (flags[2 * s + 1]) {
       set_error("Cannot update unknown centers");   // reference clustering.py:98 (AssertionError)
       return DG_EINVAL;
     }
@@ -264,28 +317,46 @@ static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* em
   return DG_OK;
 }
 
-extern "C" int dg_sweep_run(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, const double* params_host, int T,
-                            const int32_t* plan_host, int32_t* maps_dev, double* centers_dev, int32_t* header_host,
-                            uint32_t* turns_host, int turn_cap_host, int* n_turns, void* stream) {
+static int sweep_run(const char* who, dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int nf,
+                     const int32_t* chunk_off, const double* params_host, int T, const int32_t* plan_host, int32_t* maps_dev,
+                     double* centers_dev, int32_t* header_host, uint32_t* turns_host, int turn_cap_host, int* n_turns,
+                     void* stream) {
   if (!header_host || !turns_host) {
-    set_error("dg_sweep_run: bad arguments (need N >= 1, 1 <= T <= 65535, non-null buffers)");
+    set_error(std::string(who) + ": bad arguments (need N >= 1, 1 <= T <= 65535, non-null buffers)");
     return DG_EINVAL;
   }
   int rc;
-  if ((rc = sweep_check("dg_sweep_run", h, seg_dev, emb_dev, N, params_host, T, plan_host))) return rc;
+  if ((rc = sweep_check(who, h, seg_dev, emb_dev, N, nf, chunk_off, params_host, T, plan_host))) return rc;
   DG_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)stream;
   unsigned int total = 0;
-  if ((rc = sweep_cluster_post(h, seg_dev, emb_dev, N, params_host, T, plan_host, maps_dev, centers_dev, true, st, &total)))
+  if ((rc = sweep_cluster_post(h, seg_dev, emb_dev, N, nf, chunk_off, params_host, T, plan_host, maps_dev, centers_dev, true,
+                               st, &total)))
     return rc;
-  return download_turns("dg_sweep_run", h->pin.as<unsigned char>(), sweep_out(T, N), h->turns.as<uint32_t>(), header_host,
+  return download_turns(who, h->pin.as<unsigned char>(), sweep_out(nf * T, T, N), h->turns.as<uint32_t>(), header_host,
                         turns_host, turn_cap_host, n_turns, st);
 }
 
-// the reference rows: finite, start < end, labels in [0, R), each label's rows in time order without overlap
-static int sweep_check_reference(const double* ref_host, const int32_t* ref_label_host, int S, int R) {
+extern "C" int dg_sweep_run(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, const double* params_host, int T,
+                            const int32_t* plan_host, int32_t* maps_dev, double* centers_dev, int32_t* header_host,
+                            uint32_t* turns_host, int turn_cap_host, int* n_turns, void* stream) {
+  const int32_t off[2] = {0, N};
+  return sweep_run("dg_sweep_run", h, seg_dev, emb_dev, N, 1, off, params_host, T, plan_host, maps_dev, centers_dev,
+                   header_host, turns_host, turn_cap_host, n_turns, stream);
+}
+
+extern "C" int dg_sweep_run_files(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int num_files,
+                                  const int32_t* chunk_offsets_host, const double* params_host, int T,
+                                  const int32_t* plan_host, int32_t* maps_dev, double* centers_dev, int32_t* header_host,
+                                  uint32_t* turns_host, int turn_cap_host, int* n_turns, void* stream) {
+  return sweep_run("dg_sweep_run_files", h, seg_dev, emb_dev, N, num_files, chunk_offsets_host, params_host, T, plan_host,
+                   maps_dev, centers_dev, header_host, turns_host, turn_cap_host, n_turns, stream);
+}
+
+// the reference rows of one file: finite, start < end, labels in [0, R), each label's rows in time order without overlap
+static int sweep_check_reference(const char* who, const double* ref_host, const int32_t* ref_label_host, int S, int R) {
   if (R < 0 || R > 32 || S < 0 || (S > 0 && (!ref_host || !ref_label_host))) {
-    set_error("dg_sweep_score: need 0 <= reference labels <= 32, rows >= 0, non-null reference arrays");
+    set_error(std::string(who) + ": need 0 <= reference labels <= 32, rows >= 0, non-null reference arrays");
     return DG_EINVAL;
   }
   double last[32];
@@ -294,18 +365,131 @@ static int sweep_check_reference(const double* ref_host, const int32_t* ref_labe
     const double a = ref_host[2 * i], b = ref_host[2 * i + 1];
     const int r = ref_label_host[i];
     if (r < 0 || r >= R) {
-      set_error("dg_sweep_score: reference row " + std::to_string(i) + " has a label outside [0, R)");
+      set_error(std::string(who) + ": reference row " + std::to_string(i) + " has a label outside [0, R)");
       return DG_EINVAL;
     }
     if (!std::isfinite(a) || !std::isfinite(b) || !(a < b)) {
-      set_error("dg_sweep_score: reference row " + std::to_string(i) + " is not finite, empty or reversed");
+      set_error(std::string(who) + ": reference row " + std::to_string(i) + " is not finite, empty or reversed");
       return DG_EINVAL;
     }
     if (a < last[r]) {
-      set_error("dg_sweep_score: reference row " + std::to_string(i) + " is out of order or overlaps an earlier row of its label");
+      set_error(std::string(who) + ": reference row " + std::to_string(i) +
+                " is out of order or overlaps an earlier row of its label");
       return DG_EINVAL;
     }
     last[r] = b;
+  }
+  return DG_OK;
+}
+
+// dg_sweep_score(_files): the clustering and post-path of sweep_cluster_post, then the DER components of every (file, trial)
+// against the file's reference rows [ref_off[f], ref_off[f + 1]) with R[f] labels
+static int sweep_score(const char* who, dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int nf,
+                       const int32_t* chunk_off, const double* params_host, int T, const int32_t* plan_host,
+                       const double* out_start_host, const double* out_res_host, const double* shift_host, double collar,
+                       const double* ref_host, const int32_t* ref_label_host, const int32_t* ref_off, const int32_t* R_host,
+                       double* components_host, int32_t* hyp_offsets_dev, double* hyp_segments_dev, int hyp_cap,
+                       void* stream) {
+  int rc;
+  if ((rc = sweep_check(who, h, seg_dev, emb_dev, N, nf, chunk_off, params_host, T, plan_host))) return rc;
+  if (!out_start_host || !out_res_host || !components_host || hyp_cap < 0 || !shift_host || !std::isfinite(collar) ||
+      collar < 0) {
+    set_error(std::string(who) + ": bad arguments (need chunk times, a components buffer, finite shift, finite collar >= 0, "
+              "hyp_cap >= 0)");
+    return DG_EINVAL;
+  }
+  for (int f = 0; f < nf; f++)
+    if (!std::isfinite(shift_host[f])) {
+      set_error(std::string(who) + ": the shift of file " + std::to_string(f) + " is not finite");
+      return DG_EINVAL;
+    }
+  for (int c = 0; c < N; c++)
+    if (!std::isfinite(out_start_host[c]) || !std::isfinite(out_res_host[c])) {
+      set_error(std::string(who) + ": chunk " + std::to_string(c) + " has an output time that is not finite");
+      return DG_EINVAL;
+    }
+  if (!ref_off || !R_host || ref_off[0] != 0) {
+    set_error(std::string(who) + ": need reference row offsets starting at 0 and label counts");
+    return DG_EINVAL;
+  }
+  for (int f = 0; f < nf; f++)
+    if (ref_off[f + 1] < ref_off[f]) {
+      set_error(std::string(who) + ": rows >= 0 (reference row offsets of file " + std::to_string(f) + " decrease)");
+      return DG_EINVAL;
+    }
+  const int S = ref_off[nf];
+  if (S > 0 && (!ref_host || !ref_label_host)) {
+    set_error(std::string(who) + ": non-null reference arrays needed for " + std::to_string(S) + " rows");
+    return DG_EINVAL;
+  }
+  for (int f = 0; f < nf; f++)
+    if ((rc = sweep_check_reference(who, S > 0 ? ref_host + 2 * (size_t)ref_off[f] : nullptr,
+                                    S > 0 ? ref_label_host + ref_off[f] : nullptr, ref_off[f + 1] - ref_off[f], R_host[f])))
+      return rc;
+  DG_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned int total = 0;
+  if ((rc = sweep_cluster_post(h, seg_dev, emb_dev, N, nf, chunk_off, params_host, T, plan_host, nullptr, nullptr, false, st,
+                               &total)))
+    return rc;
+  const int M = h->M, NTM = nf * T * M;
+  // host -> device, one copy: out_start [N], out_res [N], shifts [nf], reference segments [S][2] grouped by label within each
+  // file, label offsets [nf][DER_ROFF], label counts [nf], chunk offsets [nf + 1]
+  const size_t times_b = (size_t)N * 16, shift_b = (size_t)nf * 8, rseg_b = (size_t)S * 16;
+  const size_t roff_b = (size_t)nf * DER_ROFF * 4, R_b = (size_t)nf * 4, off_b = (size_t)(nf + 1) * 4;
+  const size_t in_b = times_b + shift_b + rseg_b + roff_b + R_b + off_b, comp_b = (size_t)nf * T * 40;
+  if (h->score_in.ensure(in_b) || h->hoff.ensure((size_t)(NTM + 1) * 4) || h->hseg.ensure((size_t)std::max(total, 1u) * 16) ||
+      h->comp.ensure(comp_b) || h->pin.ensure(std::max(in_b, comp_b + 16)))
+    return DG_ECUDA;
+  unsigned char* pin = h->pin.as<unsigned char>();
+  memcpy(pin, out_start_host, (size_t)N * 8);
+  memcpy(pin + (size_t)N * 8, out_res_host, (size_t)N * 8);
+  memcpy(pin + times_b, shift_host, shift_b);
+  double* rseg = reinterpret_cast<double*>(pin + times_b + shift_b);
+  int32_t* roff_all = reinterpret_cast<int32_t*>(pin + times_b + shift_b + rseg_b);
+  memcpy(pin + times_b + shift_b + rseg_b + roff_b, R_host, R_b);
+  memcpy(pin + times_b + shift_b + rseg_b + roff_b + R_b, chunk_off, off_b);
+  for (int f = 0; f < nf; f++) {
+    const int a = ref_off[f], n = ref_off[f + 1] - a, R = R_host[f];
+    int32_t* roff = roff_all + (size_t)f * DER_ROFF;
+    for (int r = 0; r < DER_ROFF; r++) roff[r] = 0;
+    for (int i = 0; i < n; i++) roff[ref_label_host[a + i] + 1]++;
+    roff[0] = a;
+    for (int r = 0; r < R; r++) roff[r + 1] += roff[r];
+    int fill[32];
+    for (int r = 0; r < R; r++) fill[r] = roff[r];
+    for (int i = 0; i < n; i++) {     // stable: each label keeps its rows' order
+      const int o = fill[ref_label_host[a + i]]++;
+      rseg[2 * (size_t)o] = ref_host[2 * (size_t)(a + i)];
+      rseg[2 * (size_t)o + 1] = ref_host[2 * (size_t)(a + i) + 1];
+    }
+  }
+  unsigned char* din = h->score_in.as<unsigned char>();
+  DG_CUDA(cudaMemcpyAsync(din, pin, in_b, cudaMemcpyHostToDevice, st));
+  const double* d_start = reinterpret_cast<const double*>(din);
+  const double* d_res = d_start + N;
+  const double* d_shift = reinterpret_cast<const double*>(din + times_b);
+  const double* d_rseg = reinterpret_cast<const double*>(din + times_b + shift_b);
+  const int* d_roff = reinterpret_cast<const int*>(din + times_b + shift_b + rseg_b);
+  const int* d_R = reinterpret_cast<const int*>(din + times_b + shift_b + rseg_b + roff_b);
+  const int* d_off = reinterpret_cast<const int*>(din + times_b + shift_b + rseg_b + roff_b + R_b);
+  int* hoff = h->hoff.as<int>();
+  if ((rc = launch_der_hyp_count(h->header.as<int32_t>(), h->turns.as<uint32_t>(), nf, d_off, T, N, M, d_start, d_res, d_shift,
+                                 collar, hoff, st)) ||
+      (rc = launch_der_hyp_write(h->header.as<int32_t>(), h->turns.as<uint32_t>(), nf, d_off, T, N, M, d_start, d_res, d_shift,
+                                 collar, hoff, h->hseg.as<double>(), hyp_segments_dev, hyp_cap, st)) ||
+      (rc = launch_der_score(hoff, h->hseg.as<double>(), nf, T, M, d_roff, d_R, d_rseg, h->comp.as<double>(), st)))
+    return rc;
+  if (hyp_offsets_dev) DG_CUDA(cudaMemcpyAsync(hyp_offsets_dev, hoff, (size_t)(NTM + 1) * 4, cudaMemcpyDeviceToDevice, st));
+  DG_CUDA(cudaMemcpyAsync(pin, h->comp.p, comp_b, cudaMemcpyDeviceToHost, st));
+  DG_CUDA(cudaMemcpyAsync(pin + comp_b, hoff + NTM, 4, cudaMemcpyDeviceToHost, st));
+  DG_CUDA(cudaStreamSynchronize(st));
+  memcpy(components_host, pin, comp_b);
+  int n_seg = 0;
+  memcpy(&n_seg, pin + comp_b, 4);
+  if (hyp_segments_dev && n_seg > hyp_cap) {
+    set_error(std::string(who) + ": hypothesis segment buffer too small (" + std::to_string(n_seg) + " segments)");
+    return DG_EINVAL;
   }
   return DG_OK;
 }
@@ -315,70 +499,20 @@ extern "C" int dg_sweep_score(dg_sweep* h, const float* seg_dev, const float* em
                               double shift, double collar, const double* ref_host, const int32_t* ref_label_host, int S,
                               int R, double* components_host, int32_t* hyp_offsets_dev, double* hyp_segments_dev,
                               int hyp_cap, void* stream) {
-  int rc;
-  if ((rc = sweep_check("dg_sweep_score", h, seg_dev, emb_dev, N, params_host, T, plan_host))) return rc;
-  if (!out_start_host || !out_res_host || !components_host || hyp_cap < 0 || !std::isfinite(shift) ||
-      !std::isfinite(collar) || collar < 0) {
-    set_error("dg_sweep_score: bad arguments (need chunk times, a components buffer, finite shift, finite collar >= 0, "
-              "hyp_cap >= 0)");
-    return DG_EINVAL;
-  }
-  for (int c = 0; c < N; c++)
-    if (!std::isfinite(out_start_host[c]) || !std::isfinite(out_res_host[c])) {
-      set_error("dg_sweep_score: chunk " + std::to_string(c) + " has an output time that is not finite");
-      return DG_EINVAL;
-    }
-  if ((rc = sweep_check_reference(ref_host, ref_label_host, S, R))) return rc;
-  DG_CUDA(cudaSetDevice(h->device));
-  cudaStream_t st = (cudaStream_t)stream;
-  unsigned int total = 0;
-  if ((rc = sweep_cluster_post(h, seg_dev, emb_dev, N, params_host, T, plan_host, nullptr, nullptr, false, st, &total)))
-    return rc;
-  const int M = h->M, TM = T * M;
-  // host -> device, one copy: out_start [N], out_res [N], reference segments [S][2] grouped by label, label offsets [R + 1]
-  const size_t times_b = (size_t)N * 16, rseg_b = (size_t)S * 16, roff_b = (size_t)(R + 1) * 4;
-  const size_t in_b = times_b + rseg_b + roff_b, comp_b = (size_t)T * 40;
-  if (h->score_in.ensure(in_b) || h->hoff.ensure((size_t)(TM + 1) * 4) || h->hseg.ensure((size_t)std::max(total, 1u) * 16) ||
-      h->comp.ensure(comp_b) || h->pin.ensure(std::max(in_b, comp_b + 16)))
-    return DG_ECUDA;
-  unsigned char* pin = h->pin.as<unsigned char>();
-  memcpy(pin, out_start_host, (size_t)N * 8);
-  memcpy(pin + (size_t)N * 8, out_res_host, (size_t)N * 8);
-  double* rseg = reinterpret_cast<double*>(pin + times_b);
-  int32_t* roff = reinterpret_cast<int32_t*>(pin + times_b + rseg_b);
-  for (int r = 0; r <= R; r++) roff[r] = 0;
-  for (int i = 0; i < S; i++) roff[ref_label_host[i] + 1]++;
-  for (int r = 0; r < R; r++) roff[r + 1] += roff[r];
-  int fill[32];
-  for (int r = 0; r < R; r++) fill[r] = roff[r];
-  for (int i = 0; i < S; i++) {     // stable: each label keeps its rows' order
-    const int o = fill[ref_label_host[i]]++;
-    rseg[2 * o] = ref_host[2 * i];
-    rseg[2 * o + 1] = ref_host[2 * i + 1];
-  }
-  unsigned char* din = h->score_in.as<unsigned char>();
-  DG_CUDA(cudaMemcpyAsync(din, pin, in_b, cudaMemcpyHostToDevice, st));
-  const double* d_start = reinterpret_cast<const double*>(din);
-  const double* d_res = d_start + N;
-  const double* d_rseg = reinterpret_cast<const double*>(din + times_b);
-  const int* d_roff = reinterpret_cast<const int*>(din + times_b + rseg_b);
-  int* hoff = h->hoff.as<int>();
-  if ((rc = launch_der_hyp_count(h->header.as<int32_t>(), h->turns.as<uint32_t>(), T, N, M, d_start, d_res, shift, collar,
-                                 hoff, st)) ||
-      (rc = launch_der_hyp_write(h->header.as<int32_t>(), h->turns.as<uint32_t>(), T, N, M, d_start, d_res, shift, collar,
-                                 hoff, h->hseg.as<double>(), hyp_segments_dev, hyp_cap, st)) ||
-      (rc = launch_der_score(hoff, h->hseg.as<double>(), T, M, d_roff, d_rseg, R, h->comp.as<double>(), st)))
-    return rc;
-  if (hyp_offsets_dev) DG_CUDA(cudaMemcpyAsync(hyp_offsets_dev, hoff, (size_t)(TM + 1) * 4, cudaMemcpyDeviceToDevice, st));
-  DG_CUDA(cudaMemcpyAsync(pin, h->comp.p, comp_b, cudaMemcpyDeviceToHost, st));
-  DG_CUDA(cudaMemcpyAsync(pin + comp_b, hoff + TM, 4, cudaMemcpyDeviceToHost, st));
-  DG_CUDA(cudaStreamSynchronize(st));
-  memcpy(components_host, pin, comp_b);
-  int n_seg = 0;
-  memcpy(&n_seg, pin + comp_b, 4);
-  if (hyp_segments_dev && n_seg > hyp_cap) {
-    set_error("dg_sweep_score: hypothesis segment buffer too small (" + std::to_string(n_seg) + " segments)");
-    return DG_EINVAL;
-  }
-  return DG_OK;
+  const int32_t off[2] = {0, N}, ref_off[2] = {0, S};
+  return sweep_score("dg_sweep_score", h, seg_dev, emb_dev, N, 1, off, params_host, T, plan_host, out_start_host,
+                     out_res_host, &shift, collar, ref_host, ref_label_host, ref_off, &R, components_host, hyp_offsets_dev,
+                     hyp_segments_dev, hyp_cap, stream);
+}
+
+extern "C" int dg_sweep_score_files(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int num_files,
+                                    const int32_t* chunk_offsets_host, const double* params_host, int T,
+                                    const int32_t* plan_host, const double* out_start_host, const double* out_res_host,
+                                    const double* shifts_host, double collar, const double* ref_host,
+                                    const int32_t* ref_label_host, const int32_t* ref_offsets_host,
+                                    const int32_t* ref_label_counts_host, double* components_host, int32_t* hyp_offsets_dev,
+                                    double* hyp_segments_dev, int hyp_cap, void* stream) {
+  return sweep_score("dg_sweep_score_files", h, seg_dev, emb_dev, N, num_files, chunk_offsets_host, params_host, T, plan_host,
+                     out_start_host, out_res_host, shifts_host, collar, ref_host, ref_label_host, ref_offsets_host,
+                     ref_label_counts_host, components_host, hyp_offsets_dev, hyp_segments_dev, hyp_cap, stream);
 }

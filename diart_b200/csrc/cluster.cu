@@ -106,14 +106,17 @@ __device__ __forceinline__ void cp_async4(void* smem, const void* gmem) {
 constexpr int SEQ_THREADS = 512;        // one stream's state: the pipeline
 constexpr int SWEEP_THREADS = 256;      // many independent states (hyper-parameter sweep): 2 CTAs per SM by registers
 
-// One CTA per clustering state.  CTA t owns centroid table t ([M][D] at centers + t M D), active flags t ([32]), the
-// `initialized` pair t and the map rows t ([B][K]); `trials` (nullable) holds {tau, rho, delta} per state as float64, NULL
-// = the thresholds of `p` (single state, grid of one).  Every state reads the same chunks and the same prep results.  The
-// arithmetic does not depend on THREADS: each centroid's distances are one warp's, the updates are element-wise.  STATES =
-// false compiles the single-state form of the pipeline (no per-state indexing).
+// One CTA per clustering state.  STATES = false compiles the single-state form of the pipeline (grid of one, the thresholds
+// of `p`, no per-state indexing).  STATES = true: CTA i runs the state states[i] = {file f, trial t} over the chunks
+// [chunk_off[f], chunk_off[f + 1]) of the B concatenated ones, with {tau, rho, delta} = trials [t] (float64); state
+// s = f T + t owns centroid table s ([M][D] at centers + s M D), active flags s ([32]) and the `initialized` / error pair s,
+// and writes the map rows of its chunks in trial t's block ([B][K] at map_out + t B K).  Outputs are addressed by (f, t),
+// so the launch order (the order of `states`) changes no result.  The arithmetic does not depend on THREADS: each
+// centroid's distances are one warp's, the updates are element-wise.
 template <int THREADS, bool STATES>
 __global__ void __launch_bounds__(THREADS)
-cluster_seq_kernel(ClusterParams p, const double* __restrict__ trials, const float* __restrict__ seg,
+cluster_seq_kernel(ClusterParams p, const double* __restrict__ trials, const int2* __restrict__ states,
+                   const int* __restrict__ chunk_off, int T, const float* __restrict__ seg,
                    const float* __restrict__ emb, int B, int F, int K, double* __restrict__ centers,
                    int* __restrict__ g_active, int* __restrict__ g_init, const float* __restrict__ prep,
                    const double* __restrict__ prep_d, int32_t* __restrict__ map_out, float* __restrict__ permuted,
@@ -128,12 +131,17 @@ cluster_seq_kernel(ClusterParams p, const double* __restrict__ trials, const flo
   constexpr int NW = SEQ_THREADS / 32;
   float tau_f = p.tau_f, rho_f = p.rho_f;
   double delta = p.delta;
+  int first = 0;                                // chunk ci of this state is chunk first + ci of seg / emb / prep
   if constexpr (STATES) {
-    const int trial = blockIdx.x;
-    centers += (size_t)trial * M * D;
-    g_active += (size_t)trial * CM;
-    g_init += (size_t)trial * 2;
-    map_out += (size_t)trial * B * K;
+    const int2 fs = states[blockIdx.x];
+    const int trial = fs.y, c0 = chunk_off[fs.x];
+    const size_t s = (size_t)fs.x * T + trial;
+    centers += s * M * D;
+    g_active += s * CM;
+    g_init += s * 2;
+    map_out += ((size_t)trial * B + c0) * K;
+    B = chunk_off[fs.x + 1] - c0;              // from here on: this file's chunks, the first at c0
+    first = c0;
     // numpy compares the float32 scores with a Python float in float32 (as dg_cluster_create)
     tau_f = (float)trials[trial * 3 + 0];
     rho_f = (float)trials[trial * 3 + 1];
@@ -144,11 +152,12 @@ cluster_seq_kernel(ClusterParams p, const double* __restrict__ trials, const flo
                                                                // per chunk by all threads instead of once per centroid warp)
   float* es = reinterpret_cast<float*>(ed + (size_t)K * D);    // embeddings [2][K][D], double buffered (cp.async landing zone)
   auto prefetch = [&](int ci, int buf) {
-    const float* e = emb + (size_t)ci * K * D;
+    const size_t cg = (size_t)(first + ci);
+    const float* e = emb + cg * K * D;
     for (int i = tid; i < K * D; i += SEQ_THREADS) cp_async4(es + (size_t)buf * K * D + i, e + i);
-    if (tid < K * 3) cp_async4(&prs[buf][tid], prep + (size_t)ci * K * 3 + tid);
+    if (tid < K * 3) cp_async4(&prs[buf][tid], prep + cg * K * 3 + tid);
     if (tid < K * 2) cp_async4(reinterpret_cast<float*>(&ens[buf][0]) + tid,
-                               reinterpret_cast<const float*>(prep_d + (size_t)ci * K) + tid);
+                               reinterpret_cast<const float*>(prep_d + cg * K) + tid);
     asm volatile("cp.async.commit_group;");
   };
   prefetch(0, 0);
@@ -377,7 +386,7 @@ cluster_seq_kernel(ClusterParams p, const double* __restrict__ trials, const flo
     if (tid < K) map_out[(size_t)ci * K + tid] = sh.map[tid];
     if (permuted) {                                                                     // mapping.py:341-360
       float* o = permuted + (size_t)ci * F * M;
-      const float* s = seg + (size_t)ci * F * K;
+      const float* s = seg + (size_t)(first + ci) * F * K;
       for (int idx = tid; idx < F * M; idx += SEQ_THREADS) o[idx] = 0.f;
       __syncthreads();
       for (int k = 0; k < K; k++) {
@@ -443,8 +452,8 @@ int launch_cluster_step(const ClusterParams& p, const float* seg, const float* e
   if (timing) {   // diagnostic: SM-clock stamps per chunk (distances | assignment logic | update + hand-over), synchronises
     unsigned* dbg = nullptr;
     DG_CUDA(cudaMalloc(&dbg, (size_t)B * 4 * sizeof(unsigned)));
-    cluster_seq_kernel<SEQ_THREADS, false><<<1, SEQ_THREADS, dyn, st>>>(p, nullptr, seg, emb, B, F, K, centers, active, initialized,
-                                                                prep, prep_d, map, permuted, dbg);
+    cluster_seq_kernel<SEQ_THREADS, false><<<1, SEQ_THREADS, dyn, st>>>(p, nullptr, nullptr, nullptr, 1, seg, emb, B, F, K, centers,
+                                                                active, initialized, prep, prep_d, map, permuted, dbg);
     DG_CUDA(cudaStreamSynchronize(st));
     std::vector<unsigned> hb((size_t)B * 4);
     DG_CUDA(cudaMemcpy(hb.data(), dbg, hb.size() * 4, cudaMemcpyDeviceToHost));
@@ -462,25 +471,27 @@ int launch_cluster_step(const ClusterParams& p, const float* seg, const float* e
     DG_LAUNCHED();
     return 0;
   }
-  cluster_seq_kernel<SEQ_THREADS, false><<<1, SEQ_THREADS, dyn, st>>>(p, nullptr, seg, emb, B, F, K, centers, active, initialized,
-                                                              prep, prep_d, map, permuted, nullptr);
+  cluster_seq_kernel<SEQ_THREADS, false><<<1, SEQ_THREADS, dyn, st>>>(p, nullptr, nullptr, nullptr, 1, seg, emb, B, F, K, centers,
+                                                              active, initialized, prep, prep_d, map, permuted, nullptr);
   DG_LAUNCHED();
   return 0;
 }
 
-// T independent states over the same B chunks, each from its own {tau, rho, delta} (trials_dev [T][3] float64): one prep pass,
-// then one CTA per state.  States beyond the resident CTAs run in later waves of the same launch.
-int launch_cluster_sweep(const ClusterParams& p, const double* trials_dev, int T, const float* seg, const float* emb, int B,
-                         int F, int K, double* centers, int* active, int* initialized, float* prep, double* prep_d,
-                         int32_t* maps, cudaStream_t st) {
+// S independent (file, trial) states over the B concatenated chunks of the files, each from its trial's {tau, rho, delta}
+// (trials_dev [T][3] float64): one prep pass over all B chunks, then one CTA per state in the order of states_dev.  States
+// beyond the resident CTAs run in later waves of the same launch.
+int launch_cluster_sweep(const ClusterParams& p, const double* trials_dev, int T, const int2* states_dev, int S,
+                         const int* chunk_off_dev, const float* seg, const float* emb, int B, int F, int K, double* centers,
+                         int* active, int* initialized, float* prep, double* prep_d, int32_t* maps, cudaStream_t st) {
   ProfScope _ps("cluster_sweep", st);
   if (check_cluster_shape("cluster_sweep", p, K)) return -1;
-  if (B <= 0 || T <= 0) return 0;
+  if (B <= 0 || S <= 0) return 0;
   cluster_prep_kernel<<<B, 128, 0, st>>>(seg, emb, F, K, p.D, prep, prep_d);
   DG_LAUNCHED();
   if (int rc = cluster_seq_allow_dyn<SWEEP_THREADS, true>()) return rc;
-  cluster_seq_kernel<SWEEP_THREADS, true><<<T, SWEEP_THREADS, cluster_seq_dyn(p.M, p.D, K), st>>>(
-      p, trials_dev, seg, emb, B, F, K, centers, active, initialized, prep, prep_d, maps, nullptr, nullptr);
+  cluster_seq_kernel<SWEEP_THREADS, true><<<S, SWEEP_THREADS, cluster_seq_dyn(p.M, p.D, K), st>>>(
+      p, trials_dev, states_dev, chunk_off_dev, T, seg, emb, B, F, K, centers, active, initialized, prep, prep_d, maps,
+      nullptr, nullptr);
   DG_LAUNCHED();
   return 0;
 }

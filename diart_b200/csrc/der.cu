@@ -2,12 +2,14 @@
 // Benchmark.evaluate with DiarizationErrorRate(collar=0, skip_overlap=False), src/diart/inference.py:359-390), DESIGN.md
 // "DER scoring" for the definition.
 //
-//   der_hyp<false> / der_hyp<true>   one warp per (trial, label): walks the sweep's per-chunk turns in chunk order and merges
-//                                    that label's turns into whole-file segments with PredictionAccumulator's collar rule
-//                                    (count pass, then write pass at scanned offsets)
-//   der_scan                         exclusive prefix sum of the (trial, label) counts
-//   der_score                        one warp per trial: k-way merge of the boundary lists (one lane per hypothesis label and
-//                                    per reference label), co-occurrence matrix, LSAP, the five components
+//   der_hyp<false> / der_hyp<true>   one warp per (file, trial, label): walks the sweep's per-chunk turns of that file's
+//                                    chunk range in chunk order, with the file's timestamp shift, and merges that label's
+//                                    turns into whole-file segments with PredictionAccumulator's collar rule (count pass,
+//                                    then write pass at scanned offsets)
+//   der_scan                         exclusive prefix sum of the (file, trial, label) counts
+//   der_score                        one warp per (file, trial) against that file's reference: k-way merge of the boundary
+//                                    lists (one lane per hypothesis label and per reference label), co-occurrence matrix,
+//                                    LSAP, the five components
 //
 // Every float64 operation is explicitly rounded (no FMA contraction): the segment times equal numpy's turn_times /
 // assemble_predictions bit for bit, and the components are sums in time order, independent of the launch geometry.
@@ -19,18 +21,22 @@ namespace dg {
 constexpr int DER_THREADS = 256;
 constexpr int DER_SCORE_THREADS = 128;
 
-// whole-file segments of label g in trial t: turn times as blocks/post.py turn_times, segments with duration <= 1e-6 dropped,
-// merged in chunk order (= (start, end) order: the chunks' output regions tile the timeline) with a running maximum of the
-// ends; a segment joins when it starts less than `collar` after that maximum or not after it
+// whole-file segments of label g in trial t of file f: turn times as blocks/post.py turn_times, segments with duration <= 1e-6
+// dropped, merged in chunk order (= (start, end) order: the chunks' output regions tile the file's timeline) with a running
+// maximum of the ends; a segment joins when it starts less than `collar` after that maximum or not after it.  Six CTAs per SM
+// (at most 42 registers): without a minimum ptxas holds the kernel to 32 registers and spills in the file loop.
 template <bool WRITE>
-__global__ void __launch_bounds__(DER_THREADS)
-der_hyp_kernel(const int32_t* __restrict__ header /*[T][N][4]*/, const uint32_t* __restrict__ turns, int T, int N, int M,
-               const double* __restrict__ out_start, const double* __restrict__ out_res, double shift, double collar,
-               int* __restrict__ counts /*[T*M+1]: count pass output, write pass offsets*/, double* __restrict__ segs,
+__global__ void __launch_bounds__(DER_THREADS, 6)
+der_hyp_kernel(const int32_t* __restrict__ header /*[T][N][4]*/, const uint32_t* __restrict__ turns, int nf,
+               const int* __restrict__ chunk_off /*[nf+1]*/, int T, int N, int M, const double* __restrict__ out_start,
+               const double* __restrict__ out_res, const double* __restrict__ shifts /*[nf]*/, double collar,
+               int* __restrict__ counts /*[nf*T*M+1]: count pass output, write pass offsets*/, double* __restrict__ segs,
                double* __restrict__ segs_copy, int copy_cap) {
   const int w = (int)(((size_t)blockIdx.x * DER_THREADS + threadIdx.x) >> 5), lane = threadIdx.x & 31;
-  if (w >= T * M) return;   // the whole warp
-  const int t = w / M, g = w - t * M;
+  if (w >= nf * T * M) return;   // the whole warp
+  const int ft = w / M, g = w - ft * M, f = ft / T, t = ft - f * T;
+  const int c_begin = chunk_off[f], c_end = chunk_off[f + 1];
+  const double shift = shifts[f];
   const int32_t* hd = header + (size_t)t * N * 4;
   int n = 0, o = WRITE ? counts[w] : 0;
   bool open = false;
@@ -47,10 +53,10 @@ der_hyp_kernel(const int32_t* __restrict__ header /*[T][N][4]*/, const uint32_t*
     o++;
     n++;
   };
-  for (int c0 = 0; c0 < N; c0 += 32) {
+  for (int c0 = c_begin; c0 < c_end; c0 += 32) {
     // lane j finds label g's turns in chunk c0 + j: a chunk's turns are grouped by label in ascending order (post.cu)
     int lo = 0, hi = 0;
-    if (c0 + lane < N) {
+    if (c0 + lane < c_end) {
       const int4 h = *reinterpret_cast<const int4*>(hd + (size_t)(c0 + lane) * 4);
       int a = h.x;
       const int e = h.x + h.y;
@@ -150,14 +156,18 @@ __device__ __forceinline__ void der_walk(const double* hp, int h0, int h1, const
   }
 }
 
-// comp [T][5] = {false alarm, missed detection, confusion, correct, total}
+// comp [nf][T][5] = {false alarm, missed detection, confusion, correct, total}; warp (f, t) scores trial t of file f against
+// file f's reference: R[f] labels at offsets roff [f][DER_ROFF] into rseg
 __global__ void __launch_bounds__(DER_SCORE_THREADS)
-der_score_kernel(const int* __restrict__ hoff /*[T*M+1]*/, const double* __restrict__ hseg, int T, int M,
-                 const int* __restrict__ roff /*[R+1]*/, const double* __restrict__ rseg, int R, double* __restrict__ comp) {
+der_score_kernel(const int* __restrict__ hoff /*[nf*T*M+1]*/, const double* __restrict__ hseg, int nf, int T, int M,
+                 const int* __restrict__ roff_all /*[nf][DER_ROFF]*/, const int* __restrict__ R_all /*[nf]*/,
+                 const double* __restrict__ rseg, double* __restrict__ comp) {
   __shared__ double tr[DER_SCORE_THREADS / 32][32][33];
-  const int t = (int)(((size_t)blockIdx.x * DER_SCORE_THREADS + threadIdx.x) >> 5), lane = threadIdx.x & 31;
-  if (t >= T) return;
-  const int h0 = lane < M ? hoff[t * M + lane] : 0, h1 = lane < M ? hoff[t * M + lane + 1] : 0;
+  const int ft = (int)(((size_t)blockIdx.x * DER_SCORE_THREADS + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (ft >= nf * T) return;
+  const int f = ft / T, R = R_all[f];
+  const int* roff = roff_all + (size_t)f * DER_ROFF;
+  const int h0 = lane < M ? hoff[ft * M + lane] : 0, h1 = lane < M ? hoff[ft * M + lane + 1] : 0;
   const int r0 = lane < R ? roff[lane] : 0, r1 = lane < R ? roff[lane + 1] : 0;
   // pass 1: co-occurrence C[r][h], lane h owns column h, each entry summed in time order
   double C[32];
@@ -203,7 +213,7 @@ der_score_kernel(const int* __restrict__ hoff /*[T*M+1]*/, const double* __restr
     conf = __dadd_rn(conf, __dmul_rn(d, (double)(min(nr, nh) - c)));
   });
   if (lane == 0) {
-    double* o = comp + (size_t)t * 5;
+    double* o = comp + (size_t)ft * 5;
     o[0] = fa;
     o[1] = miss;
     o[2] = conf;
@@ -212,36 +222,37 @@ der_score_kernel(const int* __restrict__ hoff /*[T*M+1]*/, const double* __restr
   }
 }
 
-int launch_der_hyp_count(const int32_t* header, const uint32_t* turns, int T, int N, int M, const double* out_start,
-                         const double* out_res, double shift, double collar, int* offsets, cudaStream_t st) {
+int launch_der_hyp_count(const int32_t* header, const uint32_t* turns, int nf, const int* chunk_off, int T, int N, int M,
+                         const double* out_start, const double* out_res, const double* shifts, double collar, int* offsets,
+                         cudaStream_t st) {
   ProfScope _ps("der_hyp_count", st);
-  const long long warps = (long long)T * M;
+  const long long warps = (long long)nf * T * M;
   const unsigned blocks = (unsigned)((warps * 32 + DER_THREADS - 1) / DER_THREADS);
-  der_hyp_kernel<false><<<blocks, DER_THREADS, 0, st>>>(header, turns, T, N, M, out_start, out_res, shift, collar, offsets,
-                                                         nullptr, nullptr, 0);
+  der_hyp_kernel<false><<<blocks, DER_THREADS, 0, st>>>(header, turns, nf, chunk_off, T, N, M, out_start, out_res, shifts,
+                                                         collar, offsets, nullptr, nullptr, 0);
   DG_LAUNCHED();
-  der_scan_kernel<<<1, 1024, 0, st>>>(offsets, T * M);
+  der_scan_kernel<<<1, 1024, 0, st>>>(offsets, (int)warps);
   DG_LAUNCHED();
   return 0;
 }
 
-int launch_der_hyp_write(const int32_t* header, const uint32_t* turns, int T, int N, int M, const double* out_start,
-                         const double* out_res, double shift, double collar, int* offsets, double* segs, double* segs_copy,
-                         int copy_cap, cudaStream_t st) {
+int launch_der_hyp_write(const int32_t* header, const uint32_t* turns, int nf, const int* chunk_off, int T, int N, int M,
+                         const double* out_start, const double* out_res, const double* shifts, double collar, int* offsets,
+                         double* segs, double* segs_copy, int copy_cap, cudaStream_t st) {
   ProfScope _ps("der_hyp_write", st);
-  const long long warps = (long long)T * M;
+  const long long warps = (long long)nf * T * M;
   const unsigned blocks = (unsigned)((warps * 32 + DER_THREADS - 1) / DER_THREADS);
-  der_hyp_kernel<true><<<blocks, DER_THREADS, 0, st>>>(header, turns, T, N, M, out_start, out_res, shift, collar, offsets,
-                                                        segs, segs_copy, copy_cap);
+  der_hyp_kernel<true><<<blocks, DER_THREADS, 0, st>>>(header, turns, nf, chunk_off, T, N, M, out_start, out_res, shifts,
+                                                        collar, offsets, segs, segs_copy, copy_cap);
   DG_LAUNCHED();
   return 0;
 }
 
-int launch_der_score(const int* hoff, const double* hseg, int T, int M, const int* roff, const double* rseg, int R,
-                     double* comp, cudaStream_t st) {
+int launch_der_score(const int* hoff, const double* hseg, int nf, int T, int M, const int* roff, const int* R,
+                     const double* rseg, double* comp, cudaStream_t st) {
   ProfScope _ps("der_score", st);
-  const unsigned blocks = (unsigned)(((long long)T * 32 + DER_SCORE_THREADS - 1) / DER_SCORE_THREADS);
-  der_score_kernel<<<blocks, DER_SCORE_THREADS, 0, st>>>(hoff, hseg, T, M, roff, rseg, R, comp);
+  const unsigned blocks = (unsigned)(((long long)nf * T * 32 + DER_SCORE_THREADS - 1) / DER_SCORE_THREADS);
+  der_score_kernel<<<blocks, DER_SCORE_THREADS, 0, st>>>(hoff, hseg, nf, T, M, roff, R, rseg, comp);
   DG_LAUNCHED();
   return 0;
 }

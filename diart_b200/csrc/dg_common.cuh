@@ -253,11 +253,13 @@ int launch_cluster_merge(const double* records, int world, int rank, const Clust
                          int* active, double* base, int* base_active, int* initialized, int32_t* relabel,
                          cudaStream_t st);
 int launch_relabel_maps(int32_t* maps, int n, const int32_t* relabel, cudaStream_t st);
-// T independent states, thresholds trials_dev [T][3] = {tau, rho, delta} float64; centers [T][M][D], active [T][32],
-// initialized [T][2], maps [T][B][K]
-int launch_cluster_sweep(const ClusterParams& p, const double* trials_dev, int T, const float* seg, const float* emb, int B,
-                         int F, int K, double* centers, int* active, int* initialized, float* prep, double* prep_d,
-                         int32_t* maps, cudaStream_t st);
+// states = (file, trial) pairs over the concatenated chunks of several files: file f owns chunks
+// [chunk_off[f], chunk_off[f + 1]) of B; thresholds trials_dev [T][3] = {tau, rho, delta} float64; one CTA per entry of
+// states_dev [S] {file, trial} (the launch order); state s = file * T + trial owns centers [s][M][D], active [s][32] and
+// initialized [s][2]; maps [T][B][K]
+int launch_cluster_sweep(const ClusterParams& p, const double* trials_dev, int T, const int2* states_dev, int S,
+                         const int* chunk_off_dev, const float* seg, const float* emb, int B, int F, int K, double* centers,
+                         int* active, int* initialized, float* prep, double* prep_d, int32_t* maps, cudaStream_t st);
 size_t cluster_prep_floats(int B, int K);
 // post.cu -- aggregation + binarisation + run-length turns (reference diarization.py:205-232)
 int launch_post(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map, int n_hist, int B,
@@ -268,16 +270,20 @@ int launch_expand_windows(const float* ring, long long r0, int C, int hop, int S
 int launch_post_history(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map, int n_hist,
                         int B, int F, int K, int keep, float* new_seg, int32_t* new_map, cudaStream_t st);
 size_t cluster_prep_doubles(int B, int K);
-// der.cu -- DER components of sweep trials.  Hypothesis segments: count per (trial, label) and scan into offsets [T*M+1],
-// then write [offsets[T*M]][2] start / end (and, when segs_copy is given, the first copy_cap of them there too)
-int launch_der_hyp_count(const int32_t* header, const uint32_t* turns, int T, int N, int M, const double* out_start,
-                         const double* out_res, double shift, double collar, int* offsets, cudaStream_t st);
-int launch_der_hyp_write(const int32_t* header, const uint32_t* turns, int T, int N, int M, const double* out_start,
-                         const double* out_res, double shift, double collar, int* offsets, double* segs, double* segs_copy,
-                         int copy_cap, cudaStream_t st);
-// reference: R labels, offsets roff [R+1] into rseg [S][2]; comp [T][5] = {false alarm, missed, confusion, correct, total}
-int launch_der_score(const int* hoff, const double* hseg, int T, int M, const int* roff, const double* rseg, int R,
-                     double* comp, cudaStream_t st);
+// der.cu -- DER components of sweep trials over nf files (chunks [chunk_off[f], chunk_off[f + 1]) of N, timestamp shift
+// shifts[f]).  Hypothesis segments: count per (file, trial, label) and scan into offsets [nf*T*M+1], then write
+// [offsets[nf*T*M]][2] start / end (and, when segs_copy is given, the first copy_cap of them there too)
+int launch_der_hyp_count(const int32_t* header, const uint32_t* turns, int nf, const int* chunk_off, int T, int N, int M,
+                         const double* out_start, const double* out_res, const double* shifts, double collar, int* offsets,
+                         cudaStream_t st);
+int launch_der_hyp_write(const int32_t* header, const uint32_t* turns, int nf, const int* chunk_off, int T, int N, int M,
+                         const double* out_start, const double* out_res, const double* shifts, double collar, int* offsets,
+                         double* segs, double* segs_copy, int copy_cap, cudaStream_t st);
+// reference of file f: R[f] labels, offsets roff [f][DER_ROFF] (R[f] + 1 used) into rseg [S][2];
+// comp [nf][T][5] = {false alarm, missed, confusion, correct, total}
+constexpr int DER_ROFF = 33;
+int launch_der_score(const int* hoff, const double* hseg, int nf, int T, int M, const int* roff, const int* R,
+                     const double* rseg, double* comp, cudaStream_t st);
 // resample.cu -- polyphase sinc resampling (torchaudio's defaults): reduced ratio o / n, half-width w, T = 2w + o taps per phase
 struct RsGeom {
   int o, n, w, T;

@@ -18,6 +18,11 @@ computes from those predictions: the diarization error rate components of every 
 (``DiarizationErrorRate(collar=0, skip_overlap=False)``; definition in DESIGN.md "DER scoring"), evaluated on the device by
 ``dg_sweep_score`` (``csrc/der.cu``) without building any ``Annotation``.  :meth:`HyperParameterSweep.score_files` sums them over
 files: its ``total.der`` is the value ``Optimizer.objective`` minimises.
+
+:class:`DatasetSweep` does the same for a whole dataset at once: the network pass of every file runs once, in one pipelined
+flow, and its outputs stay on the device; every ``score`` / ``run`` call then clusters, post-processes and scores all
+(file, trial) pairs in one launch per kernel (``dg_sweep_score_files`` / ``dg_sweep_run_files``), without running a network
+kernel again.
 """
 from __future__ import annotations
 
@@ -37,6 +42,7 @@ from .operators import DeviceAudioStream
 
 NETWORK_BATCH = 256           # windows per network step (the benchmarked batch)
 TRIALS_PER_LAUNCH = 1024      # trials per dg_sweep_run; more run as further launches over the same network outputs
+TRIAL_CHUNKS_PER_LAUNCH = 4 << 20   # DatasetSweep: trials x chunks per launch (bounds the header, maps and turn buffers)
 PATCH_COLLAR = 0.05           # PredictionAccumulator's default (sinks.py)
 MAX_REFERENCE_LABELS = 32     # one lane per reference label in the scoring kernel
 
@@ -222,6 +228,64 @@ class SweepOutputs:
     device_seconds: float = 0.0
 
 
+_AUDIO_STREAMS = 3            # audio streams the dataset network pass uses in turn (see network_pass_files)
+
+
+def seg_resolution(config: SpeakerDiarizationConfig, start: float, F: int) -> float:
+    """seconds per score frame of a window starting at ``start``: ``SpeakerDiarization.__call__``'s
+    waveforms[0].extent.duration / F, the extent of a window of 1 / sample_rate frames"""
+    sr = config.sample_rate
+    end = start + int(np.rint(config.duration * sr)) * (1 / sr)
+    return (end - start if end > start else 0.0) / F
+
+
+def dataset_plan(fws: Sequence[FileWindows], config: SpeakerDiarizationConfig, F: int):
+    """The post-path plans of several files, each that of a fresh stream (empty history), concatenated in file order ->
+    (plan int32 (N, 4 + nw), out_start (N,), out_res (N,)).  post.cu finds chunk c's aggregated buffers at chunks
+    c - (nb - 1) .. c with nb <= (c's index in its file) + 1, so no chunk reaches into the previous file."""
+    nw = int(round(config.latency / config.step))
+    parts = [post_plan(np.asarray(fw.starts, dtype=np.float64), seg_resolution(config, float(fw.starts[0]), F), np.zeros(0),
+                       np.zeros(0), nw, F, config.step, config.latency) for fw in fws]
+    return tuple(np.ascontiguousarray(np.concatenate([p[i] for p in parts])) for i in range(3))
+
+
+def trial_groups(num_trials: int, num_chunks: int) -> List[slice]:
+    """consecutive slices of the trials, one per launch: at most TRIALS_PER_LAUNCH trials and TRIAL_CHUNKS_PER_LAUNCH
+    trial-chunks each"""
+    per = min(TRIALS_PER_LAUNCH, TRIAL_CHUNKS_PER_LAUNCH // num_chunks)
+    if per < 1:
+        raise ValueError(f"{num_chunks} chunks exceed the {TRIAL_CHUNKS_PER_LAUNCH} trial-chunks of one launch")
+    return [slice(i, min(i + per, num_trials)) for i in range(0, num_trials, per)]
+
+
+def pack_references(references: Sequence[Annotation]):
+    """per-file references -> the reference arguments of dg_sweep_score_files: (rows float64 (S, 2), labels int32 (S,),
+    row offsets int32 (files + 1,), label counts int32 (files,)); each file's rows as ``reference_arrays`` gives them"""
+    rows, labels, offsets, counts = [], [], [0], []
+    for ref in references:
+        r, lab, names = reference_arrays(ref)
+        rows.append(r)
+        labels.append(lab)
+        offsets.append(offsets[-1] + len(r))
+        counts.append(len(names))
+    return (np.ascontiguousarray(np.concatenate(rows), dtype=np.float64),
+            np.ascontiguousarray(np.concatenate(labels), dtype=np.int32), np.array(offsets, dtype=np.int32),
+            np.array(counts, dtype=np.int32))
+
+
+def file_turns(header: np.ndarray, turns: np.ndarray, c0: int, c1: int):
+    """header int32 (T, N, 4) and the packed turns of a sweep over several files -> the header (T, c1 - c0, 4) of the file
+    with chunks [c0, c1) and its turns alone (offsets renumbered so that its blocks tile its turn list)"""
+    h = np.ascontiguousarray(header[:, c0:c1])
+    flat = h.reshape(-1, 4)
+    cnt = flat[:, 1].astype(np.int64)
+    start = np.concatenate([[0], np.cumsum(cnt)[:-1]]).astype(np.int64)
+    src = np.repeat(flat[:, 0].astype(np.int64) - start, cnt) + np.arange(int(cnt.sum()))
+    flat[:, 0] = start
+    own = turns[src]
+    return h, own, len(own)
+
+
 class HyperParameterSweep:
     """Runs ``SpeakerDiarization(config)`` over a file for many (tau_active, rho_update, delta_new) trials at the cost of one
     network pass.  Needs the native segmentation and embedding models.
@@ -254,23 +318,40 @@ class HyperParameterSweep:
     def network_pass(self, fw: FileWindows):
         """scores (N, F, K) and embeddings (N, K, D) of every window, on the device: the fused pipeline in batches of 256
         (its own clustering runs too; its maps are not used)"""
+        return self.network_pass_files([fw])
+
+    def network_pass_files(self, fws: Sequence[FileWindows]):
+        """:meth:`network_pass` of several files as one pipelined flow -> their scores and embeddings concatenated in file
+        order.  Every batch holds windows of one file only, cut at the multiples of 256 from that file's window 0: the batch
+        is the unit of the network pass's arithmetic (the sinc layer's stream form covers one batch), so each file's outputs
+        are the bits :meth:`network_pass` gives for it alone.  Nothing drains or synchronises between files."""
         cfg, pipe = self.config, self.pipeline
         pipe.reset()
-        stream = DeviceAudioStream(cfg.duration, cfg.step, cfg.sample_rate, max_windows=NETWORK_BATCH, device=self.device)
-        pushed, segs, embs, inflight = fw.offset, [], [], []
+        streams: List[DeviceAudioStream] = []
+        segs, embs, inflight = [], [], []
         with torch.cuda.device(self.device):
-            for i0 in range(0, fw.num_windows, NETWORK_BATCH):
-                B = min(NETWORK_BATCH, fw.num_windows - i0)
-                need = fw.offset + (i0 + B - 1) * fw.step_samples + fw.chunk_samples
-                stream.push(fw.samples[pushed:need])
-                pushed = need
-                inflight.append(stream.windows(B))           # must stay alive until collected
-                pipe.submit(inflight[-1])
-                if len(inflight) == 2:
-                    seg, emb, _ = pipe.collect()
-                    segs.append(seg)
-                    embs.append(emb)
-                    inflight.pop(0)
+            for i, fw in enumerate(fws):
+                # a few streams in turn: a reset waits for the uploads of its stream, so reuse the one whose file was
+                # submitted longest ago (its batches have left the pipeline's slots)
+                if len(streams) < _AUDIO_STREAMS:
+                    streams.append(DeviceAudioStream(cfg.duration, cfg.step, cfg.sample_rate, max_windows=NETWORK_BATCH,
+                                                     device=self.device))
+                stream = streams[i % _AUDIO_STREAMS]
+                if i >= _AUDIO_STREAMS:
+                    stream.reset()
+                pushed = fw.offset
+                for i0 in range(0, fw.num_windows, NETWORK_BATCH):
+                    B = min(NETWORK_BATCH, fw.num_windows - i0)
+                    need = fw.offset + (i0 + B - 1) * fw.step_samples + fw.chunk_samples
+                    stream.push(fw.samples[pushed:need])
+                    pushed = need
+                    inflight.append(stream.windows(B))       # must stay alive until collected
+                    pipe.submit(inflight[-1])
+                    if len(inflight) == 2:
+                        seg, emb, _ = pipe.collect()
+                        segs.append(seg)
+                        embs.append(emb)
+                        inflight.pop(0)
             while inflight:
                 seg, emb, _ = pipe.collect()
                 segs.append(seg)
@@ -371,10 +452,7 @@ class HyperParameterSweep:
         return comp, e0.elapsed_time(e1) / 1e3, offsets, hseg
 
     def _seg_resolution(self, start: float, F: int) -> float:
-        # SpeakerDiarization.__call__: waveforms[0].extent.duration / F, the extent of a window of 1 / sample_rate frames
-        sr = self.config.sample_rate
-        end = start + int(np.rint(self.config.duration * sr)) * (1 / sr)
-        return (end - start if end > start else 0.0) / F
+        return seg_resolution(self.config, start, F)
 
     # ------------------------------------------------------------------ the public entry
     def run(self, waveform: np.ndarray, uri: Optional[str] = None,
@@ -422,10 +500,162 @@ class HyperParameterSweep:
     def score_files(self, files: Iterable[Tuple[np.ndarray, Annotation]],
                     trials: Sequence[Mapping[str, float]] = ({},)) -> Tuple[List[DERComponents], DERComponents]:
         """``files``: (waveform, reference) pairs -> (components per file, their sum).  ``total.der`` per trial is the
-        value the reference's ``Optimizer.objective`` minimises over a dataset (a fraction, not a percentage)."""
-        per_file = [self.score(waveform, reference, trials) for waveform, reference in files]
-        if not per_file:
+        value the reference's ``Optimizer.objective`` minimises over a dataset (a fraction, not a percentage).  Runs as a
+        :class:`DatasetSweep` over the files."""
+        files = [(None, waveform, reference) for waveform, reference in files]
+        if not files:
             raise ValueError("at least one file is needed")
+        dataset = DatasetSweep(self.config, files, sweep=self)
+        out = dataset.score(trials)
+        self.timing = dict(dataset.timing)
+        return out
+
+
+class DatasetSweep:
+    """A sweep over a whole dataset with the network outputs of every file kept on the device.
+
+        ds = DatasetSweep(config, [("file1", waveform1, reference1), ("file2", waveform2, reference2)])
+        per_file, total = ds.score([{"tau_active": 0.5}, {"delta_new": 0.8, "rho_update": 0.2}])
+        best = int(np.argmin(total.der))
+
+    ``files``: (uri, 1-D float32 waveform at ``config.sample_rate``, reference annotation or None).  The constructor runs
+    the network pass of all files as one pipelined flow (:meth:`HyperParameterSweep.network_pass_files`) and keeps the
+    concatenated scores and embeddings on the device: F K + K D float32 per chunk (3 516 + 6 144 B = 9.66 kB at the
+    default models, F = 293 frames, K = 3 local speakers, D = 512; two chunks per second of audio at step 0.5 s, so about
+    0.7 GB per 10 hours).  Then :meth:`score` and :meth:`run` cluster, post-process and score every (file, trial) pair in
+    one launch per kernel and per trial group (at most 1024 trials and 4 Mi trial-chunks each) and run no network kernel:
+    a tuning loop pays for the networks once.  For every file and trial the results are the bits a
+    :class:`HyperParameterSweep` of that file alone gives, whatever the other files and their order.
+    ``sweep``: a :class:`HyperParameterSweep` of the same config whose pipeline and handles to use (default: a new one).
+    """
+
+    def __init__(self, config: SpeakerDiarizationConfig, files: Iterable[Tuple[Optional[str], np.ndarray, Optional[Annotation]]],
+                 sweep: Optional[HyperParameterSweep] = None):
+        files = list(files)
+        if not files:
+            raise ValueError("at least one file is needed")
+        for i, (uri, x, _) in enumerate(files):
+            if np.asarray(x).size == 0:
+                raise ValueError(f"file {i} ({uri}) has no samples, so no windows")
+        self.config = config
+        self._sweep = sweep if sweep is not None else HyperParameterSweep(config)
+        self.device = self._sweep.device
+        self.uris = [uri for uri, _, _ in files]
+        self.references = [ref for _, _, ref in files]
+        fws = [file_windows(x, config) for _, x, _ in files]   # (the padded audio is dropped after the network pass)
+        self.offsets = np.ascontiguousarray(np.cumsum([0] + [fw.num_windows for fw in fws]), dtype=np.int32)
+        trial_groups(1, int(self.offsets[-1]))                  # a dataset too large for one launch fails here
+        t0 = time.perf_counter()
+        self.seg, self.emb = self._sweep.network_pass_files(fws)
+        torch.cuda.synchronize(self.device)
+        self.timing: Dict[str, float] = {"network": time.perf_counter() - t0}
+        self.plan, self.out_start, self.out_res = dataset_plan(fws, config, self.seg.shape[1])
+        self.shifts = np.ascontiguousarray([-fw.padding[0] for fw in fws], dtype=np.float64)
+        self._refs = None
+
+    @property
+    def num_chunks(self) -> int:
+        return int(self.offsets[-1])
+
+    @property
+    def resident_bytes(self) -> int:
+        """device bytes of the kept network outputs"""
+        return self.seg.numel() * self.seg.element_size() + self.emb.numel() * self.emb.element_size()
+
+    def file_outputs(self, f: int) -> Tuple[torch.Tensor, torch.Tensor]:
+        """file f's slice of the resident scores (n, F, K) and embeddings (n, K, D)"""
+        c0, c1 = int(self.offsets[f]), int(self.offsets[f + 1])
+        return self.seg[c0:c1], self.emb[c0:c1]
+
+    def _args(self):
+        N, F, K = self.seg.shape
+        h, _ = self._sweep._handle(F, K, self.emb.shape[2])
+        return h, N, len(self.uris)
+
+    def sweep(self, params: np.ndarray, keep_state: bool = False) -> SweepOutputs:
+        """dg_sweep_run_files over the resident outputs for params (T, 3): header (T, N, 4) and turns over the N
+        concatenated chunks; with ``keep_state`` maps (T, N, K) and centroids (files, T, M, D) on the device"""
+        h, N, nf = self._args()
+        K, D, M = self.seg.shape[2], self.emb.shape[2], int(self.config.max_speakers)
+        params = np.ascontiguousarray(params, dtype=np.float64)
+        T = len(params)
+        header = np.empty((T, N, 4), dtype=np.int32)
+        maps = torch.empty((T, N, K), dtype=torch.int32, device=self.device) if keep_state else None
+        centers = torch.empty((nf, T, M, D), dtype=torch.float64, device=self.device) if keep_state else None
+        sw = self._sweep
+        if len(sw._turns) < T * N * 8:
+            sw._turns = np.empty(T * N * 8, dtype=np.uint32)
+        n = C.c_int()
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream(self.device)
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            for attempt in range(2):
+                e0.record(st)
+                rc = _lib.lib().dg_sweep_run_files(h, self.seg.data_ptr(), self.emb.data_ptr(), N, nf, self.offsets.ctypes.data,
+                                                   params.ctypes.data, T, self.plan.ctypes.data, _lib.ptr(maps),
+                                                   _lib.ptr(centers), header.ctypes.data, sw._turns.ctypes.data,
+                                                   len(sw._turns), C.byref(n), st.cuda_stream)
+                e1.record(st)
+                if rc == -1 and n.value > len(sw._turns):     # more turns than the host buffer: grow it, run again
+                    sw._turns = np.empty(n.value, dtype=np.uint32)
+                    continue
+                _lib.check(rc)
+                break
+            e1.synchronize()
+        return SweepOutputs(header, sw._turns[:n.value].copy(), n.value, self.out_start, self.out_res, maps, centers,
+                            e0.elapsed_time(e1) / 1e3)
+
+    def run(self, trials: Sequence[Mapping[str, float]] = ({},)) -> List[List[Annotation]]:
+        """-> predictions [file][trial]: what :meth:`HyperParameterSweep.run` returns for each file alone"""
+        params = trial_params(trials, self.config)
+        labels = [f"speaker{g}" for g in range(int(self.config.max_speakers))]
+        out: List[List[Annotation]] = [[] for _ in self.uris]
+        dev = 0.0
+        for g in trial_groups(len(params), self.num_chunks):
+            r = self.sweep(params[g])
+            dev += r.device_seconds
+            for f in range(len(self.uris)):
+                c0, c1 = int(self.offsets[f]), int(self.offsets[f + 1])
+                header, turns, n = file_turns(r.header, r.turns, c0, c1)
+                out[f] += assemble_predictions(header, turns, n, self.out_start[c0:c1], self.out_res[c0:c1], labels,
+                                               float(self.shifts[f]), self.uris[f])
+        self.timing["sweep"] = dev
+        return out
+
+    def score(self, trials: Sequence[Mapping[str, float]] = ({},)) -> Tuple[List[DERComponents], DERComponents]:
+        """-> (components per file, their sum in file order): per file what :meth:`HyperParameterSweep.score` returns for
+        it alone; ``total.der`` is the value ``Optimizer.objective`` minimises.  Every file needs a reference."""
+        missing = [self.uris[i] if self.uris[i] is not None else i for i, r in enumerate(self.references) if r is None]
+        if missing:
+            raise ValueError(f"files without a reference cannot be scored: {missing}")
+        params = trial_params(trials, self.config)
+        if self._refs is None:
+            self._refs = pack_references(self.references)
+        rows, labels, roff, counts = self._refs
+        h, N, nf = self._args()
+        T = len(params)
+        comp = np.empty((nf, T, 5), dtype=np.float64)
+        dev = 0.0
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream(self.device)
+            for g in trial_groups(T, N):
+                p = np.ascontiguousarray(params[g])
+                part = np.empty((nf, len(p), 5), dtype=np.float64)
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(st)
+                rc = _lib.lib().dg_sweep_score_files(h, self.seg.data_ptr(), self.emb.data_ptr(), N, nf,
+                                                     self.offsets.ctypes.data, p.ctypes.data, len(p), self.plan.ctypes.data,
+                                                     self.out_start.ctypes.data, self.out_res.ctypes.data,
+                                                     self.shifts.ctypes.data, PATCH_COLLAR, rows.ctypes.data,
+                                                     labels.ctypes.data, roff.ctypes.data, counts.ctypes.data,
+                                                     part.ctypes.data, None, None, 0, st.cuda_stream)
+                e1.record(st)
+                _lib.check(rc)
+                e1.synchronize()
+                dev += e0.elapsed_time(e1) / 1e3
+                comp[:, g] = part
+        self.timing["score"] = dev
+        per_file = [DERComponents.from_array(comp[f]) for f in range(nf)]
         total = per_file[0]
         for c in per_file[1:]:
             total = total + c

@@ -234,6 +234,36 @@ int dg_sweep_score(dg_sweep* h, const float* seg_dev, const float* emb_dev, int 
                    const int32_t* plan_host, const double* out_start_host, const double* out_res_host, double shift,
                    double collar, const double* ref_host, const int32_t* ref_label_host, int S, int R,
                    double* components_host, int32_t* hyp_offsets_dev, double* hyp_segments_dev, int hyp_cap, void* stream);
+/* ---- dg_sweep_run_files / dg_sweep_score_files: the same for a dataset of num_files files in ONE launch per kernel (the
+ *      reference's Optimizer.objective scores a trial over every file of a dataset).  seg_dev / emb_dev hold the files'
+ *      chunks concatenated, N in all; file f owns chunks [chunk_offsets_host[f], chunk_offsets_host[f + 1]), with
+ *      chunk_offsets_host int32 [num_files + 1] starting at 0, ending at N and increasing (every file has a chunk).  A state is
+ *      a (file, trial) pair: a fresh clustering per file and trial, exactly what dg_sweep_run / dg_sweep_score give for that
+ *      file alone; num_files * T <= 2^21.  The clustering CTAs run longest file first (dg_sweep_state_order); the order
+ *      changes no result.
+ *        plan_host, out_start_host, out_res_host: each file's own (a fresh stream per file), concatenated;
+ *        maps_dev int32 [T][N][K], header_host int32 [T][N][4]: as dg_sweep_run over the concatenated chunks;
+ *        centers_dev float64 [num_files][T][M][D];
+ *        shifts_host float64 [num_files]: each file's timestamp shift;
+ *        ref_host [S][2] / ref_label_host [S]: the files' reference rows concatenated, file f's at rows
+ *        [ref_offsets_host[f], ref_offsets_host[f + 1]) (int32 [num_files + 1] from 0, not decreasing) with labels in
+ *        [0, ref_label_counts_host[f]) (int32 [num_files], each <= 32), checked per file as dg_sweep_score's;
+ *        components_host float64 [num_files][T][5];
+ *        hyp_offsets_dev int32 [num_files * T * max_speakers + 1] or NULL: (file, trial, label) major.
+ *      Every argument is checked before any launch.  Synchronous (synchronises `stream`). ---- */
+int dg_sweep_run_files(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int num_files,
+                       const int32_t* chunk_offsets_host, const double* params_host, int T, const int32_t* plan_host,
+                       int32_t* maps_dev, double* centers_dev, int32_t* header_host, uint32_t* turns_host, int turn_cap_host,
+                       int* n_turns, void* stream);
+int dg_sweep_score_files(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int num_files,
+                         const int32_t* chunk_offsets_host, const double* params_host, int T, const int32_t* plan_host,
+                         const double* out_start_host, const double* out_res_host, const double* shifts_host, double collar,
+                         const double* ref_host, const int32_t* ref_label_host, const int32_t* ref_offsets_host,
+                         const int32_t* ref_label_counts_host, double* components_host, int32_t* hyp_offsets_dev,
+                         double* hyp_segments_dev, int hyp_cap, void* stream);
+/* the launch order of the (file, trial) states of dg_sweep_*_files, states_host int32 [num_files * T][2] = {file, trial}:
+ * longest file first (equal chunk counts in file order), then trial.  Host only. */
+int dg_sweep_state_order(int num_files, const int32_t* chunk_offsets_host, int T, int32_t* states_host);
 
 /* ---- device-side audio stream: rearrange_audio_stream (reference src/diart/operators.py:44-100) with the ring buffer in
  *      HBM.  The host pushes every sample ONCE (step_samples new samples per chunk instead of chunk_samples: 8.2 MB
