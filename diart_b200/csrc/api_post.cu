@@ -1,4 +1,5 @@
-// Device post-path (dg_post_*) and the hyper-parameter sweep (dg_sweep_*), which share the turn download.
+// Device post-path (dg_post_*), the hyper-parameter sweep (dg_sweep_*) and the voice activity detection sweep (dg_vad_sweep_*),
+// which share the turn download; the two sweeps share the DER scoring sequence (der_components).
 #include <math.h>
 #include <string.h>
 
@@ -144,10 +145,16 @@ extern "C" int dg_post_step(dg_post* h, const float* seg_dev, const int32_t* map
 // tau_active, rho_update and delta_new by re-running its whole pipeline per trial (Optimizer.objective -> Benchmark), although
 // none of the three reaches the networks.  Clustering: one CTA per state (cluster.cu); post-path: one CTA per (chunk, state)
 // over all chunks at once, without history (post.cu).
+
+// the device buffers of der_components: chunk times and reference in, hypothesis offsets and segments, components out
+struct DerBufs {
+  DevBuf in, hoff, hseg, comp;
+};
+
 struct dg_sweep {
   int device = 0, M = 0, D = 0, F = 0, K = 0, nw = 1;
   DevBuf hamming, in, centers, active, init, prep, prep_d, maps, header, turns, total;
-  DevBuf score_in, hoff, hseg, comp;   // dg_sweep_score: chunk times and reference, hypothesis segments, components
+  DerBufs der;                    // dg_sweep_score
   PinnedBuf pin;                  // params, taus and plan in; error flags, header, total and a turn prefix out
 };
 
@@ -177,6 +184,20 @@ extern "C" int dg_sweep_destroy(dg_sweep* h) {
 // numbers its threads in int32
 static const long long DG_SWEEP_MAX_STATES = 1LL << 21;
 
+// chunk offsets [nf + 1] of N chunks: from 0 to N, every file with a chunk
+static int check_chunk_offsets(const char* who, int N, int nf, const int32_t* chunk_off) {
+  if (chunk_off[0] != 0 || chunk_off[nf] != N) {
+    set_error(std::string(who) + ": chunk offsets must start at 0 and end at N");
+    return DG_EINVAL;
+  }
+  for (int f = 0; f < nf; f++)
+    if (chunk_off[f + 1] <= chunk_off[f]) {
+      set_error(std::string(who) + ": file " + std::to_string(f) + " has no chunks (offsets must increase)");
+      return DG_EINVAL;
+    }
+  return DG_OK;
+}
+
 // the argument checks dg_sweep_run(_files) and dg_sweep_score(_files) share (before any launch); chunk_off [nf + 1] splits
 // the N chunks into the files' ranges
 static int sweep_check(const char* who, dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int nf,
@@ -190,15 +211,8 @@ static int sweep_check(const char* who, dg_sweep* h, const float* seg_dev, const
               std::to_string(DG_SWEEP_MAX_STATES) + " per call");
     return DG_EINVAL;
   }
-  if (chunk_off[0] != 0 || chunk_off[nf] != N) {
-    set_error(std::string(who) + ": chunk offsets must start at 0 and end at N");
-    return DG_EINVAL;
-  }
-  for (int f = 0; f < nf; f++)
-    if (chunk_off[f + 1] <= chunk_off[f]) {
-      set_error(std::string(who) + ": file " + std::to_string(f) + " has no chunks (offsets must increase)");
-      return DG_EINVAL;
-    }
+  int rc;
+  if ((rc = check_chunk_offsets(who, N, nf, chunk_off))) return rc;
   for (int i = 0; i < 3 * T; i++)
     if (!std::isfinite(params_host[i])) {
       set_error(std::string(who) + ": trial " + std::to_string(i / 3) + " has a parameter that is not finite");
@@ -382,6 +396,78 @@ static int sweep_check_reference(const char* who, const double* ref_host, const 
   return DG_OK;
 }
 
+// The der_hyp -> der_scan -> der_score sequence over a post-path result already on the device (header [T][N][4] and `total`
+// turns, M labels): the DER components comp [nf][T][5] of every (file, trial) against the file's reference rows
+// [ref_off[f], ref_off[f + 1]) with R[f] labels, the arguments checked by the caller.  Uses the pinned buffer `pinbuf`;
+// synchronises `st`.
+static int der_components(const char* who, DerBufs& b, PinnedBuf& pinbuf, const int32_t* header_dev, const uint32_t* turns_dev,
+                          unsigned int total, int N, int nf, const int32_t* chunk_off, int T, int M,
+                          const double* out_start_host, const double* out_res_host, const double* shift_host, double collar,
+                          const double* ref_host, const int32_t* ref_label_host, const int32_t* ref_off, const int32_t* R_host,
+                          double* components_host, int32_t* hyp_offsets_dev, double* hyp_segments_dev, int hyp_cap,
+                          cudaStream_t st) {
+  int rc;
+  const int NTM = nf * T * M, S = ref_off[nf];
+  // host -> device, one copy: out_start [N], out_res [N], shifts [nf], reference segments [S][2] grouped by label within each
+  // file, label offsets [nf][DER_ROFF], label counts [nf], chunk offsets [nf + 1]
+  const size_t times_b = (size_t)N * 16, shift_b = (size_t)nf * 8, rseg_b = (size_t)S * 16;
+  const size_t roff_b = (size_t)nf * DER_ROFF * 4, R_b = (size_t)nf * 4, off_b = (size_t)(nf + 1) * 4;
+  const size_t in_b = times_b + shift_b + rseg_b + roff_b + R_b + off_b, comp_b = (size_t)nf * T * 40;
+  if (b.in.ensure(in_b) || b.hoff.ensure((size_t)(NTM + 1) * 4) || b.hseg.ensure((size_t)std::max(total, 1u) * 16) ||
+      b.comp.ensure(comp_b) || pinbuf.ensure(std::max(in_b, comp_b + 16)))
+    return DG_ECUDA;
+  unsigned char* pin = pinbuf.as<unsigned char>();
+  memcpy(pin, out_start_host, (size_t)N * 8);
+  memcpy(pin + (size_t)N * 8, out_res_host, (size_t)N * 8);
+  memcpy(pin + times_b, shift_host, shift_b);
+  double* rseg = reinterpret_cast<double*>(pin + times_b + shift_b);
+  int32_t* roff_all = reinterpret_cast<int32_t*>(pin + times_b + shift_b + rseg_b);
+  memcpy(pin + times_b + shift_b + rseg_b + roff_b, R_host, R_b);
+  memcpy(pin + times_b + shift_b + rseg_b + roff_b + R_b, chunk_off, off_b);
+  for (int f = 0; f < nf; f++) {
+    const int a = ref_off[f], n = ref_off[f + 1] - a, R = R_host[f];
+    int32_t* roff = roff_all + (size_t)f * DER_ROFF;
+    for (int r = 0; r < DER_ROFF; r++) roff[r] = 0;
+    for (int i = 0; i < n; i++) roff[ref_label_host[a + i] + 1]++;
+    roff[0] = a;
+    for (int r = 0; r < R; r++) roff[r + 1] += roff[r];
+    int fill[32];
+    for (int r = 0; r < R; r++) fill[r] = roff[r];
+    for (int i = 0; i < n; i++) {     // stable: each label keeps its rows' order
+      const int o = fill[ref_label_host[a + i]]++;
+      rseg[2 * (size_t)o] = ref_host[2 * (size_t)(a + i)];
+      rseg[2 * (size_t)o + 1] = ref_host[2 * (size_t)(a + i) + 1];
+    }
+  }
+  unsigned char* din = b.in.as<unsigned char>();
+  DG_CUDA(cudaMemcpyAsync(din, pin, in_b, cudaMemcpyHostToDevice, st));
+  const double* d_start = reinterpret_cast<const double*>(din);
+  const double* d_res = d_start + N;
+  const double* d_shift = reinterpret_cast<const double*>(din + times_b);
+  const double* d_rseg = reinterpret_cast<const double*>(din + times_b + shift_b);
+  const int* d_roff = reinterpret_cast<const int*>(din + times_b + shift_b + rseg_b);
+  const int* d_R = reinterpret_cast<const int*>(din + times_b + shift_b + rseg_b + roff_b);
+  const int* d_off = reinterpret_cast<const int*>(din + times_b + shift_b + rseg_b + roff_b + R_b);
+  int* hoff = b.hoff.as<int>();
+  if ((rc = launch_der_hyp_count(header_dev, turns_dev, nf, d_off, T, N, M, d_start, d_res, d_shift, collar, hoff, st)) ||
+      (rc = launch_der_hyp_write(header_dev, turns_dev, nf, d_off, T, N, M, d_start, d_res, d_shift, collar, hoff,
+                                 b.hseg.as<double>(), hyp_segments_dev, hyp_cap, st)) ||
+      (rc = launch_der_score(hoff, b.hseg.as<double>(), nf, T, M, d_roff, d_R, d_rseg, b.comp.as<double>(), st)))
+    return rc;
+  if (hyp_offsets_dev) DG_CUDA(cudaMemcpyAsync(hyp_offsets_dev, hoff, (size_t)(NTM + 1) * 4, cudaMemcpyDeviceToDevice, st));
+  DG_CUDA(cudaMemcpyAsync(pin, b.comp.p, comp_b, cudaMemcpyDeviceToHost, st));
+  DG_CUDA(cudaMemcpyAsync(pin + comp_b, hoff + NTM, 4, cudaMemcpyDeviceToHost, st));
+  DG_CUDA(cudaStreamSynchronize(st));
+  memcpy(components_host, pin, comp_b);
+  int n_seg = 0;
+  memcpy(&n_seg, pin + comp_b, 4);
+  if (hyp_segments_dev && n_seg > hyp_cap) {
+    set_error(std::string(who) + ": hypothesis segment buffer too small (" + std::to_string(n_seg) + " segments)");
+    return DG_EINVAL;
+  }
+  return DG_OK;
+}
+
 // dg_sweep_score(_files): the clustering and post-path of sweep_cluster_post, then the DER components of every (file, trial)
 // against the file's reference rows [ref_off[f], ref_off[f + 1]) with R[f] labels
 static int sweep_score(const char* who, dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int nf,
@@ -432,66 +518,9 @@ static int sweep_score(const char* who, dg_sweep* h, const float* seg_dev, const
   if ((rc = sweep_cluster_post(h, seg_dev, emb_dev, N, nf, chunk_off, params_host, T, plan_host, nullptr, nullptr, false, st,
                                &total)))
     return rc;
-  const int M = h->M, NTM = nf * T * M;
-  // host -> device, one copy: out_start [N], out_res [N], shifts [nf], reference segments [S][2] grouped by label within each
-  // file, label offsets [nf][DER_ROFF], label counts [nf], chunk offsets [nf + 1]
-  const size_t times_b = (size_t)N * 16, shift_b = (size_t)nf * 8, rseg_b = (size_t)S * 16;
-  const size_t roff_b = (size_t)nf * DER_ROFF * 4, R_b = (size_t)nf * 4, off_b = (size_t)(nf + 1) * 4;
-  const size_t in_b = times_b + shift_b + rseg_b + roff_b + R_b + off_b, comp_b = (size_t)nf * T * 40;
-  if (h->score_in.ensure(in_b) || h->hoff.ensure((size_t)(NTM + 1) * 4) || h->hseg.ensure((size_t)std::max(total, 1u) * 16) ||
-      h->comp.ensure(comp_b) || h->pin.ensure(std::max(in_b, comp_b + 16)))
-    return DG_ECUDA;
-  unsigned char* pin = h->pin.as<unsigned char>();
-  memcpy(pin, out_start_host, (size_t)N * 8);
-  memcpy(pin + (size_t)N * 8, out_res_host, (size_t)N * 8);
-  memcpy(pin + times_b, shift_host, shift_b);
-  double* rseg = reinterpret_cast<double*>(pin + times_b + shift_b);
-  int32_t* roff_all = reinterpret_cast<int32_t*>(pin + times_b + shift_b + rseg_b);
-  memcpy(pin + times_b + shift_b + rseg_b + roff_b, R_host, R_b);
-  memcpy(pin + times_b + shift_b + rseg_b + roff_b + R_b, chunk_off, off_b);
-  for (int f = 0; f < nf; f++) {
-    const int a = ref_off[f], n = ref_off[f + 1] - a, R = R_host[f];
-    int32_t* roff = roff_all + (size_t)f * DER_ROFF;
-    for (int r = 0; r < DER_ROFF; r++) roff[r] = 0;
-    for (int i = 0; i < n; i++) roff[ref_label_host[a + i] + 1]++;
-    roff[0] = a;
-    for (int r = 0; r < R; r++) roff[r + 1] += roff[r];
-    int fill[32];
-    for (int r = 0; r < R; r++) fill[r] = roff[r];
-    for (int i = 0; i < n; i++) {     // stable: each label keeps its rows' order
-      const int o = fill[ref_label_host[a + i]]++;
-      rseg[2 * (size_t)o] = ref_host[2 * (size_t)(a + i)];
-      rseg[2 * (size_t)o + 1] = ref_host[2 * (size_t)(a + i) + 1];
-    }
-  }
-  unsigned char* din = h->score_in.as<unsigned char>();
-  DG_CUDA(cudaMemcpyAsync(din, pin, in_b, cudaMemcpyHostToDevice, st));
-  const double* d_start = reinterpret_cast<const double*>(din);
-  const double* d_res = d_start + N;
-  const double* d_shift = reinterpret_cast<const double*>(din + times_b);
-  const double* d_rseg = reinterpret_cast<const double*>(din + times_b + shift_b);
-  const int* d_roff = reinterpret_cast<const int*>(din + times_b + shift_b + rseg_b);
-  const int* d_R = reinterpret_cast<const int*>(din + times_b + shift_b + rseg_b + roff_b);
-  const int* d_off = reinterpret_cast<const int*>(din + times_b + shift_b + rseg_b + roff_b + R_b);
-  int* hoff = h->hoff.as<int>();
-  if ((rc = launch_der_hyp_count(h->header.as<int32_t>(), h->turns.as<uint32_t>(), nf, d_off, T, N, M, d_start, d_res, d_shift,
-                                 collar, hoff, st)) ||
-      (rc = launch_der_hyp_write(h->header.as<int32_t>(), h->turns.as<uint32_t>(), nf, d_off, T, N, M, d_start, d_res, d_shift,
-                                 collar, hoff, h->hseg.as<double>(), hyp_segments_dev, hyp_cap, st)) ||
-      (rc = launch_der_score(hoff, h->hseg.as<double>(), nf, T, M, d_roff, d_R, d_rseg, h->comp.as<double>(), st)))
-    return rc;
-  if (hyp_offsets_dev) DG_CUDA(cudaMemcpyAsync(hyp_offsets_dev, hoff, (size_t)(NTM + 1) * 4, cudaMemcpyDeviceToDevice, st));
-  DG_CUDA(cudaMemcpyAsync(pin, h->comp.p, comp_b, cudaMemcpyDeviceToHost, st));
-  DG_CUDA(cudaMemcpyAsync(pin + comp_b, hoff + NTM, 4, cudaMemcpyDeviceToHost, st));
-  DG_CUDA(cudaStreamSynchronize(st));
-  memcpy(components_host, pin, comp_b);
-  int n_seg = 0;
-  memcpy(&n_seg, pin + comp_b, 4);
-  if (hyp_segments_dev && n_seg > hyp_cap) {
-    set_error(std::string(who) + ": hypothesis segment buffer too small (" + std::to_string(n_seg) + " segments)");
-    return DG_EINVAL;
-  }
-  return DG_OK;
+  return der_components(who, h->der, h->pin, h->header.as<int32_t>(), h->turns.as<uint32_t>(), total, N, nf, chunk_off, T,
+                        h->M, out_start_host, out_res_host, shift_host, collar, ref_host, ref_label_host, ref_off, R_host,
+                        components_host, hyp_offsets_dev, hyp_segments_dev, hyp_cap, st);
 }
 
 extern "C" int dg_sweep_score(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, const double* params_host,
@@ -515,4 +544,235 @@ extern "C" int dg_sweep_score_files(dg_sweep* h, const float* seg_dev, const flo
   return sweep_score("dg_sweep_score_files", h, seg_dev, emb_dev, N, num_files, chunk_offsets_host, params_host, T, plan_host,
                      out_start_host, out_res_host, shifts_host, collar, ref_host, ref_label_host, ref_offsets_host,
                      ref_label_counts_host, components_host, hyp_offsets_dev, hyp_segments_dev, hyp_cap, stream);
+}
+
+// ============================================================================= voice activity detection sweep
+// tau_active trials of VoiceActivityDetection over a dataset: the speech curve of every chunk is computed once (vad_curve) and
+// kept on the device; each trial then only thresholds it (vad_binarize).  Scoring merges every (file, trial)'s turns into
+// whole-file segments and walks them against the file's speech reference with the DER kernels (der_components, M = 1, at
+// most one reference label): with one label per side their false alarm and missed detection are DetectionErrorRate's.
+struct dg_vad_sweep {
+  int device = 0, F = 0, K = 0, nw = 1;
+  int N = 0, nf = 0;                     // chunks and files of the curve; 0 until dg_vad_sweep_curve
+  std::vector<int32_t> chunk_off;        // [nf + 1]
+  DevBuf hamming, in, curve, header, turns, total, taus;
+  DerBufs der;
+  PinnedBuf pin;
+};
+
+extern "C" int dg_vad_sweep_create(int frames, int local_speakers, int num_windows, const double* hamming_host, int device,
+                                   dg_vad_sweep** out) {
+  if (!out || !hamming_host || frames < 1 || frames > 1023 || local_speakers < 1 || local_speakers > 64 || num_windows < 1 ||
+      num_windows > 256) {
+    set_error("dg_vad_sweep_create: need 1 <= frames <= 1023, 1 <= local_speakers <= 64, 1 <= num_windows <= 256");
+    return DG_EINVAL;
+  }
+  DG_CUDA(cudaSetDevice(device));
+  std::unique_ptr<dg_vad_sweep> h(new dg_vad_sweep());
+  h->device = device; h->F = frames; h->K = local_speakers; h->nw = num_windows;
+  if (h->hamming.ensure((size_t)frames * 8) || h->total.ensure(16)) return DG_ECUDA;
+  DG_CUDA(cudaMemcpy(h->hamming.p, hamming_host, (size_t)frames * 8, cudaMemcpyHostToDevice));
+  *out = h.release();
+  return DG_OK;
+}
+
+extern "C" int dg_vad_sweep_destroy(dg_vad_sweep* h) {
+  delete h;
+  return DG_OK;
+}
+
+extern "C" int dg_vad_sweep_curve(dg_vad_sweep* h, const float* seg_dev, int N, int num_files,
+                                  const int32_t* chunk_offsets_host, const int32_t* plan_host, void* stream) {
+  const char* who = "dg_vad_sweep_curve";
+  if (!h || !seg_dev || !plan_host || !chunk_offsets_host || N < 1 || num_files < 1) {
+    set_error(std::string(who) + ": bad arguments (need N >= 1, num_files >= 1, non-null buffers)");
+    return DG_EINVAL;
+  }
+  int rc;
+  if ((rc = check_chunk_offsets(who, N, num_files, chunk_offsets_host))) return rc;
+  const int stride = 4 + h->nw;
+  // the curve's offsets, and the plan rows post.cu would accept for a fresh stream per file: 1 <= nb <= nw buffers, none
+  // before the file's first chunk, 1 <= frames <= 1023 (the 10-bit frame fields of a turn)
+  std::vector<long long> off(N + 1);
+  off[0] = 0;
+  for (int f = 0, c = 0; f < num_files; f++)
+    for (; c < chunk_offsets_host[f + 1]; c++) {
+      const int32_t* pl = plan_host + (size_t)c * stride;
+      const int nb = pl[0], nf = pl[1], nfo = pl[2] > 0 ? pl[2] : nf;
+      if (nb < 1 || nb > h->nw || nb - 1 > c - chunk_offsets_host[f] || nf < 1 || pl[2] < 0 || nfo > 1023) {
+        set_error(std::string(who) + ": plan row " + std::to_string(c) + " is not a plan of its file (buffers " +
+                  std::to_string(nb) + ", frames " + std::to_string(nfo) + ")");
+        return DG_EINVAL;
+      }
+      off[c + 1] = off[c] + nfo;
+    }
+  DG_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  // host -> device, one copy: curve offsets [N + 1] (int64), plan [N][stride]
+  const size_t off_b = (size_t)(N + 1) * 8, plan_b = (size_t)N * stride * 4;
+  if (h->in.ensure(off_b + plan_b) || h->curve.ensure((size_t)off[N] * 8) || h->pin.ensure(off_b + plan_b)) return DG_ECUDA;
+  unsigned char* pin = h->pin.as<unsigned char>();
+  memcpy(pin, off.data(), off_b);
+  memcpy(pin + off_b, plan_host, plan_b);
+  unsigned char* din = h->in.as<unsigned char>();
+  DG_CUDA(cudaMemcpyAsync(din, pin, off_b + plan_b, cudaMemcpyHostToDevice, st));
+  h->N = 0;   // no curve while it is being replaced
+  if ((rc = launch_vad_curve(seg_dev, N, h->F, h->K, reinterpret_cast<const int32_t*>(din + off_b), stride,
+                             h->hamming.as<double>(), reinterpret_cast<const long long*>(din), h->curve.as<double>(), st)))
+    return rc;
+  DG_CUDA(cudaStreamSynchronize(st));
+  h->N = N;
+  h->nf = num_files;
+  h->chunk_off.assign(chunk_offsets_host, chunk_offsets_host + num_files + 1);
+  return DG_OK;
+}
+
+// the argument checks of dg_vad_sweep_run_files / _score_files (before any launch)
+static int vad_check(const char* who, dg_vad_sweep* h, const double* taus_host, int T) {
+  if (!h || !taus_host || T < 1 || T > 65535) {
+    set_error(std::string(who) + ": bad arguments (need 1 <= T <= 65535, non-null buffers)");
+    return DG_EINVAL;
+  }
+  if (h->N < 1) {
+    set_error(std::string(who) + ": no speech curve (dg_vad_sweep_curve first)");
+    return DG_EINVAL;
+  }
+  if ((long long)h->nf * T > DG_SWEEP_MAX_STATES) {
+    set_error(std::string(who) + ": " + std::to_string((long long)h->nf * T) + " (file, trial) states; at most " +
+              std::to_string(DG_SWEEP_MAX_STATES) + " per call");
+    return DG_EINVAL;
+  }
+  for (int t = 0; t < T; t++)
+    if (!std::isfinite(taus_host[t])) {
+      set_error(std::string(who) + ": the tau_active of trial " + std::to_string(t) + " is not finite");
+      return DG_EINVAL;
+    }
+  return DG_OK;
+}
+
+// pinned layout of vad_binarize_all: taus [T] in; header [T][N][4], turn count, turn prefix out
+static TurnOut vad_out(int T, int N) { return {(size_t)T * 8, (size_t)T * N * 16}; }
+
+// the turns of T thresholds over the curve: header [T][N][4] and turns stay on the device, the count comes back in *total.
+// with_header: the header and a turn prefix travel to the pinned buffer with the count (vad_out layout).  Synchronises `st`.
+static int vad_binarize_all(dg_vad_sweep* h, const double* taus_host, int T, bool with_header, cudaStream_t st,
+                            unsigned int* total_out) {
+  const int N = h->N;
+  const TurnOut lay = vad_out(T, N);
+  const size_t turn_guess = std::max<size_t>((size_t)T * N * 4, (size_t)DG_POST_PREFIX);
+  if (h->taus.ensure((size_t)T * 8) || h->header.ensure(lay.header_bytes) || h->turns.ensure(turn_guess * 4) ||
+      h->pin.ensure(lay.end()))
+    return DG_ECUDA;
+  unsigned char* pin = h->pin.as<unsigned char>();
+  memcpy(pin, taus_host, (size_t)T * 8);
+  DG_CUDA(cudaMemcpyAsync(h->taus.p, pin, (size_t)T * 8, cudaMemcpyHostToDevice, st));
+  const long long* d_off = reinterpret_cast<const long long*>(h->in.p);
+  unsigned int total = 0;
+  for (int attempt = 0; attempt < 2; attempt++) {
+    const int cap = (int)std::min<size_t>(h->turns.bytes / 4, (size_t)INT32_MAX);
+    DG_CUDA(cudaMemsetAsync(h->total.p, 0, 4, st));
+    int rc;
+    if ((rc = launch_vad_binarize(h->curve.as<double>(), d_off, N, T, h->taus.as<double>(), h->header.as<int32_t>(),
+                                  h->turns.as<uint32_t>(), cap, h->total.as<unsigned int>(), st)))
+      return rc;
+    if (with_header) DG_CUDA(cudaMemcpyAsync(pin + lay.at, h->header.p, lay.header_bytes, cudaMemcpyDeviceToHost, st));
+    DG_CUDA(cudaMemcpyAsync(pin + lay.total(), h->total.p, 4, cudaMemcpyDeviceToHost, st));
+    if (with_header)
+      DG_CUDA(cudaMemcpyAsync(pin + lay.prefix(), h->turns.p, (size_t)std::min(DG_POST_PREFIX, cap) * 4,
+                              cudaMemcpyDeviceToHost, st));
+    DG_CUDA(cudaStreamSynchronize(st));
+    memcpy(&total, pin + lay.total(), 4);
+    if (total <= (unsigned int)cap) break;
+    // more turns than the device buffer holds: grow it to the count and binarise again
+    if (h->turns.ensure((size_t)total * 4)) return DG_ECUDA;
+  }
+  *total_out = total;
+  return DG_OK;
+}
+
+extern "C" int dg_vad_sweep_run_files(dg_vad_sweep* h, const double* taus_host, int T, int32_t* header_host,
+                                      uint32_t* turns_host, int turn_cap_host, int* n_turns, void* stream) {
+  const char* who = "dg_vad_sweep_run_files";
+  int rc;
+  if ((rc = vad_check(who, h, taus_host, T))) return rc;
+  if (!header_host || !turns_host) {
+    set_error(std::string(who) + ": bad arguments (need non-null header and turn buffers)");
+    return DG_EINVAL;
+  }
+  DG_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned int total = 0;
+  if ((rc = vad_binarize_all(h, taus_host, T, true, st, &total))) return rc;
+  return download_turns(who, h->pin.as<unsigned char>(), vad_out(T, h->N), h->turns.as<uint32_t>(), header_host, turns_host,
+                        turn_cap_host, n_turns, st);
+}
+
+extern "C" int dg_vad_sweep_score_files(dg_vad_sweep* h, const double* taus_host, int T, const double* out_start_host,
+                                        const double* out_res_host, const double* shifts_host, double collar,
+                                        const double* ref_host, const int32_t* ref_offsets_host, double* components_host,
+                                        void* stream) {
+  const char* who = "dg_vad_sweep_score_files";
+  int rc;
+  if ((rc = vad_check(who, h, taus_host, T))) return rc;
+  const int N = h->N, nf = h->nf;
+  if (!out_start_host || !out_res_host || !shifts_host || !components_host || !ref_offsets_host || !std::isfinite(collar) ||
+      collar < 0) {
+    set_error(std::string(who) + ": bad arguments (need chunk times, shifts, reference offsets, a components buffer, finite "
+              "collar >= 0)");
+    return DG_EINVAL;
+  }
+  for (int f = 0; f < nf; f++)
+    if (!std::isfinite(shifts_host[f])) {
+      set_error(std::string(who) + ": the shift of file " + std::to_string(f) + " is not finite");
+      return DG_EINVAL;
+    }
+  for (int c = 0; c < N; c++)
+    if (!std::isfinite(out_start_host[c]) || !std::isfinite(out_res_host[c])) {
+      set_error(std::string(who) + ": chunk " + std::to_string(c) + " has an output time that is not finite");
+      return DG_EINVAL;
+    }
+  if (ref_offsets_host[0] != 0) {
+    set_error(std::string(who) + ": reference row offsets must start at 0");
+    return DG_EINVAL;
+  }
+  for (int f = 0; f < nf; f++)
+    if (ref_offsets_host[f + 1] < ref_offsets_host[f]) {
+      set_error(std::string(who) + ": reference row offsets of file " + std::to_string(f) + " decrease");
+      return DG_EINVAL;
+    }
+  const int S = ref_offsets_host[nf];
+  if (S > 0 && !ref_host) {
+    set_error(std::string(who) + ": non-null reference rows needed for " + std::to_string(S) + " rows");
+    return DG_EINVAL;
+  }
+  // each file's reference is one label: its rows are a support (Timeline.support), finite, in time order, apart by more than
+  // 1e-6 s (a gap that is a falsy Segment would have been merged)
+  const std::vector<int32_t> labels((size_t)std::max(S, 1), 0);
+  std::vector<int32_t> R(nf);
+  for (int f = 0; f < nf; f++) {
+    const int a = ref_offsets_host[f], n = ref_offsets_host[f + 1] - a;
+    R[f] = n > 0 ? 1 : 0;
+    if ((rc = sweep_check_reference(who, n > 0 ? ref_host + 2 * (size_t)a : nullptr, n > 0 ? labels.data() : nullptr, n, R[f])))
+      return rc;
+    for (int i = a + 1; i < a + n; i++)
+      if (!(ref_host[2 * (size_t)i] - ref_host[2 * (size_t)i - 1] > 1e-6)) {
+        set_error(std::string(who) + ": reference row " + std::to_string(i - a) + " of file " + std::to_string(f) +
+                  " is not more than 1e-6 s after the previous one (the rows must be a support)");
+        return DG_EINVAL;
+      }
+  }
+  DG_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned int total = 0;
+  if ((rc = vad_binarize_all(h, taus_host, T, false, st, &total))) return rc;
+  std::vector<double> comp((size_t)nf * T * 5);
+  if ((rc = der_components(who, h->der, h->pin, h->header.as<int32_t>(), h->turns.as<uint32_t>(), total, N, nf,
+                           h->chunk_off.data(), T, 1, out_start_host, out_res_host, shifts_host, collar, ref_host,
+                           labels.data(), ref_offsets_host, R.data(), comp.data(), nullptr, nullptr, 0, st)))
+    return rc;
+  for (size_t i = 0; i < (size_t)nf * T; i++) {
+    components_host[2 * i] = comp[5 * i];           // false alarm
+    components_host[2 * i + 1] = comp[5 * i + 1];   // missed detection
+  }
+  return DG_OK;
 }

@@ -284,6 +284,12 @@ int launch_der_hyp_write(const int32_t* header, const uint32_t* turns, int nf, c
 constexpr int DER_ROFF = 33;
 int launch_der_score(const int* hoff, const double* hseg, int nf, int T, int M, const int* roff, const int* R,
                      const double* rseg, double* comp, cudaStream_t st);
+// vad.cu -- VAD sweep: the speech curve of N chunks (max over K local speakers, aggregated as launch_post with one speaker;
+// chunk c's frames at curve [curve_off[c], curve_off[c + 1])), then per trial t the turns of curve > taus[t], header [T][N][4]
+int launch_vad_curve(const float* seg, int N, int F, int K, const int32_t* plan, int plan_stride, const double* hamming,
+                     const long long* curve_off, double* curve, cudaStream_t st);
+int launch_vad_binarize(const double* curve, const long long* curve_off, int N, int T, const double* taus, int32_t* header,
+                        uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st);
 // resample.cu -- polyphase sinc resampling (torchaudio's defaults): reduced ratio o / n, half-width w, T = 2w + o taps per phase
 struct RsGeom {
   int o, n, w, T;

@@ -20,6 +20,7 @@
 // turns of all states share one counter; each state's headers locate its turns.  STATES = false compiles the single-state
 // form of the pipeline.
 #include "dg_common.cuh"
+#include "post_agg.cuh"
 
 namespace dg {
 
@@ -70,27 +71,10 @@ post_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map, cons
   __syncthreads();
   for (int i = threadIdx.x; i < nfo * M; i += POST_THREADS) {
     const int fo = i / M, g = i - fo * M;
-    double v;
-    const int fa = fo - (nfo - nf);          // frame of the aggregated part
-    if (fa < 0) {                             // prepended part of the very first buffer: raw permuted scores
-      int idx = first_lo + fo;
-      idx = idx < 0 ? 0 : (idx > F - 1 ? F - 1 : idx);
-      const int k = inv[g];
-      v = k >= 0 ? (double)buf_seg(0)[(size_t)idx * K + k] : 0.0;
-    } else {
-      double num = 0.0, den = 0.0;
-      for (int j = 0; j < nb; j++) {
-        int idx = pl[4 + j] + fa;
-        idx = idx < 0 ? 0 : (idx > F - 1 ? F - 1 : idx);    // `fixed` crops are edge-padded
-        const int k = inv[j * M + g];
-        const double val = k >= 0 ? (double)buf_seg(j)[(size_t)idx * K + k] : 0.0;
-        const double h = hamming[idx];
-        const double p = __dmul_rn(h, val);
-        num = j ? __dadd_rn(num, p) : p;
-        den = j ? __dadd_rn(den, h) : h;
-      }
-      v = __ddiv_rn(num, den);
-    }
+    const double v = post_frame(pl, nb, nf, nfo, first_lo, F, hamming, fo, [&](int j, int idx) {
+      const int k = inv[j * M + g];
+      return k >= 0 ? (double)buf_seg(j)[(size_t)idx * K + k] : 0.0;
+    });
     act[i] = v > tau ? 1 : 0;
   }
   __syncthreads();

@@ -23,6 +23,11 @@ files: its ``total.der`` is the value ``Optimizer.objective`` minimises.
 flow, and its outputs stay on the device; every ``score`` / ``run`` call then clusters, post-processes and scores all
 (file, trial) pairs in one launch per kernel (``dg_sweep_score_files`` / ``dg_sweep_run_files``), without running a network
 kernel again.
+
+:class:`VoiceActivitySweep` does it for ``VoiceActivityDetection``, whose one hyper-parameter, ``tau_active``, is read by
+``Binarize`` alone: the segmentation runs once per dataset, the aggregated speech curve is computed once per chunk
+(``dg_vad_sweep_curve``, ``csrc/vad.cu``), and every trial only thresholds it and is scored by detection error rate
+(``DetectionErrorRate(collar=0, skip_overlap=False)``, the pipeline's ``suggest_metric()``; DESIGN.md "Detection error").
 """
 from __future__ import annotations
 
@@ -37,7 +42,9 @@ import torch
 from . import _lib
 from .blocks.diarization import SpeakerDiarization, SpeakerDiarizationConfig
 from .blocks.post import post_plan, turn_times
+from .blocks.vad import VoiceActivityDetection, VoiceActivityDetectionConfig
 from .core import Annotation, Segment
+from .models import B200PyanNet
 from .operators import DeviceAudioStream
 
 NETWORK_BATCH = 256           # windows per network step (the benchmarked batch)
@@ -47,11 +54,12 @@ PATCH_COLLAR = 0.05           # PredictionAccumulator's default (sinks.py)
 MAX_REFERENCE_LABELS = 32     # one lane per reference label in the scoring kernel
 
 
-def trial_params(trials: Sequence[Mapping[str, float]], config: SpeakerDiarizationConfig) -> np.ndarray:
-    """trials (dicts keyed by the reference's HyperParameter names) -> float64 (T, 3) {tau_active, rho_update, delta_new};
-    a missing key takes the config's value.  Other keys (gamma, beta, latency, step, max_speakers, ...) change the network
-    pass or the plan and cannot vary within one sweep: ValueError."""
-    names = [hp.name for hp in SpeakerDiarization.hyper_parameters()]
+def trial_params(trials: Sequence[Mapping[str, float]], config, names: Optional[Sequence[str]] = None) -> np.ndarray:
+    """trials (dicts keyed by the reference's HyperParameter names) -> float64 (T, len(names)), by default names =
+    {tau_active, rho_update, delta_new} (``SpeakerDiarization.hyper_parameters()``); a missing key takes the config's value.
+    Other keys (gamma, beta, latency, step, max_speakers, ...) change the network pass or the plan and cannot vary within
+    one sweep: ValueError."""
+    names = list(names) if names is not None else [hp.name for hp in SpeakerDiarization.hyper_parameters()]
     trials = list(trials)
     if not trials:
         raise ValueError("at least one trial is needed")
@@ -656,6 +664,256 @@ class DatasetSweep:
                 comp[:, g] = part
         self.timing["score"] = dev
         per_file = [DERComponents.from_array(comp[f]) for f in range(nf)]
+        total = per_file[0]
+        for c in per_file[1:]:
+            total = total + c
+        return per_file, total
+
+
+VAD_PARAMS = tuple(hp.name for hp in VoiceActivityDetection.hyper_parameters())   # ("tau_active",)
+
+
+@dataclass
+class DetectionErrorComponents:
+    """Detection error rate components in seconds, one entry per trial (float64 (T,) each)."""
+    false_alarm: np.ndarray
+    missed_detection: np.ndarray
+    total: np.ndarray
+
+    def as_array(self) -> np.ndarray:
+        """(T, 3) {false alarm, missed detection, total}"""
+        return np.stack([self.false_alarm, self.missed_detection, self.total], axis=1)
+
+    @property
+    def detection_error_rate(self) -> np.ndarray:
+        """(false alarm + missed detection) / total per trial, as a fraction; with total = 0: 0 when there is no error,
+        else 1 (pyannote's DetectionErrorRate.compute_metric)"""
+        num = self.false_alarm + self.missed_detection
+        safe = np.where(self.total > 0, self.total, 1.0)
+        return np.where(self.total > 0, num / safe, np.where(num > 0, 1.0, 0.0))
+
+    def __add__(self, other: "DetectionErrorComponents") -> "DetectionErrorComponents":
+        """the components of several files summed per trial"""
+        return DetectionErrorComponents(self.false_alarm + other.false_alarm,
+                                        self.missed_detection + other.missed_detection, self.total + other.total)
+
+
+def speech_reference(annotation: Annotation) -> Tuple[np.ndarray, float]:
+    """A reference annotation -> (rows float64 (S, 2), total): the support of all its segments, whatever their labels
+    (``annotation.get_timeline().support()``): non-empty segments in (start, end) order, a segment merged into the current
+    row when ``Segment(row end, its start)`` is falsy (it overlaps, touches or follows by at most 1e-6 s).  ``total`` is the
+    rows' durations summed in order, pyannote's ``reference.duration()``."""
+    rows: List[List[float]] = []
+    for a, b in sorted((s.start, s.end) for s, _ in annotation.itertracks() if s):
+        if rows and not (a - rows[-1][1] > 1e-6):
+            rows[-1][1] = max(rows[-1][1], b)
+        else:
+            rows.append([a, b])
+    total = 0.0
+    for a, b in rows:
+        total += b - a
+    return np.array(rows, dtype=np.float64).reshape(-1, 2), total
+
+
+def pack_speech_references(references: Sequence[Annotation]):
+    """per-file references -> the reference arguments of dg_vad_sweep_score_files and the per-file totals: (rows float64
+    (S, 2), row offsets int32 (files + 1,), totals float64 (files,))"""
+    rows, offsets, totals = [], [0], []
+    for ref in references:
+        r, total = speech_reference(ref)
+        rows.append(r)
+        offsets.append(offsets[-1] + len(r))
+        totals.append(total)
+    return (np.ascontiguousarray(np.concatenate(rows), dtype=np.float64), np.array(offsets, dtype=np.int32),
+            np.array(totals, dtype=np.float64))
+
+
+class VoiceActivitySweep:
+    """Tunes ``VoiceActivityDetection``'s ``tau_active`` over a whole dataset with the segmentation run once.
+
+        vs = VoiceActivitySweep(vad_config, [("file1", waveform1, reference1), ("file2", waveform2, reference2)])
+        per_file, total = vs.score([{"tau_active": 0.4}, {"tau_active": 0.55}, {}])
+        best = int(np.argmin(total.detection_error_rate))
+
+    ``files``: (uri, 1-D float32 waveform at ``config.sample_rate``, reference annotation or None).  The constructor runs the
+    segmentation of every file's windows (``DeviceAudioStream`` batches of 256 from the file's window 0, the
+    ``SpeakerSegmentation.forward_device`` call ``VoiceActivityDetection`` makes) as one flow without synchronising, keeps
+    the scores on the device (F K float32 per chunk: 3.5 kB at the default model) and computes the speech curve once
+    (``dg_vad_sweep_curve``: max over the local speakers, Hamming aggregation; 29 float64 per chunk at the defaults).
+    :meth:`score` and :meth:`run` then threshold the curve for every (file, trial) pair in one launch per kernel and per
+    trial group (:func:`trial_groups`), and run no network kernel.  The windows, plans and timestamp shifts are those of
+    :class:`DatasetSweep`.  Needs the native segmentation model (``B200PyanNet``).
+    """
+
+    def __init__(self, config: VoiceActivityDetectionConfig,
+                 files: Iterable[Tuple[Optional[str], np.ndarray, Optional[Annotation]]]):
+        files = list(files)
+        if not files:
+            raise ValueError("at least one file is needed")
+        for i, (uri, x, _) in enumerate(files):
+            if np.asarray(x).size == 0:
+                raise ValueError(f"file {i} ({uri}) has no samples, so no windows")
+        self.config = config
+        self.pipeline = VoiceActivityDetection(config)
+        if not isinstance(getattr(self.pipeline.segmentation.model, "model", None), B200PyanNet):
+            raise _lib.DiartB200Error("VoiceActivitySweep needs the native segmentation model (B200PyanNet)")
+        self.device = self.pipeline.segmentation.device
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.uris = [uri for uri, _, _ in files]
+        self.references = [ref for _, _, ref in files]
+        fws = [file_windows(x, config) for _, x, _ in files]
+        self.offsets = np.ascontiguousarray(np.cumsum([0] + [fw.num_windows for fw in fws]), dtype=np.int32)
+        trial_groups(1, int(self.offsets[-1]))                  # a dataset too large for one launch fails here
+        self._h: Optional[C.c_void_p] = None
+        t0 = time.perf_counter()
+        self.seg = self._segmentation(fws)
+        torch.cuda.synchronize(self.device)
+        t1 = time.perf_counter()
+        N, F, K = self.seg.shape
+        self.plan, self.out_start, self.out_res = dataset_plan(fws, config, F)
+        self.shifts = np.ascontiguousarray([-fw.padding[0] for fw in fws], dtype=np.float64)
+        self.curve_frames = int(np.where(self.plan[:, 2] > 0, self.plan[:, 2], self.plan[:, 1]).sum())
+        ham = np.ascontiguousarray(np.hamming(F), dtype=np.float64)
+        nw = int(round(config.latency / config.step))
+        h = C.c_void_p()
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().dg_vad_sweep_create(F, K, nw, ham.ctypes.data, self.device.index, C.byref(h)))
+            self._h = h
+            _lib.check(_lib.lib().dg_vad_sweep_curve(h, self.seg.data_ptr(), N, len(fws), self.offsets.ctypes.data,
+                                                     self.plan.ctypes.data, _lib.stream_ptr(self.device)))
+        self.timing: Dict[str, float] = {"network": t1 - t0, "curve": time.perf_counter() - t1}
+        self._refs = None
+        self._turns = np.empty(0, dtype=np.uint32)
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None) is not None:
+                _lib.lib().dg_vad_sweep_destroy(self._h)
+        except Exception:  # noqa: BLE001
+            pass
+
+    def _segmentation(self, fws: Sequence[FileWindows]) -> torch.Tensor:
+        """scores (N, F, K) of every window of every file, concatenated in file order, on the device: each file's windows in
+        batches cut at the multiples of 256 from its window 0, so that a file's scores are the bits
+        ``VoiceActivityDetection`` computes for it in batches of 256"""
+        cfg, seg = self.config, self.pipeline.segmentation
+        streams: List[DeviceAudioStream] = []
+        outs = []
+        with torch.cuda.device(self.device):
+            for i, fw in enumerate(fws):
+                # a few streams in turn: a reset waits for the uploads of its stream (see network_pass_files)
+                if len(streams) < _AUDIO_STREAMS:
+                    streams.append(DeviceAudioStream(cfg.duration, cfg.step, cfg.sample_rate, max_windows=NETWORK_BATCH,
+                                                     device=self.device))
+                stream = streams[i % _AUDIO_STREAMS]
+                if i >= _AUDIO_STREAMS:
+                    stream.reset()
+                pushed = fw.offset
+                for i0 in range(0, fw.num_windows, NETWORK_BATCH):
+                    B = min(NETWORK_BATCH, fw.num_windows - i0)
+                    need = fw.offset + (i0 + B - 1) * fw.step_samples + fw.chunk_samples
+                    stream.push(fw.samples[pushed:need])
+                    pushed = need
+                    outs.append(seg.forward_device(stream.windows(B)))
+            return torch.cat(outs)
+
+    @property
+    def num_chunks(self) -> int:
+        return int(self.offsets[-1])
+
+    @property
+    def resident_bytes(self) -> int:
+        """device bytes of the kept scores and speech curve"""
+        return self.seg.numel() * self.seg.element_size() + self.curve_frames * 8
+
+    def file_outputs(self, f: int) -> torch.Tensor:
+        """file f's slice of the resident scores (n, F, K)"""
+        return self.seg[int(self.offsets[f]):int(self.offsets[f + 1])]
+
+    def _taus(self, trials: Sequence[Mapping[str, float]]) -> np.ndarray:
+        return np.ascontiguousarray(trial_params(trials, self.config, VAD_PARAMS)[:, 0])
+
+    def binarize(self, taus: np.ndarray) -> SweepOutputs:
+        """dg_vad_sweep_run_files for thresholds (T,): header (T, N, 4) and turns over the N concatenated chunks"""
+        taus = np.ascontiguousarray(taus, dtype=np.float64)
+        T, N = len(taus), self.num_chunks
+        header = np.empty((T, N, 4), dtype=np.int32)
+        if len(self._turns) < T * N * 4:
+            self._turns = np.empty(T * N * 4, dtype=np.uint32)
+        n = C.c_int()
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream(self.device)
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            for attempt in range(2):
+                e0.record(st)
+                rc = _lib.lib().dg_vad_sweep_run_files(self._h, taus.ctypes.data, T, header.ctypes.data,
+                                                       self._turns.ctypes.data, len(self._turns), C.byref(n), st.cuda_stream)
+                e1.record(st)
+                if rc == -1 and n.value > len(self._turns):     # more turns than the host buffer: grow it, run again
+                    self._turns = np.empty(n.value, dtype=np.uint32)
+                    continue
+                _lib.check(rc)
+                break
+            e1.synchronize()
+        return SweepOutputs(header, self._turns[:n.value].copy(), n.value, self.out_start, self.out_res,
+                            device_seconds=e0.elapsed_time(e1) / 1e3)
+
+    def run(self, trials: Sequence[Mapping[str, float]] = ({},)) -> List[List[Annotation]]:
+        """-> predictions [file][trial]: for each file and trial what ``Benchmark.run_single`` returns for
+        ``VoiceActivityDetection`` with that tau_active (label "speech", modality "speech", the file's uri)"""
+        taus = self._taus(trials)
+        out: List[List[Annotation]] = [[] for _ in self.uris]
+        dev = 0.0
+        for g in trial_groups(len(taus), self.num_chunks):
+            r = self.binarize(taus[g])
+            dev += r.device_seconds
+            for f in range(len(self.uris)):
+                c0, c1 = int(self.offsets[f]), int(self.offsets[f + 1])
+                header, turns, n = file_turns(r.header, r.turns, c0, c1)
+                preds = assemble_predictions(header, turns, n, self.out_start[c0:c1], self.out_res[c0:c1], ["speech"],
+                                             float(self.shifts[f]), self.uris[f])
+                for p in preds:            # the per-chunk VAD annotations carry modality "speech" whatever the shift
+                    p.modality = "speech"
+                out[f] += preds
+        self.timing["sweep"] = dev
+        return out
+
+    def score(self, trials: Sequence[Mapping[str, float]] = ({},)) \
+            -> Tuple[List[DetectionErrorComponents], DetectionErrorComponents]:
+        """-> (components per file, their sum in file order): the detection error rate components of :meth:`run`'s
+        predictions against each file's reference (``DetectionErrorRate(collar=0, skip_overlap=False)``, no uem); the
+        minimum of ``total.detection_error_rate`` is the trial ``Optimizer.objective`` would pick.  Every file needs a
+        reference."""
+        missing = [self.uris[i] if self.uris[i] is not None else i for i, r in enumerate(self.references) if r is None]
+        if missing:
+            raise ValueError(f"files without a reference cannot be scored: {missing}")
+        taus = self._taus(trials)
+        if self._refs is None:
+            self._refs = pack_speech_references(self.references)
+        rows, roff, totals = self._refs
+        T, nf = len(taus), len(self.uris)
+        comp = np.empty((nf, T, 2), dtype=np.float64)
+        dev = 0.0
+        with torch.cuda.device(self.device):
+            st = torch.cuda.current_stream(self.device)
+            for g in trial_groups(T, self.num_chunks):
+                p = np.ascontiguousarray(taus[g])
+                part = np.empty((nf, len(p), 2), dtype=np.float64)
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record(st)
+                rc = _lib.lib().dg_vad_sweep_score_files(self._h, p.ctypes.data, len(p), self.out_start.ctypes.data,
+                                                         self.out_res.ctypes.data, self.shifts.ctypes.data, PATCH_COLLAR,
+                                                         rows.ctypes.data, roff.ctypes.data, part.ctypes.data,
+                                                         st.cuda_stream)
+                e1.record(st)
+                _lib.check(rc)
+                e1.synchronize()
+                dev += e0.elapsed_time(e1) / 1e3
+                comp[:, g] = part
+        self.timing["score"] = dev
+        per_file = [DetectionErrorComponents(comp[f, :, 0].copy(), comp[f, :, 1].copy(), np.full(T, totals[f]))
+                    for f in range(nf)]
         total = per_file[0]
         for c in per_file[1:]:
             total = total + c

@@ -48,6 +48,7 @@ typedef struct dg_pipeline dg_pipeline;
 typedef struct dg_post dg_post;
 typedef struct dg_stream dg_stream;
 typedef struct dg_sweep dg_sweep;
+typedef struct dg_vad_sweep dg_vad_sweep;
 
 const char* dg_last_error(void);
 int dg_version(void);
@@ -264,6 +265,37 @@ int dg_sweep_score_files(dg_sweep* h, const float* seg_dev, const float* emb_dev
 /* the launch order of the (file, trial) states of dg_sweep_*_files, states_host int32 [num_files * T][2] = {file, trial}:
  * longest file first (equal chunk counts in file order), then trial.  Host only. */
 int dg_sweep_state_order(int num_files, const int32_t* chunk_offsets_host, int T, int32_t* states_host);
+/* ---- voice activity detection sweep: the reference tunes VoiceActivityDetection's one hyper-parameter, tau_active, by
+ *      running the whole pipeline per trial and file and scoring it with DetectionErrorRate(collar=0, skip_overlap=False)
+ *      (reference blocks/vad.py:108-114, optim.py:98-122).  tau_active is read by Binarize alone, so here the speech curve of
+ *      every chunk (max over the local speakers, Hamming-aggregated as dg_post_step with one speaker) is computed once per
+ *      dataset and kept on the device; each trial thresholds it.
+ *      dg_vad_sweep_create: frames <= 1023, 1 <= local_speakers <= 64, 1 <= num_windows <= 256, hamming_host =
+ *      np.hamming(frames) in float64.
+ *      dg_vad_sweep_curve: seg_dev float32 [N][frames][local_speakers], the segmentation scores of num_files files'
+ *        chunks concatenated, file f's at [chunk_offsets_host[f], chunk_offsets_host[f + 1]) (int32 [num_files + 1] from 0 to
+ *        N, increasing); plan_host int32 [N][4 + num_windows]: each file's dg_post_step plan as one batch of a fresh stream,
+ *        concatenated.  Computes and keeps the curve (one float64 per output frame; seg_dev is no longer read afterwards).
+ *        Synchronous.
+ *      dg_vad_sweep_run_files: taus_host float64 [T] (finite), 1 <= T <= 65535, num_files * T <= 2^21; header_host int32
+ *        [T][N][4] and turns_host as dg_sweep_run_files (one speaker, 0).  Synchronous.
+ *      dg_vad_sweep_score_files: out_start_host, out_res_host float64 [N], shifts_host float64 [num_files] and collar as
+ *        dg_sweep_score_files; ref_host float64 [S][2]: each file's speech reference as one label, the support of all its
+ *        segments (rows in time order, each more than 1e-6 s after the previous one), file f's at rows
+ *        [ref_offsets_host[f], ref_offsets_host[f + 1]) (int32 [num_files + 1] from 0, not decreasing);
+ *        components_host float64 [num_files][T][2] = {false alarm, missed detection} seconds.  The total (the reference's
+ *        duration) does not depend on the trial and is the caller's.  Synchronous.
+ *      Every argument is checked before any launch. ---- */
+int dg_vad_sweep_create(int frames, int local_speakers, int num_windows, const double* hamming_host, int device,
+                        dg_vad_sweep** out);
+int dg_vad_sweep_curve(dg_vad_sweep* h, const float* seg_dev, int N, int num_files, const int32_t* chunk_offsets_host,
+                       const int32_t* plan_host, void* stream);
+int dg_vad_sweep_run_files(dg_vad_sweep* h, const double* taus_host, int T, int32_t* header_host, uint32_t* turns_host,
+                           int turn_cap_host, int* n_turns, void* stream);
+int dg_vad_sweep_score_files(dg_vad_sweep* h, const double* taus_host, int T, const double* out_start_host,
+                             const double* out_res_host, const double* shifts_host, double collar, const double* ref_host,
+                             const int32_t* ref_offsets_host, double* components_host, void* stream);
+int dg_vad_sweep_destroy(dg_vad_sweep* h);
 
 /* ---- device-side audio stream: rearrange_audio_stream (reference src/diart/operators.py:44-100) with the ring buffer in
  *      HBM.  The host pushes every sample ONCE (step_samples new samples per chunk instead of chunk_samples: 8.2 MB
