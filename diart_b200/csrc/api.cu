@@ -225,3 +225,98 @@ extern "C" int dg_selftest_gemm_tc(int M, int Cin, int KW, int dil, int N, int e
   *out_rms = (float)sqrt(ss / c0.size());
   return DG_OK;
 }
+
+// Runs one seeded shifted-window GEMM with epilogue `epi` (0..5) under SM caps of 0 (none), 1, 3 and 7 and sets *equal to 1
+// if every output is byte-equal across the four grids: float32 rows, hi/lo planes, pooling partial sums.  Per epilogue:
+// 3 = 3 x 3 Conv2d (KW must be 9; `dil` = Hp, M = whole padded maps) with residual planes and ReLU -> hi/lo planes;
+// 4 = statistics pooling of 3 speakers over items of 296 rows; 5 = MaxPool1d(3) over items of 888 rows (M a multiple of it).
+extern "C" int dg_selftest_gemm_tc_grid(int M, int Cin, int KW, int dil, int N, int epi, int* equal) {
+  if (M < 1 || Cin % 64 || KW < 1 || KW > 9 || N < 1 || N % 4 || epi < 0 || epi > 5 || !equal ||
+      (epi == 3 && (KW != 9 || dil < 3 || M % (dil * dil) || N % 32)) || (epi == 5 && (N > 64 || M % 888))) {
+    set_error("dg_selftest_gemm_tc_grid: bad arguments");
+    return DG_EINVAL;
+  }
+  const int K = KW * Cin;
+  const int npad = epi == 5 || N == 64 ? 64 : (epi == 3 && N == 32 ? 32 : (N + 127) / 128 * 128);
+  const int ldc = epi == 3 ? (N + 31) / 32 * 32 : N;
+  const int item_rows = epi == 4 ? 296 : 888, tile_rows = epi == 5 ? gemm_tc_pool3_tile_rows(item_rows) : 128;
+  const long long m_tiles = (M + tile_rows - 1) / tile_rows;
+  uint32_t seed = 777u;
+  auto rnd = [&]() {
+    seed = seed * 1664525u + 1013904223u;
+    return ((seed >> 8) & 0xFFFF) / 65536.f - 0.5f;
+  };
+  std::vector<float> A((size_t)M * Cin), Wnk((size_t)N * K), bias(N), bsc(N), bsh(N), res((size_t)M * ldc), pw((size_t)M * 4);
+  for (auto& v : A) v = 2.f * rnd();
+  for (auto& v : Wnk) v = 0.25f * rnd();
+  for (int n = 0; n < N; n++) {
+    bias[n] = rnd();
+    bsc[n] = 1.f + rnd();
+    bsh[n] = rnd();
+  }
+  for (auto& v : res) v = rnd();
+  for (auto& v : pw) v = rnd() + 0.5f;
+  // output buffers, in bytes: float32 rows, hi and lo planes, pooling partial sums
+  const size_t f32_bytes = epi == 0 || epi == 2 ? (size_t)M * ldc * 4 : (epi == 5 ? (size_t)(M / 3) * ldc * 4 : 0);
+  const size_t plane_bytes = epi == 1 || epi == 3 ? (size_t)M * ldc * 2 : 0;
+  const size_t part_bytes = epi == 4 ? (size_t)m_tiles * 2 * 4 * 2 * N * 4 : (epi == 5 ? (size_t)m_tiles * 2 * 2 * N * 4 : 0);
+  DevBuf dA, dAh, dAl, dB, dS, dH, dRes, dRh, dRl, dPw, dF, dOh, dOl, dPart;
+  WeightPlanes dW;
+  if (upload(dA, A) || upload(dB, bias) || upload(dS, bsc) || upload(dH, bsh) || upload(dRes, res) || upload(dPw, pw) ||
+      upload_split(dW, Wnk, N, npad, K))
+    return DG_ECUDA;
+  if (dAh.ensure((size_t)M * Cin * 2) || dAl.ensure((size_t)M * Cin * 2) || dRh.ensure((size_t)M * ldc * 2) ||
+      dRl.ensure((size_t)M * ldc * 2) || dF.ensure(f32_bytes + 4) || dOh.ensure(plane_bytes + 4) ||
+      dOl.ensure(plane_bytes + 4) || dPart.ensure(part_bytes + 4))
+    return DG_ECUDA;
+  int rc;
+  if ((rc = launch_split_ex(dA.as<float>(), M, Cin, Cin, Cin, 0, 1, nullptr, nullptr, dAh.p, dAl.p, nullptr)) ||
+      (rc = launch_split_ex(dRes.as<float>(), M, ldc, ldc, ldc, 0, 1, nullptr, nullptr, dRh.p, dRl.p, nullptr)))
+    return rc;
+  int taps[9];
+  for (int j = 0; j < 9; j++) taps[j] = (j / 3 - 1) * dil + (j % 3 - 1);   // Conv2d: (dw - 1) * Hp + (dh - 1)
+  TcGemm t{};
+  t.A_hi = dAh.p; t.A_lo = dAl.p; t.lda = Cin; t.Cin = Cin; t.KW = KW; t.dil = dil; t.Mtot = M; t.M = M;
+  t.N = N; t.bias = dB.as<float>(); t.bn_scale = dS.as<float>(); t.bn_shift = dH.as<float>(); t.ldc = ldc;
+  t.epi = epi; t.tag = "selftest_tc_grid";
+  t.out_f32 = f32_bytes ? dF.as<float>() : nullptr;
+  t.out_hi = plane_bytes ? dOh.p : nullptr;
+  t.out_lo = plane_bytes ? dOl.p : nullptr;
+  if (epi == 3) {
+    t.tap_off = taps; t.Wp = t.Wop = t.Hp = t.Hop = dil; t.relu = 1;
+    t.res_hi = dRh.p; t.res_lo = dRl.p;
+  }
+  if (epi == 4) {
+    t.pool_w = dPw.as<float>(); t.pool_part = dPart.as<float>(); t.pool_item_rows = item_rows; t.pool_K = 3;
+  }
+  if (epi == 5) {
+    t.pool_part = dPart.as<float>(); t.pool_item_rows = item_rows; t.pool3_T = item_rows / 3 - 2;
+    t.pool3_tile_rows = tile_rows;
+  }
+  if ((rc = set_weights(t, dW))) return rc;
+  std::vector<unsigned char> first, cur;
+  *equal = 1;
+  const int caps[4] = {0, 1, 3, 7};
+  for (int ci = 0; ci < 4; ci++) {
+    // unwritten bytes (rows outside a Conv2d map, pooling slots of absent items) compare equal because they stay zero
+    DG_CUDA(cudaMemset(dF.p, 0, f32_bytes + 4));
+    DG_CUDA(cudaMemset(dOh.p, 0, plane_bytes + 4));
+    DG_CUDA(cudaMemset(dOl.p, 0, plane_bytes + 4));
+    DG_CUDA(cudaMemset(dPart.p, 0, part_bytes + 4));
+    {
+      SmLimit cap(caps[ci]);
+      if ((rc = launch_gemm_tc(t, nullptr))) return rc;
+    }
+    DG_CUDA(cudaDeviceSynchronize());
+    cur.resize(f32_bytes + 2 * plane_bytes + part_bytes);
+    DG_CUDA(cudaMemcpy(cur.data(), dF.p, f32_bytes, cudaMemcpyDeviceToHost));
+    DG_CUDA(cudaMemcpy(cur.data() + f32_bytes, dOh.p, plane_bytes, cudaMemcpyDeviceToHost));
+    DG_CUDA(cudaMemcpy(cur.data() + f32_bytes + plane_bytes, dOl.p, plane_bytes, cudaMemcpyDeviceToHost));
+    DG_CUDA(cudaMemcpy(cur.data() + f32_bytes + 2 * plane_bytes, dPart.p, part_bytes, cudaMemcpyDeviceToHost));
+    if (ci == 0)
+      first.swap(cur);
+    else if (cur != first)
+      *equal = 0;
+  }
+  return DG_OK;
+}

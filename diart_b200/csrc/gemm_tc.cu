@@ -13,26 +13,28 @@
 // Because activations are stored time-major ([item][row][channel]) a Conv1d tap is just a TMA box whose
 // row coordinate is shifted by j*dil: no im2col is ever materialised.
 //
-// Two kernels.  gemm_tc_kernel runs the element-wise epilogues (bias, LeakyReLU + BatchNorm, Conv2d):
-// CTA = 160 threads, persistent over (m_tile, n_tile):
-//   warp 4      TMA producer: per k-block four boxes (A_hi, A_lo: 128 rows x 64 ch; W_hi, W_lo: BN x 64)
-//               into a 128B-swizzled, NSTAGE-deep shared-memory ring, completion on full[] mbarriers
-//   warps 0-3   one warpgroup: 24 wgmma per k-block (two m64 halves x four k-steps x three products) into
-//               registers, the slot is released one k-block later; then the accumulator goes through shared
-//               memory (row m of the tile -> thread m) and the same threads run the epilogue: bias, LeakyReLU,
-//               BatchNorm affine, then float32 rows or the next layer's hi/lo 16-bit planes.
-//               The producer fills the ring for the next tile meanwhile.
-// gemm_tc_pool_kernel runs the two pooling epilogues (TC_POOL, TC_MAXPOOL3), whose cross-row reductions take about as
-// long as the tile's MMAs; CTA = 384 threads, persistent over tiles taken in m-major order from a per-stream atomic
-// counter (a CTA that becomes resident late runs fewer tiles):
-//   warpgroup 0     (setmaxnreg 40) one thread fetches the CTA's next tile, hands its index to the consumer whose turn it
-//                   is, and loads per k-block four boxes (128 or BN rows x 32 ch) into a 64B-swizzled ring
-//   warpgroups 1-2  (setmaxnreg 232) ping-pong consumers: each runs whole 128 x BN tiles, alternately; an ordering barrier
-//                   hands the tensor cores to the other consumer once a tile's MMAs are issued, so one consumer's
-//                   pooling epilogue overlaps the other's mainloop.  The accumulator goes to shared memory 64 columns
-//                   at a time, already through bias / LeakyReLU / BatchNorm (TC_POOL) or the weight scale (TC_MAXPOOL3).
-// Both issue the same wgmma sequence (k order, lo.hi, hi.lo, hi.hi per k-step) and the same epilogue arithmetic for an
-// output element whichever CTA or warpgroup runs its tile.
+// One kernel, gemm_tc_kernel, for every epilogue.  CTA = 384 threads, persistent over 128 x BN tiles:
+//   warpgroup 0     (setmaxnreg 40) one thread hands the CTA's tiles to the two consumers alternately and loads per k-block
+//                   four boxes (A_hi, A_lo: 128 rows x 32 ch; W_hi, W_lo: BN rows x 32 ch) into a 64B-swizzled ring,
+//                   completion on full[] mbarriers
+//   warpgroups 1-2  (setmaxnreg 232) ping-pong consumers: each runs whole tiles, 12 wgmma per k-block (two m64 halves x
+//                   two k-steps x three products) into registers, a slot is released one k-block later; an ordering
+//                   barrier hands the tensor cores to the other consumer once a tile's MMAs are issued, so one consumer's
+//                   epilogue overlaps the other's mainloop.
+// Tile order: the element-wise epilogues (bias, LeakyReLU + BatchNorm, Conv2d) take the static order b, b + grid, ...;
+// the pooling epilogues (TC_POOL, TC_MAXPOOL3), whose cross-row reductions take about as long as the tile's MMAs, take
+// tiles in m-major order from a per-stream atomic counter (a CTA that becomes resident late runs fewer tiles).
+// Epilogues:
+//   element-wise    the two consumers share ONE full-tile staging buffer, [128][BN + 4] float32.  A consumer waits until
+//                   the other one has finished reading it (a named-barrier pair), writes its whole accumulator there and
+//                   runs the epilogue from it (row m of the tile -> thread m): bias, LeakyReLU, BatchNorm affine, then
+//                   float32 rows or the next layer's hi/lo 16-bit planes.  The accumulator is dead during the epilogue, so
+//                   it does not compete with the epilogue for registers.  One buffer is enough: a consumer needs it only
+//                   after its own mainloop, and the other consumer runs its epilogue during that mainloop.
+//   pooling         the accumulator goes to the consumer's own shared memory 64 columns at a time, already through bias /
+//                   LeakyReLU / BatchNorm (TC_POOL) or the weight scale (TC_MAXPOOL3).
+// Every output element gets the same wgmma sequence (k order, lo.hi, hi.lo, hi.hi per k-step) and the same epilogue
+// arithmetic whichever CTA or warpgroup runs its tile, so results do not depend on the grid.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <math.h>
@@ -49,8 +51,7 @@
 
 namespace dg {
 
-constexpr int TC_BM = 128, TC_BK = 64, TC_THREADS = 160;
-constexpr int TC_POOL_BK = 32, TC_POOL_THREADS = 384;   // gemm_tc_pool_kernel
+constexpr int TC_BM = 128, TC_BK = 32, TC_THREADS = 384;
 constexpr int TC_SMEM_MAX = 227 * 1024;                 // dynamic shared memory per CTA on sm_90
 
 struct TcArgs {
@@ -82,25 +83,40 @@ struct TcArgs {
   // bias + MaxPool1d(3) over rows ([M / 3, ldc]), pool_part the per-tile InstanceNorm partial sums of the pre-bias pooled values:
   // [m_tiles][2 (item of the tile)][2 (sum, sum of squares)][N] over the pooled frames < pool3_T of an item
   int tile_rows, pool3_T;
-  unsigned* tile_ctr;      // gemm_tc_pool_kernel, [2]: tiles handed out past the first wave, CTAs finished (both back to 0)
+  unsigned* tile_ctr;      // pooling epilogues, [2]: tiles handed out past the first wave, CTAs finished (both back to 0)
 };
 
 enum TcEpi { TC_BIAS_F32 = 0, TC_LEAKY_BN_SPLIT = 1, TC_LEAKY_BN_F32 = 2, TC_CONV2D = 3, TC_POOL = 4, TC_MAXPOOL3 = 5 };
 
-// ------------------------------------------------------------------------------------ the kernel
-// Layout: [NSTAGE stages of (A hi, A lo, W hi, W lo)] [parameters] [barriers] [accumulator tile]
+__host__ __device__ constexpr bool tc_pooling(int epi) { return epi == TC_POOL || epi == TC_MAXPOOL3; }
+
+// Layout: [NSTAGE stages of (A hi, A lo, W hi, W lo)] [barriers] [consumer 0: parameters | pooling: chunk | pooling staging]
+// [consumer 1: the same] [element-wise: the shared accumulator tile]
 template <int BN>
 struct TcSmem {
-  static constexpr int A_BYTES = TC_BM * TC_BK * 2;     // 16 KB per plane
+  static constexpr int A_BYTES = TC_BM * TC_BK * 2;     // 8 KB per plane
   static constexpr int W_BYTES = BN * TC_BK * 2;
   static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;
-  static constexpr int NSTAGE = BN == 128 ? 2 : 3;
-  static constexpr int PARAM_BYTES = 3 * BN * 4;
-  // the finished accumulator, one float32 row per tile row (+4 floats: 128-bit row reads without bank conflicts)
+  // 128 / 144 / 120 KB of operands in flight at BN = 128 / 64 / 32
+  static constexpr int NSTAGE = BN == 128 ? 4 : 6;
+  static constexpr int BAR_BYTES = 256;
+  static constexpr int PARAM_FLOATS = 3 * BN;
+  // pooling: CHUNK_W accumulator columns of every tile row, as [CHUNK_W / 32][128][33] (conflict-free column reads)
+  static constexpr int CHUNK_W = 64;
+  static constexpr int CHUNK_FLOATS = CHUNK_W / 32 * TC_BM * 33;
+  // TC_POOL: row weights [128][4] + cross-row-group staging [4][2][8][32]; TC_MAXPOOL3: staging [4][2][2][32]
+  __host__ __device__ static constexpr int extra_floats(int epi) { return epi == TC_POOL ? 128 * 4 + 4 * 2 * 8 * 32 : (epi == TC_MAXPOOL3 ? 4 * 2 * 2 * 32 : 0); }
+  __host__ __device__ static constexpr int consumer_floats(int epi) { return PARAM_FLOATS + (tc_pooling(epi) ? CHUNK_FLOATS + extra_floats(epi) : 0); }
+  // element-wise: the finished accumulator, one float32 row per tile row (+4 floats: 128-bit row reads without bank conflicts)
   static constexpr int ACC_LD = BN + 4;
-  static constexpr int ACC_BYTES = TC_BM * ACC_LD * 4;
-  static constexpr int TOTAL = NSTAGE * STAGE_BYTES + PARAM_BYTES + 256 + ACC_BYTES + 1024;   // + barriers + alignment slack
+  __host__ __device__ static constexpr int acc_floats(int epi) { return tc_pooling(epi) ? 0 : TC_BM * ACC_LD; }
+  __host__ __device__ static constexpr int total(int epi) {
+    return NSTAGE * STAGE_BYTES + BAR_BYTES + (2 * consumer_floats(epi) + acc_floats(epi)) * 4 + 1024;   // + alignment slack
+  }
 };
+static_assert(TcSmem<128>::total(TC_POOL) <= TC_SMEM_MAX && TcSmem<64>::total(TC_MAXPOOL3) <= TC_SMEM_MAX &&
+              TcSmem<128>::total(TC_CONV2D) <= TC_SMEM_MAX && TcSmem<64>::total(TC_CONV2D) <= TC_SMEM_MAX &&
+              TcSmem<32>::total(TC_CONV2D) <= TC_SMEM_MAX, "gemm_tc: shared memory");
 
 // 32 consecutive accumulator columns of this thread's row
 __device__ __forceinline__ void acc_ld32(const float* p, uint32_t (&r)[32]) {
@@ -115,16 +131,17 @@ __device__ __forceinline__ void acc_ld32(const float* p, uint32_t (&r)[32]) {
 }
 
 // ------------------------------------------------------------------------------------ the epilogue of one 128-row tile
-// Executed by the 128 threads of the warpgroup; thread et = 32 quad + lane owns row et of the tile.  `mt` = index of the
-// 128-row tile (rows mt * 128 ..), `acc_row` = this thread's row of the finished accumulator in shared memory.
+// Executed by the 128 threads of a consumer warpgroup; thread et = 32 quad + lane owns row et of the tile.  `mt` = index
+// of the 128-row tile (rows mt * 128 ..), `acc_row` = this thread's row of the finished accumulator in shared memory,
+// `bar` = the warpgroup's named barrier.
 template <int BN, int EPI>
-__device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params, const float* acc_row,
+__device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params, const float* acc_row, int bar,
                                                  long long mt, int n0, int quad, int lane, int et, bool stage_params) {
     const long long m = mt * TC_BM + quad * 32 + lane;
-    // stage the per-column parameters of this tile (named barrier 1: the 128 epilogue threads only); with a single
-    // column tile they are the same for every tile of this CTA: staged once
+    // stage the per-column parameters of this tile; with a single column tile they are the same for every tile of this
+    // warpgroup: staged once
     if (stage_params) {
-      asm volatile("bar.sync 1, 128;" ::: "memory");
+      named_sync(bar, 128);
       for (int i = et; i < BN; i += 128) {
         const int n = n0 + i;
         const bool ok = n < a.N;
@@ -133,12 +150,11 @@ __device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params,
         params[BN + i] = (ok && has_bn) ? a.bn_scale[n] * (EPI == TC_CONV2D ? a.acc_scale : 1.f) : 1.f;   // (2^-k: exact)
         params[2 * BN + i] = (ok && has_bn) ? a.bn_shift[n] : 0.f;
       }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
+      named_sync(bar, 128);
     }
-    // TC_CONV2D: output position of this row, and the residual of the first 32 columns requested before the wait
+    // TC_CONV2D: output position of this row
     long long mo = m;                 // output row
     bool row_ok = m < a.M;
-    uint4 rh0[4], rl0[4];
     if (EPI == TC_CONV2D) {
       const unsigned mu = (unsigned)m, per = (unsigned)(a.Wp * a.Hp);     // (the launcher checks M < 2^31)
       const unsigned item = mu / per, rem = mu - item * per;
@@ -147,15 +163,6 @@ __device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params,
       if (a.stride2) {
         row_ok = row_ok && (w & 1) && (h & 1);
         mo = ((long long)item * a.Wop + ((w - 1) >> 1) + 1) * a.Hop + ((h - 1) >> 1) + 1;
-      }
-      if (row_ok && a.res_hi) {
-        const uint4* rh = reinterpret_cast<const uint4*>(a.res_hi + mo * a.ldc + n0);
-        const uint4* rl = reinterpret_cast<const uint4*>(a.res_lo + mo * a.ldc + n0);
-#pragma unroll
-        for (int q = 0; q < 4; q++) {
-          rh0[q] = rh[q];
-          rl0[q] = rl[q];
-        }
       }
     }
 #pragma unroll 1
@@ -173,7 +180,7 @@ __device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params,
           const uint4* rl = reinterpret_cast<const uint4*>(a.res_lo + mo * a.ldc + n0 + c);
 #pragma unroll
           for (int q = 0; q < 4; q++) {
-            const uint4 hq = c == 0 ? rh0[q] : rh[q], lq = c == 0 ? rl0[q] : rl[q];
+            const uint4 hq = rh[q], lq = rl[q];
             const uint32_t hw[4] = {hq.x, hq.y, hq.z, hq.w}, lw[4] = {lq.x, lq.y, lq.z, lq.w};
 #pragma unroll
             for (int e = 0; e < 4; e++) {
@@ -273,142 +280,7 @@ __device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params,
     }
 }
 
-template <int BN, int EPI>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-               const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo, TcArgs a) {
-  using S = TcSmem<BN>;
-  constexpr int NSTAGE = S::NSTAGE;
-  extern __shared__ unsigned char smem_raw[];
-  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* params = reinterpret_cast<float*>(smem + NSTAGE * S::STAGE_BYTES);          // bias | bn_scale | bn_shift
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NSTAGE * S::STAGE_BYTES + S::PARAM_BYTES);
-  uint64_t* full = bars;                 // [NSTAGE] TMA -> MMA
-  uint64_t* empty = bars + NSTAGE;       // [NSTAGE] MMA -> TMA
-  float* acc_s = reinterpret_cast<float*>(smem + NSTAGE * S::STAGE_BYTES + S::PARAM_BYTES + 256);   // [128][ACC_LD]
-
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // warp-uniform
-  const int num_tiles = a.m_tiles * a.n_tiles;
-  const int kblocks = a.KW * a.cin_blocks;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < NSTAGE; s++) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-
-  if (warp == 4) {
-    // ===================================================================== TMA producer
-    if (lane == 0) {
-      int stage = 0, phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
-        const int m0 = mt * TC_BM, n0 = nt * BN;
-        for (int j = 0; j < a.KW; j++) {
-          for (int cb = 0; cb < a.cin_blocks; cb++) {
-            mbar_wait(&empty[stage], phase ^ 1);
-            unsigned char* st = smem + stage * S::STAGE_BYTES;
-            mbar_expect_tx(&full[stage], S::STAGE_BYTES);
-            const int kcol = (j * a.cin_blocks + cb) * TC_BK;
-            tma_load_2d(st, &tmA_hi, cb * TC_BK, m0 + a.tap_off[j], &full[stage]);
-            tma_load_2d(st + S::A_BYTES, &tmA_lo, cb * TC_BK, m0 + a.tap_off[j], &full[stage]);
-            tma_load_2d(st + 2 * S::A_BYTES, &tmW_hi, kcol, n0, &full[stage]);
-            tma_load_2d(st + 2 * S::A_BYTES + S::W_BYTES, &tmW_lo, kcol, n0, &full[stage]);
-            if (++stage == NSTAGE) {
-              stage = 0;
-              phase ^= 1;
-            }
-          }
-        }
-      }
-    }
-    return;
-  }
-  // ===================================================================== MMA + epilogue (warps 0..3)
-  const int quad = warp, et = threadIdx.x;
-  int stage = 0, phase = 0;
-  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-    const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
-    float acc[2][BN / 2];
-    int prev = -1;                       // slot of the previous k-block: released once its MMAs are complete
-    for (int kb = 0; kb < kblocks; kb++) {
-      mbar_wait(&full[stage], phase);
-      const uint32_t sa = smem_u32(smem + stage * S::STAGE_BYTES);
-      const uint64_t a_hi = wg_desc(sa), a_lo = wg_desc(sa + S::A_BYTES);
-      const uint64_t w_hi = wg_desc(sa + 2 * S::A_BYTES), w_lo = wg_desc(sa + 2 * S::A_BYTES + S::W_BYTES);
-      constexpr uint64_t HALF = (uint64_t)((64 * 128) >> 4);   // rows 64..127 of the A tile
-      wg_fence_acc(acc[0]);
-      wg_fence_acc(acc[1]);
-      wg_fence();
-#pragma unroll
-      for (int ks = 0; ks < TC_BK / 16; ks++) {
-        const uint64_t adv = (uint64_t)((ks * 32) >> 4);   // +32 bytes per 16-element k-step
-#pragma unroll
-        for (int h = 0; h < 2; h++) {
-          wgmma_ss<BN>(acc[h], a_lo + adv + h * HALF, w_hi + adv, (kb | ks) != 0);
-          wgmma_ss<BN>(acc[h], a_hi + adv + h * HALF, w_lo + adv, 1);
-          wgmma_ss<BN>(acc[h], a_hi + adv + h * HALF, w_hi + adv, 1);
-        }
-      }
-      wg_commit();
-      wg_wait<1>();
-      wg_fence_acc(acc[0]);
-      wg_fence_acc(acc[1]);
-      if (prev >= 0 && et == 0) mbar_arrive(&empty[prev]);
-      prev = stage;
-      if (++stage == NSTAGE) {
-        stage = 0;
-        phase ^= 1;
-      }
-    }
-    wg_wait<0>();
-    wg_fence_acc(acc[0]);
-    wg_fence_acc(acc[1]);
-    if (prev >= 0 && et == 0) mbar_arrive(&empty[prev]);
-    // accumulator -> shared memory (the previous tile's epilogue has read it: barrier first)
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
-      const int r0 = 64 * h + 16 * quad + (lane >> 2);
-#pragma unroll
-      for (int j = 0; j < BN / 8; j++) {
-        const int col = 8 * j + 2 * (lane & 3);
-        *reinterpret_cast<float2*>(acc_s + r0 * S::ACC_LD + col) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
-        *reinterpret_cast<float2*>(acc_s + (r0 + 8) * S::ACC_LD + col) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
-      }
-    }
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-    tc_epilogue_tile<BN, EPI>(a, params, acc_s + et * S::ACC_LD, mt, nt * BN, quad, lane, et,
-                              a.n_tiles > 1 || tile == (int)blockIdx.x);
-  }
-}
-
-// ------------------------------------------------------------------------------------ the pooling kernel
-// Layout: [NSTAGE stages of (A hi, A lo, W hi, W lo)] [barriers] [consumer 0: parameters | chunk | pooling staging]
-// [consumer 1: the same]
-template <int BN>
-struct TcPoolSmem {
-  static constexpr int A_BYTES = TC_BM * TC_POOL_BK * 2;     // 8 KB per plane
-  static constexpr int W_BYTES = BN * TC_POOL_BK * 2;
-  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;
-  // 128 / 144 KB of operands in flight at BN = 128 (TC_POOL) / 64 (TC_MAXPOOL3)
-  static constexpr int NSTAGE = BN == 128 ? 4 : 6;
-  static constexpr int BAR_BYTES = 256;
-  static constexpr int PARAM_FLOATS = 3 * BN;
-  // CHUNK_W accumulator columns of every tile row, as [CHUNK_W / 32][128][33] (conflict-free column reads)
-  static constexpr int CHUNK_W = 64;
-  static constexpr int CHUNK_FLOATS = CHUNK_W / 32 * TC_BM * 33;
-  // TC_POOL: row weights [128][4] + cross-row-group staging [4][2][8][32]; TC_MAXPOOL3: staging [4][2][2][32]
-  __host__ __device__ static constexpr int extra_floats(int epi) { return epi == 4 ? 128 * 4 + 4 * 2 * 8 * 32 : (epi == 5 ? 4 * 2 * 2 * 32 : 0); }
-  __host__ __device__ static constexpr int consumer_floats(int epi) { return PARAM_FLOATS + CHUNK_FLOATS + extra_floats(epi); }
-  __host__ __device__ static constexpr int total(int epi) { return NSTAGE * STAGE_BYTES + BAR_BYTES + 2 * consumer_floats(epi) * 4 + 1024; }   // + alignment slack
-};
-static_assert(TcPoolSmem<128>::total(4) <= TC_SMEM_MAX && TcPoolSmem<64>::total(5) <= TC_SMEM_MAX, "gemm_tc: shared memory");
-
-// ------------------------------------------------------------------------------------ the epilogue of one 128-row tile
+// ------------------------------------------------------------------------------------ the pooling epilogue of one 128-row tile
 // Executed by the 128 threads of a consumer warpgroup; thread et = 32 quad + lane owns row et of the tile.  `mt` = index
 // of the 128-row tile (rows mt * 128 ..), `acc` = the finished accumulator in registers, `bar` = the warpgroup's named
 // barrier.
@@ -446,7 +318,7 @@ __device__ __forceinline__ void tc_pool_epilogue_tile(const TcArgs& a, float* pa
     // accumulator fragment of this thread (tc_ptx.cuh): acc[h][4 j + e] is row 64 h + 16 quad + lane / 4 + 8 (e / 2),
     // column 8 j + 2 (lane % 4) + e % 2.  The tile goes through shared memory CW columns at a time (the registers of a
     // staged chunk are free for the reductions), which run 32 columns at a time.
-    constexpr int CW = TcPoolSmem<BN>::CHUNK_W;
+    constexpr int CW = TcSmem<BN>::CHUNK_W;
     const int fr0 = 16 * quad + (lane >> 2), fc0 = 2 * (lane & 3);
 #pragma unroll
     for (int c0 = 0; c0 < BN; c0 += CW) {
@@ -587,13 +459,17 @@ __device__ __forceinline__ void tc_pool_epilogue_tile(const TcArgs& a, float* pa
     }
 }
 
+// ------------------------------------------------------------------------------------ the kernel
 // Named barriers besides 0: 1 + c = the 128 threads of consumer c (epilogue staging); 3 + c = consumer c may issue its
-// mainloop (256 threads: consumer c waits, the other consumer arrives once its own MMAs are issued).
+// mainloop (256 threads: consumer c waits, the other consumer arrives once its own MMAs are issued); element-wise
+// epilogues: 5 + c = consumer c may write the shared accumulator tile (256 threads: consumer c waits, the other consumer
+// arrives once its epilogue has read the tile).
 template <int BN, int EPI>
-__global__ void __launch_bounds__(TC_POOL_THREADS, 1)
-gemm_tc_pool_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo, TcArgs a) {
-  using S = TcPoolSmem<BN>;
+  using S = TcSmem<BN>;
+  constexpr bool POOLING = tc_pooling(EPI);
   constexpr int NSTAGE = S::NSTAGE;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -604,6 +480,7 @@ gemm_tc_pool_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
   uint64_t* tile_empty = tile_full + 2;       // [2] consumer c -> producer: tile_idx[c] has been read
   volatile int* tile_idx = reinterpret_cast<volatile int*>(tile_empty + 2);   // [2]
   float* cons = reinterpret_cast<float*>(smem + NSTAGE * S::STAGE_BYTES + S::BAR_BYTES);
+  float* acc_s = cons + 2 * S::consumer_floats(EPI);   // element-wise: [128][ACC_LD], shared by the consumers
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // warp-uniform
   const int wg = warp >> 2;
@@ -629,7 +506,8 @@ gemm_tc_pool_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
     if (threadIdx.x == 0) {
       int stage = 0, phase = 0;
       // i = position in this CTA's sequence of tiles, run by consumer i % 2.  The first tile is blockIdx.x, the later ones
-      // come from the counter.  Two end marks follow the last tile: -1 (its consumer passes the turn on), then -2.
+      // come from the counter (pooling) or follow at a stride of the grid.  Two end marks follow the last tile: -1 (its
+      // consumer passes the turn on), then -2.
       for (int i = 0, tile = blockIdx.x;; i++) {
         const int c = i & 1;
         mbar_wait(&tile_empty[c], ((i >> 1) & 1) ^ 1);
@@ -650,9 +528,9 @@ gemm_tc_pool_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
             mbar_wait(&empty[stage], phase ^ 1);
             unsigned char* st = smem + stage * S::STAGE_BYTES;
             mbar_expect_tx(&full[stage], S::STAGE_BYTES);
-            const int kcol = (j * a.cin_blocks + cb) * TC_POOL_BK;
-            tma_load_2d(st, &tmA_hi, cb * TC_POOL_BK, m0 + a.tap_off[j], &full[stage]);
-            tma_load_2d(st + S::A_BYTES, &tmA_lo, cb * TC_POOL_BK, m0 + a.tap_off[j], &full[stage]);
+            const int kcol = (j * a.cin_blocks + cb) * TC_BK;
+            tma_load_2d(st, &tmA_hi, cb * TC_BK, m0 + a.tap_off[j], &full[stage]);
+            tma_load_2d(st + S::A_BYTES, &tmA_lo, cb * TC_BK, m0 + a.tap_off[j], &full[stage]);
             tma_load_2d(st + 2 * S::A_BYTES, &tmW_hi, kcol, n0, &full[stage]);
             tma_load_2d(st + 2 * S::A_BYTES + S::W_BYTES, &tmW_lo, kcol, n0, &full[stage]);
             if (++stage == NSTAGE) {
@@ -661,14 +539,16 @@ gemm_tc_pool_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
             }
           }
         }
-        tile = (int)gridDim.x + (int)atomicAdd(&a.tile_ctr[0], 1u);
+        tile = POOLING ? (int)gridDim.x + (int)atomicAdd(&a.tile_ctr[0], 1u) : tile + (int)gridDim.x;
       }
       // every CTA has taken its last tile once all have counted themselves here: the last one returns the counter to 0
       // for the next launch on this stream
-      __threadfence();
-      if (atomicAdd(&a.tile_ctr[1], 1u) == gridDim.x - 1) {
-        atomicExch(&a.tile_ctr[0], 0u);
-        atomicExch(&a.tile_ctr[1], 0u);
+      if (POOLING) {
+        __threadfence();
+        if (atomicAdd(&a.tile_ctr[1], 1u) == gridDim.x - 1) {
+          atomicExch(&a.tile_ctr[0], 0u);
+          atomicExch(&a.tile_ctr[1], 0u);
+        }
       }
     }
     return;
@@ -679,33 +559,42 @@ gemm_tc_pool_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
   float* params = cons + c * S::consumer_floats(EPI);   // bias | bn_scale | bn_shift
   float* chunk = params + S::PARAM_FLOATS;
   float* pool_stage = chunk + S::CHUNK_FLOATS;          // TC_POOL / TC_MAXPOOL3 only
-  const int bar = 1 + c, turn = 3 + c, turn_other = 3 + (c ^ 1);
-  if (c == 1) named_arrive(3, 256);                     // consumer 0 issues the first mainloop
+  const int bar = 1 + c, turn = 3 + c, turn_other = 3 + (c ^ 1), acc_free = 5 + c, acc_free_other = 5 + (c ^ 1);
+  if (c == 1) {
+    named_arrive(3, 256);                               // consumer 0 issues the first mainloop
+    if (!POOLING) named_arrive(5, 256);                 // and writes the accumulator tile first
+  }
   for (int n = 0;; n++) {
     mbar_wait(&tile_full[c], n & 1);
     const int tile = tile_idx[c];
     mbar_arrive(&tile_empty[c]);
     named_sync(turn, 256);
     if (tile < 0) {
-      if (tile == -1) named_arrive(turn_other, 256);
+      if (tile == -1) {
+        named_arrive(turn_other, 256);
+        // the last tile's consumer has handed the accumulator tile to this one: take that arrival
+        if (!POOLING) named_sync(acc_free, 256);
+      }
       break;
     }
-    const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
     const int pos = (2 * n + c) * kblocks;              // ring position of the tile's first k-block
     int stage = pos % NSTAGE, phase = (pos / NSTAGE) & 1;
+    // The first wgmma of a tile ignores the accumulator's contents.  Defined anyway: an undefined accumulator is carried
+    // around the tile loop by ptxas, i.e. kept live through the epilogue, where it forces spills.
     float acc[2][BN / 2];
-    int prev = -1;                       // slot of the previous k-block: released once its MMAs are complete
+#pragma unroll
+    for (int i = 0; i < BN / 2; i++) acc[0][i] = acc[1][i] = 0.f;
     for (int kb = 0; kb < kblocks; kb++) {
       mbar_wait(&full[stage], phase);
       const uint32_t sa = smem_u32(smem + stage * S::STAGE_BYTES);
       const uint64_t a_hi = wg_desc_sw64(sa), a_lo = wg_desc_sw64(sa + S::A_BYTES);
       const uint64_t w_hi = wg_desc_sw64(sa + 2 * S::A_BYTES), w_lo = wg_desc_sw64(sa + 2 * S::A_BYTES + S::W_BYTES);
-      constexpr uint64_t HALF = (uint64_t)((64 * TC_POOL_BK * 2) >> 4);   // rows 64..127 of the A tile
+      constexpr uint64_t HALF = (uint64_t)((64 * TC_BK * 2) >> 4);   // rows 64..127 of the A tile
       wg_fence_acc(acc[0]);
       wg_fence_acc(acc[1]);
       wg_fence();
 #pragma unroll
-      for (int ks = 0; ks < TC_POOL_BK / 16; ks++) {
+      for (int ks = 0; ks < TC_BK / 16; ks++) {
         const uint64_t adv = (uint64_t)((ks * 32) >> 4);   // +32 bytes per 16-element k-step
 #pragma unroll
         for (int h = 0; h < 2; h++) {
@@ -718,8 +607,9 @@ gemm_tc_pool_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
       wg_wait<1>();
       wg_fence_acc(acc[0]);
       wg_fence_acc(acc[1]);
-      if (prev >= 0 && et == 0) mbar_arrive(&empty[prev]);
-      prev = stage;
+      // the previous k-block's slot is released once its MMAs are complete (kept as `stage - 1`, not in a register of
+      // its own: the consumer's registers are at the 168 of the launch while the accumulator is live)
+      if (kb > 0 && et == 0) mbar_arrive(&empty[stage == 0 ? NSTAGE - 1 : stage - 1]);
       if (++stage == NSTAGE) {
         stage = 0;
         phase ^= 1;
@@ -729,8 +619,28 @@ gemm_tc_pool_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_con
     wg_wait<0>();
     wg_fence_acc(acc[0]);
     wg_fence_acc(acc[1]);
-    if (et == 0) mbar_arrive(&empty[prev]);
-    tc_pool_epilogue_tile<BN, EPI>(a, params, chunk, pool_stage, acc, bar, mt, nt * BN, quad, lane, et, a.n_tiles > 1 || n == 0);
+    if (et == 0) mbar_arrive(&empty[stage == 0 ? NSTAGE - 1 : stage - 1]);
+    const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
+    if constexpr (POOLING) {
+      tc_pool_epilogue_tile<BN, EPI>(a, params, chunk, pool_stage, acc, bar, mt, nt * BN, quad, lane, et, a.n_tiles > 1 || n == 0);
+    } else {
+      // accumulator -> the shared tile, once the other consumer's epilogue has read it; fragment (tc_ptx.cuh): acc[h][4 j + e]
+      // is row 64 h + 16 quad + lane / 4 + 8 (e / 2), column 8 j + 2 (lane % 4) + e % 2
+      named_sync(acc_free, 256);
+#pragma unroll
+      for (int h = 0; h < 2; h++) {
+        const int r0 = 64 * h + 16 * quad + (lane >> 2);
+#pragma unroll
+        for (int j = 0; j < BN / 8; j++) {
+          const int col = 8 * j + 2 * (lane & 3);
+          *reinterpret_cast<float2*>(acc_s + r0 * S::ACC_LD + col) = make_float2(acc[h][4 * j], acc[h][4 * j + 1]);
+          *reinterpret_cast<float2*>(acc_s + (r0 + 8) * S::ACC_LD + col) = make_float2(acc[h][4 * j + 2], acc[h][4 * j + 3]);
+        }
+      }
+      named_sync(bar, 128);
+      tc_epilogue_tile<BN, EPI>(a, params, acc_s + et * S::ACC_LD, bar, mt, nt * BN, quad, lane, et, a.n_tiles > 1 || n == 0);
+      named_arrive(acc_free_other, 256);
+    }
   }
 }
 
@@ -794,9 +704,9 @@ static unsigned* tile_counter(cudaStream_t st) {
   return static_cast<unsigned*>(base) + 2 * slot;
 }
 
-// operand maps and kernel arguments of one launch; tiles of `bn` columns and `bk`-wide k-blocks
-static int tc_setup(const TcGemm& g, int bn, int bk, int epi, CUtensorMap* maps, TcArgs& a) {
-  const int Ktot = g.KW * g.Cin;
+// operand maps and kernel arguments of one launch; tiles of `bn` columns
+static int tc_setup(const TcGemm& g, int bn, int epi, CUtensorMap* maps, TcArgs& a) {
+  const int Ktot = g.KW * g.Cin, bk = TC_BK;
   if (make_map(&maps[0], g.A_hi, g.Mtot, g.Cin, g.lda, bk, TC_BM) || make_map(&maps[1], g.A_lo, g.Mtot, g.Cin, g.lda, bk, TC_BM) ||
       make_map(&maps[2], g.W_hi, g.Npad, Ktot, Ktot, bk, bn) || make_map(&maps[3], g.W_lo, g.Npad, Ktot, Ktot, bk, bn))
     return -2;
@@ -834,38 +744,28 @@ static int launch_tc(const TcGemm& g, cudaStream_t st) {
   using S = TcSmem<BN>;
   CUtensorMap m[4];
   TcArgs a;
-  if (tc_setup(g, BN, TC_BK, EPI, m, a)) return -2;
+  if (tc_setup(g, BN, EPI, m, a)) return -2;
+  if (tc_pooling(EPI) && !(a.tile_ctr = tile_counter(st))) return -2;
   auto kern = gemm_tc_kernel<BN, EPI>;
   static bool attr_done[64] = {};
   if (first_use_on_device(attr_done))
-    DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::TOTAL));
-  kern<<<tc_grid(a), TC_THREADS, S::TOTAL, st>>>(m[0], m[1], m[2], m[3], a);
-  DG_LAUNCHED();
-  return 0;
-}
-
-template <int BN, int EPI>
-static int launch_tc_pool(const TcGemm& g, cudaStream_t st) {
-  using S = TcPoolSmem<BN>;
-  CUtensorMap m[4];
-  TcArgs a;
-  if (tc_setup(g, BN, TC_POOL_BK, EPI, m, a)) return -2;
-  if (!(a.tile_ctr = tile_counter(st))) return -2;
-  auto kern = gemm_tc_pool_kernel<BN, EPI>;
-  static bool attr_done[64] = {};
-  if (first_use_on_device(attr_done))
     DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::total(EPI)));
-  kern<<<tc_grid(a), TC_POOL_THREADS, S::total(EPI), st>>>(m[0], m[1], m[2], m[3], a);
+  kern<<<tc_grid(a), TC_THREADS, S::total(EPI), st>>>(m[0], m[1], m[2], m[3], a);
   DG_LAUNCHED();
   return 0;
 }
 
 int launch_gemm_tc(const TcGemm& g, cudaStream_t st) {
   ProfScope _ps(g.tag ? g.tag : "gemm_tc", st);
-  if (g.Cin % TC_BK || g.lda % 8 || g.ldc % (g.epi == TC_LEAKY_BN_SPLIT ? 8 : 4) || (g.Npad % 128 && g.Npad != 64 && g.Npad != 32) ||
+  if (g.Cin % 64 || g.lda % 8 || g.ldc % (g.epi == TC_LEAKY_BN_SPLIT ? 8 : 4) || (g.Npad % 128 && g.Npad != 64 && g.Npad != 32) ||
       g.KW < 1 || g.KW > 9) {
     set_error("gemm_tc: Cin must be a multiple of 64, A pitch a multiple of 8, output pitch a multiple of 4 "
               "(8 for 16-bit planes), padded N 32, 64 or a multiple of 128, at most 9 taps");
+    return -1;
+  }
+  if (g.epi == TC_LEAKY_BN_SPLIT && g.N % 32) {
+    // the epilogue stores the planes 32 columns at a time: a partial group would overwrite the start of the next row
+    set_error("gemm_tc (planes): N must be a multiple of 32");
     return -1;
   }
   if (g.epi == TC_CONV2D) {
@@ -882,7 +782,7 @@ int launch_gemm_tc(const TcGemm& g, cudaStream_t st) {
       set_error("gemm_tc (pool): needs 128-wide tiles, 1..4 speakers and items of at least 128 rows");
       return -1;
     }
-    return launch_tc_pool<128, TC_POOL>(g, st);
+    return launch_tc<128, TC_POOL>(g, st);
   }
   if (g.epi == TC_MAXPOOL3) {
     if (g.Npad != 64 || !g.out_f32 || !g.pool_part || g.pool3_T < 1 || g.pool3_tile_rows < 3 || g.pool3_tile_rows > 126 ||
@@ -890,7 +790,7 @@ int launch_gemm_tc(const TcGemm& g, cudaStream_t st) {
       set_error("gemm_tc (maxpool3): needs 64 output channels and tiles of 3..126 rows (a multiple of 3) that divide the item");
       return -1;
     }
-    return launch_tc_pool<64, TC_MAXPOOL3>(g, st);
+    return launch_tc<64, TC_MAXPOOL3>(g, st);
   }
   if (g.Npad == 64 && g.epi == TC_BIAS_F32) return launch_tc<64, TC_BIAS_F32>(g, st);
   switch (g.epi) {

@@ -355,6 +355,11 @@ int dg_profile_enable(int enable);
 /* test hook: the same random shifted-window GEMM through the float32 reference kernel and the wgmma (fp16 hi/lo,
  * three products) kernel; epi 0 = bias -> f32, 1 = bias+leaky+bn -> fp16 hi/lo planes, 2 = bias+leaky+bn -> f32. */
 int dg_selftest_gemm_tc(int M, int Cin, int KW, int dil, int N, int epi, float* max_abs_diff, float* out_rms);
+/* test hook: one seeded wgmma GEMM with epilogue epi (0..5) under SM caps 0, 1, 3 and 7; *equal = 1 if every output (float32
+ * rows, hi/lo planes, pooling partial sums) is byte-equal across the four grids.  epi 3: 3 x 3 Conv2d, KW = 9, dil = side
+ * of the square zero-padded maps (M a multiple of dil^2); epi 4: 3 speakers, items of 296 rows; epi 5: N <= 64, items of
+ * 888 rows (M a multiple of 888). */
+int dg_selftest_gemm_tc_grid(int M, int Cin, int KW, int dil, int N, int epi, int* equal);
 /* test hook (host only, no GPU): the weight-side split of float32 values into the two IEEE fp16 operand planes
  * (hi = rn16(x), lo = rn16(x - hi), saturating).  What the device does to activations with cvt.rn.satfinite.f16.f32. */
 int dg_selftest_split_f16_host(const float* x, long long n, unsigned short* hi, unsigned short* lo);
