@@ -320,3 +320,89 @@ extern "C" int dg_selftest_gemm_tc_grid(int M, int Cin, int KW, int dil, int N, 
   }
   return DG_OK;
 }
+
+// Runs one seeded GEMM (one tap, epilogue 0, 1 or 2) twice: into outputs of pitch N, and into outputs of pitch N + 40 with
+// 130 guard rows after M, all bytes preset to a sentinel.  Sets *outside_unchanged = 1 if the second run changed no byte
+// outside rows [0, M) x columns [0, N), *equal = 1 if inside them it wrote the first run's bytes, and *refused = 1 if the
+// launcher rejects, with DG_EINVAL and without writing, an output base 4 (float32) or 2 (planes) bytes off 16-byte
+// alignment and a pitch whose byte size is not a multiple of 16.
+extern "C" int dg_selftest_gemm_tc_bounds(int M, int Cin, int N, int epi, int* outside_unchanged, int* equal, int* refused) {
+  const bool planes = epi == 1;
+  if (M < 1 || Cin < 64 || Cin % 64 || N < 1 || N % (planes ? 32 : 4) || epi < 0 || epi > 2 || !outside_unchanged || !equal ||
+      !refused) {
+    set_error("dg_selftest_gemm_tc_bounds: bad arguments");
+    return DG_EINVAL;
+  }
+  const int npad = N <= 64 && epi == 0 ? 64 : (N + 127) / 128 * 128, esize = planes ? 2 : 4;   // 64-wide tiles: epi 0 only
+  const int ldc = N + 40;
+  const long long rows = (long long)M + 130;
+  uint32_t seed = 4242u;
+  auto rnd = [&]() {
+    seed = seed * 1664525u + 1013904223u;
+    return ((seed >> 8) & 0xFFFF) / 65536.f - 0.5f;
+  };
+  std::vector<float> A((size_t)M * Cin), Wnk((size_t)N * Cin), bias(N), bsc(N), bsh(N);
+  for (auto& v : A) v = 2.f * rnd();
+  for (auto& v : Wnk) v = 0.25f * rnd();
+  for (int n = 0; n < N; n++) {
+    bias[n] = rnd();
+    bsc[n] = 1.f + rnd();
+    bsh[n] = rnd();
+  }
+  const size_t dense_bytes = (size_t)M * N * esize, wide_bytes = (size_t)rows * ldc * esize + 16;
+  DevBuf dA, dAh, dAl, dB, dS, dH, dD0, dD1, dW0, dW1;
+  WeightPlanes dW;
+  if (upload(dA, A) || upload(dB, bias) || upload(dS, bsc) || upload(dH, bsh) || upload_split(dW, Wnk, N, npad, Cin) ||
+      dAh.ensure((size_t)M * Cin * 2) || dAl.ensure((size_t)M * Cin * 2) || dD0.ensure(dense_bytes) ||
+      dD1.ensure(dense_bytes) || dW0.ensure(wide_bytes) || dW1.ensure(wide_bytes))
+    return DG_ECUDA;
+  int rc;
+  if ((rc = launch_split_ex(dA.as<float>(), M, Cin, Cin, Cin, 0, 1, nullptr, nullptr, dAh.p, dAl.p, nullptr))) return rc;
+  TcGemm t{};
+  t.A_hi = dAh.p; t.A_lo = dAl.p; t.lda = Cin; t.Cin = Cin; t.KW = 1; t.dil = 1; t.Mtot = M; t.M = M;
+  t.N = N; t.bias = dB.as<float>(); t.bn_scale = dS.as<float>(); t.bn_shift = dH.as<float>();
+  t.epi = epi; t.tag = "selftest_tc_bounds";
+  if ((rc = set_weights(t, dW))) return rc;
+  // output 0 (float32 rows or hi plane) and 1 (lo plane) at `off` bytes into the buffers, pitch `ld`
+  auto point = [&](DevBuf& o0, DevBuf& o1, size_t off, int ld) {
+    unsigned char* b0 = static_cast<unsigned char*>(o0.p) + off;
+    unsigned char* b1 = static_cast<unsigned char*>(o1.p) + off;
+    t.out_f32 = planes ? nullptr : reinterpret_cast<float*>(b0);
+    t.out_hi = planes ? b0 : nullptr;
+    t.out_lo = planes ? b1 : nullptr;
+    t.ldc = ld;
+  };
+  const unsigned char SENTINEL = 0xA5;
+  DG_CUDA(cudaMemset(dW0.p, SENTINEL, wide_bytes));
+  DG_CUDA(cudaMemset(dW1.p, SENTINEL, wide_bytes));
+  point(dD0, dD1, 0, N);
+  if ((rc = launch_gemm_tc(t, nullptr))) return rc;
+  point(dW0, dW1, 0, ldc);
+  if ((rc = launch_gemm_tc(t, nullptr))) return rc;
+  // refusals: base off alignment, pitch off 16 bytes (both leave the sentinel in place)
+  point(dW0, dW1, (size_t)esize, ldc);
+  const int rc_base = launch_gemm_tc(t, nullptr);
+  point(dW0, dW1, 0, ldc + (planes ? 4 : 2));
+  const int rc_pitch = launch_gemm_tc(t, nullptr);
+  DG_CUDA(cudaDeviceSynchronize());
+  const int n_out = planes ? 2 : 1;
+  std::vector<unsigned char> dense(dense_bytes), wide(wide_bytes);
+  *outside_unchanged = 1;
+  *equal = 1;
+  for (int o = 0; o < n_out; o++) {
+    DG_CUDA(cudaMemcpy(dense.data(), (o ? dD1 : dD0).p, dense_bytes, cudaMemcpyDeviceToHost));
+    DG_CUDA(cudaMemcpy(wide.data(), (o ? dW1 : dW0).p, wide_bytes, cudaMemcpyDeviceToHost));
+    const size_t row_bytes = (size_t)N * esize, pitch = (size_t)ldc * esize;
+    for (long long r = 0; r < rows; r++) {
+      const unsigned char* w = wide.data() + r * pitch;
+      const bool inside = r < M;
+      if (inside && memcmp(w, dense.data() + r * row_bytes, row_bytes)) *equal = 0;
+      for (size_t b = inside ? row_bytes : 0; b < pitch; b++)
+        if (w[b] != SENTINEL) *outside_unchanged = 0;
+    }
+    for (size_t b = (size_t)rows * pitch; b < wide_bytes; b++)
+      if (wide[b] != SENTINEL) *outside_unchanged = 0;
+  }
+  *refused = rc_base == DG_EINVAL && rc_pitch == DG_EINVAL;
+  return DG_OK;
+}

@@ -25,12 +25,16 @@
 // the pooling epilogues (TC_POOL, TC_MAXPOOL3), whose cross-row reductions take about as long as the tile's MMAs, take
 // tiles in m-major order from a per-stream atomic counter (a CTA that becomes resident late runs fewer tiles).
 // Epilogues:
-//   element-wise    the two consumers share ONE full-tile staging buffer, [128][BN + 4] float32.  A consumer waits until
-//                   the other one has finished reading it (a named-barrier pair), writes its whole accumulator there and
-//                   runs the epilogue from it (row m of the tile -> thread m): bias, LeakyReLU, BatchNorm affine, then
-//                   float32 rows or the next layer's hi/lo 16-bit planes.  The accumulator is dead during the epilogue, so
-//                   it does not compete with the epilogue for registers.  One buffer is enough: a consumer needs it only
-//                   after its own mainloop, and the other consumer runs its epilogue during that mainloop.
+//   element-wise    the two consumers share ONE full-tile staging buffer.  A consumer waits until the other one's data has
+//                   left it (a named-barrier pair), then
+//                   - bias, LeakyReLU + BatchNorm -> float32 rows or the next layer's hi/lo 16-bit planes: applies the
+//                     epilogue to its accumulator fragments in registers and writes the results into 128B-swizzled boxes
+//                     (float32: 32 columns x 128 rows; planes: 64 x 128 per plane), which one thread stores with TMA.  The
+//                     hardware clips the boxes at rows M and columns N.  The buffer is handed on once TMA has read it.
+//                   - Conv2d: writes its whole accumulator as [128][BN + 4] float32 and runs the epilogue from it (row m of
+//                     the tile -> thread m: output-row remapping, residual reads, stride-2 subsampling).
+//                   One buffer is enough: a consumer needs it only after its own mainloop, and the other consumer runs its
+//                   epilogue during that mainloop.
 //   pooling         the accumulator goes to the consumer's own shared memory 64 columns at a time, already through bias /
 //                   LeakyReLU / BatchNorm (TC_POOL) or the weight scale (TC_MAXPOOL3).
 // Every output element gets the same wgmma sequence (k order, lo.hi, hi.lo, hi.hi per k-step) and the same epilogue
@@ -67,7 +71,6 @@ struct TcArgs {
   __nv_bfloat16* out_lo;
   int ldc;
   float acc_scale;      // 1 / (power-of-two scale of the weight planes): applied to the accumulator in the epilogue
-  int vec8;             // output rows are 32-byte aligned: 32 bytes per lane and store pair
   int tap_off[9];       // row offset of every tap (Conv1d: j * dil; Conv2d on a zero-padded map: (dw-1) * Hp + (dh-1))
   // TC_CONV2D: rows are positions (item, w, h) of a zero-padded [Wp][Hp] map; outputs go to the padded map [Wop][Hop] of the
   // next layer (stride 1: same geometry; stride 2: computed at every centre, only odd (w, h) are kept)
@@ -89,9 +92,12 @@ struct TcArgs {
 enum TcEpi { TC_BIAS_F32 = 0, TC_LEAKY_BN_SPLIT = 1, TC_LEAKY_BN_F32 = 2, TC_CONV2D = 3, TC_POOL = 4, TC_MAXPOOL3 = 5 };
 
 __host__ __device__ constexpr bool tc_pooling(int epi) { return epi == TC_POOL || epi == TC_MAXPOOL3; }
+// epilogues whose output tile leaves as TMA boxes
+__host__ __device__ constexpr bool tc_box_store(int epi) { return epi == TC_BIAS_F32 || epi == TC_LEAKY_BN_SPLIT || epi == TC_LEAKY_BN_F32; }
 
-// Layout: [NSTAGE stages of (A hi, A lo, W hi, W lo)] [barriers] [consumer 0: parameters | pooling: chunk | pooling staging]
-// [consumer 1: the same] [element-wise: the shared accumulator tile]
+// Layout: [NSTAGE stages of (A hi, A lo, W hi, W lo)] [element-wise: the shared staging tile] [barriers] [consumer 0:
+// parameters | pooling: chunk | pooling staging] [consumer 1: the same].  Stages and staging tile are multiples of 1 KB,
+// so the staging tile keeps the 1 KB alignment of 128B-swizzled boxes.
 template <int BN>
 struct TcSmem {
   static constexpr int A_BYTES = TC_BM * TC_BK * 2;     // 8 KB per plane
@@ -107,16 +113,89 @@ struct TcSmem {
   // TC_POOL: row weights [128][4] + cross-row-group staging [4][2][8][32]; TC_MAXPOOL3: staging [4][2][2][32]
   __host__ __device__ static constexpr int extra_floats(int epi) { return epi == TC_POOL ? 128 * 4 + 4 * 2 * 8 * 32 : (epi == TC_MAXPOOL3 ? 4 * 2 * 2 * 32 : 0); }
   __host__ __device__ static constexpr int consumer_floats(int epi) { return PARAM_FLOATS + (tc_pooling(epi) ? CHUNK_FLOATS + extra_floats(epi) : 0); }
-  // element-wise: the finished accumulator, one float32 row per tile row (+4 floats: 128-bit row reads without bank conflicts)
+  // Conv2d: the finished accumulator, one float32 row per tile row (+4 floats: 128-bit row reads without bank conflicts)
   static constexpr int ACC_LD = BN + 4;
-  __host__ __device__ static constexpr int acc_floats(int epi) { return tc_pooling(epi) ? 0 : TC_BM * ACC_LD; }
+  // box epilogues: 16 KB boxes of 128 rows x 128 bytes, float32 [BN / 32] or hi [BN / 64] then lo [BN / 64]
+  static constexpr int BOX_BYTES = TC_BM * 128;
+  __host__ __device__ static constexpr int stage_tile_bytes(int epi) {
+    return tc_pooling(epi) ? 0 : (epi == TC_CONV2D ? TC_BM * ACC_LD * 4 : TC_BM * BN * 4);
+  }
   __host__ __device__ static constexpr int total(int epi) {
-    return NSTAGE * STAGE_BYTES + BAR_BYTES + (2 * consumer_floats(epi) + acc_floats(epi)) * 4 + 1024;   // + alignment slack
+    return NSTAGE * STAGE_BYTES + stage_tile_bytes(epi) + BAR_BYTES + 2 * consumer_floats(epi) * 4 + 1024;   // + alignment slack
   }
 };
 static_assert(TcSmem<128>::total(TC_POOL) <= TC_SMEM_MAX && TcSmem<64>::total(TC_MAXPOOL3) <= TC_SMEM_MAX &&
               TcSmem<128>::total(TC_CONV2D) <= TC_SMEM_MAX && TcSmem<64>::total(TC_CONV2D) <= TC_SMEM_MAX &&
-              TcSmem<32>::total(TC_CONV2D) <= TC_SMEM_MAX, "gemm_tc: shared memory");
+              TcSmem<32>::total(TC_CONV2D) <= TC_SMEM_MAX && TcSmem<128>::total(TC_BIAS_F32) <= TC_SMEM_MAX,
+              "gemm_tc: shared memory");
+
+// Per-column parameters of the element-wise epilogues (bias | bn_scale | bn_shift) of the tile at column n0, staged by the
+// 128 threads of a consumer warpgroup.  With a single column tile they are the same for every tile of the warpgroup: staged
+// once.
+template <int BN, int EPI>
+__device__ __forceinline__ void tc_stage_params(const TcArgs& a, float* params, int bar, int n0, int et) {
+  named_sync(bar, 128);
+  for (int i = et; i < BN; i += 128) {
+    const int n = n0 + i;
+    const bool ok = n < a.N;
+    params[i] = (ok && a.bias) ? a.bias[n] : 0.f;
+    constexpr bool has_bn = EPI != TC_BIAS_F32;
+    params[BN + i] = (ok && has_bn) ? a.bn_scale[n] * (EPI == TC_CONV2D ? a.acc_scale : 1.f) : 1.f;   // (2^-k: exact)
+    params[2 * BN + i] = (ok && has_bn) ? a.bn_shift[n] : 0.f;
+  }
+  named_sync(bar, 128);
+}
+
+// ------------------------------------------------------------------------------------ the box epilogue of one 128-row tile
+// bias -> float32 rows, or bias -> LeakyReLU -> BatchNorm affine -> float32 rows / hi/lo planes, applied to the accumulator
+// fragments of the 128 threads of a consumer warpgroup and written into the 128B-swizzled boxes of `tile`.
+// Fragment (tc_ptx.cuh): acc[h][4 j + e] is row 64 h + 16 quad + lane / 4 + 8 (e / 2), column 8 j + 2 (lane % 4) + e % 2.
+// 128B swizzle: the 16-byte chunk q of box row r sits at chunk q ^ (r % 8), and r % 8 = lane / 4 for every row of a thread.
+// A warp's stores of one (h, e / 2, j) cover 8 rows x 32 bytes (float32) or 8 rows x 16 bytes per plane: no bank conflicts
+// beyond the minimum wavefronts.
+template <int BN, int EPI>
+__device__ __forceinline__ void tc_box_epilogue(const TcArgs& a, const float* params, float (&acc)[2][BN / 2],
+                                                uint32_t tile, int quad, int lane) {
+  using S = TcSmem<BN>;
+  const int r0 = 16 * quad + (lane >> 2), sw = lane >> 2, cq = lane & 3;
+#pragma unroll
+  for (int j = 0; j < BN / 8; j++) {
+    const int col = 8 * j + 2 * cq;
+    const float2 bias = *reinterpret_cast<const float2*>(params + col);
+    float2 bsc = make_float2(1.f, 1.f), bsh = make_float2(0.f, 0.f);
+    if (EPI != TC_BIAS_F32) {
+      bsc = *reinterpret_cast<const float2*>(params + BN + col);
+      bsh = *reinterpret_cast<const float2*>(params + 2 * BN + col);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+#pragma unroll
+      for (int e2 = 0; e2 < 2; e2++) {
+        const int row = 64 * h + r0 + 8 * e2;
+        float x0 = fmaf(acc[h][4 * j + 2 * e2], a.acc_scale, bias.x);
+        float x1 = fmaf(acc[h][4 * j + 2 * e2 + 1], a.acc_scale, bias.y);
+        if (EPI != TC_BIAS_F32) {
+          x0 = fmaf(leaky(x0), bsc.x, bsh.x);
+          x1 = fmaf(leaky(x1), bsc.y, bsh.y);
+        }
+        if (EPI == TC_LEAKY_BN_SPLIT) {
+          // box j / 8 of each plane (64 columns), row bytes 16 (j % 8) + 4 cq
+          uint16_t h0, l0, h1, l1;
+          split_h16(x0, h0, l0);
+          split_h16(x1, h1, l1);
+          const int off = (j / 8) * S::BOX_BYTES + row * 128 + (((j & 7) ^ sw) << 4) + 4 * cq;
+          st_shared_u32(tile + off, pack_u16x2(h0, h1));
+          st_shared_u32(tile + (BN / 64) * S::BOX_BYTES + off, pack_u16x2(l0, l1));
+        } else {
+          // box j / 4 (32 columns), row bytes 32 (j % 4) + 8 cq
+          const int q = 2 * (j & 3) + (cq >> 1);
+          const int off = (j / 4) * S::BOX_BYTES + row * 128 + ((q ^ sw) << 4) + 8 * (cq & 1);
+          st_shared_v2(tile + off, x0, x1);
+        }
+      }
+    }
+  }
+}
 
 // 32 consecutive accumulator columns of this thread's row
 __device__ __forceinline__ void acc_ld32(const float* p, uint32_t (&r)[32]) {
@@ -130,32 +209,17 @@ __device__ __forceinline__ void acc_ld32(const float* p, uint32_t (&r)[32]) {
   }
 }
 
-// ------------------------------------------------------------------------------------ the epilogue of one 128-row tile
+// ------------------------------------------------------------------------------------ the Conv2d epilogue of one 128-row tile
 // Executed by the 128 threads of a consumer warpgroup; thread et = 32 quad + lane owns row et of the tile.  `mt` = index
-// of the 128-row tile (rows mt * 128 ..), `acc_row` = this thread's row of the finished accumulator in shared memory,
-// `bar` = the warpgroup's named barrier.
-template <int BN, int EPI>
-__device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params, const float* acc_row, int bar,
-                                                 long long mt, int n0, int quad, int lane, int et, bool stage_params) {
+// of the 128-row tile (rows mt * 128 ..), `acc_row` = this thread's row of the finished accumulator in shared memory.
+template <int BN>
+__device__ __forceinline__ void tc_conv2d_epilogue_tile(const TcArgs& a, const float* params, const float* acc_row,
+                                                        long long mt, int n0, int quad, int lane) {
     const long long m = mt * TC_BM + quad * 32 + lane;
-    // stage the per-column parameters of this tile; with a single column tile they are the same for every tile of this
-    // warpgroup: staged once
-    if (stage_params) {
-      named_sync(bar, 128);
-      for (int i = et; i < BN; i += 128) {
-        const int n = n0 + i;
-        const bool ok = n < a.N;
-        params[i] = (ok && a.bias) ? a.bias[n] : 0.f;
-        constexpr bool has_bn = EPI != TC_BIAS_F32;
-        params[BN + i] = (ok && has_bn) ? a.bn_scale[n] * (EPI == TC_CONV2D ? a.acc_scale : 1.f) : 1.f;   // (2^-k: exact)
-        params[2 * BN + i] = (ok && has_bn) ? a.bn_shift[n] : 0.f;
-      }
-      named_sync(bar, 128);
-    }
-    // TC_CONV2D: output position of this row
+    // output position of this row
     long long mo = m;                 // output row
     bool row_ok = m < a.M;
-    if (EPI == TC_CONV2D) {
+    {
       const unsigned mu = (unsigned)m, per = (unsigned)(a.Wp * a.Hp);     // (the launcher checks M < 2^31)
       const unsigned item = mu / per, rem = mu - item * per;
       const int w = (int)(rem / (unsigned)a.Hp), h = (int)(rem - (unsigned)w * (unsigned)a.Hp);
@@ -171,67 +235,35 @@ __device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params,
       acc_ld32(acc_row + c, r);
       if (n0 + c >= a.N) continue;
       float v[32];
-      if (EPI == TC_CONV2D) {
-        // BatchNorm2d(eval) affine -> (+ residual) -> ReLU
+      // BatchNorm2d(eval) affine -> (+ residual) -> ReLU
 #pragma unroll
-        for (int i = 0; i < 32; i++) v[i] = fmaf(__uint_as_float(r[i]), params[BN + c + i], params[2 * BN + c + i]);
-        if (row_ok && a.res_hi) {
-          const uint4* rh = reinterpret_cast<const uint4*>(a.res_hi + mo * a.ldc + n0 + c);
-          const uint4* rl = reinterpret_cast<const uint4*>(a.res_lo + mo * a.ldc + n0 + c);
+      for (int i = 0; i < 32; i++) v[i] = fmaf(__uint_as_float(r[i]), params[BN + c + i], params[2 * BN + c + i]);
+      if (row_ok && a.res_hi) {
+        const uint4* rh = reinterpret_cast<const uint4*>(a.res_hi + mo * a.ldc + n0 + c);
+        const uint4* rl = reinterpret_cast<const uint4*>(a.res_lo + mo * a.ldc + n0 + c);
 #pragma unroll
-          for (int q = 0; q < 4; q++) {
-            const uint4 hq = rh[q], lq = rl[q];
-            const uint32_t hw[4] = {hq.x, hq.y, hq.z, hq.w}, lw[4] = {lq.x, lq.y, lq.z, lq.w};
+        for (int q = 0; q < 4; q++) {
+          const uint4 hq = rh[q], lq = rl[q];
+          const uint32_t hw[4] = {hq.x, hq.y, hq.z, hq.w}, lw[4] = {lq.x, lq.y, lq.z, lq.w};
 #pragma unroll
-            for (int e = 0; e < 4; e++) {
-              v[8 * q + 2 * e] += h16_to_f32((uint16_t)(hw[e] & 0xFFFFu)) + h16_to_f32((uint16_t)(lw[e] & 0xFFFFu));
-              v[8 * q + 2 * e + 1] += h16_to_f32((uint16_t)(hw[e] >> 16)) + h16_to_f32((uint16_t)(lw[e] >> 16));
-            }
+          for (int e = 0; e < 4; e++) {
+            v[8 * q + 2 * e] += h16_to_f32((uint16_t)(hw[e] & 0xFFFFu)) + h16_to_f32((uint16_t)(lw[e] & 0xFFFFu));
+            v[8 * q + 2 * e + 1] += h16_to_f32((uint16_t)(hw[e] >> 16)) + h16_to_f32((uint16_t)(lw[e] >> 16));
           }
         }
-        if (a.relu) {
-#pragma unroll
-          for (int i = 0; i < 32; i++) v[i] = fmaxf(v[i], 0.f);
-        }
-        if (row_ok) {
-          if (a.out_f32) {
-            float* po = a.out_f32 + mo * a.ldc + n0 + c;
-#pragma unroll
-            for (int i = 0; i < 8; i++)
-              reinterpret_cast<float4*>(po)[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-          }
-          if (a.out_hi) {
-            uint32_t hi[16], lo[16];
-#pragma unroll
-            for (int i = 0; i < 16; i++) {
-              uint16_t h0, l0, h1, l1;
-              split_h16(v[2 * i], h0, l0);
-              split_h16(v[2 * i + 1], h1, l1);
-              hi[i] = pack_u16x2(h0, h1);
-              lo[i] = pack_u16x2(l0, l1);
-            }
-            uint4* ph = reinterpret_cast<uint4*>(a.out_hi + mo * a.ldc + n0 + c);
-            uint4* pl = reinterpret_cast<uint4*>(a.out_lo + mo * a.ldc + n0 + c);
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-              ph[i] = make_uint4(hi[4 * i], hi[4 * i + 1], hi[4 * i + 2], hi[4 * i + 3]);
-              pl[i] = make_uint4(lo[4 * i], lo[4 * i + 1], lo[4 * i + 2], lo[4 * i + 3]);
-            }
-          }
-        }
-        continue;
       }
+      if (a.relu) {
 #pragma unroll
-      for (int i = 0; i < 32; i++) {
-        float x = fmaf(__uint_as_float(r[i]), a.acc_scale, params[c + i]);
-        if (EPI != TC_BIAS_F32) {
-          x = leaky(x);
-          x = fmaf(x, params[BN + c + i], params[2 * BN + c + i]);
-        }
-        v[i] = x;
+        for (int i = 0; i < 32; i++) v[i] = fmaxf(v[i], 0.f);
       }
-      if (m < a.M) {
-        if (EPI == TC_LEAKY_BN_SPLIT) {
+      if (row_ok) {
+        if (a.out_f32) {
+          float* po = a.out_f32 + mo * a.ldc + n0 + c;
+#pragma unroll
+          for (int i = 0; i < 8; i++)
+            reinterpret_cast<float4*>(po)[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
+        }
+        if (a.out_hi) {
           uint32_t hi[16], lo[16];
 #pragma unroll
           for (int i = 0; i < 16; i++) {
@@ -241,39 +273,12 @@ __device__ __forceinline__ void tc_epilogue_tile(const TcArgs& a, float* params,
             hi[i] = pack_u16x2(h0, h1);
             lo[i] = pack_u16x2(l0, l1);
           }
-          uint4* ph = reinterpret_cast<uint4*>(a.out_hi + m * a.ldc + n0 + c);
-          uint4* pl = reinterpret_cast<uint4*>(a.out_lo + m * a.ldc + n0 + c);
-          if (a.vec8) {
+          uint4* ph = reinterpret_cast<uint4*>(a.out_hi + mo * a.ldc + n0 + c);
+          uint4* pl = reinterpret_cast<uint4*>(a.out_lo + mo * a.ldc + n0 + c);
 #pragma unroll
-            for (int i = 0; i < 2; i++) {
-              st_global_v8(ph + 2 * i, hi[8 * i], hi[8 * i + 1], hi[8 * i + 2], hi[8 * i + 3], hi[8 * i + 4], hi[8 * i + 5],
-                           hi[8 * i + 6], hi[8 * i + 7]);
-              st_global_v8(pl + 2 * i, lo[8 * i], lo[8 * i + 1], lo[8 * i + 2], lo[8 * i + 3], lo[8 * i + 4], lo[8 * i + 5],
-                           lo[8 * i + 6], lo[8 * i + 7]);
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-              ph[i] = make_uint4(hi[4 * i], hi[4 * i + 1], hi[4 * i + 2], hi[4 * i + 3]);
-              pl[i] = make_uint4(lo[4 * i], lo[4 * i + 1], lo[4 * i + 2], lo[4 * i + 3]);
-            }
-          }
-        } else {
-          float* po = a.out_f32 + m * a.ldc + n0 + c;
-          if (n0 + c + 32 <= a.N && a.vec8) {
-#pragma unroll
-            for (int i = 0; i < 4; i++)
-              st_global_v8(po + 8 * i, __float_as_uint(v[8 * i]), __float_as_uint(v[8 * i + 1]), __float_as_uint(v[8 * i + 2]),
-                           __float_as_uint(v[8 * i + 3]), __float_as_uint(v[8 * i + 4]), __float_as_uint(v[8 * i + 5]),
-                           __float_as_uint(v[8 * i + 6]), __float_as_uint(v[8 * i + 7]));
-          } else if (n0 + c + 32 <= a.N) {
-#pragma unroll
-            for (int i = 0; i < 8; i++)
-              reinterpret_cast<float4*>(po)[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-          } else {
-#pragma unroll
-            for (int i = 0; i < 32; i++)
-              if (n0 + c + i < a.N) po[i] = v[i];
+          for (int i = 0; i < 4; i++) {
+            ph[i] = make_uint4(hi[4 * i], hi[4 * i + 1], hi[4 * i + 2], hi[4 * i + 3]);
+            pl[i] = make_uint4(lo[4 * i], lo[4 * i + 1], lo[4 * i + 2], lo[4 * i + 3]);
           }
         }
       }
@@ -462,25 +467,27 @@ __device__ __forceinline__ void tc_pool_epilogue_tile(const TcArgs& a, float* pa
 // ------------------------------------------------------------------------------------ the kernel
 // Named barriers besides 0: 1 + c = the 128 threads of consumer c (epilogue staging); 3 + c = consumer c may issue its
 // mainloop (256 threads: consumer c waits, the other consumer arrives once its own MMAs are issued); element-wise
-// epilogues: 5 + c = consumer c may write the shared accumulator tile (256 threads: consumer c waits, the other consumer
-// arrives once its epilogue has read the tile).
+// epilogues: 5 + c = consumer c may write the shared staging tile (256 threads: consumer c waits, the other consumer
+// arrives once the tile has been read: by its epilogue threads (Conv2d) or by TMA (box epilogues)).
+// tmC0 / tmC1: output maps of the box epilogues (float32 rows; or hi and lo planes).
 template <int BN, int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
-               const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo, TcArgs a) {
+               const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo,
+               const __grid_constant__ CUtensorMap tmC0, const __grid_constant__ CUtensorMap tmC1, TcArgs a) {
   using S = TcSmem<BN>;
   constexpr bool POOLING = tc_pooling(EPI);
   constexpr int NSTAGE = S::NSTAGE;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + NSTAGE * S::STAGE_BYTES);
+  unsigned char* tile_s = smem + NSTAGE * S::STAGE_BYTES;   // element-wise: the staging tile, shared by the consumers
+  uint64_t* bars = reinterpret_cast<uint64_t*>(tile_s + S::stage_tile_bytes(EPI));
   uint64_t* full = bars;                      // [NSTAGE] TMA -> MMA
   uint64_t* empty = bars + NSTAGE;            // [NSTAGE] MMA -> TMA
   uint64_t* tile_full = bars + 2 * NSTAGE;    // [2] producer -> consumer c: tile_idx[c] holds its next tile
   uint64_t* tile_empty = tile_full + 2;       // [2] consumer c -> producer: tile_idx[c] has been read
   volatile int* tile_idx = reinterpret_cast<volatile int*>(tile_empty + 2);   // [2]
-  float* cons = reinterpret_cast<float*>(smem + NSTAGE * S::STAGE_BYTES + S::BAR_BYTES);
-  float* acc_s = cons + 2 * S::consumer_floats(EPI);   // element-wise: [128][ACC_LD], shared by the consumers
+  float* cons = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(bars) + S::BAR_BYTES);
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // warp-uniform
   const int wg = warp >> 2;
@@ -568,11 +575,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     mbar_wait(&tile_full[c], n & 1);
     const int tile = tile_idx[c];
     mbar_arrive(&tile_empty[c]);
+    // box epilogues: the parameters are staged before the mainloop, while the accumulator is not live
+    if (tc_box_store(EPI) && tile >= 0 && (a.n_tiles > 1 || n == 0))
+      tc_stage_params<BN, EPI>(a, params, bar, (tile - tile / a.n_tiles * a.n_tiles) * BN, et);
     named_sync(turn, 256);
     if (tile < 0) {
       if (tile == -1) {
         named_arrive(turn_other, 256);
-        // the last tile's consumer has handed the accumulator tile to this one: take that arrival
+        // the last tile's consumer has handed the staging tile to this one: take that arrival
         if (!POOLING) named_sync(acc_free, 256);
       }
       break;
@@ -621,11 +631,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     wg_fence_acc(acc[1]);
     if (et == 0) mbar_arrive(&empty[stage == 0 ? NSTAGE - 1 : stage - 1]);
     const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
+    const bool stage_params = a.n_tiles > 1 || n == 0;
     if constexpr (POOLING) {
-      tc_pool_epilogue_tile<BN, EPI>(a, params, chunk, pool_stage, acc, bar, mt, nt * BN, quad, lane, et, a.n_tiles > 1 || n == 0);
-    } else {
+      tc_pool_epilogue_tile<BN, EPI>(a, params, chunk, pool_stage, acc, bar, mt, nt * BN, quad, lane, et, stage_params);
+    } else if constexpr (EPI == TC_CONV2D) {
       // accumulator -> the shared tile, once the other consumer's epilogue has read it; fragment (tc_ptx.cuh): acc[h][4 j + e]
       // is row 64 h + 16 quad + lane / 4 + 8 (e / 2), column 8 j + 2 (lane % 4) + e % 2
+      float* acc_s = reinterpret_cast<float*>(tile_s);   // [128][ACC_LD]
       named_sync(acc_free, 256);
 #pragma unroll
       for (int h = 0; h < 2; h++) {
@@ -638,29 +650,60 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         }
       }
       named_sync(bar, 128);
-      tc_epilogue_tile<BN, EPI>(a, params, acc_s + et * S::ACC_LD, bar, mt, nt * BN, quad, lane, et, a.n_tiles > 1 || n == 0);
+      if (stage_params) tc_stage_params<BN, EPI>(a, params, bar, nt * BN, et);
+      tc_conv2d_epilogue_tile<BN>(a, params, acc_s + et * S::ACC_LD, mt, nt * BN, quad, lane);
+      named_arrive(acc_free_other, 256);
+    } else {
+      named_sync(acc_free, 256);          // the other consumer's boxes have been read by TMA
+      tc_box_epilogue<BN, EPI>(a, params, acc, smem_u32(tile_s), quad, lane);
+      fence_proxy_async_smem();
+      named_sync(bar, 128);
+      if (et == 0) {
+        const int m0 = mt * TC_BM, n0 = nt * BN;
+        if (EPI == TC_LEAKY_BN_SPLIT) {
+#pragma unroll
+          for (int b = 0; b < BN / 64; b++) {
+            if (n0 + 64 * b >= a.N) break;
+            tma_store_2d(&tmC0, tile_s + b * S::BOX_BYTES, n0 + 64 * b, m0);
+            tma_store_2d(&tmC1, tile_s + (BN / 64 + b) * S::BOX_BYTES, n0 + 64 * b, m0);
+          }
+        } else {
+#pragma unroll
+          for (int b = 0; b < BN / 32; b++) {
+            if (n0 + 32 * b >= a.N) break;
+            tma_store_2d(&tmC0, tile_s + b * S::BOX_BYTES, n0 + 32 * b, m0);
+          }
+        }
+        bulk_commit();
+        bulk_wait_read_all();
+      }
+      __syncwarp();
       named_arrive(acc_free_other, 256);
     }
   }
+  // the global writes of this consumer's last boxes complete before the CTA exits
+  if (tc_box_store(EPI) && et == 0) bulk_wait_all();
 }
 
 // ------------------------------------------------------------------------------------ host side
-// 16-bit matrix [rows, cols] row-major (cols contiguous, row pitch `ld` elements); box = box_cols x box_rows, swizzled by the
-// box row's width (64 or 128 bytes)
-static int make_map(CUtensorMap* m, const void* base, long long rows, int cols, int ld, int box_cols, int box_rows) {
+// 16-bit (or, `f32`, float32) matrix [rows, cols] row-major (cols contiguous, row pitch `ld` elements); box = box_cols x
+// box_rows, swizzled by the box row's width (64 or 128 bytes)
+static int make_map(CUtensorMap* m, const void* base, long long rows, int cols, int ld, int box_cols, int box_rows,
+                    bool f32 = false) {
   EncodeTiledFn fn = encode_fn();
   if (!fn) {
     set_error("cuTensorMapEncodeTiled is not available from the driver");
     return -2;
   }
+  const int esize = f32 ? 4 : 2;
   cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 2};
+  cuuint64_t strides[1] = {(cuuint64_t)ld * esize};
   cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  box_cols * 2 == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = fn(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims,
+                  strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  box_cols * esize == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("cuTensorMapEncodeTiled failed with code " + std::to_string((int)r));
     return -2;
@@ -704,12 +747,20 @@ static unsigned* tile_counter(cudaStream_t st) {
   return static_cast<unsigned*>(base) + 2 * slot;
 }
 
-// operand maps and kernel arguments of one launch; tiles of `bn` columns
+// operand maps, output maps (box epilogues: float32 rows, or hi and lo planes, as [M, N] of pitch ldc) and kernel arguments
+// of one launch; tiles of `bn` columns
 static int tc_setup(const TcGemm& g, int bn, int epi, CUtensorMap* maps, TcArgs& a) {
   const int Ktot = g.KW * g.Cin, bk = TC_BK;
   if (make_map(&maps[0], g.A_hi, g.Mtot, g.Cin, g.lda, bk, TC_BM) || make_map(&maps[1], g.A_lo, g.Mtot, g.Cin, g.lda, bk, TC_BM) ||
       make_map(&maps[2], g.W_hi, g.Npad, Ktot, Ktot, bk, bn) || make_map(&maps[3], g.W_lo, g.Npad, Ktot, Ktot, bk, bn))
     return -2;
+  memset(&maps[4], 0, 2 * sizeof(CUtensorMap));
+  if (epi == TC_LEAKY_BN_SPLIT) {
+    if (make_map(&maps[4], g.out_hi, g.M, g.N, g.ldc, 64, TC_BM) || make_map(&maps[5], g.out_lo, g.M, g.N, g.ldc, 64, TC_BM))
+      return -2;
+  } else if (tc_box_store(epi)) {
+    if (make_map(&maps[4], g.out_f32, g.M, g.N, g.ldc, 32, TC_BM, true)) return -2;
+  }
   a = TcArgs{};
   a.M = g.M; a.N = g.N; a.n_tiles = (g.N + bn - 1) / bn;
   a.tile_rows = epi == TC_MAXPOOL3 ? g.pool3_tile_rows : TC_BM;
@@ -725,11 +776,6 @@ static int tc_setup(const TcGemm& g, int bn, int epi, CUtensorMap* maps, TcArgs&
   a.res_hi = reinterpret_cast<const __nv_bfloat16*>(g.res_hi);
   a.res_lo = reinterpret_cast<const __nv_bfloat16*>(g.res_lo);
   a.pool_w = g.pool_w; a.pool_part = g.pool_part; a.pool_item_rows = g.pool_item_rows; a.pool_K = g.pool_K;
-  {
-    const bool planes = epi == TC_LEAKY_BN_SPLIT;
-    const uintptr_t base = planes ? ((uintptr_t)g.out_hi | (uintptr_t)g.out_lo) : (uintptr_t)g.out_f32;
-    a.vec8 = base % 32 == 0 && (g.ldc * (planes ? 2 : 4)) % 32 == 0;
-  }
   return 0;
 }
 
@@ -742,7 +788,7 @@ static int tc_grid(const TcArgs& a) {
 template <int BN, int EPI>
 static int launch_tc(const TcGemm& g, cudaStream_t st) {
   using S = TcSmem<BN>;
-  CUtensorMap m[4];
+  CUtensorMap m[6];
   TcArgs a;
   if (tc_setup(g, BN, EPI, m, a)) return -2;
   if (tc_pooling(EPI) && !(a.tile_ctr = tile_counter(st))) return -2;
@@ -750,7 +796,7 @@ static int launch_tc(const TcGemm& g, cudaStream_t st) {
   static bool attr_done[64] = {};
   if (first_use_on_device(attr_done))
     DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::total(EPI)));
-  kern<<<tc_grid(a), TC_THREADS, S::total(EPI), st>>>(m[0], m[1], m[2], m[3], a);
+  kern<<<tc_grid(a), TC_THREADS, S::total(EPI), st>>>(m[0], m[1], m[2], m[3], m[4], m[5], a);
   DG_LAUNCHED();
   return 0;
 }
@@ -764,9 +810,17 @@ int launch_gemm_tc(const TcGemm& g, cudaStream_t st) {
     return -1;
   }
   if (g.epi == TC_LEAKY_BN_SPLIT && g.N % 32) {
-    // the epilogue stores the planes 32 columns at a time: a partial group would overwrite the start of the next row
     set_error("gemm_tc (planes): N must be a multiple of 32");
     return -1;
+  }
+  if (tc_box_store(g.epi)) {
+    // TMA stores: 16-byte aligned base and pitch, row coordinates below 2^31
+    const bool planes = g.epi == TC_LEAKY_BN_SPLIT;
+    const uintptr_t base = planes ? ((uintptr_t)g.out_hi | (uintptr_t)g.out_lo) : (uintptr_t)g.out_f32;
+    if (!base || (planes && (!g.out_hi || !g.out_lo)) || base % 16 || g.ldc < g.N || g.M >= (1LL << 31)) {
+      set_error("gemm_tc: the output needs a 16-byte aligned base, a pitch of at least N and fewer than 2^31 rows");
+      return -1;
+    }
   }
   if (g.epi == TC_CONV2D) {
     if (g.ldc % 32 || g.N % 32 || g.Wp < 3 || g.Hp < 3 || (!g.out_hi && !g.out_f32) || g.M >= (1LL << 31)) {

@@ -72,12 +72,27 @@ __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.
 template <int R>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
-// 32 bytes per lane as two 128-bit global stores.  `p` must be 16-byte aligned.
-__device__ __forceinline__ void st_global_v8(void* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t e, uint32_t f,
-                                             uint32_t g, uint32_t h) {
-  asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};\n\tst.global.v4.b32 [%0+16], {%5, %6, %7, %8};" ::"l"(p), "r"(a),
-               "r"(b), "r"(c), "r"(d), "r"(e), "r"(f), "r"(g), "r"(h)
+// TMA bulk tensor store of one box from shared memory to global memory at coordinates (c0, c1); the hardware clips the box
+// at the map's dimensions.  Generic-proxy writes of the box must be made visible first: fence_proxy_async_smem() by every
+// writing thread, then a barrier.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tmap, const void* smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
                : "memory");
+}
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// bulk groups belong to the issuing thread: commit and wait run on the thread that issued the stores
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// every committed store has read its shared-memory source (the buffer may be rewritten; the global writes may be pending)
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// every committed store has completed
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t a) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(a) : "memory");
+}
+__device__ __forceinline__ void st_shared_v2(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");

@@ -360,6 +360,11 @@ int dg_selftest_gemm_tc(int M, int Cin, int KW, int dil, int N, int epi, float* 
  * of the square zero-padded maps (M a multiple of dil^2); epi 4: 3 speakers, items of 296 rows; epi 5: N <= 64, items of
  * 888 rows (M a multiple of 888). */
 int dg_selftest_gemm_tc_grid(int M, int Cin, int KW, int dil, int N, int epi, int* equal);
+/* test hook: one seeded wgmma GEMM (one tap, epi 0..2) into outputs of pitch N + 40 with guard rows after M, all bytes preset
+ * to a sentinel.  *outside_unchanged = 1 if no byte outside rows [0, M) x columns [0, N) changed, *equal = 1 if the rows
+ * equal, byte for byte, those of the same GEMM written at pitch N, *refused = 1 if an output base off 16-byte alignment and
+ * a pitch that is not a multiple of 16 bytes are both rejected with DG_EINVAL.  N a multiple of 4 (32 for epi 1). */
+int dg_selftest_gemm_tc_bounds(int M, int Cin, int N, int epi, int* outside_unchanged, int* equal, int* refused);
 /* test hook (host only, no GPU): the weight-side split of float32 values into the two IEEE fp16 operand planes
  * (hi = rn16(x), lo = rn16(x - hi), saturating).  What the device does to activations with cvt.rn.satfinite.f16.f32. */
 int dg_selftest_split_f16_host(const float* x, long long n, unsigned short* hi, unsigned short* lo);
