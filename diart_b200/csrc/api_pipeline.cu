@@ -216,7 +216,7 @@ static int pipeline_nets(dg_pipeline* h, const float* wav, int S, const StepShap
   DG_DIAG(seg, s_seg);
   DG_CUDA(cudaStreamWaitEvent(h->s_emb, h->e_osp[lane], 0));
   // a fused TDNN5 needs the pooling weights: it runs here, after the segmentation of this step, with its grid capped like the
-  // trunk's (the other lane's recurrence may hold 2 x ceil(B/16) SMs at this point)
+  // trunk's (the other lane's recurrence may hold lstm_tc_ctas(B) SMs at this point)
   if ((rc = emb_tail(h->emb, B, g, osp.as<float>(), F, K, T, fuse, 1, 1.f, emb, h->s_emb, sm_cap))) return rc;
   DG_CUDA(cudaEventRecord(h->e_emb, h->s_emb));
   DG_DIAG(emb, h->s_emb);
