@@ -106,6 +106,16 @@ SIGNATURES = {
     "dg_vad_sweep_run_files": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_int, C.POINTER(C.c_int), _P]),
     "dg_vad_sweep_score_files": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, C.c_double, _P, _P, _P, _P]),
     "dg_vad_sweep_destroy": (C.c_int, [_P]),
+    "dg_multi_create": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double,
+                                  C.c_float, C.c_float, C.c_int, C.c_int, _P, C.POINTER(_P)]),
+    "dg_multi_open": (C.c_int, [_P, C.c_int]),
+    "dg_multi_close": (C.c_int, [_P, C.c_int]),
+    "dg_multi_push_host": (C.c_int, [_P, C.c_int, _P, C.c_int]),
+    "dg_multi_available": (C.c_int, [_P, C.c_int]),
+    "dg_multi_step": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, C.c_int, C.POINTER(C.c_int), _P, _P, _P]),
+    "dg_multi_last_step_ms": (C.c_int, [_P, C.POINTER(C.c_float)]),
+    "dg_multi_destroy": (C.c_int, [_P]),
+    "dg_selftest_multi_staging_host": (C.c_int, [C.c_int, C.c_int, C.c_int, _P, _P, _P, _P]),
 }
 
 

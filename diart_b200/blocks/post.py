@@ -79,20 +79,7 @@ class DevicePostPath:
     def annotations(self, header: np.ndarray, turns: np.ndarray, n_turns: int, out_start: np.ndarray,
                     out_res: np.ndarray, shift: float = 0.0, uri: Optional[str] = None) -> List[Annotation]:
         """packed turns -> one Annotation per chunk, segments at frame middles (blocks/utils.py:45-58)"""
-        B = len(header)
-        _, g, t_on, t_off = turn_times(header, turns, n_turns, out_start, out_res, shift)
-        t_on, t_off, g = t_on.tolist(), t_off.tolist(), g.tolist()
-        labels = self.labels
-        modality = "speech" if shift == 0 else None             # the reference's shifted copy drops the modality
-        out = []
-        offs, cnts = header[:, 0].tolist(), header[:, 1].tolist()
-        for cidx in range(B):
-            ann = Annotation(uri=uri, modality=modality)
-            o = offs[cidx]
-            for i in range(o, o + cnts[cidx]):
-                ann[Segment(t_on[i], t_off[i]), g[i]] = labels[g[i]]
-            out.append(ann)
-        return out
+        return chunk_annotations(header, turns, n_turns, out_start, out_res, self.labels, shift, uri)
 
     def run(self, seg: torch.Tensor, maps: torch.Tensor, starts: np.ndarray, res: float, shift: float = 0.0):
         """device scores (B,F,K) + maps (B,K) -> list of Annotation (block-level entry; the fused pipeline uses
@@ -119,22 +106,30 @@ def post_plan(starts: np.ndarray, res: float, hist_start: np.ndarray, hist_res: 
     r_all = np.concatenate([hist_res, np.full(B, res)])
     c = np.arange(B)
     nb = np.minimum(H + c + 1, nw)
-    end = starts + F * res                                  # buffers[-1].extent.end (duration == step)
-    f_start = end - latency                                 # aggregation.py:216-217
-    f_end = f_start + step
-    fixed = np.where(f_end > f_start, f_end - f_start, 0.0)  # Segment.duration
     # buffer j of chunk c (oldest first) is entry H + c - (nb - 1) + j of the concatenated history
     j = np.arange(nw)[None, :]
     idx = (H + c - (nb - 1))[:, None] + j
     valid = j < nb[:, None]
     idx = np.where(valid, idx, 0)
-    s_j, r_j = s_all[idx], r_all[idx]
+    return crop_plan(starts, np.full(B, res), s_all[idx], r_all[idx], nb, valid, nw, F, step, latency)
+
+
+def crop_plan(starts: np.ndarray, res: np.ndarray, s_j: np.ndarray, r_j: np.ndarray, nb: np.ndarray, valid: np.ndarray,
+              nw: int, F: int, step: float, latency: float):
+    """The plan rows of chunks starting at ``starts`` (B,) with ``res`` (B,) seconds per score frame, whose aggregated
+    buffers j (oldest first, ``valid`` (B, nw) for j < nb) start at ``s_j`` (B, nw) with resolution ``r_j`` (B, nw)
+    -> (plan int32 (B, 4 + nw), out_start (B,), out_res (B,)).  The float64 arithmetic of the reference's
+    ``SlidingWindow.crop(mode="loose", fixed=...)``, operation by operation."""
+    end = starts + F * res                                  # buffers[-1].extent.end (duration == step)
+    f_start = end - latency                                 # aggregation.py:216-217
+    f_end = f_start + step
+    fixed = np.where(f_end > f_start, f_end - f_start, 0.0)  # Segment.duration
     lo = np.ceil((f_start[:, None] - r_j - s_j) / r_j)      # SlidingWindow.crop, mode="loose"
     cnt = np.floor((fixed[:, None] + r_j) / r_j)            # SlidingWindow.samples(fixed, mode="loose")
     nf = cnt[:, 0]
     if np.any(valid & (cnt != nf[:, None])):
         raise ValueError("all input arrays must have the same shape")   # what np.stack raises in the reference
-    plan = np.zeros((B, 4 + nw), dtype=np.int32)
+    plan = np.zeros((len(starts), 4 + nw), dtype=np.int32)
     plan[:, 0] = nb
     plan[:, 1] = nf
     plan[:, 4:] = np.where(valid, lo, 0)
@@ -170,6 +165,31 @@ def turn_times(header: np.ndarray, turns: np.ndarray, n_turns: int, out_start: n
     t_on = 0.5 * (a + (a + r0)) + shift                     # SlidingWindow[i].middle
     t_off = 0.5 * (b + (b + r0)) + shift
     return row_of, g, t_on, t_off
+
+
+def chunk_annotations(header: np.ndarray, turns: np.ndarray, n_turns: int, out_start: np.ndarray, out_res: np.ndarray,
+                      labels: Sequence[str], shift=0.0, uri: Optional[str] = None) -> List[Annotation]:
+    """packed turns -> one Annotation per chunk (row of ``header``), segments at frame middles (blocks/utils.py:45-58).
+    ``shift``: seconds added to every time stamp, one number or one per chunk (streams with their own shifts)."""
+    B = len(header)
+    per_chunk = np.ndim(shift) > 0
+    row_of, g, t_on, t_off = turn_times(header, turns, n_turns, out_start, out_res, 0.0 if per_chunk else shift)
+    if per_chunk:                                            # x + 0.0 + s == x + s: the same bits as a scalar shift
+        s = np.asarray(shift, dtype=np.float64)[row_of]
+        t_on, t_off = t_on + s, t_off + s
+    t_on, t_off, g = t_on.tolist(), t_off.tolist(), g.tolist()
+    # the reference's shifted copy drops the modality
+    modality = [("speech" if x == 0 else None) for x in np.asarray(shift).tolist()] if per_chunk else \
+        [("speech" if shift == 0 else None)] * B
+    out = []
+    offs, cnts = header[:, 0].tolist(), header[:, 1].tolist()
+    for cidx in range(B):
+        ann = Annotation(uri=uri, modality=modality[cidx])
+        o = offs[cidx]
+        for i in range(o, o + cnts[cidx]):
+            ann[Segment(t_on[i], t_off[i]), g[i]] = labels[g[i]]
+        out.append(ann)
+    return out
 
 
 def aggregate_audio(chunk_buffer: List[SlidingWindowFeature], new: Sequence[SlidingWindowFeature], nw: int, step: float,

@@ -74,27 +74,14 @@ class GatherPool {
   bool stop_ = false;
 };
 
-// a step's outputs: scores [B, F, K], embeddings [B, K, D], speaker maps [B, K], permuted scores [B, F, M]
-struct StepShape {
-  int B = 0, F = 0, K = 0;
-  size_t seg_bytes() const { return (size_t)B * F * K * 4; }
-  size_t emb_bytes(int D) const { return (size_t)B * K * D * 4; }
-  size_t map_bytes() const { return (size_t)B * K * 4; }
-  size_t permuted_bytes(int M) const { return (size_t)B * F * M * 4; }
-};
 struct StepOut { float *seg, *emb; int32_t* map; float* permuted; };   // where a step's outputs are or go; null: not wanted
 
-struct dg_pipeline {
-  dg_seg* seg;
-  dg_emb* emb;
+// The networks' model handles, lanes and streams are the NetLanes base (host.cuh).
+struct dg_pipeline : NetLanes {
   dg_cluster* clu;
-  float gamma, beta;
-  int normalize_weights;
-  int hop = 0;          // samples between consecutive windows of a batch (hint, dg_pipeline_set_hop); 0 = unknown
   // Members are destroyed in reverse order: the streams and events (declared last) first, then the pinned staging, then
-  // the device buffers and worker threads.
-  DevBuf wav, segd, embd, mapd, permd, osp[2];
-  SincPrep prep[2];
+  // the device buffers and worker threads; the NetLanes base goes last.
+  DevBuf wav, segd, embd, mapd, permd;
   // Every step runs through pipeline_enqueue.  Submitted step n (up to DG_MAX_INFLIGHT outstanding) uses result / input slot
   // n % 3 and scratch lane n & 1: two steps compute concurrently while the host uploads step n+2.  Synchronous steps use lane
   // 0 and the caller's buffers or wav / segd / ..., never a slot (collected pointers stay valid), and do not count in next_step.
@@ -107,11 +94,8 @@ struct dg_pipeline {
   DevBuf call_stream;                   // device image of the stream a dg_pipeline_call_host batch was cut from
   long long call_h2d_bytes = 0;         // bytes the last dg_pipeline_call_host uploaded
   PinnedBuf pin_wav;                    // pinned staging of dg_pipeline_call_host (B separate host windows -> one upload)
-  Stream st;
-  // two-stream overlap inside a step: the segmentation chain (critical path, high priority) and the
-  // embedding trunk (independent of it until the pooling weights exist) run concurrently
-  Stream s_seg[2], s_emb, s_clu, s_h2d, s_d2h;
-  Event e_osp[2], e_prep[2], e_start, e_emb, e_done;
+  Stream st, s_clu, s_h2d, s_d2h;
+  Event e_start, e_done;
   Event e_h2d[3], e_slot_done[3], e_lane_done[2];
   // shared-identity mode inside the pipelined flow: export / merge run on the clustering stream, in order with the clustering
   // of the submitted steps, so the networks of the next steps keep running meanwhile (created at the first export)
@@ -139,15 +123,23 @@ extern "C" int dg_pipeline_create(dg_seg* seg, dg_emb* emb, dg_cluster* clu, flo
   DG_CUDA(cudaSetDevice(seg->device));
   int lo = 0, hi = 0;
   DG_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-  if (h->st.create() || h->s_seg[0].create(hi) || h->s_emb.create(lo) || h->s_clu.create(hi) || h->s_seg[1].create(hi) ||
-      h->s_h2d.create() || h->s_d2h.create())
-    return DG_ECUDA;
-  for (Event* e : {&h->e_start, &h->e_osp[0], &h->e_emb, &h->e_done, &h->e_osp[1], &h->e_prep[0], &h->e_prep[1], &h->e_h2d[0],
-                   &h->e_h2d[1], &h->e_h2d[2], &h->e_slot_done[0], &h->e_slot_done[1], &h->e_slot_done[2],
-                   &h->e_lane_done[0], &h->e_lane_done[1]})
+  if (net_lanes_create(*h) || h->st.create() || h->s_clu.create(hi) || h->s_h2d.create() || h->s_d2h.create()) return DG_ECUDA;
+  for (Event* e : {&h->e_start, &h->e_done, &h->e_h2d[0], &h->e_h2d[1], &h->e_h2d[2], &h->e_slot_done[0], &h->e_slot_done[1],
+                   &h->e_slot_done[2], &h->e_lane_done[0], &h->e_lane_done[1]})
     if (e->create()) return DG_ECUDA;
-  DG_CUDA(cudaEventRecord(h->e_emb, h->s_emb));   // so that the first step's wait on it is well defined
   *out = h.release();
+  return DG_OK;
+}
+
+// two-stream overlap inside a step: the segmentation chain (critical path, high priority) and the embedding trunk
+// (independent of it until the pooling weights exist) run concurrently
+int net_lanes_create(NetLanes& n) {
+  int lo = 0, hi = 0;
+  DG_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
+  if (n.s_seg[0].create(hi) || n.s_seg[1].create(hi) || n.s_emb.create(lo)) return DG_ECUDA;
+  for (Event* e : {&n.e_osp[0], &n.e_osp[1], &n.e_prep[0], &n.e_prep[1], &n.e_emb})
+    if (e->create()) return DG_ECUDA;
+  DG_CUDA(cudaEventRecord(n.e_emb, n.s_emb));   // so that the first step's wait on it is well defined
   return DG_OK;
 }
 
@@ -177,10 +169,8 @@ static int emb_sm_cap(int device, int B) {
   return sms - lstm_ctas > sms / 2 ? sms - lstm_ctas : 0;
 }
 
-// segmentation chain on s_seg and embedding chain on s_emb, both starting after `start`; on return
-// e_emb (recorded on s_emb) marks seg, osp and emb complete
-static int pipeline_nets(dg_pipeline* h, const float* wav, int S, const StepShape& sh, float* seg, float* emb,
-                         cudaEvent_t start, int lane, int stream_hop) {
+int pipeline_nets(NetLanes* h, const float* wav, int S, const StepShape& sh, float* seg, float* emb, cudaEvent_t start,
+                  int lane, int stream_hop) {
   int rc;
   const int B = sh.B, F = sh.F, K = sh.K;
   const Geom g = make_geom(S);

@@ -9,21 +9,8 @@
 
 #include "host.cuh"
 
-static const int DG_POST_PREFIX = 16384;   // turns copied back together with the header (one D2H in the common case)
-
-// Where the results of a post-path launch land in pinned memory: the header at `at`, the turn count in the 16 bytes after it,
-// then the first DG_POST_PREFIX turns.  In front of `at`: dg_post's plan, or dg_sweep's error flags.
-struct TurnOut {
-  size_t at, header_bytes;
-  size_t total() const { return at + header_bytes; }
-  size_t prefix() const { return total() + 16; }
-  size_t end() const { return prefix() + (size_t)DG_POST_PREFIX * 4; }
-};
-
-// After the stream `st` has been synchronised: hands the header and the turns of a TurnOut layout in `pin` to the caller; the
-// turns beyond the prefix come from `turns_dev`.  `who` names the entry point in the error.
-static int download_turns(const char* who, const unsigned char* pin, const TurnOut& lay, const uint32_t* turns_dev,
-                          int32_t* header_host, uint32_t* turns_host, int turn_cap_host, int* n_turns, cudaStream_t st) {
+int download_turns(const char* who, const unsigned char* pin, const TurnOut& lay, const uint32_t* turns_dev,
+                   int32_t* header_host, uint32_t* turns_host, int turn_cap_host, int* n_turns, cudaStream_t st) {
   unsigned int total = 0;
   memcpy(&total, pin + lay.total(), 4);
   if (n_turns) *n_turns = (int)total;

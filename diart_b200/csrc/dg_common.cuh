@@ -269,6 +269,26 @@ int launch_post(const float* seg, const int32_t* map, const float* hist_seg, con
 int launch_expand_windows(const float* ring, long long r0, int C, int hop, int S, int B, float* wav, cudaStream_t st);
 int launch_post_history(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map, int n_hist,
                         int B, int F, int K, int keep, float* new_seg, int32_t* new_map, cudaStream_t st);
+// post.cu -- many live streams in one batch (dg_multi).  A piece of the staging upload: n samples at staged[src] belong at
+// absolute sample dst of slot `slot`.  A slot with windows in the batch: its n windows are rows [row0, row0 + n); its post-path
+// history is copy `cur` of the two, with n_hist chunks.
+struct RingPiece {
+  long long src, dst;
+  int slot, n;
+};
+struct TickSlot {
+  int slot, row0, n, cur, n_hist, pad[3];
+};
+int launch_ring_scatter(const float* staged, const RingPiece* pieces, int n_pieces, int C, float* rings, cudaStream_t st);
+// rows [B] = {entry of act, window index within that slot's rows}; window b = samples [start[b], start[b] + S) of its ring
+int launch_ring_gather(const float* rings, int C, const TickSlot* act, const int2* rows, const long long* start, int S, int B,
+                       float* wav, cudaStream_t st);
+int launch_post_slots(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map,
+                      const TickSlot* act, const int2* rows, int slots, int B, int F, int K, int M, int nw,
+                      const int32_t* plan, int plan_stride, const double* hamming, double tau, int32_t* header,
+                      uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st);
+int launch_post_slots_history(const float* seg, const int32_t* map, float* hist_seg, int32_t* hist_map, const TickSlot* act,
+                              int n_act, int slots, int F, int K, int nw, cudaStream_t st);
 size_t cluster_prep_doubles(int B, int K);
 // der.cu -- DER components of sweep trials over nf files (chunks [chunk_off[f], chunk_off[f + 1]) of N, timestamp shift
 // shifts[f]).  Hypothesis segments: count per (file, trial, label) and scan into offsets [nf*T*M+1], then write

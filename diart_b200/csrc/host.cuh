@@ -61,8 +61,8 @@ struct Stream : Owned<cudaStream_t, cudaStreamDestroy> {
   }
 };
 struct Event : Owned<cudaEvent_t, cudaEventDestroy> {
-  int create() {
-    DG_CUDA(cudaEventCreateWithFlags(&h, cudaEventDisableTiming));
+  int create(unsigned flags = cudaEventDisableTiming) {
+    DG_CUDA(cudaEventCreateWithFlags(&h, flags));
     return 0;
   }
 };
@@ -320,3 +320,51 @@ struct dg_post {
 int post_enqueue(dg_post* h, const float* seg_dev, const int32_t* map_dev, int B, const int32_t* plan_host, cudaStream_t st);
 int post_finish(dg_post* h, int B, int32_t* header_host, uint32_t* turns_host, int turn_cap_host, int* n_turns,
                 cudaStream_t st);
+
+static const int DG_POST_PREFIX = 16384;   // turns copied back together with the header (one D2H in the common case)
+
+// Where the results of a post-path launch land in pinned memory: the header at `at`, the turn count in the 16 bytes after it,
+// then the first DG_POST_PREFIX turns.  In front of `at`: dg_post's plan, or dg_sweep's error flags.
+struct TurnOut {
+  size_t at, header_bytes;
+  size_t total() const { return at + header_bytes; }
+  size_t prefix() const { return total() + 16; }
+  size_t end() const { return prefix() + (size_t)DG_POST_PREFIX * 4; }
+};
+
+// After the stream `st` has been synchronised: hands the header and the turns of a TurnOut layout in `pin` to the caller; the
+// turns beyond the prefix come from `turns_dev`.  `who` names the entry point in the error.
+int download_turns(const char* who, const unsigned char* pin, const TurnOut& lay, const uint32_t* turns_dev,
+                   int32_t* header_host, uint32_t* turns_host, int turn_cap_host, int* n_turns, cudaStream_t st);
+
+// ============================================================================ network pass (api_pipeline.cu)
+// a step's outputs: scores [B, F, K], embeddings [B, K, D], speaker maps [B, K], permuted scores [B, F, M]
+struct StepShape {
+  int B = 0, F = 0, K = 0;
+  size_t seg_bytes() const { return (size_t)B * F * K * 4; }
+  size_t emb_bytes(int D) const { return (size_t)B * K * D * 4; }
+  size_t map_bytes() const { return (size_t)B * K * 4; }
+  size_t permuted_bytes(int M) const { return (size_t)B * F * M * 4; }
+};
+
+// What the networks of a step use besides its batch and outputs: the model handles, the overlapped-speech penalty, and per
+// scratch lane a segmentation stream, the front-end state, the OSP weights and two events; the embedding stream.  A dg_pipeline
+// is one; a dg_multi owns another over the same model handles (the lane guards order their uses).
+struct NetLanes {
+  dg_seg* seg = nullptr;
+  dg_emb* emb = nullptr;
+  float gamma = 3.f, beta = 10.f;
+  int normalize_weights = 0;
+  int hop = 0;          // samples between consecutive windows of a batch (hint, dg_pipeline_set_hop); 0 = unknown
+  DevBuf osp[2];
+  SincPrep prep[2];
+  Stream s_seg[2], s_emb;
+  Event e_osp[2], e_prep[2], e_emb;
+};
+
+// creates the streams and events of `n` (segmentation streams at high priority, the embedding stream at low priority)
+int net_lanes_create(NetLanes& n);
+// segmentation chain on s_seg[lane] and embedding chain on s_emb, both starting after `start`; on return e_emb (recorded on
+// s_emb) marks seg, osp and emb complete.  stream_hop > 0: the batch is windows of one stream that many samples apart.
+int pipeline_nets(NetLanes* h, const float* wav, int S, const StepShape& sh, float* seg, float* emb, cudaEvent_t start,
+                  int lane, int stream_hop);

@@ -28,37 +28,21 @@ constexpr int POST_THREADS = 256;
 
 // plan row (int32): [0] nb buffers aggregated, [1] nf frames of the region crop, [2] first_nf (> 0: first buffer of a
 // stream, output = crop of [0, region.end) with its last nf frames replaced), [3] first_lo, [4 ..] lo of each buffer
-template <bool STATES>
-__global__ void __launch_bounds__(POST_THREADS)
-post_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map, const float* __restrict__ hist_seg,
-            const int32_t* __restrict__ hist_map, int n_hist, int B, int F, int K, int M, int nw,
-            const int32_t* __restrict__ plan, int plan_stride, const double* __restrict__ hamming, double tau,
-            const double* __restrict__ taus, int32_t* __restrict__ header /*[gridDim.y][B][4]*/, uint32_t* __restrict__ turns,
-            int turn_cap, unsigned int* __restrict__ total) {
+//
+// The body of the post-path for chunk c (one CTA): buf_seg(j) / buf_map(j) are the scores [F][K] and map [K] of its buffer j,
+// oldest first; writes header row c and the chunk's turns.
+template <class BufSeg, class BufMap>
+__device__ __forceinline__ void post_chunk(const int32_t* __restrict__ pl, int c, int nb, int nf, int first_nf, int first_lo,
+                                           int F, int K, int M, int nw, const double* __restrict__ hamming, double tau,
+                                           int32_t* __restrict__ header, uint32_t* __restrict__ turns, int turn_cap,
+                                           unsigned int* __restrict__ total, BufSeg buf_seg, BufMap buf_map) {
   extern __shared__ unsigned char sm_raw[];
-  const int c = blockIdx.x;
-  if constexpr (STATES) {
-    map += (size_t)blockIdx.y * B * K;
-    header += (size_t)blockIdx.y * B * 4;
-    tau = taus[blockIdx.y];
-  }
-  const int32_t* pl = plan + (size_t)c * plan_stride;
-  const int nb = pl[0], nf = pl[1], first_nf = pl[2], first_lo = pl[3];
   const int nfo = first_nf > 0 ? first_nf : nf;
   signed char* inv = reinterpret_cast<signed char*>(sm_raw);           // [nb][M]: local speaker of global g, or -1
   unsigned char* act = sm_raw + ((nw * M + 15) & ~15);                    // [nfo][M]
   __shared__ int cnt[64], off[65];
   __shared__ unsigned int base_s;
 
-  // buffer j of this chunk = virtual chunk v = c - (nb - 1) + j; v < 0 lives in the history (last n_hist chunks seen)
-  auto buf_seg = [&](int j) -> const float* {
-    const int v = c - (nb - 1) + j;
-    return v >= 0 ? seg + (size_t)v * F * K : hist_seg + (size_t)(n_hist + v) * F * K;
-  };
-  auto buf_map = [&](int j) -> const int32_t* {
-    const int v = c - (nb - 1) + j;
-    return v >= 0 ? map + (size_t)v * K : hist_map + (size_t)(n_hist + v) * K;
-  };
   for (int i = threadIdx.x; i < nb * M; i += POST_THREADS) inv[i] = -1;
   __syncthreads();
   if (threadIdx.x < nb) {
@@ -118,6 +102,80 @@ post_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map, cons
       prev = a;
     }
   }
+}
+
+template <bool STATES>
+__global__ void __launch_bounds__(POST_THREADS)
+post_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map, const float* __restrict__ hist_seg,
+            const int32_t* __restrict__ hist_map, int n_hist, int B, int F, int K, int M, int nw,
+            const int32_t* __restrict__ plan, int plan_stride, const double* __restrict__ hamming, double tau,
+            const double* __restrict__ taus, int32_t* __restrict__ header /*[gridDim.y][B][4]*/, uint32_t* __restrict__ turns,
+            int turn_cap, unsigned int* __restrict__ total) {
+  const int c = blockIdx.x;
+  if constexpr (STATES) {
+    map += (size_t)blockIdx.y * B * K;
+    header += (size_t)blockIdx.y * B * 4;
+    tau = taus[blockIdx.y];
+  }
+  const int32_t* pl = plan + (size_t)c * plan_stride;
+  const int nb = pl[0], nf = pl[1], first_nf = pl[2], first_lo = pl[3];
+  // buffer j of this chunk = virtual chunk v = c - (nb - 1) + j; v < 0 lives in the history (last n_hist chunks seen)
+  auto buf_seg = [&](int j) -> const float* {
+    const int v = c - (nb - 1) + j;
+    return v >= 0 ? seg + (size_t)v * F * K : hist_seg + (size_t)(n_hist + v) * F * K;
+  };
+  auto buf_map = [&](int j) -> const int32_t* {
+    const int v = c - (nb - 1) + j;
+    return v >= 0 ? map + (size_t)v * K : hist_map + (size_t)(n_hist + v) * K;
+  };
+  post_chunk(pl, c, nb, nf, first_nf, first_lo, F, K, M, nw, hamming, tau, header, turns, turn_cap, total, buf_seg, buf_map);
+}
+
+// Many streams in one batch (dg_multi): the B chunks are grouped by stream slot.  Chunk c is window rows[c].y of this batch's
+// slot entry act[rows[c].x] (TickSlot, dg_common.cuh), whose chunks start at batch row row0.  Each slot has its own history of
+// up to nw - 1 chunks: hist_seg [2][slots][nw - 1][F][K] and hist_map [2][slots][nw - 1][K] (two copies, `cur` is the
+// current one), of which the first n_hist entries hold the last chunks seen, oldest first.
+__global__ void __launch_bounds__(POST_THREADS)
+post_slots_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map, const float* __restrict__ hist_seg,
+                  const int32_t* __restrict__ hist_map, const TickSlot* __restrict__ act, const int2* __restrict__ rows,
+                  int slots, int F, int K, int M, int nw, const int32_t* __restrict__ plan, int plan_stride,
+                  const double* __restrict__ hamming, double tau, int32_t* __restrict__ header, uint32_t* __restrict__ turns,
+                  int turn_cap, unsigned int* __restrict__ total) {
+  const int c = blockIdx.x;
+  const int2 r = rows[c];
+  const TickSlot ts = act[r.x];
+  const int32_t* pl = plan + (size_t)c * plan_stride;
+  const int nb = pl[0], nf = pl[1], first_nf = pl[2], first_lo = pl[3];
+  const size_t h0 = ((size_t)ts.cur * slots + ts.slot) * (nw - 1) + ts.n_hist;   // one past the slot's newest history entry
+  // buffer j of this chunk = virtual chunk v of its slot; v < 0 lives in the slot's history
+  auto buf_seg = [&](int j) -> const float* {
+    const int v = r.y - (nb - 1) + j;
+    return v >= 0 ? seg + (size_t)(ts.row0 + v) * F * K : hist_seg + (h0 + v) * F * K;
+  };
+  auto buf_map = [&](int j) -> const int32_t* {
+    const int v = r.y - (nb - 1) + j;
+    return v >= 0 ? map + (size_t)(ts.row0 + v) * K : hist_map + (h0 + v) * K;
+  };
+  post_chunk(pl, c, nb, nf, first_nf, first_lo, F, K, M, nw, hamming, tau, header, turns, turn_cap, total, buf_seg, buf_map);
+}
+
+// History update of the slots of a dg_multi batch: CTA (a, i) writes entry i of slot act[a]'s other history copy, the last
+// keep = min(nw - 1, n_hist + n) chunks of (its history + its n chunks of this batch).  The host then flips `cur` and sets
+// n_hist = keep.
+__global__ void __launch_bounds__(256)
+post_slots_history_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map, float* __restrict__ hist_seg,
+                          int32_t* __restrict__ hist_map, const TickSlot* __restrict__ act, int slots, int FK, int K, int nw) {
+  const TickSlot ts = act[blockIdx.x];
+  const int i = blockIdx.y;
+  const int keep = min(nw - 1, ts.n_hist + ts.n);
+  if (i >= keep) return;
+  const int v = ts.n - keep + i;                    // virtual chunk: v >= 0 is this batch's, v < 0 the history's
+  const size_t src = ((size_t)ts.cur * slots + ts.slot) * (nw - 1) + ts.n_hist;
+  const size_t dst = ((size_t)(ts.cur ^ 1) * slots + ts.slot) * (nw - 1) + i;
+  const float* s = v >= 0 ? seg + (size_t)(ts.row0 + v) * FK : hist_seg + (src + v) * FK;
+  const int32_t* m = v >= 0 ? map + (size_t)(ts.row0 + v) * K : hist_map + (src + v) * K;
+  for (int e = threadIdx.x; e < FK; e += blockDim.x) hist_seg[dst * FK + e] = s[e];
+  for (int e = threadIdx.x; e < K; e += blockDim.x) hist_map[dst * K + e] = m[e];
 }
 
 // the last `keep` chunks seen (history followed by this batch) become the new history
@@ -197,6 +255,86 @@ int launch_expand_windows(const float* ring, long long r0, int C, int hop, int S
   ProfScope _ps("expand_windows", st);
   dim3 grid(8, B);
   expand_windows_kernel<<<grid, 256, 0, st>>>(ring, r0, C, hop, S, wav);
+  DG_LAUNCHED();
+  return 0;
+}
+
+// ---- the rings of many streams (dg_multi): slot s owns rings [s][C]; absolute sample t of a slot lives at index t mod C.
+// Piece p of the staging buffer (one upload of every stream's new samples) goes to its slot's ring; CTA b takes pieces b,
+// b + gridDim.x, ..., so any number of pieces fits one launch.
+__global__ void __launch_bounds__(256) ring_scatter_kernel(const float* __restrict__ staged, const RingPiece* __restrict__ pieces,
+                                                           int n_pieces, int C, float* __restrict__ rings) {
+  for (int q = blockIdx.x; q < n_pieces; q += gridDim.x) {
+    const RingPiece p = pieces[q];
+    float* ring = rings + (size_t)p.slot * C;
+    for (int i = threadIdx.x; i < p.n; i += blockDim.x) ring[(p.dst + i) % C] = staged[p.src + i];
+  }
+}
+
+// window b of the batch = samples [start[b], start[b] + S) of the ring of slot act[rows[b].x].slot (C, start, S multiples of
+// 4: 16-byte accesses never straddle the wrap)
+__global__ void __launch_bounds__(256) ring_gather_kernel(const float* __restrict__ rings, int C, const TickSlot* __restrict__ act,
+                                                          const int2* __restrict__ rows, const long long* __restrict__ start,
+                                                          int S, float* __restrict__ wav) {
+  const int b = blockIdx.y;
+  const float* ring = rings + (size_t)act[rows[b].x].slot * C;
+  const long long base = start[b];
+  float4* dst = reinterpret_cast<float4*>(wav + (size_t)b * S);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < (S >> 2); i += gridDim.x * blockDim.x) {
+    const int idx = (int)((base + 4LL * i) % C);
+    dst[i] = *reinterpret_cast<const float4*>(ring + idx);
+  }
+}
+
+int launch_ring_scatter(const float* staged, const RingPiece* pieces, int n_pieces, int C, float* rings, cudaStream_t st) {
+  ProfScope _ps("ring_scatter", st);
+  if (n_pieces < 1) return 0;
+  ring_scatter_kernel<<<n_pieces < 4096 ? n_pieces : 4096, 256, 0, st>>>(staged, pieces, n_pieces, C, rings);
+  DG_LAUNCHED();
+  return 0;
+}
+
+int launch_ring_gather(const float* rings, int C, const TickSlot* act, const int2* rows, const long long* start, int S, int B,
+                       float* wav, cudaStream_t st) {
+  ProfScope _ps("ring_gather", st);
+  if (B > 65535) {
+    set_error("ring_gather: at most 65535 windows per batch");
+    return -1;
+  }
+  ring_gather_kernel<<<dim3(8, B), 256, 0, st>>>(rings, C, act, rows, start, S, wav);
+  DG_LAUNCHED();
+  return 0;
+}
+
+int launch_post_slots(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map,
+                      const TickSlot* act, const int2* rows, int slots, int B, int F, int K, int M, int nw,
+                      const int32_t* plan, int plan_stride, const double* hamming, double tau, int32_t* header,
+                      uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st) {
+  ProfScope _ps("post_slots", st);
+  if (M > 64 || F > 1023 || K > 127) {
+    set_error("post_slots: at most 64 global speakers, 1023 frames");
+    return -1;
+  }
+  // up to F + 1 output frames: the first chunk of a stream emits the crop of [0, region end)
+  const size_t smem = ((size_t)(nw * M + 15) & ~(size_t)15) + (size_t)(F + 1) * M;
+  if (smem > 200 * 1024) {
+    set_error("post_slots: latency / step too large for the shared-memory plan");
+    return -1;
+  }
+  static bool attr_done[64] = {};
+  if (smem > 48 * 1024 && first_use_on_device(attr_done))
+    DG_CUDA(cudaFuncSetAttribute(post_slots_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  post_slots_kernel<<<B, POST_THREADS, smem, st>>>(seg, map, hist_seg, hist_map, act, rows, slots, F, K, M, nw, plan,
+                                                   plan_stride, hamming, tau, header, turns, turn_cap, total);
+  DG_LAUNCHED();
+  return 0;
+}
+
+int launch_post_slots_history(const float* seg, const int32_t* map, float* hist_seg, int32_t* hist_map, const TickSlot* act,
+                              int n_act, int slots, int F, int K, int nw, cudaStream_t st) {
+  ProfScope _ps("post_slots_history", st);
+  if (n_act < 1 || nw < 2) return 0;
+  post_slots_history_kernel<<<dim3(n_act, nw - 1), 256, 0, st>>>(seg, map, hist_seg, hist_map, act, slots, F * K, K, nw);
   DG_LAUNCHED();
   return 0;
 }

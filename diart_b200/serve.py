@@ -1,0 +1,186 @@
+"""Many live audio streams on one GPU (``dg_multi``, ``csrc/api_multi.cu``).
+
+The reference serves a live stream with ``StreamingInference(batch_size=1)``: one 5 s window every 0.5 s, each a separate
+``SpeakerDiarization.__call__`` (``diart.stream`` / ``diart.serve``).  N streams on one GPU would be N batch-1 network passes
+per step.  ``MultiStreamDiarization`` owns up to ``max_streams`` streams with one configuration and the same native models and
+serves them in ticks: every open stream gives its complete, unconsumed windows (at most ``max_windows_per_stream``), and all
+of them run as one batch -- one upload of the new audio, one network pass, one clustering launch with a state per stream,
+one post-path launch with an aggregation history per stream.  A stream's scores are bit-identical to those its own
+``SpeakerDiarization`` computes on its windows one at a time, and so are the post-path's arithmetic and plan.  Its
+embeddings can differ in the last bits (the fused TDNN5 pooling groups its partial sums by a window's row in the batch), so
+a clustering decision that lies exactly at a threshold could go the other way; apart from that the speaker maps and turns
+are the dedicated pipeline's.  Only the turns come back (the reference's serve hook writes RTTM, no audio)."""
+from __future__ import annotations
+
+import ctypes as C
+from typing import Dict, List, Optional, Tuple
+
+import numpy as np
+import torch
+
+from . import _lib
+from . import models as m
+from .blocks.diarization import SpeakerDiarizationConfig
+from .blocks.post import chunk_annotations, crop_plan
+from .core import Annotation
+
+
+def plan_rows(idx: np.ndarray, step: float, window_samples: int, sample_rate: int, frames: int, nw: int, latency: float):
+    """The post-path plan rows (``blocks.post.post_plan``) of chunks ``idx`` (B,) of streams whose window i starts at
+    ``i * step`` and is fed to its pipeline one window per call -> (plan int32 (B, 4 + nw), out_start (B,), out_res (B,)).
+    A row depends only on the chunk's index within its stream, so one vectorised evaluation covers every stream of a tick.
+    Each buffer has its own start time and score resolution (extent duration / frames of its window, as
+    ``SpeakerDiarization.__call__`` measures it)."""
+    idx = np.asarray(idx, dtype=np.int64)
+    win = window_samples * (1 / sample_rate)                 # SlidingWindowFeature.extent: start + n * step
+
+    def start_res(k):
+        s = k * step
+        e = s + win
+        return s, np.where(e > s, e - s, 0.0) / frames       # Segment.duration / frames
+
+    starts, res = start_res(idx.astype(np.float64))
+    nb = np.minimum(idx + 1, nw)
+    j = np.arange(nw)[None, :]
+    valid = j < nb[:, None]
+    s_j, r_j = start_res(np.where(valid, (idx - (nb - 1))[:, None] + j, 0).astype(np.float64))
+    return crop_plan(starts, res, s_j, r_j, nb, valid, nw, frames, step, latency)
+
+
+def available_windows(pushed: np.ndarray, emitted: np.ndarray, window_samples: int, step_samples: int) -> np.ndarray:
+    """complete windows of streams that received ``pushed`` samples and gave ``emitted`` windows (dg_multi_available)"""
+    have = pushed - emitted * step_samples
+    return np.where(have >= window_samples, (have - window_samples) // step_samples + 1, 0)
+
+
+class MultiStreamDiarization:
+    """Up to ``max_streams`` live 16 kHz streams diarized on one device with one ``SpeakerDiarizationConfig``:
+    ``open(shift) -> sid``, ``push(sid, block)``, ``close(sid)``, and ``step() -> {sid: [Annotation, ...]}`` with one
+    ``Annotation`` per window consumed in the tick, in order -- what ``SpeakerDiarization(config)`` returns for that stream's
+    windows fed one per call, with its ``timestamp_shift`` set to ``shift``, up to the embedding caveat of the module
+    docstring.  Needs the native models (``B200*Loader``)."""
+
+    def __init__(self, config: SpeakerDiarizationConfig, max_streams: int, max_windows_per_stream: int = 4):
+        self._h: Optional[C.c_void_p] = None
+        self.config = config
+        msg = f"Latency should be in the range [{config.step}, {config.duration}]"
+        assert config.step <= config.latency <= config.duration, msg
+        for lazy in (config.segmentation, config.embedding):
+            lazy.eval()
+            lazy.to(config.device)
+        seg_net, emb_net = config.segmentation.model, config.embedding.model
+        if not isinstance(seg_net, m.B200PyanNet) or not isinstance(emb_net, m.B200XVectorSincNet):
+            raise _lib.DiartB200Error("MultiStreamDiarization needs the native segmentation and embedding models")
+        sr = config.sample_rate
+        self.window_samples = int(np.rint(config.duration * sr))
+        self.step_samples = int(round(config.step * sr))
+        self.max_streams, self.max_windows_per_stream = int(max_streams), int(max_windows_per_stream)
+        self.F, self.K = seg_net.dims(self.window_samples)
+        self.D = emb_net.dims(self.window_samples)[1]
+        self.nw = int(round(config.latency / config.step))      # DelayedAggregation.num_overlapping_windows
+        self.labels = [f"speaker{g}" for g in range(config.max_speakers)]
+        self.device = seg_net.device
+        ham = np.ascontiguousarray(np.hamming(self.F), dtype=np.float64)
+        h = C.c_void_p()
+        _lib.check(_lib.lib().dg_multi_create(seg_net.handle, emb_net.handle, self.window_samples, self.step_samples,
+                                              self.max_streams, self.max_windows_per_stream, int(config.max_speakers),
+                                              float(config.tau_active), float(config.rho_update), float(config.delta_new),
+                                              float(config.gamma), float(config.beta),
+                                              int(config.normalize_embedding_weights), self.nw, ham.ctypes.data,
+                                              C.byref(h)))
+        self._h = h
+        # host mirror of the slots: open, samples pushed, windows consumed, timestamp shift
+        self._open = np.zeros(self.max_streams, dtype=bool)
+        self._pushed = np.zeros(self.max_streams, dtype=np.int64)
+        self._emitted = np.zeros(self.max_streams, dtype=np.int64)
+        self._shift = np.zeros(self.max_streams, dtype=np.float64)
+        self._turns = np.empty(1 << 16, dtype=np.uint32)
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None) is not None:
+                _lib.lib().dg_multi_destroy(self._h)
+        except Exception:  # noqa: BLE001
+            pass
+
+    @property
+    def handle(self) -> C.c_void_p:
+        return self._h
+
+    def open(self, shift: float = 0.0) -> int:
+        """a new stream (fresh clustering and aggregation state) in the lowest free slot; returns its id"""
+        free = np.flatnonzero(~self._open)
+        if len(free) == 0:
+            raise ValueError(f"all {self.max_streams} streams are open")
+        sid = int(free[0])
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().dg_multi_open(self._h, sid))
+        self._open[sid] = True
+        self._pushed[sid] = self._emitted[sid] = 0
+        self._shift[sid] = float(shift)
+        return sid
+
+    def close(self, sid: int):
+        _lib.check(_lib.lib().dg_multi_close(self._h, int(sid)))
+        self._open[sid] = False
+
+    def push(self, sid: int, block: np.ndarray):
+        """appends a block of samples, shape (n,), (1, n) or (n, 1), to stream ``sid``; staged until the next ``step``"""
+        x = np.asarray(block, dtype=np.float32)
+        if x.ndim == 2:
+            if 1 not in x.shape:
+                raise ValueError(f"Waveform must have shape (1, samples) but {x.shape} was found")
+            x = x.reshape(-1)
+        x = np.ascontiguousarray(x)
+        _lib.check(_lib.lib().dg_multi_push_host(self._h, int(sid), x.ctypes.data, len(x)))
+        self._pushed[sid] += len(x)
+
+    def available(self, sid: int) -> int:
+        n = _lib.lib().dg_multi_available(self._h, int(sid))
+        _lib.check(min(n, 0))
+        return n
+
+    def window_start_time(self, sid: int, i: int) -> float:
+        """start of window i of stream ``sid`` in its output time base (``DeviceAudioStream.window_start_time`` + shift)"""
+        return i * self.config.step + float(self._shift[sid])
+
+    def step(self) -> Dict[int, List[Annotation]]:
+        """one tick: every open stream's complete windows (at most ``max_windows_per_stream``) -> {sid: annotations}"""
+        return self._step()[0]
+
+    def _step(self, outputs: bool = False) -> Tuple[Dict[int, List[Annotation]], Optional[tuple]]:
+        """``step``; ``outputs``: also the tick's scores (B, F, K), embeddings (B, K, D) and maps (B, K) as device tensors,
+        rows grouped by stream in slot order"""
+        counts = np.where(self._open, np.minimum(available_windows(self._pushed, self._emitted, self.window_samples,
+                                                                   self.step_samples), self.max_windows_per_stream), 0)
+        sids = np.flatnonzero(counts)
+        n = counts[sids]
+        B = int(n.sum())
+        row0 = np.cumsum(n) - n
+        idx = np.repeat(self._emitted[sids], n) + (np.arange(B) - np.repeat(row0, n))
+        cfg = self.config
+        plan, out_start, out_res = plan_rows(idx, cfg.step, self.window_samples, cfg.sample_rate, self.F, self.nw,
+                                             cfg.latency)
+        plan = np.ascontiguousarray(plan)
+        header = np.empty((B, 4), dtype=np.int32)
+        need = B * cfg.max_speakers * ((self.F + 2) // 2)
+        if len(self._turns) < need:
+            self._turns = np.empty(need, dtype=np.uint32)
+        got = np.empty(self.max_streams, dtype=np.int32)
+        n_turns = C.c_int()
+        outs = None
+        if outputs and B:
+            outs = (torch.empty((B, self.F, self.K), device=self.device), torch.empty((B, self.K, self.D), device=self.device),
+                    torch.empty((B, self.K), device=self.device, dtype=torch.int32))
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().dg_multi_step(self._h, plan.ctypes.data, B, got.ctypes.data, header.ctypes.data,
+                                                self._turns.ctypes.data, len(self._turns), C.byref(n_turns),
+                                                *([t.data_ptr() for t in outs] if outs else [None, None, None])))
+        if not np.array_equal(got, counts):
+            raise _lib.DiartB200Error("stream bookkeeping out of step with the device handle")
+        self._emitted += counts
+        if B == 0:
+            return {}, outs
+        anns = chunk_annotations(header, self._turns, n_turns.value, out_start, out_res, self.labels,
+                                 np.repeat(self._shift[sids], n))
+        return {int(s): anns[r:r + k] for s, r, k in zip(sids.tolist(), row0.tolist(), n.tolist())}, outs

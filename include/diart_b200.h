@@ -318,6 +318,54 @@ int dg_pipeline_call_stream(dg_pipeline* h, dg_post* post, dg_stream* stream, in
                             int32_t* header_host, uint32_t* turns_host, int turn_cap_host, int* n_turns,
                             float* seg_host /*nullable*/, int32_t* map_host /*nullable*/);
 
+/* ---- many live streams on one device: the reference's live loop (src/diart/inference.py: StreamingInference with
+ *      batch_size=1, one window per stream every step) runs SpeakerDiarization.__call__ (src/diart/blocks/diarization.py:172-232)
+ *      once per stream and window.  A dg_multi owns up to max_streams such streams, all with one configuration and the same
+ *      model handles, and serves them in ticks: every open stream gives its complete, unconsumed windows (at most
+ *      max_windows_per_stream) and they run as ONE batch, with every stream's result that of its own pipeline.
+ *      dg_multi_create: chunk_samples / step_samples positive multiples of 4 (window i of a stream is samples
+ *        [i * step, i * step + chunk)); max_streams * max_windows_per_stream <= 65535; tau, rho, delta = tau_active,
+ *        rho_update, delta_new (cosine clustering with max_speakers <= 32 centres; tau_active also binarises); gamma, beta,
+ *        normalize_weights as dg_pipeline_create; num_windows = latency / step and hamming_host = np.hamming(frames) in
+ *        float64, as dg_post_create.  The model handles are borrowed and may serve other pipelines meanwhile.
+ *      dg_multi_open: a new stream in `slot` (0 <= slot < max_streams, not open): no samples, fresh clustering state (the
+ *        reference's reset()), no aggregation history.  dg_multi_close: the stream in `slot` ends; its staged samples are
+ *        dropped.
+ *      dg_multi_push_host: appends n samples (any block size) to the stream in `slot`.  They are copied to pinned staging;
+ *        nothing reaches the device before the next tick.  Fails with DG_EINVAL, writing nothing, if the stream would hold
+ *        more unconsumed samples than its ring (chunk + 2 max_windows_per_stream step, rounded up to 1024).
+ *      dg_multi_available: complete windows of the stream in `slot` not yet consumed (staged samples included), or DG_EINVAL.
+ *      dg_multi_step: one tick.  Every open slot s, in slot order, gives n_s = min(available, max_windows_per_stream) windows;
+ *        counts_host int32 [max_streams] receives n_s.  The n_rows = sum n_s chunks are the tick's rows, grouped by slot, each
+ *        slot's in window order; plan_host int32 [n_rows][4 + num_windows] holds their dg_post_step plan rows (a chunk's row
+ *        depends only on its window index within its stream: diart_b200.serve.plan_rows).  n_rows must equal sum n_s, else
+ *        DG_EINVAL.  header_host int32 [n_rows][4] and turns_host as dg_post_step.  seg_dev [n_rows, F, K], emb_dev
+ *        [n_rows, K, D] and map_dev [n_rows, K] (device, nullable) receive the tick's network outputs and speaker maps.  All
+ *        staged samples go up in one copy; the networks run in sub-batches of at most 256 windows.  A tick without windows
+ *        launches nothing.  Every argument is checked before any launch.  Synchronous. ---- */
+typedef struct dg_multi dg_multi;
+int dg_multi_create(dg_seg* seg, dg_emb* emb, int chunk_samples, int step_samples, int max_streams, int max_windows_per_stream,
+                    int max_speakers, double tau, double rho, double delta, float gamma, float beta, int normalize_weights,
+                    int num_windows, const double* hamming_host, dg_multi** out);
+int dg_multi_open(dg_multi* h, int slot);
+int dg_multi_close(dg_multi* h, int slot);
+int dg_multi_push_host(dg_multi* h, int slot, const float* samples_host, int n);
+int dg_multi_available(const dg_multi* h, int slot);
+int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, int32_t* counts_host, int32_t* header_host,
+                  uint32_t* turns_host, int turn_cap_host, int* n_turns, float* seg_dev /*nullable*/,
+                  float* emb_dev /*nullable*/, int32_t* map_dev /*nullable*/);
+/* device time of the last tick that had windows, from events on the handle's stream around all of its device work (upload,
+ * networks, clustering, post-path, download), in ms; DG_EINVAL before the first such tick */
+int dg_multi_last_step_ms(const dg_multi* h, float* ms);
+int dg_multi_destroy(dg_multi* h);
+/* test hook (host only, no GPU): dg_multi's bookkeeping of pushed audio on `slots` rings of C samples, with ring_scatter's
+ * writes done on the host.  ops int32 [n_ops][3] = {kind, slot, n}: 0 open slot, 1 close slot (its staged samples are
+ * dropped), 2 push the next n samples of samples_host (a refused push still skips them), 3 consume n samples (as a tick's
+ * windows do), 4 tick (every staged sample to its ring).  result int32 [n_ops]: each op's return code, DG_EINVAL for a
+ * refused one (a push beyond the ring capacity, a closed or unknown slot).  rings_host float [slots][C]: written by ticks. */
+int dg_selftest_multi_staging_host(int slots, int C, int n_ops, const int32_t* ops, const float* samples_host, int32_t* result,
+                                   float* rings_host);
+
 /* ---- resampling: torchaudio's T.Resample(orig, new) with its defaults (sinc_interp_hann, lowpass_filter_width 6,
  *      rolloff 0.99), what the reference's blocks.Resample applies to every window of a source at another rate (reference
  *      src/diart/blocks/utils.py:62-89, inference.py:101-123).  With g = gcd(orig, new), o = orig / g, n = new / g:
