@@ -35,6 +35,9 @@ SIGNATURES = {
     "dg_selftest_gemm_tc_grid": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int)]),
     "dg_selftest_gemm_tc_bounds": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
                                              C.POINTER(C.c_int)]),
+    "dg_selftest_wgmma_row_shift": (C.c_int, [C.c_int, C.POINTER(C.c_uint)]),
+    "dg_selftest_gemm_tc_halo": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int),
+                                           C.POINTER(C.c_int)]),
     "dg_selftest_split_f16_host": (C.c_int, [_P, C.c_longlong, _P, _P]),
     "dg_seg_create": (C.c_int, [C.POINTER(DgTensor), C.c_int, C.c_int, C.POINTER(_P)]),
     "dg_seg_dims": (C.c_int, [_P, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),

@@ -138,7 +138,7 @@ extern "C" int dg_selftest_split_f16_host(const float* x, long long n, unsigned 
 // kernel on seeded random data and reports the largest absolute difference and the output scale.
 extern "C" int dg_selftest_gemm_tc(int M, int Cin, int KW, int dil, int N, int epi, float* max_abs_diff,
                                    float* out_rms) {
-  if (M < 1 || Cin % 64 || KW < 1 || N % 4 || !max_abs_diff || !out_rms) {
+  if (M < 1 || Cin < 16 || Cin % 16 || KW < 1 || N % 4 || !max_abs_diff || !out_rms) {
     set_error("dg_selftest_gemm_tc: bad arguments");
     return DG_EINVAL;
   }
@@ -314,6 +314,107 @@ extern "C" int dg_selftest_gemm_tc_grid(int M, int Cin, int KW, int dil, int N, 
     DG_CUDA(cudaMemcpy(cur.data() + f32_bytes + plane_bytes, dOl.p, plane_bytes, cudaMemcpyDeviceToHost));
     DG_CUDA(cudaMemcpy(cur.data() + f32_bytes + 2 * plane_bytes, dPart.p, part_bytes, cudaMemcpyDeviceToHost));
     if (ci == 0)
+      first.swap(cur);
+    else if (cur != first)
+      *equal = 0;
+  }
+  return DG_OK;
+}
+
+// Sets bit r of *ok_shifts when a wgmma whose A descriptor starts r = 0..8 rows into a 64B-swizzled TMA tile computes the
+// exact product of rows r..r+63; base_offset_mode 1 also sets the descriptor's matrix base offset to (address >> 7) & 7.
+extern "C" int dg_selftest_wgmma_row_shift(int base_offset_mode, unsigned* ok_shifts) {
+  if (base_offset_mode < 0 || base_offset_mode > 1 || !ok_shifts) {
+    set_error("dg_selftest_wgmma_row_shift: bad arguments");
+    return DG_EINVAL;
+  }
+  return selftest_wgmma_row_shift(base_offset_mode, ok_shifts) ? DG_ECUDA : DG_OK;
+}
+
+// Runs one seeded Conv1d GEMM (epilogue 0, 1, 2 or 5) through the halo operand mode, under no SM cap and under a cap of 3
+// SMs, and through the tap-box mode, and sets *equal = 1 if all three wrote the same bytes: float32 rows, hi/lo planes,
+// pooling partial sums.  A Cin that is not a multiple of 64 (SincNet's 80) has no tap-box form: the reference then reads
+// the taps folded into K = KW * Cin rounded up to 64 through an overlapping-row view (dil must be 1), with zero weights
+// past KW * Cin.  *halo = 1 if the launch took the halo mode.  Epilogue 5 pools items of 888 rows (M a multiple of it).
+extern "C" int dg_selftest_gemm_tc_halo(int M, int Cin, int KW, int dil, int N, int epi, int* equal, int* halo) {
+  const bool folded = Cin % 64 != 0;
+  if (M < 1 || Cin < 16 || Cin % 16 || Cin > 128 || KW < 2 || KW > 9 || dil < 1 || N < 1 || N % 4 ||
+      (epi != 0 && epi != 1 && epi != 2 && epi != 5) || (epi == 1 && N % 32) || (epi == 5 && (N > 64 || M % 888)) ||
+      (folded && dil != 1) || !equal || !halo) {
+    set_error("dg_selftest_gemm_tc_halo: bad arguments");
+    return DG_EINVAL;
+  }
+  const int K = KW * Cin, Kf = folded ? (K + 63) / 64 * 64 : K;
+  const int npad = epi == 5 || N == 64 ? 64 : (N + 127) / 128 * 128;
+  const int item_rows = 888, tile_rows = epi == 5 ? gemm_tc_pool3_tile_rows(item_rows) : 128;
+  const long long m_tiles = (M + tile_rows - 1) / tile_rows;
+  const long long tail = 64;   // zero rows after M: the folded view reads up to Kf / Cin rows past its own
+  uint32_t seed = 9090u;
+  auto rnd = [&]() {
+    seed = seed * 1664525u + 1013904223u;
+    return ((seed >> 8) & 0xFFFF) / 65536.f - 0.5f;
+  };
+  std::vector<float> A((size_t)(M + tail) * Cin, 0.f), Wnk((size_t)N * K), Wf((size_t)N * Kf, 0.f), bias(N), bsc(N), bsh(N);
+  for (size_t i = 0; i < (size_t)M * Cin; i++) A[i] = 2.f * rnd();
+  for (auto& v : Wnk) v = 0.25f * rnd();
+  for (int n = 0; n < N; n++)
+    for (int k = 0; k < K; k++) Wf[(size_t)n * Kf + k] = Wnk[(size_t)n * K + k];
+  for (int n = 0; n < N; n++) {
+    bias[n] = rnd();
+    bsc[n] = 1.f + rnd();
+    bsh[n] = rnd();
+  }
+  const size_t f32_bytes = epi == 0 || epi == 2 ? (size_t)M * N * 4 : (epi == 5 ? (size_t)(M / 3) * N * 4 : 0);
+  const size_t plane_bytes = epi == 1 ? (size_t)M * N * 2 : 0;
+  const size_t part_bytes = epi == 5 ? (size_t)m_tiles * 2 * 2 * N * 4 : 0;
+  DevBuf dA, dAh, dAl, dB, dS, dH, dF, dOh, dOl, dPart;
+  WeightPlanes dW, dWf;
+  if (upload(dA, A) || upload(dB, bias) || upload(dS, bsc) || upload(dH, bsh) || upload_split(dW, Wnk, N, npad, K) ||
+      upload_split(dWf, Wf, N, npad, Kf))
+    return DG_ECUDA;
+  if (dAh.ensure((size_t)(M + tail) * Cin * 2) || dAl.ensure((size_t)(M + tail) * Cin * 2) || dF.ensure(f32_bytes + 4) ||
+      dOh.ensure(plane_bytes + 4) || dOl.ensure(plane_bytes + 4) || dPart.ensure(part_bytes + 4))
+    return DG_ECUDA;
+  int rc;
+  if ((rc = launch_split_ex(dA.as<float>(), M + tail, Cin, Cin, Cin, 0, 1, nullptr, nullptr, dAh.p, dAl.p, nullptr))) return rc;
+  TcGemm t{};
+  t.A_hi = dAh.p; t.A_lo = dAl.p; t.lda = Cin; t.Cin = Cin; t.KW = KW; t.dil = dil; t.Mtot = M; t.M = M;
+  t.N = N; t.bias = dB.as<float>(); t.bn_scale = dS.as<float>(); t.bn_shift = dH.as<float>(); t.ldc = N;
+  t.epi = epi; t.tag = "selftest_tc_halo";
+  t.out_f32 = f32_bytes ? dF.as<float>() : nullptr;
+  t.out_hi = plane_bytes ? dOh.p : nullptr;
+  t.out_lo = plane_bytes ? dOl.p : nullptr;
+  if (epi == 5) {
+    t.pool_part = dPart.as<float>(); t.pool_item_rows = item_rows; t.pool3_T = item_rows / 3 - 2;
+    t.pool3_tile_rows = tile_rows;
+  }
+  if ((rc = set_weights(t, dW))) return rc;
+  *halo = gemm_tc_halo(t) ? 1 : 0;
+  TcGemm ref = t;
+  ref.tap_boxes = 1;
+  if (folded) {
+    ref.Cin = Kf;
+    ref.KW = 1;
+    if ((rc = set_weights(ref, dWf))) return rc;
+  }
+  std::vector<unsigned char> first, cur;
+  *equal = 1;
+  for (int run = 0; run < 3; run++) {   // halo, halo on 3 SMs, tap boxes
+    DG_CUDA(cudaMemset(dF.p, 0, f32_bytes + 4));
+    DG_CUDA(cudaMemset(dOh.p, 0, plane_bytes + 4));
+    DG_CUDA(cudaMemset(dOl.p, 0, plane_bytes + 4));
+    DG_CUDA(cudaMemset(dPart.p, 0, part_bytes + 4));
+    {
+      SmLimit cap(run == 1 ? 3 : 0);
+      if ((rc = launch_gemm_tc(run == 2 ? ref : t, nullptr))) return rc;
+    }
+    DG_CUDA(cudaDeviceSynchronize());
+    cur.resize(f32_bytes + 2 * plane_bytes + part_bytes);
+    DG_CUDA(cudaMemcpy(cur.data(), dF.p, f32_bytes, cudaMemcpyDeviceToHost));
+    DG_CUDA(cudaMemcpy(cur.data() + f32_bytes, dOh.p, plane_bytes, cudaMemcpyDeviceToHost));
+    DG_CUDA(cudaMemcpy(cur.data() + f32_bytes + plane_bytes, dOl.p, plane_bytes, cudaMemcpyDeviceToHost));
+    DG_CUDA(cudaMemcpy(cur.data() + f32_bytes + 2 * plane_bytes, dPart.p, part_bytes, cudaMemcpyDeviceToHost));
+    if (run == 0)
       first.swap(cur);
     else if (cur != first)
       *equal = 0;

@@ -82,15 +82,14 @@ int prep_sincnet(const Tensors& t, const std::string& pre, SincWeights& w) {
     return upload_split(dst, w_nk, out, 64, k * in_pad);
   };
   {
-    // Conv1d(80, 60, 5) with its taps folded into K: the input planes are 80-channel rows (pitch 160 B), so the im2col row of
-    // output row m is the 400 CONTIGUOUS values starting at row m -- read through an overlapping-row TMA view, K = 448
+    // Conv1d(80, 60, 5) over 80-channel rows: K = 5 taps x 80 channels (the GEMM's halo mode)
     const float* s1 = t.get(pre + "conv1d.1.weight", (int64_t)60 * 80 * 5);
     if (!s1) return DG_EWEIGHT;
-    std::vector<float> w_nk((size_t)60 * 448, 0.f);
+    std::vector<float> w_nk((size_t)60 * 400, 0.f);
     for (int o = 0; o < 60; o++)
       for (int c = 0; c < 80; c++)
-        for (int j = 0; j < 5; j++) w_nk[(size_t)o * 448 + j * 80 + c] = s1[((size_t)o * 80 + c) * 5 + j];
-    if (upload_split(w.w1, w_nk, 60, 64, 448)) return DG_ECUDA;
+        for (int j = 0; j < 5; j++) w_nk[(size_t)o * 400 + j * 80 + c] = s1[((size_t)o * 80 + c) * 5 + j];
+    if (upload_split(w.w1, w_nk, 60, 64, 400)) return DG_ECUDA;
   }
   if ((rc = conv_w_tc(pre + "conv1d.2.weight", 60, 60, 5, 64, w.w2))) return rc;
   return 0;
@@ -170,7 +169,7 @@ int run_sincnet(const SincWeights& w, SincWork& k, const float* wav, int B, cons
   if (tr0 && tr1) {
     if (k.part3.ensure((size_t)(M0 / tr0) * 2 * 2 * 64 * 4)) return DG_ECUDA;
     TcGemm t{};
-    t.A_hi = k.a0h.p; t.A_lo = k.a0l.p; t.lda = 80; t.Cin = 448; t.KW = 1; t.dil = 1; t.Mtot = M0; t.M = M0;
+    t.A_hi = k.a0h.p; t.A_lo = k.a0l.p; t.lda = 80; t.Cin = 80; t.KW = 5; t.dil = 1; t.Mtot = M0; t.M = M0;
     t.N = 64; t.bias = w.bias1.as<float>(); t.out_f32 = k.p1.as<float>(); t.ldc = 64; t.epi = 5; t.tag = "sinc_conv1";
     t.pool_part = k.part3.as<float>(); t.pool_item_rows = g.S0; t.pool3_T = g.T1; t.pool3_tile_rows = tr0;
     if ((rc = set_weights(t, w.w1)) || (rc = launch_gemm_tc(t, st)) ||
@@ -188,7 +187,7 @@ int run_sincnet(const SincWeights& w, SincWork& k, const float* wav, int B, cons
                                     w.b2.as<float>(), k.sc2.as<float>(), k.sh2.as<float>(), 64, st);
   }
   TcGemm t{};
-  t.A_hi = k.a0h.p; t.A_lo = k.a0l.p; t.lda = 80; t.Cin = 448; t.KW = 1; t.dil = 1; t.Mtot = M0; t.M = M0;
+  t.A_hi = k.a0h.p; t.A_lo = k.a0l.p; t.lda = 80; t.Cin = 80; t.KW = 5; t.dil = 1; t.Mtot = M0; t.M = M0;
   t.N = 64; t.bias = w.bias1.as<float>(); t.out_f32 = k.c1.as<float>(); t.ldc = 64; t.epi = 0; t.tag = "sinc_conv1";
   if ((rc = set_weights(t, w.w1)) || (rc = launch_gemm_tc(t, st))) return rc;
   if ((rc = launch_instnorm_stats(k.c1.as<float>(), B, g.S0, g.T1, 64, 64, w.g1.as<float>(), w.b1.as<float>(),

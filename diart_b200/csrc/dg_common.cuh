@@ -164,6 +164,7 @@ struct TcGemm {
   // pool_part = per-tile partial sums [M / pool3_tile_rows][2][2][N], reduced by launch_instnorm_finalize;
   // pool_item_rows = un-pooled rows per item (multiple of 3), pool3_T = valid pooled frames per item
   int pool3_T, pool3_tile_rows;
+  int tap_boxes;         // 1: load A per tap even where the halo mode applies (self-tests compare the two operand paths)
 };
 // rows an m-tile of the pooling epilogue advances by: the largest multiple of 3 up to 126 that divides the item's rows
 // (tiles never straddle items: an item's statistics are grouped identically wherever it sits in the batch); 0 if none >= 96
@@ -173,6 +174,10 @@ inline int gemm_tc_pool3_tile_rows(int item_rows) {
   return 0;
 }
 int launch_gemm_tc(const TcGemm& g, cudaStream_t st);
+bool gemm_tc_halo(const TcGemm& g);   // the launch loads each tile's rows once (halo mode) instead of once per tap
+// one m64n8k16 wgmma per row shift r = 0..8 of its A descriptor into a 64B-swizzled tile (dg_selftest_wgmma_row_shift):
+// bit r of *ok_shifts is set when the product of rows r..r+63 is exact for both k16 steps of the 32-channel row
+int selftest_wgmma_row_shift(int base_offset_mode, unsigned* ok_shifts);
 int launch_split_ex(const float* x, long long rows_out, int C, int ld_in, int ld_out, int pool, int item_rows,
                     const float* sc, const float* sh, void* hi, void* lo, cudaStream_t st, const int* skip_flag = nullptr);
 void split_weights_host(const float* w, int N, int Npad, int K, uint16_t* hi, uint16_t* lo, float scale = 1.f);

@@ -48,7 +48,9 @@
 #include <algorithm>
 #include <map>
 #include <mutex>
+#include <string>
 #include <utility>
+#include <vector>
 
 #include "dg_common.cuh"
 #include "tc_ptx.cuh"
@@ -87,6 +89,13 @@ struct TcArgs {
   // [m_tiles][2 (item of the tile)][2 (sum, sum of squares)][N] over the pooled frames < pool3_T of an item
   int tile_rows, pool3_T;
   unsigned* tile_ctr;      // pooling epilogues, [2]: tiles handed out past the first wave, CTAs finished (both back to 0)
+  // halo operand mode (gemm_tc_kernel<.., true>): a tile's A operand is its halo, rows m0 .. m0 + halo_rows - 1 of all cin
+  // channels, loaded once per tile as [hi | lo][ceil(cin / 32)] boxes of halo_rows x 32 channels (64B swizzle)
+  int halo_rows;           // rows of a halo box (tc_halo_rows)
+  int cin;                 // channels per tap, a multiple of 16 (no k16 step straddles a tap)
+  int wblocks;             // W k-blocks per tile: ceil(KW * cin / 32), two k16 steps each
+  int halo_bytes;          // one consumer's halo slot (a multiple of 1 KB)
+  int op_bytes;            // the operand region: tap-box ring, or the two halo slots + the W ring
 };
 
 enum TcEpi { TC_BIAS_F32 = 0, TC_LEAKY_BN_SPLIT = 1, TC_LEAKY_BN_F32 = 2, TC_CONV2D = 3, TC_POOL = 4, TC_MAXPOOL3 = 5 };
@@ -95,16 +104,22 @@ __host__ __device__ constexpr bool tc_pooling(int epi) { return epi == TC_POOL |
 // epilogues whose output tile leaves as TMA boxes
 __host__ __device__ constexpr bool tc_box_store(int epi) { return epi == TC_BIAS_F32 || epi == TC_LEAKY_BN_SPLIT || epi == TC_LEAKY_BN_F32; }
 
-// Layout: [NSTAGE stages of (A hi, A lo, W hi, W lo)] [element-wise: the shared staging tile] [barriers] [consumer 0:
-// parameters | pooling: chunk | pooling staging] [consumer 1: the same].  Stages and staging tile are multiples of 1 KB,
-// so the staging tile keeps the 1 KB alignment of 128B-swizzled boxes.
+// Layout: [operands] [element-wise: the shared staging tile] [barriers] [consumer 0: parameters | pooling: chunk | pooling
+// staging] [consumer 1: the same].  Operands, tap-box mode: NSTAGE stages of (A hi, A lo, W hi, W lo); halo mode: the halo
+// slots of consumer 0 and 1, then NSTAGE_HALO stages of (W hi, W lo).  Every operand block is a multiple of 1 KB, so the
+// staging tile keeps the 1 KB alignment of 128B-swizzled boxes.
 template <int BN>
 struct TcSmem {
   static constexpr int A_BYTES = TC_BM * TC_BK * 2;     // 8 KB per plane
   static constexpr int W_BYTES = BN * TC_BK * 2;
   static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;
+  static constexpr int W_STAGE_BYTES = 2 * W_BYTES;
   // 128 / 144 / 120 KB of operands in flight at BN = 128 / 64 / 32
   static constexpr int NSTAGE = BN == 128 ? 4 : 6;
+  static constexpr int NSTAGE_HALO = BN == 128 ? 5 : 6;   // 80 / 48 KB of W in flight
+  // halo slot of `cin` channels x `rows` rows, hi and lo planes
+  __host__ static int halo_bytes(int cin, int rows) { return (2 * ((cin + 31) / 32) * rows * 64 + 1023) / 1024 * 1024; }
+  __host__ static int halo_op_bytes(int cin, int rows) { return 2 * halo_bytes(cin, rows) + NSTAGE_HALO * W_STAGE_BYTES; }
   static constexpr int BAR_BYTES = 256;
   static constexpr int PARAM_FLOATS = 3 * BN;
   // pooling: CHUNK_W accumulator columns of every tile row, as [CHUNK_W / 32][128][33] (conflict-free column reads)
@@ -120,8 +135,8 @@ struct TcSmem {
   __host__ __device__ static constexpr int stage_tile_bytes(int epi) {
     return tc_pooling(epi) ? 0 : (epi == TC_CONV2D ? TC_BM * ACC_LD * 4 : TC_BM * BN * 4);
   }
-  __host__ __device__ static constexpr int total(int epi) {
-    return NSTAGE * STAGE_BYTES + stage_tile_bytes(epi) + BAR_BYTES + 2 * consumer_floats(epi) * 4 + 1024;   // + alignment slack
+  __host__ __device__ static constexpr int total(int epi, int op_bytes = NSTAGE * STAGE_BYTES) {
+    return op_bytes + stage_tile_bytes(epi) + BAR_BYTES + 2 * consumer_floats(epi) * 4 + 1024;   // + alignment slack
   }
 };
 static_assert(TcSmem<128>::total(TC_POOL) <= TC_SMEM_MAX && TcSmem<64>::total(TC_MAXPOOL3) <= TC_SMEM_MAX &&
@@ -470,29 +485,39 @@ __device__ __forceinline__ void tc_pool_epilogue_tile(const TcArgs& a, float* pa
 // epilogues: 5 + c = consumer c may write the shared staging tile (256 threads: consumer c waits, the other consumer
 // arrives once the tile has been read: by its epilogue threads (Conv2d) or by TMA (box epilogues)).
 // tmC0 / tmC1: output maps of the box epilogues (float32 rows; or hi and lo planes).
-template <int BN, int EPI>
+// HALO: Conv1d with few input channels.  The tap-box mode loads, per k-block, the 128 rows of the tile shifted by the tap's
+// offset, so every activation row crosses L2 -> SM once per tap; the halo mode loads a tile's rows m0 .. m0 + 127 +
+// (KW - 1) * dil once, into the slot of the consumer that runs the tile, and points the A descriptor of each k16 step at
+// its tap's first row inside the slot (tc_ptx.cuh: a descriptor may start any whole number of rows into a swizzled tile).
+// The k16 steps run in the tap-box mode's order (tap outer, 16 channels inner), so the results are bit-identical.
+template <int BN, int EPI, bool HALO>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo,
                const __grid_constant__ CUtensorMap tmC0, const __grid_constant__ CUtensorMap tmC1, TcArgs a) {
   using S = TcSmem<BN>;
   constexpr bool POOLING = tc_pooling(EPI);
-  constexpr int NSTAGE = S::NSTAGE;
+  constexpr int NSTAGE = HALO ? S::NSTAGE_HALO : S::NSTAGE;
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  unsigned char* tile_s = smem + NSTAGE * S::STAGE_BYTES;   // element-wise: the staging tile, shared by the consumers
+  unsigned char* ring = HALO ? smem + 2 * a.halo_bytes : smem;   // the k-block ring (halo mode: W only)
+  constexpr int RING_STAGE = HALO ? S::W_STAGE_BYTES : S::STAGE_BYTES;
+  unsigned char* tile_s = smem + a.op_bytes;   // element-wise: the staging tile, shared by the consumers
   uint64_t* bars = reinterpret_cast<uint64_t*>(tile_s + S::stage_tile_bytes(EPI));
   uint64_t* full = bars;                      // [NSTAGE] TMA -> MMA
   uint64_t* empty = bars + NSTAGE;            // [NSTAGE] MMA -> TMA
   uint64_t* tile_full = bars + 2 * NSTAGE;    // [2] producer -> consumer c: tile_idx[c] holds its next tile
   uint64_t* tile_empty = tile_full + 2;       // [2] consumer c -> producer: tile_idx[c] has been read
-  volatile int* tile_idx = reinterpret_cast<volatile int*>(tile_empty + 2);   // [2]
+  uint64_t* halo_full = tile_empty + 2;       // [2] halo mode: TMA -> consumer c, its slot holds its tile's halo
+  uint64_t* halo_empty = halo_full + 2;       // [2] consumer c -> TMA: the MMAs of its tile are complete
+  volatile int* tile_idx = reinterpret_cast<volatile int*>(halo_empty + 2);   // [2]
   float* cons = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(bars) + S::BAR_BYTES);
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // warp-uniform
   const int wg = warp >> 2;
   const int num_tiles = a.m_tiles * a.n_tiles;
-  const int kblocks = a.KW * a.cin_blocks;
+  const int kblocks = HALO ? a.wblocks : a.KW * a.cin_blocks;   // ring entries per tile
+  const int halo_box = a.halo_rows * 64, halo_cb = (a.cin + 31) / 32;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < NSTAGE; s++) {
@@ -502,6 +527,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     for (int c = 0; c < 2; c++) {
       mbar_init(&tile_full[c], 1);
       mbar_init(&tile_empty[c], 128);
+      mbar_init(&halo_full[c], 1);
+      mbar_init(&halo_empty[c], 1);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -509,9 +536,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
 
   if (wg == 0) {
     // ===================================================================== tile scheduler + TMA producer
-    setmaxnreg_dec<40>();
+    // the halo producer's look-ahead state needs 48 registers; the consumers then get 224 (the launch holds 384 x 168:
+    // 128 x 48 + 256 x 224 fit, 128 x 48 + 256 x 232 do not and setmaxnreg.inc would wait for ever)
+    setmaxnreg_dec<HALO ? 48 : 40>();
     if (threadIdx.x == 0) {
-      int stage = 0, phase = 0;
+      int stage = 0, phase = 0, next = 0;
+      bool halo_next = false;   // halo mode: the halo of the CTA's next tile is on its way
       // i = position in this CTA's sequence of tiles, run by consumer i % 2.  The first tile is blockIdx.x, the later ones
       // come from the counter (pooling) or follow at a stride of the grid.  Two end marks follow the last tile: -1 (its
       // consumer passes the turn on), then -2.
@@ -530,7 +560,49 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         mbar_arrive(&tile_full[c]);
         const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
         const int m0 = mt * (EPI == TC_MAXPOOL3 ? a.tile_rows : TC_BM), n0 = nt * BN;
-        for (int j = 0; j < a.KW; j++) {
+        if constexpr (HALO) {
+          // halo of the tile at row r0 into consumer cc's slot
+          auto load_halo = [&](int cc, int r0) {
+            unsigned char* hs = smem + cc * a.halo_bytes;
+            mbar_expect_tx(&halo_full[cc], 2 * halo_cb * halo_box);
+            for (int cb = 0; cb < halo_cb; cb++) {
+              tma_load_2d(hs + cb * halo_box, &tmA_hi, cb * TC_BK, r0, &halo_full[cc]);
+              tma_load_2d(hs + (halo_cb + cb) * halo_box, &tmA_lo, cb * TC_BK, r0, &halo_full[cc]);
+            }
+          };
+          // this tile's halo, unless it went out during the previous tile's W loads, once consumer c's previous tile has no
+          // MMA left on the slot
+          if (!halo_next) {
+            mbar_wait(&halo_empty[c], ((i >> 1) & 1) ^ 1);
+            load_halo(c, m0);
+          }
+          halo_next = false;
+          // The next tile's halo goes out as soon as the other consumer's slot is free (its MMAs end as this tile's begin),
+          // a whole mainloop before it is needed: behind this tile's W loads it would arrive late
+          next = POOLING ? (int)gridDim.x + (int)atomicAdd(&a.tile_ctr[0], 1u) : tile + (int)gridDim.x;
+          const int next_m0 = next / a.n_tiles * (EPI == TC_MAXPOOL3 ? a.tile_rows : TC_BM);
+          const uint32_t next_par = (((i + 1) >> 1) & 1) ^ 1;
+          for (int kb = 0; kb < kblocks; kb++) {
+            const long long t0 = clock64();
+            for (;;) {
+              if (!halo_next && next < num_tiles && mbar_test_wait(&halo_empty[c ^ 1], next_par)) {
+                load_halo(c ^ 1, next_m0);
+                halo_next = true;
+              }
+              if (mbar_test_wait(&empty[stage], phase ^ 1)) break;
+              if (clock64() - t0 > 4000000000LL) __trap();
+            }
+            unsigned char* st = ring + stage * RING_STAGE;
+            mbar_expect_tx(&full[stage], S::W_STAGE_BYTES);
+            tma_load_2d(st, &tmW_hi, kb * TC_BK, n0, &full[stage]);
+            tma_load_2d(st + S::W_BYTES, &tmW_lo, kb * TC_BK, n0, &full[stage]);
+            if (++stage == NSTAGE) {
+              stage = 0;
+              phase ^= 1;
+            }
+          }
+        }
+        for (int j = 0; j < (HALO ? 0 : a.KW); j++) {
           for (int cb = 0; cb < a.cin_blocks; cb++) {
             mbar_wait(&empty[stage], phase ^ 1);
             unsigned char* st = smem + stage * S::STAGE_BYTES;
@@ -546,7 +618,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
             }
           }
         }
-        tile = POOLING ? (int)gridDim.x + (int)atomicAdd(&a.tile_ctr[0], 1u) : tile + (int)gridDim.x;
+        if (!HALO) next = POOLING ? (int)gridDim.x + (int)atomicAdd(&a.tile_ctr[0], 1u) : tile + (int)gridDim.x;
+        tile = next;
       }
       // every CTA has taken its last tile once all have counted themselves here: the last one returns the counter to 0
       // for the next launch on this stream
@@ -561,7 +634,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     return;
   }
   // ===================================================================== MMA + epilogue (consumers c = 0, 1)
-  setmaxnreg_inc<232>();
+  setmaxnreg_inc<HALO ? 224 : 232>();
   const int c = wg - 1, quad = warp & 3, et = threadIdx.x - 128 * wg;
   float* params = cons + c * S::consumer_floats(EPI);   // bias | bn_scale | bn_shift
   float* chunk = params + S::PARAM_FLOATS;
@@ -594,23 +667,44 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     float acc[2][BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; i++) acc[0][i] = acc[1][i] = 0.f;
+    // halo mode: the next k16 step's first channel and its tap's first row (as a byte offset into a box)
+    uint32_t htap = 0;
+    int hch = 0;
+    if constexpr (HALO) mbar_wait(&halo_full[c], n & 1);
+    const uint32_t hs = smem_u32(smem + c * a.halo_bytes);
     for (int kb = 0; kb < kblocks; kb++) {
       mbar_wait(&full[stage], phase);
-      const uint32_t sa = smem_u32(smem + stage * S::STAGE_BYTES);
-      const uint64_t a_hi = wg_desc_sw64(sa), a_lo = wg_desc_sw64(sa + S::A_BYTES);
-      const uint64_t w_hi = wg_desc_sw64(sa + 2 * S::A_BYTES), w_lo = wg_desc_sw64(sa + 2 * S::A_BYTES + S::W_BYTES);
-      constexpr uint64_t HALF = (uint64_t)((64 * TC_BK * 2) >> 4);   // rows 64..127 of the A tile
+      const uint32_t sa = smem_u32(ring + stage * RING_STAGE);
+      const uint32_t sw = HALO ? sa : sa + 2 * S::A_BYTES;
+      const uint64_t w_hi = wg_desc_sw64(sw), w_lo = wg_desc_sw64(sw + S::W_BYTES);
+      constexpr uint64_t HALF = (uint64_t)((64 * TC_BK * 2) >> 4);   // rows 64..127 of the A tile (64-byte rows)
       wg_fence_acc(acc[0]);
       wg_fence_acc(acc[1]);
       wg_fence();
 #pragma unroll
       for (int ks = 0; ks < TC_BK / 16; ks++) {
         const uint64_t adv = (uint64_t)((ks * 32) >> 4);   // +32 bytes per 16-element k-step
+        uint64_t a_hi, a_lo;
+        if constexpr (HALO) {
+          // k16 step 2 kb + ks = (tap, channels hch .. hch + 15), no branch: a wgmma on a divergent path makes ptxas
+          // serialise them all.  With an odd number of steps per tap set (SincNet's 5 x 80 channels) the last k-block's
+          // second step reads the next tap's first 16 channels against the W columns past K, which TMA fills with zeros
+          const uint32_t aa = hs + (uint32_t)(hch >> 5) * halo_box + (uint32_t)(hch & 31) * 2 + htap;
+          a_hi = wg_desc_sw64(aa);
+          a_lo = wg_desc_sw64(aa + halo_cb * halo_box);
+          hch += 16;
+          const bool next_tap = hch == a.cin;   // a.dil rows further down
+          hch = next_tap ? 0 : hch;
+          htap += next_tap ? a.dil * 64 : 0;
+        } else {
+          a_hi = wg_desc_sw64(sa) + adv;
+          a_lo = wg_desc_sw64(sa + S::A_BYTES) + adv;
+        }
 #pragma unroll
         for (int h = 0; h < 2; h++) {
-          wgmma_ss<BN>(acc[h], a_lo + adv + h * HALF, w_hi + adv, (kb | ks) != 0);
-          wgmma_ss<BN>(acc[h], a_hi + adv + h * HALF, w_lo + adv, 1);
-          wgmma_ss<BN>(acc[h], a_hi + adv + h * HALF, w_hi + adv, 1);
+          wgmma_ss<BN>(acc[h], a_lo + h * HALF, w_hi + adv, (kb | ks) != 0);
+          wgmma_ss<BN>(acc[h], a_hi + h * HALF, w_lo + adv, 1);
+          wgmma_ss<BN>(acc[h], a_hi + h * HALF, w_hi + adv, 1);
         }
       }
       wg_commit();
@@ -630,6 +724,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     wg_fence_acc(acc[0]);
     wg_fence_acc(acc[1]);
     if (et == 0) mbar_arrive(&empty[stage == 0 ? NSTAGE - 1 : stage - 1]);
+    if (HALO && et == 0) mbar_arrive(&halo_empty[c]);
     const int mt = tile / a.n_tiles, nt = tile - mt * a.n_tiles;
     const bool stage_params = a.n_tiles > 1 || n == 0;
     if constexpr (POOLING) {
@@ -749,9 +844,28 @@ static unsigned* tile_counter(cudaStream_t st) {
 
 // operand maps, output maps (box epilogues: float32 rows, or hi and lo planes, as [M, N] of pitch ldc) and kernel arguments
 // of one launch; tiles of `bn` columns
-static int tc_setup(const TcGemm& g, int bn, int epi, CUtensorMap* maps, TcArgs& a) {
-  const int Ktot = g.KW * g.Cin, bk = TC_BK;
-  if (make_map(&maps[0], g.A_hi, g.Mtot, g.Cin, g.lda, bk, TC_BM) || make_map(&maps[1], g.A_lo, g.Mtot, g.Cin, g.lda, bk, TC_BM) ||
+// column tile width of a launch (element-wise and pooling epilogues; Conv2d picks it from Npad in launch_gemm_tc)
+static int tc_bn(const TcGemm& g) { return g.epi == TC_MAXPOOL3 || (g.Npad == 64 && g.epi == TC_BIAS_F32) ? 64 : 128; }
+// rows of a tile's halo: the 128 rows of the MMA and (KW - 1) * dil below them (KW * dil when K is an odd number of k16
+// steps: the last one reads the first rows of a tap past the last), rounded up to whole 8-row swizzle groups
+static int tc_halo_rows(const TcGemm& g) {
+  return (TC_BM + (g.KW - ((g.KW * g.Cin) % 32 ? 0 : 1)) * g.dil + 7) / 8 * 8;
+}
+template <int BN>
+static int tc_halo_smem(const TcGemm& g) { return TcSmem<BN>::total(g.epi, TcSmem<BN>::halo_op_bytes(g.Cin, tc_halo_rows(g))); }
+
+// The halo mode is taken by every Conv1d with several taps over at most 128 channels (a multiple of 16) whose halo is one
+// TMA box (at most 256 rows) and fits, with the W ring and the epilogue's buffers, in shared memory
+bool gemm_tc_halo(const TcGemm& g) {
+  if (g.tap_boxes || g.epi == TC_CONV2D || g.tap_off || g.KW < 2 || g.dil < 1 || g.Cin % 16 || g.Cin > 128 ||
+      tc_halo_rows(g) > 256)
+    return false;
+  return (tc_bn(g) == 64 ? tc_halo_smem<64>(g) : tc_halo_smem<128>(g)) <= TC_SMEM_MAX;
+}
+
+static int tc_setup(const TcGemm& g, int bn, int epi, bool halo, CUtensorMap* maps, TcArgs& a) {
+  const int Ktot = g.KW * g.Cin, bk = TC_BK, a_rows = halo ? tc_halo_rows(g) : TC_BM;
+  if (make_map(&maps[0], g.A_hi, g.Mtot, g.Cin, g.lda, bk, a_rows) || make_map(&maps[1], g.A_lo, g.Mtot, g.Cin, g.lda, bk, a_rows) ||
       make_map(&maps[2], g.W_hi, g.Npad, Ktot, Ktot, bk, bn) || make_map(&maps[3], g.W_lo, g.Npad, Ktot, Ktot, bk, bn))
     return -2;
   memset(&maps[4], 0, 2 * sizeof(CUtensorMap));
@@ -776,6 +890,16 @@ static int tc_setup(const TcGemm& g, int bn, int epi, CUtensorMap* maps, TcArgs&
   a.res_hi = reinterpret_cast<const __nv_bfloat16*>(g.res_hi);
   a.res_lo = reinterpret_cast<const __nv_bfloat16*>(g.res_lo);
   a.pool_w = g.pool_w; a.pool_part = g.pool_part; a.pool_item_rows = g.pool_item_rows; a.pool_K = g.pool_K;
+  a.cin = g.Cin;
+  if (halo) {
+    a.halo_rows = a_rows;
+    a.wblocks = (Ktot + bk - 1) / bk;     // W columns past Ktot of the last k-block are zero-filled by TMA
+    a.halo_bytes = bn == 64 ? TcSmem<64>::halo_bytes(g.Cin, a_rows) : TcSmem<128>::halo_bytes(g.Cin, a_rows);
+    a.op_bytes = bn == 64 ? TcSmem<64>::halo_op_bytes(g.Cin, a_rows) : TcSmem<128>::halo_op_bytes(g.Cin, a_rows);
+  } else {
+    a.op_bytes = bn == 128 ? TcSmem<128>::NSTAGE * TcSmem<128>::STAGE_BYTES
+                           : (bn == 64 ? TcSmem<64>::NSTAGE * TcSmem<64>::STAGE_BYTES : TcSmem<32>::NSTAGE * TcSmem<32>::STAGE_BYTES);
+  }
   return 0;
 }
 
@@ -785,27 +909,33 @@ static int tc_grid(const TcArgs& a) {
   return tiles < sms ? tiles : sms;
 }
 
-template <int BN, int EPI>
+template <int BN, int EPI, bool HALO>
 static int launch_tc(const TcGemm& g, cudaStream_t st) {
   using S = TcSmem<BN>;
   CUtensorMap m[6];
   TcArgs a;
-  if (tc_setup(g, BN, EPI, m, a)) return -2;
+  if (tc_setup(g, BN, EPI, HALO, m, a)) return -2;
   if (tc_pooling(EPI) && !(a.tile_ctr = tile_counter(st))) return -2;
-  auto kern = gemm_tc_kernel<BN, EPI>;
+  auto kern = gemm_tc_kernel<BN, EPI, HALO>;
   static bool attr_done[64] = {};
-  if (first_use_on_device(attr_done))
-    DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::total(EPI)));
-  kern<<<tc_grid(a), TC_THREADS, S::total(EPI), st>>>(m[0], m[1], m[2], m[3], m[4], m[5], a);
+  if (first_use_on_device(attr_done))   // halo mode: the size depends on the shape
+    DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, HALO ? TC_SMEM_MAX : S::total(EPI)));
+  kern<<<tc_grid(a), TC_THREADS, S::total(EPI, a.op_bytes), st>>>(m[0], m[1], m[2], m[3], m[4], m[5], a);
   DG_LAUNCHED();
   return 0;
 }
 
+template <int BN, int EPI>
+static int launch_tc(const TcGemm& g, cudaStream_t st) {
+  return gemm_tc_halo(g) ? launch_tc<BN, EPI, true>(g, st) : launch_tc<BN, EPI, false>(g, st);
+}
+
 int launch_gemm_tc(const TcGemm& g, cudaStream_t st) {
   ProfScope _ps(g.tag ? g.tag : "gemm_tc", st);
-  if (g.Cin % 64 || g.lda % 8 || g.ldc % (g.epi == TC_LEAKY_BN_SPLIT ? 8 : 4) || (g.Npad % 128 && g.Npad != 64 && g.Npad != 32) ||
-      g.KW < 1 || g.KW > 9) {
-    set_error("gemm_tc: Cin must be a multiple of 64, A pitch a multiple of 8, output pitch a multiple of 4 "
+  if (g.Cin % (gemm_tc_halo(g) ? 16 : 64) || g.lda % 8 || g.ldc % (g.epi == TC_LEAKY_BN_SPLIT ? 8 : 4) ||
+      (g.Npad % 128 && g.Npad != 64 && g.Npad != 32) || g.KW < 1 || g.KW > 9) {
+    set_error("gemm_tc: Cin must be a multiple of 64 (a Conv1d of 2..9 taps over at most 128 channels whose tile halo fits "
+              "in shared memory, e.g. Cin 80: a multiple of 16), A pitch a multiple of 8, output pitch a multiple of 4 "
               "(8 for 16-bit planes), padded N 32, 64 or a multiple of 128, at most 9 taps");
     return -1;
   }
@@ -827,9 +957,9 @@ int launch_gemm_tc(const TcGemm& g, cudaStream_t st) {
       set_error("gemm_tc (conv2d): channel counts must be multiples of 32");
       return -1;
     }
-    if (g.Npad == 32) return launch_tc<32, TC_CONV2D>(g, st);
-    if (g.Npad == 64) return launch_tc<64, TC_CONV2D>(g, st);
-    return launch_tc<128, TC_CONV2D>(g, st);
+    if (g.Npad == 32) return launch_tc<32, TC_CONV2D, false>(g, st);
+    if (g.Npad == 64) return launch_tc<64, TC_CONV2D, false>(g, st);
+    return launch_tc<128, TC_CONV2D, false>(g, st);
   }
   if (g.epi == TC_POOL) {
     if (g.Npad % 128 || !g.pool_w || !g.pool_part || g.pool_K < 1 || g.pool_K > 4 || g.pool_item_rows < TC_BM) {
@@ -855,6 +985,93 @@ int launch_gemm_tc(const TcGemm& g, cudaStream_t st) {
     default:
       return launch_tc<128, TC_LEAKY_BN_F32>(g, st);
   }
+}
+
+// ------------------------------------------------------------------------------------ descriptor row-shift probe
+// One warpgroup TMA-loads A (72 rows x 32 fp16 channels) and W (8 rows x 32) with the 64B swizzle of the GEMM's operand
+// boxes and, for every shift r = 0..8 and k16 step ks, runs one m64n8k16 product of A rows r..r+63 with W: out[r][ks][64][8].
+// base_offset_mode 1 also sets the descriptor's matrix base offset field (bits 49-51) to (start address >> 7) & 7.
+__global__ void __launch_bounds__(128) wgmma_row_shift_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                              const __grid_constant__ CUtensorMap tmW, int base_offset_mode,
+                                                              float* out) {
+  __shared__ __align__(1024) unsigned char sm[72 * 64 + 8 * 64];
+  __shared__ uint64_t bar;
+  if (threadIdx.x == 0) {
+    mbar_init(&bar, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    mbar_expect_tx(&bar, sizeof(sm));
+    tma_load_2d(sm, &tmA, 0, 0, &bar);
+    tma_load_2d(sm + 72 * 64, &tmW, 0, 0, &bar);
+  }
+  mbar_wait(&bar, 0);
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  for (int r = 0; r <= 8; r++) {
+    for (int ks = 0; ks < 2; ks++) {
+      const uint32_t sa = smem_u32(sm) + r * 64 + ks * 32;
+      uint64_t da = wg_desc_sw64(sa);
+      if (base_offset_mode) da |= (uint64_t)((sa >> 7) & 7) << 49;
+      const uint64_t dw = wg_desc_sw64(smem_u32(sm + 72 * 64) + ks * 32);
+      float d[4] = {0.f, 0.f, 0.f, 0.f};
+      wg_fence_acc(d);
+      wg_fence();
+      wgmma_ss<8>(d, da, dw, 0);
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(d);
+      for (int i = 0; i < 4; i++)
+        out[((r * 2 + ks) * 64 + 16 * w + l / 4 + 8 * ((i / 2) % 2)) * 8 + 2 * (l % 4) + i % 2] = d[i];
+    }
+  }
+}
+
+int selftest_wgmma_row_shift(int base_offset_mode, unsigned* ok_shifts) {
+  // small integers: every product and sum is exact in fp16 inputs and the float32 accumulator
+  std::vector<uint16_t> A(72 * 32), W(8 * 32);
+  std::vector<float> Af(A.size()), Wf(W.size());
+  for (size_t i = 0; i < A.size(); i++) Af[i] = (float)((int)((i * 7 + i / 32 * 3) % 9) - 4);
+  for (size_t i = 0; i < W.size(); i++) Wf[i] = (float)((int)((i * 5 + 1) % 7) - 3);
+  for (size_t i = 0; i < A.size(); i++) A[i] = host_f32_to_h16(Af[i]);
+  for (size_t i = 0; i < W.size(); i++) W[i] = host_f32_to_h16(Wf[i]);
+  void *dA = nullptr, *dW = nullptr, *dO = nullptr;
+  const size_t out_n = 9 * 2 * 64 * 8;
+  int rc = 0;
+  CUtensorMap mA, mW;
+  if (cudaMalloc(&dA, A.size() * 2) != cudaSuccess || cudaMalloc(&dW, W.size() * 2) != cudaSuccess ||
+      cudaMalloc(&dO, out_n * 4) != cudaSuccess ||
+      cudaMemcpy(dA, A.data(), A.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(dW, W.data(), W.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) {
+    set_error("selftest_wgmma_row_shift: device buffers");
+    rc = -2;
+  }
+  if (!rc && (make_map(&mA, dA, 72, 32, 32, 32, 72) || make_map(&mW, dW, 8, 32, 32, 32, 8))) rc = -2;
+  std::vector<float> out(out_n);
+  if (!rc) {
+    wgmma_row_shift_kernel<<<1, 128>>>(mA, mW, base_offset_mode, static_cast<float*>(dO));
+    if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(out.data(), dO, out_n * 4, cudaMemcpyDeviceToHost) != cudaSuccess) {
+      set_error(std::string("selftest_wgmma_row_shift: ") + cudaGetErrorString(cudaGetLastError()));
+      rc = -2;
+    }
+  }
+  cudaFree(dA);
+  cudaFree(dW);
+  cudaFree(dO);
+  if (rc) return rc;
+  *ok_shifts = 0;
+  for (int r = 0; r <= 8; r++) {
+    bool ok = true;
+    for (int ks = 0; ks < 2; ks++)
+      for (int m = 0; m < 64; m++)
+        for (int n = 0; n < 8; n++) {
+          float ref = 0.f;
+          for (int k = 0; k < 16; k++) ref += Af[(r + m) * 32 + 16 * ks + k] * Wf[n * 32 + 16 * ks + k];
+          if (out[((r * 2 + ks) * 64 + m) * 8 + n] != ref) ok = false;
+        }
+    if (ok) *ok_shifts |= 1u << r;
+  }
+  return 0;
 }
 
 // ------------------------------------------------------------------------------------ 16-bit hi/lo split

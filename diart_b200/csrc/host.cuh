@@ -155,7 +155,7 @@ int upload(DevBuf& b, const std::vector<float>& h);
 struct SincWeights {
   float wn_gamma = 1.f, wn_beta = 0.f;
   DevBuf g0, b0, bias1, g1, b1, bias2, g2, b2;
-  WeightPlanes w1, w2;                 // conv weights [64][448] (taps folded into K: 5 x 80 + pad) and [64][5*64]
+  WeightPlanes w1, w2;                 // conv weights [64][5*80] and [64][5*64] (tap-major K)
   DevBuf filt_planes;                  // sinc filter bank as fp16 planes [2][80][256] (hi, lo)
   DevBuf cf;                           // folded wav-norm affine: beta * sum_k h[f][k]
   DevBuf hsum;                         // sum_k h[f][k] (stream form of the sinc layer)

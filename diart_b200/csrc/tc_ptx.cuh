@@ -30,6 +30,16 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
+// non-blocking test of a phase (try_wait may suspend the thread for a while)
+__device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
+  uint32_t ok;
+  asm volatile(
+      "{\n.reg .pred p;\nmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
+      : "=r"(ok)
+      : "r"(smem_u32(bar)), "r"(parity)
+      : "memory");
+  return ok != 0;
+}
 // bounded wait: a protocol bug must surface as a trapped kernel, never as a hung GPU
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
@@ -119,7 +129,10 @@ __device__ __forceinline__ uint64_t wg_desc(uint32_t smem_addr) {
   d |= (uint64_t)1 << 62;                        // SWIZZLE_128B
   return d;
 }
-// K-major, 64B-swizzled operand tile: rows of 64 B (32 16-bit k-values), 8-row groups 512 B apart
+// K-major, 64B-swizzled operand tile: rows of 64 B (32 16-bit k-values), 8-row groups 512 B apart.  The start address may be
+// any whole number of rows into a TMA-written tile, also off the 512 B pattern boundary, with the matrix base offset field
+// (bits 49-51) left 0: the swizzle follows the absolute shared-memory address.  Measured on an H100 by
+// dg_selftest_wgmma_row_shift: shifts 0..8 exact with 0, shifts 2..7 wrong with the base offset set to (address >> 7) & 7.
 __device__ __forceinline__ uint64_t wg_desc_sw64(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);   // start address
