@@ -119,6 +119,11 @@ SIGNATURES = {
     "dg_multi_last_step_ms": (C.c_int, [_P, C.POINTER(C.c_float)]),
     "dg_multi_destroy": (C.c_int, [_P]),
     "dg_selftest_multi_staging_host": (C.c_int, [C.c_int, C.c_int, C.c_int, _P, _P, _P, _P]),
+    "dg_multi_add_rate": (C.c_int, [_P, _P, C.c_int, C.c_int, C.POINTER(C.c_int)]),
+    "dg_multi_open_rate": (C.c_int, [_P, C.c_int, C.c_int]),
+    "dg_multi_last_windows": (C.c_int, [_P, _P, C.c_int]),
+    "dg_selftest_multi_frames_host": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, C.c_int,
+                                                C.POINTER(C.c_int)]),
 }
 
 

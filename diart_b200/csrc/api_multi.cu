@@ -12,31 +12,105 @@
 
 #include "host.cuh"
 
-// The host bookkeeping of the streams' audio, no device work: per slot the open flag and the absolute sample counters pushed
-// (staged included) / start of the next window; the samples pushed since the last tick are [0, n_staged) of a staging buffer,
-// described by `pieces` in push order.  A piece is a run of ONE slot's samples that is contiguous both in the staging buffer
-// and in that slot's stream, so a piece is extended only by a push that continues it in both.
+// The windows of a source rate: S and hop source samples per window / between windows, ring capacity `cap` (what a stream may
+// hold unconsumed).  A declared rate (g.o > 0) resamples each window to the pipeline's chunk (taps of rs): g is its geometry, a hop is
+// fs whole 16 kHz frames, frames r_lo .. r_hi of a window have all their taps inside it, and the slot's 16 kHz ring holds Q
+// frames -- the interior frames of max_wps consecutive windows.
+struct RateGeom {
+  int S = 0, hop = 1, cap = 0;
+  const dg_resample* rs = nullptr;
+  RsGeom g{};
+  long long fs = 0, r_lo = 0, r_hi = -1, Q = 0;
+  bool resampled() const { return g.o > 0; }
+};
+
+static long long ring_capacity(long long S, long long hop, int max_wps) { return (S + 2LL * max_wps * hop + 1023) / 1024 * 1024; }
+
+// the geometry of a source rate resampled by g to windows of out_S samples, or DG_EINVAL naming what rules it out
+static int rate_geom(const RsGeom& g, int S, int hop, int out_S, int max_wps, RateGeom& r, const char* who) {
+  if (S < 1 || hop < 1 || hop > S) {
+    set_error(std::string(who) + ": chunk and step must be positive, step <= chunk");
+    return DG_EINVAL;
+  }
+  if (resample_out_len(g, S) != out_S) {
+    set_error(std::string(who) + ": a chunk of " + std::to_string(S) + " source samples resamples to " +
+              std::to_string(resample_out_len(g, S)) + " samples, not the pipeline's " + std::to_string(out_S));
+    return DG_EINVAL;
+  }
+  if (hop % g.o) {
+    set_error(std::string(who) + ": a step of " + std::to_string(hop) + " source samples is not a whole number of frames (" +
+              std::to_string(g.o) + " samples each)");
+    return DG_EINVAL;
+  }
+  r = RateGeom{};
+  r.S = S;
+  r.hop = hop;
+  r.g = g;
+  r.fs = hop / g.o;
+  r.r_lo = (g.w + g.o - 1) / g.o;
+  r.r_hi = S - g.w - g.o >= 0 ? (S - g.w - g.o) / g.o : -1;
+  r.Q = (max_wps - 1) * r.fs + std::max(0LL, r.r_hi - r.r_lo + 1);
+  const long long cap = ring_capacity(S, hop, max_wps);
+  if (cap > (1 << 30) || r.Q * g.n > (1 << 30)) {
+    set_error(std::string(who) + ": the rings of this rate exceed 2^30 samples per stream");
+    return DG_EINVAL;
+  }
+  r.cap = (int)cap;
+  return DG_OK;
+}
+
+// What a tick does besides the networks: its slots and rows (all B rows, and the rows at the pipeline's rate with their window
+// starts), and per declared rate the resampling items and the resampled rows, grouped by rate (entries [off[i], off[i + 1])
+// belong to rate 1 + i); done[a]: frames of act[a]'s stream computed once the tick has run.
+struct TickPlan {
+  std::vector<TickSlot> act;
+  int B = 0;
+  std::vector<int2> rows, rows16;
+  std::vector<long long> start, start16;
+  std::vector<RsFrames> items;
+  std::vector<RsRow> rs_rows;
+  std::vector<int> item_off, row_off;
+  std::vector<long long> done;
+};
+
+// The host bookkeeping of the streams' audio, no device work: per slot the open flag, its rate and the absolute sample counters
+// pushed (staged included) / start of the next window, and for a resampled stream the 16 kHz frames computed so far; the
+// samples pushed since the last tick are [0, n_staged) of a staging buffer, described by `pieces` in push order.  A piece is a
+// run of ONE slot's samples that is contiguous both in the staging buffer and in that slot's stream, so a piece is extended
+// only by a push that continues it in both.  Every slot's ring has stride C (the largest capacity of any rate).
 struct SlotBook {
-  int C = 0;                                  // ring capacity per slot
+  int C = 0;
+  std::vector<RateGeom> rates;                // [0]: the pipeline's rate; [1 + id]: declared rate id
   std::vector<char> open;
-  std::vector<long long> wpos, rpos;
+  std::vector<int> rate;
+  std::vector<long long> wpos, rpos, done;
   std::vector<RingPiece> pieces;
   long long n_staged = 0;
 
-  void init(int slots, int capacity) {
-    C = capacity;
+  void init(int slots, const RateGeom& base) {
+    rates.assign(1, base);
+    C = base.cap;
     open.assign(slots, 0);
+    rate.assign(slots, 0);
     wpos.assign(slots, 0);
     rpos.assign(slots, 0);
+    done.assign(slots, 0);
+  }
+  void add_rate(const RateGeom& r) {
+    rates.push_back(r);
+    C = std::max(C, r.cap);
   }
   bool ok(int slot) const { return slot >= 0 && slot < (int)open.size() && open[slot]; }
-  long long available(int s, int S, int hop) const {    // complete windows, pushed and not consumed
+  const RateGeom& geom(int s) const { return rates[rate[s]]; }
+  long long available(int s) const {    // complete windows, pushed and not consumed
+    const RateGeom& r = geom(s);
     const long long have = wpos[s] - rpos[s];
-    return have < S ? 0 : (have - S) / hop + 1;
+    return have < r.S ? 0 : (have - r.S) / r.hop + 1;
   }
-  void start(int slot) {
+  void start(int slot, int r = 0) {
     open[slot] = 1;
-    wpos[slot] = rpos[slot] = 0;
+    rate[slot] = r;
+    wpos[slot] = rpos[slot] = done[slot] = 0;
   }
   // the stream ends: its staged samples are dropped (they stay in the staging buffer, no piece refers to them)
   void stop(int slot) {
@@ -44,7 +118,7 @@ struct SlotBook {
     pieces.erase(std::remove_if(pieces.begin(), pieces.end(), [&](const RingPiece& p) { return p.slot == slot; }),
                  pieces.end());
   }
-  bool fits(int slot, int n) const { return wpos[slot] + n - rpos[slot] <= C; }
+  bool fits(int slot, int n) const { return wpos[slot] + n - rpos[slot] <= geom(slot).cap; }
   // books n > 0 samples of `slot` at staging offset n_staged (the caller copies them there)
   void push(int slot, int n) {
     RingPiece* last = pieces.empty() ? nullptr : &pieces.back();
@@ -59,6 +133,59 @@ struct SlotBook {
     pieces.clear();
     n_staged = 0;
   }
+  // the tick's plan: every open slot with windows gives up to max_wps, in slot order.  A resampled stream's item is the frames
+  // its windows' interiors need that no earlier tick computed: [max(done, first start / o + r_lo), last start / o + r_hi]
+  void plan(int max_wps, TickPlan& t) const {
+    t = TickPlan{};
+    const int nr = (int)rates.size();
+    std::vector<std::vector<RsFrames>> items(nr);
+    std::vector<std::vector<RsRow>> rs_rows(nr);
+    for (int s = 0; s < (int)open.size(); s++) {
+      const int n = open[s] ? (int)std::min<long long>(available(s), max_wps) : 0;
+      if (!n) continue;
+      const RateGeom& r = geom(s);
+      t.act.push_back(TickSlot{s, t.B, n, 0, 0, {0, 0, 0}});
+      long long d = done[s];
+      for (int i = 0; i < n; i++) {
+        const long long st = rpos[s] + (long long)i * r.hop;
+        t.rows.push_back(make_int2((int)t.act.size() - 1, i));
+        t.start.push_back(st);
+        if (r.resampled())
+          rs_rows[rate[s]].push_back(RsRow{st, st / r.g.o, s, t.B + i});
+      }
+      if (r.resampled()) {
+        const long long lo = std::max(d, rpos[s] / r.g.o + r.r_lo);
+        const long long hi = (rpos[s] + (long long)(n - 1) * r.hop) / r.g.o + r.r_hi;
+        if (hi >= lo) {
+          items[rate[s]].push_back(RsFrames{lo, s, (int)(hi - lo + 1)});
+          d = hi + 1;
+        }
+      }
+      t.done.push_back(d);
+      t.B += n;
+    }
+    for (int b = 0; b < t.B; b++)
+      if (!geom(t.act[t.rows[b].x].slot).resampled()) {
+        t.rows16.push_back(t.rows[b]);
+        t.start16.push_back(t.start[b]);
+      }
+    t.item_off.assign(1, 0);
+    t.row_off.assign(1, 0);
+    for (int i = 1; i < nr; i++) {
+      t.items.insert(t.items.end(), items[i].begin(), items[i].end());
+      t.rs_rows.insert(t.rs_rows.end(), rs_rows[i].begin(), rs_rows[i].end());
+      t.item_off.push_back((int)t.items.size());
+      t.row_off.push_back((int)t.rs_rows.size());
+    }
+  }
+  // the tick of plan t has run: its windows are consumed and its frames computed
+  void consumed(const TickPlan& t) {
+    for (size_t a = 0; a < t.act.size(); a++) {
+      const int s = t.act[a].slot;
+      rpos[s] += (long long)t.act[a].n * geom(s).hop;
+      done[s] = t.done[a];
+    }
+  }
 };
 
 struct dg_multi {
@@ -70,6 +197,10 @@ struct dg_multi {
   SlotBook book;
   PinnedBuf stage;                            // staged samples [0, book.n_staged), then a tick's tables
   std::vector<int> n_hist, cur;               // per slot: post-path history entries, current copy
+  DevBuf yrings;                              // resampled streams: 16 kHz rings [slots][Y]
+  long long Y = 0;
+  bool opened = false;                        // a stream was opened (rates can no longer be added)
+  int last_B = 0;                             // windows of the last tick that had any
   DevBuf rings, hamming, in, wav, seg, emb, maps, centers, active, init, prep, prep_d, hist_seg, hist_map, header, turns, total;
   PinnedBuf pin_out;                          // header, turn count and turn prefix of a tick (TurnOut layout at 0)
   Stream st;
@@ -116,7 +247,11 @@ extern "C" int dg_multi_create(dg_seg* seg, dg_emb* emb, int chunk_samples, int 
   h->device = seg->device; h->slots = max_streams; h->max_wps = max_windows_per_stream;
   h->S = chunk_samples; h->hop = step_samples;
   // room for the windows of a tick and as much audio again pushed ahead (as dg_stream)
-  h->book.init(max_streams, (int)(((long long)chunk_samples + 2LL * max_windows_per_stream * step_samples + 1023) / 1024 * 1024));
+  RateGeom base;
+  base.S = chunk_samples;
+  base.hop = step_samples;
+  base.cap = (int)ring_capacity(chunk_samples, step_samples, max_windows_per_stream);
+  h->book.init(max_streams, base);
   h->F = F; h->K = K; h->D = D; h->M = max_speakers; h->nw = num_windows;
   h->tau = tau; h->rho = rho; h->delta = delta;
   h->net.seg = seg; h->net.emb = emb;
@@ -140,10 +275,49 @@ extern "C" int dg_multi_destroy(dg_multi* h) {
   return DG_OK;
 }
 
-// a new stream in `slot`: empty ring, fresh clustering state (the reference's SpeakerDiarization.reset()), no history
-extern "C" int dg_multi_open(dg_multi* h, int slot) {
+// a source rate whose windows `rs` resamples to the pipeline's chunk; before any stream is opened (the rings grow)
+extern "C" int dg_multi_add_rate(dg_multi* h, dg_resample* rs, int chunk_samples, int step_samples, int* rate_id) {
+  const char* who = "dg_multi_add_rate";
+  if (!h || !rs || !rate_id) {
+    set_error(std::string(who) + ": null handle");
+    return DG_EINVAL;
+  }
+  if (h->opened) {
+    set_error(std::string(who) + ": rates are added before any stream is opened");
+    return DG_EINVAL;
+  }
+  if (rs->device != h->device) {
+    set_error(std::string(who) + ": the resampler lives on another device");
+    return DG_EINVAL;
+  }
+  for (size_t i = 1; i < h->book.rates.size(); i++)
+    if (h->book.rates[i].g.o == rs->g.o && h->book.rates[i].g.n == rs->g.n) {
+      set_error(std::string(who) + ": this rate was added before (rate id " + std::to_string(i - 1) + ")");
+      return DG_EINVAL;
+    }
+  RateGeom r;
+  int rc;
+  if ((rc = rate_geom(rs->g, chunk_samples, step_samples, h->S, h->max_wps, r, who))) return rc;
+  r.rs = rs;
+  DG_CUDA(cudaSetDevice(h->device));
+  const int C = std::max(h->book.C, r.cap);
+  const long long Y = std::max(h->Y, r.Q * r.g.n);
+  if (h->rings.ensure((size_t)h->slots * C * 4) || h->yrings.ensure((size_t)h->slots * Y * 4)) return DG_ECUDA;
+  h->book.add_rate(r);
+  h->Y = Y;
+  *rate_id = (int)h->book.rates.size() - 2;
+  return DG_OK;
+}
+
+// a new stream in `slot` at declared rate `rate_id` (-1: the pipeline's rate): empty rings, fresh clustering state (the
+// reference's SpeakerDiarization.reset()), no history
+extern "C" int dg_multi_open_rate(dg_multi* h, int slot, int rate_id) {
   if (!h || slot < 0 || slot >= h->slots || h->book.open[slot]) {
     set_error("dg_multi_open: slot " + std::to_string(slot) + " is out of range or already open");
+    return DG_EINVAL;
+  }
+  if (rate_id < -1 || rate_id + 1 >= (int)h->book.rates.size()) {
+    set_error("dg_multi_open: rate " + std::to_string(rate_id) + " was not declared");
     return DG_EINVAL;
   }
   DG_CUDA(cudaSetDevice(h->device));
@@ -151,10 +325,13 @@ extern "C" int dg_multi_open(dg_multi* h, int slot) {
   DG_CUDA(cudaMemsetAsync(h->centers.as<double>() + s * h->M * h->D, 0, (size_t)h->M * h->D * 8, h->st));
   DG_CUDA(cudaMemsetAsync(h->active.as<int>() + s * 32, 0, 32 * 4, h->st));
   DG_CUDA(cudaMemsetAsync(h->init.as<int>() + s * 2, 0, 2 * 4, h->st));
-  h->book.start(slot);
+  h->book.start(slot, rate_id + 1);
   h->n_hist[slot] = 0;
+  h->opened = true;
   return DG_OK;
 }
+
+extern "C" int dg_multi_open(dg_multi* h, int slot) { return dg_multi_open_rate(h, slot, -1); }
 
 // the stream in `slot` ends: its staged samples are dropped, the slot can be opened again
 extern "C" int dg_multi_close(dg_multi* h, int slot) {
@@ -171,7 +348,7 @@ extern "C" int dg_multi_available(const dg_multi* h, int slot) {
     set_error("dg_multi_available: slot " + std::to_string(slot) + " is not open");
     return DG_EINVAL;
   }
-  return (int)h->book.available(slot, h->S, h->hop);
+  return (int)h->book.available(slot);
 }
 
 // appends n samples to the stream in `slot`: copied into the pinned staging, uploaded at the next dg_multi_step
@@ -183,8 +360,7 @@ extern "C" int dg_multi_push_host(dg_multi* h, int slot, const float* samples, i
   if (!h->book.fits(slot, n)) {
     set_error("dg_multi_push_host: ring of slot " + std::to_string(slot) + " full (" +
               std::to_string(h->book.wpos[slot] - h->book.rpos[slot]) + " samples buffered, capacity " +
-              std::to_string(h->book.C) +
-              "): step first");
+              std::to_string(h->book.geom(slot).cap) + "): step first");
     return DG_EINVAL;
   }
   if (n == 0) return DG_OK;
@@ -212,15 +388,15 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
     return DG_EINVAL;
   }
   // this tick's slots and rows: every open slot with windows gives up to max_wps, in slot order
-  std::vector<TickSlot> act;
-  int B = 0;
-  for (int s = 0; s < h->slots; s++) {
-    const int n = h->book.open[s] ? (int)std::min<long long>(h->book.available(s, h->S, h->hop), h->max_wps) : 0;
-    counts_host[s] = n;
-    if (n) {
-      act.push_back(TickSlot{s, B, n, h->cur[s], h->n_hist[s], {0, 0, 0}});
-      B += n;
-    }
+  TickPlan tp;
+  h->book.plan(h->max_wps, tp);
+  std::vector<TickSlot>& act = tp.act;
+  const int B = tp.B;
+  for (int s = 0; s < h->slots; s++) counts_host[s] = 0;
+  for (TickSlot& ts : act) {
+    counts_host[ts.slot] = ts.n;
+    ts.cur = h->cur[ts.slot];
+    ts.n_hist = h->n_hist[ts.slot];
   }
   if (n_rows != B) {
     set_error(std::string(who) + ": " + std::to_string(n_rows) + " plan rows given, the tick has " + std::to_string(B) +
@@ -251,7 +427,13 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
   const size_t o_rows = o_act + align16((size_t)n_act * sizeof(TickSlot)), o_start = o_rows + align16((size_t)B * 8);
   const size_t o_plan = o_start + align16((size_t)B * 8), o_states = o_plan + align16((size_t)B * stride * 4);
   const size_t o_off = o_states + align16((size_t)n_act * 8), o_trials = o_off + align16((size_t)(h->slots + 1) * 4);
-  const size_t in_b = o_trials + 24;
+  // a tick with resampled rows also carries the rows at the pipeline's rate [n16] with their starts, the resampling items and
+  // the resampled rows
+  const bool mixed = !tp.rs_rows.empty();
+  const int n16 = (int)tp.rows16.size(), n_items = (int)tp.items.size(), n_rs = (int)tp.rs_rows.size();
+  const size_t o_rows16 = o_trials + 32, o_start16 = o_rows16 + align16((size_t)n16 * 8);
+  const size_t o_items = o_start16 + align16((size_t)n16 * 8), o_rs = o_items + align16((size_t)n_items * sizeof(RsFrames));
+  const size_t in_b = mixed ? o_rs + (size_t)n_rs * sizeof(RsRow) : o_trials + 24;
   const TurnOut lay = {0, (size_t)B * 16};
   const int turn_cap = B * M * ((F + 2) / 2);   // every second output frame of every speaker starts a turn
   if (h->in.ensure(in_b) || h->wav.ensure((size_t)B * S * 4) || h->seg.ensure((size_t)B * F * K * 4) ||
@@ -268,18 +450,20 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
   unsigned char* pin = h->stage.as<unsigned char>();
   if (np) memcpy(pin + o_pieces, h->book.pieces.data(), (size_t)np * sizeof(RingPiece));
   memcpy(pin + o_act, act.data(), (size_t)n_act * sizeof(TickSlot));
-  int2* rows = reinterpret_cast<int2*>(pin + o_rows);
-  long long* start = reinterpret_cast<long long*>(pin + o_start);
+  memcpy(pin + o_rows, tp.rows.data(), (size_t)B * 8);
+  memcpy(pin + o_start, tp.start.data(), (size_t)B * 8);
   int2* states = reinterpret_cast<int2*>(pin + o_states);
   int32_t* off = reinterpret_cast<int32_t*>(pin + o_off);
   for (int a = 0, s = 0; a < n_act; a++) {
     const TickSlot& ts = act[a];
     for (; s <= ts.slot; s++) off[s] = ts.row0;
-    for (int i = 0; i < ts.n; i++) {
-      rows[ts.row0 + i] = make_int2(a, i);
-      start[ts.row0 + i] = h->book.rpos[ts.slot] + (long long)i * h->hop;
-    }
     states[a] = make_int2(ts.slot, 0);
+  }
+  if (mixed) {
+    if (n16) memcpy(pin + o_rows16, tp.rows16.data(), (size_t)n16 * 8);
+    if (n16) memcpy(pin + o_start16, tp.start16.data(), (size_t)n16 * 8);
+    if (n_items) memcpy(pin + o_items, tp.items.data(), (size_t)n_items * sizeof(RsFrames));
+    memcpy(pin + o_rs, tp.rs_rows.data(), (size_t)n_rs * sizeof(RsRow));
   }
   for (int s = act.back().slot + 1; s <= h->slots; s++) off[s] = B;
   memcpy(pin + o_plan, plan_host, (size_t)B * stride * 4);
@@ -293,10 +477,31 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
   int rc;
   // audio in: the staged samples to their rings, then the batch [B, S], windows grouped by slot
   if ((rc = launch_ring_scatter(reinterpret_cast<const float*>(din), reinterpret_cast<const RingPiece*>(din + o_pieces), np,
-                                h->book.C, h->rings.as<float>(), st)) ||
-      (rc = launch_ring_gather(h->rings.as<float>(), h->book.C, d_act, d_rows, reinterpret_cast<const long long*>(din + o_start), S,
-                               B, h->wav.as<float>(), st)))
+                                h->book.C, h->rings.as<float>(), st)))
     return rc;
+  if (!mixed) {
+    if ((rc = launch_ring_gather(h->rings.as<float>(), h->book.C, d_act, d_rows, reinterpret_cast<const long long*>(din + o_start),
+                                 S, B, h->wav.as<float>(), st)))
+      return rc;
+  } else {
+    if (n16 && (rc = launch_ring_gather(h->rings.as<float>(), h->book.C, d_act, reinterpret_cast<const int2*>(din + o_rows16),
+                                        reinterpret_cast<const long long*>(din + o_start16), S, n16, h->wav.as<float>(), st)))
+      return rc;
+    // per declared rate: the new 16 kHz frames of its streams, then its windows
+    for (size_t i = 1; i < h->book.rates.size(); i++) {
+      const RateGeom& r = h->book.rates[i];
+      const int i0 = tp.item_off[i - 1], i1 = tp.item_off[i], w0 = tp.row_off[i - 1], w1 = tp.row_off[i];
+      long long max_count = 0;
+      for (int k = i0; k < i1; k++) max_count = std::max<long long>(max_count, tp.items[k].count);
+      const float* W = r.rs->taps.as<float>();
+      if ((rc = launch_resample_frames(h->rings.as<float>(), h->book.C, reinterpret_cast<const RsFrames*>(din + o_items) + i0,
+                                       i1 - i0, max_count, W, r.g, h->yrings.as<float>(), h->Y, r.Q, st)) ||
+          (rc = launch_resample_gather(h->rings.as<float>(), h->book.C, h->yrings.as<float>(), h->Y, r.Q,
+                                       reinterpret_cast<const RsRow*>(din + o_rs) + w0, w1 - w0, r.r_lo, r.r_hi, W, r.g, r.S, S,
+                                       h->wav.as<float>(), st)))
+        return rc;
+    }
+  }
   DG_CUDA(cudaEventRecord(h->e_start, st));
   // networks: sub-batches of at most 256 windows on alternating scratch lanes (the workspace of a 256-window step); a lane is
   // reused once the sub-batch before on it is past its embeddings
@@ -340,10 +545,11 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
   DG_CUDA(cudaEventRecord(h->t_end, st));
   DG_CUDA(cudaStreamSynchronize(st));
   h->timed = true;
-  // the tick is on the device: staged samples are in the rings, windows consumed, histories moved on
+  h->last_B = B;
+  // the tick is on the device: staged samples are in the rings, windows consumed, frames computed, histories moved on
   h->book.uploaded();
+  h->book.consumed(tp);
   for (const TickSlot& ts : act) {
-    h->book.rpos[ts.slot] += (long long)ts.n * h->hop;
     if (h->nw > 1) {
       h->n_hist[ts.slot] = std::min(h->nw - 1, ts.n_hist + ts.n);
       h->cur[ts.slot] ^= 1;
@@ -361,6 +567,88 @@ extern "C" int dg_multi_last_step_ms(const dg_multi* h, float* ms) {
   return DG_OK;
 }
 
+// the last tick's window batch [n_rows, chunk] (what the networks read) to wav_dev; synchronous
+extern "C" int dg_multi_last_windows(const dg_multi* h, float* wav_dev, int n_rows) {
+  if (!h || !wav_dev || !h->timed || n_rows != h->last_B) {
+    set_error("dg_multi_last_windows: n_rows must be the window count of the last tick that had windows");
+    return DG_EINVAL;
+  }
+  DG_CUDA(cudaSetDevice(h->device));
+  DG_CUDA(cudaMemcpyAsync(wav_dev, h->wav.p, (size_t)n_rows * h->S * 4, cudaMemcpyDeviceToDevice, h->st));
+  DG_CUDA(cudaStreamSynchronize(h->st));
+  return DG_OK;
+}
+
+// dg_multi's tick planning on its own (test hook, no GPU): a SlotBook whose pipeline windows are out_chunk / out_step samples,
+// with the declared rates [n_rates][5] = {o, n, w, chunk, step}, driven by ops [n_ops][3] = {kind, slot, n}.
+extern "C" int dg_selftest_multi_frames_host(int slots, int max_wps, int out_chunk, int out_step, int n_rates, const int32_t* rates,
+                                             int n_ops, const int32_t* ops, int32_t* result, int64_t* records, int cap,
+                                             int* n_records) {
+  const char* who = "dg_selftest_multi_frames_host";
+  if (slots < 1 || max_wps < 1 || out_chunk < 1 || out_step < 1 || n_rates < 0 || (n_rates && !rates) || n_ops < 0 ||
+      (n_ops && (!ops || !result)) || cap < 0 || (cap && !records) || !n_records) {
+    set_error(std::string(who) + ": bad arguments");
+    return DG_EINVAL;
+  }
+  SlotBook book;
+  RateGeom base;
+  base.S = out_chunk;
+  base.hop = out_step;
+  base.cap = (int)ring_capacity(out_chunk, out_step, max_wps);
+  book.init(slots, base);
+  for (int i = 0; i < n_rates; i++) {
+    const int32_t* q = rates + 5 * i;
+    RsGeom g{q[0], q[1], q[2], 2 * q[2] + q[0]};
+    RateGeom r;
+    if (g.o < 1 || g.n < 1 || g.w < 0) {
+      set_error(std::string(who) + ": bad rate geometry");
+      return DG_EINVAL;
+    }
+    int rc;
+    if ((rc = rate_geom(g, q[3], q[4], out_chunk, max_wps, r, who))) return rc;
+    book.add_rate(r);
+  }
+  *n_records = 0;
+  int tick = 0;
+  TickPlan tp;
+  auto record = [&](long long kind, long long slot, long long a, long long b) {
+    if (*n_records < cap) {
+      int64_t* r = records + 5 * (size_t)*n_records;
+      r[0] = tick; r[1] = kind; r[2] = slot; r[3] = a; r[4] = b;
+    }
+    ++*n_records;
+  };
+  for (int i = 0; i < n_ops; i++) {
+    const int kind = ops[3 * i], slot = ops[3 * i + 1], n = ops[3 * i + 2];
+    int rc = DG_OK;
+    if (kind == 0) {
+      if (slot < 0 || slot >= slots || book.open[slot] || n < -1 || n + 1 >= (int)book.rates.size()) rc = DG_EINVAL;
+      else book.start(slot, n + 1);
+    } else if (kind == 1) {
+      if (!book.ok(slot)) rc = DG_EINVAL;
+      else book.stop(slot);
+    } else if (kind == 2) {
+      if (!book.ok(slot) || n < 0 || !book.fits(slot, n)) rc = DG_EINVAL;
+      else if (n > 0) book.push(slot, n);
+    } else if (kind == 4) {
+      book.plan(max_wps, tp);
+      for (const RsFrames& it : tp.items) record(0, it.slot, it.first, it.count);
+      for (int b = 0; b < tp.B; b++) record(1, tp.act[tp.rows[b].x].slot, tp.start[b], b);
+      book.uploaded();
+      book.consumed(tp);
+      tick++;
+    } else {
+      rc = DG_EINVAL;
+    }
+    result[i] = rc;
+  }
+  if (*n_records > cap) {
+    set_error(std::string(who) + ": " + std::to_string(*n_records) + " records, room for " + std::to_string(cap));
+    return DG_EINVAL;
+  }
+  return DG_OK;
+}
+
 // The host half of dg_multi's audio path on its own (test hook, no GPU): a SlotBook over `slots` rings of C samples driven by
 // ops [n_ops][3] = {kind, slot, n}, with ring_scatter's writes done on the host.
 extern "C" int dg_selftest_multi_staging_host(int slots, int C, int n_ops, const int32_t* ops, const float* samples_host,
@@ -370,7 +658,9 @@ extern "C" int dg_selftest_multi_staging_host(int slots, int C, int n_ops, const
     return DG_EINVAL;
   }
   SlotBook book;
-  book.init(slots, C);
+  RateGeom base;
+  base.cap = C;
+  book.init(slots, base);
   std::vector<float> staged;
   long long next = 0;                         // samples of samples_host used so far
   for (int i = 0; i < n_ops; i++) {

@@ -12,12 +12,6 @@
 // torchaudio's T.Resample(orig, new) with its defaults (sinc_interp_hann, lowpass_filter_width 6, rolloff 0.99) -- what the
 // reference's blocks.Resample applies to every window of a source at another rate (reference blocks/utils.py:62-89).  The taps
 // come from the host (diart_b200.operators.sinc_resample_kernel), bit-identical to torchaudio's.
-struct dg_resample {
-  int device = 0;
-  RsGeom g{};
-  DevBuf taps;   // [n][T]
-};
-
 extern "C" int dg_resample_create(int orig, int new_rate, const float* kernel_host, int width, int device, dg_resample** out) {
   if (!out || !kernel_host || orig < 1 || new_rate < 1 || orig == new_rate) {
     set_error("dg_resample_create: rates must be positive and different, taps non-null");

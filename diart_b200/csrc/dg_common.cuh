@@ -285,7 +285,8 @@ struct TickSlot {
   int slot, row0, n, cur, n_hist, pad[3];
 };
 int launch_ring_scatter(const float* staged, const RingPiece* pieces, int n_pieces, int C, float* rings, cudaStream_t st);
-// rows [B] = {entry of act, window index within that slot's rows}; window b = samples [start[b], start[b] + S) of its ring
+// rows [B] = {entry of act, window index i within that slot's rows}; entry b = samples [start[b], start[b] + S) of its slot's
+// ring, written to batch row act[rows[b].x].row0 + i (any subset of a tick's rows can be gathered)
 int launch_ring_gather(const float* rings, int C, const TickSlot* act, const int2* rows, const long long* start, int S, int B,
                        float* wav, cudaStream_t st);
 int launch_post_slots(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map,
@@ -342,6 +343,25 @@ int launch_resample(const RsJob& j, int items, long long max_out, cudaStream_t s
 // ((B-1) hop / o + ceil(out_len / n)) n floats; out [B][out_len]
 int launch_resample_stream(const float* ring, long long C, long long rpos, long long hop, long long L, int B, const float* W,
                            const RsGeom& g, float* ys, float* out, cudaStream_t st);
+// dg_multi's resampled streams.  A stream at a source rate keeps its source samples in a ring of stride C (sample t at t mod C)
+// and its 16 kHz frames in a ring of Q frames (frame R at outputs [(R mod Q) n, (R mod Q) n + n), stride Y floats per slot).
+// RsFrames: stream frames [first, first + count) of `slot`, all of whose taps are pushed samples; RsRow: the window of L source
+// samples that starts at absolute sample `start` (= frame0 o) of `slot`, to batch row `row`.
+struct RsFrames {
+  long long first;
+  int slot, count;
+};
+struct RsRow {
+  long long start, frame0;
+  int slot, row;
+};
+// the frames of every item (one launch; none with more than max_count frames)
+int launch_resample_frames(const float* rings, long long C, const RsFrames* items, int n_items, long long max_count,
+                           const float* W, const RsGeom& g, float* yrings, long long Y, long long Q, cudaStream_t st);
+// the windows `rows` [n_rows] into wav [row][out_len]: interior frames r_lo .. r_hi from the 16 kHz rings, edge frames recomputed
+int launch_resample_gather(const float* rings, long long C, const float* yrings, long long Y, long long Q, const RsRow* rows,
+                           int n_rows, long long r_lo, long long r_hi, const float* W, const RsGeom& g, long long L,
+                           long long out_len, float* wav, cudaStream_t st);
 
 void fbank_frame_operator(std::vector<float>& op /*[514][400]*/);
 void fbank_mel_banks(std::vector<float>& banks /*[80][257]*/, std::vector<int>& k_lo, std::vector<int>& k_hi);

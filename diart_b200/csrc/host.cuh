@@ -283,6 +283,13 @@ struct dg_cluster {
   DevBuf base, base_active, relabel;   // shared-identity mode: table at the last merge, relabel of created centres
 };
 
+// ================================================================================== resampling (api_stream.cu)
+struct dg_resample {
+  int device = 0;
+  RsGeom g{};
+  DevBuf taps;   // [n][T]
+};
+
 // ======================================================================== device-side audio stream (api_stream.cu)
 // rearrange_audio_stream (reference src/diart/operators.py:44-100) on the device: the host pushes each sample ONCE
 // (8 000 new samples per chunk instead of the 80 000 of a stacked window: 8.2 MB instead of 82 MB per 256-chunk step),

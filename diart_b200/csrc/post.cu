@@ -271,15 +271,17 @@ __global__ void __launch_bounds__(256) ring_scatter_kernel(const float* __restri
   }
 }
 
-// window b of the batch = samples [start[b], start[b] + S) of the ring of slot act[rows[b].x].slot (C, start, S multiples of
-// 4: 16-byte accesses never straddle the wrap)
+// entry b of rows = samples [start[b], start[b] + S) of the ring of slot act[rows[b].x].slot, to batch row act[..].row0 +
+// rows[b].y (C, start, S multiples of 4: 16-byte accesses never straddle the wrap)
 __global__ void __launch_bounds__(256) ring_gather_kernel(const float* __restrict__ rings, int C, const TickSlot* __restrict__ act,
                                                           const int2* __restrict__ rows, const long long* __restrict__ start,
                                                           int S, float* __restrict__ wav) {
   const int b = blockIdx.y;
-  const float* ring = rings + (size_t)act[rows[b].x].slot * C;
+  const int2 r = rows[b];
+  const TickSlot& ts = act[r.x];
+  const float* ring = rings + (size_t)ts.slot * C;
   const long long base = start[b];
-  float4* dst = reinterpret_cast<float4*>(wav + (size_t)b * S);
+  float4* dst = reinterpret_cast<float4*>(wav + (size_t)(ts.row0 + r.y) * S);
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < (S >> 2); i += gridDim.x * blockDim.x) {
     const int idx = (int)((base + 4LL * i) % C);
     dst[i] = *reinterpret_cast<const float4*>(ring + idx);

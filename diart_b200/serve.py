@@ -9,10 +9,16 @@ one post-path launch with an aggregation history per stream.  A stream's scores 
 ``SpeakerDiarization`` computes on its windows one at a time, and so are the post-path's arithmetic and plan.  Its
 embeddings can differ in the last bits (the fused TDNN5 pooling groups its partial sums by a window's row in the batch), so
 a clustering decision that lies exactly at a threshold could go the other way; apart from that the speaker maps and turns
-are the dedicated pipeline's.  Only the turns come back (the reference's serve hook writes RTTM, no audio)."""
+are the dedicated pipeline's.  Only the turns come back (the reference's serve hook writes RTTM, no audio).
+
+Streams at other source rates (``source_sample_rates``; ``open(sample_rate=44100)``) are windowed at their own rate, as
+``rearrange_audio_stream(duration, step, rate)`` windows them, and every window is resampled on the device with the bits of
+``DeviceResample`` on that window (the reference's ``blocks.Resample``): each 16 kHz frame inside the windows is computed once
+per stream, only the frames at each window's edges once per window."""
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import Dict, List, Optional, Tuple
 
 import numpy as np
@@ -23,44 +29,75 @@ from . import models as m
 from .blocks.diarization import SpeakerDiarizationConfig
 from .blocks.post import chunk_annotations, crop_plan
 from .core import Annotation
+from .operators import DeviceResample
 
 
-def plan_rows(idx: np.ndarray, step: float, window_samples: int, sample_rate: int, frames: int, nw: int, latency: float):
+def plan_rows(idx: np.ndarray, step: float, window_samples: int, sample_rate: int, frames: int, nw: int, latency: float,
+              resolution=None):
     """The post-path plan rows (``blocks.post.post_plan``) of chunks ``idx`` (B,) of streams whose window i starts at
     ``i * step`` and is fed to its pipeline one window per call -> (plan int32 (B, 4 + nw), out_start (B,), out_res (B,)).
     A row depends only on the chunk's index within its stream, so one vectorised evaluation covers every stream of a tick.
     Each buffer has its own start time and score resolution (extent duration / frames of its window, as
-    ``SpeakerDiarization.__call__`` measures it)."""
+    ``SpeakerDiarization.__call__`` measures it).  ``resolution``: the sample spacing of each row's window, scalar or (B,)
+    (default ``1 / sample_rate``; a resampled stream's is ``(chunk / source rate) / window_samples``)."""
     idx = np.asarray(idx, dtype=np.int64)
-    win = window_samples * (1 / sample_rate)                 # SlidingWindowFeature.extent: start + n * step
+    res_row = 1 / sample_rate if resolution is None else np.asarray(resolution, dtype=np.float64)
+    win = np.broadcast_to(window_samples * res_row, idx.shape)   # SlidingWindowFeature.extent: start + n * step
 
-    def start_res(k):
+    def start_res(k, w):
         s = k * step
-        e = s + win
+        e = s + w
         return s, np.where(e > s, e - s, 0.0) / frames       # Segment.duration / frames
 
-    starts, res = start_res(idx.astype(np.float64))
+    starts, res = start_res(idx.astype(np.float64), win)
     nb = np.minimum(idx + 1, nw)
     j = np.arange(nw)[None, :]
     valid = j < nb[:, None]
-    s_j, r_j = start_res(np.where(valid, (idx - (nb - 1))[:, None] + j, 0).astype(np.float64))
+    s_j, r_j = start_res(np.where(valid, (idx - (nb - 1))[:, None] + j, 0).astype(np.float64), win[:, None])
     return crop_plan(starts, res, s_j, r_j, nb, valid, nw, frames, step, latency)
 
 
-def available_windows(pushed: np.ndarray, emitted: np.ndarray, window_samples: int, step_samples: int) -> np.ndarray:
-    """complete windows of streams that received ``pushed`` samples and gave ``emitted`` windows (dg_multi_available)"""
+def available_windows(pushed: np.ndarray, emitted: np.ndarray, window_samples, step_samples) -> np.ndarray:
+    """complete windows of streams that received ``pushed`` samples and gave ``emitted`` windows (dg_multi_available);
+    window and step samples are scalars or per stream"""
     have = pushed - emitted * step_samples
-    return np.where(have >= window_samples, (have - window_samples) // step_samples + 1, 0)
+    return np.where(have >= window_samples, (have - window_samples) // np.maximum(step_samples, 1) + 1, 0)
+
+
+def source_geometry(rate: int, sample_rate: int, duration: float, step: float) -> Tuple[int, int, float]:
+    """(chunk, step samples, window resolution) of a stream at source ``rate`` served by a pipeline at ``sample_rate``, as
+    ``DeviceAudioStream(source_sample_rate=rate)`` windows and time-stamps it.  ValueError unless the chunk resamples to the
+    pipeline's chunk and a step is a whole number of resampled frames (``step % o == 0``, ``o / n`` the reduced ratio)."""
+    rate, sample_rate = int(rate), int(sample_rate)
+    if rate < 1:
+        raise ValueError(f"sample rate {rate} must be positive")
+    chunk, hop = int(round(rate * duration)), int(round(rate * step))
+    window = int(np.rint(duration * sample_rate))
+    if rate == sample_rate:
+        return chunk, hop, 1 / sample_rate
+    o = rate // math.gcd(rate, sample_rate)
+    n = sample_rate // math.gcd(rate, sample_rate)
+    out = -(-n * chunk // o)
+    if out != window:
+        raise ValueError(f"a {duration} s chunk at {rate} Hz ({chunk} samples) resamples to {out} samples, not the "
+                         f"pipeline's {window}")
+    if hop < 1 or hop % o:
+        raise ValueError(f"a {step} s step at {rate} Hz ({hop} samples) is not a whole number of resampled frames "
+                         f"({o} source samples each)")
+    return chunk, hop, (chunk * (1 / rate)) / window
 
 
 class MultiStreamDiarization:
-    """Up to ``max_streams`` live 16 kHz streams diarized on one device with one ``SpeakerDiarizationConfig``:
-    ``open(shift) -> sid``, ``push(sid, block)``, ``close(sid)``, and ``step() -> {sid: [Annotation, ...]}`` with one
-    ``Annotation`` per window consumed in the tick, in order -- what ``SpeakerDiarization(config)`` returns for that stream's
-    windows fed one per call, with its ``timestamp_shift`` set to ``shift``, up to the embedding caveat of the module
-    docstring.  Needs the native models (``B200*Loader``)."""
+    """Up to ``max_streams`` live streams diarized on one device with one ``SpeakerDiarizationConfig``:
+    ``open(shift, sample_rate) -> sid``, ``push(sid, block)``, ``close(sid)``, and ``step() -> {sid: [Annotation, ...]}`` with
+    one ``Annotation`` per window consumed in the tick, in order -- what ``SpeakerDiarization(config)`` returns for that
+    stream's windows fed one per call, with its ``timestamp_shift`` set to ``shift``, up to the embedding caveat of the module
+    docstring.  A stream is at ``config.sample_rate`` or at one of ``source_sample_rates`` (declared here, see
+    ``source_geometry``); its blocks are at its own rate, and its windows are resampled as ``DeviceResample`` resamples them.
+    Needs the native models (``B200*Loader``)."""
 
-    def __init__(self, config: SpeakerDiarizationConfig, max_streams: int, max_windows_per_stream: int = 4):
+    def __init__(self, config: SpeakerDiarizationConfig, max_streams: int, max_windows_per_stream: int = 4,
+                 source_sample_rates=()):
         self._h: Optional[C.c_void_p] = None
         self.config = config
         msg = f"Latency should be in the range [{config.step}, {config.duration}]"
@@ -89,11 +126,26 @@ class MultiStreamDiarization:
                                               int(config.normalize_embedding_weights), self.nw, ham.ctypes.data,
                                               C.byref(h)))
         self._h = h
-        # host mirror of the slots: open, samples pushed, windows consumed, timestamp shift
+        # rate -> (rate id, chunk samples, step samples, window resolution); one DeviceResample (tap table) per declared rate
+        self.rates = {sr: (-1, self.window_samples, self.step_samples, 1 / sr)}
+        self._resamplers: Dict[int, DeviceResample] = {}
+        for rate in sorted({int(r) for r in source_sample_rates} - {sr}):
+            chunk, hop, res = source_geometry(rate, sr, config.duration, config.step)
+            rs = DeviceResample(rate, sr, self.device)
+            rid = C.c_int()
+            with torch.cuda.device(self.device):
+                _lib.check(_lib.lib().dg_multi_add_rate(self._h, rs.handle, chunk, hop, C.byref(rid)))
+            self._resamplers[rate] = rs
+            self.rates[rate] = (rid.value, chunk, hop, res)
+        # host mirror of the slots: open, samples pushed, windows consumed, timestamp shift, window / step samples and
+        # resolution at the stream's rate
         self._open = np.zeros(self.max_streams, dtype=bool)
         self._pushed = np.zeros(self.max_streams, dtype=np.int64)
         self._emitted = np.zeros(self.max_streams, dtype=np.int64)
         self._shift = np.zeros(self.max_streams, dtype=np.float64)
+        self._chunk = np.full(self.max_streams, self.window_samples, dtype=np.int64)
+        self._hop = np.full(self.max_streams, self.step_samples, dtype=np.int64)
+        self._res = np.full(self.max_streams, 1 / sr, dtype=np.float64)
         self._turns = np.empty(1 << 16, dtype=np.uint32)
 
     def __del__(self):
@@ -107,17 +159,23 @@ class MultiStreamDiarization:
     def handle(self) -> C.c_void_p:
         return self._h
 
-    def open(self, shift: float = 0.0) -> int:
-        """a new stream (fresh clustering and aggregation state) in the lowest free slot; returns its id"""
+    def open(self, shift: float = 0.0, sample_rate: Optional[int] = None) -> int:
+        """a new stream (fresh clustering and aggregation state) in the lowest free slot, its blocks at ``sample_rate``
+        (default: the pipeline's; otherwise one of ``source_sample_rates``); returns its id"""
+        rate = self.config.sample_rate if sample_rate is None else int(sample_rate)
+        if rate not in self.rates:
+            raise ValueError(f"sample rate {rate} was not declared (source_sample_rates: {sorted(self._resamplers)})")
         free = np.flatnonzero(~self._open)
         if len(free) == 0:
             raise ValueError(f"all {self.max_streams} streams are open")
         sid = int(free[0])
+        rid, chunk, hop, res = self.rates[rate]
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().dg_multi_open(self._h, sid))
+            _lib.check(_lib.lib().dg_multi_open_rate(self._h, sid, rid))
         self._open[sid] = True
         self._pushed[sid] = self._emitted[sid] = 0
         self._shift[sid] = float(shift)
+        self._chunk[sid], self._hop[sid], self._res[sid] = chunk, hop, res
         return sid
 
     def close(self, sid: int):
@@ -151,8 +209,8 @@ class MultiStreamDiarization:
     def _step(self, outputs: bool = False) -> Tuple[Dict[int, List[Annotation]], Optional[tuple]]:
         """``step``; ``outputs``: also the tick's scores (B, F, K), embeddings (B, K, D) and maps (B, K) as device tensors,
         rows grouped by stream in slot order"""
-        counts = np.where(self._open, np.minimum(available_windows(self._pushed, self._emitted, self.window_samples,
-                                                                   self.step_samples), self.max_windows_per_stream), 0)
+        counts = np.where(self._open, np.minimum(available_windows(self._pushed, self._emitted, self._chunk, self._hop),
+                                                 self.max_windows_per_stream), 0)
         sids = np.flatnonzero(counts)
         n = counts[sids]
         B = int(n.sum())
@@ -160,7 +218,7 @@ class MultiStreamDiarization:
         idx = np.repeat(self._emitted[sids], n) + (np.arange(B) - np.repeat(row0, n))
         cfg = self.config
         plan, out_start, out_res = plan_rows(idx, cfg.step, self.window_samples, cfg.sample_rate, self.F, self.nw,
-                                             cfg.latency)
+                                             cfg.latency, np.repeat(self._res[sids], n))
         plan = np.ascontiguousarray(plan)
         header = np.empty((B, 4), dtype=np.int32)
         need = B * cfg.max_speakers * ((self.F + 2) // 2)

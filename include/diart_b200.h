@@ -358,6 +358,39 @@ int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, int32_t* co
  * networks, clustering, post-path, download), in ms; DG_EINVAL before the first such tick */
 int dg_multi_last_step_ms(const dg_multi* h, float* ms);
 int dg_multi_destroy(dg_multi* h);
+/* ---- streams at other source rates (a microphone at 44.1 kHz, say), resampled on the device as the reference's
+ *      blocks.Resample resamples every window (src/diart/inference.py:101-123).
+ *      dg_multi_add_rate: declares the source rate of `rs` (borrowed, on the handle's device; dg_resample_create(rate,
+ *        pipeline rate)) with chunk_samples / step_samples source samples per window / between windows (window i of such a
+ *        stream is source samples [i * step, i * step + chunk), resampled).  *rate_id receives 0, 1, ... in declaration
+ *        order.  Only before the first dg_multi_open*, because it grows the rings.  DG_EINVAL, changing nothing, unless the
+ *        chunk resamples to exactly the handle's chunk_samples, step % o == 0 (o / n the reduced rate ratio: a hop is whole
+ *        output frames), step <= chunk, the rate was not declared before and its rings fit 2^30 samples per stream.
+ *        Memory: every slot's source ring grows to the largest capacity (chunk + 2 max_windows_per_stream step, rounded up to
+ *        1024) of any rate, and every slot gets a 16 kHz ring of ((max_windows_per_stream - 1) step / o + r_hi - r_lo + 1) n
+ *        floats (the interior frames of max_windows_per_stream consecutive windows), largest over the rates.
+ *      dg_multi_open_rate: dg_multi_open at declared rate `rate_id` (-1: the pipeline's rate, = dg_multi_open).
+ *        dg_multi_push_host and dg_multi_available then count source samples and source-rate windows, and the capacity of
+ *        the slot is its rate's: a stream at the pipeline's rate refuses exactly what it refuses without declared rates.
+ *      In a tick, a resampled stream's windows are computed from its source ring: each 16 kHz frame whose taps all lie inside
+ *        a window is computed once over the life of the stream (one launch per rate in the tick, kept in the slot's 16 kHz
+ *        ring), and the frames at each window's edges are recomputed with the window's zero padding.  Every resampled window
+ *        has the bits of dg_resample_forward on the stacked source window.  A tick whose streams are all at the pipeline's
+ *        rate launches what it launches without declared rates. ---- */
+typedef struct dg_resample dg_resample;   /* declared with its entry points below */
+int dg_multi_add_rate(dg_multi* h, dg_resample* rs, int chunk_samples, int step_samples, int* rate_id);
+int dg_multi_open_rate(dg_multi* h, int slot, int rate_id);
+/* test hook: the last tick's window batch [n_rows, chunk_samples] (what its networks read; n_rows = that tick's window count)
+ * copied to wav_dev.  Synchronous. */
+int dg_multi_last_windows(const dg_multi* h, float* wav_dev, int n_rows);
+/* test hook (host only, no GPU): dg_multi's tick planning for `slots` streams with pipeline windows of out_chunk / out_step
+ * samples and the declared rates rates int32 [n_rates][5] = {o, n, w, chunk, step} (refused as dg_multi_add_rate refuses
+ * them, DG_EINVAL).  ops int32 [n_ops][3] = {kind, slot, n}: 0 open slot at rate id n (-1: the pipeline's rate), 1 close slot,
+ * 2 push n samples, 4 tick.  result int32 [n_ops]: each op's return code.  records int64 [cap][5] = {tick, kind, slot, a, b},
+ * *n_records of them: kind 0 a resampling item (16 kHz frames [a, a + b) of the stream), kind 1 a window of the tick (it
+ * starts at source sample a, batch row b).  DG_EINVAL if more than cap records. */
+int dg_selftest_multi_frames_host(int slots, int max_wps, int out_chunk, int out_step, int n_rates, const int32_t* rates,
+                                  int n_ops, const int32_t* ops, int32_t* result, int64_t* records, int cap, int* n_records);
 /* test hook (host only, no GPU): dg_multi's bookkeeping of pushed audio on `slots` rings of C samples, with ring_scatter's
  * writes done on the host.  ops int32 [n_ops][3] = {kind, slot, n}: 0 open slot, 1 close slot (its staged samples are
  * dropped), 2 push the next n samples of samples_host (a refused push still skips them), 3 consume n samples (as a tick's
