@@ -111,6 +111,7 @@ SIGNATURES = {
     "dg_vad_sweep_destroy": (C.c_int, [_P]),
     "dg_multi_create": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double,
                                   C.c_float, C.c_float, C.c_int, C.c_int, _P, C.POINTER(_P)]),
+    "dg_multi_create_vad": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, _P, C.POINTER(_P)]),
     "dg_multi_open": (C.c_int, [_P, C.c_int]),
     "dg_multi_close": (C.c_int, [_P, C.c_int]),
     "dg_multi_push_host": (C.c_int, [_P, C.c_int, _P, C.c_int]),

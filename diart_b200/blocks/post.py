@@ -84,6 +84,10 @@ class DevicePostPath:
     def run(self, seg: torch.Tensor, maps: torch.Tensor, starts: np.ndarray, res: float, shift: float = 0.0):
         """device scores (B,F,K) + maps (B,K) -> list of Annotation (block-level entry; the fused pipeline uses
         dg_pipeline_call_host instead)"""
+        return self.annotations(*self.turns(seg, maps, starts, res), shift)
+
+    def turns(self, seg: torch.Tensor, maps: torch.Tensor, starts: np.ndarray, res: float):
+        """``run`` up to the packed turns -> (header (B, 4), turns, n_turns, out_start (B,), out_res (B,))"""
         plan, out_start, out_res = self.plan(np.asarray(starts, dtype=np.float64), res)
         B = len(plan)
         header, turns = self.buffers(B)
@@ -92,7 +96,7 @@ class DevicePostPath:
             _lib.check(_lib.lib().dg_post_step(self._h, seg.data_ptr(), maps.data_ptr(), B, plan.ctypes.data,
                                                header.ctypes.data, turns.ctypes.data, len(turns), C.byref(n),
                                                _lib.stream_ptr(self.device)))
-        return self.annotations(header, turns, n.value, out_start, out_res, shift)
+        return header, turns, n.value, out_start, out_res
 
 
 def post_plan(starts: np.ndarray, res: float, hist_start: np.ndarray, hist_res: np.ndarray, nw: int, F: int, step: float,
@@ -167,22 +171,27 @@ def turn_times(header: np.ndarray, turns: np.ndarray, n_turns: int, out_start: n
     return row_of, g, t_on, t_off
 
 
-def chunk_annotations(header: np.ndarray, turns: np.ndarray, n_turns: int, out_start: np.ndarray, out_res: np.ndarray,
-                      labels: Sequence[str], shift=0.0, uri: Optional[str] = None) -> List[Annotation]:
-    """packed turns -> one Annotation per chunk (row of ``header``), segments at frame middles (blocks/utils.py:45-58).
-    ``shift``: seconds added to every time stamp, one number or one per chunk (streams with their own shifts)."""
-    B = len(header)
+def chunk_turns(header: np.ndarray, turns: np.ndarray, n_turns: int, out_start: np.ndarray, out_res: np.ndarray, shift=0.0):
+    """packed turns -> plain lists (offset and count per chunk, then speaker, on time, off time per turn), segments at frame
+    middles (blocks/utils.py:45-58).  ``shift``: seconds added to every time stamp, one number or one per chunk."""
     per_chunk = np.ndim(shift) > 0
     row_of, g, t_on, t_off = turn_times(header, turns, n_turns, out_start, out_res, 0.0 if per_chunk else shift)
     if per_chunk:                                            # x + 0.0 + s == x + s: the same bits as a scalar shift
         s = np.asarray(shift, dtype=np.float64)[row_of]
         t_on, t_off = t_on + s, t_off + s
-    t_on, t_off, g = t_on.tolist(), t_off.tolist(), g.tolist()
+    return header[:, 0].tolist(), header[:, 1].tolist(), g.tolist(), t_on.tolist(), t_off.tolist()
+
+
+def chunk_annotations(header: np.ndarray, turns: np.ndarray, n_turns: int, out_start: np.ndarray, out_res: np.ndarray,
+                      labels: Sequence[str], shift=0.0, uri: Optional[str] = None) -> List[Annotation]:
+    """packed turns -> one Annotation per chunk (row of ``header``), segments at frame middles (blocks/utils.py:45-58).
+    ``shift``: seconds added to every time stamp, one number or one per chunk (streams with their own shifts)."""
+    B = len(header)
+    offs, cnts, g, t_on, t_off = chunk_turns(header, turns, n_turns, out_start, out_res, shift)
     # the reference's shifted copy drops the modality
-    modality = [("speech" if x == 0 else None) for x in np.asarray(shift).tolist()] if per_chunk else \
+    modality = [("speech" if x == 0 else None) for x in np.asarray(shift).tolist()] if np.ndim(shift) > 0 else \
         [("speech" if shift == 0 else None)] * B
     out = []
-    offs, cnts = header[:, 0].tolist(), header[:, 1].tolist()
     for cidx in range(B):
         ann = Annotation(uri=uri, modality=modality[cidx])
         o = offs[cidx]

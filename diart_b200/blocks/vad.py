@@ -4,16 +4,32 @@ network of the hot path, a max over the local speakers, and the same device post
 with ONE "speaker" whose turns are labelled ``"speech"``."""
 from __future__ import annotations
 
-from typing import Optional, Sequence, Tuple
+from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
 
 from .. import models as m
-from ..core import Annotation, SlidingWindowFeature
+from ..core import Annotation, Segment, SlidingWindowFeature
 from . import base
-from .post import DevicePostPath, aggregate_audio
+from .post import DevicePostPath, aggregate_audio, chunk_turns
 from .segmentation import SpeakerSegmentation
+
+
+def speech_annotations(header: np.ndarray, turns: np.ndarray, n_turns: int, out_start: np.ndarray, out_res: np.ndarray,
+                       shift=0.0) -> List[Annotation]:
+    """the device post-path's turns of one speaker (``header`` (B, 4), packed ``turns``, as ``chunk_annotations`` takes them)
+    -> what ``VoiceActivityDetection`` returns per chunk: tracks numbered in order, label ``"speech"``, modality ``"speech"``
+    (reference vad.py:172-178).  A chunk's turns come in time order and do not overlap, so their order is the tracks' order.
+    ``shift``: one number, or one per chunk."""
+    offs, cnts, _, t_on, t_off = chunk_turns(header, turns, n_turns, out_start, out_res, shift)
+    outputs = []
+    for o, k in zip(offs, cnts):
+        speech = Annotation(modality="speech")
+        for n, i in enumerate(range(o, o + k)):
+            speech[Segment(t_on[i], t_off[i]), n] = "speech"
+        outputs.append(speech)
+    return outputs
 
 
 class VoiceActivityDetectionConfig(base.WindowTiming):
@@ -72,12 +88,7 @@ class VoiceActivityDetection(base.Pipeline):
             self._post = DevicePostPath(cfg.step, cfg.latency, cfg.tau_active, F, 1, 1, device)
         starts = np.array([w.extent.start for w in waveforms], dtype=np.float64)
         to_first = torch.zeros((B, 1), dtype=torch.int32, device=device)  # the one local "speaker" is global speaker 0
-        turns = self._post.run(vad, to_first, starts, waveforms[0].extent.duration / F, self.timestamp_shift)
-        outputs = []
-        for ann in turns:                                                 # tracks numbered in order, label "speech" (vad.py:172-178)
-            speech = Annotation(uri=ann.uri, modality="speech")
-            for n, (segment, _) in enumerate(ann.itertracks()):
-                speech[segment, n] = "speech"
-            outputs.append(speech)
+        outputs = speech_annotations(*self._post.turns(vad, to_first, starts, waveforms[0].extent.duration / F),
+                                     self.timestamp_shift)
         audio, self.chunk_buffer = aggregate_audio(self.chunk_buffer, waveforms, self._post.nw, cfg.step, cfg.latency)
         return list(zip(outputs, audio))

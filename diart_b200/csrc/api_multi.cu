@@ -3,6 +3,10 @@
 // across the streams.  Work happens in ticks: every open stream contributes its complete, unconsumed windows (at most
 // max_wps), and those windows run as ONE batch -- one upload, one network pass (in sub-batches on the two scratch lanes),
 // one clustering launch with a state per stream, one post-path launch with a history per stream, one download.
+//
+// A VAD handle (dg_multi_create_vad) serves the reference's VoiceActivityDetection the same way: the same audio in, the
+// segmentation network alone, and per stream its speech curve (max over the local speakers) aggregated and binarised on the
+// device, with a history of max curves per stream.  It has no embedding model and no clustering state.
 #include <string.h>
 
 #include <algorithm>
@@ -202,6 +206,7 @@ struct dg_multi {
   bool opened = false;                        // a stream was opened (rates can no longer be added)
   int last_B = 0;                             // windows of the last tick that had any
   DevBuf rings, hamming, in, wav, seg, emb, maps, centers, active, init, prep, prep_d, hist_seg, hist_map, header, turns, total;
+  DevBuf hist_vad;                            // VAD mode (net.emb null): per slot the last nw - 1 max curves [2][slots][nw - 1][F]
   PinnedBuf pin_out;                          // header, turn count and turn prefix of a tick (TurnOut layout at 0)
   Stream st;
   Event e_start, e_lane_done[2];
@@ -210,6 +215,7 @@ struct dg_multi {
 };
 
 static bool slot_ok(const dg_multi* h, int slot) { return h && h->book.ok(slot); }
+static bool vad_mode(const dg_multi* h) { return !h->net.emb; }
 
 extern "C" int dg_multi_create(dg_seg* seg, dg_emb* emb, int chunk_samples, int step_samples, int max_streams,
                                int max_windows_per_stream, int max_speakers, double tau, double rho, double delta, float gamma,
@@ -270,6 +276,54 @@ extern "C" int dg_multi_create(dg_seg* seg, dg_emb* emb, int chunk_samples, int 
   return DG_OK;
 }
 
+// The numbers are checked before the handles, so that every refusal can be seen without a device.
+extern "C" int dg_multi_create_vad(dg_seg* seg, int chunk_samples, int step_samples, int max_streams, int max_windows_per_stream,
+                                   double tau, int num_windows, const double* hamming_host, dg_multi** out) {
+  if (chunk_samples < 4 || step_samples < 4 || chunk_samples % 4 || step_samples % 4 || step_samples > chunk_samples) {
+    set_error("dg_multi_create_vad: chunk and step must be positive multiples of 4 samples, step <= chunk");
+    return DG_EINVAL;
+  }
+  if (max_streams < 1 || max_windows_per_stream < 1 || (long long)max_streams * max_windows_per_stream > 65535 ||
+      num_windows < 1 || num_windows > 256 || !std::isfinite(tau)) {
+    set_error("dg_multi_create_vad: need max_streams, max_windows_per_stream >= 1 with a product <= 65535, 1 <= num_windows "
+              "<= 256 and a finite threshold");
+    return DG_EINVAL;
+  }
+  if (!seg || !out || !hamming_host) {
+    set_error("dg_multi_create_vad: null handle or buffer");
+    return DG_EINVAL;
+  }
+  int rc, F = 0, K = 0;
+  if ((rc = dg_seg_dims(seg, chunk_samples, &F, &K))) return rc;
+  if (K > 8 || F > 1023) {
+    set_error("dg_multi_create_vad: need local speakers <= 8 and frames <= 1023");
+    return DG_EINVAL;
+  }
+  DG_CUDA(cudaSetDevice(seg->device));
+  std::unique_ptr<dg_multi> h(new dg_multi());
+  h->device = seg->device; h->slots = max_streams; h->max_wps = max_windows_per_stream;
+  h->S = chunk_samples; h->hop = step_samples;
+  RateGeom base;
+  base.S = chunk_samples;
+  base.hop = step_samples;
+  base.cap = (int)ring_capacity(chunk_samples, step_samples, max_windows_per_stream);
+  h->book.init(max_streams, base);
+  h->F = F; h->K = K; h->M = 1; h->nw = num_windows;   // one "speaker": speech
+  h->tau = tau;
+  h->net.seg = seg;
+  const size_t n = (size_t)max_streams, hist = (size_t)std::max(1, num_windows - 1);
+  h->n_hist.assign(n, 0); h->cur.assign(n, 0);
+  if (h->rings.ensure(n * h->book.C * 4) || h->hamming.ensure((size_t)F * 8) || h->hist_vad.ensure(2 * n * hist * F * 4) ||
+      h->total.ensure(16))
+    return DG_ECUDA;
+  DG_CUDA(cudaMemcpy(h->hamming.p, hamming_host, (size_t)F * 8, cudaMemcpyHostToDevice));
+  if (net_lanes_create(h->net) || h->st.create() || h->e_start.create() || h->e_lane_done[0].create() ||
+      h->e_lane_done[1].create() || h->t_begin.create(cudaEventDefault) || h->t_end.create(cudaEventDefault))
+    return DG_ECUDA;
+  *out = h.release();
+  return DG_OK;
+}
+
 extern "C" int dg_multi_destroy(dg_multi* h) {
   delete h;
   return DG_OK;
@@ -310,7 +364,7 @@ extern "C" int dg_multi_add_rate(dg_multi* h, dg_resample* rs, int chunk_samples
 }
 
 // a new stream in `slot` at declared rate `rate_id` (-1: the pipeline's rate): empty rings, fresh clustering state (the
-// reference's SpeakerDiarization.reset()), no history
+// reference's SpeakerDiarization.reset(); a VAD handle has none), no history
 extern "C" int dg_multi_open_rate(dg_multi* h, int slot, int rate_id) {
   if (!h || slot < 0 || slot >= h->slots || h->book.open[slot]) {
     set_error("dg_multi_open: slot " + std::to_string(slot) + " is out of range or already open");
@@ -322,9 +376,11 @@ extern "C" int dg_multi_open_rate(dg_multi* h, int slot, int rate_id) {
   }
   DG_CUDA(cudaSetDevice(h->device));
   const size_t s = (size_t)slot;
-  DG_CUDA(cudaMemsetAsync(h->centers.as<double>() + s * h->M * h->D, 0, (size_t)h->M * h->D * 8, h->st));
-  DG_CUDA(cudaMemsetAsync(h->active.as<int>() + s * 32, 0, 32 * 4, h->st));
-  DG_CUDA(cudaMemsetAsync(h->init.as<int>() + s * 2, 0, 2 * 4, h->st));
+  if (!vad_mode(h)) {
+    DG_CUDA(cudaMemsetAsync(h->centers.as<double>() + s * h->M * h->D, 0, (size_t)h->M * h->D * 8, h->st));
+    DG_CUDA(cudaMemsetAsync(h->active.as<int>() + s * 32, 0, 32 * 4, h->st));
+    DG_CUDA(cudaMemsetAsync(h->init.as<int>() + s * 2, 0, 2 * 4, h->st));
+  }
   h->book.start(slot, rate_id + 1);
   h->n_hist[slot] = 0;
   h->opened = true;
@@ -379,12 +435,191 @@ extern "C" int dg_multi_push_host(dg_multi* h, int slot, const float* samples, i
 
 static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
 
+// Where the tables of a tick lie in its one host -> device copy (byte offsets into h->in): staged samples at 0, pieces [np],
+// slots [n_act], rows [B] {slot entry, window}, window starts [B], plan [B][stride], cluster states [n_act] {slot, 0}, chunk
+// offsets [slots + 1] by slot, thresholds [3] (the last three are read by a diarization tick only).  A tick with resampled rows
+// also carries the rows at the pipeline's rate [n16] with their starts, the resampling items and the resampled rows.
+struct TickIn {
+  size_t o_pieces, o_act, o_rows, o_start, o_plan, o_states, o_off, o_trials, o_rows16, o_start16, o_items, o_rs, bytes;
+  bool mixed;
+};
+
+// The audio-in half of a tick, the same in both modes: ONE copy of the staged samples and the tick's tables to h->in (t_begin
+// recorded before it), the staged samples to their rings, then the batch [B, S] of windows to h->wav, grouped by slot (windows
+// at a declared rate resampled); e_start marks the batch complete on h->st.
+static int tick_audio_in(dg_multi* h, const TickPlan& tp, const int32_t* plan_host, TickIn& L) {
+  cudaStream_t st = h->st;
+  const std::vector<TickSlot>& act = tp.act;
+  const int B = tp.B, n_act = (int)act.size(), np = (int)h->book.pieces.size(), S = h->S, stride = 4 + h->nw;
+  L.o_pieces = align16((size_t)h->book.n_staged * 4);
+  L.o_act = L.o_pieces + align16((size_t)np * sizeof(RingPiece));
+  L.o_rows = L.o_act + align16((size_t)n_act * sizeof(TickSlot));
+  L.o_start = L.o_rows + align16((size_t)B * 8);
+  L.o_plan = L.o_start + align16((size_t)B * 8);
+  L.o_states = L.o_plan + align16((size_t)B * stride * 4);
+  L.o_off = L.o_states + align16((size_t)n_act * 8);
+  L.o_trials = L.o_off + align16((size_t)(h->slots + 1) * 4);
+  L.mixed = !tp.rs_rows.empty();
+  const int n16 = (int)tp.rows16.size(), n_items = (int)tp.items.size(), n_rs = (int)tp.rs_rows.size();
+  L.o_rows16 = L.o_trials + 32;
+  L.o_start16 = L.o_rows16 + align16((size_t)n16 * 8);
+  L.o_items = L.o_start16 + align16((size_t)n16 * 8);
+  L.o_rs = L.o_items + align16((size_t)n_items * sizeof(RsFrames));
+  L.bytes = L.mixed ? L.o_rs + (size_t)n_rs * sizeof(RsRow) : L.o_trials + 24;
+  if (h->in.ensure(L.bytes) || h->wav.ensure((size_t)B * S * 4)) return DG_ECUDA;
+  if (L.bytes > h->stage.bytes) {
+    PinnedBuf bigger;
+    if (bigger.ensure(L.bytes)) return DG_ECUDA;
+    if (h->book.n_staged) memcpy(bigger.h, h->stage.h, (size_t)h->book.n_staged * 4);
+    h->stage = std::move(bigger);
+  }
+  unsigned char* pin = h->stage.as<unsigned char>();
+  if (np) memcpy(pin + L.o_pieces, h->book.pieces.data(), (size_t)np * sizeof(RingPiece));
+  memcpy(pin + L.o_act, act.data(), (size_t)n_act * sizeof(TickSlot));
+  memcpy(pin + L.o_rows, tp.rows.data(), (size_t)B * 8);
+  memcpy(pin + L.o_start, tp.start.data(), (size_t)B * 8);
+  int2* states = reinterpret_cast<int2*>(pin + L.o_states);
+  int32_t* off = reinterpret_cast<int32_t*>(pin + L.o_off);
+  for (int a = 0, s = 0; a < n_act; a++) {
+    const TickSlot& ts = act[a];
+    for (; s <= ts.slot; s++) off[s] = ts.row0;
+    states[a] = make_int2(ts.slot, 0);
+  }
+  if (L.mixed) {
+    if (n16) memcpy(pin + L.o_rows16, tp.rows16.data(), (size_t)n16 * 8);
+    if (n16) memcpy(pin + L.o_start16, tp.start16.data(), (size_t)n16 * 8);
+    if (n_items) memcpy(pin + L.o_items, tp.items.data(), (size_t)n_items * sizeof(RsFrames));
+    memcpy(pin + L.o_rs, tp.rs_rows.data(), (size_t)n_rs * sizeof(RsRow));
+  }
+  for (int s = act.back().slot + 1; s <= h->slots; s++) off[s] = B;
+  memcpy(pin + L.o_plan, plan_host, (size_t)B * stride * 4);
+  const double trials[3] = {h->tau, h->rho, h->delta};
+  memcpy(pin + L.o_trials, trials, 24);
+  unsigned char* din = h->in.as<unsigned char>();
+  DG_CUDA(cudaEventRecord(h->t_begin, st));
+  DG_CUDA(cudaMemcpyAsync(din, pin, L.bytes, cudaMemcpyHostToDevice, st));
+  const TickSlot* d_act = reinterpret_cast<const TickSlot*>(din + L.o_act);
+  const int2* d_rows = reinterpret_cast<const int2*>(din + L.o_rows);
+  int rc;
+  // audio in: the staged samples to their rings, then the batch [B, S], windows grouped by slot
+  if ((rc = launch_ring_scatter(reinterpret_cast<const float*>(din), reinterpret_cast<const RingPiece*>(din + L.o_pieces), np,
+                                h->book.C, h->rings.as<float>(), st)))
+    return rc;
+  if (!L.mixed) {
+    if ((rc = launch_ring_gather(h->rings.as<float>(), h->book.C, d_act, d_rows, reinterpret_cast<const long long*>(din + L.o_start),
+                                 S, B, h->wav.as<float>(), st)))
+      return rc;
+  } else {
+    if (n16 && (rc = launch_ring_gather(h->rings.as<float>(), h->book.C, d_act, reinterpret_cast<const int2*>(din + L.o_rows16),
+                                        reinterpret_cast<const long long*>(din + L.o_start16), S, n16, h->wav.as<float>(), st)))
+      return rc;
+    // per declared rate: the new 16 kHz frames of its streams, then its windows
+    for (size_t i = 1; i < h->book.rates.size(); i++) {
+      const RateGeom& r = h->book.rates[i];
+      const int i0 = tp.item_off[i - 1], i1 = tp.item_off[i], w0 = tp.row_off[i - 1], w1 = tp.row_off[i];
+      long long max_count = 0;
+      for (int k = i0; k < i1; k++) max_count = std::max<long long>(max_count, tp.items[k].count);
+      const float* W = r.rs->taps.as<float>();
+      if ((rc = launch_resample_frames(h->rings.as<float>(), h->book.C, reinterpret_cast<const RsFrames*>(din + L.o_items) + i0,
+                                       i1 - i0, max_count, W, r.g, h->yrings.as<float>(), h->Y, r.Q, st)) ||
+          (rc = launch_resample_gather(h->rings.as<float>(), h->book.C, h->yrings.as<float>(), h->Y, r.Q,
+                                       reinterpret_cast<const RsRow*>(din + L.o_rs) + w0, w1 - w0, r.r_lo, r.r_hi, W, r.g, r.S, S,
+                                       h->wav.as<float>(), st)))
+        return rc;
+    }
+  }
+  DG_CUDA(cudaEventRecord(h->e_start, st));
+  return DG_OK;
+}
+
+// A diarization tick after the audio in: both networks, clustering with a state per slot, the post-path with each slot's
+// history, on h->st.
+static int tick_diarize(dg_multi* h, const TickPlan& tp, const TickIn& L, int turn_cap) {
+  cudaStream_t st = h->st;
+  const int B = tp.B, n_act = (int)tp.act.size(), F = h->F, K = h->K, D = h->D, M = h->M, S = h->S;
+  const unsigned char* din = h->in.as<unsigned char>();
+  const TickSlot* d_act = reinterpret_cast<const TickSlot*>(din + L.o_act);
+  const int2* d_rows = reinterpret_cast<const int2*>(din + L.o_rows);
+  int rc;
+  // networks: sub-batches of at most 256 windows on alternating scratch lanes (the workspace of a 256-window step); a lane is
+  // reused once the sub-batch before on it is past its embeddings
+  for (int r0 = 0, j = 0; r0 < B; r0 += 256, j++) {
+    const int nb = std::min(256, B - r0), lane = j & 1;
+    for (cudaStream_t s : {(cudaStream_t)h->net.s_seg[lane], (cudaStream_t)h->net.s_emb})
+      DG_CUDA(cudaStreamWaitEvent(s, h->e_lane_done[lane], 0));
+    if ((rc = pipeline_nets(&h->net, h->wav.as<float>() + (size_t)r0 * S, S, {nb, F, K}, h->seg.as<float>() + (size_t)r0 * F * K,
+                            h->emb.as<float>() + (size_t)r0 * K * D, h->e_start, lane, 0)))
+      return rc;
+    DG_CUDA(cudaEventRecord(h->e_lane_done[lane], h->net.s_emb));
+  }
+  DG_CUDA(cudaStreamWaitEvent(st, h->net.e_emb, 0));
+  // clustering: state `slot` over that slot's rows (chunk offsets by slot), cosine
+  ClusterParams p{};
+  p.M = M;
+  p.D = D;
+  p.metric = 0;
+  if ((rc = launch_cluster_sweep(p, reinterpret_cast<const double*>(din + L.o_trials), 1,
+                                 reinterpret_cast<const int2*>(din + L.o_states), n_act, reinterpret_cast<const int*>(din + L.o_off),
+                                 h->seg.as<float>(), h->emb.as<float>(), B, F, K, h->centers.as<double>(), h->active.as<int>(),
+                                 h->init.as<int>(), h->prep.as<float>(), h->prep_d.as<double>(), h->maps.as<int32_t>(), st)))
+    return rc;
+  // post-path with each slot's history, then the histories move on
+  DG_CUDA(cudaMemsetAsync(h->total.p, 0, 4, st));
+  if ((rc = launch_post_slots(h->seg.as<float>(), h->maps.as<int32_t>(), h->hist_seg.as<float>(), h->hist_map.as<int32_t>(),
+                              d_act, d_rows, h->slots, B, F, K, M, h->nw, reinterpret_cast<const int32_t*>(din + L.o_plan),
+                              4 + h->nw, h->hamming.as<double>(), h->tau, h->header.as<int32_t>(), h->turns.as<uint32_t>(),
+                              turn_cap, h->total.as<unsigned int>(), st)) ||
+      (rc = launch_post_slots_history(h->seg.as<float>(), h->maps.as<int32_t>(), h->hist_seg.as<float>(),
+                                      h->hist_map.as<int32_t>(), d_act, n_act, h->slots, F, K, h->nw, st)))
+    return rc;
+  return DG_OK;
+}
+
+// A VAD tick after the audio in: the segmentation network alone, then each slot's speech curve binarised with its history of
+// max curves, on h->st.
+static int tick_vad(dg_multi* h, const TickPlan& tp, const TickIn& L, int turn_cap) {
+  cudaStream_t st = h->st;
+  const int B = tp.B, n_act = (int)tp.act.size(), F = h->F, K = h->K, S = h->S;
+  const unsigned char* din = h->in.as<unsigned char>();
+  const TickSlot* d_act = reinterpret_cast<const TickSlot*>(din + L.o_act);
+  int rc;
+  // segmentation: sub-batches of at most 256 windows on alternating scratch lanes, each bracketed by the lane's guard (as
+  // pipeline_nets brackets it) so that other users of the model handle are ordered against it.  A lane takes its next
+  // sub-batch in stream order, once the one before on it has its scores; e_lane_done[lane] marks the lane's last scores.
+  for (int r0 = 0, j = 0; r0 < B; r0 += 256, j++) {
+    const int nb = std::min(256, B - r0), lane = j & 1;
+    cudaStream_t s_seg = h->net.s_seg[lane];
+    DG_CUDA(cudaStreamWaitEvent(s_seg, h->e_start, 0));
+    LaneUse use(h->net.seg->guard[lane], &h->net, s_seg);
+    if ((rc = use.rc) ||
+        (rc = seg_forward_lane(h->net.seg, lane, nullptr, h->wav.as<float>() + (size_t)r0 * S, nb, S,
+                               h->seg.as<float>() + (size_t)r0 * F * K, s_seg)) ||
+        (rc = use.end()))
+      return rc;
+    DG_CUDA(cudaEventRecord(h->e_lane_done[lane], s_seg));
+  }
+  for (int lane = 0; lane < 2; lane++) DG_CUDA(cudaStreamWaitEvent(st, h->e_lane_done[lane], 0));
+  // speech curves with each slot's history, then the histories move on
+  DG_CUDA(cudaMemsetAsync(h->total.p, 0, 4, st));
+  if ((rc = launch_vad_slots(h->seg.as<float>(), h->hist_vad.as<float>(), d_act, reinterpret_cast<const int2*>(din + L.o_rows),
+                             h->slots, B, F, K, h->nw, reinterpret_cast<const int32_t*>(din + L.o_plan), 4 + h->nw,
+                             h->hamming.as<double>(), h->tau, h->header.as<int32_t>(), h->turns.as<uint32_t>(), turn_cap,
+                             h->total.as<unsigned int>(), st)) ||
+      (rc = launch_vad_slots_history(h->seg.as<float>(), h->hist_vad.as<float>(), d_act, n_act, h->slots, F, K, h->nw, st)))
+    return rc;
+  return DG_OK;
+}
+
 extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, int32_t* counts_host, int32_t* header_host,
                              uint32_t* turns_host, int turn_cap_host, int* n_turns, float* seg_dev, float* emb_dev,
                              int32_t* map_dev) {
   const char* who = "dg_multi_step";
   if (!h || !counts_host || n_rows < 0 || (n_rows > 0 && (!plan_host || !header_host || !turns_host))) {
     set_error(std::string(who) + ": bad arguments");
+    return DG_EINVAL;
+  }
+  if (vad_mode(h) && (emb_dev || map_dev)) {
+    set_error(std::string(who) + ": a VAD handle has no embeddings or speaker maps");
     return DG_EINVAL;
   }
   // this tick's slots and rows: every open slot with windows gives up to max_wps, in slot order
@@ -420,119 +655,19 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
   if (B == 0) return DG_OK;     // nothing to do: staged samples wait for the next tick
   DG_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = h->st;
-  const int n_act = (int)act.size(), np = (int)h->book.pieces.size(), F = h->F, K = h->K, D = h->D, M = h->M, S = h->S;
-  // host -> device, ONE copy: staged samples, pieces [np], slots [n_act], rows [B] {slot entry, window}, window starts [B],
-  // plan [B][stride], cluster states [n_act] {slot, 0}, chunk offsets [slots + 1] by slot, thresholds [3]
-  const size_t o_pieces = align16((size_t)h->book.n_staged * 4), o_act = o_pieces + align16((size_t)np * sizeof(RingPiece));
-  const size_t o_rows = o_act + align16((size_t)n_act * sizeof(TickSlot)), o_start = o_rows + align16((size_t)B * 8);
-  const size_t o_plan = o_start + align16((size_t)B * 8), o_states = o_plan + align16((size_t)B * stride * 4);
-  const size_t o_off = o_states + align16((size_t)n_act * 8), o_trials = o_off + align16((size_t)(h->slots + 1) * 4);
-  // a tick with resampled rows also carries the rows at the pipeline's rate [n16] with their starts, the resampling items and
-  // the resampled rows
-  const bool mixed = !tp.rs_rows.empty();
-  const int n16 = (int)tp.rows16.size(), n_items = (int)tp.items.size(), n_rs = (int)tp.rs_rows.size();
-  const size_t o_rows16 = o_trials + 32, o_start16 = o_rows16 + align16((size_t)n16 * 8);
-  const size_t o_items = o_start16 + align16((size_t)n16 * 8), o_rs = o_items + align16((size_t)n_items * sizeof(RsFrames));
-  const size_t in_b = mixed ? o_rs + (size_t)n_rs * sizeof(RsRow) : o_trials + 24;
+  const int F = h->F, K = h->K, D = h->D, M = h->M;
   const TurnOut lay = {0, (size_t)B * 16};
   const int turn_cap = B * M * ((F + 2) / 2);   // every second output frame of every speaker starts a turn
-  if (h->in.ensure(in_b) || h->wav.ensure((size_t)B * S * 4) || h->seg.ensure((size_t)B * F * K * 4) ||
-      h->emb.ensure((size_t)B * K * D * 4) || h->maps.ensure((size_t)B * K * 4) ||
-      h->prep.ensure(cluster_prep_floats(B, K) * 4 + 16) || h->prep_d.ensure(cluster_prep_doubles(B, K) * 8 + 16) ||
-      h->header.ensure(lay.header_bytes) || h->turns.ensure((size_t)turn_cap * 4) || h->pin_out.ensure(lay.end()))
+  if (h->seg.ensure((size_t)B * F * K * 4) || h->header.ensure(lay.header_bytes) || h->turns.ensure((size_t)turn_cap * 4) ||
+      h->pin_out.ensure(lay.end()))
     return DG_ECUDA;
-  if (in_b > h->stage.bytes) {
-    PinnedBuf bigger;
-    if (bigger.ensure(in_b)) return DG_ECUDA;
-    if (h->book.n_staged) memcpy(bigger.h, h->stage.h, (size_t)h->book.n_staged * 4);
-    h->stage = std::move(bigger);
-  }
-  unsigned char* pin = h->stage.as<unsigned char>();
-  if (np) memcpy(pin + o_pieces, h->book.pieces.data(), (size_t)np * sizeof(RingPiece));
-  memcpy(pin + o_act, act.data(), (size_t)n_act * sizeof(TickSlot));
-  memcpy(pin + o_rows, tp.rows.data(), (size_t)B * 8);
-  memcpy(pin + o_start, tp.start.data(), (size_t)B * 8);
-  int2* states = reinterpret_cast<int2*>(pin + o_states);
-  int32_t* off = reinterpret_cast<int32_t*>(pin + o_off);
-  for (int a = 0, s = 0; a < n_act; a++) {
-    const TickSlot& ts = act[a];
-    for (; s <= ts.slot; s++) off[s] = ts.row0;
-    states[a] = make_int2(ts.slot, 0);
-  }
-  if (mixed) {
-    if (n16) memcpy(pin + o_rows16, tp.rows16.data(), (size_t)n16 * 8);
-    if (n16) memcpy(pin + o_start16, tp.start16.data(), (size_t)n16 * 8);
-    if (n_items) memcpy(pin + o_items, tp.items.data(), (size_t)n_items * sizeof(RsFrames));
-    memcpy(pin + o_rs, tp.rs_rows.data(), (size_t)n_rs * sizeof(RsRow));
-  }
-  for (int s = act.back().slot + 1; s <= h->slots; s++) off[s] = B;
-  memcpy(pin + o_plan, plan_host, (size_t)B * stride * 4);
-  const double trials[3] = {h->tau, h->rho, h->delta};
-  memcpy(pin + o_trials, trials, 24);
-  unsigned char* din = h->in.as<unsigned char>();
-  DG_CUDA(cudaEventRecord(h->t_begin, st));
-  DG_CUDA(cudaMemcpyAsync(din, pin, in_b, cudaMemcpyHostToDevice, st));
-  const TickSlot* d_act = reinterpret_cast<const TickSlot*>(din + o_act);
-  const int2* d_rows = reinterpret_cast<const int2*>(din + o_rows);
+  if (!vad_mode(h) && (h->emb.ensure((size_t)B * K * D * 4) || h->maps.ensure((size_t)B * K * 4) ||
+                       h->prep.ensure(cluster_prep_floats(B, K) * 4 + 16) || h->prep_d.ensure(cluster_prep_doubles(B, K) * 8 + 16)))
+    return DG_ECUDA;
+  TickIn in;
   int rc;
-  // audio in: the staged samples to their rings, then the batch [B, S], windows grouped by slot
-  if ((rc = launch_ring_scatter(reinterpret_cast<const float*>(din), reinterpret_cast<const RingPiece*>(din + o_pieces), np,
-                                h->book.C, h->rings.as<float>(), st)))
-    return rc;
-  if (!mixed) {
-    if ((rc = launch_ring_gather(h->rings.as<float>(), h->book.C, d_act, d_rows, reinterpret_cast<const long long*>(din + o_start),
-                                 S, B, h->wav.as<float>(), st)))
-      return rc;
-  } else {
-    if (n16 && (rc = launch_ring_gather(h->rings.as<float>(), h->book.C, d_act, reinterpret_cast<const int2*>(din + o_rows16),
-                                        reinterpret_cast<const long long*>(din + o_start16), S, n16, h->wav.as<float>(), st)))
-      return rc;
-    // per declared rate: the new 16 kHz frames of its streams, then its windows
-    for (size_t i = 1; i < h->book.rates.size(); i++) {
-      const RateGeom& r = h->book.rates[i];
-      const int i0 = tp.item_off[i - 1], i1 = tp.item_off[i], w0 = tp.row_off[i - 1], w1 = tp.row_off[i];
-      long long max_count = 0;
-      for (int k = i0; k < i1; k++) max_count = std::max<long long>(max_count, tp.items[k].count);
-      const float* W = r.rs->taps.as<float>();
-      if ((rc = launch_resample_frames(h->rings.as<float>(), h->book.C, reinterpret_cast<const RsFrames*>(din + o_items) + i0,
-                                       i1 - i0, max_count, W, r.g, h->yrings.as<float>(), h->Y, r.Q, st)) ||
-          (rc = launch_resample_gather(h->rings.as<float>(), h->book.C, h->yrings.as<float>(), h->Y, r.Q,
-                                       reinterpret_cast<const RsRow*>(din + o_rs) + w0, w1 - w0, r.r_lo, r.r_hi, W, r.g, r.S, S,
-                                       h->wav.as<float>(), st)))
-        return rc;
-    }
-  }
-  DG_CUDA(cudaEventRecord(h->e_start, st));
-  // networks: sub-batches of at most 256 windows on alternating scratch lanes (the workspace of a 256-window step); a lane is
-  // reused once the sub-batch before on it is past its embeddings
-  for (int r0 = 0, j = 0; r0 < B; r0 += 256, j++) {
-    const int nb = std::min(256, B - r0), lane = j & 1;
-    for (cudaStream_t s : {(cudaStream_t)h->net.s_seg[lane], (cudaStream_t)h->net.s_emb})
-      DG_CUDA(cudaStreamWaitEvent(s, h->e_lane_done[lane], 0));
-    if ((rc = pipeline_nets(&h->net, h->wav.as<float>() + (size_t)r0 * S, S, {nb, F, K}, h->seg.as<float>() + (size_t)r0 * F * K,
-                            h->emb.as<float>() + (size_t)r0 * K * D, h->e_start, lane, 0)))
-      return rc;
-    DG_CUDA(cudaEventRecord(h->e_lane_done[lane], h->net.s_emb));
-  }
-  DG_CUDA(cudaStreamWaitEvent(st, h->net.e_emb, 0));
-  // clustering: state `slot` over that slot's rows (chunk offsets by slot), cosine
-  ClusterParams p{};
-  p.M = M;
-  p.D = D;
-  p.metric = 0;
-  if ((rc = launch_cluster_sweep(p, reinterpret_cast<const double*>(din + o_trials), 1,
-                                 reinterpret_cast<const int2*>(din + o_states), n_act, reinterpret_cast<const int*>(din + o_off),
-                                 h->seg.as<float>(), h->emb.as<float>(), B, F, K, h->centers.as<double>(), h->active.as<int>(),
-                                 h->init.as<int>(), h->prep.as<float>(), h->prep_d.as<double>(), h->maps.as<int32_t>(), st)))
-    return rc;
-  // post-path with each slot's history, then the histories move on
-  DG_CUDA(cudaMemsetAsync(h->total.p, 0, 4, st));
-  if ((rc = launch_post_slots(h->seg.as<float>(), h->maps.as<int32_t>(), h->hist_seg.as<float>(), h->hist_map.as<int32_t>(),
-                              d_act, d_rows, h->slots, B, F, K, M, h->nw, reinterpret_cast<const int32_t*>(din + o_plan),
-                              stride, h->hamming.as<double>(), h->tau, h->header.as<int32_t>(), h->turns.as<uint32_t>(),
-                              turn_cap, h->total.as<unsigned int>(), st)) ||
-      (rc = launch_post_slots_history(h->seg.as<float>(), h->maps.as<int32_t>(), h->hist_seg.as<float>(),
-                                      h->hist_map.as<int32_t>(), d_act, n_act, h->slots, F, K, h->nw, st)))
+  if ((rc = tick_audio_in(h, tp, plan_host, in)) ||
+      (rc = vad_mode(h) ? tick_vad(h, tp, in, turn_cap) : tick_diarize(h, tp, in, turn_cap)))
     return rc;
   if (seg_dev) DG_CUDA(cudaMemcpyAsync(seg_dev, h->seg.p, (size_t)B * F * K * 4, cudaMemcpyDeviceToDevice, st));
   if (emb_dev) DG_CUDA(cudaMemcpyAsync(emb_dev, h->emb.p, (size_t)B * K * D * 4, cudaMemcpyDeviceToDevice, st));

@@ -316,6 +316,13 @@ int launch_vad_curve(const float* seg, int N, int F, int K, const int32_t* plan,
                      const long long* curve_off, double* curve, cudaStream_t st);
 int launch_vad_binarize(const double* curve, const long long* curve_off, int N, int T, const double* taus, int32_t* header,
                         uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st);
+// vad.cu -- many live VAD streams (dg_multi): chunks grouped by slot as launch_post_slots, one speech curve per chunk, each
+// slot's history of max curves hist_vad [2][slots][nw - 1][F]
+int launch_vad_slots(const float* seg, const float* hist_vad, const TickSlot* act, const int2* rows, int slots, int B, int F,
+                     int K, int nw, const int32_t* plan, int plan_stride, const double* hamming, double tau, int32_t* header,
+                     uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st);
+int launch_vad_slots_history(const float* seg, float* hist_vad, const TickSlot* act, int n_act, int slots, int F, int K, int nw,
+                             cudaStream_t st);
 // resample.cu -- polyphase sinc resampling (torchaudio's defaults): reduced ratio o / n, half-width w, T = 2w + o taps per phase
 struct RsGeom {
   int o, n, w, T;

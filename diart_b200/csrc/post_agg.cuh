@@ -1,9 +1,20 @@
 // The per-frame Hamming aggregation of the device post-path (DelayedAggregation, reference aggregation.py:73-92,120-218),
-// shared by post_kernel (post.cu) and the speech curve of the VAD sweep (vad.cu).
+// shared by post_kernel (post.cu) and the speech curves of vad.cu.
 #pragma once
 #include "dg_common.cuh"
 
 namespace dg {
+
+// The speech score of one frame, s [K] (reference vad.py:145-148, torch.amax over the local speakers): the max in float32, and
+// a NaN, once taken, is never replaced (x > NaN is false), as torch propagates it.
+__device__ __forceinline__ float speaker_max(const float* s, int K) {
+  float m = s[0];
+  for (int k = 1; k < K; k++) {
+    const float x = s[k];
+    m = (x > m || isnan(x)) ? x : m;
+  }
+  return m;
+}
 
 // Output frame fo of a chunk whose plan row is pl ([0] nb, [1] nf, [2] first_nf, [3] first_lo, [4 ..] lo per buffer, see
 // post.cu), nfo = first_nf > 0 ? first_nf : nf.  val(j, idx) is the score of buffer j (oldest first) at frame idx, as a double.

@@ -9,6 +9,13 @@
 //                  frame's float64 value written at the chunk's offset in the curve
 //   vad_binarize   one warp per (chunk, trial): curve > tau[t], run-length encoded into post_kernel's header
 //                  {offset, count, frames, 0} and packed turns (0 << 20 | on << 10 | off), all trials sharing one counter
+//
+// Many live VAD streams (dg_multi in VAD mode) use the same two bodies, per tick and per stream:
+//
+//   vad_slots          one CTA per chunk of the tick: its speech curve (max over the local speakers of this tick's scores or
+//                      the slot's history of max curves, aggregated as vad_curve aggregates) compared with tau, run-length
+//                      encoded as vad_binarize encodes it
+//   vad_slots_history  the last nw - 1 max curves of every slot of the tick into the other copy of its history
 #include "dg_common.cuh"
 #include "post_agg.cuh"
 
@@ -17,6 +24,7 @@ namespace dg {
 constexpr unsigned VAD_FULL = 0xffffffffu;
 constexpr int VAD_CURVE_THREADS = 64;
 constexpr int VAD_BIN_THREADS = 256;
+constexpr int VAD_SLOTS_THREADS = 64;
 
 // plan [N][plan_stride] as post_kernel's, without history: chunk c aggregates chunks c - (nb - 1) .. c
 __global__ void __launch_bounds__(VAD_CURVE_THREADS)
@@ -30,37 +38,25 @@ vad_curve_kernel(const float* __restrict__ seg /*[N][F][K]*/, int F, int K, cons
   double* out = curve + curve_off[c];
   for (int fo = threadIdx.x; fo < nfo; fo += VAD_CURVE_THREADS)
     out[fo] = post_frame(pl, nb, nf, nfo, first_lo, F, hamming, fo, [&](int j, int idx) {
-      const float* s = seg + ((size_t)(c - (nb - 1) + j) * F + idx) * K;
-      float m = s[0];
-      for (int k = 1; k < K; k++) {
-        const float x = s[k];
-        m = (x > m || isnan(x)) ? x : m;      // a NaN, once taken, is never replaced: x > NaN is false
-      }
-      return (double)m;
+      return (double)speaker_max(seg + ((size_t)(c - (nb - 1) + j) * F + idx) * K, K);
     });
 }
 
-// warp (c, t): chunk c of the N, trial t of the T.  Frames 0 .. nfo are read 32 at a time with frame nfo inactive, so that a
-// turn still open at the end closes there; a turn's off frame is the lane whose frame is inactive after an active one, its on
-// frame the last start before it.
-__global__ void __launch_bounds__(VAD_BIN_THREADS)
-vad_binarize_kernel(const double* __restrict__ curve, const long long* __restrict__ curve_off /*[N + 1]*/, int N, int T,
-                    const double* __restrict__ taus /*[T]*/, int32_t* __restrict__ header /*[T][N][4]*/,
-                    uint32_t* __restrict__ turns, int turn_cap, unsigned int* __restrict__ total) {
-  const long long w = ((long long)blockIdx.x * VAD_BIN_THREADS + threadIdx.x) >> 5;
+// One warp run-length encodes the frames 0 .. nfo - 1 of a chunk into its header row hd {offset, count, frames, 0} and its
+// packed turns (0 << 20 | on << 10 | off), placed with one atomicAdd on `total`.  word(f0) is the ballot of the active frames
+// f0 .. f0 + 31 (none at or beyond nfo), read 32 at a time up to frame nfo, which is inactive, so that a turn still open at
+// the end closes there; a turn's off frame is the lane whose frame is inactive after an active one, its on frame the last
+// start before it.
+template <class Word>
+__device__ __forceinline__ void warp_turns(int nfo, Word word, int32_t* __restrict__ hd, uint32_t* __restrict__ turns,
+                                           int turn_cap, unsigned int* __restrict__ total) {
   const int lane = threadIdx.x & 31;
-  if (w >= (long long)N * T) return;   // the whole warp
-  const int t = (int)(w / N), c = (int)(w - (long long)t * N);
-  const double tau = taus[t];
-  const double* v = curve + curve_off[c];
-  const int nfo = (int)(curve_off[c + 1] - curve_off[c]);
   const unsigned below = (1u << lane) - 1u;
   // pass 1: the number of turns
   int n = 0;
   unsigned carry = 0;   // frame f0 - 1 active
   for (int f0 = 0; f0 <= nfo; f0 += 32) {
-    const int f = f0 + lane;
-    const unsigned act = __ballot_sync(VAD_FULL, f < nfo && v[f] > tau);
+    const unsigned act = word(f0);
     n += __popc(act & ~((act << 1) | carry));
     carry = act >> 31;
   }
@@ -68,7 +64,6 @@ vad_binarize_kernel(const double* __restrict__ curve, const long long* __restric
   if (lane == 0 && n > 0) base = atomicAdd(total, (unsigned)n);
   base = __shfl_sync(VAD_FULL, base, 0);
   if (lane == 0) {
-    int32_t* hd = header + ((size_t)t * N + c) * 4;
     hd[0] = (int32_t)base;
     hd[1] = n;
     hd[2] = nfo;
@@ -80,7 +75,7 @@ vad_binarize_kernel(const double* __restrict__ curve, const long long* __restric
   carry = 0;
   for (int f0 = 0; f0 <= nfo; f0 += 32) {
     const int f = f0 + lane;
-    const unsigned act = __ballot_sync(VAD_FULL, f < nfo && v[f] > tau);
+    const unsigned act = word(f0);
     const unsigned prev = (act << 1) | carry;
     const unsigned starts = act & ~prev, ends = ~act & prev;
     if ((ends >> lane) & 1u) {
@@ -93,6 +88,76 @@ vad_binarize_kernel(const double* __restrict__ curve, const long long* __restric
     if (starts) on = f0 + 31 - __clz(starts);
     carry = act >> 31;
   }
+}
+
+// warp (c, t): chunk c of the N, trial t of the T
+__global__ void __launch_bounds__(VAD_BIN_THREADS)
+vad_binarize_kernel(const double* __restrict__ curve, const long long* __restrict__ curve_off /*[N + 1]*/, int N, int T,
+                    const double* __restrict__ taus /*[T]*/, int32_t* __restrict__ header /*[T][N][4]*/,
+                    uint32_t* __restrict__ turns, int turn_cap, unsigned int* __restrict__ total) {
+  const long long w = ((long long)blockIdx.x * VAD_BIN_THREADS + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (w >= (long long)N * T) return;   // the whole warp
+  const int t = (int)(w / N), c = (int)(w - (long long)t * N);
+  const double tau = taus[t];
+  const double* v = curve + curve_off[c];
+  const int nfo = (int)(curve_off[c + 1] - curve_off[c]);
+  warp_turns(nfo, [&](int f0) {
+    const int f = f0 + lane;
+    return __ballot_sync(VAD_FULL, f < nfo && v[f] > tau);
+  }, header + ((size_t)t * N + c) * 4, turns, turn_cap, total);
+}
+
+// Many live streams (dg_multi in VAD mode), one CTA per chunk of the tick: chunk c is window rows[c].y of slot entry
+// act[rows[c].x], as in post_slots_kernel (post.cu).  Buffer j of its plan row is a row of this tick's scores seg [B][F][K],
+// max over the K local speakers, or an entry of the slot's history hist_vad [2][slots][nw - 1][F] (copy `cur`, n_hist entries,
+// oldest first), which holds such max curves already.  Each output frame is post_chunk's value with one speaker and the
+// identity map -- the same float64 expression in the same order -- compared with `> tau`; the two warps ballot 32 frames at a
+// time into `bits`, then warp 0 run-length encodes them.
+__global__ void __launch_bounds__(VAD_SLOTS_THREADS)
+vad_slots_kernel(const float* __restrict__ seg, const float* __restrict__ hist_vad, const TickSlot* __restrict__ act,
+                 const int2* __restrict__ rows, int slots, int F, int K, int nw, const int32_t* __restrict__ plan,
+                 int plan_stride, const double* __restrict__ hamming, double tau, int32_t* __restrict__ header,
+                 uint32_t* __restrict__ turns, int turn_cap, unsigned int* __restrict__ total) {
+  __shared__ unsigned bits[(1024 + 32) / 32];   // frames 0 .. nfo <= F + 1 <= 1024
+  const int c = blockIdx.x;
+  const int2 r = rows[c];
+  const TickSlot ts = act[r.x];
+  const int32_t* pl = plan + (size_t)c * plan_stride;
+  const int nb = pl[0], nf = pl[1], first_nf = pl[2], first_lo = pl[3];
+  const int nfo = first_nf > 0 ? first_nf : nf;
+  const size_t h0 = ((size_t)ts.cur * slots + ts.slot) * (nw - 1) + ts.n_hist;   // one past the slot's newest history entry
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int q = warp; q * 32 <= nfo; q += VAD_SLOTS_THREADS / 32) {
+    const int fo = q * 32 + lane;
+    bool on = false;
+    if (fo < nfo)
+      on = post_frame(pl, nb, nf, nfo, first_lo, F, hamming, fo, [&](int j, int idx) {
+             const int v = r.y - (nb - 1) + j;     // virtual chunk of the slot; v < 0 lives in its history
+             return (double)(v >= 0 ? speaker_max(seg + ((size_t)(ts.row0 + v) * F + idx) * K, K)
+                                    : hist_vad[(h0 + v) * F + idx]);
+           }) > tau;
+    const unsigned word = __ballot_sync(VAD_FULL, on);
+    if (lane == 0) bits[q] = word;
+  }
+  __syncthreads();
+  if (warp == 0) warp_turns(nfo, [&](int f0) { return bits[f0 >> 5]; }, header + (size_t)c * 4, turns, turn_cap, total);
+}
+
+// History update of the VAD slots: CTA (a, i) writes entry i of slot act[a]'s other copy, the last keep = min(nw - 1, n_hist +
+// n) chunks of (its history + its n chunks of this tick) as max curves [F].  The host then flips `cur` and sets n_hist = keep.
+__global__ void __launch_bounds__(256)
+vad_slots_history_kernel(const float* __restrict__ seg, float* hist_vad, const TickSlot* __restrict__ act, int slots, int F,
+                         int K, int nw) {
+  const TickSlot ts = act[blockIdx.x];
+  const int i = blockIdx.y;
+  const int keep = min(nw - 1, ts.n_hist + ts.n);
+  if (i >= keep) return;
+  const int v = ts.n - keep + i;                    // virtual chunk: v >= 0 is this tick's, v < 0 the history's
+  const size_t src = ((size_t)ts.cur * slots + ts.slot) * (nw - 1) + ts.n_hist;
+  const size_t dst = ((size_t)(ts.cur ^ 1) * slots + ts.slot) * (nw - 1) + i;
+  for (int f = threadIdx.x; f < F; f += blockDim.x)
+    hist_vad[dst * F + f] = v >= 0 ? speaker_max(seg + ((size_t)(ts.row0 + v) * F + f) * K, K) : hist_vad[(src + v) * F + f];
 }
 
 int launch_vad_curve(const float* seg, int N, int F, int K, const int32_t* plan, int plan_stride, const double* hamming,
@@ -108,6 +173,29 @@ int launch_vad_binarize(const double* curve, const long long* curve_off, int N, 
   ProfScope _ps("vad_binarize", st);
   const unsigned blocks = (unsigned)(((long long)N * T * 32 + VAD_BIN_THREADS - 1) / VAD_BIN_THREADS);
   vad_binarize_kernel<<<blocks, VAD_BIN_THREADS, 0, st>>>(curve, curve_off, N, T, taus, header, turns, turn_cap, total);
+  DG_LAUNCHED();
+  return 0;
+}
+
+int launch_vad_slots(const float* seg, const float* hist_vad, const TickSlot* act, const int2* rows, int slots, int B, int F,
+                     int K, int nw, const int32_t* plan, int plan_stride, const double* hamming, double tau, int32_t* header,
+                     uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st) {
+  ProfScope _ps("vad_slots", st);
+  if (F > 1023) {
+    set_error("vad_slots: at most 1023 frames");
+    return -1;
+  }
+  vad_slots_kernel<<<B, VAD_SLOTS_THREADS, 0, st>>>(seg, hist_vad, act, rows, slots, F, K, nw, plan, plan_stride, hamming, tau,
+                                                    header, turns, turn_cap, total);
+  DG_LAUNCHED();
+  return 0;
+}
+
+int launch_vad_slots_history(const float* seg, float* hist_vad, const TickSlot* act, int n_act, int slots, int F, int K, int nw,
+                             cudaStream_t st) {
+  ProfScope _ps("vad_slots_history", st);
+  if (n_act < 1 || nw < 2) return 0;
+  vad_slots_history_kernel<<<dim3(n_act, nw - 1), 256, 0, st>>>(seg, hist_vad, act, slots, F, K, nw);
   DG_LAUNCHED();
   return 0;
 }

@@ -14,7 +14,11 @@ are the dedicated pipeline's.  Only the turns come back (the reference's serve h
 Streams at other source rates (``source_sample_rates``; ``open(sample_rate=44100)``) are windowed at their own rate, as
 ``rearrange_audio_stream(duration, step, rate)`` windows them, and every window is resampled on the device with the bits of
 ``DeviceResample`` on that window (the reference's ``blocks.Resample``): each 16 kHz frame inside the windows is computed once
-per stream, only the frames at each window's edges once per window."""
+per stream, only the frames at each window's edges once per window.
+
+``MultiStreamVoiceActivityDetection`` serves the reference's ``VoiceActivityDetection`` the same way (``dg_multi_create_vad``):
+the same audio path, the segmentation network alone, and every stream's speech curve aggregated and binarised on the device.
+Its results carry no caveat: they are bit for bit those of a dedicated ``VoiceActivityDetection``."""
 from __future__ import annotations
 
 import ctypes as C
@@ -28,6 +32,7 @@ from . import _lib
 from . import models as m
 from .blocks.diarization import SpeakerDiarizationConfig
 from .blocks.post import chunk_annotations, crop_plan
+from .blocks.vad import VoiceActivityDetectionConfig, speech_annotations
 from .core import Annotation
 from .operators import DeviceResample
 
@@ -87,45 +92,32 @@ def source_geometry(rate: int, sample_rate: int, duration: float, step: float) -
     return chunk, hop, (chunk * (1 / rate)) / window
 
 
-class MultiStreamDiarization:
-    """Up to ``max_streams`` live streams diarized on one device with one ``SpeakerDiarizationConfig``:
-    ``open(shift, sample_rate) -> sid``, ``push(sid, block)``, ``close(sid)``, and ``step() -> {sid: [Annotation, ...]}`` with
-    one ``Annotation`` per window consumed in the tick, in order -- what ``SpeakerDiarization(config)`` returns for that
-    stream's windows fed one per call, with its ``timestamp_shift`` set to ``shift``, up to the embedding caveat of the module
-    docstring.  A stream is at ``config.sample_rate`` or at one of ``source_sample_rates`` (declared here, see
-    ``source_geometry``); its blocks are at its own rate, and its windows are resampled as ``DeviceResample`` resamples them.
-    Needs the native models (``B200*Loader``)."""
+class _MultiStreamServer:
+    """What the multi-stream servers share: the ``dg_multi`` handle a subclass creates (``_create``), the declared source
+    rates, the host mirror of the slots (``open`` / ``close`` / ``push`` / ``available``) and the planning of a tick."""
 
-    def __init__(self, config: SpeakerDiarizationConfig, max_streams: int, max_windows_per_stream: int = 4,
-                 source_sample_rates=()):
+    _needs = ""   # what the subclass raises when a model is not native
+
+    def __init__(self, config, max_streams: int, max_windows_per_stream: int, source_sample_rates, models):
         self._h: Optional[C.c_void_p] = None
         self.config = config
         msg = f"Latency should be in the range [{config.step}, {config.duration}]"
         assert config.step <= config.latency <= config.duration, msg
-        for lazy in (config.segmentation, config.embedding):
+        for lazy in models:
             lazy.eval()
             lazy.to(config.device)
-        seg_net, emb_net = config.segmentation.model, config.embedding.model
-        if not isinstance(seg_net, m.B200PyanNet) or not isinstance(emb_net, m.B200XVectorSincNet):
-            raise _lib.DiartB200Error("MultiStreamDiarization needs the native segmentation and embedding models")
+        seg_net = config.segmentation.model
+        if not isinstance(seg_net, m.B200PyanNet):
+            raise _lib.DiartB200Error(self._needs)
         sr = config.sample_rate
         self.window_samples = int(np.rint(config.duration * sr))
         self.step_samples = int(round(config.step * sr))
         self.max_streams, self.max_windows_per_stream = int(max_streams), int(max_windows_per_stream)
         self.F, self.K = seg_net.dims(self.window_samples)
-        self.D = emb_net.dims(self.window_samples)[1]
         self.nw = int(round(config.latency / config.step))      # DelayedAggregation.num_overlapping_windows
-        self.labels = [f"speaker{g}" for g in range(config.max_speakers)]
         self.device = seg_net.device
         ham = np.ascontiguousarray(np.hamming(self.F), dtype=np.float64)
-        h = C.c_void_p()
-        _lib.check(_lib.lib().dg_multi_create(seg_net.handle, emb_net.handle, self.window_samples, self.step_samples,
-                                              self.max_streams, self.max_windows_per_stream, int(config.max_speakers),
-                                              float(config.tau_active), float(config.rho_update), float(config.delta_new),
-                                              float(config.gamma), float(config.beta),
-                                              int(config.normalize_embedding_weights), self.nw, ham.ctypes.data,
-                                              C.byref(h)))
-        self._h = h
+        self._h = self._create(ham)
         # rate -> (rate id, chunk samples, step samples, window resolution); one DeviceResample (tap table) per declared rate
         self.rates = {sr: (-1, self.window_samples, self.step_samples, 1 / sr)}
         self._resamplers: Dict[int, DeviceResample] = {}
@@ -147,6 +139,17 @@ class MultiStreamDiarization:
         self._hop = np.full(self.max_streams, self.step_samples, dtype=np.int64)
         self._res = np.full(self.max_streams, 1 / sr, dtype=np.float64)
         self._turns = np.empty(1 << 16, dtype=np.uint32)
+
+    def _create(self, hamming: np.ndarray) -> C.c_void_p:
+        """the handle (dg_multi_create*)"""
+        raise NotImplementedError
+
+    def _outputs(self, B: int) -> tuple:
+        """the device tensors a tick with ``outputs`` fills: (scores, embeddings, maps), None where the handle has none"""
+        raise NotImplementedError
+
+    def _annotations(self, header, turns, n_turns, out_start, out_res, shifts) -> List[Annotation]:
+        raise NotImplementedError
 
     def __del__(self):
         try:
@@ -207,8 +210,8 @@ class MultiStreamDiarization:
         return self._step()[0]
 
     def _step(self, outputs: bool = False) -> Tuple[Dict[int, List[Annotation]], Optional[tuple]]:
-        """``step``; ``outputs``: also the tick's scores (B, F, K), embeddings (B, K, D) and maps (B, K) as device tensors,
-        rows grouped by stream in slot order"""
+        """``step``; ``outputs``: also the tick's device outputs (``_outputs``, the handle's ones only), rows grouped by
+        stream in slot order"""
         counts = np.where(self._open, np.minimum(available_windows(self._pushed, self._emitted, self._chunk, self._hop),
                                                  self.max_windows_per_stream), 0)
         sids = np.flatnonzero(counts)
@@ -221,24 +224,93 @@ class MultiStreamDiarization:
                                              cfg.latency, np.repeat(self._res[sids], n))
         plan = np.ascontiguousarray(plan)
         header = np.empty((B, 4), dtype=np.int32)
-        need = B * cfg.max_speakers * ((self.F + 2) // 2)
+        need = B * self._speakers * ((self.F + 2) // 2)
         if len(self._turns) < need:
             self._turns = np.empty(need, dtype=np.uint32)
         got = np.empty(self.max_streams, dtype=np.int32)
         n_turns = C.c_int()
-        outs = None
-        if outputs and B:
-            outs = (torch.empty((B, self.F, self.K), device=self.device), torch.empty((B, self.K, self.D), device=self.device),
-                    torch.empty((B, self.K), device=self.device, dtype=torch.int32))
+        outs = self._outputs(B) if outputs and B else (None, None, None)
         with torch.cuda.device(self.device):
             _lib.check(_lib.lib().dg_multi_step(self._h, plan.ctypes.data, B, got.ctypes.data, header.ctypes.data,
                                                 self._turns.ctypes.data, len(self._turns), C.byref(n_turns),
-                                                *([t.data_ptr() for t in outs] if outs else [None, None, None])))
+                                                *[_lib.ptr(t) for t in outs]))
         if not np.array_equal(got, counts):
             raise _lib.DiartB200Error("stream bookkeeping out of step with the device handle")
         self._emitted += counts
+        outs = tuple(t for t in outs if t is not None) or None
         if B == 0:
             return {}, outs
-        anns = chunk_annotations(header, self._turns, n_turns.value, out_start, out_res, self.labels,
-                                 np.repeat(self._shift[sids], n))
+        anns = self._annotations(header, self._turns, n_turns.value, out_start, out_res, np.repeat(self._shift[sids], n))
         return {int(s): anns[r:r + k] for s, r, k in zip(sids.tolist(), row0.tolist(), n.tolist())}, outs
+
+
+class MultiStreamDiarization(_MultiStreamServer):
+    """Up to ``max_streams`` live streams diarized on one device with one ``SpeakerDiarizationConfig``:
+    ``open(shift, sample_rate) -> sid``, ``push(sid, block)``, ``close(sid)``, and ``step() -> {sid: [Annotation, ...]}`` with
+    one ``Annotation`` per window consumed in the tick, in order -- what ``SpeakerDiarization(config)`` returns for that
+    stream's windows fed one per call, with its ``timestamp_shift`` set to ``shift``, up to the embedding caveat of the module
+    docstring.  A stream is at ``config.sample_rate`` or at one of ``source_sample_rates`` (declared here, see
+    ``source_geometry``); its blocks are at its own rate, and its windows are resampled as ``DeviceResample`` resamples them.
+    Needs the native models (``B200*Loader``).  ``_step(outputs=True)`` also returns the tick's scores (B, F, K), embeddings
+    (B, K, D) and maps (B, K) as device tensors."""
+
+    _needs = "MultiStreamDiarization needs the native segmentation and embedding models"
+
+    def __init__(self, config: SpeakerDiarizationConfig, max_streams: int, max_windows_per_stream: int = 4,
+                 source_sample_rates=()):
+        self._speakers = int(config.max_speakers)
+        self.labels = [f"speaker{g}" for g in range(config.max_speakers)]
+        super().__init__(config, max_streams, max_windows_per_stream, source_sample_rates,
+                         (config.segmentation, config.embedding))
+
+    def _create(self, hamming):
+        config, emb_net = self.config, self.config.embedding.model
+        if not isinstance(emb_net, m.B200XVectorSincNet):
+            raise _lib.DiartB200Error(self._needs)
+        self.D = emb_net.dims(self.window_samples)[1]
+        h = C.c_void_p()
+        _lib.check(_lib.lib().dg_multi_create(config.segmentation.model.handle, emb_net.handle, self.window_samples,
+                                              self.step_samples, self.max_streams, self.max_windows_per_stream,
+                                              int(config.max_speakers), float(config.tau_active), float(config.rho_update),
+                                              float(config.delta_new), float(config.gamma), float(config.beta),
+                                              int(config.normalize_embedding_weights), self.nw, hamming.ctypes.data,
+                                              C.byref(h)))
+        return h
+
+    def _outputs(self, B):
+        return (torch.empty((B, self.F, self.K), device=self.device), torch.empty((B, self.K, self.D), device=self.device),
+                torch.empty((B, self.K), device=self.device, dtype=torch.int32))
+
+    def _annotations(self, header, turns, n_turns, out_start, out_res, shifts):
+        return chunk_annotations(header, turns, n_turns, out_start, out_res, self.labels, shifts)
+
+
+class MultiStreamVoiceActivityDetection(_MultiStreamServer):
+    """Up to ``max_streams`` live streams through the reference's ``VoiceActivityDetection`` on one device, with the interface
+    of ``MultiStreamDiarization``: each window's ``Annotation`` is exactly what ``VoiceActivityDetection(config)`` returns
+    for it when the stream is fed one window per call with ``set_timestamp_shift(shift)``.  A tick runs the segmentation
+    network alone on all of its windows, then every stream's speech curve (max over the local speakers, aggregated over its
+    ``latency / step`` most recent windows) is binarised on the device.  The scores are batch invariant, so a stream's results
+    are bit for bit those of its dedicated pipeline whatever the other streams do.  Needs the native segmentation model
+    (``B200SegmentationLoader``, powerset checkpoints included).  ``_step(outputs=True)`` also returns ``(scores,)``, the
+    tick's scores (B, F, K) as a device tensor."""
+
+    _needs = "MultiStreamVoiceActivityDetection needs the native segmentation model (B200PyanNet)"
+    _speakers = 1
+
+    def __init__(self, config: VoiceActivityDetectionConfig, max_streams: int, max_windows_per_stream: int = 4,
+                 source_sample_rates=()):
+        super().__init__(config, max_streams, max_windows_per_stream, source_sample_rates, (config.segmentation,))
+
+    def _create(self, hamming):
+        h = C.c_void_p()
+        _lib.check(_lib.lib().dg_multi_create_vad(self.config.segmentation.model.handle, self.window_samples,
+                                                  self.step_samples, self.max_streams, self.max_windows_per_stream,
+                                                  float(self.config.tau_active), self.nw, hamming.ctypes.data, C.byref(h)))
+        return h
+
+    def _outputs(self, B):
+        return torch.empty((B, self.F, self.K), device=self.device), None, None
+
+    def _annotations(self, header, turns, n_turns, out_start, out_res, shifts):
+        return speech_annotations(header, turns, n_turns, out_start, out_res, shifts)

@@ -398,6 +398,24 @@ int dg_selftest_multi_frames_host(int slots, int max_wps, int out_chunk, int out
  * refused one (a push beyond the ring capacity, a closed or unknown slot).  rings_host float [slots][C]: written by ticks. */
 int dg_selftest_multi_staging_host(int slots, int C, int n_ops, const int32_t* ops, const float* samples_host, int32_t* result,
                                    float* rings_host);
+/* ---- many live streams of the reference's VoiceActivityDetection (src/diart/blocks/vad.py:139-191: the segmentation
+ *      network, the max over the local speakers, DelayedAggregation(hamming) and Binarize(tau_active), turns labelled
+ *      "speech"), served as dg_multi serves SpeakerDiarization.
+ *      dg_multi_create_vad: a dg_multi without an embedding model or clustering state.  Arguments as dg_multi_create's;
+ *        tau = tau_active.  DG_EINVAL, naming dg_multi_create_vad, allocating and launching nothing, unless chunk and step
+ *        are positive multiples of 4 with step <= chunk, max_streams * max_windows_per_stream <= 65535, 1 <= num_windows
+ *        <= 256, tau is finite, the model has at most 8 local speakers (classes) and the window at most 1023 frames.
+ *      Every other dg_multi_* entry point works on it as on a diarization handle, with these differences.  dg_multi_open*
+ *        resets the slot's rings and aggregation history only.  A tick runs the segmentation network alone (sub-batches of
+ *        at most 256 windows on the model handle's two scratch lanes), then per chunk the speech curve -- the max over the K
+ *        local speakers in float32 (torch.amax: a NaN propagates), aggregated over the stream's latency / step most recent
+ *        chunks in float64 -- compared with > tau: the very arithmetic of dg_post_step with one speaker and the identity map
+ *        on those max curves, so the turns are bit for bit those of a VoiceActivityDetection fed the stream one window per
+ *        call.  header_host and turns_host as dg_multi_step (every turn's speaker is 0); seg_dev receives the tick's scores
+ *        [n_rows, F, K]; emb_dev and map_dev must be null, else DG_EINVAL.
+ *      Memory per slot: its ring(s) as dg_multi_create, and a history of 2 (num_windows - 1) F floats. ---- */
+int dg_multi_create_vad(dg_seg* seg, int chunk_samples, int step_samples, int max_streams, int max_windows_per_stream,
+                        double tau, int num_windows, const double* hamming_host, dg_multi** out);
 
 /* ---- resampling: torchaudio's T.Resample(orig, new) with its defaults (sinc_interp_hann, lowpass_filter_width 6,
  *      rolloff 0.99), what the reference's blocks.Resample applies to every window of a source at another rate (reference

@@ -23,6 +23,7 @@ from __future__ import annotations
 
 import argparse
 import ctypes as C
+import functools
 import json
 import os
 import sys
@@ -41,10 +42,16 @@ from sweep_bench import card, make_config  # noqa: E402
 SR, S, HOP = 16000, 80000, 8000
 
 
+@functools.lru_cache(maxsize=4)
+def recordings(need):
+    """the seeded recordings the streams are cut from (synthesised once per length: seconds each)"""
+    return [synth.synth_audio(need + 64 * HOP, seed=900 + i) for i in range(8)]
+
+
 def stream_audio(n_streams, ticks):
     """per stream: S + (ticks - 1) HOP samples, slices of a few seeded recordings at per-stream offsets"""
     need = S + (ticks - 1) * HOP
-    base = [synth.synth_audio(need + 64 * HOP, seed=900 + i) for i in range(8)]
+    base = recordings(need)
     return [base[i % 8][(i // 8) % 64 * HOP:][:need] for i in range(n_streams)]
 
 
@@ -52,41 +59,40 @@ def block(a, t):
     return a[:S] if t == 0 else a[S + (t - 1) * HOP:S + t * HOP]
 
 
-class Timed(serve.MultiStreamDiarization):
-    """step() with the host clock around its phases (the same code path, instrumented)"""
+def timed_step(srv, phases):
+    """srv.step() with the host clock around its phases (the same code path, instrumented); any multi-stream server"""
+    t0 = time.perf_counter()
+    plan_rows, annotations = serve.plan_rows, srv._annotations
+    marks = {}
 
-    def timed_step(self, phases):
-        t0 = time.perf_counter()
-        plan_rows, chunk_annotations = serve.plan_rows, serve.chunk_annotations
-        marks = {}
+    def plan(*a, **k):
+        r = plan_rows(*a, **k)
+        marks["plan"] = time.perf_counter()
+        return r
 
-        def plan(*a, **k):
-            r = plan_rows(*a, **k)
-            marks["plan"] = time.perf_counter()
-            return r
+    def ann(*a, **k):
+        marks["ann0"] = time.perf_counter()
+        return annotations(*a, **k)
 
-        def ann(*a, **k):
-            marks["ann0"] = time.perf_counter()
-            return chunk_annotations(*a, **k)
-
-        serve.plan_rows, serve.chunk_annotations = plan, ann
-        try:
-            out = self.step()
-        finally:
-            serve.plan_rows, serve.chunk_annotations = plan_rows, chunk_annotations
-        t1 = time.perf_counter()
-        phases["plan_ms"] += (marks["plan"] - t0) * 1e3
-        phases["call_ms"] += (marks["ann0"] - marks["plan"]) * 1e3
-        phases["annotations_ms"] += (t1 - marks["ann0"]) * 1e3
-        ms = C.c_float()
-        _lib.check(_lib.lib().dg_multi_last_step_ms(self.handle, C.byref(ms)))
-        phases["device_ms"] += ms.value
-        return out
+    serve.plan_rows, srv._annotations = plan, ann
+    try:
+        out = srv.step()
+    finally:
+        serve.plan_rows = plan_rows
+        del srv._annotations
+    t1 = time.perf_counter()
+    phases["plan_ms"] += (marks["plan"] - t0) * 1e3
+    phases["call_ms"] += (marks["ann0"] - marks["plan"]) * 1e3
+    phases["annotations_ms"] += (t1 - marks["ann0"]) * 1e3
+    ms = C.c_float()
+    _lib.check(_lib.lib().dg_multi_last_step_ms(srv.handle, C.byref(ms)))
+    phases["device_ms"] += ms.value
+    return out
 
 
-def run_server(config, n, ticks, warmup):
+def run_server(config, n, ticks, warmup, server=serve.MultiStreamDiarization):
     audios = stream_audio(n, ticks + warmup)
-    srv = Timed(config, max_streams=n, max_windows_per_stream=1)
+    srv = server(config, max_streams=n, max_windows_per_stream=1)
     sids = [srv.open() for _ in range(n)]
     phases = {k: 0.0 for k in ("wall_ms", "push_ms", "plan_ms", "call_ms", "device_ms", "annotations_ms")}
     for t in range(warmup + ticks):
@@ -96,7 +102,7 @@ def run_server(config, n, ticks, warmup):
         for sid, a in zip(sids, audios):
             srv.push(sid, block(a, t))
         t1 = time.perf_counter()
-        out = srv.timed_step(phases)
+        out = timed_step(srv, phases)
         t2 = time.perf_counter()
         assert sum(len(v) for v in out.values()) == n
         phases["push_ms"] += (t1 - t0) * 1e3
