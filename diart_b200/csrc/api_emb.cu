@@ -459,7 +459,7 @@ static int build_tables(dg_emb* h, int F, int T, cudaStream_t st) {
 // `defer_last`: stop before TDNN5 (its operand planes are left in h->t4h / t4l) -- the caller runs it fused with the pooling.
 // `prep`: waveform statistics + planes the caller computed (or null)
 int emb_trunk(dg_emb* h, const float* wav, int U, const Geom& g, cudaStream_t st, int* T_out, bool defer_last,
-              const SincPrep* prep) {
+              const SincPrep* prep, int stop_after) {
   int rc;
   if (h->variant == 1) return resnet_trunk(h, wav, U, g.S, st, T_out);
   if ((rc = run_sincnet(h->sw, h->work, wav, U, g, st, prep))) return rc;
@@ -481,7 +481,7 @@ int emb_trunk(dg_emb* h, const float* wav, int U, const Geom& g, cudaStream_t st
   void* oh[2] = {h->aH.p, h->bH.p};
   void* ol[2] = {h->aL.p, h->bL.p};
   static const char* kTags[5] = {"tdnn1", "tdnn2", "tdnn3", "tdnn4", "tdnn5"};
-  for (int L = 0; L < 5; L++) {
+  for (int L = 0; L < 5 && stop_after >= 0; L++) {
     if (L == 4 && defer_last) {
       h->t4h = ih;
       h->t4l = il;
@@ -501,6 +501,7 @@ int emb_trunk(dg_emb* h, const float* wav, int U, const Geom& g, cudaStream_t st
     ih = oh[L & 1]; il = ol[L & 1];
     cin = TD_OUT[L];
     T -= (TD_K[L] - 1) * TD_DIL[L];
+    if (L == stop_after) break;
   }
   *T_out = T;
   return 0;
@@ -590,6 +591,52 @@ extern "C" int dg_emb_forward(dg_emb* h, const float* wav, const float* weights,
   const bool fuse = weights && pool_fusable(h, K, g);
   if ((rc = emb_trunk(h, wav, B, g, st, &T, fuse, nullptr))) return rc;
   return emb_tail(h, B, g, weights, F, K, T, fuse, normalize, norm, out, st);
+}
+
+// test hook: the production front end, emb_trunk and emb_tail with a host-side stop point, and one intermediate map copied to
+// the host.  Stages 9 / 11 take the fused TDNN5 + pooling (refused where pool_fusable says no), 10 / 12 the un-fused pooling.
+extern "C" int dg_emb_debug_stage(dg_emb* h, const float* wav_dev, const float* weights_dev, int B, int S, int F, int K, int hop,
+                                  int stage, float* out_host, int64_t cap, int* dims) {
+  if (!h || !wav_dev || !out_host || !dims || B < 1 || S < 3000 || hop < 0 || stage < 0 || stage > 12 ||
+      (stage >= 9 && (!weights_dev || F < 1 || K < 1)) || h->variant != 0) {
+    set_error("dg_emb_debug_stage: bad arguments (need an XVectorSincNet handle, B >= 1, S >= 3000, stage 0..12, weights from stage 9)");
+    return DG_EINVAL;
+  }
+  const Geom g = make_geom(S);
+  const bool fuse = stage == 9 || stage == 11;
+  if (fuse && !pool_fusable(h, K, g)) {
+    set_error("dg_emb_debug_stage: the fused pooling does not run at this K and chunk length");
+    return DG_EINVAL;
+  }
+  DG_CUDA(cudaSetDevice(h->device));
+  const char* who = "dg_emb_debug_stage";
+  cudaStream_t st = nullptr;
+  SincPrep shared;
+  const SincPrep* prep = nullptr;
+  DevBuf out;
+  int rc, T = 0;
+  if (stage >= 9 && out.ensure((size_t)B * K * h->D * 4)) return DG_ECUDA;
+  {
+    LaneUse use(h->guard, h, st);
+    if ((rc = use.rc)) return rc;
+    if (hop > 0) {
+      if ((rc = run_sinc_prep(shared, wav_dev, B, g, st, hop, false))) return rc;
+      prep = &shared;
+    }
+    if ((rc = emb_trunk(h, wav_dev, B, g, st, &T, fuse, prep, stage <= 3 ? -1 : stage <= 7 ? stage - 4 : 99))) return rc;
+    if (stage >= 9 && (rc = emb_tail(h, B, g, weights_dev, F, K, T, fuse, 0, 1.f, out.as<float>(), st))) return rc;
+  }
+  DG_CUDA(cudaDeviceSynchronize());
+  if ((rc = debug_front_paths(prep, g, &dims[3]))) return rc;
+  if (fuse) dims[3] |= DG_DBG_STATS_POOL_FUSED;
+  if (stage <= 3) return debug_copy_front(who, stage, h->work, prep, h->xh.p, h->xl.p, B, g, out_host, cap, dims);
+  if (stage <= 7) {
+    const int L = stage - 4;
+    return debug_copy_map(who, L & 1 ? h->bH.p : h->aH.p, L & 1 ? h->bL.p : h->aL.p, B, g.S2, 512, T, 512, out_host, cap, dims);
+  }
+  if (stage == 8) return debug_copy_map(who, h->t5.p, nullptr, B, g.S2, 1500, T, 1500, out_host, cap, dims);
+  if (stage <= 10) return debug_copy_map(who, h->pooled.p, nullptr, B * K, 1, 3000, 1, 3000, out_host, cap, dims);
+  return debug_copy_map(who, out.p, nullptr, B * K, 1, h->D, 1, h->D, out_host, cap, dims);
 }
 
 extern "C" int dg_emb_forward_rows(dg_emb* h, const float* wav, const float* weights, int N, int S, int F, float* out,

@@ -121,7 +121,7 @@ int run_sinc_prep(SincPrep& p, const float* wav, int B, const Geom& g, cudaStrea
   }
   if ((rc = launch_wave_stats(wav, B, g.S, p.wmean.as<float>(), p.wrstd.as<float>(), st, fast_stats ? p.flag.as<int>() : nullptr)))
     return rc;
-  if (p.hop && (rc = launch_stream_prep(wav, B, g, hop, p.swh.p, p.swl.p, p.flag.as<int>(), st))) return rc;
+  if (p.hop && (rc = launch_stream_prep(wav, p.wrstd.as<float>(), B, g, hop, p.swh.p, p.swl.p, p.flag.as<int>(), st))) return rc;
   return launch_sinc_prep(wav, p.wmean.as<float>(), p.wrstd.as<float>(), B, g, p.wh.p, p.wl.p, st,
                           p.hop ? p.flag.as<int>() : nullptr);
 }
@@ -206,7 +206,68 @@ int run_sincnet(const SincWeights& w, SincWork& k, const float* wav, int B, cons
                                k.sc2.as<float>(), k.sh2.as<float>(), st, 1);
 }
 
+int debug_copy_map(const char* who, const void* hi, const void* lo, int B, int item_rows, int ld, int T, int C, float* out_host,
+                   int64_t cap, int* dims) {
+  dims[0] = B; dims[1] = T; dims[2] = C;
+  if ((int64_t)B * T * C > cap) {
+    set_error(std::string(who) + ": buffer too small");
+    return DG_EINVAL;
+  }
+  const size_t n = (size_t)B * item_rows * ld;
+  std::vector<float> full(n);
+  if (lo) {
+    std::vector<uint16_t> vh(n), vl(n);
+    DG_CUDA(cudaMemcpy(vh.data(), hi, n * 2, cudaMemcpyDeviceToHost));
+    DG_CUDA(cudaMemcpy(vl.data(), lo, n * 2, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < n; i++) full[i] = host_h16_to_f32(vh[i]) + host_h16_to_f32(vl[i]);
+  } else {
+    DG_CUDA(cudaMemcpy(full.data(), hi, n * 4, cudaMemcpyDeviceToHost));
+  }
+  for (int b = 0; b < B; b++)
+    for (int t = 0; t < T; t++)
+      memcpy(out_host + ((size_t)b * T + t) * C, &full[((size_t)b * item_rows + t) * ld], (size_t)C * 4);
+  return DG_OK;
+}
+
+int debug_copy_front(const char* who, int stage, const SincWork& k, const SincPrep* prep, const void* xh, const void* xl, int B,
+                     const Geom& g, float* out_host, int64_t cap, int* dims) {
+  if (stage == 0) return debug_copy_map(who, k.a0h.p, k.a0l.p, B, g.S0, 80, g.T0, 80, out_host, cap, dims);
+  if (stage == 1) return debug_copy_map(who, k.a1h.p, k.a1l.p, B, g.S1, 64, g.T1, 60, out_host, cap, dims);
+  if (stage == 2) return debug_copy_map(who, xh, xl, B, g.S2, 64, g.T2, 60, out_host, cap, dims);
+  const SincPrep& p = prep ? *prep : k.own_prep;
+  dims[0] = 2; dims[1] = B; dims[2] = 1;
+  if (2 * B > cap) {
+    set_error(std::string(who) + ": buffer too small");
+    return DG_EINVAL;
+  }
+  DG_CUDA(cudaMemcpy(out_host, p.wmean.p, (size_t)B * 4, cudaMemcpyDeviceToHost));
+  DG_CUDA(cudaMemcpy(out_host + B, p.wrstd.p, (size_t)B * 4, cudaMemcpyDeviceToHost));
+  return DG_OK;
+}
+
+int debug_front_paths(const SincPrep* prep, const Geom& g, int* paths) {
+  *paths = 0;
+  if (prep && prep->hop) {
+    int flag = 0;
+    DG_CUDA(cudaMemcpy(&flag, prep->flag.p, sizeof(int), cudaMemcpyDeviceToHost));
+    if (flag) *paths |= DG_DBG_STREAM_FORM;
+  }
+  if (gemm_tc_pool3_tile_rows(g.S0) && gemm_tc_pool3_tile_rows(g.S1)) *paths |= DG_DBG_POOL3_FUSED;
+  return DG_OK;
+}
+
 }  // namespace dg
+
+extern "C" int dg_selftest_sinc_filters_host(const float* low_hz, const float* band_hz, float* filters) {
+  if (!low_hz || !band_hz || !filters) {
+    set_error("dg_selftest_sinc_filters_host: null argument");
+    return DG_EINVAL;
+  }
+  std::vector<float> h;
+  sinc_filters(low_hz, band_hz, h);
+  memcpy(filters, h.data(), h.size() * sizeof(float));
+  return DG_OK;
+}
 
 static int seg_prepare(dg_seg* h, const Tensors& t) {
   int rc;
@@ -335,7 +396,7 @@ static int seg_head_final(dg_seg* h, const float* y2, int B, const Geom& g, floa
 }
 
 int seg_forward_lane(dg_seg* h, int lane, const SincPrep* prep, const float* wav, int B, int S, float* seg,
-                     cudaStream_t st) {
+                     cudaStream_t st, int stop_after) {
   DG_CUDA(cudaSetDevice(h->device));
   dg_seg::Scratch& w = h->scr[lane];
   const Geom g = make_geom(S);
@@ -349,7 +410,7 @@ int seg_forward_lane(dg_seg* h, int lane, const SincPrep* prep, const float* wav
   if ((rc = launch_split_ex(w.work.out, M, 64, 64, 64, w.work.out_pool, g.S2, w.work.sc2.as<float>(), w.work.sh2.as<float>(),
                             w.xh.p, w.xl.p, st)))
     return rc;
-  for (int L = 0; L < 4; L++) {
+  for (int L = 0; L < 4 && L <= stop_after; L++) {
     const int cin = L == 0 ? 64 : 256;
     TcGemm t{};
     t.A_hi = w.xh.p; t.A_lo = w.xl.p; t.lda = cin; t.Cin = cin; t.KW = 1; t.dil = 1; t.Mtot = M; t.M = M;
@@ -361,6 +422,7 @@ int seg_forward_lane(dg_seg* h, int lane, const SincPrep* prep, const float* wav
                                    w.xh.p, w.xl.p, st)))
       return rc;
   }
+  if (stop_after < 3) return 0;
   // Linear(256,128) -> leaky -> Linear(128,128) -> leaky on the tensor-core GEMM (identity "BatchNorm")
   TcGemm t{};
   t.A_hi = w.xh.p; t.A_lo = w.xl.p; t.lda = 256; t.Cin = 256; t.KW = 1; t.dil = 1; t.Mtot = M; t.M = M;
@@ -384,6 +446,44 @@ extern "C" int dg_seg_forward(dg_seg* h, const float* wav, int B, int S, float* 
   int rc;
   if ((rc = use.rc) || (rc = seg_forward_lane(h, 0, nullptr, wav, B, S, seg, st))) return rc;
   return use.end();
+}
+
+// test hook: the production forward (run_sinc_prep with the hop hint as dg_pipeline_set_hop gives it, seg_forward_lane) with a
+// host-side stop point, and one intermediate map copied to the host
+extern "C" int dg_seg_debug_stage(dg_seg* h, const float* wav_dev, int B, int S, int hop, int stage, float* out_host, int64_t cap,
+                                  int* dims) {
+  if (!h || !wav_dev || !out_host || !dims || B < 1 || S < 3000 || hop < 0 || stage < 0 || stage > 10 || h->ps_speakers) {
+    set_error("dg_seg_debug_stage: bad arguments (need a multilabel segmentation handle, B >= 1, S >= 3000, stage 0..10)");
+    return DG_EINVAL;
+  }
+  DG_CUDA(cudaSetDevice(h->device));
+  const Geom g = make_geom(S);
+  const char* who = "dg_seg_debug_stage";
+  cudaStream_t st = nullptr;
+  SincPrep shared;
+  const SincPrep* prep = nullptr;
+  DevBuf seg;
+  int rc;
+  if (seg.ensure((size_t)B * g.T2 * h->K * 4)) return DG_ECUDA;
+  {
+    LaneUse use(h->guard[0], h, st);
+    if ((rc = use.rc)) return rc;
+    if (hop > 0) {
+      if ((rc = run_sinc_prep(shared, wav_dev, B, g, st, hop, false))) return rc;
+      prep = &shared;
+    }
+    if ((rc = seg_forward_lane(h, 0, prep, wav_dev, B, S, seg.as<float>(), st, stage <= 3 ? -1 : stage <= 7 ? stage - 4 : 99)))
+      return rc;
+  }
+  DG_CUDA(cudaDeviceSynchronize());
+  if ((rc = debug_front_paths(prep, g, &dims[3]))) return rc;
+  if (lstm_tc_rows(B) == 16) dims[3] |= DG_DBG_LSTM_16ROWS;
+  const dg_seg::Scratch& w = h->scr[0];
+  if (stage <= 3) return debug_copy_front(who, stage, w.work, prep, w.xh.p, w.xl.p, B, g, out_host, cap, dims);
+  if (stage <= 7) return debug_copy_map(who, w.xh.p, w.xl.p, B, g.S2, 256, g.T2, 256, out_host, cap, dims);
+  if (stage == 8) return debug_copy_map(who, w.y1h.p, w.y1l.p, B, g.S2, 128, g.T2, 128, out_host, cap, dims);
+  if (stage == 9) return debug_copy_map(who, w.y2.p, nullptr, B, g.S2, 128, g.T2, 128, out_host, cap, dims);
+  return debug_copy_map(who, seg.p, nullptr, B, g.T2, h->K, g.T2, h->K, out_host, cap, dims);
 }
 
 extern "C" int dg_seg_destroy(dg_seg* h) {

@@ -202,8 +202,8 @@ struct SincStreamGeom {
 };
 SincStreamGeom sinc_stream_geom(int B, const Geom& g, int hop);
 int launch_overlap_check(const float* wav, int B, int S, int hop, int* flag, cudaStream_t st);
-int launch_stream_prep(const float* wav, int B, const Geom& g, int hop, void* planes_hi, void* planes_lo, const int* flag,
-                       cudaStream_t st);
+int launch_stream_prep(const float* wav, const float* rstd, int B, const Geom& g, int hop, void* planes_hi, void* planes_lo,
+                       int* flag, cudaStream_t st);
 int launch_sinc0_tc_stream(const void* w_planes, int B, const Geom& g, int hop, const void* planes_hi, const void* planes_lo,
                            float* craw, const int* flag, cudaStream_t st);
 size_t sinc_pool_part_floats(int B, const Geom& g, int hop);
@@ -212,6 +212,7 @@ int launch_sinc_pool_fused(const float* craw, const float* mean, const float* rs
                            void* planes_hi, void* planes_lo, const int* flag, cudaStream_t st);
 // lstm_tc.cu -- recurrence on wgmma (W_hh hi plane in registers, lo plane in shared memory)
 size_t lstm_tc_plane_elems();
+int lstm_tc_rows(int B);   // batch rows per CTA of the recurrence at batch B (8 or 16)
 int lstm_tc_ctas(int B);   // CTAs (= SMs) one recurrence launch occupies at batch B
 float lstm_tc_pack_whh(const float* whh_fwd, const float* whh_bwd, uint16_t* hi, uint16_t* lo);   // -> plane scale
 // hout (float32) and / or out_hi, out_lo (16-bit planes of the next GEMM's operand) receive h_t

@@ -362,7 +362,10 @@ __global__ void __launch_bounds__(128) pool_finalize_kernel(const float* __restr
   const double s0 = v1 - (double)eps;
   const double dm = (s1 - pv * (double)eps) / v1;
   double num = s2 - 2.0 * dm * s1 + dm * dm * s0;
-  if (num < 0) num = 0;
+  // s1, s2 are float32 sums around the pivot: their rounding leaves about 2^-22 s2 in `num` where the centred sum is smaller
+  // than that (one frame carries all the weight: exactly 0, over a denominator of 1e-8).  Below 2^-20 s2 the variance is
+  // not resolved and is 0, which is what the centred two-pass pooling (stats_pool) returns there.
+  if (num < s2 * 9.5367431640625e-7) num = 0;
   const double var = num / (v1 - v2 / v1 + (double)eps);
   float* o = pooled + (size_t)q * 2 * C;
   o[c] = (float)(pv + dm);

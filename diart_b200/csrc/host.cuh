@@ -206,6 +206,20 @@ int run_sinc_prep(SincPrep& p, const float* wav, int B, const Geom& g, cudaStrea
 int run_sincnet(const SincWeights& w, SincWork& k, const float* wav, int B, const Geom& g, cudaStream_t st,
                 const SincPrep* shared = nullptr);
 
+// ---- test hooks dg_seg_debug_stage / dg_emb_debug_stage (api_seg.cu): copy-out of what a forward left on the device
+// un-padded rows and real channels of an [B * item_rows][ld] map -> out [B][T][C] float32 on the host; `lo` non-null: fp16
+// hi / lo planes, returned as hi + lo (exact in float32); `lo` null: `hi` is a float32 map.  dims = {B, T, C}.
+int debug_copy_map(const char* who, const void* hi, const void* lo, int B, int item_rows, int ld, int T, int C, float* out_host,
+                   int64_t cap, int* dims);
+// stages 0..3 of both hooks, after a forward through `k` (`prep`: the shared statistics, or null for k.own_prep): operand of
+// conv1, operand of conv2, operand of the LSTM / TDNN1 (`xh`, `xl`), waveform statistics [2][B] (mean, rstd)
+int debug_copy_front(const char* who, int stage, const SincWork& k, const SincPrep* prep, const void* xh, const void* xl, int B,
+                     const Geom& g, float* out_host, int64_t cap, int* dims);
+// dims[3] of both hooks, bit 0 and 1: the stream form of the sinc layer did the work (hint accepted AND the device flag set);
+// conv1 / conv2 ran with MaxPool1d(3) in the GEMM epilogue
+int debug_front_paths(const SincPrep* prep, const Geom& g, int* paths);
+enum { DG_DBG_STREAM_FORM = 1, DG_DBG_POOL3_FUSED = 2, DG_DBG_LSTM_16ROWS = 4, DG_DBG_STATS_POOL_FUSED = 8 };
+
 // Sets g_sm_limit for its lifetime (0: no cap).
 struct SmLimit {
   const int prev;
@@ -241,7 +255,9 @@ struct dg_seg {
 };
 
 // the forward on scratch lane `lane`, without the use bracket; `prep`: waveform statistics + planes the caller computed (or null)
-int seg_forward_lane(dg_seg* h, int lane, const SincPrep* prep, const float* wav, int B, int S, float* seg, cudaStream_t st);
+// `stop_after` (test hook dg_seg_debug_stage): -1 returns before the LSTM, L < 3 after LSTM layer L
+int seg_forward_lane(dg_seg* h, int lane, const SincPrep* prep, const float* wav, int B, int S, float* seg, cudaStream_t st,
+                     int stop_after = 99);
 
 // ===================================================================================== embedding (api_emb.cu)
 struct dg_emb {
@@ -269,8 +285,9 @@ struct dg_emb {
   std::unique_ptr<struct ResNet> rn;
 };
 
+// `stop_after` (test hook dg_emb_debug_stage): -1 returns before TDNN1, L after TDNN layer L (0-based)
 int emb_trunk(dg_emb* h, const float* wav, int U, const Geom& g, cudaStream_t st, int* T_out, bool defer_last,
-              const SincPrep* prep);
+              const SincPrep* prep, int stop_after = 99);
 bool pool_fusable(const dg_emb* h, int K, const Geom& g);
 int emb_tail(dg_emb* h, int B, const Geom& g, const float* weights, int F, int K, int T, bool fuse, int normalize, float norm,
              float* out, cudaStream_t st, int sm_cap = 0);

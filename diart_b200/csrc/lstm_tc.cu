@@ -290,6 +290,7 @@ int launch_lstm_layer_tc(const float* gx, const void* whh_hi, const void* whh_lo
   return 0;
 }
 
+int lstm_tc_rows(int B) { return lt_rows(B); }
 int lstm_tc_ctas(int B) { return 2 * ((B + lt_rows(B) - 1) / lt_rows(B)); }
 
 }  // namespace dg

@@ -337,16 +337,29 @@ SincStreamGeom sinc_stream_geom(int B, const Geom& g, int hop) {
   return sg;
 }
 
-// raw stream -> four shifted fp16 hi / lo copies:  plane[c][i] = split(stream[i + 2c])
-__global__ void __launch_bounds__(256) stream_prep_kernel(const float* __restrict__ wav, int S, int hop, int Ls, int Lp,
-                                                          size_t plane_elems, uint16_t* __restrict__ hi,
-                                                          uint16_t* __restrict__ lo, const int* __restrict__ flag) {
+// The fp16 hi / lo planes keep 22 bits of what is split, and the lo plane is subnormal below 2^-14 * 2^11.  The raw sample
+// would spend those bits on a DC offset, or lose them at a low level, before the window's mean and deviation are applied.  The
+// stream is therefore split as s (x - p): p = its first sample, s = the power of two below the first window's reciprocal
+// deviation (<= 256, from the 1e-5 epsilon), which is the precision the per-window form has.  With A = gamma rstd_b,
+//     A conv(x) + (beta - A mu_b) sum h  =  (A / s) conv(s (x - p)) + (beta - A (mu_b - p)) sum h.
+// p and s are left behind the device flag (flag[1], flag[2] as float) for the pooling kernels.
+__device__ __forceinline__ float stream_scale(float rstd0) { return exp2f(floorf(log2f(fmaxf(rstd0, 1.f)))); }
+
+// stream -> four shifted fp16 hi / lo copies:  plane[c][i] = split(s (stream[i + 2c] - p))
+__global__ void __launch_bounds__(256) stream_prep_kernel(const float* __restrict__ wav, const float* __restrict__ rstd, int S,
+                                                          int hop, int Ls, int Lp, size_t plane_elems,
+                                                          uint16_t* __restrict__ hi, uint16_t* __restrict__ lo, int* __restrict__ flag) {
   if (*flag == 0) return;
+  const float pv = wav[0], sc = stream_scale(rstd[0]);
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    reinterpret_cast<float*>(flag)[1] = pv;
+    reinterpret_cast<float*>(flag)[2] = sc;
+  }
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < Lp + 8; i += gridDim.x * blockDim.x) {
     float v = 0.f;
     if (i < Ls) {
       const int b = i < S ? 0 : (i - S) / hop + 1;          // the window that ends with this sample
-      v = wav[(size_t)b * S + (i - b * hop)];
+      v = sc * (wav[(size_t)b * S + (i - b * hop)] - pv);
     }
     uint16_t h, l;
     split_h16(v, h, l);
@@ -361,12 +374,12 @@ __global__ void __launch_bounds__(256) stream_prep_kernel(const float* __restric
   }
 }
 
-int launch_stream_prep(const float* wav, int B, const Geom& g, int hop, void* planes_hi, void* planes_lo, const int* flag,
-                       cudaStream_t st) {
+int launch_stream_prep(const float* wav, const float* rstd, int B, const Geom& g, int hop, void* planes_hi, void* planes_lo,
+                       int* flag, cudaStream_t st) {
   const SincStreamGeom sg = sinc_stream_geom(B, g, hop);
   ProfScope _ps("sinc0_prep", st);
   const int Lp = sg.rows * 120;
-  stream_prep_kernel<<<(Lp + 8 + 255) / 256, 256, 0, st>>>(wav, g.S, hop, sg.Ls, Lp, sg.plane, reinterpret_cast<uint16_t*>(planes_hi),
+  stream_prep_kernel<<<(Lp + 8 + 255) / 256, 256, 0, st>>>(wav, rstd, g.S, hop, sg.Ls, Lp, sg.plane, reinterpret_cast<uint16_t*>(planes_hi),
                                                           reinterpret_cast<uint16_t*>(planes_lo), flag);
   DG_LAUNCHED();
   return 0;
@@ -392,6 +405,9 @@ int launch_sinc0_tc_stream(const void* w_planes, int B, const Geom& g, int hop, 
 // of ten times.  Pool groups of different windows have different phases (hop / 10 is not a multiple of 3): a CTA owns the
 // groups whose FIRST row lies in its range.
 constexpr int SP_R = 96, SP_GL = 16, SP_THREADS = 20 * SP_GL;
+// pivot and scale the stream was split with (stream_prep_kernel)
+__device__ __forceinline__ float sp_pivot(const int* flag) { return reinterpret_cast<const float*>(flag)[1]; }
+__device__ __forceinline__ float sp_scale(const int* flag) { return reinterpret_cast<const float*>(flag)[2]; }
 
 __device__ __forceinline__ float4 sp_value_sm(const float4* __restrict__ rows /*[SP_R + 2][20]*/, int r, int f4, float A,
                                               const float4& bias) {
@@ -437,7 +453,7 @@ __global__ void __launch_bounds__(96) sinc_pool_pivot_kernel(const float* __rest
   if (*flag == 0) return;
   const int b = blockIdx.x, f = threadIdx.x;
   if (f >= ST_N) return;
-  const float A = gamma * rstd[b], Am = A * mean[b];
+  const float Ar = gamma * rstd[b], A = Ar / sp_scale(flag), Am = Ar * (mean[b] - sp_pivot(flag));
   const float bias = fmaf(-Am, hsum[f], cf[f]);
   const float* src = craw + (size_t)b * hop10 * ST_N + f;
   pv[(size_t)b * ST_N + f] = fmaxf(fmaxf(fabsf(fmaf(A, src[0], bias)), fabsf(fmaf(A, src[ST_N], bias))), fabsf(fmaf(A, src[2 * ST_N], bias)));
@@ -462,7 +478,7 @@ __global__ void __launch_bounds__(SP_THREADS) sinc_pool_stats_kernel(const float
   for (int b = b_lo; b <= b_hi; b++) {
     int p_lo, p_hi;
     sp_groups(r0, b, hop10, T0, p_lo, p_hi);
-    const float A = gamma * rstd[b], Am = A * mean[b];
+    const float Ar = gamma * rstd[b], A = Ar / sp_scale(flag), Am = Ar * (mean[b] - sp_pivot(flag));
     const float4 bias = sp_bias(cf, hsum, f4, Am);
     const float4 pvv = reinterpret_cast<const float4*>(pv + (size_t)b * ST_N)[f4];
     float4 s1 = make_float4(0.f, 0.f, 0.f, 0.f), s2 = s1;
@@ -535,7 +551,7 @@ __global__ void __launch_bounds__(SP_THREADS) sinc_pool_split_kernel(const float
   for (int b = b_lo; b <= b_hi; b++) {
     int p_lo, p_hi;
     sp_groups(r0, b, hop10, T0, p_lo, p_hi);
-    const float A = gamma * rstd[b], Am = A * mean[b];
+    const float Ar = gamma * rstd[b], A = Ar / sp_scale(flag), Am = Ar * (mean[b] - sp_pivot(flag));
     const float4 bias = sp_bias(cf, hsum, f4, Am);
     const float4 s4 = reinterpret_cast<const float4*>(sc + (size_t)b * ST_N)[f4], h4 = reinterpret_cast<const float4*>(sh + (size_t)b * ST_N)[f4];
     uint2* oh = reinterpret_cast<uint2*>(hi + (size_t)b * S0 * ST_N);

@@ -60,9 +60,12 @@ __global__ void __launch_bounds__(256) stream_sums_kernel(const float* __restric
   int b = (int)(first / hop);
   if (b > B - 1) b = B - 1;
   const float4* x = reinterpret_cast<const float4*>(wav + (size_t)b * S + (first - (long long)b * hop));
+  // sums of x - pivot (the stream's first sample): sum x^2 / S - mean^2 of the raw samples cancels on audio with a DC offset
+  const float pv = wav[0];
   float s1 = 0.f, s2 = 0.f;
   for (int i = threadIdx.x; i < (sub >> 2); i += blockDim.x) {
-    const float4 v = x[i];
+    float4 v = x[i];
+    v.x -= pv; v.y -= pv; v.z -= pv; v.w -= pv;
     s1 += (v.x + v.y) + (v.z + v.w);
     s2 = fmaf(v.x, v.x, fmaf(v.y, v.y, fmaf(v.z, v.z, fmaf(v.w, v.w, s2))));
   }
@@ -74,7 +77,7 @@ __global__ void __launch_bounds__(256) stream_sums_kernel(const float* __restric
   }
 }
 
-__global__ void stream_stats_kernel(const double* __restrict__ part, int B, int S, int hop, int sub, float* __restrict__ mean,
+__global__ void stream_stats_kernel(const float* __restrict__ wav, const double* __restrict__ part, int B, int S, int hop, int sub, float* __restrict__ mean,
                                     float* __restrict__ rstd, const int* __restrict__ flag) {
   if (*flag == 0) return;
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -88,7 +91,7 @@ __global__ void stream_stats_kernel(const double* __restrict__ part, int B, int 
   const double m = t1 / S;
   double var = t2 / S - m * m;
   if (var < 0) var = 0;
-  mean[b] = (float)m;
+  mean[b] = (float)((double)wav[0] + m);
   rstd[b] = (float)(1.0 / sqrt(var + 1e-5));
 }
 
@@ -102,7 +105,7 @@ int launch_stream_stats(const float* wav, int B, int S, int hop, double* part, f
   const int blocks = (B - 1) * 4 + S / sub;
   stream_sums_kernel<<<blocks, 256, 0, st>>>(wav, B, S, hop, sub, part, flag);
   DG_LAUNCHED();
-  stream_stats_kernel<<<(B + 127) / 128, 128, 0, st>>>(part, B, S, hop, sub, mean, rstd, flag);
+  stream_stats_kernel<<<(B + 127) / 128, 128, 0, st>>>(wav, part, B, S, hop, sub, mean, rstd, flag);
   DG_LAUNCHED();
   return 0;
 }

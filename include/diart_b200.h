@@ -93,6 +93,19 @@ int dg_emb_destroy(dg_emb* h);
  * stop_after (0..15), returned as float32 [U][W][H][C] (time, mel, channel) on the host; -2 = log-mel features [U][T][80].
  * dims receives {U, W, H, C}.  Synchronises the device. */
 int dg_emb_debug_trunk(dg_emb* h, const float* wav_dev, int U, int S, int stop_after, float* out_host, int64_t cap, int* dims);
+/* Test hooks of the default networks (PyanNet, XVectorSincNet): the production forward with a host-side stop point, and the
+ * map it left on the device returned as float32 on the host -- un-padded rows, real channels, fp16 hi / lo planes as hi + lo.
+ * hop > 0: the front end runs as under dg_pipeline_set_hop(hop) (stream form of the sinc layer when the device finds the batch
+ * a run of overlapping windows); hop = 0: the per-window form.  Stages shared by both: 0 operand of conv1 [B][T0][80],
+ * 1 operand of conv2 [B][T1][60], 2 operand of the LSTM / TDNN1 [B][T2][60], 3 waveform mean and rstd [2][B].
+ * dg_seg_debug_stage: 4..7 output of LSTM layer 0..3 [B][T2][256], 8 / 9 the two Linears [B][T2][128], 10 scores [B][T2][K].
+ * dg_emb_debug_stage: 4..7 TDNN1..4 [B][T][512], 8 TDNN5 [B][T][1500], 9 / 10 pooled statistics [B*K][3000] from the fused /
+ * un-fused pooling, 11 / 12 the raw embedding [B*K][D] behind either; weights_dev [B][F][K] is read from stage 9 on.
+ * dims receives the three extents and, in dims[3], the paths taken: 1 stream form, 2 MaxPool1d(3) fused into conv1 / conv2,
+ * 4 recurrence with 16 rows per CTA, 8 fused statistics pooling.  Both synchronise the device. */
+int dg_seg_debug_stage(dg_seg* h, const float* wav_dev, int B, int S, int hop, int stage, float* out_host, int64_t cap, int* dims);
+int dg_emb_debug_stage(dg_emb* h, const float* wav_dev, const float* weights_dev, int B, int S, int F, int K, int hop, int stage,
+                       float* out_host, int64_t cap, int* dims);
 
 /* ---- element-wise blocks ---- */
 /* OverlappedSpeechPenalty (reference src/diart/blocks/embedding.py:98-107, functional.py:6-13) */
@@ -476,6 +489,9 @@ int dg_selftest_gemm_tc_halo(int M, int Cin, int KW, int dil, int N, int epi, in
 /* test hook (host only, no GPU): the weight-side split of float32 values into the two IEEE fp16 operand planes
  * (hi = rn16(x), lo = rn16(x - hi), saturating).  What the device does to activations with cvt.rn.satfinite.f16.f32. */
 int dg_selftest_split_f16_host(const float* x, long long n, unsigned short* hi, unsigned short* lo);
+/* the ParamSincFB filter table the models are built with, from low_hz_ [40] and band_hz_ [40]: filters [251][80] (tap-major;
+ * 40 cosine then 40 sine filters); host only */
+int dg_selftest_sinc_filters_host(const float* low_hz, const float* band_hz, float* filters);
 int dg_profile_report(char* buf, int cap);
 
 /* ---- shared-identity mode (extension beyond the reference; SURVEY.md 8(e), BASELINE config 5): G ranks diarize

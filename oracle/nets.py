@@ -390,6 +390,85 @@ def make_wespeaker(seed: int = 2468, pool_mode: str = "3.1") -> WeSpeakerResNet3
 
 
 # --------------------------------------------------------------------------------------
+# Stage-by-stage evaluation of the default networks, the checker of tests/test_gpu_net_stages.py.  Every map is returned
+# time-major, (B, T, C), as the CUDA path stores it.  The functions work in the dtype of the net they are given; the tests run
+# them on `float64_copy(net)` and never rely on the float32 evaluation (the first float32 evaluation of a shape is not
+# reproducible on every host, see `_reproduced`).
+# --------------------------------------------------------------------------------------
+def float64_copy(net: nn.Module) -> nn.Module:
+    """`net` in float64 -- except the sinc filters: ParamSincFB.filters() is DEFINED by its float32 evaluation (the CUDA path
+    builds the same float32 table, tests/test_net_stages_host.py compares the two), so the copy convolves with the float32
+    filters cast up.  Stage 0 then measures the convolution, not the construction of the filters."""
+    import copy
+
+    with torch.no_grad():
+        filters = net.sincnet.conv1d[0].filterbank.filters().double()
+    net64 = copy.deepcopy(net).double().eval()
+    net64.sincnet.conv1d[0].filterbank.filters = lambda: filters
+    return net64
+
+
+def sincnet_stages(sincnet: SincNet, waveforms: torch.Tensor) -> dict:
+    """`wmean`, `wrstd` (B,): the statistics InstanceNorm1d(1) applies; `sinc_norm{c}`: normalised, LeakyReLU'd output of stage c"""
+    out = {"wmean": waveforms.mean(dim=(1, 2)),
+           "wrstd": 1.0 / torch.sqrt(waveforms.var(dim=(1, 2), unbiased=False) + sincnet.wav_norm1d.eps)}
+    x = sincnet.wav_norm1d(waveforms)
+    for c, (conv1d, pool1d, norm1d) in enumerate(zip(sincnet.conv1d, sincnet.pool1d, sincnet.norm1d)):
+        x = conv1d(x)
+        if c == 0:
+            x = torch.abs(x)
+        x = F.leaky_relu(norm1d(pool1d(x)))
+        out[f"sinc_norm{c}"] = x.transpose(1, 2)
+    return out
+
+
+def lstm_layers(lstm: nn.LSTM, x: torch.Tensor) -> list:
+    """outputs of every layer of a multi-layer (bi)LSTM, each from a one-layer nn.LSTM that holds that layer's tensors"""
+    outs = []
+    for layer in range(lstm.num_layers):
+        one = nn.LSTM(x.shape[-1], lstm.hidden_size, num_layers=1, bidirectional=lstm.bidirectional, batch_first=True).to(x.dtype)
+        sfx = (f"_l{layer}", f"_l{layer}_reverse")
+        one.load_state_dict({k.replace(f"_l{layer}", "_l0"): v for k, v in lstm.state_dict().items() if k.endswith(sfx)})
+        x, _ = one(x)
+        outs.append(x)
+    return outs
+
+
+def segmentation_stages(net: PyanNet, waveforms: torch.Tensor) -> dict:
+    """waveforms (B, 1, S) -> the front-end maps, `lstm0..3` (B, T, 256), `linear0`, `linear1` (after LeakyReLU), `logits`,
+    `scores`"""
+    assert net.powerset_mapping is None
+    with torch.no_grad():
+        out = sincnet_stages(net.sincnet, waveforms)
+        x = out["sinc_norm2"]
+        for layer, x in enumerate(lstm_layers(net.lstm, x)):
+            out[f"lstm{layer}"] = x
+        for i, linear in enumerate(net.linear):
+            x = F.leaky_relu(linear(x))
+            out[f"linear{i}"] = x
+        out["logits"] = net.classifier(x)
+        out["scores"] = torch.sigmoid(out["logits"])
+    return out
+
+
+def embedding_stages(net: XVectorSincNet, waveforms: torch.Tensor, weights: Optional[torch.Tensor] = None) -> dict:
+    """waveforms (B, 1, S), weights (B, F, K) -> the front-end maps, `tdnn0..4` (B, T, C) after LeakyReLU and BatchNorm, and
+    with weights `stats_pool` (B, K, 3000) and `embedding` (B, K, D), not normalised"""
+    with torch.no_grad():
+        out = sincnet_stages(net.sincnet, waveforms)
+        x = out["sinc_norm2"].transpose(1, 2)
+        for i, layer in enumerate(net.tdnns):
+            x = layer(x)
+            if i % 3 == 2:
+                out[f"tdnn{i // 3}"] = x.transpose(1, 2)
+        if weights is not None:
+            pooled = torch.stack([net.stats_pool(x, weights[:, :, k]) for k in range(weights.shape[2])], dim=1)
+            out["stats_pool"] = pooled
+            out["embedding"] = net.embedding(pooled)
+    return out
+
+
+# --------------------------------------------------------------------------------------
 # Seeded synthetic weights / audio (SURVEY.md section 8(d)): generated by diart_b200.synth so
 # that the oracle and the CUDA side are fed the very same state dicts.
 # --------------------------------------------------------------------------------------
