@@ -28,10 +28,18 @@ kernel again.
 ``Binarize`` alone: the segmentation runs once per dataset, the aggregated speech curve is computed once per chunk
 (``dg_vad_sweep_curve``, ``csrc/vad.cu``), and every trial only thresholds it and is scored by detection error rate
 (``DetectionErrorRate(collar=0, skip_overlap=False)``, the pipeline's ``suggest_metric()``; DESIGN.md "Detection error").
+
+The three classes share their mechanics: :class:`FileBatches` cuts the window batches of every network pass,
+:func:`stream_plan` is the post-path plan of one file, ``_timed`` puts CUDA events around one C call and ``_turn_list_call``
+downloads a turn list into a host buffer that grows on demand.  ``HyperParameterSweep._run_trials`` / ``_score_trials`` are the
+bodies of the one-file and the ``_files`` entry points of the diarization sweep, and ``_DatasetSweep`` is the base of the two
+dataset classes (files, offsets, plans, references and the loops over trial groups).
 """
 from __future__ import annotations
 
 import ctypes as C
+import functools
+import operator
 import time
 from dataclasses import dataclass
 from typing import Dict, Iterable, List, Mapping, Optional, Sequence, Tuple
@@ -193,6 +201,13 @@ def reference_arrays(annotation: Annotation) -> Tuple[np.ndarray, np.ndarray, Li
     return (np.array(rows, dtype=np.float64).reshape(-1, 2), np.array(labels, dtype=np.int32), names)
 
 
+def _rate(num: np.ndarray, total: np.ndarray) -> np.ndarray:
+    """num / total per trial, as a fraction; with total = 0: 0 when num is 0, else 1 (pyannote's ``compute_metric`` of both
+    error rates)"""
+    safe = np.where(total > 0, total, 1.0)
+    return np.where(total > 0, num / safe, np.where(num > 0, 1.0, 0.0))
+
+
 @dataclass
 class DERComponents:
     """Diarization error rate components in seconds, one entry per trial (float64 (T,) each)."""
@@ -213,11 +228,8 @@ class DERComponents:
 
     @property
     def der(self) -> np.ndarray:
-        """(false alarm + missed detection + confusion) / total per trial, as a fraction; with total = 0: 0 when the
-        numerator is 0, else 1"""
-        num = self.false_alarm + self.missed_detection + self.confusion
-        safe = np.where(self.total > 0, self.total, 1.0)
-        return np.where(self.total > 0, num / safe, np.where(num > 0, 1.0, 0.0))
+        """(false alarm + missed detection + confusion) / total per trial (:func:`_rate`)"""
+        return _rate(self.false_alarm + self.missed_detection + self.confusion, self.total)
 
     def __add__(self, other: "DERComponents") -> "DERComponents":
         """the components of several files summed per trial (the "TOTAL" row of pyannote's report)"""
@@ -236,7 +248,7 @@ class SweepOutputs:
     device_seconds: float = 0.0
 
 
-_AUDIO_STREAMS = 3            # audio streams the dataset network pass uses in turn (see network_pass_files)
+_AUDIO_STREAMS = 3            # audio streams a network pass over several files uses in turn (see FileBatches)
 
 
 def seg_resolution(config: SpeakerDiarizationConfig, start: float, F: int) -> float:
@@ -247,13 +259,21 @@ def seg_resolution(config: SpeakerDiarizationConfig, start: float, F: int) -> fl
     return (end - start if end > start else 0.0) / F
 
 
-def dataset_plan(fws: Sequence[FileWindows], config: SpeakerDiarizationConfig, F: int):
-    """The post-path plans of several files, each that of a fresh stream (empty history), concatenated in file order ->
-    (plan int32 (N, 4 + nw), out_start (N,), out_res (N,)).  post.cu finds chunk c's aggregated buffers at chunks
-    c - (nb - 1) .. c with nb <= (c's index in its file) + 1, so no chunk reaches into the previous file."""
+def stream_plan(starts: np.ndarray, config: SpeakerDiarizationConfig, F: int):
+    """The post-path plan of a fresh stream (empty history) whose chunks start at ``starts`` (N,), with F score frames per
+    chunk -> contiguous (plan int32 (N, 4 + nw), out_start float64 (N,), out_res float64 (N,))"""
+    starts = np.asarray(starts, dtype=np.float64)
     nw = int(round(config.latency / config.step))
-    parts = [post_plan(np.asarray(fw.starts, dtype=np.float64), seg_resolution(config, float(fw.starts[0]), F), np.zeros(0),
-                       np.zeros(0), nw, F, config.step, config.latency) for fw in fws]
+    plans = post_plan(starts, seg_resolution(config, float(starts[0]), F), np.zeros(0), np.zeros(0), nw, F, config.step,
+                      config.latency)
+    return tuple(np.ascontiguousarray(a, dtype=t) for a, t in zip(plans, (np.int32, np.float64, np.float64)))
+
+
+def dataset_plan(fws: Sequence[FileWindows], config: SpeakerDiarizationConfig, F: int):
+    """The :func:`stream_plan` of each of several files, concatenated in file order.  post.cu finds chunk c's aggregated
+    buffers at chunks c - (nb - 1) .. c with nb <= (c's index in its file) + 1, so no chunk reaches into the previous
+    file."""
+    parts = [stream_plan(fw.starts, config, F) for fw in fws]
     return tuple(np.ascontiguousarray(np.concatenate([p[i] for p in parts])) for i in range(3))
 
 
@@ -294,6 +314,80 @@ def file_turns(header: np.ndarray, turns: np.ndarray, c0: int, c1: int):
     return h, own, len(own)
 
 
+class FileBatches:
+    """Iterates over the window batches of a network pass over several files, in file then batch order: each a dense
+    (B, chunk_samples) device tensor of B <= 256 consecutive windows of one file.  Every batch holds windows of one file only,
+    cut at the multiples of 256 from that file's window 0: the batch is the unit of the network pass's arithmetic (the sinc
+    layer's stream form covers one batch), so each file's outputs are the bits a pass over it alone gives.  A file's audio
+    is pushed as its batches need it; nothing drains or synchronises between files.
+
+    Iterate under ``torch.cuda.device(device)`` and keep the object until the batches are consumed: it owns the audio
+    streams, and destroying one frees device memory, which waits for the device."""
+
+    def __init__(self, fws: Sequence[FileWindows], config, device: torch.device):
+        self.fws, self.config, self.device = fws, config, device
+        self.streams: List[DeviceAudioStream] = []
+
+    def __iter__(self):
+        cfg, streams = self.config, self.streams
+        for i, fw in enumerate(self.fws):
+            # a few streams in turn: a reset waits for the uploads of its stream, so reuse the one whose file was
+            # submitted longest ago (its batches have left the consumer's pipeline)
+            if len(streams) < _AUDIO_STREAMS:
+                streams.append(DeviceAudioStream(cfg.duration, cfg.step, cfg.sample_rate, max_windows=NETWORK_BATCH,
+                                                 device=self.device))
+            stream = streams[i % _AUDIO_STREAMS]
+            if i >= _AUDIO_STREAMS:
+                stream.reset()
+            pushed = fw.offset
+            for i0 in range(0, fw.num_windows, NETWORK_BATCH):
+                B = min(NETWORK_BATCH, fw.num_windows - i0)
+                need = fw.offset + (i0 + B - 1) * fw.step_samples + fw.chunk_samples
+                stream.push(fw.samples[pushed:need])
+                pushed = need
+                yield stream.windows(B)
+
+
+def _indexed(device: torch.device) -> torch.device:
+    """``device`` with an index: "cuda" alone is the current device"""
+    return device if device.index is not None else torch.device("cuda", torch.cuda.current_device())
+
+
+def _timed(device: torch.device, call):
+    """Runs ``call(cuda_stream)``, one C entry point that enqueues on the current stream of ``device``, between two CUDA
+    events -> (its status, seconds).  ``seconds()`` waits for the second event and returns the device time between the
+    two: for the caller to ask once it has checked the status."""
+    with torch.cuda.device(device):
+        st = torch.cuda.current_stream(device)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(st)
+        rc = call(st.cuda_stream)
+        e1.record(st)
+
+    def seconds() -> float:
+        e1.synchronize()
+        return e0.elapsed_time(e1) / 1e3
+    return rc, seconds
+
+
+def _turn_list_call(owner, device: torch.device, guess: int, call) -> Tuple[int, float]:
+    """Runs ``call(turns, capacity, n, cuda_stream)``, the last four arguments of an entry point that downloads a packed
+    turn list, into ``owner._turns`` (uint32, grown to ``guess`` entries first) -> (turns written, device seconds of the
+    call).  An entry point that finds more turns than the buffer holds reports how many: the buffer grows to that and the
+    call runs once more (its seconds are the ones returned)."""
+    if len(owner._turns) < guess:
+        owner._turns = np.empty(guess, dtype=np.uint32)
+    n = C.c_int()
+    for attempt in range(2):
+        rc, seconds = _timed(device, lambda st: call(owner._turns.ctypes.data, len(owner._turns), C.byref(n), st))
+        if rc == -1 and n.value > len(owner._turns):
+            owner._turns = np.empty(n.value, dtype=np.uint32)
+            continue
+        _lib.check(rc)
+        break
+    return n.value, seconds()
+
+
 class HyperParameterSweep:
     """Runs ``SpeakerDiarization(config)`` over a file for many (tau_active, rho_update, delta_new) trials at the cost of one
     network pass.  Needs the native segmentation and embedding models.
@@ -307,9 +401,7 @@ class HyperParameterSweep:
         self.pipeline = SpeakerDiarization(config)
         if self.pipeline._native_models() is None:
             raise _lib.DiartB200Error("HyperParameterSweep needs the native segmentation and embedding models")
-        self.device = self.pipeline.segmentation.device
-        if self.device.index is None:
-            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.device = _indexed(self.pipeline.segmentation.device)
         self._h: Optional[C.c_void_p] = None
         self._dims = None
         self._turns = np.empty(0, dtype=np.uint32)
@@ -330,43 +422,28 @@ class HyperParameterSweep:
 
     def network_pass_files(self, fws: Sequence[FileWindows]):
         """:meth:`network_pass` of several files as one pipelined flow -> their scores and embeddings concatenated in file
-        order.  Every batch holds windows of one file only, cut at the multiples of 256 from that file's window 0: the batch
-        is the unit of the network pass's arithmetic (the sinc layer's stream form covers one batch), so each file's outputs
-        are the bits :meth:`network_pass` gives for it alone.  Nothing drains or synchronises between files."""
-        cfg, pipe = self.config, self.pipeline
+        order, each file's the bits :meth:`network_pass` gives for it alone (:class:`FileBatches`).  Two batches are in
+        flight at a time; nothing drains or synchronises between files."""
+        pipe = self.pipeline
         pipe.reset()
-        streams: List[DeviceAudioStream] = []
+        batches = FileBatches(fws, self.config, self.device)
         segs, embs, inflight = [], [], []
+
+        def collect():
+            seg, emb, _ = pipe.collect()
+            segs.append(seg)
+            embs.append(emb)
+            inflight.pop(0)
+
         with torch.cuda.device(self.device):
-            for i, fw in enumerate(fws):
-                # a few streams in turn: a reset waits for the uploads of its stream, so reuse the one whose file was
-                # submitted longest ago (its batches have left the pipeline's slots)
-                if len(streams) < _AUDIO_STREAMS:
-                    streams.append(DeviceAudioStream(cfg.duration, cfg.step, cfg.sample_rate, max_windows=NETWORK_BATCH,
-                                                     device=self.device))
-                stream = streams[i % _AUDIO_STREAMS]
-                if i >= _AUDIO_STREAMS:
-                    stream.reset()
-                pushed = fw.offset
-                for i0 in range(0, fw.num_windows, NETWORK_BATCH):
-                    B = min(NETWORK_BATCH, fw.num_windows - i0)
-                    need = fw.offset + (i0 + B - 1) * fw.step_samples + fw.chunk_samples
-                    stream.push(fw.samples[pushed:need])
-                    pushed = need
-                    inflight.append(stream.windows(B))       # must stay alive until collected
-                    pipe.submit(inflight[-1])
-                    if len(inflight) == 2:
-                        seg, emb, _ = pipe.collect()
-                        segs.append(seg)
-                        embs.append(emb)
-                        inflight.pop(0)
+            for windows in batches:
+                inflight.append(windows)                      # must stay alive until collected
+                pipe.submit(windows)
+                if len(inflight) == 2:
+                    collect()
             while inflight:
-                seg, emb, _ = pipe.collect()
-                segs.append(seg)
-                embs.append(emb)
-                inflight.pop(0)
-            seg, emb = torch.cat(segs), torch.cat(embs)
-        return seg, emb
+                collect()
+            return torch.cat(segs), torch.cat(embs)
 
     # ------------------------------------------------------------------ clustering + post-path for T trials
     def _handle(self, F: int, K: int, D: int):
@@ -383,42 +460,58 @@ class HyperParameterSweep:
             self._h, self._dims = h, dims
         return self._h, nw
 
-    def sweep(self, seg: torch.Tensor, emb: torch.Tensor, starts: np.ndarray, params: np.ndarray,
-              keep_state: bool = False) -> SweepOutputs:
-        """dg_sweep_run over device scores / embeddings of N chunks starting at ``starts`` for params (T, 3)"""
+    def _run_trials(self, entry, file_args: tuple, lead: tuple, seg: torch.Tensor, emb: torch.Tensor, plans,
+                    params: np.ndarray, keep_state: bool) -> SweepOutputs:
+        """The body of :meth:`sweep` and :meth:`DatasetSweep.sweep`.  ``entry``: dg_sweep_run, or dg_sweep_run_files with
+        ``file_args`` = what it takes after the chunk count (files, chunk offsets) and ``lead`` = (files,), the leading
+        dimension of its centroids.  ``plans``: (plan, out_start, out_res) of the N chunks."""
         N, F, K = seg.shape
-        D = emb.shape[2]
-        M = int(self.config.max_speakers)
-        h, nw = self._handle(F, K, D)
-        res = self._seg_resolution(float(starts[0]), F)
-        plan, out_start, out_res = post_plan(np.asarray(starts, dtype=np.float64), res, np.zeros(0), np.zeros(0), nw, F,
-                                             self.config.step, self.config.latency)
-        plan = np.ascontiguousarray(plan)
+        D, M = emb.shape[2], int(self.config.max_speakers)
+        h, _ = self._handle(F, K, D)
+        plan, out_start, out_res = plans
         params = np.ascontiguousarray(params, dtype=np.float64)
         T = len(params)
         header = np.empty((T, N, 4), dtype=np.int32)
         maps = torch.empty((T, N, K), dtype=torch.int32, device=self.device) if keep_state else None
-        centers = torch.empty((T, M, D), dtype=torch.float64, device=self.device) if keep_state else None
-        if len(self._turns) < T * N * 8:
-            self._turns = np.empty(T * N * 8, dtype=np.uint32)
-        n = C.c_int()
-        with torch.cuda.device(self.device):
-            st = torch.cuda.current_stream(self.device)
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            for attempt in range(2):
-                e0.record(st)
-                rc = _lib.lib().dg_sweep_run(h, seg.data_ptr(), emb.data_ptr(), N, params.ctypes.data, T, plan.ctypes.data,
-                                             _lib.ptr(maps), _lib.ptr(centers), header.ctypes.data, self._turns.ctypes.data,
-                                             len(self._turns), C.byref(n), st.cuda_stream)
-                e1.record(st)
-                if rc == -1 and n.value > len(self._turns):   # more turns than the host buffer: grow it, run again
-                    self._turns = np.empty(n.value, dtype=np.uint32)
-                    continue
-                _lib.check(rc)
-                break
-            e1.synchronize()
-        return SweepOutputs(header, self._turns[:n.value].copy(), n.value, out_start, out_res, maps, centers,
-                            e0.elapsed_time(e1) / 1e3)
+        centers = torch.empty((*lead, T, M, D), dtype=torch.float64, device=self.device) if keep_state else None
+        n_turns, seconds = _turn_list_call(self, self.device, T * N * 8, lambda *turn_list: entry(
+            h, seg.data_ptr(), emb.data_ptr(), N, *file_args, params.ctypes.data, T, plan.ctypes.data, _lib.ptr(maps),
+            _lib.ptr(centers), header.ctypes.data, *turn_list))
+        return SweepOutputs(header, self._turns[:n_turns].copy(), n_turns, out_start, out_res, maps, centers, seconds)
+
+    def _score_trials(self, entry, file_args: tuple, lead: tuple, seg: torch.Tensor, emb: torch.Tensor, plans,
+                      params: np.ndarray, shift, reference: tuple, segments: bool = False):
+        """The body of :meth:`sweep_score` and of each launch of :meth:`DatasetSweep.score` -> (components ``lead`` +
+        (T, 5), device seconds, hypothesis offsets, hypothesis segments).  ``entry``: dg_sweep_score, or
+        dg_sweep_score_files with ``file_args`` and ``lead`` as in :meth:`_run_trials`.  ``shift``: the timestamp shift, or
+        the address of the per-file shifts.  ``reference``: the entry point's four reference arguments (rows, labels,
+        then the row and label counts, or the addresses of the per-file row offsets and label counts).  ``segments`` is
+        for the one-file entry point."""
+        N, F, K = seg.shape
+        h, _ = self._handle(F, K, emb.shape[2])
+        plan, out_start, out_res = plans
+        params = np.ascontiguousarray(params, dtype=np.float64)
+        T, M = len(params), int(self.config.max_speakers)
+        comp = np.empty((*lead, T, 5), dtype=np.float64)
+        offsets = hseg = None
+        if segments:
+            offsets = torch.empty(T * M + 1, dtype=torch.int32, device=self.device)
+            hseg = torch.empty((T * N * 8, 2), dtype=torch.float64, device=self.device)
+        rc, seconds = _timed(self.device, lambda st: entry(
+            h, seg.data_ptr(), emb.data_ptr(), N, *file_args, params.ctypes.data, T, plan.ctypes.data, out_start.ctypes.data,
+            out_res.ctypes.data, shift, PATCH_COLLAR, *reference, comp.ctypes.data, _lib.ptr(offsets), _lib.ptr(hseg),
+            0 if hseg is None else hseg.shape[0], st))
+        _lib.check(rc)
+        secs = seconds()
+        if segments:
+            hseg = hseg[:int(offsets[-1])]
+        return comp, secs, offsets, hseg
+
+    def sweep(self, seg: torch.Tensor, emb: torch.Tensor, starts: np.ndarray, params: np.ndarray,
+              keep_state: bool = False) -> SweepOutputs:
+        """dg_sweep_run over device scores / embeddings of N chunks starting at ``starts`` for params (T, 3)"""
+        plans = stream_plan(starts, self.config, seg.shape[1])
+        return self._run_trials(_lib.lib().dg_sweep_run, (), (), seg, emb, plans, params, keep_state)
 
     def sweep_score(self, seg: torch.Tensor, emb: torch.Tensor, fw: FileWindows, params: np.ndarray, ref_rows: np.ndarray,
                     ref_labels: np.ndarray, num_ref_labels: int, segments: bool = False):
@@ -426,38 +519,12 @@ class HyperParameterSweep:
         ``reference_arrays`` form -> (components (T, 5), device seconds, hypothesis offsets, hypothesis segments).  The last
         two are device tensors when ``segments`` (int32 (T * max_speakers + 1,) and float64 (n, 2), see the C header), else
         None."""
-        N, F, K = seg.shape
-        h, nw = self._handle(F, K, emb.shape[2])
-        res = self._seg_resolution(float(fw.starts[0]), F)
-        plan, out_start, out_res = post_plan(np.asarray(fw.starts, dtype=np.float64), res, np.zeros(0), np.zeros(0), nw, F,
-                                             self.config.step, self.config.latency)
-        plan = np.ascontiguousarray(plan)
-        out_start = np.ascontiguousarray(out_start, dtype=np.float64)
-        out_res = np.ascontiguousarray(out_res, dtype=np.float64)
-        params = np.ascontiguousarray(params, dtype=np.float64)
         rows = np.ascontiguousarray(ref_rows, dtype=np.float64)
         labels = np.ascontiguousarray(ref_labels, dtype=np.int32)
-        T, M = len(params), int(self.config.max_speakers)
-        comp = np.empty((T, 5), dtype=np.float64)
-        offsets = hseg = None
-        if segments:
-            offsets = torch.empty(T * M + 1, dtype=torch.int32, device=self.device)
-            hseg = torch.empty((T * N * 8, 2), dtype=torch.float64, device=self.device)
-        with torch.cuda.device(self.device):
-            st = torch.cuda.current_stream(self.device)
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record(st)
-            rc = _lib.lib().dg_sweep_score(h, seg.data_ptr(), emb.data_ptr(), N, params.ctypes.data, T, plan.ctypes.data,
-                                           out_start.ctypes.data, out_res.ctypes.data, -fw.padding[0], PATCH_COLLAR,
-                                           rows.ctypes.data, labels.ctypes.data, len(rows), int(num_ref_labels),
-                                           comp.ctypes.data, _lib.ptr(offsets), _lib.ptr(hseg),
-                                           0 if hseg is None else hseg.shape[0], st.cuda_stream)
-            e1.record(st)
-            _lib.check(rc)
-            e1.synchronize()
-        if segments:
-            hseg = hseg[:int(offsets[-1])]
-        return comp, e0.elapsed_time(e1) / 1e3, offsets, hseg
+        reference = (rows.ctypes.data, labels.ctypes.data, len(rows), int(num_ref_labels))
+        plans = stream_plan(fw.starts, self.config, seg.shape[1])
+        return self._score_trials(_lib.lib().dg_sweep_score, (), (), seg, emb, plans, params, -fw.padding[0], reference,
+                                  segments)
 
     def _seg_resolution(self, start: float, F: int) -> float:
         return seg_resolution(self.config, start, F)
@@ -510,16 +577,98 @@ class HyperParameterSweep:
         """``files``: (waveform, reference) pairs -> (components per file, their sum).  ``total.der`` per trial is the
         value the reference's ``Optimizer.objective`` minimises over a dataset (a fraction, not a percentage).  Runs as a
         :class:`DatasetSweep` over the files."""
-        files = [(None, waveform, reference) for waveform, reference in files]
-        if not files:
-            raise ValueError("at least one file is needed")
-        dataset = DatasetSweep(self.config, files, sweep=self)
+        dataset = DatasetSweep(self.config, [(None, waveform, reference) for waveform, reference in files], sweep=self)
         out = dataset.score(trials)
         self.timing = dict(dataset.timing)
         return out
 
 
-class DatasetSweep:
+class _DatasetSweep:
+    """What the dataset sweeps share: the checks of the files, the chunk offsets, post-path plans and timestamp shifts of
+    the concatenated files, the network pass a subclass runs once and keeps on the device (``_open``, ``_networks``), the
+    packed references (``_pack_references``) and the loops of ``run`` and ``score`` over trial groups and files
+    (``_score_group``, ``_components``)."""
+
+    _pack_references = None   # staticmethod of the subclass: references -> the reference arguments of its scoring entry
+
+    def __init__(self, config, files: Iterable[Tuple[Optional[str], np.ndarray, Optional[Annotation]]]):
+        files = list(files)
+        if not files:
+            raise ValueError("at least one file is needed")
+        for i, (uri, x, _) in enumerate(files):
+            if np.asarray(x).size == 0:
+                raise ValueError(f"file {i} ({uri}) has no samples, so no windows")
+        self.config = config
+        self.uris = [uri for uri, _, _ in files]
+        self.references = [ref for _, _, ref in files]
+        fws = [file_windows(x, config) for _, x, _ in files]   # (the padded audio is dropped after the network pass)
+        self.offsets = np.ascontiguousarray(np.cumsum([0] + [fw.num_windows for fw in fws]), dtype=np.int32)
+        trial_groups(1, self.num_chunks)                        # a dataset too large for one launch fails here
+        self.device = self._open()
+        t0 = time.perf_counter()
+        self._networks(fws)
+        torch.cuda.synchronize(self.device)
+        self.timing: Dict[str, float] = {"network": time.perf_counter() - t0}
+        self.plan, self.out_start, self.out_res = dataset_plan(fws, config, self.seg.shape[1])
+        self.shifts = np.ascontiguousarray([-fw.padding[0] for fw in fws], dtype=np.float64)
+        self._refs = None
+
+    def _open(self) -> torch.device:
+        """makes the pipeline whose networks run (an error if they are not native) -> their device"""
+        raise NotImplementedError
+
+    def _networks(self, fws: Sequence[FileWindows]):
+        """runs the networks over every window of every file and keeps their outputs on the device, the scores as
+        ``self.seg`` (N, F, K)"""
+        raise NotImplementedError
+
+    def _score_group(self, params: np.ndarray) -> Tuple[np.ndarray, float]:
+        """one scoring launch for one trial group against ``self._refs`` -> (components (files, T, width), device seconds)"""
+        raise NotImplementedError
+
+    def _components(self, f: int, comp: np.ndarray):
+        """file f's components object from its (T, width) slice of the launches' components"""
+        raise NotImplementedError
+
+    @property
+    def num_chunks(self) -> int:
+        return int(self.offsets[-1])
+
+    def _run(self, params: np.ndarray, launch, labels: Sequence[str]) -> List[List[Annotation]]:
+        """``launch``: the trials of one group -> their :class:`SweepOutputs` over the concatenated chunks.  -> predictions
+        [file][trial], each file's assembled from its own chunks and turns"""
+        out: List[List[Annotation]] = [[] for _ in self.uris]
+        dev = 0.0
+        for g in trial_groups(len(params), self.num_chunks):
+            r = launch(params[g])
+            dev += r.device_seconds
+            for f in range(len(self.uris)):
+                c0, c1 = int(self.offsets[f]), int(self.offsets[f + 1])
+                header, turns, n = file_turns(r.header, r.turns, c0, c1)
+                out[f] += assemble_predictions(header, turns, n, self.out_start[c0:c1], self.out_res[c0:c1], labels,
+                                               float(self.shifts[f]), self.uris[f])
+        self.timing["sweep"] = dev
+        return out
+
+    def _score(self, params: np.ndarray):
+        """-> (components per file, their sum in file order), one ``_score_group`` per trial group"""
+        missing = [self.uris[i] if self.uris[i] is not None else i for i, r in enumerate(self.references) if r is None]
+        if missing:
+            raise ValueError(f"files without a reference cannot be scored: {missing}")
+        if self._refs is None:
+            self._refs = self._pack_references(self.references)
+        parts, dev = [], 0.0
+        for g in trial_groups(len(params), self.num_chunks):
+            part, secs = self._score_group(params[g])
+            parts.append(part)
+            dev += secs
+        self.timing["score"] = dev
+        comp = np.concatenate(parts, axis=1)
+        per_file = [self._components(f, comp[f]) for f in range(len(self.uris))]
+        return per_file, functools.reduce(operator.add, per_file)
+
+
+class DatasetSweep(_DatasetSweep):
     """A sweep over a whole dataset with the network outputs of every file kept on the device.
 
         ds = DatasetSweep(config, [("file1", waveform1, reference1), ("file2", waveform2, reference2)])
@@ -537,33 +686,20 @@ class DatasetSweep:
     ``sweep``: a :class:`HyperParameterSweep` of the same config whose pipeline and handles to use (default: a new one).
     """
 
+    _pack_references = staticmethod(pack_references)
+
     def __init__(self, config: SpeakerDiarizationConfig, files: Iterable[Tuple[Optional[str], np.ndarray, Optional[Annotation]]],
                  sweep: Optional[HyperParameterSweep] = None):
-        files = list(files)
-        if not files:
-            raise ValueError("at least one file is needed")
-        for i, (uri, x, _) in enumerate(files):
-            if np.asarray(x).size == 0:
-                raise ValueError(f"file {i} ({uri}) has no samples, so no windows")
-        self.config = config
-        self._sweep = sweep if sweep is not None else HyperParameterSweep(config)
-        self.device = self._sweep.device
-        self.uris = [uri for uri, _, _ in files]
-        self.references = [ref for _, _, ref in files]
-        fws = [file_windows(x, config) for _, x, _ in files]   # (the padded audio is dropped after the network pass)
-        self.offsets = np.ascontiguousarray(np.cumsum([0] + [fw.num_windows for fw in fws]), dtype=np.int32)
-        trial_groups(1, int(self.offsets[-1]))                  # a dataset too large for one launch fails here
-        t0 = time.perf_counter()
-        self.seg, self.emb = self._sweep.network_pass_files(fws)
-        torch.cuda.synchronize(self.device)
-        self.timing: Dict[str, float] = {"network": time.perf_counter() - t0}
-        self.plan, self.out_start, self.out_res = dataset_plan(fws, config, self.seg.shape[1])
-        self.shifts = np.ascontiguousarray([-fw.padding[0] for fw in fws], dtype=np.float64)
-        self._refs = None
+        self._sweep = sweep
+        super().__init__(config, files)
 
-    @property
-    def num_chunks(self) -> int:
-        return int(self.offsets[-1])
+    def _open(self) -> torch.device:
+        if self._sweep is None:
+            self._sweep = HyperParameterSweep(self.config)
+        return self._sweep.device
+
+    def _networks(self, fws: Sequence[FileWindows]):
+        self.seg, self.emb = self._sweep.network_pass_files(fws)
 
     @property
     def resident_bytes(self) -> int:
@@ -575,99 +711,34 @@ class DatasetSweep:
         c0, c1 = int(self.offsets[f]), int(self.offsets[f + 1])
         return self.seg[c0:c1], self.emb[c0:c1]
 
-    def _args(self):
-        N, F, K = self.seg.shape
-        h, _ = self._sweep._handle(F, K, self.emb.shape[2])
-        return h, N, len(self.uris)
+    def _over_files(self, entry) -> tuple:
+        """the leading arguments of ``HyperParameterSweep._run_trials`` / ``_score_trials`` for the ``_files`` entry point
+        ``entry`` over the resident outputs and the concatenated plans"""
+        nf = len(self.uris)
+        return entry, (nf, self.offsets.ctypes.data), (nf,), self.seg, self.emb, (self.plan, self.out_start, self.out_res)
 
     def sweep(self, params: np.ndarray, keep_state: bool = False) -> SweepOutputs:
         """dg_sweep_run_files over the resident outputs for params (T, 3): header (T, N, 4) and turns over the N
         concatenated chunks; with ``keep_state`` maps (T, N, K) and centroids (files, T, M, D) on the device"""
-        h, N, nf = self._args()
-        K, D, M = self.seg.shape[2], self.emb.shape[2], int(self.config.max_speakers)
-        params = np.ascontiguousarray(params, dtype=np.float64)
-        T = len(params)
-        header = np.empty((T, N, 4), dtype=np.int32)
-        maps = torch.empty((T, N, K), dtype=torch.int32, device=self.device) if keep_state else None
-        centers = torch.empty((nf, T, M, D), dtype=torch.float64, device=self.device) if keep_state else None
-        sw = self._sweep
-        if len(sw._turns) < T * N * 8:
-            sw._turns = np.empty(T * N * 8, dtype=np.uint32)
-        n = C.c_int()
-        with torch.cuda.device(self.device):
-            st = torch.cuda.current_stream(self.device)
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            for attempt in range(2):
-                e0.record(st)
-                rc = _lib.lib().dg_sweep_run_files(h, self.seg.data_ptr(), self.emb.data_ptr(), N, nf, self.offsets.ctypes.data,
-                                                   params.ctypes.data, T, self.plan.ctypes.data, _lib.ptr(maps),
-                                                   _lib.ptr(centers), header.ctypes.data, sw._turns.ctypes.data,
-                                                   len(sw._turns), C.byref(n), st.cuda_stream)
-                e1.record(st)
-                if rc == -1 and n.value > len(sw._turns):     # more turns than the host buffer: grow it, run again
-                    sw._turns = np.empty(n.value, dtype=np.uint32)
-                    continue
-                _lib.check(rc)
-                break
-            e1.synchronize()
-        return SweepOutputs(header, sw._turns[:n.value].copy(), n.value, self.out_start, self.out_res, maps, centers,
-                            e0.elapsed_time(e1) / 1e3)
+        return self._sweep._run_trials(*self._over_files(_lib.lib().dg_sweep_run_files), params, keep_state)
 
     def run(self, trials: Sequence[Mapping[str, float]] = ({},)) -> List[List[Annotation]]:
         """-> predictions [file][trial]: what :meth:`HyperParameterSweep.run` returns for each file alone"""
-        params = trial_params(trials, self.config)
         labels = [f"speaker{g}" for g in range(int(self.config.max_speakers))]
-        out: List[List[Annotation]] = [[] for _ in self.uris]
-        dev = 0.0
-        for g in trial_groups(len(params), self.num_chunks):
-            r = self.sweep(params[g])
-            dev += r.device_seconds
-            for f in range(len(self.uris)):
-                c0, c1 = int(self.offsets[f]), int(self.offsets[f + 1])
-                header, turns, n = file_turns(r.header, r.turns, c0, c1)
-                out[f] += assemble_predictions(header, turns, n, self.out_start[c0:c1], self.out_res[c0:c1], labels,
-                                               float(self.shifts[f]), self.uris[f])
-        self.timing["sweep"] = dev
-        return out
+        return self._run(trial_params(trials, self.config), self.sweep, labels)
 
     def score(self, trials: Sequence[Mapping[str, float]] = ({},)) -> Tuple[List[DERComponents], DERComponents]:
         """-> (components per file, their sum in file order): per file what :meth:`HyperParameterSweep.score` returns for
         it alone; ``total.der`` is the value ``Optimizer.objective`` minimises.  Every file needs a reference."""
-        missing = [self.uris[i] if self.uris[i] is not None else i for i, r in enumerate(self.references) if r is None]
-        if missing:
-            raise ValueError(f"files without a reference cannot be scored: {missing}")
-        params = trial_params(trials, self.config)
-        if self._refs is None:
-            self._refs = pack_references(self.references)
-        rows, labels, roff, counts = self._refs
-        h, N, nf = self._args()
-        T = len(params)
-        comp = np.empty((nf, T, 5), dtype=np.float64)
-        dev = 0.0
-        with torch.cuda.device(self.device):
-            st = torch.cuda.current_stream(self.device)
-            for g in trial_groups(T, N):
-                p = np.ascontiguousarray(params[g])
-                part = np.empty((nf, len(p), 5), dtype=np.float64)
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record(st)
-                rc = _lib.lib().dg_sweep_score_files(h, self.seg.data_ptr(), self.emb.data_ptr(), N, nf,
-                                                     self.offsets.ctypes.data, p.ctypes.data, len(p), self.plan.ctypes.data,
-                                                     self.out_start.ctypes.data, self.out_res.ctypes.data,
-                                                     self.shifts.ctypes.data, PATCH_COLLAR, rows.ctypes.data,
-                                                     labels.ctypes.data, roff.ctypes.data, counts.ctypes.data,
-                                                     part.ctypes.data, None, None, 0, st.cuda_stream)
-                e1.record(st)
-                _lib.check(rc)
-                e1.synchronize()
-                dev += e0.elapsed_time(e1) / 1e3
-                comp[:, g] = part
-        self.timing["score"] = dev
-        per_file = [DERComponents.from_array(comp[f]) for f in range(nf)]
-        total = per_file[0]
-        for c in per_file[1:]:
-            total = total + c
-        return per_file, total
+        return self._score(trial_params(trials, self.config))
+
+    def _score_group(self, params: np.ndarray) -> Tuple[np.ndarray, float]:
+        reference = tuple(a.ctypes.data for a in self._refs)       # rows, labels, row offsets, label counts
+        return self._sweep._score_trials(*self._over_files(_lib.lib().dg_sweep_score_files), params,
+                                         self.shifts.ctypes.data, reference)[:2]
+
+    def _components(self, f: int, comp: np.ndarray) -> DERComponents:
+        return DERComponents.from_array(comp)
 
 
 VAD_PARAMS = tuple(hp.name for hp in VoiceActivityDetection.hyper_parameters())   # ("tau_active",)
@@ -686,11 +757,8 @@ class DetectionErrorComponents:
 
     @property
     def detection_error_rate(self) -> np.ndarray:
-        """(false alarm + missed detection) / total per trial, as a fraction; with total = 0: 0 when there is no error,
-        else 1 (pyannote's DetectionErrorRate.compute_metric)"""
-        num = self.false_alarm + self.missed_detection
-        safe = np.where(self.total > 0, self.total, 1.0)
-        return np.where(self.total > 0, num / safe, np.where(num > 0, 1.0, 0.0))
+        """(false alarm + missed detection) / total per trial (:func:`_rate`)"""
+        return _rate(self.false_alarm + self.missed_detection, self.total)
 
     def __add__(self, other: "DetectionErrorComponents") -> "DetectionErrorComponents":
         """the components of several files summed per trial"""
@@ -728,7 +796,7 @@ def pack_speech_references(references: Sequence[Annotation]):
             np.array(totals, dtype=np.float64))
 
 
-class VoiceActivitySweep:
+class VoiceActivitySweep(_DatasetSweep):
     """Tunes ``VoiceActivityDetection``'s ``tau_active`` over a whole dataset with the segmentation run once.
 
         vs = VoiceActivitySweep(vad_config, [("file1", waveform1, reference1), ("file2", waveform2, reference2)])
@@ -745,34 +813,15 @@ class VoiceActivitySweep:
     :class:`DatasetSweep`.  Needs the native segmentation model (``B200PyanNet``).
     """
 
+    _pack_references = staticmethod(pack_speech_references)
+
     def __init__(self, config: VoiceActivityDetectionConfig,
                  files: Iterable[Tuple[Optional[str], np.ndarray, Optional[Annotation]]]):
-        files = list(files)
-        if not files:
-            raise ValueError("at least one file is needed")
-        for i, (uri, x, _) in enumerate(files):
-            if np.asarray(x).size == 0:
-                raise ValueError(f"file {i} ({uri}) has no samples, so no windows")
-        self.config = config
-        self.pipeline = VoiceActivityDetection(config)
-        if not isinstance(getattr(self.pipeline.segmentation.model, "model", None), B200PyanNet):
-            raise _lib.DiartB200Error("VoiceActivitySweep needs the native segmentation model (B200PyanNet)")
-        self.device = self.pipeline.segmentation.device
-        if self.device.index is None:
-            self.device = torch.device("cuda", torch.cuda.current_device())
-        self.uris = [uri for uri, _, _ in files]
-        self.references = [ref for _, _, ref in files]
-        fws = [file_windows(x, config) for _, x, _ in files]
-        self.offsets = np.ascontiguousarray(np.cumsum([0] + [fw.num_windows for fw in fws]), dtype=np.int32)
-        trial_groups(1, int(self.offsets[-1]))                  # a dataset too large for one launch fails here
         self._h: Optional[C.c_void_p] = None
-        t0 = time.perf_counter()
-        self.seg = self._segmentation(fws)
-        torch.cuda.synchronize(self.device)
+        self._turns = np.empty(0, dtype=np.uint32)
+        super().__init__(config, files)
         t1 = time.perf_counter()
         N, F, K = self.seg.shape
-        self.plan, self.out_start, self.out_res = dataset_plan(fws, config, F)
-        self.shifts = np.ascontiguousarray([-fw.padding[0] for fw in fws], dtype=np.float64)
         self.curve_frames = int(np.where(self.plan[:, 2] > 0, self.plan[:, 2], self.plan[:, 1]).sum())
         ham = np.ascontiguousarray(np.hamming(F), dtype=np.float64)
         nw = int(round(config.latency / config.step))
@@ -780,11 +829,9 @@ class VoiceActivitySweep:
         with torch.cuda.device(self.device):
             _lib.check(_lib.lib().dg_vad_sweep_create(F, K, nw, ham.ctypes.data, self.device.index, C.byref(h)))
             self._h = h
-            _lib.check(_lib.lib().dg_vad_sweep_curve(h, self.seg.data_ptr(), N, len(fws), self.offsets.ctypes.data,
+            _lib.check(_lib.lib().dg_vad_sweep_curve(h, self.seg.data_ptr(), N, len(self.uris), self.offsets.ctypes.data,
                                                      self.plan.ctypes.data, _lib.stream_ptr(self.device)))
-        self.timing: Dict[str, float] = {"network": t1 - t0, "curve": time.perf_counter() - t1}
-        self._refs = None
-        self._turns = np.empty(0, dtype=np.uint32)
+        self.timing["curve"] = time.perf_counter() - t1
 
     def __del__(self):
         try:
@@ -793,34 +840,20 @@ class VoiceActivitySweep:
         except Exception:  # noqa: BLE001
             pass
 
-    def _segmentation(self, fws: Sequence[FileWindows]) -> torch.Tensor:
+    def _open(self) -> torch.device:
+        self.pipeline = VoiceActivityDetection(self.config)
+        if not isinstance(getattr(self.pipeline.segmentation.model, "model", None), B200PyanNet):
+            raise _lib.DiartB200Error("VoiceActivitySweep needs the native segmentation model (B200PyanNet)")
+        return _indexed(self.pipeline.segmentation.device)
+
+    def _networks(self, fws: Sequence[FileWindows]):
         """scores (N, F, K) of every window of every file, concatenated in file order, on the device: each file's windows in
         batches cut at the multiples of 256 from its window 0, so that a file's scores are the bits
         ``VoiceActivityDetection`` computes for it in batches of 256"""
-        cfg, seg = self.config, self.pipeline.segmentation
-        streams: List[DeviceAudioStream] = []
-        outs = []
+        seg = self.pipeline.segmentation
+        batches = FileBatches(fws, self.config, self.device)
         with torch.cuda.device(self.device):
-            for i, fw in enumerate(fws):
-                # a few streams in turn: a reset waits for the uploads of its stream (see network_pass_files)
-                if len(streams) < _AUDIO_STREAMS:
-                    streams.append(DeviceAudioStream(cfg.duration, cfg.step, cfg.sample_rate, max_windows=NETWORK_BATCH,
-                                                     device=self.device))
-                stream = streams[i % _AUDIO_STREAMS]
-                if i >= _AUDIO_STREAMS:
-                    stream.reset()
-                pushed = fw.offset
-                for i0 in range(0, fw.num_windows, NETWORK_BATCH):
-                    B = min(NETWORK_BATCH, fw.num_windows - i0)
-                    need = fw.offset + (i0 + B - 1) * fw.step_samples + fw.chunk_samples
-                    stream.push(fw.samples[pushed:need])
-                    pushed = need
-                    outs.append(seg.forward_device(stream.windows(B)))
-            return torch.cat(outs)
-
-    @property
-    def num_chunks(self) -> int:
-        return int(self.offsets[-1])
+            self.seg = torch.cat([seg.forward_device(windows) for windows in batches])
 
     @property
     def resident_bytes(self) -> int:
@@ -839,44 +872,18 @@ class VoiceActivitySweep:
         taus = np.ascontiguousarray(taus, dtype=np.float64)
         T, N = len(taus), self.num_chunks
         header = np.empty((T, N, 4), dtype=np.int32)
-        if len(self._turns) < T * N * 4:
-            self._turns = np.empty(T * N * 4, dtype=np.uint32)
-        n = C.c_int()
-        with torch.cuda.device(self.device):
-            st = torch.cuda.current_stream(self.device)
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            for attempt in range(2):
-                e0.record(st)
-                rc = _lib.lib().dg_vad_sweep_run_files(self._h, taus.ctypes.data, T, header.ctypes.data,
-                                                       self._turns.ctypes.data, len(self._turns), C.byref(n), st.cuda_stream)
-                e1.record(st)
-                if rc == -1 and n.value > len(self._turns):     # more turns than the host buffer: grow it, run again
-                    self._turns = np.empty(n.value, dtype=np.uint32)
-                    continue
-                _lib.check(rc)
-                break
-            e1.synchronize()
-        return SweepOutputs(header, self._turns[:n.value].copy(), n.value, self.out_start, self.out_res,
-                            device_seconds=e0.elapsed_time(e1) / 1e3)
+        n_turns, seconds = _turn_list_call(self, self.device, T * N * 4, lambda *turn_list: _lib.lib().dg_vad_sweep_run_files(
+            self._h, taus.ctypes.data, T, header.ctypes.data, *turn_list))
+        return SweepOutputs(header, self._turns[:n_turns].copy(), n_turns, self.out_start, self.out_res,
+                            device_seconds=seconds)
 
     def run(self, trials: Sequence[Mapping[str, float]] = ({},)) -> List[List[Annotation]]:
         """-> predictions [file][trial]: for each file and trial what ``Benchmark.run_single`` returns for
         ``VoiceActivityDetection`` with that tau_active (label "speech", modality "speech", the file's uri)"""
-        taus = self._taus(trials)
-        out: List[List[Annotation]] = [[] for _ in self.uris]
-        dev = 0.0
-        for g in trial_groups(len(taus), self.num_chunks):
-            r = self.binarize(taus[g])
-            dev += r.device_seconds
-            for f in range(len(self.uris)):
-                c0, c1 = int(self.offsets[f]), int(self.offsets[f + 1])
-                header, turns, n = file_turns(r.header, r.turns, c0, c1)
-                preds = assemble_predictions(header, turns, n, self.out_start[c0:c1], self.out_res[c0:c1], ["speech"],
-                                             float(self.shifts[f]), self.uris[f])
-                for p in preds:            # the per-chunk VAD annotations carry modality "speech" whatever the shift
-                    p.modality = "speech"
-                out[f] += preds
-        self.timing["sweep"] = dev
+        out = self._run(self._taus(trials), self.binarize, ["speech"])
+        for preds in out:
+            for p in preds:                # the per-chunk VAD annotations carry modality "speech" whatever the shift
+                p.modality = "speech"
         return out
 
     def score(self, trials: Sequence[Mapping[str, float]] = ({},)) \
@@ -885,36 +892,18 @@ class VoiceActivitySweep:
         predictions against each file's reference (``DetectionErrorRate(collar=0, skip_overlap=False)``, no uem); the
         minimum of ``total.detection_error_rate`` is the trial ``Optimizer.objective`` would pick.  Every file needs a
         reference."""
-        missing = [self.uris[i] if self.uris[i] is not None else i for i, r in enumerate(self.references) if r is None]
-        if missing:
-            raise ValueError(f"files without a reference cannot be scored: {missing}")
-        taus = self._taus(trials)
-        if self._refs is None:
-            self._refs = pack_speech_references(self.references)
-        rows, roff, totals = self._refs
-        T, nf = len(taus), len(self.uris)
-        comp = np.empty((nf, T, 2), dtype=np.float64)
-        dev = 0.0
-        with torch.cuda.device(self.device):
-            st = torch.cuda.current_stream(self.device)
-            for g in trial_groups(T, self.num_chunks):
-                p = np.ascontiguousarray(taus[g])
-                part = np.empty((nf, len(p), 2), dtype=np.float64)
-                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                e0.record(st)
-                rc = _lib.lib().dg_vad_sweep_score_files(self._h, p.ctypes.data, len(p), self.out_start.ctypes.data,
-                                                         self.out_res.ctypes.data, self.shifts.ctypes.data, PATCH_COLLAR,
-                                                         rows.ctypes.data, roff.ctypes.data, part.ctypes.data,
-                                                         st.cuda_stream)
-                e1.record(st)
-                _lib.check(rc)
-                e1.synchronize()
-                dev += e0.elapsed_time(e1) / 1e3
-                comp[:, g] = part
-        self.timing["score"] = dev
-        per_file = [DetectionErrorComponents(comp[f, :, 0].copy(), comp[f, :, 1].copy(), np.full(T, totals[f]))
-                    for f in range(nf)]
-        total = per_file[0]
-        for c in per_file[1:]:
-            total = total + c
-        return per_file, total
+        return self._score(self._taus(trials))
+
+    def _score_group(self, taus: np.ndarray) -> Tuple[np.ndarray, float]:
+        rows, roff, _ = self._refs
+        taus = np.ascontiguousarray(taus)
+        part = np.empty((len(self.uris), len(taus), 2), dtype=np.float64)
+        rc, seconds = _timed(self.device, lambda st: _lib.lib().dg_vad_sweep_score_files(
+            self._h, taus.ctypes.data, len(taus), self.out_start.ctypes.data, self.out_res.ctypes.data,
+            self.shifts.ctypes.data, PATCH_COLLAR, rows.ctypes.data, roff.ctypes.data, part.ctypes.data, st))
+        _lib.check(rc)
+        return part, seconds()
+
+    def _components(self, f: int, comp: np.ndarray) -> DetectionErrorComponents:
+        """false alarm and missed detection from the device; the total is the reference's duration, whatever the trial"""
+        return DetectionErrorComponents(comp[:, 0].copy(), comp[:, 1].copy(), np.full(len(comp), self._refs[2][f]))
