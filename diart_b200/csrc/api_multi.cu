@@ -2,7 +2,9 @@
 // step, SpeakerDiarization.__call__ with a batch of one, diarization.py:172-232) for up to `slots` streams at once, batched
 // across the streams.  Work happens in ticks: every open stream contributes its complete, unconsumed windows (at most
 // max_wps), and those windows run as ONE batch -- one upload, one network pass (in sub-batches on the two scratch lanes),
-// one clustering launch with a state per stream, one post-path launch with a history per stream, one download.
+// one clustering launch with a state per stream, one post-path launch with a history per stream, one download.  Each stream
+// may have its own latency (num_windows, up to the handle's) and {tau, rho, delta} (dg_multi_open_config): none of them
+// reaches the networks, so the clustering runs each state at its stream's row and the post-path each chunk at its stream's.
 //
 // A VAD handle (dg_multi_create_vad) serves the reference's VoiceActivityDetection the same way: the same audio in, the
 // segmentation network alone, and per stream its speech curve (max over the local speakers) aggregated and binarised on the
@@ -148,7 +150,7 @@ struct SlotBook {
       const int n = open[s] ? (int)std::min<long long>(available(s), max_wps) : 0;
       if (!n) continue;
       const RateGeom& r = geom(s);
-      t.act.push_back(TickSlot{s, t.B, n, 0, 0, {0, 0, 0}});
+      t.act.push_back(TickSlot{s, t.B, n, 0, 0, 1, {0, 0}});
       long long d = done[s];
       for (int i = 0; i < n; i++) {
         const long long st = rpos[s] + (long long)i * r.hop;
@@ -195,12 +197,14 @@ struct SlotBook {
 struct dg_multi {
   int device = 0, slots = 0, max_wps = 0;
   int S = 0, hop = 0;                         // samples per window, between windows
-  int F = 0, K = 0, D = 0, M = 0, nw = 1;
-  double tau = 0.5, rho = 0.3, delta = 1.0;
+  int F = 0, K = 0, D = 0, M = 0, nw = 1;     // nw: the largest latency / step of any stream (sizes the histories)
+  double tau = 0.5, rho = 0.3, delta = 1.0;   // the values of a stream opened without its own
   NetLanes net;
   SlotBook book;
   PinnedBuf stage;                            // staged samples [0, book.n_staged), then a tick's tables
   std::vector<int> n_hist, cur;               // per slot: post-path history entries, current copy
+  std::vector<int> slot_nw;                   // per slot: its stream's latency / step (<= nw)
+  std::vector<double> slot_par;               // per slot [3]: its stream's {tau, rho, delta} (a VAD handle: {tau, 0, 0})
   DevBuf yrings;                              // resampled streams: 16 kHz rings [slots][Y]
   long long Y = 0;
   bool opened = false;                        // a stream was opened (rates can no longer be added)
@@ -263,7 +267,7 @@ extern "C" int dg_multi_create(dg_seg* seg, dg_emb* emb, int chunk_samples, int 
   h->net.seg = seg; h->net.emb = emb;
   h->net.gamma = gamma; h->net.beta = beta; h->net.normalize_weights = normalize_weights;
   const size_t n = (size_t)max_streams, hist = (size_t)std::max(1, num_windows - 1);
-  h->n_hist.assign(n, 0); h->cur.assign(n, 0);
+  h->n_hist.assign(n, 0); h->cur.assign(n, 0); h->slot_nw.assign(n, num_windows); h->slot_par.assign(3 * n, 0.0);
   if (h->rings.ensure(n * h->book.C * 4) || h->hamming.ensure((size_t)F * 8) || h->centers.ensure(n * max_speakers * D * 8) ||
       h->active.ensure(n * 32 * 4) || h->init.ensure(n * 2 * 4) || h->hist_seg.ensure(2 * n * hist * F * K * 4) ||
       h->hist_map.ensure(2 * n * hist * K * 4) || h->total.ensure(16))
@@ -312,7 +316,7 @@ extern "C" int dg_multi_create_vad(dg_seg* seg, int chunk_samples, int step_samp
   h->tau = tau;
   h->net.seg = seg;
   const size_t n = (size_t)max_streams, hist = (size_t)std::max(1, num_windows - 1);
-  h->n_hist.assign(n, 0); h->cur.assign(n, 0);
+  h->n_hist.assign(n, 0); h->cur.assign(n, 0); h->slot_nw.assign(n, num_windows); h->slot_par.assign(3 * n, 0.0);
   if (h->rings.ensure(n * h->book.C * 4) || h->hamming.ensure((size_t)F * 8) || h->hist_vad.ensure(2 * n * hist * F * 4) ||
       h->total.ensure(16))
     return DG_ECUDA;
@@ -363,15 +367,26 @@ extern "C" int dg_multi_add_rate(dg_multi* h, dg_resample* rs, int chunk_samples
   return DG_OK;
 }
 
-// a new stream in `slot` at declared rate `rate_id` (-1: the pipeline's rate): empty rings, fresh clustering state (the
-// reference's SpeakerDiarization.reset(); a VAD handle has none), no history
-extern "C" int dg_multi_open_rate(dg_multi* h, int slot, int rate_id) {
+// a new stream in `slot` at declared rate `rate_id` (-1: the pipeline's rate), aggregating num_windows buffers, with
+// params {tau, rho, delta} (a VAD handle reads tau only): empty rings, fresh clustering state (the reference's
+// SpeakerDiarization.reset(); a VAD handle has none), no history.  Every argument is checked first; a refusal names `who`.
+static int open_slot(dg_multi* h, int slot, int rate_id, int num_windows, const double* params, const char* who) {
   if (!h || slot < 0 || slot >= h->slots || h->book.open[slot]) {
-    set_error("dg_multi_open: slot " + std::to_string(slot) + " is out of range or already open");
+    set_error(std::string(who) + ": slot " + std::to_string(slot) + " is out of range or already open");
     return DG_EINVAL;
   }
   if (rate_id < -1 || rate_id + 1 >= (int)h->book.rates.size()) {
-    set_error("dg_multi_open: rate " + std::to_string(rate_id) + " was not declared");
+    set_error(std::string(who) + ": rate " + std::to_string(rate_id) + " was not declared");
+    return DG_EINVAL;
+  }
+  if (num_windows < 1 || num_windows > h->nw) {
+    set_error(std::string(who) + ": num_windows " + std::to_string(num_windows) + " is outside [1, " + std::to_string(h->nw) +
+              "], the handle's maximum");
+    return DG_EINVAL;
+  }
+  const bool vad = vad_mode(h);
+  if (!params || !std::isfinite(params[0]) || (!vad && (!std::isfinite(params[1]) || !std::isfinite(params[2])))) {
+    set_error(std::string(who) + (vad ? ": need a finite tau" : ": need finite tau, rho and delta"));
     return DG_EINVAL;
   }
   DG_CUDA(cudaSetDevice(h->device));
@@ -383,8 +398,25 @@ extern "C" int dg_multi_open_rate(dg_multi* h, int slot, int rate_id) {
   }
   h->book.start(slot, rate_id + 1);
   h->n_hist[slot] = 0;
+  h->slot_nw[slot] = num_windows;
+  h->slot_par[3 * (size_t)slot + 0] = params[0];
+  h->slot_par[3 * (size_t)slot + 1] = vad ? 0.0 : params[1];
+  h->slot_par[3 * (size_t)slot + 2] = vad ? 0.0 : params[2];
   h->opened = true;
   return DG_OK;
+}
+
+extern "C" int dg_multi_open_config(dg_multi* h, int slot, int rate_id, int num_windows, const double* params) {
+  return open_slot(h, slot, rate_id, num_windows, params, "dg_multi_open_config");
+}
+
+extern "C" int dg_multi_open_rate(dg_multi* h, int slot, int rate_id) {
+  if (!h) {
+    set_error("dg_multi_open: null handle");
+    return DG_EINVAL;
+  }
+  const double params[3] = {h->tau, h->rho, h->delta};
+  return open_slot(h, slot, rate_id, h->nw, params, "dg_multi_open");
 }
 
 extern "C" int dg_multi_open(dg_multi* h, int slot) { return dg_multi_open_rate(h, slot, -1); }
@@ -436,9 +468,10 @@ extern "C" int dg_multi_push_host(dg_multi* h, int slot, const float* samples, i
 static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
 
 // Where the tables of a tick lie in its one host -> device copy (byte offsets into h->in): staged samples at 0, pieces [np],
-// slots [n_act], rows [B] {slot entry, window}, window starts [B], plan [B][stride], cluster states [n_act] {slot, 0}, chunk
-// offsets [slots + 1] by slot, thresholds [3] (the last three are read by a diarization tick only).  A tick with resampled rows
-// also carries the rows at the pipeline's rate [n16] with their starts, the resampling items and the resampled rows.
+// slots [n_act], rows [B] {slot entry, window}, window starts [B], plan [B][stride], cluster states [n_act] {slot, entry},
+// chunk offsets [slots + 1] by slot (states and offsets are read by a diarization tick only), thresholds [n_act][3] {tau, rho,
+// delta} of each slot entry.  A tick with resampled rows also carries the rows at the pipeline's rate [n16] with their starts,
+// the resampling items and the resampled rows.
 struct TickIn {
   size_t o_pieces, o_act, o_rows, o_start, o_plan, o_states, o_off, o_trials, o_rows16, o_start16, o_items, o_rs, bytes;
   bool mixed;
@@ -461,11 +494,11 @@ static int tick_audio_in(dg_multi* h, const TickPlan& tp, const int32_t* plan_ho
   L.o_trials = L.o_off + align16((size_t)(h->slots + 1) * 4);
   L.mixed = !tp.rs_rows.empty();
   const int n16 = (int)tp.rows16.size(), n_items = (int)tp.items.size(), n_rs = (int)tp.rs_rows.size();
-  L.o_rows16 = L.o_trials + 32;
+  L.o_rows16 = L.o_trials + align16((size_t)n_act * 24);
   L.o_start16 = L.o_rows16 + align16((size_t)n16 * 8);
   L.o_items = L.o_start16 + align16((size_t)n16 * 8);
   L.o_rs = L.o_items + align16((size_t)n_items * sizeof(RsFrames));
-  L.bytes = L.mixed ? L.o_rs + (size_t)n_rs * sizeof(RsRow) : L.o_trials + 24;
+  L.bytes = L.mixed ? L.o_rs + (size_t)n_rs * sizeof(RsRow) : L.o_trials + (size_t)n_act * 24;
   if (h->in.ensure(L.bytes) || h->wav.ensure((size_t)B * S * 4)) return DG_ECUDA;
   if (L.bytes > h->stage.bytes) {
     PinnedBuf bigger;
@@ -480,10 +513,12 @@ static int tick_audio_in(dg_multi* h, const TickPlan& tp, const int32_t* plan_ho
   memcpy(pin + L.o_start, tp.start.data(), (size_t)B * 8);
   int2* states = reinterpret_cast<int2*>(pin + L.o_states);
   int32_t* off = reinterpret_cast<int32_t*>(pin + L.o_off);
+  double* trials = reinterpret_cast<double*>(pin + L.o_trials);
   for (int a = 0, s = 0; a < n_act; a++) {
     const TickSlot& ts = act[a];
     for (; s <= ts.slot; s++) off[s] = ts.row0;
-    states[a] = make_int2(ts.slot, 0);
+    states[a] = make_int2(ts.slot, a);
+    memcpy(trials + 3 * (size_t)a, &h->slot_par[3 * (size_t)ts.slot], 24);
   }
   if (L.mixed) {
     if (n16) memcpy(pin + L.o_rows16, tp.rows16.data(), (size_t)n16 * 8);
@@ -493,8 +528,6 @@ static int tick_audio_in(dg_multi* h, const TickPlan& tp, const int32_t* plan_ho
   }
   for (int s = act.back().slot + 1; s <= h->slots; s++) off[s] = B;
   memcpy(pin + L.o_plan, plan_host, (size_t)B * stride * 4);
-  const double trials[3] = {h->tau, h->rho, h->delta};
-  memcpy(pin + L.o_trials, trials, 24);
   unsigned char* din = h->in.as<unsigned char>();
   DG_CUDA(cudaEventRecord(h->t_begin, st));
   DG_CUDA(cudaMemcpyAsync(din, pin, L.bytes, cudaMemcpyHostToDevice, st));
@@ -553,21 +586,22 @@ static int tick_diarize(dg_multi* h, const TickPlan& tp, const TickIn& L, int tu
     DG_CUDA(cudaEventRecord(h->e_lane_done[lane], h->net.s_emb));
   }
   DG_CUDA(cudaStreamWaitEvent(st, h->net.e_emb, 0));
-  // clustering: state `slot` over that slot's rows (chunk offsets by slot), cosine
+  // clustering: state `slot` over that slot's rows (chunk offsets by slot), cosine, at the thresholds of its entry's row
+  const double* trials = reinterpret_cast<const double*>(din + L.o_trials);
   ClusterParams p{};
   p.M = M;
   p.D = D;
   p.metric = 0;
-  if ((rc = launch_cluster_sweep(p, reinterpret_cast<const double*>(din + L.o_trials), 1,
-                                 reinterpret_cast<const int2*>(din + L.o_states), n_act, reinterpret_cast<const int*>(din + L.o_off),
-                                 h->seg.as<float>(), h->emb.as<float>(), B, F, K, h->centers.as<double>(), h->active.as<int>(),
-                                 h->init.as<int>(), h->prep.as<float>(), h->prep_d.as<double>(), h->maps.as<int32_t>(), st)))
+  if ((rc = launch_cluster_sweep(p, trials, n_act, reinterpret_cast<const int2*>(din + L.o_states), n_act,
+                                 reinterpret_cast<const int*>(din + L.o_off), h->seg.as<float>(), h->emb.as<float>(), B, F, K,
+                                 h->centers.as<double>(), h->active.as<int>(), h->init.as<int>(), h->prep.as<float>(),
+                                 h->prep_d.as<double>(), h->maps.as<int32_t>(), st, true)))
     return rc;
-  // post-path with each slot's history, then the histories move on
+  // post-path with each slot's history and tau, then the histories move on
   DG_CUDA(cudaMemsetAsync(h->total.p, 0, 4, st));
   if ((rc = launch_post_slots(h->seg.as<float>(), h->maps.as<int32_t>(), h->hist_seg.as<float>(), h->hist_map.as<int32_t>(),
                               d_act, d_rows, h->slots, B, F, K, M, h->nw, reinterpret_cast<const int32_t*>(din + L.o_plan),
-                              4 + h->nw, h->hamming.as<double>(), h->tau, h->header.as<int32_t>(), h->turns.as<uint32_t>(),
+                              4 + h->nw, h->hamming.as<double>(), trials, h->header.as<int32_t>(), h->turns.as<uint32_t>(),
                               turn_cap, h->total.as<unsigned int>(), st)) ||
       (rc = launch_post_slots_history(h->seg.as<float>(), h->maps.as<int32_t>(), h->hist_seg.as<float>(),
                                       h->hist_map.as<int32_t>(), d_act, n_act, h->slots, F, K, h->nw, st)))
@@ -599,12 +633,12 @@ static int tick_vad(dg_multi* h, const TickPlan& tp, const TickIn& L, int turn_c
     DG_CUDA(cudaEventRecord(h->e_lane_done[lane], s_seg));
   }
   for (int lane = 0; lane < 2; lane++) DG_CUDA(cudaStreamWaitEvent(st, h->e_lane_done[lane], 0));
-  // speech curves with each slot's history, then the histories move on
+  // speech curves with each slot's history and tau, then the histories move on
   DG_CUDA(cudaMemsetAsync(h->total.p, 0, 4, st));
   if ((rc = launch_vad_slots(h->seg.as<float>(), h->hist_vad.as<float>(), d_act, reinterpret_cast<const int2*>(din + L.o_rows),
                              h->slots, B, F, K, h->nw, reinterpret_cast<const int32_t*>(din + L.o_plan), 4 + h->nw,
-                             h->hamming.as<double>(), h->tau, h->header.as<int32_t>(), h->turns.as<uint32_t>(), turn_cap,
-                             h->total.as<unsigned int>(), st)) ||
+                             h->hamming.as<double>(), reinterpret_cast<const double*>(din + L.o_trials),
+                             h->header.as<int32_t>(), h->turns.as<uint32_t>(), turn_cap, h->total.as<unsigned int>(), st)) ||
       (rc = launch_vad_slots_history(h->seg.as<float>(), h->hist_vad.as<float>(), d_act, n_act, h->slots, F, K, h->nw, st)))
     return rc;
   return DG_OK;
@@ -632,6 +666,7 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
     counts_host[ts.slot] = ts.n;
     ts.cur = h->cur[ts.slot];
     ts.n_hist = h->n_hist[ts.slot];
+    ts.nw = h->slot_nw[ts.slot];
   }
   if (n_rows != B) {
     set_error(std::string(who) + ": " + std::to_string(n_rows) + " plan rows given, the tick has " + std::to_string(B) +
@@ -639,13 +674,13 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
     return DG_EINVAL;
   }
   const int stride = 4 + h->nw;
-  // plan rows post.cu accepts: 1 <= nb <= nw buffers, none before the stream's first chunk, 1 <= frames, at most F + 1 output
-  // frames (the first chunk's crop of [0, region end))
+  // plan rows post.cu accepts: 1 <= nb <= the stream's nw buffers, none before the stream's first chunk, 1 <= frames, at most
+  // F + 1 output frames (the first chunk's crop of [0, region end))
   for (const TickSlot& ts : act)
     for (int i = 0; i < ts.n; i++) {
       const int32_t* pl = plan_host + (size_t)(ts.row0 + i) * stride;
       const int nb = pl[0], nf = pl[1], nfo = pl[2] > 0 ? pl[2] : nf;
-      if (nb < 1 || nb > h->nw || nb - 1 > ts.n_hist + i || nf < 1 || pl[2] < 0 || nfo > h->F + 1) {
+      if (nb < 1 || nb > ts.nw || nb - 1 > ts.n_hist + i || nf < 1 || pl[2] < 0 || nfo > h->F + 1) {
         set_error(std::string(who) + ": plan row " + std::to_string(ts.row0 + i) + " is not a plan of its stream (buffers " +
                   std::to_string(nb) + ", frames " + std::to_string(nfo) + ")");
         return DG_EINVAL;
@@ -686,7 +721,7 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
   h->book.consumed(tp);
   for (const TickSlot& ts : act) {
     if (h->nw > 1) {
-      h->n_hist[ts.slot] = std::min(h->nw - 1, ts.n_hist + ts.n);
+      h->n_hist[ts.slot] = std::min(ts.nw - 1, ts.n_hist + ts.n);
       h->cur[ts.slot] ^= 1;
     }
   }

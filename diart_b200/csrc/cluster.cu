@@ -111,9 +111,10 @@ constexpr int SWEEP_THREADS = 256;      // many independent states (hyper-parame
 // [chunk_off[f], chunk_off[f + 1]) of the B concatenated ones, with {tau, rho, delta} = trials [t] (float64); state
 // s = f T + t owns centroid table s ([M][D] at centers + s M D), active flags s ([32]) and the `initialized` / error pair s,
 // and writes the map rows of its chunks in trial t's block ([B][K] at map_out + t B K).  Outputs are addressed by (f, t),
-// so the launch order (the order of `states`) changes no result.  The arithmetic does not depend on THREADS: each
-// centroid's distances are one warp's, the updates are element-wise.
-template <int THREADS, bool STATES>
+// so the launch order (the order of `states`) changes no result.  OWN_ROWS (STATES only; many live streams, each at its own
+// thresholds, dg_multi): t is only the row of `trials`, state s = f, and every state's maps go to block 0.  The arithmetic
+// does not depend on THREADS: each centroid's distances are one warp's, the updates are element-wise.
+template <int THREADS, bool STATES, bool OWN_ROWS = false>
 __global__ void __launch_bounds__(THREADS)
 cluster_seq_kernel(ClusterParams p, const double* __restrict__ trials, const int2* __restrict__ states,
                    const int* __restrict__ chunk_off, int T, const float* __restrict__ seg,
@@ -135,11 +136,11 @@ cluster_seq_kernel(ClusterParams p, const double* __restrict__ trials, const int
   if constexpr (STATES) {
     const int2 fs = states[blockIdx.x];
     const int trial = fs.y, c0 = chunk_off[fs.x];
-    const size_t s = (size_t)fs.x * T + trial;
+    const size_t s = OWN_ROWS ? (size_t)fs.x : (size_t)fs.x * T + trial;
     centers += s * M * D;
     g_active += s * CM;
     g_init += s * 2;
-    map_out += ((size_t)trial * B + c0) * K;
+    map_out += ((size_t)(OWN_ROWS ? 0 : trial) * B + c0) * K;
     B = chunk_off[fs.x + 1] - c0;              // from here on: this file's chunks, the first at c0
     first = c0;
     // numpy compares the float32 scores with a Python float in float32 (as dg_cluster_create)
@@ -430,11 +431,12 @@ static int check_cluster_shape(const char* who, const ClusterParams& p, int K) {
   return 0;
 }
 
-template <int THREADS, bool STATES>
+template <int THREADS, bool STATES, bool OWN_ROWS = false>
 static int cluster_seq_allow_dyn() {   // per device: the opt-in above 48 KB is a property of (function, device)
   static bool attr_done[64] = {};
   if (first_use_on_device(attr_done))
-    DG_CUDA(cudaFuncSetAttribute(cluster_seq_kernel<THREADS, STATES>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    DG_CUDA(cudaFuncSetAttribute(cluster_seq_kernel<THREADS, STATES, OWN_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 200 * 1024));
   return 0;
 }
 
@@ -482,16 +484,25 @@ int launch_cluster_step(const ClusterParams& p, const float* seg, const float* e
 // beyond the resident CTAs run in later waves of the same launch.
 int launch_cluster_sweep(const ClusterParams& p, const double* trials_dev, int T, const int2* states_dev, int S,
                          const int* chunk_off_dev, const float* seg, const float* emb, int B, int F, int K, double* centers,
-                         int* active, int* initialized, float* prep, double* prep_d, int32_t* maps, cudaStream_t st) {
+                         int* active, int* initialized, float* prep, double* prep_d, int32_t* maps, cudaStream_t st,
+                         bool own_rows) {
   ProfScope _ps("cluster_sweep", st);
   if (check_cluster_shape("cluster_sweep", p, K)) return -1;
   if (B <= 0 || S <= 0) return 0;
   cluster_prep_kernel<<<B, 128, 0, st>>>(seg, emb, F, K, p.D, prep, prep_d);
   DG_LAUNCHED();
-  if (int rc = cluster_seq_allow_dyn<SWEEP_THREADS, true>()) return rc;
-  cluster_seq_kernel<SWEEP_THREADS, true><<<S, SWEEP_THREADS, cluster_seq_dyn(p.M, p.D, K), st>>>(
-      p, trials_dev, states_dev, chunk_off_dev, T, seg, emb, B, F, K, centers, active, initialized, prep, prep_d, maps,
-      nullptr, nullptr);
+  const size_t dyn = cluster_seq_dyn(p.M, p.D, K);
+  if (own_rows) {
+    if (int rc = cluster_seq_allow_dyn<SWEEP_THREADS, true, true>()) return rc;
+    cluster_seq_kernel<SWEEP_THREADS, true, true><<<S, SWEEP_THREADS, dyn, st>>>(
+        p, trials_dev, states_dev, chunk_off_dev, T, seg, emb, B, F, K, centers, active, initialized, prep, prep_d, maps,
+        nullptr, nullptr);
+  } else {
+    if (int rc = cluster_seq_allow_dyn<SWEEP_THREADS, true>()) return rc;
+    cluster_seq_kernel<SWEEP_THREADS, true><<<S, SWEEP_THREADS, dyn, st>>>(
+        p, trials_dev, states_dev, chunk_off_dev, T, seg, emb, B, F, K, centers, active, initialized, prep, prep_d, maps,
+        nullptr, nullptr);
+  }
   DG_LAUNCHED();
   return 0;
 }

@@ -262,10 +262,12 @@ int launch_relabel_maps(int32_t* maps, int n, const int32_t* relabel, cudaStream
 // states = (file, trial) pairs over the concatenated chunks of several files: file f owns chunks
 // [chunk_off[f], chunk_off[f + 1]) of B; thresholds trials_dev [T][3] = {tau, rho, delta} float64; one CTA per entry of
 // states_dev [S] {file, trial} (the launch order); state s = file * T + trial owns centers [s][M][D], active [s][32] and
-// initialized [s][2]; maps [T][B][K]
+// initialized [s][2]; maps [T][B][K].  own_rows (many streams, each at its own thresholds): trial only selects the row of
+// trials_dev, state s = file owns the tables and every state writes maps [B][K]
 int launch_cluster_sweep(const ClusterParams& p, const double* trials_dev, int T, const int2* states_dev, int S,
                          const int* chunk_off_dev, const float* seg, const float* emb, int B, int F, int K, double* centers,
-                         int* active, int* initialized, float* prep, double* prep_d, int32_t* maps, cudaStream_t st);
+                         int* active, int* initialized, float* prep, double* prep_d, int32_t* maps, cudaStream_t st,
+                         bool own_rows = false);
 size_t cluster_prep_floats(int B, int K);
 // post.cu -- aggregation + binarisation + run-length turns (reference diarization.py:205-232)
 int launch_post(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map, int n_hist, int B,
@@ -277,22 +279,24 @@ int launch_post_history(const float* seg, const int32_t* map, const float* hist_
                         int B, int F, int K, int keep, float* new_seg, int32_t* new_map, cudaStream_t st);
 // post.cu -- many live streams in one batch (dg_multi).  A piece of the staging upload: n samples at staged[src] belong at
 // absolute sample dst of slot `slot`.  A slot with windows in the batch: its n windows are rows [row0, row0 + n); its post-path
-// history is copy `cur` of the two, with n_hist chunks.
+// history is copy `cur` of the two, with n_hist chunks, of which it keeps at most nw - 1 (nw = its stream's latency / step).
 struct RingPiece {
   long long src, dst;
   int slot, n;
 };
 struct TickSlot {
-  int slot, row0, n, cur, n_hist, pad[3];
+  int slot, row0, n, cur, n_hist, nw, pad[2];
 };
 int launch_ring_scatter(const float* staged, const RingPiece* pieces, int n_pieces, int C, float* rings, cudaStream_t st);
 // rows [B] = {entry of act, window index i within that slot's rows}; entry b = samples [start[b], start[b] + S) of its slot's
 // ring, written to batch row act[rows[b].x].row0 + i (any subset of a tick's rows can be gathered)
 int launch_ring_gather(const float* rings, int C, const TickSlot* act, const int2* rows, const long long* start, int S, int B,
                        float* wav, cudaStream_t st);
+// nw: the largest latency / step of any slot (the history stride is nw - 1); params [n_act][3]: {tau, rho, delta} of each
+// entry of act, float64 (the post-path reads tau)
 int launch_post_slots(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map,
                       const TickSlot* act, const int2* rows, int slots, int B, int F, int K, int M, int nw,
-                      const int32_t* plan, int plan_stride, const double* hamming, double tau, int32_t* header,
+                      const int32_t* plan, int plan_stride, const double* hamming, const double* params, int32_t* header,
                       uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st);
 int launch_post_slots_history(const float* seg, const int32_t* map, float* hist_seg, int32_t* hist_map, const TickSlot* act,
                               int n_act, int slots, int F, int K, int nw, cudaStream_t st);
@@ -320,8 +324,8 @@ int launch_vad_binarize(const double* curve, const long long* curve_off, int N, 
 // vad.cu -- many live VAD streams (dg_multi): chunks grouped by slot as launch_post_slots, one speech curve per chunk, each
 // slot's history of max curves hist_vad [2][slots][nw - 1][F]
 int launch_vad_slots(const float* seg, const float* hist_vad, const TickSlot* act, const int2* rows, int slots, int B, int F,
-                     int K, int nw, const int32_t* plan, int plan_stride, const double* hamming, double tau, int32_t* header,
-                     uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st);
+                     int K, int nw, const int32_t* plan, int plan_stride, const double* hamming, const double* params,
+                     int32_t* header, uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st);
 int launch_vad_slots_history(const float* seg, float* hist_vad, const TickSlot* act, int n_act, int slots, int F, int K, int nw,
                              cudaStream_t st);
 // resample.cu -- polyphase sinc resampling (torchaudio's defaults): reduced ratio o / n, half-width w, T = 2w + o taps per phase

@@ -133,17 +133,21 @@ post_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map, cons
 
 // Many streams in one batch (dg_multi): the B chunks are grouped by stream slot.  Chunk c is window rows[c].y of this batch's
 // slot entry act[rows[c].x] (TickSlot, dg_common.cuh), whose chunks start at batch row row0.  Each slot has its own history of
-// up to nw - 1 chunks: hist_seg [2][slots][nw - 1][F][K] and hist_map [2][slots][nw - 1][K] (two copies, `cur` is the
-// current one), of which the first n_hist entries hold the last chunks seen, oldest first.
+// up to ts.nw - 1 <= nw - 1 chunks: hist_seg [2][slots][nw - 1][F][K] and hist_map [2][slots][nw - 1][K] (two copies, `cur`
+// is the current one), of which the first n_hist entries hold the last chunks seen, oldest first.  nw is the largest of the
+// slots' (it sizes the history and the shared memory); a chunk aggregates the nb <= ts.nw buffers of its plan row and
+// compares with its entry's tau, params[3 * rows[c].x], the value a dedicated post-path at that stream's tau_active compares
+// with.
 __global__ void __launch_bounds__(POST_THREADS)
 post_slots_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map, const float* __restrict__ hist_seg,
                   const int32_t* __restrict__ hist_map, const TickSlot* __restrict__ act, const int2* __restrict__ rows,
                   int slots, int F, int K, int M, int nw, const int32_t* __restrict__ plan, int plan_stride,
-                  const double* __restrict__ hamming, double tau, int32_t* __restrict__ header, uint32_t* __restrict__ turns,
-                  int turn_cap, unsigned int* __restrict__ total) {
+                  const double* __restrict__ hamming, const double* __restrict__ params, int32_t* __restrict__ header,
+                  uint32_t* __restrict__ turns, int turn_cap, unsigned int* __restrict__ total) {
   const int c = blockIdx.x;
   const int2 r = rows[c];
   const TickSlot ts = act[r.x];
+  const double tau = params[(size_t)r.x * 3];
   const int32_t* pl = plan + (size_t)c * plan_stride;
   const int nb = pl[0], nf = pl[1], first_nf = pl[2], first_lo = pl[3];
   const size_t h0 = ((size_t)ts.cur * slots + ts.slot) * (nw - 1) + ts.n_hist;   // one past the slot's newest history entry
@@ -160,14 +164,14 @@ post_slots_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map
 }
 
 // History update of the slots of a dg_multi batch: CTA (a, i) writes entry i of slot act[a]'s other history copy, the last
-// keep = min(nw - 1, n_hist + n) chunks of (its history + its n chunks of this batch).  The host then flips `cur` and sets
-// n_hist = keep.
+// keep = min(ts.nw - 1, n_hist + n) chunks of (its history + its n chunks of this batch); the stride of the entries is the
+// largest slot's nw - 1.  The host then flips `cur` and sets n_hist = keep.
 __global__ void __launch_bounds__(256)
 post_slots_history_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map, float* __restrict__ hist_seg,
                           int32_t* __restrict__ hist_map, const TickSlot* __restrict__ act, int slots, int FK, int K, int nw) {
   const TickSlot ts = act[blockIdx.x];
   const int i = blockIdx.y;
-  const int keep = min(nw - 1, ts.n_hist + ts.n);
+  const int keep = min(ts.nw - 1, ts.n_hist + ts.n);
   if (i >= keep) return;
   const int v = ts.n - keep + i;                    // virtual chunk: v >= 0 is this batch's, v < 0 the history's
   const size_t src = ((size_t)ts.cur * slots + ts.slot) * (nw - 1) + ts.n_hist;
@@ -310,7 +314,7 @@ int launch_ring_gather(const float* rings, int C, const TickSlot* act, const int
 
 int launch_post_slots(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map,
                       const TickSlot* act, const int2* rows, int slots, int B, int F, int K, int M, int nw,
-                      const int32_t* plan, int plan_stride, const double* hamming, double tau, int32_t* header,
+                      const int32_t* plan, int plan_stride, const double* hamming, const double* params, int32_t* header,
                       uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st) {
   ProfScope _ps("post_slots", st);
   if (M > 64 || F > 1023 || K > 127) {
@@ -327,7 +331,7 @@ int launch_post_slots(const float* seg, const int32_t* map, const float* hist_se
   if (smem > 48 * 1024 && first_use_on_device(attr_done))
     DG_CUDA(cudaFuncSetAttribute(post_slots_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   post_slots_kernel<<<B, POST_THREADS, smem, st>>>(seg, map, hist_seg, hist_map, act, rows, slots, F, K, M, nw, plan,
-                                                   plan_stride, hamming, tau, header, turns, turn_cap, total);
+                                                   plan_stride, hamming, params, header, turns, turn_cap, total);
   DG_LAUNCHED();
   return 0;
 }

@@ -112,17 +112,19 @@ vad_binarize_kernel(const double* __restrict__ curve, const long long* __restric
 // act[rows[c].x], as in post_slots_kernel (post.cu).  Buffer j of its plan row is a row of this tick's scores seg [B][F][K],
 // max over the K local speakers, or an entry of the slot's history hist_vad [2][slots][nw - 1][F] (copy `cur`, n_hist entries,
 // oldest first), which holds such max curves already.  Each output frame is post_chunk's value with one speaker and the
-// identity map -- the same float64 expression in the same order -- compared with `> tau`; the two warps ballot 32 frames at a
-// time into `bits`, then warp 0 run-length encodes them.
+// identity map -- the same float64 expression in the same order -- compared with `> tau`, tau = params[3 * rows[c].x] (the
+// stream's tau_active); the two warps ballot 32 frames at a time into `bits`, then warp 0 run-length encodes them.  nw is the
+// largest latency / step of any slot (the history stride); the plan row's nb <= ts.nw.
 __global__ void __launch_bounds__(VAD_SLOTS_THREADS)
 vad_slots_kernel(const float* __restrict__ seg, const float* __restrict__ hist_vad, const TickSlot* __restrict__ act,
                  const int2* __restrict__ rows, int slots, int F, int K, int nw, const int32_t* __restrict__ plan,
-                 int plan_stride, const double* __restrict__ hamming, double tau, int32_t* __restrict__ header,
-                 uint32_t* __restrict__ turns, int turn_cap, unsigned int* __restrict__ total) {
+                 int plan_stride, const double* __restrict__ hamming, const double* __restrict__ params,
+                 int32_t* __restrict__ header, uint32_t* __restrict__ turns, int turn_cap, unsigned int* __restrict__ total) {
   __shared__ unsigned bits[(1024 + 32) / 32];   // frames 0 .. nfo <= F + 1 <= 1024
   const int c = blockIdx.x;
   const int2 r = rows[c];
   const TickSlot ts = act[r.x];
+  const double tau = params[(size_t)r.x * 3];
   const int32_t* pl = plan + (size_t)c * plan_stride;
   const int nb = pl[0], nf = pl[1], first_nf = pl[2], first_lo = pl[3];
   const int nfo = first_nf > 0 ? first_nf : nf;
@@ -144,14 +146,15 @@ vad_slots_kernel(const float* __restrict__ seg, const float* __restrict__ hist_v
   if (warp == 0) warp_turns(nfo, [&](int f0) { return bits[f0 >> 5]; }, header + (size_t)c * 4, turns, turn_cap, total);
 }
 
-// History update of the VAD slots: CTA (a, i) writes entry i of slot act[a]'s other copy, the last keep = min(nw - 1, n_hist +
-// n) chunks of (its history + its n chunks of this tick) as max curves [F].  The host then flips `cur` and sets n_hist = keep.
+// History update of the VAD slots: CTA (a, i) writes entry i of slot act[a]'s other copy, the last keep = min(ts.nw - 1,
+// n_hist + n) chunks of (its history + its n chunks of this tick) as max curves [F], at the stride of the largest slot's
+// nw - 1.  The host then flips `cur` and sets n_hist = keep.
 __global__ void __launch_bounds__(256)
 vad_slots_history_kernel(const float* __restrict__ seg, float* hist_vad, const TickSlot* __restrict__ act, int slots, int F,
                          int K, int nw) {
   const TickSlot ts = act[blockIdx.x];
   const int i = blockIdx.y;
-  const int keep = min(nw - 1, ts.n_hist + ts.n);
+  const int keep = min(ts.nw - 1, ts.n_hist + ts.n);
   if (i >= keep) return;
   const int v = ts.n - keep + i;                    // virtual chunk: v >= 0 is this tick's, v < 0 the history's
   const size_t src = ((size_t)ts.cur * slots + ts.slot) * (nw - 1) + ts.n_hist;
@@ -178,15 +181,15 @@ int launch_vad_binarize(const double* curve, const long long* curve_off, int N, 
 }
 
 int launch_vad_slots(const float* seg, const float* hist_vad, const TickSlot* act, const int2* rows, int slots, int B, int F,
-                     int K, int nw, const int32_t* plan, int plan_stride, const double* hamming, double tau, int32_t* header,
-                     uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st) {
+                     int K, int nw, const int32_t* plan, int plan_stride, const double* hamming, const double* params,
+                     int32_t* header, uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st) {
   ProfScope _ps("vad_slots", st);
   if (F > 1023) {
     set_error("vad_slots: at most 1023 frames");
     return -1;
   }
-  vad_slots_kernel<<<B, VAD_SLOTS_THREADS, 0, st>>>(seg, hist_vad, act, rows, slots, F, K, nw, plan, plan_stride, hamming, tau,
-                                                    header, turns, turn_cap, total);
+  vad_slots_kernel<<<B, VAD_SLOTS_THREADS, 0, st>>>(seg, hist_vad, act, rows, slots, F, K, nw, plan, plan_stride, hamming,
+                                                    params, header, turns, turn_cap, total);
   DG_LAUNCHED();
   return 0;
 }

@@ -18,7 +18,13 @@ per stream, only the frames at each window's edges once per window.
 
 ``MultiStreamVoiceActivityDetection`` serves the reference's ``VoiceActivityDetection`` the same way (``dg_multi_create_vad``):
 the same audio path, the segmentation network alone, and every stream's speech curve aggregated and binarised on the device.
-Its results carry no caveat: they are bit for bit those of a dedicated ``VoiceActivityDetection``."""
+Its results carry no caveat: they are bit for bit those of a dedicated ``VoiceActivityDetection``.
+
+Each stream may have its own latency (up to the server's ``max_latency``) and thresholds (``open(latency=...,
+tau_active=...)``, and ``rho_update`` / ``delta_new`` for diarization), none of which reaches the networks: the tick's one
+network pass is shared, the clustering runs every stream's state at that stream's thresholds, and the post-path aggregates
+each stream's own number of buffers and binarises at its own ``tau_active``.  A stream's results are then those of a
+dedicated pipeline whose configuration is the server's with that stream's values."""
 from __future__ import annotations
 
 import ctypes as C
@@ -92,17 +98,49 @@ def source_geometry(rate: int, sample_rate: int, duration: float, step: float) -
     return chunk, hop, (chunk * (1 / rate)) / window
 
 
+def stream_windows(latency: float, step: float) -> int:
+    """the buffers a stream at ``latency`` aggregates (``DelayedAggregation.num_overlapping_windows``)"""
+    return int(round(latency / step))
+
+
+def mixed_plan(idx: np.ndarray, latency: np.ndarray, step: float, window_samples: int, sample_rate: int, frames: int,
+               nw: int, resolution):
+    """``plan_rows`` of a tick whose rows (chunk indices ``idx`` (B,), row latencies ``latency`` (B,), window resolutions
+    ``resolution`` (B,)) belong to streams at several latencies: one ``plan_rows`` per distinct latency, its rows scattered
+    into plan int32 (B, 4 + nw), ``nw`` the largest number of buffers of any stream; a row with fewer buffers leaves the tail
+    0.  -> (plan, out_start (B,), out_res (B,))"""
+    idx = np.asarray(idx, dtype=np.int64)
+    latency = np.asarray(latency, dtype=np.float64)
+    res = np.broadcast_to(np.asarray(resolution, dtype=np.float64), idx.shape)
+    lats = np.unique(latency)
+    if len(lats) <= 1 and (len(lats) == 0 or stream_windows(lats[0], step) == nw):   # one latency: one evaluation
+        lat = float(lats[0]) if len(lats) else step * nw
+        return plan_rows(idx, step, window_samples, sample_rate, frames, nw, lat, res)
+    plan = np.zeros((len(idx), 4 + nw), dtype=np.int32)
+    out_start, out_res = np.empty(len(idx)), np.empty(len(idx))
+    for lat in lats.tolist():
+        rows = np.flatnonzero(latency == lat)
+        p, s, r = plan_rows(idx[rows], step, window_samples, sample_rate, frames, stream_windows(lat, step), lat, res[rows])
+        plan[rows, :p.shape[1]] = p
+        out_start[rows], out_res[rows] = s, r
+    return plan, out_start, out_res
+
+
 class _MultiStreamServer:
     """What the multi-stream servers share: the ``dg_multi`` handle a subclass creates (``_create``), the declared source
     rates, the host mirror of the slots (``open`` / ``close`` / ``push`` / ``available``) and the planning of a tick."""
 
     _needs = ""   # what the subclass raises when a model is not native
 
-    def __init__(self, config, max_streams: int, max_windows_per_stream: int, source_sample_rates, models):
+    def __init__(self, config, max_streams: int, max_windows_per_stream: int, source_sample_rates, models, max_latency=None):
         self._h: Optional[C.c_void_p] = None
         self.config = config
         msg = f"Latency should be in the range [{config.step}, {config.duration}]"
         assert config.step <= config.latency <= config.duration, msg
+        self.max_latency = float(config.latency if max_latency is None else max_latency)
+        if not config.latency <= self.max_latency <= config.duration:
+            raise ValueError(f"max_latency {self.max_latency} should be in the range [{config.latency}, {config.duration}] "
+                             "(the configuration's latency, its duration)")
         for lazy in models:
             lazy.eval()
             lazy.to(config.device)
@@ -114,7 +152,7 @@ class _MultiStreamServer:
         self.step_samples = int(round(config.step * sr))
         self.max_streams, self.max_windows_per_stream = int(max_streams), int(max_windows_per_stream)
         self.F, self.K = seg_net.dims(self.window_samples)
-        self.nw = int(round(config.latency / config.step))      # DelayedAggregation.num_overlapping_windows
+        self.nw = stream_windows(self.max_latency, config.step)   # the most buffers a stream aggregates (plan width - 4)
         self.device = seg_net.device
         ham = np.ascontiguousarray(np.hamming(self.F), dtype=np.float64)
         self._h = self._create(ham)
@@ -138,6 +176,7 @@ class _MultiStreamServer:
         self._chunk = np.full(self.max_streams, self.window_samples, dtype=np.int64)
         self._hop = np.full(self.max_streams, self.step_samples, dtype=np.int64)
         self._res = np.full(self.max_streams, 1 / sr, dtype=np.float64)
+        self._latency = np.full(self.max_streams, float(config.latency), dtype=np.float64)   # each stream's latency
         self._turns = np.empty(1 << 16, dtype=np.uint32)
 
     def _create(self, hamming: np.ndarray) -> C.c_void_p:
@@ -162,23 +201,35 @@ class _MultiStreamServer:
     def handle(self) -> C.c_void_p:
         return self._h
 
-    def open(self, shift: float = 0.0, sample_rate: Optional[int] = None) -> int:
+    def _open_stream(self, shift: float, sample_rate: Optional[int], latency: Optional[float], **thresholds) -> int:
         """a new stream (fresh clustering and aggregation state) in the lowest free slot, its blocks at ``sample_rate``
-        (default: the pipeline's; otherwise one of ``source_sample_rates``); returns its id"""
-        rate = self.config.sample_rate if sample_rate is None else int(sample_rate)
+        (default: the pipeline's; otherwise one of ``source_sample_rates``), at its own ``latency`` and ``thresholds``
+        (name -> value, in the order of the handle's {tau, rho, delta}; None: the config's).  Everything is checked before
+        the handle is touched: a refusal raises ValueError and leaves the slot closed.  Returns the stream's id"""
+        cfg = self.config
+        rate = cfg.sample_rate if sample_rate is None else int(sample_rate)
         if rate not in self.rates:
             raise ValueError(f"sample rate {rate} was not declared (source_sample_rates: {sorted(self._resamplers)})")
+        lat = float(cfg.latency if latency is None else latency)
+        if not cfg.step <= lat <= self.max_latency:
+            raise ValueError(f"latency {lat} should be in the range [{cfg.step}, {self.max_latency}] (step, max_latency)")
+        params = np.zeros(3, dtype=np.float64)
+        for i, (name, value) in enumerate(thresholds.items()):
+            params[i] = float(getattr(cfg, name) if value is None else value)
+            if not math.isfinite(params[i]):
+                raise ValueError(f"{name} must be finite, not {params[i]}")
         free = np.flatnonzero(~self._open)
         if len(free) == 0:
             raise ValueError(f"all {self.max_streams} streams are open")
         sid = int(free[0])
         rid, chunk, hop, res = self.rates[rate]
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().dg_multi_open_rate(self._h, sid, rid))
+            _lib.check(_lib.lib().dg_multi_open_config(self._h, sid, rid, stream_windows(lat, cfg.step), params.ctypes.data))
         self._open[sid] = True
         self._pushed[sid] = self._emitted[sid] = 0
         self._shift[sid] = float(shift)
         self._chunk[sid], self._hop[sid], self._res[sid] = chunk, hop, res
+        self._latency[sid] = lat
         return sid
 
     def close(self, sid: int):
@@ -220,8 +271,8 @@ class _MultiStreamServer:
         row0 = np.cumsum(n) - n
         idx = np.repeat(self._emitted[sids], n) + (np.arange(B) - np.repeat(row0, n))
         cfg = self.config
-        plan, out_start, out_res = plan_rows(idx, cfg.step, self.window_samples, cfg.sample_rate, self.F, self.nw,
-                                             cfg.latency, np.repeat(self._res[sids], n))
+        plan, out_start, out_res = mixed_plan(idx, np.repeat(self._latency[sids], n), cfg.step, self.window_samples,
+                                              cfg.sample_rate, self.F, self.nw, np.repeat(self._res[sids], n))
         plan = np.ascontiguousarray(plan)
         header = np.empty((B, 4), dtype=np.int32)
         need = B * self._speakers * ((self.F + 2) // 2)
@@ -251,17 +302,29 @@ class MultiStreamDiarization(_MultiStreamServer):
     stream's windows fed one per call, with its ``timestamp_shift`` set to ``shift``, up to the embedding caveat of the module
     docstring.  A stream is at ``config.sample_rate`` or at one of ``source_sample_rates`` (declared here, see
     ``source_geometry``); its blocks are at its own rate, and its windows are resampled as ``DeviceResample`` resamples them.
-    Needs the native models (``B200*Loader``).  ``_step(outputs=True)`` also returns the tick's scores (B, F, K), embeddings
-    (B, K, D) and maps (B, K) as device tensors."""
+    A stream may also have its own ``latency`` (``config.step <= latency <= max_latency``; ``max_latency``, default
+    ``config.latency``, at most ``config.duration``, sizes every slot's aggregation history) and ``tau_active``,
+    ``rho_update`` and ``delta_new``; its results are then those of ``SpeakerDiarization`` with the config's other values
+    and these.  Needs the native models (``B200*Loader``).  ``_step(outputs=True)`` also returns the tick's scores (B, F,
+    K), embeddings (B, K, D) and maps (B, K) as device tensors."""
 
     _needs = "MultiStreamDiarization needs the native segmentation and embedding models"
 
     def __init__(self, config: SpeakerDiarizationConfig, max_streams: int, max_windows_per_stream: int = 4,
-                 source_sample_rates=()):
+                 source_sample_rates=(), max_latency: Optional[float] = None):
         self._speakers = int(config.max_speakers)
         self.labels = [f"speaker{g}" for g in range(config.max_speakers)]
         super().__init__(config, max_streams, max_windows_per_stream, source_sample_rates,
-                         (config.segmentation, config.embedding))
+                         (config.segmentation, config.embedding), max_latency)
+
+    def open(self, shift: float = 0.0, sample_rate: Optional[int] = None, *, latency: Optional[float] = None,
+             tau_active: Optional[float] = None, rho_update: Optional[float] = None,
+             delta_new: Optional[float] = None) -> int:
+        """a new stream in the lowest free slot (``_MultiStreamServer._open_stream``): blocks at ``sample_rate``, time
+        stamps shifted by ``shift``, and its own latency and thresholds (None: the config's), fixed until it is closed;
+        returns its id"""
+        return _MultiStreamServer._open_stream(self, shift, sample_rate, latency, tau_active=tau_active,
+                                               rho_update=rho_update, delta_new=delta_new)
 
     def _create(self, hamming):
         config, emb_net = self.config, self.config.embedding.model
@@ -291,16 +354,25 @@ class MultiStreamVoiceActivityDetection(_MultiStreamServer):
     for it when the stream is fed one window per call with ``set_timestamp_shift(shift)``.  A tick runs the segmentation
     network alone on all of its windows, then every stream's speech curve (max over the local speakers, aggregated over its
     ``latency / step`` most recent windows) is binarised on the device.  The scores are batch invariant, so a stream's results
-    are bit for bit those of its dedicated pipeline whatever the other streams do.  Needs the native segmentation model
-    (``B200SegmentationLoader``, powerset checkpoints included).  ``_step(outputs=True)`` also returns ``(scores,)``, the
-    tick's scores (B, F, K) as a device tensor."""
+    are bit for bit those of its dedicated pipeline whatever the other streams do.  A stream may have its own ``latency``
+    (up to ``max_latency``, as ``MultiStreamDiarization``) and ``tau_active``, and is then bit for bit the
+    ``VoiceActivityDetection`` at those values.  Needs the native segmentation model (``B200SegmentationLoader``, powerset
+    checkpoints included).  ``_step(outputs=True)`` also returns ``(scores,)``, the tick's scores (B, F, K) as a device
+    tensor."""
 
     _needs = "MultiStreamVoiceActivityDetection needs the native segmentation model (B200PyanNet)"
     _speakers = 1
 
     def __init__(self, config: VoiceActivityDetectionConfig, max_streams: int, max_windows_per_stream: int = 4,
-                 source_sample_rates=()):
-        super().__init__(config, max_streams, max_windows_per_stream, source_sample_rates, (config.segmentation,))
+                 source_sample_rates=(), max_latency: Optional[float] = None):
+        super().__init__(config, max_streams, max_windows_per_stream, source_sample_rates, (config.segmentation,),
+                         max_latency)
+
+    def open(self, shift: float = 0.0, sample_rate: Optional[int] = None, *, latency: Optional[float] = None,
+             tau_active: Optional[float] = None) -> int:
+        """a new stream in the lowest free slot (``_MultiStreamServer._open_stream``) at its own latency and ``tau_active``
+        (None: the config's); returns its id"""
+        return _MultiStreamServer._open_stream(self, shift, sample_rate, latency, tau_active=tau_active)
 
     def _create(self, hamming):
         h = C.c_void_p()

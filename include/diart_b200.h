@@ -339,20 +339,29 @@ int dg_pipeline_call_stream(dg_pipeline* h, dg_post* post, dg_stream* stream, in
  *      dg_multi_create: chunk_samples / step_samples positive multiples of 4 (window i of a stream is samples
  *        [i * step, i * step + chunk)); max_streams * max_windows_per_stream <= 65535; tau, rho, delta = tau_active,
  *        rho_update, delta_new (cosine clustering with max_speakers <= 32 centres; tau_active also binarises); gamma, beta,
- *        normalize_weights as dg_pipeline_create; num_windows = latency / step and hamming_host = np.hamming(frames) in
- *        float64, as dg_post_create.  The model handles are borrowed and may serve other pipelines meanwhile.
- *      dg_multi_open: a new stream in `slot` (0 <= slot < max_streams, not open): no samples, fresh clustering state (the
- *        reference's reset()), no aggregation history.  dg_multi_close: the stream in `slot` ends; its staged samples are
- *        dropped.
+ *        normalize_weights as dg_pipeline_create; num_windows = max_latency / step, the largest number of aggregated
+ *        buffers of any stream (sizes every slot's history), and hamming_host = np.hamming(frames) in float64, as
+ *        dg_post_create.  tau, rho, delta and num_windows are also the values of a stream opened without its own.  The model
+ *        handles are borrowed and may serve other pipelines meanwhile.
+ *      dg_multi_open: a new stream in `slot` (0 <= slot < max_streams, not open) at the handle's values: no samples, fresh
+ *        clustering state (the reference's reset()), no aggregation history.  dg_multi_close: the stream in `slot` ends; its
+ *        staged samples are dropped.
+ *      dg_multi_open_config: dg_multi_open_rate with the stream's own latency and thresholds, fixed until it is closed:
+ *        num_windows = its latency / step (1 <= num_windows <= the handle's num_windows) buffers aggregated, params = {tau,
+ *        rho, delta} (tau_active, rho_update, delta_new; a VAD handle reads params[0] only).  Its results are those of a
+ *        dedicated pipeline at those values; its plan rows (dg_multi_step) are plan rows of that latency.  DG_EINVAL, naming
+ *        dg_multi_open_config and changing nothing, unless the slot and rate are as dg_multi_open_rate needs, num_windows is
+ *        in range and the values read are finite.
  *      dg_multi_push_host: appends n samples (any block size) to the stream in `slot`.  They are copied to pinned staging;
  *        nothing reaches the device before the next tick.  Fails with DG_EINVAL, writing nothing, if the stream would hold
  *        more unconsumed samples than its ring (chunk + 2 max_windows_per_stream step, rounded up to 1024).
  *      dg_multi_available: complete windows of the stream in `slot` not yet consumed (staged samples included), or DG_EINVAL.
  *      dg_multi_step: one tick.  Every open slot s, in slot order, gives n_s = min(available, max_windows_per_stream) windows;
  *        counts_host int32 [max_streams] receives n_s.  The n_rows = sum n_s chunks are the tick's rows, grouped by slot, each
- *        slot's in window order; plan_host int32 [n_rows][4 + num_windows] holds their dg_post_step plan rows (a chunk's row
- *        depends only on its window index within its stream: diart_b200.serve.plan_rows).  n_rows must equal sum n_s, else
- *        DG_EINVAL.  header_host int32 [n_rows][4] and turns_host as dg_post_step.  seg_dev [n_rows, F, K], emb_dev
+ *        slot's in window order; plan_host int32 [n_rows][4 + num_windows] holds their dg_post_step plan rows at each
+ *        stream's own latency (a chunk's row depends only on its window index within its stream and that latency:
+ *        diart_b200.serve.plan_rows), a row of a stream with fewer buffers leaving the tail unused.  n_rows must equal sum
+ *        n_s and no row may aggregate more buffers than its stream's num_windows, else DG_EINVAL.  header_host int32 [n_rows][4] and turns_host as dg_post_step.  seg_dev [n_rows, F, K], emb_dev
  *        [n_rows, K, D] and map_dev [n_rows, K] (device, nullable) receive the tick's network outputs and speaker maps.  All
  *        staged samples go up in one copy; the networks run in sub-batches of at most 256 windows.  A tick without windows
  *        launches nothing.  Every argument is checked before any launch.  Synchronous. ---- */
@@ -393,6 +402,7 @@ int dg_multi_destroy(dg_multi* h);
 typedef struct dg_resample dg_resample;   /* declared with its entry points below */
 int dg_multi_add_rate(dg_multi* h, dg_resample* rs, int chunk_samples, int step_samples, int* rate_id);
 int dg_multi_open_rate(dg_multi* h, int slot, int rate_id);
+int dg_multi_open_config(dg_multi* h, int slot, int rate_id, int num_windows, const double params[3] /* tau, rho, delta */);
 /* test hook: the last tick's window batch [n_rows, chunk_samples] (what its networks read; n_rows = that tick's window count)
  * copied to wav_dev.  Synchronous. */
 int dg_multi_last_windows(const dg_multi* h, float* wav_dev, int n_rows);
