@@ -107,6 +107,12 @@ SIGNATURES = {
     "dg_sweep_score_files": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, _P, _P, _P, _P, C.c_double, _P, _P,
                                        _P, _P, _P, _P, _P, C.c_int, _P]),
     "dg_sweep_state_order": (C.c_int, [C.c_int, _P, C.c_int, _P]),
+    "dg_sweep_run_latencies": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P, _P, _P, C.c_int, _P, _P,
+                                         _P, _P, C.c_int, C.POINTER(C.c_int), _P]),
+    "dg_sweep_score_latencies": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P, _P, _P, C.c_int, _P, _P,
+                                           _P, _P, C.c_double, _P, _P, _P, _P, _P, _P]),
+    "dg_sweep_check_latencies": (C.c_int, [C.c_int, C.c_int, _P, C.c_int, C.c_int, _P, _P, _P, C.c_int, C.c_int]),
+    "dg_vad_sweep_curve_latencies": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, C.c_int, C.c_int, _P, _P, _P, _P]),
     "dg_vad_sweep_create": (C.c_int, [C.c_int, C.c_int, C.c_int, _P, C.c_int, C.POINTER(_P)]),
     "dg_vad_sweep_curve": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P, _P]),
     "dg_vad_sweep_run_files": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_int, C.POINTER(C.c_int), _P]),

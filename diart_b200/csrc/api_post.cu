@@ -242,18 +242,41 @@ static TurnOut sweep_out(int S, int T, int N) { return {(size_t)S * 8, (size_t)T
 // is the files' plans, each that of a fresh stream, concatenated: a chunk's aggregated buffers are the nw - 1 chunks before
 // it at most, never those of the previous file (post.cu: chunk c reads chunks c - (nb - 1) .. c, nb <= its index in its file
 // + 1), so the post-path runs over all N chunks at once.  Synchronises `st`.
+//
+// With vchunk_host (the sweep over several latencies): the nf "files" are units, the clustering runs over them as above, and
+// the post-path runs over Nv virtual chunks instead, virtual chunk c being real chunk vchunk_host[c]; the plan [Nv][stride] and
+// the header [T][Nv][4] are over the virtual chunks (launch_post_virtual).  Without it Nv = N.  used [nf] (or null: all):
+// the units whose (unit, trial) states are clustered; the maps of the others' chunks are left unwritten.
 static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int nf, const int32_t* chunk_off,
                               const double* params_host, int T, const int32_t* plan_host, int32_t* maps_dev,
-                              double* centers_dev, bool with_header, cudaStream_t st, unsigned int* total_out) {
-  const int stride = 4 + h->nw, M = h->M, D = h->D, K = h->K, F = h->F, S = nf * T;
-  // host -> device, one copy: params [T][3], taus [T], states [S][2] (launch order), plan [N][stride], chunk offsets [nf + 1]
-  const size_t params_b = (size_t)T * 24, taus_b = (size_t)T * 8, states_b = (size_t)S * 8, plan_b = (size_t)N * stride * 4;
-  const size_t off_b = (size_t)(nf + 1) * 4;
-  const size_t in_b = params_b + taus_b + states_b + plan_b + off_b;
-  const TurnOut lay = sweep_out(S, T, N);
+                              double* centers_dev, bool with_header, cudaStream_t st, unsigned int* total_out,
+                              int Nv = 0, const int32_t* vchunk_host = nullptr, const std::vector<char>* used = nullptr) {
+  if (!vchunk_host) Nv = N;
+  // the launch order of the (file, trial) states, without those of units nobody reads
+  std::vector<int32_t> states((size_t)nf * T * 2);
+  sweep_state_order(nf, chunk_off, T, states.data());
+  if (used) {
+    size_t k = 0;
+    for (size_t i = 0; i < (size_t)nf * T; i++)
+      if ((*used)[states[2 * i]]) {
+        states[2 * k] = states[2 * i];
+        states[2 * k + 1] = states[2 * i + 1];
+        k++;
+      }
+    states.resize(2 * k);
+  }
+  // state s = f T + t owns centroid table, active flags and error pair s (cluster.cu), so those are sized for all nf T states
+  // whichever of them run; the launch runs S_run
+  const int stride = 4 + h->nw, M = h->M, D = h->D, K = h->K, F = h->F, S = nf * T, S_run = (int)(states.size() / 2);
+  // host -> device, one copy: params [T][3], taus [T], states [S_run][2] (launch order), plan [Nv][stride], chunk offsets
+  // [nf + 1], then with vchunk_host the virtual chunk table [Nv]
+  const size_t params_b = (size_t)T * 24, taus_b = (size_t)T * 8, states_b = (size_t)S_run * 8, plan_b = (size_t)Nv * stride * 4;
+  const size_t off_b = (size_t)(nf + 1) * 4, vchunk_b = vchunk_host ? (size_t)Nv * 4 : 0;
+  const size_t in_b = params_b + taus_b + states_b + plan_b + off_b + vchunk_b;
+  const TurnOut lay = sweep_out(S, T, Nv);
   const size_t init_b = lay.at, header_b = lay.header_bytes;
   // the device turn buffer starts at a guess and grows to the true count (the kernel counts every turn, writes those that fit)
-  const size_t turn_guess = std::max<size_t>((size_t)T * N * 8, (size_t)DG_POST_PREFIX);
+  const size_t turn_guess = std::max<size_t>((size_t)T * Nv * 8, (size_t)DG_POST_PREFIX);
   if (h->in.ensure(in_b) || h->centers.ensure((size_t)S * M * D * 8) || h->active.ensure((size_t)S * 32 * 4) ||
       h->init.ensure(init_b) || h->prep.ensure(cluster_prep_floats(N, K) * 4 + 16) ||
       h->prep_d.ensure(cluster_prep_doubles(N, K) * 8 + 16) || (!maps_dev && h->maps.ensure((size_t)T * N * K * 4)) ||
@@ -263,9 +286,10 @@ static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* em
   double* p_taus = reinterpret_cast<double*>(pin + params_b);
   memcpy(pin, params_host, params_b);
   for (int t = 0; t < T; t++) p_taus[t] = params_host[3 * t];
-  sweep_state_order(nf, chunk_off, T, reinterpret_cast<int32_t*>(pin + params_b + taus_b));
+  memcpy(pin + params_b + taus_b, states.data(), states_b);
   memcpy(pin + params_b + taus_b + states_b, plan_host, plan_b);
   memcpy(pin + params_b + taus_b + states_b + plan_b, chunk_off, off_b);
+  if (vchunk_host) memcpy(pin + params_b + taus_b + states_b + plan_b + off_b, vchunk_host, vchunk_b);
   unsigned char* din = h->in.as<unsigned char>();
   DG_CUDA(cudaMemcpyAsync(din, pin, in_b, cudaMemcpyHostToDevice, st));
   const double* d_params = reinterpret_cast<const double*>(din);
@@ -283,7 +307,7 @@ static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* em
   p.D = D;
   p.metric = 0;
   int rc;
-  if ((rc = launch_cluster_sweep(p, d_params, T, d_states, S, d_off, seg_dev, emb_dev, N, F, K, h->centers.as<double>(),
+  if ((rc = launch_cluster_sweep(p, d_params, T, d_states, S_run, d_off, seg_dev, emb_dev, N, F, K, h->centers.as<double>(),
                                  h->active.as<int>(), h->init.as<int>(), h->prep.as<float>(), h->prep_d.as<double>(), maps,
                                  st)))
     return rc;
@@ -293,9 +317,14 @@ static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* em
   for (int attempt = 0; attempt < 2; attempt++) {
     const int cap = (int)std::min<size_t>(h->turns.bytes / 4, (size_t)INT32_MAX);
     DG_CUDA(cudaMemsetAsync(h->total.p, 0, 4, st));
-    if ((rc = launch_post(seg_dev, maps, nullptr, nullptr, 0, N, F, K, M, h->nw, d_plan, stride, h->hamming.as<double>(), 0.0,
-                          h->header.as<int32_t>(), h->turns.as<uint32_t>(), cap, h->total.as<unsigned int>(), st, d_taus, T)))
-      return rc;
+    if (vchunk_host)
+      rc = launch_post_virtual(seg_dev, maps, N, reinterpret_cast<const int32_t*>(d_off + nf + 1), Nv, F, K, M, h->nw, d_plan,
+                               stride, h->hamming.as<double>(), d_taus, T, h->header.as<int32_t>(), h->turns.as<uint32_t>(), cap,
+                               h->total.as<unsigned int>(), st);
+    else
+      rc = launch_post(seg_dev, maps, nullptr, nullptr, 0, N, F, K, M, h->nw, d_plan, stride, h->hamming.as<double>(), 0.0,
+                       h->header.as<int32_t>(), h->turns.as<uint32_t>(), cap, h->total.as<unsigned int>(), st, d_taus, T);
+    if (rc) return rc;
     DG_CUDA(cudaMemcpyAsync(pin, h->init.p, init_b, cudaMemcpyDeviceToHost, st));
     if (with_header) DG_CUDA(cudaMemcpyAsync(pin + lay.at, h->header.p, header_b, cudaMemcpyDeviceToHost, st));
     DG_CUDA(cudaMemcpyAsync(pin + lay.total(), h->total.p, 4, cudaMemcpyDeviceToHost, st));
@@ -455,16 +484,11 @@ static int der_components(const char* who, DerBufs& b, PinnedBuf& pinbuf, const 
   return DG_OK;
 }
 
-// dg_sweep_score(_files): the clustering and post-path of sweep_cluster_post, then the DER components of every (file, trial)
-// against the file's reference rows [ref_off[f], ref_off[f + 1]) with R[f] labels
-static int sweep_score(const char* who, dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int nf,
-                       const int32_t* chunk_off, const double* params_host, int T, const int32_t* plan_host,
-                       const double* out_start_host, const double* out_res_host, const double* shift_host, double collar,
-                       const double* ref_host, const int32_t* ref_label_host, const int32_t* ref_off, const int32_t* R_host,
-                       double* components_host, int32_t* hyp_offsets_dev, double* hyp_segments_dev, int hyp_cap,
-                       void* stream) {
+// the scoring arguments of dg_sweep_score(_files) and dg_sweep_score_latencies over N chunks in nf files (before any launch)
+static int score_check(const char* who, int N, int nf, const double* out_start_host, const double* out_res_host,
+                       const double* shift_host, double collar, const double* ref_host, const int32_t* ref_label_host,
+                       const int32_t* ref_off, const int32_t* R_host, const double* components_host, int hyp_cap) {
   int rc;
-  if ((rc = sweep_check(who, h, seg_dev, emb_dev, N, nf, chunk_off, params_host, T, plan_host))) return rc;
   if (!out_start_host || !out_res_host || !components_host || hyp_cap < 0 || !shift_host || !std::isfinite(collar) ||
       collar < 0) {
     set_error(std::string(who) + ": bad arguments (need chunk times, a components buffer, finite shift, finite collar >= 0, "
@@ -499,6 +523,22 @@ static int sweep_score(const char* who, dg_sweep* h, const float* seg_dev, const
     if ((rc = sweep_check_reference(who, S > 0 ? ref_host + 2 * (size_t)ref_off[f] : nullptr,
                                     S > 0 ? ref_label_host + ref_off[f] : nullptr, ref_off[f + 1] - ref_off[f], R_host[f])))
       return rc;
+  return DG_OK;
+}
+
+// dg_sweep_score(_files): the clustering and post-path of sweep_cluster_post, then the DER components of every (file, trial)
+// against the file's reference rows [ref_off[f], ref_off[f + 1]) with R[f] labels
+static int sweep_score(const char* who, dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int nf,
+                       const int32_t* chunk_off, const double* params_host, int T, const int32_t* plan_host,
+                       const double* out_start_host, const double* out_res_host, const double* shift_host, double collar,
+                       const double* ref_host, const int32_t* ref_label_host, const int32_t* ref_off, const int32_t* R_host,
+                       double* components_host, int32_t* hyp_offsets_dev, double* hyp_segments_dev, int hyp_cap,
+                       void* stream) {
+  int rc;
+  if ((rc = sweep_check(who, h, seg_dev, emb_dev, N, nf, chunk_off, params_host, T, plan_host)) ||
+      (rc = score_check(who, N, nf, out_start_host, out_res_host, shift_host, collar, ref_host, ref_label_host, ref_off,
+                        R_host, components_host, hyp_cap)))
+    return rc;
   DG_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)stream;
   unsigned int total = 0;
@@ -531,6 +571,137 @@ extern "C" int dg_sweep_score_files(dg_sweep* h, const float* seg_dev, const flo
   return sweep_score("dg_sweep_score_files", h, seg_dev, emb_dev, N, num_files, chunk_offsets_host, params_host, T, plan_host,
                      out_start_host, out_res_host, shifts_host, collar, ref_host, ref_label_host, ref_offsets_host,
                      ref_label_counts_host, components_host, hyp_offsets_dev, hyp_segments_dev, hyp_cap, stream);
+}
+
+// ============================================================================= sweeps over several latencies
+// A file's windows at a smaller latency are a prefix of its windows at a larger one (same left padding), so the network
+// outputs of a *unit* -- the windows of a file at the largest latency of a group whose outputs are its prefixes bit for bit
+// (the host groups them, tune.LatencyUnits) -- serve every latency of the group.  A *virtual file* is one (latency, file)
+// pair: the first chunks of its unit.  Its *virtual chunks* carry the plan row, output times and timestamp shift of that
+// latency; the clustering runs over the units (it is causal and never reads the latency), the post-path and the scoring over
+// the virtual chunks.
+
+// The virtual layout over N real chunks in nu units (unit_off [nu + 1]): virtual file v holds virtual chunks [voff[v],
+// voff[v + 1]) of Nv, which must be the real chunks u0, u0 + 1, ... of one unit starting at its first chunk u0, inside it; the
+// plan row [4 + nw] of its i-th virtual chunk aggregates 1 <= nb <= min(nw, i + 1) buffers (none before the unit's first
+// chunk) over 1 <= output frames <= min(F + 1, 1023) (the first chunk of a file emits up to F + 1; the post-path's shared
+// memory holds that many).  used (or null) receives [nu]: whether a virtual file starts at unit u.  Host only.
+static int check_virtual(const char* who, int N, int nu, const int32_t* unit_off, int Nv, int nvf, const int32_t* vchunk,
+                         const int32_t* voff, const int32_t* plan, int nw, int F, std::vector<char>* used = nullptr) {
+  if (N < 1 || nu < 1 || Nv < 1 || nvf < 1 || nw < 1 || F < 1 || !unit_off || !vchunk || !voff || !plan) {
+    set_error(std::string(who) + ": bad virtual layout arguments (need chunks, units, virtual chunks and files >= 1, "
+              "non-null tables)");
+    return DG_EINVAL;
+  }
+  int rc;
+  if ((rc = check_chunk_offsets(who, N, nu, unit_off)) || (rc = check_chunk_offsets(who, Nv, nvf, voff))) return rc;
+  const int stride = 4 + nw, max_frames = std::min(F + 1, 1023);
+  if (used) used->assign(nu, 0);
+  for (int v = 0; v < nvf; v++) {
+    const int a = voff[v], n = voff[v + 1] - a, c0 = vchunk[a];
+    const int u = (int)(std::upper_bound(unit_off, unit_off + nu + 1, c0) - unit_off) - 1;
+    if (c0 < 0 || c0 >= N || u < 0 || u >= nu || unit_off[u] != c0) {
+      set_error(std::string(who) + ": virtual file " + std::to_string(v) + " does not start at the first chunk of a unit");
+      return DG_EINVAL;
+    }
+    if (n > unit_off[u + 1] - c0) {
+      set_error(std::string(who) + ": virtual file " + std::to_string(v) + " crosses into the next unit");
+      return DG_EINVAL;
+    }
+    if (used) (*used)[u] = 1;
+    for (int i = 0; i < n; i++) {
+      if (vchunk[a + i] != c0 + i) {
+        set_error(std::string(who) + ": virtual file " + std::to_string(v) + " is not a run of consecutive chunks of its unit");
+        return DG_EINVAL;
+      }
+      const int32_t* pl = plan + (size_t)(a + i) * stride;
+      const int nb = pl[0], nfr = pl[1], nfo = pl[2] > 0 ? pl[2] : nfr;
+      if (nb < 1 || nb > nw || nb - 1 > i || nfr < 1 || pl[2] < 0 || nfo > max_frames) {
+        set_error(std::string(who) + ": plan row " + std::to_string(a + i) + " is not a plan of its virtual file (buffers " +
+                  std::to_string(nb) + ", frames " + std::to_string(nfo) + ")");
+        return DG_EINVAL;
+      }
+    }
+  }
+  return DG_OK;
+}
+
+extern "C" int dg_sweep_check_latencies(int N, int num_units, const int32_t* unit_offsets_host, int num_virtual,
+                                        int num_virtual_files, const int32_t* vchunk_host,
+                                        const int32_t* virtual_offsets_host, const int32_t* plan_host, int num_windows,
+                                        int frames) {
+  return check_virtual("dg_sweep_check_latencies", N, num_units, unit_offsets_host, num_virtual, num_virtual_files,
+                       vchunk_host, virtual_offsets_host, plan_host, num_windows, frames);
+}
+
+// the checks dg_sweep_run_latencies and dg_sweep_score_latencies share: sweep_check over the units, the virtual layout, and
+// at most DG_SWEEP_MAX_STATES (virtual file, trial) states for the scoring; used [nu]: the units the virtual files read
+static int latency_check(const char* who, dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int nu,
+                         const int32_t* unit_off, int Nv, int nvf, const int32_t* vchunk, const int32_t* voff,
+                         const double* params_host, int T, const int32_t* plan_host, std::vector<char>& used) {
+  int rc;
+  if ((rc = sweep_check(who, h, seg_dev, emb_dev, N, nu, unit_off, params_host, T, plan_host))) return rc;
+  if ((long long)nvf * T > DG_SWEEP_MAX_STATES) {
+    set_error(std::string(who) + ": " + std::to_string((long long)nvf * T) + " (virtual file, trial) states; at most " +
+              std::to_string(DG_SWEEP_MAX_STATES) + " per call");
+    return DG_EINVAL;
+  }
+  return check_virtual(who, N, nu, unit_off, Nv, nvf, vchunk, voff, plan_host, h->nw, h->F, &used);
+}
+
+extern "C" int dg_sweep_run_latencies(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int num_units,
+                                      const int32_t* unit_offsets_host, int num_virtual, int num_virtual_files,
+                                      const int32_t* vchunk_host, const int32_t* virtual_offsets_host,
+                                      const double* params_host, int T, const int32_t* plan_host, int32_t* maps_dev,
+                                      int32_t* header_host, uint32_t* turns_host, int turn_cap_host, int* n_turns,
+                                      void* stream) {
+  const char* who = "dg_sweep_run_latencies";
+  std::vector<char> used;
+  int rc;
+  if ((rc = latency_check(who, h, seg_dev, emb_dev, N, num_units, unit_offsets_host, num_virtual, num_virtual_files,
+                          vchunk_host, virtual_offsets_host, params_host, T, plan_host, used)))
+    return rc;
+  if (!header_host || !turns_host) {
+    set_error(std::string(who) + ": bad arguments (need non-null header and turn buffers)");
+    return DG_EINVAL;
+  }
+  DG_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned int total = 0;
+  if ((rc = sweep_cluster_post(h, seg_dev, emb_dev, N, num_units, unit_offsets_host, params_host, T, plan_host, maps_dev,
+                               nullptr, true, st, &total, num_virtual, vchunk_host, &used)))
+    return rc;
+  return download_turns(who, h->pin.as<unsigned char>(), sweep_out(num_units * T, T, num_virtual), h->turns.as<uint32_t>(),
+                        header_host, turns_host, turn_cap_host, n_turns, st);
+}
+
+extern "C" int dg_sweep_score_latencies(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int num_units,
+                                        const int32_t* unit_offsets_host, int num_virtual, int num_virtual_files,
+                                        const int32_t* vchunk_host, const int32_t* virtual_offsets_host,
+                                        const double* params_host, int T, const int32_t* plan_host,
+                                        const double* out_start_host, const double* out_res_host, const double* shifts_host,
+                                        double collar, const double* ref_host, const int32_t* ref_label_host,
+                                        const int32_t* ref_offsets_host, const int32_t* ref_label_counts_host,
+                                        double* components_host, void* stream) {
+  const char* who = "dg_sweep_score_latencies";
+  std::vector<char> used;
+  int rc;
+  if ((rc = latency_check(who, h, seg_dev, emb_dev, N, num_units, unit_offsets_host, num_virtual, num_virtual_files,
+                          vchunk_host, virtual_offsets_host, params_host, T, plan_host, used)))
+    return rc;
+  const int Nv = num_virtual, nvf = num_virtual_files;
+  if ((rc = score_check(who, Nv, nvf, out_start_host, out_res_host, shifts_host, collar, ref_host, ref_label_host,
+                        ref_offsets_host, ref_label_counts_host, components_host, 0)))
+    return rc;
+  DG_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned int total = 0;
+  if ((rc = sweep_cluster_post(h, seg_dev, emb_dev, N, num_units, unit_offsets_host, params_host, T, plan_host, nullptr,
+                               nullptr, false, st, &total, Nv, vchunk_host, &used)))
+    return rc;
+  return der_components(who, h->der, h->pin, h->header.as<int32_t>(), h->turns.as<uint32_t>(), total, Nv, nvf,
+                        virtual_offsets_host, T, h->M, out_start_host, out_res_host, shifts_host, collar, ref_host,
+                        ref_label_host, ref_offsets_host, ref_label_counts_host, components_host, nullptr, nullptr, 0, st);
 }
 
 // ============================================================================= voice activity detection sweep
@@ -611,6 +782,55 @@ extern "C" int dg_vad_sweep_curve(dg_vad_sweep* h, const float* seg_dev, int N, 
   h->N = N;
   h->nf = num_files;
   h->chunk_off.assign(chunk_offsets_host, chunk_offsets_host + num_files + 1);
+  return DG_OK;
+}
+
+// The curve over the virtual layout of several latencies (check_virtual): the N real chunks of seg in units, the curve over the
+// Nv virtual chunks.  Afterwards the handle's chunks and files are the virtual ones, so that dg_vad_sweep_run_files and
+// dg_vad_sweep_score_files threshold and score every (latency, file) pair.
+extern "C" int dg_vad_sweep_curve_latencies(dg_vad_sweep* h, const float* seg_dev, int N, int num_units,
+                                            const int32_t* unit_offsets_host, int num_virtual, int num_virtual_files,
+                                            const int32_t* vchunk_host, const int32_t* virtual_offsets_host,
+                                            const int32_t* plan_host, void* stream) {
+  const char* who = "dg_vad_sweep_curve_latencies";
+  if (!h || !seg_dev) {
+    set_error(std::string(who) + ": bad arguments (need a handle and scores)");
+    return DG_EINVAL;
+  }
+  const int Nv = num_virtual, nvf = num_virtual_files;
+  int rc;
+  if ((rc = check_virtual(who, N, num_units, unit_offsets_host, Nv, nvf, vchunk_host, virtual_offsets_host, plan_host,
+                          h->nw, h->F)))
+    return rc;
+  const int stride = 4 + h->nw;
+  std::vector<long long> off(Nv + 1);
+  off[0] = 0;
+  for (int c = 0; c < Nv; c++) {
+    const int32_t* pl = plan_host + (size_t)c * stride;
+    off[c + 1] = off[c] + (pl[2] > 0 ? pl[2] : pl[1]);
+  }
+  DG_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  // host -> device, one copy: curve offsets [Nv + 1] (int64, first: vad_binarize_all reads them there), plan [Nv][stride],
+  // virtual chunk table [Nv]
+  const size_t off_b = (size_t)(Nv + 1) * 8, plan_b = (size_t)Nv * stride * 4, vchunk_b = (size_t)Nv * 4;
+  const size_t in_b = off_b + plan_b + vchunk_b;
+  if (h->in.ensure(in_b) || h->curve.ensure((size_t)off[Nv] * 8) || h->pin.ensure(in_b)) return DG_ECUDA;
+  unsigned char* pin = h->pin.as<unsigned char>();
+  memcpy(pin, off.data(), off_b);
+  memcpy(pin + off_b, plan_host, plan_b);
+  memcpy(pin + off_b + plan_b, vchunk_host, vchunk_b);
+  unsigned char* din = h->in.as<unsigned char>();
+  DG_CUDA(cudaMemcpyAsync(din, pin, in_b, cudaMemcpyHostToDevice, st));
+  h->N = 0;   // no curve while it is being replaced
+  if ((rc = launch_vad_curve_virtual(seg_dev, reinterpret_cast<const int32_t*>(din + off_b + plan_b), Nv, h->F, h->K,
+                                     reinterpret_cast<const int32_t*>(din + off_b), stride, h->hamming.as<double>(),
+                                     reinterpret_cast<const long long*>(din), h->curve.as<double>(), st)))
+    return rc;
+  DG_CUDA(cudaStreamSynchronize(st));
+  h->N = Nv;
+  h->nf = nvf;
+  h->chunk_off.assign(virtual_offsets_host, virtual_offsets_host + nvf + 1);
   return DG_OK;
 }
 

@@ -274,6 +274,11 @@ int launch_post(const float* seg, const int32_t* map, const float* hist_seg, con
                 int F, int K, int M, int nw, const int32_t* plan, int plan_stride, const double* hamming, double tau,
                 int32_t* header, uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st,
                 const double* taus = nullptr /*[T]: per-state thresholds, map [T][B][K], header [T][B][4]*/, int T = 1);
+// post.cu -- the sweep over several latencies: Nv virtual chunks, virtual chunk c = real chunk vchunk[c] of the N whose scores
+// seg [N][F][K] and maps [T][N][K] are given; header [T][Nv][4]; trial t thresholds at taus[t]
+int launch_post_virtual(const float* seg, const int32_t* map, int N, const int32_t* vchunk, int Nv, int F, int K, int M, int nw,
+                        const int32_t* plan, int plan_stride, const double* hamming, const double* taus, int T,
+                        int32_t* header, uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st);
 int launch_expand_windows(const float* ring, long long r0, int C, int hop, int S, int B, float* wav, cudaStream_t st);
 int launch_post_history(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map, int n_hist,
                         int B, int F, int K, int keep, float* new_seg, int32_t* new_map, cudaStream_t st);
@@ -319,6 +324,9 @@ int launch_der_score(const int* hoff, const double* hseg, int nf, int T, int M, 
 // chunk c's frames at curve [curve_off[c], curve_off[c + 1])), then per trial t the turns of curve > taus[t], header [T][N][4]
 int launch_vad_curve(const float* seg, int N, int F, int K, const int32_t* plan, int plan_stride, const double* hamming,
                      const long long* curve_off, double* curve, cudaStream_t st);
+// the curve of Nv virtual chunks, virtual chunk c = real chunk vchunk[c] of seg
+int launch_vad_curve_virtual(const float* seg, const int32_t* vchunk, int Nv, int F, int K, const int32_t* plan, int plan_stride,
+                             const double* hamming, const long long* curve_off, double* curve, cudaStream_t st);
 int launch_vad_binarize(const double* curve, const long long* curve_off, int N, int T, const double* taus, int32_t* header,
                         uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st);
 // vad.cu -- many live VAD streams (dg_multi): chunks grouped by slot as launch_post_slots, one speech curve per chunk, each

@@ -131,6 +131,28 @@ post_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map, cons
   post_chunk(pl, c, nb, nf, first_nf, first_lo, F, K, M, nw, hamming, tau, header, turns, turn_cap, total, buf_seg, buf_map);
 }
 
+// The sweep over several latencies (dg_sweep_*_latencies): CTA (c, t) is virtual chunk c of the gridDim.x and trial t.  The
+// scores seg [N][F][K] and maps [T][N][K] are over the N real chunks; virtual chunk c is real chunk vchunk[c], and buffer j of
+// its plan row the real chunk vchunk[c] - (nb - 1) + j (the host guarantees these lie in the virtual chunk's own prefix).
+// Header [T][gridDim.x][4].  The same post_chunk body as post_kernel<true>, so a virtual chunk's turns are the bits of the
+// real chunk at its latency.
+__global__ void __launch_bounds__(POST_THREADS)
+post_virtual_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map, int N, const int32_t* __restrict__ vchunk,
+                    int F, int K, int M, int nw, const int32_t* __restrict__ plan, int plan_stride,
+                    const double* __restrict__ hamming, const double* __restrict__ taus, int32_t* __restrict__ header,
+                    uint32_t* __restrict__ turns, int turn_cap, unsigned int* __restrict__ total) {
+  const int c = blockIdx.x;
+  map += (size_t)blockIdx.y * N * K;
+  header += (size_t)blockIdx.y * gridDim.x * 4;
+  const double tau = taus[blockIdx.y];
+  const int32_t* pl = plan + (size_t)c * plan_stride;
+  const int nb = pl[0], nf = pl[1], first_nf = pl[2], first_lo = pl[3];
+  const int r0 = vchunk[c] - (nb - 1);                    // real chunk of buffer 0
+  auto buf_seg = [&](int j) -> const float* { return seg + (size_t)(r0 + j) * F * K; };
+  auto buf_map = [&](int j) -> const int32_t* { return map + (size_t)(r0 + j) * K; };
+  post_chunk(pl, c, nb, nf, first_nf, first_lo, F, K, M, nw, hamming, tau, header, turns, turn_cap, total, buf_seg, buf_map);
+}
+
 // Many streams in one batch (dg_multi): the B chunks are grouped by stream slot.  Chunk c is window rows[c].y of this batch's
 // slot entry act[rows[c].x] (TickSlot, dg_common.cuh), whose chunks start at batch row row0.  Each slot has its own history of
 // up to ts.nw - 1 <= nw - 1 chunks: hist_seg [2][slots][nw - 1][F][K] and hist_map [2][slots][nw - 1][K] (two copies, `cur`
@@ -229,6 +251,33 @@ int launch_post(const float* seg, const int32_t* map, const float* hist_seg, con
   else
     post_kernel<false><<<B, POST_THREADS, smem, st>>>(seg, map, hist_seg, hist_map, n_hist, B, F, K, M, nw, plan, plan_stride,
                                                       hamming, tau, nullptr, header, turns, turn_cap, total);
+  DG_LAUNCHED();
+  return 0;
+}
+
+int launch_post_virtual(const float* seg, const int32_t* map, int N, const int32_t* vchunk, int Nv, int F, int K, int M, int nw,
+                        const int32_t* plan, int plan_stride, const double* hamming, const double* taus, int T,
+                        int32_t* header, uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st) {
+  ProfScope _ps("post_virtual", st);
+  if (T < 1 || T > 65535 || !taus || Nv < 1) {
+    set_error("post_virtual: 1 <= states <= 65535 with per-state thresholds, at least one chunk");
+    return -1;
+  }
+  if (M > 64 || F > 1023 || K > 127) {
+    set_error("post_virtual: at most 64 global speakers, 1023 frames");
+    return -1;
+  }
+  // up to F + 1 output frames: the first chunk of a file emits the crop of [0, region end)
+  const size_t smem = ((size_t)(nw * M + 15) & ~(size_t)15) + (size_t)(F + 1) * M;
+  if (smem > 200 * 1024) {
+    set_error("post_virtual: latency / step too large for the shared-memory plan");
+    return -1;
+  }
+  static bool attr_done[64] = {};
+  if (smem > 48 * 1024 && first_use_on_device(attr_done))
+    DG_CUDA(cudaFuncSetAttribute(post_virtual_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  post_virtual_kernel<<<dim3(Nv, T), POST_THREADS, smem, st>>>(seg, map, N, vchunk, F, K, M, nw, plan, plan_stride, hamming,
+                                                               taus, header, turns, turn_cap, total);
   DG_LAUNCHED();
   return 0;
 }

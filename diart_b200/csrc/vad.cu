@@ -42,6 +42,24 @@ vad_curve_kernel(const float* __restrict__ seg /*[N][F][K]*/, int F, int K, cons
     });
 }
 
+// The curve over several latencies (dg_vad_sweep_curve_latencies): chunk c is a virtual chunk, real chunk vchunk[c] of seg, and
+// buffer j of its plan row the real chunk vchunk[c] - (nb - 1) + j; otherwise vad_curve_kernel's body
+__global__ void __launch_bounds__(VAD_CURVE_THREADS)
+vad_curve_virtual_kernel(const float* __restrict__ seg /*[N][F][K]*/, const int32_t* __restrict__ vchunk, int F, int K,
+                         const int32_t* __restrict__ plan, int plan_stride, const double* __restrict__ hamming,
+                         const long long* __restrict__ curve_off /*[Nv + 1]*/, double* __restrict__ curve) {
+  const int c = blockIdx.x;
+  const int32_t* pl = plan + (size_t)c * plan_stride;
+  const int nb = pl[0], nf = pl[1], first_nf = pl[2], first_lo = pl[3];
+  const int nfo = first_nf > 0 ? first_nf : nf;
+  const int r0 = vchunk[c] - (nb - 1);
+  double* out = curve + curve_off[c];
+  for (int fo = threadIdx.x; fo < nfo; fo += VAD_CURVE_THREADS)
+    out[fo] = post_frame(pl, nb, nf, nfo, first_lo, F, hamming, fo, [&](int j, int idx) {
+      return (double)speaker_max(seg + ((size_t)(r0 + j) * F + idx) * K, K);
+    });
+}
+
 // One warp run-length encodes the frames 0 .. nfo - 1 of a chunk into its header row hd {offset, count, frames, 0} and its
 // packed turns (0 << 20 | on << 10 | off), placed with one atomicAdd on `total`.  word(f0) is the ballot of the active frames
 // f0 .. f0 + 31 (none at or beyond nfo), read 32 at a time up to frame nfo, which is inactive, so that a turn still open at
@@ -167,6 +185,14 @@ int launch_vad_curve(const float* seg, int N, int F, int K, const int32_t* plan,
                      const long long* curve_off, double* curve, cudaStream_t st) {
   ProfScope _ps("vad_curve", st);
   vad_curve_kernel<<<N, VAD_CURVE_THREADS, 0, st>>>(seg, F, K, plan, plan_stride, hamming, curve_off, curve);
+  DG_LAUNCHED();
+  return 0;
+}
+
+int launch_vad_curve_virtual(const float* seg, const int32_t* vchunk, int Nv, int F, int K, const int32_t* plan, int plan_stride,
+                             const double* hamming, const long long* curve_off, double* curve, cudaStream_t st) {
+  ProfScope _ps("vad_curve_virtual", st);
+  vad_curve_virtual_kernel<<<Nv, VAD_CURVE_THREADS, 0, st>>>(seg, vchunk, F, K, plan, plan_stride, hamming, curve_off, curve);
   DG_LAUNCHED();
   return 0;
 }

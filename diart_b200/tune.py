@@ -37,6 +37,7 @@ dataset classes (files, offsets, plans, references and the loops over trial grou
 """
 from __future__ import annotations
 
+import copy
 import ctypes as C
 import functools
 import operator
@@ -56,6 +57,7 @@ from .models import B200PyanNet
 from .operators import DeviceAudioStream
 
 NETWORK_BATCH = 256           # windows per network step (the benchmarked batch)
+STREAM_FORM_MIN_BATCH = 4     # the sinc front end's stream form runs for batches of this many windows on (api_seg.cu)
 TRIALS_PER_LAUNCH = 1024      # trials per dg_sweep_run; more run as further launches over the same network outputs
 TRIAL_CHUNKS_PER_LAUNCH = 4 << 20   # DatasetSweep: trials x chunks per launch (bounds the header, maps and turn buffers)
 PATCH_COLLAR = 0.05           # PredictionAccumulator's default (sinks.py)
@@ -314,6 +316,136 @@ def file_turns(header: np.ndarray, turns: np.ndarray, c0: int, c1: int):
     return h, own, len(own)
 
 
+def parse_latencies(config, latencies: Iterable) -> Tuple[float, ...]:
+    """the latencies a sweep over several latencies can score, ascending: ``latencies`` with ``config.latency`` added, each
+    ``"min"`` (= step), ``"max"`` (= duration) or a number in [step, duration], else ValueError"""
+    out = {float(config.latency)}
+    for lat in latencies:
+        value = config.step if lat == "min" else (config.duration if lat == "max" else lat)
+        if isinstance(value, (bool, str)) or not isinstance(value, (int, float, np.integer, np.floating)) or \
+                not config.step <= float(value) <= config.duration:
+            raise ValueError(f"latency {lat!r}: need 'min', 'max' or a number in [step, duration] = "
+                             f"[{config.step}, {config.duration}]")
+        out.add(float(value))
+    return tuple(sorted(out))
+
+
+def latency_index(config, latencies: Sequence[float], latency) -> int:
+    """the index of ``latency`` ("min" / "max" as in the configs) in ``latencies``, else ValueError"""
+    value = config.step if latency == "min" else (config.duration if latency == "max" else latency)
+    try:
+        return list(latencies).index(float(value))
+    except (TypeError, ValueError):
+        raise ValueError(f"latency {latency!r} was not constructed (the sweep's latencies: {list(latencies)})") from None
+
+
+def at_latency(config, latency: float):
+    """a shallow copy of ``config`` with another latency (everything else, the models included, shared)"""
+    out = copy.copy(config)
+    out._latency = latency
+    return out
+
+
+class LatencyUnits:
+    """The host plan of a dataset sweep over several latencies.
+
+    ``latency`` enters a file's windows only through its padding (``get_file_padding``): right padding ``latency - step``
+    and, for a file shorter than the chunk, left padding.  So the windows of a file at two latencies with the same left
+    padding are a prefix of each other: the larger latency only appends windows at the end.  A *unit* is the windows of one
+    file at the largest latency of a group with equal left padding (in samples); the network pass runs over units.  A file
+    at least one chunk long has no left padding at any latency and is one unit; a shorter one has a unit per distinct left
+    padding.
+
+    One exception (``stream_form``, the fused diarization pass): :class:`FileBatches` cuts batches of 256 windows from window
+    0, and the sinc front end runs in its stream form for batches of at least 4 windows and in its per-window form for
+    smaller ones (``run_sinc_prep``, ``csrc/api_seg.cu``), which round differently.  A latency whose last batch holds 1 to
+    3 windows would see them computed in a longer batch of its unit, so it gets a unit of its own (unless its windows are
+    the unit's exactly).  Batches of 4 or more windows give every window the same bits whatever their length
+    (``test_gpu_sweep_latencies``).  The VAD sweep's segmentation pass takes no hop hint, so always the per-window form.
+
+    A *virtual file* is a (latency, file) pair: the first ``num_windows[l, f]`` chunks of unit ``unit_of[l, f]``, each with
+    the plan row, output times and timestamp shift of that latency (:meth:`plan`, :meth:`tables`).  The clustering is causal
+    and never reads the latency, so one clustering per unit and trial serves every latency the unit holds."""
+
+    def __init__(self, waveforms: Sequence[np.ndarray], config, latencies: Iterable, stream_form: bool = True):
+        self.config = config
+        self.latencies = parse_latencies(config, latencies)
+        self.nw = int(round(self.latencies[-1] / config.step))          # plan width: the largest latency's
+        nl, nf = len(self.latencies), len(waveforms)
+        self.unit_of = np.zeros((nl, nf), dtype=np.int64)
+        self.num_windows = np.zeros((nl, nf), dtype=np.int64)
+        self.starts: List[List[np.ndarray]] = [[None] * nf for _ in range(nl)]
+        self.shifts = np.zeros((nl, nf), dtype=np.float64)
+        self.unit_windows: List[FileWindows] = []
+        for f, x in enumerate(waveforms):
+            fws = [file_windows(x, at_latency(config, lat)) for lat in self.latencies]
+            by_left: Dict[int, List[int]] = {}
+            for li, fw in enumerate(fws):
+                by_left.setdefault(int(np.rint(fw.padding[0] * config.sample_rate)) if fw.padding[0] > 0 else 0,
+                                   []).append(li)
+            groups: Dict[tuple, List[int]] = {}
+            for n_left, lis in by_left.items():
+                n_max = fws[lis[-1]].num_windows
+                for li in lis:
+                    n = fws[li].num_windows
+                    apart = stream_form and n != n_max and 0 < n % NETWORK_BATCH < STREAM_FORM_MIN_BATCH
+                    groups.setdefault((n_left, n if apart else -1), []).append(li)
+            for lis in groups.values():
+                unit = fws[lis[-1]]                                      # the group's largest latency
+                for li in lis:
+                    fw = fws[li]
+                    n = fw.num_windows
+                    if fw.offset != unit.offset or n > unit.num_windows or not np.array_equal(fw.starts, unit.starts[:n]) \
+                            or not np.array_equal(fw.samples[:len(unit.samples)], unit.samples[:len(fw.samples)]):
+                        raise AssertionError(f"file {f}: the windows at latency {self.latencies[li]} are not a prefix of "
+                                             f"those at {self.latencies[lis[-1]]}")
+                    self.unit_of[li, f] = len(self.unit_windows)
+                    self.num_windows[li, f] = n
+                    self.starts[li][f] = fw.starts
+                    self.shifts[li, f] = -fw.padding[0]
+                self.unit_windows.append(unit)
+        self.unit_offsets = np.ascontiguousarray(np.cumsum([0] + [fw.num_windows for fw in self.unit_windows]),
+                                                 dtype=np.int32)
+        self._plans: Optional[List[tuple]] = None
+
+    @property
+    def num_chunks(self) -> int:
+        """real chunks: the units' windows"""
+        return int(self.unit_offsets[-1])
+
+    def num_virtual(self, sel: Sequence[int]) -> int:
+        """virtual chunks of the latencies with indices ``sel``"""
+        return int(self.num_windows[list(sel)].sum())
+
+    def plan(self, F: int):
+        """computes each latency's plans for F score frames per chunk (once the network pass knows F) and drops the units'
+        audio"""
+        self.unit_windows = []
+        self._plans = []
+        for li, lat in enumerate(self.latencies):
+            cfg = at_latency(self.config, lat)
+            parts = [stream_plan(s, cfg, F) for s in self.starts[li]]
+            plan = np.zeros((sum(len(p[0]) for p in parts), 4 + self.nw), dtype=np.int32)
+            cat = np.concatenate([p[0] for p in parts])
+            plan[:, :cat.shape[1]] = cat                               # zero-padded to the largest latency's width
+            self._plans.append((plan, np.concatenate([p[1] for p in parts]), np.concatenate([p[2] for p in parts])))
+
+    def tables(self, sel: Sequence[int]):
+        """the virtual layout of the latencies with indices ``sel``, latency-major then file order -> (vchunk int32 (Nv,),
+        virtual file offsets int32 (nvf + 1,), plan int32 (Nv, 4 + nw), out_start, out_res float64 (Nv,), shifts float64
+        (nvf,)), all contiguous"""
+        vchunk, counts = [], []
+        for li in sel:
+            for f in range(self.num_windows.shape[1]):
+                n = int(self.num_windows[li, f])
+                vchunk.append(self.unit_offsets[self.unit_of[li, f]] + np.arange(n))
+                counts.append(n)
+        return (np.ascontiguousarray(np.concatenate(vchunk), dtype=np.int32),
+                np.ascontiguousarray(np.cumsum([0] + counts), dtype=np.int32),
+                *(np.ascontiguousarray(np.concatenate([self._plans[li][i] for li in sel])) for i in range(3)),
+                np.ascontiguousarray(self.shifts[list(sel)].reshape(-1)))
+
+
 class FileBatches:
     """Iterates over the window batches of a network pass over several files, in file then batch order: each a dense
     (B, chunk_samples) device tensor of B <= 256 consecutive windows of one file.  Every batch holds windows of one file only,
@@ -446,8 +578,10 @@ class HyperParameterSweep:
             return torch.cat(segs), torch.cat(embs)
 
     # ------------------------------------------------------------------ clustering + post-path for T trials
-    def _handle(self, F: int, K: int, D: int):
-        nw = int(round(self.config.latency / self.config.step))
+    def _handle(self, F: int, K: int, D: int, nw: Optional[int] = None):
+        """the dg_sweep handle for these dimensions; ``nw``: its plan width, by default the config's latency / step"""
+        if nw is None:
+            nw = int(round(self.config.latency / self.config.step))
         dims = (F, K, D, nw)
         if self._h is None or self._dims != dims:
             if self._h is not None:
@@ -590,8 +724,10 @@ class _DatasetSweep:
     (``_score_group``, ``_components``)."""
 
     _pack_references = None   # staticmethod of the subclass: references -> the reference arguments of its scoring entry
+    _stream_form = True       # the network pass runs the sinc front end's stream form (LatencyUnits)
 
-    def __init__(self, config, files: Iterable[Tuple[Optional[str], np.ndarray, Optional[Annotation]]]):
+    def __init__(self, config, files: Iterable[Tuple[Optional[str], np.ndarray, Optional[Annotation]]],
+                 latencies: Optional[Iterable] = None):
         files = list(files)
         if not files:
             raise ValueError("at least one file is needed")
@@ -601,17 +737,31 @@ class _DatasetSweep:
         self.config = config
         self.uris = [uri for uri, _, _ in files]
         self.references = [ref for _, _, ref in files]
-        fws = [file_windows(x, config) for _, x, _ in files]   # (the padded audio is dropped after the network pass)
-        self.offsets = np.ascontiguousarray(np.cumsum([0] + [fw.num_windows for fw in fws]), dtype=np.int32)
-        trial_groups(1, self.num_chunks)                        # a dataset too large for one launch fails here
+        self.units: Optional[LatencyUnits] = None
+        if latencies is None:
+            fws = [file_windows(x, config) for _, x, _ in files]   # (the padded audio is dropped after the network pass)
+            self.offsets = np.ascontiguousarray(np.cumsum([0] + [fw.num_windows for fw in fws]), dtype=np.int32)
+            trial_groups(1, self.num_chunks)                        # a dataset too large for one launch fails here
+        else:
+            # the network pass runs over the units; self.offsets are theirs
+            self.units = LatencyUnits([x for _, x, _ in files], config, latencies, self._stream_form)
+            fws = self.units.unit_windows
+            self.offsets = self.units.unit_offsets
+            trial_groups(1, max(self.units.num_virtual(range(len(self.units.latencies))), self.units.num_chunks))
         self.device = self._open()
         t0 = time.perf_counter()
         self._networks(fws)
         torch.cuda.synchronize(self.device)
         self.timing: Dict[str, float] = {"network": time.perf_counter() - t0}
+        self._refs = None
+        if self.units is not None:
+            self.units.plan(self.seg.shape[1])
+            self.plan = self.out_start = self.out_res = self.shifts = None
+            self._latency_refs: Dict[int, tuple] = {}
+            self._virtual: Dict[tuple, tuple] = {}
+            return
         self.plan, self.out_start, self.out_res = dataset_plan(fws, config, self.seg.shape[1])
         self.shifts = np.ascontiguousarray([-fw.padding[0] for fw in fws], dtype=np.float64)
-        self._refs = None
 
     def _open(self) -> torch.device:
         """makes the pipeline whose networks run (an error if they are not native) -> their device"""
@@ -626,8 +776,9 @@ class _DatasetSweep:
         """one scoring launch for one trial group against ``self._refs`` -> (components (files, T, width), device seconds)"""
         raise NotImplementedError
 
-    def _components(self, f: int, comp: np.ndarray):
-        """file f's components object from its (T, width) slice of the launches' components"""
+    def _components(self, f: int, comp: np.ndarray, refs: Optional[tuple] = None):
+        """file f's components object from its (T, width) slice of the launches' components; ``refs``: the packed
+        references f indexes (default ``self._refs``; a virtual file's in the sweeps over several latencies)"""
         raise NotImplementedError
 
     @property
@@ -652,9 +803,7 @@ class _DatasetSweep:
 
     def _score(self, params: np.ndarray):
         """-> (components per file, their sum in file order), one ``_score_group`` per trial group"""
-        missing = [self.uris[i] if self.uris[i] is not None else i for i, r in enumerate(self.references) if r is None]
-        if missing:
-            raise ValueError(f"files without a reference cannot be scored: {missing}")
+        self._check_references()
         if self._refs is None:
             self._refs = self._pack_references(self.references)
         parts, dev = [], 0.0
@@ -666,6 +815,104 @@ class _DatasetSweep:
         comp = np.concatenate(parts, axis=1)
         per_file = [self._components(f, comp[f]) for f in range(len(self.uris))]
         return per_file, functools.reduce(operator.add, per_file)
+
+    # ------------------------------------------------------------------ several latencies (built with ``latencies``)
+    @property
+    def latencies(self) -> Tuple[float, ...]:
+        """the latencies the sweep can score, ascending"""
+        return self.units.latencies if self.units is not None else (float(self.config.latency),)
+
+    def _selection(self, latencies) -> List[int]:
+        """the indices in :attr:`latencies` of the requested ones (None: all), ascending; ValueError for a latency that was
+        not constructed"""
+        if latencies is None:
+            return list(range(len(self.latencies)))
+        return sorted({latency_index(self.config, self.latencies, lat) for lat in latencies})
+
+    def _chunk_range(self, f: int, latency) -> Tuple[int, int]:
+        """the resident chunks [c0, c1) of file f's windows at ``latency`` (None: the config's)"""
+        li = self._selection([self.config.latency if latency is None else latency])[0]
+        if self.units is None:
+            return int(self.offsets[f]), int(self.offsets[f + 1])
+        c0 = int(self.units.unit_offsets[self.units.unit_of[li, f]])
+        return c0, c0 + int(self.units.num_windows[li, f])
+
+    def _tables(self, sel: Sequence[int]) -> tuple:
+        """``LatencyUnits.tables`` of a selection, kept for later calls (the C calls read them by address)"""
+        key = tuple(sel)
+        if key not in self._virtual:
+            self._virtual[key] = self.units.tables(key)
+        return self._virtual[key]
+
+    def _launched(self, sel: List[int]) -> List[int]:
+        """the latencies whose virtual files a call for ``sel`` launches over"""
+        return sel
+
+    def _group_chunks(self, tabs: tuple) -> int:
+        """the chunk count :func:`trial_groups` bounds for a launch over the virtual layout ``tabs``: its virtual chunks
+        (header, turns), or the real chunks where more (the clustering's maps are [T][real chunks][K])"""
+        return max(len(tabs[0]), self.units.num_chunks)
+
+    def _run_latencies(self, params: np.ndarray, sel: List[int], launch, labels: Sequence[str]):
+        """``launch(params, tables)``: the trials of one group -> their :class:`SweepOutputs` over the virtual chunks of
+        ``tables``.  -> {latency: predictions [file][trial]}, each virtual file's assembled from its own chunks and turns"""
+        run = self._launched(sel)
+        tabs = self._tables(run)
+        vchunk, voff, _, out_start, out_res, shifts = tabs
+        nf = len(self.uris)
+        out = {self.latencies[li]: [[] for _ in self.uris] for li in sel}
+        dev = 0.0
+        for g in trial_groups(len(params), self._group_chunks(tabs)):
+            r = launch(params[g], tabs)
+            dev += r.device_seconds
+            for k, li in enumerate(run):
+                if li not in sel:
+                    continue
+                for f in range(nf):
+                    v = k * nf + f
+                    c0, c1 = int(voff[v]), int(voff[v + 1])
+                    header, turns, n = file_turns(r.header, r.turns, c0, c1)
+                    out[self.latencies[li]][f] += assemble_predictions(header, turns, n, out_start[c0:c1], out_res[c0:c1],
+                                                                       labels, float(shifts[v]), self.uris[f])
+        self.timing["sweep"] = dev
+        return out
+
+    def _score_latencies(self, params: np.ndarray, sel: List[int], launch):
+        """``launch(params, tables, references)``: one scoring launch for the trials of one group -> (components (virtual
+        files, T, width), device seconds).  -> {latency: (components per file, their sum in file order)}"""
+        self._check_references()
+        run = self._launched(sel)
+        tabs = self._tables(run)
+        nf, n = len(self.uris), len(run)
+        if n not in self._latency_refs:                    # every file's reference once per latency, latency-major
+            self._latency_refs[n] = self._pack_references(self.references * n)
+        refs = self._latency_refs[n]
+        parts, dev = [], 0.0
+        for g in trial_groups(len(params), self._group_chunks(tabs)):
+            part, secs = launch(params[g], tabs, refs)
+            parts.append(part)
+            dev += secs
+        self.timing["score"] = dev
+        comp = np.concatenate(parts, axis=1)
+        out = {}
+        for k, li in enumerate(run):
+            if li in sel:
+                per_file = [self._components(k * nf + f, comp[k * nf + f], refs) for f in range(nf)]
+                out[self.latencies[li]] = (per_file, functools.reduce(operator.add, per_file))
+        return out
+
+    def _check_references(self):
+        missing = [self.uris[i] if self.uris[i] is not None else i for i, r in enumerate(self.references) if r is None]
+        if missing:
+            raise ValueError(f"files without a reference cannot be scored: {missing}")
+
+    def _layout(self, tabs: tuple) -> tuple:
+        """the layout arguments of the ``_latencies`` entry points after the device outputs: real chunks, units, unit offsets,
+        virtual chunks, virtual files, virtual chunk table, virtual file offsets"""
+        vchunk, voff = tabs[:2]
+        u = self.units
+        return (u.num_chunks, len(u.unit_offsets) - 1, u.unit_offsets.ctypes.data, len(vchunk), len(voff) - 1,
+                vchunk.ctypes.data, voff.ctypes.data)
 
 
 class DatasetSweep(_DatasetSweep):
@@ -684,14 +931,22 @@ class DatasetSweep(_DatasetSweep):
     a tuning loop pays for the networks once.  For every file and trial the results are the bits a
     :class:`HyperParameterSweep` of that file alone gives, whatever the other files and their order.
     ``sweep``: a :class:`HyperParameterSweep` of the same config whose pipeline and handles to use (default: a new one).
+
+    ``latencies``: the latencies the sweep can score besides ``config.latency`` (each ``"min"``, ``"max"`` or in [step,
+    duration]).  The network pass then runs over units (:class:`LatencyUnits`: a file at least one chunk long is one unit,
+    its windows at the largest latency, except for a latency whose last network batch holds 1 to 3 windows).
+    :meth:`score_latencies` / :meth:`run_latencies` cluster every (unit, trial) once and run the post-path and scoring
+    over every (latency, file) pair, in one launch per kernel and trial group whatever the number of latencies; for
+    every latency L the results are the bits ``DatasetSweep`` built at latency L gives.  :meth:`score` / :meth:`run`
+    return the ``config.latency`` entry.
     """
 
     _pack_references = staticmethod(pack_references)
 
     def __init__(self, config: SpeakerDiarizationConfig, files: Iterable[Tuple[Optional[str], np.ndarray, Optional[Annotation]]],
-                 sweep: Optional[HyperParameterSweep] = None):
+                 sweep: Optional[HyperParameterSweep] = None, latencies: Optional[Iterable] = None):
         self._sweep = sweep
-        super().__init__(config, files)
+        super().__init__(config, files, latencies)
 
     def _open(self) -> torch.device:
         if self._sweep is None:
@@ -706,9 +961,10 @@ class DatasetSweep(_DatasetSweep):
         """device bytes of the kept network outputs"""
         return self.seg.numel() * self.seg.element_size() + self.emb.numel() * self.emb.element_size()
 
-    def file_outputs(self, f: int) -> Tuple[torch.Tensor, torch.Tensor]:
-        """file f's slice of the resident scores (n, F, K) and embeddings (n, K, D)"""
-        c0, c1 = int(self.offsets[f]), int(self.offsets[f + 1])
+    def file_outputs(self, f: int, latency=None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """file f's slice of the resident scores (n, F, K) and embeddings (n, K, D); ``latency`` (a constructed one, default
+        the config's): its windows at that latency, the first chunks of its unit"""
+        c0, c1 = self._chunk_range(f, latency)
         return self.seg[c0:c1], self.emb[c0:c1]
 
     def _over_files(self, entry) -> tuple:
@@ -719,25 +975,90 @@ class DatasetSweep(_DatasetSweep):
 
     def sweep(self, params: np.ndarray, keep_state: bool = False) -> SweepOutputs:
         """dg_sweep_run_files over the resident outputs for params (T, 3): header (T, N, 4) and turns over the N
-        concatenated chunks; with ``keep_state`` maps (T, N, K) and centroids (files, T, M, D) on the device"""
+        concatenated chunks; with ``keep_state`` maps (T, N, K) and centroids (files, T, M, D) on the device.  Not for a
+        sweep built with ``latencies`` (:meth:`sweep_latencies`)."""
+        if self.units is not None:
+            raise ValueError("a sweep over several latencies runs through sweep_latencies")
         return self._sweep._run_trials(*self._over_files(_lib.lib().dg_sweep_run_files), params, keep_state)
 
     def run(self, trials: Sequence[Mapping[str, float]] = ({},)) -> List[List[Annotation]]:
         """-> predictions [file][trial]: what :meth:`HyperParameterSweep.run` returns for each file alone"""
+        if self.units is not None:
+            return self.run_latencies(trials, [self.config.latency])[float(self.config.latency)]
         labels = [f"speaker{g}" for g in range(int(self.config.max_speakers))]
         return self._run(trial_params(trials, self.config), self.sweep, labels)
 
     def score(self, trials: Sequence[Mapping[str, float]] = ({},)) -> Tuple[List[DERComponents], DERComponents]:
         """-> (components per file, their sum in file order): per file what :meth:`HyperParameterSweep.score` returns for
         it alone; ``total.der`` is the value ``Optimizer.objective`` minimises.  Every file needs a reference."""
+        if self.units is not None:
+            return self.score_latencies(trials, [self.config.latency])[float(self.config.latency)]
         return self._score(trial_params(trials, self.config))
+
+    def sweep_latencies(self, params: np.ndarray, latencies=None, keep_maps: bool = False) -> SweepOutputs:
+        """dg_sweep_run_latencies over the resident outputs for params (T, 3) at the constructed ``latencies`` (None: all):
+        header (T, Nv, 4), turns, out_start and out_res over the Nv virtual chunks (latency-major, then file order); with
+        ``keep_maps`` the maps (T, N, K) over the N real chunks, on the device"""
+        if self.units is None:
+            raise ValueError("built without latencies: sweep_latencies needs DatasetSweep(..., latencies=...)")
+        return self._sweep_virtual(params, self._tables(self._selection(latencies)), keep_maps)
+
+    def run_latencies(self, trials: Sequence[Mapping[str, float]] = ({},), latencies=None) \
+            -> Dict[float, List[List[Annotation]]]:
+        """-> {latency: predictions [file][trial]} for the constructed ``latencies`` (None: all): for each latency L what
+        :meth:`run` of a ``DatasetSweep`` built at L returns.  One launch per kernel and trial group for all of them."""
+        params, sel = trial_params(trials, self.config), self._selection(latencies)
+        if self.units is None:
+            return {self.latencies[0]: self.run(trials)}
+        labels = [f"speaker{g}" for g in range(int(self.config.max_speakers))]
+        return self._run_latencies(params, sel, self._sweep_virtual, labels)
+
+    def score_latencies(self, trials: Sequence[Mapping[str, float]] = ({},), latencies=None) \
+            -> Dict[float, Tuple[List[DERComponents], DERComponents]]:
+        """-> {latency: (components per file, their sum)} for the constructed ``latencies`` (None: all): for each latency L
+        what :meth:`score` of a ``DatasetSweep`` built at L returns, bit for bit.  The clustering runs once per (unit,
+        trial) whatever the number of latencies; one launch per kernel and trial group (:func:`trial_groups` over the
+        virtual chunks)."""
+        params, sel = trial_params(trials, self.config), self._selection(latencies)
+        if self.units is None:
+            return {self.latencies[0]: self.score(trials)}
+        return self._score_latencies(params, sel, self._score_virtual)
+
+    def _sweep_virtual(self, params: np.ndarray, tabs: tuple, keep_maps: bool = False) -> SweepOutputs:
+        """one dg_sweep_run_latencies over the virtual layout ``tabs`` (``LatencyUnits.tables``)"""
+        sw = self._sweep
+        N, F, K = self.seg.shape
+        h, _ = sw._handle(F, K, self.emb.shape[2], self.units.nw)
+        plan, out_start, out_res = tabs[2:5]
+        params = np.ascontiguousarray(params, dtype=np.float64)
+        T, Nv = len(params), len(tabs[0])
+        header = np.empty((T, Nv, 4), dtype=np.int32)
+        maps = torch.empty((T, N, K), dtype=torch.int32, device=self.device) if keep_maps else None
+        n_turns, seconds = _turn_list_call(sw, self.device, T * Nv * 8, lambda *turn_list: _lib.lib().dg_sweep_run_latencies(
+            h, self.seg.data_ptr(), self.emb.data_ptr(), *self._layout(tabs), params.ctypes.data, T, plan.ctypes.data,
+            _lib.ptr(maps), header.ctypes.data, *turn_list))
+        return SweepOutputs(header, sw._turns[:n_turns].copy(), n_turns, out_start, out_res, maps, None, seconds)
+
+    def _score_virtual(self, params: np.ndarray, tabs: tuple, refs: tuple) -> Tuple[np.ndarray, float]:
+        """one dg_sweep_score_latencies over the virtual layout ``tabs`` against ``refs`` (one entry per virtual file)"""
+        N, F, K = self.seg.shape
+        h, _ = self._sweep._handle(F, K, self.emb.shape[2], self.units.nw)
+        plan, out_start, out_res, shifts = tabs[2:]
+        params = np.ascontiguousarray(params, dtype=np.float64)
+        comp = np.empty((len(tabs[1]) - 1, len(params), 5), dtype=np.float64)
+        rc, seconds = _timed(self.device, lambda st: _lib.lib().dg_sweep_score_latencies(
+            h, self.seg.data_ptr(), self.emb.data_ptr(), *self._layout(tabs), params.ctypes.data, len(params),
+            plan.ctypes.data, out_start.ctypes.data, out_res.ctypes.data, shifts.ctypes.data, PATCH_COLLAR,
+            *(a.ctypes.data for a in refs), comp.ctypes.data, st))
+        _lib.check(rc)
+        return comp, seconds()
 
     def _score_group(self, params: np.ndarray) -> Tuple[np.ndarray, float]:
         reference = tuple(a.ctypes.data for a in self._refs)       # rows, labels, row offsets, label counts
         return self._sweep._score_trials(*self._over_files(_lib.lib().dg_sweep_score_files), params,
                                          self.shifts.ctypes.data, reference)[:2]
 
-    def _components(self, f: int, comp: np.ndarray) -> DERComponents:
+    def _components(self, f: int, comp: np.ndarray, refs: Optional[tuple] = None) -> DERComponents:
         return DERComponents.from_array(comp)
 
 
@@ -814,23 +1135,32 @@ class VoiceActivitySweep(_DatasetSweep):
     """
 
     _pack_references = staticmethod(pack_speech_references)
+    _stream_form = False      # forward_device passes no hop hint: the per-window form for every batch
 
     def __init__(self, config: VoiceActivityDetectionConfig,
-                 files: Iterable[Tuple[Optional[str], np.ndarray, Optional[Annotation]]]):
+                 files: Iterable[Tuple[Optional[str], np.ndarray, Optional[Annotation]]], latencies: Optional[Iterable] = None):
         self._h: Optional[C.c_void_p] = None
         self._turns = np.empty(0, dtype=np.uint32)
-        super().__init__(config, files)
+        super().__init__(config, files, latencies)
         t1 = time.perf_counter()
         N, F, K = self.seg.shape
-        self.curve_frames = int(np.where(self.plan[:, 2] > 0, self.plan[:, 2], self.plan[:, 1]).sum())
+        if self.units is None:
+            plan, nw = self.plan, int(round(config.latency / config.step))
+        else:                              # the curve of every (latency, file) pair, over the virtual chunks
+            plan, nw = self._tables(range(len(self.latencies)))[2], self.units.nw
+        self.curve_frames = int(np.where(plan[:, 2] > 0, plan[:, 2], plan[:, 1]).sum())
         ham = np.ascontiguousarray(np.hamming(F), dtype=np.float64)
-        nw = int(round(config.latency / config.step))
         h = C.c_void_p()
         with torch.cuda.device(self.device):
             _lib.check(_lib.lib().dg_vad_sweep_create(F, K, nw, ham.ctypes.data, self.device.index, C.byref(h)))
             self._h = h
-            _lib.check(_lib.lib().dg_vad_sweep_curve(h, self.seg.data_ptr(), N, len(self.uris), self.offsets.ctypes.data,
-                                                     self.plan.ctypes.data, _lib.stream_ptr(self.device)))
+            if self.units is None:
+                _lib.check(_lib.lib().dg_vad_sweep_curve(h, self.seg.data_ptr(), N, len(self.uris), self.offsets.ctypes.data,
+                                                         self.plan.ctypes.data, _lib.stream_ptr(self.device)))
+            else:
+                tabs = self._tables(range(len(self.latencies)))
+                _lib.check(_lib.lib().dg_vad_sweep_curve_latencies(h, self.seg.data_ptr(), *self._layout(tabs),
+                                                                   tabs[2].ctypes.data, _lib.stream_ptr(self.device)))
         self.timing["curve"] = time.perf_counter() - t1
 
     def __del__(self):
@@ -860,26 +1190,31 @@ class VoiceActivitySweep(_DatasetSweep):
         """device bytes of the kept scores and speech curve"""
         return self.seg.numel() * self.seg.element_size() + self.curve_frames * 8
 
-    def file_outputs(self, f: int) -> torch.Tensor:
-        """file f's slice of the resident scores (n, F, K)"""
-        return self.seg[int(self.offsets[f]):int(self.offsets[f + 1])]
+    def file_outputs(self, f: int, latency=None) -> torch.Tensor:
+        """file f's slice of the resident scores (n, F, K); ``latency`` (a constructed one, default the config's): its windows
+        at that latency, the first chunks of its unit"""
+        c0, c1 = self._chunk_range(f, latency)
+        return self.seg[c0:c1]
 
     def _taus(self, trials: Sequence[Mapping[str, float]]) -> np.ndarray:
         return np.ascontiguousarray(trial_params(trials, self.config, VAD_PARAMS)[:, 0])
 
     def binarize(self, taus: np.ndarray) -> SweepOutputs:
-        """dg_vad_sweep_run_files for thresholds (T,): header (T, N, 4) and turns over the N concatenated chunks"""
+        """dg_vad_sweep_run_files for thresholds (T,): header (T, N, 4) and turns over the N concatenated chunks (for a
+        sweep built with ``latencies``, the virtual chunks of every latency)"""
         taus = np.ascontiguousarray(taus, dtype=np.float64)
-        T, N = len(taus), self.num_chunks
+        T, N = len(taus), self.num_chunks if self.units is None else len(self._tables(self._launched([]))[0])
         header = np.empty((T, N, 4), dtype=np.int32)
         n_turns, seconds = _turn_list_call(self, self.device, T * N * 4, lambda *turn_list: _lib.lib().dg_vad_sweep_run_files(
             self._h, taus.ctypes.data, T, header.ctypes.data, *turn_list))
-        return SweepOutputs(header, self._turns[:n_turns].copy(), n_turns, self.out_start, self.out_res,
-                            device_seconds=seconds)
+        out_start, out_res = (self.out_start, self.out_res) if self.units is None else self._tables(self._launched([]))[3:5]
+        return SweepOutputs(header, self._turns[:n_turns].copy(), n_turns, out_start, out_res, device_seconds=seconds)
 
     def run(self, trials: Sequence[Mapping[str, float]] = ({},)) -> List[List[Annotation]]:
         """-> predictions [file][trial]: for each file and trial what ``Benchmark.run_single`` returns for
         ``VoiceActivityDetection`` with that tau_active (label "speech", modality "speech", the file's uri)"""
+        if self.units is not None:
+            return self.run_latencies(trials, [self.config.latency])[float(self.config.latency)]
         out = self._run(self._taus(trials), self.binarize, ["speech"])
         for preds in out:
             for p in preds:                # the per-chunk VAD annotations carry modality "speech" whatever the shift
@@ -892,18 +1227,58 @@ class VoiceActivitySweep(_DatasetSweep):
         predictions against each file's reference (``DetectionErrorRate(collar=0, skip_overlap=False)``, no uem); the
         minimum of ``total.detection_error_rate`` is the trial ``Optimizer.objective`` would pick.  Every file needs a
         reference."""
+        if self.units is not None:
+            return self.score_latencies(trials, [self.config.latency])[float(self.config.latency)]
         return self._score(self._taus(trials))
 
+    def run_latencies(self, trials: Sequence[Mapping[str, float]] = ({},), latencies=None) \
+            -> Dict[float, List[List[Annotation]]]:
+        """-> {latency: predictions [file][trial]} for the constructed ``latencies`` (None: all): for each latency L what
+        :meth:`run` of a ``VoiceActivitySweep`` built at L returns.  The thresholds run over the curve of every constructed
+        latency (computed once, by the constructor), one launch per kernel and trial group."""
+        taus, sel = self._taus(trials), self._selection(latencies)
+        if self.units is None:
+            return {self.latencies[0]: self.run(trials)}
+        out = self._run_latencies(taus, sel, lambda t, tabs: self.binarize(t), ["speech"])
+        for runs in out.values():
+            for preds in runs:
+                for p in preds:
+                    p.modality = "speech"
+        return out
+
+    def score_latencies(self, trials: Sequence[Mapping[str, float]] = ({},), latencies=None) \
+            -> Dict[float, Tuple[List[DetectionErrorComponents], DetectionErrorComponents]]:
+        """-> {latency: (components per file, their sum)} for the constructed ``latencies`` (None: all): for each latency L
+        what :meth:`score` of a ``VoiceActivitySweep`` built at L returns, bit for bit.  One launch per kernel and trial
+        group over every constructed latency."""
+        taus, sel = self._taus(trials), self._selection(latencies)
+        if self.units is None:
+            return {self.latencies[0]: self.score(trials)}
+        return self._score_latencies(taus, sel, lambda t, tabs, refs: self._vad_score(t, *tabs[3:6], refs))
+
+    def _launched(self, sel: List[int]) -> List[int]:
+        return list(range(len(self.latencies)))       # the curve covers every constructed latency
+
+    def _group_chunks(self, tabs: tuple) -> int:
+        return len(tabs[0])                            # no clustering: header and turns over the virtual chunks
+
     def _score_group(self, taus: np.ndarray) -> Tuple[np.ndarray, float]:
-        rows, roff, _ = self._refs
+        return self._vad_score(taus, self.out_start, self.out_res, self.shifts, self._refs)
+
+    def _vad_score(self, taus: np.ndarray, out_start: np.ndarray, out_res: np.ndarray, shifts: np.ndarray,
+                   refs: tuple) -> Tuple[np.ndarray, float]:
+        """one dg_vad_sweep_score_files against ``refs`` (``pack_speech_references`` of the curve's files) -> (components
+        (files, T, 2), device seconds)"""
+        rows, roff, _ = refs
         taus = np.ascontiguousarray(taus)
-        part = np.empty((len(self.uris), len(taus), 2), dtype=np.float64)
+        part = np.empty((len(roff) - 1, len(taus), 2), dtype=np.float64)
         rc, seconds = _timed(self.device, lambda st: _lib.lib().dg_vad_sweep_score_files(
-            self._h, taus.ctypes.data, len(taus), self.out_start.ctypes.data, self.out_res.ctypes.data,
-            self.shifts.ctypes.data, PATCH_COLLAR, rows.ctypes.data, roff.ctypes.data, part.ctypes.data, st))
+            self._h, taus.ctypes.data, len(taus), out_start.ctypes.data, out_res.ctypes.data,
+            shifts.ctypes.data, PATCH_COLLAR, rows.ctypes.data, roff.ctypes.data, part.ctypes.data, st))
         _lib.check(rc)
         return part, seconds()
 
-    def _components(self, f: int, comp: np.ndarray) -> DetectionErrorComponents:
+    def _components(self, f: int, comp: np.ndarray, refs: Optional[tuple] = None) -> DetectionErrorComponents:
         """false alarm and missed detection from the device; the total is the reference's duration, whatever the trial"""
-        return DetectionErrorComponents(comp[:, 0].copy(), comp[:, 1].copy(), np.full(len(comp), self._refs[2][f]))
+        refs = self._refs if refs is None else refs
+        return DetectionErrorComponents(comp[:, 0].copy(), comp[:, 1].copy(), np.full(len(comp), refs[2][f]))

@@ -278,6 +278,46 @@ int dg_sweep_score_files(dg_sweep* h, const float* seg_dev, const float* emb_dev
 /* the launch order of the (file, trial) states of dg_sweep_*_files, states_host int32 [num_files * T][2] = {file, trial}:
  * longest file first (equal chunk counts in file order), then trial.  Host only. */
 int dg_sweep_state_order(int num_files, const int32_t* chunk_offsets_host, int T, int32_t* states_host);
+/* ---- dg_sweep_run_latencies / dg_sweep_score_latencies: dg_sweep_*_files at several latencies from one set of network
+ *      outputs.  A file's windows at a smaller latency are a prefix of its windows at a larger one with the same left
+ *      padding.  seg_dev / emb_dev hold the chunks of num_units *units*, N in all, unit u at [unit_offsets_host[u],
+ *      unit_offsets_host[u + 1]) (as chunk_offsets_host above); a unit is the windows of one file at the largest latency of a
+ *      group whose outputs are prefixes of the unit's, bit for bit (the caller groups them).  A *virtual file* is one
+ *      (latency, file) pair, the first chunks of its unit; the num_virtual_files virtual files hold the num_virtual virtual
+ *      chunks, virtual file v at [virtual_offsets_host[v], virtual_offsets_host[v + 1]) (int32 [num_virtual_files + 1] from 0
+ *      to num_virtual, increasing), and vchunk_host int32 [num_virtual] gives the real chunk of each virtual chunk.  Every
+ *      virtual file must be the real chunks u0, u0 + 1, ... of one unit starting at its first chunk u0 and not crossing into
+ *      the next unit, and every plan row must aggregate no buffer before that first chunk, at most num_windows (the
+ *      handle's) of them, over at most frames + 1 output frames; otherwise DG_EINVAL before any launch.
+ *        params_host float64 [T][3] as dg_sweep_run: the clustering runs once per (unit, trial) for the units some virtual
+ *        file starts at, longest unit first, whatever the number of latencies;
+ *        plan_host int32 [num_virtual][4 + num_windows]: each virtual file's plan at its own latency (a fresh stream),
+ *        zero-padded to the handle's num_windows (that of the largest latency);
+ *        maps_dev int32 [T][N][K] or NULL: over the real chunks (those of units no virtual file reads are not written);
+ *        header_host int32 [T][num_virtual][4], turns: as dg_sweep_run_files over the virtual chunks;
+ *        out_start_host, out_res_host float64 [num_virtual], shifts_host float64 [num_virtual_files] and the references
+ *        (ref_offsets_host, ref_label_counts_host per virtual file) as dg_sweep_score_files with the virtual files as files;
+ *        components_host float64 [num_virtual_files][T][5]; num_virtual_files * T <= 2^21.
+ *      For a virtual file of latency L every result is what dg_sweep_*_files gives for that file's windows at latency L
+ *      alone.  One difference: a clustering error ("Cannot update unknown centers") in the chunks of a unit beyond a smaller
+ *      latency's prefix fails the call for every latency that reads the unit, not only for those whose windows reach it.
+ *      Synchronous.
+ *      dg_sweep_check_latencies: the layout checks alone, for a handle of num_windows and frames (host only, no device). ---- */
+int dg_sweep_run_latencies(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int num_units,
+                           const int32_t* unit_offsets_host, int num_virtual, int num_virtual_files, const int32_t* vchunk_host,
+                           const int32_t* virtual_offsets_host, const double* params_host, int T, const int32_t* plan_host,
+                           int32_t* maps_dev, int32_t* header_host, uint32_t* turns_host, int turn_cap_host, int* n_turns,
+                           void* stream);
+int dg_sweep_score_latencies(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int num_units,
+                             const int32_t* unit_offsets_host, int num_virtual, int num_virtual_files,
+                             const int32_t* vchunk_host, const int32_t* virtual_offsets_host, const double* params_host, int T,
+                             const int32_t* plan_host, const double* out_start_host, const double* out_res_host,
+                             const double* shifts_host, double collar, const double* ref_host, const int32_t* ref_label_host,
+                             const int32_t* ref_offsets_host, const int32_t* ref_label_counts_host, double* components_host,
+                             void* stream);
+int dg_sweep_check_latencies(int N, int num_units, const int32_t* unit_offsets_host, int num_virtual, int num_virtual_files,
+                             const int32_t* vchunk_host, const int32_t* virtual_offsets_host, const int32_t* plan_host,
+                             int num_windows, int frames);
 /* ---- voice activity detection sweep: the reference tunes VoiceActivityDetection's one hyper-parameter, tau_active, by
  *      running the whole pipeline per trial and file and scoring it with DetectionErrorRate(collar=0, skip_overlap=False)
  *      (reference blocks/vad.py:108-114, optim.py:98-122).  tau_active is read by Binarize alone, so here the speech curve of
@@ -298,11 +338,19 @@ int dg_sweep_state_order(int num_files, const int32_t* chunk_offsets_host, int T
  *        [ref_offsets_host[f], ref_offsets_host[f + 1]) (int32 [num_files + 1] from 0, not decreasing);
  *        components_host float64 [num_files][T][2] = {false alarm, missed detection} seconds.  The total (the reference's
  *        duration) does not depend on the trial and is the caller's.  Synchronous.
+ *      dg_vad_sweep_curve_latencies: the curve over the virtual layout of several latencies (units, virtual chunks and files,
+ *        plan zero-padded to the handle's num_windows, all as dg_sweep_run_latencies): virtual chunk c's curve is that of
+ *        real chunk vchunk_host[c] at its virtual file's latency.  Afterwards the handle's N and files are the virtual chunks
+ *        and files: dg_vad_sweep_run_files / dg_vad_sweep_score_files threshold and score every (latency, file) pair, with
+ *        out_start, out_res, shifts and references per virtual chunk and file.  Synchronous.
  *      Every argument is checked before any launch. ---- */
 int dg_vad_sweep_create(int frames, int local_speakers, int num_windows, const double* hamming_host, int device,
                         dg_vad_sweep** out);
 int dg_vad_sweep_curve(dg_vad_sweep* h, const float* seg_dev, int N, int num_files, const int32_t* chunk_offsets_host,
                        const int32_t* plan_host, void* stream);
+int dg_vad_sweep_curve_latencies(dg_vad_sweep* h, const float* seg_dev, int N, int num_units, const int32_t* unit_offsets_host,
+                                 int num_virtual, int num_virtual_files, const int32_t* vchunk_host,
+                                 const int32_t* virtual_offsets_host, const int32_t* plan_host, void* stream);
 int dg_vad_sweep_run_files(dg_vad_sweep* h, const double* taus_host, int T, int32_t* header_host, uint32_t* turns_host,
                            int turn_cap_host, int* n_turns, void* stream);
 int dg_vad_sweep_score_files(dg_vad_sweep* h, const double* taus_host, int T, const double* out_start_host,
