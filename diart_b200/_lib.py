@@ -100,6 +100,7 @@ SIGNATURES = {
     "dg_sweep_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, C.POINTER(_P)]),
     "dg_sweep_run": (C.c_int, [_P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, C.c_int, C.POINTER(C.c_int), _P]),
     "dg_sweep_destroy": (C.c_int, [_P]),
+    "dg_sweep_set_scored_regions": (C.c_int, [_P, C.c_int, _P, _P]),
     "dg_sweep_score": (C.c_int, [_P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, C.c_double, C.c_double, _P, _P, C.c_int,
                                  C.c_int, _P, _P, _P, C.c_int, _P]),
     "dg_sweep_run_files": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, _P, _P, _P, _P, _P, C.c_int,
@@ -118,6 +119,7 @@ SIGNATURES = {
     "dg_vad_sweep_run_files": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_int, C.POINTER(C.c_int), _P]),
     "dg_vad_sweep_score_files": (C.c_int, [_P, _P, C.c_int, _P, _P, _P, C.c_double, _P, _P, _P, _P]),
     "dg_vad_sweep_destroy": (C.c_int, [_P]),
+    "dg_vad_sweep_set_scored_regions": (C.c_int, [_P, C.c_int, _P, _P]),
     "dg_multi_create": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double,
                                   C.c_float, C.c_float, C.c_int, C.c_int, _P, C.POINTER(_P)]),
     "dg_multi_create_vad": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, _P, C.POINTER(_P)]),

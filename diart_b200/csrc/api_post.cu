@@ -138,10 +138,77 @@ struct DerBufs {
   DevBuf in, hoff, hseg, comp;
 };
 
+// The scored pieces of every file a scoring call covers (dg_sweep_set_scored_regions / dg_vad_sweep_set_scored_regions): file
+// f's pieces are rows [off[f], off[f + 1]), sorted, apart by more than 1e-6 s, finite and each truthy.  nf = 0: none, the
+// hypotheses are scored whole.
+struct ScoredRegions {
+  int nf = 0;
+  std::vector<double> rows;    // [S][2]
+  std::vector<int32_t> off;    // [nf + 1]
+};
+
+// the arguments are checked before the handle, so that the checks run without a device; r: the handle's regions
+static int set_scored_regions(const char* who, ScoredRegions* r, int nf, const double* rows, const int32_t* off) {
+  if (nf < 0 || (nf > 0 && !off)) {
+    set_error(std::string(who) + ": bad arguments (need num_files >= 0 and row offsets when num_files > 0)");
+    return DG_EINVAL;
+  }
+  if (nf > 0 && off[0] != 0) {
+    set_error(std::string(who) + ": scored region offsets must start at 0");
+    return DG_EINVAL;
+  }
+  for (int f = 0; f < nf; f++)
+    if (off[f + 1] < off[f]) {
+      set_error(std::string(who) + ": scored region offsets of file " + std::to_string(f) + " decrease");
+      return DG_EINVAL;
+    }
+  const int S = nf > 0 ? off[nf] : 0;
+  if (S > 0 && !rows) {
+    set_error(std::string(who) + ": non-null rows needed for " + std::to_string(S) + " scored regions");
+    return DG_EINVAL;
+  }
+  for (int f = 0; f < nf; f++)
+    for (int i = off[f]; i < off[f + 1]; i++) {
+      const double a = rows[2 * (size_t)i], b = rows[2 * (size_t)i + 1];
+      if (!std::isfinite(a) || !std::isfinite(b) || !(b - a > 1e-6)) {
+        set_error(std::string(who) + ": scored region " + std::to_string(i - off[f]) + " of file " + std::to_string(f) +
+                  " is not finite or not longer than 1e-6 s");
+        return DG_EINVAL;
+      }
+      if (i > off[f] && !(a - rows[2 * (size_t)i - 1] > 1e-6)) {
+        set_error(std::string(who) + ": scored region " + std::to_string(i - off[f]) + " of file " + std::to_string(f) +
+                  " does not start more than 1e-6 s after the previous one ends");
+        return DG_EINVAL;
+      }
+    }
+  if (!r) {
+    set_error(std::string(who) + ": null handle");
+    return DG_EINVAL;
+  }
+  r->nf = nf;
+  r->rows.assign(rows, rows + 2 * (size_t)S);
+  if (nf > 0)
+    r->off.assign(off, off + nf + 1);
+  else
+    r->off.clear();
+  return DG_OK;
+}
+
+// a scoring call over nf files while regions are set must cover exactly their files (before any launch)
+static int regions_check(const char* who, const ScoredRegions& r, int nf) {
+  if (r.nf > 0 && r.nf != nf) {
+    set_error(std::string(who) + ": scored regions are set for " + std::to_string(r.nf) + " files, the call scores " +
+              std::to_string(nf) + " (set them again, or clear them with num_files = 0)");
+    return DG_EINVAL;
+  }
+  return DG_OK;
+}
+
 struct dg_sweep {
   int device = 0, M = 0, D = 0, F = 0, K = 0, nw = 1;
   DevBuf hamming, in, centers, active, init, prep, prep_d, maps, header, turns, total;
   DerBufs der;                    // dg_sweep_score
+  ScoredRegions regions;          // dg_sweep_set_scored_regions
   PinnedBuf pin;                  // params, taus and plan in; error flags, header, total and a turn prefix out
 };
 
@@ -165,6 +232,11 @@ extern "C" int dg_sweep_create(int max_speakers, int dim, int frames, int local_
 extern "C" int dg_sweep_destroy(dg_sweep* h) {
   delete h;
   return DG_OK;
+}
+
+extern "C" int dg_sweep_set_scored_regions(dg_sweep* h, int num_files, const double* rows_host,
+                                           const int32_t* offsets_host) {
+  return set_scored_regions("dg_sweep_set_scored_regions", h ? &h->regions : nullptr, num_files, rows_host, offsets_host);
 }
 
 // at most this many (file, trial) states per call: der_hyp runs one warp per (state, label) with up to 32 labels and
@@ -414,21 +486,26 @@ static int sweep_check_reference(const char* who, const double* ref_host, const 
 
 // The der_hyp -> der_scan -> der_score sequence over a post-path result already on the device (header [T][N][4] and `total`
 // turns, M labels): the DER components comp [nf][T][5] of every (file, trial) against the file's reference rows
-// [ref_off[f], ref_off[f + 1]) with R[f] labels, the arguments checked by the caller.  Uses the pinned buffer `pinbuf`;
+// [ref_off[f], ref_off[f + 1]) with R[f] labels, the arguments checked by the caller.  With regions (nf files), der_score
+// crops each hypothesis to its file's scored pieces; the reference rows come cropped.  Uses the pinned buffer `pinbuf`;
 // synchronises `st`.
 static int der_components(const char* who, DerBufs& b, PinnedBuf& pinbuf, const int32_t* header_dev, const uint32_t* turns_dev,
                           unsigned int total, int N, int nf, const int32_t* chunk_off, int T, int M,
                           const double* out_start_host, const double* out_res_host, const double* shift_host, double collar,
                           const double* ref_host, const int32_t* ref_label_host, const int32_t* ref_off, const int32_t* R_host,
                           double* components_host, int32_t* hyp_offsets_dev, double* hyp_segments_dev, int hyp_cap,
-                          cudaStream_t st) {
+                          cudaStream_t st, const ScoredRegions* regions = nullptr) {
   int rc;
   const int NTM = nf * T * M, S = ref_off[nf];
+  const bool crop = regions && regions->nf > 0;
   // host -> device, one copy: out_start [N], out_res [N], shifts [nf], reference segments [S][2] grouped by label within each
-  // file, label offsets [nf][DER_ROFF], label counts [nf], chunk offsets [nf + 1]
+  // file, label offsets [nf][DER_ROFF], label counts [nf], chunk offsets [nf + 1], then with regions the scored pieces [U][2]
+  // (at the next multiple of 8 bytes) and their offsets [nf + 1]
   const size_t times_b = (size_t)N * 16, shift_b = (size_t)nf * 8, rseg_b = (size_t)S * 16;
   const size_t roff_b = (size_t)nf * DER_ROFF * 4, R_b = (size_t)nf * 4, off_b = (size_t)(nf + 1) * 4;
-  const size_t in_b = times_b + shift_b + rseg_b + roff_b + R_b + off_b, comp_b = (size_t)nf * T * 40;
+  const size_t base_b = times_b + shift_b + rseg_b + roff_b + R_b + off_b, useg_at = (base_b + 7) & ~(size_t)7;
+  const size_t useg_b = crop ? regions->rows.size() * 8 : 0, uoff_b = crop ? (size_t)(nf + 1) * 4 : 0;
+  const size_t in_b = crop ? useg_at + useg_b + uoff_b : base_b, comp_b = (size_t)nf * T * 40;
   if (b.in.ensure(in_b) || b.hoff.ensure((size_t)(NTM + 1) * 4) || b.hseg.ensure((size_t)std::max(total, 1u) * 16) ||
       b.comp.ensure(comp_b) || pinbuf.ensure(std::max(in_b, comp_b + 16)))
     return DG_ECUDA;
@@ -440,6 +517,10 @@ static int der_components(const char* who, DerBufs& b, PinnedBuf& pinbuf, const 
   int32_t* roff_all = reinterpret_cast<int32_t*>(pin + times_b + shift_b + rseg_b);
   memcpy(pin + times_b + shift_b + rseg_b + roff_b, R_host, R_b);
   memcpy(pin + times_b + shift_b + rseg_b + roff_b + R_b, chunk_off, off_b);
+  if (crop) {
+    if (useg_b) memcpy(pin + useg_at, regions->rows.data(), useg_b);
+    memcpy(pin + useg_at + useg_b, regions->off.data(), uoff_b);
+  }
   for (int f = 0; f < nf; f++) {
     const int a = ref_off[f], n = ref_off[f + 1] - a, R = R_host[f];
     int32_t* roff = roff_all + (size_t)f * DER_ROFF;
@@ -464,11 +545,14 @@ static int der_components(const char* who, DerBufs& b, PinnedBuf& pinbuf, const 
   const int* d_roff = reinterpret_cast<const int*>(din + times_b + shift_b + rseg_b);
   const int* d_R = reinterpret_cast<const int*>(din + times_b + shift_b + rseg_b + roff_b);
   const int* d_off = reinterpret_cast<const int*>(din + times_b + shift_b + rseg_b + roff_b + R_b);
+  const double* d_useg = crop ? reinterpret_cast<const double*>(din + useg_at) : nullptr;
+  const int* d_uoff = crop ? reinterpret_cast<const int*>(din + useg_at + useg_b) : nullptr;
   int* hoff = b.hoff.as<int>();
   if ((rc = launch_der_hyp_count(header_dev, turns_dev, nf, d_off, T, N, M, d_start, d_res, d_shift, collar, hoff, st)) ||
       (rc = launch_der_hyp_write(header_dev, turns_dev, nf, d_off, T, N, M, d_start, d_res, d_shift, collar, hoff,
                                  b.hseg.as<double>(), hyp_segments_dev, hyp_cap, st)) ||
-      (rc = launch_der_score(hoff, b.hseg.as<double>(), nf, T, M, d_roff, d_R, d_rseg, b.comp.as<double>(), st)))
+      (rc = launch_der_score(hoff, b.hseg.as<double>(), nf, T, M, d_roff, d_R, d_rseg, b.comp.as<double>(), st, d_uoff,
+                             d_useg)))
     return rc;
   if (hyp_offsets_dev) DG_CUDA(cudaMemcpyAsync(hyp_offsets_dev, hoff, (size_t)(NTM + 1) * 4, cudaMemcpyDeviceToDevice, st));
   DG_CUDA(cudaMemcpyAsync(pin, b.comp.p, comp_b, cudaMemcpyDeviceToHost, st));
@@ -537,7 +621,8 @@ static int sweep_score(const char* who, dg_sweep* h, const float* seg_dev, const
   int rc;
   if ((rc = sweep_check(who, h, seg_dev, emb_dev, N, nf, chunk_off, params_host, T, plan_host)) ||
       (rc = score_check(who, N, nf, out_start_host, out_res_host, shift_host, collar, ref_host, ref_label_host, ref_off,
-                        R_host, components_host, hyp_cap)))
+                        R_host, components_host, hyp_cap)) ||
+      (rc = regions_check(who, h->regions, nf)))
     return rc;
   DG_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)stream;
@@ -547,7 +632,7 @@ static int sweep_score(const char* who, dg_sweep* h, const float* seg_dev, const
     return rc;
   return der_components(who, h->der, h->pin, h->header.as<int32_t>(), h->turns.as<uint32_t>(), total, N, nf, chunk_off, T,
                         h->M, out_start_host, out_res_host, shift_host, collar, ref_host, ref_label_host, ref_off, R_host,
-                        components_host, hyp_offsets_dev, hyp_segments_dev, hyp_cap, st);
+                        components_host, hyp_offsets_dev, hyp_segments_dev, hyp_cap, st, &h->regions);
 }
 
 extern "C" int dg_sweep_score(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, const double* params_host,
@@ -691,7 +776,8 @@ extern "C" int dg_sweep_score_latencies(dg_sweep* h, const float* seg_dev, const
     return rc;
   const int Nv = num_virtual, nvf = num_virtual_files;
   if ((rc = score_check(who, Nv, nvf, out_start_host, out_res_host, shifts_host, collar, ref_host, ref_label_host,
-                        ref_offsets_host, ref_label_counts_host, components_host, 0)))
+                        ref_offsets_host, ref_label_counts_host, components_host, 0)) ||
+      (rc = regions_check(who, h->regions, nvf)))
     return rc;
   DG_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)stream;
@@ -701,7 +787,8 @@ extern "C" int dg_sweep_score_latencies(dg_sweep* h, const float* seg_dev, const
     return rc;
   return der_components(who, h->der, h->pin, h->header.as<int32_t>(), h->turns.as<uint32_t>(), total, Nv, nvf,
                         virtual_offsets_host, T, h->M, out_start_host, out_res_host, shifts_host, collar, ref_host,
-                        ref_label_host, ref_offsets_host, ref_label_counts_host, components_host, nullptr, nullptr, 0, st);
+                        ref_label_host, ref_offsets_host, ref_label_counts_host, components_host, nullptr, nullptr, 0, st,
+                        &h->regions);
 }
 
 // ============================================================================= voice activity detection sweep
@@ -715,6 +802,7 @@ struct dg_vad_sweep {
   std::vector<int32_t> chunk_off;        // [nf + 1]
   DevBuf hamming, in, curve, header, turns, total, taus;
   DerBufs der;
+  ScoredRegions regions;                 // dg_vad_sweep_set_scored_regions
   PinnedBuf pin;
 };
 
@@ -737,6 +825,12 @@ extern "C" int dg_vad_sweep_create(int frames, int local_speakers, int num_windo
 extern "C" int dg_vad_sweep_destroy(dg_vad_sweep* h) {
   delete h;
   return DG_OK;
+}
+
+extern "C" int dg_vad_sweep_set_scored_regions(dg_vad_sweep* h, int num_files, const double* rows_host,
+                                               const int32_t* offsets_host) {
+  return set_scored_regions("dg_vad_sweep_set_scored_regions", h ? &h->regions : nullptr, num_files, rows_host,
+                            offsets_host);
 }
 
 extern "C" int dg_vad_sweep_curve(dg_vad_sweep* h, const float* seg_dev, int N, int num_files,
@@ -920,7 +1014,7 @@ extern "C" int dg_vad_sweep_score_files(dg_vad_sweep* h, const double* taus_host
                                         void* stream) {
   const char* who = "dg_vad_sweep_score_files";
   int rc;
-  if ((rc = vad_check(who, h, taus_host, T))) return rc;
+  if ((rc = vad_check(who, h, taus_host, T)) || (rc = regions_check(who, h->regions, h->nf))) return rc;
   const int N = h->N, nf = h->nf;
   if (!out_start_host || !out_res_host || !shifts_host || !components_host || !ref_offsets_host || !std::isfinite(collar) ||
       collar < 0) {
@@ -975,7 +1069,7 @@ extern "C" int dg_vad_sweep_score_files(dg_vad_sweep* h, const double* taus_host
   std::vector<double> comp((size_t)nf * T * 5);
   if ((rc = der_components(who, h->der, h->pin, h->header.as<int32_t>(), h->turns.as<uint32_t>(), total, N, nf,
                            h->chunk_off.data(), T, 1, out_start_host, out_res_host, shifts_host, collar, ref_host,
-                           labels.data(), ref_offsets_host, R.data(), comp.data(), nullptr, nullptr, 0, st)))
+                           labels.data(), ref_offsets_host, R.data(), comp.data(), nullptr, nullptr, 0, st, &h->regions)))
     return rc;
   for (size_t i = 0; i < (size_t)nf * T; i++) {
     components_host[2 * i] = comp[5 * i];           // false alarm

@@ -1,6 +1,6 @@
 // Diarization error rate of hyper-parameter trials on the device (the `metric(reference, hypothesis)` step of the reference's
-// Benchmark.evaluate with DiarizationErrorRate(collar=0, skip_overlap=False), src/diart/inference.py:359-390), DESIGN.md
-// "DER scoring" for the definition.
+// Benchmark.evaluate with DiarizationErrorRate, src/diart/inference.py:359-390), DESIGN.md "DER scoring" for the definition:
+// collar=0, skip_overlap=False and no uem, or any of them through the scored regions the hypotheses are cropped to.
 //
 //   der_hyp<false> / der_hyp<true>   one warp per (file, trial, label): walks the sweep's per-chunk turns of that file's
 //                                    chunk range in chunk order, with the file's timestamp shift, and merges that label's
@@ -9,7 +9,8 @@
 //   der_scan                         exclusive prefix sum of the (file, trial, label) counts
 //   der_score                        one warp per (file, trial) against that file's reference: k-way merge of the boundary
 //                                    lists (one lane per hypothesis label and per reference label), co-occurrence matrix,
-//                                    LSAP, the five components
+//                                    LSAP, the five components; der_score<true> first crops each hypothesis label to the
+//                                    file's scored pieces (CropList)
 //
 // Every float64 operation is explicitly rounded (no FMA contraction): the segment times equal numpy's turn_times /
 // assemble_predictions bit for bit, and the components are sums in time order, independent of the launch geometry.
@@ -136,11 +137,56 @@ struct SegList {
   __device__ double next(double b) const { return i < n ? (s > b ? s : e) : INFINITY; }
 };
 
+// One hypothesis label's segments cropped to the file's scored pieces (DESIGN.md "DER scoring", step 4), read one piece at a
+// time with SegList's interface: segment i is cut against each scored piece k it intersects (Segment.intersects with
+// pyannote.core's 1e-6 s precision, in float64 as oracle/detection.py has it), and a falsy intersection is dropped.  The
+// label's segments are sorted and apart, so its pieces are too.  j: the first scored piece that does not end at or before
+// segment i's start; k: the next candidate for segment i.
+struct CropList {
+  const double* p;
+  int i, n;
+  const double* u;
+  int j, m, k;
+  double hs, he, s, e;
+  __device__ void start_segment() {
+    hs = p[(size_t)i * 2];
+    he = p[(size_t)i * 2 + 1];
+    while (j < m && u[(size_t)j * 2 + 1] <= hs) j++;
+    k = j;
+  }
+  __device__ void seek() {   // from candidate (i, k) on, to the next truthy piece (i = n: none)
+    while (i < n) {
+      if (k < m && u[(size_t)k * 2] < he) {
+        const double bs = u[(size_t)k * 2], be = u[(size_t)k * 2 + 1];
+        k++;
+        const bool hit = (hs < bs && bs < __dsub_rn(he, 1e-6)) || (hs > bs && hs < __dsub_rn(be, 1e-6)) || hs == bs;
+        const double cs = fmax(hs, bs), ce = fmin(he, be);
+        if (hit && __dsub_rn(ce, cs) > 1e-6) {
+          s = cs;
+          e = ce;
+          return;
+        }
+      } else if (++i < n) {
+        start_segment();
+      }
+    }
+  }
+  __device__ void load() {
+    if (i < n) start_segment();
+    seek();
+  }
+  __device__ void advance(double b) {
+    while (i < n && e <= b) seek();
+  }
+  __device__ bool active(double b) const { return i < n && s <= b; }
+  __device__ double next(double b) const { return i < n ? (s > b ? s : e) : INFINITY; }
+};
+
 // Walks the elementary intervals [b, bn) of the union of all boundaries in time order and calls body(d, hyp active, ref active)
-// for each one with Segment(b, bn) truthy.  Lane l holds hypothesis label l and reference label l.
-template <typename Body>
-__device__ __forceinline__ void der_walk(const double* hp, int h0, int h1, const double* rp, int r0, int r1, Body body) {
-  SegList hl{hp, h0, h1, 0.0, 0.0}, rl{rp, r0, r1, 0.0, 0.0};
+// for each one with Segment(b, bn) truthy.  Lane l holds hypothesis label l (`hl`: a SegList, or a CropList) and reference
+// label l.
+template <typename HypList, typename Body>
+__device__ __forceinline__ void der_walk_list(HypList& hl, SegList& rl, Body body) {
   hl.load();
   rl.load();
   double b = warp_min_d(fmin(hl.next(-INFINITY), rl.next(-INFINITY)));
@@ -156,12 +202,29 @@ __device__ __forceinline__ void der_walk(const double* hp, int h0, int h1, const
   }
 }
 
+// der_walk_list over hypothesis segments [h0, h1) of hp, cropped to the scored pieces [u0, u1) of up when CROP
+template <bool CROP, typename Body>
+__device__ __forceinline__ void der_walk(const double* hp, int h0, int h1, const double* up, int u0, int u1,
+                                         const double* rp, int r0, int r1, Body body) {
+  if constexpr (CROP) {
+    CropList hl{hp, h0, h1, up, u0, u1, 0, 0.0, 0.0, 0.0, 0.0};
+    SegList rl{rp, r0, r1, 0.0, 0.0};
+    der_walk_list(hl, rl, body);
+  } else {
+    SegList hl{hp, h0, h1, 0.0, 0.0}, rl{rp, r0, r1, 0.0, 0.0};
+    der_walk_list(hl, rl, body);
+  }
+}
+
 // comp [nf][T][5] = {false alarm, missed detection, confusion, correct, total}; warp (f, t) scores trial t of file f against
-// file f's reference: R[f] labels at offsets roff [f][DER_ROFF] into rseg
+// file f's reference: R[f] labels at offsets roff [f][DER_ROFF] into rseg.  CROP: every hypothesis label is first cropped to
+// file f's scored pieces [uoff[f], uoff[f + 1]) of useg (CropList); the reference comes cropped from the host.
+template <bool CROP>
 __global__ void __launch_bounds__(DER_SCORE_THREADS)
 der_score_kernel(const int* __restrict__ hoff /*[nf*T*M+1]*/, const double* __restrict__ hseg, int nf, int T, int M,
                  const int* __restrict__ roff_all /*[nf][DER_ROFF]*/, const int* __restrict__ R_all /*[nf]*/,
-                 const double* __restrict__ rseg, double* __restrict__ comp) {
+                 const double* __restrict__ rseg, double* __restrict__ comp, const int* __restrict__ uoff /*[nf+1]*/,
+                 const double* __restrict__ useg) {
   __shared__ double tr[DER_SCORE_THREADS / 32][32][33];
   const int ft = (int)(((size_t)blockIdx.x * DER_SCORE_THREADS + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (ft >= nf * T) return;
@@ -169,11 +232,12 @@ der_score_kernel(const int* __restrict__ hoff /*[nf*T*M+1]*/, const double* __re
   const int* roff = roff_all + (size_t)f * DER_ROFF;
   const int h0 = lane < M ? hoff[ft * M + lane] : 0, h1 = lane < M ? hoff[ft * M + lane + 1] : 0;
   const int r0 = lane < R ? roff[lane] : 0, r1 = lane < R ? roff[lane + 1] : 0;
+  const int u0 = CROP ? uoff[f] : 0, u1 = CROP ? uoff[f + 1] : 0;
   // pass 1: co-occurrence C[r][h], lane h owns column h, each entry summed in time order
   double C[32];
 #pragma unroll
   for (int q = 0; q < 32; q++) C[q] = 0.0;
-  der_walk(hseg, h0, h1, rseg, r0, r1, [&](double d, bool ah, bool ar) {
+  der_walk<CROP>(hseg, h0, h1, useg, u0, u1, rseg, r0, r1, [&](double d, bool ah, bool ar) {
     const unsigned rmask = __ballot_sync(FULL, ar);
 #pragma unroll
     for (int q = 0; q < 32; q++)
@@ -202,7 +266,7 @@ der_score_kernel(const int* __restrict__ hoff /*[nf*T*M+1]*/, const double* __re
   }
   // pass 2: the components, in time order
   double fa = 0.0, miss = 0.0, conf = 0.0, corr = 0.0, tot = 0.0;
-  der_walk(hseg, h0, h1, rseg, r0, r1, [&](double d, bool ah, bool ar) {
+  der_walk<CROP>(hseg, h0, h1, useg, u0, u1, rseg, r0, r1, [&](double d, bool ah, bool ar) {
     const unsigned hmask = __ballot_sync(FULL, ah);
     const int nr = __popc(__ballot_sync(FULL, ar)), nh = __popc(hmask);
     const int c = __popc(__ballot_sync(FULL, ar && partner >= 0 && ((hmask >> partner) & 1u)));
@@ -249,10 +313,14 @@ int launch_der_hyp_write(const int32_t* header, const uint32_t* turns, int nf, c
 }
 
 int launch_der_score(const int* hoff, const double* hseg, int nf, int T, int M, const int* roff, const int* R,
-                     const double* rseg, double* comp, cudaStream_t st) {
+                     const double* rseg, double* comp, cudaStream_t st, const int* uoff, const double* useg) {
   ProfScope _ps("der_score", st);
   const unsigned blocks = (unsigned)(((long long)nf * T * 32 + DER_SCORE_THREADS - 1) / DER_SCORE_THREADS);
-  der_score_kernel<<<blocks, DER_SCORE_THREADS, 0, st>>>(hoff, hseg, nf, T, M, roff, R, rseg, comp);
+  if (uoff)
+    der_score_kernel<true><<<blocks, DER_SCORE_THREADS, 0, st>>>(hoff, hseg, nf, T, M, roff, R, rseg, comp, uoff, useg);
+  else
+    der_score_kernel<false><<<blocks, DER_SCORE_THREADS, 0, st>>>(hoff, hseg, nf, T, M, roff, R, rseg, comp, nullptr,
+                                                                 nullptr);
   DG_LAUNCHED();
   return 0;
 }

@@ -316,10 +316,12 @@ int launch_der_hyp_write(const int32_t* header, const uint32_t* turns, int nf, c
                          const double* out_start, const double* out_res, const double* shifts, double collar, int* offsets,
                          double* segs, double* segs_copy, int copy_cap, cudaStream_t st);
 // reference of file f: R[f] labels, offsets roff [f][DER_ROFF] (R[f] + 1 used) into rseg [S][2];
-// comp [nf][T][5] = {false alarm, missed, confusion, correct, total}
+// comp [nf][T][5] = {false alarm, missed, confusion, correct, total}.  With uoff (device [nf + 1]) the hypothesis of file f is
+// cropped to its scored pieces useg [uoff[f], uoff[f + 1])[2] (sorted, apart by more than 1e-6 s, each truthy)
 constexpr int DER_ROFF = 33;
 int launch_der_score(const int* hoff, const double* hseg, int nf, int T, int M, const int* roff, const int* R,
-                     const double* rseg, double* comp, cudaStream_t st);
+                     const double* rseg, double* comp, cudaStream_t st, const int* uoff = nullptr,
+                     const double* useg = nullptr);
 // vad.cu -- VAD sweep: the speech curve of N chunks (max over K local speakers, aggregated as launch_post with one speaker;
 // chunk c's frames at curve [curve_off[c], curve_off[c + 1])), then per trial t the turns of curve > taus[t], header [T][N][4]
 int launch_vad_curve(const float* seg, int N, int F, int K, const int32_t* plan, int plan_stride, const double* hamming,

@@ -29,6 +29,11 @@ kernel again.
 (``dg_vad_sweep_curve``, ``csrc/vad.cu``), and every trial only thresholds it and is scored by detection error rate
 (``DetectionErrorRate(collar=0, skip_overlap=False)``, the pipeline's ``suggest_metric()``; DESIGN.md "Detection error").
 
+Every ``score`` method also takes a ``metric`` (:class:`DiarizationErrorRate` / :class:`DetectionErrorRate`, or
+pyannote.metrics' own, with a forgiveness collar and ``skip_overlap``) and the dataset sweeps a uem per file
+(``uems``): :func:`scored_regions` computes each file's scored regions once, the references are cropped to them on the
+host and the hypotheses on the device (``dg_sweep_set_scored_regions``; DESIGN.md "DER scoring", steps 1-5).
+
 The three classes share their mechanics: :class:`FileBatches` cuts the window batches of every network pass,
 :func:`stream_plan` is the post-path plan of one file, ``_timed`` puts CUDA events around one C call and ``_turn_list_call``
 downloads a turn list into a host buffer that grows on demand.  ``HyperParameterSweep._run_trials`` / ``_score_trials`` are the
@@ -37,9 +42,12 @@ dataset classes (files, offsets, plans, references and the loops over trial grou
 """
 from __future__ import annotations
 
+import bisect
 import copy
 import ctypes as C
 import functools
+import itertools
+import math
 import operator
 import time
 from dataclasses import dataclass
@@ -62,6 +70,8 @@ TRIALS_PER_LAUNCH = 1024      # trials per dg_sweep_run; more run as further lau
 TRIAL_CHUNKS_PER_LAUNCH = 4 << 20   # DatasetSweep: trials x chunks per launch (bounds the header, maps and turn buffers)
 PATCH_COLLAR = 0.05           # PredictionAccumulator's default (sinks.py)
 MAX_REFERENCE_LABELS = 32     # one lane per reference label in the scoring kernel
+PRECISION = 1e-6              # pyannote.core's SEGMENT_PRECISION: Segment.__bool__, Segment.intersects
+WHOLE_LINE = (-1e300, 1e300)  # the uem of a file that has none (scored_regions: the scored regions do not depend on the trial)
 
 
 def trial_params(trials: Sequence[Mapping[str, float]], config, names: Optional[Sequence[str]] = None) -> np.ndarray:
@@ -172,18 +182,172 @@ def assemble_predictions(header: np.ndarray, turns: np.ndarray, n_turns: int, ou
     return out
 
 
-def reference_arrays(annotation: Annotation) -> Tuple[np.ndarray, np.ndarray, List]:
+# ---------------------------------------------------------------------- scoring protocols (DESIGN.md "DER scoring", steps 1-4)
+@dataclass(frozen=True)
+class DiarizationErrorRate:
+    """The constructor arguments of pyannote.metrics' ``DiarizationErrorRate`` a diarization sweep can score with: a
+    forgiveness ``collar`` (seconds, removed around every reference boundary, half on each side) and ``skip_overlap``
+    (leave out the reference's overlapped speech).  The default is the pipelines' ``suggest_metric()``."""
+    collar: float = 0.0
+    skip_overlap: bool = False
+
+
+@dataclass(frozen=True)
+class DetectionErrorRate:
+    """The same for pyannote.metrics' ``DetectionErrorRate``, the metric of :class:`VoiceActivitySweep`."""
+    collar: float = 0.0
+    skip_overlap: bool = False
+
+
+def metric_protocol(metric, kind: str) -> Tuple[float, bool]:
+    """``metric`` (None: the default) -> (collar, skip_overlap).  Accepted: an object whose class is named ``kind``
+    (:class:`DiarizationErrorRate` / :class:`DetectionErrorRate`, or pyannote.metrics' class of that name) with ``collar``
+    and ``skip_overlap`` attributes; the collar must be a finite number >= 0.  Anything else: ValueError."""
+    if metric is None:
+        return 0.0, False
+    if type(metric).__name__ != kind or not hasattr(metric, "collar") or not hasattr(metric, "skip_overlap"):
+        raise ValueError(f"metric {metric!r}: this sweep scores a {kind} (collar, skip_overlap)")
+    collar = metric.collar
+    if isinstance(collar, bool) or not isinstance(collar, (int, float, np.integer, np.floating)) or \
+            not math.isfinite(float(collar)) or float(collar) < 0:
+        raise ValueError(f"metric collar {collar!r}: need a finite number >= 0")
+    return float(collar), bool(metric.skip_overlap)
+
+
+def check_uem(uem) -> Optional[List[Tuple[float, float]]]:
+    """A uem (None, or a list of ``(start, end)`` pairs or ``Segment``s sorted by (start, end), each finite and truthy)
+    -> a list of float pairs; anything else: ValueError"""
+    if uem is None:
+        return None
+    if not isinstance(uem, (list, tuple)):
+        raise ValueError(f"a uem is a list of (start, end) pairs or Segments, not {type(uem).__name__}")
+    out = []
+    for i, piece in enumerate(uem):
+        try:
+            start, end = (piece.start, piece.end) if hasattr(piece, "start") else piece
+            start, end = float(start), float(end)
+        except (TypeError, ValueError):
+            raise ValueError(f"uem piece {i} ({piece!r}) is not a (start, end) pair or a Segment") from None
+        if not (math.isfinite(start) and math.isfinite(end)) or not end - start > PRECISION:
+            raise ValueError(f"uem piece {i} ({start}, {end}) is not finite or not longer than {PRECISION} s (falsy)")
+        out.append((start, end))
+    if out != sorted(out):
+        raise ValueError("the uem pieces are not sorted by (start, end)")
+    return out
+
+
+def _truthy(a: float, b: float) -> bool:
+    """``bool(Segment(a, b))``"""
+    return (b - a) > PRECISION
+
+
+def _co_iter(a: List[Tuple[float, float]], b: List[Tuple[float, float]]):
+    """``Timeline.co_iter``: pairs (x, y), x of sorted ``a`` in order, y of sorted ``b`` in order, with ``x.intersects(y)``
+    (pyannote.core's rule).  The y before the first whose running maximum of ends reaches x's start end before x starts,
+    so cannot intersect it: they are skipped by bisection."""
+    ends = list(itertools.accumulate((y[1] for y in b), max))
+    for x in a:
+        for y in b[bisect.bisect_left(ends, x[0]):]:
+            if y > (x[1], x[1]):
+                break
+            if (x[0] < y[0] and y[0] < x[1] - PRECISION) or (x[0] > y[0] and x[0] < y[1] - PRECISION) or x[0] == y[0]:
+                yield x, y
+
+
+def _support(segs) -> List[Tuple[float, float]]:
+    """``Timeline.support()`` of the unique segments in (start, end) order"""
+    out: List[Tuple[float, float]] = []
+    for s in sorted(set(segs)):
+        if out and not _truthy(min(s[1], out[-1][1]), max(s[0], out[-1][0])):
+            out[-1] = (min(out[-1][0], s[0]), max(out[-1][1], s[1]))
+        else:
+            out.append(s)
+    return out
+
+
+def _gaps(segs, uem) -> List[Tuple[float, float]]:
+    """``Timeline(segs).gaps(support=uem)``: per piece of the uem's support, the truthy gaps between the support of the
+    segments cropped to it"""
+    out = []
+    for u in _support(uem):
+        end = u[0]
+        inside = [(max(x[0], y[0]), min(x[1], y[1])) for x, y in _co_iter(sorted(set(segs)), [u])]
+        for s in _support(p for p in inside if _truthy(*p)):
+            if _truthy(end, s[0]):
+                out.append((end, s[0]))
+            end = s[1]
+        if _truthy(end, u[1]):
+            out.append((end, u[1]))
+    return out
+
+
+def scored_regions(reference: Annotation, collar: float = 0.0, skip_overlap: bool = False,
+                   uem=None) -> List[Tuple[float, float]]:
+    """The regions of a file that pyannote.metrics scores with ``collar`` / ``skip_overlap`` within ``uem`` (steps 1-3 of
+    DESIGN.md "DER scoring"): the gaps, within the uem, of the support of the removed regions -- a ``collar``-wide segment
+    around both ends of every unique non-empty reference segment, and the intersection of every pair of intersecting
+    reference tracks other than a track with itself.  Sorted, each truthy, apart by more than 1e-6 s.
+
+    Without a uem pyannote takes the extent of both sides, which depends on the hypothesis.  Nothing is active outside
+    it, so the regions are computed within :data:`WHOLE_LINE` instead, once per file: the same scores except where a
+    removed region starts within 1e-6 s of the extent's end or ends within 1e-6 s of its start (out of contract)."""
+    collar, skip_overlap = metric_protocol(DiarizationErrorRate(collar, skip_overlap), "DiarizationErrorRate")
+    uem = check_uem(uem)
+    tracks: Dict[Tuple[float, float], int] = {}
+    for segment, _ in reference.itertracks():
+        if segment:
+            key = (segment.start, segment.end)
+            tracks[key] = tracks.get(key, 0) + 1
+    segs = sorted(tracks)
+    removed = []
+    if collar > 0:
+        for s, e in segs:
+            removed += [(s - .5 * collar, s + .5 * collar), (e - .5 * collar, e + .5 * collar)]
+    if skip_overlap:
+        for x, y in _co_iter(segs, segs):
+            if x != y or tracks[x] > 1:           # every pair of tracks but a track with itself
+                removed.append((max(x[0], y[0]), min(x[1], y[1])))
+    return _gaps(_support(r for r in removed if _truthy(*r)), [WHOLE_LINE] if uem is None else uem)
+
+
+def cropped_tracks(annotation: Annotation, regions: Optional[Sequence[Tuple[float, float]]] = None) -> List[tuple]:
+    """(start, end, label) of every non-empty track; with ``regions`` (sorted, apart) each cut against every region it
+    intersects, the falsy pieces dropped: ``annotation.crop(regions, mode="intersection")`` (step 4)"""
+    rows = [(s.start, s.end, label) for s, _, label in annotation.itertracks(yield_label=True) if s]
+    if regions is None:
+        return rows
+    labels: Dict[Tuple[float, float], list] = {}
+    for a, b, label in rows:
+        labels.setdefault((a, b), []).append(label)
+    out = []
+    for x, r in _co_iter(sorted(labels), list(regions)):
+        a, b = max(x[0], r[0]), min(x[1], r[1])
+        if _truthy(a, b):
+            out += [(a, b, label) for label in labels[x]]
+    return out
+
+
+def pack_regions(regions: Sequence[Sequence[Tuple[float, float]]]) -> Tuple[np.ndarray, np.ndarray]:
+    """per-file scored regions -> the arguments of dg_sweep_set_scored_regions: (rows float64 (S, 2), offsets int32
+    (files + 1,))"""
+    rows = [np.asarray(r, dtype=np.float64).reshape(-1, 2) for r in regions]
+    return (np.ascontiguousarray(np.concatenate(rows), dtype=np.float64),
+            np.array(np.cumsum([0] + [len(r) for r in rows]), dtype=np.int32))
+
+
+def reference_arrays(annotation: Annotation, regions: Optional[Sequence[Tuple[float, float]]] = None) \
+        -> Tuple[np.ndarray, np.ndarray, List]:
     """A reference annotation -> (rows float64 (S, 2) start / end, labels int32 (S,), label names) for ``dg_sweep_score``:
     labels numbered in string order, empty segments dropped (``Segment.__bool__``), each label reduced to the union of its
-    segments (rows of one label sorted, touching or overlapping segments merged).
+    segments (rows of one label sorted, touching or overlapping segments merged).  With ``regions`` (:func:`scored_regions`)
+    every segment is first cropped to them (:func:`cropped_tracks`); a label left without a piece disappears.
 
     pyannote.metrics scores a reference as given; where one label overlaps itself it may count that label twice in the
     overlap.  The union counts it once: the two agree for every reference in which no label overlaps itself.
     More than 32 labels: ValueError."""
     by_label: Dict = {}
-    for segment, _, label in annotation.itertracks(yield_label=True):
-        if segment:
-            by_label.setdefault(label, []).append((segment.start, segment.end))
+    for start, end, label in cropped_tracks(annotation, regions):
+        by_label.setdefault(label, []).append((start, end))
     names = sorted(by_label, key=str)
     if len(names) > MAX_REFERENCE_LABELS:
         raise ValueError(f"the reference has {len(names)} labels; at most {MAX_REFERENCE_LABELS} can be scored")
@@ -288,12 +452,13 @@ def trial_groups(num_trials: int, num_chunks: int) -> List[slice]:
     return [slice(i, min(i + per, num_trials)) for i in range(0, num_trials, per)]
 
 
-def pack_references(references: Sequence[Annotation]):
+def pack_references(references: Sequence[Annotation], regions: Optional[Sequence] = None):
     """per-file references -> the reference arguments of dg_sweep_score_files: (rows float64 (S, 2), labels int32 (S,),
-    row offsets int32 (files + 1,), label counts int32 (files,)); each file's rows as ``reference_arrays`` gives them"""
+    row offsets int32 (files + 1,), label counts int32 (files,)); each file's rows as ``reference_arrays`` gives them, cropped
+    to the file's entry of ``regions`` when given"""
     rows, labels, offsets, counts = [], [], [0], []
-    for ref in references:
-        r, lab, names = reference_arrays(ref)
+    for f, ref in enumerate(references):
+        r, lab, names = reference_arrays(ref, None if regions is None else regions[f])
         rows.append(r)
         labels.append(lab)
         offsets.append(offsets[-1] + len(r))
@@ -502,6 +667,16 @@ def _timed(device: torch.device, call):
     return rc, seconds
 
 
+def _set_regions(setter, handle, regions: Optional[tuple]):
+    """``setter`` (dg_sweep_set_scored_regions / dg_vad_sweep_set_scored_regions): the handle's scored regions for its next
+    scoring calls, ``pack_regions``' (rows, offsets), or none (None: the hypotheses are scored whole)"""
+    if regions is None:
+        _lib.check(setter(handle, 0, None, None))
+    else:
+        rows, offsets = regions
+        _lib.check(setter(handle, len(offsets) - 1, rows.ctypes.data, offsets.ctypes.data))
+
+
 def _turn_list_call(owner, device: torch.device, guess: int, call) -> Tuple[int, float]:
     """Runs ``call(turns, capacity, n, cuda_stream)``, the last four arguments of an entry point that downloads a packed
     turn list, into ``owner._turns`` (uint32, grown to ``guess`` entries first) -> (turns written, device seconds of the
@@ -614,15 +789,16 @@ class HyperParameterSweep:
         return SweepOutputs(header, self._turns[:n_turns].copy(), n_turns, out_start, out_res, maps, centers, seconds)
 
     def _score_trials(self, entry, file_args: tuple, lead: tuple, seg: torch.Tensor, emb: torch.Tensor, plans,
-                      params: np.ndarray, shift, reference: tuple, segments: bool = False):
+                      params: np.ndarray, shift, reference: tuple, segments: bool = False, regions: Optional[tuple] = None):
         """The body of :meth:`sweep_score` and of each launch of :meth:`DatasetSweep.score` -> (components ``lead`` +
         (T, 5), device seconds, hypothesis offsets, hypothesis segments).  ``entry``: dg_sweep_score, or
         dg_sweep_score_files with ``file_args`` and ``lead`` as in :meth:`_run_trials`.  ``shift``: the timestamp shift, or
         the address of the per-file shifts.  ``reference``: the entry point's four reference arguments (rows, labels,
         then the row and label counts, or the addresses of the per-file row offsets and label counts).  ``segments`` is
-        for the one-file entry point."""
+        for the one-file entry point.  ``regions``: ``pack_regions`` of the files' scored regions, or None."""
         N, F, K = seg.shape
         h, _ = self._handle(F, K, emb.shape[2])
+        _set_regions(_lib.lib().dg_sweep_set_scored_regions, h, regions)
         plan, out_start, out_res = plans
         params = np.ascontiguousarray(params, dtype=np.float64)
         T, M = len(params), int(self.config.max_speakers)
@@ -648,17 +824,18 @@ class HyperParameterSweep:
         return self._run_trials(_lib.lib().dg_sweep_run, (), (), seg, emb, plans, params, keep_state)
 
     def sweep_score(self, seg: torch.Tensor, emb: torch.Tensor, fw: FileWindows, params: np.ndarray, ref_rows: np.ndarray,
-                    ref_labels: np.ndarray, num_ref_labels: int, segments: bool = False):
+                    ref_labels: np.ndarray, num_ref_labels: int, segments: bool = False, regions: Optional[tuple] = None):
         """dg_sweep_score over device scores / embeddings of ``fw``'s chunks for params (T, 3) against a reference in
         ``reference_arrays`` form -> (components (T, 5), device seconds, hypothesis offsets, hypothesis segments).  The last
         two are device tensors when ``segments`` (int32 (T * max_speakers + 1,) and float64 (n, 2), see the C header), else
-        None."""
+        None; the hypothesis segments are the uncropped predictions.  ``regions``: ``pack_regions([scored regions])`` to
+        crop the hypotheses to (the reference rows cropped alike), or None."""
         rows = np.ascontiguousarray(ref_rows, dtype=np.float64)
         labels = np.ascontiguousarray(ref_labels, dtype=np.int32)
         reference = (rows.ctypes.data, labels.ctypes.data, len(rows), int(num_ref_labels))
         plans = stream_plan(fw.starts, self.config, seg.shape[1])
         return self._score_trials(_lib.lib().dg_sweep_score, (), (), seg, emb, plans, params, -fw.padding[0], reference,
-                                  segments)
+                                  segments, regions)
 
     def _seg_resolution(self, start: float, F: int) -> float:
         return seg_resolution(self.config, start, F)
@@ -686,13 +863,22 @@ class HyperParameterSweep:
         self.timing = {"network": t1 - t0, "sweep": dev, "assembly": host}
         return out
 
-    def score(self, waveform: np.ndarray, reference: Annotation,
-              trials: Sequence[Mapping[str, float]] = ({},)) -> DERComponents:
+    def score(self, waveform: np.ndarray, reference: Annotation, trials: Sequence[Mapping[str, float]] = ({},),
+              metric=None, uem=None) -> DERComponents:
         """1-D float32 waveform at ``config.sample_rate`` and its reference annotation -> the diarization error rate
         components of every trial's whole-file prediction (the one :meth:`run` returns) against the reference.  One network
-        pass, one ``dg_sweep_score`` per 1024 trials; no annotation is built.  At most 32 reference labels."""
+        pass, one ``dg_sweep_score`` per 1024 trials; no annotation is built.  At most 32 reference labels.
+
+        ``metric``: a :class:`DiarizationErrorRate` (or pyannote.metrics' own) with a forgiveness collar and / or
+        ``skip_overlap``; None is ``DiarizationErrorRate()``.  ``uem``: the scored parts of the file, ``(start, end)`` pairs
+        or ``Segment``s in the reference's time base; None scores everything (DESIGN.md "DER scoring")."""
         params = trial_params(trials, self.config)
-        rows, labels, names = reference_arrays(reference)
+        collar, skip_overlap = metric_protocol(metric, "DiarizationErrorRate")
+        uem = check_uem(uem)
+        regions = None
+        if collar > 0 or skip_overlap or uem is not None:
+            regions = scored_regions(reference, collar, skip_overlap, uem)
+        rows, labels, names = reference_arrays(reference, regions)
         t0 = time.perf_counter()
         fw = file_windows(waveform, self.config)
         seg, emb = self.network_pass(fw)
@@ -700,19 +886,21 @@ class HyperParameterSweep:
         t1 = time.perf_counter()
         comps, dev = [], 0.0
         for i in range(0, len(params), TRIALS_PER_LAUNCH):
-            comp, secs, _, _ = self.sweep_score(seg, emb, fw, params[i:i + TRIALS_PER_LAUNCH], rows, labels, len(names))
+            comp, secs, _, _ = self.sweep_score(seg, emb, fw, params[i:i + TRIALS_PER_LAUNCH], rows, labels, len(names),
+                                                regions=None if regions is None else pack_regions([regions]))
             comps.append(comp)
             dev += secs
         self.timing = {"network": t1 - t0, "score": dev}
         return DERComponents.from_array(np.concatenate(comps))
 
-    def score_files(self, files: Iterable[Tuple[np.ndarray, Annotation]],
-                    trials: Sequence[Mapping[str, float]] = ({},)) -> Tuple[List[DERComponents], DERComponents]:
+    def score_files(self, files: Iterable[Tuple[np.ndarray, Annotation]], trials: Sequence[Mapping[str, float]] = ({},),
+                    metric=None) -> Tuple[List[DERComponents], DERComponents]:
         """``files``: (waveform, reference) pairs -> (components per file, their sum).  ``total.der`` per trial is the
         value the reference's ``Optimizer.objective`` minimises over a dataset (a fraction, not a percentage).  Runs as a
-        :class:`DatasetSweep` over the files."""
+        :class:`DatasetSweep` over the files.  ``metric`` as in :meth:`score`."""
+        metric_protocol(metric, "DiarizationErrorRate")        # a bad metric fails before the network pass
         dataset = DatasetSweep(self.config, [(None, waveform, reference) for waveform, reference in files], sweep=self)
-        out = dataset.score(trials)
+        out = dataset.score(trials, metric)
         self.timing = dict(dataset.timing)
         return out
 
@@ -723,17 +911,21 @@ class _DatasetSweep:
     packed references (``_pack_references``) and the loops of ``run`` and ``score`` over trial groups and files
     (``_score_group``, ``_components``)."""
 
-    _pack_references = None   # staticmethod of the subclass: references -> the reference arguments of its scoring entry
+    _pack_references = None   # staticmethod of the subclass: (references, regions) -> the reference arguments of its scoring entry
     _stream_form = True       # the network pass runs the sinc front end's stream form (LatencyUnits)
+    _metric = ""              # the class name of the metric the subclass scores (metric_protocol)
 
     def __init__(self, config, files: Iterable[Tuple[Optional[str], np.ndarray, Optional[Annotation]]],
-                 latencies: Optional[Iterable] = None):
+                 latencies: Optional[Iterable] = None, uems: Optional[Sequence] = None):
         files = list(files)
         if not files:
             raise ValueError("at least one file is needed")
         for i, (uri, x, _) in enumerate(files):
             if np.asarray(x).size == 0:
                 raise ValueError(f"file {i} ({uri}) has no samples, so no windows")
+        if uems is not None and (not isinstance(uems, (list, tuple)) or len(uems) != len(files)):
+            raise ValueError(f"uems: need one entry (a uem or None) per file, {len(files)} in all")
+        self.uems = [check_uem(u) for u in uems] if uems is not None else [None] * len(files)
         self.config = config
         self.uris = [uri for uri, _, _ in files]
         self.references = [ref for _, _, ref in files]
@@ -753,11 +945,10 @@ class _DatasetSweep:
         self._networks(fws)
         torch.cuda.synchronize(self.device)
         self.timing: Dict[str, float] = {"network": time.perf_counter() - t0}
-        self._refs = None
+        self._packs: Dict[tuple, tuple] = {}
         if self.units is not None:
             self.units.plan(self.seg.shape[1])
             self.plan = self.out_start = self.out_res = self.shifts = None
-            self._latency_refs: Dict[int, tuple] = {}
             self._virtual: Dict[tuple, tuple] = {}
             return
         self.plan, self.out_start, self.out_res = dataset_plan(fws, config, self.seg.shape[1])
@@ -772,14 +963,32 @@ class _DatasetSweep:
         ``self.seg`` (N, F, K)"""
         raise NotImplementedError
 
-    def _score_group(self, params: np.ndarray) -> Tuple[np.ndarray, float]:
-        """one scoring launch for one trial group against ``self._refs`` -> (components (files, T, width), device seconds)"""
+    def _score_group(self, params: np.ndarray, refs: tuple, regions: Optional[tuple]) -> Tuple[np.ndarray, float]:
+        """one scoring launch for one trial group against the packed references ``refs``, the hypotheses cropped to
+        ``regions`` (``pack_regions``, or None) -> (components (files, T, width), device seconds)"""
         raise NotImplementedError
 
-    def _components(self, f: int, comp: np.ndarray, refs: Optional[tuple] = None):
+    def _components(self, f: int, comp: np.ndarray, refs: tuple):
         """file f's components object from its (T, width) slice of the launches' components; ``refs``: the packed
-        references f indexes (default ``self._refs``; a virtual file's in the sweeps over several latencies)"""
+        references f indexes (a virtual file's in the sweeps over several latencies)"""
         raise NotImplementedError
+
+    def _packed(self, metric, copies: int = 1) -> Tuple[tuple, Optional[tuple]]:
+        """the packed references and scored regions (``pack_regions``, or None where nothing is cropped) of ``metric``
+        (:func:`metric_protocol`) with the files' uems, every file ``copies`` times (latency-major), kept per (copies,
+        collar, skip_overlap) for later calls.  ``regions_seconds``: host seconds spent packing (about 0 when kept)."""
+        protocol = metric_protocol(metric, self._metric)
+        self._check_references()
+        key = (copies, *protocol)
+        t0 = time.perf_counter()
+        if key not in self._packs:
+            regions = None
+            if protocol != (0.0, False) or any(u is not None for u in self.uems):
+                regions = [scored_regions(ref, *protocol, uem) for ref, uem in zip(self.references, self.uems)] * copies
+            self._packs[key] = (self._pack_references(self.references * copies, regions),
+                                None if regions is None else pack_regions(regions))
+        self.regions_seconds = time.perf_counter() - t0
+        return self._packs[key]
 
     @property
     def num_chunks(self) -> int:
@@ -801,19 +1010,17 @@ class _DatasetSweep:
         self.timing["sweep"] = dev
         return out
 
-    def _score(self, params: np.ndarray):
-        """-> (components per file, their sum in file order), one ``_score_group`` per trial group"""
-        self._check_references()
-        if self._refs is None:
-            self._refs = self._pack_references(self.references)
+    def _score(self, params: np.ndarray, metric=None):
+        """-> (components per file, their sum in file order) under ``metric``, one ``_score_group`` per trial group"""
+        refs, regions = self._packed(metric)
         parts, dev = [], 0.0
         for g in trial_groups(len(params), self.num_chunks):
-            part, secs = self._score_group(params[g])
+            part, secs = self._score_group(params[g], refs, regions)
             parts.append(part)
             dev += secs
         self.timing["score"] = dev
         comp = np.concatenate(parts, axis=1)
-        per_file = [self._components(f, comp[f]) for f in range(len(self.uris))]
+        per_file = [self._components(f, comp[f], refs) for f in range(len(self.uris))]
         return per_file, functools.reduce(operator.add, per_file)
 
     # ------------------------------------------------------------------ several latencies (built with ``latencies``)
@@ -877,19 +1084,17 @@ class _DatasetSweep:
         self.timing["sweep"] = dev
         return out
 
-    def _score_latencies(self, params: np.ndarray, sel: List[int], launch):
-        """``launch(params, tables, references)``: one scoring launch for the trials of one group -> (components (virtual
-        files, T, width), device seconds).  -> {latency: (components per file, their sum in file order)}"""
-        self._check_references()
+    def _score_latencies(self, params: np.ndarray, sel: List[int], launch, metric=None):
+        """``launch(params, tables, references, regions)``: one scoring launch for the trials of one group -> (components
+        (virtual files, T, width), device seconds).  -> {latency: (components per file, their sum in file order)} under
+        ``metric``"""
         run = self._launched(sel)
         tabs = self._tables(run)
         nf, n = len(self.uris), len(run)
-        if n not in self._latency_refs:                    # every file's reference once per latency, latency-major
-            self._latency_refs[n] = self._pack_references(self.references * n)
-        refs = self._latency_refs[n]
+        refs, regions = self._packed(metric, n)            # every file's reference and regions once per latency
         parts, dev = [], 0.0
         for g in trial_groups(len(params), self._group_chunks(tabs)):
-            part, secs = launch(params[g], tabs, refs)
+            part, secs = launch(params[g], tabs, refs, regions)
             parts.append(part)
             dev += secs
         self.timing["score"] = dev
@@ -939,14 +1144,21 @@ class DatasetSweep(_DatasetSweep):
     over every (latency, file) pair, in one launch per kernel and trial group whatever the number of latencies; for
     every latency L the results are the bits ``DatasetSweep`` built at latency L gives.  :meth:`score` / :meth:`run`
     return the ``config.latency`` entry.
+
+    ``uems``: per file its uem (``(start, end)`` pairs or ``Segment``s in the reference's time base) or None, for every
+    scoring call.  ``score`` and ``score_latencies`` take a ``metric`` (:class:`DiarizationErrorRate`, or
+    pyannote.metrics' own) with a forgiveness collar and / or ``skip_overlap``; the default is ``DiarizationErrorRate()``.
+    The packed references and scored regions are kept per metric.
     """
 
     _pack_references = staticmethod(pack_references)
+    _metric = "DiarizationErrorRate"
 
     def __init__(self, config: SpeakerDiarizationConfig, files: Iterable[Tuple[Optional[str], np.ndarray, Optional[Annotation]]],
-                 sweep: Optional[HyperParameterSweep] = None, latencies: Optional[Iterable] = None):
+                 sweep: Optional[HyperParameterSweep] = None, latencies: Optional[Iterable] = None,
+                 uems: Optional[Sequence] = None):
         self._sweep = sweep
-        super().__init__(config, files, latencies)
+        super().__init__(config, files, latencies, uems)
 
     def _open(self) -> torch.device:
         if self._sweep is None:
@@ -988,12 +1200,14 @@ class DatasetSweep(_DatasetSweep):
         labels = [f"speaker{g}" for g in range(int(self.config.max_speakers))]
         return self._run(trial_params(trials, self.config), self.sweep, labels)
 
-    def score(self, trials: Sequence[Mapping[str, float]] = ({},)) -> Tuple[List[DERComponents], DERComponents]:
+    def score(self, trials: Sequence[Mapping[str, float]] = ({},), metric=None) \
+            -> Tuple[List[DERComponents], DERComponents]:
         """-> (components per file, their sum in file order): per file what :meth:`HyperParameterSweep.score` returns for
-        it alone; ``total.der`` is the value ``Optimizer.objective`` minimises.  Every file needs a reference."""
+        it alone with the same ``metric`` and the file's uem; ``total.der`` is the value ``Optimizer.objective``
+        minimises.  Every file needs a reference."""
         if self.units is not None:
-            return self.score_latencies(trials, [self.config.latency])[float(self.config.latency)]
-        return self._score(trial_params(trials, self.config))
+            return self.score_latencies(trials, [self.config.latency], metric)[float(self.config.latency)]
+        return self._score(trial_params(trials, self.config), metric)
 
     def sweep_latencies(self, params: np.ndarray, latencies=None, keep_maps: bool = False) -> SweepOutputs:
         """dg_sweep_run_latencies over the resident outputs for params (T, 3) at the constructed ``latencies`` (None: all):
@@ -1013,16 +1227,16 @@ class DatasetSweep(_DatasetSweep):
         labels = [f"speaker{g}" for g in range(int(self.config.max_speakers))]
         return self._run_latencies(params, sel, self._sweep_virtual, labels)
 
-    def score_latencies(self, trials: Sequence[Mapping[str, float]] = ({},), latencies=None) \
+    def score_latencies(self, trials: Sequence[Mapping[str, float]] = ({},), latencies=None, metric=None) \
             -> Dict[float, Tuple[List[DERComponents], DERComponents]]:
         """-> {latency: (components per file, their sum)} for the constructed ``latencies`` (None: all): for each latency L
-        what :meth:`score` of a ``DatasetSweep`` built at L returns, bit for bit.  The clustering runs once per (unit,
-        trial) whatever the number of latencies; one launch per kernel and trial group (:func:`trial_groups` over the
-        virtual chunks)."""
+        what :meth:`score` of a ``DatasetSweep`` built at L returns with the same ``metric``, bit for bit.  The clustering
+        runs once per (unit, trial) whatever the number of latencies; one launch per kernel and trial group
+        (:func:`trial_groups` over the virtual chunks)."""
         params, sel = trial_params(trials, self.config), self._selection(latencies)
         if self.units is None:
-            return {self.latencies[0]: self.score(trials)}
-        return self._score_latencies(params, sel, self._score_virtual)
+            return {self.latencies[0]: self.score(trials, metric)}
+        return self._score_latencies(params, sel, self._score_virtual, metric)
 
     def _sweep_virtual(self, params: np.ndarray, tabs: tuple, keep_maps: bool = False) -> SweepOutputs:
         """one dg_sweep_run_latencies over the virtual layout ``tabs`` (``LatencyUnits.tables``)"""
@@ -1039,10 +1253,13 @@ class DatasetSweep(_DatasetSweep):
             _lib.ptr(maps), header.ctypes.data, *turn_list))
         return SweepOutputs(header, sw._turns[:n_turns].copy(), n_turns, out_start, out_res, maps, None, seconds)
 
-    def _score_virtual(self, params: np.ndarray, tabs: tuple, refs: tuple) -> Tuple[np.ndarray, float]:
-        """one dg_sweep_score_latencies over the virtual layout ``tabs`` against ``refs`` (one entry per virtual file)"""
+    def _score_virtual(self, params: np.ndarray, tabs: tuple, refs: tuple, regions: Optional[tuple]) \
+            -> Tuple[np.ndarray, float]:
+        """one dg_sweep_score_latencies over the virtual layout ``tabs`` against ``refs`` and ``regions`` (one entry per
+        virtual file)"""
         N, F, K = self.seg.shape
         h, _ = self._sweep._handle(F, K, self.emb.shape[2], self.units.nw)
+        _set_regions(_lib.lib().dg_sweep_set_scored_regions, h, regions)
         plan, out_start, out_res, shifts = tabs[2:]
         params = np.ascontiguousarray(params, dtype=np.float64)
         comp = np.empty((len(tabs[1]) - 1, len(params), 5), dtype=np.float64)
@@ -1053,12 +1270,12 @@ class DatasetSweep(_DatasetSweep):
         _lib.check(rc)
         return comp, seconds()
 
-    def _score_group(self, params: np.ndarray) -> Tuple[np.ndarray, float]:
-        reference = tuple(a.ctypes.data for a in self._refs)       # rows, labels, row offsets, label counts
+    def _score_group(self, params: np.ndarray, refs: tuple, regions: Optional[tuple]) -> Tuple[np.ndarray, float]:
+        reference = tuple(a.ctypes.data for a in refs)             # rows, labels, row offsets, label counts
         return self._sweep._score_trials(*self._over_files(_lib.lib().dg_sweep_score_files), params,
-                                         self.shifts.ctypes.data, reference)[:2]
+                                         self.shifts.ctypes.data, reference, regions=regions)[:2]
 
-    def _components(self, f: int, comp: np.ndarray, refs: Optional[tuple] = None) -> DERComponents:
+    def _components(self, f: int, comp: np.ndarray, refs: tuple) -> DERComponents:
         return DERComponents.from_array(comp)
 
 
@@ -1087,13 +1304,15 @@ class DetectionErrorComponents:
                                         self.missed_detection + other.missed_detection, self.total + other.total)
 
 
-def speech_reference(annotation: Annotation) -> Tuple[np.ndarray, float]:
+def speech_reference(annotation: Annotation, regions: Optional[Sequence[Tuple[float, float]]] = None) \
+        -> Tuple[np.ndarray, float]:
     """A reference annotation -> (rows float64 (S, 2), total): the support of all its segments, whatever their labels
     (``annotation.get_timeline().support()``): non-empty segments in (start, end) order, a segment merged into the current
     row when ``Segment(row end, its start)`` is falsy (it overlaps, touches or follows by at most 1e-6 s).  ``total`` is the
-    rows' durations summed in order, pyannote's ``reference.duration()``."""
+    rows' durations summed in order, pyannote's ``reference.duration()``.  With ``regions`` (:func:`scored_regions`) the
+    segments are first cropped to them (:func:`cropped_tracks`), so ``total`` is the cropped support's duration."""
     rows: List[List[float]] = []
-    for a, b in sorted((s.start, s.end) for s, _ in annotation.itertracks() if s):
+    for a, b in sorted((s, e) for s, e, _ in cropped_tracks(annotation, regions)):
         if rows and not (a - rows[-1][1] > 1e-6):
             rows[-1][1] = max(rows[-1][1], b)
         else:
@@ -1104,12 +1323,12 @@ def speech_reference(annotation: Annotation) -> Tuple[np.ndarray, float]:
     return np.array(rows, dtype=np.float64).reshape(-1, 2), total
 
 
-def pack_speech_references(references: Sequence[Annotation]):
+def pack_speech_references(references: Sequence[Annotation], regions: Optional[Sequence] = None):
     """per-file references -> the reference arguments of dg_vad_sweep_score_files and the per-file totals: (rows float64
-    (S, 2), row offsets int32 (files + 1,), totals float64 (files,))"""
+    (S, 2), row offsets int32 (files + 1,), totals float64 (files,)), cropped to each file's entry of ``regions`` when given"""
     rows, offsets, totals = [], [0], []
-    for ref in references:
-        r, total = speech_reference(ref)
+    for f, ref in enumerate(references):
+        r, total = speech_reference(ref, None if regions is None else regions[f])
         rows.append(r)
         offsets.append(offsets[-1] + len(r))
         totals.append(total)
@@ -1131,17 +1350,21 @@ class VoiceActivitySweep(_DatasetSweep):
     (``dg_vad_sweep_curve``: max over the local speakers, Hamming aggregation; 29 float64 per chunk at the defaults).
     :meth:`score` and :meth:`run` then threshold the curve for every (file, trial) pair in one launch per kernel and per
     trial group (:func:`trial_groups`), and run no network kernel.  The windows, plans and timestamp shifts are those of
-    :class:`DatasetSweep`.  Needs the native segmentation model (``B200PyanNet``).
+    :class:`DatasetSweep`.  Needs the native segmentation model (``B200PyanNet``).  ``uems`` and the ``metric`` of
+    :meth:`score` / :meth:`score_latencies` (a :class:`DetectionErrorRate`, or pyannote.metrics' own) as in
+    :class:`DatasetSweep`.
     """
 
     _pack_references = staticmethod(pack_speech_references)
     _stream_form = False      # forward_device passes no hop hint: the per-window form for every batch
+    _metric = "DetectionErrorRate"
 
     def __init__(self, config: VoiceActivityDetectionConfig,
-                 files: Iterable[Tuple[Optional[str], np.ndarray, Optional[Annotation]]], latencies: Optional[Iterable] = None):
+                 files: Iterable[Tuple[Optional[str], np.ndarray, Optional[Annotation]]], latencies: Optional[Iterable] = None,
+                 uems: Optional[Sequence] = None):
         self._h: Optional[C.c_void_p] = None
         self._turns = np.empty(0, dtype=np.uint32)
-        super().__init__(config, files, latencies)
+        super().__init__(config, files, latencies, uems)
         t1 = time.perf_counter()
         N, F, K = self.seg.shape
         if self.units is None:
@@ -1221,15 +1444,15 @@ class VoiceActivitySweep(_DatasetSweep):
                 p.modality = "speech"
         return out
 
-    def score(self, trials: Sequence[Mapping[str, float]] = ({},)) \
+    def score(self, trials: Sequence[Mapping[str, float]] = ({},), metric=None) \
             -> Tuple[List[DetectionErrorComponents], DetectionErrorComponents]:
         """-> (components per file, their sum in file order): the detection error rate components of :meth:`run`'s
-        predictions against each file's reference (``DetectionErrorRate(collar=0, skip_overlap=False)``, no uem); the
-        minimum of ``total.detection_error_rate`` is the trial ``Optimizer.objective`` would pick.  Every file needs a
-        reference."""
+        predictions against each file's reference under ``metric`` (default ``DetectionErrorRate(collar=0,
+        skip_overlap=False)``) within the file's uem (default: none); the minimum of ``total.detection_error_rate`` is the
+        trial ``Optimizer.objective`` would pick.  Every file needs a reference."""
         if self.units is not None:
-            return self.score_latencies(trials, [self.config.latency])[float(self.config.latency)]
-        return self._score(self._taus(trials))
+            return self.score_latencies(trials, [self.config.latency], metric)[float(self.config.latency)]
+        return self._score(self._taus(trials), metric)
 
     def run_latencies(self, trials: Sequence[Mapping[str, float]] = ({},), latencies=None) \
             -> Dict[float, List[List[Annotation]]]:
@@ -1246,15 +1469,16 @@ class VoiceActivitySweep(_DatasetSweep):
                     p.modality = "speech"
         return out
 
-    def score_latencies(self, trials: Sequence[Mapping[str, float]] = ({},), latencies=None) \
+    def score_latencies(self, trials: Sequence[Mapping[str, float]] = ({},), latencies=None, metric=None) \
             -> Dict[float, Tuple[List[DetectionErrorComponents], DetectionErrorComponents]]:
         """-> {latency: (components per file, their sum)} for the constructed ``latencies`` (None: all): for each latency L
-        what :meth:`score` of a ``VoiceActivitySweep`` built at L returns, bit for bit.  One launch per kernel and trial
-        group over every constructed latency."""
+        what :meth:`score` of a ``VoiceActivitySweep`` built at L returns with the same ``metric``, bit for bit.  One launch
+        per kernel and trial group over every constructed latency."""
         taus, sel = self._taus(trials), self._selection(latencies)
         if self.units is None:
-            return {self.latencies[0]: self.score(trials)}
-        return self._score_latencies(taus, sel, lambda t, tabs, refs: self._vad_score(t, *tabs[3:6], refs))
+            return {self.latencies[0]: self.score(trials, metric)}
+        return self._score_latencies(taus, sel, lambda t, tabs, refs, regions: self._vad_score(t, *tabs[3:6], refs, regions),
+                                     metric)
 
     def _launched(self, sel: List[int]) -> List[int]:
         return list(range(len(self.latencies)))       # the curve covers every constructed latency
@@ -1262,15 +1486,16 @@ class VoiceActivitySweep(_DatasetSweep):
     def _group_chunks(self, tabs: tuple) -> int:
         return len(tabs[0])                            # no clustering: header and turns over the virtual chunks
 
-    def _score_group(self, taus: np.ndarray) -> Tuple[np.ndarray, float]:
-        return self._vad_score(taus, self.out_start, self.out_res, self.shifts, self._refs)
+    def _score_group(self, taus: np.ndarray, refs: tuple, regions: Optional[tuple]) -> Tuple[np.ndarray, float]:
+        return self._vad_score(taus, self.out_start, self.out_res, self.shifts, refs, regions)
 
     def _vad_score(self, taus: np.ndarray, out_start: np.ndarray, out_res: np.ndarray, shifts: np.ndarray,
-                   refs: tuple) -> Tuple[np.ndarray, float]:
-        """one dg_vad_sweep_score_files against ``refs`` (``pack_speech_references`` of the curve's files) -> (components
-        (files, T, 2), device seconds)"""
+                   refs: tuple, regions: Optional[tuple] = None) -> Tuple[np.ndarray, float]:
+        """one dg_vad_sweep_score_files against ``refs`` (``pack_speech_references`` of the curve's files), the hypotheses
+        cropped to ``regions`` (or None) -> (components (files, T, 2), device seconds)"""
         rows, roff, _ = refs
         taus = np.ascontiguousarray(taus)
+        _set_regions(_lib.lib().dg_vad_sweep_set_scored_regions, self._h, regions)
         part = np.empty((len(roff) - 1, len(taus), 2), dtype=np.float64)
         rc, seconds = _timed(self.device, lambda st: _lib.lib().dg_vad_sweep_score_files(
             self._h, taus.ctypes.data, len(taus), out_start.ctypes.data, out_res.ctypes.data,
@@ -1278,7 +1503,7 @@ class VoiceActivitySweep(_DatasetSweep):
         _lib.check(rc)
         return part, seconds()
 
-    def _components(self, f: int, comp: np.ndarray, refs: Optional[tuple] = None) -> DetectionErrorComponents:
-        """false alarm and missed detection from the device; the total is the reference's duration, whatever the trial"""
-        refs = self._refs if refs is None else refs
+    def _components(self, f: int, comp: np.ndarray, refs: tuple) -> DetectionErrorComponents:
+        """false alarm and missed detection from the device; the total is the (cropped) reference's duration, whatever the
+        trial"""
         return DetectionErrorComponents(comp[:, 0].copy(), comp[:, 1].copy(), np.full(len(comp), refs[2][f]))

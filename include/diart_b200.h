@@ -230,9 +230,22 @@ int dg_sweep_run(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N,
                  const int32_t* plan_host, int32_t* maps_dev, double* centers_dev, int32_t* header_host, uint32_t* turns_host,
                  int turn_cap_host, int* n_turns, void* stream);
 int dg_sweep_destroy(dg_sweep* h);
+/* ---- dg_sweep_set_scored_regions / dg_vad_sweep_set_scored_regions: the scored regions of a metric with a forgiveness
+ *      collar, skip_overlap or a uem (DESIGN.md "DER scoring", steps 1-4) for the handle's later scoring calls.  File f's
+ *      pieces are rows_host float64 [S][2] {start, end} at [offsets_host[f], offsets_host[f + 1]) (int32 [num_files + 1] from
+ *      0, not decreasing): sorted, each more than 1e-6 s long and starting more than 1e-6 s after the previous one ends, all
+ *      finite; otherwise DG_EINVAL and the previous regions stay.  Every (file, trial) hypothesis is cropped to its file's
+ *      pieces before the scoring walk; the caller passes references already cropped to them.  num_files = 0 clears them (the
+ *      default: hypotheses scored whole).  While they are set, every dg_sweep_score* / dg_vad_sweep_score_files call must
+ *      score exactly num_files files (the virtual files of the _latencies entry points and of a curve over several
+ *      latencies), else DG_EINVAL before any launch.  Host only (the pieces travel with the next scoring call). ---- */
+int dg_sweep_set_scored_regions(dg_sweep* h, int num_files, const double* rows_host, const int32_t* offsets_host);
+int dg_vad_sweep_set_scored_regions(dg_vad_sweep* h, int num_files, const double* rows_host, const int32_t* offsets_host);
 /* ---- dg_sweep_score: the same clustering and post-path as dg_sweep_run, then each trial's diarization error rate components
- *      against one reference (DiarizationErrorRate(collar=0, skip_overlap=False), the metric of the reference's
- *      Benchmark.evaluate; definition in DESIGN.md "DER scoring").  The turns never leave the device.
+ *      against one reference (DiarizationErrorRate, the metric of the reference's Benchmark.evaluate; definition in
+ *      DESIGN.md "DER scoring"): collar=0, skip_overlap=False and no uem, or, with scored regions set
+ *      (dg_sweep_set_scored_regions), the hypothesis cropped to them and the reference as given (cropped by the caller).
+ *      The turns never leave the device.
  *        seg_dev ... plan_host   as dg_sweep_run;
  *        out_start_host, out_res_host float64 [N]: each chunk's output start and frame resolution (blocks/post.py post_plan),
  *        shift: added to every turn time (the file's timestamp shift), collar >= 0: the merge collar of the whole-file
@@ -320,7 +333,8 @@ int dg_sweep_check_latencies(int N, int num_units, const int32_t* unit_offsets_h
                              int num_windows, int frames);
 /* ---- voice activity detection sweep: the reference tunes VoiceActivityDetection's one hyper-parameter, tau_active, by
  *      running the whole pipeline per trial and file and scoring it with DetectionErrorRate(collar=0, skip_overlap=False)
- *      (reference blocks/vad.py:108-114, optim.py:98-122).  tau_active is read by Binarize alone, so here the speech curve of
+ *      (reference blocks/vad.py:108-114, optim.py:98-122); with scored regions set (dg_vad_sweep_set_scored_regions) any
+ *      collar, skip_overlap and uem.  tau_active is read by Binarize alone, so here the speech curve of
  *      every chunk (max over the local speakers, Hamming-aggregated as dg_post_step with one speaker) is computed once per
  *      dataset and kept on the device; each trial thresholds it.
  *      dg_vad_sweep_create: frames <= 1023, 1 <= local_speakers <= 64, 1 <= num_windows <= 256, hamming_host =
@@ -334,7 +348,7 @@ int dg_sweep_check_latencies(int N, int num_units, const int32_t* unit_offsets_h
  *        [T][N][4] and turns_host as dg_sweep_run_files (one speaker, 0).  Synchronous.
  *      dg_vad_sweep_score_files: out_start_host, out_res_host float64 [N], shifts_host float64 [num_files] and collar as
  *        dg_sweep_score_files; ref_host float64 [S][2]: each file's speech reference as one label, the support of all its
- *        segments (rows in time order, each more than 1e-6 s after the previous one), file f's at rows
+ *        segments (cropped to the file's scored regions when they are set; rows in time order, each more than 1e-6 s after the previous one), file f's at rows
  *        [ref_offsets_host[f], ref_offsets_host[f + 1]) (int32 [num_files + 1] from 0, not decreasing);
  *        components_host float64 [num_files][T][2] = {false alarm, missed detection} seconds.  The total (the reference's
  *        duration) does not depend on the trial and is the caller's.  Synchronous.
