@@ -77,6 +77,7 @@ SIGNATURES = {
     "dg_pipeline_submit_host": (C.c_int, [_P, _P, C.c_int, C.c_int]),
     "dg_pipeline_collect_host": (C.c_int, [_P, _P, _P, _P]),
     "dg_pipeline_destroy": (C.c_int, [_P]),
+    "dg_pipeline_nets_sets": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, C.c_int64, _P]),
     "dg_post_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_double, C.c_int, C.POINTER(_P)]),
     "dg_post_step": (C.c_int, [_P, _P, _P, C.c_int, _P, _P, _P, C.c_int, C.POINTER(C.c_int), _P]),
     "dg_post_reset": (C.c_int, [_P]),
@@ -101,6 +102,7 @@ SIGNATURES = {
     "dg_sweep_run": (C.c_int, [_P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, C.c_int, C.POINTER(C.c_int), _P]),
     "dg_sweep_destroy": (C.c_int, [_P]),
     "dg_sweep_set_scored_regions": (C.c_int, [_P, C.c_int, _P, _P]),
+    "dg_sweep_set_trial_sets": (C.c_int, [_P, C.c_int, _P, C.c_int]),
     "dg_sweep_score": (C.c_int, [_P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, C.c_double, C.c_double, _P, _P, C.c_int,
                                  C.c_int, _P, _P, _P, C.c_int, _P]),
     "dg_sweep_run_files": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, _P, _P, _P, _P, _P, C.c_int,

@@ -507,28 +507,35 @@ int emb_trunk(dg_emb* h, const float* wav, int U, const Geom& g, cudaStream_t st
   return 0;
 }
 
-// TDNN5 (Conv1d(512, 1500, 1) -> LeakyReLU -> BatchNorm) fused with the K weighted statistics poolings: the [rows, 1500] map
-// (455 MB at B = 256) is never written; the epilogue leaves per-tile partial sums, pool_finalize turns them into mean / std.
-static int emb_tdnn5_pool(dg_emb* h, int U, const Geom& g, const float* weights, int F, int K, int T, float eps,
-                          cudaStream_t st) {
+// TDNN5 (Conv1d(512, 1500, 1) -> LeakyReLU -> BatchNorm) fused with the K weighted statistics poolings over the row weights
+// `row_w` and weight sums `vsum` of launch_pool_weights: the [rows, 1500] map (455 MB at B = 256) is never written; the
+// epilogue leaves per-tile partial sums, pool_finalize turns them into mean / std.
+static int emb_tdnn5_pool_rows(dg_emb* h, int U, const Geom& g, const float* row_w, const float* vsum, int K, int T, float eps,
+                               cudaStream_t st) {
   int rc;
   const long long M = (long long)U * g.S2;
   const int m_tiles = (int)((M + 127) / 128);
-  if (h->pool_rw.ensure(((size_t)M + 128) * 16) || h->pool_vs.ensure((size_t)U * K * 8) ||
-      h->pool_part.ensure((size_t)m_tiles * 2 * 8 * 1500 * 4) || h->pooled.ensure((size_t)U * K * 3000 * 4))
-    return DG_ECUDA;
-  if ((rc = launch_pool_weights(weights, U, F, K, g.S2, T, h->idx0.as<int>(), h->idx1.as<int>(), h->lam1.as<float>(), eps,
-                                h->pool_rw.as<float>(), h->pool_vs.as<float>(), st)))
-    return rc;
+  if (h->pool_part.ensure((size_t)m_tiles * 2 * 8 * 1500 * 4) || h->pooled.ensure((size_t)U * K * 3000 * 4)) return DG_ECUDA;
   TcGemm t{};
   t.A_hi = h->t4h; t.A_lo = h->t4l; t.lda = 512; t.Cin = 512; t.KW = 1; t.dil = 1; t.Mtot = M; t.M = M;
   t.N = 1500; t.bias = h->tb[4].as<float>(); t.bn_scale = h->bns[4].as<float>(); t.bn_shift = h->bnh[4].as<float>();
   t.ldc = 1500; t.epi = 4; t.tag = "tdnn5";
-  t.pool_w = h->pool_rw.as<float>(); t.pool_part = h->pool_part.as<float>(); t.pool_item_rows = g.S2; t.pool_K = K;
+  t.pool_w = row_w; t.pool_part = h->pool_part.as<float>(); t.pool_item_rows = g.S2; t.pool_K = K;
   if ((rc = set_weights(t, h->tw[4])) || (rc = launch_gemm_tc(t, st))) return rc;
   h->pool_C = 1500;
-  return launch_pool_finalize(h->pool_part.as<float>(), h->pool_vs.as<float>(), h->bnh[4].as<float>(), U, K, 1500, g.S2, T, eps,
+  return launch_pool_finalize(h->pool_part.as<float>(), vsum, h->bnh[4].as<float>(), U, K, 1500, g.S2, T, eps,
                               h->pooled.as<float>(), st);
+}
+
+static int emb_tdnn5_pool(dg_emb* h, int U, const Geom& g, const float* weights, int F, int K, int T, float eps,
+                          cudaStream_t st) {
+  int rc;
+  const long long M = (long long)U * g.S2;
+  if (h->pool_rw.ensure(((size_t)M + 128) * 16) || h->pool_vs.ensure((size_t)U * K * 8)) return DG_ECUDA;
+  if ((rc = launch_pool_weights(weights, U, F, K, g.S2, T, h->idx0.as<int>(), h->idx1.as<int>(), h->lam1.as<float>(), eps,
+                                h->pool_rw.as<float>(), h->pool_vs.as<float>(), st)))
+    return rc;
+  return emb_tdnn5_pool_rows(h, U, g, h->pool_rw.as<float>(), h->pool_vs.as<float>(), K, T, eps, st);
 }
 
 static int emb_project(dg_emb* h, int rows, int normalize, float norm, float* out, cudaStream_t st) {
@@ -574,6 +581,35 @@ int emb_tail(dg_emb* h, int B, const Geom& g, const float* weights, int F, int K
                               h->lam1.as<float>(), eps, h->pooled.as<float>(), st, h->pool_item_pitch, h->pool_row_pitch)))
     return rc;
   return emb_project(h, B * K, normalize, norm, out, st);
+}
+
+// emb_tail for G OSP sets over one trunk pass: weights [G][B][F][K], set g's embeddings [B*K, D] at out + g out_stride.  The
+// fused form computes the row weights of all sets in one launch and then runs TDNN5 + pooling, the finaliser and the projection
+// once per set over the kept TDNN5 operand planes; the un-fused form runs emb_tail per set over the kept trunk map.  Either way
+// set g's embeddings are the bits emb_tail gives for weights g.
+int emb_tail_sets(dg_emb* h, int B, const Geom& g, const float* weights, int G, int F, int K, int T, bool fuse, float* out,
+                  int64_t out_stride, cudaStream_t st, int sm_cap) {
+  int rc;
+  const size_t wstride = (size_t)B * F * K;
+  if (!fuse) {
+    for (int s = 0; s < G; s++)
+      if ((rc = emb_tail(h, B, g, weights + s * wstride, F, K, T, false, 1, 1.f, out + s * out_stride, st))) return rc;
+    return 0;
+  }
+  if ((rc = build_tables(h, F, T, st))) return rc;
+  const float eps = pool_eps(h, weights);
+  const long long M = (long long)B * g.S2, rw_stride = (M + 128) * 4;
+  if (h->pool_rw.ensure((size_t)G * rw_stride * 4) || h->pool_vs.ensure((size_t)G * B * K * 8)) return DG_ECUDA;
+  SmLimit cap(sm_cap);
+  if ((rc = launch_pool_weights_sets(weights, B, G, F, K, g.S2, T, h->idx0.as<int>(), h->idx1.as<int>(), h->lam1.as<float>(), eps,
+                                     h->pool_rw.as<float>(), rw_stride, h->pool_vs.as<float>(), st)))
+    return rc;
+  for (int s = 0; s < G; s++)
+    if ((rc = emb_tdnn5_pool_rows(h, B, g, h->pool_rw.as<float>() + s * rw_stride, h->pool_vs.as<float>() + (size_t)s * B * K * 2,
+                                  K, T, eps, st)) ||
+        (rc = emb_project(h, B * K, 1, 1.f, out + s * out_stride, st)))
+      return rc;
+  return 0;
 }
 
 extern "C" int dg_emb_forward(dg_emb* h, const float* wav, const float* weights, int B, int S, int F, int K,

@@ -1,5 +1,6 @@
 // The fused pipeline (dg_pipeline_*): synchronous and submitted steps, the whole-call entry points and the shared-identity
 // exchange.
+#include <math.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -89,6 +90,7 @@ struct dg_pipeline : NetLanes {
   StepShape slot_shape[3];
   int outstanding = 0;
   long long next_step = 0;
+  long long nets_calls = 0;             // dg_pipeline_nets_sets calls: call n runs on scratch lane n & 1
   long long ident_merged_upto = 0;      // steps below this index have had their maps relabelled by a merge
   std::unique_ptr<GatherPool> gather;   // worker threads of the host gather (created at the first dg_pipeline_call_host)
   DevBuf call_stream;                   // device image of the stream a dg_pipeline_call_host batch was cut from
@@ -170,7 +172,7 @@ static int emb_sm_cap(int device, int B) {
 }
 
 int pipeline_nets(NetLanes* h, const float* wav, int S, const StepShape& sh, float* seg, float* emb, cudaEvent_t start,
-                  int lane, int stream_hop) {
+                  int lane, int stream_hop, const OspSets* sets, int G, int64_t emb_stride) {
   int rc;
   const int B = sh.B, F = sh.F, K = sh.K;
   const Geom g = make_geom(S);
@@ -178,7 +180,7 @@ int pipeline_nets(NetLanes* h, const float* wav, int S, const StepShape& sh, flo
   // alternate, so step i+1's segmentation chain can start while step i's is still in its recurrence)
   cudaStream_t s_seg = h->s_seg[lane];
   DevBuf& osp = h->osp[lane];
-  if (osp.ensure(sh.seg_bytes())) return DG_ECUDA;
+  if (osp.ensure(sh.seg_bytes() * (sets ? G : 1))) return DG_ECUDA;
   DG_CUDA(cudaStreamWaitEvent(s_seg, start, 0));
   DG_CUDA(cudaStreamWaitEvent(h->s_emb, start, 0));
   // another pipeline (or a block-level call) that used these model handles' scratch last: stream-ordered hand-over
@@ -200,14 +202,18 @@ int pipeline_nets(NetLanes* h, const float* wav, int S, const StepShape& sh, flo
   }
   DG_DIAG(trunk, h->s_emb);
   if ((rc = seg_forward_lane(h->seg, lane, &prep, wav, B, S, seg, s_seg))) return rc;
-  if ((rc = dg_osp(seg, B, F, K, h->gamma, h->beta, h->normalize_weights, osp.as<float>(), s_seg))) return rc;
+  if (sets) rc = launch_osp_sets(seg, B, F, K, *sets, G, osp.as<float>(), s_seg);
+  else rc = dg_osp(seg, B, F, K, h->gamma, h->beta, h->normalize_weights, osp.as<float>(), s_seg);
+  if (rc) return rc;
   DG_CUDA(cudaEventRecord(h->e_osp[lane], s_seg));
   if ((rc = seg_use.end())) return rc;
   DG_DIAG(seg, s_seg);
   DG_CUDA(cudaStreamWaitEvent(h->s_emb, h->e_osp[lane], 0));
   // a fused TDNN5 needs the pooling weights: it runs here, after the segmentation of this step, with its grid capped like the
   // trunk's (the other lane's recurrence may hold lstm_tc_ctas(B) SMs at this point)
-  if ((rc = emb_tail(h->emb, B, g, osp.as<float>(), F, K, T, fuse, 1, 1.f, emb, h->s_emb, sm_cap))) return rc;
+  if (sets) rc = emb_tail_sets(h->emb, B, g, osp.as<float>(), G, F, K, T, fuse, emb, emb_stride, h->s_emb, sm_cap);
+  else rc = emb_tail(h->emb, B, g, osp.as<float>(), F, K, T, fuse, 1, 1.f, emb, h->s_emb, sm_cap);
+  if (rc) return rc;
   DG_CUDA(cudaEventRecord(h->e_emb, h->s_emb));
   DG_DIAG(emb, h->s_emb);
   return emb_use.end();
@@ -726,6 +732,54 @@ extern "C" int dg_pipeline_call_stream(dg_pipeline* h, dg_post* post, dg_stream*
   const StepOut dev = {h->segd.as<float>(), h->embd.as<float>(), h->mapd.as<int32_t>(), nullptr};
   if ((rc = pipeline_step(h, h->wav.as<float>(), S, sh, dev, h->st, s->rs ? 0 : s->hop))) return rc;
   return call_finish(h, post, sh, plan_host, header_host, turns_host, turn_cap_host, n_turns, seg_host, map_host, nullptr);
+}
+
+// The networks of one batch without clustering, for G OSP sets: scores [B, F, K] to seg_dev and set g's embeddings [B, K, D] to
+// emb_dev + g emb_set_stride.  Consecutive calls alternate the two scratch lanes like submitted steps, so the segmentation of
+// call n + 1 overlaps the embedding tail of call n; `stream` waits for this call's outputs.  The sinc front end takes the form
+// the hop hint (dg_pipeline_set_hop) selects, as in dg_pipeline_submit.
+extern "C" int dg_pipeline_nets_sets(dg_pipeline* h, const float* wav_dev, int B, int S, int num_sets, const float* osp_host,
+                                     const int32_t* normalize_host, float* seg_dev, float* emb_dev, int64_t emb_set_stride,
+                                     void* stream) {
+  const char* who = "dg_pipeline_nets_sets";
+  if (!h || !wav_dev || !seg_dev || !emb_dev || !osp_host || !normalize_host || B < 1 || num_sets < 1 ||
+      num_sets > DG_MAX_OSP_SETS) {
+    set_error(std::string(who) + ": bad arguments (need B >= 1, 1 <= num_sets <= 64, non-null buffers)");
+    return DG_EINVAL;
+  }
+  OspSets sets{};
+  for (int g = 0; g < num_sets; g++) {
+    sets.gamma[g] = osp_host[2 * g];
+    sets.beta[g] = osp_host[2 * g + 1];
+    sets.normalize[g] = normalize_host[g];
+    if (!std::isfinite(sets.gamma[g]) || !std::isfinite(sets.beta[g]) || (unsigned)sets.normalize[g] > 1u) {
+      set_error(std::string(who) + ": set " + std::to_string(g) + " needs finite gamma and beta and normalize 0 or 1");
+      return DG_EINVAL;
+    }
+  }
+  int rc, F = 0, K = 0;
+  if ((rc = dg_seg_dims(h->seg, S, &F, &K))) return rc;
+  const int64_t per_set = (int64_t)B * K * h->emb->D;
+  if (num_sets > 1 && emb_set_stride < per_set) {
+    set_error(std::string(who) + ": emb_set_stride " + std::to_string(emb_set_stride) + " is below one set's B K D = " +
+              std::to_string(per_set));
+    return DG_EINVAL;
+  }
+  if (h->outstanding) {
+    set_error(std::string(who) + ": submitted steps are outstanding; collect them first");
+    return DG_EINVAL;
+  }
+  DG_CUDA(cudaSetDevice(h->seg->device));
+  const int lane = (int)(h->nets_calls & 1);
+  DG_CUDA(cudaEventRecord(h->e_start, (cudaStream_t)stream));
+  // the lane's previous user must be past its embeddings before its scratch is rewritten
+  for (cudaStream_t s : {(cudaStream_t)h->s_seg[lane], (cudaStream_t)h->s_emb}) DG_CUDA(cudaStreamWaitEvent(s, h->e_lane_done[lane], 0));
+  if ((rc = pipeline_nets(h, wav_dev, S, {B, F, K}, seg_dev, emb_dev, h->e_start, lane, 0, &sets, num_sets, emb_set_stride)))
+    return rc;
+  DG_CUDA(cudaEventRecord(h->e_lane_done[lane], h->s_emb));
+  DG_CUDA(cudaStreamWaitEvent((cudaStream_t)stream, h->e_lane_done[lane], 0));
+  h->nets_calls++;
+  return DG_OK;
 }
 
 extern "C" int dg_pipeline_destroy(dg_pipeline* h) {

@@ -209,6 +209,8 @@ struct dg_sweep {
   DevBuf hamming, in, centers, active, init, prep, prep_d, maps, header, turns, total;
   DerBufs der;                    // dg_sweep_score
   ScoredRegions regions;          // dg_sweep_set_scored_regions
+  int num_sets = 0;               // dg_sweep_set_trial_sets: > 0: emb is [num_sets][N][K][D], trial t reads set trial_set[t]
+  std::vector<int32_t> trial_set;
   PinnedBuf pin;                  // params, taus and plan in; error flags, header, total and a turn prefix out
 };
 
@@ -237,6 +239,28 @@ extern "C" int dg_sweep_destroy(dg_sweep* h) {
 extern "C" int dg_sweep_set_scored_regions(dg_sweep* h, int num_files, const double* rows_host,
                                            const int32_t* offsets_host) {
   return set_scored_regions("dg_sweep_set_scored_regions", h ? &h->regions : nullptr, num_files, rows_host, offsets_host);
+}
+
+extern "C" int dg_sweep_set_trial_sets(dg_sweep* h, int num_sets, const int32_t* trial_set_host, int T) {
+  const char* who = "dg_sweep_set_trial_sets";
+  if (num_sets < 0 || num_sets > DG_MAX_OSP_SETS || (num_sets > 0 && (!trial_set_host || T < 1 || T > 65535))) {
+    set_error(std::string(who) + ": bad arguments (need 0 <= num_sets <= 64, and 1 <= T <= 65535 trial sets when num_sets > 0)");
+    return DG_EINVAL;
+  }
+  for (int t = 0; num_sets > 0 && t < T; t++)
+    if (trial_set_host[t] < 0 || trial_set_host[t] >= num_sets) {
+      set_error(std::string(who) + ": trial " + std::to_string(t) + " has set " + std::to_string(trial_set_host[t]) +
+                ", outside [0, " + std::to_string(num_sets) + ")");
+      return DG_EINVAL;
+    }
+  if (!h) {
+    set_error(std::string(who) + ": null handle");
+    return DG_EINVAL;
+  }
+  h->num_sets = num_sets;
+  if (num_sets > 0) h->trial_set.assign(trial_set_host, trial_set_host + T);
+  else h->trial_set.clear();
+  return DG_OK;
 }
 
 // at most this many (file, trial) states per call: der_hyp runs one warp per (state, label) with up to 32 labels and
@@ -268,6 +292,11 @@ static int sweep_check(const char* who, dg_sweep* h, const float* seg_dev, const
   if ((long long)nf * T > DG_SWEEP_MAX_STATES) {
     set_error(std::string(who) + ": " + std::to_string((long long)nf * T) + " (file, trial) states; at most " +
               std::to_string(DG_SWEEP_MAX_STATES) + " per call");
+    return DG_EINVAL;
+  }
+  if (h->num_sets > 0 && (int)h->trial_set.size() != T) {
+    set_error(std::string(who) + ": trial sets are set for " + std::to_string(h->trial_set.size()) + " trials, the call runs " +
+              std::to_string(T) + " (set them again, or clear them with num_sets = 0)");
     return DG_EINVAL;
   }
   int rc;
@@ -340,9 +369,11 @@ static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* em
   // state s = f T + t owns centroid table, active flags and error pair s (cluster.cu), so those are sized for all nf T states
   // whichever of them run; the launch runs S_run
   const int stride = 4 + h->nw, M = h->M, D = h->D, K = h->K, F = h->F, S = nf * T, S_run = (int)(states.size() / 2);
-  // host -> device, one copy: params [T][3], taus [T], states [S_run][2] (launch order), plan [Nv][stride], chunk offsets
+  // with trial sets (dg_sweep_set_trial_sets) a trial row is {tau, rho, delta, set}, and the prep rows are per set
+  const int G = h->num_sets, PS = G > 0 ? 4 : 3;
+  // host -> device, one copy: params [T][PS], taus [T], states [S_run][2] (launch order), plan [Nv][stride], chunk offsets
   // [nf + 1], then with vchunk_host the virtual chunk table [Nv]
-  const size_t params_b = (size_t)T * 24, taus_b = (size_t)T * 8, states_b = (size_t)S_run * 8, plan_b = (size_t)Nv * stride * 4;
+  const size_t params_b = (size_t)T * PS * 8, taus_b = (size_t)T * 8, states_b = (size_t)S_run * 8, plan_b = (size_t)Nv * stride * 4;
   const size_t off_b = (size_t)(nf + 1) * 4, vchunk_b = vchunk_host ? (size_t)Nv * 4 : 0;
   const size_t in_b = params_b + taus_b + states_b + plan_b + off_b + vchunk_b;
   const TurnOut lay = sweep_out(S, T, Nv);
@@ -350,13 +381,21 @@ static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* em
   // the device turn buffer starts at a guess and grows to the true count (the kernel counts every turn, writes those that fit)
   const size_t turn_guess = std::max<size_t>((size_t)T * Nv * 8, (size_t)DG_POST_PREFIX);
   if (h->in.ensure(in_b) || h->centers.ensure((size_t)S * M * D * 8) || h->active.ensure((size_t)S * 32 * 4) ||
-      h->init.ensure(init_b) || h->prep.ensure(cluster_prep_floats(N, K) * 4 + 16) ||
-      h->prep_d.ensure(cluster_prep_doubles(N, K) * 8 + 16) || (!maps_dev && h->maps.ensure((size_t)T * N * K * 4)) ||
+      h->init.ensure(init_b) || h->prep.ensure(cluster_prep_floats(N, K) * 4 * std::max(G, 1) + 16) ||
+      h->prep_d.ensure(cluster_prep_doubles(N, K) * 8 * std::max(G, 1) + 16) || (!maps_dev && h->maps.ensure((size_t)T * N * K * 4)) ||
       h->header.ensure(header_b) || h->turns.ensure(turn_guess * 4) || h->pin.ensure(std::max(in_b, lay.end())))
     return DG_ECUDA;
   unsigned char* pin = h->pin.as<unsigned char>();
   double* p_taus = reinterpret_cast<double*>(pin + params_b);
-  memcpy(pin, params_host, params_b);
+  if (G > 0) {
+    double* rows = reinterpret_cast<double*>(pin);
+    for (int t = 0; t < T; t++) {
+      for (int j = 0; j < 3; j++) rows[4 * t + j] = params_host[3 * t + j];
+      rows[4 * t + 3] = (double)h->trial_set[t];
+    }
+  } else {
+    memcpy(pin, params_host, params_b);
+  }
   for (int t = 0; t < T; t++) p_taus[t] = params_host[3 * t];
   memcpy(pin + params_b + taus_b, states.data(), states_b);
   memcpy(pin + params_b + taus_b + states_b, plan_host, plan_b);
@@ -379,10 +418,13 @@ static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* em
   p.D = D;
   p.metric = 0;
   int rc;
-  if ((rc = launch_cluster_sweep(p, d_params, T, d_states, S_run, d_off, seg_dev, emb_dev, N, F, K, h->centers.as<double>(),
-                                 h->active.as<int>(), h->init.as<int>(), h->prep.as<float>(), h->prep_d.as<double>(), maps,
-                                 st)))
-    return rc;
+  if (G > 0)
+    rc = launch_cluster_sweep_sets(p, d_params, T, d_states, S_run, d_off, seg_dev, emb_dev, G, N, F, K, h->centers.as<double>(),
+                                   h->active.as<int>(), h->init.as<int>(), h->prep.as<float>(), h->prep_d.as<double>(), maps, st);
+  else
+    rc = launch_cluster_sweep(p, d_params, T, d_states, S_run, d_off, seg_dev, emb_dev, N, F, K, h->centers.as<double>(),
+                              h->active.as<int>(), h->init.as<int>(), h->prep.as<float>(), h->prep_d.as<double>(), maps, st);
+  if (rc) return rc;
   if (centers_dev)
     DG_CUDA(cudaMemcpyAsync(centers_dev, h->centers.p, (size_t)S * M * D * 8, cudaMemcpyDeviceToDevice, st));
   unsigned int total = 0;

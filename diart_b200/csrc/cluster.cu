@@ -34,11 +34,11 @@ size_t cluster_prep_floats(int B, int K) { return (size_t)B * K * 3; }     // ma
 size_t cluster_prep_doubles(int B, int K) { return (size_t)B * K; }        // ||e||
 
 // numpy semantics: np.max / np.mean over axis 0 of a float32 (F,K) array.  The mean is a float32
-// running sum in frame order followed by one float32 division (clustering.py:137-142).
-__global__ void __launch_bounds__(128) cluster_prep_kernel(const float* __restrict__ seg, const float* __restrict__ emb,
-                                                           int F, int K, int D, float* __restrict__ prep,
-                                                           double* __restrict__ prep_d) {
-  const int i = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+// running sum in frame order followed by one float32 division (clustering.py:137-142).  Chunk i; shared by cluster_prep_kernel
+// and cluster_prep_sets_kernel.
+__device__ __forceinline__ void cluster_prep_chunk(const float* __restrict__ seg, const float* __restrict__ emb, int i, int F,
+                                                   int K, int D, float* __restrict__ prep, double* __restrict__ prep_d) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const float* s = seg + (size_t)i * F * K;
   if (threadIdx.x < K) {
     float mx = -INFINITY, sum = 0.f;
@@ -68,6 +68,21 @@ __global__ void __launch_bounds__(128) cluster_prep_kernel(const float* __restri
       prep_d[(size_t)i * K + k] = sqrt(ss);
     }
   }
+}
+
+__global__ void __launch_bounds__(128) cluster_prep_kernel(const float* __restrict__ seg, const float* __restrict__ emb,
+                                                           int F, int K, int D, float* __restrict__ prep,
+                                                           double* __restrict__ prep_d) {
+  cluster_prep_chunk(seg, emb, blockIdx.x, F, K, D, prep, prep_d);
+}
+
+// one CTA per (chunk, set) over the embeddings of G sets [G][B][K][D]: set g's rows at prep + g B K 3 and prep_d + g B K (the
+// score statistics are the same in every set)
+__global__ void __launch_bounds__(128) cluster_prep_sets_kernel(const float* __restrict__ seg, const float* __restrict__ emb,
+                                                                int F, int K, int D, float* __restrict__ prep,
+                                                                double* __restrict__ prep_d) {
+  const size_t g = blockIdx.y, B = gridDim.x;
+  cluster_prep_chunk(seg, emb + g * B * K * D, blockIdx.x, F, K, D, prep + g * B * K * 3, prep_d + g * B * K);
 }
 
 __device__ __forceinline__ void put(double (&c)[CK], int i, double v) {
@@ -113,8 +128,10 @@ constexpr int SWEEP_THREADS = 256;      // many independent states (hyper-parame
 // and writes the map rows of its chunks in trial t's block ([B][K] at map_out + t B K).  Outputs are addressed by (f, t),
 // so the launch order (the order of `states`) changes no result.  OWN_ROWS (STATES only; many live streams, each at its own
 // thresholds, dg_multi): t is only the row of `trials`, state s = f, and every state's maps go to block 0.  The arithmetic
-// does not depend on THREADS: each centroid's distances are one warp's, the updates are element-wise.
-template <int THREADS, bool STATES, bool OWN_ROWS = false>
+// does not depend on THREADS: each centroid's distances are one warp's, the updates are element-wise.  SETS (STATES only; sweeps
+// over OSP sets): a trial row is {tau, rho, delta, set} and the state reads the embeddings and prep rows of that set, emb
+// [G][B][K][D], prep [G][B][K][3], prep_d [G][B][K] (64-bit offsets: G B K D exceeds 2^31 on large datasets).
+template <int THREADS, bool STATES, bool OWN_ROWS = false, bool SETS = false>
 __global__ void __launch_bounds__(THREADS)
 cluster_seq_kernel(ClusterParams p, const double* __restrict__ trials, const int2* __restrict__ states,
                    const int* __restrict__ chunk_off, int T, const float* __restrict__ seg,
@@ -136,6 +153,13 @@ cluster_seq_kernel(ClusterParams p, const double* __restrict__ trials, const int
   if constexpr (STATES) {
     const int2 fs = states[blockIdx.x];
     const int trial = fs.y, c0 = chunk_off[fs.x];
+    constexpr int PS = SETS ? 4 : 3;                     // doubles per trial row
+    if constexpr (SETS) {
+      const size_t set = (size_t)trials[trial * PS + 3], n = (size_t)B * K;   // B: all chunks of the launch here
+      emb += set * n * p.D;
+      prep += set * n * 3;
+      prep_d += set * n;
+    }
     const size_t s = OWN_ROWS ? (size_t)fs.x : (size_t)fs.x * T + trial;
     centers += s * M * D;
     g_active += s * CM;
@@ -144,9 +168,9 @@ cluster_seq_kernel(ClusterParams p, const double* __restrict__ trials, const int
     B = chunk_off[fs.x + 1] - c0;              // from here on: this file's chunks, the first at c0
     first = c0;
     // numpy compares the float32 scores with a Python float in float32 (as dg_cluster_create)
-    tau_f = (float)trials[trial * 3 + 0];
-    rho_f = (float)trials[trial * 3 + 1];
-    delta = trials[trial * 3 + 2];
+    tau_f = (float)trials[trial * PS + 0];
+    rho_f = (float)trials[trial * PS + 1];
+    delta = trials[trial * PS + 2];
   }
   double* cs = reinterpret_cast<double*>(dyn);                 // centroids [M][D], resident for the whole batch
   double* ed = cs + (size_t)M * D;                             // the current chunk's embeddings as float64 [K][D] (converted once
@@ -431,11 +455,11 @@ static int check_cluster_shape(const char* who, const ClusterParams& p, int K) {
   return 0;
 }
 
-template <int THREADS, bool STATES, bool OWN_ROWS = false>
+template <int THREADS, bool STATES, bool OWN_ROWS = false, bool SETS = false>
 static int cluster_seq_allow_dyn() {   // per device: the opt-in above 48 KB is a property of (function, device)
   static bool attr_done[64] = {};
   if (first_use_on_device(attr_done))
-    DG_CUDA(cudaFuncSetAttribute(cluster_seq_kernel<THREADS, STATES, OWN_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    DG_CUDA(cudaFuncSetAttribute(cluster_seq_kernel<THREADS, STATES, OWN_ROWS, SETS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  200 * 1024));
   return 0;
 }
@@ -503,6 +527,24 @@ int launch_cluster_sweep(const ClusterParams& p, const double* trials_dev, int T
         p, trials_dev, states_dev, chunk_off_dev, T, seg, emb, B, F, K, centers, active, initialized, prep, prep_d, maps,
         nullptr, nullptr);
   }
+  DG_LAUNCHED();
+  return 0;
+}
+
+int launch_cluster_sweep_sets(const ClusterParams& p, const double* trials_dev, int T, const int2* states_dev, int S,
+                              const int* chunk_off_dev, const float* seg, const float* emb, int G, int B, int F, int K,
+                              double* centers, int* active, int* initialized, float* prep, double* prep_d, int32_t* maps,
+                              cudaStream_t st) {
+  ProfScope _ps("cluster_sweep", st);
+  if (check_cluster_shape("cluster_sweep", p, K)) return -1;
+  if (B <= 0 || S <= 0) return 0;
+  cluster_prep_sets_kernel<<<dim3(B, G), 128, 0, st>>>(seg, emb, F, K, p.D, prep, prep_d);
+  DG_LAUNCHED();
+  const size_t dyn = cluster_seq_dyn(p.M, p.D, K);
+  if (int rc = cluster_seq_allow_dyn<SWEEP_THREADS, true, false, true>()) return rc;
+  cluster_seq_kernel<SWEEP_THREADS, true, false, true><<<S, SWEEP_THREADS, dyn, st>>>(
+      p, trials_dev, states_dev, chunk_off_dev, T, seg, emb, B, F, K, centers, active, initialized, prep, prep_d, maps,
+      nullptr, nullptr);
   DG_LAUNCHED();
   return 0;
 }

@@ -225,12 +225,23 @@ int launch_seg_powerset(const float* y, const float* wc, const float* bc, int B,
                         const unsigned* masks_dev, float* seg /*[B,T,num_speakers]*/, cudaStream_t st);
 int launch_osp(const float* seg, int B, int F, int K, float gamma, float beta, int normalize, float* out,
                cudaStream_t st);
+// OSP sets (sweeps over overlap-aware weightings): set g = {gamma[g], beta[g], normalize[g]}, passed by value
+constexpr int DG_MAX_OSP_SETS = 64;
+struct OspSets {
+  float gamma[DG_MAX_OSP_SETS], beta[DG_MAX_OSP_SETS];
+  int normalize[DG_MAX_OSP_SETS];
+};
+// one launch over (item, set): set g's weights [B,F,K] at out + g B F K, the bits launch_osp gives at that set
+int launch_osp_sets(const float* seg, int B, int F, int K, const OspSets& sets, int G, float* out, cudaStream_t st);
 int launch_stats_pool(const float* x /*[B*stride,C]*/, int B, int stride, int T, int C, const float* w /*[B,F,K]*/,
                       int F, int K, const int* idx0, const int* idx1, const float* lam1, float eps,
                       float* pooled /*[B*K, 2C]*/, cudaStream_t st, long long item_pitch = 0, int row_pitch = 0);
 // fused pooling (epi 4 of gemm_tc): row weights + their sums, and the final mean / std from the per-tile partial sums
 int launch_pool_weights(const float* w /*[B,F,K]*/, int B, int F, int K, int item_rows, int T, const int* idx0, const int* idx1,
                         const float* lam1, float eps, float* row_w /*[B*item_rows][4]*/, float* vsum /*[B*K][2]*/, cudaStream_t st);
+// launch_pool_weights for G sets in one launch: set g reads w + g B F K, writes row_w + g rw_stride and vsum + g B K 2
+int launch_pool_weights_sets(const float* w, int B, int G, int F, int K, int item_rows, int T, const int* idx0, const int* idx1,
+                             const float* lam1, float eps, float* row_w, long long rw_stride, float* vsum, cudaStream_t st);
 int launch_pool_finalize(const float* part, const float* vsum, const float* pivot, int B, int K, int C, int item_rows, int T,
                          float eps, float* pooled /*[B*K][2C]*/, cudaStream_t st);
 int launch_l2norm(const float* in, int rows, int D, float norm, float* out, cudaStream_t st);
@@ -268,6 +279,13 @@ int launch_cluster_sweep(const ClusterParams& p, const double* trials_dev, int T
                          const int* chunk_off_dev, const float* seg, const float* emb, int B, int F, int K, double* centers,
                          int* active, int* initialized, float* prep, double* prep_d, int32_t* maps, cudaStream_t st,
                          bool own_rows = false);
+// launch_cluster_sweep over the embeddings of G OSP sets, emb [G][B][K][D]: the prep pass runs over (chunk, set) into prep
+// [G][B][K][3] / prep_d [G][B][K], and a state of trial t reads the embeddings and prep rows of set (int)trials_dev[t * 4 + 3]
+// (trials_dev [T][4] = {tau, rho, delta, set})
+int launch_cluster_sweep_sets(const ClusterParams& p, const double* trials_dev, int T, const int2* states_dev, int S,
+                              const int* chunk_off_dev, const float* seg, const float* emb, int G, int B, int F, int K,
+                              double* centers, int* active, int* initialized, float* prep, double* prep_d, int32_t* maps,
+                              cudaStream_t st);
 size_t cluster_prep_floats(int B, int K);
 // post.cu -- aggregation + binarisation + run-length turns (reference diarization.py:205-232)
 int launch_post(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map, int n_hist, int B,

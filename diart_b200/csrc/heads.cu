@@ -109,12 +109,10 @@ __device__ __forceinline__ float pow_like_torch(float x, float g) {
   return powf(x, g);
 }
 
-// one CTA per item; weights for all frames staged in shared memory so the optional min-max
-// normalisation over frames (embedding.py:102-106) needs no second launch.
-__global__ void __launch_bounds__(256) osp_kernel(const float* __restrict__ seg, int F, int K, float gamma, float beta,
-                                                  int normalize, float* __restrict__ out) {
-  extern __shared__ float sw[];   // [F*K] (+ 2*K min/max)
-  const int b = blockIdx.x;
+// Item b of an OSP launch: weights for all frames staged in shared memory so the optional min-max normalisation over frames
+// (embedding.py:102-106) needs no second launch.  Shared by osp_kernel and osp_sets_kernel.
+__device__ __forceinline__ void osp_item(const float* __restrict__ seg, int b, int F, int K, float gamma, float beta,
+                                         int normalize, float* __restrict__ out, float* sw) {
   const float* s = seg + (size_t)b * F * K;
   for (int f = threadIdx.x; f < F; f += blockDim.x) {
     float mx = -INFINITY;
@@ -155,6 +153,21 @@ __global__ void __launch_bounds__(256) osp_kernel(const float* __restrict__ seg,
   }
 }
 
+// one CTA per item
+__global__ void __launch_bounds__(256) osp_kernel(const float* __restrict__ seg, int F, int K, float gamma, float beta,
+                                                  int normalize, float* __restrict__ out) {
+  extern __shared__ float sw[];   // [F*K] (+ 2*K min/max)
+  osp_item(seg, blockIdx.x, F, K, gamma, beta, normalize, out, sw);
+}
+
+// one CTA per (item, set): set g's weights of item b go to out + g B F K, from that set's gamma, beta and normalize
+__global__ void __launch_bounds__(256) osp_sets_kernel(const float* __restrict__ seg, int F, int K, OspSets sets,
+                                                       float* __restrict__ out) {
+  extern __shared__ float sw[];   // [F*K] (+ 2*K min/max)
+  const int g = blockIdx.y;
+  osp_item(seg, blockIdx.x, F, K, sets.gamma[g], sets.beta[g], sets.normalize[g], out + (size_t)g * gridDim.x * F * K, sw);
+}
+
 int launch_osp(const float* seg, int B, int F, int K, float gamma, float beta, int normalize, float* out,
                cudaStream_t st) {
   ProfScope _ps("osp", st);
@@ -164,6 +177,18 @@ int launch_osp(const float* seg, int B, int F, int K, float gamma, float beta, i
     return -1;
   }
   osp_kernel<<<B, 256, smem, st>>>(seg, F, K, gamma, beta, normalize, out);
+  DG_LAUNCHED();
+  return 0;
+}
+
+int launch_osp_sets(const float* seg, int B, int F, int K, const OspSets& sets, int G, float* out, cudaStream_t st) {
+  ProfScope _ps("osp", st);
+  const size_t smem = ((size_t)F * K + 2 * K) * sizeof(float);
+  if (smem > 48 * 1024 || G < 1 || G > DG_MAX_OSP_SETS) {
+    set_error("osp_sets: frames*speakers too large, or not 1..64 sets");
+    return -1;
+  }
+  osp_sets_kernel<<<dim3(B, G), 256, smem, st>>>(seg, F, K, sets, out);
   DG_LAUNCHED();
   return 0;
 }
@@ -301,12 +326,11 @@ int launch_stats_pool(const float* x, int B, int stride, int T, int C, const flo
 // Row weights of the fused TDNN5 + pooling epilogue (gemm_tc.cu, TC_POOL): the OSP weights resized from F to T frames exactly
 // like stats_pool_kernel does, one float4 per trunk row (zero past the T valid frames of an item / for absent speakers), and
 // v1 = sum w (+ eps), v2 = sum w^2 per (item, speaker) in the same summation order as stats_pool_kernel.
-__global__ void __launch_bounds__(256) pool_weights_kernel(const float* __restrict__ w, int F, int K, int item_rows, int T,
-                                                           const int* __restrict__ idx0, const int* __restrict__ idx1,
-                                                           const float* __restrict__ lam1, float eps, float* __restrict__ row_w,
-                                                           float* __restrict__ vsum) {
-  extern __shared__ float wr[];      // [T][4]
-  const int b = blockIdx.x;
+// Item b's row weights and weight sums; shared by pool_weights_kernel and pool_weights_sets_kernel.
+__device__ __forceinline__ void pool_weights_item(const float* __restrict__ w, int b, int F, int K, int item_rows, int T,
+                                                  const int* __restrict__ idx0, const int* __restrict__ idx1,
+                                                  const float* __restrict__ lam1, float eps, float* __restrict__ row_w,
+                                                  float* __restrict__ vsum, float* wr /*[T][4] shared*/) {
   for (int i = threadIdx.x; i < item_rows * 4; i += blockDim.x) {
     const int t = i >> 2, k = i & 3;
     float v = 0.f;
@@ -332,10 +356,41 @@ __global__ void __launch_bounds__(256) pool_weights_kernel(const float* __restri
   }
 }
 
+__global__ void __launch_bounds__(256) pool_weights_kernel(const float* __restrict__ w, int F, int K, int item_rows, int T,
+                                                           const int* __restrict__ idx0, const int* __restrict__ idx1,
+                                                           const float* __restrict__ lam1, float eps, float* __restrict__ row_w,
+                                                           float* __restrict__ vsum) {
+  extern __shared__ float wr[];      // [T][4]
+  pool_weights_item(w, blockIdx.x, F, K, item_rows, T, idx0, idx1, lam1, eps, row_w, vsum, wr);
+}
+
+// one CTA per (item, set): set g reads its OSP weights at w + g B F K and writes its row weights at row_w + g rw_stride and its
+// weight sums at vsum + g B K 2
+__global__ void __launch_bounds__(256) pool_weights_sets_kernel(const float* __restrict__ w, int F, int K, int item_rows, int T,
+                                                                const int* __restrict__ idx0, const int* __restrict__ idx1,
+                                                                const float* __restrict__ lam1, float eps,
+                                                                float* __restrict__ row_w, long long rw_stride,
+                                                                float* __restrict__ vsum) {
+  extern __shared__ float wr[];      // [T][4]
+  const int g = blockIdx.y;
+  const size_t B = gridDim.x;
+  pool_weights_item(w + g * B * F * K, blockIdx.x, F, K, item_rows, T, idx0, idx1, lam1, eps, row_w + g * rw_stride,
+                    vsum + g * B * K * 2, wr);
+}
+
 int launch_pool_weights(const float* w, int B, int F, int K, int item_rows, int T, const int* idx0, const int* idx1,
                         const float* lam1, float eps, float* row_w, float* vsum, cudaStream_t st) {
   ProfScope _ps("pool_weights", st);
   pool_weights_kernel<<<B, 256, (size_t)T * 4 * sizeof(float), st>>>(w, F, K, item_rows, T, idx0, idx1, lam1, eps, row_w, vsum);
+  DG_LAUNCHED();
+  return 0;
+}
+
+int launch_pool_weights_sets(const float* w, int B, int G, int F, int K, int item_rows, int T, const int* idx0, const int* idx1,
+                             const float* lam1, float eps, float* row_w, long long rw_stride, float* vsum, cudaStream_t st) {
+  ProfScope _ps("pool_weights", st);
+  pool_weights_sets_kernel<<<dim3(B, G), 256, (size_t)T * 4 * sizeof(float), st>>>(w, F, K, item_rows, T, idx0, idx1, lam1, eps,
+                                                                                 row_w, rw_stride, vsum);
   DG_LAUNCHED();
   return 0;
 }

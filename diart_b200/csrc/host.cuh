@@ -291,6 +291,8 @@ int emb_trunk(dg_emb* h, const float* wav, int U, const Geom& g, cudaStream_t st
 bool pool_fusable(const dg_emb* h, int K, const Geom& g);
 int emb_tail(dg_emb* h, int B, const Geom& g, const float* weights, int F, int K, int T, bool fuse, int normalize, float norm,
              float* out, cudaStream_t st, int sm_cap = 0);
+int emb_tail_sets(dg_emb* h, int B, const Geom& g, const float* weights /*[G][B][F][K]*/, int G, int F, int K, int T, bool fuse,
+                  float* out, int64_t out_stride, cudaStream_t st, int sm_cap = 0);
 
 // ==================================================================================== clustering (api_cluster.cu)
 struct dg_cluster {
@@ -390,5 +392,7 @@ struct NetLanes {
 int net_lanes_create(NetLanes& n);
 // segmentation chain on s_seg[lane] and embedding chain on s_emb, both starting after `start`; on return e_emb (recorded on
 // s_emb) marks seg, osp and emb complete.  stream_hop > 0: the batch is windows of one stream that many samples apart.
+// sets (or null: the handle's own gamma, beta, normalize): the OSP weights and embeddings of G sets over one trunk pass, set g's
+// embeddings at emb + g emb_stride.
 int pipeline_nets(NetLanes* h, const float* wav, int S, const StepShape& sh, float* seg, float* emb, cudaEvent_t start,
-                  int lane, int stream_hop);
+                  int lane, int stream_hop, const OspSets* sets = nullptr, int G = 1, int64_t emb_stride = 0);

@@ -34,6 +34,12 @@ pyannote.metrics' own, with a forgiveness collar and ``skip_overlap``) and the d
 (``uems``): :func:`scored_regions` computes each file's scored regions once, the references are cropped to them on the
 host and the hypotheses on the device (``dg_sweep_set_scored_regions``; DESIGN.md "DER scoring", steps 1-5).
 
+:class:`DatasetSweep` also tunes the overlap-aware embedding parameters ``gamma``, ``beta`` and
+``normalize_embedding_weights`` (``osp=``): they reach the networks only at the embedding's statistics pooling, so one network
+pass computes the scores once and the embeddings of every constructed *OSP set* (``dg_pipeline_nets_sets``), and each trial's
+clustering reads the embeddings of its own set (``dg_sweep_set_trial_sets``; DESIGN.md "Sweeps over overlap-aware
+weightings").
+
 The three classes share their mechanics: :class:`FileBatches` cuts the window batches of every network pass,
 :func:`stream_plan` is the post-path plan of one file, ``_timed`` puts CUDA events around one C call and ``_turn_list_call``
 downloads a turn list into a host buffer that grows on demand.  ``HyperParameterSweep._run_trials`` / ``_score_trials`` are the
@@ -71,6 +77,7 @@ TRIAL_CHUNKS_PER_LAUNCH = 4 << 20   # DatasetSweep: trials x chunks per launch (
 PATCH_COLLAR = 0.05           # PredictionAccumulator's default (sinks.py)
 MAX_REFERENCE_LABELS = 32     # one lane per reference label in the scoring kernel
 PRECISION = 1e-6              # pyannote.core's SEGMENT_PRECISION: Segment.__bool__, Segment.intersects
+MAX_OSP_SETS = 64            # OSP sets per network pass (dg_pipeline_nets_sets)
 WHOLE_LINE = (-1e300, 1e300)  # the uem of a file that has none (scored_regions: the scored regions do not depend on the trial)
 
 
@@ -91,6 +98,79 @@ def trial_params(trials: Sequence[Mapping[str, float]], config, names: Optional[
                              f"the plan and stay fixed per sweep)")
         out[i] = [float(trial.get(n, getattr(config, n))) for n in names]
     return out
+
+
+OSP_PARAMS = ("gamma", "beta", "normalize_embedding_weights")   # the config keys of an OSP set
+
+
+def osp_set(entry: Mapping, config) -> Tuple[float, float, bool]:
+    """one OSP set -> (gamma, beta, normalize) as the pipeline receives them: gamma and beta rounded to float32, a missing key
+    the config's value.  ValueError for another key or a non-finite gamma / beta."""
+    unknown = sorted(set(entry) - set(OSP_PARAMS))
+    if unknown:
+        raise ValueError(f"OSP set {dict(entry)}: unknown keys {unknown} (only {list(OSP_PARAMS)})")
+    values = [float(entry.get(n, getattr(config, n))) for n in OSP_PARAMS[:2]]
+    if not all(math.isfinite(v) for v in values):
+        raise ValueError(f"OSP set {dict(entry)}: gamma and beta must be finite")
+    gamma, beta = (float(np.float32(v)) for v in values)
+    return gamma, beta, bool(entry.get(OSP_PARAMS[2], config.normalize_embedding_weights))
+
+
+def osp_sets(config, osp: Iterable[Mapping] = ()) -> Tuple[Tuple[float, float, bool], ...]:
+    """the OSP sets a sweep constructs: the config's own first, then those of ``osp`` (entries keyed like the config, see
+    :func:`osp_set`) in order, duplicates (equal float32 gamma and beta, equal normalize) once"""
+    out = [osp_set({}, config)]
+    for entry in osp:
+        s = osp_set(entry, config)
+        if s not in out:
+            out.append(s)
+    if len(out) > MAX_OSP_SETS:
+        raise ValueError(f"{len(out)} OSP sets; at most {MAX_OSP_SETS} per sweep")
+    return tuple(out)
+
+
+def osp_index(config, sets: Sequence[Tuple[float, float, bool]], entry: Mapping) -> int:
+    """the index in ``sets`` of the OSP set ``entry`` (:func:`osp_set`), else ValueError naming the constructed sets"""
+    s = osp_set(entry, config)
+    if s not in sets:
+        raise ValueError(f"OSP set {osp_dict(s)} was not constructed (the sweep's sets: {[osp_dict(x) for x in sets]})")
+    return list(sets).index(s)
+
+
+def osp_dict(s: Tuple[float, float, bool]) -> Dict[str, object]:
+    """(gamma, beta, normalize) -> the config-keyed dict of that set"""
+    return dict(zip(OSP_PARAMS, s))
+
+
+def trial_osp_params(trials: Sequence[Mapping[str, float]], config,
+                     sets: Sequence[Tuple[float, float, bool]]) -> Tuple[np.ndarray, np.ndarray]:
+    """trials that may also carry ``gamma``, ``beta`` and ``normalize_embedding_weights`` -> (each trial's OSP set index in
+    ``sets`` int32 (T,), :func:`trial_params` of the rest float64 (T, 3)).  ValueError for a set that is not in ``sets``."""
+    trials = list(trials)
+    index = np.empty(len(trials), dtype=np.int32)
+    rest = []
+    for i, trial in enumerate(trials):
+        try:
+            index[i] = osp_index(config, sets, {k: trial[k] for k in OSP_PARAMS if k in trial})
+        except ValueError as e:
+            raise ValueError(f"trial {i}: {e}") from None
+        rest.append({k: v for k, v in trial.items() if k not in OSP_PARAMS})
+    return index, trial_params(rest, config)
+
+
+def trial_osp_sets(config, trials: Sequence[Mapping[str, float]]) -> Tuple[Tuple[float, float, bool], ...]:
+    """:func:`osp_sets` of the distinct OSP sets the trials name (the config's own first)"""
+    return osp_sets(config, [{k: t[k] for k in OSP_PARAMS if k in t} for t in trials])
+
+
+def _set_trial_sets(handle, trial_sets: Optional[Tuple[int, np.ndarray]]):
+    """the handle's trial sets for its next call: (number of sets, int32 (T,) set per trial), or None (embeddings of one set)"""
+    if trial_sets is None:
+        _lib.check(_lib.lib().dg_sweep_set_trial_sets(handle, 0, None, 0))
+    else:
+        G, index = trial_sets
+        index = np.ascontiguousarray(index, dtype=np.int32)
+        _lib.check(_lib.lib().dg_sweep_set_trial_sets(handle, int(G), index.ctypes.data, len(index)))
 
 
 @dataclass
@@ -752,6 +832,39 @@ class HyperParameterSweep:
                 collect()
             return torch.cat(segs), torch.cat(embs)
 
+    def network_pass_sets(self, fws: Sequence[FileWindows], sets: Sequence[Tuple[float, float, bool]]):
+        """:meth:`network_pass_files` for several OSP sets (:func:`osp_sets`) -> scores (N, F, K) and the embeddings of
+        every set (G, N, K, D), set g's the bits :meth:`network_pass_files` gives under a config with that set.  One
+        ``dg_pipeline_nets_sets`` per batch writes into the two tensors; consecutive batches run on two streams in turn, so
+        two are in flight."""
+        pipe = self.pipeline
+        pipe.reset()
+        h, F, K, D = pipe._ensure_fused(fws[0].chunk_samples)
+        N, G = sum(fw.num_windows for fw in fws), len(sets)
+        osp = np.ascontiguousarray([s[:2] for s in sets], dtype=np.float32)
+        normalize = np.ascontiguousarray([int(s[2]) for s in sets], dtype=np.int32)
+        seg = torch.empty((N, F, K), device=self.device)
+        embs = torch.empty((G, N, K, D), device=self.device)
+        batches = FileBatches(fws, self.config, self.device)
+        with torch.cuda.device(self.device):
+            current = torch.cuda.current_stream(self.device)
+            lanes = [torch.cuda.Stream(self.device), torch.cuda.Stream(self.device)]
+            inflight, n0 = [], 0
+            for i, windows in enumerate(batches):
+                lane = lanes[i % 2]
+                lane.wait_stream(current)
+                B = windows.shape[0]
+                _lib.check(_lib.lib().dg_pipeline_nets_sets(h, windows.data_ptr(), B, windows.shape[1], G, osp.ctypes.data,
+                                                            normalize.ctypes.data, seg[n0].data_ptr(), embs[0, n0].data_ptr(),
+                                                            N * K * D, lane.cuda_stream))
+                n0 += B
+                inflight.append((windows, lane))             # the windows must stay alive until their lane is waited for
+                if len(inflight) == 2:
+                    current.wait_stream(inflight.pop(0)[1])
+            while inflight:
+                current.wait_stream(inflight.pop(0)[1])
+        return seg, embs
+
     # ------------------------------------------------------------------ clustering + post-path for T trials
     def _handle(self, F: int, K: int, D: int, nw: Optional[int] = None):
         """the dg_sweep handle for these dimensions; ``nw``: its plan width, by default the config's latency / step"""
@@ -770,13 +883,15 @@ class HyperParameterSweep:
         return self._h, nw
 
     def _run_trials(self, entry, file_args: tuple, lead: tuple, seg: torch.Tensor, emb: torch.Tensor, plans,
-                    params: np.ndarray, keep_state: bool) -> SweepOutputs:
+                    params: np.ndarray, keep_state: bool, trial_sets: Optional[Tuple[int, np.ndarray]] = None) -> SweepOutputs:
         """The body of :meth:`sweep` and :meth:`DatasetSweep.sweep`.  ``entry``: dg_sweep_run, or dg_sweep_run_files with
         ``file_args`` = what it takes after the chunk count (files, chunk offsets) and ``lead`` = (files,), the leading
-        dimension of its centroids.  ``plans``: (plan, out_start, out_res) of the N chunks."""
+        dimension of its centroids.  ``plans``: (plan, out_start, out_res) of the N chunks.  ``trial_sets``: (G, set of each
+        trial) with ``emb`` (G, N, K, D), or None with ``emb`` (N, K, D)."""
         N, F, K = seg.shape
-        D, M = emb.shape[2], int(self.config.max_speakers)
+        D, M = emb.shape[-1], int(self.config.max_speakers)
         h, _ = self._handle(F, K, D)
+        _set_trial_sets(h, trial_sets)
         plan, out_start, out_res = plans
         params = np.ascontiguousarray(params, dtype=np.float64)
         T = len(params)
@@ -789,16 +904,19 @@ class HyperParameterSweep:
         return SweepOutputs(header, self._turns[:n_turns].copy(), n_turns, out_start, out_res, maps, centers, seconds)
 
     def _score_trials(self, entry, file_args: tuple, lead: tuple, seg: torch.Tensor, emb: torch.Tensor, plans,
-                      params: np.ndarray, shift, reference: tuple, segments: bool = False, regions: Optional[tuple] = None):
+                      params: np.ndarray, shift, reference: tuple, segments: bool = False, regions: Optional[tuple] = None,
+                      trial_sets: Optional[Tuple[int, np.ndarray]] = None):
         """The body of :meth:`sweep_score` and of each launch of :meth:`DatasetSweep.score` -> (components ``lead`` +
         (T, 5), device seconds, hypothesis offsets, hypothesis segments).  ``entry``: dg_sweep_score, or
         dg_sweep_score_files with ``file_args`` and ``lead`` as in :meth:`_run_trials`.  ``shift``: the timestamp shift, or
         the address of the per-file shifts.  ``reference``: the entry point's four reference arguments (rows, labels,
         then the row and label counts, or the addresses of the per-file row offsets and label counts).  ``segments`` is
-        for the one-file entry point.  ``regions``: ``pack_regions`` of the files' scored regions, or None."""
+        for the one-file entry point.  ``regions``: ``pack_regions`` of the files' scored regions, or None.  ``trial_sets``
+        as in :meth:`_run_trials`."""
         N, F, K = seg.shape
-        h, _ = self._handle(F, K, emb.shape[2])
+        h, _ = self._handle(F, K, emb.shape[-1])
         _set_regions(_lib.lib().dg_sweep_set_scored_regions, h, regions)
+        _set_trial_sets(h, trial_sets)
         plan, out_start, out_res = plans
         params = np.ascontiguousarray(params, dtype=np.float64)
         T, M = len(params), int(self.config.max_speakers)
@@ -818,13 +936,15 @@ class HyperParameterSweep:
         return comp, secs, offsets, hseg
 
     def sweep(self, seg: torch.Tensor, emb: torch.Tensor, starts: np.ndarray, params: np.ndarray,
-              keep_state: bool = False) -> SweepOutputs:
-        """dg_sweep_run over device scores / embeddings of N chunks starting at ``starts`` for params (T, 3)"""
+              keep_state: bool = False, trial_sets: Optional[Tuple[int, np.ndarray]] = None) -> SweepOutputs:
+        """dg_sweep_run over device scores / embeddings of N chunks starting at ``starts`` for params (T, 3); ``trial_sets``
+        as in :meth:`_run_trials`"""
         plans = stream_plan(starts, self.config, seg.shape[1])
-        return self._run_trials(_lib.lib().dg_sweep_run, (), (), seg, emb, plans, params, keep_state)
+        return self._run_trials(_lib.lib().dg_sweep_run, (), (), seg, emb, plans, params, keep_state, trial_sets)
 
     def sweep_score(self, seg: torch.Tensor, emb: torch.Tensor, fw: FileWindows, params: np.ndarray, ref_rows: np.ndarray,
-                    ref_labels: np.ndarray, num_ref_labels: int, segments: bool = False, regions: Optional[tuple] = None):
+                    ref_labels: np.ndarray, num_ref_labels: int, segments: bool = False, regions: Optional[tuple] = None,
+                    trial_sets: Optional[Tuple[int, np.ndarray]] = None):
         """dg_sweep_score over device scores / embeddings of ``fw``'s chunks for params (T, 3) against a reference in
         ``reference_arrays`` form -> (components (T, 5), device seconds, hypothesis offsets, hypothesis segments).  The last
         two are device tensors when ``segments`` (int32 (T * max_speakers + 1,) and float64 (n, 2), see the C header), else
@@ -835,7 +955,19 @@ class HyperParameterSweep:
         reference = (rows.ctypes.data, labels.ctypes.data, len(rows), int(num_ref_labels))
         plans = stream_plan(fw.starts, self.config, seg.shape[1])
         return self._score_trials(_lib.lib().dg_sweep_score, (), (), seg, emb, plans, params, -fw.padding[0], reference,
-                                  segments, regions)
+                                  segments, regions, trial_sets)
+
+    def _network_pass_trials(self, fw: FileWindows, trials: Sequence[Mapping[str, float]]):
+        """the network pass of one file for trials that may carry OSP sets -> (params (T, 3), scores, embeddings, set of each
+        trial): without other sets than the config's :meth:`network_pass` and no trial sets, else :meth:`network_pass_sets`
+        over the distinct sets the trials name"""
+        sets = trial_osp_sets(self.config, trials)
+        index, params = trial_osp_params(trials, self.config, sets)
+        if len(sets) == 1:
+            seg, emb = self.network_pass(fw)
+            return params, seg, emb, None
+        seg, embs = self.network_pass_sets([fw], sets)
+        return params, seg, embs, (len(sets), index)
 
     def _seg_resolution(self, start: float, F: int) -> float:
         return seg_resolution(self.config, start, F)
@@ -844,18 +976,21 @@ class HyperParameterSweep:
     def run(self, waveform: np.ndarray, uri: Optional[str] = None,
             trials: Sequence[Mapping[str, float]] = ({},)) -> List[Annotation]:
         """1-D float32 waveform at ``config.sample_rate`` -> one whole-file prediction per trial (the prediction
-        ``Benchmark.run_single`` returns for a pipeline with that trial's tau_active / rho_update / delta_new)"""
-        params = trial_params(trials, self.config)
+        ``Benchmark.run_single`` returns for a pipeline with that trial's tau_active / rho_update / delta_new).  A trial may
+        also carry ``gamma``, ``beta`` and ``normalize_embedding_weights``: the network pass then computes the embeddings of
+        every distinct such set once (:meth:`network_pass_sets`)."""
+        trial_osp_params(trials, self.config, trial_osp_sets(self.config, trials))    # bad trials fail before the networks
         t0 = time.perf_counter()
         fw = file_windows(waveform, self.config)
-        seg, emb = self.network_pass(fw)
+        params, seg, emb, sets = self._network_pass_trials(fw, trials)
         torch.cuda.synchronize(self.device)
         t1 = time.perf_counter()
         labels = [f"speaker{g}" for g in range(int(self.config.max_speakers))]
         shift = -fw.padding[0]
         out, dev, host = [], 0.0, 0.0
         for i in range(0, len(params), TRIALS_PER_LAUNCH):
-            r = self.sweep(seg, emb, fw.starts, params[i:i + TRIALS_PER_LAUNCH])
+            part = None if sets is None else (sets[0], sets[1][i:i + TRIALS_PER_LAUNCH])
+            r = self.sweep(seg, emb, fw.starts, params[i:i + TRIALS_PER_LAUNCH], trial_sets=part)
             dev += r.device_seconds
             t2 = time.perf_counter()
             out += assemble_predictions(r.header, r.turns, r.n_turns, r.out_start, r.out_res, labels, shift, uri)
@@ -871,8 +1006,9 @@ class HyperParameterSweep:
 
         ``metric``: a :class:`DiarizationErrorRate` (or pyannote.metrics' own) with a forgiveness collar and / or
         ``skip_overlap``; None is ``DiarizationErrorRate()``.  ``uem``: the scored parts of the file, ``(start, end)`` pairs
-        or ``Segment``s in the reference's time base; None scores everything (DESIGN.md "DER scoring")."""
-        params = trial_params(trials, self.config)
+        or ``Segment``s in the reference's time base; None scores everything (DESIGN.md "DER scoring").  Trials may carry OSP
+        sets as in :meth:`run`."""
+        trial_osp_params(trials, self.config, trial_osp_sets(self.config, trials))
         collar, skip_overlap = metric_protocol(metric, "DiarizationErrorRate")
         uem = check_uem(uem)
         regions = None
@@ -881,13 +1017,14 @@ class HyperParameterSweep:
         rows, labels, names = reference_arrays(reference, regions)
         t0 = time.perf_counter()
         fw = file_windows(waveform, self.config)
-        seg, emb = self.network_pass(fw)
+        params, seg, emb, sets = self._network_pass_trials(fw, trials)
         torch.cuda.synchronize(self.device)
         t1 = time.perf_counter()
         comps, dev = [], 0.0
         for i in range(0, len(params), TRIALS_PER_LAUNCH):
+            part = None if sets is None else (sets[0], sets[1][i:i + TRIALS_PER_LAUNCH])
             comp, secs, _, _ = self.sweep_score(seg, emb, fw, params[i:i + TRIALS_PER_LAUNCH], rows, labels, len(names),
-                                                regions=None if regions is None else pack_regions([regions]))
+                                                regions=None if regions is None else pack_regions([regions]), trial_sets=part)
             comps.append(comp)
             dev += secs
         self.timing = {"network": t1 - t0, "score": dev}
@@ -897,9 +1034,11 @@ class HyperParameterSweep:
                     metric=None) -> Tuple[List[DERComponents], DERComponents]:
         """``files``: (waveform, reference) pairs -> (components per file, their sum).  ``total.der`` per trial is the
         value the reference's ``Optimizer.objective`` minimises over a dataset (a fraction, not a percentage).  Runs as a
-        :class:`DatasetSweep` over the files.  ``metric`` as in :meth:`score`."""
+        :class:`DatasetSweep` over the files, built with the OSP sets the trials name.  ``metric`` as in :meth:`score`."""
         metric_protocol(metric, "DiarizationErrorRate")        # a bad metric fails before the network pass
-        dataset = DatasetSweep(self.config, [(None, waveform, reference) for waveform, reference in files], sweep=self)
+        sets = trial_osp_sets(self.config, trials)
+        dataset = DatasetSweep(self.config, [(None, waveform, reference) for waveform, reference in files], sweep=self,
+                               osp=[osp_dict(s) for s in sets[1:]])
         out = dataset.score(trials, metric)
         self.timing = dict(dataset.timing)
         return out
@@ -1149,6 +1288,14 @@ class DatasetSweep(_DatasetSweep):
     scoring call.  ``score`` and ``score_latencies`` take a ``metric`` (:class:`DiarizationErrorRate`, or
     pyannote.metrics' own) with a forgiveness collar and / or ``skip_overlap``; the default is ``DiarizationErrorRate()``.
     The packed references and scored regions are kept per metric.
+
+    ``osp``: OSP sets besides the config's own, each a dict with any of ``gamma``, ``beta`` and
+    ``normalize_embedding_weights`` (a missing key takes the config's value; equal float32 values collapse).  The network pass
+    then computes the scores once and the embeddings of every set (``osp_sets`` lists them, the config's first; ``embs`` is
+    (G, N, K, D), ``emb`` set 0), at (F K + G K D) float32 per chunk.  Trials of every method may carry those three keys, and
+    each is clustered over its own set's embeddings in the same launches as the others: for every set the results are the
+    bits a ``DatasetSweep`` whose config has that set's values gives.  A trial whose set was not constructed raises
+    ValueError before any launch.  Without ``osp`` (or with only the config's set) the sweep runs as before.
     """
 
     _pack_references = staticmethod(pack_references)
@@ -1156,8 +1303,9 @@ class DatasetSweep(_DatasetSweep):
 
     def __init__(self, config: SpeakerDiarizationConfig, files: Iterable[Tuple[Optional[str], np.ndarray, Optional[Annotation]]],
                  sweep: Optional[HyperParameterSweep] = None, latencies: Optional[Iterable] = None,
-                 uems: Optional[Sequence] = None):
+                 uems: Optional[Sequence] = None, osp: Optional[Iterable[Mapping]] = None):
         self._sweep = sweep
+        self.osp_sets = osp_sets(config, osp if osp is not None else ())
         super().__init__(config, files, latencies, uems)
 
     def _open(self) -> torch.device:
@@ -1166,39 +1314,61 @@ class DatasetSweep(_DatasetSweep):
         return self._sweep.device
 
     def _networks(self, fws: Sequence[FileWindows]):
-        self.seg, self.emb = self._sweep.network_pass_files(fws)
+        if len(self.osp_sets) == 1:
+            self.seg, self.emb = self._sweep.network_pass_files(fws)
+            self.embs = self.emb[None]
+        else:
+            self.seg, self.embs = self._sweep.network_pass_sets(fws, self.osp_sets)
+            self.emb = self.embs[0]
 
     @property
     def resident_bytes(self) -> int:
         """device bytes of the kept network outputs"""
-        return self.seg.numel() * self.seg.element_size() + self.emb.numel() * self.emb.element_size()
+        return self.seg.numel() * self.seg.element_size() + self.embs.numel() * self.embs.element_size()
 
-    def file_outputs(self, f: int, latency=None) -> Tuple[torch.Tensor, torch.Tensor]:
+    def file_outputs(self, f: int, latency=None, osp: Optional[Mapping] = None) -> Tuple[torch.Tensor, torch.Tensor]:
         """file f's slice of the resident scores (n, F, K) and embeddings (n, K, D); ``latency`` (a constructed one, default
-        the config's): its windows at that latency, the first chunks of its unit"""
+        the config's): its windows at that latency, the first chunks of its unit; ``osp`` (a constructed OSP set, keyed like
+        the config; default the config's): that set's embeddings"""
         c0, c1 = self._chunk_range(f, latency)
-        return self.seg[c0:c1], self.emb[c0:c1]
+        g = 0 if osp is None else osp_index(self.config, self.osp_sets, osp)
+        return self.seg[c0:c1], self.embs[g, c0:c1]
 
-    def _over_files(self, entry) -> tuple:
+    def _rows(self, trials: Sequence[Mapping[str, float]]) -> np.ndarray:
+        """trials -> float64 (T, 4): :func:`trial_params` and the index of the trial's OSP set in :attr:`osp_sets`"""
+        index, params = trial_osp_params(trials, self.config, self.osp_sets)
+        return np.column_stack([params, index.astype(np.float64)])
+
+    def _trial_sets(self, params: np.ndarray) -> Tuple[np.ndarray, torch.Tensor, Optional[Tuple[int, np.ndarray]]]:
+        """params (T, 3), or (T, 4) with each trial's OSP set index -> (params (T, 3), the embeddings a launch reads, its
+        trial sets): the resident embeddings of one set without trial sets when the sweep has one set or no set index is
+        given, else those of all sets"""
+        params = np.asarray(params, dtype=np.float64)
+        if params.ndim == 2 and params.shape[1] == 4 and len(self.osp_sets) > 1:
+            return params[:, :3], self.embs, (len(self.osp_sets), params[:, 3].astype(np.int32))
+        return (params[:, :3] if params.ndim == 2 else params), self.emb, None
+
+    def _over_files(self, entry, emb: torch.Tensor) -> tuple:
         """the leading arguments of ``HyperParameterSweep._run_trials`` / ``_score_trials`` for the ``_files`` entry point
         ``entry`` over the resident outputs and the concatenated plans"""
         nf = len(self.uris)
-        return entry, (nf, self.offsets.ctypes.data), (nf,), self.seg, self.emb, (self.plan, self.out_start, self.out_res)
+        return entry, (nf, self.offsets.ctypes.data), (nf,), self.seg, emb, (self.plan, self.out_start, self.out_res)
 
     def sweep(self, params: np.ndarray, keep_state: bool = False) -> SweepOutputs:
-        """dg_sweep_run_files over the resident outputs for params (T, 3): header (T, N, 4) and turns over the N
-        concatenated chunks; with ``keep_state`` maps (T, N, K) and centroids (files, T, M, D) on the device.  Not for a
-        sweep built with ``latencies`` (:meth:`sweep_latencies`)."""
+        """dg_sweep_run_files over the resident outputs for params (T, 3), or (T, 4) with each trial's OSP set index:
+        header (T, N, 4) and turns over the N concatenated chunks; with ``keep_state`` maps (T, N, K) and centroids (files,
+        T, M, D) on the device.  Not for a sweep built with ``latencies`` (:meth:`sweep_latencies`)."""
         if self.units is not None:
             raise ValueError("a sweep over several latencies runs through sweep_latencies")
-        return self._sweep._run_trials(*self._over_files(_lib.lib().dg_sweep_run_files), params, keep_state)
+        params, emb, sets = self._trial_sets(params)
+        return self._sweep._run_trials(*self._over_files(_lib.lib().dg_sweep_run_files, emb), params, keep_state, sets)
 
     def run(self, trials: Sequence[Mapping[str, float]] = ({},)) -> List[List[Annotation]]:
         """-> predictions [file][trial]: what :meth:`HyperParameterSweep.run` returns for each file alone"""
         if self.units is not None:
             return self.run_latencies(trials, [self.config.latency])[float(self.config.latency)]
         labels = [f"speaker{g}" for g in range(int(self.config.max_speakers))]
-        return self._run(trial_params(trials, self.config), self.sweep, labels)
+        return self._run(self._rows(trials), self.sweep, labels)
 
     def score(self, trials: Sequence[Mapping[str, float]] = ({},), metric=None) \
             -> Tuple[List[DERComponents], DERComponents]:
@@ -1207,7 +1377,7 @@ class DatasetSweep(_DatasetSweep):
         minimises.  Every file needs a reference."""
         if self.units is not None:
             return self.score_latencies(trials, [self.config.latency], metric)[float(self.config.latency)]
-        return self._score(trial_params(trials, self.config), metric)
+        return self._score(self._rows(trials), metric)
 
     def sweep_latencies(self, params: np.ndarray, latencies=None, keep_maps: bool = False) -> SweepOutputs:
         """dg_sweep_run_latencies over the resident outputs for params (T, 3) at the constructed ``latencies`` (None: all):
@@ -1221,7 +1391,7 @@ class DatasetSweep(_DatasetSweep):
             -> Dict[float, List[List[Annotation]]]:
         """-> {latency: predictions [file][trial]} for the constructed ``latencies`` (None: all): for each latency L what
         :meth:`run` of a ``DatasetSweep`` built at L returns.  One launch per kernel and trial group for all of them."""
-        params, sel = trial_params(trials, self.config), self._selection(latencies)
+        params, sel = self._rows(trials), self._selection(latencies)
         if self.units is None:
             return {self.latencies[0]: self.run(trials)}
         labels = [f"speaker{g}" for g in range(int(self.config.max_speakers))]
@@ -1233,7 +1403,7 @@ class DatasetSweep(_DatasetSweep):
         what :meth:`score` of a ``DatasetSweep`` built at L returns with the same ``metric``, bit for bit.  The clustering
         runs once per (unit, trial) whatever the number of latencies; one launch per kernel and trial group
         (:func:`trial_groups` over the virtual chunks)."""
-        params, sel = trial_params(trials, self.config), self._selection(latencies)
+        params, sel = self._rows(trials), self._selection(latencies)
         if self.units is None:
             return {self.latencies[0]: self.score(trials, metric)}
         return self._score_latencies(params, sel, self._score_virtual, metric)
@@ -1243,13 +1413,15 @@ class DatasetSweep(_DatasetSweep):
         sw = self._sweep
         N, F, K = self.seg.shape
         h, _ = sw._handle(F, K, self.emb.shape[2], self.units.nw)
+        params, emb, sets = self._trial_sets(params)
+        _set_trial_sets(h, sets)
         plan, out_start, out_res = tabs[2:5]
         params = np.ascontiguousarray(params, dtype=np.float64)
         T, Nv = len(params), len(tabs[0])
         header = np.empty((T, Nv, 4), dtype=np.int32)
         maps = torch.empty((T, N, K), dtype=torch.int32, device=self.device) if keep_maps else None
         n_turns, seconds = _turn_list_call(sw, self.device, T * Nv * 8, lambda *turn_list: _lib.lib().dg_sweep_run_latencies(
-            h, self.seg.data_ptr(), self.emb.data_ptr(), *self._layout(tabs), params.ctypes.data, T, plan.ctypes.data,
+            h, self.seg.data_ptr(), emb.data_ptr(), *self._layout(tabs), params.ctypes.data, T, plan.ctypes.data,
             _lib.ptr(maps), header.ctypes.data, *turn_list))
         return SweepOutputs(header, sw._turns[:n_turns].copy(), n_turns, out_start, out_res, maps, None, seconds)
 
@@ -1260,11 +1432,13 @@ class DatasetSweep(_DatasetSweep):
         N, F, K = self.seg.shape
         h, _ = self._sweep._handle(F, K, self.emb.shape[2], self.units.nw)
         _set_regions(_lib.lib().dg_sweep_set_scored_regions, h, regions)
+        params, emb, sets = self._trial_sets(params)
+        _set_trial_sets(h, sets)
         plan, out_start, out_res, shifts = tabs[2:]
         params = np.ascontiguousarray(params, dtype=np.float64)
         comp = np.empty((len(tabs[1]) - 1, len(params), 5), dtype=np.float64)
         rc, seconds = _timed(self.device, lambda st: _lib.lib().dg_sweep_score_latencies(
-            h, self.seg.data_ptr(), self.emb.data_ptr(), *self._layout(tabs), params.ctypes.data, len(params),
+            h, self.seg.data_ptr(), emb.data_ptr(), *self._layout(tabs), params.ctypes.data, len(params),
             plan.ctypes.data, out_start.ctypes.data, out_res.ctypes.data, shifts.ctypes.data, PATCH_COLLAR,
             *(a.ctypes.data for a in refs), comp.ctypes.data, st))
         _lib.check(rc)
@@ -1272,8 +1446,9 @@ class DatasetSweep(_DatasetSweep):
 
     def _score_group(self, params: np.ndarray, refs: tuple, regions: Optional[tuple]) -> Tuple[np.ndarray, float]:
         reference = tuple(a.ctypes.data for a in refs)             # rows, labels, row offsets, label counts
-        return self._sweep._score_trials(*self._over_files(_lib.lib().dg_sweep_score_files), params,
-                                         self.shifts.ctypes.data, reference, regions=regions)[:2]
+        params, emb, sets = self._trial_sets(params)
+        return self._sweep._score_trials(*self._over_files(_lib.lib().dg_sweep_score_files, emb), params,
+                                         self.shifts.ctypes.data, reference, regions=regions, trial_sets=sets)[:2]
 
     def _components(self, f: int, comp: np.ndarray, refs: tuple) -> DERComponents:
         return DERComponents.from_array(comp)

@@ -166,6 +166,17 @@ int dg_pipeline_collect(dg_pipeline* h, const float** seg_dev, const float** emb
 int dg_pipeline_collect_copy(dg_pipeline* h, float* seg_dev, float* emb_dev, int32_t* map_dev, void* stream);
 int dg_pipeline_submit_host(dg_pipeline* h, const float* wav_host /*pinned memory recommended*/, int B, int S);
 int dg_pipeline_collect_host(dg_pipeline* h, float* seg_host, float* emb_host, int32_t* map_host);
+/* The networks of one batch without clustering, for num_sets (1..64) overlap-aware weightings ("OSP sets"): osp_host float32
+ * [num_sets][2] = {gamma, beta} (finite), normalize_host int32 [num_sets] (0 or 1).  The segmentation, the sinc front end and
+ * the embedding trunk run once; the OSP weights, the pooling row weights, TDNN5 + pooling (or the un-fused pooling of the
+ * WeSpeaker embedding), the finaliser and the projection run per set.  seg_dev [B,F,K]; set g's embeddings [B,K,D] at
+ * emb_dev + g * emb_set_stride floats (emb_set_stride >= B K D when num_sets > 1).  Set g's outputs are the bits a pipeline
+ * created with that set's gamma, beta and normalize gives in dg_pipeline_submit.  Consecutive calls alternate the two scratch
+ * lanes like submitted steps, so two batches can be in flight; `stream` waits for the call's outputs, and wav_dev must stay
+ * valid until then.  The sinc front end follows the hop hint (dg_pipeline_set_hop).  DG_EINVAL, with nothing launched, for bad
+ * arguments or while submitted steps are outstanding. */
+int dg_pipeline_nets_sets(dg_pipeline* h, const float* wav_dev, int B, int S, int num_sets, const float* osp_host,
+                          const int32_t* normalize_host, float* seg_dev, float* emb_dev, int64_t emb_set_stride, void* stream);
 int dg_pipeline_destroy(dg_pipeline* h);
 
 /* ---- post-path of SpeakerDiarization.__call__ on the device (reference src/diart/blocks/diarization.py:205-232):
@@ -241,6 +252,13 @@ int dg_sweep_destroy(dg_sweep* h);
  *      latencies), else DG_EINVAL before any launch.  Host only (the pieces travel with the next scoring call). ---- */
 int dg_sweep_set_scored_regions(dg_sweep* h, int num_files, const double* rows_host, const int32_t* offsets_host);
 int dg_vad_sweep_set_scored_regions(dg_vad_sweep* h, int num_files, const double* rows_host, const int32_t* offsets_host);
+/* ---- dg_sweep_set_trial_sets: sweeps over overlap-aware weightings (dg_pipeline_nets_sets).  For the handle's later
+ *      dg_sweep_run* / dg_sweep_score* calls emb_dev is [num_sets][N][K][D] (the embeddings of every set over the same
+ *      chunks), and trial t's clustering reads set trial_set_host[t] (int32 [T], each in [0, num_sets)); the post-path and the
+ *      scoring read only the scores and maps and are unchanged.  Every such call must run exactly T trials, else DG_EINVAL
+ *      before any launch.  num_sets = 0 clears them (the default: emb_dev is [N][K][D]).  DG_EINVAL for an index out of range
+ *      or num_sets outside 0..64, and the previous state stays.  Host only. ---- */
+int dg_sweep_set_trial_sets(dg_sweep* h, int num_sets, const int32_t* trial_set_host, int T);
 /* ---- dg_sweep_score: the same clustering and post-path as dg_sweep_run, then each trial's diarization error rate components
  *      against one reference (DiarizationErrorRate, the metric of the reference's Benchmark.evaluate; definition in
  *      DESIGN.md "DER scoring"): collar=0, skip_overlap=False and no uem, or, with scored regions set
