@@ -53,6 +53,7 @@ SIGNATURES = {
     "dg_seg_debug_stage": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int64, _P]),
     "dg_emb_debug_stage": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int64, _P]),
     "dg_selftest_sinc_filters_host": (C.c_int, [_P, _P, _P]),
+    "dg_selftest_fbank_tables_host": (C.c_int, [_P, _P]),
     "dg_osp": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_int, _P, _P]),
     "dg_normalize_embeddings": (C.c_int, [_P, C.c_int, C.c_int, C.c_float, _P, _P]),
     "dg_cluster_create": (C.c_int, [C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, C.POINTER(_P)]),

@@ -32,8 +32,9 @@ struct ResNet {
   DevBuf banks, k_lo, k_hi, stem_w, stem_sc, stem_sh;
   std::vector<ResBlock> blocks;
   int stage_of[16];
-  // work buffers: planes of the waveform, spectrum, log-mel map, three plane pairs per stage, float32 final map
-  DevBuf wav_hi, wav_lo, spec, logmel, mean, act[4][3][2], fin;
+  // work buffers: planes of the waveform, 1 / their scale per item and the level of its constant 80-sample pieces, spectrum,
+  // log-mel map, three plane pairs per stage, float32 final map
+  DevBuf wav_hi, wav_lo, inv_s, level, spec, logmel, mean, act[4][3][2], fin;
   int last_S = 0;                // the padding rings are only valid for one geometry: buffers are cleared when it changes
   int stop_after = 99;           // test hook (dg_emb_debug_trunk): stop after the stem (-1) / after block k
   int dbg_stage = 0, dbg_buf = 0;
@@ -261,7 +262,8 @@ static int resnet_trunk(dg_emb* h, const float* wav, int U, int S, cudaStream_t 
   const long long n = (long long)U * S;
   if (r.wav_hi.ensure(((size_t)n + 1024) * 2) || r.wav_lo.ensure(((size_t)n + 1024) * 2) ||
       r.spec.ensure(((size_t)U * rpi + 128) * 640 * 4) || r.logmel.ensure((size_t)U * g.T0 * 80 * 4) ||
-      r.mean.ensure((size_t)U * 80 * 4))
+      r.mean.ensure((size_t)U * 80 * 4) || r.inv_s.ensure((size_t)U * 4) ||
+      r.level.ensure((size_t)U * (S / 80) * 4))
     return DG_ECUDA;
   for (int s = 0; s < 4; s++) {
     const size_t rows = (size_t)U * (g.W[s] + 2) * (g.H[s] + 2) + 256;      // + tail: overlapping-row reads of the last rows
@@ -277,8 +279,8 @@ static int resnet_trunk(dg_emb* h, const float* wav, int U, int S, cudaStream_t 
           for (int p = 0; p < 2; p++) DG_CUDA(cudaMemsetAsync(r.act[s][b][p].p, 0, r.act[s][b][p].bytes, st));
     r.last_S = S;
   }
-  // ---- kaldi fbank: planes of x * 2^15, [rows, 448] x [448, 640] on the tensor cores, power -> mel -> log, time mean
-  if ((rc = launch_fb_planes(wav, n, r.wav_hi.p, r.wav_lo.p, st))) return rc;
+  // ---- kaldi fbank: planes of s (x * 2^15 - p), [rows, 448] x [448, 640] on the tensor cores, power -> mel -> log, time mean
+  if ((rc = launch_fb_planes(wav, U, S, r.wav_hi.p, r.wav_lo.p, r.inv_s.as<float>(), r.level.as<float>(), st))) return rc;
   {
     TcGemm t{};
     t.A_hi = r.wav_hi.p; t.A_lo = r.wav_lo.p; t.lda = 160; t.Cin = 448; t.KW = 1; t.dil = 1;
@@ -286,8 +288,8 @@ static int resnet_trunk(dg_emb* h, const float* wav, int U, int S, cudaStream_t 
     t.N = 640; t.out_f32 = r.spec.as<float>(); t.ldc = 640; t.epi = 0; t.tag = "fbank_dft";
     if ((rc = set_weights(t, r.fb)) || (rc = launch_gemm_tc(t, st))) return rc;
   }
-  if ((rc = launch_fb_mel(r.spec.as<float>(), 640, rpi, g.T0, U, r.banks.as<float>(), r.k_lo.as<int>(), r.k_hi.as<int>(),
-                          r.logmel.as<float>(), st)) ||
+  if ((rc = launch_fb_mel(r.spec.as<float>(), 640, rpi, g.T0, U, r.inv_s.as<float>(), r.level.as<float>(), r.banks.as<float>(),
+                          r.k_lo.as<int>(), r.k_hi.as<int>(), r.logmel.as<float>(), st)) ||
       (rc = launch_fb_mean(r.logmel.as<float>(), U, g.T0, r.mean.as<float>(), st)) ||
       (rc = launch_rn_stem(r.logmel.as<float>(), r.mean.as<float>(), U, g.T0, r.stem_w.as<float>(), r.stem_sc.as<float>(),
                            r.stem_sh.as<float>(), r.act[0][0][0].p, r.act[0][0][1].p, st)))
@@ -382,6 +384,20 @@ extern "C" int dg_emb_debug_trunk(dg_emb* h, const float* wav_dev, int U, int S,
     for (int w = 0; w < W; w++)
       for (int hh = 0; hh < H; hh++)
         memcpy(out_host + (((size_t)u * W + w) * H + hh) * C, &full[(((size_t)u * Wp + w + 1) * Hp + hh + 1) * C], (size_t)C * 4);
+  return DG_OK;
+}
+
+extern "C" int dg_selftest_fbank_tables_host(float* frame_operator, float* mel_banks) {
+  if (!frame_operator || !mel_banks) {
+    set_error("dg_selftest_fbank_tables_host: null argument");
+    return DG_EINVAL;
+  }
+  std::vector<float> op, banks;
+  std::vector<int> lo, hi;
+  fbank_frame_operator(op);
+  fbank_mel_banks(banks, lo, hi);
+  memcpy(frame_operator, op.data(), op.size() * sizeof(float));
+  memcpy(mel_banks, banks.data(), banks.size() * sizeof(float));
   return DG_OK;
 }
 

@@ -452,10 +452,11 @@ extern "C" int dg_seg_forward(dg_seg* h, const float* wav, int B, int S, float* 
 // host-side stop point, and one intermediate map copied to the host
 extern "C" int dg_seg_debug_stage(dg_seg* h, const float* wav_dev, int B, int S, int hop, int stage, float* out_host, int64_t cap,
                                   int* dims) {
-  if (!h || !wav_dev || !out_host || !dims || B < 1 || S < 3000 || hop < 0 || stage < 0 || stage > 10 || h->ps_speakers) {
-    set_error("dg_seg_debug_stage: bad arguments (need a multilabel segmentation handle, B >= 1, S >= 3000, stage 0..10)");
+  if (!h || !wav_dev || !out_host || !dims || B < 1 || S < 3000 || hop < 0 || stage < 0 || stage > 10) {
+    set_error("dg_seg_debug_stage: bad arguments (need a segmentation handle, B >= 1, S >= 3000, stage 0..10)");
     return DG_EINVAL;
   }
+  const int speakers = h->ps_speakers ? h->ps_speakers : h->K;     // columns of the scores (powerset: decoded labels)
   DG_CUDA(cudaSetDevice(h->device));
   const Geom g = make_geom(S);
   const char* who = "dg_seg_debug_stage";
@@ -464,7 +465,7 @@ extern "C" int dg_seg_debug_stage(dg_seg* h, const float* wav_dev, int B, int S,
   const SincPrep* prep = nullptr;
   DevBuf seg;
   int rc;
-  if (seg.ensure((size_t)B * g.T2 * h->K * 4)) return DG_ECUDA;
+  if (seg.ensure((size_t)B * g.T2 * speakers * 4)) return DG_ECUDA;
   {
     LaneUse use(h->guard[0], h, st);
     if ((rc = use.rc)) return rc;
@@ -483,7 +484,7 @@ extern "C" int dg_seg_debug_stage(dg_seg* h, const float* wav_dev, int B, int S,
   if (stage <= 7) return debug_copy_map(who, w.xh.p, w.xl.p, B, g.S2, 256, g.T2, 256, out_host, cap, dims);
   if (stage == 8) return debug_copy_map(who, w.y1h.p, w.y1l.p, B, g.S2, 128, g.T2, 128, out_host, cap, dims);
   if (stage == 9) return debug_copy_map(who, w.y2.p, nullptr, B, g.S2, 128, g.T2, 128, out_host, cap, dims);
-  return debug_copy_map(who, seg.p, nullptr, B, g.T2, h->K, g.T2, h->K, out_host, cap, dims);
+  return debug_copy_map(who, seg.p, nullptr, B, g.T2, speakers, g.T2, speakers, out_host, cap, dims);
 }
 
 extern "C" int dg_seg_destroy(dg_seg* h) {

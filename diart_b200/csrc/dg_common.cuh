@@ -248,9 +248,11 @@ int launch_l2norm(const float* in, int rows, int D, float norm, float* out, cuda
 int launch_row_equal_flags(const float* wav, int N, int S, int* flags, cudaStream_t st);
 int launch_gather_rows(const float* src, const int* index, int rows, int cols, float* dst, cudaStream_t st);
 // resnet.cu -- variant B of the embedding (WeSpeaker ResNet34): fbank front end and stem around the Conv2d GEMMs
-int launch_fb_planes(const float* wav, long long n, void* hi, void* lo, cudaStream_t st);
-int launch_fb_mel(const float* spec, int ld, int rows_per_item, int T, int B, const float* banks, const int* k_lo, const int* k_hi,
-                  float* logmel, cudaStream_t st);
+// planes of s_b (x * 2^15 - p_b) per item b, with p_b and s_b from the item's range; inv_scale [B] receives 1 / s_b, level
+// [B][S / 80] the value of every constant 80-sample piece (NaN for the others)
+int launch_fb_planes(const float* wav, int B, int S, void* hi, void* lo, float* inv_scale, float* level, cudaStream_t st);
+int launch_fb_mel(const float* spec, int ld, int rows_per_item, int T, int B, const float* inv_scale, const float* level,
+                  const float* banks, const int* k_lo, const int* k_hi, float* logmel, cudaStream_t st);
 int launch_fb_mean(const float* logmel, int B, int T, float* mean, cudaStream_t st);
 int launch_rn_stem(const float* logmel, const float* mean, int B, int T, const float* w, const float* sc, const float* sh,
                    void* hi, void* lo, cudaStream_t st);

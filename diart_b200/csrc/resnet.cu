@@ -22,37 +22,93 @@
 
 namespace dg {
 
-// waveform [B, S] float32 -> hi / lo fp16 planes of x * 2^15 (what pyannote feeds kaldi.fbank), [B * S (+ tail zeros)]
-__global__ void __launch_bounds__(256) fb_planes_kernel(const float* __restrict__ wav, long long n, uint16_t* __restrict__ hi,
-                                                        uint16_t* __restrict__ lo) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < (n >> 2); i += (long long)gridDim.x * blockDim.x) {
-    const float4 v = reinterpret_cast<const float4*>(wav)[i];
+// waveform [B, S] float32 -> hi / lo fp16 planes of s_b (x * 2^15 - p_b), [B * S (+ tail)], and 1 / s_b; one block per item.
+// The pair keeps 22 bits of what it is given and saturates at 65504.  Given x * 2^15 (what pyannote feeds kaldi.fbank) it
+// spends those bits on a DC offset that the frame operator then has to cancel -- rounded to fp16 pairs the operator does not
+// annihilate a constant, so a constant stretch at 0.5 gave bins near -5 instead of the floor log(eps) -- and it clips above
+// |x| = 4.  p_b is the midpoint of the item's range and s_b the power of two that puts max |x * 2^15 - p_b| in [2^14, 2^15):
+// the operator annihilates constants, so p_b drops out of the spectrum (a constant item splits into exact zeros, and each
+// frame sees only its own item's pivot), and fb_mel divides s_b back out before the power spectrum.  A constant stretch
+// inside an item (digital silence before speech) is not at p_b: `level` [B][S / 80] receives the value of every 80-sample
+// piece that is constant, NaN for the others, and fb_mel gives a frame whose five pieces hold one value the floor, which is
+// what DC removal leaves of it in exact arithmetic.
+__global__ void __launch_bounds__(1024) fb_planes_kernel(const float* __restrict__ wav, int S, uint16_t* __restrict__ hi,
+                                                         uint16_t* __restrict__ lo, float* __restrict__ inv_scale,
+                                                         float* __restrict__ level) {
+  __shared__ float red_mn[32], red_mx[32];
+  __shared__ float piv[2];
+  const int b = blockIdx.x, n4 = S >> 2;
+  const float4* x = reinterpret_cast<const float4*>(wav + (size_t)b * S);
+  float mn = INFINITY, mx = -INFINITY;
+  for (int i = threadIdx.x; i < n4; i += blockDim.x) {
+    const float4 v = x[i];
+    mn = fminf(mn, fminf(fminf(v.x, v.y), fminf(v.z, v.w)));
+    mx = fmaxf(mx, fmaxf(fmaxf(v.x, v.y), fmaxf(v.z, v.w)));
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  }
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, warps = blockDim.x >> 5;
+  if (lane == 0) {
+    red_mn[warp] = mn;
+    red_mx[warp] = mx;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < warps; w++) {
+      mn = fminf(mn, red_mn[w]);
+      mx = fmaxf(mx, red_mx[w]);
+    }
+    const float p = (0.5f * mn + 0.5f * mx) * 32768.f;          // = the level itself when the item is constant
+    const float r = fmaxf(mx * 32768.f - p, p - mn * 32768.f);  // the largest |x * 2^15 - p| of the item, rounded as below
+    int e = 0;
+    if (r > 0.f) frexpf(r, &e);                                 // r < 2^e
+    e = min(max(e, -100), 115);
+    piv[0] = p;
+    piv[1] = ldexpf(1.f, 15 - e);
+    inv_scale[b] = ldexpf(1.f, e - 15);
+  }
+  __syncthreads();
+  const float p = piv[0], s = piv[1];
+  uint2* ho = reinterpret_cast<uint2*>(hi + (size_t)b * S);
+  uint2* lw = reinterpret_cast<uint2*>(lo + (size_t)b * S);
+  const int pieces = S / 80;                                    // one warp per piece: lanes 0..19 hold its 20 float4
+  for (int q = warp; q < pieces; q += warps) {
+    const int i = q * 20 + lane;
+    const float4 v = lane < 20 ? x[i] : make_float4(0.f, 0.f, 0.f, 0.f);
+    const float v0 = __shfl_sync(0xffffffffu, v.x, 0);
+    const bool same = lane >= 20 || (v.x == v0 && v.y == v0 && v.z == v0 && v.w == v0);
+    const bool flat = __all_sync(0xffffffffu, same);
+    if (lane == 0) level[(size_t)b * pieces + q] = flat ? v0 : __int_as_float(0x7fc00000);
+    if (lane >= 20) continue;
     uint16_t h0, h1, h2, h3, l0, l1, l2, l3;
-    split_h16(v.x * 32768.f, h0, l0);
-    split_h16(v.y * 32768.f, h1, l1);
-    split_h16(v.z * 32768.f, h2, l2);
-    split_h16(v.w * 32768.f, h3, l3);
-    reinterpret_cast<uint2*>(hi)[i] = make_uint2(pack_u16x2(h0, h1), pack_u16x2(h2, h3));
-    reinterpret_cast<uint2*>(lo)[i] = make_uint2(pack_u16x2(l0, l1), pack_u16x2(l2, l3));
+    split_h16((v.x * 32768.f - p) * s, h0, l0);
+    split_h16((v.y * 32768.f - p) * s, h1, l1);
+    split_h16((v.z * 32768.f - p) * s, h2, l2);
+    split_h16((v.w * 32768.f - p) * s, h3, l3);
+    ho[i] = make_uint2(pack_u16x2(h0, h1), pack_u16x2(h2, h3));
+    lw[i] = make_uint2(pack_u16x2(l0, l1), pack_u16x2(l2, l3));
   }
 }
 
-int launch_fb_planes(const float* wav, long long n, void* hi, void* lo, cudaStream_t st) {
+int launch_fb_planes(const float* wav, int B, int S, void* hi, void* lo, float* inv_scale, float* level, cudaStream_t st) {
   ProfScope _ps("fbank_planes", st);
-  if (n % 4) {
-    set_error("fbank: sample count must be a multiple of 4");
+  if (S % 80) {
+    set_error("fbank: sample count must be a multiple of 80");
     return -1;
   }
-  const long long want = ((n >> 2) + 255) / 256;
-  const long long cap = usable_sms() * 16LL;
-  fb_planes_kernel<<<(int)(want < cap ? want : cap), 256, 0, st>>>(wav, n, reinterpret_cast<uint16_t*>(hi),
-                                                                             reinterpret_cast<uint16_t*>(lo));
+  fb_planes_kernel<<<B, 1024, 0, st>>>(wav, S, reinterpret_cast<uint16_t*>(hi), reinterpret_cast<uint16_t*>(lo), inv_scale,
+                                       level);
   DG_LAUNCHED();
   return 0;
 }
 
-// spectrum rows [B * rows_per_item][ld] (re 0..256 | im 257..513) -> log mel energies [B][T][80]; one warp per frame
+// spectrum rows [B * rows_per_item][ld] (re 0..256 | im 257..513) of item b scaled by s_b -> log mel energies [B][T][80]; one
+// warp per frame.  1 / s_b is a power of two, so re / s_b and im / s_b are exact: the eps clamp sees the unscaled energies.
+// A frame whose 400 samples are one value (`level`, fb_planes) has no energy: the floor.
 __global__ void __launch_bounds__(256) fb_mel_kernel(const float* __restrict__ spec, int ld, int rows_per_item, int T, int B,
+                                                     const float* __restrict__ inv_scale, const float* __restrict__ level,
                                                      const float* __restrict__ banks /*[80][257]*/, const int* __restrict__ k_lo,
                                                      const int* __restrict__ k_hi, float* __restrict__ logmel) {
   __shared__ float pw[8][260];
@@ -61,8 +117,11 @@ __global__ void __launch_bounds__(256) fb_mel_kernel(const float* __restrict__ s
   if (frame >= (long long)B * T) return;
   const int b = (int)(frame / T), t = (int)(frame - (long long)b * T);
   const float* row = spec + ((size_t)b * rows_per_item + t) * ld;
+  const float inv = inv_scale[b];
+  const float* lv = level + (size_t)b * 2 * rows_per_item + 2 * t;        // frame t = 80-sample pieces 2t .. 2t + 4
+  const bool flat = lv[0] == lv[1] && lv[0] == lv[2] && lv[0] == lv[3] && lv[0] == lv[4];     // false on NaN
   for (int k = lane; k < 257; k += 32) {
-    const float re = row[k], im = row[257 + k];
+    const float re = row[k] * inv, im = row[257 + k] * inv;
     pw[warp][k] = re * re + im * im;
   }
   __syncwarp();
@@ -70,15 +129,17 @@ __global__ void __launch_bounds__(256) fb_mel_kernel(const float* __restrict__ s
     float acc = 0.f;
     const float* bk = banks + m * 257;
     for (int k = k_lo[m]; k < k_hi[m]; k++) acc = fmaf(bk[k], pw[warp][k], acc);
+    if (flat) acc = 0.f;
     logmel[(size_t)frame * 80 + m] = logf(fmaxf(acc, 1.1920928955078125e-07f));     // max(mel, float32 eps)
   }
 }
 
-int launch_fb_mel(const float* spec, int ld, int rows_per_item, int T, int B, const float* banks, const int* k_lo, const int* k_hi,
-                  float* logmel, cudaStream_t st) {
+int launch_fb_mel(const float* spec, int ld, int rows_per_item, int T, int B, const float* inv_scale, const float* level,
+                  const float* banks, const int* k_lo, const int* k_hi, float* logmel, cudaStream_t st) {
   ProfScope _ps("fbank_mel", st);
   const long long frames = (long long)B * T;
-  fb_mel_kernel<<<(int)((frames + 7) / 8), 256, 0, st>>>(spec, ld, rows_per_item, T, B, banks, k_lo, k_hi, logmel);
+  fb_mel_kernel<<<(int)((frames + 7) / 8), 256, 0, st>>>(spec, ld, rows_per_item, T, B, inv_scale, level, banks, k_lo, k_hi,
+                                                         logmel);
   DG_LAUNCHED();
   return 0;
 }

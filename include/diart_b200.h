@@ -98,7 +98,8 @@ int dg_emb_debug_trunk(dg_emb* h, const float* wav_dev, int U, int S, int stop_a
  * hop > 0: the front end runs as under dg_pipeline_set_hop(hop) (stream form of the sinc layer when the device finds the batch
  * a run of overlapping windows); hop = 0: the per-window form.  Stages shared by both: 0 operand of conv1 [B][T0][80],
  * 1 operand of conv2 [B][T1][60], 2 operand of the LSTM / TDNN1 [B][T2][60], 3 waveform mean and rstd [2][B].
- * dg_seg_debug_stage: 4..7 output of LSTM layer 0..3 [B][T2][256], 8 / 9 the two Linears [B][T2][128], 10 scores [B][T2][K].
+ * dg_seg_debug_stage: 4..7 output of LSTM layer 0..3 [B][T2][256], 8 / 9 the two Linears [B][T2][128], 10 scores [B][T2][K]
+ * (powerset handles: the decoded {0, 1} labels [B][T2][num_speakers]).
  * dg_emb_debug_stage: 4..7 TDNN1..4 [B][T][512], 8 TDNN5 [B][T][1500], 9 / 10 pooled statistics [B*K][3000] from the fused /
  * un-fused pooling, 11 / 12 the raw embedding [B*K][D] behind either; weights_dev [B][F][K] is read from stage 9 on.
  * dims receives the three extents and, in dims[3], the paths taken: 1 stream form, 2 MaxPool1d(3) fused into conv1 / conv2,
@@ -582,6 +583,9 @@ int dg_selftest_split_f16_host(const float* x, long long n, unsigned short* hi, 
 /* the ParamSincFB filter table the models are built with, from low_hz_ [40] and band_hz_ [40]: filters [251][80] (tap-major;
  * 40 cosine then 40 sine filters); host only */
 int dg_selftest_sinc_filters_host(const float* low_hz, const float* band_hz, float* filters);
+/* the kaldi fbank tables variant-B models are built with: frame_operator [514][400] (DC removal, pre-emphasis, Hamming window
+ * and the 512-point real DFT; rows 0..256 real, 257..513 imaginary part) and mel_banks [80][257]; host only */
+int dg_selftest_fbank_tables_host(float* frame_operator, float* mel_banks);
 int dg_profile_report(char* buf, int cap);
 
 /* ---- shared-identity mode (extension beyond the reference; SURVEY.md 8(e), BASELINE config 5): G ranks diarize

@@ -349,13 +349,17 @@ class WeSpeakerResNet34(_Reproducible, nn.Module):
         self.sample_rate = sample_rate
         self.resnet = _ResNet34(pool_mode=pool_mode)
 
-    def compute_fbank(self, waveforms: torch.Tensor) -> torch.Tensor:
+    def log_mel(self, waveforms: torch.Tensor) -> torch.Tensor:
+        """waveforms (N, 1, S) -> kaldi log mel energies (N, T, 80), before the mean normalisation"""
         from torchaudio.compliance import kaldi
 
         x = waveforms * (1 << 15)
-        feats = torch.stack([kaldi.fbank(w, num_mel_bins=80, frame_length=25, frame_shift=10, dither=0.0,
-                                         sample_frequency=self.sample_rate, window_type="hamming", use_energy=False)
-                             for w in x])                           # (N, 498, 80) for 80 000 samples
+        return torch.stack([kaldi.fbank(w, num_mel_bins=80, frame_length=25, frame_shift=10, dither=0.0,
+                                        sample_frequency=self.sample_rate, window_type="hamming", use_energy=False)
+                            for w in x])                            # (N, 498, 80) for 80 000 samples
+
+    def compute_fbank(self, waveforms: torch.Tensor) -> torch.Tensor:
+        feats = self.log_mel(waveforms)
         return feats - feats.mean(dim=1, keepdim=True)
 
     def forward(self, waveforms: torch.Tensor, weights: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -398,12 +402,15 @@ def make_wespeaker(seed: int = 2468, pool_mode: str = "3.1") -> WeSpeakerResNet3
 def float64_copy(net: nn.Module) -> nn.Module:
     """`net` in float64 -- except the sinc filters: ParamSincFB.filters() is DEFINED by its float32 evaluation (the CUDA path
     builds the same float32 table, tests/test_net_stages_host.py compares the two), so the copy convolves with the float32
-    filters cast up.  Stage 0 then measures the convolution, not the construction of the filters."""
+    filters cast up.  Stage 0 then measures the convolution, not the construction of the filters.  WeSpeakerResNet34 has no
+    sinc layer; its kaldi fbank likewise builds the mel banks in float32 and casts them (torchaudio's definition)."""
     import copy
 
+    net64 = copy.deepcopy(net).double().eval()
+    if isinstance(net, WeSpeakerResNet34):
+        return net64
     with torch.no_grad():
         filters = net.sincnet.conv1d[0].filterbank.filters().double()
-    net64 = copy.deepcopy(net).double().eval()
     net64.sincnet.conv1d[0].filterbank.filters = lambda: filters
     return net64
 
@@ -436,8 +443,7 @@ def lstm_layers(lstm: nn.LSTM, x: torch.Tensor) -> list:
 
 def segmentation_stages(net: PyanNet, waveforms: torch.Tensor) -> dict:
     """waveforms (B, 1, S) -> the front-end maps, `lstm0..3` (B, T, 256), `linear0`, `linear1` (after LeakyReLU), `logits`,
-    `scores`"""
-    assert net.powerset_mapping is None
+    `scores`; a powerset net also gives `log_probabilities`, and its `scores` are the multilabel {0, 1} (B, T, speakers)"""
     with torch.no_grad():
         out = sincnet_stages(net.sincnet, waveforms)
         x = out["sinc_norm2"]
@@ -447,7 +453,11 @@ def segmentation_stages(net: PyanNet, waveforms: torch.Tensor) -> dict:
             x = F.leaky_relu(linear(x))
             out[f"linear{i}"] = x
         out["logits"] = net.classifier(x)
-        out["scores"] = torch.sigmoid(out["logits"])
+        if net.powerset_mapping is None:
+            out["scores"] = torch.sigmoid(out["logits"])
+        else:
+            out["log_probabilities"] = F.log_softmax(out["logits"], dim=-1)
+            out["scores"] = to_multilabel(out["log_probabilities"], net.powerset_mapping)
     return out
 
 
@@ -465,6 +475,31 @@ def embedding_stages(net: XVectorSincNet, waveforms: torch.Tensor, weights: Opti
             pooled = torch.stack([net.stats_pool(x, weights[:, :, k]) for k in range(weights.shape[2])], dim=1)
             out["stats_pool"] = pooled
             out["embedding"] = net.embedding(pooled)
+    return out
+
+
+def wespeaker_blocks(resnet: _ResNet34) -> list:
+    """the 16 BasicBlocks of the trunk, in order"""
+    return [blk for layer in (resnet.layer1, resnet.layer2, resnet.layer3, resnet.layer4) for blk in layer]
+
+
+def wespeaker_stages(net: WeSpeakerResNet34, waveforms: torch.Tensor, weights: Optional[torch.Tensor] = None) -> dict:
+    """waveforms (U, 1, S), weights (U, F, K) -> `logmel` (U, T, 80) before the mean normalisation, and `stem`, `block0` ..
+    `block15` as the CUDA path stores them (dg_emb_debug_trunk): (U, W, H, C) = (item, time, mel, channel); with weights the
+    raw `embedding` (U, K, 256)"""
+    with torch.no_grad():
+        feats = net.log_mel(waveforms)
+        out = {"logmel": feats}
+        r = net.resnet
+        x = (feats - feats.mean(dim=1, keepdim=True)).permute(0, 2, 1).unsqueeze(1)     # (U, 1, mel, time)
+        x = F.relu(r.bn1(r.conv1(x)))
+        out["stem"] = x.permute(0, 3, 2, 1)
+        for i, blk in enumerate(wespeaker_blocks(r)):
+            x = blk(x)
+            out[f"block{i}"] = x.permute(0, 3, 2, 1)
+        if weights is not None:
+            x = x.reshape(x.shape[0], x.shape[1] * x.shape[2], x.shape[3])
+            out["embedding"] = torch.stack([r.seg_1(r.pool(x, weights[:, :, k])) for k in range(weights.shape[2])], dim=1)
     return out
 
 

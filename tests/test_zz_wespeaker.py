@@ -1,10 +1,8 @@
 """Variant B of the embedding row (SURVEY.md 8(a) A8'): pyannote/wespeaker-voxceleb-resnet34-LM on the GPU -- kaldi fbank as a
 wgmma GEMM over an overlapping-row view of the waveform, ResNet34 as shifted-window Conv2d GEMMs on zero-padded channels-last
 maps (csrc/resnet.cu, TC_CONV2D epilogue of csrc/gemm_tc.cu) -- against the oracle restatement oracle.nets.WeSpeakerResNet34
-(pinned by parameter count and map sizes in tests/test_oracle_golden.py).  Bars: stage by stage 2e-4 of the map's scale,
-unit-norm embeddings 1e-4 (the bar of variant A)."""
-import ctypes as C
-
+(pinned by parameter count and map sizes in tests/test_oracle_golden.py).  Bar: unit-norm embeddings 1e-4 (the bar of
+variant A); the stages against float64 are in tests/test_zz_wespeaker_stages.py."""
 import numpy as np
 import pytest
 import torch
@@ -31,52 +29,6 @@ def test_variant_is_recognised_without_gpu():
     lib = _lib.lib()
     assert hasattr(lib, "dg_emb_debug_trunk")
     assert lib.dg_emb_debug_trunk(None, None, 1, 80000, 0, None, 0, None) == -1
-
-
-@pytest.mark.gpu
-def test_fbank_and_every_stage_match_the_oracle(wespeaker, audio, cuda_device):
-    from torchaudio.compliance import kaldi
-
-    lib = _lib.lib()
-    emb = models.B200EmbeddingLoader(wespeaker.state_dict())().to(cuda_device)
-    assert emb.dims(80000) == (63, 256)
-    x = audio.to(cuda_device)
-    dims = (C.c_int * 4)()
-
-    def stage(stop, numel):
-        out = np.empty(numel, np.float32)
-        _lib.check(lib.dg_emb_debug_trunk(emb.handle, x.data_ptr(), N, 80000, stop, out.ctypes.data, out.size, dims))
-        return out.reshape(tuple(dims))
-
-    with torch.no_grad():
-        raw = torch.stack([kaldi.fbank(w[None, :] * (1 << 15), num_mel_bins=80, frame_length=25, frame_shift=10, dither=0.0,
-                                       sample_frequency=16000, window_type="hamming", use_energy=False) for w in audio])
-        got = stage(-2, N * 498 * 80)[..., 0]
-        err = np.abs(got - raw.numpy()).max()
-        print(f"log-mel max abs err {err:.2e} (values in [{raw.min():.1f}, {raw.max():.1f}])")
-        assert err < 2e-3, "fbank"         # float32 FFT vs split-precision DFT on int16-scaled audio: log domain
-        r = wespeaker.resnet
-        fb = wespeaker.compute_fbank(audio[:, None, :])
-        cur = fb.permute(0, 2, 1).unsqueeze(1)
-        cur = torch.relu(r.bn1(r.conv1(cur)))
-        want = {-1: cur}
-        bi = 0
-        for layer in (r.layer1, r.layer2, r.layer3, r.layer4):
-            for blk in layer:
-                cur = blk(cur)
-                want[bi] = cur
-                bi += 1
-        failed = []
-        for stop in (-1, 0, 1, 2, 3, 4, 7, 8, 12, 13, 14, 15):
-            ref = want[stop].permute(0, 3, 2, 1).numpy()            # (N, C, mel, time) -> (N, time, mel, C)
-            got = stage(stop, ref.size)
-            assert got.shape == ref.shape, (stop, got.shape, ref.shape)
-            scale = np.abs(ref).max()
-            err = np.abs(got - ref).max() / scale
-            print(f"after {'stem' if stop < 0 else 'block %d' % stop}: shape {ref.shape}, max abs err / scale {err:.2e}")
-            if not err < 2e-4:
-                failed.append((stop, float(err)))
-        assert not failed, f"stages beyond the bar: {failed}"
 
 
 @pytest.mark.gpu
