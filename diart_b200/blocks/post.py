@@ -71,7 +71,7 @@ class DevicePostPath:
 
     # ------------------------------------------------------------------ results
     def buffers(self, B: int):
-        need = B * self.M * ((self.F + 1) // 2)
+        need = turn_capacity(B, self.M, self.F)
         if len(self._turns) < need:
             self._turns = np.empty(need, dtype=np.uint32)
         return np.empty((B, 4), dtype=np.int32), self._turns
@@ -97,6 +97,12 @@ class DevicePostPath:
                                                header.ctypes.data, turns.ctypes.data, len(turns), C.byref(n),
                                                _lib.stream_ptr(self.device)))
         return header, turns, n.value, out_start, out_res
+
+
+def turn_capacity(B: int, speakers: int, frames: int) -> int:
+    """the most turns B chunks can emit: up to frames + 1 output frames each (a stream's first chunk), every second one
+    starting a turn of every speaker"""
+    return B * speakers * ((frames + 2) // 2)
 
 
 def post_plan(starts: np.ndarray, res: float, hist_start: np.ndarray, hist_res: np.ndarray, nw: int, F: int, step: float,

@@ -674,25 +674,18 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
     return DG_EINVAL;
   }
   const int stride = 4 + h->nw;
-  // plan rows post.cu accepts: 1 <= nb <= the stream's nw buffers, none before the stream's first chunk, 1 <= frames, at most
-  // F + 1 output frames (the first chunk's crop of [0, region end))
+  int rc;
   for (const TickSlot& ts : act)
-    for (int i = 0; i < ts.n; i++) {
-      const int32_t* pl = plan_host + (size_t)(ts.row0 + i) * stride;
-      const int nb = pl[0], nf = pl[1], nfo = pl[2] > 0 ? pl[2] : nf;
-      if (nb < 1 || nb > ts.nw || nb - 1 > ts.n_hist + i || nf < 1 || pl[2] < 0 || nfo > h->F + 1) {
-        set_error(std::string(who) + ": plan row " + std::to_string(ts.row0 + i) + " is not a plan of its stream (buffers " +
-                  std::to_string(nb) + ", frames " + std::to_string(nfo) + ")");
-        return DG_EINVAL;
-      }
-    }
+    for (int i = 0; i < ts.n; i++)
+      if ((rc = check_plan_row(who, plan_host + (size_t)(ts.row0 + i) * stride, ts.row0 + i, ts.nw, ts.n_hist + i, h->F)))
+        return rc;
   if (n_turns) *n_turns = 0;
   if (B == 0) return DG_OK;     // nothing to do: staged samples wait for the next tick
   DG_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = h->st;
   const int F = h->F, K = h->K, D = h->D, M = h->M;
   const TurnOut lay = {0, (size_t)B * 16};
-  const int turn_cap = B * M * ((F + 2) / 2);   // every second output frame of every speaker starts a turn
+  const int turn_cap = post_turn_cap(B, M, F);
   if (h->seg.ensure((size_t)B * F * K * 4) || h->header.ensure(lay.header_bytes) || h->turns.ensure((size_t)turn_cap * 4) ||
       h->pin_out.ensure(lay.end()))
     return DG_ECUDA;
@@ -700,7 +693,6 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
                        h->prep.ensure(cluster_prep_floats(B, K) * 4 + 16) || h->prep_d.ensure(cluster_prep_doubles(B, K) * 8 + 16)))
     return DG_ECUDA;
   TickIn in;
-  int rc;
   if ((rc = tick_audio_in(h, tp, plan_host, in)) ||
       (rc = vad_mode(h) ? tick_vad(h, tp, in, turn_cap) : tick_diarize(h, tp, in, turn_cap)))
     return rc;

@@ -505,8 +505,8 @@ static bool post_fits(const dg_pipeline* h, const dg_post* post, const StepShape
   return sh.F == post->F && sh.K == post->K && h->clu->p.M == post->M && post->device == h->seg->device;
 }
 
-// end of dg_pipeline_call_host / _call_stream, with the batch's scores and maps in segd / mapd (ordered on h->st): post-path,
-// optional downloads, one synchronise (time stamp in *synced, if given), turn list
+// end of dg_pipeline_call_host / _call_stream, with the batch's scores and maps in segd / mapd (ordered on h->st) and the plan
+// rows checked at entry (post_check): post-path, optional downloads, one synchronise (time stamp in *synced, if given), turn list
 static int call_finish(dg_pipeline* h, dg_post* post, const StepShape& sh, const int32_t* plan_host, int32_t* header_host,
                        uint32_t* turns_host, int turn_cap_host, int* n_turns, float* seg_host, int32_t* map_host,
                        std::chrono::steady_clock::time_point* synced) {
@@ -537,6 +537,7 @@ extern "C" int dg_pipeline_call_host(dg_pipeline* h, dg_post* post, const float*
     set_error("dg_pipeline_call_host: submitted steps are outstanding; collect them first");
     return DG_EINVAL;
   }
+  if ((rc = post_check("dg_pipeline_call_host", post, B, plan_host))) return rc;
   DG_CUDA(cudaSetDevice(h->seg->device));
   // DG_CALL_TIMING=1: host wall-clock phases of the call on stderr (diagnostic)
   static const bool call_timing = getenv("DG_CALL_TIMING") && getenv("DG_CALL_TIMING")[0] == '1';
@@ -724,6 +725,7 @@ extern "C" int dg_pipeline_call_stream(dg_pipeline* h, dg_post* post, dg_stream*
     set_error("dg_pipeline_call_stream: handles were created for other dimensions / devices");
     return DG_EINVAL;
   }
+  if ((rc = post_check("dg_pipeline_call_stream", post, B, plan_host))) return rc;
   DG_CUDA(cudaSetDevice(h->seg->device));
   if (h->wav.ensure((size_t)B * S * 4) || h->segd.ensure(sh.seg_bytes()) || h->embd.ensure(sh.emb_bytes(h->emb->D)) ||
       h->mapd.ensure(sh.map_bytes()))

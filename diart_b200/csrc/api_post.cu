@@ -28,8 +28,40 @@ int download_turns(const char* who, const unsigned char* pin, const TurnOut& lay
   return DG_OK;
 }
 
-// pinned layout of a dg_post step over B chunks: plan [B][4 + nw], then header [B][4], turn count, turn prefix
-static TurnOut post_out(const dg_post* h, int B) { return {(size_t)B * (4 + h->nw) * 4, (size_t)B * 16}; }
+// ============================================================================= plan rows
+int check_plan_row(const char* who, const int32_t* pl, int row, int nw, int before, int F) {
+  const int nb = pl[0], nf = pl[1], nfo = pl[2] > 0 ? pl[2] : nf;
+  if (nb < 1 || nb > nw || nb - 1 > before || nf < 1 || pl[2] < 0 || nfo > std::min(F + 1, 1023)) {
+    set_error(std::string(who) + ": plan row " + std::to_string(row) + " is not a plan of its stream or file (buffers " +
+              std::to_string(nb) + ", frames " + std::to_string(nfo) + ")");
+    return DG_EINVAL;
+  }
+  return DG_OK;
+}
+
+// the plan rows of N chunks in nf files (chunk_off [nf + 1], checked), each file a fresh stream
+static int check_file_plans(const char* who, const int32_t* plan, int nf, const int32_t* chunk_off, int nw, int F) {
+  int rc;
+  for (int f = 0; f < nf; f++)
+    for (int c = chunk_off[f]; c < chunk_off[f + 1]; c++)
+      if ((rc = check_plan_row(who, plan + (size_t)c * (4 + nw), c, nw, c - chunk_off[f], F))) return rc;
+  return DG_OK;
+}
+
+int post_check(const char* who, const dg_post* h, int B, const int32_t* plan_host) {
+  int rc;
+  for (int c = 0; c < B; c++)
+    if ((rc = check_plan_row(who, plan_host + (size_t)c * (4 + h->nw), c, h->nw, h->n_hist + c, h->F))) return rc;
+  return DG_OK;
+}
+
+// ============================================================================= device post-path of one stream
+// A dg_post step is one stream in slot 0 of post_slots_kernel.  Pinned layout over B chunks: what travels to h->in in one
+// copy -- {tau, 0, 0} float64, the stream's TickSlot, rows [B] {0, c}, plan [B][4 + nw] -- then header [B][4], turn count,
+// turn prefix
+static const size_t POST_ROWS_AT = 24 + sizeof(TickSlot);
+static size_t post_in_bytes(const dg_post* h, int B) { return POST_ROWS_AT + (size_t)B * 8 + (size_t)B * (4 + h->nw) * 4; }
+static TurnOut post_out(const dg_post* h, int B) { return {post_in_bytes(h, B), (size_t)B * 16}; }
 
 extern "C" int dg_post_create(int frames, int local_speakers, int max_speakers, int num_windows, const double* hamming_host,
                               double tau, int device, dg_post** out) {
@@ -44,8 +76,8 @@ extern "C" int dg_post_create(int frames, int local_speakers, int max_speakers, 
   if (h->hamming.ensure((size_t)frames * 8) || h->total.ensure(16)) return DG_ECUDA;
   DG_CUDA(cudaMemcpy(h->hamming.p, hamming_host, (size_t)frames * 8, cudaMemcpyHostToDevice));
   const size_t hs = (size_t)std::max(1, num_windows - 1);
-  for (int i = 0; i < 2; i++)
-    if (h->hist_seg[i].ensure(hs * frames * local_speakers * 4) || h->hist_map[i].ensure(hs * local_speakers * 4)) return DG_ECUDA;
+  if (h->hist_seg.ensure(2 * hs * frames * local_speakers * 4) || h->hist_map.ensure(2 * hs * local_speakers * 4))
+    return DG_ECUDA;
   *out = h.release();
   return DG_OK;
 }
@@ -63,41 +95,46 @@ extern "C" int dg_post_destroy(dg_post* h) {
 
 static int post_ensure(dg_post* h, int B) {
   if (B <= h->cap_B) return 0;
-  const int stride = 4 + h->nw;
-  // worst case: every second frame of every speaker starts a turn
-  h->turn_cap = B * h->M * ((h->F + 1) / 2);
-  if (h->plan.ensure((size_t)B * stride * 4) || h->header.ensure((size_t)B * 16 + 16) ||
-      h->turns.ensure((size_t)h->turn_cap * 4))
+  h->turn_cap = post_turn_cap(B, h->M, h->F);
+  if (h->in.ensure(post_in_bytes(h, B)) || h->header.ensure((size_t)B * 16 + 16) || h->turns.ensure((size_t)h->turn_cap * 4))
     return DG_ECUDA;
   if (h->pin.ensure(post_out(h, B).end())) return DG_ECUDA;
   h->cap_B = B;
   return 0;
 }
 
-// enqueues plan upload, aggregation + binarisation + run-length kernel, history update and the D2H of the results on `st`
+// enqueues the upload, aggregation + binarisation + run-length kernel, history update and the D2H of the results on `st`
+// (plan rows checked by post_check)
 int post_enqueue(dg_post* h, const float* seg_dev, const int32_t* map_dev, int B, const int32_t* plan_host,
                  cudaStream_t st) {
   int rc;
   if ((rc = post_ensure(h, B))) return rc;
   const int stride = 4 + h->nw;
+  const size_t plan_at = POST_ROWS_AT + (size_t)B * 8;
   unsigned char* pin = h->pin.as<unsigned char>();
-  const size_t plan_bytes = (size_t)B * stride * 4;
-  memcpy(pin, plan_host, plan_bytes);
-  DG_CUDA(cudaMemcpyAsync(h->plan.p, pin, plan_bytes, cudaMemcpyHostToDevice, st));
+  const double params[3] = {h->tau, 0.0, 0.0};
+  const TickSlot ts{0, 0, B, h->cur, h->n_hist, h->nw, {0, 0}};
+  memcpy(pin, params, 24);
+  memcpy(pin + 24, &ts, sizeof ts);
+  int2* rows = reinterpret_cast<int2*>(pin + POST_ROWS_AT);
+  for (int c = 0; c < B; c++) rows[c] = make_int2(0, c);
+  memcpy(pin + plan_at, plan_host, (size_t)B * stride * 4);
+  unsigned char* din = h->in.as<unsigned char>();
+  DG_CUDA(cudaMemcpyAsync(din, pin, post_in_bytes(h, B), cudaMemcpyHostToDevice, st));
   DG_CUDA(cudaMemsetAsync(h->total.p, 0, 4, st));
-  if ((rc = launch_post(seg_dev, map_dev, h->hist_seg[h->cur].as<float>(), h->hist_map[h->cur].as<int32_t>(), h->n_hist, B,
-                        h->F, h->K, h->M, h->nw, h->plan.as<int32_t>(), stride, h->hamming.as<double>(), h->tau,
-                        h->header.as<int32_t>(), h->turns.as<uint32_t>(), h->turn_cap, h->total.as<unsigned int>(), st)))
+  const TickSlot* d_ts = reinterpret_cast<const TickSlot*>(din + 24);
+  if ((rc = launch_post_slots(seg_dev, map_dev, h->hist_seg.as<float>(), h->hist_map.as<int32_t>(), d_ts,
+                              reinterpret_cast<const int2*>(din + POST_ROWS_AT), 1, B, h->F, h->K, h->M, h->nw,
+                              reinterpret_cast<const int32_t*>(din + plan_at), stride, h->hamming.as<double>(),
+                              reinterpret_cast<const double*>(din), h->header.as<int32_t>(), h->turns.as<uint32_t>(),
+                              h->turn_cap, h->total.as<unsigned int>(), st)) ||
+      (rc = launch_post_slots_history(seg_dev, map_dev, h->hist_seg.as<float>(), h->hist_map.as<int32_t>(), d_ts, 1, 1, h->F,
+                                      h->K, h->nw, st)))
     return rc;
-  const int keep = std::min(h->nw - 1, h->n_hist + B);
-  if (keep > 0) {
-    if ((rc = launch_post_history(seg_dev, map_dev, h->hist_seg[h->cur].as<float>(), h->hist_map[h->cur].as<int32_t>(),
-                                  h->n_hist, B, h->F, h->K, keep, h->hist_seg[h->cur ^ 1].as<float>(),
-                                  h->hist_map[h->cur ^ 1].as<int32_t>(), st)))
-      return rc;
+  if (h->nw > 1) {
+    h->n_hist = std::min(h->nw - 1, h->n_hist + B);
     h->cur ^= 1;
   }
-  h->n_hist = keep;
   const TurnOut lay = post_out(h, B);
   DG_CUDA(cudaMemcpyAsync(pin + lay.at, h->header.p, lay.header_bytes, cudaMemcpyDeviceToHost, st));
   DG_CUDA(cudaMemcpyAsync(pin + lay.total(), h->total.p, 4, cudaMemcpyDeviceToHost, st));
@@ -119,9 +156,10 @@ extern "C" int dg_post_step(dg_post* h, const float* seg_dev, const int32_t* map
     set_error("dg_post_step: bad arguments");
     return DG_EINVAL;
   }
+  int rc;
+  if ((rc = post_check("dg_post_step", h, B, plan_host))) return rc;
   DG_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)stream;
-  int rc;
   if ((rc = post_enqueue(h, seg_dev, map_dev, B, plan_host, st))) return rc;
   DG_CUDA(cudaStreamSynchronize(st));
   return post_finish(h, B, header_host, turns_host, turn_cap_host, n_turns, st);
@@ -341,13 +379,13 @@ static TurnOut sweep_out(int S, int T, int N) { return {(size_t)S * 8, (size_t)T
 // header [T][N][4] and turns stay on the device (h->header, h->turns), the turn count comes back in *total.  with_header: the
 // header and a prefix of the turns travel to the pinned buffer in the same copy as the count (sweep_out layout).  The plan
 // is the files' plans, each that of a fresh stream, concatenated: a chunk's aggregated buffers are the nw - 1 chunks before
-// it at most, never those of the previous file (post.cu: chunk c reads chunks c - (nb - 1) .. c, nb <= its index in its file
-// + 1), so the post-path runs over all N chunks at once.  Synchronises `st`.
+// it at most, never those of the previous file (check_file_plans: chunk c reads chunks c - (nb - 1) .. c, nb <= its index in
+// its file + 1), so the post-path runs over all N chunks at once.  Synchronises `st`.
 //
 // With vchunk_host (the sweep over several latencies): the nf "files" are units, the clustering runs over them as above, and
 // the post-path runs over Nv virtual chunks instead, virtual chunk c being real chunk vchunk_host[c]; the plan [Nv][stride] and
-// the header [T][Nv][4] are over the virtual chunks (launch_post_virtual).  Without it Nv = N.  used [nf] (or null: all):
-// the units whose (unit, trial) states are clustered; the maps of the others' chunks are left unwritten.
+// the header [T][Nv][4] are over the virtual chunks.  Without it Nv = N, virtual chunk c being chunk c.  used [nf] (or null:
+// all): the units whose (unit, trial) states are clustered; the maps of the others' chunks are left unwritten.
 static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, int nf, const int32_t* chunk_off,
                               const double* params_host, int T, const int32_t* plan_host, int32_t* maps_dev,
                               double* centers_dev, bool with_header, cudaStream_t st, unsigned int* total_out,
@@ -431,14 +469,10 @@ static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* em
   for (int attempt = 0; attempt < 2; attempt++) {
     const int cap = (int)std::min<size_t>(h->turns.bytes / 4, (size_t)INT32_MAX);
     DG_CUDA(cudaMemsetAsync(h->total.p, 0, 4, st));
-    if (vchunk_host)
-      rc = launch_post_virtual(seg_dev, maps, N, reinterpret_cast<const int32_t*>(d_off + nf + 1), Nv, F, K, M, h->nw, d_plan,
-                               stride, h->hamming.as<double>(), d_taus, T, h->header.as<int32_t>(), h->turns.as<uint32_t>(), cap,
-                               h->total.as<unsigned int>(), st);
-    else
-      rc = launch_post(seg_dev, maps, nullptr, nullptr, 0, N, F, K, M, h->nw, d_plan, stride, h->hamming.as<double>(), 0.0,
-                       h->header.as<int32_t>(), h->turns.as<uint32_t>(), cap, h->total.as<unsigned int>(), st, d_taus, T);
-    if (rc) return rc;
+    if ((rc = launch_post_virtual(seg_dev, maps, N, vchunk_host ? reinterpret_cast<const int32_t*>(d_off + nf + 1) : nullptr, Nv,
+                                  F, K, M, h->nw, d_plan, stride, h->hamming.as<double>(), d_taus, T, h->header.as<int32_t>(),
+                                  h->turns.as<uint32_t>(), cap, h->total.as<unsigned int>(), st)))
+      return rc;
     DG_CUDA(cudaMemcpyAsync(pin, h->init.p, init_b, cudaMemcpyDeviceToHost, st));
     if (with_header) DG_CUDA(cudaMemcpyAsync(pin + lay.at, h->header.p, header_b, cudaMemcpyDeviceToHost, st));
     DG_CUDA(cudaMemcpyAsync(pin + lay.total(), h->total.p, 4, cudaMemcpyDeviceToHost, st));
@@ -470,7 +504,9 @@ static int sweep_run(const char* who, dg_sweep* h, const float* seg_dev, const f
     return DG_EINVAL;
   }
   int rc;
-  if ((rc = sweep_check(who, h, seg_dev, emb_dev, N, nf, chunk_off, params_host, T, plan_host))) return rc;
+  if ((rc = sweep_check(who, h, seg_dev, emb_dev, N, nf, chunk_off, params_host, T, plan_host)) ||
+      (rc = check_file_plans(who, plan_host, nf, chunk_off, h->nw, h->F)))
+    return rc;
   DG_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)stream;
   unsigned int total = 0;
@@ -662,6 +698,7 @@ static int sweep_score(const char* who, dg_sweep* h, const float* seg_dev, const
                        void* stream) {
   int rc;
   if ((rc = sweep_check(who, h, seg_dev, emb_dev, N, nf, chunk_off, params_host, T, plan_host)) ||
+      (rc = check_file_plans(who, plan_host, nf, chunk_off, h->nw, h->F)) ||
       (rc = score_check(who, N, nf, out_start_host, out_res_host, shift_host, collar, ref_host, ref_label_host, ref_off,
                         R_host, components_host, hyp_cap)) ||
       (rc = regions_check(who, h->regions, nf)))
@@ -710,9 +747,8 @@ extern "C" int dg_sweep_score_files(dg_sweep* h, const float* seg_dev, const flo
 
 // The virtual layout over N real chunks in nu units (unit_off [nu + 1]): virtual file v holds virtual chunks [voff[v],
 // voff[v + 1]) of Nv, which must be the real chunks u0, u0 + 1, ... of one unit starting at its first chunk u0, inside it; the
-// plan row [4 + nw] of its i-th virtual chunk aggregates 1 <= nb <= min(nw, i + 1) buffers (none before the unit's first
-// chunk) over 1 <= output frames <= min(F + 1, 1023) (the first chunk of a file emits up to F + 1; the post-path's shared
-// memory holds that many).  used (or null) receives [nu]: whether a virtual file starts at unit u.  Host only.
+// plan row [4 + nw] of its i-th virtual chunk is that of the i-th chunk of a fresh stream (check_plan_row).  used (or null)
+// receives [nu]: whether a virtual file starts at unit u.  Host only.
 static int check_virtual(const char* who, int N, int nu, const int32_t* unit_off, int Nv, int nvf, const int32_t* vchunk,
                          const int32_t* voff, const int32_t* plan, int nw, int F, std::vector<char>* used = nullptr) {
   if (N < 1 || nu < 1 || Nv < 1 || nvf < 1 || nw < 1 || F < 1 || !unit_off || !vchunk || !voff || !plan) {
@@ -722,7 +758,7 @@ static int check_virtual(const char* who, int N, int nu, const int32_t* unit_off
   }
   int rc;
   if ((rc = check_chunk_offsets(who, N, nu, unit_off)) || (rc = check_chunk_offsets(who, Nv, nvf, voff))) return rc;
-  const int stride = 4 + nw, max_frames = std::min(F + 1, 1023);
+  const int stride = 4 + nw;
   if (used) used->assign(nu, 0);
   for (int v = 0; v < nvf; v++) {
     const int a = voff[v], n = voff[v + 1] - a, c0 = vchunk[a];
@@ -741,13 +777,7 @@ static int check_virtual(const char* who, int N, int nu, const int32_t* unit_off
         set_error(std::string(who) + ": virtual file " + std::to_string(v) + " is not a run of consecutive chunks of its unit");
         return DG_EINVAL;
       }
-      const int32_t* pl = plan + (size_t)(a + i) * stride;
-      const int nb = pl[0], nfr = pl[1], nfo = pl[2] > 0 ? pl[2] : nfr;
-      if (nb < 1 || nb > nw || nb - 1 > i || nfr < 1 || pl[2] < 0 || nfo > max_frames) {
-        set_error(std::string(who) + ": plan row " + std::to_string(a + i) + " is not a plan of its virtual file (buffers " +
-                  std::to_string(nb) + ", frames " + std::to_string(nfo) + ")");
-        return DG_EINVAL;
-      }
+      if ((rc = check_plan_row(who, plan + (size_t)(a + i) * stride, a + i, nw, i, F))) return rc;
     }
   }
   return DG_OK;
@@ -875,6 +905,43 @@ extern "C" int dg_vad_sweep_set_scored_regions(dg_vad_sweep* h, int num_files, c
                             offsets_host);
 }
 
+// The curve of Nv chunks with checked plan rows over the scores seg, chunk c being real chunk vchunk_host[c] of seg (null:
+// chunk c); afterwards the handle's chunks and files are these, in nf files (file_off [nf + 1]).  Synchronises the stream.
+static int vad_curve(dg_vad_sweep* h, const float* seg_dev, int Nv, const int32_t* plan_host, const int32_t* vchunk_host, int nf,
+                     const int32_t* file_off, void* stream) {
+  const int stride = 4 + h->nw;
+  std::vector<long long> off(Nv + 1);
+  off[0] = 0;
+  for (int c = 0; c < Nv; c++) {
+    const int32_t* pl = plan_host + (size_t)c * stride;
+    off[c + 1] = off[c] + (pl[2] > 0 ? pl[2] : pl[1]);
+  }
+  DG_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  // host -> device, one copy: curve offsets [Nv + 1] (int64, first: vad_binarize_all reads them there), plan [Nv][stride],
+  // then with vchunk_host the chunk table [Nv]
+  const size_t off_b = (size_t)(Nv + 1) * 8, plan_b = (size_t)Nv * stride * 4, vchunk_b = vchunk_host ? (size_t)Nv * 4 : 0;
+  const size_t in_b = off_b + plan_b + vchunk_b;
+  if (h->in.ensure(in_b) || h->curve.ensure((size_t)off[Nv] * 8) || h->pin.ensure(in_b)) return DG_ECUDA;
+  unsigned char* pin = h->pin.as<unsigned char>();
+  memcpy(pin, off.data(), off_b);
+  memcpy(pin + off_b, plan_host, plan_b);
+  if (vchunk_host) memcpy(pin + off_b + plan_b, vchunk_host, vchunk_b);
+  unsigned char* din = h->in.as<unsigned char>();
+  DG_CUDA(cudaMemcpyAsync(din, pin, in_b, cudaMemcpyHostToDevice, st));
+  h->N = 0;   // no curve while it is being replaced
+  int rc;
+  if ((rc = launch_vad_curve_virtual(seg_dev, vchunk_host ? reinterpret_cast<const int32_t*>(din + off_b + plan_b) : nullptr, Nv,
+                                     h->F, h->K, reinterpret_cast<const int32_t*>(din + off_b), stride, h->hamming.as<double>(),
+                                     reinterpret_cast<const long long*>(din), h->curve.as<double>(), st)))
+    return rc;
+  DG_CUDA(cudaStreamSynchronize(st));
+  h->N = Nv;
+  h->nf = nf;
+  h->chunk_off.assign(file_off, file_off + nf + 1);
+  return DG_OK;
+}
+
 extern "C" int dg_vad_sweep_curve(dg_vad_sweep* h, const float* seg_dev, int N, int num_files,
                                   const int32_t* chunk_offsets_host, const int32_t* plan_host, void* stream) {
   const char* who = "dg_vad_sweep_curve";
@@ -883,42 +950,10 @@ extern "C" int dg_vad_sweep_curve(dg_vad_sweep* h, const float* seg_dev, int N, 
     return DG_EINVAL;
   }
   int rc;
-  if ((rc = check_chunk_offsets(who, N, num_files, chunk_offsets_host))) return rc;
-  const int stride = 4 + h->nw;
-  // the curve's offsets, and the plan rows post.cu would accept for a fresh stream per file: 1 <= nb <= nw buffers, none
-  // before the file's first chunk, 1 <= frames <= 1023 (the 10-bit frame fields of a turn)
-  std::vector<long long> off(N + 1);
-  off[0] = 0;
-  for (int f = 0, c = 0; f < num_files; f++)
-    for (; c < chunk_offsets_host[f + 1]; c++) {
-      const int32_t* pl = plan_host + (size_t)c * stride;
-      const int nb = pl[0], nf = pl[1], nfo = pl[2] > 0 ? pl[2] : nf;
-      if (nb < 1 || nb > h->nw || nb - 1 > c - chunk_offsets_host[f] || nf < 1 || pl[2] < 0 || nfo > 1023) {
-        set_error(std::string(who) + ": plan row " + std::to_string(c) + " is not a plan of its file (buffers " +
-                  std::to_string(nb) + ", frames " + std::to_string(nfo) + ")");
-        return DG_EINVAL;
-      }
-      off[c + 1] = off[c] + nfo;
-    }
-  DG_CUDA(cudaSetDevice(h->device));
-  cudaStream_t st = (cudaStream_t)stream;
-  // host -> device, one copy: curve offsets [N + 1] (int64), plan [N][stride]
-  const size_t off_b = (size_t)(N + 1) * 8, plan_b = (size_t)N * stride * 4;
-  if (h->in.ensure(off_b + plan_b) || h->curve.ensure((size_t)off[N] * 8) || h->pin.ensure(off_b + plan_b)) return DG_ECUDA;
-  unsigned char* pin = h->pin.as<unsigned char>();
-  memcpy(pin, off.data(), off_b);
-  memcpy(pin + off_b, plan_host, plan_b);
-  unsigned char* din = h->in.as<unsigned char>();
-  DG_CUDA(cudaMemcpyAsync(din, pin, off_b + plan_b, cudaMemcpyHostToDevice, st));
-  h->N = 0;   // no curve while it is being replaced
-  if ((rc = launch_vad_curve(seg_dev, N, h->F, h->K, reinterpret_cast<const int32_t*>(din + off_b), stride,
-                             h->hamming.as<double>(), reinterpret_cast<const long long*>(din), h->curve.as<double>(), st)))
+  if ((rc = check_chunk_offsets(who, N, num_files, chunk_offsets_host)) ||
+      (rc = check_file_plans(who, plan_host, num_files, chunk_offsets_host, h->nw, h->F)))
     return rc;
-  DG_CUDA(cudaStreamSynchronize(st));
-  h->N = N;
-  h->nf = num_files;
-  h->chunk_off.assign(chunk_offsets_host, chunk_offsets_host + num_files + 1);
-  return DG_OK;
+  return vad_curve(h, seg_dev, N, plan_host, nullptr, num_files, chunk_offsets_host, stream);
 }
 
 // The curve over the virtual layout of several latencies (check_virtual): the N real chunks of seg in units, the curve over the
@@ -933,41 +968,11 @@ extern "C" int dg_vad_sweep_curve_latencies(dg_vad_sweep* h, const float* seg_de
     set_error(std::string(who) + ": bad arguments (need a handle and scores)");
     return DG_EINVAL;
   }
-  const int Nv = num_virtual, nvf = num_virtual_files;
   int rc;
-  if ((rc = check_virtual(who, N, num_units, unit_offsets_host, Nv, nvf, vchunk_host, virtual_offsets_host, plan_host,
-                          h->nw, h->F)))
+  if ((rc = check_virtual(who, N, num_units, unit_offsets_host, num_virtual, num_virtual_files, vchunk_host,
+                          virtual_offsets_host, plan_host, h->nw, h->F)))
     return rc;
-  const int stride = 4 + h->nw;
-  std::vector<long long> off(Nv + 1);
-  off[0] = 0;
-  for (int c = 0; c < Nv; c++) {
-    const int32_t* pl = plan_host + (size_t)c * stride;
-    off[c + 1] = off[c] + (pl[2] > 0 ? pl[2] : pl[1]);
-  }
-  DG_CUDA(cudaSetDevice(h->device));
-  cudaStream_t st = (cudaStream_t)stream;
-  // host -> device, one copy: curve offsets [Nv + 1] (int64, first: vad_binarize_all reads them there), plan [Nv][stride],
-  // virtual chunk table [Nv]
-  const size_t off_b = (size_t)(Nv + 1) * 8, plan_b = (size_t)Nv * stride * 4, vchunk_b = (size_t)Nv * 4;
-  const size_t in_b = off_b + plan_b + vchunk_b;
-  if (h->in.ensure(in_b) || h->curve.ensure((size_t)off[Nv] * 8) || h->pin.ensure(in_b)) return DG_ECUDA;
-  unsigned char* pin = h->pin.as<unsigned char>();
-  memcpy(pin, off.data(), off_b);
-  memcpy(pin + off_b, plan_host, plan_b);
-  memcpy(pin + off_b + plan_b, vchunk_host, vchunk_b);
-  unsigned char* din = h->in.as<unsigned char>();
-  DG_CUDA(cudaMemcpyAsync(din, pin, in_b, cudaMemcpyHostToDevice, st));
-  h->N = 0;   // no curve while it is being replaced
-  if ((rc = launch_vad_curve_virtual(seg_dev, reinterpret_cast<const int32_t*>(din + off_b + plan_b), Nv, h->F, h->K,
-                                     reinterpret_cast<const int32_t*>(din + off_b), stride, h->hamming.as<double>(),
-                                     reinterpret_cast<const long long*>(din), h->curve.as<double>(), st)))
-    return rc;
-  DG_CUDA(cudaStreamSynchronize(st));
-  h->N = Nv;
-  h->nf = nvf;
-  h->chunk_off.assign(virtual_offsets_host, virtual_offsets_host + nvf + 1);
-  return DG_OK;
+  return vad_curve(h, seg_dev, num_virtual, plan_host, vchunk_host, num_virtual_files, virtual_offsets_host, stream);
 }
 
 // the argument checks of dg_vad_sweep_run_files / _score_files (before any launch)

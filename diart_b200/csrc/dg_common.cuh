@@ -289,22 +289,17 @@ int launch_cluster_sweep_sets(const ClusterParams& p, const double* trials_dev, 
                               double* centers, int* active, int* initialized, float* prep, double* prep_d, int32_t* maps,
                               cudaStream_t st);
 size_t cluster_prep_floats(int B, int K);
-// post.cu -- aggregation + binarisation + run-length turns (reference diarization.py:205-232)
-int launch_post(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map, int n_hist, int B,
-                int F, int K, int M, int nw, const int32_t* plan, int plan_stride, const double* hamming, double tau,
-                int32_t* header, uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st,
-                const double* taus = nullptr /*[T]: per-state thresholds, map [T][B][K], header [T][B][4]*/, int T = 1);
-// post.cu -- the sweep over several latencies: Nv virtual chunks, virtual chunk c = real chunk vchunk[c] of the N whose scores
-// seg [N][F][K] and maps [T][N][K] are given; header [T][Nv][4]; trial t thresholds at taus[t]
+// post.cu -- aggregation + binarisation + run-length turns (reference diarization.py:205-232) of the sweeps: Nv virtual chunks,
+// virtual chunk c = real chunk vchunk[c] (vchunk null: chunk c) of the N whose scores seg [N][F][K] and maps [T][N][K] are
+// given; header [T][Nv][4]; trial t thresholds at taus[t]
 int launch_post_virtual(const float* seg, const int32_t* map, int N, const int32_t* vchunk, int Nv, int F, int K, int M, int nw,
                         const int32_t* plan, int plan_stride, const double* hamming, const double* taus, int T,
                         int32_t* header, uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st);
 int launch_expand_windows(const float* ring, long long r0, int C, int hop, int S, int B, float* wav, cudaStream_t st);
-int launch_post_history(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map, int n_hist,
-                        int B, int F, int K, int keep, float* new_seg, int32_t* new_map, cudaStream_t st);
-// post.cu -- many live streams in one batch (dg_multi).  A piece of the staging upload: n samples at staged[src] belong at
-// absolute sample dst of slot `slot`.  A slot with windows in the batch: its n windows are rows [row0, row0 + n); its post-path
-// history is copy `cur` of the two, with n_hist chunks, of which it keeps at most nw - 1 (nw = its stream's latency / step).
+// post.cu -- live streams in one batch (dg_multi; dg_post is one stream).  A piece of the staging upload: n samples at
+// staged[src] belong at absolute sample dst of slot `slot`.  A slot with windows in the batch: its n windows are rows [row0,
+// row0 + n); its post-path history is copy `cur` of the two, with n_hist chunks, of which it keeps at most nw - 1 (nw = its
+// stream's latency / step).
 struct RingPiece {
   long long src, dst;
   int slot, n;
@@ -342,11 +337,9 @@ constexpr int DER_ROFF = 33;
 int launch_der_score(const int* hoff, const double* hseg, int nf, int T, int M, const int* roff, const int* R,
                      const double* rseg, double* comp, cudaStream_t st, const int* uoff = nullptr,
                      const double* useg = nullptr);
-// vad.cu -- VAD sweep: the speech curve of N chunks (max over K local speakers, aggregated as launch_post with one speaker;
-// chunk c's frames at curve [curve_off[c], curve_off[c + 1])), then per trial t the turns of curve > taus[t], header [T][N][4]
-int launch_vad_curve(const float* seg, int N, int F, int K, const int32_t* plan, int plan_stride, const double* hamming,
-                     const long long* curve_off, double* curve, cudaStream_t st);
-// the curve of Nv virtual chunks, virtual chunk c = real chunk vchunk[c] of seg
+// vad.cu -- VAD sweep: the speech curve of Nv chunks (max over K local speakers, aggregated as the post-path with one speaker;
+// chunk c's frames at curve [curve_off[c], curve_off[c + 1])), chunk c = real chunk vchunk[c] of seg (vchunk null: chunk c);
+// then per trial t the turns of curve > taus[t], header [T][N][4]
 int launch_vad_curve_virtual(const float* seg, const int32_t* vchunk, int Nv, int F, int K, const int32_t* plan, int plan_stride,
                              const double* hamming, const long long* curve_off, double* curve, cudaStream_t st);
 int launch_vad_binarize(const double* curve, const long long* curve_off, int N, int T, const double* taus, int32_t* header,

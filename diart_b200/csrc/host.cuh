@@ -337,11 +337,21 @@ int stream_expand(dg_stream* h, int B, float* wav_dev, cudaStream_t st);
 struct dg_post {
   int device = 0, F = 0, K = 0, M = 0, nw = 1;
   double tau = 0.5;
-  DevBuf hamming, hist_seg[2], hist_map[2], plan, header, turns, total;
+  DevBuf hamming, hist_seg, hist_map, in, header, turns, total;   // history [2][nw - 1] (copy `cur` holds n_hist chunks)
   int cur = 0, n_hist = 0, cap_B = 0;
   int turn_cap = 0;
-  PinnedBuf pin;                  // pinned staging: plan in, header + total + turn prefix out
+  PinnedBuf pin;                  // pinned staging: tau, slot, rows and plan in, header + total + turn prefix out
 };
+
+// The plan rows every post-path launch (post.cu, vad.cu) relies on, checked on the host before any launch.  Row `row` at pl
+// [4 + nw] aggregates 1 <= nb <= min(nw, before + 1) buffers, `before` being the chunks of its stream or file ahead of it (none
+// is read before the first), over nf >= 1 frames with first_nf >= 0, into at most min(F + 1, 1023) output frames (the first
+// chunk of a stream emits up to F + 1, which the post kernels' shared memory holds; a turn's frame fields have 10 bits).
+int check_plan_row(const char* who, const int32_t* pl, int row, int nw, int before, int F);
+// the B plan rows of a dg_post step, after the n_hist chunks of its history
+int post_check(const char* who, const dg_post* h, int B, const int32_t* plan_host);
+// the most turns B chunks of M speakers can emit: up to F + 1 output frames, every second one starting a turn
+inline int post_turn_cap(int B, int M, int F) { return B * M * ((F + 2) / 2); }
 
 int post_enqueue(dg_post* h, const float* seg_dev, const int32_t* map_dev, int B, const int32_t* plan_host, cudaStream_t st);
 int post_finish(dg_post* h, int B, int32_t* header_host, uint32_t* turns_host, int turn_cap_host, int* n_turns,

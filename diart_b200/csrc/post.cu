@@ -15,10 +15,9 @@
 // One CTA per chunk.  Output: per chunk {offset, count, frames} and a packed turn list (speaker << 20 | on << 10 | off),
 // each chunk's turns contiguous, ordered by speaker then time (the order Binarize emits them).
 //
-// A second grid dimension runs independent states over the same scores and plan (hyper-parameter sweep): CTA (c, t) reads
-// maps row block t ([B][K] at map + t B K), thresholds at taus[t] (NULL: `tau`, one state) and writes header row block t.  The
-// turns of all states share one counter; each state's headers locate its turns.  STATES = false compiles the single-state
-// form of the pipeline.
+// Two kernels run that body: post_slots_kernel over the chunks of live streams, each with its history (dg_post is one such
+// stream, dg_multi many), and post_virtual_kernel over the chunks of a sweep, without history, with a second grid dimension
+// for independent states (trials) over the same scores.  Every plan row they read has passed check_plan_row (api_post.cu).
 #include "dg_common.cuh"
 #include "post_agg.cuh"
 
@@ -104,38 +103,10 @@ __device__ __forceinline__ void post_chunk(const int32_t* __restrict__ pl, int c
   }
 }
 
-template <bool STATES>
-__global__ void __launch_bounds__(POST_THREADS)
-post_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map, const float* __restrict__ hist_seg,
-            const int32_t* __restrict__ hist_map, int n_hist, int B, int F, int K, int M, int nw,
-            const int32_t* __restrict__ plan, int plan_stride, const double* __restrict__ hamming, double tau,
-            const double* __restrict__ taus, int32_t* __restrict__ header /*[gridDim.y][B][4]*/, uint32_t* __restrict__ turns,
-            int turn_cap, unsigned int* __restrict__ total) {
-  const int c = blockIdx.x;
-  if constexpr (STATES) {
-    map += (size_t)blockIdx.y * B * K;
-    header += (size_t)blockIdx.y * B * 4;
-    tau = taus[blockIdx.y];
-  }
-  const int32_t* pl = plan + (size_t)c * plan_stride;
-  const int nb = pl[0], nf = pl[1], first_nf = pl[2], first_lo = pl[3];
-  // buffer j of this chunk = virtual chunk v = c - (nb - 1) + j; v < 0 lives in the history (last n_hist chunks seen)
-  auto buf_seg = [&](int j) -> const float* {
-    const int v = c - (nb - 1) + j;
-    return v >= 0 ? seg + (size_t)v * F * K : hist_seg + (size_t)(n_hist + v) * F * K;
-  };
-  auto buf_map = [&](int j) -> const int32_t* {
-    const int v = c - (nb - 1) + j;
-    return v >= 0 ? map + (size_t)v * K : hist_map + (size_t)(n_hist + v) * K;
-  };
-  post_chunk(pl, c, nb, nf, first_nf, first_lo, F, K, M, nw, hamming, tau, header, turns, turn_cap, total, buf_seg, buf_map);
-}
-
-// The sweep over several latencies (dg_sweep_*_latencies): CTA (c, t) is virtual chunk c of the gridDim.x and trial t.  The
-// scores seg [N][F][K] and maps [T][N][K] are over the N real chunks; virtual chunk c is real chunk vchunk[c], and buffer j of
-// its plan row the real chunk vchunk[c] - (nb - 1) + j (the host guarantees these lie in the virtual chunk's own prefix).
-// Header [T][gridDim.x][4].  The same post_chunk body as post_kernel<true>, so a virtual chunk's turns are the bits of the
-// real chunk at its latency.
+// The sweeps (dg_sweep_*): CTA (c, t) is virtual chunk c of the gridDim.x and trial t.  The scores seg [N][F][K] and maps
+// [T][N][K] are over the N real chunks; virtual chunk c is real chunk vchunk[c] (vchunk null: chunk c), and buffer j of its
+// plan row the real chunk vchunk[c] - (nb - 1) + j, inside the chunk's own file.  Header [T][gridDim.x][4]; trial t
+// thresholds at taus[t].  A virtual chunk's turns are the bits of the real chunk at its latency.
 __global__ void __launch_bounds__(POST_THREADS)
 post_virtual_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map, int N, const int32_t* __restrict__ vchunk,
                     int F, int K, int M, int nw, const int32_t* __restrict__ plan, int plan_stride,
@@ -147,19 +118,19 @@ post_virtual_kernel(const float* __restrict__ seg, const int32_t* __restrict__ m
   const double tau = taus[blockIdx.y];
   const int32_t* pl = plan + (size_t)c * plan_stride;
   const int nb = pl[0], nf = pl[1], first_nf = pl[2], first_lo = pl[3];
-  const int r0 = vchunk[c] - (nb - 1);                    // real chunk of buffer 0
+  const int r0 = (vchunk ? vchunk[c] : c) - (nb - 1);     // real chunk of buffer 0
   auto buf_seg = [&](int j) -> const float* { return seg + (size_t)(r0 + j) * F * K; };
   auto buf_map = [&](int j) -> const int32_t* { return map + (size_t)(r0 + j) * K; };
   post_chunk(pl, c, nb, nf, first_nf, first_lo, F, K, M, nw, hamming, tau, header, turns, turn_cap, total, buf_seg, buf_map);
 }
 
-// Many streams in one batch (dg_multi): the B chunks are grouped by stream slot.  Chunk c is window rows[c].y of this batch's
-// slot entry act[rows[c].x] (TickSlot, dg_common.cuh), whose chunks start at batch row row0.  Each slot has its own history of
-// up to ts.nw - 1 <= nw - 1 chunks: hist_seg [2][slots][nw - 1][F][K] and hist_map [2][slots][nw - 1][K] (two copies, `cur`
-// is the current one), of which the first n_hist entries hold the last chunks seen, oldest first.  nw is the largest of the
-// slots' (it sizes the history and the shared memory); a chunk aggregates the nb <= ts.nw buffers of its plan row and
-// compares with its entry's tau, params[3 * rows[c].x], the value a dedicated post-path at that stream's tau_active compares
-// with.
+// Live streams in one batch (dg_multi; dg_post is one stream in slot 0): the B chunks are grouped by stream slot.  Chunk c
+// is window rows[c].y of this batch's slot entry act[rows[c].x] (TickSlot, dg_common.cuh), whose chunks start at batch row
+// row0.  Each slot has its own history of up to ts.nw - 1 <= nw - 1 chunks: hist_seg [2][slots][nw - 1][F][K] and hist_map
+// [2][slots][nw - 1][K] (two copies, `cur` is the current one), of which the first n_hist entries hold the last chunks seen,
+// oldest first.  nw is the largest of the slots' (it sizes the history and the shared memory); a chunk aggregates the
+// nb <= ts.nw buffers of its plan row and compares with its entry's tau, params[3 * rows[c].x], the value a dedicated
+// post-path at that stream's tau_active compares with.
 __global__ void __launch_bounds__(POST_THREADS)
 post_slots_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map, const float* __restrict__ hist_seg,
                   const int32_t* __restrict__ hist_map, const TickSlot* __restrict__ act, const int2* __restrict__ rows,
@@ -204,54 +175,22 @@ post_slots_history_kernel(const float* __restrict__ seg, const int32_t* __restri
   for (int e = threadIdx.x; e < K; e += blockDim.x) hist_map[dst * K + e] = m[e];
 }
 
-// the last `keep` chunks seen (history followed by this batch) become the new history
-__global__ void post_history_kernel(const float* __restrict__ seg, const int32_t* __restrict__ map,
-                                    const float* __restrict__ hist_seg, const int32_t* __restrict__ hist_map, int n_hist,
-                                    int B, int FK, int K, int keep, float* __restrict__ new_seg,
-                                    int32_t* __restrict__ new_map) {
-  const int i = blockIdx.x;                       // new history slot
-  const int v = B - keep + i;                     // virtual chunk
-  const float* s = v >= 0 ? seg + (size_t)v * FK : hist_seg + (size_t)(n_hist + v) * FK;
-  const int32_t* m = v >= 0 ? map + (size_t)v * K : hist_map + (size_t)(n_hist + v) * K;
-  for (int e = threadIdx.x; e < FK; e += blockDim.x) new_seg[(size_t)i * FK + e] = s[e];
-  for (int e = threadIdx.x; e < K; e += blockDim.x) new_map[(size_t)i * K + e] = m[e];
-}
-
-int launch_post(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map, int n_hist, int B,
-                int F, int K, int M, int nw, const int32_t* plan, int plan_stride, const double* hamming, double tau,
-                int32_t* header, uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st, const double* taus,
-                int T) {
-  ProfScope _ps("post_aggregate", st);
-  if (T < 1 || T > 65535 || (T > 1 && !taus)) {
-    set_error("post: 1 <= states <= 65535, per-state thresholds for more than one");
-    return -1;
-  }
+// The launch set-up of both post kernels: the limit checks and post_chunk's dynamic shared memory, inv [nw][M] then act
+// [F + 1][M] (the first chunk of a stream or file emits the crop of [0, region end), up to F + 1 frames), with the opt-in
+// above 48 KB once per device (`attr_done`: the launcher's flags).
+template <class Kern>
+static int post_setup(const char* who, Kern* kern, bool* attr_done, int F, int K, int M, int nw, size_t* smem) {
   if (M > 64 || F > 1023 || K > 127) {
-    set_error("post: at most 64 global speakers, 1023 frames");
+    set_error(std::string(who) + ": at most 64 global speakers, 1023 frames");
     return -1;
   }
-  const size_t smem = ((size_t)(nw * M + 15) & ~(size_t)15) + (size_t)F * M;
-  if (smem > 200 * 1024) {
-    set_error("post: latency / step too large for the shared-memory plan");
+  *smem = ((size_t)(nw * M + 15) & ~(size_t)15) + (size_t)(F + 1) * M;
+  if (*smem > 200 * 1024) {
+    set_error(std::string(who) + ": latency / step too large for the shared-memory plan");
     return -1;
   }
-  if (smem > 48 * 1024) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    static bool done[64] = {};
-    if (dev < 64 && !done[dev]) {
-      DG_CUDA(cudaFuncSetAttribute(post_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-      DG_CUDA(cudaFuncSetAttribute(post_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-      done[dev] = true;
-    }
-  }
-  if (taus)
-    post_kernel<true><<<dim3(B, T), POST_THREADS, smem, st>>>(seg, map, hist_seg, hist_map, n_hist, B, F, K, M, nw, plan,
-                                                              plan_stride, hamming, tau, taus, header, turns, turn_cap, total);
-  else
-    post_kernel<false><<<B, POST_THREADS, smem, st>>>(seg, map, hist_seg, hist_map, n_hist, B, F, K, M, nw, plan, plan_stride,
-                                                      hamming, tau, nullptr, header, turns, turn_cap, total);
-  DG_LAUNCHED();
+  if (*smem > 48 * 1024 && first_use_on_device(attr_done))
+    DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   return 0;
 }
 
@@ -263,29 +202,12 @@ int launch_post_virtual(const float* seg, const int32_t* map, int N, const int32
     set_error("post_virtual: 1 <= states <= 65535 with per-state thresholds, at least one chunk");
     return -1;
   }
-  if (M > 64 || F > 1023 || K > 127) {
-    set_error("post_virtual: at most 64 global speakers, 1023 frames");
-    return -1;
-  }
-  // up to F + 1 output frames: the first chunk of a file emits the crop of [0, region end)
-  const size_t smem = ((size_t)(nw * M + 15) & ~(size_t)15) + (size_t)(F + 1) * M;
-  if (smem > 200 * 1024) {
-    set_error("post_virtual: latency / step too large for the shared-memory plan");
-    return -1;
-  }
   static bool attr_done[64] = {};
-  if (smem > 48 * 1024 && first_use_on_device(attr_done))
-    DG_CUDA(cudaFuncSetAttribute(post_virtual_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  size_t smem = 0;
+  int rc;
+  if ((rc = post_setup("post_virtual", post_virtual_kernel, attr_done, F, K, M, nw, &smem))) return rc;
   post_virtual_kernel<<<dim3(Nv, T), POST_THREADS, smem, st>>>(seg, map, N, vchunk, F, K, M, nw, plan, plan_stride, hamming,
                                                                taus, header, turns, turn_cap, total);
-  DG_LAUNCHED();
-  return 0;
-}
-
-int launch_post_history(const float* seg, const int32_t* map, const float* hist_seg, const int32_t* hist_map, int n_hist,
-                        int B, int F, int K, int keep, float* new_seg, int32_t* new_map, cudaStream_t st) {
-  if (keep < 1) return 0;
-  post_history_kernel<<<keep, 256, 0, st>>>(seg, map, hist_seg, hist_map, n_hist, B, F * K, K, keep, new_seg, new_map);
   DG_LAUNCHED();
   return 0;
 }
@@ -366,19 +288,10 @@ int launch_post_slots(const float* seg, const int32_t* map, const float* hist_se
                       const int32_t* plan, int plan_stride, const double* hamming, const double* params, int32_t* header,
                       uint32_t* turns, int turn_cap, unsigned int* total, cudaStream_t st) {
   ProfScope _ps("post_slots", st);
-  if (M > 64 || F > 1023 || K > 127) {
-    set_error("post_slots: at most 64 global speakers, 1023 frames");
-    return -1;
-  }
-  // up to F + 1 output frames: the first chunk of a stream emits the crop of [0, region end)
-  const size_t smem = ((size_t)(nw * M + 15) & ~(size_t)15) + (size_t)(F + 1) * M;
-  if (smem > 200 * 1024) {
-    set_error("post_slots: latency / step too large for the shared-memory plan");
-    return -1;
-  }
   static bool attr_done[64] = {};
-  if (smem > 48 * 1024 && first_use_on_device(attr_done))
-    DG_CUDA(cudaFuncSetAttribute(post_slots_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  size_t smem = 0;
+  int rc;
+  if ((rc = post_setup("post_slots", post_slots_kernel, attr_done, F, K, M, nw, &smem))) return rc;
   post_slots_kernel<<<B, POST_THREADS, smem, st>>>(seg, map, hist_seg, hist_map, act, rows, slots, F, K, M, nw, plan,
                                                    plan_stride, hamming, params, header, turns, turn_cap, total);
   DG_LAUNCHED();

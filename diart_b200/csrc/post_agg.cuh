@@ -1,5 +1,5 @@
 // The per-frame Hamming aggregation of the device post-path (DelayedAggregation, reference aggregation.py:73-92,120-218),
-// shared by post_kernel (post.cu) and the speech curves of vad.cu.
+// shared by post_chunk (post.cu) and the speech curves of vad.cu.
 #pragma once
 #include "dg_common.cuh"
 

@@ -5,9 +5,9 @@
 // only compares it with its own threshold.
 //
 //   vad_curve      one CTA per chunk: max over the K local speakers in float32 (torch.amax: NaN propagates), then the Hamming
-//                  aggregation of post_kernel with one global speaker and the identity map (post_agg.cuh), every output
+//                  aggregation of the post-path with one global speaker and the identity map (post_agg.cuh), every output
 //                  frame's float64 value written at the chunk's offset in the curve
-//   vad_binarize   one warp per (chunk, trial): curve > tau[t], run-length encoded into post_kernel's header
+//   vad_binarize   one warp per (chunk, trial): curve > tau[t], run-length encoded into the post-path's header
 //                  {offset, count, frames, 0} and packed turns (0 << 20 | on << 10 | off), all trials sharing one counter
 //
 // Many live VAD streams (dg_multi in VAD mode) use the same two bodies, per tick and per stream:
@@ -26,24 +26,8 @@ constexpr int VAD_CURVE_THREADS = 64;
 constexpr int VAD_BIN_THREADS = 256;
 constexpr int VAD_SLOTS_THREADS = 64;
 
-// plan [N][plan_stride] as post_kernel's, without history: chunk c aggregates chunks c - (nb - 1) .. c
-__global__ void __launch_bounds__(VAD_CURVE_THREADS)
-vad_curve_kernel(const float* __restrict__ seg /*[N][F][K]*/, int F, int K, const int32_t* __restrict__ plan, int plan_stride,
-                 const double* __restrict__ hamming, const long long* __restrict__ curve_off /*[N + 1]*/,
-                 double* __restrict__ curve) {
-  const int c = blockIdx.x;
-  const int32_t* pl = plan + (size_t)c * plan_stride;
-  const int nb = pl[0], nf = pl[1], first_nf = pl[2], first_lo = pl[3];
-  const int nfo = first_nf > 0 ? first_nf : nf;
-  double* out = curve + curve_off[c];
-  for (int fo = threadIdx.x; fo < nfo; fo += VAD_CURVE_THREADS)
-    out[fo] = post_frame(pl, nb, nf, nfo, first_lo, F, hamming, fo, [&](int j, int idx) {
-      return (double)speaker_max(seg + ((size_t)(c - (nb - 1) + j) * F + idx) * K, K);
-    });
-}
-
-// The curve over several latencies (dg_vad_sweep_curve_latencies): chunk c is a virtual chunk, real chunk vchunk[c] of seg, and
-// buffer j of its plan row the real chunk vchunk[c] - (nb - 1) + j; otherwise vad_curve_kernel's body
+// plan [Nv][plan_stride] as the post-path's, without history: chunk c is real chunk vchunk[c] of seg (vchunk null: chunk c),
+// and buffer j of its plan row the real chunk vchunk[c] - (nb - 1) + j
 __global__ void __launch_bounds__(VAD_CURVE_THREADS)
 vad_curve_virtual_kernel(const float* __restrict__ seg /*[N][F][K]*/, const int32_t* __restrict__ vchunk, int F, int K,
                          const int32_t* __restrict__ plan, int plan_stride, const double* __restrict__ hamming,
@@ -52,7 +36,7 @@ vad_curve_virtual_kernel(const float* __restrict__ seg /*[N][F][K]*/, const int3
   const int32_t* pl = plan + (size_t)c * plan_stride;
   const int nb = pl[0], nf = pl[1], first_nf = pl[2], first_lo = pl[3];
   const int nfo = first_nf > 0 ? first_nf : nf;
-  const int r0 = vchunk[c] - (nb - 1);
+  const int r0 = (vchunk ? vchunk[c] : c) - (nb - 1);
   double* out = curve + curve_off[c];
   for (int fo = threadIdx.x; fo < nfo; fo += VAD_CURVE_THREADS)
     out[fo] = post_frame(pl, nb, nf, nfo, first_lo, F, hamming, fo, [&](int j, int idx) {
@@ -181,17 +165,9 @@ vad_slots_history_kernel(const float* __restrict__ seg, float* hist_vad, const T
     hist_vad[dst * F + f] = v >= 0 ? speaker_max(seg + ((size_t)(ts.row0 + v) * F + f) * K, K) : hist_vad[(src + v) * F + f];
 }
 
-int launch_vad_curve(const float* seg, int N, int F, int K, const int32_t* plan, int plan_stride, const double* hamming,
-                     const long long* curve_off, double* curve, cudaStream_t st) {
-  ProfScope _ps("vad_curve", st);
-  vad_curve_kernel<<<N, VAD_CURVE_THREADS, 0, st>>>(seg, F, K, plan, plan_stride, hamming, curve_off, curve);
-  DG_LAUNCHED();
-  return 0;
-}
-
 int launch_vad_curve_virtual(const float* seg, const int32_t* vchunk, int Nv, int F, int K, const int32_t* plan, int plan_stride,
                              const double* hamming, const long long* curve_off, double* curve, cudaStream_t st) {
-  ProfScope _ps("vad_curve_virtual", st);
+  ProfScope _ps("vad_curve", st);
   vad_curve_virtual_kernel<<<Nv, VAD_CURVE_THREADS, 0, st>>>(seg, vchunk, F, K, plan, plan_stride, hamming, curve_off, curve);
   DG_LAUNCHED();
   return 0;

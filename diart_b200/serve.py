@@ -37,7 +37,7 @@ import torch
 from . import _lib
 from . import models as m
 from .blocks.diarization import SpeakerDiarizationConfig
-from .blocks.post import chunk_annotations, crop_plan
+from .blocks.post import chunk_annotations, crop_plan, turn_capacity
 from .blocks.vad import VoiceActivityDetectionConfig, speech_annotations
 from .core import Annotation
 from .operators import DeviceResample
@@ -275,7 +275,7 @@ class _MultiStreamServer:
                                               cfg.sample_rate, self.F, self.nw, np.repeat(self._res[sids], n))
         plan = np.ascontiguousarray(plan)
         header = np.empty((B, 4), dtype=np.int32)
-        need = B * self._speakers * ((self.F + 2) // 2)
+        need = turn_capacity(B, self._speakers, self.F)
         if len(self._turns) < need:
             self._turns = np.empty(need, dtype=np.uint32)
         got = np.empty(self.max_streams, dtype=np.int32)

@@ -146,6 +146,36 @@ def test_call_uploads_a_stream_once_and_falls_back_for_anything_else(oracle_nets
                 assert not expect_stream and clearance < 2e-4, f"{name}: chunk {i} differs, threshold clearance {clearance:.1e}"
 
 
+def test_call_refuses_a_bad_plan_before_touching_any_state(oracle_nets, stream, cuda_device):
+    """dg_pipeline_call_host checks the plan rows at entry: a row whose buffers reach before the stream's first chunk is
+    refused before any launch, and the calls after it give what a pipeline that never saw it gives"""
+    import ctypes
+
+    from diart_b200.blocks.post import post_plan
+
+    pipe = make_pipeline(oracle_nets, cuda_device, latency=1.5)
+    ref = make_pipeline(oracle_nets, cuda_device, latency=1.5)
+    sr, step, n = 16000, 0.5, 12
+    chunks = [SlidingWindowFeature(np.ascontiguousarray(stream[8000 * i:8000 * i + 80000, None]),
+                                   SlidingWindow(start=step * i, duration=1 / sr, step=1 / sr)) for i in range(n)]
+    h, F, K, _ = pipe._ensure_fused(80000)
+    post = pipe._ensure_post(F, K)
+    plan = np.ascontiguousarray(post_plan(np.arange(5) * step, 5 / F, np.zeros(0), np.zeros(0), post.nw, F, step, 1.5)[0])
+    plan[1, 0] = 3
+    header, turns = post.buffers(5)
+    rows = (ctypes.c_void_p * 5)(*[c.data.ctypes.data for c in chunks[:5]])
+    lib = _lib.lib()
+    before = lib.dg_launch_count()
+    rc = lib.dg_pipeline_call_host(h, post.handle, rows, 5, 80000, plan.ctypes.data, header.ctypes.data, turns.ctypes.data,
+                                   len(turns), ctypes.byref(ctypes.c_int()), None, None)
+    assert rc == -1 and lib.dg_launch_count() == before
+    assert b"dg_pipeline_call_host: plan row 1 " in lib.dg_last_error()
+    got = pipe(chunks[:5]) + pipe(chunks[5:])
+    want = ref(chunks[:5]) + ref(chunks[5:])
+    assert [a.to_rttm() for a, _ in got] == [a.to_rttm() for a, _ in want]
+    assert sum(len(a.to_rttm()) for a, _ in got) > 0
+
+
 def test_two_pipelines_on_the_same_model_handles(oracle_nets, stream, cuda_device):
     """two SpeakerDiarization instances built on the SAME SegmentationModel / EmbeddingModel objects (two audio streams, one set
     of weights) share the handles' activation buffers: submits of both in flight at once must hand the buffers over in stream order

@@ -8,7 +8,7 @@ import pytest
 import torch
 
 from diart_b200 import _lib, blocks, models, synth
-from diart_b200.blocks.post import turn_times
+from diart_b200.blocks.post import post_plan, turn_times
 from diart_b200.core import SlidingWindow, SlidingWindowFeature
 from diart_b200.sinks import PredictionAccumulator
 from diart_b200.tune import HyperParameterSweep, assemble_predictions, file_windows, trial_params
@@ -189,3 +189,25 @@ def test_run_time_argument_checks_never_launch(file_600):
                               None, header.ctypes.data, turns.ctypes.data, len(turns), ctypes.byref(n), None)
         assert rc == -1 and lib.dg_launch_count() == before, (params, T, n_chunks)
         assert b"dg_sweep_run" in lib.dg_last_error()
+    # plan rows the file's chunks cannot have: more buffers than latency / step, buffers before the file's first chunk, F + 2
+    # output frames, and (two files) the second file's first chunk reaching into the first file; at latency = 4 steps
+    h, nw = sweep._handle(F, K, emb.shape[2], 4)
+    plan = np.ascontiguousarray(post_plan(fw.starts, sweep._seg_resolution(float(fw.starts[0]), F), np.zeros(0), np.zeros(0),
+                                          nw, F, cfg.step, nw * cfg.step)[0])
+    wide, early, long_first = plan.copy(), plan.copy(), plan.copy()
+    wide[N - 1, 0] = nw + 1
+    early[1, 0] = 3
+    long_first[0, 2] = F + 2
+    two_files = np.array([0, 300, N], np.int32)
+    for name, bad, offs in (("nb > nw", wide, None), ("before the first chunk", early, None), ("F + 2 frames", long_first, None),
+                            ("into the previous file", plan, two_files)):
+        before = lib.dg_launch_count()
+        if offs is None:
+            rc = lib.dg_sweep_run(h, seg.data_ptr(), emb.data_ptr(), N, good.ctypes.data, 1, bad.ctypes.data, None, None,
+                                  header.ctypes.data, turns.ctypes.data, len(turns), ctypes.byref(n), None)
+        else:
+            rc = lib.dg_sweep_run_files(h, seg.data_ptr(), emb.data_ptr(), N, len(offs) - 1, offs.ctypes.data, good.ctypes.data,
+                                        1, bad.ctypes.data, None, None, header.ctypes.data, turns.ctypes.data, len(turns),
+                                        ctypes.byref(n), None)
+        assert rc == -1 and lib.dg_launch_count() == before, name
+        assert b": plan row" in lib.dg_last_error(), name
