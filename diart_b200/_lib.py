@@ -137,6 +137,8 @@ SIGNATURES = {
     "dg_multi_add_rate": (C.c_int, [_P, _P, C.c_int, C.c_int, C.POINTER(C.c_int)]),
     "dg_multi_open_rate": (C.c_int, [_P, C.c_int, C.c_int]),
     "dg_multi_open_config": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P]),
+    "dg_multi_open_seeded": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int]),
+    "dg_multi_get_state": (C.c_int, [_P, C.c_int, _P, _P, C.POINTER(C.c_int)]),
     "dg_multi_last_windows": (C.c_int, [_P, _P, C.c_int]),
     "dg_selftest_multi_frames_host": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, C.c_int,
                                                 C.POINTER(C.c_int)]),

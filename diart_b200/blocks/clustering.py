@@ -36,10 +36,14 @@ class OnlineSpeakerClustering:
         self.blocked_centers = set()   # reference clustering.py:46 -- never populated there either
         self._h: Optional[C.c_void_p] = None
         self._dim: Optional[int] = None
+        self._seed: Optional[np.ndarray] = None   # initial centroids (n, D) written when the handle is created
 
     # ------------------------------------------------------------------ handle management
     def _handle(self, dim: int) -> C.c_void_p:
         if self._h is None:
+            if self._seed is not None and self._seed.shape[1] != dim:
+                raise ValueError(f"the known speakers' centroids have dimension {self._seed.shape[1]}, the embeddings "
+                                 f"{dim}")
             _lib.require_cuda(self.device)
             h = C.c_void_p()
             _lib.check(_lib.lib().dg_cluster_create(self.max_speakers, dim, self.tau_active, self.rho_update,
@@ -47,8 +51,32 @@ class OnlineSpeakerClustering:
             if METRICS[self.metric]:
                 _lib.check(_lib.lib().dg_cluster_set_metric(h, METRICS[self.metric]))
             self._h, self._dim = h, dim
+            if self._seed is not None:
+                self._write_seed()
         assert dim == self._dim, "embedding dimension changed"
         return self._h
+
+    def seed(self, centroids: Optional[np.ndarray]):
+        """the initial state before the first step: centres 0 .. n - 1 hold ``centroids`` (float64 (n, D)) and are active,
+        and the state is initialised, so the first step takes the reference's distance path.  None or n = 0: the fresh
+        state (not initialised).  Written now if the handle exists, else when it is created (the dimension is checked
+        then, before any launch)."""
+        c = None if centroids is None or len(centroids) == 0 else np.ascontiguousarray(centroids, dtype=np.float64)
+        if c is not None and len(c) > self.max_speakers:
+            raise ValueError(f"{len(c)} known speakers, at most max_speakers = {self.max_speakers}")
+        if c is not None and self._h is not None and c.shape[1] != self._dim:
+            raise ValueError(f"the known speakers' centroids have dimension {c.shape[1]}, the embeddings {self._dim}")
+        self._seed = c
+        if self._h is not None:
+            if c is None:
+                self.reset()
+            else:
+                self._write_seed()
+
+    def _write_seed(self):
+        centers = np.zeros((self.max_speakers, self._dim))
+        centers[:len(self._seed)] = self._seed
+        self._set_state(centers, range(len(self._seed)), True)
 
     def __del__(self):
         try:

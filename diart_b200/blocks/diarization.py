@@ -18,6 +18,7 @@ import torch
 from .. import _lib
 from .. import models as m
 from ..core import Annotation, Segment, SlidingWindow, SlidingWindowFeature, extent_bounds
+from ..speakers import KnownSpeakers, exported, speaker_labels
 from . import base
 from .aggregation import DelayedAggregation
 from .clustering import OnlineSpeakerClustering
@@ -64,6 +65,8 @@ class SpeakerDiarization(base.Pipeline):
         self._pinned: Optional[torch.Tensor] = None
         self._post: Optional[DevicePostPath] = None
         self.call_profile: Optional[dict] = None       # set to {} to accumulate seconds per phase of __call__
+        self._known: Optional[KnownSpeakers] = None
+        self.labels = speaker_labels(None, self._config.max_speakers)
         self.reset()
 
     @staticmethod
@@ -93,9 +96,40 @@ class SpeakerDiarization(base.Pipeline):
         self.clustering = OnlineSpeakerClustering(self.config.tau_active, self.config.rho_update,
                                                   self.config.delta_new, "cosine", self.config.max_speakers,
                                                   device=self.segmentation.device)
+        self.clustering.seed(None if self._known is None else self._known.centroids)
+        self._started = False                          # a chunk went through since construction or reset()
         self.chunk_buffer, self.pred_buffer = [], []
         if self._post is not None:
             self._post.reset()
+
+    # ------------------------------------------------------------------ known speakers
+    def set_known_speakers(self, known: Optional[KnownSpeakers]):
+        """makes ``known`` the initial clustering state (``diart_b200.speakers``): centres 0 .. n - 1 hold its centroids and
+        are active, the state is initialised, and centre g < n is labelled ``names[g]`` in every annotation.  None or an
+        empty one: the fresh state.  Only before the first chunk after construction or :meth:`reset`, which re-applies
+        it; ValueError otherwise, or for more than ``max_speakers`` speakers.  The dimension is checked against the
+        embeddings' before the first clustering launch."""
+        if self._started:
+            raise ValueError("known speakers are set before the first chunk after construction or reset()")
+        if known is not None and not isinstance(known, KnownSpeakers):
+            raise TypeError(f"expected KnownSpeakers or None, got {type(known).__name__}")
+        known = known if known is not None and len(known) else None
+        self.clustering.seed(None if known is None else known.centroids)
+        self._known = known
+        self.labels = speaker_labels(known, self.config.max_speakers)
+        self.binarize.labels = self.labels
+        if self._post is not None:
+            self._post.labels = self.labels
+
+    def speakers(self) -> KnownSpeakers:
+        """the clustering's active centres in index order (a prefix 0 .. k - 1) with their labels: what
+        :meth:`set_known_speakers` of a later pipeline resumes from.  The aggregation history is not part of it."""
+        if self.clustering._h is None:                # no chunk yet: the initial state
+            return self._known if self._known is not None else KnownSpeakers([], np.zeros((0, 0)))
+        centers, active, _ = self.clustering._state()
+        flags = np.zeros(self.config.max_speakers, dtype=np.int32)
+        flags[sorted(active)] = 1
+        return exported(self.labels, centers, flags)
 
     # ------------------------------------------------------------------ fused device step
     def _drop_fused(self):
@@ -134,6 +168,7 @@ class SpeakerDiarization(base.Pipeline):
             # hint for the stream form of the sinc layer; the device verifies it per batch
             _lib.check(_lib.lib().dg_pipeline_set_hop(h, int(round(self.config.step * self.config.sample_rate))))
             self._fused = h
+        self._started = True
         return self._fused, F, K, D
 
     def submit(self, batch: torch.Tensor):
@@ -165,6 +200,7 @@ class SpeakerDiarization(base.Pipeline):
         native = self._native_models()
         device = self.segmentation.device
         if native is None:  # foreign models behind the loader API: block by block, still on the device
+            self._started = True
             seg = self.segmentation.forward_device(batch)
             emb = self.embedding.forward_device(batch, seg)
             maps, _ = self.clustering.step_batch(seg, emb)
@@ -305,6 +341,7 @@ class SpeakerDiarization(base.Pipeline):
         if self._post is None:
             self._post = DevicePostPath(self.config.step, self.config.latency, self.config.tau_active, F, K,
                                         self.config.max_speakers, self.segmentation.device)
+            self._post.labels = self.labels
         return self._post
 
     def _call_blockwise(self, waveforms, expected):

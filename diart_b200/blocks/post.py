@@ -189,20 +189,24 @@ def chunk_turns(header: np.ndarray, turns: np.ndarray, n_turns: int, out_start: 
 
 
 def chunk_annotations(header: np.ndarray, turns: np.ndarray, n_turns: int, out_start: np.ndarray, out_res: np.ndarray,
-                      labels: Sequence[str], shift=0.0, uri: Optional[str] = None) -> List[Annotation]:
+                      labels: Sequence, shift=0.0, uri: Optional[str] = None) -> List[Annotation]:
     """packed turns -> one Annotation per chunk (row of ``header``), segments at frame middles (blocks/utils.py:45-58).
-    ``shift``: seconds added to every time stamp, one number or one per chunk (streams with their own shifts)."""
+    ``labels``: the label of each global speaker, one list for every chunk or one list per chunk (streams with their own
+    known speakers).  ``shift``: seconds added to every time stamp, one number or one per chunk (streams with their own
+    shifts)."""
     B = len(header)
     offs, cnts, g, t_on, t_off = chunk_turns(header, turns, n_turns, out_start, out_res, shift)
     # the reference's shifted copy drops the modality
     modality = [("speech" if x == 0 else None) for x in np.asarray(shift).tolist()] if np.ndim(shift) > 0 else \
         [("speech" if shift == 0 else None)] * B
+    per_chunk = B > 0 and not isinstance(labels[0], str)
     out = []
     for cidx in range(B):
         ann = Annotation(uri=uri, modality=modality[cidx])
+        labels_c = labels[cidx] if per_chunk else labels
         o = offs[cidx]
         for i in range(o, o + cnts[cidx]):
-            ann[Segment(t_on[i], t_off[i]), g[i]] = labels[g[i]]
+            ann[Segment(t_on[i], t_off[i]), g[i]] = labels_c[g[i]]
         out.append(ann)
     return out
 

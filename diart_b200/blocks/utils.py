@@ -1,8 +1,8 @@
 """``Binarize`` (mirrors reference ``src/diart/blocks/utils.py:11-59``): discrete-time scores ->
-speaker turns at frame middles, label ``speaker<g>``."""
+speaker turns at frame middles, label ``speaker<g>`` (or ``labels[g]``)."""
 from __future__ import annotations
 
-from typing import Optional
+from typing import Optional, Sequence
 
 import numpy as np
 
@@ -10,9 +10,10 @@ from ..core import Annotation, Segment, SlidingWindowFeature
 
 
 class Binarize:
-    def __init__(self, threshold: float, uri: Optional[str] = None):
+    def __init__(self, threshold: float, uri: Optional[str] = None, labels: Optional[Sequence[str]] = None):
         self.uri = uri
         self.threshold = threshold
+        self.labels = labels          # the label of each global speaker (known speakers' names); None: speaker<g>
 
     def __call__(self, segmentation: SlidingWindowFeature) -> Annotation:
         num_frames, num_speakers = segmentation.data.shape
@@ -26,7 +27,8 @@ class Binarize:
             change = np.flatnonzero(col[1:] != col[:-1])       # on/off boundaries, in frame units
             # a turn that is active from frame 0 starts at the first frame's middle
             for on, off in zip(change[0::2], change[1::2]):
-                annotation[Segment(middles[on], middles[off]), int(spk)] = f"speaker{spk}"
+                label = f"speaker{spk}" if self.labels is None else self.labels[spk]
+                annotation[Segment(middles[on], middles[off]), int(spk)] = label
         return annotation
 
 

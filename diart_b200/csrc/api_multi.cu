@@ -368,9 +368,12 @@ extern "C" int dg_multi_add_rate(dg_multi* h, dg_resample* rs, int chunk_samples
 }
 
 // a new stream in `slot` at declared rate `rate_id` (-1: the pipeline's rate), aggregating num_windows buffers, with
-// params {tau, rho, delta} (a VAD handle reads tau only): empty rings, fresh clustering state (the reference's
-// SpeakerDiarization.reset(); a VAD handle has none), no history.  Every argument is checked first; a refusal names `who`.
-static int open_slot(dg_multi* h, int slot, int rate_id, int num_windows, const double* params, const char* who) {
+// params {tau, rho, delta} (a VAD handle reads tau only): empty rings, no history, and the clustering state (a VAD handle has
+// none) fresh (the reference's SpeakerDiarization.reset()) for n = 0, else seeded with the n known centroids centers_host
+// [n][D]: rows 0 .. n - 1 written and active, the rest zero, initialised.  Every argument is checked first; a refusal names
+// `who` and changes nothing.
+static int open_slot(dg_multi* h, int slot, int rate_id, int num_windows, const double* params, const double* centers_host,
+                     int n, const char* who) {
   if (!h || slot < 0 || slot >= h->slots || h->book.open[slot]) {
     set_error(std::string(who) + ": slot " + std::to_string(slot) + " is out of range or already open");
     return DG_EINVAL;
@@ -389,12 +392,40 @@ static int open_slot(dg_multi* h, int slot, int rate_id, int num_windows, const 
     set_error(std::string(who) + (vad ? ": need a finite tau" : ": need finite tau, rho and delta"));
     return DG_EINVAL;
   }
+  if (n < 0 || n > h->M || (n > 0 && (vad || !centers_host))) {
+    set_error(std::string(who) + ": need 0 <= n <= max_speakers (" + std::to_string(h->M) + ") known centroids and a "
+              "non-null table, got n = " + std::to_string(n));
+    return DG_EINVAL;
+  }
+  const int D = h->D;
+  for (int i = 0; i < n; i++) {
+    double ss = 0.0;
+    bool finite = true;
+    for (int d = 0; d < D; d++) {
+      const double x = centers_host[(size_t)i * D + d];
+      finite = finite && std::isfinite(x);
+      ss += x * x;
+    }
+    if (!finite || !(ss > 0.0)) {
+      set_error(std::string(who) + ": centroid " + std::to_string(i) + (finite ? " has a zero norm" : " is not finite"));
+      return DG_EINVAL;
+    }
+  }
   DG_CUDA(cudaSetDevice(h->device));
   const size_t s = (size_t)slot;
-  if (!vad_mode(h)) {
-    DG_CUDA(cudaMemsetAsync(h->centers.as<double>() + s * h->M * h->D, 0, (size_t)h->M * h->D * 8, h->st));
+  if (!vad) {
+    double* centers = h->centers.as<double>() + s * h->M * D;
+    DG_CUDA(cudaMemsetAsync(centers, 0, (size_t)h->M * D * 8, h->st));
     DG_CUDA(cudaMemsetAsync(h->active.as<int>() + s * 32, 0, 32 * 4, h->st));
     DG_CUDA(cudaMemsetAsync(h->init.as<int>() + s * 2, 0, 2 * 4, h->st));
+    if (n > 0) {
+      // copies from pageable memory: the source is staged before cudaMemcpyAsync returns, so it may be freed then
+      const std::vector<int> flags((size_t)n, 1);
+      const int init[2] = {1, 0};
+      DG_CUDA(cudaMemcpyAsync(centers, centers_host, (size_t)n * D * 8, cudaMemcpyHostToDevice, h->st));
+      DG_CUDA(cudaMemcpyAsync(h->active.as<int>() + s * 32, flags.data(), (size_t)n * 4, cudaMemcpyHostToDevice, h->st));
+      DG_CUDA(cudaMemcpyAsync(h->init.as<int>() + s * 2, init, 2 * 4, cudaMemcpyHostToDevice, h->st));
+    }
   }
   h->book.start(slot, rate_id + 1);
   h->n_hist[slot] = 0;
@@ -407,7 +438,16 @@ static int open_slot(dg_multi* h, int slot, int rate_id, int num_windows, const 
 }
 
 extern "C" int dg_multi_open_config(dg_multi* h, int slot, int rate_id, int num_windows, const double* params) {
-  return open_slot(h, slot, rate_id, num_windows, params, "dg_multi_open_config");
+  return open_slot(h, slot, rate_id, num_windows, params, nullptr, 0, "dg_multi_open_config");
+}
+
+extern "C" int dg_multi_open_seeded(dg_multi* h, int slot, int rate_id, int num_windows, const double* params,
+                                    const double* centers_host, int n) {
+  if (h && vad_mode(h)) {
+    set_error("dg_multi_open_seeded: a VAD handle has no clustering state to seed");
+    return DG_EINVAL;
+  }
+  return open_slot(h, slot, rate_id, num_windows, params, centers_host, n, "dg_multi_open_seeded");
 }
 
 extern "C" int dg_multi_open_rate(dg_multi* h, int slot, int rate_id) {
@@ -416,7 +456,7 @@ extern "C" int dg_multi_open_rate(dg_multi* h, int slot, int rate_id) {
     return DG_EINVAL;
   }
   const double params[3] = {h->tau, h->rho, h->delta};
-  return open_slot(h, slot, rate_id, h->nw, params, "dg_multi_open");
+  return open_slot(h, slot, rate_id, h->nw, params, nullptr, 0, "dg_multi_open");
 }
 
 extern "C" int dg_multi_open(dg_multi* h, int slot) { return dg_multi_open_rate(h, slot, -1); }
@@ -428,6 +468,28 @@ extern "C" int dg_multi_close(dg_multi* h, int slot) {
     return DG_EINVAL;
   }
   h->book.stop(slot);
+  return DG_OK;
+}
+
+// the clustering state of the open stream in `slot` after the last tick: centroids [M][D], active flags [M], initialised
+extern "C" int dg_multi_get_state(dg_multi* h, int slot, double* centers_host, int32_t* active_host, int* initialized) {
+  if (!slot_ok(h, slot) || vad_mode(h) || !centers_host || !active_host || !initialized) {
+    set_error("dg_multi_get_state: need an open slot of a diarization handle and non-null outputs");
+    return DG_EINVAL;
+  }
+  DG_CUDA(cudaSetDevice(h->device));
+  const size_t s = (size_t)slot;
+  int init[2] = {0, 0};
+  DG_CUDA(cudaMemcpyAsync(centers_host, h->centers.as<double>() + s * h->M * h->D, (size_t)h->M * h->D * 8,
+                          cudaMemcpyDeviceToHost, h->st));
+  DG_CUDA(cudaMemcpyAsync(active_host, h->active.as<int>() + s * 32, (size_t)h->M * 4, cudaMemcpyDeviceToHost, h->st));
+  DG_CUDA(cudaMemcpyAsync(init, h->init.as<int>() + s * 2, 2 * 4, cudaMemcpyDeviceToHost, h->st));
+  DG_CUDA(cudaStreamSynchronize(h->st));
+  if (init[1]) {
+    set_error("Cannot update unknown centers");   // reference clustering.py:98 (AssertionError)
+    return DG_EINVAL;
+  }
+  *initialized = init[0];
   return DG_OK;
 }
 

@@ -24,7 +24,11 @@ Each stream may have its own latency (up to the server's ``max_latency``) and th
 tau_active=...)``, and ``rho_update`` / ``delta_new`` for diarization), none of which reaches the networks: the tick's one
 network pass is shared, the clustering runs every stream's state at that stream's thresholds, and the post-path aggregates
 each stream's own number of buffers and binarises at its own ``tau_active``.  A stream's results are then those of a
-dedicated pipeline whose configuration is the server's with that stream's values."""
+dedicated pipeline whose configuration is the server's with that stream's values.
+
+A diarization stream may also start from known speakers (``open(speakers=...)``, ``diart_b200.speakers``): its clustering
+state is seeded with their centroids and its annotations name them; ``speakers(sid)`` exports a stream's state, so that a
+closed stream can be resumed with the same centroids and labels."""
 from __future__ import annotations
 
 import ctypes as C
@@ -41,6 +45,7 @@ from .blocks.post import chunk_annotations, crop_plan, turn_capacity
 from .blocks.vad import VoiceActivityDetectionConfig, speech_annotations
 from .core import Annotation
 from .operators import DeviceResample
+from .speakers import KnownSpeakers, exported, speaker_labels
 
 
 def plan_rows(idx: np.ndarray, step: float, window_samples: int, sample_rate: int, frames: int, nw: int, latency: float,
@@ -188,6 +193,7 @@ class _MultiStreamServer:
         raise NotImplementedError
 
     def _annotations(self, header, turns, n_turns, out_start, out_res, shifts) -> List[Annotation]:
+        """the tick's annotations; ``shifts``: the timestamp shift of each row (``_row_sids``: its stream)"""
         raise NotImplementedError
 
     def __del__(self):
@@ -201,11 +207,13 @@ class _MultiStreamServer:
     def handle(self) -> C.c_void_p:
         return self._h
 
-    def _open_stream(self, shift: float, sample_rate: Optional[int], latency: Optional[float], **thresholds) -> int:
+    def _open_stream(self, shift: float, sample_rate: Optional[int], latency: Optional[float],
+                     seed: Optional[np.ndarray] = None, **thresholds) -> int:
         """a new stream (fresh clustering and aggregation state) in the lowest free slot, its blocks at ``sample_rate``
         (default: the pipeline's; otherwise one of ``source_sample_rates``), at its own ``latency`` and ``thresholds``
-        (name -> value, in the order of the handle's {tau, rho, delta}; None: the config's).  Everything is checked before
-        the handle is touched: a refusal raises ValueError and leaves the slot closed.  Returns the stream's id"""
+        (name -> value, in the order of the handle's {tau, rho, delta}; None: the config's).  ``seed``: known centroids
+        float64 (n, D) its clustering state starts from (dg_multi_open_seeded).  Everything is checked before the handle is
+        touched: a refusal raises ValueError and leaves the slot closed.  Returns the stream's id"""
         cfg = self.config
         rate = cfg.sample_rate if sample_rate is None else int(sample_rate)
         if rate not in self.rates:
@@ -224,7 +232,13 @@ class _MultiStreamServer:
         sid = int(free[0])
         rid, chunk, hop, res = self.rates[rate]
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().dg_multi_open_config(self._h, sid, rid, stream_windows(lat, cfg.step), params.ctypes.data))
+            if seed is None:
+                _lib.check(_lib.lib().dg_multi_open_config(self._h, sid, rid, stream_windows(lat, cfg.step),
+                                                           params.ctypes.data))
+            else:
+                seed = np.ascontiguousarray(seed, dtype=np.float64)
+                _lib.check(_lib.lib().dg_multi_open_seeded(self._h, sid, rid, stream_windows(lat, cfg.step),
+                                                           params.ctypes.data, seed.ctypes.data, len(seed)))
         self._open[sid] = True
         self._pushed[sid] = self._emitted[sid] = 0
         self._shift[sid] = float(shift)
@@ -291,6 +305,7 @@ class _MultiStreamServer:
         outs = tuple(t for t in outs if t is not None) or None
         if B == 0:
             return {}, outs
+        self._row_sids = np.repeat(sids, n)
         anns = self._annotations(header, self._turns, n_turns.value, out_start, out_res, np.repeat(self._shift[sids], n))
         return {int(s): anns[r:r + k] for s, r, k in zip(sids.tolist(), row0.tolist(), n.tolist())}, outs
 
@@ -306,7 +321,14 @@ class MultiStreamDiarization(_MultiStreamServer):
     ``config.latency``, at most ``config.duration``, sizes every slot's aggregation history) and ``tau_active``,
     ``rho_update`` and ``delta_new``; its results are then those of ``SpeakerDiarization`` with the config's other values
     and these.  Needs the native models (``B200*Loader``).  ``_step(outputs=True)`` also returns the tick's scores (B, F,
-    K), embeddings (B, K, D) and maps (B, K) as device tensors."""
+    K), embeddings (B, K, D) and maps (B, K) as device tensors.
+
+    ``open(speakers=known)`` starts a stream from known speakers (:class:`~diart_b200.speakers.KnownSpeakers`, at most
+    ``max_speakers`` of the embedding dimension): its results are then those of ``SpeakerDiarization`` with
+    ``set_known_speakers(known)``, and its global speaker g < n is labelled ``known.names[g]``.  ``speakers(sid)`` returns the
+    stream's active centres with their labels after the last tick; opening a stream with them resumes its clustering state
+    exactly (not its aggregation history: the first ``latency / step - 1`` outputs aggregate fewer buffers, as those of any
+    new stream do)."""
 
     _needs = "MultiStreamDiarization needs the native segmentation and embedding models"
 
@@ -316,15 +338,40 @@ class MultiStreamDiarization(_MultiStreamServer):
         self.labels = [f"speaker{g}" for g in range(config.max_speakers)]
         super().__init__(config, max_streams, max_windows_per_stream, source_sample_rates,
                          (config.segmentation, config.embedding), max_latency)
+        self._seeded = np.zeros(self.max_streams, dtype=bool)          # the stream in the slot started from known speakers
+        self._stream_labels = [self.labels] * self.max_streams          # each slot's label list (unseeded: the shared one)
 
     def open(self, shift: float = 0.0, sample_rate: Optional[int] = None, *, latency: Optional[float] = None,
              tau_active: Optional[float] = None, rho_update: Optional[float] = None,
-             delta_new: Optional[float] = None) -> int:
+             delta_new: Optional[float] = None, speakers: Optional[KnownSpeakers] = None) -> int:
         """a new stream in the lowest free slot (``_MultiStreamServer._open_stream``): blocks at ``sample_rate``, time
-        stamps shifted by ``shift``, and its own latency and thresholds (None: the config's), fixed until it is closed;
-        returns its id"""
-        return _MultiStreamServer._open_stream(self, shift, sample_rate, latency, tau_active=tau_active,
-                                               rho_update=rho_update, delta_new=delta_new)
+        stamps shifted by ``shift``, its own latency and thresholds (None: the config's), fixed until it is closed, and its
+        clustering state seeded with ``speakers`` (None or empty: fresh); returns its id.  ValueError, with the slot left
+        closed, for known speakers of another dimension or more than ``max_speakers`` of them."""
+        if speakers is not None and not isinstance(speakers, KnownSpeakers):
+            raise TypeError(f"speakers: expected KnownSpeakers or None, got {type(speakers).__name__}")
+        known = speakers if speakers is not None and len(speakers) else None
+        if known is not None:
+            if known.dimension != self.D:
+                raise ValueError(f"the known speakers' centroids have dimension {known.dimension}, the embeddings {self.D}")
+            if len(known) > self._speakers:
+                raise ValueError(f"{len(known)} known speakers, at most max_speakers = {self._speakers}")
+        sid = _MultiStreamServer._open_stream(self, shift, sample_rate, latency, None if known is None else known.centroids,
+                                              tau_active=tau_active, rho_update=rho_update, delta_new=delta_new)
+        self._seeded[sid] = known is not None
+        self._stream_labels[sid] = self.labels if known is None else speaker_labels(known, self._speakers)
+        return sid
+
+    def speakers(self, sid: int) -> KnownSpeakers:
+        """the clustering state of open stream ``sid`` after the last tick: its active centres in index order (a prefix
+        0 .. k - 1) with their labels, what ``open(speakers=...)`` resumes from"""
+        if not (0 <= sid < self.max_streams and self._open[sid]):
+            raise ValueError(f"stream {sid} is not open")
+        centers = np.empty((self._speakers, self.D), dtype=np.float64)
+        active = np.empty(self._speakers, dtype=np.int32)
+        init = C.c_int()
+        _lib.check(_lib.lib().dg_multi_get_state(self._h, int(sid), centers.ctypes.data, active.ctypes.data, C.byref(init)))
+        return exported(self._stream_labels[sid], centers, active)
 
     def _create(self, hamming):
         config, emb_net = self.config, self.config.embedding.model
@@ -345,7 +392,9 @@ class MultiStreamDiarization(_MultiStreamServer):
                 torch.empty((B, self.K), device=self.device, dtype=torch.int32))
 
     def _annotations(self, header, turns, n_turns, out_start, out_res, shifts):
-        return chunk_annotations(header, turns, n_turns, out_start, out_res, self.labels, shifts)
+        sids = self._row_sids
+        labels = [self._stream_labels[s] for s in sids.tolist()] if self._seeded[sids].any() else self.labels
+        return chunk_annotations(header, turns, n_turns, out_start, out_res, labels, shifts)
 
 
 class MultiStreamVoiceActivityDetection(_MultiStreamServer):

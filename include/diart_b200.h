@@ -484,6 +484,21 @@ typedef struct dg_resample dg_resample;   /* declared with its entry points belo
 int dg_multi_add_rate(dg_multi* h, dg_resample* rs, int chunk_samples, int step_samples, int* rate_id);
 int dg_multi_open_rate(dg_multi* h, int slot, int rate_id);
 int dg_multi_open_config(dg_multi* h, int slot, int rate_id, int num_windows, const double params[3] /* tau, rho, delta */);
+/* ---- known speakers: a stream that starts from a given clustering state (diart_b200.speakers).  The reference's
+ *      OnlineSpeakerClustering.identify (src/diart/blocks/clustering.py:149) takes its first-chunk path only while its centers
+ *      are None; a state filled beforehand goes straight to the distance path.
+ *      dg_multi_open_seeded: dg_multi_open_config, with the slot's clustering state seeded from centers_host float64 [n][D]:
+ *        rows 0 .. n - 1 written from it and active, rows n .. max_speakers - 1 zero, initialised iff n > 0 (n = 0 is
+ *        dg_multi_open_config).  The writes are ordered on the handle's stream; centers_host may be freed when the call
+ *        returns.  DG_EINVAL, naming dg_multi_open_seeded and changing nothing, if dg_multi_open_config would refuse, the
+ *        handle is a VAD handle, n < 0 or n > max_speakers, or a centroid is not finite or has a zero norm.
+ *      dg_multi_get_state: the clustering state of the open stream in `slot` after its last tick: centers_host float64
+ *        [max_speakers][D], active_host int32 [max_speakers] (1: active), *initialized.  DG_EINVAL for a closed slot or a VAD
+ *        handle.  Synchronous (dg_multi_step is, so the state is that of the last tick). ---- */
+int dg_multi_open_seeded(dg_multi* h, int slot, int rate_id, int num_windows, const double params[3] /* tau, rho, delta */,
+                         const double* centers_host /* [n][D] */, int n);
+int dg_multi_get_state(dg_multi* h, int slot, double* centers_host /* [M][D] */, int32_t* active_host /* [M] */,
+                       int* initialized);
 /* test hook: the last tick's window batch [n_rows, chunk_samples] (what its networks read; n_rows = that tick's window count)
  * copied to wav_dev.  Synchronous. */
 int dg_multi_last_windows(const dg_multi* h, float* wav_dev, int n_rows);
