@@ -104,6 +104,8 @@ SIGNATURES = {
     "dg_sweep_destroy": (C.c_int, [_P]),
     "dg_sweep_set_scored_regions": (C.c_int, [_P, C.c_int, _P, _P]),
     "dg_sweep_set_trial_sets": (C.c_int, [_P, C.c_int, _P, C.c_int]),
+    "dg_sweep_set_seeds": (C.c_int, [_P, C.c_int, _P, _P]),
+    "dg_sweep_set_identities": (C.c_int, [_P, C.c_int, _P]),
     "dg_sweep_score": (C.c_int, [_P, _P, _P, C.c_int, _P, C.c_int, _P, _P, _P, C.c_double, C.c_double, _P, _P, C.c_int,
                                  C.c_int, _P, _P, _P, C.c_int, _P]),
     "dg_sweep_run_files": (C.c_int, [_P, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, _P, _P, _P, _P, _P, C.c_int,

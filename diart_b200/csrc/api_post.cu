@@ -249,6 +249,11 @@ struct dg_sweep {
   ScoredRegions regions;          // dg_sweep_set_scored_regions
   int num_sets = 0;               // dg_sweep_set_trial_sets: > 0: emb is [num_sets][N][K][D], trial t reads set trial_set[t]
   std::vector<int32_t> trial_set;
+  int seed_nf = 0;                // dg_sweep_set_seeds: > 0: file f's states start from rows [seed_off[f], seed_off[f + 1])
+  std::vector<int32_t> seed_off;  // [seed_nf + 1]
+  std::vector<double> seeds;      // [seed_off[seed_nf]][D]
+  int named_nf = 0;               // dg_sweep_set_identities: > 0: the scoring calls score identification error
+  std::vector<int32_t> named;     // [named_nf][32]: per file and reference label, the hypothesis label of the same name or -1
   PinnedBuf pin;                  // params, taus and plan in; error flags, header, total and a turn prefix out
 };
 
@@ -301,6 +306,98 @@ extern "C" int dg_sweep_set_trial_sets(dg_sweep* h, int num_sets, const int32_t*
   return DG_OK;
 }
 
+extern "C" int dg_sweep_set_seeds(dg_sweep* h, int num_files, const int32_t* offsets_host, const double* centers_host) {
+  const char* who = "dg_sweep_set_seeds";
+  if (!h) {
+    set_error(std::string(who) + ": null handle");
+    return DG_EINVAL;
+  }
+  if (num_files < 0 || (num_files > 0 && !offsets_host)) {
+    set_error(std::string(who) + ": bad arguments (need num_files >= 0 and offsets when num_files > 0)");
+    return DG_EINVAL;
+  }
+  if (num_files > 0 && offsets_host[0] != 0) {
+    set_error(std::string(who) + ": seed offsets must start at 0");
+    return DG_EINVAL;
+  }
+  for (int f = 0; f < num_files; f++) {
+    const int n = offsets_host[f + 1] - offsets_host[f];
+    if (n < 0 || n > h->M) {
+      set_error(std::string(who) + ": file " + std::to_string(f) + " has " + std::to_string(n) + " centroids (need 0 .. "
+                "max_speakers = " + std::to_string(h->M) + "; offsets must not decrease)");
+      return DG_EINVAL;
+    }
+  }
+  const int n_total = num_files > 0 ? offsets_host[num_files] : 0;
+  if (n_total > 0 && !centers_host) {
+    set_error(std::string(who) + ": non-null centroids needed for " + std::to_string(n_total) + " rows");
+    return DG_EINVAL;
+  }
+  const int D = h->D;
+  for (int f = 0; f < num_files; f++)   // the rules of dg_multi_open_seeded
+    for (int i = offsets_host[f]; i < offsets_host[f + 1]; i++) {
+      double ss = 0.0;
+      bool finite = true;
+      for (int d = 0; d < D; d++) {
+        const double x = centers_host[(size_t)i * D + d];
+        finite = finite && std::isfinite(x);
+        ss += x * x;
+      }
+      if (!finite || !(ss > 0.0)) {
+        set_error(std::string(who) + ": centroid " + std::to_string(i - offsets_host[f]) + " of file " + std::to_string(f) +
+                  (finite ? " has a zero norm" : " is not finite"));
+        return DG_EINVAL;
+      }
+    }
+  h->seed_nf = num_files;
+  if (num_files > 0) h->seed_off.assign(offsets_host, offsets_host + num_files + 1);
+  else h->seed_off.clear();
+  h->seeds.assign(centers_host, centers_host + (size_t)n_total * D);
+  return DG_OK;
+}
+
+extern "C" int dg_sweep_set_identities(dg_sweep* h, int num_files, const int32_t* hyp_of_ref_host) {
+  const char* who = "dg_sweep_set_identities";
+  if (!h) {
+    set_error(std::string(who) + ": null handle");
+    return DG_EINVAL;
+  }
+  if (num_files < 0 || (num_files > 0 && !hyp_of_ref_host)) {
+    set_error(std::string(who) + ": bad arguments (need num_files >= 0 and a table when num_files > 0)");
+    return DG_EINVAL;
+  }
+  for (int f = 0; f < num_files; f++) {
+    unsigned seen = 0;
+    for (int r = 0; r < 32; r++) {
+      const int g = hyp_of_ref_host[(size_t)f * 32 + r];
+      if (g < -1 || g >= h->M) {
+        set_error(std::string(who) + ": file " + std::to_string(f) + ", reference label " + std::to_string(r) + ": entry " +
+                  std::to_string(g) + " outside [-1, max_speakers = " + std::to_string(h->M) + ")");
+        return DG_EINVAL;
+      }
+      if (g >= 0 && ((seen >> g) & 1u)) {
+        set_error(std::string(who) + ": file " + std::to_string(f) + ": hypothesis label " + std::to_string(g) +
+                  " is given to two reference labels");
+        return DG_EINVAL;
+      }
+      if (g >= 0) seen |= 1u << g;
+    }
+  }
+  h->named_nf = num_files;
+  h->named.assign(hyp_of_ref_host, hyp_of_ref_host + (size_t)num_files * 32);
+  return DG_OK;
+}
+
+// a scoring call over nf files while identities are set must cover exactly their files (before any launch)
+static int identities_check(const char* who, const dg_sweep* h, int nf) {
+  if (h->named_nf > 0 && h->named_nf != nf) {
+    set_error(std::string(who) + ": identities are set for " + std::to_string(h->named_nf) + " files, the call scores " +
+              std::to_string(nf) + " (set them again, or clear them with num_files = 0)");
+    return DG_EINVAL;
+  }
+  return DG_OK;
+}
+
 // at most this many (file, trial) states per call: der_hyp runs one warp per (state, label) with up to 32 labels and
 // numbers its threads in int32
 static const long long DG_SWEEP_MAX_STATES = 1LL << 21;
@@ -335,6 +432,11 @@ static int sweep_check(const char* who, dg_sweep* h, const float* seg_dev, const
   if (h->num_sets > 0 && (int)h->trial_set.size() != T) {
     set_error(std::string(who) + ": trial sets are set for " + std::to_string(h->trial_set.size()) + " trials, the call runs " +
               std::to_string(T) + " (set them again, or clear them with num_sets = 0)");
+    return DG_EINVAL;
+  }
+  if (h->seed_nf > 0 && h->seed_nf != nf) {
+    set_error(std::string(who) + ": seeds are set for " + std::to_string(h->seed_nf) + " files, the call clusters " +
+              std::to_string(nf) + " (set them again, or clear them with num_files = 0)");
     return DG_EINVAL;
   }
   int rc;
@@ -410,10 +512,14 @@ static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* em
   // with trial sets (dg_sweep_set_trial_sets) a trial row is {tau, rho, delta, set}, and the prep rows are per set
   const int G = h->num_sets, PS = G > 0 ? 4 : 3;
   // host -> device, one copy: params [T][PS], taus [T], states [S_run][2] (launch order), plan [Nv][stride], chunk offsets
-  // [nf + 1], then with vchunk_host the virtual chunk table [Nv]
+  // [nf + 1], then with vchunk_host the virtual chunk table [Nv], then with seeds (dg_sweep_set_seeds) their offsets [nf + 1]
+  // and, at the next multiple of 8 bytes, their centroids [n][D]
   const size_t params_b = (size_t)T * PS * 8, taus_b = (size_t)T * 8, states_b = (size_t)S_run * 8, plan_b = (size_t)Nv * stride * 4;
   const size_t off_b = (size_t)(nf + 1) * 4, vchunk_b = vchunk_host ? (size_t)Nv * 4 : 0;
-  const size_t in_b = params_b + taus_b + states_b + plan_b + off_b + vchunk_b;
+  const bool seeded = h->seed_nf > 0;
+  const size_t base_b = params_b + taus_b + states_b + plan_b + off_b + vchunk_b;
+  const size_t soff_b = seeded ? off_b : 0, seeds_at = (base_b + soff_b + 7) & ~(size_t)7;
+  const size_t in_b = seeded ? seeds_at + h->seeds.size() * 8 : base_b;
   const TurnOut lay = sweep_out(S, T, Nv);
   const size_t init_b = lay.at, header_b = lay.header_bytes;
   // the device turn buffer starts at a guess and grows to the true count (the kernel counts every turn, writes those that fit)
@@ -439,6 +545,10 @@ static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* em
   memcpy(pin + params_b + taus_b + states_b, plan_host, plan_b);
   memcpy(pin + params_b + taus_b + states_b + plan_b, chunk_off, off_b);
   if (vchunk_host) memcpy(pin + params_b + taus_b + states_b + plan_b + off_b, vchunk_host, vchunk_b);
+  if (seeded) {
+    memcpy(pin + base_b, h->seed_off.data(), soff_b);
+    if (!h->seeds.empty()) memcpy(pin + seeds_at, h->seeds.data(), h->seeds.size() * 8);
+  }
   unsigned char* din = h->in.as<unsigned char>();
   DG_CUDA(cudaMemcpyAsync(din, pin, in_b, cudaMemcpyHostToDevice, st));
   const double* d_params = reinterpret_cast<const double*>(din);
@@ -451,11 +561,15 @@ static int sweep_cluster_post(dg_sweep* h, const float* seg_dev, const float* em
   DG_CUDA(cudaMemsetAsync(h->centers.p, 0, (size_t)S * M * D * 8, st));
   DG_CUDA(cudaMemsetAsync(h->active.p, 0, (size_t)S * 32 * 4, st));
   DG_CUDA(cudaMemsetAsync(h->init.p, 0, init_b, st));
+  int rc;
+  // a seeded file's states start from its known centroids instead (dg_multi_open_seeded's state)
+  if (seeded && (rc = launch_sweep_seed(reinterpret_cast<const int*>(din + base_b), reinterpret_cast<const double*>(din + seeds_at),
+                                        nf, T, M, D, h->centers.as<double>(), h->active.as<int>(), h->init.as<int>(), st)))
+    return rc;
   ClusterParams p{};
   p.M = M;
   p.D = D;
   p.metric = 0;
-  int rc;
   if (G > 0)
     rc = launch_cluster_sweep_sets(p, d_params, T, d_states, S_run, d_off, seg_dev, emb_dev, G, N, F, K, h->centers.as<double>(),
                                    h->active.as<int>(), h->init.as<int>(), h->prep.as<float>(), h->prep_d.as<double>(), maps, st);
@@ -572,18 +686,19 @@ static int der_components(const char* who, DerBufs& b, PinnedBuf& pinbuf, const 
                           const double* out_start_host, const double* out_res_host, const double* shift_host, double collar,
                           const double* ref_host, const int32_t* ref_label_host, const int32_t* ref_off, const int32_t* R_host,
                           double* components_host, int32_t* hyp_offsets_dev, double* hyp_segments_dev, int hyp_cap,
-                          cudaStream_t st, const ScoredRegions* regions = nullptr) {
+                          cudaStream_t st, const ScoredRegions* regions = nullptr, const int32_t* named = nullptr) {
   int rc;
   const int NTM = nf * T * M, S = ref_off[nf];
   const bool crop = regions && regions->nf > 0;
   // host -> device, one copy: out_start [N], out_res [N], shifts [nf], reference segments [S][2] grouped by label within each
   // file, label offsets [nf][DER_ROFF], label counts [nf], chunk offsets [nf + 1], then with regions the scored pieces [U][2]
-  // (at the next multiple of 8 bytes) and their offsets [nf + 1]
+  // (at the next multiple of 8 bytes) and their offsets [nf + 1], then with named (identification error) its table [nf][32]
   const size_t times_b = (size_t)N * 16, shift_b = (size_t)nf * 8, rseg_b = (size_t)S * 16;
   const size_t roff_b = (size_t)nf * DER_ROFF * 4, R_b = (size_t)nf * 4, off_b = (size_t)(nf + 1) * 4;
   const size_t base_b = times_b + shift_b + rseg_b + roff_b + R_b + off_b, useg_at = (base_b + 7) & ~(size_t)7;
   const size_t useg_b = crop ? regions->rows.size() * 8 : 0, uoff_b = crop ? (size_t)(nf + 1) * 4 : 0;
-  const size_t in_b = crop ? useg_at + useg_b + uoff_b : base_b, comp_b = (size_t)nf * T * 40;
+  const size_t named_at = crop ? useg_at + useg_b + uoff_b : base_b, named_b = named ? (size_t)nf * 32 * 4 : 0;
+  const size_t in_b = named_at + named_b, comp_b = (size_t)nf * T * 40;
   if (b.in.ensure(in_b) || b.hoff.ensure((size_t)(NTM + 1) * 4) || b.hseg.ensure((size_t)std::max(total, 1u) * 16) ||
       b.comp.ensure(comp_b) || pinbuf.ensure(std::max(in_b, comp_b + 16)))
     return DG_ECUDA;
@@ -599,6 +714,7 @@ static int der_components(const char* who, DerBufs& b, PinnedBuf& pinbuf, const 
     if (useg_b) memcpy(pin + useg_at, regions->rows.data(), useg_b);
     memcpy(pin + useg_at + useg_b, regions->off.data(), uoff_b);
   }
+  if (named) memcpy(pin + named_at, named, named_b);
   for (int f = 0; f < nf; f++) {
     const int a = ref_off[f], n = ref_off[f + 1] - a, R = R_host[f];
     int32_t* roff = roff_all + (size_t)f * DER_ROFF;
@@ -625,12 +741,13 @@ static int der_components(const char* who, DerBufs& b, PinnedBuf& pinbuf, const 
   const int* d_off = reinterpret_cast<const int*>(din + times_b + shift_b + rseg_b + roff_b + R_b);
   const double* d_useg = crop ? reinterpret_cast<const double*>(din + useg_at) : nullptr;
   const int* d_uoff = crop ? reinterpret_cast<const int*>(din + useg_at + useg_b) : nullptr;
+  const int* d_named = named ? reinterpret_cast<const int*>(din + named_at) : nullptr;
   int* hoff = b.hoff.as<int>();
   if ((rc = launch_der_hyp_count(header_dev, turns_dev, nf, d_off, T, N, M, d_start, d_res, d_shift, collar, hoff, st)) ||
       (rc = launch_der_hyp_write(header_dev, turns_dev, nf, d_off, T, N, M, d_start, d_res, d_shift, collar, hoff,
                                  b.hseg.as<double>(), hyp_segments_dev, hyp_cap, st)) ||
       (rc = launch_der_score(hoff, b.hseg.as<double>(), nf, T, M, d_roff, d_R, d_rseg, b.comp.as<double>(), st, d_uoff,
-                             d_useg)))
+                             d_useg, d_named)))
     return rc;
   if (hyp_offsets_dev) DG_CUDA(cudaMemcpyAsync(hyp_offsets_dev, hoff, (size_t)(NTM + 1) * 4, cudaMemcpyDeviceToDevice, st));
   DG_CUDA(cudaMemcpyAsync(pin, b.comp.p, comp_b, cudaMemcpyDeviceToHost, st));
@@ -701,7 +818,7 @@ static int sweep_score(const char* who, dg_sweep* h, const float* seg_dev, const
       (rc = check_file_plans(who, plan_host, nf, chunk_off, h->nw, h->F)) ||
       (rc = score_check(who, N, nf, out_start_host, out_res_host, shift_host, collar, ref_host, ref_label_host, ref_off,
                         R_host, components_host, hyp_cap)) ||
-      (rc = regions_check(who, h->regions, nf)))
+      (rc = regions_check(who, h->regions, nf)) || (rc = identities_check(who, h, nf)))
     return rc;
   DG_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)stream;
@@ -711,7 +828,8 @@ static int sweep_score(const char* who, dg_sweep* h, const float* seg_dev, const
     return rc;
   return der_components(who, h->der, h->pin, h->header.as<int32_t>(), h->turns.as<uint32_t>(), total, N, nf, chunk_off, T,
                         h->M, out_start_host, out_res_host, shift_host, collar, ref_host, ref_label_host, ref_off, R_host,
-                        components_host, hyp_offsets_dev, hyp_segments_dev, hyp_cap, st, &h->regions);
+                        components_host, hyp_offsets_dev, hyp_segments_dev, hyp_cap, st, &h->regions,
+                        h->named_nf > 0 ? h->named.data() : nullptr);
 }
 
 extern "C" int dg_sweep_score(dg_sweep* h, const float* seg_dev, const float* emb_dev, int N, const double* params_host,
@@ -849,7 +967,7 @@ extern "C" int dg_sweep_score_latencies(dg_sweep* h, const float* seg_dev, const
   const int Nv = num_virtual, nvf = num_virtual_files;
   if ((rc = score_check(who, Nv, nvf, out_start_host, out_res_host, shifts_host, collar, ref_host, ref_label_host,
                         ref_offsets_host, ref_label_counts_host, components_host, 0)) ||
-      (rc = regions_check(who, h->regions, nvf)))
+      (rc = regions_check(who, h->regions, nvf)) || (rc = identities_check(who, h, nvf)))
     return rc;
   DG_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)stream;
@@ -860,7 +978,7 @@ extern "C" int dg_sweep_score_latencies(dg_sweep* h, const float* seg_dev, const
   return der_components(who, h->der, h->pin, h->header.as<int32_t>(), h->turns.as<uint32_t>(), total, Nv, nvf,
                         virtual_offsets_host, T, h->M, out_start_host, out_res_host, shifts_host, collar, ref_host,
                         ref_label_host, ref_offsets_host, ref_label_counts_host, components_host, nullptr, nullptr, 0, st,
-                        &h->regions);
+                        &h->regions, h->named_nf > 0 ? h->named.data() : nullptr);
 }
 
 // ============================================================================= voice activity detection sweep

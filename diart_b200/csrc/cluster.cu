@@ -549,6 +549,31 @@ int launch_cluster_sweep_sets(const ClusterParams& p, const double* trials_dev, 
   return 0;
 }
 
+// One CTA per sweep state s = f T + t: copies file f's known centroids into rows 0 .. n_f - 1 of centroid table s and marks
+// them active; the state counts as initialised when n_f > 0, so cluster_seq takes the distance path from its first chunk (the
+// reference's identify with `centers` already set).  Tables of states whose file has no centroids stay as zeroed.
+__global__ void __launch_bounds__(256) sweep_seed_kernel(const int* __restrict__ seed_off, const double* __restrict__ seeds,
+                                                         int T, int M, int D, double* __restrict__ centers,
+                                                         int* __restrict__ active, int* __restrict__ initialized) {
+  const size_t s = blockIdx.x;
+  const int f = (int)(s / T), a = seed_off[f], n = seed_off[f + 1] - a;
+  if (n == 0) return;
+  const double* src = seeds + (size_t)a * D;
+  double* dst = centers + s * M * D;
+  for (int i = threadIdx.x; i < n * D; i += blockDim.x) dst[i] = src[i];
+  if ((int)threadIdx.x < n) active[s * CM + threadIdx.x] = 1;
+  if (threadIdx.x == 0) initialized[s * 2] = 1;
+}
+
+int launch_sweep_seed(const int* seed_off, const double* seeds, int nf, int T, int M, int D, double* centers, int* active,
+                      int* initialized, cudaStream_t st) {
+  ProfScope _ps("sweep_seed", st);
+  if (nf <= 0 || T <= 0) return 0;
+  sweep_seed_kernel<<<(unsigned)((long long)nf * T), 256, 0, st>>>(seed_off, seeds, T, M, D, centers, active, initialized);
+  DG_LAUNCHED();
+  return 0;
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // Shared-identity mode (extension beyond the reference, SURVEY.md 8(e) / BASELINE config 5): G ranks diarize
 // independent streams against ONE table of global speakers.  After every pipeline step each rank exports a

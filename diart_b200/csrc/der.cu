@@ -9,8 +9,10 @@
 //   der_scan                         exclusive prefix sum of the (file, trial, label) counts
 //   der_score                        one warp per (file, trial) against that file's reference: k-way merge of the boundary
 //                                    lists (one lane per hypothesis label and per reference label), co-occurrence matrix,
-//                                    LSAP, the five components; der_score<true> first crops each hypothesis label to the
-//                                    file's scored pieces (CropList)
+//                                    LSAP, the five components; der_score<true, *> first crops each hypothesis label to the
+//                                    file's scored pieces (CropList); der_score<*, true> scores the identification error
+//                                    rate: no co-occurrence and no LSAP, each reference label's partner is the hypothesis
+//                                    label of the same name, from a per-file table
 //
 // Every float64 operation is explicitly rounded (no FMA contraction): the segment times equal numpy's turn_times /
 // assemble_predictions bit for bit, and the components are sums in time order, independent of the launch geometry.
@@ -218,13 +220,15 @@ __device__ __forceinline__ void der_walk(const double* hp, int h0, int h1, const
 
 // comp [nf][T][5] = {false alarm, missed detection, confusion, correct, total}; warp (f, t) scores trial t of file f against
 // file f's reference: R[f] labels at offsets roff [f][DER_ROFF] into rseg.  CROP: every hypothesis label is first cropped to
-// file f's scored pieces [uoff[f], uoff[f + 1]) of useg (CropList); the reference comes cropped from the host.
-template <bool CROP>
+// file f's scored pieces [uoff[f], uoff[f + 1]) of useg (CropList); the reference comes cropped from the host.  NAMED (the
+// identification error rate, DESIGN.md "Identification error"): reference label r of file f is matched to hypothesis label
+// named [f][r] (-1: none) instead of the LSAP's partner; pass 2 is the same.
+template <bool CROP, bool NAMED>
 __global__ void __launch_bounds__(DER_SCORE_THREADS)
 der_score_kernel(const int* __restrict__ hoff /*[nf*T*M+1]*/, const double* __restrict__ hseg, int nf, int T, int M,
                  const int* __restrict__ roff_all /*[nf][DER_ROFF]*/, const int* __restrict__ R_all /*[nf]*/,
                  const double* __restrict__ rseg, double* __restrict__ comp, const int* __restrict__ uoff /*[nf+1]*/,
-                 const double* __restrict__ useg) {
+                 const double* __restrict__ useg, const int* __restrict__ named /*[nf][32]*/) {
   __shared__ double tr[DER_SCORE_THREADS / 32][32][33];
   const int ft = (int)(((size_t)blockIdx.x * DER_SCORE_THREADS + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (ft >= nf * T) return;
@@ -233,6 +237,10 @@ der_score_kernel(const int* __restrict__ hoff /*[nf*T*M+1]*/, const double* __re
   const int h0 = lane < M ? hoff[ft * M + lane] : 0, h1 = lane < M ? hoff[ft * M + lane + 1] : 0;
   const int r0 = lane < R ? roff[lane] : 0, r1 = lane < R ? roff[lane + 1] : 0;
   const int u0 = CROP ? uoff[f] : 0, u1 = CROP ? uoff[f + 1] : 0;
+  int partner = -1;   // lane r: the hypothesis label mapped to reference label r
+  if constexpr (NAMED) {
+    if (lane < R) partner = named[(size_t)f * 32 + lane];
+  } else {
   // pass 1: co-occurrence C[r][h], lane h owns column h, each entry summed in time order
   double C[32];
 #pragma unroll
@@ -244,7 +252,6 @@ der_score_kernel(const int* __restrict__ hoff /*[nf*T*M+1]*/, const double* __re
       if (ah && ((rmask >> q) & 1u)) C[q] = __dadd_rn(C[q], d);
   });
   // the one-to-one mapping of maximal total co-occurrence: LSAP on -C, rows = the smaller side (scipy transposes a tall matrix)
-  int partner = -1;   // lane r: the hypothesis label mapped to reference label r
   if (R > 0) {
     double(&s)[32][33] = tr[threadIdx.x >> 5];
 #pragma unroll
@@ -263,6 +270,7 @@ der_score_kernel(const int* __restrict__ hoff /*[nf*T*M+1]*/, const double* __re
         if (lane == r) partner = h;
       }
     }
+  }
   }
   // pass 2: the components, in time order
   double fa = 0.0, miss = 0.0, conf = 0.0, corr = 0.0, tot = 0.0;
@@ -313,14 +321,21 @@ int launch_der_hyp_write(const int32_t* header, const uint32_t* turns, int nf, c
 }
 
 int launch_der_score(const int* hoff, const double* hseg, int nf, int T, int M, const int* roff, const int* R,
-                     const double* rseg, double* comp, cudaStream_t st, const int* uoff, const double* useg) {
+                     const double* rseg, double* comp, cudaStream_t st, const int* uoff, const double* useg, const int* named) {
   ProfScope _ps("der_score", st);
   const unsigned blocks = (unsigned)(((long long)nf * T * 32 + DER_SCORE_THREADS - 1) / DER_SCORE_THREADS);
-  if (uoff)
-    der_score_kernel<true><<<blocks, DER_SCORE_THREADS, 0, st>>>(hoff, hseg, nf, T, M, roff, R, rseg, comp, uoff, useg);
+  if (uoff && named)
+    der_score_kernel<true, true><<<blocks, DER_SCORE_THREADS, 0, st>>>(hoff, hseg, nf, T, M, roff, R, rseg, comp, uoff, useg,
+                                                                      named);
+  else if (uoff)
+    der_score_kernel<true, false><<<blocks, DER_SCORE_THREADS, 0, st>>>(hoff, hseg, nf, T, M, roff, R, rseg, comp, uoff, useg,
+                                                                       nullptr);
+  else if (named)
+    der_score_kernel<false, true><<<blocks, DER_SCORE_THREADS, 0, st>>>(hoff, hseg, nf, T, M, roff, R, rseg, comp, nullptr,
+                                                                       nullptr, named);
   else
-    der_score_kernel<false><<<blocks, DER_SCORE_THREADS, 0, st>>>(hoff, hseg, nf, T, M, roff, R, rseg, comp, nullptr,
-                                                                 nullptr);
+    der_score_kernel<false, false><<<blocks, DER_SCORE_THREADS, 0, st>>>(hoff, hseg, nf, T, M, roff, R, rseg, comp, nullptr,
+                                                                        nullptr, nullptr);
   DG_LAUNCHED();
   return 0;
 }

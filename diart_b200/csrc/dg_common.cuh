@@ -289,6 +289,11 @@ int launch_cluster_sweep_sets(const ClusterParams& p, const double* trials_dev, 
                               double* centers, int* active, int* initialized, float* prep, double* prep_d, int32_t* maps,
                               cudaStream_t st);
 size_t cluster_prep_floats(int B, int K);
+// the seeded start of nf * T sweep states (state s = f T + t, tables as launch_cluster_sweep, already zeroed): file f's known
+// centroids are rows [seed_off[f], seed_off[f + 1]) of seeds [n][D]; state s gets them as centres 0 .. n_f - 1, active, and
+// initialized [s][0] = 1 when n_f > 0 (dg_multi_open_seeded's state for a stream)
+int launch_sweep_seed(const int* seed_off, const double* seeds, int nf, int T, int M, int D, double* centers, int* active,
+                      int* initialized, cudaStream_t st);
 // post.cu -- aggregation + binarisation + run-length turns (reference diarization.py:205-232) of the sweeps: Nv virtual chunks,
 // virtual chunk c = real chunk vchunk[c] (vchunk null: chunk c) of the N whose scores seg [N][F][K] and maps [T][N][K] are
 // given; header [T][Nv][4]; trial t thresholds at taus[t]
@@ -332,11 +337,13 @@ int launch_der_hyp_write(const int32_t* header, const uint32_t* turns, int nf, c
                          double* segs, double* segs_copy, int copy_cap, cudaStream_t st);
 // reference of file f: R[f] labels, offsets roff [f][DER_ROFF] (R[f] + 1 used) into rseg [S][2];
 // comp [nf][T][5] = {false alarm, missed, confusion, correct, total}.  With uoff (device [nf + 1]) the hypothesis of file f is
-// cropped to its scored pieces useg [uoff[f], uoff[f + 1])[2] (sorted, apart by more than 1e-6 s, each truthy)
+// cropped to its scored pieces useg [uoff[f], uoff[f + 1])[2] (sorted, apart by more than 1e-6 s, each truthy).  With named
+// (device [nf][32]) the identification error: reference label r of file f is matched to hypothesis label named[f][r] (-1:
+// none) instead of the optimal mapping
 constexpr int DER_ROFF = 33;
 int launch_der_score(const int* hoff, const double* hseg, int nf, int T, int M, const int* roff, const int* R,
                      const double* rseg, double* comp, cudaStream_t st, const int* uoff = nullptr,
-                     const double* useg = nullptr);
+                     const double* useg = nullptr, const int* named = nullptr);
 // vad.cu -- VAD sweep: the speech curve of Nv chunks (max over K local speakers, aggregated as the post-path with one speaker;
 // chunk c's frames at curve [curve_off[c], curve_off[c + 1])), chunk c = real chunk vchunk[c] of seg (vchunk null: chunk c);
 // then per trial t the turns of curve > taus[t], header [T][N][4]

@@ -143,7 +143,7 @@ def enroll(config, clips: Sequence[Tuple[str, np.ndarray]], timing: Optional[Dic
     params = trial_params([{}], config)
     out = ds.sweep(params, keep_state=True)
     labels = speaker_labels(None, config.max_speakers)
-    predictions = ds._run(params, lambda _: out, labels)        # the Annotations DatasetSweep.run([{}]) builds
+    predictions = ds._run(params, lambda _: out, ds.labels)     # the Annotations DatasetSweep.run([{}]) builds
     dominant = []
     for name, (prediction,) in zip(names, predictions):
         g = dominant_speaker(prediction, labels)

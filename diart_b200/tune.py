@@ -40,6 +40,12 @@ pass computes the scores once and the embeddings of every constructed *OSP set* 
 clustering reads the embeddings of its own set (``dg_sweep_set_trial_sets``; DESIGN.md "Sweeps over overlap-aware
 weightings").
 
+With known speakers (``DatasetSweep(..., speakers=...)``, :class:`~diart_b200.speakers.KnownSpeakers` per file) every
+(file, trial) clustering starts from the file's centroids, as ``SpeakerDiarization.set_known_speakers`` starts a pipeline
+(``dg_sweep_set_seeds``), and the speakers carry their names.  :class:`IdentificationErrorRate` then scores whether the names
+are right: the DER components with each reference label matched to the hypothesis label of the same name instead of by the
+optimal mapping (``dg_sweep_set_identities``; DESIGN.md "Identification error").
+
 The three classes share their mechanics: :class:`FileBatches` cuts the window batches of every network pass,
 :func:`stream_plan` is the post-path plan of one file, ``_timed`` puts CUDA events around one C call and ``_turn_list_call``
 downloads a turn list into a host buffer that grows on demand.  ``HyperParameterSweep._run_trials`` / ``_score_trials`` are the
@@ -69,6 +75,7 @@ from .blocks.vad import VoiceActivityDetection, VoiceActivityDetectionConfig
 from .core import Annotation, Segment
 from .models import B200PyanNet
 from .operators import DeviceAudioStream
+from .speakers import KnownSpeakers, speaker_labels
 
 NETWORK_BATCH = 256           # windows per network step (the benchmarked batch)
 STREAM_FORM_MIN_BATCH = 4     # the sinc front end's stream form runs for batches of this many windows on (api_seg.cu)
@@ -173,6 +180,24 @@ def _set_trial_sets(handle, trial_sets: Optional[Tuple[int, np.ndarray]]):
         _lib.check(_lib.lib().dg_sweep_set_trial_sets(handle, int(G), index.ctypes.data, len(index)))
 
 
+def _set_seeds(handle, seeds: Optional[Tuple[np.ndarray, np.ndarray]]):
+    """the handle's known centroids for its next clustering calls: (offsets int32 (files + 1,), centroids float64 (n, D)) per
+    clustering file, or None (every state starts fresh)"""
+    if seeds is None:
+        _lib.check(_lib.lib().dg_sweep_set_seeds(handle, 0, None, None))
+    else:
+        offsets, centers = seeds
+        _lib.check(_lib.lib().dg_sweep_set_seeds(handle, len(offsets) - 1, offsets.ctypes.data, centers.ctypes.data))
+
+
+def _set_identities(handle, table: Optional[np.ndarray]):
+    """the handle's name matching for its next scoring calls: :func:`pack_identities`' table, or None (DER)"""
+    if table is None:
+        _lib.check(_lib.lib().dg_sweep_set_identities(handle, 0, None))
+    else:
+        _lib.check(_lib.lib().dg_sweep_set_identities(handle, len(table), table.ctypes.data))
+
+
 @dataclass
 class FileWindows:
     """What ``FileAudioSource`` + ``rearrange_audio_stream`` make of one file."""
@@ -273,6 +298,15 @@ class DiarizationErrorRate:
 
 
 @dataclass(frozen=True)
+class IdentificationErrorRate:
+    """The same for pyannote.metrics' ``IdentificationErrorRate``: DER's components with the labels matched by name instead
+    of by the optimal mapping, for a :class:`DatasetSweep` whose speakers carry names (``speakers=``).  Only unit weights
+    (pyannote's ``confusion``, ``miss`` and ``false_alarm`` arguments) are supported."""
+    collar: float = 0.0
+    skip_overlap: bool = False
+
+
+@dataclass(frozen=True)
 class DetectionErrorRate:
     """The same for pyannote.metrics' ``DetectionErrorRate``, the metric of :class:`VoiceActivitySweep`."""
     collar: float = 0.0
@@ -292,6 +326,23 @@ def metric_protocol(metric, kind: str) -> Tuple[float, bool]:
             not math.isfinite(float(collar)) or float(collar) < 0:
         raise ValueError(f"metric collar {collar!r}: need a finite number >= 0")
     return float(collar), bool(metric.skip_overlap)
+
+
+IER_WEIGHTS = ("confusion", "miss", "false_alarm")   # pyannote's IdentificationErrorRate weights; only 1 is supported
+
+
+def diarization_metric(metric) -> Tuple[str, float, bool]:
+    """``metric`` of a :class:`DatasetSweep` (None: the default) -> (its class name, collar, skip_overlap): a
+    :class:`DiarizationErrorRate` or an :class:`IdentificationErrorRate` (or pyannote.metrics' class of either name) as
+    :func:`metric_protocol` accepts them; an identification error rate whose ``confusion``, ``miss`` or ``false_alarm``
+    weight is not 1: ValueError."""
+    kind = "IdentificationErrorRate" if type(metric).__name__ == "IdentificationErrorRate" else "DiarizationErrorRate"
+    if kind == "IdentificationErrorRate":
+        for name in IER_WEIGHTS:
+            w = getattr(metric, name, 1.0)
+            if isinstance(w, bool) or not isinstance(w, (int, float, np.integer, np.floating)) or float(w) != 1.0:
+                raise ValueError(f"metric {name} weight {w!r}: only unit weights are supported")
+    return (kind, *metric_protocol(metric, kind))
 
 
 def check_uem(uem) -> Optional[List[Tuple[float, float]]]:
@@ -447,6 +498,25 @@ def reference_arrays(annotation: Annotation, regions: Optional[Sequence[Tuple[fl
     return (np.array(rows, dtype=np.float64).reshape(-1, 2), np.array(labels, dtype=np.int32), names)
 
 
+def identity_table(names: Sequence, labels: Sequence[str]) -> np.ndarray:
+    """reference label names (string order, ``reference_arrays``) and a file's hypothesis labels -> int32 (32,): for reference
+    label r the index g of the hypothesis label equal to its name, else -1 (also for r >= len(names))"""
+    index = {label: g for g, label in enumerate(labels)}
+    out = np.full(MAX_REFERENCE_LABELS, -1, dtype=np.int32)
+    for r, name in enumerate(names):
+        out[r] = index.get(name, -1)
+    return out
+
+
+def pack_identities(references: Sequence[Annotation], regions: Optional[Sequence], labels: Sequence[Sequence[str]]) \
+        -> np.ndarray:
+    """per-file references, scored regions (or None) and hypothesis labels -> the table of dg_sweep_set_identities, int32
+    (files, 32): each file's :func:`identity_table` of the reference's names after cropping to its regions"""
+    return np.ascontiguousarray(np.stack([
+        identity_table(reference_arrays(ref, None if regions is None else regions[f])[2], labels[f])
+        for f, ref in enumerate(references)]), dtype=np.int32)
+
+
 def _rate(num: np.ndarray, total: np.ndarray) -> np.ndarray:
     """num / total per trial, as a fraction; with total = 0: 0 when num is 0, else 1 (pyannote's ``compute_metric`` of both
     error rates)"""
@@ -480,6 +550,21 @@ class DERComponents:
     def __add__(self, other: "DERComponents") -> "DERComponents":
         """the components of several files summed per trial (the "TOTAL" row of pyannote's report)"""
         return DERComponents.from_array(self.as_array() + other.as_array())
+
+
+@dataclass
+class IdentificationErrorComponents(DERComponents):
+    """Identification error rate components in seconds, one entry per trial: the fields of :class:`DERComponents`, the
+    labels matched by name."""
+
+    @property
+    def ier(self) -> np.ndarray:
+        """(false alarm + missed detection + confusion) / total per trial (:func:`_rate`)"""
+        return _rate(self.false_alarm + self.missed_detection + self.confusion, self.total)
+
+    def __add__(self, other: "IdentificationErrorComponents") -> "IdentificationErrorComponents":
+        """the components of several files summed per trial"""
+        return IdentificationErrorComponents.from_array(self.as_array() + other.as_array())
 
 
 @dataclass
@@ -883,15 +968,18 @@ class HyperParameterSweep:
         return self._h, nw
 
     def _run_trials(self, entry, file_args: tuple, lead: tuple, seg: torch.Tensor, emb: torch.Tensor, plans,
-                    params: np.ndarray, keep_state: bool, trial_sets: Optional[Tuple[int, np.ndarray]] = None) -> SweepOutputs:
+                    params: np.ndarray, keep_state: bool, trial_sets: Optional[Tuple[int, np.ndarray]] = None,
+                    seeds: Optional[Tuple[np.ndarray, np.ndarray]] = None) -> SweepOutputs:
         """The body of :meth:`sweep` and :meth:`DatasetSweep.sweep`.  ``entry``: dg_sweep_run, or dg_sweep_run_files with
         ``file_args`` = what it takes after the chunk count (files, chunk offsets) and ``lead`` = (files,), the leading
         dimension of its centroids.  ``plans``: (plan, out_start, out_res) of the N chunks.  ``trial_sets``: (G, set of each
-        trial) with ``emb`` (G, N, K, D), or None with ``emb`` (N, K, D)."""
+        trial) with ``emb`` (G, N, K, D), or None with ``emb`` (N, K, D).  ``seeds``: the files' known centroids
+        (:func:`_set_seeds`), or None."""
         N, F, K = seg.shape
         D, M = emb.shape[-1], int(self.config.max_speakers)
         h, _ = self._handle(F, K, D)
         _set_trial_sets(h, trial_sets)
+        _set_seeds(h, seeds)
         plan, out_start, out_res = plans
         params = np.ascontiguousarray(params, dtype=np.float64)
         T = len(params)
@@ -905,18 +993,22 @@ class HyperParameterSweep:
 
     def _score_trials(self, entry, file_args: tuple, lead: tuple, seg: torch.Tensor, emb: torch.Tensor, plans,
                       params: np.ndarray, shift, reference: tuple, segments: bool = False, regions: Optional[tuple] = None,
-                      trial_sets: Optional[Tuple[int, np.ndarray]] = None):
+                      trial_sets: Optional[Tuple[int, np.ndarray]] = None,
+                      seeds: Optional[Tuple[np.ndarray, np.ndarray]] = None, identities: Optional[np.ndarray] = None):
         """The body of :meth:`sweep_score` and of each launch of :meth:`DatasetSweep.score` -> (components ``lead`` +
         (T, 5), device seconds, hypothesis offsets, hypothesis segments).  ``entry``: dg_sweep_score, or
         dg_sweep_score_files with ``file_args`` and ``lead`` as in :meth:`_run_trials`.  ``shift``: the timestamp shift, or
         the address of the per-file shifts.  ``reference``: the entry point's four reference arguments (rows, labels,
         then the row and label counts, or the addresses of the per-file row offsets and label counts).  ``segments`` is
         for the one-file entry point.  ``regions``: ``pack_regions`` of the files' scored regions, or None.  ``trial_sets``
-        as in :meth:`_run_trials`."""
+        and ``seeds`` as in :meth:`_run_trials`.  ``identities``: :func:`pack_identities`' table to score the identification
+        error rate, or None (DER)."""
         N, F, K = seg.shape
         h, _ = self._handle(F, K, emb.shape[-1])
         _set_regions(_lib.lib().dg_sweep_set_scored_regions, h, regions)
         _set_trial_sets(h, trial_sets)
+        _set_seeds(h, seeds)
+        _set_identities(h, identities)
         plan, out_start, out_res = plans
         params = np.ascontiguousarray(params, dtype=np.float64)
         T, M = len(params), int(self.config.max_speakers)
@@ -1112,19 +1204,29 @@ class _DatasetSweep:
         references f indexes (a virtual file's in the sweeps over several latencies)"""
         raise NotImplementedError
 
+    def _metric_kind(self, metric) -> Tuple[str, float, bool]:
+        """``metric`` -> (the class name it scores, collar, skip_overlap); anything this sweep does not score: ValueError"""
+        return (self._metric, *metric_protocol(metric, self._metric))
+
+    def _pack(self, kind: str, references: List[Annotation], regions: Optional[list], copies: int) -> tuple:
+        """the reference arguments of the scoring entry for metric class ``kind`` (files ``copies`` times)"""
+        return self._pack_references(references, regions)
+
     def _packed(self, metric, copies: int = 1) -> Tuple[tuple, Optional[tuple]]:
-        """the packed references and scored regions (``pack_regions``, or None where nothing is cropped) of ``metric``
-        (:func:`metric_protocol`) with the files' uems, every file ``copies`` times (latency-major), kept per (copies,
-        collar, skip_overlap) for later calls.  ``regions_seconds``: host seconds spent packing (about 0 when kept)."""
-        protocol = metric_protocol(metric, self._metric)
+        """the packed references (``_pack``) and scored regions (``pack_regions``, or None where nothing is cropped) of
+        ``metric`` (:meth:`_metric_kind`) with the files' uems, every file ``copies`` times (latency-major), kept per (copies,
+        metric kind, collar, skip_overlap) for later calls.  ``regions_seconds``: host seconds spent packing (about 0 when
+        kept)."""
+        kind, *protocol = self._metric_kind(metric)
+        protocol = tuple(protocol)
         self._check_references()
-        key = (copies, *protocol)
+        key = (copies, kind, *protocol)
         t0 = time.perf_counter()
         if key not in self._packs:
             regions = None
             if protocol != (0.0, False) or any(u is not None for u in self.uems):
                 regions = [scored_regions(ref, *protocol, uem) for ref, uem in zip(self.references, self.uems)] * copies
-            self._packs[key] = (self._pack_references(self.references * copies, regions),
+            self._packs[key] = (self._pack(kind, self.references * copies, regions, copies),
                                 None if regions is None else pack_regions(regions))
         self.regions_seconds = time.perf_counter() - t0
         return self._packs[key]
@@ -1133,9 +1235,9 @@ class _DatasetSweep:
     def num_chunks(self) -> int:
         return int(self.offsets[-1])
 
-    def _run(self, params: np.ndarray, launch, labels: Sequence[str]) -> List[List[Annotation]]:
+    def _run(self, params: np.ndarray, launch, labels: Sequence[Sequence[str]]) -> List[List[Annotation]]:
         """``launch``: the trials of one group -> their :class:`SweepOutputs` over the concatenated chunks.  -> predictions
-        [file][trial], each file's assembled from its own chunks and turns"""
+        [file][trial], each file's assembled from its own chunks and turns with its own speaker labels ``labels[f]``"""
         out: List[List[Annotation]] = [[] for _ in self.uris]
         dev = 0.0
         for g in trial_groups(len(params), self.num_chunks):
@@ -1144,7 +1246,7 @@ class _DatasetSweep:
             for f in range(len(self.uris)):
                 c0, c1 = int(self.offsets[f]), int(self.offsets[f + 1])
                 header, turns, n = file_turns(r.header, r.turns, c0, c1)
-                out[f] += assemble_predictions(header, turns, n, self.out_start[c0:c1], self.out_res[c0:c1], labels,
+                out[f] += assemble_predictions(header, turns, n, self.out_start[c0:c1], self.out_res[c0:c1], labels[f],
                                                float(self.shifts[f]), self.uris[f])
         self.timing["sweep"] = dev
         return out
@@ -1199,9 +1301,10 @@ class _DatasetSweep:
         (header, turns), or the real chunks where more (the clustering's maps are [T][real chunks][K])"""
         return max(len(tabs[0]), self.units.num_chunks)
 
-    def _run_latencies(self, params: np.ndarray, sel: List[int], launch, labels: Sequence[str]):
+    def _run_latencies(self, params: np.ndarray, sel: List[int], launch, labels: Sequence[Sequence[str]]):
         """``launch(params, tables)``: the trials of one group -> their :class:`SweepOutputs` over the virtual chunks of
-        ``tables``.  -> {latency: predictions [file][trial]}, each virtual file's assembled from its own chunks and turns"""
+        ``tables``.  -> {latency: predictions [file][trial]}, each virtual file's assembled from its own chunks and turns with
+        its file's speaker labels ``labels[f]``"""
         run = self._launched(sel)
         tabs = self._tables(run)
         vchunk, voff, _, out_start, out_res, shifts = tabs
@@ -1219,7 +1322,7 @@ class _DatasetSweep:
                     c0, c1 = int(voff[v]), int(voff[v + 1])
                     header, turns, n = file_turns(r.header, r.turns, c0, c1)
                     out[self.latencies[li]][f] += assemble_predictions(header, turns, n, out_start[c0:c1], out_res[c0:c1],
-                                                                       labels, float(shifts[v]), self.uris[f])
+                                                                       labels[f], float(shifts[v]), self.uris[f])
         self.timing["sweep"] = dev
         return out
 
@@ -1296,6 +1399,16 @@ class DatasetSweep(_DatasetSweep):
     each is clustered over its own set's embeddings in the same launches as the others: for every set the results are the
     bits a ``DatasetSweep`` whose config has that set's values gives.  A trial whose set was not constructed raises
     ValueError before any launch.  Without ``osp`` (or with only the config's set) the sweep runs as before.
+
+    ``speakers``: known speakers (:class:`~diart_b200.speakers.KnownSpeakers`), one for every file or a sequence with one
+    entry (a ``KnownSpeakers`` or None) per file; an empty one is None.  Every (file, trial) clustering then starts from the
+    file's centroids, and file f's global speaker g is labelled ``labels[f][g]`` (``speaker_labels``): for every file and
+    trial the results are those of ``SpeakerDiarization`` with ``set_known_speakers`` at that trial's values.  The latency
+    units of a file and every OSP set take the file's seeds.  A wrong length or type, another dimension than the
+    embeddings' or more than ``max_speakers`` speakers raises ValueError naming the file, before the network pass.
+    ``score`` and ``score_latencies`` also take an :class:`IdentificationErrorRate` (or pyannote.metrics' own, unit weights):
+    each reference label is matched to the hypothesis label of the same name, and the components come back as
+    :class:`IdentificationErrorComponents`.
     """
 
     _pack_references = staticmethod(pack_references)
@@ -1303,10 +1416,49 @@ class DatasetSweep(_DatasetSweep):
 
     def __init__(self, config: SpeakerDiarizationConfig, files: Iterable[Tuple[Optional[str], np.ndarray, Optional[Annotation]]],
                  sweep: Optional[HyperParameterSweep] = None, latencies: Optional[Iterable] = None,
-                 uems: Optional[Sequence] = None, osp: Optional[Iterable[Mapping]] = None):
+                 uems: Optional[Sequence] = None, osp: Optional[Iterable[Mapping]] = None, speakers=None):
         self._sweep = sweep
         self.osp_sets = osp_sets(config, osp if osp is not None else ())
+        self._speakers_arg = speakers
         super().__init__(config, files, latencies, uems)
+        self.labels = [speaker_labels(k, config.max_speakers) for k in self.speakers]
+        self._seeds = None
+        if any(k is not None for k in self.speakers):
+            # one seed table per clustering file: the files, or the latency units (each takes its file's centroids)
+            if self.units is None:
+                owner = list(range(len(self.uris)))
+            else:
+                owner = [0] * (len(self.units.unit_offsets) - 1)
+                for li in range(len(self.latencies)):
+                    for f in range(len(self.uris)):
+                        owner[int(self.units.unit_of[li, f])] = f
+            rows = [self.speakers[f].centroids if self.speakers[f] is not None else np.zeros((0, self.emb.shape[-1]))
+                    for f in owner]
+            self._seeds = (np.ascontiguousarray(np.cumsum([0] + [len(r) for r in rows]), dtype=np.int32),
+                           np.ascontiguousarray(np.concatenate(rows), dtype=np.float64))
+
+    def _check_speakers(self, chunk_samples: int):
+        """``speakers`` -> ``self.speakers``, one KnownSpeakers or None per file (ValueError naming the file)"""
+        speakers, nf, M = self._speakers_arg, len(self.uris), int(self.config.max_speakers)
+        if speakers is None or isinstance(speakers, KnownSpeakers):
+            speakers = [speakers] * nf
+        elif not isinstance(speakers, (list, tuple)) or len(speakers) != nf:
+            raise ValueError(f"speakers: need one KnownSpeakers for every file or one entry per file, {nf} in all")
+        D = self._sweep.pipeline._native_models()[1].dims(chunk_samples)[1]
+        out = []
+        for f, known in enumerate(speakers):
+            name = self.uris[f] if self.uris[f] is not None else f
+            if known is not None and not isinstance(known, KnownSpeakers):
+                raise ValueError(f"file {name}: speakers entry must be KnownSpeakers or None, not {type(known).__name__}")
+            if known is not None and len(known) == 0:
+                known = None
+            if known is not None and known.dimension != D:
+                raise ValueError(f"file {name}: the known speakers' centroids have dimension {known.dimension}, the "
+                                 f"embeddings {D}")
+            if known is not None and len(known) > M:
+                raise ValueError(f"file {name}: {len(known)} known speakers, at most max_speakers = {M}")
+            out.append(known)
+        self.speakers: List[Optional[KnownSpeakers]] = out
 
     def _open(self) -> torch.device:
         if self._sweep is None:
@@ -1314,6 +1466,7 @@ class DatasetSweep(_DatasetSweep):
         return self._sweep.device
 
     def _networks(self, fws: Sequence[FileWindows]):
+        self._check_speakers(fws[0].chunk_samples)              # the models are open; nothing has run yet
         if len(self.osp_sets) == 1:
             self.seg, self.emb = self._sweep.network_pass_files(fws)
             self.embs = self.emb[None]
@@ -1361,20 +1514,22 @@ class DatasetSweep(_DatasetSweep):
         if self.units is not None:
             raise ValueError("a sweep over several latencies runs through sweep_latencies")
         params, emb, sets = self._trial_sets(params)
-        return self._sweep._run_trials(*self._over_files(_lib.lib().dg_sweep_run_files, emb), params, keep_state, sets)
+        return self._sweep._run_trials(*self._over_files(_lib.lib().dg_sweep_run_files, emb), params, keep_state, sets,
+                                       self._seeds)
 
     def run(self, trials: Sequence[Mapping[str, float]] = ({},)) -> List[List[Annotation]]:
-        """-> predictions [file][trial]: what :meth:`HyperParameterSweep.run` returns for each file alone"""
+        """-> predictions [file][trial]: what :meth:`HyperParameterSweep.run` returns for each file alone (with known
+        speakers, what a pipeline seeded with the file's gives, its speakers labelled ``labels[f]``)"""
         if self.units is not None:
             return self.run_latencies(trials, [self.config.latency])[float(self.config.latency)]
-        labels = [f"speaker{g}" for g in range(int(self.config.max_speakers))]
-        return self._run(self._rows(trials), self.sweep, labels)
+        return self._run(self._rows(trials), self.sweep, self.labels)
 
     def score(self, trials: Sequence[Mapping[str, float]] = ({},), metric=None) \
             -> Tuple[List[DERComponents], DERComponents]:
         """-> (components per file, their sum in file order): per file what :meth:`HyperParameterSweep.score` returns for
         it alone with the same ``metric`` and the file's uem; ``total.der`` is the value ``Optimizer.objective``
-        minimises.  Every file needs a reference."""
+        minimises.  Every file needs a reference.  With an :class:`IdentificationErrorRate` the components are
+        :class:`IdentificationErrorComponents` (``total.ier``)."""
         if self.units is not None:
             return self.score_latencies(trials, [self.config.latency], metric)[float(self.config.latency)]
         return self._score(self._rows(trials), metric)
@@ -1394,8 +1549,7 @@ class DatasetSweep(_DatasetSweep):
         params, sel = self._rows(trials), self._selection(latencies)
         if self.units is None:
             return {self.latencies[0]: self.run(trials)}
-        labels = [f"speaker{g}" for g in range(int(self.config.max_speakers))]
-        return self._run_latencies(params, sel, self._sweep_virtual, labels)
+        return self._run_latencies(params, sel, self._sweep_virtual, self.labels)
 
     def score_latencies(self, trials: Sequence[Mapping[str, float]] = ({},), latencies=None, metric=None) \
             -> Dict[float, Tuple[List[DERComponents], DERComponents]]:
@@ -1415,6 +1569,7 @@ class DatasetSweep(_DatasetSweep):
         h, _ = sw._handle(F, K, self.emb.shape[2], self.units.nw)
         params, emb, sets = self._trial_sets(params)
         _set_trial_sets(h, sets)
+        _set_seeds(h, self._seeds)
         plan, out_start, out_res = tabs[2:5]
         params = np.ascontiguousarray(params, dtype=np.float64)
         T, Nv = len(params), len(tabs[0])
@@ -1434,24 +1589,37 @@ class DatasetSweep(_DatasetSweep):
         _set_regions(_lib.lib().dg_sweep_set_scored_regions, h, regions)
         params, emb, sets = self._trial_sets(params)
         _set_trial_sets(h, sets)
+        _set_seeds(h, self._seeds)
+        _set_identities(h, refs[4] if len(refs) > 4 else None)
         plan, out_start, out_res, shifts = tabs[2:]
         params = np.ascontiguousarray(params, dtype=np.float64)
         comp = np.empty((len(tabs[1]) - 1, len(params), 5), dtype=np.float64)
         rc, seconds = _timed(self.device, lambda st: _lib.lib().dg_sweep_score_latencies(
             h, self.seg.data_ptr(), emb.data_ptr(), *self._layout(tabs), params.ctypes.data, len(params),
             plan.ctypes.data, out_start.ctypes.data, out_res.ctypes.data, shifts.ctypes.data, PATCH_COLLAR,
-            *(a.ctypes.data for a in refs), comp.ctypes.data, st))
+            *(a.ctypes.data for a in refs[:4]), comp.ctypes.data, st))
         _lib.check(rc)
         return comp, seconds()
 
     def _score_group(self, params: np.ndarray, refs: tuple, regions: Optional[tuple]) -> Tuple[np.ndarray, float]:
-        reference = tuple(a.ctypes.data for a in refs)             # rows, labels, row offsets, label counts
+        reference = tuple(a.ctypes.data for a in refs[:4])         # rows, labels, row offsets, label counts
         params, emb, sets = self._trial_sets(params)
         return self._sweep._score_trials(*self._over_files(_lib.lib().dg_sweep_score_files, emb), params,
-                                         self.shifts.ctypes.data, reference, regions=regions, trial_sets=sets)[:2]
+                                         self.shifts.ctypes.data, reference, regions=regions, trial_sets=sets,
+                                         seeds=self._seeds, identities=refs[4] if len(refs) > 4 else None)[:2]
+
+    def _metric_kind(self, metric) -> Tuple[str, float, bool]:
+        return diarization_metric(metric)
+
+    def _pack(self, kind: str, references: List[Annotation], regions: Optional[list], copies: int) -> tuple:
+        """``pack_references``; for the identification error rate followed by the name table (:func:`pack_identities`)"""
+        refs = pack_references(references, regions)
+        if kind == "IdentificationErrorRate":
+            refs = (*refs, pack_identities(references, regions, self.labels * copies))
+        return refs
 
     def _components(self, f: int, comp: np.ndarray, refs: tuple) -> DERComponents:
-        return DERComponents.from_array(comp)
+        return (IdentificationErrorComponents if len(refs) > 4 else DERComponents).from_array(comp)
 
 
 VAD_PARAMS = tuple(hp.name for hp in VoiceActivityDetection.hyper_parameters())   # ("tau_active",)
@@ -1613,7 +1781,7 @@ class VoiceActivitySweep(_DatasetSweep):
         ``VoiceActivityDetection`` with that tau_active (label "speech", modality "speech", the file's uri)"""
         if self.units is not None:
             return self.run_latencies(trials, [self.config.latency])[float(self.config.latency)]
-        out = self._run(self._taus(trials), self.binarize, ["speech"])
+        out = self._run(self._taus(trials), self.binarize, [["speech"]] * len(self.uris))
         for preds in out:
             for p in preds:                # the per-chunk VAD annotations carry modality "speech" whatever the shift
                 p.modality = "speech"
@@ -1637,7 +1805,7 @@ class VoiceActivitySweep(_DatasetSweep):
         taus, sel = self._taus(trials), self._selection(latencies)
         if self.units is None:
             return {self.latencies[0]: self.run(trials)}
-        out = self._run_latencies(taus, sel, lambda t, tabs: self.binarize(t), ["speech"])
+        out = self._run_latencies(taus, sel, lambda t, tabs: self.binarize(t), [["speech"]] * len(self.uris))
         for runs in out.values():
             for preds in runs:
                 for p in preds:

@@ -260,6 +260,26 @@ int dg_vad_sweep_set_scored_regions(dg_vad_sweep* h, int num_files, const double
  *      before any launch.  num_sets = 0 clears them (the default: emb_dev is [N][K][D]).  DG_EINVAL for an index out of range
  *      or num_sets outside 0..64, and the previous state stays.  Host only. ---- */
 int dg_sweep_set_trial_sets(dg_sweep* h, int num_sets, const int32_t* trial_set_host, int T);
+/* ---- dg_sweep_set_seeds: known speakers for the handle's later dg_sweep_run* / dg_sweep_score* calls.  File f's known
+ *      centroids are rows [offsets_host[f], offsets_host[f + 1]) of centers_host float64 [n][D] (offsets int32 [num_files + 1]
+ *      from 0, not decreasing).  The files are the ones a call clusters: one for dg_sweep_run / dg_sweep_score, the files of
+ *      the _files entry points, the units of the _latencies ones.  Every (file, trial) state then starts as
+ *      dg_multi_open_seeded starts a stream: centres 0 .. n_f - 1 hold the centroids and are active, and the state counts as
+ *      initialised when n_f > 0 (so the clustering takes the distance path from the first chunk); a file without centroids
+ *      starts fresh.  num_files = 0 clears them (the default).  DG_EINVAL, changing nothing, for offsets that do not start at 0
+ *      or decrease, more than max_speakers centroids for one file, or a centroid that is not finite or has a zero norm.  A
+ *      later call that clusters another number of files gets DG_EINVAL before any launch.  Host only (the centroids travel in
+ *      the next call's upload). ---- */
+int dg_sweep_set_seeds(dg_sweep* h, int num_files, const int32_t* offsets_host, const double* centers_host);
+/* ---- dg_sweep_set_identities: identification error (DESIGN.md "Identification error") for the handle's later
+ *      dg_sweep_score* calls.  hyp_of_ref_host int32 [num_files][32]: for each scored file (the virtual files of
+ *      dg_sweep_score_latencies) and reference label r (string order, as the reference rows number them), the hypothesis label
+ *      g of the same name, or -1.  Each reference label is then matched to that label instead of by the optimal mapping; the
+ *      five components are otherwise computed as for DER.  Entries for r >= the file's label count are ignored.  num_files = 0
+ *      clears the table (the default: DER).  DG_EINVAL, changing nothing, for an entry outside [-1, max_speakers) or a g given
+ *      twice in one file.  A later scoring call over another number of files gets DG_EINVAL before any launch.  Host
+ *      only. ---- */
+int dg_sweep_set_identities(dg_sweep* h, int num_files, const int32_t* hyp_of_ref_host);
 /* ---- dg_sweep_score: the same clustering and post-path as dg_sweep_run, then each trial's diarization error rate components
  *      against one reference (DiarizationErrorRate, the metric of the reference's Benchmark.evaluate; definition in
  *      DESIGN.md "DER scoring"): collar=0, skip_overlap=False and no uem, or, with scored regions set
