@@ -142,6 +142,12 @@ SIGNATURES = {
     "dg_multi_open_seeded": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, _P, _P, C.c_int]),
     "dg_multi_get_state": (C.c_int, [_P, C.c_int, _P, _P, C.POINTER(C.c_int)]),
     "dg_multi_last_windows": (C.c_int, [_P, _P, C.c_int]),
+    "dg_gallery_create": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
+    "dg_gallery_destroy": (C.c_int, [_P]),
+    "dg_gallery_query": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_double, _P, _P, _P]),
+    "dg_multi_set_gallery": (C.c_int, [_P, _P, C.c_double]),
+    "dg_multi_set_names": (C.c_int, [_P, C.c_int, C.c_uint32, _P]),
+    "dg_multi_last_names": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int)]),
     "dg_selftest_multi_frames_host": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, C.c_int,
                                                 C.POINTER(C.c_int)]),
 }

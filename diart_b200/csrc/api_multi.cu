@@ -216,7 +216,18 @@ struct dg_multi {
   Event e_start, e_lane_done[2];
   Event t_begin, t_end;                       // timing events around the last tick's device work on `st`
   bool timed = false;                         // a tick has run
+  // gallery naming (dg_multi_set_gallery): per slot the named global speakers (bit g) and their claimed entries [slots][32],
+  // on the device and mirrored on the host; a tick's queries, segments, split partials and new names {slot, g, entry}
+  dg_gallery* gal = nullptr;
+  double gal_threshold = 0.0;
+  DevBuf gal_named, gal_claimed, gal_q, gal_seg, gal_n, gal_d, gal_e, gal_list;
+  std::vector<uint32_t> named_host;
+  std::vector<int32_t> names_last;            // the names the last dg_multi_step decided, [n][3]
 };
+
+// In front of the header in h->header and in the tick's pinned download: with a gallery, the count of the tick's new names
+// (16 bytes) and the first GAL_NAME_PREFIX of them, so that they travel in the header's copy
+static size_t names_bytes(const dg_multi* h) { return h->gal ? 16 + (size_t)GAL_NAME_PREFIX * 12 : 0; }
 
 static bool slot_ok(const dg_multi* h, int slot) { return h && h->book.ok(slot); }
 static bool vad_mode(const dg_multi* h) { return !h->net.emb; }
@@ -426,6 +437,11 @@ static int open_slot(dg_multi* h, int slot, int rate_id, int num_windows, const 
       DG_CUDA(cudaMemcpyAsync(h->active.as<int>() + s * 32, flags.data(), (size_t)n * 4, cudaMemcpyHostToDevice, h->st));
       DG_CUDA(cudaMemcpyAsync(h->init.as<int>() + s * 2, init, 2 * 4, cudaMemcpyHostToDevice, h->st));
     }
+  }
+  if (h->gal) {   // a stream opens with no speaker named
+    DG_CUDA(cudaMemsetAsync(h->gal_named.as<uint32_t>() + s, 0, 4, h->st));
+    DG_CUDA(cudaMemsetAsync(h->gal_claimed.as<int32_t>() + s * 32, 0xff, 32 * 4, h->st));
+    h->named_host[slot] = 0;
   }
   h->book.start(slot, rate_id + 1);
   h->n_hist[slot] = 0;
@@ -661,12 +677,38 @@ static int tick_diarize(dg_multi* h, const TickPlan& tp, const TickIn& L, int tu
     return rc;
   // post-path with each slot's history and tau, then the histories move on
   DG_CUDA(cudaMemsetAsync(h->total.p, 0, 4, st));
+  int32_t* header = reinterpret_cast<int32_t*>(h->header.as<unsigned char>() + names_bytes(h));
   if ((rc = launch_post_slots(h->seg.as<float>(), h->maps.as<int32_t>(), h->hist_seg.as<float>(), h->hist_map.as<int32_t>(),
                               d_act, d_rows, h->slots, B, F, K, M, h->nw, reinterpret_cast<const int32_t*>(din + L.o_plan),
-                              4 + h->nw, h->hamming.as<double>(), trials, h->header.as<int32_t>(), h->turns.as<uint32_t>(),
+                              4 + h->nw, h->hamming.as<double>(), trials, header, h->turns.as<uint32_t>(),
                               turn_cap, h->total.as<unsigned int>(), st)) ||
       (rc = launch_post_slots_history(h->seg.as<float>(), h->maps.as<int32_t>(), h->hist_seg.as<float>(),
                                       h->hist_map.as<int32_t>(), d_act, n_act, h->slots, F, K, h->nw, st)))
+    return rc;
+  return DG_OK;
+}
+
+// Gallery naming after a diarization tick, on h->st: the active, unnamed global speakers of the tick's slots (at most
+// `queries`, from the host mirror of the named tables) against the gallery; the new names go to the front of h->header.
+static int tick_gallery(dg_multi* h, const TickPlan& tp, const TickIn& L, int queries) {
+  cudaStream_t st = h->st;
+  const dg_gallery* g = h->gal;
+  const int n_act = (int)tp.act.size(), splits = gallery_splits(g->G, queries);
+  if (h->gal_q.ensure((size_t)queries * 8) || h->gal_seg.ensure((size_t)(n_act + 1) * 4) || h->gal_n.ensure(16) ||
+      h->gal_d.ensure((size_t)splits * queries * 8) || h->gal_e.ensure((size_t)splits * queries * 4) ||
+      h->gal_list.ensure((size_t)queries * 12))
+    return DG_ECUDA;
+  const TickSlot* d_act = reinterpret_cast<const TickSlot*>(h->in.as<unsigned char>() + L.o_act);
+  int* names = h->header.as<int>();
+  int rc;
+  if ((rc = launch_gallery_queries(d_act, n_act, h->active.as<int>(), h->gal_named.as<uint32_t>(), h->M, h->gal_q.as<int2>(),
+                                   h->gal_seg.as<int>(), h->gal_n.as<int>(), names, st)) ||
+      (rc = launch_gallery_nearest(g->E.as<double>(), g->En.as<double>(), g->G, g->Gp, g->Dp, h->centers.as<double>(), h->D,
+                                   h->gal_q.as<int2>(), h->gal_n.as<int>(), queries, h->gal_claimed.as<int32_t>(), splits,
+                                   h->gal_d.as<double>(), h->gal_e.as<int>(), st)) ||
+      (rc = launch_gallery_claim(h->gal_d.as<double>(), h->gal_e.as<int>(), splits, queries, h->gal_q.as<int2>(),
+                                 h->gal_seg.as<int>(), n_act, h->gal_threshold, h->gal_claimed.as<int32_t>(), nullptr, nullptr,
+                                 h->gal_named.as<uint32_t>(), h->M, names, h->gal_list.as<int32_t>(), names + 4, st)))
     return rc;
   return DG_OK;
 }
@@ -742,27 +784,32 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
       if ((rc = check_plan_row(who, plan_host + (size_t)(ts.row0 + i) * stride, ts.row0 + i, ts.nw, ts.n_hist + i, h->F)))
         return rc;
   if (n_turns) *n_turns = 0;
+  h->names_last.clear();
   if (B == 0) return DG_OK;     // nothing to do: staged samples wait for the next tick
   DG_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = h->st;
   const int F = h->F, K = h->K, D = h->D, M = h->M;
-  const TurnOut lay = {0, (size_t)B * 16};
+  const TurnOut lay = {names_bytes(h), (size_t)B * 16};
   const int turn_cap = post_turn_cap(B, M, F);
-  if (h->seg.ensure((size_t)B * F * K * 4) || h->header.ensure(lay.header_bytes) || h->turns.ensure((size_t)turn_cap * 4) ||
+  if (h->seg.ensure((size_t)B * F * K * 4) || h->header.ensure(lay.at + lay.header_bytes) || h->turns.ensure((size_t)turn_cap * 4) ||
       h->pin_out.ensure(lay.end()))
     return DG_ECUDA;
   if (!vad_mode(h) && (h->emb.ensure((size_t)B * K * D * 4) || h->maps.ensure((size_t)B * K * 4) ||
                        h->prep.ensure(cluster_prep_floats(B, K) * 4 + 16) || h->prep_d.ensure(cluster_prep_doubles(B, K) * 8 + 16)))
     return DG_ECUDA;
+  int queries = 0;             // with a gallery: the unnamed global speakers of the tick's slots, an upper bound of its queries
+  if (h->gal)
+    for (const TickSlot& ts : act) queries += M - __builtin_popcount(h->named_host[ts.slot]);
   TickIn in;
   if ((rc = tick_audio_in(h, tp, plan_host, in)) ||
-      (rc = vad_mode(h) ? tick_vad(h, tp, in, turn_cap) : tick_diarize(h, tp, in, turn_cap)))
+      (rc = vad_mode(h) ? tick_vad(h, tp, in, turn_cap) : tick_diarize(h, tp, in, turn_cap)) ||
+      (queries > 0 && (rc = tick_gallery(h, tp, in, queries))))
     return rc;
   if (seg_dev) DG_CUDA(cudaMemcpyAsync(seg_dev, h->seg.p, (size_t)B * F * K * 4, cudaMemcpyDeviceToDevice, st));
   if (emb_dev) DG_CUDA(cudaMemcpyAsync(emb_dev, h->emb.p, (size_t)B * K * D * 4, cudaMemcpyDeviceToDevice, st));
   if (map_dev) DG_CUDA(cudaMemcpyAsync(map_dev, h->maps.p, (size_t)B * K * 4, cudaMemcpyDeviceToDevice, st));
   unsigned char* po = h->pin_out.as<unsigned char>();
-  DG_CUDA(cudaMemcpyAsync(po + lay.at, h->header.p, lay.header_bytes, cudaMemcpyDeviceToHost, st));
+  DG_CUDA(cudaMemcpyAsync(po, h->header.p, lay.at + lay.header_bytes, cudaMemcpyDeviceToHost, st));
   DG_CUDA(cudaMemcpyAsync(po + lay.total(), h->total.p, 4, cudaMemcpyDeviceToHost, st));
   DG_CUDA(cudaMemcpyAsync(po + lay.prefix(), h->turns.p, (size_t)std::min(DG_POST_PREFIX, turn_cap) * 4, cudaMemcpyDeviceToHost,
                           st));
@@ -779,7 +826,93 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
       h->cur[ts.slot] ^= 1;
     }
   }
+  if (queries > 0) {   // the new names: the prefix came with the header, the rest (if any) is copied now
+    int count = 0;
+    memcpy(&count, po, 4);
+    h->names_last.resize((size_t)count * 3);
+    const int pre = std::min(count, GAL_NAME_PREFIX);
+    memcpy(h->names_last.data(), po + 16, (size_t)pre * 12);
+    if (count > pre) {
+      DG_CUDA(cudaMemcpyAsync(h->names_last.data() + (size_t)pre * 3, h->gal_list.as<int32_t>() + (size_t)pre * 3,
+                              (size_t)(count - pre) * 12, cudaMemcpyDeviceToHost, st));
+      DG_CUDA(cudaStreamSynchronize(st));
+    }
+    for (int i = 0; i < count; i++) h->named_host[h->names_last[3 * i]] |= 1u << h->names_last[3 * i + 1];
+  }
   return download_turns(who, po, lay, h->turns.as<uint32_t>(), header_host, turns_host, turn_cap_host, n_turns, st);
+}
+
+extern "C" int dg_multi_set_gallery(dg_multi* h, dg_gallery* g, double threshold) {
+  const char* who = "dg_multi_set_gallery";
+  if (!h || !g) {
+    set_error(std::string(who) + ": null handle");
+    return DG_EINVAL;
+  }
+  if (vad_mode(h) || h->opened) {
+    set_error(std::string(who) + (vad_mode(h) ? ": a VAD handle has no speakers to name"
+                                               : ": a gallery is set before any stream is opened"));
+    return DG_EINVAL;
+  }
+  if (g->D != h->D || g->device != h->device) {
+    set_error(std::string(who) + ": the gallery's entries have dimension " + std::to_string(g->D) + " on device " +
+              std::to_string(g->device) + ", the embeddings " + std::to_string(h->D) + " on device " + std::to_string(h->device));
+    return DG_EINVAL;
+  }
+  if (!(std::isfinite(threshold) && threshold > 0.0 && threshold <= 2.0)) {
+    set_error(std::string(who) + ": need a finite threshold in (0, 2]");
+    return DG_EINVAL;
+  }
+  DG_CUDA(cudaSetDevice(h->device));
+  if (h->gal_named.ensure((size_t)h->slots * 4) || h->gal_claimed.ensure((size_t)h->slots * 32 * 4)) return DG_ECUDA;
+  h->named_host.assign(h->slots, 0);
+  h->gal = g;
+  h->gal_threshold = threshold;
+  return DG_OK;
+}
+
+extern "C" int dg_multi_set_names(dg_multi* h, int slot, uint32_t named, const int32_t* claimed_host) {
+  const char* who = "dg_multi_set_names";
+  if (!slot_ok(h, slot) || !h->gal || !claimed_host) {
+    set_error(std::string(who) + ": need an open slot of a handle with a gallery and a non-null table");
+    return DG_EINVAL;
+  }
+  const int M = h->M;
+  std::vector<int32_t> row(32, -1);
+  for (int g = 0; g < M; g++) {
+    const int e = claimed_host[g];
+    const bool ok = e == -1 || (e >= 0 && e < h->gal->G && ((named >> g) & 1) &&
+                                std::find(claimed_host, claimed_host + g, e) == claimed_host + g);
+    if (!ok) {
+      set_error(std::string(who) + ": speaker " + std::to_string(g) + " claims entry " + std::to_string(e) +
+                " (an entry of the gallery, claimed once, by a named speaker)");
+      return DG_EINVAL;
+    }
+    row[g] = e;
+  }
+  if (M < 32 && (named >> M)) {
+    set_error(std::string(who) + ": named speakers beyond max_speakers");
+    return DG_EINVAL;
+  }
+  DG_CUDA(cudaSetDevice(h->device));
+  DG_CUDA(cudaMemcpyAsync(h->gal_named.as<uint32_t>() + slot, &named, 4, cudaMemcpyHostToDevice, h->st));
+  DG_CUDA(cudaMemcpyAsync(h->gal_claimed.as<int32_t>() + (size_t)slot * 32, row.data(), 32 * 4, cudaMemcpyHostToDevice, h->st));
+  h->named_host[slot] = named;
+  return DG_OK;
+}
+
+extern "C" int dg_multi_last_names(const dg_multi* h, int32_t* out_host, int cap, int* n) {
+  if (!h || !n || cap < 0 || (cap > 0 && !out_host)) {
+    set_error("dg_multi_last_names: bad arguments");
+    return DG_EINVAL;
+  }
+  const int count = (int)(h->names_last.size() / 3);
+  *n = count;
+  if (count > cap) {
+    set_error("dg_multi_last_names: " + std::to_string(count) + " names, room for " + std::to_string(cap));
+    return DG_EINVAL;
+  }
+  if (count) memcpy(out_host, h->names_last.data(), h->names_last.size() * 4);
+  return DG_OK;
 }
 
 extern "C" int dg_multi_last_step_ms(const dg_multi* h, float* ms) {

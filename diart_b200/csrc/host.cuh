@@ -309,6 +309,13 @@ struct dg_resample {
   DevBuf taps;   // [n][T]
 };
 
+// ==================================================================================== gallery (api_gallery.cu)
+// entries E [Gp][Dp] float64, zero padded (gallery.cu), norms En [G]; ws_*: the workspace of dg_gallery_query
+struct dg_gallery {
+  int device = 0, G = 0, Gp = 0, D = 0, Dp = 0;
+  DevBuf E, En, ws_q, ws_seg, ws_d, ws_e;
+};
+
 // ======================================================================== device-side audio stream (api_stream.cu)
 // rearrange_audio_stream (reference src/diart/operators.py:44-100) on the device: the host pushes each sample ONCE
 // (8 000 new samples per chunk instead of the 80 000 of a stacked window: 8.2 MB instead of 82 MB per 256-chunk step),

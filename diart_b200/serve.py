@@ -28,7 +28,8 @@ dedicated pipeline whose configuration is the server's with that stream's values
 
 A diarization stream may also start from known speakers (``open(speakers=...)``, ``diart_b200.speakers``): its clustering
 state is seeded with their centroids and its annotations name them; ``speakers(sid)`` exports a stream's state, so that a
-closed stream can be resumed with the same centroids and labels."""
+closed stream can be resumed with the same centroids and labels.  With a ``gallery`` (``speakers.SpeakerGallery``), every tick
+also names the streams' discovered speakers from it on the device."""
 from __future__ import annotations
 
 import ctypes as C
@@ -45,7 +46,7 @@ from .blocks.post import chunk_annotations, crop_plan, turn_capacity
 from .blocks.vad import VoiceActivityDetectionConfig, speech_annotations
 from .core import Annotation
 from .operators import DeviceResample
-from .speakers import KnownSpeakers, exported, speaker_labels
+from .speakers import KnownSpeakers, SpeakerGallery, check_gallery, exported, speaker_labels
 
 
 def plan_rows(idx: np.ndarray, step: float, window_samples: int, sample_rate: int, frames: int, nw: int, latency: float,
@@ -196,6 +197,9 @@ class _MultiStreamServer:
         """the tick's annotations; ``shifts``: the timestamp shift of each row (``_row_sids``: its stream)"""
         raise NotImplementedError
 
+    def _after_tick(self, B: int):
+        """called once a tick of B windows has run, before its annotations are built"""
+
     def __del__(self):
         try:
             if getattr(self, "_h", None) is not None:
@@ -302,6 +306,7 @@ class _MultiStreamServer:
         if not np.array_equal(got, counts):
             raise _lib.DiartB200Error("stream bookkeeping out of step with the device handle")
         self._emitted += counts
+        self._after_tick(B)
         outs = tuple(t for t in outs if t is not None) or None
         if B == 0:
             return {}, outs
@@ -328,18 +333,30 @@ class MultiStreamDiarization(_MultiStreamServer):
     ``set_known_speakers(known)``, and its global speaker g < n is labelled ``known.names[g]``.  ``speakers(sid)`` returns the
     stream's active centres with their labels after the last tick; opening a stream with them resumes its clustering state
     exactly (not its aggregation history: the first ``latency / step - 1`` outputs aggregate fewer buffers, as those of any
-    new stream do)."""
+    new stream do).
+
+    ``gallery`` (a :class:`~diart_b200.speakers.SpeakerGallery` of the embedding dimension; the configuration's metric must
+    be cosine): after every tick, each stream that had windows names its active, unnamed global speakers from the gallery by
+    the gallery's rule, on the device; the tick's annotations already carry the names it decided, and a name stays for the
+    rest of the stream's life.  A stream opened with known speakers counts them as named and their gallery entries as
+    claimed, so ``open(speakers=speakers(sid))`` resumes its names and claims.  Names change labels, never segments."""
 
     _needs = "MultiStreamDiarization needs the native segmentation and embedding models"
 
     def __init__(self, config: SpeakerDiarizationConfig, max_streams: int, max_windows_per_stream: int = 4,
-                 source_sample_rates=(), max_latency: Optional[float] = None):
+                 source_sample_rates=(), max_latency: Optional[float] = None, gallery: Optional[SpeakerGallery] = None):
         self._speakers = int(config.max_speakers)
         self.labels = [f"speaker{g}" for g in range(config.max_speakers)]
+        self.gallery = gallery
         super().__init__(config, max_streams, max_windows_per_stream, source_sample_rates,
                          (config.segmentation, config.embedding), max_latency)
-        self._seeded = np.zeros(self.max_streams, dtype=bool)          # the stream in the slot started from known speakers
-        self._stream_labels = [self.labels] * self.max_streams          # each slot's label list (unseeded: the shared one)
+        if gallery is not None:
+            check_gallery(gallery, config, self.D)
+            with torch.cuda.device(self.device):
+                _lib.check(_lib.lib().dg_multi_set_gallery(self._h, gallery.handle, gallery.threshold))
+        self._own_labels = np.zeros(self.max_streams, dtype=bool)      # the slot's labels are its own list, not the shared one
+        self._stream_labels = [self.labels] * self.max_streams          # each slot's label list
+        self._names = np.empty((0, 3), dtype=np.int32)
 
     def open(self, shift: float = 0.0, sample_rate: Optional[int] = None, *, latency: Optional[float] = None,
              tau_active: Optional[float] = None, rho_update: Optional[float] = None,
@@ -358,8 +375,11 @@ class MultiStreamDiarization(_MultiStreamServer):
                 raise ValueError(f"{len(known)} known speakers, at most max_speakers = {self._speakers}")
         sid = _MultiStreamServer._open_stream(self, shift, sample_rate, latency, None if known is None else known.centroids,
                                               tau_active=tau_active, rho_update=rho_update, delta_new=delta_new)
-        self._seeded[sid] = known is not None
+        self._own_labels[sid] = known is not None
         self._stream_labels[sid] = self.labels if known is None else speaker_labels(known, self._speakers)
+        if self.gallery is not None and known is not None:
+            named, claimed = self.gallery.claims(self._stream_labels[sid])
+            _lib.check(_lib.lib().dg_multi_set_names(self._h, sid, named, claimed.ctypes.data))
         return sid
 
     def speakers(self, sid: int) -> KnownSpeakers:
@@ -391,9 +411,24 @@ class MultiStreamDiarization(_MultiStreamServer):
         return (torch.empty((B, self.F, self.K), device=self.device), torch.empty((B, self.K, self.D), device=self.device),
                 torch.empty((B, self.K), device=self.device, dtype=torch.int32))
 
+    def _after_tick(self, B):
+        """the names the tick decided {slot, g, entry} to the slots' labels"""
+        if self.gallery is None or B == 0:
+            return
+        n = C.c_int()
+        cap = self.max_streams * self._speakers
+        if len(self._names) < cap:
+            self._names = np.empty((cap, 3), dtype=np.int32)
+        _lib.check(_lib.lib().dg_multi_last_names(self._h, self._names.ctypes.data, cap, C.byref(n)))
+        for sid, g, e in self._names[:n.value].tolist():
+            if not self._own_labels[sid]:
+                self._stream_labels[sid] = list(self.labels)
+                self._own_labels[sid] = True
+            self._stream_labels[sid][g] = self.gallery.names[e]
+
     def _annotations(self, header, turns, n_turns, out_start, out_res, shifts):
         sids = self._row_sids
-        labels = [self._stream_labels[s] for s in sids.tolist()] if self._seeded[sids].any() else self.labels
+        labels = [self._stream_labels[s] for s in sids.tolist()] if self._own_labels[sids].any() else self.labels
         return chunk_annotations(header, turns, n_turns, out_start, out_res, labels, shifts)
 
 
@@ -413,7 +448,9 @@ class MultiStreamVoiceActivityDetection(_MultiStreamServer):
     _speakers = 1
 
     def __init__(self, config: VoiceActivityDetectionConfig, max_streams: int, max_windows_per_stream: int = 4,
-                 source_sample_rates=(), max_latency: Optional[float] = None):
+                 source_sample_rates=(), max_latency: Optional[float] = None, gallery=None):
+        if gallery is not None:
+            raise ValueError("voice activity detection has no speakers to name: a gallery needs MultiStreamDiarization")
         super().__init__(config, max_streams, max_windows_per_stream, source_sample_rates, (config.segmentation,),
                          max_latency)
 

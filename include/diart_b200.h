@@ -519,6 +519,34 @@ int dg_multi_open_seeded(dg_multi* h, int slot, int rate_id, int num_windows, co
                          const double* centers_host /* [n][D] */, int n);
 int dg_multi_get_state(dg_multi* h, int slot, double* centers_host /* [M][D] */, int32_t* active_host /* [M] */,
                        int* initialized);
+/* ---- speaker gallery: names for discovered speakers from an enrolled gallery of any size (DESIGN.md "Gallery naming").
+ *      The cosine distance 1 - clip(u.v / (|u| |v|), -1, 1) is evaluated in float64 (dot products on the float64 tensor
+ *      cores, each summed in one fixed order: identical entries give identical distances).
+ *      dg_gallery_create: uploads centroids_host float64 [G][D] to `device` and computes the entries' norms.  DG_EINVAL unless
+ *        1 <= G <= 1048576, D >= 2 is even, and every entry is finite with a non-zero norm.
+ *      dg_gallery_query: per query q of queries_dev float64 [Q][D] (row stride D), on `stream`: dist_dev [q] the distance to
+ *        the nearest entry its group has not claimed (ties: the lowest entry; +inf when none is left), entry_dev [q] that
+ *        entry if the distance is < threshold and q wins it within its group, else -1.  group_dev int32 [Q]: the query's claim
+ *        group, >= 0, each group one contiguous run of at most 32 queries; claimed_dev int32 [groups][32] (null: none): the
+ *        entries group r has claimed, -1 padded.  Within a group, candidates for one entry are resolved by the smallest
+ *        distance, ties to the earliest query.  group_dev is read back on `stream` (the call waits for it) to check it.
+ *      dg_multi_set_gallery: every later tick names the active, unnamed global speakers of its streams from the gallery
+ *        (dg_multi_last_names).  DG_EINVAL on a VAD handle, once a stream has opened, for a gallery of another dimension or
+ *        device, or unless 0 < threshold <= 2.
+ *      dg_multi_set_names: the names of the open stream in `slot` (a handle with a gallery): bit g of `named` set for a
+ *        named global speaker g < max_speakers, claimed_host int32 [max_speakers] its gallery entry (-1: none; only named
+ *        speakers claim, each entry once).  A stream opens with none named.
+ *      dg_multi_last_names: the names decided by the last dg_multi_step, out_host int32 [cap][3] = {slot, g, entry}, *n of
+ *        them; DG_EINVAL if more than cap. ---- */
+typedef struct dg_gallery dg_gallery;
+int dg_gallery_create(const double* centroids_host, int G, int D, int device, dg_gallery** out);
+int dg_gallery_destroy(dg_gallery* g);
+int dg_gallery_query(dg_gallery* g, const double* queries_dev /* [Q][D] */, int Q, const int32_t* group_dev /* [Q] */,
+                     const int32_t* claimed_dev /* [groups][32] */, double threshold, int32_t* entry_dev /* [Q] */,
+                     double* dist_dev /* [Q] */, void* stream);
+int dg_multi_set_gallery(dg_multi* h, dg_gallery* g, double threshold);
+int dg_multi_set_names(dg_multi* h, int slot, uint32_t named, const int32_t* claimed_host /* [max_speakers] */);
+int dg_multi_last_names(const dg_multi* h, int32_t* out_host /* [cap][3] */, int cap, int* n);
 /* test hook: the last tick's window batch [n_rows, chunk_samples] (what its networks read; n_rows = that tick's window count)
  * copied to wav_dev.  Synchronous. */
 int dg_multi_last_windows(const dg_multi* h, float* wav_dev, int n_rows);
