@@ -259,7 +259,7 @@ extern "C" int dg_selftest_gemm_tc_grid(int M, int Cin, int KW, int dil, int N, 
   // output buffers, in bytes: float32 rows, hi and lo planes, pooling partial sums
   const size_t f32_bytes = epi == 0 || epi == 2 ? (size_t)M * ldc * 4 : (epi == 5 ? (size_t)(M / 3) * ldc * 4 : 0);
   const size_t plane_bytes = epi == 1 || epi == 3 ? (size_t)M * ldc * 2 : 0;
-  const size_t part_bytes = epi == 4 ? (size_t)m_tiles * 2 * 4 * 2 * N * 4 : (epi == 5 ? (size_t)m_tiles * 2 * 2 * N * 4 : 0);
+  const size_t part_bytes = epi == 4 ? (size_t)m_tiles * 2 * TC_POOL_SLOTS * N * 4 : (epi == 5 ? (size_t)m_tiles * 2 * TC_POOL3_SLOTS * N * 4 : 0);
   DevBuf dA, dAh, dAl, dB, dS, dH, dRes, dRh, dRl, dPw, dF, dOh, dOl, dPart;
   WeightPlanes dW;
   if (upload(dA, A) || upload(dB, bias) || upload(dS, bsc) || upload(dH, bsh) || upload(dRes, res) || upload(dPw, pw) ||
@@ -287,7 +287,7 @@ extern "C" int dg_selftest_gemm_tc_grid(int M, int Cin, int KW, int dil, int N, 
     t.res_hi = dRh.p; t.res_lo = dRl.p;
   }
   if (epi == 4) {
-    t.pool_w = dPw.as<float>(); t.pool_part = dPart.as<float>(); t.pool_item_rows = item_rows; t.pool_K = 3;
+    t.pool_w = dPw.as<float>(); t.pool_part = dPart.as<float>(); t.pool_item_rows = item_rows; t.pool_K = 3; t.pool_T = item_rows;
   }
   if (epi == 5) {
     t.pool_part = dPart.as<float>(); t.pool_item_rows = item_rows; t.pool3_T = item_rows / 3 - 2;
@@ -366,7 +366,7 @@ extern "C" int dg_selftest_gemm_tc_halo(int M, int Cin, int KW, int dil, int N, 
   }
   const size_t f32_bytes = epi == 0 || epi == 2 ? (size_t)M * N * 4 : (epi == 5 ? (size_t)(M / 3) * N * 4 : 0);
   const size_t plane_bytes = epi == 1 ? (size_t)M * N * 2 : 0;
-  const size_t part_bytes = epi == 5 ? (size_t)m_tiles * 2 * 2 * N * 4 : 0;
+  const size_t part_bytes = epi == 5 ? (size_t)m_tiles * 2 * TC_POOL3_SLOTS * N * 4 : 0;
   DevBuf dA, dAh, dAl, dB, dS, dH, dF, dOh, dOl, dPart;
   WeightPlanes dW, dWf;
   if (upload(dA, A) || upload(dB, bias) || upload(dS, bsc) || upload(dH, bsh) || upload_split(dW, Wnk, N, npad, K) ||

@@ -531,15 +531,15 @@ static int emb_tdnn5_pool_rows(dg_emb* h, int U, const Geom& g, const float* row
   int rc;
   const long long M = (long long)U * g.S2;
   const int m_tiles = (int)((M + 127) / 128);
-  if (h->pool_part.ensure((size_t)m_tiles * 2 * 8 * 1500 * 4) || h->pooled.ensure((size_t)U * K * 3000 * 4)) return DG_ECUDA;
+  if (h->pool_part.ensure((size_t)m_tiles * 2 * TC_POOL_SLOTS * 1500 * 4) || h->pooled.ensure((size_t)U * K * 3000 * 4)) return DG_ECUDA;
   TcGemm t{};
   t.A_hi = h->t4h; t.A_lo = h->t4l; t.lda = 512; t.Cin = 512; t.KW = 1; t.dil = 1; t.Mtot = M; t.M = M;
   t.N = 1500; t.bias = h->tb[4].as<float>(); t.bn_scale = h->bns[4].as<float>(); t.bn_shift = h->bnh[4].as<float>();
   t.ldc = 1500; t.epi = 4; t.tag = "tdnn5";
-  t.pool_w = row_w; t.pool_part = h->pool_part.as<float>(); t.pool_item_rows = g.S2; t.pool_K = K;
+  t.pool_w = row_w; t.pool_part = h->pool_part.as<float>(); t.pool_item_rows = g.S2; t.pool_K = K; t.pool_T = T;
   if ((rc = set_weights(t, h->tw[4])) || (rc = launch_gemm_tc(t, st))) return rc;
   h->pool_C = 1500;
-  return launch_pool_finalize(h->pool_part.as<float>(), vsum, h->bnh[4].as<float>(), U, K, 1500, g.S2, T, eps,
+  return launch_pool_finalize(h->pool_part.as<float>(), row_w, vsum, h->bnh[4].as<float>(), U, K, 1500, g.S2, T, eps,
                               h->pooled.as<float>(), st);
 }
 

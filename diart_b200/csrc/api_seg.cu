@@ -163,11 +163,11 @@ int run_sincnet(const SincWeights& w, SincWork& k, const float* wav, int B, cons
                             k.a0h.p, k.a0l.p, st, stream_flag)))
     return rc;
   // conv1 / conv2 with MaxPool1d(3) and the InstanceNorm partial sums in the GEMM epilogue (TC_MAXPOOL3): the un-pooled maps are
-  // never written, the statistics pass reads 2 x 2 x 64 floats per tile.  Needs a tile of 96..126 rows that divides the item at both
+  // never written, the statistics pass reads 2 x 3 x 64 floats per tile.  Needs a tile of 96..126 rows that divides the item at both
   // stages; otherwise the un-pooled float32 map -> instnorm_stats -> split with pooling on load
   const int tr0 = gemm_tc_pool3_tile_rows(g.S0), tr1 = gemm_tc_pool3_tile_rows(g.S1);
   if (tr0 && tr1) {
-    if (k.part3.ensure((size_t)(M0 / tr0) * 2 * 2 * 64 * 4)) return DG_ECUDA;
+    if (k.part3.ensure((size_t)(M0 / tr0) * 2 * TC_POOL3_SLOTS * 64 * 4)) return DG_ECUDA;
     TcGemm t{};
     t.A_hi = k.a0h.p; t.A_lo = k.a0l.p; t.lda = 80; t.Cin = 80; t.KW = 5; t.dil = 1; t.Mtot = M0; t.M = M0;
     t.N = 64; t.bias = w.bias1.as<float>(); t.out_f32 = k.p1.as<float>(); t.ldc = 64; t.epi = 5; t.tag = "sinc_conv1";

@@ -130,6 +130,7 @@ struct GemmArgs {
 };
 int launch_gemm(const GemmArgs& a, cudaStream_t st);
 // gemm_tc.cu -- wgmma / TMA path (hi/lo split precision, three products)
+constexpr int TC_POOL_SLOTS = 9, TC_POOL3_SLOTS = 3;   // pool_part values per (tile, item, column) of epi 4 / epi 5
 struct TcGemm {
   const void* A_hi;    // fp16 [Mtot, lda]
   const void* A_lo;
@@ -156,12 +157,15 @@ struct TcGemm {
   const void* res_hi;
   const void* res_lo;
   // epi 4 (TDNN5 + weighted statistics pooling, heads.cu: pool_finalize): bias -> LeakyReLU -> BatchNorm, then per 128-row tile
-  // and item the sums  S1 = sum_t w_k[t] d,  S2 = sum_t w_k[t] d^2  of d = x - bn_shift  for the K local speakers
+  // and item the sums  S1 = sum_t w_k[t] e,  S2 = sum_t w_k[t] e^2  of e = d - p, d = x - bn_shift, for the K local speakers,
+  // around a pivot p: 0, or for a channel far from its BatchNorm shift the average of d at two of the item's valid rows
   const float* pool_w;   // [Mtot][4]
-  float* pool_part;      // [m_tiles][2][4][2][N]
+  float* pool_part;      // [m_tiles][2][TC_POOL_SLOTS][N]: [4][2] sums, then p
   int pool_item_rows, pool_K;
+  int pool_T;            // valid rows of an item (the rows after them hold garbage and weight 0)
   // epi 5 (SincNet Conv1d + MaxPool1d(3) + InstanceNorm statistics): out_f32 = bias + max over row triplets ([M / 3, ldc]),
-  // pool_part = per-tile partial sums [M / pool3_tile_rows][2][2][N], reduced by launch_instnorm_finalize;
+  // pool_part = per-tile partial sums [M / pool3_tile_rows][2][TC_POOL3_SLOTS][N] (sum and sum of squares of v - p, p = the
+  // item's first pooled value in the tile, then p), reduced by launch_instnorm_finalize;
   // pool_item_rows = un-pooled rows per item (multiple of 3), pool3_T = valid pooled frames per item
   int pool3_T, pool3_tile_rows;
   int tap_boxes;         // 1: load A per tap even where the halo mode applies (self-tests compare the two operand paths)
@@ -242,8 +246,8 @@ int launch_pool_weights(const float* w /*[B,F,K]*/, int B, int F, int K, int ite
 // launch_pool_weights for G sets in one launch: set g reads w + g B F K, writes row_w + g rw_stride and vsum + g B K 2
 int launch_pool_weights_sets(const float* w, int B, int G, int F, int K, int item_rows, int T, const int* idx0, const int* idx1,
                              const float* lam1, float eps, float* row_w, long long rw_stride, float* vsum, cudaStream_t st);
-int launch_pool_finalize(const float* part, const float* vsum, const float* pivot, int B, int K, int C, int item_rows, int T,
-                         float eps, float* pooled /*[B*K][2C]*/, cudaStream_t st);
+int launch_pool_finalize(const float* part, const float* row_w, const float* vsum, const float* pivot, int B, int K, int C,
+                         int item_rows, int T, float eps, float* pooled /*[B*K][2C]*/, cudaStream_t st);
 int launch_l2norm(const float* in, int rows, int D, float norm, float* out, cudaStream_t st);
 int launch_row_equal_flags(const float* wav, int N, int S, int* flags, cudaStream_t st);
 int launch_gather_rows(const float* src, const int* index, int rows, int cols, float* dst, cudaStream_t st);

@@ -81,12 +81,14 @@ struct TcArgs {
   const __nv_bfloat16* res_lo;
   // TC_POOL: weighted statistics pooling fused into the epilogue (the activation map is never written)
   const float* pool_w;     // [rows][4]: pooling weight of (row, speaker), zero for rows past an item's valid frames
-  float* pool_part;        // [m_tiles][2 (item of the tile)][4 (speaker)][2 (sum w d, sum w d^2)][N]
-  int pool_item_rows, pool_K;
+  float* pool_part;        // [m_tiles][2 (item of the tile)][TC_POOL_SLOTS][N]: 4 (speaker) x 2 (sum w e, sum w e^2), pivot;
+                           // e = d - pivot
+  int pool_item_rows, pool_K, pool_T;   // pool_T: valid frames of an item (its later rows hold garbage and weight 0)
   // TC_MAXPOOL3: m-tiles advance by `tile_rows` <= 126 rows (whole pooling windows, a divisor of the item's rows, so that every
   // item is summed in the same grouping wherever it sits in the batch; the MMA still covers 128 rows), out_f32 receives
   // bias + MaxPool1d(3) over rows ([M / 3, ldc]), pool_part the per-tile InstanceNorm partial sums of the pre-bias pooled values:
-  // [m_tiles][2 (item of the tile)][2 (sum, sum of squares)][N] over the pooled frames < pool3_T of an item
+  // [m_tiles][2 (item of the tile)][TC_POOL3_SLOTS][N] = (sum, sum of squares) of v - pivot over the pooled frames < pool3_T of
+  // an item, pivot
   int tile_rows, pool3_T;
   unsigned* tile_ctr;      // pooling epilogues, [2]: tiles handed out past the first wave, CTAs finished (both back to 0)
   // halo operand mode (gemm_tc_kernel<.., true>): a tile's A operand is its halo, rows m0 .. m0 + halo_rows - 1 of all cin
@@ -325,7 +327,7 @@ __device__ __forceinline__ void tc_pool_epilogue_tile(const TcArgs& a, float* pa
     }
     // TC_POOL: the rows' pooling weights go to shared memory; `brow` = first row of the tile that belongs to the NEXT item
     // (a 128-row tile covers at most two items)
-    int brow = TC_BM;
+    int brow = TC_BM, valid0 = 0, valid1 = 0;   // TC_POOL: valid rows of the tile's two items ([0, valid0), [brow, brow + valid1))
     if (EPI == TC_POOL) {
       float4 pw = make_float4(0.f, 0.f, 0.f, 0.f);
       if (m < a.M) pw = *reinterpret_cast<const float4*>(a.pool_w + m * 4);
@@ -333,6 +335,8 @@ __device__ __forceinline__ void tc_pool_epilogue_tile(const TcArgs& a, float* pa
       const long long first = (long long)mt * TC_BM;
       const long long nxt = (first / a.pool_item_rows + 1) * a.pool_item_rows;
       brow = nxt - first < TC_BM ? (int)(nxt - first) : TC_BM;
+      valid0 = min(brow, max(0, a.pool_T - (a.pool_item_rows - (int)(nxt - first))));
+      valid1 = max(0, min(TC_BM - brow, a.pool_T));
       named_sync(bar, 128);
     }
     // accumulator fragment of this thread (tc_ptx.cuh): acc[h][4 j + e] is row 64 h + 16 quad + lane / 4 + 8 (e / 2),
@@ -378,21 +382,35 @@ __device__ __forceinline__ void tc_pool_epilogue_tile(const TcArgs& a, float* pa
       for (int c = c0; c < c0 + CW; c += 32) {
         if (EPI == TC_POOL) {
           // thread (row group rg, column col) sums its 32 rows of d for the K speakers -- independent accumulators, no
-          // cross-lane traffic -- split at `brow` between the tile's two items
+          // cross-lane traffic -- split at `brow` between the tile's two items.  The sums are taken around `piv`: 0, i.e. the
+          // BatchNorm shift, the channel's mean under its running statistics; but where two of the item's valid rows in the
+          // tile (rows past its pool_T frames hold garbage) sit far from it next to their difference, the channel's mean is
+          // not near the shift, and the pivot is their average: a mean-dominated channel loses nothing to cancellation.
+          // Where the running statistics do describe the channel, the shift is a better pivot than any one row: it is the
+          // channel's mean, while a row can sit several weighted deviations from a speaker's mean (the fused pooling then
+          // matches the two-pass stats_pool to 2e-6 instead of 2e-5 on OSP weights).  A row pair misses a mean-dominated
+          // channel only if the two rows differ by 1/8 of the mean: a spike of 125 deviations at mean / std 1000.
           const float* dsm = chunk + (c - c0) / 32 * (128 * 33);
           const float4* wsm = reinterpret_cast<const float4*>(pool_stage);
           float* stg = pool_stage + 128 * 4;          // [rg 4][item 2][8][32]
+          const int col = et & 31;
+          auto pivot = [&](int lo, int n) {
+            if (n <= 0) return 0.f;
+            const float pa = dsm[lo * 33 + col], pb = dsm[(lo + n / 2) * 33 + col];
+            return fabsf(pa + pb) > 16.f * fabsf(pa - pb) ? 0.5f * (pa + pb) : 0.f;
+          };
           if (c != c0) named_sync(bar, 128);   // the previous 32 columns' totals are read from stg
           {
-            const int rg = et >> 5, col = et & 31, r_lo = rg * 32, r_hi = r_lo + 32;
+            const int rg = et >> 5, r_lo = rg * 32, r_hi = r_lo + 32;
 #pragma unroll
             for (int sg = 0; sg < 2; sg++) {
               const int lo = sg == 0 ? r_lo : max(r_lo, brow), hi = sg == 0 ? min(r_hi, brow) : r_hi;
+              const float piv = sg ? pivot(brow < TC_BM ? brow : 0, valid1) : pivot(0, valid0);
               float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
               if (a.pool_K <= 3) {               // the usual three local speakers: the fourth weight is not touched
 #pragma unroll 8
                 for (int rr = lo; rr < hi; rr++) {
-                  const float dv = dsm[rr * 33 + col];
+                  const float dv = dsm[rr * 33 + col] - piv;
                   const float4 w4 = wsm[rr];
                   const float a0 = w4.x * dv, a1 = w4.y * dv, a2 = w4.z * dv;
                   s1[0] += a0; s1[1] += a1; s1[2] += a2;
@@ -401,7 +419,7 @@ __device__ __forceinline__ void tc_pool_epilogue_tile(const TcArgs& a, float* pa
               } else {
 #pragma unroll 8
                 for (int rr = lo; rr < hi; rr++) {
-                  const float dv = dsm[rr * 33 + col];
+                  const float dv = dsm[rr * 33 + col] - piv;
                   const float4 w4 = wsm[rr];
                   const float a0 = w4.x * dv, a1 = w4.y * dv, a2 = w4.z * dv, a3 = w4.w * dv;
                   s1[0] += a0; s1[1] += a1; s1[2] += a2; s1[3] += a3;
@@ -416,15 +434,20 @@ __device__ __forceinline__ void tc_pool_epilogue_tile(const TcArgs& a, float* pa
             }
           }
           named_sync(bar, 128);
-          // 2 items x K speakers x 2 sums x 32 columns: the four row groups' totals are added in a fixed order
+          // 2 items x K speakers x 2 sums x 32 columns: the four row groups' totals are added in a fixed order; slot 8 of an
+          // item is its pivot
           {
-            const int col = et & 31, twoK = 2 * a.pool_K;
+            const int twoK = 2 * a.pool_K, n = n0 + c + col;
             for (int q = et >> 5; q < 2 * twoK; q += 4) {
               const int sg = q >= twoK ? 1 : 0, j = q - sg * twoK;
               const float tot = ((stg[((0 * 2 + sg) * 8 + j) * 32 + col] + stg[((1 * 2 + sg) * 8 + j) * 32 + col]) +
                                  stg[((2 * 2 + sg) * 8 + j) * 32 + col]) + stg[((3 * 2 + sg) * 8 + j) * 32 + col];
-              const int n = n0 + c + col;
-              if (n < a.N && mt < a.m_tiles) a.pool_part[(((size_t)mt * 2 + sg) * 8 + j) * a.N + n] = tot;
+              if (n < a.N && mt < a.m_tiles) a.pool_part[(((size_t)mt * 2 + sg) * TC_POOL_SLOTS + j) * a.N + n] = tot;
+            }
+            if (et < 64 && n < a.N && mt < a.m_tiles) {
+              const int sg = et >> 5;
+              a.pool_part[(((size_t)mt * 2 + sg) * TC_POOL_SLOTS + 8) * a.N + n] = sg ? pivot(brow < TC_BM ? brow : 0, valid1)
+                                                                                      : pivot(0, valid0);
             }
           }
           if (c + 32 == c0 + CW) named_sync(bar, 128);     // the chunk buffer is rewritten by the next chunk
@@ -445,17 +468,23 @@ __device__ __forceinline__ void tc_pool_epilogue_tile(const TcArgs& a, float* pa
             const int f0 = (int)(p_first - item0 * (a.pool_item_rows / 3));       // its frame index inside item0
             const long long Mp = a.M / 3;
             const float bias = params[c + col];
+            // the sums are taken around the pooled value of the item's first window in the tile (`piv`)
+            auto pooled = [&](int pr) {
+              return fmaxf(fmaxf(dsm[(3 * pr) * 33 + col], dsm[(3 * pr + 1) * 33 + col]), dsm[(3 * pr + 2) * 33 + col]);
+            };
+            const float piv0 = pooled(0), piv1 = pooled(brow3 < a.tile_rows / 3 ? brow3 : 0);
             float s1[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};
             for (int pr = rg; pr < a.tile_rows / 3; pr += 4) {
-              const float v = fmaxf(fmaxf(dsm[(3 * pr) * 33 + col], dsm[(3 * pr + 1) * 33 + col]), dsm[(3 * pr + 2) * 33 + col]);
+              const float v = pooled(pr);
               const int sg = pr >= brow3 ? 1 : 0;
               const int frame = sg ? pr - brow3 : f0 + pr;
               const long long P = p_first + pr;
               if (P < Mp) {
                 if (n < a.N) a.out_f32[P * a.ldc + n] = v + bias;
                 if (frame < a.pool3_T) {
-                  s1[sg] += v;
-                  s2[sg] = fmaf(v, v, s2[sg]);
+                  const float dv = v - (sg ? piv1 : piv0);
+                  s1[sg] += dv;
+                  s2[sg] = fmaf(dv, dv, s2[sg]);
                 }
               }
             }
@@ -464,13 +493,16 @@ __device__ __forceinline__ void tc_pool_epilogue_tile(const TcArgs& a, float* pa
               stg[((rg * 2 + sg) * 2 + 0) * 32 + col] = s1[sg];
               stg[((rg * 2 + sg) * 2 + 1) * 32 + col] = s2[sg];
             }
+            if (rg == 0 && n < a.N)
+#pragma unroll
+              for (int sg = 0; sg < 2; sg++) a.pool_part[(((size_t)mt * 2 + sg) * TC_POOL3_SLOTS + 2) * a.N + n] = sg ? piv1 : piv0;
           }
           named_sync(bar, 128);
           {   // 2 items x 2 sums x 32 columns = 128 values, one per thread: the four row groups in a fixed order
             const int col = et & 31, q = et >> 5, sg = q >> 1, j = q & 1, n = n0 + c + col;
             const float tot = ((stg[((0 * 2 + sg) * 2 + j) * 32 + col] + stg[((1 * 2 + sg) * 2 + j) * 32 + col]) +
                                stg[((2 * 2 + sg) * 2 + j) * 32 + col]) + stg[((3 * 2 + sg) * 2 + j) * 32 + col];
-            if (n < a.N) a.pool_part[(((size_t)mt * 2 + sg) * 2 + j) * a.N + n] = tot;
+            if (n < a.N) a.pool_part[(((size_t)mt * 2 + sg) * TC_POOL3_SLOTS + j) * a.N + n] = tot;
           }
           named_sync(bar, 128);     // stg (and after the last 32 columns the chunk buffer) is rewritten next
           continue;
@@ -889,7 +921,7 @@ static int tc_setup(const TcGemm& g, int bn, int epi, bool halo, CUtensorMap* ma
   a.Wp = g.Wp; a.Hp = g.Hp; a.Wop = g.Wop; a.Hop = g.Hop; a.stride2 = g.stride2; a.relu = g.relu;
   a.res_hi = reinterpret_cast<const __nv_bfloat16*>(g.res_hi);
   a.res_lo = reinterpret_cast<const __nv_bfloat16*>(g.res_lo);
-  a.pool_w = g.pool_w; a.pool_part = g.pool_part; a.pool_item_rows = g.pool_item_rows; a.pool_K = g.pool_K;
+  a.pool_w = g.pool_w; a.pool_part = g.pool_part; a.pool_item_rows = g.pool_item_rows; a.pool_K = g.pool_K; a.pool_T = g.pool_T;
   a.cin = g.Cin;
   if (halo) {
     a.halo_rows = a_rows;
@@ -962,8 +994,9 @@ int launch_gemm_tc(const TcGemm& g, cudaStream_t st) {
     return launch_tc<128, TC_CONV2D, false>(g, st);
   }
   if (g.epi == TC_POOL) {
-    if (g.Npad % 128 || !g.pool_w || !g.pool_part || g.pool_K < 1 || g.pool_K > 4 || g.pool_item_rows < TC_BM) {
-      set_error("gemm_tc (pool): needs 128-wide tiles, 1..4 speakers and items of at least 128 rows");
+    if (g.Npad % 128 || !g.pool_w || !g.pool_part || g.pool_K < 1 || g.pool_K > 4 || g.pool_item_rows < TC_BM || g.pool_T < 1 ||
+        g.pool_T > g.pool_item_rows) {
+      set_error("gemm_tc (pool): needs 128-wide tiles, 1..4 speakers, items of at least 128 rows and 1..item rows valid frames");
       return -1;
     }
     return launch_tc<128, TC_POOL>(g, st);

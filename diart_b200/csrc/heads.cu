@@ -395,43 +395,67 @@ int launch_pool_weights_sets(const float* w, int B, int G, int F, int K, int ite
   return 0;
 }
 
-// pyannote StatsPool from the partial sums of the fused epilogue (d = x - pivot):
-//   mean = sum(w x) / v1,  std = sqrt( sum(w (x - mean)^2) / (v1 - v2 / v1 + eps) ),  v1 = sum w + eps, v2 = sum w^2
-// with sum(w (x - mean)^2) = S2 - 2 dm S1 + dm^2 S0, dm = mean - pivot = (S1 - pivot * eps) / v1, S0 = v1 - eps.  The partials of
-// the tiles that cover an item are added in tile order in float64.
-__global__ void __launch_bounds__(128) pool_finalize_kernel(const float* __restrict__ part, const float* __restrict__ vsum,
-                                                            const float* __restrict__ pivot, int K, int C, int item_rows, int T,
-                                                            float eps, float* __restrict__ pooled) {
+// pyannote StatsPool from the partial sums of the fused epilogue (d = x - pivot, pivot = the BatchNorm shift):
+//   mean = sum(w x) / v1,  std = sqrt( sum(w (x - mean)^2) / (v1 - v2 / v1 + eps) ),  v1 = sum w + eps, v2 = sum w^2,
+// v1, v2 as launch_pool_weights sums them (one near-one-hot speaker makes v1 - v2 / v1 a cancellation whose rounding must match
+// the un-fused pooling's).  Tile t of the item holds S1_t = sum w e, S2_t = sum w e^2 of e = d - p_t around its own pivot p_t
+// (a value of the channel).  In double, in tile order, each tile is shifted to the pivot P of the item's first tile,
+//   sum w (d - P) += S1_t + W_t (p_t - P),  sum w (d - P)^2 += S2_t + 2 (p_t - P) S1_t + W_t (p_t - P)^2,
+// with W_t = sum w over the tile's rows (from the row weights, once per (item, speaker)).  Every term is of the size of the
+// channel's spread, so a channel whose mean is large next to its spread loses nothing to cancellation.
+constexpr int POOL_FIN_TILES = 32;   // tile weights staged per round
+__global__ void __launch_bounds__(128) pool_finalize_kernel(const float* __restrict__ part, const float* __restrict__ row_w,
+                                                            const float* __restrict__ vsum, const float* __restrict__ pivot, int K,
+                                                            int C, int item_rows, int T, float eps, float* __restrict__ pooled) {
+  __shared__ double wt[POOL_FIN_TILES];
   const int q = blockIdx.y, b = q / K, k = q - b * K;
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= C) return;
-  const long long r0 = (long long)b * item_rows, r1 = r0 + T - 1;
-  double s1 = 0, s2 = 0;
-  for (long long mt = r0 / 128; mt <= r1 / 128; mt++) {
-    const int sg = (int)(b - (mt * 128) / item_rows);
-    const float* p = part + (((size_t)mt * 2 + sg) * 8 + 2 * k) * C + c;
-    s1 += p[0];
-    s2 += p[C];
+  const int c = blockIdx.x * blockDim.x + threadIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long r0 = (long long)b * item_rows, r1 = r0 + T - 1, mt_lo = r0 / 128;
+  const int ntiles = (int)(r1 / 128 - mt_lo + 1);
+  auto slots = [&](long long mt) { return part + (((size_t)mt * 2 + (int)(b - (mt * 128) / item_rows)) * TC_POOL_SLOTS) * C + c; };
+  const double P = c < C ? slots(mt_lo)[8 * C] : 0.0;
+  double W = 0, s1 = 0, s2 = 0, s2c = 0;
+  for (int t0 = 0; t0 < ntiles; t0 += POOL_FIN_TILES) {
+    const int nt = min(POOL_FIN_TILES, ntiles - t0);
+    if (t0) __syncthreads();                // the previous round's weights are read
+    // the item's weight in each tile (rows past T carry weight 0): warp w sums tiles w, w + 4, ..., a fixed shuffle tree
+    for (int t = warp; t < nt; t += 4) {
+      const long long mt = mt_lo + t0 + t;
+      double sw = 0;
+      for (long long r = max(r0, mt * 128) + lane; r <= min(r1, mt * 128 + 127); r += 32) sw += row_w[r * 4 + k];
+      for (int o = 16; o > 0; o >>= 1) sw += __shfl_xor_sync(0xffffffffu, sw, o);
+      if (lane == 0) wt[t] = sw;
+    }
+    __syncthreads();
+    if (c < C)
+      for (int t = 0; t < nt; t++) {
+        const float* p = slots(mt_lo + t0 + t);
+        const double w = wt[t], a1 = p[2 * k * C], a2 = p[(2 * k + 1) * C], dp = (double)p[8 * C] - P;
+        W += w;
+        s1 += a1 + w * dp;
+        s2 += a2 + dp * (2.0 * a1 + w * dp);
+        s2c += a2;
+      }
   }
+  if (c >= C) return;
   const double v1 = vsum[(size_t)q * 2], v2 = vsum[(size_t)q * 2 + 1], pv = pivot[c];
-  const double s0 = v1 - (double)eps;
-  const double dm = (s1 - pv * (double)eps) / v1;
-  double num = s2 - 2.0 * dm * s1 + dm * dm * s0;
-  // s1, s2 are float32 sums around the pivot: their rounding leaves about 2^-22 s2 in `num` where the centred sum is smaller
-  // than that (one frame carries all the weight: exactly 0, over a denominator of 1e-8).  Below 2^-20 s2 the variance is
-  // not resolved and is 0, which is what the centred two-pass pooling (stats_pool) returns there.
-  if (num < s2 * 9.5367431640625e-7) num = 0;
+  const double dm = (s1 + W * P - pv * (double)eps) / v1, dq = dm - P;     // mean - pivot; mean - P
+  double num = s2 - 2.0 * dq * s1 + dq * dq * W;
+  // The float32 sums around the pivots leave about 2^-22 of s2c in `num`.  Below 2^-20 s2c the variance is not resolved and
+  // is 0: that happens only when the weight sits on frames far from the pivots (one frame carries all the weight: exactly 0
+  // over a denominator of 1e-8), which is what the centred two-pass pooling (stats_pool) returns there.
+  if (num < s2c * 9.5367431640625e-7 || num < 0) num = 0;
   const double var = num / (v1 - v2 / v1 + (double)eps);
   float* o = pooled + (size_t)q * 2 * C;
   o[c] = (float)(pv + dm);
   o[C + c] = (float)sqrt(var);
 }
 
-int launch_pool_finalize(const float* part, const float* vsum, const float* pivot, int B, int K, int C, int item_rows, int T,
-                         float eps, float* pooled, cudaStream_t st) {
+int launch_pool_finalize(const float* part, const float* row_w, const float* vsum, const float* pivot, int B, int K, int C,
+                         int item_rows, int T, float eps, float* pooled, cudaStream_t st) {
   ProfScope _ps("pool_finalize", st);
   dim3 grid((C + 127) / 128, B * K);
-  pool_finalize_kernel<<<grid, 128, 0, st>>>(part, vsum, pivot, K, C, item_rows, T, eps, pooled);
+  pool_finalize_kernel<<<grid, 128, 0, st>>>(part, row_w, vsum, pivot, K, C, item_rows, T, eps, pooled);
   DG_LAUNCHED();
   return 0;
 }

@@ -170,22 +170,28 @@ int launch_instnorm_stats(const float* x, int B, int stride_rows, int T, int C, 
 }
 
 // InstanceNorm1d(affine) scale / shift from the per-tile partial sums of gemm_tc's TC_MAXPOOL3 epilogue (tiles of `tile_rows`
-// un-pooled rows, a divisor of the item's rows: slot 0 of the item's own tiles).  The sums are of the pooled values BEFORE the
-// bias, which serves as the pivot; the tiles of an item are added in tile order, in double.
-__global__ void __launch_bounds__(256) instnorm_finalize_kernel(const float* __restrict__ part, int tiles_per_item, int T, int C, int N,
-                                                                const float* __restrict__ bias, const float* __restrict__ gamma,
-                                                                const float* __restrict__ beta, float* __restrict__ sc,
-                                                                float* __restrict__ sh, int ld) {
+// un-pooled rows, a divisor of the item's rows: slot 0 of the item's own tiles).  Tile i holds, for its n_i pooled frames
+// v < T of the item (before the bias), the sums S1_i, S2_i of e = v - p_i and e^2 around its pivot p_i (a value of the channel).
+// In double, each tile is shifted to the pivot P of the item's first tile,
+//   sum (v - P) += S1_i + n_i (p_i - P),  sum (v - P)^2 += S2_i + 2 (p_i - P) S1_i + n_i (p_i - P)^2,
+// every term of the size of the channel's spread: no cancellation against the mean however large it is next to the spread.
+__global__ void __launch_bounds__(256) instnorm_finalize_kernel(const float* __restrict__ part, int tiles_per_item, int tile_frames,
+                                                                int T, int C, int N, const float* __restrict__ bias,
+                                                                const float* __restrict__ gamma, const float* __restrict__ beta,
+                                                                float* __restrict__ sc, float* __restrict__ sh, int ld) {
   // 4 tile groups x 64 channels: the loads of a group are independent, the groups are added in a fixed order
   __shared__ double s1[4][64], s2[4][64];
   const int b = blockIdx.x, c = threadIdx.x & 63, grp = threadIdx.x >> 6;
   const long long mt0 = (long long)b * tiles_per_item;
   const int per = (tiles_per_item + 3) / 4, lo = grp * per, hi = min(tiles_per_item, lo + per);
+  auto slot = [&](int i, int j) { return (double)part[(((mt0 + i) * 2 + 0) * TC_POOL3_SLOTS + j) * N + c]; };
+  const double P = c < C ? slot(0, 2) : 0.0;
   double t1 = 0, t2 = 0;
   if (c < C)
     for (int i = lo; i < hi; i++) {
-      t1 += part[(((mt0 + i) * 2 + 0) * 2 + 0) * N + c];
-      t2 += part[(((mt0 + i) * 2 + 0) * 2 + 1) * N + c];
+      const double n = max(0, min(tile_frames, T - i * tile_frames)), a1 = slot(i, 0), dp = slot(i, 2) - P;
+      t1 += a1 + n * dp;
+      t2 += slot(i, 1) + dp * (2.0 * a1 + n * dp);
     }
   s1[grp][c] = t1;
   s2[grp][c] = t2;
@@ -196,7 +202,7 @@ __global__ void __launch_bounds__(256) instnorm_finalize_kernel(const float* __r
   const double m = t1 / T;
   double var = t2 / T - m * m;
   if (var < 0) var = 0;
-  const double mean = m + (double)bias[c];
+  const double mean = P + m + (double)bias[c];
   const float r = (float)(1.0 / sqrt(var + 1e-5));
   const float gsc = gamma[c] * r;
   sc[(size_t)b * ld + c] = gsc;
@@ -206,11 +212,11 @@ __global__ void __launch_bounds__(256) instnorm_finalize_kernel(const float* __r
 int launch_instnorm_finalize(const float* part, int B, int item_rows, int tile_rows, int T, int C, int N, const float* bias,
                              const float* gamma, const float* beta, float* sc, float* sh, int ld, cudaStream_t st) {
   ProfScope _ps("instnorm_finalize", st);
-  if (C > 64 || tile_rows < 1 || item_rows % tile_rows) {
-    set_error("instnorm_finalize: at most 64 channels, tiles must divide the item");
+  if (C > 64 || tile_rows < 3 || tile_rows % 3 || item_rows % tile_rows) {
+    set_error("instnorm_finalize: at most 64 channels, tiles of whole pooling windows must divide the item");
     return -1;
   }
-  instnorm_finalize_kernel<<<B, 256, 0, st>>>(part, item_rows / tile_rows, T, C, N, bias, gamma, beta, sc, sh, ld);
+  instnorm_finalize_kernel<<<B, 256, 0, st>>>(part, item_rows / tile_rows, tile_rows / 3, T, C, N, bias, gamma, beta, sc, sh, ld);
   DG_LAUNCHED();
   return 0;
 }
