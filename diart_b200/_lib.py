@@ -147,6 +147,10 @@ SIGNATURES = {
     "dg_gallery_query": (C.c_int, [_P, _P, C.c_int, _P, _P, C.c_double, _P, _P, _P]),
     "dg_multi_set_gallery": (C.c_int, [_P, _P, C.c_double]),
     "dg_multi_set_names": (C.c_int, [_P, C.c_int, C.c_uint32, _P]),
+    "dg_multi_set_slot_gallery": (C.c_int, [_P, C.c_int, _P, C.c_double]),
+    "dg_selftest_gallery_plan_host": (C.c_int, [C.c_int, _P, C.c_int, _P, _P, _P, _P, _P, C.c_int, _P]),
+    "dg_selftest_multi_gallery_host": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, C.c_char_p,
+                                                 C.c_int]),
     "dg_multi_last_names": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int)]),
     "dg_selftest_multi_frames_host": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, C.c_int,
                                                 C.POINTER(C.c_int)]),

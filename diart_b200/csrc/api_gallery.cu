@@ -1,6 +1,8 @@
 // Speaker gallery (dg_gallery_*): an enrolled gallery on the device and the standalone nearest-entry query.  A dg_multi with
 // a gallery (dg_multi_set_gallery, api_multi.cu) runs the same kernels in its ticks.
+#include <limits.h>
 #include <math.h>
+#include <string.h>
 
 #include <algorithm>
 #include <cmath>
@@ -56,6 +58,51 @@ extern "C" int dg_gallery_destroy(dg_gallery* g) {
   return DG_OK;
 }
 
+// One launch of the standalone search over queries X [Q][D] whose claim-group segments start at seg [n_seg + 1] (seg[0] = 0,
+// seg[n_seg] = Q), query q in claim group grp[q]; Q * D <= INT_MAX (gallery_nearest's row offsets).
+static int query_launch(dg_gallery* g, const double* queries_dev, int Q, const int32_t* grp, const std::vector<int>& seg,
+                        const int32_t* claimed_dev, double threshold, int32_t* entry_dev, double* dist_dev, cudaStream_t st) {
+  const int n_seg = (int)seg.size() - 1;
+  if ((long long)Q * g->D > INT_MAX) {   // only a claim group of 32 rows of more than 67 million dimensions gets here
+    set_error("dg_gallery_query: " + std::to_string(Q) + " rows of dimension " + std::to_string(g->D) +
+              " in one claim group exceed 2^31 - 1 elements");
+    return DG_EINVAL;
+  }
+  std::vector<int2> qd((size_t)Q);
+  for (int q = 0; q < Q; q++) qd[q] = make_int2(q, grp[q]);
+  // the one-group plan of the tick's grouped search; every table travels in one copy
+  std::vector<GalGroup> groups(1, GalGroup{g->E.as<double>(), g->En.as<double>(), threshold, g->G, 0, 0, 0, Q, 0, n_seg, 0});
+  std::vector<GalWork> work;
+  const int splits = gallery_plan(groups, work), n_work = (int)work.size();
+  const std::vector<int2> segs((size_t)n_seg, make_int2(0, 0));
+  const int2 gq = make_int2(0, Q);
+  const size_t o_seg = ((size_t)Q * 8 + 15) & ~(size_t)15, o_segs = (o_seg + seg.size() * 4 + 15) & ~(size_t)15,
+               o_groups = (o_segs + (size_t)n_seg * 8 + 15) & ~(size_t)15, o_gq = o_groups + sizeof(GalGroup),
+               o_work = o_gq + 16, bytes = o_work + (size_t)n_work * sizeof(GalWork);
+  std::vector<unsigned char> in(bytes);
+  memcpy(in.data(), qd.data(), (size_t)Q * 8);
+  memcpy(in.data() + o_seg, seg.data(), seg.size() * 4);
+  memcpy(in.data() + o_segs, segs.data(), (size_t)n_seg * 8);
+  memcpy(in.data() + o_groups, groups.data(), sizeof(GalGroup));
+  memcpy(in.data() + o_gq, &gq, 8);
+  memcpy(in.data() + o_work, work.data(), (size_t)n_work * sizeof(GalWork));
+  if (g->ws_in.ensure(bytes) || g->ws_d.ensure((size_t)splits * Q * 8) || g->ws_e.ensure((size_t)splits * Q * 4)) return DG_ECUDA;
+  // a copy from pageable memory: staged before cudaMemcpyAsync returns
+  DG_CUDA(cudaMemcpyAsync(g->ws_in.p, in.data(), bytes, cudaMemcpyHostToDevice, st));
+  const unsigned char* din = g->ws_in.as<unsigned char>();
+  const int2* d_qd = reinterpret_cast<const int2*>(din);
+  const GalGroup* d_groups = reinterpret_cast<const GalGroup*>(din + o_groups);
+  int rc;
+  if ((rc = launch_gallery_nearest(d_groups, reinterpret_cast<const GalWork*>(din + o_work), n_work,
+                                   reinterpret_cast<const int2*>(din + o_gq), g->Dp, queries_dev, g->D, d_qd, Q, claimed_dev,
+                                   g->ws_d.as<double>(), g->ws_e.as<int>(), st)) ||
+      (rc = launch_gallery_claim(g->ws_d.as<double>(), g->ws_e.as<int>(), Q, d_qd, reinterpret_cast<const int*>(din + o_seg),
+                                 reinterpret_cast<const int2*>(din + o_segs), n_seg, d_groups, const_cast<int32_t*>(claimed_dev),
+                                 entry_dev, dist_dev, nullptr, 0, nullptr, nullptr, nullptr, st)))
+    return rc;
+  return DG_OK;
+}
+
 extern "C" int dg_gallery_query(dg_gallery* g, const double* queries_dev, int Q, const int32_t* group_dev,
                                 const int32_t* claimed_dev, double threshold, int32_t* entry_dev, double* dist_dev, void* stream) {
   const char* who = "dg_gallery_query";
@@ -73,7 +120,6 @@ extern "C" int dg_gallery_query(dg_gallery* g, const double* queries_dev, int Q,
   DG_CUDA(cudaMemcpyAsync(grp.data(), group_dev, (size_t)Q * 4, cudaMemcpyDeviceToHost, st));
   DG_CUDA(cudaStreamSynchronize(st));
   // the segments: each group one contiguous run of at most 32 queries
-  std::vector<int2> qd((size_t)Q);
   std::vector<int> seg(1, 0);
   std::vector<char> seen;
   for (int q = 0; q < Q; q++) {
@@ -95,23 +141,22 @@ extern "C" int dg_gallery_query(dg_gallery* g, const double* queries_dev, int Q,
       set_error(std::string(who) + ": group " + std::to_string(r) + " has more than 32 queries");
       return DG_EINVAL;
     }
-    qd[q] = make_int2(q, r);
   }
   seg.push_back(Q);
-  const int n_seg = (int)seg.size() - 1, splits = gallery_splits(g->G, Q);
-  if (g->ws_q.ensure((size_t)Q * 8) || g->ws_seg.ensure(seg.size() * 4) || g->ws_d.ensure((size_t)splits * Q * 8) ||
-      g->ws_e.ensure((size_t)splits * Q * 4))
-    return DG_ECUDA;
-  // copies from pageable memory: staged before cudaMemcpyAsync returns
-  DG_CUDA(cudaMemcpyAsync(g->ws_q.p, qd.data(), (size_t)Q * 8, cudaMemcpyHostToDevice, st));
-  DG_CUDA(cudaMemcpyAsync(g->ws_seg.p, seg.data(), seg.size() * 4, cudaMemcpyHostToDevice, st));
-  int rc;
-  if ((rc = launch_gallery_nearest(g->E.as<double>(), g->En.as<double>(), g->G, g->Gp, g->Dp, queries_dev, g->D,
-                                   g->ws_q.as<int2>(), nullptr, Q, claimed_dev, splits, g->ws_d.as<double>(), g->ws_e.as<int>(),
-                                   st)) ||
-      (rc = launch_gallery_claim(g->ws_d.as<double>(), g->ws_e.as<int>(), splits, Q, g->ws_q.as<int2>(), g->ws_seg.as<int>(),
-                                 n_seg, threshold, const_cast<int32_t*>(claimed_dev), entry_dev, dist_dev, nullptr, 0, nullptr,
-                                 nullptr, nullptr, st)))
-    return rc;
+  // one launch per run of whole segments of at most INT_MAX / D rows (gallery_nearest keeps 32-bit row offsets): a single
+  // launch unless Q * D exceeds 2^31 - 1
+  const int rows_max = (int)std::max<long long>(32, INT_MAX / g->D);
+  for (size_t s0 = 0; s0 + 1 < seg.size();) {
+    size_t s1 = s0 + 1;
+    while (s1 + 1 < seg.size() && seg[s1 + 1] - seg[s0] <= rows_max) s1++;
+    const int q0 = seg[s0], n = seg[s1] - q0;
+    std::vector<int> local(seg.begin() + s0, seg.begin() + s1 + 1);
+    for (int& o : local) o -= q0;
+    int rc;
+    if ((rc = query_launch(g, queries_dev + (size_t)q0 * g->D, n, grp.data() + q0, local, claimed_dev, threshold,
+                           entry_dev + q0, dist_dev + q0, st)))
+      return rc;
+    s0 = s1;
+  }
   return DG_OK;
 }

@@ -13,6 +13,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <map>
 #include <memory>
 #include <vector>
 
@@ -216,18 +217,71 @@ struct dg_multi {
   Event e_start, e_lane_done[2];
   Event t_begin, t_end;                       // timing events around the last tick's device work on `st`
   bool timed = false;                         // a tick has run
-  // gallery naming (dg_multi_set_gallery): per slot the named global speakers (bit g) and their claimed entries [slots][32],
-  // on the device and mirrored on the host; a tick's queries, segments, split partials and new names {slot, g, entry}
+  // gallery naming: the default gallery and threshold of every stream (dg_multi_set_gallery), and per slot the gallery and
+  // threshold its stream is named from (dg_multi_set_slot_gallery; null: none) and whether it has had a tick.  Once the
+  // handle has received a gallery: per slot the named global speakers (bit g) and their claimed entries [slots][32], indices
+  // into the slot's gallery, on the device and mirrored on the host (named_host non-empty); a tick's queries, segments, query
+  // offset and count per group, split partials and new names {slot, g, entry}
   dg_gallery* gal = nullptr;
   double gal_threshold = 0.0;
-  DevBuf gal_named, gal_claimed, gal_q, gal_seg, gal_n, gal_d, gal_e, gal_list;
+  std::vector<dg_gallery*> slot_gal;
+  std::vector<double> slot_thr;
+  std::vector<char> slot_ticked;
+  DevBuf gal_named, gal_claimed, gal_q, gal_seg, gal_gq, gal_d, gal_e, gal_list;
   std::vector<uint32_t> named_host;
   std::vector<int32_t> names_last;            // the names the last dg_multi_step decided, [n][3]
 };
 
-// In front of the header in h->header and in the tick's pinned download: with a gallery, the count of the tick's new names
-// (16 bytes) and the first GAL_NAME_PREFIX of them, so that they travel in the header's copy
-static size_t names_bytes(const dg_multi* h) { return h->gal ? 16 + (size_t)GAL_NAME_PREFIX * 12 : 0; }
+// In front of the header in h->header and in the tick's pinned download, once the handle has received a gallery: the count
+// of the tick's new names (16 bytes) and the first GAL_NAME_PREFIX of them, so that they travel in the header's copy
+static size_t names_bytes(const dg_multi* h) { return h->named_host.empty() ? 0 : 16 + (size_t)GAL_NAME_PREFIX * 12; }
+
+// The grouped gallery search of a tick (gallery_plan): groups (one per distinct gallery and threshold, in order of their
+// first slot), the tick's slots with a gallery as segments {slot, group} (group by group, slots in order), the work list,
+// the upper bound of the queries and the largest split count.
+struct GalTick {
+  std::vector<GalGroup> groups;
+  std::vector<int> keys;        // the gallery key of each group
+  std::vector<int2> segs;
+  std::vector<GalWork> work;
+  int queries = 0, splits = 0;
+};
+
+// the plan of n slots in slot order: slot[a], its gallery key[a] (-1: none; keys index G / thr), its unnamed speakers
+// unnamed[a]; the groups' gallery pointers are left null
+static void gallery_tick_plan(const int* slot, const int* key, const int* unnamed, int n, const int* G, const double* thr,
+                              GalTick& t) {
+  t = GalTick{};
+  std::vector<int> group_of_key;
+  std::vector<int>& keys = t.keys;
+  for (int a = 0; a < n; a++) {
+    const int k = key[a];
+    if (k < 0) continue;
+    if (k >= (int)group_of_key.size()) group_of_key.resize(k + 1, -1);
+    if (group_of_key[k] < 0) {
+      group_of_key[k] = (int)keys.size();
+      keys.push_back(k);
+    }
+  }
+  // the segments bucketed by group in one pass (a counting sort, stable in slot order): O(slots + groups)
+  const int ng = (int)keys.size();
+  t.groups.resize(ng);
+  std::vector<int> fill(ng + 1, 0);
+  for (int a = 0; a < n; a++)
+    if (key[a] >= 0) fill[group_of_key[key[a]] + 1]++;
+  for (int r = 0; r < ng; r++) fill[r + 1] += fill[r];
+  for (int r = 0; r < ng; r++)
+    t.groups[r] = GalGroup{nullptr, nullptr, thr[keys[r]], G[keys[r]], 0, 0, 0, 0, fill[r], fill[r + 1], 0};
+  t.segs.resize(fill[ng]);
+  for (int a = 0; a < n; a++) {
+    if (key[a] < 0) continue;
+    const int r = group_of_key[key[a]];
+    t.segs[fill[r]++] = make_int2(slot[a], r);
+    t.groups[r].q_ub += unnamed[a];
+    t.queries += unnamed[a];
+  }
+  t.splits = gallery_plan(t.groups, t.work);
+}
 
 static bool slot_ok(const dg_multi* h, int slot) { return h && h->book.ok(slot); }
 static bool vad_mode(const dg_multi* h) { return !h->net.emb; }
@@ -279,6 +333,7 @@ extern "C" int dg_multi_create(dg_seg* seg, dg_emb* emb, int chunk_samples, int 
   h->net.gamma = gamma; h->net.beta = beta; h->net.normalize_weights = normalize_weights;
   const size_t n = (size_t)max_streams, hist = (size_t)std::max(1, num_windows - 1);
   h->n_hist.assign(n, 0); h->cur.assign(n, 0); h->slot_nw.assign(n, num_windows); h->slot_par.assign(3 * n, 0.0);
+  h->slot_gal.assign(n, nullptr); h->slot_thr.assign(n, 0.0); h->slot_ticked.assign(n, 0);
   if (h->rings.ensure(n * h->book.C * 4) || h->hamming.ensure((size_t)F * 8) || h->centers.ensure(n * max_speakers * D * 8) ||
       h->active.ensure(n * 32 * 4) || h->init.ensure(n * 2 * 4) || h->hist_seg.ensure(2 * n * hist * F * K * 4) ||
       h->hist_map.ensure(2 * n * hist * K * 4) || h->total.ensure(16))
@@ -328,6 +383,7 @@ extern "C" int dg_multi_create_vad(dg_seg* seg, int chunk_samples, int step_samp
   h->net.seg = seg;
   const size_t n = (size_t)max_streams, hist = (size_t)std::max(1, num_windows - 1);
   h->n_hist.assign(n, 0); h->cur.assign(n, 0); h->slot_nw.assign(n, num_windows); h->slot_par.assign(3 * n, 0.0);
+  h->slot_gal.assign(n, nullptr); h->slot_thr.assign(n, 0.0); h->slot_ticked.assign(n, 0);
   if (h->rings.ensure(n * h->book.C * 4) || h->hamming.ensure((size_t)F * 8) || h->hist_vad.ensure(2 * n * hist * F * 4) ||
       h->total.ensure(16))
     return DG_ECUDA;
@@ -438,10 +494,15 @@ static int open_slot(dg_multi* h, int slot, int rate_id, int num_windows, const 
       DG_CUDA(cudaMemcpyAsync(h->init.as<int>() + s * 2, init, 2 * 4, cudaMemcpyHostToDevice, h->st));
     }
   }
-  if (h->gal) {   // a stream opens with no speaker named
+  if (!h->named_host.empty()) {   // a stream opens with no speaker named
     DG_CUDA(cudaMemsetAsync(h->gal_named.as<uint32_t>() + s, 0, 4, h->st));
     DG_CUDA(cudaMemsetAsync(h->gal_claimed.as<int32_t>() + s * 32, 0xff, 32 * 4, h->st));
     h->named_host[slot] = 0;
+  }
+  if (!vad) {   // named from the default gallery unless dg_multi_set_slot_gallery gives it its own
+    h->slot_gal[slot] = h->gal;
+    h->slot_thr[slot] = h->gal_threshold;
+    h->slot_ticked[slot] = 0;
   }
   h->book.start(slot, rate_id + 1);
   h->n_hist[slot] = 0;
@@ -484,6 +545,7 @@ extern "C" int dg_multi_close(dg_multi* h, int slot) {
     return DG_EINVAL;
   }
   h->book.stop(slot);
+  h->slot_gal[slot] = nullptr;   // the handle no longer refers to the stream's gallery
   return DG_OK;
 }
 
@@ -552,13 +614,15 @@ static size_t align16(size_t b) { return (b + 15) & ~(size_t)15; }
 // the resampling items and the resampled rows.
 struct TickIn {
   size_t o_pieces, o_act, o_rows, o_start, o_plan, o_states, o_off, o_trials, o_rows16, o_start16, o_items, o_rs, bytes;
+  size_t o_groups, o_segs, o_work;   // with gallery queries: the groups, segments and work list of the grouped search
   bool mixed;
 };
 
 // The audio-in half of a tick, the same in both modes: ONE copy of the staged samples and the tick's tables to h->in (t_begin
 // recorded before it), the staged samples to their rings, then the batch [B, S] of windows to h->wav, grouped by slot (windows
-// at a declared rate resampled); e_start marks the batch complete on h->st.
-static int tick_audio_in(dg_multi* h, const TickPlan& tp, const int32_t* plan_host, TickIn& L) {
+// at a declared rate resampled); e_start marks the batch complete on h->st.  A tick with gallery queries (gt) carries the
+// plan of its grouped search after the other tables.
+static int tick_audio_in(dg_multi* h, const TickPlan& tp, const int32_t* plan_host, const GalTick* gt, TickIn& L) {
   cudaStream_t st = h->st;
   const std::vector<TickSlot>& act = tp.act;
   const int B = tp.B, n_act = (int)act.size(), np = (int)h->book.pieces.size(), S = h->S, stride = 4 + h->nw;
@@ -577,6 +641,12 @@ static int tick_audio_in(dg_multi* h, const TickPlan& tp, const int32_t* plan_ho
   L.o_items = L.o_start16 + align16((size_t)n16 * 8);
   L.o_rs = L.o_items + align16((size_t)n_items * sizeof(RsFrames));
   L.bytes = L.mixed ? L.o_rs + (size_t)n_rs * sizeof(RsRow) : L.o_trials + (size_t)n_act * 24;
+  if (gt) {
+    L.o_groups = align16(L.bytes);
+    L.o_segs = L.o_groups + align16(gt->groups.size() * sizeof(GalGroup));
+    L.o_work = L.o_segs + align16(gt->segs.size() * 8);
+    L.bytes = L.o_work + gt->work.size() * sizeof(GalWork);
+  }
   if (h->in.ensure(L.bytes) || h->wav.ensure((size_t)B * S * 4)) return DG_ECUDA;
   if (L.bytes > h->stage.bytes) {
     PinnedBuf bigger;
@@ -606,6 +676,11 @@ static int tick_audio_in(dg_multi* h, const TickPlan& tp, const int32_t* plan_ho
   }
   for (int s = act.back().slot + 1; s <= h->slots; s++) off[s] = B;
   memcpy(pin + L.o_plan, plan_host, (size_t)B * stride * 4);
+  if (gt) {
+    memcpy(pin + L.o_groups, gt->groups.data(), gt->groups.size() * sizeof(GalGroup));
+    memcpy(pin + L.o_segs, gt->segs.data(), gt->segs.size() * 8);
+    memcpy(pin + L.o_work, gt->work.data(), gt->work.size() * sizeof(GalWork));
+  }
   unsigned char* din = h->in.as<unsigned char>();
   DG_CUDA(cudaEventRecord(h->t_begin, st));
   DG_CUDA(cudaMemcpyAsync(din, pin, L.bytes, cudaMemcpyHostToDevice, st));
@@ -688,27 +763,29 @@ static int tick_diarize(dg_multi* h, const TickPlan& tp, const TickIn& L, int tu
   return DG_OK;
 }
 
-// Gallery naming after a diarization tick, on h->st: the active, unnamed global speakers of the tick's slots (at most
-// `queries`, from the host mirror of the named tables) against the gallery; the new names go to the front of h->header.
-static int tick_gallery(dg_multi* h, const TickPlan& tp, const TickIn& L, int queries) {
+// Gallery naming after a diarization tick, on h->st: the active, unnamed global speakers of the tick's slots with a gallery
+// (at most gt.queries, from the host mirror of the named tables), each against its slot's gallery, in one grouped search;
+// the new names go to the front of h->header.
+static int tick_gallery(dg_multi* h, const GalTick& gt, const TickIn& L) {
   cudaStream_t st = h->st;
-  const dg_gallery* g = h->gal;
-  const int n_act = (int)tp.act.size(), splits = gallery_splits(g->G, queries);
-  if (h->gal_q.ensure((size_t)queries * 8) || h->gal_seg.ensure((size_t)(n_act + 1) * 4) || h->gal_n.ensure(16) ||
+  const int n = (int)gt.segs.size(), n_groups = (int)gt.groups.size(), queries = gt.queries, splits = gt.splits;
+  if (h->gal_q.ensure((size_t)queries * 8) || h->gal_seg.ensure((size_t)(n + 1) * 4) || h->gal_gq.ensure((size_t)n_groups * 8) ||
       h->gal_d.ensure((size_t)splits * queries * 8) || h->gal_e.ensure((size_t)splits * queries * 4) ||
       h->gal_list.ensure((size_t)queries * 12))
     return DG_ECUDA;
-  const TickSlot* d_act = reinterpret_cast<const TickSlot*>(h->in.as<unsigned char>() + L.o_act);
+  const unsigned char* din = h->in.as<unsigned char>();
+  const GalGroup* groups = reinterpret_cast<const GalGroup*>(din + L.o_groups);
+  const int2* segs = reinterpret_cast<const int2*>(din + L.o_segs);
   int* names = h->header.as<int>();
   int rc;
-  if ((rc = launch_gallery_queries(d_act, n_act, h->active.as<int>(), h->gal_named.as<uint32_t>(), h->M, h->gal_q.as<int2>(),
-                                   h->gal_seg.as<int>(), h->gal_n.as<int>(), names, st)) ||
-      (rc = launch_gallery_nearest(g->E.as<double>(), g->En.as<double>(), g->G, g->Gp, g->Dp, h->centers.as<double>(), h->D,
-                                   h->gal_q.as<int2>(), h->gal_n.as<int>(), queries, h->gal_claimed.as<int32_t>(), splits,
+  if ((rc = launch_gallery_queries(segs, n, groups, n_groups, h->active.as<int>(), h->gal_named.as<uint32_t>(), h->M,
+                                   h->gal_q.as<int2>(), h->gal_seg.as<int>(), h->gal_gq.as<int2>(), names, st)) ||
+      (rc = launch_gallery_nearest(groups, reinterpret_cast<const GalWork*>(din + L.o_work), (int)gt.work.size(),
+                                   h->gal_gq.as<int2>(), (h->D + GAL_KC - 1) / GAL_KC * GAL_KC, h->centers.as<double>(), h->D, h->gal_q.as<int2>(), queries, h->gal_claimed.as<int32_t>(),
                                    h->gal_d.as<double>(), h->gal_e.as<int>(), st)) ||
-      (rc = launch_gallery_claim(h->gal_d.as<double>(), h->gal_e.as<int>(), splits, queries, h->gal_q.as<int2>(),
-                                 h->gal_seg.as<int>(), n_act, h->gal_threshold, h->gal_claimed.as<int32_t>(), nullptr, nullptr,
-                                 h->gal_named.as<uint32_t>(), h->M, names, h->gal_list.as<int32_t>(), names + 4, st)))
+      (rc = launch_gallery_claim(h->gal_d.as<double>(), h->gal_e.as<int>(), queries, h->gal_q.as<int2>(), h->gal_seg.as<int>(),
+                                 segs, n, groups, h->gal_claimed.as<int32_t>(), nullptr, nullptr, h->gal_named.as<uint32_t>(),
+                                 h->M, names, h->gal_list.as<int32_t>(), names + 4, st)))
     return rc;
   return DG_OK;
 }
@@ -797,13 +874,41 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
   if (!vad_mode(h) && (h->emb.ensure((size_t)B * K * D * 4) || h->maps.ensure((size_t)B * K * 4) ||
                        h->prep.ensure(cluster_prep_floats(B, K) * 4 + 16) || h->prep_d.ensure(cluster_prep_doubles(B, K) * 8 + 16)))
     return DG_ECUDA;
-  int queries = 0;             // with a gallery: the unnamed global speakers of the tick's slots, an upper bound of its queries
-  if (h->gal)
-    for (const TickSlot& ts : act) queries += M - __builtin_popcount(h->named_host[ts.slot]);
+  // with galleries: the tick's slots grouped by gallery and threshold; the unnamed global speakers of a slot are an upper
+  // bound of its queries
+  GalTick gt;
+  if (!h->named_host.empty()) {
+    std::vector<int> slot, key, unnamed, G;
+    std::vector<double> thr;
+    std::vector<const dg_gallery*> gals;
+    std::map<std::pair<const dg_gallery*, double>, int> key_of;   // (gallery, threshold) -> key
+    for (const TickSlot& ts : act) {
+      const dg_gallery* g = h->slot_gal[ts.slot];
+      int k = -1;
+      if (g) {
+        const auto it = key_of.emplace(std::make_pair(g, h->slot_thr[ts.slot]), (int)gals.size()).first;
+        k = it->second;
+        if (k == (int)gals.size()) {
+          gals.push_back(g);
+          thr.push_back(h->slot_thr[ts.slot]);
+          G.push_back(g->G);
+        }
+      }
+      slot.push_back(ts.slot);
+      key.push_back(k);
+      unnamed.push_back(M - __builtin_popcount(h->named_host[ts.slot]));
+    }
+    gallery_tick_plan(slot.data(), key.data(), unnamed.data(), (int)act.size(), G.data(), thr.data(), gt);
+    for (size_t r = 0; r < gt.groups.size(); r++) {
+      gt.groups[r].E = gals[gt.keys[r]]->E.as<double>();
+      gt.groups[r].En = gals[gt.keys[r]]->En.as<double>();
+    }
+  }
+  const int queries = gt.queries;
   TickIn in;
-  if ((rc = tick_audio_in(h, tp, plan_host, in)) ||
+  if ((rc = tick_audio_in(h, tp, plan_host, queries > 0 ? &gt : nullptr, in)) ||
       (rc = vad_mode(h) ? tick_vad(h, tp, in, turn_cap) : tick_diarize(h, tp, in, turn_cap)) ||
-      (queries > 0 && (rc = tick_gallery(h, tp, in, queries))))
+      (queries > 0 && (rc = tick_gallery(h, gt, in))))
     return rc;
   if (seg_dev) DG_CUDA(cudaMemcpyAsync(seg_dev, h->seg.p, (size_t)B * F * K * 4, cudaMemcpyDeviceToDevice, st));
   if (emb_dev) DG_CUDA(cudaMemcpyAsync(emb_dev, h->emb.p, (size_t)B * K * D * 4, cudaMemcpyDeviceToDevice, st));
@@ -821,6 +926,7 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
   h->book.uploaded();
   h->book.consumed(tp);
   for (const TickSlot& ts : act) {
+    h->slot_ticked[ts.slot] = 1;
     if (h->nw > 1) {
       h->n_hist[ts.slot] = std::min(ts.nw - 1, ts.n_hist + ts.n);
       h->cur[ts.slot] ^= 1;
@@ -842,6 +948,30 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
   return download_turns(who, po, lay, h->turns.as<uint32_t>(), header_host, turns_host, turn_cap_host, n_turns, st);
 }
 
+// the named and claimed tables, on the first gallery the handle receives: every slot with nothing named or claimed
+static int gallery_tables(dg_multi* h) {
+  if (!h->named_host.empty()) return DG_OK;
+  if (h->gal_named.ensure((size_t)h->slots * 4) || h->gal_claimed.ensure((size_t)h->slots * 32 * 4)) return DG_ECUDA;
+  DG_CUDA(cudaMemsetAsync(h->gal_named.p, 0, (size_t)h->slots * 4, h->st));
+  DG_CUDA(cudaMemsetAsync(h->gal_claimed.p, 0xff, (size_t)h->slots * 32 * 4, h->st));
+  h->named_host.assign(h->slots, 0);
+  return DG_OK;
+}
+
+// a gallery and threshold `who` may give a stream of h: DG_EINVAL naming what rules them out
+static int check_gallery_for(const dg_multi* h, const dg_gallery* g, double threshold, const char* who) {
+  if (g->D != h->D || g->device != h->device) {
+    set_error(std::string(who) + ": the gallery's entries have dimension " + std::to_string(g->D) + " on device " +
+              std::to_string(g->device) + ", the embeddings " + std::to_string(h->D) + " on device " + std::to_string(h->device));
+    return DG_EINVAL;
+  }
+  if (!(std::isfinite(threshold) && threshold > 0.0 && threshold <= 2.0)) {
+    set_error(std::string(who) + ": need a finite threshold in (0, 2]");
+    return DG_EINVAL;
+  }
+  return DG_OK;
+}
+
 extern "C" int dg_multi_set_gallery(dg_multi* h, dg_gallery* g, double threshold) {
   const char* who = "dg_multi_set_gallery";
   if (!h || !g) {
@@ -853,38 +983,58 @@ extern "C" int dg_multi_set_gallery(dg_multi* h, dg_gallery* g, double threshold
                                                : ": a gallery is set before any stream is opened"));
     return DG_EINVAL;
   }
-  if (g->D != h->D || g->device != h->device) {
-    set_error(std::string(who) + ": the gallery's entries have dimension " + std::to_string(g->D) + " on device " +
-              std::to_string(g->device) + ", the embeddings " + std::to_string(h->D) + " on device " + std::to_string(h->device));
-    return DG_EINVAL;
-  }
-  if (!(std::isfinite(threshold) && threshold > 0.0 && threshold <= 2.0)) {
-    set_error(std::string(who) + ": need a finite threshold in (0, 2]");
-    return DG_EINVAL;
-  }
+  int rc;
+  if ((rc = check_gallery_for(h, g, threshold, who))) return rc;
   DG_CUDA(cudaSetDevice(h->device));
-  if (h->gal_named.ensure((size_t)h->slots * 4) || h->gal_claimed.ensure((size_t)h->slots * 32 * 4)) return DG_ECUDA;
-  h->named_host.assign(h->slots, 0);
+  if ((rc = gallery_tables(h))) return rc;
   h->gal = g;
   h->gal_threshold = threshold;
   return DG_OK;
 }
 
-extern "C" int dg_multi_set_names(dg_multi* h, int slot, uint32_t named, const int32_t* claimed_host) {
-  const char* who = "dg_multi_set_names";
-  if (!slot_ok(h, slot) || !h->gal || !claimed_host) {
-    set_error(std::string(who) + ": need an open slot of a handle with a gallery and a non-null table");
+extern "C" int dg_multi_set_slot_gallery(dg_multi* h, int slot, dg_gallery* g, double threshold) {
+  const char* who = "dg_multi_set_slot_gallery";
+  if (!h || !g) {
+    set_error(std::string(who) + ": null handle");
     return DG_EINVAL;
   }
-  const int M = h->M;
+  if (vad_mode(h)) {
+    set_error(std::string(who) + ": a VAD handle has no speakers to name");
+    return DG_EINVAL;
+  }
+  if (!slot_ok(h, slot) || h->slot_ticked[slot]) {
+    set_error(std::string(who) + ": slot " + std::to_string(slot) +
+              (slot_ok(h, slot) ? " has had a tick: a stream's gallery is set before its first tick" : " is not open"));
+    return DG_EINVAL;
+  }
+  int rc;
+  if ((rc = check_gallery_for(h, g, threshold, who))) return rc;
+  DG_CUDA(cudaSetDevice(h->device));
+  if ((rc = gallery_tables(h))) return rc;
+  // the stream starts over with nothing named or claimed in its gallery
+  DG_CUDA(cudaMemsetAsync(h->gal_named.as<uint32_t>() + slot, 0, 4, h->st));
+  DG_CUDA(cudaMemsetAsync(h->gal_claimed.as<int32_t>() + (size_t)slot * 32, 0xff, 32 * 4, h->st));
+  h->named_host[slot] = 0;
+  h->slot_gal[slot] = g;
+  h->slot_thr[slot] = threshold;
+  return DG_OK;
+}
+
+extern "C" int dg_multi_set_names(dg_multi* h, int slot, uint32_t named, const int32_t* claimed_host) {
+  const char* who = "dg_multi_set_names";
+  if (!slot_ok(h, slot) || vad_mode(h) || !h->slot_gal[slot] || !claimed_host) {
+    set_error(std::string(who) + ": need an open slot with a gallery and a non-null table");
+    return DG_EINVAL;
+  }
+  const int M = h->M, G = h->slot_gal[slot]->G;
   std::vector<int32_t> row(32, -1);
   for (int g = 0; g < M; g++) {
     const int e = claimed_host[g];
-    const bool ok = e == -1 || (e >= 0 && e < h->gal->G && ((named >> g) & 1) &&
+    const bool ok = e == -1 || (e >= 0 && e < G && ((named >> g) & 1) &&
                                 std::find(claimed_host, claimed_host + g, e) == claimed_host + g);
     if (!ok) {
       set_error(std::string(who) + ": speaker " + std::to_string(g) + " claims entry " + std::to_string(e) +
-                " (an entry of the gallery, claimed once, by a named speaker)");
+                " (an entry of the slot's gallery of " + std::to_string(G) + ", claimed once, by a named speaker)");
       return DG_EINVAL;
     }
     row[g] = e;
@@ -1050,5 +1200,121 @@ extern "C" int dg_selftest_multi_staging_host(int slots, int C, int n_ops, const
     }
     result[i] = rc;
   }
+  return DG_OK;
+}
+
+// The grouped gallery search plan of a tick on its own (test hook, no GPU): the tick's slots [n][3] = {slot, gallery key
+// (-1: none), unnamed speakers} in slot order, galleries G [n_keys] at thresholds thr [n_keys] -> groups [.][6] = {key, G,
+// tiles, per_split, splits, q_ub}, segments [.][2] = {slot, group}, work list [cap][3] = {group, tile, split}, counts [4] =
+// {groups, segments, work items, splits}.  groups and segments need room for n entries.
+extern "C" int dg_selftest_gallery_plan_host(int n, const int32_t* slots, int n_keys, const int32_t* G, const double* thr,
+                                             int32_t* groups_out, int32_t* segs_out, int32_t* work_out, int cap,
+                                             int32_t* counts) {
+  const char* who = "dg_selftest_gallery_plan_host";
+  if (n < 0 || (n && (!slots || !groups_out || !segs_out)) || n_keys < 0 || (n_keys && (!G || !thr)) || cap < 0 ||
+      (cap && !work_out) || !counts) {
+    set_error(std::string(who) + ": bad arguments");
+    return DG_EINVAL;
+  }
+  std::vector<int> slot(n), key(n), unnamed(n);
+  for (int a = 0; a < n; a++) {
+    slot[a] = slots[3 * a];
+    key[a] = slots[3 * a + 1];
+    unnamed[a] = slots[3 * a + 2];
+    if (key[a] < -1 || key[a] >= n_keys || unnamed[a] < 0 || unnamed[a] > 32) {
+      set_error(std::string(who) + ": slot entry " + std::to_string(a) + " is out of range");
+      return DG_EINVAL;
+    }
+  }
+  for (int k = 0; k < n_keys; k++)
+    if (G[k] < 1) {
+      set_error(std::string(who) + ": gallery " + std::to_string(k) + " is empty");
+      return DG_EINVAL;
+    }
+  GalTick t;
+  gallery_tick_plan(slot.data(), key.data(), unnamed.data(), n, G, thr, t);
+  counts[0] = (int)t.groups.size();
+  counts[1] = (int)t.segs.size();
+  counts[2] = (int)t.work.size();
+  counts[3] = t.splits;
+  for (size_t r = 0; r < t.groups.size(); r++) {
+    const GalGroup& g = t.groups[r];
+    const int32_t row[6] = {t.keys[r], g.G, g.tiles, g.per_split, g.splits, g.q_ub};
+    memcpy(groups_out + 6 * r, row, sizeof(row));
+  }
+  memcpy(segs_out, t.segs.data(), t.segs.size() * 8);
+  if ((int)t.work.size() > cap) {
+    set_error(std::string(who) + ": " + std::to_string(t.work.size()) + " work items, room for " + std::to_string(cap));
+    return DG_EINVAL;
+  }
+  memcpy(work_out, t.work.data(), t.work.size() * sizeof(GalWork));
+  return DG_OK;
+}
+
+// dg_multi_set_slot_gallery and dg_multi_set_names on a handle without a device (test hook): `slots` slots of a diarization
+// handle with embeddings of dimension D and M speakers on device 0, galleries gal [n_gal][3] = {G, D, device}, driven by
+// ops [n_ops][4] = {kind, slot, arg, x}: 0 open the slot (no default gallery), 1 dg_multi_set_slot_gallery(slot, gallery
+// arg (-1: null), threshold x), 2 give the slot gallery arg as dg_multi_set_slot_gallery leaves it (host state only),
+// 3 dg_multi_set_names(slot, named = arg, speaker 0 claiming entry x, the others none), 4 the slot has had a tick, 5 close
+// the slot.  result [n_ops]: each op's return code; messages [msg_cap]: each op's error message ("" when none), one per line.
+// Only refusals reach the device-free end of an entry point: an accepted call 1 or 3 fails with DG_ECUDA where no device is.
+extern "C" int dg_selftest_multi_gallery_host(int slots, int D, int M, int n_gal, const int32_t* gal, int n_ops,
+                                              const double* ops, int32_t* result, char* messages, int msg_cap) {
+  const char* who = "dg_selftest_multi_gallery_host";
+  if (slots < 1 || D < 2 || M < 1 || M > 32 || n_gal < 0 || (n_gal && !gal) || n_ops < 0 || (n_ops && (!ops || !result)) ||
+      msg_cap < 1 || !messages) {
+    set_error(std::string(who) + ": bad arguments");
+    return DG_EINVAL;
+  }
+  std::vector<dg_gallery> gals((size_t)n_gal);
+  for (int i = 0; i < n_gal; i++) {
+    gals[i].G = gal[3 * i];
+    gals[i].D = gal[3 * i + 1];
+    gals[i].device = gal[3 * i + 2];
+  }
+  dg_multi h;
+  h.slots = slots;
+  h.D = D;
+  h.M = M;
+  h.net.emb = reinterpret_cast<dg_emb*>(&h);   // a diarization handle (never dereferenced here)
+  h.book.init(slots, RateGeom{});
+  h.slot_gal.assign(slots, nullptr);
+  h.slot_thr.assign(slots, 0.0);
+  h.slot_ticked.assign(slots, 0);
+  std::string text;
+  for (int i = 0; i < n_ops; i++) {
+    const int kind = (int)ops[4 * i], slot = (int)ops[4 * i + 1], arg = (int)ops[4 * i + 2];
+    const double x = ops[4 * i + 3];
+    const bool in_range = slot >= 0 && slot < slots;
+    int rc = DG_OK;
+    set_error("");
+    if (kind == 0 && in_range && !h.book.open[slot]) {
+      h.book.start(slot);
+      h.slot_gal[slot] = nullptr;
+      h.slot_ticked[slot] = 0;
+    } else if (kind == 1 && arg >= -1 && arg < n_gal) {
+      rc = dg_multi_set_slot_gallery(&h, slot, arg < 0 ? nullptr : &gals[arg], x);
+    } else if (kind == 2 && in_range && arg >= 0 && arg < n_gal) {
+      h.slot_gal[slot] = &gals[arg];
+    } else if (kind == 3) {
+      std::vector<int32_t> claimed((size_t)M, -1);
+      claimed[0] = (int32_t)x;
+      rc = dg_multi_set_names(&h, slot, (uint32_t)arg, claimed.data());
+    } else if (kind == 4 && in_range) {
+      h.slot_ticked[slot] = 1;
+    } else if (kind == 5 && in_range && h.book.open[slot]) {
+      h.book.stop(slot);
+    } else {
+      rc = DG_EINVAL;
+      set_error(std::string(who) + ": op " + std::to_string(i) + " is not valid");
+    }
+    result[i] = rc;
+    text += rc ? std::string(dg_last_error()) : std::string();
+    text += '\n';
+  }
+  h.net.emb = nullptr;
+  const size_t n = std::min(text.size(), (size_t)msg_cap - 1);
+  memcpy(messages, text.data(), n);
+  messages[n] = 0;
   return DG_OK;
 }

@@ -412,31 +412,49 @@ int launch_resample_gather(const float* rings, long long C, const float* yrings,
 void fbank_frame_operator(std::vector<float>& op /*[514][400]*/);
 void fbank_mel_banks(std::vector<float>& banks /*[80][257]*/, std::vector<int>& k_lo, std::vector<int>& k_hi);
 
-// gallery.cu -- nearest-centroid search over a speaker gallery E [Gp][Dp] float64 (rows >= G and columns >= D zero; Gp a
-// multiple of GAL_TILE_E, Dp of GAL_KC) with norms En [G].  A query q is row qd[q].x of X [*][D] (row stride D) in claim
-// group qd[q].y; group r's claimed entries are claimed [r][32] (-1: none; claimed null: no claims).  The cosine distance is
-// 1 - clip(u.v / (|u| |v|), -1, 1) in float64.
+// gallery.cu -- nearest-centroid search over speaker galleries, each E [Gp][Dp] float64 (rows >= G and columns >= D zero;
+// Gp a multiple of GAL_TILE_E, Dp of GAL_KC, Dp the same for every gallery of a launch) with norms En [G].  A launch serves
+// one or more groups, each one gallery at one threshold; a group's queries are one contiguous run.  A query q is row
+// qd[q].x of X [*][D] (row stride D) in claim group qd[q].y; claim group r's claimed entries are claimed [r][32], indices
+// into its group's gallery (-1: none; claimed null: no claims).  The cosine distance is 1 - clip(u.v / (|u| |v|), -1, 1) in
+// float64.
 constexpr int GAL_TILE_E = 64, GAL_TILE_Q = 128, GAL_KC = 16, GAL_NAME_PREFIX = 1024;
+// A group of a launch: its gallery (E, En, G entries), threshold, and from gallery_plan its GAL_TILE_E-entry tiles split
+// into `splits` runs of per_split tiles; q_ub an upper bound of its queries (host); its segments [seg0, seg1).
+struct GalGroup {
+  const double* E;
+  const double* En;
+  double threshold;
+  int G, tiles, per_split, splits, q_ub, seg0, seg1, pad;
+};
+// one CTA of gallery_nearest: query tile `tile` of group `group` against split `split` of its gallery's tiles
+struct GalWork {
+  int group, tile, split;
+};
 int launch_gallery_norms(const double* E, int G, int Dp, double* En, cudaStream_t st);
-// the number of gallery splits of a launch over Qmax queries (partials [splits][Qmax])
-int gallery_splits(int G, int Qmax);
-// per query and split, the lexicographic minimum (distance, entry) over the unclaimed entries of the split: part_d / part_e
-// [splits][Qmax] (+inf / -1 when none).  The query count is *n_dev (n_dev null: Qmax).
-int launch_gallery_nearest(const double* E, const double* En, int G, int Gp, int Dp, const double* X, int D, const int2* qd,
-                           const int* n_dev, int Qmax, const int32_t* claimed, int splits, double* part_d, int* part_e,
+// The grouped search plan: each group's tiles and splits, and the work list.  The split count is chosen over the query
+// tiles of all groups (about two CTAs per SM in total, at most 64, at most a group's tiles); items are split-major, then
+// group, then query tile, so one group is the grid (query tiles, splits).  Returns the largest split count (partials
+// [splits][Qmax]).
+int gallery_plan(std::vector<GalGroup>& groups, std::vector<GalWork>& work);
+// per query and split of its group, the lexicographic minimum (distance, entry) over the unclaimed entries of the split:
+// part_d / part_e [splits][Qmax] (+inf / -1 when none).  Group r's queries are [gq[r].x, gq[r].x + gq[r].y).
+int launch_gallery_nearest(const GalGroup* groups, const GalWork* work, int n_work, const int2* gq, int Dp, const double* X,
+                           int D, const int2* qd, int Qmax, const int32_t* claimed, double* part_d, int* part_e,
                            cudaStream_t st);
 // the multi-stream queries of a tick: every active (active [slot][32]), unnamed (named [slot] bit g) global speaker g < M of
-// the slots of act [n_act], in slot then g order, as qd = {slot M + g, slot}; seg_off [n_act + 1] its queries per entry of
-// act, *n_dev their number; names [0] (the count of new names) reset to 0.
-int launch_gallery_queries(const TickSlot* act, int n_act, const int* active, const uint32_t* named, int M, int2* qd,
-                           int* seg_off, int* n_dev, int* names, cudaStream_t st);
-// One warp per segment [seg_off[s], seg_off[s + 1]) (at most 32 queries of one claim group): each query's best over the
-// splits; a candidate when distance < threshold; among candidates for one entry the smallest (distance, position) wins.
-// entry_out / dist_out (standalone, may be null): per query the winner's entry or -1, and its best distance.  named non-null
-// (streams): each winner g = qd.x mod M of group r sets named [r] bit g and claimed [r][g], and appends {r, g, entry} to
-// list [.][3] at names [0]++ (the first GAL_NAME_PREFIX entries also to prefix [.][3]).
-int launch_gallery_claim(const double* part_d, const int* part_e, int splits, int Qmax, const int2* qd, const int* seg_off,
-                         int n_seg, double threshold, int32_t* claimed, int32_t* entry_out, double* dist_out, uint32_t* named,
-                         int M, int* names, int32_t* list, int32_t* prefix, cudaStream_t st);
+// the tick's segments segs [n] = {slot, group} (group by group, slots in order), in segment then g order, as
+// qd = {slot M + g, slot}; seg_off [n + 1] its queries per segment, gq [group] = {offset, count} of each group's queries
+// (groups [n_groups]: its segments); names [0] (the count of new names) reset to 0.
+int launch_gallery_queries(const int2* segs, int n, const GalGroup* groups, int n_groups, const int* active,
+                           const uint32_t* named, int M, int2* qd, int* seg_off, int2* gq, int* names, cudaStream_t st);
+// One warp per segment [seg_off[s], seg_off[s + 1]) (at most 32 queries of one claim group) of group segs[s].y: each
+// query's best over its group's splits; a candidate when distance < the group's threshold; among candidates for one entry the
+// smallest (distance, position) wins.  entry_out / dist_out (standalone, may be null): per query the winner's entry or -1, and
+// its best distance.  named non-null (streams): each winner g = qd.x mod M of claim group r sets named [r] bit g and claimed
+// [r][g], and appends {r, g, entry} to list [.][3] at names [0]++ (the first GAL_NAME_PREFIX entries also to prefix [.][3]).
+int launch_gallery_claim(const double* part_d, const int* part_e, int Qmax, const int2* qd, const int* seg_off,
+                         const int2* segs, int n_seg, const GalGroup* groups, int32_t* claimed, int32_t* entry_out,
+                         double* dist_out, uint32_t* named, int M, int* names, int32_t* list, int32_t* prefix, cudaStream_t st);
 
 }  // namespace dg

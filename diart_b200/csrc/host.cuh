@@ -310,10 +310,11 @@ struct dg_resample {
 };
 
 // ==================================================================================== gallery (api_gallery.cu)
-// entries E [Gp][Dp] float64, zero padded (gallery.cu), norms En [G]; ws_*: the workspace of dg_gallery_query
+// entries E [Gp][Dp] float64, zero padded (gallery.cu), norms En [G]; ws_*: the workspace of dg_gallery_query (its tables
+// in one copy, the split partials)
 struct dg_gallery {
   int device = 0, G = 0, Gp = 0, D = 0, Dp = 0;
-  DevBuf E, En, ws_q, ws_seg, ws_d, ws_e;
+  DevBuf E, En, ws_in, ws_d, ws_e;
 };
 
 // ======================================================================== device-side audio stream (api_stream.cu)

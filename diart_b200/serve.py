@@ -29,7 +29,8 @@ dedicated pipeline whose configuration is the server's with that stream's values
 A diarization stream may also start from known speakers (``open(speakers=...)``, ``diart_b200.speakers``): its clustering
 state is seeded with their centroids and its annotations name them; ``speakers(sid)`` exports a stream's state, so that a
 closed stream can be resumed with the same centroids and labels.  With a ``gallery`` (``speakers.SpeakerGallery``), every tick
-also names the streams' discovered speakers from it on the device."""
+also names the streams' discovered speakers from it on the device; ``open(gallery=...)`` gives a stream its own gallery and
+threshold instead, and one grouped search per tick serves every gallery in use."""
 from __future__ import annotations
 
 import ctypes as C
@@ -72,6 +73,17 @@ def plan_rows(idx: np.ndarray, step: float, window_samples: int, sample_rate: in
     valid = j < nb[:, None]
     s_j, r_j = start_res(np.where(valid, (idx - (nb - 1))[:, None] + j, 0).astype(np.float64), win[:, None])
     return crop_plan(starts, res, s_j, r_j, nb, valid, nw, frames, step, latency)
+
+
+def same_device(a, b) -> bool:
+    """whether torch devices ``a`` and ``b`` are the same CUDA device (an index-less ``cuda`` is the current one)"""
+    a, b = torch.device(a), torch.device(b)
+    if a.type != b.type:
+        return False
+    if a.type != "cuda":
+        return True
+    index = lambda d: d.index if d.index is not None else torch.cuda.current_device()  # noqa: E731
+    return index(a) == index(b)
 
 
 def available_windows(pushed: np.ndarray, emitted: np.ndarray, window_samples, step_samples) -> np.ndarray:
@@ -339,7 +351,13 @@ class MultiStreamDiarization(_MultiStreamServer):
     be cosine): after every tick, each stream that had windows names its active, unnamed global speakers from the gallery by
     the gallery's rule, on the device; the tick's annotations already carry the names it decided, and a name stays for the
     rest of the stream's life.  A stream opened with known speakers counts them as named and their gallery entries as
-    claimed, so ``open(speakers=speakers(sid))`` resumes its names and claims.  Names change labels, never segments."""
+    claimed, so ``open(speakers=speakers(sid))`` resumes its names and claims.  Names change labels, never segments.
+
+    ``open(gallery=g)`` names that stream from its own gallery ``g`` at ``g.threshold`` for its whole life, whether or not
+    the server has a default gallery (``gallery=None``: the server's, if any).  Its names and claims are entries of ``g``,
+    so a stream is never named from another stream's gallery, and ``open(speakers=speakers(sid), gallery=g)`` resumes its
+    names and claims in ``g``.  Any number of galleries may be in use at once; each tick searches all of them in one grouped
+    launch, and a ``SpeakerGallery`` given to many streams is uploaded once.  The server holds each open stream's gallery."""
 
     _needs = "MultiStreamDiarization needs the native segmentation and embedding models"
 
@@ -356,17 +374,27 @@ class MultiStreamDiarization(_MultiStreamServer):
                 _lib.check(_lib.lib().dg_multi_set_gallery(self._h, gallery.handle, gallery.threshold))
         self._own_labels = np.zeros(self.max_streams, dtype=bool)      # the slot's labels are its own list, not the shared one
         self._stream_labels = [self.labels] * self.max_streams          # each slot's label list
+        # each open slot's gallery (cleared when the slot closes), and whether any stream may be named at all
+        self._slot_gallery: List[Optional[SpeakerGallery]] = [None] * self.max_streams
+        self._naming = gallery is not None
         self._names = np.empty((0, 3), dtype=np.int32)
 
     def open(self, shift: float = 0.0, sample_rate: Optional[int] = None, *, latency: Optional[float] = None,
              tau_active: Optional[float] = None, rho_update: Optional[float] = None,
-             delta_new: Optional[float] = None, speakers: Optional[KnownSpeakers] = None) -> int:
+             delta_new: Optional[float] = None, speakers: Optional[KnownSpeakers] = None,
+             gallery: Optional[SpeakerGallery] = None) -> int:
         """a new stream in the lowest free slot (``_MultiStreamServer._open_stream``): blocks at ``sample_rate``, time
-        stamps shifted by ``shift``, its own latency and thresholds (None: the config's), fixed until it is closed, and its
-        clustering state seeded with ``speakers`` (None or empty: fresh); returns its id.  ValueError, with the slot left
-        closed, for known speakers of another dimension or more than ``max_speakers`` of them."""
+        stamps shifted by ``shift``, its own latency and thresholds (None: the config's), fixed until it is closed, its
+        clustering state seeded with ``speakers`` (None or empty: fresh), and named from ``gallery`` (None: the server's);
+        returns its id.  ValueError, with the slot left closed and nothing launched, for known speakers of another
+        dimension or more than ``max_speakers`` of them, and for a gallery of another dimension or device (or a
+        configuration whose metric is not cosine)."""
         if speakers is not None and not isinstance(speakers, KnownSpeakers):
             raise TypeError(f"speakers: expected KnownSpeakers or None, got {type(speakers).__name__}")
+        if gallery is not None:
+            check_gallery(gallery, self.config, self.D)
+            if not same_device(gallery.device, self.device):
+                raise ValueError(f"the gallery is on {gallery.device}, the server on {self.device}")
         known = speakers if speakers is not None and len(speakers) else None
         if known is not None:
             if known.dimension != self.D:
@@ -377,10 +405,24 @@ class MultiStreamDiarization(_MultiStreamServer):
                                               tau_active=tau_active, rho_update=rho_update, delta_new=delta_new)
         self._own_labels[sid] = known is not None
         self._stream_labels[sid] = self.labels if known is None else speaker_labels(known, self._speakers)
-        if self.gallery is not None and known is not None:
-            named, claimed = self.gallery.claims(self._stream_labels[sid])
-            _lib.check(_lib.lib().dg_multi_set_names(self._h, sid, named, claimed.ctypes.data))
+        self._slot_gallery[sid] = gal = self.gallery if gallery is None else gallery
+        self._naming = self._naming or gal is not None
+        try:
+            with torch.cuda.device(self.device):
+                if gallery is not None:
+                    _lib.check(_lib.lib().dg_multi_set_slot_gallery(self._h, sid, gallery.handle, gallery.threshold))
+                if gal is not None and known is not None:
+                    named, claimed = gal.claims(self._stream_labels[sid])
+                    _lib.check(_lib.lib().dg_multi_set_names(self._h, sid, named, claimed.ctypes.data))
+        except BaseException:
+            self.close(sid)
+            raise
         return sid
+
+    def close(self, sid: int):
+        """ends stream ``sid``; the server lets go of its gallery"""
+        _MultiStreamServer.close(self, sid)
+        self._slot_gallery[sid] = None
 
     def speakers(self, sid: int) -> KnownSpeakers:
         """the clustering state of open stream ``sid`` after the last tick: its active centres in index order (a prefix
@@ -413,7 +455,7 @@ class MultiStreamDiarization(_MultiStreamServer):
 
     def _after_tick(self, B):
         """the names the tick decided {slot, g, entry} to the slots' labels"""
-        if self.gallery is None or B == 0:
+        if B == 0 or not self._naming:
             return
         n = C.c_int()
         cap = self.max_streams * self._speakers
@@ -424,7 +466,7 @@ class MultiStreamDiarization(_MultiStreamServer):
             if not self._own_labels[sid]:
                 self._stream_labels[sid] = list(self.labels)
                 self._own_labels[sid] = True
-            self._stream_labels[sid][g] = self.gallery.names[e]
+            self._stream_labels[sid][g] = self._slot_gallery[sid].names[e]
 
     def _annotations(self, header, turns, n_turns, out_start, out_res, shifts):
         sids = self._row_sids
@@ -455,9 +497,11 @@ class MultiStreamVoiceActivityDetection(_MultiStreamServer):
                          max_latency)
 
     def open(self, shift: float = 0.0, sample_rate: Optional[int] = None, *, latency: Optional[float] = None,
-             tau_active: Optional[float] = None) -> int:
+             tau_active: Optional[float] = None, gallery=None) -> int:
         """a new stream in the lowest free slot (``_MultiStreamServer._open_stream``) at its own latency and ``tau_active``
-        (None: the config's); returns its id"""
+        (None: the config's); returns its id.  ValueError for a ``gallery``: there are no speakers to name"""
+        if gallery is not None:
+            raise ValueError("voice activity detection has no speakers to name: a gallery needs MultiStreamDiarization")
         return _MultiStreamServer._open_stream(self, shift, sample_rate, latency, tau_active=tau_active)
 
     def _create(self, hamming):

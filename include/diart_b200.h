@@ -530,12 +530,20 @@ int dg_multi_get_state(dg_multi* h, int slot, double* centers_host /* [M][D] */,
  *        group, >= 0, each group one contiguous run of at most 32 queries; claimed_dev int32 [groups][32] (null: none): the
  *        entries group r has claimed, -1 padded.  Within a group, candidates for one entry are resolved by the smallest
  *        distance, ties to the earliest query.  group_dev is read back on `stream` (the call waits for it) to check it.
+ *        Queries of more than 2^31 - 1 elements are searched in several launches of whole groups (DG_EINVAL only when
+ *        one group alone exceeds that: a dimension above 67 million).
  *      dg_multi_set_gallery: every later tick names the active, unnamed global speakers of its streams from the gallery
  *        (dg_multi_last_names).  DG_EINVAL on a VAD handle, once a stream has opened, for a gallery of another dimension or
  *        device, or unless 0 < threshold <= 2.
- *      dg_multi_set_names: the names of the open stream in `slot` (a handle with a gallery): bit g of `named` set for a
- *        named global speaker g < max_speakers, claimed_host int32 [max_speakers] its gallery entry (-1: none; only named
- *        speakers claim, each entry once).  A stream opens with none named.
+ *      dg_multi_set_slot_gallery: the stream in `slot` is named from gallery g at `threshold` instead of the default
+ *        (dg_multi_set_gallery) for the rest of its life, starting with nothing named or claimed.  Any number of streams
+ *        may have their own galleries, the same or different ones; a tick searches all of them in one grouped launch.  The
+ *        handle refers to g until the slot is closed: g must outlive that.  DG_EINVAL for a null handle or gallery, a VAD
+ *        handle, a slot that is not open or has had a tick, a gallery of another dimension or device, or unless
+ *        0 < threshold <= 2.
+ *      dg_multi_set_names: the names of the open stream in `slot` (a slot with a gallery, its own or the default): bit g of
+ *        `named` set for a named global speaker g < max_speakers, claimed_host int32 [max_speakers] its entry in the slot's
+ *        gallery (-1: none; only named speakers claim, each entry once).  A stream opens with none named.
  *      dg_multi_last_names: the names decided by the last dg_multi_step, out_host int32 [cap][3] = {slot, g, entry}, *n of
  *        them; DG_EINVAL if more than cap. ---- */
 typedef struct dg_gallery dg_gallery;
@@ -545,6 +553,7 @@ int dg_gallery_query(dg_gallery* g, const double* queries_dev /* [Q][D] */, int 
                      const int32_t* claimed_dev /* [groups][32] */, double threshold, int32_t* entry_dev /* [Q] */,
                      double* dist_dev /* [Q] */, void* stream);
 int dg_multi_set_gallery(dg_multi* h, dg_gallery* g, double threshold);
+int dg_multi_set_slot_gallery(dg_multi* h, int slot, dg_gallery* g, double threshold);
 int dg_multi_set_names(dg_multi* h, int slot, uint32_t named, const int32_t* claimed_host /* [max_speakers] */);
 int dg_multi_last_names(const dg_multi* h, int32_t* out_host /* [cap][3] */, int cap, int* n);
 /* test hook: the last tick's window batch [n_rows, chunk_samples] (what its networks read; n_rows = that tick's window count)
@@ -565,6 +574,23 @@ int dg_selftest_multi_frames_host(int slots, int max_wps, int out_chunk, int out
  * refused one (a push beyond the ring capacity, a closed or unknown slot).  rings_host float [slots][C]: written by ticks. */
 int dg_selftest_multi_staging_host(int slots, int C, int n_ops, const int32_t* ops, const float* samples_host, int32_t* result,
                                    float* rings_host);
+/* test hook (host only, no GPU): the plan of a tick's grouped gallery search.  slots int32 [n][3] = {slot, gallery key (-1:
+ * none), unnamed speakers} of the tick's slots in slot order; G int32 [n_keys] and thr [n_keys] the galleries' sizes and
+ * thresholds.  Outputs: groups int32 [n][6] = {key, G, tiles, per_split, splits, query upper bound} in order of each key's
+ * first slot, segs int32 [n][2] = {slot, group} group by group, work int32 [cap][3] = {group, query tile, split} (the CTAs of
+ * gallery_nearest, split-major), counts int32 [4] = {groups, segments, work items, largest split count}.  DG_EINVAL if
+ * more than cap work items. */
+int dg_selftest_gallery_plan_host(int n, const int32_t* slots, int n_keys, const int32_t* G, const double* thr,
+                                  int32_t* groups_out, int32_t* segs_out, int32_t* work_out, int cap, int32_t* counts);
+/* test hook (host only, no GPU): dg_multi_set_slot_gallery and dg_multi_set_names on a diarization handle of `slots` slots,
+ * embeddings of dimension D and M speakers on device 0 that owns no device memory.  gal int32 [n_gal][3] = {G, D, device}
+ * describe galleries (no entries).  ops double [n_ops][4] = {kind, slot, arg, x}: 0 open the slot (no default gallery),
+ * 1 dg_multi_set_slot_gallery(slot, gallery arg or null for -1, threshold x), 2 give the slot gallery arg (host state only),
+ * 3 dg_multi_set_names(slot, named = arg, speaker 0 claiming entry x), 4 the slot has had a tick, 5 close the slot.
+ * result int32 [n_ops]: each op's return code; messages: each op's error message ("" when none), one per line.  Meant
+ * for refusals: an accepted call 1 or 3 goes on to the device. */
+int dg_selftest_multi_gallery_host(int slots, int D, int M, int n_gal, const int32_t* gal, int n_ops, const double* ops,
+                                   int32_t* result, char* messages, int msg_cap);
 /* ---- many live streams of the reference's VoiceActivityDetection (src/diart/blocks/vad.py:139-191: the segmentation
  *      network, the max over the local speakers, DelayedAggregation(hamming) and Binarize(tau_active), turns labelled
  *      "speech"), served as dg_multi serves SpeakerDiarization.
