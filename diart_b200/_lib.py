@@ -154,6 +154,11 @@ SIGNATURES = {
     "dg_multi_last_names": (C.c_int, [_P, _P, C.c_int, C.POINTER(C.c_int)]),
     "dg_selftest_multi_frames_host": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _P, C.c_int, _P, _P, _P, C.c_int,
                                                 C.POINTER(C.c_int)]),
+    "dg_multi_export_bytes": (C.c_int, [_P, _P, C.c_int, _P]),
+    "dg_multi_export": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, C.c_int64]),
+    "dg_multi_import": (C.c_int, [_P, _P, C.c_int64, C.c_int, _P, _P]),
+    "dg_selftest_multi_transfer_host": (C.c_int, [_P, C.c_int, _P, _P, _P, C.c_int, C.c_int, _P, _P, _P, C.c_int64, _P,
+                                                  C.c_char_p, C.c_int]),
 }
 
 

@@ -15,7 +15,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libdiartb200.so")
 SOURCES = ["api.cu", "api_seg.cu", "api_emb.cu", "api_cluster.cu", "api_stream.cu", "api_post.cu", "api_pipeline.cu", "api_multi.cu",
            "sincnet.cu", "gemm.cu", "gemm_tc.cu", "sinc_tc.cu", "lstm_tc.cu", "heads.cu", "cluster.cu", "post.cu", "resnet.cu", "resample.cu", "der.cu",
-           "vad.cu", "api_gallery.cu", "gallery.cu"]
+           "vad.cu", "api_gallery.cu", "gallery.cu", "transfer.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 

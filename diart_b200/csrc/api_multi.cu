@@ -230,6 +230,11 @@ struct dg_multi {
   DevBuf gal_named, gal_claimed, gal_q, gal_seg, gal_gq, gal_d, gal_e, gal_list;
   std::vector<uint32_t> named_host;
   std::vector<int32_t> names_last;            // the names the last dg_multi_step decided, [n][3]
+  // dg_multi_export / dg_multi_import: one round's packed states and its piece list, on the device and pinned.  Allocated
+  // by the first move that needs them (a growth synchronises the device, as every DevBuf growth does) and kept for the
+  // handle's life: at most XFER_STAGING bytes of states plus the pieces, each.
+  DevBuf xfer;
+  PinnedBuf xfer_pin;
 };
 
 // In front of the header in h->header and in the tick's pinned download, once the handle has received a gallery: the count
@@ -1086,6 +1091,437 @@ extern "C" int dg_multi_last_windows(const dg_multi* h, float* wav_dev, int n_ro
   return DG_OK;
 }
 
+// ================================================================================ moving streams (export / import)
+// A stream's state after its last tick, packed (include/diart_b200.h documents the layout): the fixed XferHead, then the
+// audio [rpos, wpos), the computed 16 kHz frames a future window still reads, the n_hist history entries oldest first, and
+// for a diarization stream its centroids, active flags and claimed gallery entries.  Every section starts at a multiple of
+// 16 bytes; a state's size is a multiple of 16, so packed states follow each other directly.
+static const uint32_t XFER_MAGIC = 0x54534744u;          // "DGST"
+static const int XFER_VERSION = 1;
+static const size_t XFER_STAGING = (size_t)256 << 20;    // packed states per round of one launch and one copy
+
+struct XferHead {
+  uint32_t magic, version;
+  int32_t kind;                    // 0 diarization, 1 VAD
+  int32_t S, hop, F, K, D, M;      // the pipeline's window and step, the networks' frames, local speakers, embedding, speakers
+  int32_t rs_o, rs_n, rs_w;        // the source rate's resampling (reduced ratio o / n, half-width w; all 0: the pipeline's)
+  int32_t chunk, step;             // window and step at the source rate
+  int32_t nw, n_hist;              // buffers aggregated (latency / step), history entries held
+  int32_t init[2];                 // clustering: initialised, "cannot update unknown centers"
+  uint32_t named;                  // named global speakers (bit g)
+  int32_t gallery_G;               // entries of the gallery the stream is named from (0: none)
+  int32_t ticked, pad0;
+  int64_t wpos, rpos, done;        // absolute source samples pushed / start of the next window, 16 kHz frames computed
+  int64_t frame0, n_frames;        // the frames carried: [frame0, frame0 + n_frames)
+  double params[3];                // tau, rho, delta
+  double threshold;                // gallery threshold
+  float gamma, beta;
+  int32_t normalize, pad1;
+  int64_t bytes;                   // the packed state, head included
+};
+
+// byte offsets of a state's sections
+struct XferLayout {
+  size_t audio, frames, hist, hmap, centers, active, claimed, bytes;
+};
+
+static XferLayout xfer_layout(const XferHead& hd) {
+  XferLayout L{};
+  const bool vad = hd.kind == 1;
+  L.audio = align16(sizeof(XferHead));
+  L.frames = L.audio + align16((size_t)(hd.wpos - hd.rpos) * 4);
+  L.hist = L.frames + align16((size_t)hd.n_frames * hd.rs_n * 4);
+  L.hmap = L.hist + align16((size_t)hd.n_hist * hd.F * (vad ? 1 : hd.K) * 4);
+  L.centers = L.hmap + (vad ? 0 : align16((size_t)hd.n_hist * hd.K * 4));
+  L.active = L.centers + (vad ? 0 : align16((size_t)hd.M * hd.D * 8));
+  L.claimed = L.active + (vad ? 0 : 32 * 4);
+  L.bytes = L.claimed + (vad ? 0 : 32 * 4);
+  return L;
+}
+
+// the device arrays a move reads or writes, as 32-bit words (a test hook points them at host memory)
+struct XferDev {
+  uint32_t *rings = nullptr, *yrings = nullptr, *hist_seg = nullptr, *hist_map = nullptr, *hist_vad = nullptr;
+  uint32_t *centers = nullptr, *active = nullptr, *init = nullptr, *named = nullptr, *claimed = nullptr;
+  long long C = 0, Y = 0;
+};
+
+static XferDev xfer_dev(const dg_multi* h) {
+  XferDev d;
+  d.rings = h->rings.as<uint32_t>(); d.yrings = h->yrings.as<uint32_t>();
+  d.hist_seg = h->hist_seg.as<uint32_t>(); d.hist_map = h->hist_map.as<uint32_t>(); d.hist_vad = h->hist_vad.as<uint32_t>();
+  d.centers = h->centers.as<uint32_t>(); d.active = h->active.as<uint32_t>(); d.init = h->init.as<uint32_t>();
+  if (!h->named_host.empty()) {
+    d.named = h->gal_named.as<uint32_t>();
+    d.claimed = h->gal_claimed.as<uint32_t>();
+  }
+  d.C = h->book.C;
+  d.Y = h->Y;
+  return d;
+}
+
+// the head of open slot s (init words: the device's, filled in by the gather)
+static XferHead xfer_head(const dg_multi* h, int s) {
+  XferHead hd{};
+  const RateGeom& r = h->book.geom(s);
+  hd.magic = XFER_MAGIC;
+  hd.version = XFER_VERSION;
+  hd.kind = vad_mode(h) ? 1 : 0;
+  hd.S = h->S; hd.hop = h->hop; hd.F = h->F; hd.K = h->K; hd.D = h->D; hd.M = h->M;
+  if (r.resampled()) {
+    hd.rs_o = r.g.o; hd.rs_n = r.g.n; hd.rs_w = r.g.w;
+  }
+  hd.chunk = r.S; hd.step = r.hop;
+  hd.nw = h->slot_nw[s];
+  hd.n_hist = h->n_hist[s];
+  hd.named = h->named_host.empty() ? 0 : h->named_host[s];
+  hd.gallery_G = h->slot_gal[s] ? h->slot_gal[s]->G : 0;
+  hd.ticked = h->slot_ticked[s];
+  hd.wpos = h->book.wpos[s]; hd.rpos = h->book.rpos[s]; hd.done = h->book.done[s];
+  if (r.resampled()) {   // frames computed that a future window still reads
+    hd.frame0 = hd.rpos / r.g.o + r.r_lo;
+    hd.n_frames = std::max<int64_t>(0, hd.done - hd.frame0);
+  }
+  memcpy(hd.params, &h->slot_par[3 * (size_t)s], 24);
+  hd.threshold = h->slot_gal[s] ? h->slot_thr[s] : 0.0;
+  hd.gamma = h->net.gamma; hd.beta = h->net.beta; hd.normalize = h->net.normalize_weights;
+  hd.bytes = (int64_t)xfer_layout(hd).bytes;
+  return hd;
+}
+
+// The pieces between slot s (history copy `cur`, history stride nw - 1) and its packed state at `blob`: the first n_ring
+// samples of the audio, the frames, the history and (diarization) the clustering and naming tables.  to_blob: export
+// (the slot is the source), else import.  An export gathers no named bits (the host mirror has them).
+static void xfer_pieces(const XferDev& d, const RateGeom& r, int slots, int nw, int s, int cur, const XferHead& hd,
+                        uint32_t* blob, long long n_ring, bool to_blob, std::vector<XferPiece>& out) {
+  const XferLayout L = xfer_layout(hd);
+  auto add = [&](uint32_t* dev, long long pos, long long mod, size_t off, long long n) {
+    if (n <= 0) return;
+    uint32_t* b = blob + off / 4;
+    out.push_back(to_blob ? XferPiece{dev, b, n, pos, mod, 0, 0} : XferPiece{b, dev, n, 0, 0, pos, mod});
+  };
+  add(d.rings + (size_t)s * d.C, hd.rpos, d.C, L.audio, n_ring);
+  if (hd.n_frames) add(d.yrings + (size_t)s * d.Y, hd.frame0 * r.g.n, r.Q * r.g.n, L.frames, hd.n_frames * r.g.n);
+  const size_t h0 = ((size_t)cur * slots + s) * (nw - 1), FK = (size_t)hd.F * hd.K;
+  if (hd.kind == 1) {
+    add(d.hist_vad + h0 * hd.F, 0, 0, L.hist, (long long)hd.n_hist * hd.F);
+    return;
+  }
+  add(d.hist_seg + h0 * FK, 0, 0, L.hist, (long long)(hd.n_hist * FK));
+  add(d.hist_map + h0 * hd.K, 0, 0, L.hmap, (long long)hd.n_hist * hd.K);
+  add(d.centers + (size_t)s * hd.M * hd.D * 2, 0, 0, L.centers, 2LL * hd.M * hd.D);
+  add(d.active + (size_t)s * 32, 0, 0, L.active, 32);
+  add(d.init + (size_t)s * 2, 0, 0, offsetof(XferHead, init), 2);
+  if (d.claimed) {
+    add(d.claimed + (size_t)s * 32, 0, 0, L.claimed, 32);
+    if (!to_blob) add(d.named + s, 0, 0, offsetof(XferHead, named), 1);
+  }
+}
+
+// The staged pieces of each slot (samples pushed since the last tick, still in the pinned staging), in one pass over them
+struct StagedBySlot {
+  std::vector<int> off, idx;   // slot s: pieces idx [off[s], off[s + 1]) of book.pieces, in push (= stream) order
+  std::vector<long long> n;    // slot s: its staged samples
+  explicit StagedBySlot(const SlotBook& b) : off(b.open.size() + 1, 0), idx(b.pieces.size()), n(b.open.size(), 0) {
+    for (const RingPiece& p : b.pieces) {
+      off[p.slot + 1]++;
+      n[p.slot] += p.n;
+    }
+    for (size_t s = 0; s + 1 < off.size(); s++) off[s + 1] += off[s];
+    std::vector<int> fill(off.begin(), off.end() - 1);
+    for (size_t q = 0; q < b.pieces.size(); q++) idx[fill[b.pieces[q].slot]++] = (int)q;
+  }
+};
+
+// After the gather of slot s into `out`: its head (keeping the gathered init words), its staged samples, without naming
+// tables no claims, and zeros in the gaps that align the sections, so that a state's bytes depend on the stream alone.
+static void xfer_finish(const dg_multi* h, int s, const XferHead& head, const float* stage, const StagedBySlot& sb,
+                        unsigned char* out) {
+  XferHead hd = head;
+  const XferLayout L = xfer_layout(hd);
+  if (hd.kind == 0) memcpy(hd.init, out + offsetof(XferHead, init), 8);
+  memcpy(out, &hd, sizeof(hd));
+  for (int q = sb.off[s]; q < sb.off[s + 1]; q++) {
+    const RingPiece& p = h->book.pieces[sb.idx[q]];
+    memcpy(out + L.audio + (size_t)(p.dst - hd.rpos) * 4, stage + p.src, (size_t)p.n * 4);
+  }
+  if (hd.kind == 0 && h->named_host.empty()) memset(out + L.claimed, 0xff, 32 * 4);
+  const size_t vad = hd.kind == 1, FK = (size_t)hd.F * (vad ? 1 : hd.K);
+  const size_t used[][2] = {{sizeof(XferHead), L.audio},
+                            {L.audio + (size_t)(hd.wpos - hd.rpos) * 4, L.frames},
+                            {L.frames + (size_t)hd.n_frames * hd.rs_n * 4, L.hist},
+                            {L.hist + (size_t)hd.n_hist * FK * 4, L.hmap},
+                            {L.hmap + (vad ? 0 : (size_t)hd.n_hist * hd.K * 4), L.centers},
+                            {L.centers + (vad ? 0 : (size_t)hd.M * hd.D * 8), L.active}};
+  for (const auto& g : used) memset(out + g[0], 0, g[1] - g[0]);
+}
+
+static int xfer_slots_ok(const dg_multi* h, const int32_t* slots, int n, const char* who) {
+  if (!h || n < 0 || (n > 0 && !slots)) {
+    set_error(std::string(who) + ": bad arguments (a handle, n >= 0 slots)");
+    return DG_EINVAL;
+  }
+  std::vector<char> seen(h->slots, 0);
+  for (int a = 0; a < n; a++) {
+    const int s = slots[a];
+    if (!slot_ok(h, s) || seen[s]) {
+      set_error(std::string(who) + ": slot " + std::to_string(s) + " is not open or is listed twice");
+      return DG_EINVAL;
+    }
+    seen[s] = 1;
+  }
+  return DG_OK;
+}
+
+// Checks packed state a (head hd, its bytes at `blob`, at most `avail` of them) against h before anything is written:
+// DG_EINVAL naming who, the state and the reason.  On success rid is its declared rate (-1: the pipeline's) and g the gallery
+// it is named from (null: none).
+static int xfer_check(const dg_multi* h, const XferHead& hd, const unsigned char* blob, size_t avail, int a,
+                      dg_gallery* const* gals, int& rid, dg_gallery*& g, const char* who) {
+  const std::string at = std::string(who) + ": state " + std::to_string(a);
+  auto fail = [&](const std::string& why) {
+    set_error(at + " " + why);
+    return DG_EINVAL;
+  };
+  if (hd.magic != XFER_MAGIC) return fail("is not a packed stream state");
+  if (hd.version != (uint32_t)XFER_VERSION)
+    return fail("has format version " + std::to_string(hd.version) + ", this build reads version " +
+                std::to_string(XFER_VERSION));
+  const int kind = vad_mode(h) ? 1 : 0;
+  if (hd.kind != kind)
+    return fail(kind ? "is a diarization stream, the handle serves voice activity detection"
+                     : "is a voice activity detection stream, the handle serves diarization");
+  if (hd.S != h->S || hd.hop != h->hop || hd.F != h->F || hd.K != h->K || hd.D != h->D || hd.M != h->M)
+    return fail("has windows of " + std::to_string(hd.S) + " / " + std::to_string(hd.hop) + " samples, F = " +
+                std::to_string(hd.F) + ", K = " + std::to_string(hd.K) + ", D = " + std::to_string(hd.D) + ", M = " +
+                std::to_string(hd.M) + "; the handle " + std::to_string(h->S) + " / " + std::to_string(h->hop) + ", " +
+                std::to_string(h->F) + ", " + std::to_string(h->K) + ", " + std::to_string(h->D) + ", " + std::to_string(h->M));
+  if (!kind && (hd.gamma != h->net.gamma || hd.beta != h->net.beta || hd.normalize != h->net.normalize_weights))
+    return fail("was diarized with other gamma, beta or normalize_embedding_weights");
+  const long long wlen = hd.wpos - hd.rpos;
+  const XferLayout L = xfer_layout(hd);
+  if (hd.rpos < 0 || wlen < 0 || hd.n_hist < 0 || hd.n_frames < 0 || hd.rs_n < 0) return fail("is malformed");
+  rid = -2;
+  for (size_t i = 0; i < h->book.rates.size(); i++) {
+    const RateGeom& r = h->book.rates[i];
+    const bool same = r.resampled() ? (hd.rs_o == r.g.o && hd.rs_n == r.g.n && hd.rs_w == r.g.w)
+                                    : (hd.rs_o == 0 && hd.rs_n == 0 && hd.rs_w == 0);
+    if (same && hd.chunk == r.S && hd.step == r.hop) rid = (int)i - 1;
+  }
+  if (rid == -2)
+    return fail("is at a source rate the handle did not declare (resampling " + std::to_string(hd.rs_o) + " / " +
+                std::to_string(hd.rs_n) + ", window " + std::to_string(hd.chunk) + " samples)");
+  const RateGeom& r = h->book.rates[rid + 1];
+  if (hd.nw < 1 || hd.nw > h->nw)
+    return fail("aggregates " + std::to_string(hd.nw) + " buffers, the handle at most " + std::to_string(h->nw) +
+                " (its max_latency)");
+  if (hd.n_hist > hd.nw - 1 || hd.rpos % r.hop) return fail("is malformed (history or window position)");
+  if (wlen > r.cap)
+    return fail("holds " + std::to_string(wlen) + " samples of audio, more than the ring's capacity of " +
+                std::to_string(r.cap));
+  if (hd.bytes != (int64_t)L.bytes || (size_t)hd.bytes > avail) return fail("is malformed or cut short");
+  if (r.resampled() ? (hd.n_frames > r.Q || (hd.n_frames && (hd.frame0 != hd.rpos / r.g.o + r.r_lo ||
+                                                              hd.done != hd.frame0 + hd.n_frames)) || hd.done < 0)
+                    : (hd.n_frames || hd.done))
+    return fail("is malformed (16 kHz frames)");
+  if (hd.init[1]) return fail("holds a clustering state that failed on its source (unknown centers)");
+  if (!std::isfinite(hd.params[0]) || !std::isfinite(hd.params[1]) || !std::isfinite(hd.params[2]))
+    return fail("has thresholds that are not finite");
+  g = nullptr;
+  const int32_t* claimed = reinterpret_cast<const int32_t*>(blob + L.claimed);
+  if (hd.gallery_G > 0) {
+    if (kind) return fail("is a voice activity detection stream with a gallery");
+    g = gals && gals[a] ? gals[a] : h->gal;
+    if (!g) return fail("was named from a gallery of " + std::to_string(hd.gallery_G) + " entries: give that gallery");
+    if (g->G != hd.gallery_G)
+      return fail("was named from a gallery of " + std::to_string(hd.gallery_G) + " entries, the one given has " +
+                  std::to_string(g->G));
+    if (check_gallery_for(h, g, hd.threshold, at.c_str())) return DG_EINVAL;
+    if (h->M < 32 && (hd.named >> h->M)) return fail("names speakers beyond max_speakers");
+    for (int k = 0; k < h->M; k++) {
+      const int e = claimed[k];
+      if (!(e == -1 || (e >= 0 && e < g->G && ((hd.named >> k) & 1) && std::find(claimed, claimed + k, e) == claimed + k)))
+        return fail("has a claim of entry " + std::to_string(e) + " by speaker " + std::to_string(k) + " that is not valid");
+    }
+  } else if (hd.gallery_G < 0 || hd.named || (!kind && std::any_of(claimed, claimed + 32, [](int32_t e) { return e != -1; }))) {
+    return fail("names speakers without a gallery");
+  }
+  return DG_OK;
+}
+
+// the stream of state hd (checked) opens in free slot t: host bookkeeping only
+static void xfer_open(dg_multi* h, int t, int rid, const XferHead& hd, dg_gallery* g) {
+  h->book.start(t, rid + 1);
+  h->book.wpos[t] = hd.wpos;
+  h->book.rpos[t] = hd.rpos;
+  h->book.done[t] = hd.done;
+  h->cur[t] = 0;
+  h->n_hist[t] = hd.n_hist;
+  h->slot_nw[t] = hd.nw;
+  memcpy(&h->slot_par[3 * (size_t)t], hd.params, 24);
+  h->slot_gal[t] = g;
+  h->slot_thr[t] = g ? hd.threshold : 0.0;
+  h->slot_ticked[t] = hd.ticked;
+  if (!h->named_host.empty()) h->named_host[t] = hd.named;
+  h->opened = true;
+}
+
+// consecutive states [a0, a1) of one round: as many as fit XFER_STAGING, at least one
+static int xfer_round(const std::vector<size_t>& bytes, int a0) {
+  int a1 = a0;
+  size_t sum = 0;
+  while (a1 < (int)bytes.size() && (a1 == a0 || sum + bytes[a1] <= XFER_STAGING)) sum += bytes[a1++];
+  return a1;
+}
+
+// the device staging and pinned buffer of a round: `bytes` of states, then up to n_pieces descriptors
+static int xfer_buffers(dg_multi* h, size_t bytes, size_t n_pieces, size_t& o_desc) {
+  o_desc = align16(bytes);
+  const size_t need = o_desc + n_pieces * sizeof(XferPiece);
+  if (h->xfer.ensure(need) || h->xfer_pin.ensure(need)) return DG_ECUDA;
+  return DG_OK;
+}
+
+extern "C" int dg_multi_export_bytes(const dg_multi* h, const int32_t* slots, int n, int64_t* bytes_out) {
+  int rc;
+  if ((rc = xfer_slots_ok(h, slots, n, "dg_multi_export_bytes"))) return rc;
+  if (n > 0 && !bytes_out) {
+    set_error("dg_multi_export_bytes: null output");
+    return DG_EINVAL;
+  }
+  for (int a = 0; a < n; a++) bytes_out[a] = xfer_head(h, slots[a]).bytes;
+  return DG_OK;
+}
+
+extern "C" int dg_multi_export(dg_multi* h, const int32_t* slots, int n, int close, void* out_host, int64_t out_bytes) {
+  const char* who = "dg_multi_export";
+  int rc;
+  if ((rc = xfer_slots_ok(h, slots, n, who))) return rc;
+  std::vector<XferHead> hd(n);
+  std::vector<size_t> bytes(n), off(n + 1, 0);
+  for (int a = 0; a < n; a++) {
+    hd[a] = xfer_head(h, slots[a]);
+    bytes[a] = (size_t)hd[a].bytes;
+    off[a + 1] = off[a] + bytes[a];
+  }
+  if (n > 0 && (!out_host || out_bytes < 0 || (size_t)out_bytes < off[n])) {
+    set_error(std::string(who) + ": the states take " + std::to_string(off[n]) + " bytes, room for " +
+              std::to_string(out_bytes));
+    return DG_EINVAL;
+  }
+  if (n == 0) return DG_OK;
+  DG_CUDA(cudaSetDevice(h->device));
+  unsigned char* out = static_cast<unsigned char*>(out_host);
+  const StagedBySlot sb(h->book);
+  for (int a0 = 0, a1; a0 < n; a0 = a1) {
+    a1 = xfer_round(bytes, a0);
+    const size_t round = off[a1] - off[a0];
+    size_t o_desc;
+    if ((rc = xfer_buffers(h, round, (size_t)(a1 - a0) * 9, o_desc))) return rc;
+    const XferDev d = xfer_dev(h);
+    std::vector<XferPiece> pc;
+    for (int a = a0; a < a1; a++) {
+      const int s = slots[a];
+      xfer_pieces(d, h->book.geom(s), h->slots, h->nw, s, h->cur[s], hd[a], h->xfer.as<uint32_t>() + (off[a] - off[a0]) / 4,
+                  hd[a].wpos - hd[a].rpos - sb.n[s], true, pc);
+    }
+    unsigned char* pin = h->xfer_pin.as<unsigned char>();
+    memcpy(pin + o_desc, pc.data(), pc.size() * sizeof(XferPiece));
+    const XferPiece* d_pc = reinterpret_cast<const XferPiece*>(h->xfer.as<unsigned char>() + o_desc);
+    DG_CUDA(cudaMemcpyAsync(const_cast<XferPiece*>(d_pc), pin + o_desc, pc.size() * sizeof(XferPiece), cudaMemcpyHostToDevice,
+                            h->st));
+    if ((rc = launch_slot_transfer(d_pc, (int)pc.size(), "slot_transfer_export", h->st))) return rc;
+    {
+      ProfScope _ps("slot_transfer_d2h", h->st);   // the copy, timed when profiling
+      DG_CUDA(cudaMemcpyAsync(pin, h->xfer.p, round, cudaMemcpyDeviceToHost, h->st));
+    }
+    DG_CUDA(cudaStreamSynchronize(h->st));
+    memcpy(out + off[a0], pin, round);
+    for (int a = a0; a < a1; a++) xfer_finish(h, slots[a], hd[a], h->stage.as<float>(), sb, out + off[a]);
+  }
+  for (int a = 0; a < n; a++) {
+    int init[2];
+    memcpy(init, out + off[a] + offsetof(XferHead, init), 8);
+    if (init[1]) {   // as dg_multi_get_state reports it; no slot is closed
+      set_error(std::string(who) + ": the stream in slot " + std::to_string(slots[a]) + ": Cannot update unknown centers");
+      return DG_EINVAL;
+    }
+  }
+  if (close)
+    for (int a = 0; a < n; a++) {
+      h->book.stop(slots[a]);
+      h->slot_gal[slots[a]] = nullptr;
+    }
+  return DG_OK;
+}
+
+extern "C" int dg_multi_import(dg_multi* h, const void* blob_host, int64_t blob_bytes, int n, dg_gallery* const* gals,
+                               int32_t* slots_out) {
+  const char* who = "dg_multi_import";
+  if (!h || n < 0 || blob_bytes < 0 || (n > 0 && (!blob_host || !slots_out))) {
+    set_error(std::string(who) + ": bad arguments (a handle, n >= 0 packed states and room for their slots)");
+    return DG_EINVAL;
+  }
+  const unsigned char* blob = static_cast<const unsigned char*>(blob_host);
+  std::vector<XferHead> hd(n);
+  std::vector<size_t> bytes(n), off(n + 1, 0);
+  std::vector<int> rid(n), slot(n);
+  std::vector<dg_gallery*> gal(n);
+  int rc;
+  for (int a = 0; a < n; a++) {
+    const size_t avail = (size_t)blob_bytes - off[a];
+    if (avail < sizeof(XferHead)) {
+      set_error(std::string(who) + ": state " + std::to_string(a) + " is cut short");
+      return DG_EINVAL;
+    }
+    memcpy(&hd[a], blob + off[a], sizeof(XferHead));
+    if ((rc = xfer_check(h, hd[a], blob + off[a], avail, a, gals, rid[a], gal[a], who))) return rc;
+    bytes[a] = (size_t)hd[a].bytes;
+    off[a + 1] = off[a] + bytes[a];
+  }
+  for (int a = 0, s = 0; a < n; a++, s++) {   // the lowest free slots
+    while (s < h->slots && h->book.open[s]) s++;
+    if (s == h->slots) {
+      set_error(std::string(who) + ": " + std::to_string(n) + " states, fewer free slots");
+      return DG_EINVAL;
+    }
+    slot[a] = s;
+  }
+  if (n == 0) return DG_OK;
+  DG_CUDA(cudaSetDevice(h->device));
+  if (std::any_of(gal.begin(), gal.end(), [](dg_gallery* g) { return g != nullptr; }) && (rc = gallery_tables(h))) return rc;
+  for (int a0 = 0, a1; a0 < n; a0 = a1) {
+    a1 = xfer_round(bytes, a0);
+    const size_t round = off[a1] - off[a0];
+    size_t o_desc;
+    if ((rc = xfer_buffers(h, round, (size_t)(a1 - a0) * 9, o_desc))) return rc;
+    const XferDev d = xfer_dev(h);
+    std::vector<XferPiece> pc;
+    for (int a = a0; a < a1; a++) {
+      const int t = slot[a];
+      xfer_pieces(d, h->book.rates[rid[a] + 1], h->slots, h->nw, t, 0, hd[a], h->xfer.as<uint32_t>() + (off[a] - off[a0]) / 4,
+                  hd[a].wpos - hd[a].rpos, false, pc);
+    }
+    unsigned char* pin = h->xfer_pin.as<unsigned char>();
+    memcpy(pin, blob + off[a0], round);
+    memcpy(pin + o_desc, pc.data(), pc.size() * sizeof(XferPiece));
+    const XferPiece* d_pc = reinterpret_cast<const XferPiece*>(h->xfer.as<unsigned char>() + o_desc);
+    {
+      ProfScope _ps("slot_transfer_h2d", h->st);   // the copy, timed when profiling
+      DG_CUDA(cudaMemcpyAsync(h->xfer.p, pin, o_desc + pc.size() * sizeof(XferPiece), cudaMemcpyHostToDevice, h->st));
+    }
+    if ((rc = launch_slot_transfer(d_pc, (int)pc.size(), "slot_transfer_import", h->st))) return rc;
+    DG_CUDA(cudaStreamSynchronize(h->st));   // the pinned buffer is reused by the next round
+  }
+  // the slots open once every round has landed: an error above leaves them closed (what was written is reset by the next
+  // open of those slots, and never read before)
+  for (int a = 0; a < n; a++) {
+    xfer_open(h, slot[a], rid[a], hd[a], gal[a]);
+    slots_out[a] = slot[a];
+  }
+  return DG_OK;
+}
+
 // dg_multi's tick planning on its own (test hook, no GPU): a SlotBook whose pipeline windows are out_chunk / out_step samples,
 // with the declared rates [n_rates][5] = {o, n, w, chunk, step}, driven by ops [n_ops][3] = {kind, slot, n}.
 extern "C" int dg_selftest_multi_frames_host(int slots, int max_wps, int out_chunk, int out_step, int n_rates, const int32_t* rates,
@@ -1316,5 +1752,182 @@ extern "C" int dg_selftest_multi_gallery_host(int slots, int D, int M, int n_gal
   const size_t n = std::min(text.size(), (size_t)msg_cap - 1);
   memcpy(messages, text.data(), n);
   messages[n] = 0;
+  return DG_OK;
+}
+
+// dg_multi_export / dg_multi_import between two VAD handles without a device (test hook): the pieces run on the host over
+// host arrays.  geom [14] = {slots, max_wps, nw, out_chunk, out_step, F, o, n, w, chunk, step, target slots, target max_wps,
+// target nw}: a source handle at the pipeline's windows out_chunk / out_step and (o > 0) one declared rate {o, n, w, chunk,
+// step}, and a target with its own slots, max_wps and nw.  ops [n_ops][3] = {kind, slot, n} drive the source: 0 open slot at
+// rate id n (-1: the pipeline's rate), 1 close, 2 push the next n samples of samples_host, 4 tick.  A tick writes the staged
+// samples to the rings, 16 kHz frame R as the values R n + p (p < n), and moves the histories on as post_slots_history
+// does, chunk c of a stream being the F values c F + j.  Then slot src_slot is exported, its head patched (patch: 0 none,
+// 1 version, 2 kind, 3 window, 4 nw beyond the target's, 5 backlog beyond the target's ring, 6 unknown centers, 7 undeclared
+// rate, 8 magic) and imported into the target's slot 0.  info [16] = {import rc, C, Q, Y, wpos, rpos, done, n_hist, frame0,
+// n_frames, state bytes, source C, source Q}; the target's ring [C], frame ring [Y] and history copy 0 [(nw - 1) F] go to
+// the outputs of `cap` floats each; message: the import's error ("" when none).
+extern "C" int dg_selftest_multi_transfer_host(const int32_t* geom, int n_ops, const int32_t* ops, const float* samples_host,
+                                               int32_t* result, int src_slot, int patch, float* ring_out, float* yring_out,
+                                               float* hist_out, int64_t cap, int64_t* info, char* message, int msg_cap) {
+  const char* who = "dg_selftest_multi_transfer_host";
+  if (!geom || n_ops < 0 || (n_ops && (!ops || !result || !samples_host)) || !ring_out || !yring_out || !hist_out ||
+      cap < 1 || !info || !message || msg_cap < 1) {
+    set_error(std::string(who) + ": bad arguments");
+    return DG_EINVAL;
+  }
+  const int F = geom[5];
+  // a host-only VAD handle: the bookkeeping of dg_multi_create_vad, host vectors for the device arrays
+  struct Side {
+    dg_multi h;
+    std::vector<float> rings, yrings, hist;
+    XferDev d;
+  };
+  auto make = [&](Side& x, int slots, int max_wps, int nw) -> int {
+    dg_multi& h = x.h;
+    h.slots = slots; h.max_wps = max_wps; h.S = geom[3]; h.hop = geom[4]; h.F = F; h.K = 1; h.M = 1; h.nw = nw;
+    RateGeom base;
+    base.S = geom[3];
+    base.hop = geom[4];
+    base.cap = (int)ring_capacity(geom[3], geom[4], max_wps);
+    h.book.init(slots, base);
+    if (geom[6] > 0) {
+      RsGeom g{geom[6], geom[7], geom[8], 2 * geom[8] + geom[6]};
+      RateGeom r;
+      int rc;
+      if ((rc = rate_geom(g, geom[9], geom[10], geom[3], max_wps, r, who))) return rc;
+      h.book.add_rate(r);
+      h.Y = r.Q * r.g.n;
+    }
+    h.n_hist.assign(slots, 0); h.cur.assign(slots, 0); h.slot_nw.assign(slots, nw); h.slot_par.assign(3 * (size_t)slots, 0.5);
+    h.slot_gal.assign(slots, nullptr); h.slot_thr.assign(slots, 0.0); h.slot_ticked.assign(slots, 0);
+    x.rings.assign((size_t)slots * h.book.C, 0.f);
+    x.yrings.assign((size_t)slots * std::max(1LL, h.Y), 0.f);
+    x.hist.assign(2 * (size_t)slots * std::max(1, nw - 1) * F, 0.f);
+    x.d.rings = reinterpret_cast<uint32_t*>(x.rings.data());
+    x.d.yrings = reinterpret_cast<uint32_t*>(x.yrings.data());
+    x.d.hist_vad = reinterpret_cast<uint32_t*>(x.hist.data());
+    x.d.C = h.book.C;
+    x.d.Y = h.Y;
+    return DG_OK;
+  };
+  auto run = [](const std::vector<XferPiece>& pc) {   // what slot_transfer_kernel does
+    for (const XferPiece& p : pc)
+      for (long long i = 0; i < p.n; i++)
+        p.dst[p.dst_mod ? (p.dst_pos + i) % p.dst_mod : p.dst_pos + i] = p.src[p.src_mod ? (p.src_pos + i) % p.src_mod : p.src_pos + i];
+  };
+  Side src, dst;
+  int rc;
+  if ((rc = make(src, geom[0], geom[1], geom[2])) || (rc = make(dst, geom[11], geom[12], geom[13]))) return rc;
+  dg_multi& h = src.h;
+  h.net.emb = nullptr;
+  std::vector<float> staged;
+  long long next = 0;
+  for (int i = 0; i < n_ops; i++) {
+    const int kind = ops[3 * i], slot = ops[3 * i + 1], n = ops[3 * i + 2];
+    rc = DG_OK;
+    if (kind == 0) {
+      if (slot < 0 || slot >= h.slots || h.book.open[slot] || n < -1 || n + 1 >= (int)h.book.rates.size()) rc = DG_EINVAL;
+      else {
+        h.book.start(slot, n + 1);
+        h.n_hist[slot] = 0;
+      }
+    } else if (kind == 1) {
+      if (!h.book.ok(slot)) rc = DG_EINVAL;
+      else h.book.stop(slot);
+    } else if (kind == 2) {
+      if (!h.book.ok(slot) || n < 0 || !h.book.fits(slot, n)) rc = DG_EINVAL;
+      else if (n > 0) {
+        staged.resize((size_t)h.book.n_staged);
+        staged.insert(staged.end(), samples_host + next, samples_host + next + n);
+        h.book.push(slot, n);
+        next += n;
+      }
+    } else if (kind == 4) {
+      const long long C = h.book.C;
+      for (const RingPiece& p : h.book.pieces)
+        for (int k = 0; k < p.n; k++) src.rings[(size_t)p.slot * C + (p.dst + k) % C] = staged[p.src + k];
+      TickPlan tp;
+      h.book.plan(h.max_wps, tp);
+      for (const RsFrames& it : tp.items) {
+        const RateGeom& r = h.book.geom(it.slot);
+        for (long long R = it.first; R < it.first + it.count; R++)
+          for (int p = 0; p < r.g.n; p++) src.yrings[(size_t)it.slot * h.Y + (R % r.Q) * r.g.n + p] = (float)(R * r.g.n + p);
+      }
+      const size_t stride = (size_t)std::max(1, h.nw - 1);
+      for (const TickSlot& ts : tp.act) {   // post_slots_history on the host, chunk c = the values c F + j
+        const int s = ts.slot, cur = h.cur[s], nh = h.n_hist[s], keep = std::min(h.slot_nw[s] - 1, nh + ts.n);
+        const long long c0 = h.book.rpos[s] / h.book.geom(s).hop;
+        for (int e = 0; e < keep; e++) {
+          const int v = ts.n - keep + e;
+          float* out = &src.hist[(((size_t)(cur ^ 1) * h.slots + s) * stride + e) * F];
+          for (int j = 0; j < F; j++)
+            out[j] = v >= 0 ? (float)((c0 + v) * F + j) : src.hist[(((size_t)cur * h.slots + s) * stride + nh + v) * F + j];
+        }
+        if (h.nw > 1) {
+          h.n_hist[s] = keep;
+          h.cur[s] ^= 1;
+        }
+      }
+      h.book.uploaded();
+      h.book.consumed(tp);
+      staged.clear();
+    } else {
+      rc = DG_EINVAL;
+    }
+    result[i] = rc;
+  }
+  if (!h.book.ok(src_slot)) {
+    set_error(std::string(who) + ": slot " + std::to_string(src_slot) + " is not open");
+    return DG_EINVAL;
+  }
+  staged.resize((size_t)h.book.n_staged);
+  XferHead hd = xfer_head(&h, src_slot);
+  std::vector<uint32_t> blob((size_t)hd.bytes / 4, 0);
+  std::vector<XferPiece> pc;
+  xfer_pieces(src.d, h.book.geom(src_slot), h.slots, h.nw, src_slot, h.cur[src_slot], hd, blob.data(),
+              hd.wpos - hd.rpos - StagedBySlot(h.book).n[src_slot], true, pc);
+  run(pc);
+  xfer_finish(&h, src_slot, hd, staged.data(), StagedBySlot(h.book), reinterpret_cast<unsigned char*>(blob.data()));
+  XferHead* ph = reinterpret_cast<XferHead*>(blob.data());
+  dg_multi& t = dst.h;
+  switch (patch) {
+    case 1: ph->version += 1; break;
+    case 2: ph->kind = 0; break;
+    case 3: ph->S += 4; break;
+    case 4: ph->nw = t.nw + 1; break;
+    case 5: ph->wpos = ph->rpos + t.book.rates[h.book.rate[src_slot]].cap + 1; break;
+    case 6: ph->init[1] = 1; break;
+    case 7: ph->rs_o += 1; break;
+    case 8: ph->magic = 0; break;
+    default: break;
+  }
+  int rid = -1;
+  dg_gallery* g = nullptr;
+  set_error("");
+  memset(info, 0, 16 * sizeof(int64_t));
+  const int irc = xfer_check(&t, *ph, reinterpret_cast<const unsigned char*>(blob.data()), blob.size() * 4, 0, nullptr, rid, g,
+                             "dg_multi_import");
+  const std::string msg = irc ? std::string(dg_last_error()) : std::string();
+  const size_t m = std::min(msg.size(), (size_t)msg_cap - 1);
+  memcpy(message, msg.data(), m);
+  message[m] = 0;
+  const RateGeom& tr = t.book.rates[h.book.rate[src_slot]];
+  const RateGeom& sr = h.book.geom(src_slot);
+  const int64_t row[13] = {irc, t.book.C, tr.Q, t.Y, hd.wpos, hd.rpos, hd.done, hd.n_hist, hd.frame0, hd.n_frames, hd.bytes,
+                           h.book.C, sr.Q};
+  memcpy(info, row, sizeof(row));
+  if (irc) return DG_OK;
+  const size_t need = std::max({(size_t)t.book.C, (size_t)std::max(1LL, t.Y), (size_t)std::max(1, t.nw - 1) * F});
+  if ((size_t)cap < need) {
+    set_error(std::string(who) + ": outputs of " + std::to_string(cap) + " floats, the target needs " + std::to_string(need));
+    return DG_EINVAL;
+  }
+  pc.clear();
+  xfer_pieces(dst.d, t.book.rates[rid + 1], t.slots, t.nw, 0, 0, *ph, blob.data(), ph->wpos - ph->rpos, false, pc);
+  run(pc);
+  xfer_open(&t, 0, rid, *ph, nullptr);
+  memcpy(ring_out, dst.rings.data(), (size_t)t.book.C * 4);
+  memcpy(yring_out, dst.yrings.data(), (size_t)std::max(1LL, t.Y) * 4);
+  memcpy(hist_out, dst.hist.data(), (size_t)std::max(1, t.nw - 1) * F * 4);
   return DG_OK;
 }

@@ -457,4 +457,14 @@ int launch_gallery_claim(const double* part_d, const int* part_e, int Qmax, cons
                          const int2* segs, int n_seg, const GalGroup* groups, int32_t* claimed, int32_t* entry_out,
                          double* dist_out, uint32_t* named, int M, int* names, int32_t* list, int32_t* prefix, cudaStream_t st);
 
+// transfer.cu -- n 32-bit words from src to dst: word i at src [(src_pos + i) mod src_mod] (src_mod 0: src [src_pos + i]),
+// likewise for dst.  A ring piece is addressed by absolute position mod its ring's capacity on each side.
+struct XferPiece {
+  const uint32_t* src;
+  uint32_t* dst;
+  long long n, src_pos, src_mod, dst_pos, dst_mod;
+};
+// every piece in one launch (pieces is a device array); `tag` names the launch in the profile
+int launch_slot_transfer(const XferPiece* pieces, int n_pieces, const char* tag, cudaStream_t st);
+
 }  // namespace dg

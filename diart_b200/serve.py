@@ -30,7 +30,11 @@ A diarization stream may also start from known speakers (``open(speakers=...)``,
 state is seeded with their centroids and its annotations name them; ``speakers(sid)`` exports a stream's state, so that a
 closed stream can be resumed with the same centroids and labels.  With a ``gallery`` (``speakers.SpeakerGallery``), every tick
 also names the streams' discovered speakers from it on the device; ``open(gallery=...)`` gives a stream its own gallery and
-threshold instead, and one grouped search per tick serves every gallery in use."""
+threshold instead, and one grouped search per tick serves every gallery in use.
+
+``export(sids)`` takes streams out of a server with their whole state (``transfer.StreamState``), and ``restore(states)``
+opens them in this or another compatible server, on this or another GPU or machine: the next tick continues each stream
+bit for bit as if it had never moved.  ``export(sids, close=False)`` is a checkpoint that leaves the streams running."""
 from __future__ import annotations
 
 import ctypes as C
@@ -48,6 +52,8 @@ from .blocks.vad import VoiceActivityDetectionConfig, speech_annotations
 from .core import Annotation
 from .operators import DeviceResample
 from .speakers import KnownSpeakers, SpeakerGallery, check_gallery, exported, speaker_labels
+from .transfer import VERSION as STATE_VERSION
+from .transfer import StreamState, gallery_fingerprint, model_fingerprint
 
 
 def plan_rows(idx: np.ndarray, step: float, window_samples: int, sample_rate: int, frames: int, nw: int, latency: float,
@@ -264,7 +270,117 @@ class _MultiStreamServer:
 
     def close(self, sid: int):
         _lib.check(_lib.lib().dg_multi_close(self._h, int(sid)))
+        self._release(sid)
+
+    def _release(self, sid: int):
+        """the host mirror of a slot that was closed"""
         self._open[sid] = False
+
+    _kind = ""   # StreamState.kind of the subclass's streams
+
+    def _settings(self) -> dict:
+        """what a stream's results depend on besides its own values and the models: a restored state must have them"""
+        cfg = self.config
+        return dict(duration=float(cfg.duration), step=float(cfg.step), sample_rate=int(cfg.sample_rate),
+                    window_samples=self.window_samples, step_samples=self.step_samples, F=self.F, K=self.K)
+
+    def _models(self) -> list:
+        return [model_fingerprint(self.config.segmentation.model)]
+
+    def _stream_meta(self, sid: int) -> dict:
+        """the host part of stream ``sid``'s state"""
+        rate = next(r for r, (rid, chunk, hop, res) in self.rates.items() if chunk == self._chunk[sid] and
+                    hop == self._hop[sid] and res == self._res[sid])
+        return dict(version=STATE_VERSION, kind=self._kind, models=self._models(), settings=self._settings(), rate=rate,
+                    latency=float(self._latency[sid]), shift=float(self._shift[sid]), pushed=int(self._pushed[sid]),
+                    emitted=int(self._emitted[sid]))
+
+    def _restore_gallery(self, state: StreamState, gallery):
+        """the gallery state ``state`` is named from here (None: none), or ValueError"""
+        return None
+
+    def _restored(self, sid: int, state: StreamState, gallery):
+        """the host mirror of a slot a state was restored into"""
+        meta = state._meta
+        rid, chunk, hop, res = self.rates[meta["rate"]]
+        self._open[sid] = True
+        self._pushed[sid], self._emitted[sid] = meta["pushed"], meta["emitted"]
+        self._shift[sid] = meta["shift"]
+        self._chunk[sid], self._hop[sid], self._res[sid] = chunk, hop, res
+        self._latency[sid] = meta["latency"]
+
+    def export(self, sids, *, close: bool = True) -> List[StreamState]:
+        """the whole state of each open stream in ``sids`` after the last tick, its samples pushed since then included, in
+        one launch and one copy (per 256 MiB).  ``close=True`` closes the streams as ``close`` does; ``close=False`` leaves
+        them running untouched (a checkpoint).  ValueError, closing nothing, for a stream that is not open or listed twice;
+        AssertionError for a diarization stream in the "Cannot update unknown centers" state (as ``speakers``)."""
+        sids = [int(s) for s in sids]
+        for s in sids:
+            if not (0 <= s < self.max_streams and self._open[s]):
+                raise ValueError(f"stream {s} is not open")
+        slots = np.asarray(sids, dtype=np.int32)
+        sizes = np.zeros(len(sids), dtype=np.int64)
+        lib = _lib.lib()
+        _lib.check(lib.dg_multi_export_bytes(self._h, slots.ctypes.data, len(sids), sizes.ctypes.data))
+        out = np.empty(int(sizes.sum()), dtype=np.uint8)
+        with torch.cuda.device(self.device):
+            _lib.check(lib.dg_multi_export(self._h, slots.ctypes.data, len(sids), int(bool(close)), out.ctypes.data,
+                                           len(out)))
+        off = np.concatenate([[0], np.cumsum(sizes)])
+        # each state views its part of the one output buffer (no second copy of a drain's gigabytes)
+        states = [StreamState(out[off[a]:off[a + 1]], self._stream_meta(s)) for a, s in enumerate(sids)]
+        if close:
+            for s in sids:
+                self._release(s)
+        return states
+
+    def restore(self, states, *, gallery=None) -> List[int]:
+        """opens each exported state in the lowest free slot, in order, with everything it had (counters, timestamp
+        shift, source rate, latency, thresholds, history, clustering, labels, names and claims): the next ``step``
+        continues each stream as if it had never left.  ``gallery``: the gallery of the states named from one (one
+        ``SpeakerGallery`` for all, or one entry per state; None: the server's default); it must be the very gallery the
+        stream was named from (same names and centroids), and the stream keeps its own threshold.  Returns the stream ids.
+        ValueError, naming the reason, with every slot left closed and nothing launched: another kind of stream, other
+        models or settings, a latency above ``max_latency``, an undeclared source rate, a backlog beyond the ring, a
+        missing or different gallery, no free slot, another format version."""
+        states = list(states)
+        n = len(states)
+        gals = list(gallery) if isinstance(gallery, (list, tuple)) else [gallery] * n
+        if len(gals) != n:
+            raise ValueError(f"{len(gals)} galleries for {n} states")
+        models, settings = self._models(), self._settings()
+        use = []
+        for a, st in enumerate(states):
+            if not isinstance(st, StreamState):
+                raise TypeError(f"states[{a}]: expected StreamState, got {type(st).__name__}")
+            meta = st._meta
+            if meta.get("version") != STATE_VERSION:
+                raise ValueError(f"state {a} has format version {meta.get('version')}; this build reads {STATE_VERSION}")
+            if meta["kind"] != self._kind:
+                raise ValueError(f"state {a} is a {meta['kind']} stream, this server serves {self._kind} streams")
+            if meta["models"] != models:
+                raise ValueError(f"state {a} was computed with other models")
+            if meta["settings"] != settings:
+                diff = sorted(k for k in settings if meta["settings"].get(k) != settings[k])
+                raise ValueError(f"state {a} was computed with other settings: {', '.join(diff)}")
+            if not meta["latency"] <= self.max_latency:
+                raise ValueError(f"state {a} has latency {meta['latency']}, above this server's max_latency "
+                                 f"{self.max_latency}")
+            if meta["rate"] not in self.rates:
+                raise ValueError(f"state {a} is at {meta['rate']} Hz, a rate this server did not declare "
+                                 f"(source_sample_rates: {sorted(self._resamplers)})")
+            use.append(self._restore_gallery(st, gals[a]))
+        if n > int((~self._open).sum()):
+            raise ValueError(f"{n} states, {int((~self._open).sum())} free slots")
+        blob = np.concatenate([st._blob for st in states]) if n else np.empty(0, np.uint8)
+        handles = (C.c_void_p * max(n, 1))(*[None if g is None else g.handle for g in use])
+        slots = np.empty(max(n, 1), dtype=np.int32)
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().dg_multi_import(self._h, blob.ctypes.data, len(blob), n, handles, slots.ctypes.data))
+        sids = slots[:n].tolist()
+        for sid, st, g in zip(sids, states, use):
+            self._restored(sid, st, g)
+        return sids
 
     def push(self, sid: int, block: np.ndarray):
         """appends a block of samples, shape (n,), (1, n) or (n, 1), to stream ``sid``; staged until the next ``step``"""
@@ -419,10 +535,53 @@ class MultiStreamDiarization(_MultiStreamServer):
             raise
         return sid
 
+    _kind = "diarization"
+
     def close(self, sid: int):
         """ends stream ``sid``; the server lets go of its gallery"""
         _MultiStreamServer.close(self, sid)
+
+    def _release(self, sid: int):
+        _MultiStreamServer._release(self, sid)
         self._slot_gallery[sid] = None
+
+    def _settings(self) -> dict:
+        cfg = self.config
+        return dict(_MultiStreamServer._settings(self), D=self.D, max_speakers=int(cfg.max_speakers),
+                    gamma=float(cfg.gamma), beta=float(cfg.beta),
+                    normalize_embedding_weights=bool(cfg.normalize_embedding_weights),
+                    metric=str(getattr(cfg, "metric", "cosine")))
+
+    def _models(self) -> list:
+        return _MultiStreamServer._models(self) + [model_fingerprint(self.config.embedding.model)]
+
+    def _stream_meta(self, sid: int) -> dict:
+        g = self._slot_gallery[sid]
+        return dict(_MultiStreamServer._stream_meta(self, sid),
+                    labels=list(self._stream_labels[sid]) if self._own_labels[sid] else None,
+                    gallery=None if g is None else gallery_fingerprint(g))
+
+    def _restore_gallery(self, state, gallery):
+        want = state._meta["gallery"]
+        if want is None:
+            return None
+        g = self.gallery if gallery is None else gallery
+        if g is None:
+            raise ValueError("the stream was named from a gallery: give it (gallery=) or serve it as the default")
+        if gallery_fingerprint(g) != want:
+            raise ValueError("the stream was named from another gallery (names or centroids differ)")
+        check_gallery(g, self.config, self.D)
+        if not same_device(g.device, self.device):
+            raise ValueError(f"the gallery is on {g.device}, the server on {self.device}")
+        return g
+
+    def _restored(self, sid, state, gallery):
+        _MultiStreamServer._restored(self, sid, state, gallery)
+        labels = state._meta["labels"]
+        self._own_labels[sid] = labels is not None
+        self._stream_labels[sid] = self.labels if labels is None else list(labels)
+        self._slot_gallery[sid] = gallery
+        self._naming = self._naming or gallery is not None
 
     def speakers(self, sid: int) -> KnownSpeakers:
         """the clustering state of open stream ``sid`` after the last tick: its active centres in index order (a prefix
@@ -488,6 +647,7 @@ class MultiStreamVoiceActivityDetection(_MultiStreamServer):
 
     _needs = "MultiStreamVoiceActivityDetection needs the native segmentation model (B200PyanNet)"
     _speakers = 1
+    _kind = "vad"
 
     def __init__(self, config: VoiceActivityDetectionConfig, max_streams: int, max_windows_per_stream: int = 4,
                  source_sample_rates=(), max_latency: Optional[float] = None, gallery=None):

@@ -559,6 +559,51 @@ int dg_multi_last_names(const dg_multi* h, int32_t* out_host /* [cap][3] */, int
 /* test hook: the last tick's window batch [n_rows, chunk_samples] (what its networks read; n_rows = that tick's window count)
  * copied to wav_dev.  Synchronous. */
 int dg_multi_last_windows(const dg_multi* h, float* wav_dev, int n_rows);
+/* ---- moving live streams between handles (diarization and VAD handles alike), e.g. to drain a GPU, rebalance or keep a
+ *      checkpoint.  A stream's packed state holds everything its next ticks read, so the stream continues on the target
+ *      exactly as on the source.  Layout, format version 1 (host byte order; every section starts at a multiple of 16 bytes
+ *      from the state's start, and a state's size is a multiple of 16, so states follow each other directly):
+ *        head (a fixed struct, csrc/api_multi.cu XferHead): magic "DGST", version, kind (0 diarization, 1 VAD); the
+ *          pipeline's window and step samples, F, K, D, M; the source rate's resampling {o, n, w} (all 0 at the pipeline's
+ *          rate), window and step at that rate; the stream's buffers (latency / step) and history entries n_hist; the
+ *          clustering's two init words; the named speakers (bit g) and the size of the gallery they are named from (0:
+ *          none); whether it has had a tick; the absolute wpos, rpos and done (16 kHz frames computed), and the frames
+ *          carried [frame0, frame0 + n_frames); {tau, rho, delta}; the gallery threshold; gamma, beta,
+ *          normalize_weights; the state's bytes;
+ *        audio float32 [wpos - rpos]: the samples from the start of the next window on, staged ones included;
+ *        frames float32 [n_frames][n]: for a resampled stream, the computed 16 kHz frames a future window still reads;
+ *        history, oldest first: diarization scores float32 [n_hist][F][K] then maps int32 [n_hist][K]; VAD max curves
+ *          float32 [n_hist][F];
+ *        diarization only: centroids float64 [M][D], active int32 [32], claimed gallery entries int32 [32] (-1: none).
+ *      dg_multi_export_bytes: the size of each listed slot's state now (it grows with pushes).
+ *      dg_multi_export: the states of the n listed open slots (distinct), packed in list order into out_host (out_bytes:
+ *        its size).  One launch gathers the device state of every slot of a round into a staging buffer, one copy brings
+ *        it back through pinned memory (rounds of at most 256 MiB of states).  close != 0 then closes the slots as
+ *        dg_multi_close does; close = 0 leaves them untouched (a checkpoint).  Synchronous.  DG_EINVAL, closing nothing,
+ *        for a slot that is not open or listed twice, too small an output, or a stream in the "Cannot update unknown
+ *        centers" state (as dg_multi_get_state reports it).
+ *      dg_multi_import: opens n packed states (blob_host, blob_bytes in all) in the lowest free slots, in order, into
+ *        slots_out.  Each continues its stream: the next dg_multi_step gives it the windows, results and names it would
+ *        have had on its source.  The audio goes to the slot's ring and frames to its 16 kHz ring at absolute position
+ *        mod their capacities, the history is written at this handle's history stride.  gals (null, or n entries, null
+ *        meaning the handle's default gallery): the gallery of each state that was named from one, named at the state's
+ *        own threshold; it must outlive the slot.  One copy, one launch per round.  Synchronous.  DG_EINVAL, naming the
+ *        state and the reason, opening nothing and launching nothing, for: another format version or kind, other windows,
+ *        F, K, D, M, gamma, beta or normalize_weights, a source rate this handle did not declare, more buffers than the
+ *        handle's num_windows, audio beyond the ring's capacity, a clustering state that failed on its source, a state named
+ *        from a gallery without one (or one of another size, dimension or device), a malformed state, or too few free
+ *        slots.  Both calls keep a device staging buffer and a pinned buffer of up to 256 MiB of states (plus the piece
+ *        list) for the handle's life once a move needed them; the call that first grows them synchronises the device.
+ *        The gaps that align the sections are zero, so a state's bytes depend on the stream alone. ---- */
+int dg_multi_export_bytes(const dg_multi* h, const int32_t* slots, int n, int64_t* bytes_out);
+int dg_multi_export(dg_multi* h, const int32_t* slots, int n, int close, void* out_host, int64_t out_bytes);
+int dg_multi_import(dg_multi* h, const void* blob_host, int64_t blob_bytes, int n, dg_gallery* const* gals,
+                    int32_t* slots_out);
+/* test hook (host only, no GPU): dg_multi_export of one stream of a VAD handle and dg_multi_import of its state into another
+ * with other slots, max_windows_per_stream and num_windows, the pieces run on the host; see csrc/api_multi.cu. */
+int dg_selftest_multi_transfer_host(const int32_t* geom, int n_ops, const int32_t* ops, const float* samples_host,
+                                    int32_t* result, int src_slot, int patch, float* ring_out, float* yring_out, float* hist_out,
+                                    int64_t cap, int64_t* info, char* message, int msg_cap);
 /* test hook (host only, no GPU): dg_multi's tick planning for `slots` streams with pipeline windows of out_chunk / out_step
  * samples and the declared rates rates int32 [n_rates][5] = {o, n, w, chunk, step} (refused as dg_multi_add_rate refuses
  * them, DG_EINVAL).  ops int32 [n_ops][3] = {kind, slot, n}: 0 open slot at rate id n (-1: the pipeline's rate), 1 close slot,
