@@ -80,61 +80,71 @@ struct TickPlan {
   std::vector<long long> done;
 };
 
-// The host bookkeeping of the streams' audio, no device work: per slot the open flag, its rate and the absolute sample counters
-// pushed (staged included) / start of the next window, and for a resampled stream the 16 kHz frames computed so far; the
-// samples pushed since the last tick are [0, n_staged) of a staging buffer, described by `pieces` in push order.  A piece is a
-// run of ONE slot's samples that is contiguous both in the staging buffer and in that slot's stream, so a piece is extended
-// only by a push that continues it in both.  Every slot's ring has stride C (the largest capacity of any rate).
+// the pipeline's own rate: a ring with room for the windows of a tick and as much audio again pushed ahead (as dg_stream)
+static RateGeom pipeline_rate(int S, int hop, int max_wps) {
+  RateGeom r;
+  r.S = S;
+  r.hop = hop;
+  r.cap = (int)ring_capacity(S, hop, max_wps);
+  return r;
+}
+
+// The audio of the stream in a slot: its rate (index into SlotBook::rates), whether the slot is open, and the absolute sample
+// counters pushed (staged included) / start of the next window, and for a resampled stream the 16 kHz frames computed so far.
+struct SlotAudio {
+  int rate = 0;
+  bool open = false;
+  long long wpos = 0, rpos = 0, done = 0;
+};
+
+// The host bookkeeping of the streams' audio, no device work: a SlotAudio per slot; the samples pushed since the last tick
+// are [0, n_staged) of a staging buffer, described by `pieces` in push order.  A piece is a run of ONE slot's samples that is
+// contiguous both in the staging buffer and in that slot's stream, so a piece is extended only by a push that continues it
+// in both.  Every slot's ring has stride C (the largest capacity of any rate).
 struct SlotBook {
   int C = 0;
   std::vector<RateGeom> rates;                // [0]: the pipeline's rate; [1 + id]: declared rate id
-  std::vector<char> open;
-  std::vector<int> rate;
-  std::vector<long long> wpos, rpos, done;
+  std::vector<SlotAudio> audio;
   std::vector<RingPiece> pieces;
   long long n_staged = 0;
 
   void init(int slots, const RateGeom& base) {
     rates.assign(1, base);
     C = base.cap;
-    open.assign(slots, 0);
-    rate.assign(slots, 0);
-    wpos.assign(slots, 0);
-    rpos.assign(slots, 0);
-    done.assign(slots, 0);
+    audio.assign(slots, SlotAudio{});
   }
   void add_rate(const RateGeom& r) {
     rates.push_back(r);
     C = std::max(C, r.cap);
   }
-  bool ok(int slot) const { return slot >= 0 && slot < (int)open.size() && open[slot]; }
-  const RateGeom& geom(int s) const { return rates[rate[s]]; }
+  bool ok(int slot) const { return slot >= 0 && slot < (int)audio.size() && audio[slot].open; }
+  const RateGeom& geom(int s) const { return rates[audio[s].rate]; }
   long long available(int s) const {    // complete windows, pushed and not consumed
     const RateGeom& r = geom(s);
-    const long long have = wpos[s] - rpos[s];
+    const long long have = audio[s].wpos - audio[s].rpos;
     return have < r.S ? 0 : (have - r.S) / r.hop + 1;
   }
-  void start(int slot, int r = 0) {
-    open[slot] = 1;
-    rate[slot] = r;
-    wpos[slot] = rpos[slot] = done[slot] = 0;
+  // a stream starts in `slot` at a's rate and counters (a new stream: all zero)
+  void start(int slot, SlotAudio a = {}) {
+    a.open = true;
+    audio[slot] = a;
   }
   // the stream ends: its staged samples are dropped (they stay in the staging buffer, no piece refers to them)
   void stop(int slot) {
-    open[slot] = 0;
+    audio[slot].open = false;
     pieces.erase(std::remove_if(pieces.begin(), pieces.end(), [&](const RingPiece& p) { return p.slot == slot; }),
                  pieces.end());
   }
-  bool fits(int slot, int n) const { return wpos[slot] + n - rpos[slot] <= geom(slot).cap; }
+  bool fits(int slot, int n) const { return audio[slot].wpos + n - audio[slot].rpos <= geom(slot).cap; }
   // books n > 0 samples of `slot` at staging offset n_staged (the caller copies them there)
   void push(int slot, int n) {
     RingPiece* last = pieces.empty() ? nullptr : &pieces.back();
-    if (last && last->slot == slot && last->src + last->n == n_staged && last->dst + last->n == wpos[slot])
+    if (last && last->slot == slot && last->src + last->n == n_staged && last->dst + last->n == audio[slot].wpos)
       last->n += n;
     else
-      pieces.push_back(RingPiece{n_staged, wpos[slot], slot, n});
+      pieces.push_back(RingPiece{n_staged, audio[slot].wpos, slot, n});
     n_staged += n;
-    wpos[slot] += n;
+    audio[slot].wpos += n;
   }
   void uploaded() {
     pieces.clear();
@@ -147,24 +157,25 @@ struct SlotBook {
     const int nr = (int)rates.size();
     std::vector<std::vector<RsFrames>> items(nr);
     std::vector<std::vector<RsRow>> rs_rows(nr);
-    for (int s = 0; s < (int)open.size(); s++) {
-      const int n = open[s] ? (int)std::min<long long>(available(s), max_wps) : 0;
+    for (int s = 0; s < (int)audio.size(); s++) {
+      const SlotAudio& a = audio[s];
+      const int n = a.open ? (int)std::min<long long>(available(s), max_wps) : 0;
       if (!n) continue;
       const RateGeom& r = geom(s);
       t.act.push_back(TickSlot{s, t.B, n, 0, 0, 1, {0, 0}});
-      long long d = done[s];
+      long long d = a.done;
       for (int i = 0; i < n; i++) {
-        const long long st = rpos[s] + (long long)i * r.hop;
+        const long long st = a.rpos + (long long)i * r.hop;
         t.rows.push_back(make_int2((int)t.act.size() - 1, i));
         t.start.push_back(st);
         if (r.resampled())
-          rs_rows[rate[s]].push_back(RsRow{st, st / r.g.o, s, t.B + i});
+          rs_rows[a.rate].push_back(RsRow{st, st / r.g.o, s, t.B + i});
       }
       if (r.resampled()) {
-        const long long lo = std::max(d, rpos[s] / r.g.o + r.r_lo);
-        const long long hi = (rpos[s] + (long long)(n - 1) * r.hop) / r.g.o + r.r_hi;
+        const long long lo = std::max(d, a.rpos / r.g.o + r.r_lo);
+        const long long hi = (a.rpos + (long long)(n - 1) * r.hop) / r.g.o + r.r_hi;
         if (hi >= lo) {
-          items[rate[s]].push_back(RsFrames{lo, s, (int)(hi - lo + 1)});
+          items[a.rate].push_back(RsFrames{lo, s, (int)(hi - lo + 1)});
           d = hi + 1;
         }
       }
@@ -189,10 +200,22 @@ struct SlotBook {
   void consumed(const TickPlan& t) {
     for (size_t a = 0; a < t.act.size(); a++) {
       const int s = t.act[a].slot;
-      rpos[s] += (long long)t.act[a].n * geom(s).hop;
-      done[s] = t.done[a];
+      audio[s].rpos += (long long)t.act[a].n * geom(s).hop;
+      audio[s].done = t.done[a];
     }
   }
+};
+
+// The values of the stream in a slot besides its audio (SlotAudio): its latency / step nw (<= the handle's), post-path
+// history entries and current copy, {tau, rho, delta} (a VAD handle: {tau, 0, 0}), the gallery and threshold it is named from
+// (null: none), whether it has had a tick, and its named global speakers (bit g; the host mirror of the device's table).
+struct SlotStream {
+  int nw = 1, n_hist = 0, cur = 0;
+  double par[3] = {0.0, 0.0, 0.0};
+  dg_gallery* gal = nullptr;
+  double thr = 0.0;
+  bool ticked = false;
+  uint32_t named = 0;
 };
 
 struct dg_multi {
@@ -202,10 +225,8 @@ struct dg_multi {
   double tau = 0.5, rho = 0.3, delta = 1.0;   // the values of a stream opened without its own
   NetLanes net;
   SlotBook book;
+  std::vector<SlotStream> streams;            // per slot
   PinnedBuf stage;                            // staged samples [0, book.n_staged), then a tick's tables
-  std::vector<int> n_hist, cur;               // per slot: post-path history entries, current copy
-  std::vector<int> slot_nw;                   // per slot: its stream's latency / step (<= nw)
-  std::vector<double> slot_par;               // per slot [3]: its stream's {tau, rho, delta} (a VAD handle: {tau, 0, 0})
   DevBuf yrings;                              // resampled streams: 16 kHz rings [slots][Y]
   long long Y = 0;
   bool opened = false;                        // a stream was opened (rates can no longer be added)
@@ -217,18 +238,14 @@ struct dg_multi {
   Event e_start, e_lane_done[2];
   Event t_begin, t_end;                       // timing events around the last tick's device work on `st`
   bool timed = false;                         // a tick has run
-  // gallery naming: the default gallery and threshold of every stream (dg_multi_set_gallery), and per slot the gallery and
-  // threshold its stream is named from (dg_multi_set_slot_gallery; null: none) and whether it has had a tick.  Once the
-  // handle has received a gallery: per slot the named global speakers (bit g) and their claimed entries [slots][32], indices
-  // into the slot's gallery, on the device and mirrored on the host (named_host non-empty); a tick's queries, segments, query
-  // offset and count per group, split partials and new names {slot, g, entry}
+  // gallery naming: the default gallery and threshold of every stream (dg_multi_set_gallery).  Once the handle has received a
+  // gallery (naming): per slot the named global speakers (bit g) and their claimed entries [slots][32], indices into the
+  // slot's gallery, on the device (the named bits mirrored in SlotStream::named); a tick's queries, segments, query offset
+  // and count per group, split partials and new names {slot, g, entry}
   dg_gallery* gal = nullptr;
   double gal_threshold = 0.0;
-  std::vector<dg_gallery*> slot_gal;
-  std::vector<double> slot_thr;
-  std::vector<char> slot_ticked;
+  bool naming = false;
   DevBuf gal_named, gal_claimed, gal_q, gal_seg, gal_gq, gal_d, gal_e, gal_list;
-  std::vector<uint32_t> named_host;
   std::vector<int32_t> names_last;            // the names the last dg_multi_step decided, [n][3]
   // dg_multi_export / dg_multi_import: one round's packed states and its piece list, on the device and pinned.  Allocated
   // by the first move that needs them (a growth synchronises the device, as every DevBuf growth does) and kept for the
@@ -239,7 +256,7 @@ struct dg_multi {
 
 // In front of the header in h->header and in the tick's pinned download, once the handle has received a gallery: the count
 // of the tick's new names (16 bytes) and the first GAL_NAME_PREFIX of them, so that they travel in the header's copy
-static size_t names_bytes(const dg_multi* h) { return h->named_host.empty() ? 0 : 16 + (size_t)GAL_NAME_PREFIX * 12; }
+static size_t names_bytes(const dg_multi* h) { return h->naming ? 16 + (size_t)GAL_NAME_PREFIX * 12 : 0; }
 
 // The grouped gallery search of a tick (gallery_plan): groups (one per distinct gallery and threshold, in order of their
 // first slot), the tick's slots with a gallery as segments {slot, group} (group by group, slots in order), the work list,
@@ -291,6 +308,33 @@ static void gallery_tick_plan(const int* slot, const int* key, const int* unname
 static bool slot_ok(const dg_multi* h, int slot) { return h && h->book.ok(slot); }
 static bool vad_mode(const dg_multi* h) { return !h->net.emb; }
 
+// The host side of a handle, no device work: `slots` slots, all closed, taking up to max_wps windows of S samples every hop
+// at the pipeline's rate, of F frames and K local speakers, aggregating up to nw buffers
+static void multi_init(dg_multi& h, int device, int slots, int max_wps, int S, int hop, int F, int K, int nw) {
+  h.device = device; h.slots = slots; h.max_wps = max_wps;
+  h.S = S; h.hop = hop; h.F = F; h.K = K; h.nw = nw;
+  h.book.init(slots, pipeline_rate(S, hop, max_wps));
+  h.streams.assign(slots, SlotStream{});
+}
+
+// The device side of a handle set up by multi_init (its mode, M and D set): the rings, the Hamming window, the histories and
+// (diarization) clustering states of every slot, the scratch lanes, stream and events.  On success *out owns the handle.
+static int multi_alloc(std::unique_ptr<dg_multi> h, const double* hamming_host, dg_multi** out) {
+  const size_t n = (size_t)h->slots, hist = (size_t)std::max(1, h->nw - 1), F = (size_t)h->F, K = (size_t)h->K;
+  DG_CUDA(cudaSetDevice(h->device));
+  if (h->rings.ensure(n * h->book.C * 4) || h->hamming.ensure(F * 8) || h->total.ensure(16)) return DG_ECUDA;
+  if (vad_mode(h.get()) ? h->hist_vad.ensure(2 * n * hist * F * 4)
+                        : (h->centers.ensure(n * h->M * h->D * 8) || h->active.ensure(n * 32 * 4) || h->init.ensure(n * 2 * 4) ||
+                           h->hist_seg.ensure(2 * n * hist * F * K * 4) || h->hist_map.ensure(2 * n * hist * K * 4)))
+    return DG_ECUDA;
+  DG_CUDA(cudaMemcpy(h->hamming.p, hamming_host, F * 8, cudaMemcpyHostToDevice));
+  if (net_lanes_create(h->net) || h->st.create() || h->e_start.create() || h->e_lane_done[0].create() ||
+      h->e_lane_done[1].create() || h->t_begin.create(cudaEventDefault) || h->t_end.create(cudaEventDefault))
+    return DG_ECUDA;
+  *out = h.release();
+  return DG_OK;
+}
+
 extern "C" int dg_multi_create(dg_seg* seg, dg_emb* emb, int chunk_samples, int step_samples, int max_streams,
                                int max_windows_per_stream, int max_speakers, double tau, double rho, double delta, float gamma,
                                float beta, int normalize_weights, int num_windows, const double* hamming_host, dg_multi** out) {
@@ -322,33 +366,13 @@ extern "C" int dg_multi_create(dg_seg* seg, dg_emb* emb, int chunk_samples, int 
               "200 KB");
     return DG_EINVAL;
   }
-  DG_CUDA(cudaSetDevice(seg->device));
   std::unique_ptr<dg_multi> h(new dg_multi());
-  h->device = seg->device; h->slots = max_streams; h->max_wps = max_windows_per_stream;
-  h->S = chunk_samples; h->hop = step_samples;
-  // room for the windows of a tick and as much audio again pushed ahead (as dg_stream)
-  RateGeom base;
-  base.S = chunk_samples;
-  base.hop = step_samples;
-  base.cap = (int)ring_capacity(chunk_samples, step_samples, max_windows_per_stream);
-  h->book.init(max_streams, base);
-  h->F = F; h->K = K; h->D = D; h->M = max_speakers; h->nw = num_windows;
+  multi_init(*h, seg->device, max_streams, max_windows_per_stream, chunk_samples, step_samples, F, K, num_windows);
+  h->D = D; h->M = max_speakers;
   h->tau = tau; h->rho = rho; h->delta = delta;
   h->net.seg = seg; h->net.emb = emb;
   h->net.gamma = gamma; h->net.beta = beta; h->net.normalize_weights = normalize_weights;
-  const size_t n = (size_t)max_streams, hist = (size_t)std::max(1, num_windows - 1);
-  h->n_hist.assign(n, 0); h->cur.assign(n, 0); h->slot_nw.assign(n, num_windows); h->slot_par.assign(3 * n, 0.0);
-  h->slot_gal.assign(n, nullptr); h->slot_thr.assign(n, 0.0); h->slot_ticked.assign(n, 0);
-  if (h->rings.ensure(n * h->book.C * 4) || h->hamming.ensure((size_t)F * 8) || h->centers.ensure(n * max_speakers * D * 8) ||
-      h->active.ensure(n * 32 * 4) || h->init.ensure(n * 2 * 4) || h->hist_seg.ensure(2 * n * hist * F * K * 4) ||
-      h->hist_map.ensure(2 * n * hist * K * 4) || h->total.ensure(16))
-    return DG_ECUDA;
-  DG_CUDA(cudaMemcpy(h->hamming.p, hamming_host, (size_t)F * 8, cudaMemcpyHostToDevice));
-  if (net_lanes_create(h->net) || h->st.create() || h->e_start.create() || h->e_lane_done[0].create() ||
-      h->e_lane_done[1].create() || h->t_begin.create(cudaEventDefault) || h->t_end.create(cudaEventDefault))
-    return DG_ECUDA;
-  *out = h.release();
-  return DG_OK;
+  return multi_alloc(std::move(h), hamming_host, out);
 }
 
 // The numbers are checked before the handles, so that every refusal can be seen without a device.
@@ -374,30 +398,12 @@ extern "C" int dg_multi_create_vad(dg_seg* seg, int chunk_samples, int step_samp
     set_error("dg_multi_create_vad: need local speakers <= 8 and frames <= 1023");
     return DG_EINVAL;
   }
-  DG_CUDA(cudaSetDevice(seg->device));
   std::unique_ptr<dg_multi> h(new dg_multi());
-  h->device = seg->device; h->slots = max_streams; h->max_wps = max_windows_per_stream;
-  h->S = chunk_samples; h->hop = step_samples;
-  RateGeom base;
-  base.S = chunk_samples;
-  base.hop = step_samples;
-  base.cap = (int)ring_capacity(chunk_samples, step_samples, max_windows_per_stream);
-  h->book.init(max_streams, base);
-  h->F = F; h->K = K; h->M = 1; h->nw = num_windows;   // one "speaker": speech
+  multi_init(*h, seg->device, max_streams, max_windows_per_stream, chunk_samples, step_samples, F, K, num_windows);
+  h->M = 1;   // one "speaker": speech
   h->tau = tau;
   h->net.seg = seg;
-  const size_t n = (size_t)max_streams, hist = (size_t)std::max(1, num_windows - 1);
-  h->n_hist.assign(n, 0); h->cur.assign(n, 0); h->slot_nw.assign(n, num_windows); h->slot_par.assign(3 * n, 0.0);
-  h->slot_gal.assign(n, nullptr); h->slot_thr.assign(n, 0.0); h->slot_ticked.assign(n, 0);
-  if (h->rings.ensure(n * h->book.C * 4) || h->hamming.ensure((size_t)F * 8) || h->hist_vad.ensure(2 * n * hist * F * 4) ||
-      h->total.ensure(16))
-    return DG_ECUDA;
-  DG_CUDA(cudaMemcpy(h->hamming.p, hamming_host, (size_t)F * 8, cudaMemcpyHostToDevice));
-  if (net_lanes_create(h->net) || h->st.create() || h->e_start.create() || h->e_lane_done[0].create() ||
-      h->e_lane_done[1].create() || h->t_begin.create(cudaEventDefault) || h->t_end.create(cudaEventDefault))
-    return DG_ECUDA;
-  *out = h.release();
-  return DG_OK;
+  return multi_alloc(std::move(h), hamming_host, out);
 }
 
 extern "C" int dg_multi_destroy(dg_multi* h) {
@@ -439,6 +445,28 @@ extern "C" int dg_multi_add_rate(dg_multi* h, dg_resample* rs, int chunk_samples
   return DG_OK;
 }
 
+// The host bookkeeping of a stream that starts in `slot` (closed) with values x and audio a (a new stream: fresh values and
+// zero counters at its rate; a restored one: what it had)
+static void stream_begin(dg_multi* h, int slot, const SlotStream& x, const SlotAudio& a) {
+  h->book.start(slot, a);
+  h->streams[slot] = x;
+  h->opened = true;
+}
+
+// the stream in open `slot` ends: its staged samples are dropped, and the handle no longer refers to its gallery
+static void stream_end(dg_multi* h, int slot) {
+  h->book.stop(slot);
+  h->streams[slot].gal = nullptr;
+}
+
+// slots [s0, s0 + n) with nothing named or claimed, on the device (on h->st) and in the host mirror; the tables exist
+static int clear_names(dg_multi* h, int s0, int n) {
+  DG_CUDA(cudaMemsetAsync(h->gal_named.as<uint32_t>() + s0, 0, (size_t)n * 4, h->st));
+  DG_CUDA(cudaMemsetAsync(h->gal_claimed.as<int32_t>() + (size_t)s0 * 32, 0xff, (size_t)n * 32 * 4, h->st));
+  for (int s = s0; s < s0 + n; s++) h->streams[s].named = 0;
+  return DG_OK;
+}
+
 // a new stream in `slot` at declared rate `rate_id` (-1: the pipeline's rate), aggregating num_windows buffers, with
 // params {tau, rho, delta} (a VAD handle reads tau only): empty rings, no history, and the clustering state (a VAD handle has
 // none) fresh (the reference's SpeakerDiarization.reset()) for n = 0, else seeded with the n known centroids centers_host
@@ -446,7 +474,7 @@ extern "C" int dg_multi_add_rate(dg_multi* h, dg_resample* rs, int chunk_samples
 // `who` and changes nothing.
 static int open_slot(dg_multi* h, int slot, int rate_id, int num_windows, const double* params, const double* centers_host,
                      int n, const char* who) {
-  if (!h || slot < 0 || slot >= h->slots || h->book.open[slot]) {
+  if (!h || slot < 0 || slot >= h->slots || h->book.audio[slot].open) {
     set_error(std::string(who) + ": slot " + std::to_string(slot) + " is out of range or already open");
     return DG_EINVAL;
   }
@@ -499,23 +527,14 @@ static int open_slot(dg_multi* h, int slot, int rate_id, int num_windows, const 
       DG_CUDA(cudaMemcpyAsync(h->init.as<int>() + s * 2, init, 2 * 4, cudaMemcpyHostToDevice, h->st));
     }
   }
-  if (!h->named_host.empty()) {   // a stream opens with no speaker named
-    DG_CUDA(cudaMemsetAsync(h->gal_named.as<uint32_t>() + s, 0, 4, h->st));
-    DG_CUDA(cudaMemsetAsync(h->gal_claimed.as<int32_t>() + s * 32, 0xff, 32 * 4, h->st));
-    h->named_host[slot] = 0;
-  }
+  int rc;
+  if (h->naming && (rc = clear_names(h, slot, 1))) return rc;   // a stream opens with no speaker named
+  SlotStream x{num_windows, 0, 0, {params[0], vad ? 0.0 : params[1], vad ? 0.0 : params[2]}};
   if (!vad) {   // named from the default gallery unless dg_multi_set_slot_gallery gives it its own
-    h->slot_gal[slot] = h->gal;
-    h->slot_thr[slot] = h->gal_threshold;
-    h->slot_ticked[slot] = 0;
+    x.gal = h->gal;
+    x.thr = h->gal_threshold;
   }
-  h->book.start(slot, rate_id + 1);
-  h->n_hist[slot] = 0;
-  h->slot_nw[slot] = num_windows;
-  h->slot_par[3 * (size_t)slot + 0] = params[0];
-  h->slot_par[3 * (size_t)slot + 1] = vad ? 0.0 : params[1];
-  h->slot_par[3 * (size_t)slot + 2] = vad ? 0.0 : params[2];
-  h->opened = true;
+  stream_begin(h, slot, x, SlotAudio{rate_id + 1});
   return DG_OK;
 }
 
@@ -549,8 +568,7 @@ extern "C" int dg_multi_close(dg_multi* h, int slot) {
     set_error("dg_multi_close: slot " + std::to_string(slot) + " is not open");
     return DG_EINVAL;
   }
-  h->book.stop(slot);
-  h->slot_gal[slot] = nullptr;   // the handle no longer refers to the stream's gallery
+  stream_end(h, slot);
   return DG_OK;
 }
 
@@ -592,7 +610,7 @@ extern "C" int dg_multi_push_host(dg_multi* h, int slot, const float* samples, i
   }
   if (!h->book.fits(slot, n)) {
     set_error("dg_multi_push_host: ring of slot " + std::to_string(slot) + " full (" +
-              std::to_string(h->book.wpos[slot] - h->book.rpos[slot]) + " samples buffered, capacity " +
+              std::to_string(h->book.audio[slot].wpos - h->book.audio[slot].rpos) + " samples buffered, capacity " +
               std::to_string(h->book.geom(slot).cap) + "): step first");
     return DG_EINVAL;
   }
@@ -671,7 +689,7 @@ static int tick_audio_in(dg_multi* h, const TickPlan& tp, const int32_t* plan_ho
     const TickSlot& ts = act[a];
     for (; s <= ts.slot; s++) off[s] = ts.row0;
     states[a] = make_int2(ts.slot, a);
-    memcpy(trials + 3 * (size_t)a, &h->slot_par[3 * (size_t)ts.slot], 24);
+    memcpy(trials + 3 * (size_t)a, h->streams[ts.slot].par, 24);
   }
   if (L.mixed) {
     if (n16) memcpy(pin + L.o_rows16, tp.rows16.data(), (size_t)n16 * 8);
@@ -849,10 +867,11 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
   const int B = tp.B;
   for (int s = 0; s < h->slots; s++) counts_host[s] = 0;
   for (TickSlot& ts : act) {
+    const SlotStream& x = h->streams[ts.slot];
     counts_host[ts.slot] = ts.n;
-    ts.cur = h->cur[ts.slot];
-    ts.n_hist = h->n_hist[ts.slot];
-    ts.nw = h->slot_nw[ts.slot];
+    ts.cur = x.cur;
+    ts.n_hist = x.n_hist;
+    ts.nw = x.nw;
   }
   if (n_rows != B) {
     set_error(std::string(who) + ": " + std::to_string(n_rows) + " plan rows given, the tick has " + std::to_string(B) +
@@ -882,26 +901,26 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
   // with galleries: the tick's slots grouped by gallery and threshold; the unnamed global speakers of a slot are an upper
   // bound of its queries
   GalTick gt;
-  if (!h->named_host.empty()) {
+  if (h->naming) {
     std::vector<int> slot, key, unnamed, G;
     std::vector<double> thr;
     std::vector<const dg_gallery*> gals;
     std::map<std::pair<const dg_gallery*, double>, int> key_of;   // (gallery, threshold) -> key
     for (const TickSlot& ts : act) {
-      const dg_gallery* g = h->slot_gal[ts.slot];
+      const SlotStream& x = h->streams[ts.slot];
       int k = -1;
-      if (g) {
-        const auto it = key_of.emplace(std::make_pair(g, h->slot_thr[ts.slot]), (int)gals.size()).first;
+      if (x.gal) {
+        const auto it = key_of.emplace(std::make_pair(x.gal, x.thr), (int)gals.size()).first;
         k = it->second;
         if (k == (int)gals.size()) {
-          gals.push_back(g);
-          thr.push_back(h->slot_thr[ts.slot]);
-          G.push_back(g->G);
+          gals.push_back(x.gal);
+          thr.push_back(x.thr);
+          G.push_back(x.gal->G);
         }
       }
       slot.push_back(ts.slot);
       key.push_back(k);
-      unnamed.push_back(M - __builtin_popcount(h->named_host[ts.slot]));
+      unnamed.push_back(M - __builtin_popcount(x.named));
     }
     gallery_tick_plan(slot.data(), key.data(), unnamed.data(), (int)act.size(), G.data(), thr.data(), gt);
     for (size_t r = 0; r < gt.groups.size(); r++) {
@@ -931,10 +950,11 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
   h->book.uploaded();
   h->book.consumed(tp);
   for (const TickSlot& ts : act) {
-    h->slot_ticked[ts.slot] = 1;
+    SlotStream& x = h->streams[ts.slot];
+    x.ticked = true;
     if (h->nw > 1) {
-      h->n_hist[ts.slot] = std::min(ts.nw - 1, ts.n_hist + ts.n);
-      h->cur[ts.slot] ^= 1;
+      x.n_hist = std::min(ts.nw - 1, ts.n_hist + ts.n);
+      x.cur ^= 1;
     }
   }
   if (queries > 0) {   // the new names: the prefix came with the header, the rest (if any) is copied now
@@ -948,19 +968,18 @@ extern "C" int dg_multi_step(dg_multi* h, const int32_t* plan_host, int n_rows, 
                               (size_t)(count - pre) * 12, cudaMemcpyDeviceToHost, st));
       DG_CUDA(cudaStreamSynchronize(st));
     }
-    for (int i = 0; i < count; i++) h->named_host[h->names_last[3 * i]] |= 1u << h->names_last[3 * i + 1];
+    for (int i = 0; i < count; i++) h->streams[h->names_last[3 * i]].named |= 1u << h->names_last[3 * i + 1];
   }
   return download_turns(who, po, lay, h->turns.as<uint32_t>(), header_host, turns_host, turn_cap_host, n_turns, st);
 }
 
 // the named and claimed tables, on the first gallery the handle receives: every slot with nothing named or claimed
 static int gallery_tables(dg_multi* h) {
-  if (!h->named_host.empty()) return DG_OK;
+  if (h->naming) return DG_OK;
   if (h->gal_named.ensure((size_t)h->slots * 4) || h->gal_claimed.ensure((size_t)h->slots * 32 * 4)) return DG_ECUDA;
-  DG_CUDA(cudaMemsetAsync(h->gal_named.p, 0, (size_t)h->slots * 4, h->st));
-  DG_CUDA(cudaMemsetAsync(h->gal_claimed.p, 0xff, (size_t)h->slots * 32 * 4, h->st));
-  h->named_host.assign(h->slots, 0);
-  return DG_OK;
+  const int rc = clear_names(h, 0, h->slots);
+  h->naming = rc == DG_OK;
+  return rc;
 }
 
 // a gallery and threshold `who` may give a stream of h: DG_EINVAL naming what rules them out
@@ -1007,7 +1026,7 @@ extern "C" int dg_multi_set_slot_gallery(dg_multi* h, int slot, dg_gallery* g, d
     set_error(std::string(who) + ": a VAD handle has no speakers to name");
     return DG_EINVAL;
   }
-  if (!slot_ok(h, slot) || h->slot_ticked[slot]) {
+  if (!slot_ok(h, slot) || h->streams[slot].ticked) {
     set_error(std::string(who) + ": slot " + std::to_string(slot) +
               (slot_ok(h, slot) ? " has had a tick: a stream's gallery is set before its first tick" : " is not open"));
     return DG_EINVAL;
@@ -1015,23 +1034,20 @@ extern "C" int dg_multi_set_slot_gallery(dg_multi* h, int slot, dg_gallery* g, d
   int rc;
   if ((rc = check_gallery_for(h, g, threshold, who))) return rc;
   DG_CUDA(cudaSetDevice(h->device));
-  if ((rc = gallery_tables(h))) return rc;
   // the stream starts over with nothing named or claimed in its gallery
-  DG_CUDA(cudaMemsetAsync(h->gal_named.as<uint32_t>() + slot, 0, 4, h->st));
-  DG_CUDA(cudaMemsetAsync(h->gal_claimed.as<int32_t>() + (size_t)slot * 32, 0xff, 32 * 4, h->st));
-  h->named_host[slot] = 0;
-  h->slot_gal[slot] = g;
-  h->slot_thr[slot] = threshold;
+  if ((rc = gallery_tables(h)) || (rc = clear_names(h, slot, 1))) return rc;
+  h->streams[slot].gal = g;
+  h->streams[slot].thr = threshold;
   return DG_OK;
 }
 
 extern "C" int dg_multi_set_names(dg_multi* h, int slot, uint32_t named, const int32_t* claimed_host) {
   const char* who = "dg_multi_set_names";
-  if (!slot_ok(h, slot) || vad_mode(h) || !h->slot_gal[slot] || !claimed_host) {
+  if (!slot_ok(h, slot) || vad_mode(h) || !h->streams[slot].gal || !claimed_host) {
     set_error(std::string(who) + ": need an open slot with a gallery and a non-null table");
     return DG_EINVAL;
   }
-  const int M = h->M, G = h->slot_gal[slot]->G;
+  const int M = h->M, G = h->streams[slot].gal->G;
   std::vector<int32_t> row(32, -1);
   for (int g = 0; g < M; g++) {
     const int e = claimed_host[g];
@@ -1051,7 +1067,7 @@ extern "C" int dg_multi_set_names(dg_multi* h, int slot, uint32_t named, const i
   DG_CUDA(cudaSetDevice(h->device));
   DG_CUDA(cudaMemcpyAsync(h->gal_named.as<uint32_t>() + slot, &named, 4, cudaMemcpyHostToDevice, h->st));
   DG_CUDA(cudaMemcpyAsync(h->gal_claimed.as<int32_t>() + (size_t)slot * 32, row.data(), 32 * 4, cudaMemcpyHostToDevice, h->st));
-  h->named_host[slot] = named;
+  h->streams[slot].named = named;
   return DG_OK;
 }
 
@@ -1151,13 +1167,27 @@ static XferDev xfer_dev(const dg_multi* h) {
   d.rings = h->rings.as<uint32_t>(); d.yrings = h->yrings.as<uint32_t>();
   d.hist_seg = h->hist_seg.as<uint32_t>(); d.hist_map = h->hist_map.as<uint32_t>(); d.hist_vad = h->hist_vad.as<uint32_t>();
   d.centers = h->centers.as<uint32_t>(); d.active = h->active.as<uint32_t>(); d.init = h->init.as<uint32_t>();
-  if (!h->named_host.empty()) {
+  if (h->naming) {
     d.named = h->gal_named.as<uint32_t>();
     d.claimed = h->gal_claimed.as<uint32_t>();
   }
   d.C = h->book.C;
   d.Y = h->Y;
   return d;
+}
+
+// The one mapping between a stream's slot (its values x, its audio counters a) and the head of its packed state: to_head
+// fills hd from (x, a), else (x, a) from hd.  The gallery is the caller's (x.gal); without one, no threshold travels.  A
+// restored stream's history is copy 0 (x.cur as given).
+static void xfer_map(XferHead& hd, SlotStream& x, SlotAudio& a, bool to_head) {
+  auto map = [to_head](auto& field, auto& value) {
+    if (to_head) field = value; else value = field;
+  };
+  map(hd.nw, x.nw); map(hd.n_hist, x.n_hist);
+  map(hd.params[0], x.par[0]); map(hd.params[1], x.par[1]); map(hd.params[2], x.par[2]);
+  map(hd.threshold, x.thr); map(hd.ticked, x.ticked); map(hd.named, x.named);
+  map(hd.wpos, a.wpos); map(hd.rpos, a.rpos); map(hd.done, a.done);
+  if (!x.gal) (to_head ? hd.threshold : x.thr) = 0.0;
 }
 
 // the head of open slot s (init words: the device's, filled in by the gather)
@@ -1172,18 +1202,14 @@ static XferHead xfer_head(const dg_multi* h, int s) {
     hd.rs_o = r.g.o; hd.rs_n = r.g.n; hd.rs_w = r.g.w;
   }
   hd.chunk = r.S; hd.step = r.hop;
-  hd.nw = h->slot_nw[s];
-  hd.n_hist = h->n_hist[s];
-  hd.named = h->named_host.empty() ? 0 : h->named_host[s];
-  hd.gallery_G = h->slot_gal[s] ? h->slot_gal[s]->G : 0;
-  hd.ticked = h->slot_ticked[s];
-  hd.wpos = h->book.wpos[s]; hd.rpos = h->book.rpos[s]; hd.done = h->book.done[s];
+  SlotStream x = h->streams[s];
+  SlotAudio a = h->book.audio[s];
+  xfer_map(hd, x, a, true);
+  hd.gallery_G = x.gal ? x.gal->G : 0;
   if (r.resampled()) {   // frames computed that a future window still reads
     hd.frame0 = hd.rpos / r.g.o + r.r_lo;
     hd.n_frames = std::max<int64_t>(0, hd.done - hd.frame0);
   }
-  memcpy(hd.params, &h->slot_par[3 * (size_t)s], 24);
-  hd.threshold = h->slot_gal[s] ? h->slot_thr[s] : 0.0;
   hd.gamma = h->net.gamma; hd.beta = h->net.beta; hd.normalize = h->net.normalize_weights;
   hd.bytes = (int64_t)xfer_layout(hd).bytes;
   return hd;
@@ -1222,7 +1248,7 @@ static void xfer_pieces(const XferDev& d, const RateGeom& r, int slots, int nw, 
 struct StagedBySlot {
   std::vector<int> off, idx;   // slot s: pieces idx [off[s], off[s + 1]) of book.pieces, in push (= stream) order
   std::vector<long long> n;    // slot s: its staged samples
-  explicit StagedBySlot(const SlotBook& b) : off(b.open.size() + 1, 0), idx(b.pieces.size()), n(b.open.size(), 0) {
+  explicit StagedBySlot(const SlotBook& b) : off(b.audio.size() + 1, 0), idx(b.pieces.size()), n(b.audio.size(), 0) {
     for (const RingPiece& p : b.pieces) {
       off[p.slot + 1]++;
       n[p.slot] += p.n;
@@ -1245,7 +1271,7 @@ static void xfer_finish(const dg_multi* h, int s, const XferHead& head, const fl
     const RingPiece& p = h->book.pieces[sb.idx[q]];
     memcpy(out + L.audio + (size_t)(p.dst - hd.rpos) * 4, stage + p.src, (size_t)p.n * 4);
   }
-  if (hd.kind == 0 && h->named_host.empty()) memset(out + L.claimed, 0xff, 32 * 4);
+  if (hd.kind == 0 && !h->naming) memset(out + L.claimed, 0xff, 32 * 4);
   const size_t vad = hd.kind == 1, FK = (size_t)hd.F * (vad ? 1 : hd.K);
   const size_t used[][2] = {{sizeof(XferHead), L.audio},
                             {L.audio + (size_t)(hd.wpos - hd.rpos) * 4, L.frames},
@@ -1349,21 +1375,13 @@ static int xfer_check(const dg_multi* h, const XferHead& hd, const unsigned char
   return DG_OK;
 }
 
-// the stream of state hd (checked) opens in free slot t: host bookkeeping only
-static void xfer_open(dg_multi* h, int t, int rid, const XferHead& hd, dg_gallery* g) {
-  h->book.start(t, rid + 1);
-  h->book.wpos[t] = hd.wpos;
-  h->book.rpos[t] = hd.rpos;
-  h->book.done[t] = hd.done;
-  h->cur[t] = 0;
-  h->n_hist[t] = hd.n_hist;
-  h->slot_nw[t] = hd.nw;
-  memcpy(&h->slot_par[3 * (size_t)t], hd.params, 24);
-  h->slot_gal[t] = g;
-  h->slot_thr[t] = g ? hd.threshold : 0.0;
-  h->slot_ticked[t] = hd.ticked;
-  if (!h->named_host.empty()) h->named_host[t] = hd.named;
-  h->opened = true;
+// the stream of state hd (checked) opens in free slot t at declared rate rid, named from g: host bookkeeping only
+static void xfer_open(dg_multi* h, int t, int rid, XferHead hd, dg_gallery* g) {
+  SlotStream x;
+  x.gal = g;
+  SlotAudio a{rid + 1};
+  xfer_map(hd, x, a, false);
+  stream_begin(h, t, x, a);
 }
 
 // consecutive states [a0, a1) of one round: as many as fit XFER_STAGING, at least one
@@ -1422,8 +1440,8 @@ extern "C" int dg_multi_export(dg_multi* h, const int32_t* slots, int n, int clo
     std::vector<XferPiece> pc;
     for (int a = a0; a < a1; a++) {
       const int s = slots[a];
-      xfer_pieces(d, h->book.geom(s), h->slots, h->nw, s, h->cur[s], hd[a], h->xfer.as<uint32_t>() + (off[a] - off[a0]) / 4,
-                  hd[a].wpos - hd[a].rpos - sb.n[s], true, pc);
+      xfer_pieces(d, h->book.geom(s), h->slots, h->nw, s, h->streams[s].cur, hd[a],
+                  h->xfer.as<uint32_t>() + (off[a] - off[a0]) / 4, hd[a].wpos - hd[a].rpos - sb.n[s], true, pc);
     }
     unsigned char* pin = h->xfer_pin.as<unsigned char>();
     memcpy(pin + o_desc, pc.data(), pc.size() * sizeof(XferPiece));
@@ -1448,10 +1466,7 @@ extern "C" int dg_multi_export(dg_multi* h, const int32_t* slots, int n, int clo
     }
   }
   if (close)
-    for (int a = 0; a < n; a++) {
-      h->book.stop(slots[a]);
-      h->slot_gal[slots[a]] = nullptr;
-    }
+    for (int a = 0; a < n; a++) stream_end(h, slots[a]);
   return DG_OK;
 }
 
@@ -1480,7 +1495,7 @@ extern "C" int dg_multi_import(dg_multi* h, const void* blob_host, int64_t blob_
     off[a + 1] = off[a] + bytes[a];
   }
   for (int a = 0, s = 0; a < n; a++, s++) {   // the lowest free slots
-    while (s < h->slots && h->book.open[s]) s++;
+    while (s < h->slots && h->book.audio[s].open) s++;
     if (s == h->slots) {
       set_error(std::string(who) + ": " + std::to_string(n) + " states, fewer free slots");
       return DG_EINVAL;
@@ -1534,11 +1549,7 @@ extern "C" int dg_selftest_multi_frames_host(int slots, int max_wps, int out_chu
     return DG_EINVAL;
   }
   SlotBook book;
-  RateGeom base;
-  base.S = out_chunk;
-  base.hop = out_step;
-  base.cap = (int)ring_capacity(out_chunk, out_step, max_wps);
-  book.init(slots, base);
+  book.init(slots, pipeline_rate(out_chunk, out_step, max_wps));
   for (int i = 0; i < n_rates; i++) {
     const int32_t* q = rates + 5 * i;
     RsGeom g{q[0], q[1], q[2], 2 * q[2] + q[0]};
@@ -1565,8 +1576,8 @@ extern "C" int dg_selftest_multi_frames_host(int slots, int max_wps, int out_chu
     const int kind = ops[3 * i], slot = ops[3 * i + 1], n = ops[3 * i + 2];
     int rc = DG_OK;
     if (kind == 0) {
-      if (slot < 0 || slot >= slots || book.open[slot] || n < -1 || n + 1 >= (int)book.rates.size()) rc = DG_EINVAL;
-      else book.start(slot, n + 1);
+      if (slot < 0 || slot >= slots || book.audio[slot].open || n < -1 || n + 1 >= (int)book.rates.size()) rc = DG_EINVAL;
+      else book.start(slot, SlotAudio{n + 1});
     } else if (kind == 1) {
       if (!book.ok(slot)) rc = DG_EINVAL;
       else book.stop(slot);
@@ -1610,7 +1621,7 @@ extern "C" int dg_selftest_multi_staging_host(int slots, int C, int n_ops, const
     const int kind = ops[3 * i], slot = ops[3 * i + 1], n = ops[3 * i + 2];
     int rc = DG_OK;
     if (kind == 0) {
-      if (slot < 0 || slot >= slots || book.open[slot]) rc = DG_EINVAL;
+      if (slot < 0 || slot >= slots || book.audio[slot].open) rc = DG_EINVAL;
       else book.start(slot);
     } else if (kind == 1) {
       if (!book.ok(slot)) rc = DG_EINVAL;
@@ -1624,8 +1635,8 @@ extern "C" int dg_selftest_multi_staging_host(int slots, int C, int n_ops, const
       }
       if (n > 0) next += n;                   // a refused block is skipped in the sample stream too
     } else if (kind == 3) {
-      if (!book.ok(slot) || n < 0 || book.rpos[slot] + n > book.wpos[slot]) rc = DG_EINVAL;
-      else book.rpos[slot] += n;
+      if (!book.ok(slot) || n < 0 || book.audio[slot].rpos + n > book.audio[slot].wpos) rc = DG_EINVAL;
+      else book.audio[slot].rpos += n;
     } else if (kind == 4) {
       for (const RingPiece& p : book.pieces)   // what ring_scatter_kernel writes
         for (int k = 0; k < p.n; k++) rings_host[(size_t)p.slot * C + (p.dst + k) % C] = staged[p.src + k];
@@ -1709,14 +1720,10 @@ extern "C" int dg_selftest_multi_gallery_host(int slots, int D, int M, int n_gal
     gals[i].device = gal[3 * i + 2];
   }
   dg_multi h;
-  h.slots = slots;
+  multi_init(h, 0, slots, 1, 0, 1, 0, 0, 1);   // no audio: the ops never reach it
   h.D = D;
   h.M = M;
   h.net.emb = reinterpret_cast<dg_emb*>(&h);   // a diarization handle (never dereferenced here)
-  h.book.init(slots, RateGeom{});
-  h.slot_gal.assign(slots, nullptr);
-  h.slot_thr.assign(slots, 0.0);
-  h.slot_ticked.assign(slots, 0);
   std::string text;
   for (int i = 0; i < n_ops; i++) {
     const int kind = (int)ops[4 * i], slot = (int)ops[4 * i + 1], arg = (int)ops[4 * i + 2];
@@ -1724,22 +1731,20 @@ extern "C" int dg_selftest_multi_gallery_host(int slots, int D, int M, int n_gal
     const bool in_range = slot >= 0 && slot < slots;
     int rc = DG_OK;
     set_error("");
-    if (kind == 0 && in_range && !h.book.open[slot]) {
-      h.book.start(slot);
-      h.slot_gal[slot] = nullptr;
-      h.slot_ticked[slot] = 0;
+    if (kind == 0 && in_range && !h.book.audio[slot].open) {
+      stream_begin(&h, slot, SlotStream{}, SlotAudio{});
     } else if (kind == 1 && arg >= -1 && arg < n_gal) {
       rc = dg_multi_set_slot_gallery(&h, slot, arg < 0 ? nullptr : &gals[arg], x);
     } else if (kind == 2 && in_range && arg >= 0 && arg < n_gal) {
-      h.slot_gal[slot] = &gals[arg];
+      h.streams[slot].gal = &gals[arg];
     } else if (kind == 3) {
       std::vector<int32_t> claimed((size_t)M, -1);
       claimed[0] = (int32_t)x;
       rc = dg_multi_set_names(&h, slot, (uint32_t)arg, claimed.data());
     } else if (kind == 4 && in_range) {
-      h.slot_ticked[slot] = 1;
-    } else if (kind == 5 && in_range && h.book.open[slot]) {
-      h.book.stop(slot);
+      h.streams[slot].ticked = true;
+    } else if (kind == 5 && in_range && h.book.audio[slot].open) {
+      stream_end(&h, slot);
     } else {
       rc = DG_EINVAL;
       set_error(std::string(who) + ": op " + std::to_string(i) + " is not valid");
@@ -1784,12 +1789,8 @@ extern "C" int dg_selftest_multi_transfer_host(const int32_t* geom, int n_ops, c
   };
   auto make = [&](Side& x, int slots, int max_wps, int nw) -> int {
     dg_multi& h = x.h;
-    h.slots = slots; h.max_wps = max_wps; h.S = geom[3]; h.hop = geom[4]; h.F = F; h.K = 1; h.M = 1; h.nw = nw;
-    RateGeom base;
-    base.S = geom[3];
-    base.hop = geom[4];
-    base.cap = (int)ring_capacity(geom[3], geom[4], max_wps);
-    h.book.init(slots, base);
+    multi_init(h, 0, slots, max_wps, geom[3], geom[4], F, 1, nw);
+    h.M = 1;
     if (geom[6] > 0) {
       RsGeom g{geom[6], geom[7], geom[8], 2 * geom[8] + geom[6]};
       RateGeom r;
@@ -1798,8 +1799,6 @@ extern "C" int dg_selftest_multi_transfer_host(const int32_t* geom, int n_ops, c
       h.book.add_rate(r);
       h.Y = r.Q * r.g.n;
     }
-    h.n_hist.assign(slots, 0); h.cur.assign(slots, 0); h.slot_nw.assign(slots, nw); h.slot_par.assign(3 * (size_t)slots, 0.5);
-    h.slot_gal.assign(slots, nullptr); h.slot_thr.assign(slots, 0.0); h.slot_ticked.assign(slots, 0);
     x.rings.assign((size_t)slots * h.book.C, 0.f);
     x.yrings.assign((size_t)slots * std::max(1LL, h.Y), 0.f);
     x.hist.assign(2 * (size_t)slots * std::max(1, nw - 1) * F, 0.f);
@@ -1818,22 +1817,18 @@ extern "C" int dg_selftest_multi_transfer_host(const int32_t* geom, int n_ops, c
   Side src, dst;
   int rc;
   if ((rc = make(src, geom[0], geom[1], geom[2])) || (rc = make(dst, geom[11], geom[12], geom[13]))) return rc;
-  dg_multi& h = src.h;
-  h.net.emb = nullptr;
+  dg_multi& h = src.h;   // a VAD handle (no embedding model)
   std::vector<float> staged;
   long long next = 0;
   for (int i = 0; i < n_ops; i++) {
     const int kind = ops[3 * i], slot = ops[3 * i + 1], n = ops[3 * i + 2];
     rc = DG_OK;
     if (kind == 0) {
-      if (slot < 0 || slot >= h.slots || h.book.open[slot] || n < -1 || n + 1 >= (int)h.book.rates.size()) rc = DG_EINVAL;
-      else {
-        h.book.start(slot, n + 1);
-        h.n_hist[slot] = 0;
-      }
+      if (slot < 0 || slot >= h.slots || h.book.audio[slot].open || n < -1 || n + 1 >= (int)h.book.rates.size()) rc = DG_EINVAL;
+      else stream_begin(&h, slot, SlotStream{h.nw, 0, 0, {h.tau, 0.0, 0.0}}, SlotAudio{n + 1});   // as dg_multi_open_rate
     } else if (kind == 1) {
       if (!h.book.ok(slot)) rc = DG_EINVAL;
-      else h.book.stop(slot);
+      else stream_end(&h, slot);
     } else if (kind == 2) {
       if (!h.book.ok(slot) || n < 0 || !h.book.fits(slot, n)) rc = DG_EINVAL;
       else if (n > 0) {
@@ -1855,8 +1850,10 @@ extern "C" int dg_selftest_multi_transfer_host(const int32_t* geom, int n_ops, c
       }
       const size_t stride = (size_t)std::max(1, h.nw - 1);
       for (const TickSlot& ts : tp.act) {   // post_slots_history on the host, chunk c = the values c F + j
-        const int s = ts.slot, cur = h.cur[s], nh = h.n_hist[s], keep = std::min(h.slot_nw[s] - 1, nh + ts.n);
-        const long long c0 = h.book.rpos[s] / h.book.geom(s).hop;
+        const int s = ts.slot;
+        SlotStream& x = h.streams[s];
+        const int cur = x.cur, nh = x.n_hist, keep = std::min(x.nw - 1, nh + ts.n);
+        const long long c0 = h.book.audio[s].rpos / h.book.geom(s).hop;
         for (int e = 0; e < keep; e++) {
           const int v = ts.n - keep + e;
           float* out = &src.hist[(((size_t)(cur ^ 1) * h.slots + s) * stride + e) * F];
@@ -1864,8 +1861,8 @@ extern "C" int dg_selftest_multi_transfer_host(const int32_t* geom, int n_ops, c
             out[j] = v >= 0 ? (float)((c0 + v) * F + j) : src.hist[(((size_t)cur * h.slots + s) * stride + nh + v) * F + j];
         }
         if (h.nw > 1) {
-          h.n_hist[s] = keep;
-          h.cur[s] ^= 1;
+          x.n_hist = keep;
+          x.cur ^= 1;
         }
       }
       h.book.uploaded();
@@ -1884,7 +1881,7 @@ extern "C" int dg_selftest_multi_transfer_host(const int32_t* geom, int n_ops, c
   XferHead hd = xfer_head(&h, src_slot);
   std::vector<uint32_t> blob((size_t)hd.bytes / 4, 0);
   std::vector<XferPiece> pc;
-  xfer_pieces(src.d, h.book.geom(src_slot), h.slots, h.nw, src_slot, h.cur[src_slot], hd, blob.data(),
+  xfer_pieces(src.d, h.book.geom(src_slot), h.slots, h.nw, src_slot, h.streams[src_slot].cur, hd, blob.data(),
               hd.wpos - hd.rpos - StagedBySlot(h.book).n[src_slot], true, pc);
   run(pc);
   xfer_finish(&h, src_slot, hd, staged.data(), StagedBySlot(h.book), reinterpret_cast<unsigned char*>(blob.data()));
@@ -1895,7 +1892,7 @@ extern "C" int dg_selftest_multi_transfer_host(const int32_t* geom, int n_ops, c
     case 2: ph->kind = 0; break;
     case 3: ph->S += 4; break;
     case 4: ph->nw = t.nw + 1; break;
-    case 5: ph->wpos = ph->rpos + t.book.rates[h.book.rate[src_slot]].cap + 1; break;
+    case 5: ph->wpos = ph->rpos + t.book.rates[h.book.audio[src_slot].rate].cap + 1; break;
     case 6: ph->init[1] = 1; break;
     case 7: ph->rs_o += 1; break;
     case 8: ph->magic = 0; break;
@@ -1911,7 +1908,7 @@ extern "C" int dg_selftest_multi_transfer_host(const int32_t* geom, int n_ops, c
   const size_t m = std::min(msg.size(), (size_t)msg_cap - 1);
   memcpy(message, msg.data(), m);
   message[m] = 0;
-  const RateGeom& tr = t.book.rates[h.book.rate[src_slot]];
+  const RateGeom& tr = t.book.rates[h.book.audio[src_slot].rate];
   const RateGeom& sr = h.book.geom(src_slot);
   const int64_t row[13] = {irc, t.book.C, tr.Q, t.Y, hd.wpos, hd.rpos, hd.done, hd.n_hist, hd.frame0, hd.n_frames, hd.bytes,
                            h.book.C, sr.Q};

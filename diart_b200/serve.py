@@ -252,7 +252,7 @@ class _MultiStreamServer:
         if len(free) == 0:
             raise ValueError(f"all {self.max_streams} streams are open")
         sid = int(free[0])
-        rid, chunk, hop, res = self.rates[rate]
+        rid = self.rates[rate][0]
         with torch.cuda.device(self.device):
             if seed is None:
                 _lib.check(_lib.lib().dg_multi_open_config(self._h, sid, rid, stream_windows(lat, cfg.step),
@@ -261,12 +261,17 @@ class _MultiStreamServer:
                 seed = np.ascontiguousarray(seed, dtype=np.float64)
                 _lib.check(_lib.lib().dg_multi_open_seeded(self._h, sid, rid, stream_windows(lat, cfg.step),
                                                            params.ctypes.data, seed.ctypes.data, len(seed)))
-        self._open[sid] = True
-        self._pushed[sid] = self._emitted[sid] = 0
-        self._shift[sid] = float(shift)
-        self._chunk[sid], self._hop[sid], self._res[sid] = chunk, hop, res
-        self._latency[sid] = lat
+        self._begin(sid, rate, lat, shift, 0, 0)
         return sid
+
+    def _begin(self, sid: int, rate: int, latency: float, shift: float, pushed: int, emitted: int):
+        """the host mirror of a stream that starts in slot ``sid`` (new or restored): at source ``rate`` and ``latency``,
+        time stamps shifted by ``shift``, ``pushed`` samples pushed and ``emitted`` windows consumed so far"""
+        self._open[sid] = True
+        self._pushed[sid], self._emitted[sid] = pushed, emitted
+        self._shift[sid] = float(shift)
+        _, self._chunk[sid], self._hop[sid], self._res[sid] = self.rates[rate]
+        self._latency[sid] = latency
 
     def close(self, sid: int):
         _lib.check(_lib.lib().dg_multi_close(self._h, int(sid)))
@@ -302,12 +307,7 @@ class _MultiStreamServer:
     def _restored(self, sid: int, state: StreamState, gallery):
         """the host mirror of a slot a state was restored into"""
         meta = state._meta
-        rid, chunk, hop, res = self.rates[meta["rate"]]
-        self._open[sid] = True
-        self._pushed[sid], self._emitted[sid] = meta["pushed"], meta["emitted"]
-        self._shift[sid] = meta["shift"]
-        self._chunk[sid], self._hop[sid], self._res[sid] = chunk, hop, res
-        self._latency[sid] = meta["latency"]
+        self._begin(sid, meta["rate"], meta["latency"], meta["shift"], meta["pushed"], meta["emitted"])
 
     def export(self, sids, *, close: bool = True) -> List[StreamState]:
         """the whole state of each open stream in ``sids`` after the last tick, its samples pushed since then included, in
@@ -519,10 +519,8 @@ class MultiStreamDiarization(_MultiStreamServer):
                 raise ValueError(f"{len(known)} known speakers, at most max_speakers = {self._speakers}")
         sid = _MultiStreamServer._open_stream(self, shift, sample_rate, latency, None if known is None else known.centroids,
                                               tau_active=tau_active, rho_update=rho_update, delta_new=delta_new)
-        self._own_labels[sid] = known is not None
-        self._stream_labels[sid] = self.labels if known is None else speaker_labels(known, self._speakers)
-        self._slot_gallery[sid] = gal = self.gallery if gallery is None else gallery
-        self._naming = self._naming or gal is not None
+        gal = self.gallery if gallery is None else gallery
+        self._named_by(sid, None if known is None else speaker_labels(known, self._speakers), gal)
         try:
             with torch.cuda.device(self.device):
                 if gallery is not None:
@@ -534,6 +532,14 @@ class MultiStreamDiarization(_MultiStreamServer):
             self.close(sid)
             raise
         return sid
+
+    def _named_by(self, sid: int, labels: Optional[List[str]], gallery: Optional[SpeakerGallery]):
+        """the labels of the stream that starts in slot ``sid`` (None: the server's) and the gallery it is named from
+        (None: none)"""
+        self._own_labels[sid] = labels is not None
+        self._stream_labels[sid] = self.labels if labels is None else list(labels)
+        self._slot_gallery[sid] = gallery
+        self._naming = self._naming or gallery is not None
 
     _kind = "diarization"
 
@@ -577,11 +583,7 @@ class MultiStreamDiarization(_MultiStreamServer):
 
     def _restored(self, sid, state, gallery):
         _MultiStreamServer._restored(self, sid, state, gallery)
-        labels = state._meta["labels"]
-        self._own_labels[sid] = labels is not None
-        self._stream_labels[sid] = self.labels if labels is None else list(labels)
-        self._slot_gallery[sid] = gallery
-        self._naming = self._naming or gallery is not None
+        self._named_by(sid, state._meta["labels"], gallery)
 
     def speakers(self, sid: int) -> KnownSpeakers:
         """the clustering state of open stream ``sid`` after the last tick: its active centres in index order (a prefix
