@@ -36,6 +36,9 @@ SIGNATURES = {
     "dg_selftest_gemm_tc_bounds": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
                                              C.POINTER(C.c_int)]),
     "dg_selftest_wgmma_row_shift": (C.c_int, [C.c_int, C.POINTER(C.c_uint)]),
+    "dg_selftest_wgmma_b_row_shift": (C.c_int, [C.c_int, C.POINTER(C.c_uint)]),
+    "dg_selftest_gemm_tc_pool3_simt": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float),
+                                                 C.POINTER(C.c_float), C.POINTER(C.c_int)]),
     "dg_selftest_gemm_tc_halo": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int),
                                            C.POINTER(C.c_int)]),
     "dg_selftest_split_f16_host": (C.c_int, [_P, C.c_longlong, _P, _P]),

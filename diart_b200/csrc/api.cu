@@ -331,6 +331,77 @@ extern "C" int dg_selftest_wgmma_row_shift(int base_offset_mode, unsigned* ok_sh
   return selftest_wgmma_row_shift(base_offset_mode, ok_shifts) ? DG_ECUDA : DG_OK;
 }
 
+// Sets bit r of *ok_shifts when a wgmma whose B descriptor starts r = 0..8 rows into a 64B-swizzled TMA tile computes the
+// exact product with rows r..r+63 (the weight-stationary MaxPool3 kernel's time rows); base_offset_mode as above.
+extern "C" int dg_selftest_wgmma_b_row_shift(int base_offset_mode, unsigned* ok_shifts) {
+  if (base_offset_mode < 0 || base_offset_mode > 1 || !ok_shifts) {
+    set_error("dg_selftest_wgmma_b_row_shift: bad arguments");
+    return DG_EINVAL;
+  }
+  return selftest_wgmma_b_row_shift(base_offset_mode, ok_shifts) ? DG_ECUDA : DG_OK;
+}
+
+// Runs one seeded Conv1d with the MaxPool1d(3) epilogue (epilogue 5, items of 888 rows, M a multiple of them) through
+// launch_gemm_tc, and the same convolution through the float32 reference GEMM (gemm.cu) pooled on the host; reports the
+// largest absolute difference of the pooled rows and their scale.  *ws = 1 if the launch took the weight-stationary kernel.
+extern "C" int dg_selftest_gemm_tc_pool3_simt(int M, int Cin, int KW, int dil, int N, float* max_abs_diff, float* out_rms,
+                                              int* ws) {
+  if (M < 888 || M % 888 || Cin < 16 || Cin % 16 || Cin > 128 || KW < 2 || KW > 9 || dil < 1 || N < 1 || N > 64 || N % 4 ||
+      !max_abs_diff || !out_rms || !ws) {
+    set_error("dg_selftest_gemm_tc_pool3_simt: bad arguments");
+    return DG_EINVAL;
+  }
+  const int K = KW * Cin, item_rows = 888, tile_rows = gemm_tc_pool3_tile_rows(item_rows);
+  const long long m_tiles = (M + tile_rows - 1) / tile_rows, tail = (long long)(KW - 1) * dil;
+  uint32_t seed = 4242u;
+  auto rnd = [&]() {
+    seed = seed * 1664525u + 1013904223u;
+    return ((seed >> 8) & 0xFFFF) / 65536.f - 0.5f;
+  };
+  // the reference reads KW - 1 taps past M: zero rows, as TMA fills them
+  std::vector<float> A((size_t)(M + tail) * Cin, 0.f), Wkn((size_t)K * N), Wnk((size_t)N * K), bias(N);
+  for (size_t i = 0; i < (size_t)M * Cin; i++) A[i] = 2.f * rnd();
+  for (int k = 0; k < K; k++)
+    for (int n = 0; n < N; n++) Wkn[(size_t)k * N + n] = Wnk[(size_t)n * K + k] = 0.25f * rnd();
+  for (auto& v : bias) v = rnd();
+  DevBuf dA, dWkn, dB, dAh, dAl, dC0, dP, dPart;
+  WeightPlanes dW;
+  if (upload(dA, A) || upload(dWkn, Wkn) || upload(dB, bias) || upload_split(dW, Wnk, N, 64, K)) return DG_ECUDA;
+  if (dAh.ensure((size_t)M * Cin * 2) || dAl.ensure((size_t)M * Cin * 2) || dC0.ensure((size_t)M * N * 4) ||
+      dP.ensure((size_t)(M / 3) * N * 4) || dPart.ensure((size_t)m_tiles * 2 * TC_POOL3_SLOTS * N * 4))
+    return DG_ECUDA;
+  int rc;
+  GemmArgs g{};
+  g.A = dA.as<float>(); g.lda = Cin; g.Cin = Cin; g.KW = KW; g.dil = dil; g.Mtot = M + tail; g.M = M;
+  g.W = dWkn.as<float>(); g.ldw = N; g.N = N; g.bias = dB.as<float>(); g.C = dC0.as<float>(); g.ldc = N; g.epi = EPI_BIAS;
+  g.tag = "selftest_simt";
+  if ((rc = launch_gemm(g, nullptr))) return rc;
+  if ((rc = launch_split_ex(dA.as<float>(), M, Cin, Cin, Cin, 0, 1, nullptr, nullptr, dAh.p, dAl.p, nullptr))) return rc;
+  TcGemm t{};
+  t.A_hi = dAh.p; t.A_lo = dAl.p; t.lda = Cin; t.Cin = Cin; t.KW = KW; t.dil = dil; t.Mtot = M; t.M = M;
+  t.N = N; t.bias = dB.as<float>(); t.out_f32 = dP.as<float>(); t.ldc = N; t.epi = 5; t.tag = "selftest_tc_pool3";
+  t.pool_part = dPart.as<float>(); t.pool_item_rows = item_rows; t.pool3_T = item_rows / 3 - 2; t.pool3_tile_rows = tile_rows;
+  if ((rc = set_weights(t, dW))) return rc;
+  *ws = gemm_tc_ws(t) ? 1 : 0;
+  if ((rc = launch_gemm_tc(t, nullptr))) return rc;
+  DG_CUDA(cudaDeviceSynchronize());
+  std::vector<float> c0((size_t)M * N), p1((size_t)(M / 3) * N);
+  DG_CUDA(cudaMemcpy(c0.data(), dC0.p, c0.size() * 4, cudaMemcpyDeviceToHost));
+  DG_CUDA(cudaMemcpy(p1.data(), dP.p, p1.size() * 4, cudaMemcpyDeviceToHost));
+  double md = 0, ss = 0;
+  for (long long r = 0; r < M / 3; r++)
+    for (int n = 0; n < N; n++) {
+      const float* x = &c0[(size_t)(3 * r) * N + n];
+      const double ref = std::max(std::max(x[0], x[N]), x[2 * N]);
+      const double d = fabs(ref - (double)p1[(size_t)r * N + n]);
+      if (!(d <= md)) md = d;     // NaN-propagating max
+      ss += ref * ref;
+    }
+  *max_abs_diff = (float)md;
+  *out_rms = (float)sqrt(ss / p1.size());
+  return DG_OK;
+}
+
 // Runs one seeded Conv1d GEMM (epilogue 0, 1, 2 or 5) through the halo operand mode, under no SM cap and under a cap of 3
 // SMs, and through the tap-box mode, and sets *equal = 1 if all three wrote the same bytes: float32 rows, hi/lo planes,
 // pooling partial sums.  A Cin that is not a multiple of 64 (SincNet's 80) has no tap-box form: the reference then reads

@@ -302,6 +302,66 @@ __device__ __forceinline__ void tc_conv2d_epilogue_tile(const TcArgs& a, const f
     }
 }
 
+// ------------------------------------------------------------------------------------ MaxPool1d(3) of 32 columns of a tile
+// bias + MaxPool1d(3) over the rows of the m-tile `mt` (tile_rows / 3 windows of three rows), and the InstanceNorm partial
+// sums of the pooled values, split at `brow3` between the tile's two items.  `dsm` = the tile's 32 accumulator columns
+// [row][33] after the weight scale, `bias_c` = theirs, `nc` = the first one's output channel, `stg` = [rg 4][item 2][2][32].
+// Executed by the 128 threads of a consumer warpgroup: thread (rg, col) = (et / 32, et % 32) pools windows rg, rg + 4, ...
+// of column col; `bar` = the warpgroup's named barrier.  Ends with a barrier: dsm and stg may be rewritten.
+// STG_IN_DSM: stg may overlap dsm (one more barrier: every thread is past its reads of dsm before stg is written).
+template <bool STG_IN_DSM = false>
+__device__ __forceinline__ void tc_maxpool3_cols(const TcArgs& a, const float* dsm, float* stg, const float* bias_c,
+                                                 long long mt, int nc, int et, int bar) {
+  {
+    const int col = et & 31, rg = et >> 5, n = nc + col;
+    const long long first = mt * (long long)a.tile_rows;                  // first un-pooled row of the tile
+    const long long item0 = first / a.pool_item_rows;
+    const long long nxt = (item0 + 1) * a.pool_item_rows;
+    const int brow3 = nxt - first < a.tile_rows ? (int)(nxt - first) / 3 : a.tile_rows / 3;   // first window of the next item
+    const long long p_first = first / 3;                                  // first pooled row of the tile
+    const int f0 = (int)(p_first - item0 * (a.pool_item_rows / 3));       // its frame index inside item0
+    const long long Mp = a.M / 3;
+    const float bias = bias_c[col];
+    // the sums are taken around the pooled value of the item's first window in the tile (`piv`)
+    auto pooled = [&](int pr) {
+      return fmaxf(fmaxf(dsm[(3 * pr) * 33 + col], dsm[(3 * pr + 1) * 33 + col]), dsm[(3 * pr + 2) * 33 + col]);
+    };
+    const float piv0 = pooled(0), piv1 = pooled(brow3 < a.tile_rows / 3 ? brow3 : 0);
+    float s1[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};
+    for (int pr = rg; pr < a.tile_rows / 3; pr += 4) {
+      const float v = pooled(pr);
+      const int sg = pr >= brow3 ? 1 : 0;
+      const int frame = sg ? pr - brow3 : f0 + pr;
+      const long long P = p_first + pr;
+      if (P < Mp) {
+        if (n < a.N) a.out_f32[P * a.ldc + n] = v + bias;
+        if (frame < a.pool3_T) {
+          const float dv = v - (sg ? piv1 : piv0);
+          s1[sg] += dv;
+          s2[sg] = fmaf(dv, dv, s2[sg]);
+        }
+      }
+    }
+    if (STG_IN_DSM) named_sync(bar, 128);
+#pragma unroll
+    for (int sg = 0; sg < 2; sg++) {
+      stg[((rg * 2 + sg) * 2 + 0) * 32 + col] = s1[sg];
+      stg[((rg * 2 + sg) * 2 + 1) * 32 + col] = s2[sg];
+    }
+    if (rg == 0 && n < a.N)
+#pragma unroll
+      for (int sg = 0; sg < 2; sg++) a.pool_part[(((size_t)mt * 2 + sg) * TC_POOL3_SLOTS + 2) * a.N + n] = sg ? piv1 : piv0;
+  }
+  named_sync(bar, 128);
+  {   // 2 items x 2 sums x 32 columns = 128 values, one per thread: the four row groups in a fixed order
+    const int col = et & 31, q = et >> 5, sg = q >> 1, j = q & 1, n = nc + col;
+    const float tot = ((stg[((0 * 2 + sg) * 2 + j) * 32 + col] + stg[((1 * 2 + sg) * 2 + j) * 32 + col]) +
+                       stg[((2 * 2 + sg) * 2 + j) * 32 + col]) + stg[((3 * 2 + sg) * 2 + j) * 32 + col];
+    if (n < a.N) a.pool_part[(((size_t)mt * 2 + sg) * TC_POOL3_SLOTS + j) * a.N + n] = tot;
+  }
+  named_sync(bar, 128);     // stg and dsm are rewritten next
+}
+
 // ------------------------------------------------------------------------------------ the pooling epilogue of one 128-row tile
 // Executed by the 128 threads of a consumer warpgroup; thread et = 32 quad + lane owns row et of the tile.  `mt` = index
 // of the 128-row tile (rows mt * 128 ..), `acc` = the finished accumulator in registers, `bar` = the warpgroup's named
@@ -454,57 +514,7 @@ __device__ __forceinline__ void tc_pool_epilogue_tile(const TcArgs& a, float* pa
           continue;
         }
         if (EPI == TC_MAXPOOL3) {
-          // bias + MaxPool1d(3) over the rows of the tile (42 windows of three rows: through shared memory), and the
-          // InstanceNorm partial sums of the pooled values, split at `brow3` between the tile's two items
-          const float* dsm = chunk + (c - c0) / 32 * (128 * 33);   // [128][33]
-          float* stg = pool_stage;                    // [rg 4][item 2][2][32]
-          {
-            const int col = et & 31, rg = et >> 5, n = n0 + c + col;
-            const long long first = mt * (long long)a.tile_rows;                  // first un-pooled row of the tile
-            const long long item0 = first / a.pool_item_rows;
-            const long long nxt = (item0 + 1) * a.pool_item_rows;
-            const int brow3 = nxt - first < a.tile_rows ? (int)(nxt - first) / 3 : a.tile_rows / 3;   // first window of the next item
-            const long long p_first = first / 3;                                  // first pooled row of the tile
-            const int f0 = (int)(p_first - item0 * (a.pool_item_rows / 3));       // its frame index inside item0
-            const long long Mp = a.M / 3;
-            const float bias = params[c + col];
-            // the sums are taken around the pooled value of the item's first window in the tile (`piv`)
-            auto pooled = [&](int pr) {
-              return fmaxf(fmaxf(dsm[(3 * pr) * 33 + col], dsm[(3 * pr + 1) * 33 + col]), dsm[(3 * pr + 2) * 33 + col]);
-            };
-            const float piv0 = pooled(0), piv1 = pooled(brow3 < a.tile_rows / 3 ? brow3 : 0);
-            float s1[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};
-            for (int pr = rg; pr < a.tile_rows / 3; pr += 4) {
-              const float v = pooled(pr);
-              const int sg = pr >= brow3 ? 1 : 0;
-              const int frame = sg ? pr - brow3 : f0 + pr;
-              const long long P = p_first + pr;
-              if (P < Mp) {
-                if (n < a.N) a.out_f32[P * a.ldc + n] = v + bias;
-                if (frame < a.pool3_T) {
-                  const float dv = v - (sg ? piv1 : piv0);
-                  s1[sg] += dv;
-                  s2[sg] = fmaf(dv, dv, s2[sg]);
-                }
-              }
-            }
-#pragma unroll
-            for (int sg = 0; sg < 2; sg++) {
-              stg[((rg * 2 + sg) * 2 + 0) * 32 + col] = s1[sg];
-              stg[((rg * 2 + sg) * 2 + 1) * 32 + col] = s2[sg];
-            }
-            if (rg == 0 && n < a.N)
-#pragma unroll
-              for (int sg = 0; sg < 2; sg++) a.pool_part[(((size_t)mt * 2 + sg) * TC_POOL3_SLOTS + 2) * a.N + n] = sg ? piv1 : piv0;
-          }
-          named_sync(bar, 128);
-          {   // 2 items x 2 sums x 32 columns = 128 values, one per thread: the four row groups in a fixed order
-            const int col = et & 31, q = et >> 5, sg = q >> 1, j = q & 1, n = n0 + c + col;
-            const float tot = ((stg[((0 * 2 + sg) * 2 + j) * 32 + col] + stg[((1 * 2 + sg) * 2 + j) * 32 + col]) +
-                               stg[((2 * 2 + sg) * 2 + j) * 32 + col]) + stg[((3 * 2 + sg) * 2 + j) * 32 + col];
-            if (n < a.N) a.pool_part[(((size_t)mt * 2 + sg) * TC_POOL3_SLOTS + j) * a.N + n] = tot;
-          }
-          named_sync(bar, 128);     // stg (and after the last 32 columns the chunk buffer) is rewritten next
+          tc_maxpool3_cols(a, chunk + (c - c0) / 32 * (128 * 33), pool_stage, params + c, mt, n0 + c, et, bar);
           continue;
         }
       }
@@ -812,6 +822,183 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
   if (tc_box_store(EPI) && et == 0) bulk_wait_all();
 }
 
+// ------------------------------------------------------------------------------------ the weight-stationary MaxPool3 kernel
+// TC_MAXPOOL3 for Conv1d over few channels (SincNet's conv1 and conv2) with the operands swapped: D^T = W . X^T.  The A
+// operand is W, its 64 (padded) output channels one m64; the B operand is the tile's halo, N = TCW_N time rows, so one MMA
+// covers a tile of up to 112 rows (tile_rows = 111 for SincNet) instead of 128 for 111.  W, hi and lo, goes to shared
+// memory once per CTA and stays there for every tile: nothing streams through a ring, and the producer only loads halos.
+// The halo slots are the same 64B-swizzled [hi | lo][ceil(cin / 32)] boxes as in gemm_tc_kernel<.., true>, and the B
+// descriptor of each k16 step starts its tap's offset rows into the slot (dg_selftest_wgmma_b_row_shift).
+// Per output element the products and their order are those of gemm_tc_kernel: k16 steps tap outer, 16 channels inner,
+// lo.hi, hi.lo, hi.hi per step; a K of an odd number of k16 steps runs no zero step at the end, which adds nothing.
+// The accumulator fragment (tc_ptx.cuh) is transposed: acc[4 j + e] is output channel 16 quad + lane / 4 + 8 (e / 2), tile
+// row 8 j + 2 (lane % 4) + e % 2.  The epilogue stages it 32 channels at a time as [row][33] and pools it with the tap-box
+// kernel's code, so the pooled rows and the InstanceNorm partials are bit-identical.  Each consumer has its own staging
+// chunk, so the two epilogues may run at once (the epilogue of a tile takes longer than its MMAs); to fit one per consumer
+// next to 104 KB of W (conv1) and two halo slots, the cross-row-group sums are staged in the chunk itself once it has been
+// read, and the bias is staged once for both.
+constexpr int TCW_N = 112;
+struct TcWsSmem {
+  static constexpr int W_BOX = 64 * TC_BK * 2;                          // 64 channels x 32 k of one plane: 4 KB
+  static constexpr int BAR_BYTES = 128;
+  static constexpr int CHUNK_FLOATS = TCW_N * 33;                      // [112][33]; then the [4][2][2][32] sums
+  static constexpr int STAGE_FLOATS = 64 + 2 * CHUNK_FLOATS;            // bias | consumer 0's chunk | consumer 1's chunk
+  __host__ static int halo_rows(int KW, int dil) { return (TCW_N + (KW - 1) * dil + 7) / 8 * 8; }
+  __host__ static int w_plane_bytes(int K) { return (K + TC_BK - 1) / TC_BK * W_BOX; }
+  // [W hi][W lo][halo slot 0][halo slot 1][barriers][epilogue staging]
+  __host__ static int op_bytes(int cin, int KW, int dil) {
+    return 2 * w_plane_bytes(KW * cin) + 2 * TcSmem<64>::halo_bytes(cin, halo_rows(KW, dil));
+  }
+  __host__ static int total(int op) { return op + BAR_BYTES + STAGE_FLOATS * 4 + 1024; }   // + alignment slack
+};
+
+__global__ void __launch_bounds__(TC_THREADS, 1)
+gemm_tc_ws_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
+                  const __grid_constant__ CUtensorMap tmW_hi, const __grid_constant__ CUtensorMap tmW_lo, TcArgs a) {
+  using S = TcWsSmem;
+  extern __shared__ unsigned char smem_raw[];
+  unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  const int w_plane = a.wblocks * S::W_BOX;
+  unsigned char* halo = smem + 2 * w_plane;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + a.op_bytes);
+  uint64_t* w_full = bars;                    // [1] TMA -> consumers: W is resident
+  uint64_t* tile_full = bars + 1;             // [2] producer -> consumer c: tile_idx[c] holds its next tile
+  uint64_t* tile_empty = bars + 3;            // [2] consumer c -> producer: tile_idx[c] has been read
+  uint64_t* halo_full = bars + 5;             // [2] TMA -> consumer c: its slot holds its tile's halo
+  uint64_t* halo_empty = bars + 7;            // [2] consumer c -> producer: the MMAs of its tile are complete
+  volatile int* tile_idx = reinterpret_cast<volatile int*>(bars + 9);   // [2]
+  float* bias_s = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(bars) + S::BAR_BYTES);
+
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // warp-uniform
+  const int wg = warp >> 2;
+  const int num_tiles = a.m_tiles;
+  const int halo_box = a.halo_rows * 64, halo_cb = (a.cin + 31) / 32;
+
+  if (threadIdx.x == 0) {
+    mbar_init(w_full, 1);
+    for (int c = 0; c < 2; c++) {
+      mbar_init(&tile_full[c], 1);
+      mbar_init(&tile_empty[c], 128);
+      mbar_init(&halo_full[c], 1);
+      mbar_init(&halo_empty[c], 1);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  if (threadIdx.x < 64) bias_s[threadIdx.x] = (int)threadIdx.x < a.N && a.bias ? a.bias[threadIdx.x] : 0.f;
+  __syncthreads();
+
+  if (wg == 0) {
+    // ===================================================================== tile scheduler + TMA producer
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      mbar_expect_tx(w_full, 2 * w_plane);
+      for (int b = 0; b < a.wblocks; b++) {   // W columns past K are zero-filled by TMA
+        tma_load_2d(smem + b * S::W_BOX, &tmW_hi, b * TC_BK, 0, w_full);
+        tma_load_2d(smem + w_plane + b * S::W_BOX, &tmW_lo, b * TC_BK, 0, w_full);
+      }
+      // i = position in this CTA's sequence of tiles, run by consumer i % 2: the first is blockIdx.x, the later ones come
+      // from the counter.  A tile's halo goes out as soon as its consumer's previous tile has no MMA left on the slot, i.e.
+      // while that tile's epilogue runs.  Two end marks follow the last tile: -1 (its consumer passes the turn on), then -2.
+      for (int i = 0, tile = blockIdx.x;; i++) {
+        const int c = i & 1;
+        if (tile < num_tiles) {
+          mbar_wait(&halo_empty[c], ((i >> 1) & 1) ^ 1);
+          unsigned char* hs = halo + c * a.halo_bytes;
+          const int r0 = tile * a.tile_rows;
+          mbar_expect_tx(&halo_full[c], 2 * halo_cb * halo_box);
+          for (int cb = 0; cb < halo_cb; cb++) {
+            tma_load_2d(hs + cb * halo_box, &tmA_hi, cb * TC_BK, r0, &halo_full[c]);
+            tma_load_2d(hs + (halo_cb + cb) * halo_box, &tmA_lo, cb * TC_BK, r0, &halo_full[c]);
+          }
+        }
+        mbar_wait(&tile_empty[c], ((i >> 1) & 1) ^ 1);
+        if (tile >= num_tiles) {
+          tile_idx[c] = -1;
+          mbar_arrive(&tile_full[c]);
+          mbar_wait(&tile_empty[c ^ 1], (((i + 1) >> 1) & 1) ^ 1);
+          tile_idx[c ^ 1] = -2;
+          mbar_arrive(&tile_full[c ^ 1]);
+          break;
+        }
+        tile_idx[c] = tile;
+        mbar_arrive(&tile_full[c]);
+        tile = (int)gridDim.x + (int)atomicAdd(&a.tile_ctr[0], 1u);
+      }
+      // every CTA has taken its last tile once all have counted themselves here: the last one returns the counter to 0
+      // for the next launch on this stream
+      __threadfence();
+      if (atomicAdd(&a.tile_ctr[1], 1u) == gridDim.x - 1) {
+        atomicExch(&a.tile_ctr[0], 0u);
+        atomicExch(&a.tile_ctr[1], 0u);
+      }
+    }
+    return;
+  }
+  // ===================================================================== MMA + epilogue (consumers c = 0, 1)
+  setmaxnreg_inc<232>();
+  const int c = wg - 1, quad = warp & 3, et = threadIdx.x - 128 * wg;
+  // named barriers besides 0: 1 + c = the 128 threads of consumer c; 3 + c = consumer c may issue its mainloop
+  const int bar = 1 + c, turn = 3 + c, turn_other = 3 + (c ^ 1);
+  float* chunk = bias_s + 64 + c * S::CHUNK_FLOATS;   // [TCW_N][33]: 32 accumulator channels of every tile row
+  if (c == 1) named_arrive(3, 256);           // consumer 0 issues the first mainloop
+  const int ksteps = a.KW * a.cin / 16;
+  const uint32_t w_s = smem_u32(smem), hs = smem_u32(halo + c * a.halo_bytes);
+  mbar_wait(w_full, 0);
+  for (int n = 0;; n++) {
+    mbar_wait(&tile_full[c], n & 1);
+    const int tile = tile_idx[c];
+    mbar_arrive(&tile_empty[c]);
+    named_sync(turn, 256);
+    if (tile < 0) {
+      if (tile == -1) named_arrive(turn_other, 256);
+      break;
+    }
+    // defined before the first wgmma, which ignores it: an undefined accumulator is kept live through the epilogue
+    float acc[TCW_N / 2];
+#pragma unroll
+    for (int i = 0; i < TCW_N / 2; i++) acc[i] = 0.f;
+    mbar_wait(&halo_full[c], n & 1);
+    // the next k16 step's first channel and its tap's first row (as a byte offset into a box)
+    uint32_t htap = 0;
+    int hch = 0;
+    wg_fence_acc(acc);
+    wg_fence();
+    for (int s = 0; s < ksteps; s++) {
+      const uint32_t wa = w_s + (uint32_t)(s >> 1) * S::W_BOX + (uint32_t)(s & 1) * 32;
+      const uint64_t w_hi = wg_desc_sw64(wa), w_lo = wg_desc_sw64(wa + w_plane);
+      const uint32_t xa = hs + (uint32_t)(hch >> 5) * halo_box + (uint32_t)(hch & 31) * 2 + htap;
+      const uint64_t x_hi = wg_desc_sw64(xa), x_lo = wg_desc_sw64(xa + halo_cb * halo_box);
+      hch += 16;
+      const bool next_tap = hch == a.cin;   // a.dil rows further down
+      hch = next_tap ? 0 : hch;
+      htap += next_tap ? a.dil * 64 : 0;
+      wgmma_ss<TCW_N>(acc, w_hi, x_lo, s != 0);
+      wgmma_ss<TCW_N>(acc, w_lo, x_hi, 1);
+      wgmma_ss<TCW_N>(acc, w_hi, x_hi, 1);
+    }
+    wg_commit();
+    named_arrive(turn_other, 256);            // the other consumer's MMAs queue behind these while they drain
+    wg_wait<0>();
+    wg_fence_acc(acc);
+    if (et == 0) mbar_arrive(&halo_empty[c]);
+    // channels c0 .. c0 + 31 are held by warps c0 / 16 and c0 / 16 + 1 of the warpgroup; `frag` = this thread's first
+    // element (row 2 (lane % 4), channel 16 (quad % 2) + lane / 4) in the chunk
+    const uint32_t frag = smem_u32(chunk) + 4 * (2 * (lane & 3) * 33 + 16 * (quad & 1) + (lane >> 2));
+#pragma unroll
+    for (int c0 = 0; c0 < 64; c0 += 32) {
+      if ((quad >> 1) == (c0 >> 5)) {
+#pragma unroll
+        for (int j = 0; j < TCW_N / 8; j++)
+#pragma unroll
+          for (int e = 0; e < 4; e++)
+            st_shared_u32(frag + 4 * ((8 * j + (e & 1)) * 33 + 8 * (e >> 1)), __float_as_uint(acc[4 * j + e] * a.acc_scale));
+      }
+      named_sync(bar, 128);
+      tc_maxpool3_cols<true>(a, chunk, chunk, bias_s + c0, tile, c0, et, bar);
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------ host side
 // 16-bit (or, `f32`, float32) matrix [rows, cols] row-major (cols contiguous, row pitch `ld` elements); box = box_cols x
 // box_rows, swizzled by the box row's width (64 or 128 bytes)
@@ -886,17 +1073,26 @@ static int tc_halo_rows(const TcGemm& g) {
 template <int BN>
 static int tc_halo_smem(const TcGemm& g) { return TcSmem<BN>::total(g.epi, TcSmem<BN>::halo_op_bytes(g.Cin, tc_halo_rows(g))); }
 
+// TC_MAXPOOL3 takes the weight-stationary kernel where its tiles fit the MMA's 112 rows and W, both halo slots and the
+// epilogue's buffers fit in shared memory (SincNet's conv1: 104 KB of W, 2 x 45 KB of halo)
+bool gemm_tc_ws(const TcGemm& g) {
+  if (g.epi != TC_MAXPOOL3 || g.tap_boxes || g.tap_off || g.KW < 2 || g.dil < 1 || g.Cin % 16 || g.Cin > 128 ||
+      g.pool3_tile_rows > TCW_N || TcWsSmem::halo_rows(g.KW, g.dil) > 256)
+    return false;
+  return TcWsSmem::total(TcWsSmem::op_bytes(g.Cin, g.KW, g.dil)) <= TC_SMEM_MAX;
+}
+
 // The halo mode is taken by every Conv1d with several taps over at most 128 channels (a multiple of 16) whose halo is one
 // TMA box (at most 256 rows) and fits, with the W ring and the epilogue's buffers, in shared memory
 bool gemm_tc_halo(const TcGemm& g) {
   if (g.tap_boxes || g.epi == TC_CONV2D || g.tap_off || g.KW < 2 || g.dil < 1 || g.Cin % 16 || g.Cin > 128 ||
       tc_halo_rows(g) > 256)
     return false;
-  return (tc_bn(g) == 64 ? tc_halo_smem<64>(g) : tc_halo_smem<128>(g)) <= TC_SMEM_MAX;
+  return gemm_tc_ws(g) || (tc_bn(g) == 64 ? tc_halo_smem<64>(g) : tc_halo_smem<128>(g)) <= TC_SMEM_MAX;
 }
 
-static int tc_setup(const TcGemm& g, int bn, int epi, bool halo, CUtensorMap* maps, TcArgs& a) {
-  const int Ktot = g.KW * g.Cin, bk = TC_BK, a_rows = halo ? tc_halo_rows(g) : TC_BM;
+static int tc_setup(const TcGemm& g, int bn, int epi, bool halo, CUtensorMap* maps, TcArgs& a, bool ws = false) {
+  const int Ktot = g.KW * g.Cin, bk = TC_BK, a_rows = ws ? TcWsSmem::halo_rows(g.KW, g.dil) : (halo ? tc_halo_rows(g) : TC_BM);
   if (make_map(&maps[0], g.A_hi, g.Mtot, g.Cin, g.lda, bk, a_rows) || make_map(&maps[1], g.A_lo, g.Mtot, g.Cin, g.lda, bk, a_rows) ||
       make_map(&maps[2], g.W_hi, g.Npad, Ktot, Ktot, bk, bn) || make_map(&maps[3], g.W_lo, g.Npad, Ktot, Ktot, bk, bn))
     return -2;
@@ -923,7 +1119,12 @@ static int tc_setup(const TcGemm& g, int bn, int epi, bool halo, CUtensorMap* ma
   a.res_lo = reinterpret_cast<const __nv_bfloat16*>(g.res_lo);
   a.pool_w = g.pool_w; a.pool_part = g.pool_part; a.pool_item_rows = g.pool_item_rows; a.pool_K = g.pool_K; a.pool_T = g.pool_T;
   a.cin = g.Cin;
-  if (halo) {
+  if (ws) {
+    a.halo_rows = a_rows;
+    a.wblocks = (Ktot + bk - 1) / bk;
+    a.halo_bytes = TcSmem<64>::halo_bytes(g.Cin, a_rows);
+    a.op_bytes = TcWsSmem::op_bytes(g.Cin, g.KW, g.dil);
+  } else if (halo) {
     a.halo_rows = a_rows;
     a.wblocks = (Ktot + bk - 1) / bk;     // W columns past Ktot of the last k-block are zero-filled by TMA
     a.halo_bytes = bn == 64 ? TcSmem<64>::halo_bytes(g.Cin, a_rows) : TcSmem<128>::halo_bytes(g.Cin, a_rows);
@@ -953,6 +1154,18 @@ static int launch_tc(const TcGemm& g, cudaStream_t st) {
   if (first_use_on_device(attr_done))   // halo mode: the size depends on the shape
     DG_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, HALO ? TC_SMEM_MAX : S::total(EPI)));
   kern<<<tc_grid(a), TC_THREADS, S::total(EPI, a.op_bytes), st>>>(m[0], m[1], m[2], m[3], m[4], m[5], a);
+  DG_LAUNCHED();
+  return 0;
+}
+
+static int launch_tc_ws(const TcGemm& g, cudaStream_t st) {
+  CUtensorMap m[6];
+  TcArgs a;
+  if (tc_setup(g, 64, TC_MAXPOOL3, true, m, a, true) || !(a.tile_ctr = tile_counter(st))) return -2;
+  static bool attr_done[64] = {};
+  if (first_use_on_device(attr_done))   // the size depends on the shape
+    DG_CUDA(cudaFuncSetAttribute(gemm_tc_ws_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_MAX));
+  gemm_tc_ws_kernel<<<tc_grid(a), TC_THREADS, TcWsSmem::total(a.op_bytes), st>>>(m[0], m[1], m[2], m[3], a);
   DG_LAUNCHED();
   return 0;
 }
@@ -1007,6 +1220,7 @@ int launch_gemm_tc(const TcGemm& g, cudaStream_t st) {
       set_error("gemm_tc (maxpool3): needs 64 output channels and tiles of 3..126 rows (a multiple of 3) that divide the item");
       return -1;
     }
+    if (gemm_tc_ws(g)) return launch_tc_ws(g, st);
     return launch_tc<64, TC_MAXPOOL3>(g, st);
   }
   if (g.Npad == 64 && g.epi == TC_BIAS_F32) return launch_tc<64, TC_BIAS_F32>(g, st);
@@ -1101,6 +1315,93 @@ int selftest_wgmma_row_shift(int base_offset_mode, unsigned* ok_shifts) {
           float ref = 0.f;
           for (int k = 0; k < 16; k++) ref += Af[(r + m) * 32 + 16 * ks + k] * Wf[n * 32 + 16 * ks + k];
           if (out[((r * 2 + ks) * 64 + m) * 8 + n] != ref) ok = false;
+        }
+    if (ok) *ok_shifts |= 1u << r;
+  }
+  return 0;
+}
+
+// The B-operand twin: one warpgroup TMA-loads A (64 rows x 32 channels) and B (72 rows x 32) with the same 64B swizzle and,
+// for every shift r = 0..8 of the B descriptor and k16 step ks, runs one m64n64k16 product of A with B rows r..r+63:
+// out[r][ks][64][64].
+__global__ void __launch_bounds__(128) wgmma_b_row_shift_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                const __grid_constant__ CUtensorMap tmB, int base_offset_mode,
+                                                                float* out) {
+  __shared__ __align__(1024) unsigned char sm[64 * 64 + 72 * 64];
+  __shared__ uint64_t bar;
+  if (threadIdx.x == 0) {
+    mbar_init(&bar, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    mbar_expect_tx(&bar, sizeof(sm));
+    tma_load_2d(sm, &tmA, 0, 0, &bar);
+    tma_load_2d(sm + 64 * 64, &tmB, 0, 0, &bar);
+  }
+  mbar_wait(&bar, 0);
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  for (int r = 0; r <= 8; r++) {
+    for (int ks = 0; ks < 2; ks++) {
+      const uint32_t sb = smem_u32(sm + 64 * 64) + r * 64 + ks * 32;
+      uint64_t db = wg_desc_sw64(sb);
+      if (base_offset_mode) db |= (uint64_t)((sb >> 7) & 7) << 49;
+      const uint64_t da = wg_desc_sw64(smem_u32(sm) + ks * 32);
+      float d[32];
+      for (int i = 0; i < 32; i++) d[i] = 0.f;
+      wg_fence_acc(d);
+      wg_fence();
+      wgmma_ss<64>(d, da, db, 0);
+      wg_commit();
+      wg_wait<0>();
+      wg_fence_acc(d);
+      for (int i = 0; i < 32; i++)
+        out[((r * 2 + ks) * 64 + 16 * w + l / 4 + 8 * ((i / 2) % 2)) * 64 + 8 * (i / 4) + 2 * (l % 4) + i % 2] = d[i];
+    }
+  }
+}
+
+int selftest_wgmma_b_row_shift(int base_offset_mode, unsigned* ok_shifts) {
+  // small integers: every product and sum is exact in fp16 inputs and the float32 accumulator
+  std::vector<uint16_t> A(64 * 32), B(72 * 32);
+  std::vector<float> Af(A.size()), Bf(B.size());
+  for (size_t i = 0; i < A.size(); i++) Af[i] = (float)((int)((i * 5 + i / 32) % 7) - 3);
+  for (size_t i = 0; i < B.size(); i++) Bf[i] = (float)((int)((i * 7 + i / 32 * 3) % 9) - 4);
+  for (size_t i = 0; i < A.size(); i++) A[i] = host_f32_to_h16(Af[i]);
+  for (size_t i = 0; i < B.size(); i++) B[i] = host_f32_to_h16(Bf[i]);
+  void *dA = nullptr, *dB = nullptr, *dO = nullptr;
+  const size_t out_n = 9 * 2 * 64 * 64;
+  int rc = 0;
+  CUtensorMap mA, mB;
+  if (cudaMalloc(&dA, A.size() * 2) != cudaSuccess || cudaMalloc(&dB, B.size() * 2) != cudaSuccess ||
+      cudaMalloc(&dO, out_n * 4) != cudaSuccess ||
+      cudaMemcpy(dA, A.data(), A.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(dB, B.data(), B.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) {
+    set_error("selftest_wgmma_b_row_shift: device buffers");
+    rc = -2;
+  }
+  if (!rc && (make_map(&mA, dA, 64, 32, 32, 32, 64) || make_map(&mB, dB, 72, 32, 32, 32, 72))) rc = -2;
+  std::vector<float> out(out_n);
+  if (!rc) {
+    wgmma_b_row_shift_kernel<<<1, 128>>>(mA, mB, base_offset_mode, static_cast<float*>(dO));
+    if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(out.data(), dO, out_n * 4, cudaMemcpyDeviceToHost) != cudaSuccess) {
+      set_error(std::string("selftest_wgmma_b_row_shift: ") + cudaGetErrorString(cudaGetLastError()));
+      rc = -2;
+    }
+  }
+  cudaFree(dA);
+  cudaFree(dB);
+  cudaFree(dO);
+  if (rc) return rc;
+  *ok_shifts = 0;
+  for (int r = 0; r <= 8; r++) {
+    bool ok = true;
+    for (int ks = 0; ks < 2; ks++)
+      for (int m = 0; m < 64; m++)
+        for (int n = 0; n < 64; n++) {
+          float ref = 0.f;
+          for (int k = 0; k < 16; k++) ref += Af[m * 32 + 16 * ks + k] * Bf[(r + n) * 32 + 16 * ks + k];
+          if (out[((r * 2 + ks) * 64 + m) * 64 + n] != ref) ok = false;
         }
     if (ok) *ok_shifts |= 1u << r;
   }

@@ -706,11 +706,18 @@ int dg_selftest_gemm_tc_bounds(int M, int Cin, int N, int epi, int* outside_unch
  * *ok_shifts is set if the product of rows r..r+63 is exact.  base_offset_mode 1 also sets the descriptor's matrix base
  * offset field to (start address >> 7) & 7, mode 0 leaves it 0. */
 int dg_selftest_wgmma_row_shift(int base_offset_mode, unsigned* ok_shifts);
+/* test hook: the same for the B operand, one m64n64k16 wgmma per row shift r = 0..8 of its B descriptor into a 64B-swizzled
+ * TMA tile; bit r of *ok_shifts is set if the product with rows r..r+63 is exact. */
+int dg_selftest_wgmma_b_row_shift(int base_offset_mode, unsigned* ok_shifts);
 /* test hook: one seeded Conv1d GEMM (KW 2..9, Cin a multiple of 16 up to 128, epi 0, 1, 2 or 5) through the halo operand
  * mode (with and without an SM cap of 3) and the tap-box mode (Cin not a multiple of 64: taps folded into K through an
  * overlapping-row view, dil 1); *equal = 1 if all outputs are byte-equal, *halo = 1 if the shape takes the halo mode.
  * epi 5: N <= 64, items of 888 rows (M a multiple of 888). */
 int dg_selftest_gemm_tc_halo(int M, int Cin, int KW, int dil, int N, int epi, int* equal, int* halo);
+/* test hook: one seeded Conv1d with the MaxPool1d(3) epilogue (epi 5; KW 2..9, Cin a multiple of 16 up to 128, N <= 64,
+ * items of 888 rows, M a multiple of 888) against the float32 reference GEMM pooled on the host: largest absolute
+ * difference of the pooled rows and their rms; *ws = 1 if the launch took the weight-stationary kernel. */
+int dg_selftest_gemm_tc_pool3_simt(int M, int Cin, int KW, int dil, int N, float* max_abs_diff, float* out_rms, int* ws);
 /* test hook (host only, no GPU): the weight-side split of float32 values into the two IEEE fp16 operand planes
  * (hi = rn16(x), lo = rn16(x - hi), saturating).  What the device does to activations with cvt.rn.satfinite.f16.f32. */
 int dg_selftest_split_f16_host(const float* x, long long n, unsigned short* hi, unsigned short* lo);
