@@ -5,6 +5,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
+#include <initializer_list>
 #include <map>
 #include <sstream>
 #include <vector>
@@ -134,6 +136,117 @@ extern "C" int dg_selftest_split_f16_host(const float* x, long long n, unsigned 
   return DG_OK;
 }
 
+// ---- shared by the gemm_tc self-tests
+// Seeded operands of a shifted-window GEMM, drawn in one order: A [M][Cin] (amplitude 2, then `tail_rows` zero rows), W in
+// [K][N] order, then bias, BatchNorm scale and shift per column.  A caller draws its extras from rnd() afterwards.  On the
+// device: A in float32 and as fp16 hi/lo planes (all M + tail_rows rows), W as weight planes of Npad rows, the three vectors.
+struct GemmFixture {
+  int M = 0, Cin = 0, KW = 0, N = 0;
+  long long rows = 0;
+  uint32_t seed = 0;
+  std::vector<float> W;   // [K][N]
+  DevBuf dA, dAh, dAl, dB, dS, dH;
+  WeightPlanes planes;
+
+  float rnd() {
+    seed = seed * 1664525u + 1013904223u;
+    return ((seed >> 8) & 0xFFFF) / 65536.f - 0.5f;
+  }
+  int init(int M_, int Cin_, int KW_, int N_, int npad, uint32_t seed_, long long tail_rows = 0) {
+    M = M_, Cin = Cin_, KW = KW_, N = N_, rows = M + tail_rows, seed = seed_;
+    const int K = KW * Cin;
+    std::vector<float> A((size_t)rows * Cin, 0.f), Wnk((size_t)N * K), bias(N), bsc(N), bsh(N);
+    W.resize((size_t)K * N);
+    for (size_t i = 0; i < (size_t)M * Cin; i++) A[i] = 2.f * rnd();
+    for (auto& v : W) v = 0.25f * rnd();
+    for (int n = 0; n < N; n++) {
+      bias[n] = rnd();
+      bsc[n] = 1.f + rnd();
+      bsh[n] = rnd();
+    }
+    for (int k = 0; k < K; k++)
+      for (int n = 0; n < N; n++) Wnk[(size_t)n * K + k] = W[(size_t)k * N + n];
+    if (upload(dA, A) || upload(dB, bias) || upload(dS, bsc) || upload(dH, bsh) || upload_split(planes, Wnk, N, npad, K) ||
+        dAh.ensure((size_t)rows * Cin * 2) || dAl.ensure((size_t)rows * Cin * 2))
+      return DG_ECUDA;
+    return launch_split_ex(dA.as<float>(), rows, Cin, Cin, Cin, 0, 1, nullptr, nullptr, dAh.p, dAl.p, nullptr);
+  }
+  // `t` over these operands with epilogue `epi`, output pitch N and no outputs yet
+  int gemm(TcGemm& t, int dil, int epi, const char* tag) const {
+    t = TcGemm{};
+    t.A_hi = dAh.p; t.A_lo = dAl.p; t.lda = Cin; t.Cin = Cin; t.KW = KW; t.dil = dil; t.Mtot = M; t.M = M;
+    t.N = N; t.bias = dB.as<float>(); t.bn_scale = dS.as<float>(); t.bn_shift = dH.as<float>(); t.ldc = N;
+    t.epi = epi; t.tag = tag;
+    return set_weights(t, planes);
+  }
+  // the float32 reference GEMM (gemm.cu) over all rows of A: bias (epi 0) or bias + LeakyReLU + BatchNorm -> c [M][N]
+  int simt(int dil, int epi, std::vector<float>& c) const {
+    DevBuf dW, dC;
+    if (upload(dW, W) || dC.ensure((size_t)M * N * 4)) return DG_ECUDA;
+    GemmArgs g{};
+    g.A = dA.as<float>(); g.lda = Cin; g.Cin = Cin; g.KW = KW; g.dil = dil; g.Mtot = rows; g.M = M;
+    g.W = dW.as<float>(); g.ldw = N; g.N = N; g.bias = dB.as<float>(); g.bn_scale = dS.as<float>();
+    g.bn_shift = dH.as<float>(); g.C = dC.as<float>(); g.ldc = N; g.epi = epi == 0 ? EPI_BIAS : EPI_BIAS_LEAKY_BN;
+    g.tag = "selftest_simt";
+    int rc;
+    if ((rc = launch_gemm(g, nullptr))) return rc;
+    c.resize((size_t)M * N);
+    DG_CUDA(cudaMemcpy(c.data(), dC.p, c.size() * 4, cudaMemcpyDeviceToHost));
+    return 0;
+  }
+};
+
+// The outputs of a TcGemm: float32 rows, hi plane, lo plane and pooling partial sums, each sized by the epilogue (empty if
+// it writes none).
+struct GemmOutputs {
+  DevBuf buf[4];
+  size_t bytes[4] = {};
+  // sizes the outputs from t's epilogue, rows, pitch and columns and the rows an m-tile advances by, and points t at them
+  int attach(TcGemm& t, int tile_rows) {
+    const int epi = t.epi;
+    const size_t m_tiles = (t.M + tile_rows - 1) / tile_rows, cells = (size_t)(epi == 5 ? t.M / 3 : t.M) * t.ldc;
+    bytes[0] = epi == 1 || epi == 3 || epi == 4 ? 0 : cells * 4;   // the launcher runs an unknown epilogue as 2
+    bytes[1] = bytes[2] = epi == 1 || epi == 3 ? cells * 2 : 0;
+    bytes[3] = epi == 4 || epi == 5 ? m_tiles * 2 * (epi == 4 ? TC_POOL_SLOTS : TC_POOL3_SLOTS) * t.N * 4 : 0;
+    for (int i = 0; i < 4; i++)
+      if (buf[i].ensure(bytes[i] + 4)) return DG_ECUDA;
+    t.out_f32 = bytes[0] ? buf[0].as<float>() : nullptr;
+    t.out_hi = bytes[1] ? buf[1].p : nullptr;
+    t.out_lo = bytes[2] ? buf[2].p : nullptr;
+    t.pool_part = bytes[3] ? buf[3].as<float>() : nullptr;
+    return 0;
+  }
+  // clears the outputs, runs `t` on at most `sm_cap` SMs (0: all) and returns what it wrote, the four outputs back to back;
+  // bytes it leaves unwritten (rows outside a Conv2d map, pooling slots of absent items) read as zero
+  int run(const TcGemm& t, int sm_cap, std::vector<unsigned char>& out) {
+    for (int i = 0; i < 4; i++) DG_CUDA(cudaMemset(buf[i].p, 0, bytes[i] + 4));
+    int rc;
+    {
+      SmLimit cap(sm_cap);
+      if ((rc = launch_gemm_tc(t, nullptr))) return rc;
+    }
+    DG_CUDA(cudaDeviceSynchronize());
+    out.resize(bytes[0] + bytes[1] + bytes[2] + bytes[3]);
+    size_t at = 0;
+    for (int i = 0; i < 4; at += bytes[i++]) DG_CUDA(cudaMemcpy(out.data() + at, buf[i].p, bytes[i], cudaMemcpyDeviceToHost));
+    return 0;
+  }
+  // runs each (launch, SM cap) in turn and sets *equal = 1 if all of them wrote the same bytes
+  int equal_runs(std::initializer_list<std::pair<const TcGemm*, int>> runs, int* equal) {
+    std::vector<unsigned char> first, cur;
+    *equal = 1;
+    int rc;
+    for (const auto& r : runs) {
+      if ((rc = run(*r.first, r.second, cur))) return rc;
+      if (first.empty())
+        first.swap(cur);
+      else if (cur != first)
+        *equal = 0;
+    }
+    return 0;
+  }
+};
+
 // Runs the same shifted-window GEMM through the float32 reference kernel (gemm.cu) and through the wgmma split-precision
 // kernel on seeded random data and reports the largest absolute difference and the output scale.
 extern "C" int dg_selftest_gemm_tc(int M, int Cin, int KW, int dil, int N, int epi, float* max_abs_diff,
@@ -142,63 +255,21 @@ extern "C" int dg_selftest_gemm_tc(int M, int Cin, int KW, int dil, int N, int e
     set_error("dg_selftest_gemm_tc: bad arguments");
     return DG_EINVAL;
   }
-  const int K = KW * Cin, npad = N == 64 ? 64 : (N + 255) / 256 * 256;
-  const long long Mtot = M;
-  std::vector<float> A((size_t)Mtot * Cin), Wkn((size_t)K * N), Wnk((size_t)N * K), bias(N), bsc(N), bsh(N);
-  uint32_t seed = 12345u;
-  auto rnd = [&]() {
-    seed = seed * 1664525u + 1013904223u;
-    return ((seed >> 8) & 0xFFFF) / 65536.f - 0.5f;
-  };
-  // DG_SELFTEST_AMP: amplitude of the A operand (default 2): small values put the whole lo plane into fp16's subnormal range
-  static const float amp = getenv("DG_SELFTEST_AMP") ? (float)atof(getenv("DG_SELFTEST_AMP")) : 2.f;
-  for (auto& v : A) v = amp * rnd();
-  for (int k = 0; k < K; k++)
-    for (int n = 0; n < N; n++) {
-      const float w = rnd() * 0.25f;
-      Wkn[(size_t)k * N + n] = w;
-      Wnk[(size_t)n * K + k] = w;
-    }
-  for (int n = 0; n < N; n++) {
-    bias[n] = rnd();
-    bsc[n] = 1.f + rnd();
-    bsh[n] = rnd();
-  }
-  DevBuf dA, dWkn, dB, dS, dH, dAh, dAl, dC0, dC1, dOh, dOl;
-  WeightPlanes dW;
-  if (upload(dA, A) || upload(dWkn, Wkn) || upload(dB, bias) || upload(dS, bsc) || upload(dH, bsh) ||
-      upload_split(dW, Wnk, N, npad, K))
-    return DG_ECUDA;
-  if (dAh.ensure((size_t)Mtot * Cin * 2) || dAl.ensure((size_t)Mtot * Cin * 2) || dC0.ensure((size_t)M * N * 4) ||
-      dC1.ensure((size_t)M * N * 4) || dOh.ensure((size_t)M * N * 2) || dOl.ensure((size_t)M * N * 2))
-    return DG_ECUDA;
+  GemmFixture f;
+  TcGemm t;
+  GemmOutputs o;
+  std::vector<float> c0;
+  std::vector<unsigned char> out;
   int rc;
-  GemmArgs g{};
-  g.A = dA.as<float>(); g.lda = Cin; g.Cin = Cin; g.KW = KW; g.dil = dil; g.Mtot = Mtot; g.M = M;
-  g.W = dWkn.as<float>(); g.ldw = N; g.N = N; g.bias = dB.as<float>(); g.bn_scale = dS.as<float>();
-  g.bn_shift = dH.as<float>(); g.C = dC0.as<float>(); g.ldc = N; g.epi = epi == 0 ? EPI_BIAS : EPI_BIAS_LEAKY_BN;
-  g.tag = "selftest_simt";
-  if ((rc = launch_gemm(g, nullptr))) return rc;
-  if ((rc = launch_split_ex(dA.as<float>(), Mtot, Cin, Cin, Cin, 0, 1, nullptr, nullptr, dAh.p, dAl.p, nullptr))) return rc;
-  TcGemm t{};
-  t.A_hi = dAh.p; t.A_lo = dAl.p; t.lda = Cin; t.Cin = Cin; t.KW = KW; t.dil = dil; t.Mtot = Mtot; t.M = M;
-  t.N = N; t.bias = dB.as<float>(); t.bn_scale = dS.as<float>();
-  t.bn_shift = dH.as<float>(); t.out_f32 = dC1.as<float>(); t.out_hi = dOh.p; t.out_lo = dOl.p; t.ldc = N;
-  t.epi = epi; t.tag = "selftest_tc";
-  if ((rc = set_weights(t, dW)) || (rc = launch_gemm_tc(t, nullptr))) return rc;
-  DG_CUDA(cudaDeviceSynchronize());
-  std::vector<float> c0((size_t)M * N), c1((size_t)M * N);
-  DG_CUDA(cudaMemcpy(c0.data(), dC0.p, c0.size() * 4, cudaMemcpyDeviceToHost));
-  std::vector<uint16_t> oh, ol;
-  if (epi == 1) {
-    oh.resize((size_t)M * N);
-    ol.resize((size_t)M * N);
-    DG_CUDA(cudaMemcpy(oh.data(), dOh.p, oh.size() * 2, cudaMemcpyDeviceToHost));
-    DG_CUDA(cudaMemcpy(ol.data(), dOl.p, ol.size() * 2, cudaMemcpyDeviceToHost));
-    for (size_t i = 0; i < c1.size(); i++) c1[i] = host_h16_to_f32(oh[i]) + host_h16_to_f32(ol[i]);
-  } else {
-    DG_CUDA(cudaMemcpy(c1.data(), dC1.p, c1.size() * 4, cudaMemcpyDeviceToHost));
-  }
+  if ((rc = f.init(M, Cin, KW, N, N == 64 ? 64 : (N + 255) / 256 * 256, 12345u)) || (rc = f.simt(dil, epi, c0)) ||
+      (rc = f.gemm(t, dil, epi, "selftest_tc")) || (rc = o.attach(t, 128)) || (rc = o.run(t, 0, out)))
+    return rc;
+  const size_t cells = (size_t)M * N;
+  std::vector<float> c1(cells);
+  std::vector<uint16_t> hl(epi == 1 ? 2 * cells : 0);   // epi 1: hi plane, then lo plane
+  memcpy(epi == 1 ? (void*)hl.data() : (void*)c1.data(), out.data(), std::min(out.size(), cells * 4));
+  if (epi == 1)
+    for (size_t i = 0; i < cells; i++) c1[i] = host_h16_to_f32(hl[i]) + host_h16_to_f32(hl[cells + i]);
   double md = 0, ss = 0;
   size_t worst = 0, n_big = 0;
   for (size_t i = 0; i < c0.size(); i++) {
@@ -217,7 +288,7 @@ extern "C" int dg_selftest_gemm_tc(int M, int Cin, int KW, int dil, int N, int e
     size_t shown = 0;
     for (size_t i = 0; i < c0.size() && shown < 12; i++)
       if (!(fabs((double)c0[i] - (double)c1[i]) <= 1e-2)) {
-        fprintf(stderr, "   row %zu col %zu: simt %g, planes hi 0x%04x lo 0x%04x\n", i / N, i % N, c0[i], oh[i], ol[i]);
+        fprintf(stderr, "   row %zu col %zu: simt %g, planes hi 0x%04x lo 0x%04x\n", i / N, i % N, c0[i], hl[i], hl[cells + i]);
         shown++;
       }
   }
@@ -236,109 +307,55 @@ extern "C" int dg_selftest_gemm_tc_grid(int M, int Cin, int KW, int dil, int N, 
     set_error("dg_selftest_gemm_tc_grid: bad arguments");
     return DG_EINVAL;
   }
-  const int K = KW * Cin;
   const int npad = epi == 5 || N == 64 ? 64 : (epi == 3 && N == 32 ? 32 : (N + 127) / 128 * 128);
   const int ldc = epi == 3 ? (N + 31) / 32 * 32 : N;
   const int item_rows = epi == 4 ? 296 : 888, tile_rows = epi == 5 ? gemm_tc_pool3_tile_rows(item_rows) : 128;
-  const long long m_tiles = (M + tile_rows - 1) / tile_rows;
-  uint32_t seed = 777u;
-  auto rnd = [&]() {
-    seed = seed * 1664525u + 1013904223u;
-    return ((seed >> 8) & 0xFFFF) / 65536.f - 0.5f;
-  };
-  std::vector<float> A((size_t)M * Cin), Wnk((size_t)N * K), bias(N), bsc(N), bsh(N), res((size_t)M * ldc), pw((size_t)M * 4);
-  for (auto& v : A) v = 2.f * rnd();
-  for (auto& v : Wnk) v = 0.25f * rnd();
-  for (int n = 0; n < N; n++) {
-    bias[n] = rnd();
-    bsc[n] = 1.f + rnd();
-    bsh[n] = rnd();
-  }
-  for (auto& v : res) v = rnd();
-  for (auto& v : pw) v = rnd() + 0.5f;
-  // output buffers, in bytes: float32 rows, hi and lo planes, pooling partial sums
-  const size_t f32_bytes = epi == 0 || epi == 2 ? (size_t)M * ldc * 4 : (epi == 5 ? (size_t)(M / 3) * ldc * 4 : 0);
-  const size_t plane_bytes = epi == 1 || epi == 3 ? (size_t)M * ldc * 2 : 0;
-  const size_t part_bytes = epi == 4 ? (size_t)m_tiles * 2 * TC_POOL_SLOTS * N * 4 : (epi == 5 ? (size_t)m_tiles * 2 * TC_POOL3_SLOTS * N * 4 : 0);
-  DevBuf dA, dAh, dAl, dB, dS, dH, dRes, dRh, dRl, dPw, dF, dOh, dOl, dPart;
-  WeightPlanes dW;
-  if (upload(dA, A) || upload(dB, bias) || upload(dS, bsc) || upload(dH, bsh) || upload(dRes, res) || upload(dPw, pw) ||
-      upload_split(dW, Wnk, N, npad, K))
-    return DG_ECUDA;
-  if (dAh.ensure((size_t)M * Cin * 2) || dAl.ensure((size_t)M * Cin * 2) || dRh.ensure((size_t)M * ldc * 2) ||
-      dRl.ensure((size_t)M * ldc * 2) || dF.ensure(f32_bytes + 4) || dOh.ensure(plane_bytes + 4) ||
-      dOl.ensure(plane_bytes + 4) || dPart.ensure(part_bytes + 4))
-    return DG_ECUDA;
+  GemmFixture f;
   int rc;
-  if ((rc = launch_split_ex(dA.as<float>(), M, Cin, Cin, Cin, 0, 1, nullptr, nullptr, dAh.p, dAl.p, nullptr)) ||
-      (rc = launch_split_ex(dRes.as<float>(), M, ldc, ldc, ldc, 0, 1, nullptr, nullptr, dRh.p, dRl.p, nullptr)))
-    return rc;
+  if ((rc = f.init(M, Cin, KW, N, npad, 777u))) return rc;
+  std::vector<float> res((size_t)M * ldc), pw((size_t)M * 4);
+  for (auto& v : res) v = f.rnd();
+  for (auto& v : pw) v = f.rnd() + 0.5f;
+  DevBuf dRes, dRh, dRl, dPw;
+  if (upload(dRes, res) || upload(dPw, pw) || dRh.ensure((size_t)M * ldc * 2) || dRl.ensure((size_t)M * ldc * 2))
+    return DG_ECUDA;
+  if ((rc = launch_split_ex(dRes.as<float>(), M, ldc, ldc, ldc, 0, 1, nullptr, nullptr, dRh.p, dRl.p, nullptr))) return rc;
   int taps[9];
   for (int j = 0; j < 9; j++) taps[j] = (j / 3 - 1) * dil + (j % 3 - 1);   // Conv2d: (dw - 1) * Hp + (dh - 1)
-  TcGemm t{};
-  t.A_hi = dAh.p; t.A_lo = dAl.p; t.lda = Cin; t.Cin = Cin; t.KW = KW; t.dil = dil; t.Mtot = M; t.M = M;
-  t.N = N; t.bias = dB.as<float>(); t.bn_scale = dS.as<float>(); t.bn_shift = dH.as<float>(); t.ldc = ldc;
-  t.epi = epi; t.tag = "selftest_tc_grid";
-  t.out_f32 = f32_bytes ? dF.as<float>() : nullptr;
-  t.out_hi = plane_bytes ? dOh.p : nullptr;
-  t.out_lo = plane_bytes ? dOl.p : nullptr;
+  TcGemm t;
+  if ((rc = f.gemm(t, dil, epi, "selftest_tc_grid"))) return rc;
+  t.ldc = ldc;
   if (epi == 3) {
     t.tap_off = taps; t.Wp = t.Wop = t.Hp = t.Hop = dil; t.relu = 1;
     t.res_hi = dRh.p; t.res_lo = dRl.p;
   }
   if (epi == 4) {
-    t.pool_w = dPw.as<float>(); t.pool_part = dPart.as<float>(); t.pool_item_rows = item_rows; t.pool_K = 3; t.pool_T = item_rows;
+    t.pool_w = dPw.as<float>(); t.pool_item_rows = item_rows; t.pool_K = 3; t.pool_T = item_rows;
   }
   if (epi == 5) {
-    t.pool_part = dPart.as<float>(); t.pool_item_rows = item_rows; t.pool3_T = item_rows / 3 - 2;
-    t.pool3_tile_rows = tile_rows;
+    t.pool_item_rows = item_rows; t.pool3_T = item_rows / 3 - 2; t.pool3_tile_rows = tile_rows;
   }
-  if ((rc = set_weights(t, dW))) return rc;
-  std::vector<unsigned char> first, cur;
-  *equal = 1;
-  const int caps[4] = {0, 1, 3, 7};
-  for (int ci = 0; ci < 4; ci++) {
-    // unwritten bytes (rows outside a Conv2d map, pooling slots of absent items) compare equal because they stay zero
-    DG_CUDA(cudaMemset(dF.p, 0, f32_bytes + 4));
-    DG_CUDA(cudaMemset(dOh.p, 0, plane_bytes + 4));
-    DG_CUDA(cudaMemset(dOl.p, 0, plane_bytes + 4));
-    DG_CUDA(cudaMemset(dPart.p, 0, part_bytes + 4));
-    {
-      SmLimit cap(caps[ci]);
-      if ((rc = launch_gemm_tc(t, nullptr))) return rc;
-    }
-    DG_CUDA(cudaDeviceSynchronize());
-    cur.resize(f32_bytes + 2 * plane_bytes + part_bytes);
-    DG_CUDA(cudaMemcpy(cur.data(), dF.p, f32_bytes, cudaMemcpyDeviceToHost));
-    DG_CUDA(cudaMemcpy(cur.data() + f32_bytes, dOh.p, plane_bytes, cudaMemcpyDeviceToHost));
-    DG_CUDA(cudaMemcpy(cur.data() + f32_bytes + plane_bytes, dOl.p, plane_bytes, cudaMemcpyDeviceToHost));
-    DG_CUDA(cudaMemcpy(cur.data() + f32_bytes + 2 * plane_bytes, dPart.p, part_bytes, cudaMemcpyDeviceToHost));
-    if (ci == 0)
-      first.swap(cur);
-    else if (cur != first)
-      *equal = 0;
-  }
-  return DG_OK;
+  GemmOutputs o;
+  if (o.attach(t, tile_rows)) return DG_ECUDA;
+  return o.equal_runs({{&t, 0}, {&t, 1}, {&t, 3}, {&t, 7}}, equal);
 }
 
-// Sets bit r of *ok_shifts when a wgmma whose A descriptor starts r = 0..8 rows into a 64B-swizzled TMA tile computes the
-// exact product of rows r..r+63; base_offset_mode 1 also sets the descriptor's matrix base offset to (address >> 7) & 7.
+// Sets bit r of *ok_shifts when a wgmma whose A descriptor (dg_selftest_wgmma_row_shift) or B descriptor
+// (dg_selftest_wgmma_b_row_shift: the weight-stationary MaxPool3 kernel's time rows) starts r = 0..8 rows into a 64B-swizzled
+// TMA tile computes the exact product with rows r..r+63; base_offset_mode 1 also sets the descriptor's matrix base offset
+// to (address >> 7) & 7.
+static int row_shift(const char* who, bool shift_b, int base_offset_mode, unsigned* ok_shifts) {
+  if (base_offset_mode < 0 || base_offset_mode > 1 || !ok_shifts) {
+    set_error(std::string(who) + ": bad arguments");
+    return DG_EINVAL;
+  }
+  return selftest_wgmma_row_shift(shift_b, base_offset_mode, ok_shifts) ? DG_ECUDA : DG_OK;
+}
 extern "C" int dg_selftest_wgmma_row_shift(int base_offset_mode, unsigned* ok_shifts) {
-  if (base_offset_mode < 0 || base_offset_mode > 1 || !ok_shifts) {
-    set_error("dg_selftest_wgmma_row_shift: bad arguments");
-    return DG_EINVAL;
-  }
-  return selftest_wgmma_row_shift(base_offset_mode, ok_shifts) ? DG_ECUDA : DG_OK;
+  return row_shift("dg_selftest_wgmma_row_shift", false, base_offset_mode, ok_shifts);
 }
-
-// Sets bit r of *ok_shifts when a wgmma whose B descriptor starts r = 0..8 rows into a 64B-swizzled TMA tile computes the
-// exact product with rows r..r+63 (the weight-stationary MaxPool3 kernel's time rows); base_offset_mode as above.
 extern "C" int dg_selftest_wgmma_b_row_shift(int base_offset_mode, unsigned* ok_shifts) {
-  if (base_offset_mode < 0 || base_offset_mode > 1 || !ok_shifts) {
-    set_error("dg_selftest_wgmma_b_row_shift: bad arguments");
-    return DG_EINVAL;
-  }
-  return selftest_wgmma_b_row_shift(base_offset_mode, ok_shifts) ? DG_ECUDA : DG_OK;
+  return row_shift("dg_selftest_wgmma_b_row_shift", true, base_offset_mode, ok_shifts);
 }
 
 // Runs one seeded Conv1d with the MaxPool1d(3) epilogue (epilogue 5, items of 888 rows, M a multiple of them) through
@@ -351,43 +368,23 @@ extern "C" int dg_selftest_gemm_tc_pool3_simt(int M, int Cin, int KW, int dil, i
     set_error("dg_selftest_gemm_tc_pool3_simt: bad arguments");
     return DG_EINVAL;
   }
-  const int K = KW * Cin, item_rows = 888, tile_rows = gemm_tc_pool3_tile_rows(item_rows);
-  const long long m_tiles = (M + tile_rows - 1) / tile_rows, tail = (long long)(KW - 1) * dil;
-  uint32_t seed = 4242u;
-  auto rnd = [&]() {
-    seed = seed * 1664525u + 1013904223u;
-    return ((seed >> 8) & 0xFFFF) / 65536.f - 0.5f;
-  };
-  // the reference reads KW - 1 taps past M: zero rows, as TMA fills them
-  std::vector<float> A((size_t)(M + tail) * Cin, 0.f), Wkn((size_t)K * N), Wnk((size_t)N * K), bias(N);
-  for (size_t i = 0; i < (size_t)M * Cin; i++) A[i] = 2.f * rnd();
-  for (int k = 0; k < K; k++)
-    for (int n = 0; n < N; n++) Wkn[(size_t)k * N + n] = Wnk[(size_t)n * K + k] = 0.25f * rnd();
-  for (auto& v : bias) v = rnd();
-  DevBuf dA, dWkn, dB, dAh, dAl, dC0, dP, dPart;
-  WeightPlanes dW;
-  if (upload(dA, A) || upload(dWkn, Wkn) || upload(dB, bias) || upload_split(dW, Wnk, N, 64, K)) return DG_ECUDA;
-  if (dAh.ensure((size_t)M * Cin * 2) || dAl.ensure((size_t)M * Cin * 2) || dC0.ensure((size_t)M * N * 4) ||
-      dP.ensure((size_t)(M / 3) * N * 4) || dPart.ensure((size_t)m_tiles * 2 * TC_POOL3_SLOTS * N * 4))
-    return DG_ECUDA;
+  const int item_rows = 888, tile_rows = gemm_tc_pool3_tile_rows(item_rows);
+  GemmFixture f;
+  TcGemm t;
+  GemmOutputs o;
+  std::vector<float> c0;
+  std::vector<unsigned char> out;
   int rc;
-  GemmArgs g{};
-  g.A = dA.as<float>(); g.lda = Cin; g.Cin = Cin; g.KW = KW; g.dil = dil; g.Mtot = M + tail; g.M = M;
-  g.W = dWkn.as<float>(); g.ldw = N; g.N = N; g.bias = dB.as<float>(); g.C = dC0.as<float>(); g.ldc = N; g.epi = EPI_BIAS;
-  g.tag = "selftest_simt";
-  if ((rc = launch_gemm(g, nullptr))) return rc;
-  if ((rc = launch_split_ex(dA.as<float>(), M, Cin, Cin, Cin, 0, 1, nullptr, nullptr, dAh.p, dAl.p, nullptr))) return rc;
-  TcGemm t{};
-  t.A_hi = dAh.p; t.A_lo = dAl.p; t.lda = Cin; t.Cin = Cin; t.KW = KW; t.dil = dil; t.Mtot = M; t.M = M;
-  t.N = N; t.bias = dB.as<float>(); t.out_f32 = dP.as<float>(); t.ldc = N; t.epi = 5; t.tag = "selftest_tc_pool3";
-  t.pool_part = dPart.as<float>(); t.pool_item_rows = item_rows; t.pool3_T = item_rows / 3 - 2; t.pool3_tile_rows = tile_rows;
-  if ((rc = set_weights(t, dW))) return rc;
+  // the reference reads KW - 1 taps past M: zero rows, as TMA fills them
+  if ((rc = f.init(M, Cin, KW, N, 64, 4242u, (long long)(KW - 1) * dil)) || (rc = f.simt(dil, 0, c0)) ||
+      (rc = f.gemm(t, dil, 5, "selftest_tc_pool3")))
+    return rc;
+  t.pool_item_rows = item_rows; t.pool3_T = item_rows / 3 - 2; t.pool3_tile_rows = tile_rows;
+  if (o.attach(t, tile_rows)) return DG_ECUDA;
   *ws = gemm_tc_ws(t) ? 1 : 0;
-  if ((rc = launch_gemm_tc(t, nullptr))) return rc;
-  DG_CUDA(cudaDeviceSynchronize());
-  std::vector<float> c0((size_t)M * N), p1((size_t)(M / 3) * N);
-  DG_CUDA(cudaMemcpy(c0.data(), dC0.p, c0.size() * 4, cudaMemcpyDeviceToHost));
-  DG_CUDA(cudaMemcpy(p1.data(), dP.p, p1.size() * 4, cudaMemcpyDeviceToHost));
+  if ((rc = o.run(t, 0, out))) return rc;
+  std::vector<float> p1((size_t)(M / 3) * N);
+  memcpy(p1.data(), out.data(), p1.size() * 4);
   double md = 0, ss = 0;
   for (long long r = 0; r < M / 3; r++)
     for (int n = 0; n < N; n++) {
@@ -418,79 +415,30 @@ extern "C" int dg_selftest_gemm_tc_halo(int M, int Cin, int KW, int dil, int N, 
   const int K = KW * Cin, Kf = folded ? (K + 63) / 64 * 64 : K;
   const int npad = epi == 5 || N == 64 ? 64 : (N + 127) / 128 * 128;
   const int item_rows = 888, tile_rows = epi == 5 ? gemm_tc_pool3_tile_rows(item_rows) : 128;
-  const long long m_tiles = (M + tile_rows - 1) / tile_rows;
-  const long long tail = 64;   // zero rows after M: the folded view reads up to Kf / Cin rows past its own
-  uint32_t seed = 9090u;
-  auto rnd = [&]() {
-    seed = seed * 1664525u + 1013904223u;
-    return ((seed >> 8) & 0xFFFF) / 65536.f - 0.5f;
-  };
-  std::vector<float> A((size_t)(M + tail) * Cin, 0.f), Wnk((size_t)N * K), Wf((size_t)N * Kf, 0.f), bias(N), bsc(N), bsh(N);
-  for (size_t i = 0; i < (size_t)M * Cin; i++) A[i] = 2.f * rnd();
-  for (auto& v : Wnk) v = 0.25f * rnd();
-  for (int n = 0; n < N; n++)
-    for (int k = 0; k < K; k++) Wf[(size_t)n * Kf + k] = Wnk[(size_t)n * K + k];
-  for (int n = 0; n < N; n++) {
-    bias[n] = rnd();
-    bsc[n] = 1.f + rnd();
-    bsh[n] = rnd();
-  }
-  const size_t f32_bytes = epi == 0 || epi == 2 ? (size_t)M * N * 4 : (epi == 5 ? (size_t)(M / 3) * N * 4 : 0);
-  const size_t plane_bytes = epi == 1 ? (size_t)M * N * 2 : 0;
-  const size_t part_bytes = epi == 5 ? (size_t)m_tiles * 2 * TC_POOL3_SLOTS * N * 4 : 0;
-  DevBuf dA, dAh, dAl, dB, dS, dH, dF, dOh, dOl, dPart;
-  WeightPlanes dW, dWf;
-  if (upload(dA, A) || upload(dB, bias) || upload(dS, bsc) || upload(dH, bsh) || upload_split(dW, Wnk, N, npad, K) ||
-      upload_split(dWf, Wf, N, npad, Kf))
-    return DG_ECUDA;
-  if (dAh.ensure((size_t)(M + tail) * Cin * 2) || dAl.ensure((size_t)(M + tail) * Cin * 2) || dF.ensure(f32_bytes + 4) ||
-      dOh.ensure(plane_bytes + 4) || dOl.ensure(plane_bytes + 4) || dPart.ensure(part_bytes + 4))
-    return DG_ECUDA;
+  GemmFixture f;
+  TcGemm t;
+  GemmOutputs o;
   int rc;
-  if ((rc = launch_split_ex(dA.as<float>(), M + tail, Cin, Cin, Cin, 0, 1, nullptr, nullptr, dAh.p, dAl.p, nullptr))) return rc;
-  TcGemm t{};
-  t.A_hi = dAh.p; t.A_lo = dAl.p; t.lda = Cin; t.Cin = Cin; t.KW = KW; t.dil = dil; t.Mtot = M; t.M = M;
-  t.N = N; t.bias = dB.as<float>(); t.bn_scale = dS.as<float>(); t.bn_shift = dH.as<float>(); t.ldc = N;
-  t.epi = epi; t.tag = "selftest_tc_halo";
-  t.out_f32 = f32_bytes ? dF.as<float>() : nullptr;
-  t.out_hi = plane_bytes ? dOh.p : nullptr;
-  t.out_lo = plane_bytes ? dOl.p : nullptr;
+  // 64 zero rows after M: the folded view reads up to Kf / Cin rows past its own
+  if ((rc = f.init(M, Cin, KW, N, npad, 9090u, 64)) || (rc = f.gemm(t, dil, epi, "selftest_tc_halo"))) return rc;
   if (epi == 5) {
-    t.pool_part = dPart.as<float>(); t.pool_item_rows = item_rows; t.pool3_T = item_rows / 3 - 2;
-    t.pool3_tile_rows = tile_rows;
+    t.pool_item_rows = item_rows; t.pool3_T = item_rows / 3 - 2; t.pool3_tile_rows = tile_rows;
   }
-  if ((rc = set_weights(t, dW))) return rc;
+  if (o.attach(t, tile_rows)) return DG_ECUDA;
   *halo = gemm_tc_halo(t) ? 1 : 0;
   TcGemm ref = t;
   ref.tap_boxes = 1;
+  WeightPlanes wf;
   if (folded) {
+    std::vector<float> Wf((size_t)N * Kf, 0.f);
+    for (int k = 0; k < K; k++)
+      for (int n = 0; n < N; n++) Wf[(size_t)n * Kf + k] = f.W[(size_t)k * N + n];
+    if (upload_split(wf, Wf, N, npad, Kf)) return DG_ECUDA;
     ref.Cin = Kf;
     ref.KW = 1;
-    if ((rc = set_weights(ref, dWf))) return rc;
+    if ((rc = set_weights(ref, wf))) return rc;
   }
-  std::vector<unsigned char> first, cur;
-  *equal = 1;
-  for (int run = 0; run < 3; run++) {   // halo, halo on 3 SMs, tap boxes
-    DG_CUDA(cudaMemset(dF.p, 0, f32_bytes + 4));
-    DG_CUDA(cudaMemset(dOh.p, 0, plane_bytes + 4));
-    DG_CUDA(cudaMemset(dOl.p, 0, plane_bytes + 4));
-    DG_CUDA(cudaMemset(dPart.p, 0, part_bytes + 4));
-    {
-      SmLimit cap(run == 1 ? 3 : 0);
-      if ((rc = launch_gemm_tc(run == 2 ? ref : t, nullptr))) return rc;
-    }
-    DG_CUDA(cudaDeviceSynchronize());
-    cur.resize(f32_bytes + 2 * plane_bytes + part_bytes);
-    DG_CUDA(cudaMemcpy(cur.data(), dF.p, f32_bytes, cudaMemcpyDeviceToHost));
-    DG_CUDA(cudaMemcpy(cur.data() + f32_bytes, dOh.p, plane_bytes, cudaMemcpyDeviceToHost));
-    DG_CUDA(cudaMemcpy(cur.data() + f32_bytes + plane_bytes, dOl.p, plane_bytes, cudaMemcpyDeviceToHost));
-    DG_CUDA(cudaMemcpy(cur.data() + f32_bytes + 2 * plane_bytes, dPart.p, part_bytes, cudaMemcpyDeviceToHost));
-    if (run == 0)
-      first.swap(cur);
-    else if (cur != first)
-      *equal = 0;
-  }
-  return DG_OK;
+  return o.equal_runs({{&t, 0}, {&t, 3}, {&ref, 0}}, equal);   // halo, halo on 3 SMs, tap boxes
 }
 
 // Runs one seeded GEMM (one tap, epilogue 0, 1 or 2) twice: into outputs of pitch N, and into outputs of pitch N + 40 with
@@ -508,37 +456,21 @@ extern "C" int dg_selftest_gemm_tc_bounds(int M, int Cin, int N, int epi, int* o
   const int npad = N <= 64 && epi == 0 ? 64 : (N + 127) / 128 * 128, esize = planes ? 2 : 4;   // 64-wide tiles: epi 0 only
   const int ldc = N + 40;
   const long long rows = (long long)M + 130;
-  uint32_t seed = 4242u;
-  auto rnd = [&]() {
-    seed = seed * 1664525u + 1013904223u;
-    return ((seed >> 8) & 0xFFFF) / 65536.f - 0.5f;
-  };
-  std::vector<float> A((size_t)M * Cin), Wnk((size_t)N * Cin), bias(N), bsc(N), bsh(N);
-  for (auto& v : A) v = 2.f * rnd();
-  for (auto& v : Wnk) v = 0.25f * rnd();
-  for (int n = 0; n < N; n++) {
-    bias[n] = rnd();
-    bsc[n] = 1.f + rnd();
-    bsh[n] = rnd();
-  }
   const size_t dense_bytes = (size_t)M * N * esize, wide_bytes = (size_t)rows * ldc * esize + 16;
-  DevBuf dA, dAh, dAl, dB, dS, dH, dD0, dD1, dW0, dW1;
-  WeightPlanes dW;
-  if (upload(dA, A) || upload(dB, bias) || upload(dS, bsc) || upload(dH, bsh) || upload_split(dW, Wnk, N, npad, Cin) ||
-      dAh.ensure((size_t)M * Cin * 2) || dAl.ensure((size_t)M * Cin * 2) || dD0.ensure(dense_bytes) ||
-      dD1.ensure(dense_bytes) || dW0.ensure(wide_bytes) || dW1.ensure(wide_bytes))
-    return DG_ECUDA;
+  GemmFixture f;
+  TcGemm t;
+  GemmOutputs o;
+  std::vector<unsigned char> dense;   // pitch N: float32 rows, or the hi plane and then the lo plane
   int rc;
-  if ((rc = launch_split_ex(dA.as<float>(), M, Cin, Cin, Cin, 0, 1, nullptr, nullptr, dAh.p, dAl.p, nullptr))) return rc;
-  TcGemm t{};
-  t.A_hi = dAh.p; t.A_lo = dAl.p; t.lda = Cin; t.Cin = Cin; t.KW = 1; t.dil = 1; t.Mtot = M; t.M = M;
-  t.N = N; t.bias = dB.as<float>(); t.bn_scale = dS.as<float>(); t.bn_shift = dH.as<float>();
-  t.epi = epi; t.tag = "selftest_tc_bounds";
-  if ((rc = set_weights(t, dW))) return rc;
-  // output 0 (float32 rows or hi plane) and 1 (lo plane) at `off` bytes into the buffers, pitch `ld`
-  auto point = [&](DevBuf& o0, DevBuf& o1, size_t off, int ld) {
-    unsigned char* b0 = static_cast<unsigned char*>(o0.p) + off;
-    unsigned char* b1 = static_cast<unsigned char*>(o1.p) + off;
+  if ((rc = f.init(M, Cin, 1, N, npad, 4242u)) || (rc = f.gemm(t, 1, epi, "selftest_tc_bounds")) || (rc = o.attach(t, 128)) ||
+      (rc = o.run(t, 0, dense)))
+    return rc;
+  DevBuf dW0, dW1;
+  if (dW0.ensure(wide_bytes) || dW1.ensure(wide_bytes)) return DG_ECUDA;
+  // output 0 (float32 rows or hi plane) and 1 (lo plane) at `off` bytes into the wide buffers, pitch `ld`
+  auto point = [&](size_t off, int ld) {
+    unsigned char* b0 = static_cast<unsigned char*>(dW0.p) + off;
+    unsigned char* b1 = static_cast<unsigned char*>(dW1.p) + off;
     t.out_f32 = planes ? nullptr : reinterpret_cast<float*>(b0);
     t.out_hi = planes ? b0 : nullptr;
     t.out_lo = planes ? b1 : nullptr;
@@ -547,28 +479,25 @@ extern "C" int dg_selftest_gemm_tc_bounds(int M, int Cin, int N, int epi, int* o
   const unsigned char SENTINEL = 0xA5;
   DG_CUDA(cudaMemset(dW0.p, SENTINEL, wide_bytes));
   DG_CUDA(cudaMemset(dW1.p, SENTINEL, wide_bytes));
-  point(dD0, dD1, 0, N);
-  if ((rc = launch_gemm_tc(t, nullptr))) return rc;
-  point(dW0, dW1, 0, ldc);
+  point(0, ldc);
   if ((rc = launch_gemm_tc(t, nullptr))) return rc;
   // refusals: base off alignment, pitch off 16 bytes (both leave the sentinel in place)
-  point(dW0, dW1, (size_t)esize, ldc);
+  point((size_t)esize, ldc);
   const int rc_base = launch_gemm_tc(t, nullptr);
-  point(dW0, dW1, 0, ldc + (planes ? 4 : 2));
+  point(0, ldc + (planes ? 4 : 2));
   const int rc_pitch = launch_gemm_tc(t, nullptr);
   DG_CUDA(cudaDeviceSynchronize());
   const int n_out = planes ? 2 : 1;
-  std::vector<unsigned char> dense(dense_bytes), wide(wide_bytes);
+  std::vector<unsigned char> wide(wide_bytes);
   *outside_unchanged = 1;
   *equal = 1;
-  for (int o = 0; o < n_out; o++) {
-    DG_CUDA(cudaMemcpy(dense.data(), (o ? dD1 : dD0).p, dense_bytes, cudaMemcpyDeviceToHost));
-    DG_CUDA(cudaMemcpy(wide.data(), (o ? dW1 : dW0).p, wide_bytes, cudaMemcpyDeviceToHost));
+  for (int i = 0; i < n_out; i++) {
+    DG_CUDA(cudaMemcpy(wide.data(), (i ? dW1 : dW0).p, wide_bytes, cudaMemcpyDeviceToHost));
     const size_t row_bytes = (size_t)N * esize, pitch = (size_t)ldc * esize;
     for (long long r = 0; r < rows; r++) {
       const unsigned char* w = wide.data() + r * pitch;
       const bool inside = r < M;
-      if (inside && memcmp(w, dense.data() + r * row_bytes, row_bytes)) *equal = 0;
+      if (inside && memcmp(w, dense.data() + i * dense_bytes + r * row_bytes, row_bytes)) *equal = 0;
       for (size_t b = inside ? row_bytes : 0; b < pitch; b++)
         if (w[b] != SENTINEL) *outside_unchanged = 0;
     }

@@ -180,11 +180,10 @@ inline int gemm_tc_pool3_tile_rows(int item_rows) {
 int launch_gemm_tc(const TcGemm& g, cudaStream_t st);
 bool gemm_tc_halo(const TcGemm& g);   // the launch loads each tile's rows once (halo mode) instead of once per tap
 bool gemm_tc_ws(const TcGemm& g);     // epi 5: the weight-stationary kernel (W resident in shared memory, D^T = W . X^T)
-// one m64n8k16 wgmma per row shift r = 0..8 of its A descriptor into a 64B-swizzled tile (dg_selftest_wgmma_row_shift):
-// bit r of *ok_shifts is set when the product of rows r..r+63 is exact for both k16 steps of the 32-channel row
-int selftest_wgmma_row_shift(int base_offset_mode, unsigned* ok_shifts);
-// the same for the B operand: one m64n64k16 wgmma per row shift r = 0..8 of its B descriptor (dg_selftest_wgmma_b_row_shift)
-int selftest_wgmma_b_row_shift(int base_offset_mode, unsigned* ok_shifts);
+// one wgmma per row shift r = 0..8 of its A descriptor (m64n8k16), or with `shift_b` of its B descriptor (m64n64k16), into a
+// 64B-swizzled tile (dg_selftest_wgmma_row_shift, dg_selftest_wgmma_b_row_shift): bit r of *ok_shifts is set when the
+// product with rows r..r+63 is exact for both k16 steps of the 32-channel row
+int selftest_wgmma_row_shift(bool shift_b, int base_offset_mode, unsigned* ok_shifts);
 int launch_split_ex(const float* x, long long rows_out, int C, int ld_in, int ld_out, int pool, int item_rows,
                     const float* sc, const float* sh, void* hi, void* lo, cudaStream_t st, const int* skip_flag = nullptr);
 void split_weights_host(const float* w, int N, int Npad, int K, uint16_t* hi, uint16_t* lo, float scale = 1.f);

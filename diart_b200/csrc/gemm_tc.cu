@@ -53,6 +53,7 @@
 #include <vector>
 
 #include "dg_common.cuh"
+#include "host.cuh"
 #include "tc_ptx.cuh"
 
 namespace dg {
@@ -1235,13 +1236,21 @@ int launch_gemm_tc(const TcGemm& g, cudaStream_t st) {
 }
 
 // ------------------------------------------------------------------------------------ descriptor row-shift probe
-// One warpgroup TMA-loads A (72 rows x 32 fp16 channels) and W (8 rows x 32) with the 64B swizzle of the GEMM's operand
-// boxes and, for every shift r = 0..8 and k16 step ks, runs one m64n8k16 product of A rows r..r+63 with W: out[r][ks][64][8].
-// base_offset_mode 1 also sets the descriptor's matrix base offset field (bits 49-51) to (start address >> 7) & 7.
+// One warpgroup TMA-loads A and B (32 fp16 channels per row) with the 64B swizzle of the GEMM's operand boxes and, for every
+// shift r = 0..8 and k16 step ks, runs one m64nBNk16 product whose SHIFT_B operand descriptor starts r rows into its tile:
+// A rows r..r+63 with B's 8 rows (m64n8), or A's 64 rows with B rows r..r+63 (m64n64); out[r][ks][64][BN].
+// base_offset_mode 1 also sets the shifted descriptor's matrix base offset field (bits 49-51) to (start address >> 7) & 7.
+template <bool SHIFT_B>
+struct RowShiftProbe {
+  static constexpr int BN = SHIFT_B ? 64 : 8, A_ROWS = SHIFT_B ? 64 : 72, B_ROWS = SHIFT_B ? 72 : 8;
+};
+
+template <bool SHIFT_B>
 __global__ void __launch_bounds__(128) wgmma_row_shift_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                              const __grid_constant__ CUtensorMap tmW, int base_offset_mode,
+                                                              const __grid_constant__ CUtensorMap tmB, int base_offset_mode,
                                                               float* out) {
-  __shared__ __align__(1024) unsigned char sm[72 * 64 + 8 * 64];
+  using P = RowShiftProbe<SHIFT_B>;
+  __shared__ __align__(1024) unsigned char sm[(P::A_ROWS + P::B_ROWS) * 64];
   __shared__ uint64_t bar;
   if (threadIdx.x == 0) {
     mbar_init(&bar, 1);
@@ -1251,161 +1260,69 @@ __global__ void __launch_bounds__(128) wgmma_row_shift_kernel(const __grid_const
   if (threadIdx.x == 0) {
     mbar_expect_tx(&bar, sizeof(sm));
     tma_load_2d(sm, &tmA, 0, 0, &bar);
-    tma_load_2d(sm + 72 * 64, &tmW, 0, 0, &bar);
+    tma_load_2d(sm + P::A_ROWS * 64, &tmB, 0, 0, &bar);
   }
   mbar_wait(&bar, 0);
   const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
   for (int r = 0; r <= 8; r++) {
     for (int ks = 0; ks < 2; ks++) {
-      const uint32_t sa = smem_u32(sm) + r * 64 + ks * 32;
-      uint64_t da = wg_desc_sw64(sa);
-      if (base_offset_mode) da |= (uint64_t)((sa >> 7) & 7) << 49;
-      const uint64_t dw = wg_desc_sw64(smem_u32(sm + 72 * 64) + ks * 32);
-      float d[4] = {0.f, 0.f, 0.f, 0.f};
+      const uint32_t sa = smem_u32(sm) + (SHIFT_B ? 0 : r * 64) + ks * 32;
+      const uint32_t sb = smem_u32(sm + P::A_ROWS * 64) + (SHIFT_B ? r * 64 : 0) + ks * 32;
+      const uint64_t base = base_offset_mode ? (uint64_t)(((SHIFT_B ? sb : sa) >> 7) & 7) << 49 : 0;
+      const uint64_t da = wg_desc_sw64(sa) | (SHIFT_B ? 0 : base), db = wg_desc_sw64(sb) | (SHIFT_B ? base : 0);
+      float d[P::BN / 2];
+      for (int i = 0; i < P::BN / 2; i++) d[i] = 0.f;
       wg_fence_acc(d);
       wg_fence();
-      wgmma_ss<8>(d, da, dw, 0);
+      wgmma_ss<P::BN>(d, da, db, 0);
       wg_commit();
       wg_wait<0>();
       wg_fence_acc(d);
-      for (int i = 0; i < 4; i++)
-        out[((r * 2 + ks) * 64 + 16 * w + l / 4 + 8 * ((i / 2) % 2)) * 8 + 2 * (l % 4) + i % 2] = d[i];
+      for (int i = 0; i < P::BN / 2; i++)
+        out[((r * 2 + ks) * 64 + 16 * w + l / 4 + 8 * ((i / 2) % 2)) * P::BN + 8 * (i / 4) + 2 * (l % 4) + i % 2] = d[i];
     }
   }
 }
 
-int selftest_wgmma_row_shift(int base_offset_mode, unsigned* ok_shifts) {
+template <bool SHIFT_B>
+static int selftest_row_shift(int base_offset_mode, unsigned* ok_shifts) {
+  using P = RowShiftProbe<SHIFT_B>;
   // small integers: every product and sum is exact in fp16 inputs and the float32 accumulator
-  std::vector<uint16_t> A(72 * 32), W(8 * 32);
-  std::vector<float> Af(A.size()), Wf(W.size());
-  for (size_t i = 0; i < A.size(); i++) Af[i] = (float)((int)((i * 7 + i / 32 * 3) % 9) - 4);
-  for (size_t i = 0; i < W.size(); i++) Wf[i] = (float)((int)((i * 5 + 1) % 7) - 3);
-  for (size_t i = 0; i < A.size(); i++) A[i] = host_f32_to_h16(Af[i]);
-  for (size_t i = 0; i < W.size(); i++) W[i] = host_f32_to_h16(Wf[i]);
-  void *dA = nullptr, *dW = nullptr, *dO = nullptr;
-  const size_t out_n = 9 * 2 * 64 * 8;
-  int rc = 0;
-  CUtensorMap mA, mW;
-  if (cudaMalloc(&dA, A.size() * 2) != cudaSuccess || cudaMalloc(&dW, W.size() * 2) != cudaSuccess ||
-      cudaMalloc(&dO, out_n * 4) != cudaSuccess ||
-      cudaMemcpy(dA, A.data(), A.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemcpy(dW, W.data(), W.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) {
-    set_error("selftest_wgmma_row_shift: device buffers");
-    rc = -2;
-  }
-  if (!rc && (make_map(&mA, dA, 72, 32, 32, 32, 72) || make_map(&mW, dW, 8, 32, 32, 32, 8))) rc = -2;
-  std::vector<float> out(out_n);
-  if (!rc) {
-    wgmma_row_shift_kernel<<<1, 128>>>(mA, mW, base_offset_mode, static_cast<float*>(dO));
-    if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(out.data(), dO, out_n * 4, cudaMemcpyDeviceToHost) != cudaSuccess) {
-      set_error(std::string("selftest_wgmma_row_shift: ") + cudaGetErrorString(cudaGetLastError()));
-      rc = -2;
-    }
-  }
-  cudaFree(dA);
-  cudaFree(dW);
-  cudaFree(dO);
-  if (rc) return rc;
-  *ok_shifts = 0;
-  for (int r = 0; r <= 8; r++) {
-    bool ok = true;
-    for (int ks = 0; ks < 2; ks++)
-      for (int m = 0; m < 64; m++)
-        for (int n = 0; n < 8; n++) {
-          float ref = 0.f;
-          for (int k = 0; k < 16; k++) ref += Af[(r + m) * 32 + 16 * ks + k] * Wf[n * 32 + 16 * ks + k];
-          if (out[((r * 2 + ks) * 64 + m) * 8 + n] != ref) ok = false;
-        }
-    if (ok) *ok_shifts |= 1u << r;
-  }
-  return 0;
-}
-
-// The B-operand twin: one warpgroup TMA-loads A (64 rows x 32 channels) and B (72 rows x 32) with the same 64B swizzle and,
-// for every shift r = 0..8 of the B descriptor and k16 step ks, runs one m64n64k16 product of A with B rows r..r+63:
-// out[r][ks][64][64].
-__global__ void __launch_bounds__(128) wgmma_b_row_shift_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                const __grid_constant__ CUtensorMap tmB, int base_offset_mode,
-                                                                float* out) {
-  __shared__ __align__(1024) unsigned char sm[64 * 64 + 72 * 64];
-  __shared__ uint64_t bar;
-  if (threadIdx.x == 0) {
-    mbar_init(&bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    mbar_expect_tx(&bar, sizeof(sm));
-    tma_load_2d(sm, &tmA, 0, 0, &bar);
-    tma_load_2d(sm + 64 * 64, &tmB, 0, 0, &bar);
-  }
-  mbar_wait(&bar, 0);
-  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
-  for (int r = 0; r <= 8; r++) {
-    for (int ks = 0; ks < 2; ks++) {
-      const uint32_t sb = smem_u32(sm + 64 * 64) + r * 64 + ks * 32;
-      uint64_t db = wg_desc_sw64(sb);
-      if (base_offset_mode) db |= (uint64_t)((sb >> 7) & 7) << 49;
-      const uint64_t da = wg_desc_sw64(smem_u32(sm) + ks * 32);
-      float d[32];
-      for (int i = 0; i < 32; i++) d[i] = 0.f;
-      wg_fence_acc(d);
-      wg_fence();
-      wgmma_ss<64>(d, da, db, 0);
-      wg_commit();
-      wg_wait<0>();
-      wg_fence_acc(d);
-      for (int i = 0; i < 32; i++)
-        out[((r * 2 + ks) * 64 + 16 * w + l / 4 + 8 * ((i / 2) % 2)) * 64 + 8 * (i / 4) + 2 * (l % 4) + i % 2] = d[i];
-    }
-  }
-}
-
-int selftest_wgmma_b_row_shift(int base_offset_mode, unsigned* ok_shifts) {
-  // small integers: every product and sum is exact in fp16 inputs and the float32 accumulator
-  std::vector<uint16_t> A(64 * 32), B(72 * 32);
-  std::vector<float> Af(A.size()), Bf(B.size());
-  for (size_t i = 0; i < A.size(); i++) Af[i] = (float)((int)((i * 5 + i / 32) % 7) - 3);
-  for (size_t i = 0; i < B.size(); i++) Bf[i] = (float)((int)((i * 7 + i / 32 * 3) % 9) - 4);
+  std::vector<float> Af(P::A_ROWS * 32), Bf(P::B_ROWS * 32);
+  std::vector<float>& shifted = SHIFT_B ? Bf : Af;
+  std::vector<float>& fixed = SHIFT_B ? Af : Bf;
+  for (size_t i = 0; i < shifted.size(); i++) shifted[i] = (float)((int)((i * 7 + i / 32 * 3) % 9) - 4);
+  for (size_t i = 0; i < fixed.size(); i++) fixed[i] = (float)((int)((i * 5 + i / 32) % 7) - 3);
+  std::vector<uint16_t> A(Af.size()), B(Bf.size());
   for (size_t i = 0; i < A.size(); i++) A[i] = host_f32_to_h16(Af[i]);
   for (size_t i = 0; i < B.size(); i++) B[i] = host_f32_to_h16(Bf[i]);
-  void *dA = nullptr, *dB = nullptr, *dO = nullptr;
-  const size_t out_n = 9 * 2 * 64 * 64;
-  int rc = 0;
+  std::vector<float> out(9 * 2 * 64 * P::BN);
+  DevBuf dA, dB, dO;
   CUtensorMap mA, mB;
-  if (cudaMalloc(&dA, A.size() * 2) != cudaSuccess || cudaMalloc(&dB, B.size() * 2) != cudaSuccess ||
-      cudaMalloc(&dO, out_n * 4) != cudaSuccess ||
-      cudaMemcpy(dA, A.data(), A.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemcpy(dB, B.data(), B.size() * 2, cudaMemcpyHostToDevice) != cudaSuccess) {
-    set_error("selftest_wgmma_b_row_shift: device buffers");
-    rc = -2;
-  }
-  if (!rc && (make_map(&mA, dA, 64, 32, 32, 32, 64) || make_map(&mB, dB, 72, 32, 32, 32, 72))) rc = -2;
-  std::vector<float> out(out_n);
-  if (!rc) {
-    wgmma_b_row_shift_kernel<<<1, 128>>>(mA, mB, base_offset_mode, static_cast<float*>(dO));
-    if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpy(out.data(), dO, out_n * 4, cudaMemcpyDeviceToHost) != cudaSuccess) {
-      set_error(std::string("selftest_wgmma_b_row_shift: ") + cudaGetErrorString(cudaGetLastError()));
-      rc = -2;
-    }
-  }
-  cudaFree(dA);
-  cudaFree(dB);
-  cudaFree(dO);
-  if (rc) return rc;
+  if (upload_u16(dA, A) || upload_u16(dB, B) || dO.ensure(out.size() * 4) ||
+      make_map(&mA, dA.p, P::A_ROWS, 32, 32, 32, P::A_ROWS) || make_map(&mB, dB.p, P::B_ROWS, 32, 32, 32, P::B_ROWS))
+    return -2;
+  wgmma_row_shift_kernel<SHIFT_B><<<1, 128>>>(mA, mB, base_offset_mode, dO.as<float>());
+  DG_CUDA(cudaGetLastError());
+  DG_CUDA(cudaMemcpy(out.data(), dO.p, out.size() * 4, cudaMemcpyDeviceToHost));
   *ok_shifts = 0;
   for (int r = 0; r <= 8; r++) {
     bool ok = true;
     for (int ks = 0; ks < 2; ks++)
       for (int m = 0; m < 64; m++)
-        for (int n = 0; n < 64; n++) {
+        for (int n = 0; n < P::BN; n++) {
           float ref = 0.f;
-          for (int k = 0; k < 16; k++) ref += Af[m * 32 + 16 * ks + k] * Bf[(r + n) * 32 + 16 * ks + k];
-          if (out[((r * 2 + ks) * 64 + m) * 64 + n] != ref) ok = false;
+          for (int k = 0; k < 16; k++)
+            ref += Af[(m + (SHIFT_B ? 0 : r)) * 32 + 16 * ks + k] * Bf[(n + (SHIFT_B ? r : 0)) * 32 + 16 * ks + k];
+          if (out[((r * 2 + ks) * 64 + m) * P::BN + n] != ref) ok = false;
         }
     if (ok) *ok_shifts |= 1u << r;
   }
   return 0;
+}
+
+int selftest_wgmma_row_shift(bool shift_b, int base_offset_mode, unsigned* ok_shifts) {
+  return shift_b ? selftest_row_shift<true>(base_offset_mode, ok_shifts) : selftest_row_shift<false>(base_offset_mode, ok_shifts);
 }
 
 // ------------------------------------------------------------------------------------ 16-bit hi/lo split
